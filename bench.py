@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- LU GFLOP/s (FP64, (2/3)N^3) of the CONFLUX hot path on 1/2/4/8 B200 (BASELINE.json's metric).
+"""bench.py -- LU GFLOP/s (FP64, (2/3)N^3) of the CONFLUX hot path on 1/2/4/8 H100 (BASELINE.json's metric).
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...     (N > 1: one rank per GPU)
 
 A "step" is one LU factorisation of one synthetic matrix (lu_params::InitMatrix generator, seed 42):
@@ -14,6 +14,8 @@ A "step" is one LU factorisation of one synthetic matrix (lu_params::InitMatrix 
 memory and the device->host read of the permutation inside the timed region (streamed: the upload of the next
 matrix overlaps the current factorisation; `e2e.single_shot` is the un-overlapped latency of one call).  PyTorch is plumbing only
 (torch.distributed bootstrap, pinned host memory).
+`--dump-outputs DIR` writes what the last timed step computed (see dump_outputs) so that two builds can be compared
+output for output; the inputs are the seeded generator's, identical from run to run.
 """
 import argparse
 import ctypes
@@ -29,11 +31,12 @@ sys.path.insert(0, ROOT)
 
 WORKLOADS = {1: (16384, 256, (1, 1, 1)), 2: (32768, 512, (1, 1, 2)), 4: (32768, 512, (2, 2, 1)),
              8: (65536, 512, (2, 2, 2))}
-FP64_TENSOR_NOMINAL_TFLOPS = 40.0  # NVIDIA B200 datasheet (FP64 / FP64 tensor), context only
+FP64_TENSOR_NOMINAL_TFLOPS = 67.0  # NVIDIA H100 SXM data sheet (FP64 tensor core, 700 W), context only
+DUMP_BUDGET_BYTES = 64 * 10 ** 6 - (64 << 10)   # 64 MB in all, npy headers included
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region, and the card's name and power limit."""
 
     def __init__(self, index=0):
         self.index, self.rows, self.proc = index, [], None
@@ -62,8 +65,14 @@ class ClockSampler:
         reasons = [n for i, n in enumerate(names) if any(len(r) > 3 + i and r[3 + i].lower().startswith("active") for r in self.rows)]
         # median over the samples taken under load (upper half of the sorted clocks)
         load = sm[len(sm) // 2:] if sm else []
+        try:
+            name, plimit = subprocess.run(["nvidia-smi", f"--id={self.index}", "--query-gpu=name,power.limit",
+                                           "--format=csv,noheader,nounits"], capture_output=True, text=True,
+                                          timeout=30).stdout.strip().split(", ")[:2]
+        except Exception:  # noqa: BLE001
+            name, plimit = None, None
         return {"sm_mhz": load[len(load) // 2] if load else None, "sm_max_mhz": max(mx) if mx else None,
-                "reasons": reasons, "samples": len(sm)}
+                "reasons": reasons, "samples": len(sm), "gpu": name, "power_limit_w": plimit}
 
 
 CPU_THREAD_CAP = 32  # OpenBLAS (pthreads) + the reference's OpenMP loops oversubscribe badly beyond this
@@ -216,21 +225,23 @@ def load_golden_perm(N, v, grid):
     return None
 
 
-def load_traffic(M, N, K, kernel="dmma"):
-    """dram__bytes_read.sum + dram__bytes_write.sum of ONE launch of the trailing-update kernel, from the committed
-    summary of an `ncu --set full` capture (profiles/r02_gemm_traffic.json, written by tools/summarize_ncu.py)."""
-    path = os.path.join(ROOT, "profiles", "r02_gemm_traffic.json")
-    try:
-        d = json.load(open(path))
-    except Exception:  # noqa: BLE001
-        return None, None
-    for e in d.get("launches", []):
-        if (e.get("kernel", "dmma"), e.get("M"), e.get("N"), e.get("K")) == (kernel, M, N, K):
-            return e.get("dram_bytes"), e.get("source")
-    return None, None
+def dump_outputs(out_dir, rank, world, local, perm=None):
+    """What a caller of the timed path receives: this rank's local factor (Ml x Nl) and the permutation.  The factor is
+    sampled at a fixed, seeded set of flat indices (stored beside the values) so that all files stay within
+    DUMP_BUDGET_BYTES; float64 throughout."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    flat = local.reshape(-1)
+    n = min(flat.size, (DUMP_BUDGET_BYTES // world - 8 * (perm.size if perm is not None else 0)) // 16)
+    idx = np.sort(np.random.default_rng(1234).choice(flat.size, size=n, replace=False)) if n < flat.size else np.arange(flat.size)
+    sfx = f"_rank{rank}" if world > 1 else ""
+    np.save(os.path.join(out_dir, f"factor_sample{sfx}.npy"), flat[idx].astype(np.float64))
+    np.save(os.path.join(out_dir, f"factor_sample_index{sfx}.npy"), idx.astype(np.float64))
+    if perm is not None and rank == 0:
+        np.save(os.path.join(out_dir, "permutation.npy"), perm.astype(np.float64))
 
 
-CHOL_WORKLOAD = (32768, 512)     # BASELINE.json configs[4]: cholesky_miniapp --dim=32768 --tile=512 (8 x B200)
+CHOL_WORKLOAD = (32768, 512)     # BASELINE.json configs[4]: cholesky_miniapp --dim=32768 --tile=512 (8 GPUs)
 
 
 def run_cholesky(args, rank, world, local_rank):
@@ -282,6 +293,8 @@ def run_cholesky(args, rank, world, local_rank):
     for _ in range(args.steps):
         dev_ms += ch.parallelCholesky(upload=False)
     barrier()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, rank, world, ch.local_factor())
     clocks = sampler.stop() if rank == 0 else None
     _lib.lib().cflx_chol_launch_count(ch._h, ctypes.byref(cnt), 1)
     dev_ms = max_over_ranks(dev_ms)
@@ -340,7 +353,11 @@ def main():
     ap.add_argument("--v", type=int, default=0)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-validate", action="store_true", help="skip the grid-wide residual (debugging only)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the factor (seeded sample) and permutation of the last timed step to DIR/*.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -396,9 +413,9 @@ def main():
 
     # FP64 tensor-pipe peak of THIS GPU, measured before the runs (burst) -- MEASURED_PEAKS.json has no FP64 entry
     peak_burst = cb.dbg.fp64_peak_ex(0)[0] if rank == 0 else None
-    tcgen05 = bool(L.cflx_lu_uses_tcgen05(gv._h))
-    # raw int8 rate of the tensor pipe (back-to-back tcgen05.mma 128x256x32, operands resident): the ceiling of the tcgen05 path
-    i8_tmacs = cb.dbg.umma_peak(0, 256) if (rank == 0 and tcgen05) else None
+    ozaki = bool(L.cflx_lu_uses_ozaki(gv._h))
+    # raw int8 rate of the tensor cores (back-to-back wgmma 64x256x32, operands resident): the ceiling of the int8 path
+    i8_tmacs = cb.dbg.wgmma_peak(256) if (rank == 0 and ozaki) else None
     sampler = ClockSampler(local_rank)
     if rank == 0:
         sampler.start()
@@ -421,6 +438,12 @@ def main():
     barrier()
     wall_ms = (time.perf_counter() - t0) * 1e3
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs:                                   # the factors of the last timed step, read back untimed
+        factor = np.empty((gv.Ml, gv.Nl))
+        last_perm = np.empty(gv.M, dtype=np.int32)
+        _lib.check(L.cflx_lu_get_factors(gv._h, factor.ctypes.data, last_perm.ctypes.data), "lu_get_factors")
+        dump_outputs(args.dump_outputs, rank, world, factor, last_perm)
+        del factor
     L.cflx_lu_launch_count(gv._h, ctypes.byref(cnt), 1)
     launches = cnt.value
     L.cflx_lu_set_kernel_timing(gv._h, 0)
@@ -467,11 +490,10 @@ def main():
     if rank == 0:
         dmma_peak = peak_burst
         g_tf = gemm_flops / (gemm_ms * 1e-3) / 1e12 if gemm_ms > 0 else None
-        n1 = gv.Ml - gv.v                             # first-step shape of the trailing update (the ncu-captured launch)
-        traffic, traffic_src = load_traffic(n1, gv.Nl - gv.v, gv.nlayr, "ozaki" if tcgen05 else "dmma")
+        n1 = gv.Ml - gv.v                             # first-step shape of the trailing update
         # FP64-equivalent ceiling of the int8 path: 36 exact int8 plane products per FP64 product
         i8_equiv = (2.0 * i8_tmacs / 36.0) if i8_tmacs else None
-        roof_peak = i8_equiv if tcgen05 else dmma_peak
+        roof_peak = i8_equiv if ozaki else dmma_peak
         grid = (Px, Py, Pz)
         line = {
             "metric": "LU GFLOP/s (FP64, (2/3)N^3)", "value": value, "unit": "GFLOP/s", "n_gpus": args.gpus,
@@ -490,23 +512,20 @@ def main():
             "gpu_launches": int(launches),
             "clocks": clocks,
             "roofline": {"bound": "tensor",
-                         "kernel": ("ozaki_gemm_kernel (int8 tcgen05.mma + TMEM + TMA, 36 exact digit-plane products per FP64 product)"
-                                    if tcgen05 else "gemm_tn_kernel (FP64 DMMA.8x8x4)") + ", trailing update",
-                         "achieved": g_tf, "peak": roof_peak, "unit": "TFLOP/s (FP64-equivalent)" if tcgen05 else "TFLOP/s",
+                         "kernel": ("ozaki_gemm_kernel (int8 wgmma + TMA, 36 exact digit-plane products per FP64 product)"
+                                    if ozaki else "gemm_tn_kernel (FP64 DMMA.8x8x4)") + ", trailing update",
+                         "achieved": g_tf, "peak": roof_peak, "unit": "TFLOP/s (FP64-equivalent)" if ozaki else "TFLOP/s",
                          "frac": (g_tf / roof_peak) if (g_tf and roof_peak) else None,
                          "frac_of_fp64_dmma_peak": (g_tf / dmma_peak) if g_tf else None, "fp64_dmma_peak": dmma_peak,
                          "int8_pipe_measured_pops": (2.0 * i8_tmacs / 1e3) if i8_tmacs else None,
-                         # dram__bytes_read+write of ONE launch of the first-step shape, read from the committed summary of
-                         # an `ncu --set full` capture; algorithmic bytes = 16*M*N + 8*K*(M+N) (C read+write, operands once)
-                         "traffic": traffic, "traffic_source": traffic_src,
+                         # algorithmic bytes = 16*M*N + 8*K*(M+N) (C read+write, operands once)
                          "traffic_launch": f"M={n1} N={gv.Nl - gv.v} K={gv.nlayr} (step 0), algorithmic "
                                            f"{16.0 * n1 * (gv.Nl - gv.v) + 8.0 * gv.nlayr * (n1 + gv.Nl - gv.v):.4g} B",
-                         "peak_source": ("tcgen05 path: peak = raw int8 rate of the tensor pipe measured live (cflx_dbg_umma_peak: back-to-back "
-                                         "tcgen05.mma.kind::i8 128x256x32, one CTA per SM; nominal 4.5 POP/s) x 2 / 36 digit-plane products; "
-                                         if tcgen05 else "") +
+                         "peak_source": ("int8 path: peak = raw int8 rate of the tensor cores measured live (cflx_dbg_wgmma_peak: back-to-back "
+                                         "wgmma 64x256x32 s8, two warpgroups per SM; nominal 1979 TOP/s dense) x 2 / 36 digit-plane products; "
+                                         if ozaki else "") +
                                         "fp64_dmma_peak = FP64 tensor (DMMA.8x8x4) burst peak measured live by cflx_dbg_fp64_peak_ex "
-                                        "(best ~2 ms launch; = 148 SM x 4 x 32 flop/clk x 1.965 GHz); MEASURED_PEAKS.json has no "
-                                        "FP64 / int8 entry; nominal FP64 %.0f TFLOP/s" % FP64_TENSOR_NOMINAL_TFLOPS,
+                                        "(best ~2 ms launch); nominal FP64 tensor %.0f TFLOP/s" % FP64_TENSOR_NOMINAL_TFLOPS,
                          "share_of_step": gemm_ms / dev_ms if dev_ms else None,
                          "whole_path_frac": value / 1e3 / (args.gpus * dmma_peak)},
             "parity": {"permutation_is_permutation": bool(ok_perm), "pivots_equal_reference": pivots_equal,

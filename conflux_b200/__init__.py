@@ -1,4 +1,4 @@
-"""conflux_b200 -- B200-native (sm_100a) implementation of CONFLUX's LU hot path.
+"""conflux_b200 -- H100-native (sm_90a) implementation of CONFLUX's LU hot path.
 
 Python mirror of the reference's driver-facing interface for this path (same names, argument meaning and
 error behaviour; reference file:line relative to eth-cscs/conflux):
@@ -319,7 +319,7 @@ class dbg:
 
     @staticmethod
     def ozaki_gemm(AT, B, C=None, reps=1, want_planes=False):
-        """D = C - AT^T @ B on the int8 tcgen05 path.  Returns dict(D, ms, split_ms[, pa, pb, ea, eb])."""
+        """D = C - AT^T @ B on the int8 wgmma path.  Returns dict(D, ms, split_ms[, pa, pb, ea, eb])."""
         AT = np.ascontiguousarray(AT, dtype=np.float64)
         B = np.ascontiguousarray(B, dtype=np.float64)
         K, M = AT.shape
@@ -348,10 +348,10 @@ class dbg:
         return A, gri, a01[:len(piv)]
 
     @staticmethod
-    def umma_peak(which, n):
-        """tera-MACs/s of back-to-back tcgen05.mma 128 x n x 32B-K: which 0 = kind::i8, 1 = kind::f16 (bf16)."""
+    def wgmma_peak(n):
+        """tera-MACs/s of back-to-back int8 wgmma 64 x n x 32 (n = 64, 128, 192, 256)."""
         t = ctypes.c_double()
-        check(lib().cflx_dbg_umma_peak(int(which), int(n), ctypes.byref(t)), "dbg_umma_peak")
+        check(lib().cflx_dbg_wgmma_peak(int(n), ctypes.byref(t)), "dbg_wgmma_peak")
         return t.value
 
     @staticmethod

@@ -22,10 +22,10 @@ SYMBOLS = [
     "cflx_last_error", "cflx_version", "cflx_device_count", "cflx_get_unique_id", "cflx_comm_create",
     "cflx_comm_barrier", "cflx_comm_destroy", "cflx_host_alloc", "cflx_host_free", "cflx_auto_grid", "cflx_lu_dims", "cflx_init_matrix_host",
     "cflx_lu_create", "cflx_lu_info", "cflx_lu_set_local", "cflx_lu_queue_next_local", "cflx_lu_factor", "cflx_lu_get_factors",
-    "cflx_lu_get_permutation", "cflx_lu_residual", "cflx_lu_validate", "cflx_lu_launch_count", "cflx_lu_uses_tcgen05", "cflx_lu_set_profiling", "cflx_lu_phase_ms", "cflx_lu_timeline",
+    "cflx_lu_get_permutation", "cflx_lu_residual", "cflx_lu_validate", "cflx_lu_launch_count", "cflx_lu_uses_ozaki", "cflx_lu_set_profiling", "cflx_lu_phase_ms", "cflx_lu_timeline",
     "cflx_lu_set_kernel_timing", "cflx_lu_trailing_stats", "cflx_lu_destroy", "cflx_chol_auto_grid", "cflx_chol_auto_tile", "cflx_chol_dims", "cflx_chol_init_matrix_host",
     "cflx_chol_create", "cflx_chol_info", "cflx_chol_set_local", "cflx_chol_factor", "cflx_chol_get_local", "cflx_chol_validate",
-    "cflx_chol_launch_count", "cflx_chol_destroy", "cflx_dbg_gemm_tn", "cflx_dbg_panel", "cflx_dbg_trsm", "cflx_dbg_push_pivots", "cflx_dbg_ozaki_gemm", "cflx_dbg_umma_peak", "cflx_dbg_last_panel_cycles", "cflx_dbg_fp64_peak", "cflx_dbg_fp64_peak_ex",
+    "cflx_chol_launch_count", "cflx_chol_destroy", "cflx_dbg_gemm_tn", "cflx_dbg_panel", "cflx_dbg_trsm", "cflx_dbg_push_pivots", "cflx_dbg_ozaki_gemm", "cflx_dbg_wgmma_peak", "cflx_dbg_last_panel_cycles", "cflx_dbg_fp64_peak", "cflx_dbg_fp64_peak_ex",
 ]
 
 
@@ -74,7 +74,7 @@ def lib():
         L.cflx_lu_get_permutation.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
         L.cflx_lu_residual.argtypes = [ctypes.c_void_p, c_double_p]
         L.cflx_lu_validate.argtypes = [ctypes.c_void_p, c_double_p, c_double_p]
-        L.cflx_lu_uses_tcgen05.argtypes = [ctypes.c_void_p]
+        L.cflx_lu_uses_ozaki.argtypes = [ctypes.c_void_p]
         L.cflx_lu_launch_count.argtypes = [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int64), ctypes.c_int]
         L.cflx_lu_set_profiling.argtypes = [ctypes.c_void_p, ctypes.c_int]
         L.cflx_lu_phase_ms.argtypes = [ctypes.c_void_p, c_double_p]
@@ -102,7 +102,7 @@ def lib():
         L.cflx_dbg_push_pivots.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
                                            ctypes.c_void_p, ctypes.c_void_p]
         L.cflx_dbg_ozaki_gemm.argtypes = [ctypes.c_int] * 3 + [ctypes.c_void_p] * 8 + [ctypes.c_int, c_double_p, c_double_p]
-        L.cflx_dbg_umma_peak.argtypes = [ctypes.c_int, ctypes.c_int, c_double_p]
+        L.cflx_dbg_wgmma_peak.argtypes = [ctypes.c_int, c_double_p]
         L.cflx_dbg_fp64_peak.argtypes = [ctypes.c_int, c_double_p]
         L.cflx_dbg_fp64_peak_ex.argtypes = [ctypes.c_int, c_double_p, c_double_p]
         _lib = L

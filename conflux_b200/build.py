@@ -1,6 +1,6 @@
-"""conflux_b200/build.py -- compiles the CUDA sources in-tree into conflux_b200/libconflux_b200.so (sm_100a only).
+"""conflux_b200/build.py -- compiles the CUDA sources in-tree into conflux_b200/libconflux_b200.so (sm_90a only).
 
-nvcc cross-compiles without a GPU; the built .so travels to the GPU box with the repo snapshot."""
+nvcc cross-compiles without a GPU."""
 import os
 import subprocess
 import sys
@@ -10,7 +10,8 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libconflux_b200.so")
 SOURCES = ["gemm.cu", "ozaki.cu", "panel.cu", "rows.cu", "trsm.cu", "lu.cu", "validate.cu", "chol.cu", "dbg.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC,-O3",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC,-O3",
          "-ccbin", "g++", "--expt-relaxed-constexpr"]
 
 
@@ -24,6 +25,7 @@ def _stale(target, deps):
 def build(force=False, verbose=False):
     hdrs = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".h", ".cuh"))]
     hdrs.append(os.path.join(os.path.dirname(HERE), "include", "conflux_b200.h"))
+    hdrs.append(os.path.abspath(__file__))          # the flags live here: objects built with other flags are stale
     objs = []
     bdir = os.path.join(HERE, "build")
     os.makedirs(bdir, exist_ok=True)
@@ -44,7 +46,7 @@ def build(force=False, verbose=False):
     if failed:
         raise RuntimeError("nvcc failed")
     if force or procs or _stale(OUT, objs):
-        cmd = [NVCC, "-shared", "-o", OUT] + objs + ["-lnccl", "-Xlinker", "--no-as-needed"]
+        cmd = [NVCC] + ARCH + ["-shared", "-o", OUT] + objs + ["-lnccl", "-Xlinker", "--no-as-needed"]
         subprocess.check_call(cmd)
     return OUT
 

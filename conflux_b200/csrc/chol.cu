@@ -1,5 +1,5 @@
 // conflux_b200/csrc/chol.cu -- CONFCHOX: the reference's communication-avoiding Cholesky factorisation (A = L L^T, lower),
-// re-designed for a grid of B200s.  BASELINE config C5: cholesky_miniapp --dim=32768 --tile=512 on 8 GPUs.
+// re-designed for a grid of H100s.  BASELINE config C5: cholesky_miniapp --dim=32768 --tile=512 on 8 GPUs.
 //
 // Reference (relative to /root/reference/src/conflux/cholesky):
 //   Cholesky.cpp:60-160        initialize(): grid / tile-size choice, buffers, input generation      -> cflx_chol_create,
@@ -12,7 +12,7 @@
 //   Cholesky.cpp:580-612       reduceA11: the next tile column is summed over the z layers            -> ncclReduce (k-communicator)
 //   Cholesky.cpp:620-700       scatterA11 / A00 broadcast                                            -> ncclBroadcast of L_kk^T and of the
 //                                                                                                      panel pieces
-// B200-first layout instead of the reference's tile objects (TileMatrix.h): every rank keeps its 2-D block-cyclic share
+// GPU-first layout instead of the reference's tile objects (TileMatrix.h): every rank keeps its 2-D block-cyclic share
 // of the matrix as ONE row-major Ml x Nl array in HBM (tile (gi, gj) on rank (gi % Px, gj % Py) at local tile (gi / Px,
 // gj / Py); the lower triangle is meaningful), the tile column of a step is handled as a transposed (K-major) panel like
 // in the LU path, so the TRSM and the rank-v update run on the same FP64 tensor-core GEMM (gemm.cu) on long contiguous
@@ -35,7 +35,7 @@ struct cflx_chol {
            *W = nullptr, *Uinv = nullptr, *LinvT = nullptr, *acc = nullptr, *Q = nullptr /* scratch of the blocked tile Cholesky */;
     int* info = nullptr;
     int64_t ldp = 0, ldb = 0;
-    OzakiWorkspace oz{};                    // digit planes of the int8 tcgen05 rank-v update (default when v / Pz is 128..512)
+    OzakiWorkspace oz{};                    // digit planes of the int8 wgmma rank-v update (CFLX_GEMM=ozaki, v / Pz 128..512)
     bool use_ozaki = false;
     cudaStream_t side = nullptr;            // panel pipeline of step k+1 (all NCCL traffic lives here) under the update of step k
     cudaEvent_t ev_col[2] = {nullptr, nullptr}, ev_panel[2] = {nullptr, nullptr};
@@ -399,7 +399,7 @@ int broadcast_pieces(cflx_chol* ch, int t, int gfirst, int jmin, int buf, cudaSt
 }
 // X[i][j] -= L[i][t] * L[j][t]^T on the local tiles with global tile row i >= tile column j, j in the local column tiles
 // [lj_lo, lj_hi) (global index >= jmin; lower triangle), each z layer with its own slab of the v contraction indices.
-// SMs the persistent tcgen05 update leaves to the look-ahead panel pipeline on the side stream (CFLX_CHOL_LEAVE)
+// SMs the persistent int8 update leaves to the look-ahead panel pipeline on the side stream (CFLX_CHOL_LEAVE)
 static int chol_leave_sms() {
     static int leave = -1;
     if (leave < 0) {
@@ -478,8 +478,8 @@ int broadcast_and_update(cflx_chol* ch, int t, int jmin, bool below_only, double
 
 // Panel pipeline of step k on stream s: z-reduce of tile column k, Cholesky of the diagonal tile, L_kk^T down the grid
 // column, the panel solve, the stores, and (k < Kappa - 1) the broadcast of the panel pieces into buffer set k & 1.
-// (1) Cholesky of the v x v diagonal tile.  One CTA needs 2.2 ms for a 512 x 512 tile (measured: 2/3 of a whole 16384^2
-// factorisation), so the tile is itself factored in 128-wide block columns: the 128 x 128 diagonal block on one CTA, the
+// (1) Cholesky of the v x v diagonal tile.  One CTA alone is far too slow for a 512 x 512 tile (it would sit on
+// the critical path of every step), so the tile is itself factored in 128-wide block columns: the 128 x 128 diagonal block on one CTA, the
 // block column below it by ONE GEMM with the inverted block, the trailing part of the tile by one rank-128 GEMM -- both on
 // the whole GPU (FP64 DMMA kernel).  Tiles that are not a multiple of 128 (tests) keep the one-CTA kernel.
 int potrf_tile(cflx_chol* ch, size_t psm, cudaStream_t s) {
@@ -703,7 +703,7 @@ int cflx_chol_create(cflx_comm* c, int N, int v, int Px, int Py, int Pz, cflx_ch
     if ((rc = gemm_tn_setup())) return fail(rc);
     {
         const char* e = getenv("CFLX_GEMM");
-        if (!(e && !strcmp(e, "dmma")) && ch->nlayr % 128 == 0 && ch->nlayr <= 512) {
+        if (e && !strcmp(e, "ozaki") && ch->nlayr % 128 == 0 && ch->nlayr <= 512) {   // as in cflx_lu_create
             if ((rc = ozaki_workspace_create(&ch->oz, ch->Ml, ch->Nl, ch->nlayr))) return fail(rc);
             ch->use_ozaki = true;
         }
@@ -774,7 +774,7 @@ int cflx_chol_factor(cflx_chol* ch, double* ms_out) {
     for (int k = 0; k + 1 < ch->Kappa; ++k) {
         const int b = k & 1, nb1 = (k + 1) & 1;
         CFLX_CUDA(cudaStreamWaitEvent(s, ch->ev_panel[b], 0));             // pieces of step k are in buffer set b
-        CFLX_TRY(split_planes(ch, k + 1, k + 1, b, s));                     // (int8 tcgen05 path) digit planes of both operands
+        CFLX_TRY(split_planes(ch, k + 1, k + 1, b, s));                     // (int8 wgmma path) digit planes of both operands
         const int ljn = (k + 1) / Py;                                        // local tile of column k+1 on its owners
         const bool own_next = (pj == (k + 1) % Py);
         if (own_next) CFLX_TRY(update_columns(ch, k + 1, k + 1, b, ch->A11, ljn, ljn + 1, s, b));

@@ -1,4 +1,4 @@
-// conflux_b200/csrc/common.cuh -- shared device/host helpers (sm_100a only).
+// conflux_b200/csrc/common.cuh -- shared device/host helpers (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -93,7 +93,7 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint3
                  : "memory");
 }
 
-// FP64 tensor-core MMA (DMMA.8x8x4 in sm_100a SASS): D(8x8) += A(8x4, row) * B(4x8, col)
+// FP64 tensor-core MMA (DMMA.8x8x4 in sm_90a SASS): D(8x8) += A(8x4, row) * B(4x8, col)
 // lane l holds a = A[l>>2][l&3], b = B[l&3][l>>2], c0/c1 = C[l>>2][2*(l&3)+{0,1}]
 __device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b) {
     asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"

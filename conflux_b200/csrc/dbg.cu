@@ -303,7 +303,7 @@ int cflx_dbg_push_pivots(int n_rows, int n_cols, double* A_inout, int npiv, cons
     return CFLX_OK;
 }
 
-// D = C - AT^T * B on the int8 tcgen05 path (ozaki.cu): AT [K x M], B [K x N], C/D [M x N] row-major dense host arrays,
+// D = C - AT^T * B on the int8 wgmma path (ozaki.cu): AT [K x M], B [K x N], C/D [M x N] row-major dense host arrays,
 // K a multiple of 128, N even.  Optional outputs for tests: the digit planes [8][M][K] / [8][N][K] (int8) and the
 // exponents [M] / [N], exactly as the kernels produced them.  ms_out = mean device time of the GEMM kernel alone.
 int cflx_dbg_ozaki_gemm(int M, int N, int K, const double* AT, const double* B, const double* C, double* D,
@@ -361,13 +361,6 @@ int cflx_dbg_ozaki_gemm(int M, int N, int K, const double* AT, const double* B, 
         }
         if (ea_out) cudaMemcpy(ea_out, ws.ea, sizeof(int) * M, cudaMemcpyDeviceToHost);
         if (eb_out) cudaMemcpy(eb_out, ws.eb, sizeof(int) * N, cudaMemcpyDeviceToHost);
-        if (ws.dbg) {
-            long long h[16];
-            cudaMemcpy(h, ws.dbg, sizeof(h), cudaMemcpyDeviceToHost);
-            fprintf(stderr, "[ozaki cycles, CTA 0] producer: wait emptyB %lld emptyA %lld total %lld | mma: wait fullA %lld fullB %lld tempty %lld "
-                            "total %lld | epilogue: wait tfull %lld drain %lld rmw %lld total %lld\n",
-                    h[0], h[1], h[3], h[4], h[5], h[6], h[7], h[8], h[9], h[10], h[11]);
-        }
         if (cudaDeviceSynchronize() != cudaSuccess) rc = CFLX_ERR_CUDA;
     }
     ozaki_workspace_destroy(&ws);
@@ -376,12 +369,12 @@ int cflx_dbg_ozaki_gemm(int M, int N, int K, const double* AT, const double* B, 
     return rc;
 }
 
-// raw tensor-pipe rate of back-to-back tcgen05.mma 128 x n x 32-byte-K instructions (one CTA per SM, operands resident in
-// shared memory): which = 0 kind::i8, 1 kind::f16 (bf16).  Returns tera-MACs per second (x2 = TOP/s / TFLOP/s).
-int cflx_dbg_umma_peak(int which, int n, double* tmacs_out) {
+// raw int8 tensor-core rate of back-to-back wgmma 64 x n x 32 instructions (two warpgroups per CTA, one CTA per SM,
+// operands resident in shared memory).  Returns tera-MACs per second (x2 = TOP/s).
+int cflx_dbg_wgmma_peak(int n, double* tmacs_out) {
     CFLX_TRY(check_device());
     if (!tmacs_out) return CFLX_ERR_ARG;
-    return umma_peak_probe(n, which, tmacs_out);
+    return wgmma_peak_probe(n, tmacs_out);
 }
 
 }  // extern "C"

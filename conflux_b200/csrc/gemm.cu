@@ -7,7 +7,7 @@
 // (L is stored transposed, L^T[k][row]; U is U[k][col]) so that every operand row a CTA needs is one contiguous
 // 1 KB segment: the producer warp stages tiles with 1-D bulk asynchronous copies (cp.async.bulk -> UBLKCP, the
 // TMA engine) into a 4-stage shared-memory ring guarded by mbarriers, and 8 consumer warps run
-// mma.sync.m8n8k4.f64 (DMMA.8x8x4 -- the native FP64 tensor instruction of sm_100a; tcgen05 has no f64 kind)
+// mma.sync.m8n8k4.f64 (DMMA.8x8x4 -- the native FP64 tensor instruction of sm_90a; wgmma has no f64 kind)
 // on 64x32 warp tiles with accumulators in registers.  Shared-memory row stride is 132 doubles (== 4 mod 16) so
 // both fragment loads (lane -> [k = lane&3][outer = lane>>2]) are bank-conflict free per half-warp.
 #include <cstdlib>
@@ -177,7 +177,7 @@ int launch_one(const GemmArgs& g, cudaStream_t stream) {
     CFLX_CUDA(cudaGetLastError());
     return CFLX_OK;
 }
-int tile_variant() {  // default: 64x128 tile, two CTAs per SM (measured 33.5 vs 30.6 TFLOP/s at K = 256);
+int tile_variant() {  // default: 64x128 tile, two CTAs per SM;
                       // CFLX_GEMM_TILE=128 selects the 128x128 tile with one CTA per SM
     static int v = -1;
     if (v < 0) {

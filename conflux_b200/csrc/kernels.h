@@ -1,4 +1,4 @@
-// conflux_b200/csrc/kernels.h -- host-callable launchers of the sm_100a kernels (internal; the public boundary is
+// conflux_b200/csrc/kernels.h -- host-callable launchers of the sm_90a kernels (internal; the public boundary is
 // include/conflux_b200.h).
 #pragma once
 #include <cuda_runtime.h>
@@ -24,14 +24,13 @@ int gemm_tn_setup();
 int launch_gemm_tn(const GemmArgs& g, cudaStream_t stream);
 
 // ---------------------------------------------------------------- ozaki.cu
-// FP64 trailing update on the int8 tcgen05 path (error-free digit planes): C -= L * U with L^T, U K-major in HBM.
+// FP64 trailing update on the int8 wgmma path (error-free digit planes): C -= L * U with L^T, U K-major in HBM.
 struct OzakiWorkspace {
     struct Maps;              // the two CUtensorMap objects (kept out of this header)
     int8_t* planesA = nullptr;  // [8][cap_a][K]
     int8_t* planesB = nullptr;  // [8][cap_b][K]
     int* ea = nullptr;          // [cap_a]
     int* eb = nullptr;          // [cap_b]
-    long long* dbg = nullptr;   // [16] cycle counters of CTA 0 (CFLX_OZAKI_DBG=1)
     Maps* maps = nullptr;
     int K = 0, cap_a = 0, cap_b = 0, sms = 0;
 };
@@ -39,7 +38,7 @@ int ozaki_workspace_create(OzakiWorkspace* ws, int max_rows, int max_cols, int K
 void ozaki_workspace_destroy(OzakiWorkspace* ws);
 int ozaki_split_a(OzakiWorkspace* ws, const double* LT, int64_t ld, int n, cudaStream_t s);
 int ozaki_split_b(OzakiWorkspace* ws, const double* U, int64_t ld, int col0, int n, cudaStream_t s);
-int umma_peak_probe(int n, int use_f16, double* tmacs_out);
+int wgmma_peak_probe(int n, double* tmacs_out);
 int launch_ozaki_gemm(OzakiWorkspace* ws, int M, int N, int row0, int col0, double* C, int64_t ldc, int max_ctas, cudaStream_t s);
 
 // ---------------------------------------------------------------- panel.cu
@@ -48,11 +47,11 @@ int launch_ozaki_gemm(OzakiWorkspace* ws, int M, int N, int row0, int col0, doub
 // multipliers only for the others).  perm_out[0..v) = LAPACK-equivalent winners (row index chosen at step j,
 // identity beyond min(n, v)); see panel.cu for the tie-breaking contract.
 struct PanelWorkspace {
-    void* slot_hdr;     // [2][148][4]  LL words (payload32, epoch)
-    void* slot_rows;    // [2][148][64] LL words
+    void* slot_hdr;     // [2][132][4]  LL words (payload32, epoch)
+    void* slot_rows;    // [2][132][64] LL words
     long long* dbg;     // [8] cycle counters of CTA 0 of the last launch (profiling aid)
     int epoch;          // host-side running epoch (monotonic across launches)
-    int max_ctas;       // co-resident CTA budget (<= 148)
+    int max_ctas;       // co-resident CTA budget (<= 132)
     int cta_cap;        // optional cap on the grid (look-ahead: leave SMs to the trailing update); 0 = none
     // column-owner kernel for panels of <= 1024 rows (tournament stacks)
     unsigned* sk_flags;  // [1024] epoch of the last publication of column block b

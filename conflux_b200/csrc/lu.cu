@@ -1,8 +1,8 @@
-// conflux_b200/csrc/lu.cu -- host orchestration of the CONFLUX LU step loop on B200 + the C ABI.
+// conflux_b200/csrc/lu.cu -- host orchestration of the CONFLUX LU step loop on H100 + the C ABI.
 //
 // One rank = one GPU = one host thread/process (SPMD, like the reference's MPI ranks).  The step order follows
 // conflux::LU_rep<T> (/root/reference/src/conflux/lu/conflux_opt.hpp:535-1803, blueprint in SURVEY.md appendix A)
-// but the data layout and the division of labour are B200-first:
+// but the data layout and the division of labour are GPU-first:
 //   * A11 stays resident in HBM (row-major Ml x Nl, 64-bit indexing); L and U are written IN PLACE into it
 //     (the reference keeps a second Ml x Nl array A10resultBuff + a caller-owned C and MPI_Puts into it);
 //   * panels are kept transposed/K-major (see gemm.cu, panel.cu) so every kernel streams contiguous rows;
@@ -283,7 +283,7 @@ int panel_phase(cflx_lu* lu, int k, int fnpr, cudaStream_t s) {
     return CFLX_OK;
 }
 
-// digit planes of the operands of this step's trailing update (int8 tcgen05 path): L^T slab of this layer, U slab columns
+// digit planes of the operands of this step's trailing update (int8 wgmma path): L^T slab of this layer, U slab columns
 int ozaki_planes_a(cflx_lu* lu, int n_act, int64_t ld2, cudaStream_t s) {
     if (!lu->use_ozaki || n_act <= 0) return CFLX_OK;
     PhaseTimer t(lu, RG_step6_dgemm, s);
@@ -483,7 +483,7 @@ int finish_step(cflx_lu* lu, int k, int& fnpr) {
         }
         if (split_u) CFLX_TRY(store_factors());
         if (split_u && n_act > 0) CFLX_TRY(ozaki_planes_b(lu, w, ncols - w, ldu, s));
-        // the persistent tcgen05 kernel leaves the SMs of the concurrent pivot search alone
+        // the persistent int8 kernel leaves the SMs of the concurrent pivot search alone
         const int leave = (side && lu->use_ozaki) ? lu->pws.cta_cap : 0;
         CFLX_TRY(trailing_gemm(lu, k, 1, fnpr, n_act, c0 + w, ncols - w, ld2, ldu, w, s, leave > 0 ? lu->oz.sms - leave : 0));
         if (side) CFLX_CUDA(cudaStreamWaitEvent(s, lu->ev_join, 0));
@@ -524,7 +524,7 @@ void free_lu(cflx_lu* lu) {
 extern "C" {
 
 const char* cflx_last_error(void) { return g_err; }
-const char* cflx_version(void) { return "conflux_b200 0.1 (sm_100a)"; }
+const char* cflx_version(void) { return "conflux_b200 0.1 (sm_90a)"; }
 
 int cflx_device_count(int* count) {
     int n = 0;
@@ -731,10 +731,12 @@ int cflx_lu_create(cflx_comm* c, int M, int N, int v, int Px, int Py, int Pz, cf
     if ((rc = panel_workspace_create(&lu->pws))) return fail(rc);
     if ((rc = gemm_tn_setup())) return fail(rc);
     {
-        // Trailing update on the int8 tcgen05 path (ozaki.cu) whenever the layer's contraction length is a whole number
-        // of 128-element k chunks (v = 256 / 512 of the BASELINE configs); CFLX_GEMM=dmma selects the FP64 DMMA anchor.
+        // Trailing update: the FP64 DMMA kernel (gemm.cu).  On H100 the FP64 tensor rate (67 TFLOP/s) is above what
+        // the int8 digit-plane path can reach (989 int8 TMAC/s / 36 plane products = 55 TFLOP/s FP64-equivalent), so the
+        // int8 wgmma path (ozaki.cu) runs only on request, CFLX_GEMM=ozaki, where the layer's contraction length is a
+        // whole number of 128-element k chunks.
         const char* e = getenv("CFLX_GEMM");
-        const bool want = !(e && !strcmp(e, "dmma"));
+        const bool want = e && !strcmp(e, "ozaki");
         if (want && lu->nlayr % 128 == 0 && lu->nlayr <= 512) {
             if ((rc = ozaki_workspace_create(&lu->oz, lu->Ml, lu->Nl, lu->nlayr))) return fail(rc);
             lu->use_ozaki = true;
@@ -756,8 +758,8 @@ int cflx_lu_create(cflx_comm* c, int M, int N, int v, int Px, int Py, int Pz, cf
             if (cudaEventCreateWithFlags(&lu->ev_fork, cudaEventDisableTiming) != cudaSuccess) return fail(CFLX_ERR_CUDA);
             if (cudaEventCreateWithFlags(&lu->ev_join, cudaEventDisableTiming) != cudaSuccess) return fail(CFLX_ERR_CUDA);
             const char* c = getenv("CFLX_PANEL_CTAS");
-            // measured: 1x1x1 (C2) 32 -> 96.9 ms, 48 -> 96.7, 64 -> 102.6; 2x2x1 (C3) 48 -> 308 ms, 64 -> 283, 96 -> 309;
-            // 1x1x2 was measured at 48 only (no tournament there, the trailing update is twice as large per rank)
+            // SMs of the look-ahead pivot search: fewer on one GPU (no tournament), more where the tournament exchanges
+            // sit on the critical path; CFLX_PANEL_CTAS overrides
             lu->pws.cta_cap = c ? atoi(c) : (lu->P == 1 ? 32 : (lu->Px == 1 ? 48 : 64));
         }
     }
@@ -989,7 +991,7 @@ int cflx_host_free(void* p) {
     return CFLX_OK;
 }
 
-int cflx_lu_uses_tcgen05(const cflx_lu* lu) { return lu && lu->use_ozaki ? 1 : 0; }
+int cflx_lu_uses_ozaki(const cflx_lu* lu) { return lu && lu->use_ozaki ? 1 : 0; }
 int cflx_lu_launch_count(cflx_lu* lu, int64_t* count_out, int reset) {
     if (!lu || !count_out) return CFLX_ERR_ARG;
     *count_out = lu->launches;

@@ -76,7 +76,7 @@ struct cflx_lu {
         *tagsS = nullptr, *hist = nullptr, *plan_mem = nullptr, *idx_buf = nullptr;
     cflx::MovePlan plan{};
     cflx::PanelWorkspace pws{};
-    cflx::OzakiWorkspace oz{};   // digit planes of the int8 tcgen05 trailing update (CFLX_GEMM=ozaki)
+    cflx::OzakiWorkspace oz{};   // digit planes of the int8 wgmma trailing update (CFLX_GEMM=ozaki)
     bool use_ozaki = false;
     int64_t ldp_max = 0;
     int* h_npiv = nullptr;  // pinned

@@ -1,31 +1,29 @@
-// conflux_b200/csrc/ozaki.cu -- the trailing update  C -= L * U  on the 5th-generation tensor cores (tcgen05, int8).
+// conflux_b200/csrc/ozaki.cu -- the trailing update  C -= L * U  as exact int8 tensor-core products (Hopper wgmma).
 //
-// Replaces cblas_dgemm at /root/reference/src/conflux/lu/conflux_opt.hpp:1628-1632 on the path selected by
-// CFLX_GEMM=ozaki (gemm.cu's DMMA kernel stays the anchor and serves the TRSM sweeps).  tcgen05.mma has no f64 kind, so
-// FP64 accuracy is recovered with error-free slicing (Ozaki scheme):
+// Replaces cblas_dgemm at conflux_opt.hpp:1628-1632 of the reference on the path selected by CFLX_GEMM=ozaki (gemm.cu's
+// FP64 DMMA kernel is the default trailing update on H100 and serves the TRSM sweeps).  wgmma has no f64 kind, so FP64
+// accuracy is recovered with error-free slicing (Ozaki scheme):
 //   * every row m of L and every column n of U gets ONE power-of-two scale 2^ea[m] / 2^eb[n] (its largest magnitude);
 //   * the scaled entries are cut into S = 8 signed digits (first 6 bits, then 7 bits each, round-to-nearest so every
 //     digit fits [-64, 64]): x = 2^(e-6) * sum_s d_s 2^(-7s), exact to 55 bits relative to the row/column maximum;
 //   * every digit-plane product  sum_k da_s[m][k] * db_t[k][n]  is an EXACT int8 x int8 -> int32 GEMM
-//     (tcgen05.mma.kind::i8, accumulators in tensor memory); the planes with s + t = g share one accumulator (their
+//     (wgmma.mma_async .s32.s8.s8, accumulators in registers); the planes with s + t = g share one accumulator (their
 //     weight 2^(-7g) is the same; at most 8 products of <= 2^12 * K, K <= 512: < 2^25), only g <= 7 is kept (36 MMAs);
-//   * the epilogue recombines  sum_g 2^(-7g) acc_g  in FP64, applies 2^(ea+eb-12) and subtracts from C in place.
+//   * the epilogue recombines  sum_g 2^(-7g) acc_g  in FP64 in the order g = 0, 1, ..., 7, applies 2^(ea+eb-12) and
+//     subtracts from C in place.
 // The neglected planes (g >= 8) are below 2^-56 of |row max| * |column max| per term: the same order as the rounding of
 // a native FP64 dot product of that length (tools/ozaki_study.py: residual and pivots unchanged at 8 slices).
 //
-// Kernel structure (one CTA per SM, 640 threads, all 512 TMEM columns):
-//   warp 0     TMA producer: digit planes are K-major int8 ([plane][row][K], 128-byte swizzled boxes of 128 k) fetched
-//              with cp.async.bulk.tensor.3d through two tensor maps; per 128-k chunk the 8 B planes stay resident
-//              (double-buffered set, ONE barrier pair per set) while the 8 A planes stream through a ring of three
-//              two-plane slots: every plane chunk is loaded exactly once per tile;
-//   warp 1     MMA issuer: one thread, UMMA 128 x (64..256) x 32 (up to four B planes per instruction), smem descriptors (SWIZZLE_128B, K-major), tcgen05.commit
-//              onto the mbarriers that free operand slots and publish finished accumulators;
-//   warp 2     TMEM allocation / release;
-//   warps 4-19 epilogue: tcgen05.ld 16x256b (accumulator-fragment layout), software-pipelined int32 -> FP64 recombination in
-//              registers; the negated update is staged in shared memory and ADDED to C by the L2 through bulk reduce
-//              operations (cp.reduce.async.bulk .add.f64, SASS UBLKRED): the SM never reads C.
-// The 8 accumulators are the pipeline between MMA and epilogue: the epilogue drains group g while the MMAs of the later
-// groups still run, and the C update of a tile overlaps the MMAs of the next one.
+// Kernel structure (one CTA per SM, 2 consumer warpgroups + 1 producer warp, CTA tile 128 x 64):
+//   warp 8         TMA producer: digit planes are K-major int8 ([plane][row][K], 64-byte swizzled boxes of 64 k) fetched
+//                  with cp.async.bulk.tensor.3d through two tensor maps into a two-stage ring; one stage holds one 64-k
+//                  chunk of every plane the current pass needs, for both operands;
+//   warps 0-7      two warpgroups, 64 rows of the tile each.  The 8 groups are accumulated in passes of OZ_GP groups
+//                  (int32 registers: OZ_GP x 32 per thread); after each pass the finished groups are folded into the
+//                  FP64 running sum in group order, so the recombination is the same sequence of roundings as a single
+//                  pass.  The B planes t, t+1, ... of a stage are contiguous 64-row tiles and the accumulators of their
+//                  groups are contiguous registers: all planes of one A_s in the pass go through ONE wgmma of
+//                  N = 64 * planes, so A_s is read from shared memory once per pass and k step.
 #include <cuda.h>
 
 #include <algorithm>
@@ -38,16 +36,17 @@
 namespace cflx {
 
 namespace {
-constexpr int OZ_S = 8;           // digit planes per operand
-constexpr int OZ_BM = 128, OZ_BN = 64, OZ_KC = 128;  // CTA tile, k-chunk (bytes = int8 elements)
-constexpr int OZ_A_SLOTS = 2;      // each slot holds TWO consecutive A planes (one full/empty barrier pair per two rows)
-constexpr int OZ_A_BYTES = OZ_BM * OZ_KC, OZ_B_BYTES = OZ_BN * OZ_KC;
-constexpr int OZ_A_SLOT_BYTES = 2 * OZ_A_BYTES;
-constexpr int OZ_EPI_WARPS = 16;  // 4 per TMEM lane quadrant, 16 columns each
-constexpr int OZ_THREADS = 128 + 32 * OZ_EPI_WARPS;
-constexpr size_t OZ_SMEM_OPERANDS = (size_t)2 * OZ_S * OZ_B_BYTES + (size_t)OZ_A_SLOTS * OZ_A_SLOT_BYTES;
-constexpr int OZ_STAGE_DOUBLES = 16 * OZ_BN;   // per TMEM lane quadrant: 16 rows x 64 columns of (-update), source of the bulk reduce-add
-constexpr size_t OZ_SMEM = 1024 /*alignment slack*/ + OZ_SMEM_OPERANDS + (size_t)4 * OZ_STAGE_DOUBLES * sizeof(double) + 512 /*barriers*/;
+constexpr int OZ_S = 8;                               // digit planes per operand
+constexpr int OZ_BM = 128, OZ_BN = 64, OZ_KC = 64;    // CTA tile, k-chunk of a pipeline stage (bytes = int8 elements)
+constexpr int OZ_GP = 3;                              // accumulator groups per pass
+constexpr int OZ_NPASS = (OZ_S + OZ_GP - 1) / OZ_GP;
+constexpr int OZ_STAGES = 2;
+constexpr int OZ_A_BYTES = OZ_BM * OZ_KC, OZ_B_BYTES = OZ_BN * OZ_KC;   // one plane of one stage
+constexpr int OZ_STAGE_BYTES = OZ_S * (OZ_A_BYTES + OZ_B_BYTES);
+constexpr int OZ_CONS_WARPS = 8;
+constexpr int OZ_THREADS = 32 * OZ_CONS_WARPS + 32;
+constexpr size_t OZ_SMEM = 1024 /*alignment slack*/ + (size_t)OZ_STAGES * OZ_STAGE_BYTES + 64 /*barriers*/;
+constexpr int OZ_SPLIT_KC = 128;                      // k-chunk of the digit-plane split (K is a multiple of it)
 
 // ---------------------------------------------------------------------------------------------- PTX wrappers
 __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* map, int c0, int c1, int c2, uint64_t* bar) {
@@ -57,86 +56,62 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
         "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar))
         : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+// shared-memory matrix descriptor of a K-major, 64-byte-swizzled operand tile (rows of 64 bytes, 8-row groups 512 B
+// apart): start address >> 4 | LBO (unused for swizzled K-major) = 1 at bit 16 | SBO = 512 >> 4 at bit 32 |
+// SWIZZLE_64B (2) at bit 62.  Stepping 32 bytes along K inside the swizzle atom adds 2 to the start address field.
+__device__ __forceinline__ uint64_t smem_desc_sw64(uint32_t saddr) {
+    return (uint64_t)((saddr & 0x3FFFF) >> 4) | (1ull << 16) | ((uint64_t)(512 >> 4) << 32) | (2ull << 62);
 }
-// D(tmem) (+)= A(smem desc) * B(smem desc), int8 x int8 -> int32
-__device__ __forceinline__ void umma_i8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// D(64 x n, int32 registers in the wgmma accumulator layout) += A(64 x 32, smem desc) * B(32 x n, smem desc), int8.
+// Accumulator layout (thread T of the warpgroup, warp w = T / 32, lane l): d[4j + 2h + x] is row 16w + l/4 + 8h,
+// column 8j + 2(l%4) + x.
+__device__ __forceinline__ void wgmma_s8_n64(int* d, uint64_t da, uint64_t db) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p;\n\t}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+        : "l"(da), "l"(db), "r"(1)
         : "memory");
 }
-// same, descriptors given as (low word, shared high word); ACC = true: D += A*B unconditionally
-template <bool ACC>
-__device__ __forceinline__ void umma_i8_lo(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t hi, uint32_t idesc, uint32_t accumulate) {
-    if constexpr (ACC) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-            "mov.b64 da, {%1, %3};\n\tmov.b64 db, {%2, %3};\n\t"
-            "setp.eq.u32 p, 0, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::i8 [%0], da, db, %4, p;\n\t}" ::"r"(tmem_d),
-            "r"(a_lo), "r"(b_lo), "r"(hi), "r"(idesc)
-            : "memory");
-    } else {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-            "mov.b64 da, {%1, %3};\n\tmov.b64 db, {%2, %3};\n\t"
-            "setp.ne.b32 p, %5, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::i8 [%0], da, db, %4, p;\n\t}" ::"r"(tmem_d),
-            "r"(a_lo), "r"(b_lo), "r"(hi), "r"(idesc), "r"(accumulate)
-            : "memory");
-    }
-}
-// 16 TMEM lanes x 16 columns in the accumulator-fragment layout (shape 16x256b, two 8-column repeats): thread T receives
-//   r[4*c8 + 0..1] = lane T/4,     columns 8*c8 + 2*(T%4) + {0, 1}
-//   r[4*c8 + 2..3] = lane T/4 + 8, same columns
-// i.e. four lanes cover one 64-byte row segment of 8 int32 -- the mapping a coalesced C access wants.
-__device__ __forceinline__ void tmem_ld_frag16(uint32_t taddr, int (&r)[8]) {
-    asm volatile("tcgen05.ld.sync.aligned.16x256b.x2.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, int (&r)[16]) {  // lane = thread, 16 consecutive columns
+__device__ __forceinline__ void wgmma_s8_n128(int* d, uint64_t da, uint64_t db) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p;\n\t}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+        : "l"(da), "l"(db), "r"(1)
         : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
 }
-// shared-memory matrix descriptor of a K-major, 128-byte-swizzled operand tile (rows of 128 bytes, 8-row groups 1024 B
-// apart): start address >> 4 | SBO = 1024 >> 4 at bit 32 | version 1 at bit 46 | SWIZZLE_128B (2) at bit 61
-__device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t saddr) {
-    return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
+__device__ __forceinline__ void wgmma_s8_n192(int* d, uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %98, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n192k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}, %96, %97, p;\n\t}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63]), "+r"(d[64]), "+r"(d[65]), "+r"(d[66]), "+r"(d[67]), "+r"(d[68]), "+r"(d[69]), "+r"(d[70]), "+r"(d[71]), "+r"(d[72]), "+r"(d[73]), "+r"(d[74]), "+r"(d[75]), "+r"(d[76]), "+r"(d[77]), "+r"(d[78]), "+r"(d[79]), "+r"(d[80]), "+r"(d[81]), "+r"(d[82]), "+r"(d[83]), "+r"(d[84]), "+r"(d[85]), "+r"(d[86]), "+r"(d[87]), "+r"(d[88]), "+r"(d[89]), "+r"(d[90]), "+r"(d[91]), "+r"(d[92]), "+r"(d[93]), "+r"(d[94]), "+r"(d[95])
+        : "l"(da), "l"(db), "r"(1)
+        : "memory");
 }
-// instruction descriptor, kind::i8: D = S32 (2 at bit 4), A = B = signed int8 (1 at bits 7 / 10), both K-major,
-// N >> 3 at bit 17, M >> 4 at bit 24
-__host__ __device__ constexpr uint32_t oz_idesc(int n) {
-    return (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(OZ_BM >> 4) << 24);
+__device__ __forceinline__ void wgmma_s8_n256(int* d, uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p;\n\t}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63]), "+r"(d[64]), "+r"(d[65]), "+r"(d[66]), "+r"(d[67]), "+r"(d[68]), "+r"(d[69]), "+r"(d[70]), "+r"(d[71]), "+r"(d[72]), "+r"(d[73]), "+r"(d[74]), "+r"(d[75]), "+r"(d[76]), "+r"(d[77]), "+r"(d[78]), "+r"(d[79]), "+r"(d[80]), "+r"(d[81]), "+r"(d[82]), "+r"(d[83]), "+r"(d[84]), "+r"(d[85]), "+r"(d[86]), "+r"(d[87]), "+r"(d[88]), "+r"(d[89]), "+r"(d[90]), "+r"(d[91]), "+r"(d[92]), "+r"(d[93]), "+r"(d[94]), "+r"(d[95]), "+r"(d[96]), "+r"(d[97]), "+r"(d[98]), "+r"(d[99]), "+r"(d[100]), "+r"(d[101]), "+r"(d[102]), "+r"(d[103]), "+r"(d[104]), "+r"(d[105]), "+r"(d[106]), "+r"(d[107]), "+r"(d[108]), "+r"(d[109]), "+r"(d[110]), "+r"(d[111]), "+r"(d[112]), "+r"(d[113]), "+r"(d[114]), "+r"(d[115]), "+r"(d[116]), "+r"(d[117]), "+r"(d[118]), "+r"(d[119]), "+r"(d[120]), "+r"(d[121]), "+r"(d[122]), "+r"(d[123]), "+r"(d[124]), "+r"(d[125]), "+r"(d[126]), "+r"(d[127])
+        : "l"(da), "l"(db), "r"(1)
+        : "memory");
 }
 
-// C[...] += smem[...] (FP64, round-to-nearest) done by the L2 through the TMA engine (SASS UBLKRED.ADD.F64): no C load, no
-// load latency on the SM; bytes a multiple of 16, both addresses 16-byte aligned
-__device__ __forceinline__ void bulk_reduce_add_f64(double* gdst, const double* ssrc, uint32_t bytes) {
-    asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f64 [%0], [%1], %2;" ::"l"(gdst), "r"(smem_u32(ssrc)), "r"(bytes)
-                 : "memory");
+// acc[0 .. 32 * planes) += A * (planes consecutive B tiles of 64 rows)
+template <int PLANES>
+__device__ __forceinline__ void wgmma_s8(int* acc, uint64_t da, uint64_t db) {
+    if constexpr (PLANES == 1) wgmma_s8_n64(acc, da, db);
+    else if constexpr (PLANES == 2) wgmma_s8_n128(acc, da, db);
+    else if constexpr (PLANES == 3) wgmma_s8_n192(acc, da, db);
+    else wgmma_s8_n256(acc, da, db);
 }
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void l2_prefetch_128(const void* p) {  // 16-byte aligned, 128 bytes
-    asm volatile("cp.async.bulk.prefetch.L2.global [%0], 128;" ::"l"(p) : "memory");
-}
+
 __host__ __device__ constexpr double pow2c(int e) {  // compile-time 2^e, e <= 0
     double x = 1.0;
     for (int i = 0; i < -e; ++i) x *= 0.5;
@@ -153,301 +128,164 @@ struct OzArgs {
     const int* ea;         // [M]   row exponents of A
     const int* eb;         // [...] column exponents of B, indexed like the B planes (b_row0 + n)
     int tiles_m, tiles_n;
-    long long* dbg;        // optional [16] cycle counters of CTA 0: see cflx_dbg_ozaki_cycles
 };
 
-template <bool DBG>
+// the plane products of groups [G0, G0 + OZ_GP) for one 64-k chunk held in one stage: for every A plane s, the B planes
+// t = max(0, G0 - s) .. G1 - s in one instruction (their groups s + t are consecutive accumulators)
+template <int G0, int S>
+__device__ __forceinline__ void pass_products(int* acc, uint32_t a_base, uint32_t b_base) {
+    constexpr int G1 = (G0 + OZ_GP < OZ_S ? G0 + OZ_GP : OZ_S) - 1;
+    if constexpr (S <= G1) {
+        constexpr int T_LO = G0 - S > 0 ? G0 - S : 0;
+        constexpr int PLANES = G1 - S - T_LO + 1;
+#pragma unroll
+        for (int k = 0; k < OZ_KC / 32; ++k)
+            wgmma_s8<PLANES>(acc + 32 * (S + T_LO - G0), smem_desc_sw64(a_base + S * OZ_A_BYTES + 32 * k),
+                             smem_desc_sw64(b_base + T_LO * OZ_B_BYTES + 32 * k));
+        pass_products<G0, S + 1>(acc, a_base, b_base);
+    }
+}
+
+template <int P>
+__device__ __forceinline__ void consume_pass(const OzArgs& g, uint64_t* full, uint64_t* empty, uint32_t sbase, int wg, int lane,
+                                             uint32_t& q, double (&sum)[32]) {
+    if constexpr (P < OZ_NPASS) {
+        constexpr int G0 = P * OZ_GP;
+        constexpr int NG = (G0 + OZ_GP < OZ_S ? OZ_GP : OZ_S - G0);
+        int acc[OZ_GP * 32];
+#pragma unroll
+        for (int i = 0; i < OZ_GP * 32; ++i) acc[i] = 0;
+        const int KC = g.K / OZ_KC;
+        for (int kc = 0; kc < KC; ++kc, ++q) {
+            const int st = q % OZ_STAGES;
+            mbar_wait(&full[st], (q / OZ_STAGES) & 1);
+            const uint32_t a_base = sbase + st * OZ_STAGE_BYTES + wg * (64 * OZ_KC);   // rows 64 wg .. of every A plane
+            const uint32_t b_base = sbase + st * OZ_STAGE_BYTES + OZ_S * OZ_A_BYTES;
+            wgmma_fence();
+            pass_products<G0, 0>(acc, a_base, b_base);
+            wgmma_commit();
+            wgmma_wait<0>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[st]);                  // this warp is done with the stage
+        }
+#pragma unroll
+        for (int gi = 0; gi < NG; ++gi) {
+            const double w = pow2c(-7 * (G0 + gi));
+#pragma unroll
+            for (int i = 0; i < 32; ++i) {
+                // exact int32 -> double without the conversion pipe: 2^52 + 2^31 + x, then subtract the bias
+                const double x = __hiloint2double(0x43300000, acc[32 * gi + i] ^ 0x80000000) - 4503601774854144.0;
+                sum[i] = fma(x, w, sum[i]);
+            }
+        }
+        consume_pass<P + 1>(g, full, empty, sbase, wg, lane, q, sum);
+    }
+}
+
 __global__ void __launch_bounds__(OZ_THREADS, 1)
 ozaki_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, OzArgs g) {
     extern __shared__ unsigned char oz_smem_raw[];
     unsigned char* base = reinterpret_cast<unsigned char*>(((uintptr_t)oz_smem_raw + 1023) & ~(uintptr_t)1023);
-    unsigned char* sB = base;                                        // [2][8][64 x 128 B]
-    unsigned char* sA = base + (size_t)2 * OZ_S * OZ_B_BYTES;         // [3][128 x 128 B]
-    double* stage = reinterpret_cast<double*>(base + OZ_SMEM_OPERANDS);   // [4 lane quadrants][16 rows][64 columns]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(stage + 4 * OZ_STAGE_DOUBLES);
-    uint64_t* fullB = bars;                 // [2]  one per B set (8 planes land on it)
-    uint64_t* emptyB = bars + 2;            // [2]
-    uint64_t* fullA = bars + 4;             // [2..3]  one per A slot (2 planes)
-    uint64_t* emptyA = bars + 7;            // [2..3]
-    uint64_t* tfull = bars + 10;            // [8]  accumulator (group) g is complete
-    uint64_t* tdone = bars + 18;            // [1]  the epilogue has drained all 8 accumulators of the tile
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 20);
+    // stage st: A planes [8][128 rows][64 B], then B planes [8][64 rows][64 B]
+    uint64_t* full = reinterpret_cast<uint64_t*>(base + (size_t)OZ_STAGES * OZ_STAGE_BYTES);
+    uint64_t* empty = full + OZ_STAGES;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int ntiles = g.tiles_m * g.tiles_n;
     const int KC = g.K / OZ_KC;
 
     if (threadIdx.x == 0) {
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&fullB[i], 1);
-            mbar_init(&emptyB[i], 1);
+        for (int i = 0; i < OZ_STAGES; ++i) {
+            mbar_init(&full[i], 1);
+            mbar_init(&empty[i], OZ_CONS_WARPS);
         }
-        for (int i = 0; i < OZ_A_SLOTS; ++i) {
-            mbar_init(&fullA[i], 1);
-            mbar_init(&emptyA[i], 1);
-        }
-        for (int i = 0; i < OZ_S; ++i) mbar_init(&tfull[i], 1);
-        mbar_init(tdone, OZ_EPI_WARPS);  // one arrival per epilogue warp
         fence_barrier_init();
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(tmem_slot)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    long long tm[4] = {0, 0, 0, 0};
-    long long tc0 = 0;
-#define OZ_T0() if constexpr (DBG) tc0 = clock64();
-#define OZ_T1(i) if constexpr (DBG) tm[i] += clock64() - tc0;
-    const long long t_begin = DBG ? clock64() : 0;
-    if (warp == 0) {
+    if (warp == OZ_CONS_WARPS) {
         // ================================================================== TMA producer
-        uint32_t q = 0, acnt = 0;  // k-chunks and A slots (plane pairs) loaded so far by this CTA
-        for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-            const int m0 = (tile / g.tiles_n) * OZ_BM, n0 = (tile % g.tiles_n) * OZ_BN;
-            for (int kc = 0; kc < KC; ++kc, ++q) {
-                const int set = q & 1;
-                const uint32_t useB = q >> 1;
-                OZ_T0() mbar_wait(&emptyB[set], (useB & 1) ^ 1); OZ_T1(0)
-                if (lane == 0) {
-                    mbar_arrive_expect_tx(&fullB[set], OZ_S * OZ_B_BYTES);
-                    for (int t = 0; t < OZ_S; ++t)
-                        tma_load_3d(sB + (size_t)(set * 8 + t) * OZ_B_BYTES, &mapB, kc * OZ_KC, g.b_row0 + n0, t, &fullB[set]);
-                }
-                for (int sp = 0; sp < OZ_S / 2; ++sp, ++acnt) {
-                    const int slot = acnt % OZ_A_SLOTS;
-                    const uint32_t useA = acnt / OZ_A_SLOTS;
-                    OZ_T0() mbar_wait(&emptyA[slot], (useA & 1) ^ 1); OZ_T1(1)
-                    if (lane == 0) {
-                        mbar_arrive_expect_tx(&fullA[slot], OZ_A_SLOT_BYTES);
-                        tma_load_3d(sA + (size_t)slot * OZ_A_SLOT_BYTES, &mapA, kc * OZ_KC, g.a_row0 + m0, 2 * sp, &fullA[slot]);
-                        tma_load_3d(sA + (size_t)slot * OZ_A_SLOT_BYTES + OZ_A_BYTES, &mapA, kc * OZ_KC, g.a_row0 + m0, 2 * sp + 1, &fullA[slot]);
-                    }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ================================================================== MMA issuer
-        // One CTA per SM owns all 512 TMEM columns, so the allocation starts at column 0 and every accumulator address is
-        // a compile-time constant; the plane loop is fully unrolled so that each UMMA is issued from immediates + two
-        // descriptor low words (the issue path of this single thread is what the tensor pipe waits for).
-        if (tmem_base != 0) __trap();
-        const uint32_t sA0 = smem_u32(sA), sB0 = smem_u32(sB);
-        constexpr uint32_t DESC_HI = (uint32_t)((((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61)) >> 32);
-        uint32_t q = 0, acnt = 0, it = 0;
-        for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-            for (int kc = 0; kc < KC; ++kc, ++q) {
-                const int set = q & 1;
-                const uint32_t useB = q >> 1;
-                const uint32_t b_lo = ((sB0 + (uint32_t)set * 8u * OZ_B_BYTES) & 0x3FFFF) >> 4;
-                OZ_T0() mbar_wait(&fullB[set], useB & 1); OZ_T1(1)
-                OZ_T0() if (kc == 0) mbar_wait(tdone, (it & 1) ^ 1); OZ_T1(2)   // the epilogue drained the previous tile
-#pragma unroll
-                for (int sp = 0; sp < OZ_S / 2; ++sp, ++acnt) {
-                    const int slot = acnt % OZ_A_SLOTS;
-                    OZ_T0() mbar_wait(&fullA[slot], (acnt / OZ_A_SLOTS) & 1); OZ_T1(0)
-                    tc_fence_after();
-                    if (lane == 0) {
-#pragma unroll
-                        for (int half = 0; half < 2; ++half) {
-                            const int s = 2 * sp + half;
-                            const uint32_t a_lo = ((sA0 + (uint32_t)slot * OZ_A_SLOT_BYTES + (uint32_t)half * OZ_A_BYTES) & 0x3FFFF) >> 4;
-                            // The B planes t, t+1, ... of a set are contiguous 64-row tiles and their accumulators (groups
-                            // s+t, s+t+1, ...) are contiguous 64-column blocks of tensor memory: up to four planes go through
-                            // ONE UMMA of N = 64 * planes, so A_s is read from shared memory once per four products.
-#pragma unroll
-                            for (int t = 0; t < OZ_S - s; t += 4) {
-                                const int np = (OZ_S - s - t) < 4 ? (OZ_S - s - t) : 4;
-                                const uint32_t bt_lo = b_lo + (uint32_t)t * (OZ_B_BYTES >> 4);
-                                const uint32_t d = (uint32_t)(s + t) * OZ_BN;
-#pragma unroll
-                                for (int k = 0; k < OZ_KC / 32; ++k) {  // +32 bytes along K inside the swizzle atom: +2 in the descriptor
-                                    if (s == 0 && k == 0) umma_i8_lo<false>(d, a_lo, bt_lo, DESC_HI, oz_idesc(np * OZ_BN), kc > 0 ? 1u : 0u);
-                                    else umma_i8_lo<true>(d, a_lo + 2 * k, bt_lo + 2 * k, DESC_HI, oz_idesc(np * OZ_BN), 1u);
-                                }
-                            }
-                            if (kc == KC - 1) tc_commit(&tfull[s]);       // groups <= s are complete
+        if (lane == 0) {
+            uint32_t q = 0;  // stage fills issued so far by this CTA
+            for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+                const int m0 = (tile / g.tiles_n) * OZ_BM, n0 = (tile % g.tiles_n) * OZ_BN;
+                for (int p = 0; p < OZ_NPASS; ++p) {
+                    const int np = (p + 1) * OZ_GP < OZ_S ? (p + 1) * OZ_GP : OZ_S;   // the pass needs planes 0 .. np-1 of both operands
+                    for (int kc = 0; kc < KC; ++kc, ++q) {
+                        const int st = q % OZ_STAGES;
+                        const uint32_t use = q / OZ_STAGES;
+                        if (use > 0) mbar_wait(&empty[st], (use - 1) & 1);
+                        unsigned char* sa = base + (size_t)st * OZ_STAGE_BYTES;
+                        unsigned char* sb = sa + OZ_S * OZ_A_BYTES;
+                        mbar_arrive_expect_tx(&full[st], (uint32_t)(np * (OZ_A_BYTES + OZ_B_BYTES)));
+                        for (int t = 0; t < np; ++t) {
+                            tma_load_3d(sa + t * OZ_A_BYTES, &mapA, kc * OZ_KC, g.a_row0 + m0, t, &full[st]);
+                            tma_load_3d(sb + t * OZ_B_BYTES, &mapB, kc * OZ_KC, g.b_row0 + n0, t, &full[st]);
                         }
-                        tc_commit(&emptyA[slot]);                         // planes 2sp, 2sp+1 of A are consumed
-                        if (sp == OZ_S / 2 - 1) tc_commit(&emptyB[set]);  // the whole B set of this k chunk is consumed
                     }
-                    __syncwarp();
                 }
             }
         }
-    } else if (warp >= 4) {
-        // ================================================================== epilogue (16 warps)
-        // warp -> TMEM lane quadrant lq (32 rows) x 16-column quarter cq.  The accumulators are read in the fragment layout
-        // (tmem_ld_frag16): thread T holds rows {T/4, T/4+8, T/4+16, T/4+24} x column pairs {2(T%4), 8+2(T%4)}, so four
-        // lanes cover a 64-byte row segment and the C read-modify-write needs no shared-memory transpose.
-        const int ew = warp - 4;
-        const int lq = warp & 3;
-        const int cq = ew >> 2;
-        const int cp = lane & 3, r8 = lane >> 2;
-        uint32_t it = 0;
-        for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-            const int m0 = (tile / g.tiles_n) * OZ_BM, n0 = (tile % g.tiles_n) * OZ_BN;
-            {   // pull my row's 128-byte segment of the C tile into L2 now; it is needed after the 8 accumulators
-                const int prow = m0 + lq * 32 + lane, pcol = n0 + cq * 16;
-                if (prow < g.M && pcol + 16 <= g.N) l2_prefetch_128(g.C + (int64_t)prow * g.ldc + pcol);
+        return;
+    }
+
+    // ====================================================================== consumers (two warpgroups)
+    const int wg = warp >> 2;
+    const uint32_t sbase = smem_u32(base);
+    uint32_t q = 0;
+    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+        const int m0 = (tile / g.tiles_n) * OZ_BM, n0 = (tile % g.tiles_n) * OZ_BN;
+        double sum[32];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) sum[i] = 0.0;
+        consume_pass<0>(g, full, empty, sbase, wg, lane, q, sum);
+        // ---- C -= sum * 2^(ea - 12) * 2^eb, as C + (sum * -2^(ea - 12)) * 2^eb: each element has exactly one owner thread
+        const int r0 = m0 + 64 * wg + 16 * (warp & 3) + (lane >> 2);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = r0 + 8 * h;
+            if (row >= g.M) continue;
+            const double sr = -pow2i(g.ea[g.a_row0 + row] - 12);
+            double* crow = g.C + (int64_t)row * g.ldc;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int col = n0 + 8 * j + 2 * (lane & 3);
+                if (col >= g.N) continue;                              // N is even: col + 1 < N too
+                double2 c = *reinterpret_cast<const double2*>(crow + col);
+                c.x += (sum[4 * j + 2 * h] * sr) * pow2i(g.eb[g.b_row0 + col]);
+                c.y += (sum[4 * j + 2 * h + 1] * sr) * pow2i(g.eb[g.b_row0 + col + 1]);
+                *reinterpret_cast<double2*>(crow + col) = c;
             }
-            const int rowbase = m0 + lq * 32 + r8;             // my rows: rowbase + 8 * j, j = 0..3
-            const int colbase = n0 + cq * 16 + 2 * cp;          // my column pairs: colbase + 8 * c8
-            // exponents of my 4 rows and 4 columns (kept as ints: half the registers; the powers of two are rebuilt at use)
-            int erow[4], ecol[2][2];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) erow[j] = (rowbase + 8 * j < g.M) ? g.ea[g.a_row0 + rowbase + 8 * j] - 12 : 0;
-#pragma unroll
-            for (int c8 = 0; c8 < 2; ++c8) {
-                const int col = colbase + 8 * c8;
-                ecol[c8][0] = col < g.N ? g.eb[g.b_row0 + col] : 0;
-                ecol[c8][1] = col < g.N ? g.eb[g.b_row0 + col + 1] : 0;
-            }
-            // sum[h][i]: lane half h (rows 16h..16h+15 of the quadrant), i = 4*c8 + 2*rsel + x as delivered by tmem_ld_frag16
-            double sum[2][8];
-#pragma unroll
-            for (int h = 0; h < 2; ++h)
-#pragma unroll
-                for (int i = 0; i < 8; ++i) sum[h][i] = 0.0;
-            // 16 half-steps (group g, lane half h), two 8-register buffers: the TMEM load of the NEXT half-step is issued
-            // right after the current one has landed and BEFORE its FP64 work, so load latency and recombination overlap.
-            int acc[2][8];
-            const uint32_t ta0 = ((uint32_t)(lq * 32) << 16) + (uint32_t)(cq * 16);
-            OZ_T0() mbar_wait(&tfull[0], it & 1); OZ_T1(0)
-            tc_fence_after();
-            tmem_ld_frag16(ta0, acc[0]);
-#pragma unroll
-            for (int step = 0; step < 2 * OZ_S; ++step) {
-                const int grp = step >> 1, h = step & 1;
-                OZ_T0()
-                tmem_ld_wait();                                  // acc[step & 1] has landed
-                bool issued = true;
-                if (step + 1 < 2 * OZ_S) {
-                    const uint32_t tn = ta0 + (uint32_t)(((step + 1) >> 1) * OZ_BN) + ((uint32_t)(((step + 1) & 1) * 16) << 16);
-                    if (h == 0) {
-                        tmem_ld_frag16(tn, acc[(step + 1) & 1]);  // other lane half of the same group
-                    } else if (mbar_test(&tfull[grp + 1], it & 1)) {
-                        tc_fence_after();
-                        tmem_ld_frag16(tn, acc[(step + 1) & 1]);  // next group is already complete
-                    } else {
-                        issued = false;
-                    }
-                } else {
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(tdone);            // all 8 accumulators are in registers
-                }
-                const double w = pow2c(-7 * grp);
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    // exact int32 -> double without the conversion pipe: 2^52 + 2^31 + x, then subtract the bias
-                    const double x = __hiloint2double(0x43300000, acc[step & 1][i] ^ 0x80000000) - 4503601774854144.0;
-                    sum[h][i] = fma(x, w, sum[h][i]);
-                }
-                OZ_T1(1)
-                if (!issued) {
-                    OZ_T0() mbar_wait(&tfull[grp + 1], it & 1); OZ_T1(0)
-                    tc_fence_after();
-                    tmem_ld_frag16(ta0 + (uint32_t)((grp + 1) * OZ_BN), acc[(step + 1) & 1]);
-                }
-            }
-            OZ_T0()
-            // ---- C -= sum * 2^(ea - 12) * 2^eb: the NEGATED update is staged in shared memory (16 rows x 16 columns per lane
-            // half) and added to C by the L2 through a bulk reduce (one 128-byte row segment per lane): the SM never loads C
-            // (the rows were pulled into L2 by the prefetch at the top of the tile).
-            // The four warps of a lane quadrant share one 16-row x 64-column staging tile, so that ONE bulk reduce moves a whole
-            // 512-byte row segment (the TMA engine's cost is per operation: 128 operations per tile instead of 512).
-            double* stg = stage + (size_t)lq * OZ_STAGE_DOUBLES;
-            const int segcols = min(OZ_BN, g.N - n0);            // valid columns of the tile (even)
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                bulk_wait_read();                                 // my previous reduces have read their staging rows
-                named_bar_sync(1 + lq, 128);                      // ... and so have those of the other three warps
-#pragma unroll
-                for (int rsel = 0; rsel < 2; ++rsel) {
-                    const double sr = -pow2i(erow[2 * h + rsel]);
-#pragma unroll
-                    for (int c8 = 0; c8 < 2; ++c8) {
-                        double2 o;
-                        o.x = (sum[h][4 * c8 + 2 * rsel] * sr) * pow2i(ecol[c8][0]);
-                        o.y = (sum[h][4 * c8 + 2 * rsel + 1] * sr) * pow2i(ecol[c8][1]);
-                        *reinterpret_cast<double2*>(stg + (8 * rsel + r8) * OZ_BN + cq * 16 + 8 * c8 + 2 * cp) = o;
-                    }
-                }
-                fence_proxy_async();
-                named_bar_sync(1 + lq, 128);                      // the whole 16 x 64 tile is staged
-                if (lane < 4) {                                   // warp cq issues rows 4cq .. 4cq+3 of this half
-                    const int lr = 4 * cq + lane;
-                    const int r = m0 + lq * 32 + 16 * h + lr;
-                    if (r < g.M && segcols > 0)
-                        bulk_reduce_add_f64(g.C + (int64_t)r * g.ldc + n0, stg + lr * OZ_BN, (uint32_t)segcols * 8u);
-                    bulk_commit();
-                }
-            }
-            OZ_T1(2)
         }
     }
-    if (DBG && blockIdx.x == 0 && lane == 0 && (warp == 0 || warp == 1 || warp == 4)) {
-        const int o = warp == 0 ? 0 : (warp == 1 ? 4 : 8);
-        for (int i = 0; i < 3; ++i) g.dbg[o + i] = tm[i];
-        g.dbg[o + 3] = clock64() - t_begin;
-    }
-#undef OZ_T0
-#undef OZ_T1
-    if (warp >= 4) bulk_wait_all();   // every reduce-add of this thread has been performed
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
 }
 
-// ---------------------------------------------------------------------------------------------- raw UMMA rate probe
-// Back-to-back tcgen05.mma on one resident shared-memory tile per SM (no TMA, no epilogue): the tensor pipe's own rate
-// for kind::i8 (and kind::f16 for calibration against the bf16 peak in MEASURED_PEAKS.json).
-__global__ void __launch_bounds__(128, 1) umma_peak_kernel(int n, int use_f16, int iters) {
+// ---------------------------------------------------------------------------------------------- raw wgmma rate probe
+// Back-to-back wgmma m64 x n x 32 (int8) on resident shared-memory tiles, two warpgroups per CTA, one CTA per SM (no TMA,
+// no epilogue): the tensor cores' own int8 rate, the ceiling of the digit-plane GEMM.
+template <int PLANES>
+__global__ void __launch_bounds__(256, 1) wgmma_peak_kernel(int iters, int* sink) {
     extern __shared__ unsigned char pk_smem_raw[];
     unsigned char* base = reinterpret_cast<unsigned char*>(((uintptr_t)pk_smem_raw + 1023) & ~(uintptr_t)1023);
-    __shared__ uint64_t bar;
-    __shared__ uint32_t tslot;
-    for (int i = threadIdx.x; i < (16384 + 32768) / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(base)[i] = 0x01010101u * (i & 3);
-    if (threadIdx.x == 0) {
-        mbar_init(&bar, 1);
-        fence_barrier_init();
-    }
+    for (int i = threadIdx.x; i < (4096 + 16384) / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(base)[i] = 0x01010101u * (i & 3);
     fence_proxy_async();
-    if (threadIdx.x < 32) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(&tslot)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tb = tslot;
-    if (threadIdx.x == 0) {
-        const uint64_t adesc = smem_desc_sw128(smem_u32(base)), bdesc = smem_desc_sw128(smem_u32(base + 16384));
-        // f16 kind: D = F32 (1 at bit 4), A = B = BF16 (1 at bits 7 / 10); i8 kind as in the GEMM
-        const uint32_t idesc = use_f16 ? ((1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | (8u << 24)) : oz_idesc(n);
-        for (int it = 0; it < iters; ++it) {
+    int acc[32 * PLANES];
 #pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                if (use_f16)
-                    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                                 "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tb + (uint32_t)((it & 1) * 256)),
-                                 "l"(adesc + 2 * k), "l"(bdesc + 2 * k), "r"(idesc), "r"(1u)
-                                 : "memory");
-                else
-                    umma_i8(tb + (uint32_t)((it & 1) * 256), adesc + 2 * k, bdesc + 2 * k, idesc, 1u);
-            }
-        }
-        tc_commit(&bar);
-        mbar_wait(&bar, 0);
+    for (int i = 0; i < 32 * PLANES; ++i) acc[i] = 0;
+    const uint32_t a = smem_u32(base), b = smem_u32(base + 4096);
+    wgmma_fence();
+    for (int it = 0; it < iters; ++it) {
+#pragma unroll
+        for (int k = 0; k < 2; ++k) wgmma_s8<PLANES>(acc, smem_desc_sw64(a + 32 * k), smem_desc_sw64(b + 32 * k));
+        wgmma_commit();
+        wgmma_wait<1>();
     }
-    tc_fence_before();
-    __syncthreads();
-    if (threadIdx.x < 32) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tb) : "memory");
+    wgmma_wait<0>();
+    int x = 0;
+#pragma unroll
+    for (int i = 0; i < 32 * PLANES; ++i) x ^= acc[i];
+    if (x == 0x7fffffff) *sink = x;   // keeps the MMAs alive
 }
 
 // ---------------------------------------------------------------------------------------------- digit planes
@@ -457,7 +295,7 @@ constexpr int OZ_SPLIT_OUT = 32;
 __global__ void __launch_bounds__(256) ozaki_split_kernel(const double* __restrict__ src, int64_t ld, int n_outer, int K,
                                                           int8_t* __restrict__ planes, int64_t plane_stride, int o0,
                                                           int* __restrict__ exps) {
-    constexpr int PITCH = OZ_KC + 4;  // bytes per smem row: 33 words, conflict-free byte scatter
+    constexpr int PITCH = OZ_SPLIT_KC + 4;  // bytes per smem row: 33 words, conflict-free byte scatter
     __shared__ __align__(16) unsigned char tile[OZ_S][OZ_SPLIT_OUT][PITCH];
     __shared__ double red[8][OZ_SPLIT_OUT];
     __shared__ int s_exp[OZ_SPLIT_OUT];
@@ -479,8 +317,8 @@ __global__ void __launch_bounds__(256) ozaki_split_kernel(const double* __restri
     }
     __syncthreads();
     const double inv = pow2i(-s_exp[tx]);
-    for (int k0 = 0; k0 < K; k0 += OZ_KC) {
-        for (int kk = ty; kk < OZ_KC; kk += 8) {
+    for (int k0 = 0; k0 < K; k0 += OZ_SPLIT_KC) {
+        for (int kk = ty; kk < OZ_SPLIT_KC; kk += 8) {
             double r = valid ? src[(int64_t)(k0 + kk) * ld + o] * inv : 0.0;
             r *= 64.0;  // first digit: 6 bits
 #pragma unroll
@@ -519,7 +357,7 @@ EncodeTiledFn encode_fn() {
     }
     return fn;
 }
-// planes: [OZ_S][cap_rows][K] int8; box = 128 bytes of k x box_rows rows of one plane, 128-byte swizzle
+// planes: [OZ_S][cap_rows][K] int8; box = 64 bytes of k x box_rows rows of one plane, 64-byte swizzle
 int make_plane_map(CUtensorMap* map, const int8_t* planes, int K, int cap_rows, int box_rows) {
     EncodeTiledFn fn = encode_fn();
     if (!fn) {
@@ -531,7 +369,7 @@ int make_plane_map(CUtensorMap* map, const int8_t* planes, int K, int cap_rows, 
     cuuint32_t box[3] = {(cuuint32_t)OZ_KC, (cuuint32_t)box_rows, 1};
     cuuint32_t estr[3] = {1, 1, 1};
     CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, (void*)planes, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                    CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
         set_last_error("cuTensorMapEncodeTiled failed (%d) for K=%d rows=%d", (int)r, K, cap_rows);
         return CFLX_ERR_CUDA;
@@ -546,7 +384,7 @@ struct OzakiWorkspace::Maps {
 
 int ozaki_workspace_create(OzakiWorkspace* ws, int max_rows, int max_cols, int K) {
     *ws = OzakiWorkspace{};
-    if (K <= 0 || K % OZ_KC != 0 || K > 512) {
+    if (K <= 0 || K % OZ_SPLIT_KC != 0 || K > 512) {
         set_last_error("ozaki: contraction length %d unsupported (multiple of 128, <= 512)", K);
         return CFLX_ERR_UNSUPPORTED;
     }
@@ -561,18 +399,12 @@ int ozaki_workspace_create(OzakiWorkspace* ws, int max_rows, int max_cols, int K
     CFLX_CUDA(cudaMalloc((void**)&ws->eb, sizeof(int) * ws->cap_b));
     CFLX_CUDA(cudaMemset(ws->ea, 0, sizeof(int) * ws->cap_a));
     CFLX_CUDA(cudaMemset(ws->eb, 0, sizeof(int) * ws->cap_b));
-    if (getenv("CFLX_OZAKI_DBG")) {
-        CFLX_CUDA(cudaMalloc((void**)&ws->dbg, sizeof(long long) * 16));
-        CFLX_CUDA(cudaMemset(ws->dbg, 0, sizeof(long long) * 16));
-    }
     ws->maps = new OzakiWorkspace::Maps;
     CFLX_TRY(make_plane_map(&ws->maps->a, ws->planesA, K, ws->cap_a, OZ_BM));
     CFLX_TRY(make_plane_map(&ws->maps->b, ws->planesB, K, ws->cap_b, OZ_BN));
     static PerDeviceMax cfg;
-    if (cfg.raise(OZ_SMEM)) {
-        CFLX_CUDA(cudaFuncSetAttribute(ozaki_gemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)OZ_SMEM));
-        CFLX_CUDA(cudaFuncSetAttribute(ozaki_gemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)OZ_SMEM));
-    }
+    if (cfg.raise(OZ_SMEM))
+        CFLX_CUDA(cudaFuncSetAttribute(ozaki_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)OZ_SMEM));
     int dev = 0;
     CFLX_CUDA(cudaGetDevice(&dev));
     CFLX_CUDA(cudaDeviceGetAttribute(&ws->sms, cudaDevAttrMultiProcessorCount, dev));
@@ -583,20 +415,23 @@ void ozaki_workspace_destroy(OzakiWorkspace* ws) {
     cudaFree(ws->planesB);
     cudaFree(ws->ea);
     cudaFree(ws->eb);
-    cudaFree(ws->dbg);
     delete ws->maps;
     *ws = OzakiWorkspace{};
 }
 
-// Tera-MACs/s of back-to-back UMMA 128 x n x (32 bytes of K) instructions, one CTA per SM: use_f16 = 0 -> kind::i8
-// (32 int8 per instruction), 1 -> kind::f16 on bf16 (16 elements per instruction).
-int umma_peak_probe(int n, int use_f16, double* tmacs_out) {
-    if (n < 16 || n > 256 || n % 16) return CFLX_ERR_ARG;
+// Tera-MACs/s of back-to-back int8 wgmma 64 x n x 32 instructions (n = 64, 128, 192 or 256), two warpgroups per CTA,
+// one CTA per SM.
+int wgmma_peak_probe(int n, double* tmacs_out) {
+    void (*kern)(int, int*) = n == 64 ? wgmma_peak_kernel<1> : n == 128 ? wgmma_peak_kernel<2> : n == 192 ? wgmma_peak_kernel<3>
+                            : n == 256 ? wgmma_peak_kernel<4> : nullptr;
+    if (!kern) return CFLX_ERR_ARG;
     int dev = 0, sms = 0;
     CFLX_CUDA(cudaGetDevice(&dev));
     CFLX_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    const size_t smem = 1024 + 16384 + 32768;
-    CFLX_CUDA(cudaFuncSetAttribute(umma_peak_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const size_t smem = 1024 + 4096 + 16384;
+    CFLX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int* sink = nullptr;
+    CFLX_CUDA(cudaMalloc((void**)&sink, sizeof(int)));
     cudaEvent_t e0, e1;
     CFLX_CUDA(cudaEventCreate(&e0));
     CFLX_CUDA(cudaEventCreate(&e1));
@@ -604,17 +439,17 @@ int umma_peak_probe(int n, int use_f16, double* tmacs_out) {
     double best = 0;
     for (int rep = 0; rep < 3; ++rep) {
         CFLX_CUDA(cudaEventRecord(e0));
-        umma_peak_kernel<<<sms, 128, smem>>>(n, use_f16, iters);
+        kern<<<sms, 256, smem>>>(iters, sink);
         CFLX_CUDA(cudaEventRecord(e1));
         CFLX_CUDA(cudaEventSynchronize(e1));
         float ms = 0;
         CFLX_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-        const double kper = use_f16 ? 16.0 : 32.0;
-        const double macs = (double)sms * iters * 4 * 128.0 * n * kper;
+        const double macs = (double)sms * 2 * iters * 2 * 64.0 * n * 32.0;
         best = std::max(best, macs / (ms * 1e-3) / 1e12);
     }
     cudaEventDestroy(e0);
     cudaEventDestroy(e1);
+    cudaFree(sink);
     CFLX_CUDA(cudaGetLastError());
     *tmacs_out = best;
     return CFLX_OK;
@@ -651,13 +486,11 @@ int launch_ozaki_gemm(OzakiWorkspace* ws, int M, int N, int row0, int col0, doub
     g.ea = ws->ea; g.eb = ws->eb;
     g.tiles_m = (M + OZ_BM - 1) / OZ_BM;
     g.tiles_n = (N + OZ_BN - 1) / OZ_BN;
-    g.dbg = ws->dbg;
     int grid = g.tiles_m * g.tiles_n;
     int cap = ws->sms;
     if (max_ctas > 0 && max_ctas < cap) cap = max_ctas;
     if (grid > cap) grid = cap;
-    if (ws->dbg) ozaki_gemm_kernel<true><<<grid, OZ_THREADS, OZ_SMEM, s>>>(ws->maps->a, ws->maps->b, g);
-    else ozaki_gemm_kernel<false><<<grid, OZ_THREADS, OZ_SMEM, s>>>(ws->maps->a, ws->maps->b, g);
+    ozaki_gemm_kernel<<<grid, OZ_THREADS, OZ_SMEM, s>>>(ws->maps->a, ws->maps->b, g);
     CFLX_CUDA(cudaGetLastError());
     return CFLX_OK;
 }

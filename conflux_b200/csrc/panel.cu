@@ -5,9 +5,9 @@
 // every 2v x v tournament round).  Only two things of that factorisation are kept by the reference: the winners
 // perm[0..v) and (last round) the top v x v block L00\U00; this kernel produces exactly those.
 //
-// Design (B200-first, not a LAPACK translation):
+// Design (GPU-first, not a LAPACK translation):
 //   * the panel is stored TRANSPOSED, W[c][r]: a pivot search over column c is a coalesced scan of one row of W;
-//   * one persistent cooperative grid (<= 148 CTAs, one per SM); thread <-> matrix row; rows NEVER move: LAPACK's
+//   * one persistent cooperative grid (<= 132 CTAs, one per SM of an H100); thread <-> matrix row; rows NEVER move: LAPACK's
 //     interchanges are tracked as a per-row "position" so that idamax tie-breaking (first maximal |a| in the
 //     swapped order) is reproduced exactly (needed for the reference's integer test matrices);
 //   * right-looking with an NB-column inner block held in shared memory; per column ONE grid-wide exchange:
@@ -33,7 +33,7 @@ namespace cflx {
 namespace {
 constexpr int PT_THREADS = 256;  // 8 warps: two per scheduler, so dependent DFMA/LDS chains of one warp are covered
 constexpr int PT_WARPS = PT_THREADS / 32;
-constexpr int MAXG = 148;
+constexpr int MAXG = 132;   // SMs of an H100 SXM
 constexpr int RPT_LIMIT = 8;  // rows per thread -> R <= 1024 rows per CTA
 
 struct PanelArgs {
@@ -856,11 +856,11 @@ int launch_panel_getrf_a00(double* W, int64_t ldw, int n, int v, int* perm_out, 
     a.nsteps = n < v ? n : v;
     // Small panels (tournament stacks, late steps) are latency-bound by the per-column exchange: they run as ONE cluster of
     // <= 8 CTAs that exchanges candidates through distributed shared memory.  CFLX_CLUSTER_ROWS = largest n handled that
-    // way (0 = never, the default: on B200 the remote-store fan-out measured SLOWER than the L2 exchange, see profiles/).
+    // way (0 = never, the default: the cluster path is kept as an option, the L2 exchange is the tested default).
     static int cluster_rows = -1;
     if (cluster_rows < 0) {
         const char* e = getenv("CFLX_CLUSTER_ROWS");
-        cluster_rows = e ? atoi(e) : 0;  // measured on B200: 2.02 vs 1.58 ms for the 1024 x 512 stack -> off by default
+        cluster_rows = e ? atoi(e) : 0;
     }
     const bool cluster = n > 0 && n <= cluster_rows;
     // as many CTAs as the cap allows down to 32 rows per CTA: small panels (late steps, tournament stacks) are spread

@@ -1,4 +1,4 @@
-// examples/cholesky_miniapp.cpp -- the reference's Cholesky miniapp on the B200 path: same flags, same report block
+// examples/cholesky_miniapp.cpp -- the reference's Cholesky miniapp on the H100 path: same flags, same report block
 // (reference: examples/cholesky_miniapp.cpp:36-159).  Ranks are host threads of this process, one GPU each.
 //
 //   cholesky_miniapp --dim 32768 --tile 512 [--grid 4,2,1] [--run 5] [--ranks 8] [--validate]
@@ -40,7 +40,7 @@ int main(int argc, char** argv) {
         else if (is("--ranks", "--ranks") && i + 1 < argc) P = std::atoi(argv[++i]);
         else if (is("--validate", "--validate")) validate = true;
         else if (is("-h", "--help")) {
-            std::puts("Cholesky Mini-App (B200): -N/--dim <n> -v/--tile <v> -g/--grid Px,Py,Pz -r/--run <runs> [--ranks P] [--validate]");
+            std::puts("Cholesky Mini-App (H100): -N/--dim <n> -v/--tile <v> -g/--grid Px,Py,Pz -r/--run <runs> [--ranks P] [--validate]");
             return 0;
         }
     }

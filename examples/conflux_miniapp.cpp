@@ -1,4 +1,4 @@
-// examples/conflux_miniapp.cpp -- the reference's LU miniapp on the B200 path: same flags, same `_result_` line
+// examples/conflux_miniapp.cpp -- the reference's LU miniapp on the H100 path: same flags, same `_result_` line
 // (reference: examples/conflux_miniapp.cpp:39-167).  Ranks are host threads of this process, one GPU each (the image
 // has no MPI); a multi-process launcher would create the cflx_comm from an id shipped by its own transport instead.
 //
@@ -33,7 +33,7 @@ int main(int argc, char** argv) {
         else if (is("-l", "--print_limit") && i + 1 < argc) ++i;
         else if (is("--validate", "--validate")) validate = true;
         else if (is("-h", "--help")) {
-            std::puts("conflux miniapp (B200): -N <cols> -b <block> -p Px,Py,Pz -r <reps> -t weak|strong|other");
+            std::puts("conflux miniapp (H100): -N <cols> -b <block> -p Px,Py,Pz -r <reps> -t weak|strong|other");
             return 0;
         }
     }

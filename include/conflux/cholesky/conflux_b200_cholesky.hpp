@@ -73,7 +73,7 @@ inline void finalize(bool clean = false) {
         s.data.shrink_to_fit();
     }
 }
-// extras of the B200 path: device time of the last factorisation, tile size in use, grid-wide residual
+// extras of the H100 path: device time of the last factorisation, tile size in use, grid-wide residual
 inline double last_factorization_ms() { return chol_detail::state().last_ms; }
 inline int tile_size() { return chol_detail::state().info[1]; }
 inline int matrix_size() { return chol_detail::state().info[0]; }

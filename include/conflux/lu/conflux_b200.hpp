@@ -175,7 +175,7 @@ grid_layout<T> conflux_layout(T* data, int M, int N, int v, char ordering, const
 
 template <typename T>
 class lu_params {
-    static_assert(sizeof(T) == sizeof(double), "the B200 path is FP64 only (BASELINE.json)");
+    static_assert(sizeof(T) == sizeof(double), "the H100 path is FP64 only (BASELINE.json)");
 
    public:
     cart_t lu_comm;
@@ -187,7 +187,7 @@ class lu_params {
     std::vector<T> data;     // local tiles, row-major Ml x Nl (conflux/COSTA tile layout, layout.cpp:95-109)
     grid_layout<T> matrix;   // non-owning descriptor of `data` (lu_params.hpp:118)
     bool use_collectives = false;
-    cflx_lu* plan = nullptr;  // device side of this object (B200 only)
+    cflx_lu* plan = nullptr;  // device side of this object (H100 only)
 
     lu_params() = default;
     lu_params(int inpM, int inpN, int v_, comm_t comm) { initialize(inpM, inpN, v_, -1, -1, -1, comm); }

@@ -1,5 +1,5 @@
 /*
- * include/conflux_b200.h -- C ABI of the B200-native CONFLUX LU hot path (libconflux_b200.so).
+ * include/conflux_b200.h -- C ABI of the H100-native CONFLUX LU hot path (libconflux_b200.so).
  *
  * This is the drop-in boundary for ONE path of eth-cscs/conflux: conflux::LU_rep<double> and the parts of
  * conflux::lu_params<double> it needs.  Plain pointers and sizes only; every function returns 0 on success or
@@ -95,8 +95,9 @@ int cflx_lu_get_permutation(cflx_lu*, int* permutation_out);
 int cflx_lu_validate(cflx_lu*, double* frob_abs_out, double* frob_rel_out);
 /* COLLECTIVE.  = cflx_lu_validate(lu, NULL, rel_out) */
 int cflx_lu_residual(cflx_lu*, double* rel_out);
-/* 1 when this plan's trailing update runs on the int8 tcgen05 path (ozaki.cu), 0 for the FP64 DMMA kernel (gemm.cu) */
-int cflx_lu_uses_tcgen05(const cflx_lu*);
+/* 1 when this plan's trailing update runs on the int8 wgmma digit-plane path (ozaki.cu), 0 for the FP64 DMMA kernel
+ * (gemm.cu) */
+int cflx_lu_uses_ozaki(const cflx_lu*);
 /* number of kernels this plan launched since the last call (for bench.py's gpu_launches) */
 int cflx_lu_launch_count(cflx_lu*, int64_t* count_out, int reset);
 /* per-phase device time of the last cflx_lu_factor when profiling was enabled: ms_out[8] =
@@ -152,15 +153,15 @@ int cflx_dbg_panel(int n, int v, const double* panel, int* perm_out, double* A00
                    double* ms_out);
 /* X = B * U^-1 (right, upper, non-unit; B n x v) and Y = L^-1 * R (left, lower, unit; R v x n), A00 = L\U packed */
 int cflx_dbg_trsm(int n, int v, const double* A00, const double* B, double* X_out, const double* R, double* Y_out);
-/* D = C - AT^T * B on the int8 tcgen05 path (error-free digit planes, ozaki.cu); K % 128 == 0, N even.  Optional test
+/* D = C - AT^T * B on the int8 wgmma path (error-free digit planes, ozaki.cu); K % 128 == 0, N even.  Optional test
  * outputs: digit planes [8][M][K] / [8][N][K], exponents [M] / [N].  ms_out / split_ms_out: mean device time of the GEMM
  * kernel / of the two digit-plane kernels. */
 int cflx_dbg_ozaki_gemm(int M, int N, int K, const double* AT, const double* B, const double* C, double* D,
                         signed char* planesA_out, signed char* planesB_out, int* ea_out, int* eb_out, int reps,
                         double* ms_out, double* split_ms_out);
-/* raw tensor-pipe rate of back-to-back tcgen05.mma (128 x n x 32 bytes of K, operands resident in shared memory, one
- * CTA per SM): which = 0 kind::i8, 1 kind::f16 on bf16.  tmacs_out = tera-MACs/s (x2 = TOP/s). */
-int cflx_dbg_umma_peak(int which, int n, double* tmacs_out);
+/* raw int8 tensor-core rate of back-to-back wgmma (64 x n x 32, n = 64/128/192/256, operands resident in shared memory,
+ * two warpgroups per CTA, one CTA per SM).  tmacs_out = tera-MACs/s (x2 = TOP/s). */
+int cflx_dbg_wgmma_peak(int n, double* tmacs_out);
 /* plan_moves + push_phase1..3 + gri bookkeeping on one rank: the npiv pivot rows (local indices >= fnpr, tournament
  * order) are pushed to rows [fnpr, fnpr+npiv) exactly like push_pivots_up (conflux_opt.hpp:176-218, tests/unit/
  * test_utils.cpp:8-84).  n_cols even.  gri_out[n_rows] = new row -> old row, a01_out[npiv*n_cols] = extracted rows. */

@@ -9,7 +9,12 @@ Fixtures:
   lu_cases.npz - full LU_rep outputs (input A, C, permutation) on small grids, incl. the hard-coded
                  matrices of lu_params.hpp:157-363 (N = 16, 27, 32) and multi-rank / multi-layer grids.
   lu_perms.npz - permutation-only known answers for larger seeded inputs (N = 256, 1024, 2048).
+  ref_cases.npz - LU_rep of the seeded generator on the grids of tests/test_oracle_vs_reference.py: SHA-256 of every
+                 rank's input, the permutation, and a seeded sample of REF_SAMPLES entries of the concatenated factors.
+  layout_ref.txt - the COSTA descriptors the reference's conflux_layout produces (both overloads, several grids),
+                 printed by tests/cpp/layout_dump_ref.cpp (compiled against the reference tree and COSTA).
 """
+import hashlib
 import ctypes
 import os
 import sys
@@ -81,6 +86,40 @@ def helpers():
     np.savez_compressed(os.path.join(HERE, "helpers.npz"), **out)
 
 
+def ref_cases():
+    from tests.test_oracle_vs_reference import REF_CASES, ref_sample_index
+    out = {"cases": np.array(REF_CASES, dtype=np.int32)}
+    for i, c in enumerate(REF_CASES):
+        r = ref.lu_run(*c)
+        out[f"c{i}_A_sha256"] = np.stack([np.frombuffer(hashlib.sha256(np.ascontiguousarray(a).tobytes()).digest(), np.uint8)
+                                          for a in r["A"]])
+        out[f"c{i}_perm"] = r["perm"]
+        C = np.concatenate([x.reshape(-1) for x in r["C"]])
+        out[f"c{i}_C_sample"] = C[ref_sample_index(C.size)]
+    np.savez_compressed(os.path.join(HERE, "ref_cases.npz"), **out)
+
+
+def layout_descriptors():
+    import subprocess
+    import sysconfig
+    import tempfile
+    ref_root = os.environ.get("CONFLUX_REFERENCE", "/root/reference")
+    costa = os.path.join(ref_root, "libs", "costa", "src")
+    sp = sysconfig.get_paths()["purelib"]
+    libdir = os.path.join(sp, "opencv_python_headless.libs")
+    blas = [os.path.join(libdir, f) for f in os.listdir(libdir) if f.startswith("libopenblasp")][0]
+    srcs = [os.path.join(ROOT, "tests", "cpp", "layout_dump_ref.cpp"), os.path.join(ROOT, "oracle", "mpi_stub", "mpi_threads.cpp"),
+            os.path.join(ref_root, "src", "conflux", "lu", "layout.cpp"), os.path.join(costa, "costa", "layout.cpp")] + \
+           [os.path.join(costa, "costa", "grid2grid", f + ".cpp") for f in ("block", "grid2D", "interval", "scalapack_layout", "ranks_reordering")]
+    with tempfile.TemporaryDirectory() as td:
+        exe = os.path.join(td, "layout_dump_ref")
+        subprocess.check_call(["g++", "-O1", "-std=c++17", "-fopenmp", "-w", "-DNDEBUG", f"-I{ROOT}/oracle/mpi_stub", f"-I{costa}",
+                               f"-I{ref_root}/src"] + srcs + [blas, f"-Wl,-rpath,{libdir}", f"-Wl,-rpath,{sp}/scipy.libs", "-lpthread",
+                                                               "-o", exe])
+        txt = subprocess.run([exe], check=True, capture_output=True, text=True).stdout
+    open(os.path.join(HERE, "layout_ref.txt"), "w").write(txt)
+
+
 def lu_cases():
     out = {}
     cases = [(16, 4, 1, 1, 1), (16, 4, 2, 2, 1), (27, 3, 3, 3, 1), (32, 4, 2, 2, 2), (64, 8, 1, 1, 1),
@@ -107,6 +146,9 @@ def lu_cases():
 if __name__ == "__main__":
     if not ref.available():
         sys.exit("oracle/_ref/libref_lu.so missing: run oracle/build_ref.sh in the build container first")
-    helpers()
-    lu_cases()
+    if "--ref-cases-only" not in sys.argv:
+        helpers()
+        lu_cases()
+    ref_cases()
+    layout_descriptors()
     print("golden fixtures written to", HERE)

@@ -65,3 +65,18 @@ def test_reference_arm_prints_the_contract_line_on_a_small_override():
     assert line["e2e"] == {"value": line["value"], "unit": "GFLOP/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}
     assert "size override" in line["config"]["workload"] and line["steps_done"] == 1
     assert time.time() - t0 < 120
+
+
+def test_dump_outputs_is_seeded_float64_and_within_budget(tmp_path):
+    loc = np.arange(3000 * 3000, dtype=np.float64).reshape(3000, 3000)
+    perm = np.arange(3000, dtype=np.int32)[::-1].copy()
+    for d in ("a", "b"):
+        bench.dump_outputs(str(tmp_path / d), 0, 1, loc, perm)
+    files = sorted(os.listdir(tmp_path / "a"))
+    assert files == ["factor_sample.npy", "factor_sample_index.npy", "permutation.npy"]
+    assert sum(os.path.getsize(tmp_path / "a" / f) for f in files) <= 64 * 10 ** 6
+    for f in files:
+        a, b = np.load(tmp_path / "a" / f), np.load(tmp_path / "b" / f)
+        assert a.dtype == np.float64 and np.array_equal(a, b)
+    idx = np.load(tmp_path / "a" / "factor_sample_index.npy").astype(np.int64)
+    assert np.array_equal(np.load(tmp_path / "a" / "factor_sample.npy"), loc.reshape(-1)[idx])

@@ -1,7 +1,7 @@
-"""GPU: the int8 tcgen05 trailing update (conflux_b200/csrc/ozaki.cu) in isolation, through the C ABI.
+"""GPU: the int8 wgmma trailing update (conflux_b200/csrc/ozaki.cu) in isolation, through the C ABI.
   * the digit planes and exponents equal the numpy restatement exactly;
   * the result equals the restatement BIT FOR BIT (all plane products are exact integers and the FP64 recombination is
-    reproduced in the kernel's order) -- this pins the TMA / UMMA descriptor / TMEM addressing logic;
+    reproduced in the kernel's order) -- this pins the TMA / wgmma descriptor / accumulator layout logic;
   * the result agrees with a plain FP64 product to rounding level (what cblas_dgemm gives the reference)."""
 import numpy as np
 import pytest
@@ -56,7 +56,7 @@ def test_ozaki_gemm_speed_probe():
     B = rng.standard_normal((K, N))
     r = cb.dbg.ozaki_gemm(AT, B, None, reps=3)
     tf = 2.0 * M * N * K / (r["ms"] * 1e-3) / 1e12
-    print(f"ozaki int8 tcgen05 trailing update {M}x{N}x{K}: {r['ms']:.3f} ms = {tf:.1f} TFLOP/s FP64-equivalent, "
+    print(f"ozaki int8 wgmma trailing update {M}x{N}x{K}: {r['ms']:.3f} ms = {tf:.1f} TFLOP/s FP64-equivalent, "
           f"digit planes {r['split_ms']:.3f} ms")
     _, dm = cb.dbg.gemm_tn(AT, B, None, -1.0, 0.0, reps=3)
     print(f"DMMA kernel same shape: {dm:.3f} ms = {2.0 * M * N * K / (dm * 1e-3) / 1e12:.1f} TFLOP/s")

@@ -1,9 +1,9 @@
-"""tools/ozaki_study.py -- CPU feasibility study for the round-2 item "FP64 trailing update on the int8 tcgen05 path".
+"""tools/ozaki_study.py -- CPU feasibility study for the round-2 item "FP64 trailing update on the int8 tensor cores".
 
 Emulates, in numpy with exact integer arithmetic, an Ozaki-style error-free-slicing DGEMM
     C -= L * U,   L = sum_p 2^(eL_i - 7p) Lp,  U = sum_q 2^(eU_j - 7q) Uq,   Lp, Uq int8 slices (7 magnitude bits),
 where row i of L and column j of U share one exponent each, every slice product Lp*Uq is an exact int8 x int8 -> int32
-GEMM (what tcgen05.mma kind::i8 computes), and only the products with p + q <= s + 1 are formed.  It then runs the
+GEMM (what an int8 tensor-core MMA computes), and only the products with p + q <= s + 1 are formed.  It then runs the
 blocked right-looking LU (partial pivoting inside each panel, exactly the P = 1 data flow of this repo) with that GEMM as
 the trailing update and reports ||PA - LU||_F / ||A||_F against the number of slices s, on the bench's generator.
 

@@ -1,6 +1,6 @@
 """tools/timeline.py -- per-region device time of one factorisation at a bench configuration, WITHOUT serialising the run:
 CUDA event pairs on the launching streams (cflx_lu_set_profiling mode 2), region names = the reference's semiprof regions.
-    python tools/timeline.py --gpus 1 [--mode 2] [--out profiles/r02_timeline_N1.json]
+    python tools/timeline.py --gpus 1 [--mode 2] [--out timeline.json]
     python -m torch.distributed.run --nproc-per-node 4 --master-addr 127.0.0.1 tools/timeline.py --gpus 4 ...
 Every rank prints/saves its own table (roles differ: panel column, pivot row, other layers)."""
 import argparse
@@ -39,7 +39,7 @@ tl = cb.timeline(gv)
 _lib.lib().cflx_lu_set_profiling(gv._h, 0)
 rec = {"workload": f"LU N={gv.N} v={gv.v} grid {g[0]}x{g[1]}x{g[2]}", "rank": gv.rank, "coords": [gv.pi, gv.pj, gv.pk],
        "mode": "serialising timers" if a.mode == 1 else "event pairs on the launching streams (not serialised)",
-       "factor_ms_unprofiled": ms_plain, "factor_ms_profiled": ms, "gemm": "ozaki (int8 tcgen05)" if _lib.lib().cflx_lu_uses_tcgen05(gv._h) else "dmma", "regions": tl}
+       "factor_ms_unprofiled": ms_plain, "factor_ms_profiled": ms, "gemm": "ozaki (int8 wgmma)" if _lib.lib().cflx_lu_uses_ozaki(gv._h) else "dmma", "regions": tl}
 out = a.out or ""
 if out:
     path = out.replace(".json", f"_rank{gv.rank}.json") if world > 1 else out
