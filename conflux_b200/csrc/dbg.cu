@@ -61,14 +61,7 @@ __global__ void dfma_peak_kernel(double* out, int iters) {
 }
 }  // namespace
 
-static long long g_panel_cycles[8] = {0};
-
 extern "C" {
-
-int cflx_dbg_last_panel_cycles(long long* out8) {
-    for (int i = 0; i < 8; ++i) out8[i] = g_panel_cycles[i];
-    return CFLX_OK;
-}
 
 // burst = best of a few ~2 ms launches (what a kernel timed alone can reach at the maximum clock); sustained = one
 // ~0.5 s launch (what survives the power cap inside a long step)
@@ -193,7 +186,6 @@ int cflx_dbg_panel(int n, int v, const double* panel, int* perm_out, double* A00
     cudaEventDestroy(e1);
     if (rc == CFLX_OK && n >= v)
         rc = launch_gather_a00(dW.as<double>(), ld, dperm.as<int>(), v, nb, dA00.as<double>(), dA00T.as<double>(), 0);
-    cudaMemcpy(g_panel_cycles, ws.dbg, sizeof(g_panel_cycles), cudaMemcpyDeviceToHost);
     panel_workspace_destroy(&ws);
     if (rc != CFLX_OK) {
         if (rc == CFLX_ERR_CUDA) set_last_error("panel kernel failed: %s", cudaGetErrorString(cudaGetLastError()));

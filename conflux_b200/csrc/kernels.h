@@ -49,7 +49,6 @@ int launch_ozaki_gemm(OzakiWorkspace* ws, int M, int N, int row0, int col0, doub
 struct PanelWorkspace {
     void* slot_hdr;     // [2][132][4]  LL words (payload32, epoch)
     void* slot_rows;    // [2][132][64] LL words
-    long long* dbg;     // [8] cycle counters of CTA 0 of the last launch (profiling aid)
     int epoch;          // host-side running epoch (monotonic across launches)
     int max_ctas;       // co-resident CTA budget (<= 132)
     int cta_cap;        // optional cap on the grid (look-ahead: leave SMs to the trailing update); 0 = none

@@ -13,7 +13,8 @@
 //   * right-looking with an NB-column inner block held in shared memory; per column ONE grid-wide exchange:
 //     every CTA publishes its best candidate together with that row's inner-block values into a double-buffered
 //     global slot as "LL" words (payload + epoch in one 8-byte volatile store: the flag travels with the data), then
-//     polls all slots and picks the winner redundantly -- no second round trip for the pivot row, no grid barrier.
+//     polls all headers, picks the winner redundantly and reads the winner's row from its slot -- two dependent L2
+//     round trips per column, no reply from the owner, no grid barrier.
 //     The LL words order only their own payload; the trailing columns of W that phase C writes with plain stores and
 //     that OTHER CTAs gather as pivot rows one block later are ordered by a gpu-scope fence pair per NB-column block
 //     (writer: __threadfence() after the phase-C write-back; reader: __threadfence() before the U12 gathers);
@@ -46,9 +47,6 @@ struct PanelArgs {
     uint2* slot_hdr;   // [2][MAXG][4]  LL words {payload32, epoch}: val_lo, val_hi, pos, row
     uint2* slot_rows;  // [2][MAXG][64] LL words: inner-block row of the candidate, two words per double
     int epoch_base;
-    int spec;          // G <= 32: warps 1..7 fetch every CTA's candidate row speculatively (else warp 0 fetches the winner's)
-    long long* dbg;    // optional: 8 cycle counters of CTA 0 (cand+argmax, exchange, argmax2, row fetch, eliminate,
-                       // load/write-back, U12 gather+solve, rank update)
 };
 
 // "LL" exchange (flag travels with the data in one 8-byte word, so no fence / separate flag / L1 invalidate):
@@ -59,25 +57,6 @@ __device__ __forceinline__ uint4 ld_ll2(const uint2* p) {  // two consecutive LL
     uint4 v;
     asm volatile("ld.volatile.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
     return v;
-}
-
-// ---- cluster variant (small panels): the LL slots live in the SHARED MEMORY of every CTA of one thread-block cluster;
-// a candidate is published with remote shared-memory stores (DSMEM, ~200 cycles) into all peers and every CTA polls its
-// own shared memory -- no L2 round trip, no cluster barrier per column.
-constexpr int CS_MAX = 8;  // portable cluster size
-__device__ __forceinline__ void st_ll_dsmem(const uint2* local_slot, unsigned peer, unsigned data, unsigned epoch) {
-    unsigned remote;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(local_slot)), "r"(peer));
-    asm volatile("st.shared::cluster.v2.u32 [%0], {%1, %2};" ::"r"(remote), "r"(data), "r"(epoch) : "memory");
-}
-__device__ __forceinline__ uint4 ld_ll2_smem(const uint2* p) {  // two consecutive LL words of my own shared memory
-    uint4 v;
-    asm volatile("ld.volatile.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(smem_u32(p)) : "memory");
-    return v;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
 struct Cand {
@@ -127,23 +106,20 @@ __device__ __forceinline__ Cand block_argmax(Cand c, unsigned long long* red_key
     return best;
 }
 
-template <int NB, int RPT_MAX, bool DSM>
+template <int NB, int RPT_MAX>
 __global__ void __launch_bounds__(PT_THREADS, 1) panel_getrf_kernel(PanelArgs p) {
+    // layout and size: panel_smem_bytes<NB>
     extern __shared__ __align__(16) unsigned char smem_raw[];
     double* Ab = reinterpret_cast<double*>(smem_raw);  // [NB][Rpad] inner block, column-major per CTA
     double* U12 = Ab + (size_t)NB * p.Rpad;            // [NB][v]
     double* LU11 = U12 + (size_t)NB * p.v;             // [NB][NB+1] LU rows of this block's pivots
-    double* prow = LU11 + NB * (NB + 1);               // [2][NB] winner rows, double-buffered by column parity (G > 32)
-    double* crow = prow + 2 * NB;                      // [2][32][NB] EVERY CTA's candidate row (G <= 32), by parity
-    unsigned long long* red_key = reinterpret_cast<unsigned long long*>(crow + 2 * 32 * NB);
+    double* prow = LU11 + NB * (NB + 1);               // [2][NB] winner rows, double-buffered by column parity
+    unsigned long long* red_key = reinterpret_cast<unsigned long long*>(prow + 2 * NB);
     int* red_pos = reinterpret_cast<int*>(red_key + 2 * PT_WARPS);
     int* red_row = red_pos + 2 * PT_WARPS;
     int* pivrow_blk = red_row + 2 * PT_WARPS;  // [NB]
     int* win_sh = pivrow_blk + NB;  // [2][2] winner {pos, row} broadcast by the gathering warp, by column parity
-    // cluster variant: cs_hdr[parity][cta][4], cs_row[parity][cta][2 * NB] LL words written by the peers
-    uint2* cs_hdr = reinterpret_cast<uint2*>(win_sh + 4);
-    uint2* cs_row = cs_hdr + 2 * CS_MAX * 4;
-    unsigned char* s_act = reinterpret_cast<unsigned char*>(cs_row + 2 * CS_MAX * 2 * NB);  // [Rpad] row still active?
+    unsigned char* s_act = reinterpret_cast<unsigned char*>(win_sh + 4);  // [Rpad] row still active?
     int rb = 0;
 
     const int t = threadIdx.x;
@@ -154,29 +130,15 @@ __global__ void __launch_bounds__(PT_THREADS, 1) panel_getrf_kernel(PanelArgs p)
     double* __restrict__ W = p.W;
     const int64_t ldw = p.ldw;
 
-    long long tm[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    long long t0 = clock64(), t1;
-#define TICK(i)            \
-    t1 = clock64();        \
-    tm[i] += t1 - t0;      \
-    t0 = t1;
     int pos[RPT_MAX];
     bool active[RPT_MAX];
-    int pib[RPT_MAX];  // pivot index inside the current block, -1 otherwise
 #pragma unroll
     for (int q = 0; q < RPT_MAX; ++q) {
         const int lr = t + q * PT_THREADS;
         pos[q] = row_base + lr;
         active[q] = lr < Rloc;
-        pib[q] = -1;
     }
     for (int lr = t; lr < Rpad; lr += PT_THREADS) s_act[lr] = lr < Rloc ? 1 : 0;
-    if constexpr (DSM) {
-        // no slot may carry a stale epoch: clear them, then let every CTA of the cluster see that before anyone publishes
-        for (int e = t; e < 2 * CS_MAX * (4 + 2 * NB); e += PT_THREADS) cs_hdr[e] = make_uint2(0u, 0u);
-        __syncthreads();
-        cluster_sync_all();
-    }
 
     for (int jb = 0; jb < p.nsteps; jb += NB) {
         const int nbc = min(NB, v - jb);         // columns in this block
@@ -188,7 +150,6 @@ __global__ void __launch_bounds__(PT_THREADS, 1) panel_getrf_kernel(PanelArgs p)
         }
         __syncthreads();
         // (each thread touches only its own rows of Ab until a winner row is published after a block sync)
-        TICK(5)
 
         // ---- phase B: nsb pivot steps, software-pipelined across columns ----
         // The candidate of column j+1 is found and PUBLISHED as soon as the multipliers of column j are known (only
@@ -212,39 +173,13 @@ __global__ void __launch_bounds__(PT_THREADS, 1) panel_getrf_kernel(PanelArgs p)
         auto publish = [&](const Cand& mine, int jg, int jprev, const double* pw) {
             const unsigned epoch = (unsigned)(p.epoch_base + jg + 1);
             const int par = jg & 1;
-            if constexpr (DSM) {
-                // header + row words into the slot [par][cta] of EVERY CTA of the cluster (remote shared-memory stores)
-                const int words = 4 + 2 * nbc;
-                for (int e = t; e < p.G * words; e += PT_THREADS) {
-                    const int peer = e / words, w = e % words;
-                    unsigned val;
-                    const uint2* slot;
-                    if (w < 4) {
-                        val = w == 0 ? (unsigned)mine.key : w == 1 ? (unsigned)(mine.key >> 32) : w == 2 ? (unsigned)mine.pos : (unsigned)mine.row;
-                        slot = cs_hdr + (size_t)(par * CS_MAX + cta) * 4 + w;
-                    } else {
-                        const int c = (w - 4) >> 1;
-                        double x = 0.0;
-                        if (mine.row >= 0) {
-                            const int lrw = mine.row - row_base;
-                            x = Ab[c * Rpad + lrw];
-                            if (jprev >= 0 && c > jprev + 1) x = fma(-Ab[jprev * Rpad + lrw], pw[c], x);
-                        }
-                        const unsigned long long xb = (unsigned long long)__double_as_longlong(x);
-                        val = ((w - 4) & 1) ? (unsigned)(xb >> 32) : (unsigned)xb;
-                        slot = cs_row + (size_t)(par * CS_MAX + cta) * 2 * NB + (w - 4);
-                    }
-                    st_ll_dsmem(slot, (unsigned)peer, val, epoch);
-                }
-                return;
-            }
             uint2* myhdr = p.slot_hdr + (size_t)(par * MAXG + cta) * 4;
             if (t < 4) {
                 const unsigned w = t == 0 ? (unsigned)mine.key : t == 1 ? (unsigned)(mine.key >> 32)
                                  : t == 2 ? (unsigned)mine.pos : (unsigned)mine.row;
                 st_ll(myhdr + t, w, epoch);
             }
-            if (t < nbc) {  // (zeros when this CTA has no active row left: the row words are fetched speculatively)
+            if (t < nbc) {  // (zeros when this CTA has no active row left: only the winner's row words are read)
                 double x = 0.0;
                 if (mine.row >= 0) {
                     const int lrw = mine.row - row_base;
@@ -259,7 +194,6 @@ __global__ void __launch_bounds__(PT_THREADS, 1) panel_getrf_kernel(PanelArgs p)
         };
         {
             const Cand mine0 = local_candidate(0);
-            TICK(0)
             if (t < 32) __threadfence();  // publisher-side half of the per-block release of my phase-C stores (cumulative)
             publish(mine0, jb, -1, nullptr);
         }
@@ -271,109 +205,37 @@ __global__ void __launch_bounds__(PT_THREADS, 1) panel_getrf_kernel(PanelArgs p)
                 // gather every CTA's candidate for column jg, pick the winner, fetch its inner-block row.  G <= 32: warp 0
                 // alone (one slot per lane, warp-level argmax, no block barrier); larger grids poll with all warps.
                 const unsigned epoch = (unsigned)(p.epoch_base + jg + 1);
-                if (p.G > 32) {
-                    Cand gc{0ull, INT_MAX, -1};
-                    for (int g = t; g < p.G; g += PT_THREADS) {
-                        const uint2* h = p.slot_hdr + (size_t)(par * MAXG + g) * 4;
-                        uint4 a, b;
-                        do {
-                            a = ld_ll2(h);
-                            b = ld_ll2(h + 2);
-                        } while (a.y != epoch || a.w != epoch || b.y != epoch || b.w != epoch);
-                        Cand o{((unsigned long long)a.z << 32) | a.x, (int)b.x, (int)b.z};
-                        if (better(o, gc)) gc = o;
-                    }
-                    TICK(1)
-                    const Cand w = block_argmax(gc, red_key, red_pos, red_row, rb);
-                    TICK(2)
-                    const int wcta = w.row / p.R;
-                    if (t < nbc) {
-                        const uint2* wr = p.slot_rows + (size_t)(par * MAXG + wcta) * 64 + 2 * t;
-                        uint4 a;
-                        do {
-                            a = ld_ll2(wr);
-                        } while (a.y != epoch || a.w != epoch);
-                        const double x = __longlong_as_double((long long)(((unsigned long long)a.z << 32) | a.x));
-                        pr[t] = x;
-                        LU11[j * (NB + 1) + t] = x;
-                    }
-                    if (t == 0) {
-                        win_sh[2 * par] = w.pos;
-                        win_sh[2 * par + 1] = w.row;
-                    }
-                } else if (t < 32) {
-                    // warp 0: one header per lane -> warp-level argmax -> winner (no block barrier)
-                    Cand gc{0ull, INT_MAX, -1};
-                    if (t < p.G) {
-                        uint4 a, b;
-                        if constexpr (DSM) {
-                            const uint2* h = cs_hdr + (size_t)(par * CS_MAX + t) * 4;   // my own shared memory
-                            do {
-                                a = ld_ll2_smem(h);
-                                b = ld_ll2_smem(h + 2);
-                            } while (a.y != epoch || a.w != epoch || b.y != epoch || b.w != epoch);
-                        } else {
-                            const uint2* h = p.slot_hdr + (size_t)(par * MAXG + t) * 4;
-                            do {
-                                a = ld_ll2(h);
-                                b = ld_ll2(h + 2);
-                            } while (a.y != epoch || a.w != epoch || b.y != epoch || b.w != epoch);
-                        }
-                        gc = Cand{((unsigned long long)a.z << 32) | a.x, (int)b.x, (int)b.z};
-                    }
-                    TICK(1)
-                    const Cand w = warp_argmax(gc);
-                    TICK(2)
-                    // (w.row < 0 cannot happen while jg < nsteps = min(n, v): some row is still active)
-                    if ((DSM || !p.spec) && t < nbc) {  // the winner's row: second L2 round trip, or (cluster) already in my smem
-                        uint4 a;
-                        if constexpr (DSM) {
-                            const uint2* wr = cs_row + (size_t)(par * CS_MAX + w.row / p.R) * 2 * NB + 2 * t;
-                            do {
-                                a = ld_ll2_smem(wr);
-                            } while (a.y != epoch || a.w != epoch);
-                        } else {
-                            const uint2* wr = p.slot_rows + (size_t)(par * MAXG + w.row / p.R) * 64 + 2 * t;
-                            do {
-                                a = ld_ll2(wr);
-                            } while (a.y != epoch || a.w != epoch);
-                        }
-                        crow[(size_t)par * 32 * NB + (size_t)(w.row / p.R) * NB + t] =
-                            __longlong_as_double((long long)(((unsigned long long)a.z << 32) | a.x));
-                    }
-                    if (t == 0) {
-                        win_sh[2 * par] = w.pos;
-                        win_sh[2 * par + 1] = w.row;
-                    }
-                } else if (!DSM && p.spec) {
-                    // warps 1..7: fetch EVERY CTA's candidate row speculatively, all loads of a lane in flight together, so
-                    // the winner's row costs no second dependent L2 round trip after the argmax
-                    double* cr = crow + (size_t)par * 32 * NB;
-                    constexpr int SPEC_T = PT_THREADS - 32;
-                    constexpr int SPEC_MAX = (32 * NB + SPEC_T - 1) / SPEC_T;
-                    const int e0 = t - 32, tot = p.G * nbc;
-                    uint4 a[SPEC_MAX];
-                    unsigned pending = 0;
-#pragma unroll
-                    for (int i = 0; i < SPEC_MAX; ++i)
-                        if (e0 + i * SPEC_T < tot) pending |= 1u << i;
-                    while (pending) {
-#pragma unroll
-                        for (int i = 0; i < SPEC_MAX; ++i) {
-                            if (pending & (1u << i)) {
-                                const int e = e0 + i * SPEC_T;
-                                a[i] = ld_ll2(p.slot_rows + (size_t)(par * MAXG + e / nbc) * 64 + 2 * (e % nbc));
-                            }
-                        }
-#pragma unroll
-                        for (int i = 0; i < SPEC_MAX; ++i) {
-                            if ((pending & (1u << i)) && a[i].y == epoch && a[i].w == epoch) {
-                                const int e = e0 + i * SPEC_T;
-                                cr[(e / nbc) * NB + e % nbc] = __longlong_as_double((long long)(((unsigned long long)a[i].z << 32) | a[i].x));
-                                pending &= ~(1u << i);
-                            }
-                        }
-                    }
+                Cand gc{0ull, INT_MAX, -1};
+                for (int g = t; g < p.G; g += PT_THREADS) {
+                    const uint2* h = p.slot_hdr + (size_t)(par * MAXG + g) * 4;
+                    uint4 a, b;
+                    do {
+                        a = ld_ll2(h);
+                        b = ld_ll2(h + 2);
+                    } while (a.y != epoch || a.w != epoch || b.y != epoch || b.w != epoch);
+                    Cand o{((unsigned long long)a.z << 32) | a.x, (int)b.x, (int)b.z};
+                    if (better(o, gc)) gc = o;
+                }
+                Cand w = gc;  // (G <= 32: only warp 0 reduces; the other warps go straight to the barrier)
+                if (p.G > 32) w = block_argmax(gc, red_key, red_pos, red_row, rb);
+                else if (t < 32) w = warp_argmax(gc);
+                // (w.row < 0 cannot happen while jg < nsteps = min(n, v): some row is still active)
+                if (t < nbc) {  // the winner's row: second L2 round trip
+                    const uint2* wr = p.slot_rows + (size_t)(par * MAXG + w.row / p.R) * 64 + 2 * t;
+                    uint4 a;
+                    do {
+                        a = ld_ll2(wr);
+                    } while (a.y != epoch || a.w != epoch);
+                    const double x = __longlong_as_double((long long)(((unsigned long long)a.z << 32) | a.x));
+                    // safe before the barrier below: prow is double-buffered by column parity, and the last reader of
+                    // prow[par] (elimination jg - 2) finished before the barrier of column jg - 1; LU11 row j is read
+                    // only by phase C and the A00 emission, after the block's later barriers
+                    pr[t] = x;
+                    LU11[j * (NB + 1) + t] = x;
+                }
+                if (t == 0) {
+                    win_sh[2 * par] = w.pos;
+                    win_sh[2 * par + 1] = w.row;
                 }
             }
             __syncthreads();  // winner + its row are in shared memory; every thread has finished elimination j-1
@@ -381,15 +243,10 @@ __global__ void __launch_bounds__(PT_THREADS, 1) panel_getrf_kernel(PanelArgs p)
             win.key = 0;
             win.pos = win_sh[2 * par];
             win.row = win_sh[2 * par + 1];
-            if (p.G <= 32) {
-                pr = crow + (size_t)par * 32 * NB + (size_t)(win.row / p.R) * NB;
-                if (t < nbc) LU11[j * (NB + 1) + t] = pr[t];   // (read by phase C / the A00 emission, after later barriers)
-            }
             if (t == 0) {
                 pivrow_blk[j] = win.row;
                 if (cta == 0) p.perm_out[jg] = win.row;
             }
-            TICK(3)
             const double pivot = pr[j];
             const double rinv = pivot != 0.0 ? 1.0 / pivot : 0.0;
             const bool have_next = (j + 1 < nbc);
@@ -403,7 +260,6 @@ __global__ void __launch_bounds__(PT_THREADS, 1) panel_getrf_kernel(PanelArgs p)
                 if (row_base + lr == win.row) {
                     active[q] = false;
                     s_act[lr] = 0;
-                    pib[q] = j;
                     continue;
                 }
                 if (pos[q] == jg) pos[q] = win.pos;  // the row that sat at position jg moves to the winner's slot
@@ -415,7 +271,6 @@ __global__ void __launch_bounds__(PT_THREADS, 1) panel_getrf_kernel(PanelArgs p)
             }
             if (j + 1 < nsb) {
                 const Cand mine = local_candidate(j + 1);  // (its block barrier also orders the multiplier stores above)
-                TICK(0)
                 publish(mine, jg + 1, j, pr);
                 __syncthreads();  // the candidate row's pre-update values have been read before its owner updates them
             }
@@ -431,7 +286,6 @@ __global__ void __launch_bounds__(PT_THREADS, 1) panel_getrf_kernel(PanelArgs p)
                     }
                 }
             }
-            TICK(4)
         }
 
         // ---- write the inner block back (L multipliers; pivot rows keep their LU row) ----
@@ -447,7 +301,6 @@ __global__ void __launch_bounds__(PT_THREADS, 1) panel_getrf_kernel(PanelArgs p)
             }
         }
 
-        TICK(5)
         // ---- phase C: U12 = L11^-1 A12, trailing columns of my rows -= L21 * U12 ----
         const int cstart = jb + nbc;
         const int rem = v - cstart;
@@ -477,7 +330,6 @@ __global__ void __launch_bounds__(PT_THREADS, 1) panel_getrf_kernel(PanelArgs p)
                 }
             }
             __syncthreads();
-            TICK(6)
             // rank-NB update of my rows.  One thread per (row, column group): with R >= 256 rows per CTA a thread walks
             // all trailing columns of its row(s); with fewer rows the PT_THREADS / R threads that share a row split the
             // columns (groups of 4, interleaved), so small panels still use every thread of every CTA.
@@ -544,21 +396,14 @@ __global__ void __launch_bounds__(PT_THREADS, 1) panel_getrf_kernel(PanelArgs p)
                 }
             }
         }
-#pragma unroll
-        for (int q = 0; q < RPT_MAX; ++q) pib[q] = -1;
         // release: my phase-C stores to W must be visible gpu-wide before any LL word of the NEXT block is published
         // (other CTAs gather these rows as pivot rows after observing that block's epochs)
         __threadfence();
         __syncthreads();  // Ab / U12 / LU11 are rewritten by the next block
-        TICK(7)
     }
     // identity tail of perm (n < v): LAPACK leaves perm[i] = i for i >= n (conflux_opt.hpp:150-165)
     if (cta == 0)
         for (int i = p.nsteps + t; i < v; i += PT_THREADS) p.perm_out[i] = i;
-    if (cta == 0 && t == 0 && p.dbg != nullptr)
-        for (int i = 0; i < 8; ++i) p.dbg[i] = tm[i];
-    if constexpr (DSM) cluster_sync_all();  // nobody may exit while a peer can still store into its shared memory
-#undef TICK
 }
 
 // =====================================================================================================================
@@ -755,49 +600,44 @@ int launch_stack_getrf(double* W, int64_t ldw, int n, int v, int* perm_out, Pane
     return CFLX_OK;
 }
 
+// the dynamic shared memory of panel_getrf_kernel<NB, *>, laid out in that order
 template <int NB>
 size_t panel_smem_bytes(int Rpad, int v) {
-    return ((size_t)NB * Rpad + (size_t)NB * v + NB * (NB + 1) + 2 * NB + 2 * 32 * NB) * sizeof(double) +
-           2 * PT_WARPS * (sizeof(unsigned long long) + 2 * sizeof(int)) + (NB + 4) * sizeof(int) +
-           2 * CS_MAX * (4 + 2 * NB) * sizeof(uint2) + (size_t)Rpad + 64;
+    return ((size_t)NB * Rpad + (size_t)NB * v + NB * (NB + 1) + 2 * NB) * sizeof(double) +  // Ab, U12, LU11, prow
+           2 * PT_WARPS * (sizeof(unsigned long long) + 2 * sizeof(int)) +                  // red_key, red_pos, red_row
+           (NB + 4) * sizeof(int) + (size_t)Rpad;                                           // pivrow_blk, win_sh, s_act
+}
+
+// Inner block size NB of the row-owner kernel: the first of 32, 16, 8, 4 that is <= v (4 always is) and satisfies
+// (8 NB + 1) Rpad + 8 NB v <= 222 KiB - (8 NB^2 + 796 NB + 848).  These are the thresholds the kernel was validated and
+// benchmarked with: they come from an earlier, larger shared-memory layout, so NB is smaller than panel_smem_bytes would
+// allow for some shapes.  NB sets the blocking of the U12 solve and of the rank-NB update, and with it the rounding of
+// the factors; raising it where it now fits is a change of its own that has to be measured.  0 = no NB fits.
+int panel_nb(int Rpad, int v) {
+    for (int nb = 32; nb >= 4; nb /= 2) {
+        const long long limit = 222 * 1024 - (8LL * nb * nb + 796LL * nb + 848);
+        if ((nb <= v || nb == 4) && (8LL * nb + 1) * Rpad + 8LL * nb * v <= limit) return nb;
+    }
+    return 0;
 }
 
 template <int NB, int RPT>
-int launch_nb_rpt(PanelArgs& a, bool cluster, cudaStream_t stream) {
+int launch_nb_rpt(PanelArgs& a, cudaStream_t stream) {
     const size_t smem = panel_smem_bytes<NB>(a.Rpad, a.v);
     void* params[] = {&a};
-    if (cluster) {  // the whole grid is ONE thread-block cluster (<= 8 CTAs): DSMEM exchange
-        static PerDeviceMax cfg;
-        if (cfg.raise(smem))
-            CFLX_CUDA(cudaFuncSetAttribute(panel_getrf_kernel<NB, RPT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        cudaLaunchConfig_t lc{};
-        lc.gridDim = dim3(a.G);
-        lc.blockDim = dim3(PT_THREADS);
-        lc.dynamicSmemBytes = smem;
-        lc.stream = stream;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeClusterDimension;
-        at[0].val.clusterDim.x = a.G;
-        at[0].val.clusterDim.y = 1;
-        at[0].val.clusterDim.z = 1;
-        lc.attrs = at;
-        lc.numAttrs = 1;
-        CFLX_CUDA(cudaLaunchKernelExC(&lc, (const void*)panel_getrf_kernel<NB, RPT, true>, params));
-        return CFLX_OK;
-    }
     static PerDeviceMax cfg;
     if (cfg.raise(smem))
-        CFLX_CUDA(cudaFuncSetAttribute(panel_getrf_kernel<NB, RPT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CFLX_CUDA(cudaLaunchCooperativeKernel((void*)panel_getrf_kernel<NB, RPT, false>, dim3(a.G), dim3(PT_THREADS), params, smem, stream));
+        CFLX_CUDA(cudaFuncSetAttribute(panel_getrf_kernel<NB, RPT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CFLX_CUDA(cudaLaunchCooperativeKernel((void*)panel_getrf_kernel<NB, RPT>, dim3(a.G), dim3(PT_THREADS), params, smem, stream));
     return CFLX_OK;
 }
 template <int NB>
-int launch_nb(PanelArgs& a, bool cluster, cudaStream_t stream) {
+int launch_nb(PanelArgs& a, cudaStream_t stream) {
     const int rpt = (a.R + PT_THREADS - 1) / PT_THREADS;
-    if (rpt <= 1) return launch_nb_rpt<NB, 1>(a, cluster, stream);
-    if (rpt <= 2) return launch_nb_rpt<NB, 2>(a, cluster, stream);
-    if (rpt <= 4) return launch_nb_rpt<NB, 4>(a, cluster, stream);
-    return launch_nb_rpt<NB, 8>(a, cluster, stream);
+    if (rpt <= 1) return launch_nb_rpt<NB, 1>(a, stream);
+    if (rpt <= 2) return launch_nb_rpt<NB, 2>(a, stream);
+    if (rpt <= 4) return launch_nb_rpt<NB, 4>(a, stream);
+    return launch_nb_rpt<NB, 8>(a, stream);
 }
 }  // namespace
 
@@ -810,8 +650,6 @@ int panel_workspace_create(PanelWorkspace* ws) {
     ws->cta_cap = 0;
     CFLX_CUDA(cudaMalloc(&ws->slot_hdr, sizeof(uint2) * 2 * MAXG * 4));
     CFLX_CUDA(cudaMalloc(&ws->slot_rows, sizeof(uint2) * 2 * MAXG * 64));
-    CFLX_CUDA(cudaMalloc(&ws->dbg, sizeof(long long) * 8));
-    CFLX_CUDA(cudaMemset(ws->dbg, 0, sizeof(long long) * 8));
     CFLX_CUDA(cudaMemset(ws->slot_hdr, 0, sizeof(uint2) * 2 * MAXG * 4));
     CFLX_CUDA(cudaMemset(ws->slot_rows, 0, sizeof(uint2) * 2 * MAXG * 64));
     // column-owner kernel for panels of <= 1024 rows: per-block flags, pivot positions, the CTA ticket
@@ -830,7 +668,6 @@ int panel_workspace_create(PanelWorkspace* ws) {
 }
 void panel_workspace_destroy(PanelWorkspace* ws) {
     cudaFree(ws->slot_hdr);
-    cudaFree(ws->dbg);
     cudaFree(ws->slot_rows);
     cudaFree(ws->sk_flags);
     cudaFree(ws->sk_ppos);
@@ -854,15 +691,6 @@ int launch_panel_getrf_a00(double* W, int64_t ldw, int n, int v, int* perm_out, 
     a.n = n;
     a.v = v;
     a.nsteps = n < v ? n : v;
-    // Small panels (tournament stacks, late steps) are latency-bound by the per-column exchange: they run as ONE cluster of
-    // <= 8 CTAs that exchanges candidates through distributed shared memory.  CFLX_CLUSTER_ROWS = largest n handled that
-    // way (0 = never, the default: the cluster path is kept as an option, the L2 exchange is the tested default).
-    static int cluster_rows = -1;
-    if (cluster_rows < 0) {
-        const char* e = getenv("CFLX_CLUSTER_ROWS");
-        cluster_rows = e ? atoi(e) : 0;
-    }
-    const bool cluster = n > 0 && n <= cluster_rows;
     // as many CTAs as the cap allows down to 32 rows per CTA: small panels (late steps, tournament stacks) are spread
     // over up to 32 SMs and the threads that share a row split the trailing columns in phase C
     int G = (n + 31) / 32;
@@ -874,7 +702,6 @@ int launch_panel_getrf_a00(double* W, int64_t ldw, int n, int v, int* perm_out, 
         const int need = (n + RPT_LIMIT * PT_THREADS - 1) / (RPT_LIMIT * PT_THREADS);
         if (G < need) G = need < ws->max_ctas ? need : ws->max_ctas;
     }
-    if (cluster && G > CS_MAX) G = CS_MAX;
     int R = (n + G - 1) / G;
     R = (int)round_up(R > 0 ? R : 1, 32);
     G = n > 0 ? (n + R - 1) / R : 1;
@@ -891,32 +718,19 @@ int launch_panel_getrf_a00(double* W, int64_t ldw, int n, int v, int* perm_out, 
     a.slot_hdr = reinterpret_cast<uint2*>(ws->slot_hdr);
     a.slot_rows = reinterpret_cast<uint2*>(ws->slot_rows);
     a.epoch_base = ws->epoch;
-    {
-        static int spec = -1;
-        if (spec < 0) {
-            const char* e = getenv("CFLX_PANEL_SPEC");
-            spec = e ? atoi(e) : 0;
-        }
-        a.spec = spec;
-    }
-    a.dbg = ws->dbg;
     ws->epoch += v + 2 + (v & 1);  // keep the base even so slot parity == column parity
-    const size_t budget = 222 * 1024;
-    int nb = v >= 32 ? 32 : (v >= 16 ? 16 : (v >= 8 ? 8 : 4));
-    if (nb == 32 && panel_smem_bytes<32>(a.Rpad, v) > budget) nb = 16;
-    if (nb == 16 && panel_smem_bytes<16>(a.Rpad, v) > budget) nb = 8;
-    if (nb == 8 && panel_smem_bytes<8>(a.Rpad, v) > budget) nb = 4;
-    if (nb == 4 && panel_smem_bytes<4>(a.Rpad, v) > budget) {
-        set_last_error("panel_getrf: v=%d with %d rows per CTA needs %zu B of shared memory (budget %zu)", v, a.Rpad,
-                       panel_smem_bytes<4>(a.Rpad, v), budget);
+    const int nb = panel_nb(a.Rpad, v);
+    if (nb == 0) {
+        set_last_error("panel_getrf: v=%d with %d rows per CTA exceeds the shared-memory budget of the inner block", v,
+                       a.Rpad);
         return CFLX_ERR_UNSUPPORTED;
     }
     if (nb_used) *nb_used = nb;
     switch (nb) {
-        case 32: return launch_nb<32>(a, cluster, stream);
-        case 16: return launch_nb<16>(a, cluster, stream);
-        case 8: return launch_nb<8>(a, cluster, stream);
-        default: return launch_nb<4>(a, cluster, stream);
+        case 32: return launch_nb<32>(a, stream);
+        case 16: return launch_nb<16>(a, stream);
+        case 8: return launch_nb<8>(a, stream);
+        default: return launch_nb<4>(a, stream);
     }
 }
 

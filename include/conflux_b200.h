@@ -167,9 +167,6 @@ int cflx_dbg_wgmma_peak(int n, double* tmacs_out);
  * test_utils.cpp:8-84).  n_cols even.  gri_out[n_rows] = new row -> old row, a01_out[npiv*n_cols] = extracted rows. */
 int cflx_dbg_push_pivots(int n_rows, int n_cols, double* A_inout, int npiv, const int* pivot_rows, int fnpr, int* gri_out,
                          double* a01_out);
-/* cycle counters of CTA 0 of the last cflx_dbg_panel launch: {candidate+argmax, exchange, argmax2, row fetch,
- * eliminate, load/write-back, U12 gather+solve, rank update} */
-int cflx_dbg_last_panel_cycles(long long* out8);
 /* raw FP64 pipe micro-benchmarks: which = 0 DMMA (mma.sync m8n8k4 f64), 1 DFMA; returns TFLOP/s */
 int cflx_dbg_fp64_peak(int which, double* tflops_out);
 /* same probe: burst (best of ~2 ms launches) and sustained (one ~0.5 s launch, power-capped) TFLOP/s */
