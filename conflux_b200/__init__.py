@@ -356,7 +356,8 @@ class dbg:
 
     @staticmethod
     def fp64_peak_ex(which):
-        """(burst, sustained) TFLOP/s of the DMMA (0) / DFMA (1) pipe."""
+        """(burst, sustained) TFLOP/s of the FP64 pipes: 0 the MMA shape gemm_tn_kernel issues (m16n8k8), 1 DFMA,
+        2 / 3 / 4 mma m16n8k4 / m16n8k8 / m16n8k16, 5 mma m8n8k4."""
         a, b = ctypes.c_double(), ctypes.c_double()
         check(lib().cflx_dbg_fp64_peak_ex(int(which), ctypes.byref(a), ctypes.byref(b)), "dbg_fp64_peak_ex")
         return a.value, b.value

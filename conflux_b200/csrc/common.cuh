@@ -101,6 +101,31 @@ __device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double
                  : "d"(a), "d"(b));
 }
 
+// The Hopper f64 shapes, D(16x8) += A(16xk, row) * B(kx8, col), with g = lane>>2 and t = lane&3 (PTX ISA f64 fragment
+// layouts).  Accumulators of all three: c0/c1 = C[g][2t+{0,1}], c2/c3 = C[g+8][2t+{0,1}].  Not volatile: the MMA has no
+// side effect beyond its outputs, so ptxas may interleave the fragment loads of the next step with it.  gemm.cu issues
+// m16n8k8 (its layout is checked against numpy by the GEMM tests); k4 and k16 run only in the rate probes of dbg.cu.
+//   m16n8k4  (DMMA.16x8x4):  a0 = A[g][t], a1 = A[g+8][t];                                    b0 = B[t][g]
+//   m16n8k8  (DMMA.16x8x8):  a0..a3 = A[g][t], A[g+8][t], A[g][t+4], A[g+8][t+4];           b0, b1 = B[t][g], B[t+4][g]
+//   m16n8k16 (DMMA.16x8x16): a(2i), a(2i+1) = A[g][t+4i], A[g+8][t+4i] (i = 0..3);           b(i) = B[t+4i][g]
+__device__ __forceinline__ void dmma16x8x4(double (&c)[4], const double (&a)[2], double b) {
+    asm("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+        : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+        : "d"(a[0]), "d"(a[1]), "d"(b));
+}
+__device__ __forceinline__ void dmma16x8x8(double (&c)[4], const double (&a)[4], const double (&b)[2]) {
+    asm("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+        : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+        : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(b[0]), "d"(b[1]));
+}
+__device__ __forceinline__ void dmma16x8x16(double (&c)[4], const double (&a)[8], const double (&b)[4]) {
+    asm("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, "
+        "{%12,%13,%14,%15}, {%0,%1,%2,%3};"
+        : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+        : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]), "d"(b[0]),
+          "d"(b[1]), "d"(b[2]), "d"(b[3]));
+}
+
 // gpu-scope acquire/release accessors for the grid-wide pivot exchange
 __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
     int v;

@@ -45,6 +45,30 @@ __global__ void dmma_peak_kernel(double* out, int iters) {
     for (int i = 0; i < 16; ++i) s += c[i][0] + c[i][1];
     out[blockIdx.x * blockDim.x + threadIdx.x] = s;
 }
+// m16n8kK, K = 4, 8, 16: 16 independent accumulator chains per warp, so the probe measures issue rate, not latency
+template <int K>
+__global__ void dmma16x8_peak_kernel(double* out, int iters) {
+    double c[16][4];
+#pragma unroll
+    for (int i = 0; i < 16; ++i) c[i][0] = c[i][1] = c[i][2] = c[i][3] = 0.0;
+    double a[K / 2], b[K / 4];
+#pragma unroll
+    for (int i = 0; i < K / 2; ++i) a[i] = 1.0 + (threadIdx.x + i) * 1e-9;
+#pragma unroll
+    for (int i = 0; i < K / 4; ++i) b[i] = 1.0 - (threadIdx.x + i) * 1e-9;
+    for (int it = 0; it < iters; ++it) {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+            if constexpr (K == 4) dmma16x8x4(c[i], a, b[0]);
+            else if constexpr (K == 8) dmma16x8x8(c[i], a, b);
+            else dmma16x8x16(c[i], a, b);
+        }
+    }
+    double s = 0;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) s += c[i][0] + c[i][1] + c[i][2] + c[i][3];
+    out[blockIdx.x * blockDim.x + threadIdx.x] = s;
+}
 __global__ void dfma_peak_kernel(double* out, int iters) {
     double c[16];
 #pragma unroll
@@ -63,10 +87,16 @@ __global__ void dfma_peak_kernel(double* out, int iters) {
 
 extern "C" {
 
-// burst = best of a few ~2 ms launches (what a kernel timed alone can reach at the maximum clock); sustained = one
-// ~0.5 s launch (what survives the power cap inside a long step)
+// which: 0 = the shape gemm_tn_kernel issues (m16n8k8), 1 = DFMA, 2/3/4 = mma m16n8k4/k8/k16 f64, 5 = mma m8n8k4 f64.
+// burst = best of a few short launches (what a kernel timed alone can reach at the maximum clock); sustained = one
+// launch 256x longer (what survives the power cap inside a long step)
 int cflx_dbg_fp64_peak_ex(int which, double* burst_out, double* sustained_out) {
     CFLX_TRY(check_device());
+    if (which == 0) which = 3;
+    if (which < 1 || which > 5) {
+        set_last_error("fp64_peak: unknown probe %d", which);
+        return CFLX_ERR_ARG;
+    }
     int dev = 0, sms = 0;
     CFLX_CUDA(cudaGetDevice(&dev));
     CFLX_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
@@ -76,17 +106,27 @@ int cflx_dbg_fp64_peak_ex(int which, double* burst_out, double* sustained_out) {
     cudaEvent_t e0, e1;
     CFLX_CUDA(cudaEventCreate(&e0));
     CFLX_CUDA(cudaEventCreate(&e1));
+    // flop per warp instruction: m16n8kK = 2*16*8*K (1024 / 2048 / 4096), m8n8k4 = 512; DFMA = 2 flop per lane.
+    // The larger shapes run proportionally fewer iterations, so every probe's launches do about the same work.
+    const double per_warp_instr = which == 2 ? 1024.0 : which == 3 ? 2048.0 : which == 4 ? 4096.0 : 512.0;
+    const int shrink = which == 1 ? 1 : (int)(per_warp_instr / 512.0);
     auto run = [&](int iters, double* tf) -> int {
+        iters /= shrink;
         CFLX_CUDA(cudaEventRecord(e0));
-        if (which == 0) dmma_peak_kernel<<<blocks, threads>>>(out.as<double>(), iters);
-        else dfma_peak_kernel<<<blocks, threads>>>(out.as<double>(), iters);
+        switch (which) {
+            case 1: dfma_peak_kernel<<<blocks, threads>>>(out.as<double>(), iters); break;
+            case 2: dmma16x8_peak_kernel<4><<<blocks, threads>>>(out.as<double>(), iters); break;
+            case 3: dmma16x8_peak_kernel<8><<<blocks, threads>>>(out.as<double>(), iters); break;
+            case 4: dmma16x8_peak_kernel<16><<<blocks, threads>>>(out.as<double>(), iters); break;
+            default: dmma_peak_kernel<<<blocks, threads>>>(out.as<double>(), iters); break;
+        }
+        CFLX_CUDA(cudaGetLastError());
         CFLX_CUDA(cudaEventRecord(e1));
         CFLX_CUDA(cudaEventSynchronize(e1));
         float ms = 0;
         CFLX_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-        // DMMA 8x8x4 = 256 FMA = 512 flop per warp instruction; DFMA = 2 flop per lane
-        const double flop = which == 0 ? (double)blocks * (threads / 32) * iters * 16 * 512.0
-                                       : (double)blocks * threads * iters * 16 * 2.0;
+        const double flop = which == 1 ? (double)blocks * threads * iters * 16 * 2.0
+                                       : (double)blocks * (threads / 32) * iters * 16 * per_warp_instr;
         *tf = flop / (ms * 1e-3) / 1e12;
         return CFLX_OK;
     };

@@ -6,10 +6,11 @@
 // through trsm.cu, the two cblas_dtrsm calls at :1347 and :1539.  Both operands are kept K-MAJOR in HBM
 // (L is stored transposed, L^T[k][row]; U is U[k][col]) so that every operand row a CTA needs is one contiguous
 // 1 KB segment: the producer warp stages tiles with 1-D bulk asynchronous copies (cp.async.bulk -> UBLKCP, the
-// TMA engine) into a 4-stage shared-memory ring guarded by mbarriers, and 8 consumer warps run
-// mma.sync.m8n8k4.f64 (DMMA.8x8x4 -- the native FP64 tensor instruction of sm_90a; wgmma has no f64 kind)
-// on 64x32 warp tiles with accumulators in registers.  Shared-memory row stride is 132 doubles (== 4 mod 16) so
-// both fragment loads (lane -> [k = lane&3][outer = lane>>2]) are bank-conflict free per half-warp.
+// TMA engine) into a 4-stage shared-memory ring guarded by mbarriers, and the consumer warps run
+// mma.sync.m16n8k8.f64 (DMMA.16x8x8 in sm_90a SASS; wgmma has no f64 kind) on 64x32 warp tiles with accumulators in
+// registers.  In a K tail of 4 rows (K % 8 == 4) the fragments of the 4 rows the copy did not fill are zeros, so no
+// stale ring data reaches the MMA.  Shared-memory row strides are == 4 (mod 16) doubles so both fragment loads
+// (lane -> [k = lane&3 (+4)][outer = lane>>2 (+8)]) are bank-conflict free per half-warp.
 #include <cstdlib>
 
 #include "common.cuh"
@@ -21,9 +22,12 @@ namespace {
 constexpr int BK = 16, STAGES = 4;
 
 // WM x WN consumer warps, each owning a 64 x 32 tile of C: CTA tile (64*WM) x (32*WN).
-//   <2,4,1>: 128x128, 8+1 warps, one CTA per SM (largest reuse per byte staged);
+//   <2,4,1>: 128x128, 8+1 warps, one CTA per SM (largest reuse per byte staged; the default);
 //   <1,4,2>:  64x128, 4+1 warps, TWO CTAs per SM so that one CTA's prologue/epilogue (operand fill, C read-modify-
 //             write) overlaps the other's DMMA main loop.
+// Register budget: ptxas sizes registers for the worst SM sub-partition, which holds 3 of the 9 (one CTA of <2,4,1>) or
+// 10 (two CTAs of <1,4,2>) warps, so both run at 16384 / (3 * 32) -> 168 registers per thread.  The 64 accumulators
+// take 128 of them, so a k-step holds all B fragments (8 doubles) but only one m16 tile's A fragment (4) at a time.
 template <int WM, int WN>
 struct Cfg {
     static constexpr int BM = 64 * WM, BN = 32 * WN;
@@ -54,7 +58,6 @@ __global__ void __launch_bounds__(Cfg<WM, WN>::NTHREADS, MINB) gemm_tn_kernel(Ge
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
-    const int KT = (g.K + BK - 1) / BK;
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < STAGES; ++s) {
@@ -72,7 +75,7 @@ __global__ void __launch_bounds__(Cfg<WM, WN>::NTHREADS, MINB) gemm_tn_kernel(Ge
         int wn = g.N - n0;
         wn = wn > BN ? BN : ((wn + 1) & ~1);
         const int rr = lane & 15;
-        for (int kt = 0; kt < KT; ++kt) {
+        for (int kt = 0; kt * BK < g.K; ++kt) {
             const int s = kt % STAGES, u = kt / STAGES;
             if (u > 0) mbar_wait(&empty[s], (u - 1) & 1);
             const int rows = min(BK, g.K - kt * BK);
@@ -92,30 +95,41 @@ __global__ void __launch_bounds__(Cfg<WM, WN>::NTHREADS, MINB) gemm_tn_kernel(Ge
     // ===== consumers =====
     const int wm_off = (warp / WN) * 64, wn_off = (warp % WN) * 32;
     const int g4 = lane >> 2, t4 = lane & 3;
-    double acc[8][4][2];
+    // acc[i][j]: the m16n8 accumulator fragment of rows 16i.., columns 8j.. of the warp tile
+    double acc[4][4][4];
 #pragma unroll
-    for (int i = 0; i < 8; ++i)
+    for (int i = 0; i < 4; ++i)
 #pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j][0] = acc[i][j][1] = 0.0;
+        for (int j = 0; j < 4; ++j) acc[i][j][0] = acc[i][j][1] = acc[i][j][2] = acc[i][j][3] = 0.0;
 
-    for (int kt = 0; kt < KT; ++kt) {
+    for (int kt = 0; kt * BK < g.K; ++kt) {
         const int s = kt % STAGES, u = kt / STAGES;
         mbar_wait(&full[s], u & 1);
         const double* a_s = sA + s * BK * LDA + wm_off + g4;
         const double* b_s = sB + s * BK * LDB + wn_off + g4;
-        const int rows = min(BK, g.K - kt * BK);
+        const int rows = min(BK, g.K - kt * BK);  // rows of this stage the copy filled, a multiple of 4
 #pragma unroll
-        for (int kk = 0; kk < BK; kk += 4) {
+        for (int kk = 0; kk < BK; kk += 8) {
             if (kk < rows) {
-                double a[8], b[4];
+                // K tail (rows == kk + 4): rows kk+4..kk+7 of the stage hold stale data, possibly NaN, which would
+                // reach every output through the MMA; their fragments are zeros instead.
+                const bool hi = kk + 4 < rows;
+                const double* a_k = a_s + (kk + t4) * LDA;
+                const double* b_k = b_s + (kk + t4) * LDB;
+                // all B fragments of the k-step, the A fragments one m16 tile at a time (register budget, above)
+                double b[4][2];
 #pragma unroll
-                for (int i = 0; i < 8; ++i) a[i] = a_s[(kk + t4) * LDA + 8 * i];
+                for (int j = 0; j < 4; ++j) {
+                    b[j][0] = b_k[8 * j];
+                    b[j][1] = hi ? b_k[4 * LDB + 8 * j] : 0.0;
+                }
 #pragma unroll
-                for (int j = 0; j < 4; ++j) b[j] = b_s[(kk + t4) * LDB + 8 * j];
+                for (int i = 0; i < 4; ++i) {
+                    const double a[4] = {a_k[16 * i], a_k[16 * i + 8], hi ? a_k[4 * LDA + 16 * i] : 0.0,
+                                         hi ? a_k[4 * LDA + 16 * i + 8] : 0.0};
 #pragma unroll
-                for (int i = 0; i < 8; ++i)
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) dmma884(acc[i][j][0], acc[i][j][1], a[i], b[j]);
+                    for (int j = 0; j < 4; ++j) dmma16x8x8(acc[i][j], a, b[j]);
+                }
             }
         }
         __syncwarp();
@@ -123,36 +137,30 @@ __global__ void __launch_bounds__(Cfg<WM, WN>::NTHREADS, MINB) gemm_tn_kernel(Ge
     }
 
     // ===== epilogue: registers <-> HBM directly, 16-byte accesses (each quad covers one 64 B row segment).
-    // C and D may alias, so the compiler must not be left to order loads after earlier stores: all C loads of a
-    // batch of two 8-row slabs are issued first (8 independent 16 B loads in flight per thread), then the stores.
+    // C and D may alias, so the compiler must not be left to order loads after earlier stores: all C loads of an
+    // 8-row slab are issued first (4 independent 16 B loads in flight per thread), then its stores.  One slab per
+    // batch: with all 128 accumulator registers live, a second slab's loads would not fit the register budget.
     const double alpha = g.alpha, beta = g.beta;
     const bool use_c = (beta != 0.0);
+    const int row0 = m0 + wm_off + g4, col0 = n0 + wn_off + 2 * t4;
 #pragma unroll
-    for (int ib = 0; ib < 8; ib += 2) {
-        double2 cv[2][4];
+    for (int sl = 0; sl < 8; ++sl) {
+        const int row = row0 + 8 * sl;
+        double2 cv[4];
 #pragma unroll
-        for (int ii = 0; ii < 2; ++ii) {
-            const int row = m0 + wm_off + 8 * (ib + ii) + g4;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const int col = n0 + wn_off + 8 * j + 2 * t4;
-                cv[ii][j] = make_double2(0.0, 0.0);
-                if (use_c && row < g.M && col < g.N)
-                    cv[ii][j] = ld_c2(g.C + (int64_t)row * g.ldc + col);
-            }
+        for (int j = 0; j < 4; ++j) {
+            const int col = col0 + 8 * j;
+            cv[j] = make_double2(0.0, 0.0);
+            if (use_c && row < g.M && col < g.N) cv[j] = ld_c2(g.C + (int64_t)row * g.ldc + col);
         }
 #pragma unroll
-        for (int ii = 0; ii < 2; ++ii) {
-            const int row = m0 + wm_off + 8 * (ib + ii) + g4;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const int col = n0 + wn_off + 8 * j + 2 * t4;
-                if (row < g.M && col < g.N) {
-                    double2 out;
-                    out.x = fma(alpha, acc[ib + ii][j][0], beta * cv[ii][j].x);
-                    out.y = fma(alpha, acc[ib + ii][j][1], beta * cv[ii][j].y);
-                    *reinterpret_cast<double2*>(g.D + (int64_t)row * g.ldd + col) = out;
-                }
+        for (int j = 0; j < 4; ++j) {
+            const int col = col0 + 8 * j;
+            if (row < g.M && col < g.N) {
+                double2 out;
+                out.x = fma(alpha, acc[sl / 2][j][2 * (sl & 1)], beta * cv[j].x);
+                out.y = fma(alpha, acc[sl / 2][j][2 * (sl & 1) + 1], beta * cv[j].y);
+                *reinterpret_cast<double2*>(g.D + (int64_t)row * g.ldd + col) = out;
             }
         }
     }
@@ -177,12 +185,12 @@ int launch_one(const GemmArgs& g, cudaStream_t stream) {
     CFLX_CUDA(cudaGetLastError());
     return CFLX_OK;
 }
-int tile_variant() {  // default: 64x128 tile, two CTAs per SM;
-                      // CFLX_GEMM_TILE=128 selects the 128x128 tile with one CTA per SM
+int tile_variant() {  // default: 128x128 tile, one CTA per SM (16 flop per operand byte at K = 256, against 10.7 for
+                      // 64x128: measured faster on m16n8k8); CFLX_GEMM_TILE=64 selects the 64x128 tile, two CTAs per SM
     static int v = -1;
     if (v < 0) {
         const char* e = getenv("CFLX_GEMM_TILE");
-        v = (e && atoi(e) == 128) ? 128 : 64;
+        v = (e && atoi(e) == 64) ? 64 : 128;
     }
     return v;
 }

@@ -167,7 +167,8 @@ int cflx_dbg_wgmma_peak(int n, double* tmacs_out);
  * test_utils.cpp:8-84).  n_cols even.  gri_out[n_rows] = new row -> old row, a01_out[npiv*n_cols] = extracted rows. */
 int cflx_dbg_push_pivots(int n_rows, int n_cols, double* A_inout, int npiv, const int* pivot_rows, int fnpr, int* gri_out,
                          double* a01_out);
-/* raw FP64 pipe micro-benchmarks: which = 0 DMMA (mma.sync m8n8k4 f64), 1 DFMA; returns TFLOP/s */
+/* raw FP64 pipe micro-benchmarks, TFLOP/s: which = 0 the MMA shape gemm_tn_kernel issues (mma.sync m16n8k8 f64),
+ * 1 DFMA, 2 / 3 / 4 mma.sync m16n8k4 / m16n8k8 / m16n8k16 f64, 5 mma.sync m8n8k4 f64 */
 int cflx_dbg_fp64_peak(int which, double* tflops_out);
 /* same probe: burst (best of ~2 ms launches) and sustained (one ~0.5 s launch, power-capped) TFLOP/s */
 int cflx_dbg_fp64_peak_ex(int which, double* burst_out, double* sustained_out);
