@@ -15,7 +15,7 @@ import numpy as np
 
 from ._lib import ConfluxError, LIB_PATH, SYMBOLS, check, lib
 
-__all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "residual", "validate", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
+__all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "residual", "validate", "lu_solve", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
 
 
 def auto_grid(M, N, P):
@@ -201,6 +201,20 @@ def residual(gv):
     return validate(gv)[1]
 
 
+def lu_solve(gv, B):
+    """Solves A X = B with the factors of the last LU_rep (P A = L U) on the GPU grid, like LAPACK's getrs.  COLLECTIVE
+    over gv.lu_comm; every rank passes the same B, (M,) or (M, nrhs) with M = gv.M (the padded size), and gets the same X
+    in the same shape.  The factors and the input matrix are left as they are."""
+    B = np.asarray(B, dtype=np.float64)
+    if B.ndim not in (1, 2) or B.shape[0] != gv.M:
+        raise ValueError(f"lu_solve: B must have shape ({gv.M},) or ({gv.M}, nrhs), got {B.shape}")
+    B2 = np.ascontiguousarray(B.reshape(gv.M, -1))
+    nrhs = B2.shape[1]
+    X = np.empty_like(B2)
+    check(lib().cflx_lu_solve(gv._h, nrhs, B2.ctypes.data, max(nrhs, 1), X.ctypes.data, max(nrhs, 1)), "lu_solve")
+    return X.reshape(B.shape)
+
+
 class cholesky:
     """Mirror of the reference's CONFCHOX driver interface (src/conflux/cholesky/Cholesky.h:20-22):
         initialize(N, v, grid, comm) -> object;  obj.parallelCholesky() -> ms;  obj.finalize().
@@ -286,6 +300,25 @@ class dbg:
             Cp = C.ctypes.data
         check(lib().cflx_dbg_gemm_tn(M, N, K, AT.ctypes.data, B.ctypes.data, Cp, float(alpha), float(beta), D.ctypes.data,
                                      int(reps), ctypes.byref(ms)), "dbg_gemm_tn")
+        return D, ms.value
+
+    @staticmethod
+    def gemm_narrow(A, B, C=None, alpha=1.0, beta=0.0, reps=1, out=None):
+        """D = beta*C + alpha * A @ B on the solve's narrow GEMM (K % 4 == 0).  Returns (D, mean ms of one launch).
+        out: the array to write D into; passing C itself runs the kernel with D aliasing C."""
+        A = np.ascontiguousarray(A, dtype=np.float64)
+        B = np.ascontiguousarray(B, dtype=np.float64)
+        M, K = A.shape
+        N = B.shape[1]
+        Cp = None
+        if C is not None:
+            assert C.dtype == np.float64 and C.flags.c_contiguous and C.shape == (M, N)
+            Cp = C.ctypes.data
+        D = np.empty((M, N)) if out is None else out
+        assert D.dtype == np.float64 and D.flags.c_contiguous and D.shape == (M, N)
+        ms = ctypes.c_double()
+        check(lib().cflx_dbg_gemm_narrow(M, N, K, A.ctypes.data, B.ctypes.data, Cp, float(alpha), float(beta), D.ctypes.data,
+                                         int(reps), ctypes.byref(ms)), "dbg_gemm_narrow")
         return D, ms.value
 
     @staticmethod

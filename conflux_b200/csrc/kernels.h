@@ -115,7 +115,9 @@ int launch_store_diag(double* A, int64_t lda, int fnpr_old, MovePlan plan, const
 // residual helpers (validation only)
 int launch_split_factors(const double* F, int64_t ldf, int n, double* LT, double* U, cudaStream_t stream);
 int launch_gather_perm_rows(const double* A, int64_t lda, const int* perm, int n, double* out, cudaStream_t stream);
-int launch_sumsq(const double* X, int64_t count, double* out, cudaStream_t stream);
+// *out += sum of X[i]^2, deterministic (the same rounding on every call); partials: SUMSQ_PARTIALS doubles of scratch
+constexpr int SUMSQ_PARTIALS = 1184;
+int launch_sumsq(const double* X, int64_t count, double* out, double* partials, cudaStream_t stream);
 // misc
 int launch_fill(double* p, int64_t n, double val, cudaStream_t stream);
 int launch_iota_gri(int* gri, int* igri, int Ml, int v, int Px, int pi, cudaStream_t stream);
@@ -132,5 +134,16 @@ int trsm_right_upper_T(const double* A00, const double* Uinv, int v, int nb, dou
 // U = L00^-1 * R : R, U are [v][ld] with n columns; R is destroyed
 int trsm_left_lower_unit(const double* A00T, const double* LinvT, int v, int nb, double* R, double* U, int64_t ld,
                          int n, cudaStream_t stream);
+
+// ---------------------------------------------------------------- validate.cu
+// out[i][c] = A[src_rows[i] * lda + c] for i < nrows, c < ncols (ncols, lda even; 16-byte aligned rows)
+int launch_gather_rows(const double* A, int64_t lda, const int* src_rows, int nrows, int ncols, double* out,
+                       cudaStream_t stream);
+
+// ---------------------------------------------------------------- solve.cu
+// D = beta * C + alpha * A * B: A [M x K] row-major (lda even, 16-byte aligned), B [K x N], C / D [M x N] (D may alias
+// C; C is read only when beta != 0).  K % 4 == 0; any M, N >= 1.  Memory-bound on A: the narrow GEMM of the solve.
+int launch_gemm_narrow(int M, int N, int K, const double* A, int64_t lda, const double* B, int64_t ldb, const double* C,
+                       int64_t ldc, double* D, int64_t ldd, double alpha, double beta, cudaStream_t stream);
 
 }  // namespace cflx

@@ -497,10 +497,11 @@ void free_lu(cflx_lu* lu) {
     if (!lu) return;
     cudaSetDevice(lu->comm->device);
     double* dbl[] = {lu->A0, lu->A11, lu->PT, lu->PT2, lu->W, lu->LT, lu->A01raw, lu->U, lu->tmp, lu->A00, lu->A00T,
-                     lu->Uinv, lu->LinvT, lu->candH, lu->S, lu->W2, lu->bcast, lu->Cbuf, lu->xbuf};
+                     lu->Uinv, lu->LinvT, lu->candH, lu->S, lu->W2, lu->bcast, lu->Cbuf, lu->xbuf, lu->sv_inv,
+                     lu->sv_B, lu->sv_W, lu->sv_R, lu->sv_Y, lu->sv_X};
     for (double* p : dbl) cudaFree(p);
     int* ints[] = {lu->gri, lu->gri_tmp, lu->igri, lu->perm, lu->gpivots, lu->tagsH, lu->tagsS, lu->hist, lu->plan_mem,
-                   lu->idx_buf};
+                   lu->idx_buf, lu->sv_rows};
     for (int* p : ints) cudaFree(p);
     if (lu->h_npiv) cudaFreeHost(lu->h_npiv);
     if (lu->pws.slot_hdr) panel_workspace_destroy(&lu->pws);
@@ -792,6 +793,7 @@ int cflx_lu_set_local(cflx_lu* lu, const double* host_local) {
     CFLX_CUDA(cudaStreamSynchronize(lu->comm->stream));
     lu->have_input = true;
     lu->factored = false;
+    lu->solve_ready = false;
     lu->a0_is_next = false;
     lu->next_host = nullptr;
     return CFLX_OK;
@@ -834,6 +836,7 @@ int cflx_lu_factor(cflx_lu* lu, double* ms_out) {
         CFLX_CUDA(cudaMemcpyAsync(lu->A11, lu->A0, loc * sizeof(double), cudaMemcpyDeviceToDevice, s));
     }
     lu->a0_is_next = false;
+    lu->solve_ready = false;
     if (lu->next_host) {  // queued next input: overwrite A0 behind the working copy, concurrently with everything below
         CFLX_CUDA(cudaEventRecord(lu->ev_a0_read, s));
         CFLX_CUDA(cudaStreamWaitEvent(lu->copy, lu->ev_a0_read, 0));
@@ -973,6 +976,17 @@ int cflx_lu_validate(cflx_lu* lu, double* frob_abs_out, double* frob_rel_out) {
 int cflx_lu_residual(cflx_lu* lu, double* rel_out) {
     if (!rel_out) return CFLX_ERR_ARG;
     return cflx_lu_validate(lu, nullptr, rel_out);
+}
+
+// Reads only the factors, so a run whose input buffer was handed to the queued next matrix can still be solved.
+int cflx_lu_solve(cflx_lu* lu, int nrhs, const double* B, int ldb, double* X, int ldx) {
+    if (!lu || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B) return CFLX_ERR_ARG;
+    if (!lu->factored) {
+        set_last_error("solve requested before cflx_lu_factor, or after cflx_lu_set_local without a factorisation");
+        return CFLX_ERR_STATE;
+    }
+    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    return lu_solve_grid(lu, nrhs, B, ldb, X, ldx);
 }
 
 int cflx_host_alloc(size_t bytes, void** out) {

@@ -101,10 +101,18 @@ struct cflx_lu {
     std::vector<char> ev_used;
     cudaStream_t side = nullptr;  // high-priority look-ahead stream (null: no overlap)
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_npiv = nullptr;
+    // cflx_lu_solve (solve.cu): prepared by the first solve after a factorisation, dropped by set_local / factor
+    bool solve_ready = false;
+    double* sv_inv = nullptr;  // per owned diagonal tile: Linv blocks (v x nb, row-major nb x nb each), then Uinv blocks
+    int* sv_rows = nullptr;    // [Ml] row of B that local row r of P*B comes from (ranks (pi, 0, 0))
+    double *sv_B = nullptr, *sv_W = nullptr, *sv_R = nullptr, *sv_Y = nullptr, *sv_X = nullptr;  // work, sv_ldn columns
+    int sv_ldn = 0;
 };
 
 namespace cflx {
 // validate.cu
 int redistribute_pivoted_rows(cflx_lu* lu, const std::vector<int>& hist, bool factors, const double* src, double* dst);
 int lu_residual_grid(cflx_lu* lu, const std::vector<int>& hist, double* abs_out, double* rel_out);
+// solve.cu
+int lu_solve_grid(cflx_lu* lu, int nrhs, const double* B, int ldb, double* X, int ldx);
 }  // namespace cflx

@@ -281,10 +281,8 @@ __global__ void gather_perm_rows_kernel(const double* __restrict__ A, int64_t ld
     double* dst = out + (int64_t)r * n;
     for (int c = blockIdx.y * blockDim.x + threadIdx.x; c < n; c += gridDim.y * blockDim.x) dst[c] = src[c];
 }
-__global__ void sumsq_kernel(const double* __restrict__ X, int64_t count, double* __restrict__ out) {
-    double s = 0.0;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x)
-        s = fma(X[i], X[i], s);
+// sum of a block's values in a fixed order (warp shuffles, then the warps' sums by warp 0); the result is in thread 0
+__device__ __forceinline__ double block_sum(double s) {
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
     __shared__ double w[32];
     if ((threadIdx.x & 31) == 0) w[threadIdx.x >> 5] = s;
@@ -292,8 +290,24 @@ __global__ void sumsq_kernel(const double* __restrict__ X, int64_t count, double
     if (threadIdx.x < 32) {
         s = threadIdx.x < (blockDim.x >> 5) ? w[threadIdx.x] : 0.0;
         for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-        if (threadIdx.x == 0) atomicAdd(out, s);
     }
+    return s;
+}
+// Two passes with a fixed grid, so the sum is rounded the same way on every call: each CTA writes its partial sum, then
+// one CTA adds the partials in index order.  (One pass with an atomicAdd per CTA rounds in whatever order the CTAs
+// finish, so two runs over the same data could differ in the last bit.)
+__global__ void sumsq_partial_kernel(const double* __restrict__ X, int64_t count, double* __restrict__ partials) {
+    double s = 0.0;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x)
+        s = fma(X[i], X[i], s);
+    s = block_sum(s);
+    if (threadIdx.x == 0) partials[blockIdx.x] = s;
+}
+__global__ void sumsq_final_kernel(const double* __restrict__ partials, int n, double* __restrict__ out) {
+    double s = 0.0;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) s += partials[i];
+    s = block_sum(s);
+    if (threadIdx.x == 0) *out += s;
 }
 
 inline int row_chunks(int len) {
@@ -396,8 +410,10 @@ int launch_gather_perm_rows(const double* A, int64_t lda, const int* perm, int n
     gather_perm_rows_kernel<<<grid, 256, 0, s>>>(A, lda, perm, n, out);
     POST_LAUNCH();
 }
-int launch_sumsq(const double* X, int64_t count, double* out, cudaStream_t s) {
-    sumsq_kernel<<<1184, 256, 0, s>>>(X, count, out);
+int launch_sumsq(const double* X, int64_t count, double* out, double* partials, cudaStream_t s) {
+    sumsq_partial_kernel<<<SUMSQ_PARTIALS, 256, 0, s>>>(X, count, partials);
+    CFLX_CUDA(cudaGetLastError());
+    sumsq_final_kernel<<<1, 1024, 0, s>>>(partials, SUMSQ_PARTIALS, out);
     POST_LAUNCH();
 }
 int launch_fill(double* p, int64_t n, double val, cudaStream_t s) {

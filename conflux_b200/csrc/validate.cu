@@ -77,6 +77,15 @@ __global__ void extract_u_block_kernel(const double* __restrict__ C, int64_t ldc
 }
 }  // namespace
 
+int launch_gather_rows(const double* A, int64_t lda, const int* src_rows, int nrows, int ncols, double* out,
+                       cudaStream_t stream) {
+    if (nrows <= 0 || ncols <= 0) return CFLX_OK;
+    dim3 grid(std::max(1, std::min(32, ncols / 512)), nrows);
+    gather_rows_kernel<<<grid, 256, 0, stream>>>(A, lda, src_rows, nrows, ncols, out);
+    CFLX_CUDA(cudaGetLastError());
+    return CFLX_OK;
+}
+
 // dst (Ml x Nl, conflux layout of the PIVOTED matrix) <- rows of src.  factors: src = A11 (row i of a rank = its i-th
 // promoted row);  otherwise src = the pristine input A0 (row of global id g at its original local slot), i.e. dst = P*A.
 // Collective over the i-communicator of layer 0 (ranks with pk != 0 must not call).
@@ -160,7 +169,7 @@ int lu_residual_grid(cflx_lu* lu, const std::vector<int>& hist, double* abs_out,
         cudaFree(lu->xbuf);  // 2 x local matrix of staging: do not keep it alive after validation
         lu->xbuf = nullptr;
     };
-    if ((rc = dmalloc(&acc, 2))) return rc;
+    if ((rc = dmalloc(&acc, 2 + SUMSQ_PARTIALS))) return rc;  // the two sums, then the partials of launch_sumsq
     if (cudaMemsetAsync(acc, 0, 2 * sizeof(double), s) != cudaSuccess) rc = CFLX_ERR_CUDA;
     if (!rc && layer0) {
         if (!lu->Cbuf) rc = dmalloc(&lu->Cbuf, loc);
@@ -215,8 +224,8 @@ int lu_residual_grid(cflx_lu* lu, const std::vector<int>& hist, double* abs_out,
     }
     if (!rc && cudaGetLastError() != cudaSuccess) rc = CFLX_ERR_CUDA;
     if (!rc && layer0) {
-        rc = launch_sumsq(R, (int64_t)loc, acc, s);
-        if (!rc) rc = launch_sumsq(lu->A0, (int64_t)loc, acc + 1, s);
+        rc = launch_sumsq(R, (int64_t)loc, acc, acc + 2, s);
+        if (!rc) rc = launch_sumsq(lu->A0, (int64_t)loc, acc + 1, acc + 2, s);
     }
     if (!rc && lu->P > 1) {
         ncclResult_t r = ncclAllReduce(acc, acc, 2, ncclDouble, ncclSum, c->world, s);

@@ -254,4 +254,11 @@ double validate(lu_params<T>& gv, double* relative = nullptr) {
     return a;
 }
 
+// Solves A X = B with the factors of the last LU_rep (P A = L U), on the GPU grid, like LAPACK's getrs.  Collective.
+// B / X: M x nrhs row-major (M = gv.M, the padded size), ldb / ldx >= nrhs; B the same on every rank, X may be null.
+template <class T>
+void LU_solve(lu_params<T>& gv, int nrhs, const T* B, int ldb, T* X, int ldx) {
+    check(cflx_lu_solve(gv.plan, nrhs, B, ldb, X, ldx), "LU_solve");
+}
+
 }  // namespace conflux

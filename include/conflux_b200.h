@@ -95,6 +95,12 @@ int cflx_lu_get_permutation(cflx_lu*, int* permutation_out);
 int cflx_lu_validate(cflx_lu*, double* frob_abs_out, double* frob_rel_out);
 /* COLLECTIVE.  = cflx_lu_validate(lu, NULL, rel_out) */
 int cflx_lu_residual(cflx_lu*, double* rel_out);
+/* COLLECTIVE.  Solves A X = B with the factors of the last cflx_lu_factor (P A = L U), on the GPU grid.
+ * B: M x nrhs row-major host array (M = the padded size, info_out[0]), leading dimension ldb >= nrhs, the same on every
+ * rank.  X: M x nrhs row-major, ldx >= nrhs, may be NULL on any rank; the result is identical on every rank.
+ * The first call after a factorisation prepares and caches per-rank solve data; cflx_lu_set_local / cflx_lu_factor
+ * drop it.  Does not modify the factors or the input.  No singularity check (like getrs). */
+int cflx_lu_solve(cflx_lu*, int nrhs, const double* B, int ldb, double* X, int ldx);
 /* 1 when this plan's trailing update runs on the int8 wgmma digit-plane path (ozaki.cu), 0 for the FP64 DMMA kernel
  * (gemm.cu) */
 int cflx_lu_uses_ozaki(const cflx_lu*);
@@ -148,6 +154,9 @@ void cflx_chol_destroy(cflx_chol*);
 /* D = beta*C + alpha * AT^T * B with AT [K x M], B [K x N], C/D [M x N], all row-major, dense */
 int cflx_dbg_gemm_tn(int M, int N, int K, const double* AT, const double* B, const double* C, double alpha, double beta,
                      double* D, int reps, double* ms_out);
+/* D = beta*C + alpha * A * B with A [M x K], B [K x N], C/D [M x N], all row-major, dense: the narrow GEMM of the solve */
+int cflx_dbg_gemm_narrow(int M, int N, int K, const double* A, const double* B, const double* C, double alpha, double beta,
+                         double* D, int reps, double* ms_out);
 /* partial-pivot LU of an n x v row-major panel: perm_out[v], A00_out[v*v] (L00\U00), LU_out[n*v] rows unpermuted */
 int cflx_dbg_panel(int n, int v, const double* panel, int* perm_out, double* A00_out, double* LU_out, int reps,
                    double* ms_out);
