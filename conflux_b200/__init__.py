@@ -351,6 +351,31 @@ class dbg:
         return X, Y
 
     @staticmethod
+    def diag_inverse(A00, nb):
+        """Inverses of the nb x nb diagonal blocks of A00 = L\\U (v x v) on diag_inverse_kernel, as the TRSMs use them.
+        Returns (Uinv, LinvT), each (v // nb, nb, nb): inv(U_jj) and inv(L_jj)^T with L unit lower."""
+        A00 = np.ascontiguousarray(A00, dtype=np.float64)
+        v = A00.shape[0]
+        Uinv = np.empty((max(v // nb, 1), nb, nb))
+        LinvT = np.empty_like(Uinv)
+        check(lib().cflx_dbg_diag_inverse(v, int(nb), A00.ctypes.data, Uinv.ctypes.data, LinvT.ctypes.data), "dbg_diag_inverse")
+        return Uinv, LinvT
+
+    @staticmethod
+    def potrf_tile(A, variant=0):
+        """Cholesky of one v x v tile (lower triangle read) on the factorisation's kernels: variant 0 the one-CTA kernel,
+        1 the 128 x 128 block kernel, 2 the 128-block tile driver.  Returns (L, L^T, info); info = 1 + the first
+        non-positive pivot's column, 0 on success."""
+        A = np.ascontiguousarray(A, dtype=np.float64)
+        v = A.shape[0]
+        L = np.empty((v, v))
+        LT = np.empty((v, v))
+        info = ctypes.c_int()
+        check(lib().cflx_dbg_potrf_tile(v, A.ctypes.data, L.ctypes.data, LT.ctypes.data, ctypes.byref(info), int(variant)),
+              "dbg_potrf_tile")
+        return L, LT, info.value
+
+    @staticmethod
     def ozaki_gemm(AT, B, C=None, reps=1, want_planes=False):
         """D = C - AT^T @ B on the int8 wgmma path.  Returns dict(D, ms, split_ms[, pa, pb, ea, eb])."""
         AT = np.ascontiguousarray(AT, dtype=np.float64)

@@ -18,6 +18,7 @@
 // in the LU path, so the TRSM and the rank-v update run on the same FP64 tensor-core GEMM (gemm.cu) on long contiguous
 // operands instead of v x v tile calls.  The "A10 -> A01 representative" exchange of the reference (every rank needs the
 // panel rows of its tile rows AND of its tile columns) is one grouped broadcast of the Px panel pieces to all ranks.
+#include <climits>
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
@@ -49,10 +50,12 @@ namespace {
 // Cholesky of one v x v tile (row-major, lower triangle referenced) by ONE CTA: right-looking, 32-column blocks.
 //   D   in: the tile; out: L in the lower triangle, zeros above
 //   UT  out: L^T (upper triangular, row-major) -- the operand of the panel TRSM and what is broadcast
-// info[0] = 1 + index of the first non-positive pivot (0 = success), like LAPACK's dpotrf.
+// info[0] = 1 + global index of the first non-positive pivot (0 = success), like LAPACK's dpotrf.  It is written with
+// atomicCAS(info, 0, .), so the first failure of a factorisation is kept: after it, NaNs reach every later diagonal
+// block, and each of those fails again.
 constexpr int PB = 32;
 // D: v x v window (leading dimension ldd) of the tile, UT: the same window of L^T (leading dimension ldu); Uc (optional): a
-// contiguous v x v copy of the factored block's L^T; col_off: column of the window inside the whole tile (for *info)
+// contiguous v x v copy of the factored block's L^T; col_off: global column of the window's first column (for *info)
 __global__ void __launch_bounds__(1024) potrf_tile_kernel(double* __restrict__ D, int v, int ldd, double* __restrict__ UT, int ldu,
                                                           double* __restrict__ Uc, int* __restrict__ info, int col_off) {
     extern __shared__ double sm[];
@@ -168,7 +171,7 @@ __global__ void __launch_bounds__(1024) potrf_tile_kernel(double* __restrict__ D
         __syncthreads();
         for (int e = t; e < v * v; e += blockDim.x) Uc[e] = UT[(size_t)(e / v) * ldu + e % v];
     }
-    if (t == 0 && s_bad) info[0] = s_bad;
+    if (t == 0 && s_bad) atomicCAS(info, 0, s_bad);
 }
 
 // Cholesky of ONE 128 x 128 diagonal block held entirely in shared memory (the building block of potrf_tile): all 512
@@ -248,7 +251,7 @@ __global__ void __launch_bounds__(QTHREADS) potrf128_kernel(double* __restrict__
         UT[(size_t)r * ldu + c] = lt;
         Uc[e] = lt;
     }
-    if (t == 0 && s_bad) info[0] = s_bad;
+    if (t == 0 && s_bad) atomicCAS(info, 0, s_bad);
 }
 
 // zeros above the diagonal of D (= L) and below the diagonal of UT (= L^T)
@@ -291,9 +294,10 @@ __global__ void gather_cols_kernel(GatherArgs a) {
     double* dst = a.Bc + (int64_t)c * a.ldb + (int64_t)t * a.v;
     for (int x = threadIdx.x; x < a.v; x += blockDim.x) dst[x] = src[x];
 }
-// sum of squares of the lower triangle (global row >= global column) of a local block-cyclic array
+// sum of squares of the lower triangle (global row >= global column) of a local block-cyclic array: partials[blockIdx.x]
+// = this CTA's share; launch_sum_partials then adds them in index order, so every call rounds the same way
 __global__ void sumsq_lower_kernel(const double* __restrict__ X, int Ml, int Nl, int v, int Px, int Py, int pi, int pj,
-                                   double* __restrict__ out) {
+                                   double* __restrict__ partials) {
     double s = 0.0;
     const int64_t total = (int64_t)Ml * Nl;
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
@@ -308,9 +312,12 @@ __global__ void sumsq_lower_kernel(const double* __restrict__ X, int Ml, int Nl,
     if (threadIdx.x < 32) {
         s = threadIdx.x < (blockDim.x >> 5) ? w[threadIdx.x] : 0.0;
         for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-        if (threadIdx.x == 0) atomicAdd(out, s);
+        if (threadIdx.x == 0) partials[blockIdx.x] = s;
     }
 }
+// info[2] = info[1], or INT_MAX when this rank saw no failure: the operand of the ncclMin that finds the first failing
+// column over the grid
+__global__ void info_min_operand_kernel(int* info) { info[2] = info[1] ? info[1] : INT_MAX; }
 // validation: transposed panel of column block t out of the stored factor, the diagonal tile masked to its lower triangle
 __global__ void extract_l_panel_T_kernel(const double* __restrict__ A, int64_t lda, int row0, int col0, int n, int v, int Px,
                                          int pi, int t, double* __restrict__ PT, int64_t ldp) {
@@ -476,21 +483,40 @@ int broadcast_and_update(cflx_chol* ch, int t, int jmin, bool below_only, double
     return update_columns(ch, gfirst, jmin, 0, X, 0, ch->Nl / ch->v, s);
 }
 
-// Panel pipeline of step k on stream s: z-reduce of tile column k, Cholesky of the diagonal tile, L_kk^T down the grid
-// column, the panel solve, the stores, and (k < Kappa - 1) the broadcast of the panel pieces into buffer set k & 1.
-// (1) Cholesky of the v x v diagonal tile.  One CTA alone is far too slow for a 512 x 512 tile (it would sit on
+size_t potrf_tile_smem(int v) { return ((size_t)PB * (PB + 1) + (size_t)v * (PB + 1)) * sizeof(double); }
+}  // namespace
+
+namespace cflx {
+size_t potrf_tile_scratch(int v) { return (v % QBK == 0 && v >= 2 * QBK) ? (size_t)3 * QBK * QBK + (size_t)2 * QBK * v : 0; }
+
+// raise-only: a smaller v (another object, a test hook) never lowers the limit a live object relies on
+int potrf_setup(int v) {
+    static PerDeviceMax tile_cfg, blk_cfg;
+    if (tile_cfg.raise(potrf_tile_smem(v)))
+        CFLX_CUDA(cudaFuncSetAttribute(potrf_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)potrf_tile_smem(v)));
+    if (blk_cfg.raise(QBK * QPITCH * sizeof(double)))
+        CFLX_CUDA(cudaFuncSetAttribute(potrf128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(QBK * QPITCH * sizeof(double))));
+    return CFLX_OK;
+}
+
+int potrf_block128(double* D, int ldd, double* UT, int ldu, double* Uc, int* info, int col0, cudaStream_t s) {
+    potrf128_kernel<<<1, QTHREADS, QBK * QPITCH * sizeof(double), s>>>(D, ldd, UT, ldu, Uc, info, col0);
+    CFLX_CUDA(cudaGetLastError());
+    return CFLX_OK;
+}
+
+// Cholesky of the v x v diagonal tile.  One CTA alone is far too slow for a 512 x 512 tile (it would sit on
 // the critical path of every step), so the tile is itself factored in 128-wide block columns: the 128 x 128 diagonal block on one CTA, the
 // block column below it by ONE GEMM with the inverted block, the trailing part of the tile by one rank-128 GEMM -- both on
-// the whole GPU (FP64 DMMA kernel).  Tiles that are not a multiple of 128 (tests) keep the one-CTA kernel.
-int potrf_tile(cflx_chol* ch, size_t psm, cudaStream_t s) {
-    const int v = ch->v;
+// the whole GPU (FP64 DMMA kernel).  Tiles that are not a multiple of 128 (tests), or Q == nullptr, keep the one-CTA kernel.
+int potrf_tile(double* D, double* A00, double* Q, int* info, int col0, int v, cudaStream_t s, int64_t* launches) {
     constexpr int QB = 128;
-    if (v % QB != 0 || v < 2 * QB || ch->Q == nullptr) {
-        potrf_tile_kernel<<<1, 1024, psm, s>>>(ch->D, v, v, ch->A00, v, nullptr, ch->info + 1, 0);
+    if (v % QB != 0 || v < 2 * QB || Q == nullptr) {
+        potrf_tile_kernel<<<1, 1024, potrf_tile_smem(v), s>>>(D, v, v, A00, v, nullptr, info, col0);
         CFLX_CUDA(cudaGetLastError());
         return CFLX_OK;
     }
-    double* U128 = ch->Q;                      // [QB][QB]  L_d^T of the current diagonal block, contiguous
+    double* U128 = Q;                          // [QB][QB]  L_d^T of the current diagonal block, contiguous
     double* Ui = U128 + QB * QB;               // [QB][QB]  its inverse
     double* Li = Ui + QB * QB;                 // [QB][QB]  (unit-lower companion of launch_diag_inverses, unused)
     double* XT0 = Li + QB * QB;                // [QB][v]   block column below the diagonal block, transposed
@@ -498,34 +524,36 @@ int potrf_tile(cflx_chol* ch, size_t psm, cudaStream_t s) {
     static_assert(QB == QBK, "block width of the tile Cholesky");
     for (int jb = 0; jb < v; jb += QB) {
         const int m = v - jb - QB;
-        potrf128_kernel<<<1, QTHREADS, QBK * QPITCH * sizeof(double), s>>>(ch->D + (size_t)jb * v + jb, v, ch->A00 + (size_t)jb * v + jb, v,
-                                                                        U128, ch->info + 1, jb);
-        CFLX_CUDA(cudaGetLastError());
-        ch->launches++;
+        CFLX_TRY(potrf_block128(D + (size_t)jb * v + jb, v, A00 + (size_t)jb * v + jb, v, U128, info, col0 + jb, s));
+        ++*launches;
         if (m <= 0) break;
         const int64_t ldx = m;
-        CFLX_TRY(launch_extract_panel_T(ch->D, v, jb + QB, jb, m, QB, XT0, ldx, s));
+        CFLX_TRY(launch_extract_panel_T(D, v, jb + QB, jb, m, QB, XT0, ldx, s));
         CFLX_TRY(launch_diag_inverses(U128, QB, QB, Ui, Li, s));
         CFLX_TRY(trsm_right_upper_T(U128, Ui, QB, QB, XT0, XT, ldx, m, s));          // X^T = L_d^-1 P^T
-        CFLX_TRY(launch_store_panel_T(ch->D, v, jb + QB, jb, m, QB, XT, ldx, s));
-        CFLX_CUDA(cudaMemcpy2DAsync(ch->A00 + (size_t)jb * v + jb + QB, (size_t)v * sizeof(double), XT, ldx * sizeof(double),
+        CFLX_TRY(launch_store_panel_T(D, v, jb + QB, jb, m, QB, XT, ldx, s));
+        CFLX_CUDA(cudaMemcpy2DAsync(A00 + (size_t)jb * v + jb + QB, (size_t)v * sizeof(double), XT, ldx * sizeof(double),
                                     (size_t)m * sizeof(double), QB, cudaMemcpyDeviceToDevice, s));
         GemmArgs g{};                                                                 // T -= X X^T
         g.M = m; g.N = m; g.K = QB;
         g.AT = XT; g.ldat = ldx;
         g.B = XT; g.ldb = ldx;
-        g.C = ch->D + (size_t)(jb + QB) * v + jb + QB; g.ldc = v;
-        g.D = ch->D + (size_t)(jb + QB) * v + jb + QB; g.ldd = v;
+        g.C = D + (size_t)(jb + QB) * v + jb + QB; g.ldc = v;
+        g.D = D + (size_t)(jb + QB) * v + jb + QB; g.ldd = v;
         g.alpha = -1.0; g.beta = 1.0;
         CFLX_TRY(launch_gemm_tn(g, s));
-        ch->launches += 6;
+        *launches += 6;
     }
-    tri_clean_kernel<<<(v * v + 255) / 256, 256, 0, s>>>(ch->D, ch->A00, v);
+    tri_clean_kernel<<<(v * v + 255) / 256, 256, 0, s>>>(D, A00, v);
     CFLX_CUDA(cudaGetLastError());
-    ch->launches++;
+    ++*launches;
     return CFLX_OK;
 }
+}  // namespace cflx
 
+namespace {
+// Panel pipeline of step k on stream s: z-reduce of tile column k, Cholesky of the diagonal tile, L_kk^T down the grid
+// column, the panel solve, the stores, and (k < Kappa - 1) the broadcast of the panel pieces into buffer set k & 1.
 int panel_step(cflx_chol* ch, int k, cudaStream_t s) {
     const int v = ch->v, Px = ch->Px, Py = ch->Py, Pz = ch->Pz, Ml = ch->Ml, Nl = ch->Nl;
     const int pi = ch->pi, pj = ch->pj, pk = ch->pk;
@@ -538,7 +566,6 @@ int panel_step(cflx_chol* ch, int k, cudaStream_t s) {
     const int64_t ld1 = piece_ld(ch, k + 1, pi);                 // rows strictly below tile k (what is broadcast)
     const bool on_col = (pj == pjk);
     const bool owner = on_col && pi == pik && pk == 0;
-    const size_t psm = ((size_t)PB * (PB + 1) + (size_t)v * (PB + 1)) * sizeof(double);
     // (4 of the previous step) tile column k summed over the z layers                  Cholesky.cpp:580-612
     if (on_col && n0 > 0) {
         CFLX_TRY(launch_extract_panel_T(ch->A11, Nl, row0, loff, n0, v, ch->PT, ld, s));
@@ -548,7 +575,7 @@ int panel_step(cflx_chol* ch, int k, cudaStream_t s) {
     // (1) Cholesky of the diagonal tile                                                 Cholesky.cpp:188-193
     if (owner) {
         tile_from_panel_kernel<<<(v * v + 255) / 256, 256, 0, s>>>(ch->PT, ld, v, ch->D);
-        CFLX_TRY(potrf_tile(ch, psm, s));
+        CFLX_TRY(potrf_tile(ch->D, ch->A00, ch->Q, ch->info + 1, k * v, v, s, &ch->launches));
         tile_store_kernel<<<(v * v + 255) / 256, 256, 0, s>>>(ch->D, v, ch->A11 + (int64_t)row0 * Nl + loff, Nl);
         CFLX_CUDA(cudaGetLastError());
         ch->launches += 3;
@@ -689,9 +716,9 @@ int cflx_chol_create(cflx_comm* c, int N, int v, int Px, int Py, int Pz, cflx_ch
     ALLOC(ch->A0, loc); ALLOC(ch->A11, loc);
     ALLOC(ch->PT, (size_t)v * ch->ldp); ALLOC(ch->LT, (size_t)v * ch->ldp); ALLOC(ch->W, (size_t)v * ch->ldp);
     ALLOC(ch->G, 2 * (size_t)Px * v * ch->ldp); ALLOC(ch->Bc, 2 * (size_t)v * ch->ldb);
-    ALLOC(ch->D, vv); ALLOC(ch->A00, vv); ALLOC(ch->Uinv, vv); ALLOC(ch->LinvT, vv); ALLOC(ch->acc, 4);
+    ALLOC(ch->D, vv); ALLOC(ch->A00, vv); ALLOC(ch->Uinv, vv); ALLOC(ch->LinvT, vv); ALLOC(ch->acc, 2 + SUMSQ_PARTIALS);
     ALLOC(ch->info, 4);
-    if (v % 128 == 0 && v >= 256) ALLOC(ch->Q, (size_t)3 * 128 * 128 + (size_t)2 * 128 * v);
+    if (potrf_tile_scratch(v)) ALLOC(ch->Q, potrf_tile_scratch(v));
 #undef ALLOC
     cudaMemsetAsync(ch->PT, 0, (size_t)v * ch->ldp * sizeof(double), c->stream);
     cudaMemsetAsync(ch->LT, 0, (size_t)v * ch->ldp * sizeof(double), c->stream);
@@ -717,9 +744,7 @@ int cflx_chol_create(cflx_comm* c, int N, int v, int Px, int Py, int Pz, cflx_ch
                 cudaEventCreateWithFlags(&ch->ev_panel[i], cudaEventDisableTiming) != cudaSuccess)
                 return fail(CFLX_ERR_CUDA);
     }
-    const size_t psm = ((size_t)PB * (PB + 1) + (size_t)v * (PB + 1)) * sizeof(double);
-    if (cudaFuncSetAttribute(potrf_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm) != cudaSuccess) return fail(CFLX_ERR_CUDA);
-    if (cudaFuncSetAttribute(potrf128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(QBK * QPITCH * sizeof(double))) != cudaSuccess) return fail(CFLX_ERR_CUDA);
+    if ((rc = potrf_setup(v))) return fail(rc);
     if (cudaStreamSynchronize(c->stream) != cudaSuccess) return fail(CFLX_ERR_CUDA);
     *out = ch;
     return CFLX_OK;
@@ -794,8 +819,20 @@ int cflx_chol_factor(cflx_chol* ch, double* ms_out) {
     CFLX_CUDA(cudaGetLastError());
     int h[4] = {0, 0, 0, 0};
     CFLX_CUDA(cudaMemcpy(h, ch->info, sizeof(h), cudaMemcpyDeviceToHost));
-    if (h[1] != 0) {
-        set_last_error("cholesky: the matrix is not positive definite (a diagonal tile failed at column %d)", h[1]);
+    int bad = h[1];   // 1 + first failing global column of the diagonal tiles this rank factored, 0 = none
+    if (ch->P > 1) {  // the first one over the grid, so that every rank returns the same status and column
+        // info[2] is prepared on s, in stream order with the all-reduce that reads it (not an error-handling launch of
+        // the factorisation, so it is not counted)
+        info_min_operand_kernel<<<1, 1, 0, s>>>(ch->info);
+        CFLX_CUDA(cudaGetLastError());
+        CFLX_NCCL(ncclAllReduce(ch->info + 2, ch->info + 2, 1, ncclInt, ncclMin, c->world, s));
+        int x = 0;
+        CFLX_CUDA(cudaMemcpyAsync(&x, ch->info + 2, sizeof(int), cudaMemcpyDeviceToHost, s));
+        CFLX_CUDA(cudaStreamSynchronize(s));
+        bad = x == INT_MAX ? 0 : x;
+    }
+    if (bad != 0) {
+        set_last_error("cholesky: the matrix is not positive definite (first non-positive pivot in column %d, counted from 1 like LAPACK dpotrf's info)", bad);
         return CFLX_ERR_STATE;
     }
     if (ms_out) *ms_out = ms;
@@ -865,9 +902,19 @@ int cflx_chol_validate(cflx_chol* ch, double* abs_out, double* rel_out) {
         ch->pk = pk_save;
     }
     if (!rc && cudaMemsetAsync(ch->acc, 0, 2 * sizeof(double), s) != cudaSuccess) rc = CFLX_ERR_CUDA;
-    if (!rc && pk_save == 0) {
-        sumsq_lower_kernel<<<1184, 256, 0, s>>>(R, Ml, Nl, v, Px, Py, ch->pi, ch->pj, ch->acc);
-        sumsq_lower_kernel<<<1184, 256, 0, s>>>(ch->A0, Ml, Nl, v, Px, Py, ch->pi, ch->pj, ch->acc + 1);
+    if (!rc && pk_save == 0) {   // acc = {the two sums, the per-CTA partials}
+        auto launch_error = []() -> int {
+            CFLX_CUDA(cudaGetLastError());
+            return CFLX_OK;
+        };
+        sumsq_lower_kernel<<<SUMSQ_PARTIALS, 256, 0, s>>>(R, Ml, Nl, v, Px, Py, ch->pi, ch->pj, ch->acc + 2);
+        rc = launch_error();
+        if (!rc) rc = launch_sum_partials(ch->acc + 2, SUMSQ_PARTIALS, ch->acc, s);
+        if (!rc) {
+            sumsq_lower_kernel<<<SUMSQ_PARTIALS, 256, 0, s>>>(ch->A0, Ml, Nl, v, Px, Py, ch->pi, ch->pj, ch->acc + 2);
+            rc = launch_error();
+        }
+        if (!rc) rc = launch_sum_partials(ch->acc + 2, SUMSQ_PARTIALS, ch->acc + 1, s);
     }
     if (!rc && ch->P > 1 && ncclAllReduce(ch->acc, ch->acc, 2, ncclDouble, ncclSum, c->world, s) != ncclSuccess) rc = CFLX_ERR_NCCL;
     double h[2] = {0, 0};

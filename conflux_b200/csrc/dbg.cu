@@ -329,6 +329,54 @@ int cflx_dbg_trsm(int n, int v, const double* A00, const double* B, double* X_ou
     return CFLX_OK;
 }
 
+// inverses of the nb x nb diagonal blocks of the v x v row-major A00 = L\U: Uinv_out / LinvT_out are [v / nb][nb][nb]
+int cflx_dbg_diag_inverse(int v, int nb, const double* A00, double* Uinv_out, double* LinvT_out) {
+    CFLX_TRY(check_device());
+    if (v <= 0 || nb <= 0 || v % nb != 0 || !A00) return CFLX_ERR_ARG;
+    const size_t vv = (size_t)v * v, blocks = (size_t)v * nb;
+    DevBuf dA, dU, dL;
+    CFLX_TRY(dA.alloc(8 * vv));
+    CFLX_TRY(dU.alloc(8 * blocks));
+    CFLX_TRY(dL.alloc(8 * blocks));
+    CFLX_CUDA(cudaMemcpy(dA.p, A00, 8 * vv, cudaMemcpyHostToDevice));
+    CFLX_TRY(launch_diag_inverses(dA.as<double>(), v, nb, dU.as<double>(), dL.as<double>(), 0));
+    if (Uinv_out) CFLX_CUDA(cudaMemcpy(Uinv_out, dU.p, 8 * blocks, cudaMemcpyDeviceToHost));
+    if (LinvT_out) CFLX_CUDA(cudaMemcpy(LinvT_out, dL.p, 8 * blocks, cudaMemcpyDeviceToHost));
+    CFLX_CUDA(cudaDeviceSynchronize());
+    return CFLX_OK;
+}
+
+// Cholesky of one v x v row-major tile A (lower triangle read) on the kernels of the factorisation.  variant 0: the
+// one-CTA potrf_tile_kernel (4 <= v <= 512); 1: potrf128_kernel (v == 128); 2: the 128-block driver potrf_tile()
+// (v % 128 == 0, v >= 256).  L_out = L (zeros above the diagonal), LT_out = L^T, info_out = 1 + first failing column or 0.
+int cflx_dbg_potrf_tile(int v, const double* A, double* L_out, double* LT_out, int* info_out, int variant) {
+    CFLX_TRY(check_device());
+    if (!A || v < 4 || v > 512 || variant < 0 || variant > 2 || (variant == 1 && v != 128) ||
+        (variant == 2 && potrf_tile_scratch(v) == 0))
+        return CFLX_ERR_ARG;
+    const size_t vv = (size_t)v * v;
+    DevBuf dD, dUT, dUc, dQ, dinfo;
+    CFLX_TRY(dD.alloc(8 * vv));
+    CFLX_TRY(dUT.alloc(8 * vv));
+    CFLX_TRY(dUc.alloc(8 * vv));
+    CFLX_TRY(dinfo.alloc(sizeof(int)));
+    if (variant == 2) CFLX_TRY(dQ.alloc(8 * potrf_tile_scratch(v)));
+    CFLX_CUDA(cudaMemcpy(dD.p, A, 8 * vv, cudaMemcpyHostToDevice));
+    CFLX_CUDA(cudaMemset(dUT.p, 0, 8 * vv));
+    CFLX_CUDA(cudaMemset(dinfo.p, 0, sizeof(int)));
+    CFLX_TRY(potrf_setup(v));
+    int64_t launches = 0;
+    if (variant == 1)
+        CFLX_TRY(potrf_block128(dD.as<double>(), v, dUT.as<double>(), v, dUc.as<double>(), dinfo.as<int>(), 0, 0));
+    else
+        CFLX_TRY(potrf_tile(dD.as<double>(), dUT.as<double>(), dQ.as<double>(), dinfo.as<int>(), 0, v, 0, &launches));
+    if (L_out) CFLX_CUDA(cudaMemcpy(L_out, dD.p, 8 * vv, cudaMemcpyDeviceToHost));
+    if (LT_out) CFLX_CUDA(cudaMemcpy(LT_out, dUT.p, 8 * vv, cudaMemcpyDeviceToHost));
+    if (info_out) CFLX_CUDA(cudaMemcpy(info_out, dinfo.p, sizeof(int), cudaMemcpyDeviceToHost));
+    CFLX_CUDA(cudaDeviceSynchronize());
+    return CFLX_OK;
+}
+
 // step 2 of the LU loop in isolation on ONE rank (Px = 1): plan_moves (analyze_pivots) + push_phase1..3 (push_pivots_up,
 // conflux_opt.hpp:176-218) + the gri/igri bookkeeping, on an n_rows x n_cols row-major matrix (n_cols even).  The npiv
 // pivot rows (local indices >= fnpr, tournament order) end up in rows [fnpr, fnpr+npiv) in that order.

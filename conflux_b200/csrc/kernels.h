@@ -118,6 +118,8 @@ int launch_gather_perm_rows(const double* A, int64_t lda, const int* perm, int n
 // *out += sum of X[i]^2, deterministic (the same rounding on every call); partials: SUMSQ_PARTIALS doubles of scratch
 constexpr int SUMSQ_PARTIALS = 1184;
 int launch_sumsq(const double* X, int64_t count, double* out, double* partials, cudaStream_t stream);
+// *out += partials[0] + ... + partials[n - 1], added in a fixed order (the second pass of launch_sumsq)
+int launch_sum_partials(const double* partials, int n, double* out, cudaStream_t stream);
 // misc
 int launch_fill(double* p, int64_t n, double val, cudaStream_t stream);
 int launch_iota_gri(int* gri, int* igri, int Ml, int v, int Px, int pi, cudaStream_t stream);
@@ -134,6 +136,17 @@ int trsm_right_upper_T(const double* A00, const double* Uinv, int v, int nb, dou
 // U = L00^-1 * R : R, U are [v][ld] with n columns; R is destroyed
 int trsm_left_lower_unit(const double* A00T, const double* LinvT, int v, int nb, double* R, double* U, int64_t ld,
                          int n, cudaStream_t stream);
+
+// ---------------------------------------------------------------- chol.cu
+// Cholesky of one v x v diagonal tile D (row-major, lower triangle read) in place: L in the lower triangle, zeros above,
+// and L^T into UT.  Q (potrf_tile_scratch(v) doubles) selects the 128-block path for v % 128 == 0, v >= 256; Q == nullptr
+// or any other v runs the one-CTA kernel (4 <= v <= 512).  A non-positive pivot at local column j sets *info = col0 + j + 1
+// unless *info is already non-zero.  *launches grows by the launches the 128-block path counts.  potrf_setup(v) first.
+size_t potrf_tile_scratch(int v);
+int potrf_setup(int v);
+int potrf_tile(double* D, double* UT, double* Q, int* info, int col0, int v, cudaStream_t stream, int64_t* launches);
+// one 128 x 128 block (leading dimensions ldd / ldu) on potrf128_kernel; Uc: a contiguous 128 x 128 copy of L^T
+int potrf_block128(double* D, int ldd, double* UT, int ldu, double* Uc, int* info, int col0, cudaStream_t stream);
 
 // ---------------------------------------------------------------- validate.cu
 // out[i][c] = A[src_rows[i] * lda + c] for i < nrows, c < ncols (ncols, lda even; 16-byte aligned rows)

@@ -413,7 +413,10 @@ int launch_gather_perm_rows(const double* A, int64_t lda, const int* perm, int n
 int launch_sumsq(const double* X, int64_t count, double* out, double* partials, cudaStream_t s) {
     sumsq_partial_kernel<<<SUMSQ_PARTIALS, 256, 0, s>>>(X, count, partials);
     CFLX_CUDA(cudaGetLastError());
-    sumsq_final_kernel<<<1, 1024, 0, s>>>(partials, SUMSQ_PARTIALS, out);
+    return launch_sum_partials(partials, SUMSQ_PARTIALS, out, s);
+}
+int launch_sum_partials(const double* partials, int n, double* out, cudaStream_t s) {
+    sumsq_final_kernel<<<1, 1024, 0, s>>>(partials, n, out);
     POST_LAUNCH();
 }
 int launch_fill(double* p, int64_t n, double val, cudaStream_t s) {

@@ -162,6 +162,13 @@ int cflx_dbg_panel(int n, int v, const double* panel, int* perm_out, double* A00
                    double* ms_out);
 /* X = B * U^-1 (right, upper, non-unit; B n x v) and Y = L^-1 * R (left, lower, unit; R v x n), A00 = L\U packed */
 int cflx_dbg_trsm(int n, int v, const double* A00, const double* B, double* X_out, const double* R, double* Y_out);
+/* inverses of the nb x nb diagonal blocks of A00 = L\U (v x v, nb in 4, 8, ..., 128, v % nb == 0) as the TRSMs use them:
+ * Uinv_out[v / nb][nb][nb] = inv(U_jj), LinvT_out[v / nb][nb][nb] = inv(L_jj)^T (L unit lower); only the blocks are read */
+int cflx_dbg_diag_inverse(int v, int nb, const double* A00, double* Uinv_out, double* LinvT_out);
+/* Cholesky of one v x v row-major tile (lower triangle read) as the factorisation runs it.  variant 0: one-CTA kernel,
+ * 4 <= v <= 512; 1: the 128 x 128 block kernel, v == 128; 2: the 128-block tile driver, v % 128 == 0 and v >= 256.
+ * L_out = L with zeros above the diagonal, LT_out = L^T, info_out = 1 + first non-positive pivot's column, or 0. */
+int cflx_dbg_potrf_tile(int v, const double* A, double* L_out, double* LT_out, int* info_out, int variant);
 /* D = C - AT^T * B on the int8 wgmma path (error-free digit planes, ozaki.cu); K % 128 == 0, N even.  Optional test
  * outputs: digit planes [8][M][K] / [8][N][K], exponents [M] / [N].  ms_out / split_ms_out: mean device time of the GEMM
  * kernel / of the two digit-plane kernels. */

@@ -52,3 +52,24 @@ def init_matrix(N, v):
             A[i * v:(i + 1) * v, j * v:(j + 1) * v] = T
         A[i * v:(i + 1) * v, i * v:(i + 1) * v][np.diag_indices(v)] = mx
     return A, T, mx
+
+
+# fixed inputs whose default-path factors are pinned bit for bit by tests/golden/chol_factor_bits.json
+# (tests/golden/make_chol_golden.py): the library's own generator, and integer matrices M M^T + N I, exact in any
+# summation order, so the input is the same bits on every machine
+BITS_CASES = [("gen", 100, 16), ("gen", 256, 32), ("gen", 512, 128), ("gen", 1024, 256), ("gen", 2048, 512),
+              ("int", 480, 48), ("int", 800, 100), ("int", 1152, 384), ("int", 2048, 256)]
+
+
+def bits_case_input(kind, N):
+    """None = the library's generator; else the integer SPD matrix of the case (float64, exact)"""
+    if kind == "gen":
+        return None
+    M = np.random.default_rng(N).integers(-8, 9, (N, N)).astype(np.float64)
+    return M @ M.T + N * np.eye(N)       # every entry: N products of magnitude <= 64, exact in float64
+
+
+def factor_digest(L):
+    """sha256 of the lower triangle of a factor, as float64 bytes"""
+    import hashlib
+    return hashlib.sha256(np.ascontiguousarray(np.tril(L), dtype=np.float64).tobytes()).hexdigest()

@@ -1,0 +1,144 @@
+"""CPU: the extended-precision references of oracle/hp_ref.py are accurate, and each error-bound check they provide is
+sharp: it accepts a correctly rounded float64 restatement of the algorithm and rejects the same computation with one
+realistic defect (a term dropped from one trailing update, one wrong entry in one inverse block, a one-column shift in
+one 32-column block)."""
+from fractions import Fraction
+
+import numpy as np
+import pytest
+import scipy.linalg
+
+from oracle import hp_ref as hp
+
+LD = hp.LD
+
+
+def _chol64(A, drop=None):
+    """right-looking Cholesky in float64, 32-column blocks like potrf_tile_kernel; drop = (i, j, k): leave the term
+    L[i,k] L[j,k] out of the update of entry (i, j)"""
+    S = np.tril(np.array(A, dtype=np.float64))
+    n = S.shape[0]
+    for k in range(n):
+        S[k, k] = np.sqrt(S[k, k])
+        S[k + 1:, k] /= S[k, k]
+        upd = np.tril(np.outer(S[k + 1:, k], S[k + 1:, k]))
+        if drop is not None and drop[2] == k:
+            upd[drop[0] - k - 1, drop[1] - k - 1] = 0.0
+        S[k + 1:, k + 1:] -= upd
+    return np.tril(S)
+
+
+def _inv_upper64(U, drop=None):
+    """inv(U) by substitution, column by column, in float64; drop = (r, c, t): leave U[r,t] X[t,c] out of entry (r, c)"""
+    n = U.shape[0]
+    X = np.zeros((n, n))
+    for c in range(n):
+        X[c, c] = 1.0 / U[c, c]
+        for r in range(c - 1, -1, -1):
+            terms = U[r, r + 1:c + 1] * X[r + 1:c + 1, c]
+            if drop is not None and drop[:2] == (r, c):
+                terms[drop[2] - r - 1] = 0.0
+            X[r, c] = -terms.sum() / U[r, r]
+    return X
+
+
+def test_matmul_is_exact_to_extended_precision():
+    rng = np.random.default_rng(0)
+    X = rng.standard_normal((6, 300)) * np.logspace(-3, 3, 300)
+    Y = rng.standard_normal((300, 5))
+    C = hp.matmul(X, Y)
+    for i in range(6):
+        for j in range(5):
+            exact = sum(Fraction(float(a)) * Fraction(float(b)) for a, b in zip(X[i], Y[:, j]))
+            scale = Fraction(float(np.abs(X[i]) @ np.abs(Y[:, j])))
+            assert abs(Fraction(float(C[i, j])) + Fraction(float(C[i, j] - LD(float(C[i, j])))) - exact) <= scale * Fraction(2) ** -62
+
+
+def test_longdouble_cholesky_and_inverse_are_extended_precision():
+    rng = np.random.default_rng(1)
+    A = hp.random_spd(300, 1e6, rng)
+    L, info = hp.cholesky(A, block=64)
+    assert info == 0
+    R = np.abs(np.tril(A.astype(LD) - L @ L.T))          # longdouble matmul: slow, but exact enough at n = 300
+    assert np.all(R <= LD(2.0 ** -64 * 4 * 300) * np.tril(np.abs(L) @ np.abs(L).T))
+    X = hp.tri_inverse(L, lower=True)
+    assert np.all(np.abs(L @ X - np.eye(300, dtype=LD)) <= LD(2.0 ** -64 * 4 * 300) * (np.abs(L) @ np.abs(X)))
+    # and the factor is the one LAPACK approximates
+    assert np.abs(np.asarray(L, dtype=np.float64) - np.linalg.cholesky(A)).max() <= 1e-9
+
+
+def test_exact_input_is_factored_exactly():
+    rng = np.random.default_rng(2)
+    A, L0 = hp.exact_spd(96, rng)
+    L, info = hp.cholesky(A, block=32)
+    assert info == 0 and np.array_equal(np.asarray(L, dtype=np.float64), L0)
+    assert np.array_equal(_chol64(A), L0)
+
+
+@pytest.mark.parametrize("k0", [0, 37, 95])
+def test_not_positive_definite_info_is_lapacks(k0):
+    rng = np.random.default_rng(3)
+    A, L0 = hp.exact_spd(96, rng)
+    A[k0, k0] -= L0[k0, k0] ** 2 + 0.5
+    assert hp.cholesky(A, block=32)[1] == k0 + 1 == scipy.linalg.lapack.dpotrf(A, lower=1)[1]
+
+
+def test_cholesky_checks_accept_float64_and_reject_a_dropped_update_term():
+    rng = np.random.default_rng(4)
+    n = 160
+    A = hp.random_spd(n, 1e4, rng)
+    Lref, _ = hp.cholesky(A)
+    L = _chol64(A)
+    kmax = hp.diag_block_kappa(L, 32)
+    assert hp.chol_componentwise_ok(A, L) and hp.chol_normwise_ok(A, L, kmax) and hp.chol_forward_ok(A, L, Lref, kmax)
+    Lbad = _chol64(A, drop=(120, 70, 40))                  # one term of one trailing update missing
+    assert not hp.chol_componentwise_ok(A, Lbad)
+    assert not hp.chol_normwise_ok(A, Lbad, kmax)
+    assert not hp.chol_forward_ok(A, Lbad, Lref, kmax)
+
+
+def test_cholesky_checks_reject_a_one_column_shift_in_one_block():
+    rng = np.random.default_rng(5)
+    n = 128
+    A = hp.random_spd(n, 1e2, rng)
+    L = _chol64(A)
+    Lbad = L.copy()
+    Lbad[64:, 33:64] = L[64:, 32:63]                       # the block below diagonal block 1 stored one column right
+    kmax = hp.diag_block_kappa(L, 32)
+    assert hp.chol_componentwise_ok(A, L)
+    assert not hp.chol_componentwise_ok(A, Lbad)
+    assert not hp.chol_normwise_ok(A, Lbad, kmax)
+
+
+def test_transposed_factor_is_rejected():
+    rng = np.random.default_rng(6)
+    A = hp.random_spd(64, 10.0, rng)
+    L = _chol64(A)
+    assert not hp.chol_componentwise_ok(A, L.T)
+
+
+@pytest.mark.parametrize("kind", ["plain", "graded"])
+def test_inverse_check_accepts_substitution_and_rejects_one_wrong_entry(kind):
+    rng = np.random.default_rng(7)
+    n = 64
+    U = np.triu(rng.uniform(-1, 1, (n, n))) * 0.2 + np.diag(1.0 + rng.random(n))
+    if kind == "graded":
+        U = np.logspace(-6, 6, n)[:, None] * U
+    X = _inv_upper64(U)
+    assert hp.inverse_componentwise_ok(U, X)
+    Xlong = hp.tri_inverse(U, lower=False)
+    assert np.abs(X - np.asarray(Xlong, dtype=np.float64)).max() <= 1e-10 * np.abs(X).max()
+    assert not hp.inverse_componentwise_ok(U, _inv_upper64(U, drop=(10, 40, 25)))
+    Xbad = X.copy()
+    Xbad[5, 50] *= 1 + 2.0 ** -30                          # one entry off at the 2^-30 level
+    assert not hp.inverse_componentwise_ok(U, Xbad)
+
+
+def test_power_of_two_grading_commutes_with_the_factorisation():
+    """the property the graded GPU test relies on: for D = diag(2^k), the float64 factor of D S D is D times the float64
+    factor of S, bit for bit (in every order of summation; shown here for the right-looking restatement)"""
+    rng = np.random.default_rng(8)
+    n = 96
+    S = hp.random_spd(n, 1e2, rng)
+    d = 2.0 ** np.round(np.linspace(-10, 10, n))
+    assert np.array_equal(_chol64(d[:, None] * S * d[None, :]), d[:, None] * _chol64(S))
