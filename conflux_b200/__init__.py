@@ -259,6 +259,19 @@ class cholesky:
         check(lib().cflx_chol_validate(self._h, ctypes.byref(a), ctypes.byref(r)), "chol_validate")
         return a.value, r.value
 
+    def solve(self, B):
+        """Solves A X = B with the factor of the last parallelCholesky (A = L L^T) on the GPU grid, like LAPACK's potrs.
+        COLLECTIVE over the object's comm; every rank passes the same B, (N,) or (N, nrhs) with N = self.N (the padded
+        size), and gets the same X in the same shape.  The factor and the input are left as they are."""
+        B = np.asarray(B, dtype=np.float64)
+        if B.ndim not in (1, 2) or B.shape[0] != self.N:
+            raise ValueError(f"cholesky.solve: B must have shape ({self.N},) or ({self.N}, nrhs), got {B.shape}")
+        B2 = np.ascontiguousarray(B.reshape(self.N, -1))
+        nrhs = B2.shape[1]
+        X = np.empty_like(B2)
+        check(lib().cflx_chol_solve(self._h, nrhs, B2.ctypes.data, max(nrhs, 1), X.ctypes.data, max(nrhs, 1)), "chol_solve")
+        return X.reshape(B.shape)
+
     def finalize(self, clean=True):
         if self._h:
             lib().cflx_chol_destroy(self._h)
@@ -319,6 +332,28 @@ class dbg:
         ms = ctypes.c_double()
         check(lib().cflx_dbg_gemm_narrow(M, N, K, A.ctypes.data, B.ctypes.data, Cp, float(alpha), float(beta), D.ctypes.data,
                                          int(reps), ctypes.byref(ms)), "dbg_gemm_narrow")
+        return D, ms.value
+
+    @staticmethod
+    def gemm_narrow_tn(AT, B, C=None, alpha=1.0, beta=0.0, reps=1, out=None):
+        """D = beta*C + alpha * AT^T @ B on the Cholesky solve's transposed narrow GEMM (AT is K x M, read in place; any
+        K).  Returns (D, mean ms of one launch).  out: the array to write D into; passing C itself runs the kernel with D
+        aliasing C."""
+        AT = np.ascontiguousarray(AT, dtype=np.float64)
+        B = np.ascontiguousarray(B, dtype=np.float64)
+        K, M = AT.shape
+        if B.ndim != 2 or B.shape[0] != K:
+            raise ValueError(f"gemm_narrow_tn: B must have {K} rows, got shape {B.shape}")
+        N = B.shape[1]
+        Cp = None
+        if C is not None:
+            assert C.dtype == np.float64 and C.flags.c_contiguous and C.shape == (M, N)
+            Cp = C.ctypes.data
+        D = np.empty((M, N)) if out is None else out
+        assert D.dtype == np.float64 and D.flags.c_contiguous and D.shape == (M, N)
+        ms = ctypes.c_double()
+        check(lib().cflx_dbg_gemm_narrow_tn(M, N, K, AT.ctypes.data, B.ctypes.data, Cp, float(alpha), float(beta),
+                                            D.ctypes.data, int(reps), ctypes.byref(ms)), "dbg_gemm_narrow_tn")
         return D, ms.value
 
     @staticmethod

@@ -229,6 +229,51 @@ int cflx_dbg_gemm_narrow(int M, int N, int K, const double* A, const double* B, 
     return CFLX_OK;
 }
 
+// D = beta*C + alpha * AT^T * B on the transposed narrow GEMM (solve.cu), like cflx_dbg_gemm_narrow; AT [K x M] is stored
+// on the device with the even leading dimension round_up(M, 2), the kernel's condition, so odd M can be run.
+int cflx_dbg_gemm_narrow_tn(int M, int N, int K, const double* AT, const double* B, const double* C, double alpha,
+                            double beta, double* D, int reps, double* ms_out) {
+    CFLX_TRY(check_device());
+    if (M <= 0 || N <= 0 || K < 0 || !AT || !B) return CFLX_ERR_ARG;
+    const int64_t ldat = round_up(M, 2);
+    const size_t a_n = (size_t)K * ldat, b_n = (size_t)K * N, c_n = (size_t)M * N;
+    DevBuf dA, dB, dC, dT;
+    CFLX_TRY(dA.alloc(sizeof(double) * a_n));
+    CFLX_TRY(dB.alloc(sizeof(double) * b_n));
+    CFLX_TRY(dC.alloc(sizeof(double) * c_n));
+    CFLX_TRY(dT.alloc(sizeof(double) * c_n));
+    if (K > 0) {
+        CFLX_CUDA(cudaMemcpy2D(dA.p, ldat * 8, AT, (size_t)M * 8, (size_t)M * 8, K, cudaMemcpyHostToDevice));
+        CFLX_CUDA(cudaMemcpy(dB.p, B, sizeof(double) * b_n, cudaMemcpyHostToDevice));
+    }
+    if (C) CFLX_CUDA(cudaMemcpy(dC.p, C, sizeof(double) * c_n, cudaMemcpyHostToDevice));
+    else CFLX_CUDA(cudaMemset(dC.p, 0, sizeof(double) * c_n));
+    const bool alias = C && D == C;
+    auto run = [&](double* out) {
+        return launch_gemm_narrow_tn(M, N, K, dA.as<double>(), ldat, dB.as<double>(), N, dC.as<double>(), N, out, N, alpha,
+                                     beta, 0);
+    };
+    cudaEvent_t e0, e1;
+    CFLX_CUDA(cudaEventCreate(&e0));
+    CFLX_CUDA(cudaEventCreate(&e1));
+    if (reps < 1) reps = 1;
+    CFLX_TRY(run(dT.as<double>()));  // warm-up
+    CFLX_CUDA(cudaEventRecord(e0));
+    for (int r = 0; r < reps; ++r) CFLX_TRY(run(dT.as<double>()));
+    CFLX_CUDA(cudaEventRecord(e1));
+    CFLX_CUDA(cudaEventSynchronize(e1));
+    float ms = 0;
+    CFLX_CUDA(cudaEventElapsedTime(&ms, e0, e1));
+    if (ms_out) *ms_out = ms / reps;
+    cudaEventDestroy(e0);
+    cudaEventDestroy(e1);
+    double* out = alias ? dC.as<double>() : dT.as<double>();
+    CFLX_TRY(run(out));
+    if (D) CFLX_CUDA(cudaMemcpy(D, out, sizeof(double) * c_n, cudaMemcpyDeviceToHost));
+    CFLX_CUDA(cudaDeviceSynchronize());
+    return CFLX_OK;
+}
+
 int cflx_dbg_panel(int n, int v, const double* panel, int* perm_out, double* A00_out, double* LU_out, int reps,
                    double* ms_out) {
     CFLX_TRY(check_device());

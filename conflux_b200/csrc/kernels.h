@@ -158,5 +158,13 @@ int launch_gather_rows(const double* A, int64_t lda, const int* src_rows, int nr
 // C; C is read only when beta != 0).  K % 4 == 0; any M, N >= 1.  Memory-bound on A: the narrow GEMM of the solve.
 int launch_gemm_narrow(int M, int N, int K, const double* A, int64_t lda, const double* B, int64_t ldb, const double* C,
                        int64_t ldc, double* D, int64_t ldd, double alpha, double beta, cudaStream_t stream);
+// D = beta * C + alpha * AT^T * B: AT [K x M] row-major, read in place (ldat even and >= M, AT 16-byte aligned), B [K x N],
+// C / D [M x N] (D may alias C; C is read only when beta != 0).  Any K >= 0 and M, N >= 1; nothing beyond M, K or N is
+// read.  Otherwise CFLX_ERR_UNSUPPORTED.  The backward sweep of the Cholesky solve (L^T with only L stored).
+int launch_gemm_narrow_tn(int M, int N, int K, const double* AT, int64_t ldat, const double* B, int64_t ldb,
+                          const double* C, int64_t ldc, double* D, int64_t ldd, double alpha, double beta,
+                          cudaStream_t stream);
+// out[j][r][c] = in[j][c][r] for the nb x nb blocks of a total-element array (the block transposes of diagonal inverses)
+int launch_transpose_blocks(const double* in, int nb, int64_t total, double* out, cudaStream_t stream);
 
 }  // namespace cflx

@@ -82,6 +82,30 @@ __device__ __forceinline__ void stage_b(const NarrowArgs& g, int kc, int n0, dou
     cp_async_commit();
 }
 
+// epilogue of one m16n8 tile row pair: acc[j][0..1] = D[row_a][n0 + 8j + 2t + {0,1}], acc[j][2..3] the same of row_b.  C
+// may alias D: each element is read and then written by the same thread, so plain (coherent) accesses suffice.
+template <int NT>
+__device__ __forceinline__ void store_d(const NarrowArgs& g, const double (&acc)[NT][4], int64_t row_a, int64_t row_b,
+                                        int n0, int t4) {
+    const bool use_c = g.beta != 0.0;
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        const int64_t row = r ? row_b : row_a;
+        if (row >= g.M) continue;
+#pragma unroll
+        for (int j = 0; j < NT; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int col = n0 + 8 * j + 2 * t4 + e;
+                if (col < g.N) {
+                    const double c = use_c ? g.C[row * g.ldc + col] : 0.0;
+                    g.D[row * g.ldd + col] = fma(g.alpha, acc[j][2 * r + e], g.beta * c);
+                }
+            }
+        }
+    }
+}
+
 template <int NT>
 __global__ void __launch_bounds__(NW * 32, 1) gemm_narrow_kernel(NarrowArgs g) {
     constexpr int BN = NarrowCfg<NT>::BN, LDP = NarrowCfg<NT>::LDP, STEPS = KC / 16;
@@ -135,25 +159,8 @@ __global__ void __launch_bounds__(NW * 32, 1) gemm_narrow_kernel(NarrowArgs g) {
         }
     }
 
-    // epilogue: c0/c1 = D[g][2t + {0,1}], c2/c3 = D[g + 8][2t + {0,1}] of every 8-column tile.  C may alias D: each
-    // element is read and then written by the same thread, so plain (coherent) accesses suffice.
-    const bool use_c = g.beta != 0.0;
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-        const int64_t row = row0 + 8 * r;
-        if (row >= g.M) continue;
-#pragma unroll
-        for (int j = 0; j < NT; ++j) {
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-                const int col = n0 + 8 * j + 2 * t4 + e;
-                if (col < g.N) {
-                    const double c = use_c ? g.C[row * g.ldc + col] : 0.0;
-                    g.D[row * g.ldd + col] = fma(g.alpha, acc[j][2 * r + e], g.beta * c);
-                }
-            }
-        }
-    }
+    // epilogue: c0/c1 = D[g][2t + {0,1}], c2/c3 = D[g + 8][2t + {0,1}] of every 8-column tile
+    store_d<NT>(g, acc, row0, row0 + 8, n0, t4);
 }
 
 template <int NT>
@@ -164,6 +171,107 @@ int launch_narrow_nt(const NarrowArgs& g, cudaStream_t s) {
         CFLX_CUDA(cudaFuncSetAttribute(gemm_narrow_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
     dim3 grid((unsigned)((g.M + BM - 1) / BM), (unsigned)((g.N + C::BN - 1) / C::BN));
     gemm_narrow_kernel<NT><<<grid, NW * 32, C::SMEM, s>>>(g);
+    CFLX_CUDA(cudaGetLastError());
+    return CFLX_OK;
+}
+
+// ---------------------------------------------------------------- the transposed narrow GEMM
+// D = beta * C + alpha * AT^T * B, AT [K x M] row-major (NarrowArgs::A / lda), read in place: the backward sweep of the
+// Cholesky solve applies L^T with only L stored.  Bound by reading AT like the kernel above, so every element of AT is
+// loaded once per slab of BN columns, with 16-byte loads straight into the MMA fragments.  AT is contiguous in m, so one
+// double2 holds two output rows of one k:
+//   * a warp owns 32 rows m0 .. m0 + 31; lane (g, t) loads AT[k][m0 + 2g .. 2g+1] and AT[k][m0 + 16 + 2g .. 2g+1] for
+//     the four k = 4t .. 4t+3 of every 16-wide k step (the eight lanes of one t read one 128-byte segment of a k row);
+//   * MMA p in {0, 1} takes component p of every double2: row slot g is m0 + 2g + p and row slot g + 8 is
+//     m0 + 16 + 2g + p.  The epilogue un-permutes by storing the two MMAs' tiles at those rows (store_d);
+//   * the k slots are permuted as in the NN kernel (in MMA half h, slot t is k = 4t + 2h and slot t + 4 is k = 4t + 2h + 1),
+//     so B is staged by the same stage_b and each B fragment is one conflict-free 16-byte shared-memory load;
+//   * a 16-wide k step is 16 doubles of AT per lane against 8 * NT accumulators, so AT goes into registers KA k rows at a
+//     time within each 64-row chunk of B (TnCfg: fewer rows as the accumulators grow, to stay clear of spills).
+// No K condition: every k row is masked on its own and B is zero-filled beyond K and N.  With an odd M the last pair's
+// second row is beyond M, and that pair is loaded as one double, so nothing beyond M, K or N is read.
+constexpr int BM_TN = 32 * NW;  // rows per CTA
+
+template <int NT>
+struct TnCfg {
+    static constexpr int KA = NT >= 8 ? 16 : (NT >= 4 ? 32 : 64);  // k rows of AT per register load
+};
+
+template <int NT>
+__global__ void __launch_bounds__(NW * 32, 1) gemm_narrow_tn_kernel(NarrowArgs g) {
+    constexpr int LDP = NarrowCfg<NT>::LDP, KA = TnCfg<NT>::KA, SUB = KA / 16;
+    extern __shared__ double2 sB[];  // [2][KC / 2][LDP]
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g4 = lane >> 2, t4 = lane & 3;
+    const int64_t ma = (int64_t)blockIdx.x * BM_TN + warp * 32 + 2 * g4, mb = ma + 16;
+    const int n0 = blockIdx.y * NarrowCfg<NT>::BN;
+    double acc[2][NT][4];
+#pragma unroll
+    for (int p = 0; p < 2; ++p)
+#pragma unroll
+        for (int j = 0; j < NT; ++j) acc[p][j][0] = acc[p][j][1] = acc[p][j][2] = acc[p][j][3] = 0.0;
+
+    auto load_pair = [&](const double* row, int64_t m) -> double2 {  // AT[k][m .. m+1], zero beyond M
+        if (m + 1 < g.M) return __ldg(reinterpret_cast<const double2*>(row + m));
+        return make_double2(m < g.M ? __ldg(row + m) : 0.0, 0.0);
+    };
+    // a[s][2i + r] = AT[k][m_r .. m_r + 1] with k = kk + 16s + 4t + i, m_0 = m0 + 2g, m_1 = m0 + 16 + 2g
+    auto load_a = [&](double2 (&a)[SUB][8], int kk) {
+#pragma unroll
+        for (int s = 0; s < SUB; ++s) {
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int k = kk + 16 * s + 4 * t4 + i;
+                const double2 z = make_double2(0.0, 0.0);
+                a[s][2 * i] = k < g.K ? load_pair(g.A + (int64_t)k * g.lda, ma) : z;
+                a[s][2 * i + 1] = k < g.K ? load_pair(g.A + (int64_t)k * g.lda, mb) : z;
+            }
+        }
+    };
+    if (g.K > 0) stage_b<NT>(g, 0, n0, sB);
+    for (int kc = 0, c = 0; kc < g.K; kc += KC, ++c) {
+        const double2* sb = sB + (c & 1) * NarrowCfg<NT>::STAGE;
+#pragma unroll 1
+        for (int ks = 0; ks < KC && kc + ks < g.K; ks += KA) {  // uniform over the CTA
+            double2 a[SUB][8];
+            load_a(a, kc + ks);  // the first load of a chunk is in flight while the chunk's B lands
+            if (ks == 0) {
+                cp_async_wait_all();  // chunk c has landed (this thread's copies) ...
+                __syncthreads();      // ... for every thread, and every warp is done with chunk c - 1's buffer
+                if (kc + KC < g.K) stage_b<NT>(g, kc + KC, n0, sB + ((c + 1) & 1) * NarrowCfg<NT>::STAGE);
+            }
+#pragma unroll
+            for (int s = 0; s < SUB; ++s) {
+                if (kc + ks + 16 * s < g.K) {  // uniform over the CTA
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const double2 *k0 = a[s] + 4 * h, *k1 = a[s] + 4 * h + 2;  // k = 4t + 2h and 4t + 2h + 1
+                        const double af0[4] = {k0[0].x, k0[1].x, k1[0].x, k1[1].x};
+                        const double af1[4] = {k0[0].y, k0[1].y, k1[0].y, k1[1].y};
+                        const double2* b_k = sb + ((ks >> 1) + 8 * s + 2 * t4 + h) * LDP + g4;
+#pragma unroll
+                        for (int j = 0; j < NT; ++j) {
+                            const double2 bb = b_k[8 * j];
+                            const double bf[2] = {bb.x, bb.y};
+                            dmma16x8x8(acc[0][j], af0, bf);
+                            dmma16x8x8(acc[1][j], af1, bf);
+                        }
+                    }
+                }
+            }
+        }
+    }
+#pragma unroll
+    for (int p = 0; p < 2; ++p) store_d<NT>(g, acc[p], ma + p, mb + p, n0, t4);
+}
+
+template <int NT>
+int launch_narrow_tn(const NarrowArgs& g, cudaStream_t s) {
+    using C = NarrowCfg<NT>;
+    static PerDeviceMax cfg;
+    if (cfg.raise(C::SMEM))
+        CFLX_CUDA(cudaFuncSetAttribute(gemm_narrow_tn_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
+    dim3 grid((unsigned)((g.M + BM_TN - 1) / BM_TN), (unsigned)((g.N + C::BN - 1) / C::BN));
+    gemm_narrow_tn_kernel<NT><<<grid, NW * 32, C::SMEM, s>>>(g);
     CFLX_CUDA(cudaGetLastError());
     return CFLX_OK;
 }
@@ -191,6 +299,27 @@ int launch_gemm_narrow(int M, int N, int K, const double* A, int64_t lda, const 
     if (N <= 16) return launch_narrow_nt<2>(g, stream);
     if (N <= 32) return launch_narrow_nt<4>(g, stream);
     return launch_narrow_nt<8>(g, stream);  // wider B: slabs of 64 columns, one per blockIdx.y
+}
+
+int launch_gemm_narrow_tn(int M, int N, int K, const double* AT, int64_t ldat, const double* B, int64_t ldb, const double* C,
+                          int64_t ldc, double* D, int64_t ldd, double alpha, double beta, cudaStream_t stream) {
+    if (M <= 0 || N <= 0) return CFLX_OK;
+    if (K < 0 || (ldat & 1) || ldat < M || (reinterpret_cast<uintptr_t>(AT) & 15)) {
+        set_last_error("gemm_narrow_tn: unsupported shape M=%d N=%d K=%d ldat=%lld (need K >= 0, even ldat >= M, 16-byte aligned AT)",
+                       M, N, K, (long long)ldat);
+        return CFLX_ERR_UNSUPPORTED;
+    }
+    const NarrowArgs g{M, N, K, AT, ldat, B, ldb, C, ldc, D, ldd, alpha, beta};
+    if (N <= 8) return launch_narrow_tn<1>(g, stream);
+    if (N <= 16) return launch_narrow_tn<2>(g, stream);
+    if (N <= 32) return launch_narrow_tn<4>(g, stream);
+    return launch_narrow_tn<8>(g, stream);
+}
+
+int launch_transpose_blocks(const double* in, int nb, int64_t total, double* out, cudaStream_t stream) {
+    transpose_blocks_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(in, nb, total, out);
+    CFLX_CUDA(cudaGetLastError());
+    return CFLX_OK;
 }
 
 namespace {
@@ -239,11 +368,7 @@ int solve_prepare(cflx_lu* lu) {
                 break;
             }
             rc = launch_diag_inverses(tile, v, nb, inv + (size_t)v * nb, linvT, s);
-            if (!rc) {
-                const int64_t total = (int64_t)v * nb;
-                transpose_blocks_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(linvT, nb, total, inv);
-                if (cudaGetLastError() != cudaSuccess) rc = CFLX_ERR_CUDA;
-            }
+            if (!rc) rc = launch_transpose_blocks(linvT, nb, (int64_t)v * nb, inv, s);
         }
         if (cudaStreamSynchronize(s) != cudaSuccess && !rc) rc = CFLX_ERR_CUDA;
         cudaFree(tile);

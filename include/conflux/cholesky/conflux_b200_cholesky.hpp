@@ -84,5 +84,12 @@ inline double validate(double* relative = nullptr) {
     if (relative) *relative = r;
     return a;
 }
+// A X = B with the factor of the last parallelCholesky() (cflx_chol_solve, collective; the reference has no solve).  B and
+// X are matrix_size() x nrhs row-major; X may be nullptr on any rank.
+inline void choleskySolve(int nrhs, const double* B, int ldb, double* X, int ldx) {
+    auto& s = chol_detail::state();
+    if (!s.plan) throw CholeskyException("choleskySolve() before initialize()");
+    chol_detail::check(cflx_chol_solve(s.plan, nrhs, B, ldb, X, ldx), "choleskySolve");
+}
 
 }  // namespace conflux

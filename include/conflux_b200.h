@@ -147,6 +147,15 @@ int cflx_chol_factor(cflx_chol*, double* ms_out);
 int cflx_chol_get_local(cflx_chol*, double* L_host);
 /* COLLECTIVE.  ||A - L L^T||_F over the lower triangle, absolute and relative to ||A||_F, computed on the GPU grid. */
 int cflx_chol_validate(cflx_chol*, double* frob_abs_out, double* frob_rel_out);
+/* COLLECTIVE.  Solves A X = B with the factor of the last successful cflx_chol_factor (A = L L^T), on the GPU grid, like
+ * LAPACK's potrs.  B: N x nrhs row-major host array (N = the padded size, info_out[0]), leading dimension ldb >= nrhs, the
+ * same on every rank.  X: N x nrhs row-major, ldx >= nrhs, may be NULL on any rank; the result is identical on every rank.
+ * CFLX_ERR_ARG for nrhs < 1, ldb < nrhs, ldx < nrhs with X set, or a NULL B.  CFLX_ERR_STATE before a successful
+ * cflx_chol_factor, after cflx_chol_set_local, and after a factorisation that found a non-positive pivot.  The first call
+ * after a factorisation prepares and caches per-rank solve data; cflx_chol_set_local / cflx_chol_factor drop it.  Does not
+ * modify the factor or the input. */
+int cflx_chol_solve(cflx_chol*, int nrhs, const double* B, int ldb, double* X, int ldx);
+/* number of kernels this object counted since the last reset (bench.py's gpu_launches); cflx_chol_solve adds none */
 int cflx_chol_launch_count(cflx_chol*, int64_t* count_out, int reset);
 void cflx_chol_destroy(cflx_chol*);
 
@@ -157,6 +166,10 @@ int cflx_dbg_gemm_tn(int M, int N, int K, const double* AT, const double* B, con
 /* D = beta*C + alpha * A * B with A [M x K], B [K x N], C/D [M x N], all row-major, dense: the narrow GEMM of the solve */
 int cflx_dbg_gemm_narrow(int M, int N, int K, const double* A, const double* B, const double* C, double alpha, double beta,
                          double* D, int reps, double* ms_out);
+/* D = beta*C + alpha * AT^T * B with AT [K x M], B [K x N], C/D [M x N], all row-major, dense: the transposed narrow GEMM
+ * of the Cholesky solve.  On the device AT gets an even leading dimension >= M, so any M >= 1 can be run. */
+int cflx_dbg_gemm_narrow_tn(int M, int N, int K, const double* AT, const double* B, const double* C, double alpha,
+                            double beta, double* D, int reps, double* ms_out);
 /* partial-pivot LU of an n x v row-major panel: perm_out[v], A00_out[v*v] (L00\U00), LU_out[n*v] rows unpermuted */
 int cflx_dbg_panel(int n, int v, const double* panel, int* perm_out, double* A00_out, double* LU_out, int reps,
                    double* ms_out);
