@@ -42,13 +42,8 @@ struct cflx_chol {
     cudaEvent_t ev_col[2] = {nullptr, nullptr}, ev_panel[2] = {nullptr, nullptr};
     bool have_input = false, factored = false;
     int64_t launches = 0;
-    // cflx_chol_solve: prepared by the first solve after a factorisation, dropped by set_local / factor
-    bool solve_ready = false;
     SubComm j_comm;                  // grid row of one layer (color pi * Pz + pk, key pj), made by the first solve
-    double* sv_inv = nullptr;        // per owned diagonal tile: inv(L_jj) blocks, then inv(L_jj)^T blocks (v x nb each)
-    int* sv_rows = nullptr;          // [Ml] row of B of each real local row (ranks (pi, 0, 0))
-    double *sv_B = nullptr, *sv_W = nullptr, *sv_Z = nullptr, *sv_R = nullptr, *sv_Y = nullptr, *sv_X = nullptr;
-    int sv_ldn = 0;                  // columns of the work buffers
+    SolveCache sv;                   // cflx_chol_solve: inv(L_jj) blocks forward, inv(L_jj)^T backward; rows of real tiles
 };
 
 namespace {
@@ -347,10 +342,6 @@ __global__ void extract_l_panel_T_kernel(const double* __restrict__ A, int64_t l
     }
 }
 
-int ceil_div_pos(int a, int b) { return a <= 0 ? 0 : (a + b - 1) / b; }
-// first local tile row / column whose global tile index is >= g
-int first_local_tile(int g, int p, int P) { return ceil_div_pos(g - p, P); }
-
 int chol_pick_nb(int v) {
     for (int nb : {128, 64, 32, 16, 8, 4})
         if (v % nb == 0) return nb;
@@ -361,8 +352,7 @@ void free_chol(cflx_chol* ch) {
     if (!ch) return;
     cudaSetDevice(ch->comm->device);
     for (double* p : {ch->A0, ch->A11, ch->PT, ch->LT, ch->W, ch->G, ch->Bc, ch->D, ch->A00, ch->Uinv, ch->LinvT, ch->acc, ch->Q}) cudaFree(p);
-    for (double* p : {ch->sv_inv, ch->sv_B, ch->sv_W, ch->sv_Z, ch->sv_R, ch->sv_Y, ch->sv_X}) cudaFree(p);
-    cudaFree(ch->sv_rows);
+    solve_cache_free(&ch->sv);
     cudaFree(ch->info);
     if (ch->use_ozaki) ozaki_workspace_destroy(&ch->oz);
     if (ch->side) cudaStreamDestroy(ch->side);
@@ -611,182 +601,31 @@ int panel_step(cflx_chol* ch, int k, cudaStream_t s) {
 // ---------------------------------------------------------------------------------------------- solve, A X = B
 // After the factorisation, layer 0's A11 holds L: tile (gi, gj), gi >= gj, on rank (gi % Px, gj % Py, 0) at local tile
 // (gi / Px, gj / Py), the diagonal tiles with zeros above the diagonal.  The solve reads nothing else: not the tiles above
-// the diagonal (leftovers of the update), not the local tiles with a global index >= Kappa, not the layers pk != 0.
-//   Forward sweep, L Y = B (the LU solve's forward sweep with a non-unit L and no permutation): W (Ml x ldn, by local
-//   tile row) is each rank's partial right-hand side, seeded with B's rows on the ranks (pi, 0, 0).  Step t: reduce of W's
-//   tile t over the grid row (j_comm) onto the owner (t % Px, t % Py, 0), the nb-block sweep there, broadcast of Y_t over
-//   the grid column (i_comm), and W[tiles I > t] -= L[I, t] Y_t on that grid column.
-//   Backward sweep, L^T X = Y, the transpose: Z (Nl x ldn, by local tile COLUMN) starts with Y_t at the owner's local
-//   column t / Py.  Step t = Kappa - 1 .. 0: reduce of Z's tile t over the grid column onto the owner, X_j = inv(L_jj)^T R_j
-//   and R_i -= L_ji^T X_j (i < j) there, broadcast of X_t over the grid row, and Z[columns gj < t] -= L[t, gj]^T X_t on
-//   that grid row: one gemm_narrow_tn on a prefix of the local tile row t / Px, L read transposed in place.
-// The owners write X_t into a zeroed N x ldn buffer, and one all-reduce over the world gives every rank the same bits.
-
-// slot of diagonal tile t in sv_inv on this rank (-1: not owned)
-int chol_diag_slot(const cflx_chol* ch, int t) {
-    if (ch->pk != 0 || t % ch->Px != ch->pi || t % ch->Py != ch->pj) return -1;
-    int n = 0;
-    for (int u = 0; u < t; ++u) n += (u % ch->Px == ch->pi && u % ch->Py == ch->pj);
-    return n;
+// the diagonal (leftovers of the update), not the local tiles with a global index >= Kappa, not the layers pk != 0.  It
+// is the engine's row-partial sweep L Y = B (W seeded with B's rows on the ranks (pi, 0, 0); Y_t kept at the owner's
+// local column t / Py of Z), then its column-partial sweep L^T X = Y.  The grid row and column are those of layer 0
+// (j_comm / i_comm, one layer each); the layers pk != 0 only join the final all-reduce.
+SolveFactor chol_solve_factor(cflx_chol* ch) {
+    return SolveFactor{ch->comm, ch->A11, ch->N, ch->Ml, ch->Nl, first_local_tile(ch->Kappa, ch->pi, ch->Px) * ch->v,
+                       ch->v, ch->nb, ch->Kappa, ch->P, ch->Px, ch->Py, ch->pi, ch->pj, ch->pk, &ch->j_comm, &ch->i_comm, 1};
 }
 
 // First call after a factorisation: the grid-row communicator (once per object), the inverses of the nb x nb diagonal
 // blocks of every owned diagonal tile, and on the ranks that seed W, the row of B of each of their real local rows.
 int chol_solve_prepare(cflx_chol* ch) {
     cflx_comm* c = ch->comm;
-    cudaStream_t s = c->stream;
-    const int v = ch->v, nb = ch->nb, Px = ch->Px, Py = ch->Py, Nl = ch->Nl;
-    if (c->world_size > 1 && !ch->j_comm.c) CFLX_TRY(make_sub(c, ch->pi * ch->Pz + ch->pk, ch->pj, Py, &ch->j_comm));
-    cudaFree(ch->sv_inv);
-    ch->sv_inv = nullptr;
-    if (ch->pk != 0) {
-        ch->solve_ready = true;
-        return CFLX_OK;
-    }
-    int nown = 0;
-    for (int t = 0; t < ch->Kappa; ++t) nown += chol_diag_slot(ch, t) >= 0;
-    const size_t per = 2 * (size_t)v * nb;
-    CFLX_TRY(dmalloc(&ch->sv_inv, std::max(1, nown) * per));
-    double *lt = nullptr, *unit = nullptr;
-    int rc = dmalloc(&lt, (size_t)v * v);
-    if (!rc) rc = dmalloc(&unit, (size_t)v * nb);
-    for (int t = 0; t < ch->Kappa && !rc; ++t) {
-        const int slot = chol_diag_slot(ch, t);
-        if (slot < 0) continue;
-        double* inv = ch->sv_inv + slot * per;
-        // launch_diag_inverses on A00 = L_tt^T, as panel_step runs it: Uinv_j = inv(L_jj)^T (for the backward sweep); the
-        // unit-lower part of L_tt^T is the identity.  The block transposes inv(L_jj) serve the forward sweep.
-        rc = launch_extract_panel_T(ch->A11, Nl, (int64_t)(t / Px) * v, (int64_t)(t / Py) * v, v, v, lt, v, s);
-        if (!rc) rc = launch_diag_inverses(lt, v, nb, inv + (size_t)v * nb, unit, s);
-        if (!rc) rc = launch_transpose_blocks(inv + (size_t)v * nb, nb, (int64_t)v * nb, inv, s);
-    }
-    if (cudaStreamSynchronize(s) != cudaSuccess && !rc) rc = CFLX_ERR_CUDA;
-    cudaFree(lt);
-    cudaFree(unit);
-    if (rc) return rc;
-    if (ch->pj == 0 && !ch->sv_rows) {  // local row r of a real tile holds global row ((r / v) * Px + pi) * v + r % v
-        const int rows_real = first_local_tile(ch->Kappa, ch->pi, Px) * v;
-        std::vector<int> rows(std::max(rows_real, 1), 0);
-        for (int r = 0; r < rows_real; ++r) rows[r] = ((r / v) * Px + ch->pi) * v + r % v;
-        CFLX_TRY(dmalloc(&ch->sv_rows, rows.size()));
-        CFLX_CUDA(cudaMemcpyAsync(ch->sv_rows, rows.data(), sizeof(int) * rows.size(), cudaMemcpyHostToDevice, s));
-        CFLX_CUDA(cudaStreamSynchronize(s));  // `rows` is a host temporary
-    }
-    ch->solve_ready = true;
-    return CFLX_OK;
-}
-
-int chol_solve_buffers(cflx_chol* ch, int ldn) {
-    if (ldn <= ch->sv_ldn) return CFLX_OK;
-    for (double** p : {&ch->sv_B, &ch->sv_W, &ch->sv_Z, &ch->sv_R, &ch->sv_Y, &ch->sv_X}) {
-        cudaFree(*p);
-        *p = nullptr;
-    }
-    ch->sv_ldn = 0;
-    const size_t N = ch->N, v = ch->v;
+    if (c->world_size > 1 && !ch->j_comm.c) CFLX_TRY(make_sub(c, ch->pi * ch->Pz + ch->pk, ch->pj, ch->Py, &ch->j_comm));
     if (ch->pk == 0) {
-        if (ch->pj == 0) CFLX_TRY(dmalloc(&ch->sv_B, N * ldn));
-        CFLX_TRY(dmalloc(&ch->sv_W, (size_t)ch->Ml * ldn));
-        CFLX_TRY(dmalloc(&ch->sv_Z, (size_t)ch->Nl * ldn));
-        CFLX_TRY(dmalloc(&ch->sv_R, v * ldn));
-        CFLX_TRY(dmalloc(&ch->sv_Y, v * ldn));
-    }
-    CFLX_TRY(dmalloc(&ch->sv_X, N * ldn));
-    ch->sv_ldn = ldn;
-    return CFLX_OK;
-}
-
-// on the owner of diagonal tile t, R (v x ldn) overwritten:
-//   forward:  Y = L_tt^-1 R:  Y_j = inv(L_jj) R_j, then R_i -= L_ij Y_j for i > j (L_tt read in place)
-//   backward: Y = L_tt^-T R:  Y_j = inv(L_jj)^T R_j, then R_i -= L_ji^T Y_j for i < j (L_tt read transposed in place)
-int chol_diag_solve(cflx_chol* ch, int t, bool forward, double* R, double* Y, int ldn, cudaStream_t s) {
-    const int v = ch->v, nb = ch->nb, Nl = ch->Nl, nblk = v / nb;
-    const double* inv = ch->sv_inv + chol_diag_slot(ch, t) * 2 * (size_t)v * nb + (forward ? 0 : (size_t)v * nb);
-    const double* ltt = ch->A11 + (int64_t)(t / ch->Px) * v * Nl + (int64_t)(t / ch->Py) * v;
-    for (int i = 0; i < nblk; ++i) {
-        const int j = forward ? i : nblk - 1 - i;
-        const int64_t o = (int64_t)j * nb * ldn;
-        CFLX_TRY(launch_gemm_narrow(nb, ldn, nb, inv + (size_t)j * nb * nb, nb, R + o, ldn, nullptr, ldn, Y + o, ldn, 1.0,
-                                    0.0, s));
-        if (forward && j + 1 < nblk) {
-            const int64_t o1 = (int64_t)(j + 1) * nb;
-            CFLX_TRY(launch_gemm_narrow(v - (j + 1) * nb, ldn, nb, ltt + o1 * Nl + (int64_t)j * nb, Nl, Y + o, ldn,
-                                        R + o1 * ldn, ldn, R + o1 * ldn, ldn, -1.0, 1.0, s));
-        }
-        if (!forward && j > 0)  // block row j of L_tt left of its diagonal block, as AT
-            CFLX_TRY(launch_gemm_narrow_tn(j * nb, ldn, nb, ltt + (int64_t)j * nb * Nl, Nl, Y + o, ldn, R, ldn, R, ldn,
-                                           -1.0, 1.0, s));
-    }
-    return CFLX_OK;
-}
-
-int chol_solve_grid(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X, int ldx) {
-    cflx_comm* c = ch->comm;
-    cudaStream_t s = c->stream;
-    if (!ch->solve_ready) CFLX_TRY(chol_solve_prepare(ch));
-    const int v = ch->v, Px = ch->Px, Py = ch->Py, Ml = ch->Ml, Nl = ch->Nl, Kappa = ch->Kappa, N = ch->N;
-    const int pi = ch->pi, pj = ch->pj;
-    const int ldn = (int)round_up(nrhs, 8);
-    CFLX_TRY(chol_solve_buffers(ch, ldn));
-    double *W = ch->sv_W, *Z = ch->sv_Z, *Y = ch->sv_Y, *Xd = ch->sv_X;
-    const size_t tile = (size_t)v * ldn;
-    CFLX_CUDA(cudaMemsetAsync(Xd, 0, sizeof(double) * N * ldn, s));
-    if (ch->pk == 0) {  // the other layers hold no part of L: they only join the final all-reduce
-        const int row_end = first_local_tile(Kappa, pi, Px) * v;  // local rows of real tiles
-        CFLX_CUDA(cudaMemsetAsync(W, 0, sizeof(double) * Ml * ldn, s));
-        CFLX_CUDA(cudaMemsetAsync(Z, 0, sizeof(double) * Nl * ldn, s));
-        if (pj == 0 && row_end > 0) {
-            CFLX_CUDA(cudaMemsetAsync(ch->sv_B, 0, sizeof(double) * N * ldn, s));
-            CFLX_CUDA(cudaMemcpy2DAsync(ch->sv_B, ldn * sizeof(double), B, (size_t)ldb * sizeof(double),
-                                        nrhs * sizeof(double), N, cudaMemcpyHostToDevice, s));
-            CFLX_TRY(launch_gather_rows(ch->sv_B, ldn, ch->sv_rows, row_end, ldn, W, s));
-        }
-        // ---- forward sweep: L Y = B
-        for (int t = 0; t < Kappa; ++t) {
-            const bool in_row = pi == t % Px, in_col = pj == t % Py, owner = in_row && in_col;
-            double* R = W + (int64_t)(t / Px) * tile;
-            if (in_row && Py > 1) {
-                CFLX_NCCL(ncclReduce(R, ch->sv_R, tile, ncclDouble, ncclSum, t % Py, ch->j_comm.c, s));
-                R = ch->sv_R;
-            }
-            if (owner) {
-                CFLX_TRY(chol_diag_solve(ch, t, true, R, Y, ldn, s));
-                CFLX_CUDA(cudaMemcpyAsync(Z + (int64_t)(t / Py) * tile, Y, tile * sizeof(double), cudaMemcpyDeviceToDevice, s));
-            }
-            if (!in_col) continue;
-            if (Px > 1) CFLX_NCCL(ncclBroadcast(Y, Y, tile, ncclDouble, t % Px, ch->i_comm.c, s));
-            const int row_lo = first_local_tile(t + 1, pi, Px) * v;
-            if (row_lo < row_end)  // W[tiles I > t] -= L[I, t] Y_t
-                CFLX_TRY(launch_gemm_narrow(row_end - row_lo, ldn, v, ch->A11 + (int64_t)row_lo * Nl + (int64_t)(t / Py) * v,
-                                            Nl, Y, ldn, W + (int64_t)row_lo * ldn, ldn, W + (int64_t)row_lo * ldn, ldn, -1.0,
-                                            1.0, s));
-        }
-        // ---- backward sweep: L^T X = Y
-        for (int t = Kappa - 1; t >= 0; --t) {
-            const bool in_row = pi == t % Px, in_col = pj == t % Py, owner = in_row && in_col;
-            double* R = Z + (int64_t)(t / Py) * tile;
-            if (in_col && Px > 1) {
-                CFLX_NCCL(ncclReduce(R, ch->sv_R, tile, ncclDouble, ncclSum, t % Px, ch->i_comm.c, s));
-                R = ch->sv_R;
-            }
-            if (owner) {
-                CFLX_TRY(chol_diag_solve(ch, t, false, R, Y, ldn, s));
-                CFLX_CUDA(cudaMemcpyAsync(Xd + (int64_t)t * tile, Y, tile * sizeof(double), cudaMemcpyDeviceToDevice, s));
-            }
-            if (!in_row) continue;
-            if (Py > 1) CFLX_NCCL(ncclBroadcast(Y, Y, tile, ncclDouble, t % Py, ch->j_comm.c, s));
-            const int m = first_local_tile(t, pj, Py) * v;  // local columns with gj < t: a prefix of the tile row
-            if (m > 0)  // Z[columns gj < t] -= L[t, gj]^T X_t
-                CFLX_TRY(launch_gemm_narrow_tn(m, ldn, v, ch->A11 + (int64_t)(t / Px) * v * Nl, Nl, Y, ldn, Z, ldn, Z, ldn,
-                                               -1.0, 1.0, s));
+        const SolveFactor f = chol_solve_factor(ch);
+        CFLX_TRY(solve_inverses(&ch->sv, f, true));
+        if (ch->pj == 0 && !ch->sv.rows) {  // local row r of a real tile holds global row ((r / v) * Px + pi) * v + r % v
+            const int v = ch->v;
+            std::vector<int> rows(std::max(f.rows, 1), 0);
+            for (int r = 0; r < f.rows; ++r) rows[r] = ((r / v) * ch->Px + ch->pi) * v + r % v;
+            CFLX_TRY(solve_set_rows(&ch->sv, rows, c->stream));
         }
     }
-    // exactly one rank contributes each element: the sum is X itself, bit for bit, on every rank
-    if (ch->P > 1) CFLX_NCCL(ncclAllReduce(Xd, Xd, (size_t)N * ldn, ncclDouble, ncclSum, c->world, s));
-    if (X)
-        CFLX_CUDA(cudaMemcpy2DAsync(X, (size_t)ldx * sizeof(double), Xd, ldn * sizeof(double), nrhs * sizeof(double), N,
-                                    cudaMemcpyDeviceToHost, s));
-    CFLX_CUDA(cudaStreamSynchronize(s));
+    ch->sv.ready = true;
     return CFLX_OK;
 }
 
@@ -957,7 +796,7 @@ int cflx_chol_set_local(cflx_chol* ch, const double* host_local) {
     CFLX_CUDA(cudaStreamSynchronize(ch->comm->stream));
     ch->have_input = true;
     ch->factored = false;
-    ch->solve_ready = false;
+    ch->sv.ready = false;
     return CFLX_OK;
 }
 
@@ -971,7 +810,7 @@ int cflx_chol_factor(cflx_chol* ch, double* ms_out) {
     cflx_comm* c = ch->comm;
     cudaStream_t s = c->stream;
     CFLX_CUDA(cudaSetDevice(c->device));
-    ch->solve_ready = false;
+    ch->sv.ready = false;
     const int v = ch->v, Py = ch->Py, Ml = ch->Ml, Nl = ch->Nl;
     const int pj = ch->pj;
     CFLX_CUDA(cudaMemcpyAsync(ch->A11, ch->A0, (size_t)Ml * Nl * sizeof(double), cudaMemcpyDeviceToDevice, s));
@@ -1132,7 +971,17 @@ int cflx_chol_solve(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X
         return CFLX_ERR_STATE;
     }
     CFLX_CUDA(cudaSetDevice(ch->comm->device));
-    return chol_solve_grid(ch, nrhs, B, ldb, X, ldx);
+    if (!ch->sv.ready) CFLX_TRY(chol_solve_prepare(ch));
+    const SolveFactor f = chol_solve_factor(ch);
+    SolveCache* sc = &ch->sv;
+    const int ldn = (int)round_up(nrhs, 8);
+    CFLX_TRY(solve_cache_grow(sc, f, ldn, ch->pk == 0, true));
+    CFLX_TRY(solve_seed(sc, f, ldn, nrhs, B, ldb));
+    if (ch->pk == 0) {  // L Y = B keeping Y_t in Z, then L^T X = Y from Z
+        CFLX_TRY(solve_row_sweep(sc, f, ldn, true, sc->Z, ch->Py, false));
+        CFLX_TRY(solve_col_sweep(sc, f, ldn));
+    }
+    return solve_finish(sc, f, ldn, nrhs, X, ldx);
 }
 
 int cflx_chol_launch_count(cflx_chol* ch, int64_t* count_out, int reset) {

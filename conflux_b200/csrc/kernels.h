@@ -164,7 +164,5 @@ int launch_gemm_narrow(int M, int N, int K, const double* A, int64_t lda, const 
 int launch_gemm_narrow_tn(int M, int N, int K, const double* AT, int64_t ldat, const double* B, int64_t ldb,
                           const double* C, int64_t ldc, double* D, int64_t ldd, double alpha, double beta,
                           cudaStream_t stream);
-// out[j][r][c] = in[j][c][r] for the nb x nb blocks of a total-element array (the block transposes of diagonal inverses)
-int launch_transpose_blocks(const double* in, int nb, int64_t total, double* out, cudaStream_t stream);
 
 }  // namespace cflx

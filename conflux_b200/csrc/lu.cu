@@ -497,12 +497,12 @@ void free_lu(cflx_lu* lu) {
     if (!lu) return;
     cudaSetDevice(lu->comm->device);
     double* dbl[] = {lu->A0, lu->A11, lu->PT, lu->PT2, lu->W, lu->LT, lu->A01raw, lu->U, lu->tmp, lu->A00, lu->A00T,
-                     lu->Uinv, lu->LinvT, lu->candH, lu->S, lu->W2, lu->bcast, lu->Cbuf, lu->xbuf, lu->sv_inv,
-                     lu->sv_B, lu->sv_W, lu->sv_R, lu->sv_Y, lu->sv_X};
+                     lu->Uinv, lu->LinvT, lu->candH, lu->S, lu->W2, lu->bcast, lu->Cbuf, lu->xbuf};
     for (double* p : dbl) cudaFree(p);
     int* ints[] = {lu->gri, lu->gri_tmp, lu->igri, lu->perm, lu->gpivots, lu->tagsH, lu->tagsS, lu->hist, lu->plan_mem,
-                   lu->idx_buf, lu->sv_rows};
+                   lu->idx_buf};
     for (int* p : ints) cudaFree(p);
+    solve_cache_free(&lu->sv);
     if (lu->h_npiv) cudaFreeHost(lu->h_npiv);
     if (lu->pws.slot_hdr) panel_workspace_destroy(&lu->pws);
     if (lu->use_ozaki) ozaki_workspace_destroy(&lu->oz);
@@ -518,6 +518,44 @@ void free_lu(cflx_lu* lu) {
     for (SubComm* sc : {&lu->k_comm, &lu->i_comm, &lu->jk_comm, &lu->ik_comm})
         if (sc->c) ncclCommDestroy(sc->c);
     delete lu;
+}
+
+// ---------------------------------------------------------------------------------------------- solve, A X = B
+// The factors in the conflux layout of the validation path (Cbuf, as cflx_lu_get_factors leaves them), described to the
+// solve engine (solve.cu).  Every layer joins the grid-row reduces and grid-column broadcasts (jk / ik communicators,
+// layer 0 at rank p * Pz), the layers pk != 0 with zeros.
+SolveFactor lu_solve_factor(cflx_lu* lu) {
+    return SolveFactor{lu->comm, lu->Cbuf, lu->M, lu->Ml, lu->Nl, lu->Ml, lu->v, lu->nb, lu->Nt, lu->P, lu->Px, lu->Py,
+                       lu->pi, lu->pj, lu->pk, &lu->jk_comm, &lu->ik_comm, lu->Pz};
+}
+
+// First call after a factorisation: the factors redistributed into Cbuf, the diagonal-block inverses, and on the ranks
+// that seed the right-hand side, the row of B that each local row of P*B comes from.
+int lu_solve_prepare(cflx_lu* lu) {
+    cudaStream_t s = lu->comm->stream;
+    const int v = lu->v, Px = lu->Px, Ml = lu->Ml;
+    std::vector<int> hist(lu->M);
+    CFLX_TRY(cflx_lu_get_permutation(lu, hist.data()));
+    if (lu->pk == 0) {
+        cudaFree(lu->sv.inv);  // before the redistribution allocates its staging
+        lu->sv.inv = nullptr;
+        if (!lu->Cbuf) CFLX_TRY(dmalloc(&lu->Cbuf, (size_t)Ml * lu->Nl));
+        int rc = redistribute_pivoted_rows(lu, hist, true, lu->A11, lu->Cbuf);
+        cudaFree(lu->xbuf);  // 2 x local matrix of staging: do not keep it alive
+        lu->xbuf = nullptr;
+        if (rc) return rc;
+        CFLX_TRY(solve_inverses(&lu->sv, lu_solve_factor(lu), false));
+        if (lu->pj == 0) {  // local row (k / Px)*v + i of P*B is row hist[k*v + i] of B, for the tiles k of this grid row
+            std::vector<int> rows(Ml, 0);
+            for (int q = 0; q < lu->M; ++q) {
+                const int k = q / v;
+                if (k % Px == lu->pi) rows[(k / Px) * v + q % v] = hist[q];
+            }
+            CFLX_TRY(solve_set_rows(&lu->sv, rows, s));
+        }
+    }
+    lu->sv.ready = true;
+    return CFLX_OK;
 }
 }  // namespace
 
@@ -793,7 +831,7 @@ int cflx_lu_set_local(cflx_lu* lu, const double* host_local) {
     CFLX_CUDA(cudaStreamSynchronize(lu->comm->stream));
     lu->have_input = true;
     lu->factored = false;
-    lu->solve_ready = false;
+    lu->sv.ready = false;
     lu->a0_is_next = false;
     lu->next_host = nullptr;
     return CFLX_OK;
@@ -836,7 +874,7 @@ int cflx_lu_factor(cflx_lu* lu, double* ms_out) {
         CFLX_CUDA(cudaMemcpyAsync(lu->A11, lu->A0, loc * sizeof(double), cudaMemcpyDeviceToDevice, s));
     }
     lu->a0_is_next = false;
-    lu->solve_ready = false;
+    lu->sv.ready = false;
     if (lu->next_host) {  // queued next input: overwrite A0 behind the working copy, concurrently with everything below
         CFLX_CUDA(cudaEventRecord(lu->ev_a0_read, s));
         CFLX_CUDA(cudaStreamWaitEvent(lu->copy, lu->ev_a0_read, 0));
@@ -986,7 +1024,16 @@ int cflx_lu_solve(cflx_lu* lu, int nrhs, const double* B, int ldb, double* X, in
         return CFLX_ERR_STATE;
     }
     CFLX_CUDA(cudaSetDevice(lu->comm->device));
-    return lu_solve_grid(lu, nrhs, B, ldb, X, ldx);
+    if (!lu->sv.ready) CFLX_TRY(lu_solve_prepare(lu));
+    const SolveFactor f = lu_solve_factor(lu);
+    SolveCache* sc = &lu->sv;
+    const int ldn = (int)round_up(nrhs, 8);
+    CFLX_TRY(solve_cache_grow(sc, f, ldn, true, false));
+    CFLX_TRY(solve_seed(sc, f, ldn, nrhs, B, ldb));
+    // L Y = P B keeping Y_t as the owner's W rows, so that U X = Y starts from W = Y
+    CFLX_TRY(solve_row_sweep(sc, f, ldn, true, sc->W, lu->Px, true));
+    CFLX_TRY(solve_row_sweep(sc, f, ldn, false, sc->X, 1, false));
+    return solve_finish(sc, f, ldn, nrhs, X, ldx);
 }
 
 int cflx_host_alloc(size_t bytes, void** out) {

@@ -1,5 +1,6 @@
 // conflux_b200/csrc/lu_state.h -- internal state of a process-grid handle and of one factorisation plan, shared by the
-// orchestration (lu.cu), the validation path (validate.cu) and the Cholesky path (chol.cu).  Not part of the C ABI.
+// orchestration (lu.cu), the validation path (validate.cu), the solve engine (solve.cu) and the Cholesky path (chol.cu).
+// Not part of the C ABI.
 #pragma once
 #include <nccl.h>
 
@@ -61,6 +62,35 @@ inline int dmalloc(T** p, size_t n) {
 }
 int make_sub(cflx_comm* c, int color, int key, int size, SubComm* out);
 int grid_barrier(cflx_comm* c);
+
+// first local tile row (column) whose global tile index is >= g, on grid row (column) p of P
+inline int first_local_tile(int g, int p, int P) { return g <= p ? 0 : (g - p + P - 1) / P; }
+
+// ---------------------------------------------------------------- the solve engine (solve.cu)
+// What a solve keeps between calls: prepared by the first solve after a factorisation, dropped (ready = false) by
+// set_local / factor, freed with the object.  The work buffers have ldn columns and are grown, never shrunk.
+struct SolveCache {
+    bool ready = false;
+    double* inv = nullptr;  // per owned diagonal tile: the forward inverse blocks (v x nb, row-major nb x nb each), then
+                            // the backward ones
+    int* rows = nullptr;    // row of B of each seeded local row (ranks (pi, 0, 0))
+    double *B = nullptr, *W = nullptr, *Z = nullptr, *R = nullptr, *Y = nullptr, *X = nullptr;
+    int ldn = 0;
+};
+
+// One factor in the conflux block-cyclic layout, as the engine reads it: tile (I, J) on rank (I % Px, J % Py, 0) at
+// local tile (I / Px, J / Py) of F (layer 0, row-major, leading dimension Nl).  A rank's NCCL rank in the grid-row
+// communicator is pj * stride (+ pk), in the grid-column communicator pi * stride (+ pk).
+struct SolveFactor {
+    cflx_comm* comm;
+    const double* F;
+    int M, Ml, Nl;  // rows of B and X; local rows (of W) and columns (of F and Z)
+    int rows;       // local rows of the tiles the sweeps read and seed
+    int v, nb, Nt;  // tile, diagonal inverse block, tiles on the diagonal
+    int P, Px, Py, pi, pj, pk;
+    const SubComm *row_comm, *col_comm;
+    int stride;
+};
 }  // namespace cflx
 
 struct cflx_lu {
@@ -101,18 +131,33 @@ struct cflx_lu {
     std::vector<char> ev_used;
     cudaStream_t side = nullptr;  // high-priority look-ahead stream (null: no overlap)
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_npiv = nullptr;
-    // cflx_lu_solve (solve.cu): prepared by the first solve after a factorisation, dropped by set_local / factor
-    bool solve_ready = false;
-    double* sv_inv = nullptr;  // per owned diagonal tile: Linv blocks (v x nb, row-major nb x nb each), then Uinv blocks
-    int* sv_rows = nullptr;    // [Ml] row of B that local row r of P*B comes from (ranks (pi, 0, 0))
-    double *sv_B = nullptr, *sv_W = nullptr, *sv_R = nullptr, *sv_Y = nullptr, *sv_X = nullptr;  // work, sv_ldn columns
-    int sv_ldn = 0;
+    cflx::SolveCache sv;  // cflx_lu_solve: Linv blocks forward, Uinv blocks backward; rows: row of B of each row of P*B
 };
 
 namespace cflx {
 // validate.cu
 int redistribute_pivoted_rows(cflx_lu* lu, const std::vector<int>& hist, bool factors, const double* src, double* dst);
 int lu_residual_grid(cflx_lu* lu, const std::vector<int>& hist, double* abs_out, double* rel_out);
-// solve.cu
-int lu_solve_grid(cflx_lu* lu, int nrhs, const double* B, int ldb, double* X, int ldx);
+
+// solve.cu: the solve engine.  Every function returns CFLX_OK or an error code; all work goes on f.comm->stream.
+void solve_cache_free(SolveCache* sc);
+// grow the work buffers to ldn columns: B (M rows) on rank (pi, 0, 0), W (Ml) and R, Y (v) where `work`, Z (Nl) where
+// `work && col_partials`, X (M) on every rank
+int solve_cache_grow(SolveCache* sc, const SolveFactor& f, int ldn, bool work, bool col_partials);
+// the inverses of the nb x nb diagonal blocks of every owned diagonal tile, into sc->inv (freed and allocated again here).
+// lower: the tile is L with its own diagonal and zeros above, inverted as A00 = L^T; otherwise it is L\U with a unit L.
+int solve_inverses(SolveCache* sc, const SolveFactor& f, bool lower);
+// sc->rows = rows (allocated on first use), waited for
+int solve_set_rows(SolveCache* sc, const std::vector<int>& rows, cudaStream_t s);
+// zero X, W and Z, and on the ranks holding B: W[r] = B[rows[r]] for the f.rows seeded rows
+int solve_seed(SolveCache* sc, const SolveFactor& f, int ldn, int nrhs, const double* B, int ldb);
+// row-partial sweep over the tile diagonal: forward with the lower triangle (NN), backward with the upper one (NN).  The
+// diagonal owner keeps each solved tile t at tile t / keep_div of `keep`; with clear_row, keep is W and the other layer-0
+// ranks of the grid row zero their copy of that tile.
+int solve_row_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward, double* keep, int keep_div,
+                    bool clear_row);
+// column-partial backward sweep L^T X = Y (Z by local tile column, L read transposed), solved tiles into X; layer 0 only
+int solve_col_sweep(SolveCache* sc, const SolveFactor& f, int ldn);
+// X (nrhs columns, ldx) = the world sum of the owners' tiles of sc->X, downloaded when X is not null; synchronises
+int solve_finish(SolveCache* sc, const SolveFactor& f, int ldn, int nrhs, double* X, int ldx);
 }  // namespace cflx

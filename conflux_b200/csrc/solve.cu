@@ -1,16 +1,18 @@
-// conflux_b200/csrc/solve.cu -- A X = B with the factors of the last cflx_lu_factor (P A = L U), on the GPU grid.
+// conflux_b200/csrc/solve.cu -- the triangular-solve engine of cflx_lu_solve (lu.cu) and cflx_chol_solve (chol.cu).
 //
-// The factors are first brought into the conflux block-cyclic layout of the validation path (redistribute_pivoted_rows,
-// validate.cu): tile (I, J) of L\U on rank (I % Px, J % Py, 0).  The solve is then a forward and a backward sweep over
-// the tile diagonal.  Every rank keeps a partial right-hand side W (Ml x ldn, its tile rows); the sum of W over a grid
-// row is the current right-hand side of those tile rows.  Step t of a sweep:
-//   ncclReduce of tile t's rows of W over the grid row (jk-communicator) onto the diagonal owner (t % Px, t % Py, 0);
-//   the owner solves with L_tt (U_tt) by an nb-block sweep with the inverses of the nb x nb diagonal blocks;
-//   ncclBroadcast of the solved tile over the grid column (ik-communicator);
-//   every layer-0 rank of that grid column subtracts L[I, t] * Y_t (U[I, t] * X_t) from its rows of the tiles I > t
-//   (I < t).
-// The diagonal owners write X_t into a zeroed M x ldn buffer, and one all-reduce makes X identical on every rank.  All
-// arithmetic is gemm_narrow_kernel: a factor block (row-major, read in place) times a few right-hand sides.
+// A factor in the conflux block-cyclic layout (SolveFactor: tile (I, J) on rank (I % Px, J % Py, 0)) is solved against
+// a few right-hand sides by sweeps over the tile diagonal.  In the row-partial sweep every rank keeps a partial
+// right-hand side W (Ml x ldn, by local tile row); its sum over a grid row is the current right-hand side of those tile
+// rows.  Step t:
+//   ncclReduce of tile t's rows of W over the grid row onto the diagonal owner (t % Px, t % Py, 0);
+//   the owner solves with the diagonal tile by an nb-block sweep with the inverses of its nb x nb diagonal blocks, and
+//   keeps the solved tile where its caller asks;
+//   ncclBroadcast of the solved tile over the grid column;
+//   every layer-0 rank of that grid column updates its rows of the tiles past t.
+// The column-partial sweep (L^T X = Y with only L stored) is the transpose: partials Z by local tile column, the reduce
+// over the grid column, the broadcast over the grid row, and the update read transposed in place.  The owners write
+// X_t into a zeroed M x ldn buffer, and one all-reduce makes X identical on every rank.  All arithmetic is the narrow
+// GEMM below: a factor block (row-major, read in place) times a few right-hand sides.
 #include <cstring>
 
 #include "lu_state.h"
@@ -316,190 +318,207 @@ int launch_gemm_narrow_tn(int M, int N, int K, const double* AT, int64_t ldat, c
     return launch_narrow_tn<8>(g, stream);
 }
 
+// ---------------------------------------------------------------- the solve engine
+namespace {
 int launch_transpose_blocks(const double* in, int nb, int64_t total, double* out, cudaStream_t stream) {
     transpose_blocks_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(in, nb, total, out);
     CFLX_CUDA(cudaGetLastError());
     return CFLX_OK;
 }
 
-namespace {
-// ---------------------------------------------------------------- solve
-// slot of diagonal tile t in sv_inv on this rank (-1: not owned)
-int diag_slot(const cflx_lu* lu, int t) {
-    if (lu->pk != 0 || t % lu->Px != lu->pi || t % lu->Py != lu->pj) return -1;
+// slot of diagonal tile t in SolveCache::inv on this rank (-1: not owned)
+int diag_slot(const SolveFactor& f, int t) {
+    if (f.pk != 0 || t % f.Px != f.pi || t % f.Py != f.pj) return -1;
     int n = 0;
-    for (int u = 0; u < t; ++u) n += (u % lu->Px == lu->pi && u % lu->Py == lu->pj);
+    for (int u = 0; u < t; ++u) n += (u % f.Px == f.pi && u % f.Py == f.pj);
     return n;
 }
 
-// First call after a factorisation: factors in the conflux layout (Cbuf, as cflx_lu_get_factors leaves them), the
-// inverses of the nb x nb diagonal blocks of every owned diagonal tile (Linv row-major, then Uinv), and on the ranks
-// that seed the right-hand side, the row of B that each local row of P*B comes from.
-int solve_prepare(cflx_lu* lu) {
-    cflx_comm* c = lu->comm;
-    cudaStream_t s = c->stream;
-    const int v = lu->v, nb = lu->nb, Px = lu->Px, Py = lu->Py, Ml = lu->Ml, Nl = lu->Nl;
-    std::vector<int> hist(lu->M);
-    CFLX_TRY(cflx_lu_get_permutation(lu, hist.data()));
-    cudaFree(lu->sv_inv);
-    lu->sv_inv = nullptr;
-    if (lu->pk == 0) {
-        if (!lu->Cbuf) CFLX_TRY(dmalloc(&lu->Cbuf, (size_t)Ml * Nl));
-        int rc = redistribute_pivoted_rows(lu, hist, true, lu->A11, lu->Cbuf);
-        cudaFree(lu->xbuf);  // 2 x local matrix of staging: do not keep it alive
-        lu->xbuf = nullptr;
-        if (rc) return rc;
-        int nown = 0;
-        for (int t = 0; t < lu->Nt; ++t) nown += diag_slot(lu, t) >= 0;
-        const size_t per = 2 * (size_t)v * nb;
-        CFLX_TRY(dmalloc(&lu->sv_inv, std::max(1, nown) * per));
-        double *tile = nullptr, *linvT = nullptr;
-        rc = dmalloc(&tile, (size_t)v * v);
-        if (!rc) rc = dmalloc(&linvT, (size_t)v * nb);
-        for (int t = 0; t < lu->Nt && !rc; ++t) {
-            const int slot = diag_slot(lu, t);
-            if (slot < 0) continue;
-            double* inv = lu->sv_inv + slot * per;
-            const double* ctt = lu->Cbuf + (int64_t)(t / Px) * v * Nl + (int64_t)(t / Py) * v;
-            if (cudaMemcpy2DAsync(tile, v * sizeof(double), ctt, Nl * sizeof(double), v * sizeof(double), v,
-                                  cudaMemcpyDeviceToDevice, s) != cudaSuccess) {
-                set_last_error("solve: diagonal tile copy failed");
-                rc = CFLX_ERR_CUDA;
-                break;
-            }
-            rc = launch_diag_inverses(tile, v, nb, inv + (size_t)v * nb, linvT, s);
-            if (!rc) rc = launch_transpose_blocks(linvT, nb, (int64_t)v * nb, inv, s);
-        }
-        if (cudaStreamSynchronize(s) != cudaSuccess && !rc) rc = CFLX_ERR_CUDA;
-        cudaFree(tile);
-        cudaFree(linvT);
-        if (rc) return rc;
-        if (lu->pj == 0) {  // local row (k / Px)*v + i of P*B is row hist[k*v + i] of B, for the tiles k of this grid row
-            std::vector<int> rows(Ml, 0);
-            for (int q = 0; q < lu->M; ++q) {
-                const int k = q / v;
-                if (k % Px == lu->pi) rows[(k / Px) * v + q % v] = hist[q];
-            }
-            if (!lu->sv_rows) CFLX_TRY(dmalloc(&lu->sv_rows, (size_t)Ml));
-            CFLX_CUDA(cudaMemcpyAsync(lu->sv_rows, rows.data(), sizeof(int) * Ml, cudaMemcpyHostToDevice, s));
-            CFLX_CUDA(cudaStreamSynchronize(s));  // `rows` is a host temporary
-        }
-    }
-    lu->solve_ready = true;
-    return CFLX_OK;
+const double* diag_tile(const SolveFactor& f, int t) {
+    return f.F + (int64_t)(t / f.Px) * f.v * f.Nl + (int64_t)(t / f.Py) * f.v;
 }
 
-int ensure_solve_buffers(cflx_lu* lu, int ldn) {
-    if (ldn <= lu->sv_ldn) return CFLX_OK;
-    for (double** p : {&lu->sv_B, &lu->sv_W, &lu->sv_R, &lu->sv_Y, &lu->sv_X}) {
-        cudaFree(*p);
-        *p = nullptr;
-    }
-    lu->sv_ldn = 0;
-    const size_t M = lu->M, Ml = lu->Ml, v = lu->v;
-    if (lu->pk == 0 && lu->pj == 0) CFLX_TRY(dmalloc(&lu->sv_B, M * ldn));
-    CFLX_TRY(dmalloc(&lu->sv_W, Ml * ldn));
-    CFLX_TRY(dmalloc(&lu->sv_R, v * ldn));
-    CFLX_TRY(dmalloc(&lu->sv_Y, v * ldn));
-    CFLX_TRY(dmalloc(&lu->sv_X, M * ldn));
-    lu->sv_ldn = ldn;
-    return CFLX_OK;
-}
+enum class Tri { Lower, Upper, LowerT };
 
-// Y = L_tt^-1 R (forward) or Y = U_tt^-1 R (backward) on the diagonal owner; R (v x ldn) is overwritten
-int diag_solve(cflx_lu* lu, int t, bool lower, double* R, double* Y, int ldn, cudaStream_t s) {
-    const int v = lu->v, nb = lu->nb, Nl = lu->Nl, nblk = v / nb;
-    const double* inv = lu->sv_inv + diag_slot(lu, t) * 2 * (size_t)v * nb + (lower ? 0 : (size_t)v * nb);
-    const double* ctt = lu->Cbuf + (int64_t)(t / lu->Px) * v * Nl + (int64_t)(t / lu->Py) * v;
+// Y = T^-1 R on the owner of diagonal tile t, by an nb-block sweep with the cached inverses; R (v x ldn) is overwritten.
+//   Lower:  T = L_tt:    Y_j = inv(L_jj) R_j, then R_i -= L_ij Y_j for i > j (the forward inverses)
+//   Upper:  T = U_tt:    Y_j = inv(U_jj) R_j, then R_i -= U_ij Y_j for i < j (the backward inverses)
+//   LowerT: T = L_tt^T:  Y_j = inv(L_jj)^T R_j, then R_i -= L_ji^T Y_j for i < j (the backward inverses; L_tt read
+//           transposed in place)
+int diag_solve(const SolveCache& sc, const SolveFactor& f, int t, Tri tri, double* R, int ldn, cudaStream_t s) {
+    const int v = f.v, nb = f.nb, Nl = f.Nl, nblk = v / nb;
+    const bool fwd = tri == Tri::Lower;
+    const double* inv = sc.inv + diag_slot(f, t) * 2 * (size_t)v * nb + (fwd ? 0 : (size_t)v * nb);
+    const double* ftt = diag_tile(f, t);
+    double* Y = sc.Y;
     for (int i = 0; i < nblk; ++i) {
-        const int j = lower ? i : nblk - 1 - i;
+        const int j = fwd ? i : nblk - 1 - i;
         const int64_t o = (int64_t)j * nb * ldn;
         CFLX_TRY(launch_gemm_narrow(nb, ldn, nb, inv + (size_t)j * nb * nb, nb, R + o, ldn, nullptr, ldn, Y + o, ldn, 1.0,
                                     0.0, s));
-        if (lower && j + 1 < nblk) {  // R_i -= L_ij Y_j, i > j
+        if (fwd && j + 1 < nblk) {
             const int64_t o1 = (int64_t)(j + 1) * nb;
-            CFLX_TRY(launch_gemm_narrow(v - (j + 1) * nb, ldn, nb, ctt + o1 * Nl + (int64_t)j * nb, Nl, Y + o, ldn,
+            CFLX_TRY(launch_gemm_narrow(v - (j + 1) * nb, ldn, nb, ftt + o1 * Nl + (int64_t)j * nb, Nl, Y + o, ldn,
                                         R + o1 * ldn, ldn, R + o1 * ldn, ldn, -1.0, 1.0, s));
         }
-        if (!lower && j > 0)  // R_i -= U_ij X_j, i < j
-            CFLX_TRY(launch_gemm_narrow(j * nb, ldn, nb, ctt + (int64_t)j * nb, Nl, Y + o, ldn, R, ldn, R, ldn, -1.0, 1.0, s));
+        if (tri == Tri::Upper && j > 0)
+            CFLX_TRY(launch_gemm_narrow(j * nb, ldn, nb, ftt + (int64_t)j * nb, Nl, Y + o, ldn, R, ldn, R, ldn, -1.0, 1.0, s));
+        if (tri == Tri::LowerT && j > 0)  // block row j of L_tt left of its diagonal block, as AT
+            CFLX_TRY(launch_gemm_narrow_tn(j * nb, ldn, nb, ftt + (int64_t)j * nb * Nl, Nl, Y + o, ldn, R, ldn, R, ldn,
+                                           -1.0, 1.0, s));
     }
     return CFLX_OK;
 }
 }  // namespace
 
-int lu_solve_grid(cflx_lu* lu, int nrhs, const double* B, int ldb, double* X, int ldx) {
-    cflx_comm* c = lu->comm;
-    cudaStream_t s = c->stream;
-    if (!lu->solve_ready) CFLX_TRY(solve_prepare(lu));
-    const int v = lu->v, Px = lu->Px, Py = lu->Py, Pz = lu->Pz, Ml = lu->Ml, Nl = lu->Nl, Nt = lu->Nt, M = lu->M;
-    const int pi = lu->pi, pj = lu->pj;
-    const bool layer0 = lu->pk == 0;
-    const int ldn = (int)round_up(nrhs, 8);
-    CFLX_TRY(ensure_solve_buffers(lu, ldn));
-    double *W = lu->sv_W, *Y = lu->sv_Y, *Xd = lu->sv_X;
-    const size_t tile = (size_t)v * ldn;
-    CFLX_CUDA(cudaMemsetAsync(W, 0, sizeof(double) * Ml * ldn, s));
-    CFLX_CUDA(cudaMemsetAsync(Xd, 0, sizeof(double) * M * ldn, s));
-    // W = rows of P*B on the first grid column, 0 elsewhere
-    if (layer0 && pj == 0) {
-        CFLX_CUDA(cudaMemsetAsync(lu->sv_B, 0, sizeof(double) * M * ldn, s));
-        CFLX_CUDA(cudaMemcpy2DAsync(lu->sv_B, ldn * sizeof(double), B, (size_t)ldb * sizeof(double), nrhs * sizeof(double), M,
+void solve_cache_free(SolveCache* sc) {
+    for (double* p : {sc->inv, sc->B, sc->W, sc->Z, sc->R, sc->Y, sc->X}) cudaFree(p);
+    cudaFree(sc->rows);
+    *sc = SolveCache{};
+}
+
+int solve_cache_grow(SolveCache* sc, const SolveFactor& f, int ldn, bool work, bool col_partials) {
+    if (ldn <= sc->ldn) return CFLX_OK;
+    for (double** p : {&sc->B, &sc->W, &sc->Z, &sc->R, &sc->Y, &sc->X}) {
+        cudaFree(*p);
+        *p = nullptr;
+    }
+    sc->ldn = 0;
+    const size_t M = f.M, v = f.v;
+    if (f.pk == 0 && f.pj == 0) CFLX_TRY(dmalloc(&sc->B, M * ldn));
+    if (work) {
+        CFLX_TRY(dmalloc(&sc->W, (size_t)f.Ml * ldn));
+        if (col_partials) CFLX_TRY(dmalloc(&sc->Z, (size_t)f.Nl * ldn));
+        CFLX_TRY(dmalloc(&sc->R, v * ldn));
+        CFLX_TRY(dmalloc(&sc->Y, v * ldn));
+    }
+    CFLX_TRY(dmalloc(&sc->X, M * ldn));
+    sc->ldn = ldn;
+    return CFLX_OK;
+}
+
+int solve_inverses(SolveCache* sc, const SolveFactor& f, bool lower) {
+    cudaStream_t s = f.comm->stream;
+    const int v = f.v, nb = f.nb;
+    cudaFree(sc->inv);
+    sc->inv = nullptr;
+    int nown = 0;
+    for (int t = 0; t < f.Nt; ++t) nown += diag_slot(f, t) >= 0;
+    const size_t per = 2 * (size_t)v * nb;
+    CFLX_TRY(dmalloc(&sc->inv, std::max(1, nown) * per));
+    double *tile = nullptr, *linvT = nullptr;
+    int rc = dmalloc(&tile, (size_t)v * v);
+    if (!rc) rc = dmalloc(&linvT, (size_t)v * nb);
+    for (int t = 0; t < f.Nt && !rc; ++t) {
+        const int slot = diag_slot(f, t);
+        if (slot < 0) continue;
+        double* inv = sc->inv + slot * per;
+        // launch_diag_inverses takes an A00 = L\U.  A lower L goes in as L_tt^T, as the Cholesky panel step runs it:
+        // Uinv_j = inv(L_jj)^T is then the backward half, its block transpose inv(L_jj) the forward half, and the
+        // unit-lower part is the identity.  For L\U, the forward half is the block transpose of LinvT.
+        if (lower) {
+            rc = launch_extract_panel_T(f.F, f.Nl, (int64_t)(t / f.Px) * v, (int64_t)(t / f.Py) * v, v, v, tile, v, s);
+        } else if (cudaMemcpy2DAsync(tile, v * sizeof(double), diag_tile(f, t), f.Nl * sizeof(double), v * sizeof(double),
+                                     v, cudaMemcpyDeviceToDevice, s) != cudaSuccess) {
+            set_last_error("solve: diagonal tile copy failed");
+            rc = CFLX_ERR_CUDA;
+        }
+        if (!rc) rc = launch_diag_inverses(tile, v, nb, inv + (size_t)v * nb, linvT, s);
+        if (!rc) rc = launch_transpose_blocks(lower ? inv + (size_t)v * nb : linvT, nb, (int64_t)v * nb, inv, s);
+    }
+    if (cudaStreamSynchronize(s) != cudaSuccess && !rc) rc = CFLX_ERR_CUDA;
+    cudaFree(tile);
+    cudaFree(linvT);
+    return rc;
+}
+
+int solve_set_rows(SolveCache* sc, const std::vector<int>& rows, cudaStream_t s) {
+    if (!sc->rows) CFLX_TRY(dmalloc(&sc->rows, rows.size()));
+    CFLX_CUDA(cudaMemcpyAsync(sc->rows, rows.data(), sizeof(int) * rows.size(), cudaMemcpyHostToDevice, s));
+    CFLX_CUDA(cudaStreamSynchronize(s));  // `rows` is a host temporary
+    return CFLX_OK;
+}
+
+int solve_seed(SolveCache* sc, const SolveFactor& f, int ldn, int nrhs, const double* B, int ldb) {
+    cudaStream_t s = f.comm->stream;
+    CFLX_CUDA(cudaMemsetAsync(sc->X, 0, sizeof(double) * f.M * ldn, s));
+    if (sc->W) CFLX_CUDA(cudaMemsetAsync(sc->W, 0, sizeof(double) * f.Ml * ldn, s));
+    if (sc->Z) CFLX_CUDA(cudaMemsetAsync(sc->Z, 0, sizeof(double) * f.Nl * ldn, s));
+    if (sc->B && f.rows > 0) {
+        CFLX_CUDA(cudaMemsetAsync(sc->B, 0, sizeof(double) * f.M * ldn, s));
+        CFLX_CUDA(cudaMemcpy2DAsync(sc->B, ldn * sizeof(double), B, (size_t)ldb * sizeof(double), nrhs * sizeof(double), f.M,
                                     cudaMemcpyHostToDevice, s));
-        CFLX_TRY(launch_gather_rows(lu->sv_B, ldn, lu->sv_rows, Ml, ldn, W, s));
+        CFLX_TRY(launch_gather_rows(sc->B, ldn, sc->rows, f.rows, ldn, sc->W, s));
     }
-    auto first_local_tile = [&](int t) { return std::min(Ml / v, (t - pi + Px - 1) / Px); };  // first local tile >= t
-    // tile t's rows of W, summed over the grid row, onto the diagonal owner; returns where the sum is
-    auto reduce_tile = [&](int t, double** R) -> int {
-        *R = W + (int64_t)(t / Px) * tile;
-        if (Py * Pz > 1) {
-            CFLX_NCCL(ncclReduce(*R, lu->sv_R, tile, ncclDouble, ncclSum, (t % Py) * Pz, lu->jk_comm.c, s));
-            *R = lu->sv_R;
+    return CFLX_OK;
+}
+
+int solve_row_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward, double* keep, int keep_div,
+                    bool clear_row) {
+    cudaStream_t s = f.comm->stream;
+    const int v = f.v, Px = f.Px, Py = f.Py, Nl = f.Nl, tiles = f.rows / v;
+    const bool layer0 = f.pk == 0;
+    const size_t tile = (size_t)v * ldn;
+    for (int i = 0; i < f.Nt; ++i) {
+        const int t = forward ? i : f.Nt - 1 - i;
+        const bool in_row = f.pi == t % Px, in_col = f.pj == t % Py, owner = layer0 && in_row && in_col;
+        double* const Wt = sc->W + (int64_t)(t / Px) * tile;
+        double* R = Wt;  // tile t's rows of W, summed over the grid row onto the diagonal owner
+        if (in_row && Py * f.stride > 1) {
+            CFLX_NCCL(ncclReduce(Wt, sc->R, tile, ncclDouble, ncclSum, (t % Py) * f.stride, f.row_comm->c, s));
+            R = sc->R;
         }
-        return CFLX_OK;
-    };
-    auto bcast_tile = [&](int t) -> int {
-        if (Px * Pz > 1) CFLX_NCCL(ncclBroadcast(Y, Y, tile, ncclDouble, (t % Px) * Pz, lu->ik_comm.c, s));
-        return CFLX_OK;
-    };
-    // ---- forward sweep: L Y = P B
-    for (int t = 0; t < Nt; ++t) {
-        const bool in_row = pi == t % Px, in_col = pj == t % Py, owner = layer0 && in_row && in_col;
-        double* R = nullptr;
-        if (in_row) CFLX_TRY(reduce_tile(t, &R));
-        if (owner) CFLX_TRY(diag_solve(lu, t, true, R, Y, ldn, s));
-        if (in_col) CFLX_TRY(bcast_tile(t));
-        if (in_row && layer0) {  // the backward sweep starts from W = Y, held by the diagonal owners
-            double* Wt = W + (int64_t)(t / Px) * tile;
-            if (owner) CFLX_CUDA(cudaMemcpyAsync(Wt, Y, tile * sizeof(double), cudaMemcpyDeviceToDevice, s));
-            else CFLX_CUDA(cudaMemsetAsync(Wt, 0, tile * sizeof(double), s));
-        }
-        const int row_lo = first_local_tile(t + 1) * v;
-        if (in_col && layer0 && row_lo < Ml) {  // W[tiles I > t] -= L[I, t] Y_t
-            CFLX_TRY(launch_gemm_narrow(Ml - row_lo, ldn, v, lu->Cbuf + (int64_t)row_lo * Nl + (int64_t)(t / Py) * v, Nl, Y,
-                                        ldn, W + (int64_t)row_lo * ldn, ldn, W + (int64_t)row_lo * ldn, ldn, -1.0, 1.0, s));
-        }
-    }
-    // ---- backward sweep: U X = Y
-    for (int t = Nt - 1; t >= 0; --t) {
-        const bool in_row = pi == t % Px, in_col = pj == t % Py, owner = layer0 && in_row && in_col;
-        double* R = nullptr;
-        if (in_row) CFLX_TRY(reduce_tile(t, &R));
         if (owner) {
-            CFLX_TRY(diag_solve(lu, t, false, R, Y, ldn, s));
-            CFLX_CUDA(cudaMemcpyAsync(Xd + (int64_t)t * tile, Y, tile * sizeof(double), cudaMemcpyDeviceToDevice, s));
+            CFLX_TRY(diag_solve(*sc, f, t, forward ? Tri::Lower : Tri::Upper, R, ldn, s));
+            CFLX_CUDA(cudaMemcpyAsync(keep + (int64_t)(t / keep_div) * tile, sc->Y, tile * sizeof(double),
+                                      cudaMemcpyDeviceToDevice, s));
+        } else if (clear_row && in_row && layer0) {
+            CFLX_CUDA(cudaMemsetAsync(Wt, 0, tile * sizeof(double), s));
         }
-        if (in_col) CFLX_TRY(bcast_tile(t));
-        const int row_hi = first_local_tile(t) * v;
-        if (in_col && layer0 && row_hi > 0) {  // W[tiles I < t] -= U[I, t] X_t
-            CFLX_TRY(launch_gemm_narrow(row_hi, ldn, v, lu->Cbuf + (int64_t)(t / Py) * v, Nl, Y, ldn, W, ldn, W, ldn, -1.0,
-                                        1.0, s));
-        }
+        if (in_col && Px * f.stride > 1)
+            CFLX_NCCL(ncclBroadcast(sc->Y, sc->Y, tile, ncclDouble, (t % Px) * f.stride, f.col_comm->c, s));
+        // W[tiles I > t] -= L[I, t] Y_t (forward), W[tiles I < t] -= U[I, t] X_t (backward), on the grid column
+        const int lo = forward ? std::min(tiles, first_local_tile(t + 1, f.pi, Px)) * v : 0;
+        const int hi = forward ? f.rows : std::min(tiles, first_local_tile(t, f.pi, Px)) * v;
+        if (in_col && layer0 && lo < hi)
+            CFLX_TRY(launch_gemm_narrow(hi - lo, ldn, v, f.F + (int64_t)lo * Nl + (int64_t)(t / Py) * v, Nl, sc->Y, ldn,
+                                        sc->W + (int64_t)lo * ldn, ldn, sc->W + (int64_t)lo * ldn, ldn, -1.0, 1.0, s));
     }
+    return CFLX_OK;
+}
+
+int solve_col_sweep(SolveCache* sc, const SolveFactor& f, int ldn) {
+    cudaStream_t s = f.comm->stream;
+    const int v = f.v, Px = f.Px, Py = f.Py, Nl = f.Nl;
+    const size_t tile = (size_t)v * ldn;
+    for (int t = f.Nt - 1; t >= 0; --t) {
+        const bool in_row = f.pi == t % Px, in_col = f.pj == t % Py, owner = in_row && in_col;
+        double* R = sc->Z + (int64_t)(t / Py) * tile;  // tile t's columns of Z, summed over the grid column onto the owner
+        if (in_col && Px * f.stride > 1) {
+            CFLX_NCCL(ncclReduce(R, sc->R, tile, ncclDouble, ncclSum, (t % Px) * f.stride, f.col_comm->c, s));
+            R = sc->R;
+        }
+        if (owner) {
+            CFLX_TRY(diag_solve(*sc, f, t, Tri::LowerT, R, ldn, s));
+            CFLX_CUDA(cudaMemcpyAsync(sc->X + (int64_t)t * tile, sc->Y, tile * sizeof(double), cudaMemcpyDeviceToDevice, s));
+        }
+        if (!in_row) continue;
+        if (Py * f.stride > 1)
+            CFLX_NCCL(ncclBroadcast(sc->Y, sc->Y, tile, ncclDouble, (t % Py) * f.stride, f.row_comm->c, s));
+        const int m = first_local_tile(t, f.pj, Py) * v;  // local columns with gj < t: a prefix of the tile row
+        if (m > 0)  // Z[columns gj < t] -= L[t, gj]^T X_t
+            CFLX_TRY(launch_gemm_narrow_tn(m, ldn, v, f.F + (int64_t)(t / Px) * v * Nl, Nl, sc->Y, ldn, sc->Z, ldn, sc->Z,
+                                           ldn, -1.0, 1.0, s));
+    }
+    return CFLX_OK;
+}
+
+int solve_finish(SolveCache* sc, const SolveFactor& f, int ldn, int nrhs, double* X, int ldx) {
+    cudaStream_t s = f.comm->stream;
     // exactly one rank contributes each element: the sum is X itself, bit for bit, on every rank
-    if (lu->P > 1) CFLX_NCCL(ncclAllReduce(Xd, Xd, (size_t)M * ldn, ncclDouble, ncclSum, c->world, s));
+    if (f.P > 1) CFLX_NCCL(ncclAllReduce(sc->X, sc->X, (size_t)f.M * ldn, ncclDouble, ncclSum, f.comm->world, s));
     if (X)
-        CFLX_CUDA(cudaMemcpy2DAsync(X, (size_t)ldx * sizeof(double), Xd, ldn * sizeof(double), nrhs * sizeof(double), M,
+        CFLX_CUDA(cudaMemcpy2DAsync(X, (size_t)ldx * sizeof(double), sc->X, ldn * sizeof(double), nrhs * sizeof(double), f.M,
                                     cudaMemcpyDeviceToHost, s));
     CFLX_CUDA(cudaStreamSynchronize(s));
     return CFLX_OK;

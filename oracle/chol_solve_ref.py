@@ -1,4 +1,5 @@
-"""oracle/chol_solve_ref.py -- TEST INFRASTRUCTURE: numpy restatement of cflx_chol_solve (conflux_b200/csrc/chol.cu).
+"""oracle/chol_solve_ref.py -- TEST INFRASTRUCTURE: numpy restatement of cflx_chol_solve (conflux_b200/csrc/chol.cu,
+solve.cu).
 
 The specification of the Cholesky solve's schedule, checkable without GPUs.  It takes every rank's local share of the
 factor in the CONFCHOX layout (what cflx_chol_get_local returns: tile (gi, gj), gi >= gj, of L on rank (gi % Px, gj % Py,
@@ -18,14 +19,7 @@ communicator of one rank are skipped, as on the device."""
 import numpy as np
 
 from . import chol_ref, layout
-
-
-def pick_nb(v):
-    """Block size of the diagonal inverses (chol.cu chol_pick_nb)."""
-    for nb in (128, 64, 32, 16, 8, 4):
-        if v % nb == 0:
-            return nb
-    raise ValueError(f"v={v}: no supported block size")
+from .solve_ref import backward_error, pick_nb  # noqa: F401  (backward_error: for the tests)
 
 
 def scatter(A, N, v, Px=1, Py=1, Pz=1, upper=None, pad=0.0, layers=0.0):
@@ -135,8 +129,3 @@ def solve(L_locals, B, N, v, Px=1, Py=1, Pz=1, log=None):
     X = sum(Xr.values())[:, :nrhs]                                  # one contributor per element
     return X.reshape(Np) if vec else X
 
-
-def backward_error(A, X, B):
-    """Normwise backward error ||B - A X||_F / (||A||_F ||X||_F + ||B||_F)."""
-    X, B = np.asarray(X).reshape(len(B), -1), np.asarray(B).reshape(len(B), -1)
-    return float(np.linalg.norm(B - A @ X) / (np.linalg.norm(A) * np.linalg.norm(X) + np.linalg.norm(B)))

@@ -1,4 +1,4 @@
-"""oracle/solve_ref.py -- TEST INFRASTRUCTURE: numpy restatement of cflx_lu_solve (conflux_b200/csrc/solve.cu).
+"""oracle/solve_ref.py -- TEST INFRASTRUCTURE: numpy restatement of cflx_lu_solve (conflux_b200/csrc/lu.cu, solve.cu).
 
 The specification of the solve's communication schedule, checkable without GPUs.  It takes every rank's factors in the
 conflux block-cyclic layout (what cflx_lu_get_factors / restate.lu return: tile (I, J) of L\\U on rank (I % Px, J % Py, 0))
@@ -18,7 +18,7 @@ from . import layout
 
 
 def pick_nb(v):
-    """Block size of the diagonal inverses (lu.cu pick_nb with its default cap of 128)."""
+    """Block size of the diagonal inverses (lu.cu pick_nb with its default cap of 128, and chol.cu chol_pick_nb)."""
     for nb in (128, 64, 32, 16, 8, 4):
         if v % nb == 0:
             return nb
@@ -105,5 +105,6 @@ def host_solve(LU, perm, B):
 
 
 def backward_error(A, X, B):
-    """Normwise backward error ||B - A X||_F / (||A||_F ||X||_F + ||B||_F)."""
+    """Normwise backward error ||B - A X||_F / (||A||_F ||X||_F + ||B||_F); X and B may be vectors."""
+    X, B = np.asarray(X).reshape(len(B), -1), np.asarray(B).reshape(len(B), -1)
     return float(np.linalg.norm(B - A @ X) / (np.linalg.norm(A) * np.linalg.norm(X) + np.linalg.norm(B)))

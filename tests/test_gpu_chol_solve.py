@@ -3,7 +3,11 @@ scipy's cho_solve on the device's own factor and the schedule restatement (oracl
 ill-conditioned matrices; its state rules; and that it leaves the factorisation untouched.
 
 Tolerances: the backward error ||B - A X||_F / (||A||_F ||X||_F + ||B||_F) <= 1e-13, and X within 1e-10 max|X| of the
-host solve and of the restatement on the same factor (the same operations, in other summation orders)."""
+host solve and of the restatement on the same factor (the same operations, in other summation orders).  X of integer
+right-hand sides is bit for bit the one pinned in tests/golden/solve_bits.json."""
+import json
+import os
+
 import numpy as np
 import pytest
 import scipy.linalg
@@ -11,6 +15,7 @@ import scipy.linalg
 import conflux_b200 as cb
 from oracle import chol_ref, chol_solve_ref, hp_ref as hp
 from tests._harness import n_gpus, run_ranks
+from tests.golden import make_solve_golden
 
 pytestmark = pytest.mark.gpu
 ETA_TOL = 1e-13
@@ -239,6 +244,14 @@ def test_solve_is_deterministic():
     assert np.array_equal(ch.solve(B), ch.solve(B))
     ch.finalize()
     comm.close()
+
+
+def test_solve_bits_are_pinned(golden_dir):
+    """X of integer right-hand sides is the one recorded by tests/golden/make_solve_golden.py"""
+    with open(os.path.join(golden_dir, "solve_bits.json")) as f:
+        want = json.load(f)
+    for kind, N, v in make_solve_golden.CHOL_CASES:
+        assert make_solve_golden.chol_solve_bits(kind, N, v) == want[f"chol_{kind}_{N}_{v}"], (kind, N, v)
 
 
 @pytest.mark.parametrize("v", [128, 512])

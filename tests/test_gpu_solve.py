@@ -1,12 +1,16 @@
 """GPU: cflx_lu_solve (A X = B with the factors left on the device) and its narrow GEMM, against numpy, the host
 triangular solves on the gathered factors and the schedule restatement (oracle/solve_ref.py); its state rules; and that
-it leaves the factorisation untouched."""
+it leaves the factorisation untouched; and that X is bit for bit the one pinned in tests/golden/solve_bits.json."""
+import json
+import os
+
 import numpy as np
 import pytest
 
 import conflux_b200 as cb
 from oracle import layout, solve_ref
 from tests._harness import n_gpus, run_ranks
+from tests.golden import make_solve_golden
 
 pytestmark = pytest.mark.gpu
 ETA_TOL = 1e-13           # normwise backward error ||B - A X||_F / (||A||_F ||X||_F + ||B||_F)
@@ -172,6 +176,14 @@ def test_solve_is_deterministic():
     assert np.array_equal(cb.lu_solve(gv, B), cb.lu_solve(gv, B))
     gv.free_comms()
     comm.close()
+
+
+def test_solve_bits_are_pinned(golden_dir):
+    """X of integer right-hand sides is the one recorded by tests/golden/make_solve_golden.py"""
+    with open(os.path.join(golden_dir, "solve_bits.json")) as f:
+        want = json.load(f)
+    for N, v in make_solve_golden.LU_CASES:
+        assert make_solve_golden.lu_solve_bits(N, v) == want[f"lu_{N}_{v}"], (N, v)
 
 
 @pytest.mark.parametrize("N,v,Px,Py,Pz", GRIDS)
