@@ -15,7 +15,7 @@ import numpy as np
 
 from ._lib import ConfluxError, LIB_PATH, SYMBOLS, check, lib
 
-__all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "residual", "validate", "lu_solve", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
+__all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "residual", "validate", "lu_solve", "lu_rcond", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
 
 
 def auto_grid(M, N, P):
@@ -201,18 +201,27 @@ def residual(gv):
     return validate(gv)[1]
 
 
-def lu_solve(gv, B):
-    """Solves A X = B with the factors of the last LU_rep (P A = L U) on the GPU grid, like LAPACK's getrs.  COLLECTIVE
-    over gv.lu_comm; every rank passes the same B, (M,) or (M, nrhs) with M = gv.M (the padded size), and gets the same X
-    in the same shape.  The factors and the input matrix are left as they are."""
+def lu_solve(gv, B, trans=False):
+    """Solves A X = B (A^T X = B when trans) with the factors of the last LU_rep (P A = L U) on the GPU grid, like
+    LAPACK's getrs.  COLLECTIVE over gv.lu_comm; every rank passes the same B, (M,) or (M, nrhs) with M = gv.M (the padded
+    size), and gets the same X in the same shape.  The factors and the input matrix are left as they are."""
     B = np.asarray(B, dtype=np.float64)
     if B.ndim not in (1, 2) or B.shape[0] != gv.M:
         raise ValueError(f"lu_solve: B must have shape ({gv.M},) or ({gv.M}, nrhs), got {B.shape}")
     B2 = np.ascontiguousarray(B.reshape(gv.M, -1))
     nrhs = B2.shape[1]
     X = np.empty_like(B2)
-    check(lib().cflx_lu_solve(gv._h, nrhs, B2.ctypes.data, max(nrhs, 1), X.ctypes.data, max(nrhs, 1)), "lu_solve")
+    fn = lib().cflx_lu_solve_trans if trans else lib().cflx_lu_solve
+    check(fn(gv._h, nrhs, B2.ctypes.data, max(nrhs, 1), X.ctypes.data, max(nrhs, 1)), "lu_solve")
     return X.reshape(B.shape)
+
+
+def lu_rcond(gv):
+    """LAPACK dgecon (1-norm) of the last LU_rep on the GPU grid: (rcond, anorm) with anorm = ||A||_1 of the padded input
+    and rcond = 1 / (anorm * estimate of ||A^-1||_1), 0 for an exactly singular U.  COLLECTIVE; identical on every rank."""
+    r, a = ctypes.c_double(), ctypes.c_double()
+    check(lib().cflx_lu_rcond(gv._h, ctypes.byref(r), ctypes.byref(a)), "lu_rcond")
+    return r.value, a.value
 
 
 class cholesky:
@@ -271,6 +280,13 @@ class cholesky:
         X = np.empty_like(B2)
         check(lib().cflx_chol_solve(self._h, nrhs, B2.ctypes.data, max(nrhs, 1), X.ctypes.data, max(nrhs, 1)), "chol_solve")
         return X.reshape(B.shape)
+
+    def rcond(self):
+        """LAPACK dpocon of the last parallelCholesky on the GPU grid: (rcond, anorm) with anorm = ||A||_1 of the padded
+        symmetric input and rcond = 1 / (anorm * estimate of ||A^-1||_1).  COLLECTIVE; identical on every rank."""
+        r, a = ctypes.c_double(), ctypes.c_double()
+        check(lib().cflx_chol_rcond(self._h, ctypes.byref(r), ctypes.byref(a)), "chol_rcond")
+        return r.value, a.value
 
     def finalize(self, clean=True):
         if self._h:

@@ -622,7 +622,7 @@ int chol_solve_prepare(cflx_chol* ch) {
             const int v = ch->v;
             std::vector<int> rows(std::max(f.rows, 1), 0);
             for (int r = 0; r < f.rows; ++r) rows[r] = ((r / v) * ch->Px + ch->pi) * v + r % v;
-            CFLX_TRY(solve_set_rows(&ch->sv, rows, c->stream));
+            CFLX_TRY(solve_set_rows(&ch->sv.rows, rows, c->stream));
         }
     }
     ch->sv.ready = true;
@@ -976,12 +976,36 @@ int cflx_chol_solve(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X
     SolveCache* sc = &ch->sv;
     const int ldn = (int)round_up(nrhs, 8);
     CFLX_TRY(solve_cache_grow(sc, f, ldn, ch->pk == 0, true));
-    CFLX_TRY(solve_seed(sc, f, ldn, nrhs, B, ldb));
+    CFLX_TRY(solve_seed(sc, f, ldn, nrhs, B, ldb, SolveSeed{false, sc->rows, f.rows, sc->W}));
     if (ch->pk == 0) {  // L Y = B keeping Y_t in Z, then L^T X = Y from Z
         CFLX_TRY(solve_row_sweep(sc, f, ldn, true, sc->Z, ch->Py, false));
-        CFLX_TRY(solve_col_sweep(sc, f, ldn));
+        CFLX_TRY(solve_col_sweep(sc, f, ldn, false, Tri::LowerT, sc->X, 1, false));
     }
     return solve_finish(sc, f, ldn, nrhs, X, ldx);
+}
+
+// COLLECTIVE.  LAPACK dpocon on the grid: ||A||_1 of the symmetric input (its stored lower triangle, real tiles only) and
+// the Hager-Higham estimate of ||inv(A)||_1, whose products inv(A) x are solves with the factor.
+int cflx_chol_rcond(cflx_chol* ch, double* rcond_out, double* anorm_out) {
+    if (!ch || !rcond_out) return CFLX_ERR_ARG;
+    if (!ch->factored) {
+        set_last_error("cholesky condition estimate requested before a successful cflx_chol_factor, or after cflx_chol_set_local without one");
+        return CFLX_ERR_STATE;
+    }
+    CFLX_CUDA(cudaSetDevice(ch->comm->device));
+    double anorm = 0.0, ainvnm = 0.0;
+    CFLX_TRY(norm1_grid(ch->comm, ch->A0, ch->N, ch->Ml, ch->Nl, ch->v, ch->Kappa, ch->Px, ch->Py, ch->pi, ch->pj, ch->pk,
+                        true, &anorm));
+    if (anorm > 0.0) {
+        // every rank runs the estimator on the X of solve_finish, bit-identical on every rank, so every rank makes the
+        // same choices and issues the same solves (the same collectives) in the same order; A is symmetric, so both
+        // kinds of product are the same solve
+        auto apply = [&](int, double* x) { return cflx_chol_solve(ch, 1, x, 1, x, 1); };
+        CFLX_TRY(estimate_inv_norm1(ch->N, apply, &ainvnm));
+    }
+    *rcond_out = rcond_from(anorm, ainvnm);
+    if (anorm_out) *anorm_out = anorm;
+    return CFLX_OK;
 }
 
 int cflx_chol_launch_count(cflx_chol* ch, int64_t* count_out, int reset) {

@@ -551,11 +551,64 @@ int lu_solve_prepare(cflx_lu* lu) {
                 const int k = q / v;
                 if (k % Px == lu->pi) rows[(k / Px) * v + q % v] = hist[q];
             }
-            CFLX_TRY(solve_set_rows(&lu->sv, rows, s));
+            CFLX_TRY(solve_set_rows(&lu->sv.rows, rows, s));
         }
     }
     lu->sv.ready = true;
+    lu->sv.trans_ready = false;
     return CFLX_OK;
+}
+
+// First transposed solve or condition estimate after a factorisation: the seeding maps of P*A solved without P (B by
+// local tile row on the ranks (pi, 0, 0) and by local tile column on the ranks (0, pj, 0), identity in both), and on every
+// rank the inverse permutation that puts W[q] at row perm[q] of X.
+int lu_solve_prepare_trans(cflx_lu* lu) {
+    cudaStream_t s = lu->comm->stream;
+    const int v = lu->v, Px = lu->Px, Py = lu->Py;
+    std::vector<int> hist(lu->M);
+    CFLX_TRY(cflx_lu_get_permutation(lu, hist.data()));
+    std::vector<int> unperm(lu->M);
+    for (int q = 0; q < lu->M; ++q) unperm[hist[q]] = q;
+    CFLX_TRY(solve_set_rows(&lu->sv.unperm, unperm, s));
+    if (lu->pk == 0 && lu->pj == 0) {
+        std::vector<int> rows(lu->Ml, 0);
+        for (int q = 0; q < lu->M; ++q)
+            if ((q / v) % Px == lu->pi) rows[(q / v / Px) * v + q % v] = q;
+        CFLX_TRY(solve_set_rows(&lu->sv.rows_id, rows, s));
+    }
+    if (lu->pk == 0 && lu->pi == 0) {
+        std::vector<int> cols(lu->Nl, 0);
+        for (int q = 0; q < lu->M; ++q)
+            if ((q / v) % Py == lu->pj) cols[(q / v / Py) * v + q % v] = q;
+        CFLX_TRY(solve_set_rows(&lu->sv.cols, cols, s));
+    }
+    lu->sv.trans_ready = true;
+    return CFLX_OK;
+}
+
+// One solve with the factors of the last factorisation.  transposed: A^T X = B, else A X = B.  pa: the system is P*A
+// (no row map of B in A X = B, no final P^T in A^T X = B), as the condition estimate runs it.  X may be null (the solved
+// system then stays in lu->sv.X, or sv.Xg after P^T).
+int lu_sweeps(cflx_lu* lu, bool transposed, bool pa, int nrhs, const double* B, int ldb, double* X, int ldx) {
+    if (!lu->sv.ready) CFLX_TRY(lu_solve_prepare(lu));
+    if ((transposed || pa) && !lu->sv.trans_ready) CFLX_TRY(lu_solve_prepare_trans(lu));
+    const SolveFactor f = lu_solve_factor(lu);
+    SolveCache* sc = &lu->sv;
+    const int ldn = (int)round_up(nrhs, 8);
+    CFLX_TRY(solve_cache_grow(sc, f, ldn, true, transposed, transposed));
+    if (!transposed) {
+        CFLX_TRY(solve_seed(sc, f, ldn, nrhs, B, ldb, SolveSeed{false, pa ? sc->rows_id : sc->rows, lu->Ml, sc->W}));
+        // L Y = P B keeping Y_t as the owner's W rows, so that U X = Y starts from W = Y
+        CFLX_TRY(solve_row_sweep(sc, f, ldn, true, sc->W, lu->Px, true));
+        CFLX_TRY(solve_row_sweep(sc, f, ldn, false, sc->X, 1, false));
+        return solve_finish(sc, f, ldn, nrhs, X, ldx);
+    }
+    // A^T X = B <=> U^T (L^T W) = B, X[perm[q]] = W[q]: U^T Y = B keeping Y_t as the owner's Z columns, so that L^T W = Y
+    // starts from Z = Y
+    CFLX_TRY(solve_seed(sc, f, ldn, nrhs, B, ldb, SolveSeed{true, sc->cols, lu->Nl, sc->Z}));
+    CFLX_TRY(solve_col_sweep(sc, f, ldn, true, Tri::UpperT, sc->Z, lu->Py, true));
+    CFLX_TRY(solve_col_sweep(sc, f, ldn, false, Tri::UnitLowerT, sc->X, 1, false));
+    return solve_finish(sc, f, ldn, nrhs, X, ldx, pa ? nullptr : sc->unperm);
 }
 }  // namespace
 
@@ -1024,16 +1077,45 @@ int cflx_lu_solve(cflx_lu* lu, int nrhs, const double* B, int ldb, double* X, in
         return CFLX_ERR_STATE;
     }
     CFLX_CUDA(cudaSetDevice(lu->comm->device));
-    if (!lu->sv.ready) CFLX_TRY(lu_solve_prepare(lu));
-    const SolveFactor f = lu_solve_factor(lu);
-    SolveCache* sc = &lu->sv;
-    const int ldn = (int)round_up(nrhs, 8);
-    CFLX_TRY(solve_cache_grow(sc, f, ldn, true, false));
-    CFLX_TRY(solve_seed(sc, f, ldn, nrhs, B, ldb));
-    // L Y = P B keeping Y_t as the owner's W rows, so that U X = Y starts from W = Y
-    CFLX_TRY(solve_row_sweep(sc, f, ldn, true, sc->W, lu->Px, true));
-    CFLX_TRY(solve_row_sweep(sc, f, ldn, false, sc->X, 1, false));
-    return solve_finish(sc, f, ldn, nrhs, X, ldx);
+    return lu_sweeps(lu, false, false, nrhs, B, ldb, X, ldx);
+}
+
+// A^T X = B with the same factors and state rules: U^T Y = B, L^T W = Y by column-partial sweeps, then X = P^T W.
+int cflx_lu_solve_trans(cflx_lu* lu, int nrhs, const double* B, int ldb, double* X, int ldx) {
+    if (!lu || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B) return CFLX_ERR_ARG;
+    if (!lu->factored) {
+        set_last_error("transposed solve requested before cflx_lu_factor, or after cflx_lu_set_local without a factorisation");
+        return CFLX_ERR_STATE;
+    }
+    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    return lu_sweeps(lu, true, false, nrhs, B, ldb, X, ldx);
+}
+
+// LAPACK dgecon (NORM = '1') on the grid: ||A||_1 of the input A0 (the padded M x M matrix), and the Hager-Higham estimate
+// of ||inv(P A)||_1 = ||inv(A)||_1 from inv(U) inv(L) x and inv(L)^T inv(U)^T x, as dgecon runs it on L and U alone.
+int cflx_lu_rcond(cflx_lu* lu, double* rcond_out, double* anorm_out) {
+    if (!lu || !rcond_out) return CFLX_ERR_ARG;
+    if (!lu->factored) {
+        set_last_error("condition estimate requested before cflx_lu_factor, or after cflx_lu_set_local without a factorisation");
+        return CFLX_ERR_STATE;
+    }
+    if (lu->a0_is_next) {
+        set_last_error("condition estimate refused: the input buffer of the last run was handed to the queued next matrix");
+        return CFLX_ERR_STATE;
+    }
+    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    double anorm = 0.0, ainvnm = 0.0;
+    CFLX_TRY(norm1_grid(lu->comm, lu->A0, lu->M, lu->Ml, lu->Nl, lu->v, lu->Nt, lu->Px, lu->Py, lu->pi, lu->pj, lu->pk,
+                        false, &anorm));
+    if (anorm > 0.0) {
+        // every rank runs the estimator on the X of solve_finish, bit-identical on every rank, so every rank makes the
+        // same choices and issues the same solves (the same collectives) in the same order
+        auto apply = [&](int kase, double* x) { return lu_sweeps(lu, kase == 2, true, 1, x, 1, x, 1); };
+        CFLX_TRY(estimate_inv_norm1(lu->M, apply, &ainvnm));
+    }
+    *rcond_out = rcond_from(anorm, ainvnm);
+    if (anorm_out) *anorm_out = anorm;
+    return CFLX_OK;
 }
 
 int cflx_host_alloc(size_t bytes, void** out) {

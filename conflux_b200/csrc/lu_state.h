@@ -5,6 +5,7 @@
 #include <nccl.h>
 
 #include <algorithm>
+#include <functional>
 #include <vector>
 
 #include "../../include/conflux_b200.h"
@@ -74,8 +75,30 @@ struct SolveCache {
     double* inv = nullptr;  // per owned diagonal tile: the forward inverse blocks (v x nb, row-major nb x nb each), then
                             // the backward ones
     int* rows = nullptr;    // row of B of each seeded local row (ranks (pi, 0, 0))
-    double *B = nullptr, *W = nullptr, *Z = nullptr, *R = nullptr, *Y = nullptr, *X = nullptr;
+    // the transposed LU solve and the LU condition estimate, prepared on first use after solve data is prepared
+    bool trans_ready = false;
+    int* rows_id = nullptr;  // identity row map by local tile row (ranks (pi, 0, 0)): P*A solved without P
+    int* cols = nullptr;     // row of B of each seeded local column (ranks (0, pj, 0))
+    int* unperm = nullptr;   // row of the solved system that lands in each row of X: X[perm[q]] = W[q] (every rank)
+    double *B = nullptr, *W = nullptr, *Z = nullptr, *R = nullptr, *Y = nullptr, *X = nullptr, *Xg = nullptr;
     int ldn = 0;
+    bool col_partials = false, col_seed = false;  // what the buffers were grown for (kept across growth)
+};
+
+// The triangle a diagonal-tile solve applies, and how (solve.cu diag_solve):
+//   Lower:      L_tt       (forward inverses, NN)          Upper:  U_tt   (backward inverses, NN)
+//   LowerT:     L_tt^T     (backward inverses, NN: the Cholesky's inv(L_jj)^T)
+//   UnitLowerT: L_tt^T     (forward inverses read transposed, TN: the LU's unit L)
+//   UpperT:     U_tt^T     (backward inverses read transposed, TN)
+enum class Tri { Lower, Upper, LowerT, UnitLowerT, UpperT };
+
+// Where a right-hand side enters the sweeps: B is held on the layer-0 ranks of grid column 0 (by_col = false, dst = W by
+// local tile row) or of grid row 0 (by_col, dst = Z by local tile column), and dst[r] = B[rows[r]] for r < n there.
+struct SolveSeed {
+    bool by_col;
+    const int* rows;
+    int n;
+    double* dst;
 };
 
 // One factor in the conflux block-cyclic layout, as the engine reads it: tile (I, J) on rank (I % Px, J % Py, 0) at
@@ -142,22 +165,40 @@ int lu_residual_grid(cflx_lu* lu, const std::vector<int>& hist, double* abs_out,
 // solve.cu: the solve engine.  Every function returns CFLX_OK or an error code; all work goes on f.comm->stream.
 void solve_cache_free(SolveCache* sc);
 // grow the work buffers to ldn columns: B (M rows) on rank (pi, 0, 0), W (Ml) and R, Y (v) where `work`, Z (Nl) where
-// `work && col_partials`, X (M) on every rank
-int solve_cache_grow(SolveCache* sc, const SolveFactor& f, int ldn, bool work, bool col_partials);
+// `work && col_partials`, X (M) on every rank.  col_seed: also B on rank (0, pj, 0) and Xg (M) on every rank.  What was
+// once asked for stays allocated.
+int solve_cache_grow(SolveCache* sc, const SolveFactor& f, int ldn, bool work, bool col_partials, bool col_seed = false);
 // the inverses of the nb x nb diagonal blocks of every owned diagonal tile, into sc->inv (freed and allocated again here).
 // lower: the tile is L with its own diagonal and zeros above, inverted as A00 = L^T; otherwise it is L\U with a unit L.
 int solve_inverses(SolveCache* sc, const SolveFactor& f, bool lower);
-// sc->rows = rows (allocated on first use), waited for
-int solve_set_rows(SolveCache* sc, const std::vector<int>& rows, cudaStream_t s);
-// zero X, W and Z, and on the ranks holding B: W[r] = B[rows[r]] for the f.rows seeded rows
-int solve_seed(SolveCache* sc, const SolveFactor& f, int ldn, int nrhs, const double* B, int ldb);
+// *dst = rows (allocated on first use), waited for
+int solve_set_rows(int** dst, const std::vector<int>& rows, cudaStream_t s);
+// zero X, W and Z, and on the ranks holding B (`at`): at.dst[r] = B[at.rows[r]] for r < at.n
+int solve_seed(SolveCache* sc, const SolveFactor& f, int ldn, int nrhs, const double* B, int ldb, const SolveSeed& at);
 // row-partial sweep over the tile diagonal: forward with the lower triangle (NN), backward with the upper one (NN).  The
 // diagonal owner keeps each solved tile t at tile t / keep_div of `keep`; with clear_row, keep is W and the other layer-0
 // ranks of the grid row zero their copy of that tile.
 int solve_row_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward, double* keep, int keep_div,
                     bool clear_row);
-// column-partial backward sweep L^T X = Y (Z by local tile column, L read transposed), solved tiles into X; layer 0 only
-int solve_col_sweep(SolveCache* sc, const SolveFactor& f, int ldn);
-// X (nrhs columns, ldx) = the world sum of the owners' tiles of sc->X, downloaded when X is not null; synchronises
-int solve_finish(SolveCache* sc, const SolveFactor& f, int ldn, int nrhs, double* X, int ldx);
+// column-partial sweep over the tile diagonal (Z by local tile column, the factor read transposed): backward with L^T
+// (tri LowerT or UnitLowerT; update of the local columns gj < t), forward with U^T (UpperT; update of the columns
+// gj > t).  The diagonal owner keeps each solved tile t at tile t / keep_div of `keep`; with clear_col, keep is Z and the
+// other layer-0 ranks of the grid column zero their copy of that tile.  Ranks pk != 0 join the collectives only.
+int solve_col_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward, Tri tri, double* keep, int keep_div,
+                    bool clear_col);
+// X (nrhs columns, ldx) = the world sum of the owners' tiles of sc->X, downloaded when X is not null; synchronises.
+// unperm (M rows, every rank): row i of X is row unperm[i] of that sum.
+int solve_finish(SolveCache* sc, const SolveFactor& f, int ldn, int nrhs, double* X, int ldx, const int* unperm = nullptr);
+// Hager-Higham estimate of ||inv(A)||_1 for an order-n A, as LAPACK's dlacn2 runs it (x = 1/n, at most 5 iterations,
+// the sign-vector test, the final alternating vector).  apply(kase, x) overwrites the host vector x with inv(A) x
+// (kase 1) or inv(A)^T x (kase 2) and returns a status.  Pure host logic on x: ranks that pass bit-identical vectors
+// make the same choices, so every rank calls `apply` the same number of times with the same kase.
+int estimate_inv_norm1(int n, const std::function<int(int, double*)>& apply, double* est);
+// the collective 1-norm of the matrix whose layer-0 shares are A (Ml x Nl, conflux layout), into *anorm (every rank).
+// lower_sym: only the lower triangle of the real tiles (global tile index < Nt) is stored and the matrix is its symmetric
+// completion; otherwise every local entry of the M x M matrix counts.  Deterministic: no floating-point atomics.
+int norm1_grid(cflx_comm* c, const double* A, int M, int Ml, int Nl, int v, int Nt, int Px, int Py, int pi, int pj,
+               int pk, bool lower_sym, double* anorm);
+// rcond = (1 / ainvnm) / anorm as LAPACK's dgecon / dpocon form it; 0 when anorm is 0 or the estimate is not finite
+double rcond_from(double anorm, double ainvnm);
 }  // namespace cflx

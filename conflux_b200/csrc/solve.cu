@@ -13,6 +13,7 @@
 // over the grid column, the broadcast over the grid row, and the update read transposed in place.  The owners write
 // X_t into a zeroed M x ldn buffer, and one all-reduce makes X identical on every rank.  All arithmetic is the narrow
 // GEMM below: a factor block (row-major, read in place) times a few right-hand sides.
+#include <cmath>
 #include <cstring>
 
 #include "lu_state.h"
@@ -338,24 +339,30 @@ const double* diag_tile(const SolveFactor& f, int t) {
     return f.F + (int64_t)(t / f.Px) * f.v * f.Nl + (int64_t)(t / f.Py) * f.v;
 }
 
-enum class Tri { Lower, Upper, LowerT };
-
 // Y = T^-1 R on the owner of diagonal tile t, by an nb-block sweep with the cached inverses; R (v x ldn) is overwritten.
-//   Lower:  T = L_tt:    Y_j = inv(L_jj) R_j, then R_i -= L_ij Y_j for i > j (the forward inverses)
-//   Upper:  T = U_tt:    Y_j = inv(U_jj) R_j, then R_i -= U_ij Y_j for i < j (the backward inverses)
-//   LowerT: T = L_tt^T:  Y_j = inv(L_jj)^T R_j, then R_i -= L_ji^T Y_j for i < j (the backward inverses; L_tt read
-//           transposed in place)
+//   Lower:      T = L_tt:    Y_j = inv(L_jj) R_j, then R_i -= L_ij Y_j for i > j (the forward inverses)
+//   Upper:      T = U_tt:    Y_j = inv(U_jj) R_j, then R_i -= U_ij Y_j for i < j (the backward inverses)
+//   LowerT:     T = L_tt^T:  Y_j = inv(L_jj)^T R_j, then R_i -= L_ji^T Y_j for i < j (the backward inverses; L_tt read
+//               transposed in place)
+//   UnitLowerT: as LowerT, but inv(L_jj)^T is the forward inverse block read transposed (the LU's unit L)
+//   UpperT:     T = U_tt^T:  Y_j = inv(U_jj)^T R_j (the backward inverse block read transposed), then R_i -= U_ji^T Y_j
+//               for i > j: one TN launch on block row j of U_tt right of its diagonal block
 int diag_solve(const SolveCache& sc, const SolveFactor& f, int t, Tri tri, double* R, int ldn, cudaStream_t s) {
     const int v = f.v, nb = f.nb, Nl = f.Nl, nblk = v / nb;
-    const bool fwd = tri == Tri::Lower;
-    const double* inv = sc.inv + diag_slot(f, t) * 2 * (size_t)v * nb + (fwd ? 0 : (size_t)v * nb);
+    const bool fwd = tri == Tri::Lower, ascending = fwd || tri == Tri::UpperT;
+    const bool fwd_half = fwd || tri == Tri::UnitLowerT, inv_tn = tri == Tri::UnitLowerT || tri == Tri::UpperT;
+    const double* inv = sc.inv + diag_slot(f, t) * 2 * (size_t)v * nb + (fwd_half ? 0 : (size_t)v * nb);
     const double* ftt = diag_tile(f, t);
     double* Y = sc.Y;
     for (int i = 0; i < nblk; ++i) {
-        const int j = fwd ? i : nblk - 1 - i;
+        const int j = ascending ? i : nblk - 1 - i;
         const int64_t o = (int64_t)j * nb * ldn;
-        CFLX_TRY(launch_gemm_narrow(nb, ldn, nb, inv + (size_t)j * nb * nb, nb, R + o, ldn, nullptr, ldn, Y + o, ldn, 1.0,
-                                    0.0, s));
+        if (inv_tn)
+            CFLX_TRY(launch_gemm_narrow_tn(nb, ldn, nb, inv + (size_t)j * nb * nb, nb, R + o, ldn, nullptr, ldn, Y + o, ldn,
+                                           1.0, 0.0, s));
+        else
+            CFLX_TRY(launch_gemm_narrow(nb, ldn, nb, inv + (size_t)j * nb * nb, nb, R + o, ldn, nullptr, ldn, Y + o, ldn,
+                                        1.0, 0.0, s));
         if (fwd && j + 1 < nblk) {
             const int64_t o1 = (int64_t)(j + 1) * nb;
             CFLX_TRY(launch_gemm_narrow(v - (j + 1) * nb, ldn, nb, ftt + o1 * Nl + (int64_t)j * nb, Nl, Y + o, ldn,
@@ -363,36 +370,45 @@ int diag_solve(const SolveCache& sc, const SolveFactor& f, int t, Tri tri, doubl
         }
         if (tri == Tri::Upper && j > 0)
             CFLX_TRY(launch_gemm_narrow(j * nb, ldn, nb, ftt + (int64_t)j * nb, Nl, Y + o, ldn, R, ldn, R, ldn, -1.0, 1.0, s));
-        if (tri == Tri::LowerT && j > 0)  // block row j of L_tt left of its diagonal block, as AT
+        if ((tri == Tri::LowerT || tri == Tri::UnitLowerT) && j > 0)  // block row j of L_tt left of its diagonal block, as AT
             CFLX_TRY(launch_gemm_narrow_tn(j * nb, ldn, nb, ftt + (int64_t)j * nb * Nl, Nl, Y + o, ldn, R, ldn, R, ldn,
                                            -1.0, 1.0, s));
+        if (tri == Tri::UpperT && j + 1 < nblk) {  // block row j of U_tt right of its diagonal block, as AT
+            const int64_t o1 = (int64_t)(j + 1) * nb;
+            CFLX_TRY(launch_gemm_narrow_tn(v - (j + 1) * nb, ldn, nb, ftt + (int64_t)j * nb * Nl + o1, Nl, Y + o, ldn,
+                                           R + o1 * ldn, ldn, R + o1 * ldn, ldn, -1.0, 1.0, s));
+        }
     }
     return CFLX_OK;
 }
 }  // namespace
 
 void solve_cache_free(SolveCache* sc) {
-    for (double* p : {sc->inv, sc->B, sc->W, sc->Z, sc->R, sc->Y, sc->X}) cudaFree(p);
-    cudaFree(sc->rows);
+    for (double* p : {sc->inv, sc->B, sc->W, sc->Z, sc->R, sc->Y, sc->X, sc->Xg}) cudaFree(p);
+    for (int* p : {sc->rows, sc->rows_id, sc->cols, sc->unperm}) cudaFree(p);
     *sc = SolveCache{};
 }
 
-int solve_cache_grow(SolveCache* sc, const SolveFactor& f, int ldn, bool work, bool col_partials) {
-    if (ldn <= sc->ldn) return CFLX_OK;
-    for (double** p : {&sc->B, &sc->W, &sc->Z, &sc->R, &sc->Y, &sc->X}) {
+int solve_cache_grow(SolveCache* sc, const SolveFactor& f, int ldn, bool work, bool col_partials, bool col_seed) {
+    if (ldn <= sc->ldn && (sc->col_partials || !col_partials) && (sc->col_seed || !col_seed)) return CFLX_OK;
+    ldn = std::max(ldn, sc->ldn);
+    sc->col_partials |= col_partials;
+    sc->col_seed |= col_seed;
+    for (double** p : {&sc->B, &sc->W, &sc->Z, &sc->R, &sc->Y, &sc->X, &sc->Xg}) {
         cudaFree(*p);
         *p = nullptr;
     }
     sc->ldn = 0;
     const size_t M = f.M, v = f.v;
-    if (f.pk == 0 && f.pj == 0) CFLX_TRY(dmalloc(&sc->B, M * ldn));
+    if (f.pk == 0 && (f.pj == 0 || (sc->col_seed && f.pi == 0))) CFLX_TRY(dmalloc(&sc->B, M * ldn));
     if (work) {
         CFLX_TRY(dmalloc(&sc->W, (size_t)f.Ml * ldn));
-        if (col_partials) CFLX_TRY(dmalloc(&sc->Z, (size_t)f.Nl * ldn));
+        if (sc->col_partials) CFLX_TRY(dmalloc(&sc->Z, (size_t)f.Nl * ldn));
         CFLX_TRY(dmalloc(&sc->R, v * ldn));
         CFLX_TRY(dmalloc(&sc->Y, v * ldn));
     }
     CFLX_TRY(dmalloc(&sc->X, M * ldn));
+    if (sc->col_seed) CFLX_TRY(dmalloc(&sc->Xg, M * ldn));
     sc->ldn = ldn;
     return CFLX_OK;
 }
@@ -432,23 +448,24 @@ int solve_inverses(SolveCache* sc, const SolveFactor& f, bool lower) {
     return rc;
 }
 
-int solve_set_rows(SolveCache* sc, const std::vector<int>& rows, cudaStream_t s) {
-    if (!sc->rows) CFLX_TRY(dmalloc(&sc->rows, rows.size()));
-    CFLX_CUDA(cudaMemcpyAsync(sc->rows, rows.data(), sizeof(int) * rows.size(), cudaMemcpyHostToDevice, s));
+int solve_set_rows(int** dst, const std::vector<int>& rows, cudaStream_t s) {
+    if (!*dst) CFLX_TRY(dmalloc(dst, rows.size()));
+    CFLX_CUDA(cudaMemcpyAsync(*dst, rows.data(), sizeof(int) * rows.size(), cudaMemcpyHostToDevice, s));
     CFLX_CUDA(cudaStreamSynchronize(s));  // `rows` is a host temporary
     return CFLX_OK;
 }
 
-int solve_seed(SolveCache* sc, const SolveFactor& f, int ldn, int nrhs, const double* B, int ldb) {
+int solve_seed(SolveCache* sc, const SolveFactor& f, int ldn, int nrhs, const double* B, int ldb, const SolveSeed& at) {
     cudaStream_t s = f.comm->stream;
     CFLX_CUDA(cudaMemsetAsync(sc->X, 0, sizeof(double) * f.M * ldn, s));
     if (sc->W) CFLX_CUDA(cudaMemsetAsync(sc->W, 0, sizeof(double) * f.Ml * ldn, s));
     if (sc->Z) CFLX_CUDA(cudaMemsetAsync(sc->Z, 0, sizeof(double) * f.Nl * ldn, s));
-    if (sc->B && f.rows > 0) {
+    const bool holds = f.pk == 0 && (at.by_col ? f.pi : f.pj) == 0;
+    if (holds && at.n > 0) {
         CFLX_CUDA(cudaMemsetAsync(sc->B, 0, sizeof(double) * f.M * ldn, s));
         CFLX_CUDA(cudaMemcpy2DAsync(sc->B, ldn * sizeof(double), B, (size_t)ldb * sizeof(double), nrhs * sizeof(double), f.M,
                                     cudaMemcpyHostToDevice, s));
-        CFLX_TRY(launch_gather_rows(sc->B, ldn, sc->rows, f.rows, ldn, sc->W, s));
+        CFLX_TRY(launch_gather_rows(sc->B, ldn, at.rows, at.n, ldn, at.dst, s));
     }
     return CFLX_OK;
 }
@@ -487,41 +504,132 @@ int solve_row_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward,
     return CFLX_OK;
 }
 
-int solve_col_sweep(SolveCache* sc, const SolveFactor& f, int ldn) {
+int solve_col_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward, Tri tri, double* keep, int keep_div,
+                    bool clear_col) {
     cudaStream_t s = f.comm->stream;
     const int v = f.v, Px = f.Px, Py = f.Py, Nl = f.Nl;
+    const bool layer0 = f.pk == 0;
     const size_t tile = (size_t)v * ldn;
-    for (int t = f.Nt - 1; t >= 0; --t) {
-        const bool in_row = f.pi == t % Px, in_col = f.pj == t % Py, owner = in_row && in_col;
-        double* R = sc->Z + (int64_t)(t / Py) * tile;  // tile t's columns of Z, summed over the grid column onto the owner
+    for (int i = 0; i < f.Nt; ++i) {
+        const int t = forward ? i : f.Nt - 1 - i;
+        const bool in_row = f.pi == t % Px, in_col = f.pj == t % Py, owner = layer0 && in_row && in_col;
+        double* const Zt = sc->Z + (int64_t)(t / Py) * tile;
+        double* R = Zt;  // tile t's columns of Z, summed over the grid column onto the owner
         if (in_col && Px * f.stride > 1) {
-            CFLX_NCCL(ncclReduce(R, sc->R, tile, ncclDouble, ncclSum, (t % Px) * f.stride, f.col_comm->c, s));
+            CFLX_NCCL(ncclReduce(Zt, sc->R, tile, ncclDouble, ncclSum, (t % Px) * f.stride, f.col_comm->c, s));
             R = sc->R;
         }
         if (owner) {
-            CFLX_TRY(diag_solve(*sc, f, t, Tri::LowerT, R, ldn, s));
-            CFLX_CUDA(cudaMemcpyAsync(sc->X + (int64_t)t * tile, sc->Y, tile * sizeof(double), cudaMemcpyDeviceToDevice, s));
+            CFLX_TRY(diag_solve(*sc, f, t, tri, R, ldn, s));
+            CFLX_CUDA(cudaMemcpyAsync(keep + (int64_t)(t / keep_div) * tile, sc->Y, tile * sizeof(double),
+                                      cudaMemcpyDeviceToDevice, s));
+        } else if (clear_col && in_col && layer0) {
+            CFLX_CUDA(cudaMemsetAsync(Zt, 0, tile * sizeof(double), s));
         }
         if (!in_row) continue;
         if (Py * f.stride > 1)
             CFLX_NCCL(ncclBroadcast(sc->Y, sc->Y, tile, ncclDouble, (t % Py) * f.stride, f.row_comm->c, s));
-        const int m = first_local_tile(t, f.pj, Py) * v;  // local columns with gj < t: a prefix of the tile row
-        if (m > 0)  // Z[columns gj < t] -= L[t, gj]^T X_t
-            CFLX_TRY(launch_gemm_narrow_tn(m, ldn, v, f.F + (int64_t)(t / Px) * v * Nl, Nl, sc->Y, ldn, sc->Z, ldn, sc->Z,
-                                           ldn, -1.0, 1.0, s));
+        if (!layer0) continue;
+        const double* Ft = f.F + (int64_t)(t / Px) * v * Nl;  // local tile row t / Px
+        if (forward) {  // Z[columns gj > t] -= U[t, gj]^T Y_t: a suffix of the tile row
+            const int lo = first_local_tile(t + 1, f.pj, Py) * v;
+            if (lo < Nl)
+                CFLX_TRY(launch_gemm_narrow_tn(Nl - lo, ldn, v, Ft + lo, Nl, sc->Y, ldn, sc->Z + (int64_t)lo * ldn, ldn,
+                                               sc->Z + (int64_t)lo * ldn, ldn, -1.0, 1.0, s));
+        } else {
+            const int m = first_local_tile(t, f.pj, Py) * v;  // local columns with gj < t: a prefix of the tile row
+            if (m > 0)  // Z[columns gj < t] -= L[t, gj]^T X_t
+                CFLX_TRY(launch_gemm_narrow_tn(m, ldn, v, Ft, Nl, sc->Y, ldn, sc->Z, ldn, sc->Z, ldn, -1.0, 1.0, s));
+        }
     }
     return CFLX_OK;
 }
 
-int solve_finish(SolveCache* sc, const SolveFactor& f, int ldn, int nrhs, double* X, int ldx) {
+int solve_finish(SolveCache* sc, const SolveFactor& f, int ldn, int nrhs, double* X, int ldx, const int* unperm) {
     cudaStream_t s = f.comm->stream;
     // exactly one rank contributes each element: the sum is X itself, bit for bit, on every rank
     if (f.P > 1) CFLX_NCCL(ncclAllReduce(sc->X, sc->X, (size_t)f.M * ldn, ncclDouble, ncclSum, f.comm->world, s));
+    const double* out = sc->X;
+    if (unperm) {
+        CFLX_TRY(launch_gather_rows(sc->X, ldn, unperm, f.M, ldn, sc->Xg, s));
+        out = sc->Xg;
+    }
     if (X)
-        CFLX_CUDA(cudaMemcpy2DAsync(X, (size_t)ldx * sizeof(double), sc->X, ldn * sizeof(double), nrhs * sizeof(double), f.M,
+        CFLX_CUDA(cudaMemcpy2DAsync(X, (size_t)ldx * sizeof(double), out, ldn * sizeof(double), nrhs * sizeof(double), f.M,
                                     cudaMemcpyDeviceToHost, s));
     CFLX_CUDA(cudaStreamSynchronize(s));
     return CFLX_OK;
+}
+
+// ---------------------------------------------------------------- the 1-norm condition estimate
+// LAPACK's dlacn2 (Higham, ACM TOMS 14 (1988) 381-396, Algorithm 4.1 with the safeguards of dlacn2), with its reverse
+// communication unrolled: kase 1 asks for inv(A) x, kase 2 for inv(A)^T x.  The sign vector is +1 for x >= 0 (so -0 and
+// NaN are told apart exactly as LAPACK does), idamax takes the first index of the largest |x|, and the sums of |x| run in
+// index order.
+int estimate_inv_norm1(int n, const std::function<int(int, double*)>& apply, double* est_out) {
+    constexpr int ITMAX = 5;
+    std::vector<double> x(n, 1.0 / n), v(n);
+    std::vector<int> isgn(n);
+    auto asum = [&](const std::vector<double>& a) {
+        double s = 0.0;
+        for (double e : a) s += std::fabs(e);
+        return s;
+    };
+    auto idamax = [&]() {
+        int j = 0;
+        double m = std::fabs(x[0]);
+        for (int i = 1; i < n; ++i)
+            if (std::fabs(x[i]) > m) m = std::fabs(x[i]), j = i;
+        return j;
+    };
+    auto signs = [&]() {
+        for (int i = 0; i < n; ++i) {
+            x[i] = x[i] >= 0.0 ? 1.0 : -1.0;
+            isgn[i] = (int)x[i];
+        }
+    };
+    double est = 0.0;
+    CFLX_TRY(apply(1, x.data()));
+    if (n == 1) {
+        *est_out = std::fabs(x[0]);
+        return CFLX_OK;
+    }
+    est = asum(x);
+    signs();
+    CFLX_TRY(apply(2, x.data()));
+    int j = idamax();
+    for (int iter = 2;; ++iter) {
+        std::fill(x.begin(), x.end(), 0.0);
+        x[j] = 1.0;
+        CFLX_TRY(apply(1, x.data()));
+        v = x;
+        const double estold = est;
+        est = asum(v);
+        bool repeated = true;
+        for (int i = 0; i < n && repeated; ++i) repeated = (x[i] >= 0.0 ? 1 : -1) == isgn[i];
+        if (repeated || est <= estold) break;  // converged, or cycling
+        signs();
+        CFLX_TRY(apply(2, x.data()));
+        const int jlast = j;
+        j = idamax();
+        if (!(x[jlast] != std::fabs(x[j]) && iter < ITMAX)) break;
+    }
+    double altsgn = 1.0;  // the final stage: x_i = (-1)^i (1 + i / (n - 1))
+    for (int i = 0; i < n; ++i) {
+        x[i] = altsgn * (1.0 + (double)i / (double)(n - 1));
+        altsgn = -altsgn;
+    }
+    CFLX_TRY(apply(1, x.data()));
+    const double temp = 2.0 * (asum(x) / (double)(3 * n));
+    if (temp > est) est = temp;
+    *est_out = est;
+    return CFLX_OK;
+}
+
+double rcond_from(double anorm, double ainvnm) {
+    if (!(anorm > 0.0) || !(ainvnm > 0.0) || !std::isfinite(ainvnm)) return 0.0;
+    const double r = (1.0 / ainvnm) / anorm;
+    return std::isfinite(r) ? r : 0.0;
 }
 
 }  // namespace cflx

@@ -91,5 +91,15 @@ inline void choleskySolve(int nrhs, const double* B, int ldb, double* X, int ldx
     if (!s.plan) throw CholeskyException("choleskySolve() before initialize()");
     chol_detail::check(cflx_chol_solve(s.plan, nrhs, B, ldb, X, ldx), "choleskySolve");
 }
+// LAPACK dpocon of the last parallelCholesky() (cflx_chol_rcond, collective).  Returns the estimate of
+// 1 / (||A||_1 ||A^-1||_1); *anorm = ||A||_1 of the padded symmetric input.
+inline double choleskyRcond(double* anorm = nullptr) {
+    auto& s = chol_detail::state();
+    if (!s.plan) throw CholeskyException("choleskyRcond() before initialize()");
+    double r = 0, a = 0;
+    chol_detail::check(cflx_chol_rcond(s.plan, &r, &a), "choleskyRcond");
+    if (anorm) *anorm = a;
+    return r;
+}
 
 }  // namespace conflux

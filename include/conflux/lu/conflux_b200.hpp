@@ -254,11 +254,23 @@ double validate(lu_params<T>& gv, double* relative = nullptr) {
     return a;
 }
 
-// Solves A X = B with the factors of the last LU_rep (P A = L U), on the GPU grid, like LAPACK's getrs.  Collective.
-// B / X: M x nrhs row-major (M = gv.M, the padded size), ldb / ldx >= nrhs; B the same on every rank, X may be null.
+// Solves A X = B (A^T X = B when transposed) with the factors of the last LU_rep (P A = L U), on the GPU grid, like
+// LAPACK's getrs.  Collective.  B / X: M x nrhs row-major (M = gv.M, the padded size), ldb / ldx >= nrhs; B the same on
+// every rank, X may be null.
 template <class T>
-void LU_solve(lu_params<T>& gv, int nrhs, const T* B, int ldb, T* X, int ldx) {
-    check(cflx_lu_solve(gv.plan, nrhs, B, ldb, X, ldx), "LU_solve");
+void LU_solve(lu_params<T>& gv, int nrhs, const T* B, int ldb, T* X, int ldx, bool transposed = false) {
+    if (transposed) check(cflx_lu_solve_trans(gv.plan, nrhs, B, ldb, X, ldx), "LU_solve");
+    else check(cflx_lu_solve(gv.plan, nrhs, B, ldb, X, ldx), "LU_solve");
+}
+
+// LAPACK dgecon (1-norm) of the last LU_rep on the GPU grid.  Collective.  Returns the estimate of 1 / (||A||_1 ||A^-1||_1)
+// (0 for an exactly singular U); *anorm = ||A||_1 of the padded input.
+template <class T>
+double LU_rcond(lu_params<T>& gv, double* anorm = nullptr) {
+    double r = 0, a = 0;
+    check(cflx_lu_rcond(gv.plan, &r, &a), "LU_rcond");
+    if (anorm) *anorm = a;
+    return r;
 }
 
 }  // namespace conflux

@@ -101,6 +101,16 @@ int cflx_lu_residual(cflx_lu*, double* rel_out);
  * The first call after a factorisation prepares and caches per-rank solve data; cflx_lu_set_local / cflx_lu_factor
  * drop it.  Does not modify the factors or the input.  No singularity check (like getrs). */
 int cflx_lu_solve(cflx_lu*, int nrhs, const double* B, int ldb, double* X, int ldx);
+/* COLLECTIVE.  Solves A^T X = B with the factors of the last cflx_lu_factor, on the GPU grid, like LAPACK's getrs with
+ * TRANS = 'T'.  Arguments, state rules and caching as cflx_lu_solve. */
+int cflx_lu_solve_trans(cflx_lu*, int nrhs, const double* B, int ldb, double* X, int ldx);
+/* COLLECTIVE.  LAPACK dgecon (NORM = '1') on the GPU grid: rcond_out = 1 / (||A||_1 ||inv(A)||_1) with ||inv(A)||_1
+ * estimated by Hager-Higham's method (dlacn2: at most 5 iterations, a few solves with one right-hand side), anorm_out
+ * (may be NULL) = ||A||_1 of the padded M x M input.  rcond is 0 when ||A||_1 is 0 or the estimate is not finite (an
+ * exactly singular U), with CFLX_OK.  Identical on every rank.  CFLX_ERR_STATE as cflx_lu_solve, and when the input
+ * buffer of the last run was handed to the queued next matrix.  Leaves the factors, the permutation and any later solve
+ * as they are. */
+int cflx_lu_rcond(cflx_lu*, double* rcond_out, double* anorm_out);
 /* 1 when this plan's trailing update runs on the int8 wgmma digit-plane path (ozaki.cu), 0 for the FP64 DMMA kernel
  * (gemm.cu) */
 int cflx_lu_uses_ozaki(const cflx_lu*);
@@ -155,6 +165,10 @@ int cflx_chol_validate(cflx_chol*, double* frob_abs_out, double* frob_rel_out);
  * after a factorisation prepares and caches per-rank solve data; cflx_chol_set_local / cflx_chol_factor drop it.  Does not
  * modify the factor or the input. */
 int cflx_chol_solve(cflx_chol*, int nrhs, const double* B, int ldb, double* X, int ldx);
+/* COLLECTIVE.  LAPACK dpocon on the GPU grid: rcond_out = 1 / (||A||_1 ||inv(A)||_1), ||A||_1 of the symmetric input
+ * whose lower triangle is stored (anorm_out, may be NULL), ||inv(A)||_1 estimated by Hager-Higham's method with solves.
+ * Identical on every rank.  CFLX_ERR_STATE as cflx_chol_solve.  Leaves the factor and any later solve as they are. */
+int cflx_chol_rcond(cflx_chol*, double* rcond_out, double* anorm_out);
 /* number of kernels this object counted since the last reset (bench.py's gpu_launches); cflx_chol_solve adds none */
 int cflx_chol_launch_count(cflx_chol*, int64_t* count_out, int reset);
 void cflx_chol_destroy(cflx_chol*);
