@@ -15,7 +15,7 @@ import numpy as np
 
 from ._lib import ConfluxError, LIB_PATH, SYMBOLS, check, lib
 
-__all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "residual", "validate", "lu_solve", "lu_rcond", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
+__all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "residual", "validate", "lu_solve", "lu_rcond", "lu_refine", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
 
 
 def auto_grid(M, N, P):
@@ -224,6 +224,31 @@ def lu_rcond(gv):
     return r.value, a.value
 
 
+def _refine_args(n, B, X, what):
+    B = np.asarray(B, dtype=np.float64)
+    X = np.asarray(X, dtype=np.float64)
+    if B.ndim not in (1, 2) or B.shape[0] != n:
+        raise ValueError(f"{what}: B must have shape ({n},) or ({n}, nrhs), got {B.shape}")
+    if X.shape != B.shape:
+        raise ValueError(f"{what}: X must have the shape of B, {B.shape}, got {X.shape}")
+    B2 = np.ascontiguousarray(B.reshape(n, -1))
+    X2 = np.array(X.reshape(n, -1), dtype=np.float64, order="C")
+    nrhs = B2.shape[1]
+    return B.shape, B2, X2, nrhs, np.empty(nrhs), np.empty(nrhs)
+
+
+def lu_refine(gv, B, X, trans=False, ferr=True):
+    """LAPACK dgerfs with the factors of the last LU_rep on the GPU grid: refines X, a solution of A X = B (A^T X = B when
+    trans), e.g. from lu_solve, and returns (X, ferr, berr) -- the refined X in B's shape, and per right-hand side the
+    estimated forward error bound ||x - x_true||_inf / ||x||_inf and the componentwise backward error.  ferr=False skips
+    the estimator (ferr is then None).  COLLECTIVE over gv.lu_comm; every rank passes the same B and X and gets the same
+    results.  The factors, the input and later solves are left as they are."""
+    shape, B2, X2, nrhs, fe, be = _refine_args(gv.M, B, X, "lu_refine")
+    check(lib().cflx_lu_refine(gv._h, 1 if trans else 0, nrhs, B2.ctypes.data, nrhs, X2.ctypes.data, nrhs,
+                               fe.ctypes.data if ferr else None, be.ctypes.data), "lu_refine")
+    return X2.reshape(shape), (fe if ferr else None), be
+
+
 class cholesky:
     """Mirror of the reference's CONFCHOX driver interface (src/conflux/cholesky/Cholesky.h:20-22):
         initialize(N, v, grid, comm) -> object;  obj.parallelCholesky() -> ms;  obj.finalize().
@@ -287,6 +312,14 @@ class cholesky:
         r, a = ctypes.c_double(), ctypes.c_double()
         check(lib().cflx_chol_rcond(self._h, ctypes.byref(r), ctypes.byref(a)), "chol_rcond")
         return r.value, a.value
+
+    def refine(self, B, X, ferr=True):
+        """LAPACK dporfs with the factor of the last parallelCholesky on the GPU grid: refines X, a solution of A X = B (e.g.
+        from solve), and returns (X, ferr, berr) as lu_refine does.  COLLECTIVE; identical on every rank."""
+        shape, B2, X2, nrhs, fe, be = _refine_args(self.N, B, X, "cholesky.refine")
+        check(lib().cflx_chol_refine(self._h, nrhs, B2.ctypes.data, nrhs, X2.ctypes.data, nrhs,
+                                     fe.ctypes.data if ferr else None, be.ctypes.data), "chol_refine")
+        return X2.reshape(shape), (fe if ferr else None), be
 
     def finalize(self, clean=True):
         if self._h:
@@ -371,6 +404,28 @@ class dbg:
         check(lib().cflx_dbg_gemm_narrow_tn(M, N, K, AT.ctypes.data, B.ctypes.data, Cp, float(alpha), float(beta),
                                             D.ctypes.data, int(reps), ctypes.byref(ms)), "dbg_gemm_narrow_tn")
         return D, ms.value
+
+    @staticmethod
+    def residual(A, mode, v, Kappa=None, grid=(1, 1), pos=(0, 0), Xc=None, Xr=None, reps=1):
+        """The residual kernels of lu_refine / cholesky.refine on one layer-0 share A (Ml x Nl, conflux layout of tile v at
+        grid position pos of grid = (Px, Py)).  mode "nn": P = A @ Xc, Q = |A| @ |Xc| (Xc: Nl x nrhs, X by local column);
+        "tn": P = A.T @ Xr, Q = |A|.T @ |Xr| (Xr: Ml x nrhs, X by local row); "sym": the stored lower triangle of the real
+        tiles (global tile index < Kappa), rows [0, Ml) the NN product over global row >= column and rows [Ml, Ml + Nl)
+        the TN product over global row > column.  Returns (P, Q, mean ms of one launch)."""
+        A = np.ascontiguousarray(A, dtype=np.float64)
+        Ml, Nl = A.shape
+        m = {"nn": 0, "tn": 1, "sym": 2}[mode]
+        cvt = lambda X: None if X is None else np.ascontiguousarray(np.asarray(X, dtype=np.float64).reshape(X.shape[0], -1))
+        Xc, Xr = cvt(Xc), cvt(Xr)
+        nrhs = (Xc if Xc is not None else Xr).shape[1]
+        rows = (Ml, Nl, Ml + Nl)[m]
+        P, Q = np.empty((rows, nrhs)), np.empty((rows, nrhs))
+        ms = ctypes.c_double()
+        ptr = lambda a: a.ctypes.data if a is not None else None
+        check(lib().cflx_dbg_residual(m, Ml, Nl, A.ctypes.data, int(v), int(Kappa if Kappa is not None else 1 << 30),
+                                      int(grid[0]), int(grid[1]), int(pos[0]), int(pos[1]), nrhs, ptr(Xc), ptr(Xr),
+                                      P.ctypes.data, Q.ctypes.data, int(reps), ctypes.byref(ms)), "dbg_residual")
+        return P, Q, ms.value
 
     @staticmethod
     def panel(P, reps=1):

@@ -1008,6 +1008,22 @@ int cflx_chol_rcond(cflx_chol* ch, double* rcond_out, double* anorm_out) {
     return CFLX_OK;
 }
 
+// COLLECTIVE.  LAPACK dporfs (UPLO = 'L') on the grid: residuals of the symmetric input from its stored lower triangle
+// (refine.cu), corrections and both kinds of estimator product by cflx_chol_solve's sweeps.
+int cflx_chol_refine(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X, int ldx, double* ferr_out,
+                     double* berr_out) {
+    if (!ch || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B || !X) return CFLX_ERR_ARG;
+    if (!ch->factored) {
+        set_last_error("cholesky refinement requested before a successful cflx_chol_factor, or after cflx_chol_set_local without one");
+        return CFLX_ERR_STATE;
+    }
+    CFLX_CUDA(cudaSetDevice(ch->comm->device));
+    auto solve = [ch](bool, int n, const double* b, int lb, double* x, int lx) { return cflx_chol_solve(ch, n, b, lb, x, lx); };
+    const RefineOp op{ch->comm, ch->A0, ResidMode::SymLower, ch->N, ch->Ml, ch->Nl, ch->v, ch->Kappa, ch->Px, ch->Py,
+                      ch->Pz, ch->pi, ch->pj, ch->pk, true, solve};
+    return refine_run(&ch->sv.rf, op, nrhs, B, ldb, X, ldx, ferr_out, berr_out);
+}
+
 int cflx_chol_launch_count(cflx_chol* ch, int64_t* count_out, int reset) {
     if (!ch || !count_out) return CFLX_ERR_ARG;
     *count_out = ch->launches;

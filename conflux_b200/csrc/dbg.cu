@@ -1,6 +1,7 @@
 // conflux_b200/csrc/dbg.cu -- single-device test / micro-benchmark hooks of the C ABI (cflx_dbg_*).
 // They drive the SAME kernels the factorisation uses, with host buffers in and out, so that tests/ can check every
 // kernel in isolation against numpy / the oracle, and bench.py can time the dominant kernel alone.
+#include <algorithm>
 #include <vector>
 
 #include "../../include/conflux_b200.h"
@@ -270,6 +271,53 @@ int cflx_dbg_gemm_narrow_tn(int M, int N, int K, const double* AT, const double*
     double* out = alias ? dC.as<double>() : dT.as<double>();
     CFLX_TRY(run(out));
     if (D) CFLX_CUDA(cudaMemcpy(D, out, sizeof(double) * c_n, cudaMemcpyDeviceToHost));
+    CFLX_CUDA(cudaDeviceSynchronize());
+    return CFLX_OK;
+}
+
+// the residual kernels of the refinement (refine.cu) on one layer-0 share; the timed repetitions run first, then the
+// launch whose result is returned
+int cflx_dbg_residual(int mode, int Ml, int Nl, const double* A, int v, int Kappa, int Px, int Py, int pi, int pj,
+                      int nrhs, const double* Xc, const double* Xr, double* P_out, double* Q_out, int reps, double* ms_out) {
+    CFLX_TRY(check_device());
+    if (mode < 0 || mode > 2 || Ml < 0 || Nl < 0 || (Nl & 1) || v < 4 || (v & 3) || nrhs < 1 || !A || Px < 1 || Py < 1 ||
+        pi < 0 || pi >= Px || pj < 0 || pj >= Py || (mode != 1 && !Xc) || (mode != 0 && !Xr))
+        return CFLX_ERR_ARG;
+    const ResidMode m = mode == 0 ? ResidMode::NN : mode == 1 ? ResidMode::TN : ResidMode::SymLower;
+    const int rows = mode == 0 ? Ml : mode == 1 ? Nl : Ml + Nl;
+    const size_t a_n = (size_t)Ml * Nl, o_n = (size_t)std::max(rows, 1) * nrhs;
+    DevBuf dA, dXc, dXr, dP, dQ;
+    CFLX_TRY(dA.alloc(sizeof(double) * a_n));
+    CFLX_TRY(dXc.alloc(sizeof(double) * (size_t)Nl * nrhs));
+    CFLX_TRY(dXr.alloc(sizeof(double) * (size_t)Ml * nrhs));
+    CFLX_TRY(dP.alloc(sizeof(double) * o_n));
+    CFLX_TRY(dQ.alloc(sizeof(double) * o_n));
+    CFLX_CUDA(cudaMemcpy(dA.p, A, sizeof(double) * a_n, cudaMemcpyHostToDevice));
+    if (Xc) CFLX_CUDA(cudaMemcpy(dXc.p, Xc, sizeof(double) * (size_t)Nl * nrhs, cudaMemcpyHostToDevice));
+    if (Xr) CFLX_CUDA(cudaMemcpy(dXr.p, Xr, sizeof(double) * (size_t)Ml * nrhs, cudaMemcpyHostToDevice));
+    auto run = [&]() {
+        return launch_residual(m, dA.as<double>(), Nl, Ml, Nl, v, Kappa, Px, Py, pi, pj, dXc.as<double>(), dXr.as<double>(),
+                               nrhs, nrhs, dP.as<double>(), dQ.as<double>(), nrhs, 0);
+    };
+    cudaEvent_t e0, e1;
+    CFLX_CUDA(cudaEventCreate(&e0));
+    CFLX_CUDA(cudaEventCreate(&e1));
+    if (reps < 1) reps = 1;
+    CFLX_TRY(run());  // warm-up
+    CFLX_CUDA(cudaEventRecord(e0));
+    for (int r = 0; r < reps; ++r) CFLX_TRY(run());
+    CFLX_CUDA(cudaEventRecord(e1));
+    CFLX_CUDA(cudaEventSynchronize(e1));
+    float ms = 0;
+    CFLX_CUDA(cudaEventElapsedTime(&ms, e0, e1));
+    if (ms_out) *ms_out = ms / reps;
+    cudaEventDestroy(e0);
+    cudaEventDestroy(e1);
+    CFLX_CUDA(cudaMemset(dP.p, 0, sizeof(double) * o_n));
+    CFLX_CUDA(cudaMemset(dQ.p, 0, sizeof(double) * o_n));
+    CFLX_TRY(run());
+    if (P_out) CFLX_CUDA(cudaMemcpy(P_out, dP.p, sizeof(double) * (size_t)rows * nrhs, cudaMemcpyDeviceToHost));
+    if (Q_out) CFLX_CUDA(cudaMemcpy(Q_out, dQ.p, sizeof(double) * (size_t)rows * nrhs, cudaMemcpyDeviceToHost));
     CFLX_CUDA(cudaDeviceSynchronize());
     return CFLX_OK;
 }

@@ -1118,6 +1118,30 @@ int cflx_lu_rcond(cflx_lu* lu, double* rcond_out, double* anorm_out) {
     return CFLX_OK;
 }
 
+// COLLECTIVE.  LAPACK dgerfs on the grid: residuals of the input A0 (refine.cu), corrections and the forward-error
+// estimator's products by the solves above.  For trans = 0 the estimator's kase 1 (inv(A)^T) is the transposed solve and
+// kase 2 the plain one; for trans = 1 they swap.
+int cflx_lu_refine(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, double* X, int ldx, double* ferr_out,
+                   double* berr_out) {
+    if (!lu || (trans != 0 && trans != 1) || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B || !X) return CFLX_ERR_ARG;
+    if (!lu->factored) {
+        set_last_error("refinement requested before cflx_lu_factor, or after cflx_lu_set_local without a factorisation");
+        return CFLX_ERR_STATE;
+    }
+    if (lu->a0_is_next) {
+        set_last_error("refinement refused: the input buffer of the last run was handed to the queued next matrix");
+        return CFLX_ERR_STATE;
+    }
+    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    const bool t = trans != 0;
+    auto solve = [lu, t](bool tk, int n, const double* b, int lb, double* x, int lx) {
+        return lu_sweeps(lu, t != tk, false, n, b, lb, x, lx);
+    };
+    const RefineOp op{lu->comm, lu->A0, t ? ResidMode::TN : ResidMode::NN, lu->M, lu->Ml, lu->Nl, lu->v, lu->Nt, lu->Px,
+                      lu->Py, lu->Pz, lu->pi, lu->pj, lu->pk, false, solve};
+    return refine_run(&lu->sv.rf, op, nrhs, B, ldb, X, ldx, ferr_out, berr_out);
+}
+
 int cflx_host_alloc(size_t bytes, void** out) {
     if (!out) return CFLX_ERR_ARG;
     int n = 0;

@@ -68,6 +68,17 @@ int grid_barrier(cflx_comm* c);
 inline int first_local_tile(int g, int p, int P) { return g <= p ? 0 : (g - p + P - 1) / P; }
 
 // ---------------------------------------------------------------- the solve engine (solve.cu)
+// ---------------------------------------------------------------- iterative refinement (refine.cu)
+// Device buffers of cflx_lu_refine / cflx_chol_refine, grown and never shrunk, freed with the solve cache.  gl_cols /
+// gl_rows: the row of X that each local column / row of the layer-0 share multiplies (made on first use; the layout does
+// not change with the matrix).
+struct RefineCache {
+    int *gl_rows = nullptr, *gl_cols = nullptr, *active = nullptr;
+    double *X = nullptr, *B = nullptr, *R = nullptr, *D = nullptr, *rhs = nullptr, *ratio = nullptr, *W = nullptr;
+    double *Xc = nullptr, *Xr = nullptr, *part = nullptr, *all = nullptr, *berr = nullptr;
+    size_t cap_m = 0, cap_c = 0, cap_r = 0, cap_part = 0, cap_all = 0, cap_berr = 0, cap_active = 0;
+};
+
 // What a solve keeps between calls: prepared by the first solve after a factorisation, dropped (ready = false) by
 // set_local / factor, freed with the object.  The work buffers have ldn columns and are grown, never shrunk.
 struct SolveCache {
@@ -83,6 +94,7 @@ struct SolveCache {
     double *B = nullptr, *W = nullptr, *Z = nullptr, *R = nullptr, *Y = nullptr, *X = nullptr, *Xg = nullptr;
     int ldn = 0;
     bool col_partials = false, col_seed = false;  // what the buffers were grown for (kept across growth)
+    RefineCache rf;
 };
 
 // The triangle a diagonal-tile solve applies, and how (solve.cu diag_solve):
@@ -173,7 +185,7 @@ int solve_cache_grow(SolveCache* sc, const SolveFactor& f, int ldn, bool work, b
 int solve_inverses(SolveCache* sc, const SolveFactor& f, bool lower);
 // *dst = rows (allocated on first use), waited for
 int solve_set_rows(int** dst, const std::vector<int>& rows, cudaStream_t s);
-// zero X, W and Z, and on the ranks holding B (`at`): at.dst[r] = B[at.rows[r]] for r < at.n
+// zero X, W and Z, and on the ranks holding B (`at`): at.dst[r] = B[at.rows[r]] for r < at.n; B is a host or device array
 int solve_seed(SolveCache* sc, const SolveFactor& f, int ldn, int nrhs, const double* B, int ldb, const SolveSeed& at);
 // row-partial sweep over the tile diagonal: forward with the lower triangle (NN), backward with the upper one (NN).  The
 // diagonal owner keeps each solved tile t at tile t / keep_div of `keep`; with clear_row, keep is W and the other layer-0
@@ -186,7 +198,8 @@ int solve_row_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward,
 // other layer-0 ranks of the grid column zero their copy of that tile.  Ranks pk != 0 join the collectives only.
 int solve_col_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward, Tri tri, double* keep, int keep_div,
                     bool clear_col);
-// X (nrhs columns, ldx) = the world sum of the owners' tiles of sc->X, downloaded when X is not null; synchronises.
+// X (nrhs columns, ldx; host or device) = the world sum of the owners' tiles of sc->X, copied when X is not null;
+// synchronises.
 // unperm (M rows, every rank): row i of X is row unperm[i] of that sum.
 int solve_finish(SolveCache* sc, const SolveFactor& f, int ldn, int nrhs, double* X, int ldx, const int* unperm = nullptr);
 // Hager-Higham estimate of ||inv(A)||_1 for an order-n A, as LAPACK's dlacn2 runs it (x = 1/n, at most 5 iterations,
@@ -201,4 +214,36 @@ int norm1_grid(cflx_comm* c, const double* A, int M, int Ml, int Nl, int v, int 
                int pk, bool lower_sym, double* anorm);
 // rcond = (1 / ainvnm) / anorm as LAPACK's dgecon / dpocon form it; 0 when anorm is 0 or the estimate is not finite
 double rcond_from(double anorm, double ainvnm);
+
+// LAPACK's dlacn2 as a reverse-communication step (Higham, ACM TOMS 14 (1988) 381-396, Algorithm 4.1 with dlacn2's
+// safeguards): start(n) sets x = 1/n and kase = 1; the caller overwrites x with A x (kase 1) or A^T x (kase 2) and calls
+// step(), which sets the next x and kase, until kase == 0 and est is the estimate of ||A||_1.  The sign vector is +1 for
+// x >= 0, idamax takes the first index of the largest |x|, and the sums of |x| run in index order.  Pure host logic:
+// callers that pass bit-identical vectors take the same steps.
+struct Lacn2 {
+    int n = 0, kase = 0, jump = 0, j = 0, iter = 0;
+    double est = 0.0;
+    bool pending = false;  // a product was written into x and step() has not taken it yet (refine_run's bookkeeping)
+    std::vector<double> x, v;
+    std::vector<int> isgn;
+    void start(int n);
+    int step();
+};
+
+// What refine_run needs of a factorisation: the input's layer-0 share and its layout, and the solves.
+// solve(transposed, nrhs, B, ldb, X, ldx) overwrites X with inv(op A) B (transposed: inv(op A)^T B); B and X are host or
+// device arrays of M rows; it synchronises the stream.  symmetric: both kinds are the same solve.
+struct RefineOp {
+    cflx_comm* comm;
+    const double* A;
+    ResidMode mode;
+    int M, Ml, Nl, v, Kappa, Px, Py, Pz, pi, pj, pk;
+    bool symmetric;
+    std::function<int(bool, int, const double*, int, double*, int)> solve;
+};
+// LAPACK dgerfs / dporfs on the grid (collective): X (host, M x nrhs, ldx) refined in place, ferr (may be null: no
+// estimator) and berr (may be null) per column.  Every column runs LAPACK's own decisions, all in lockstep.
+int refine_run(RefineCache* rc, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx, double* ferr,
+               double* berr);
+void refine_cache_free(RefineCache* rc);
 }  // namespace cflx

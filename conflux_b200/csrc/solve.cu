@@ -17,6 +17,7 @@
 #include <cstring>
 
 #include "lu_state.h"
+#include "narrow.cuh"
 
 namespace cflx {
 namespace {
@@ -39,52 +40,6 @@ namespace {
 //     16 dependent L2 round trips per chunk were the whole kernel time.
 // K % 4 == 0 is the only shape condition: a lane's four k indices are either all in range or all out of it, and both A
 // (masked loads) and B (zero-filled staging) are zero beyond K, so nothing stale or NaN reaches the MMA.
-constexpr int NW = 4;         // warps per CTA
-constexpr int BM = 16 * NW;   // rows per CTA
-constexpr int KC = 64;        // k rows per chunk (B in shared memory, A in registers)
-
-struct NarrowArgs {
-    int M, N, K;
-    const double* A;
-    int64_t lda;
-    const double* B;
-    int64_t ldb;
-    const double* C;  // read only when beta != 0; may alias D
-    int64_t ldc;
-    double* D;
-    int64_t ldd;
-    double alpha, beta;
-};
-
-__device__ __forceinline__ void cp_async8(double* smem, const double* gmem, bool valid) {  // zero-fills when !valid
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 8, %2;" ::"r"(smem_u32(smem)), "l"(gmem), "r"(valid ? 8 : 0)
-                 : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
-
-// k-pair rows of BN + 1 double2: the 8 lanes of a quarter warp (g = 0, 1; t = 0..3) read k pairs 2t + h, and
-// 2t * (BN + 1) + g covers 8 distinct 16-byte bank groups
-template <int NT>
-struct NarrowCfg {
-    static constexpr int BN = 8 * NT, LDP = BN + 1;
-    static constexpr size_t STAGE = (size_t)KC / 2 * LDP;  // double2 per buffer
-    static constexpr size_t SMEM = 2 * STAGE * sizeof(double2);
-};
-
-// B rows [kc, kc + KC) x columns [n0, n0 + BN) of chunk kc into one buffer, as k pairs
-template <int NT>
-__device__ __forceinline__ void stage_b(const NarrowArgs& g, int kc, int n0, double2* buf) {
-    constexpr int BN = NarrowCfg<NT>::BN, LDP = NarrowCfg<NT>::LDP;
-    double* d = reinterpret_cast<double*>(buf);
-    for (int e = threadIdx.x; e < KC * BN; e += NW * 32) {
-        const int kk = e / BN, n = e % BN, k = kc + kk, col = n0 + n;
-        const bool ok = k < g.K && col < g.N;
-        cp_async8(d + 2 * ((kk >> 1) * LDP + n) + (kk & 1), ok ? g.B + (int64_t)k * g.ldb + col : g.B, ok);
-    }
-    cp_async_commit();
-}
-
 // epilogue of one m16n8 tile row pair: acc[j][0..1] = D[row_a][n0 + 8j + 2t + {0,1}], acc[j][2..3] the same of row_b.  C
 // may alias D: each element is read and then written by the same thread, so plain (coherent) accesses suffice.
 template <int NT>
@@ -386,6 +341,7 @@ int diag_solve(const SolveCache& sc, const SolveFactor& f, int t, Tri tri, doubl
 void solve_cache_free(SolveCache* sc) {
     for (double* p : {sc->inv, sc->B, sc->W, sc->Z, sc->R, sc->Y, sc->X, sc->Xg}) cudaFree(p);
     for (int* p : {sc->rows, sc->rows_id, sc->cols, sc->unperm}) cudaFree(p);
+    refine_cache_free(&sc->rf);
     *sc = SolveCache{};
 }
 
@@ -464,7 +420,7 @@ int solve_seed(SolveCache* sc, const SolveFactor& f, int ldn, int nrhs, const do
     if (holds && at.n > 0) {
         CFLX_CUDA(cudaMemsetAsync(sc->B, 0, sizeof(double) * f.M * ldn, s));
         CFLX_CUDA(cudaMemcpy2DAsync(sc->B, ldn * sizeof(double), B, (size_t)ldb * sizeof(double), nrhs * sizeof(double), f.M,
-                                    cudaMemcpyHostToDevice, s));
+                                    cudaMemcpyDefault, s));
         CFLX_TRY(launch_gather_rows(sc->B, ldn, at.rows, at.n, ldn, at.dst, s));
     }
     return CFLX_OK;
@@ -556,73 +512,21 @@ int solve_finish(SolveCache* sc, const SolveFactor& f, int ldn, int nrhs, double
     }
     if (X)
         CFLX_CUDA(cudaMemcpy2DAsync(X, (size_t)ldx * sizeof(double), out, ldn * sizeof(double), nrhs * sizeof(double), f.M,
-                                    cudaMemcpyDeviceToHost, s));
+                                    cudaMemcpyDefault, s));
     CFLX_CUDA(cudaStreamSynchronize(s));
     return CFLX_OK;
 }
 
 // ---------------------------------------------------------------- the 1-norm condition estimate
-// LAPACK's dlacn2 (Higham, ACM TOMS 14 (1988) 381-396, Algorithm 4.1 with the safeguards of dlacn2), with its reverse
-// communication unrolled: kase 1 asks for inv(A) x, kase 2 for inv(A)^T x.  The sign vector is +1 for x >= 0 (so -0 and
-// NaN are told apart exactly as LAPACK does), idamax takes the first index of the largest |x|, and the sums of |x| run in
-// index order.
+// LAPACK's dlacn2 (Lacn2, refine.cu) driven to the end: kase 1 asks for inv(A) x, kase 2 for inv(A)^T x.
 int estimate_inv_norm1(int n, const std::function<int(int, double*)>& apply, double* est_out) {
-    constexpr int ITMAX = 5;
-    std::vector<double> x(n, 1.0 / n), v(n);
-    std::vector<int> isgn(n);
-    auto asum = [&](const std::vector<double>& a) {
-        double s = 0.0;
-        for (double e : a) s += std::fabs(e);
-        return s;
-    };
-    auto idamax = [&]() {
-        int j = 0;
-        double m = std::fabs(x[0]);
-        for (int i = 1; i < n; ++i)
-            if (std::fabs(x[i]) > m) m = std::fabs(x[i]), j = i;
-        return j;
-    };
-    auto signs = [&]() {
-        for (int i = 0; i < n; ++i) {
-            x[i] = x[i] >= 0.0 ? 1.0 : -1.0;
-            isgn[i] = (int)x[i];
-        }
-    };
-    double est = 0.0;
-    CFLX_TRY(apply(1, x.data()));
-    if (n == 1) {
-        *est_out = std::fabs(x[0]);
-        return CFLX_OK;
+    Lacn2 st;
+    st.start(n);
+    while (st.kase != 0) {
+        CFLX_TRY(apply(st.kase, st.x.data()));
+        st.step();
     }
-    est = asum(x);
-    signs();
-    CFLX_TRY(apply(2, x.data()));
-    int j = idamax();
-    for (int iter = 2;; ++iter) {
-        std::fill(x.begin(), x.end(), 0.0);
-        x[j] = 1.0;
-        CFLX_TRY(apply(1, x.data()));
-        v = x;
-        const double estold = est;
-        est = asum(v);
-        bool repeated = true;
-        for (int i = 0; i < n && repeated; ++i) repeated = (x[i] >= 0.0 ? 1 : -1) == isgn[i];
-        if (repeated || est <= estold) break;  // converged, or cycling
-        signs();
-        CFLX_TRY(apply(2, x.data()));
-        const int jlast = j;
-        j = idamax();
-        if (!(x[jlast] != std::fabs(x[j]) && iter < ITMAX)) break;
-    }
-    double altsgn = 1.0;  // the final stage: x_i = (-1)^i (1 + i / (n - 1))
-    for (int i = 0; i < n; ++i) {
-        x[i] = altsgn * (1.0 + (double)i / (double)(n - 1));
-        altsgn = -altsgn;
-    }
-    CFLX_TRY(apply(1, x.data()));
-    const double temp = 2.0 * (asum(x) / (double)(3 * n));
-    if (temp > est) est = temp;
-    *est_out = est;
+    *est_out = st.est;
     return CFLX_OK;
 }
 

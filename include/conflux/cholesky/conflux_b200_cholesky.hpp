@@ -101,5 +101,13 @@ inline double choleskyRcond(double* anorm = nullptr) {
     if (anorm) *anorm = a;
     return r;
 }
+// LAPACK dporfs with the factor of the last parallelCholesky() (cflx_chol_refine, collective): X (matrix_size() x nrhs)
+// holds a solution of A X = B and is refined in place; ferr / berr as conflux::LU_refine.
+inline void choleskyRefine(int nrhs, const double* B, int ldb, double* X, int ldx, double* ferr = nullptr,
+                           double* berr = nullptr) {
+    auto& s = chol_detail::state();
+    if (!s.plan) throw CholeskyException("choleskyRefine() before initialize()");
+    chol_detail::check(cflx_chol_refine(s.plan, nrhs, B, ldb, X, ldx, ferr, berr), "choleskyRefine");
+}
 
 }  // namespace conflux

@@ -273,4 +273,13 @@ double LU_rcond(lu_params<T>& gv, double* anorm = nullptr) {
     return r;
 }
 
+// LAPACK dgerfs with the factors of the last LU_rep on the GPU grid.  Collective.  X (M x nrhs, ldx) holds a solution of
+// A X = B (A^T X = B when transposed) and is refined in place, identical on every rank; ferr / berr (nrhs each, may be
+// null; a null ferr skips the estimator): the estimated forward error bound and the componentwise backward error.
+template <class T>
+void LU_refine(lu_params<T>& gv, int nrhs, const T* B, int ldb, T* X, int ldx, double* ferr = nullptr,
+               double* berr = nullptr, bool transposed = false) {
+    check(cflx_lu_refine(gv.plan, transposed ? 1 : 0, nrhs, B, ldb, X, ldx, ferr, berr), "LU_refine");
+}
+
 }  // namespace conflux

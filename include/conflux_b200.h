@@ -111,6 +111,17 @@ int cflx_lu_solve_trans(cflx_lu*, int nrhs, const double* B, int ldb, double* X,
  * buffer of the last run was handed to the queued next matrix.  Leaves the factors, the permutation and any later solve
  * as they are. */
 int cflx_lu_rcond(cflx_lu*, double* rcond_out, double* anorm_out);
+/* COLLECTIVE.  LAPACK dgerfs on the GPU grid with the factors of the last cflx_lu_factor and the input it kept:
+ * trans 0: A X = B, 1: A^T X = B.  B, X: M x nrhs row-major host arrays (M = the padded size), ldb / ldx >= nrhs, the same
+ * on every rank; X holds a solution on entry (e.g. from cflx_lu_solve) and the refined one on return, identical on
+ * every rank.  ferr_out / berr_out: nrhs doubles each, either may be NULL; with ferr_out NULL the estimator does not run.
+ * Per column, as dgerfs: at most 5 corrections while the componentwise backward error berr = max_i |b - op(A) x|_i /
+ * (|op(A)| |x| + |b|)_i exceeds 2^-53 and at least halves; ferr bounds ||x - x_true||_inf / ||x||_inf by the Hager-Higham
+ * estimate of || |inv(op A)| (|r| + (M + 1) 2^-53 (|op(A)| |x| + |b|)) ||_inf.  CFLX_ERR_ARG for trans not 0 / 1, nrhs < 1,
+ * ldb or ldx < nrhs, a NULL B or X; CFLX_ERR_STATE as cflx_lu_rcond.  No singularity check (like dgerfs).  Leaves the
+ * factors, the permutation, the input, later solves and the launch count as they are. */
+int cflx_lu_refine(cflx_lu*, int trans, int nrhs, const double* B, int ldb, double* X, int ldx, double* ferr_out,
+                   double* berr_out);
 /* 1 when this plan's trailing update runs on the int8 wgmma digit-plane path (ozaki.cu), 0 for the FP64 DMMA kernel
  * (gemm.cu) */
 int cflx_lu_uses_ozaki(const cflx_lu*);
@@ -169,6 +180,10 @@ int cflx_chol_solve(cflx_chol*, int nrhs, const double* B, int ldb, double* X, i
  * whose lower triangle is stored (anorm_out, may be NULL), ||inv(A)||_1 estimated by Hager-Higham's method with solves.
  * Identical on every rank.  CFLX_ERR_STATE as cflx_chol_solve.  Leaves the factor and any later solve as they are. */
 int cflx_chol_rcond(cflx_chol*, double* rcond_out, double* anorm_out);
+/* COLLECTIVE.  LAPACK dporfs (UPLO = 'L') with the factor of the last successful cflx_chol_factor and the input it kept
+ * (its lower triangle); the arguments and results of cflx_lu_refine without trans.  CFLX_ERR_STATE as cflx_chol_solve. */
+int cflx_chol_refine(cflx_chol*, int nrhs, const double* B, int ldb, double* X, int ldx, double* ferr_out,
+                     double* berr_out);
 /* number of kernels this object counted since the last reset (bench.py's gpu_launches); cflx_chol_solve adds none */
 int cflx_chol_launch_count(cflx_chol*, int64_t* count_out, int reset);
 void cflx_chol_destroy(cflx_chol*);
@@ -184,6 +199,13 @@ int cflx_dbg_gemm_narrow(int M, int N, int K, const double* A, const double* B, 
  * of the Cholesky solve.  On the device AT gets an even leading dimension >= M, so any M >= 1 can be run. */
 int cflx_dbg_gemm_narrow_tn(int M, int N, int K, const double* AT, const double* B, const double* C, double alpha,
                             double beta, double* D, int reps, double* ms_out);
+/* the residual kernels of cflx_*_refine on one layer-0 share A (Ml x Nl row-major, conflux layout of tile v on grid
+ * position (pi, pj) of Px x Py): mode 0 (NN) P = A Xc, Q = |A| |Xc| (Ml rows); 1 (TN) P = A^T Xr, Q = |A|^T |Xr| (Nl rows);
+ * 2 the stored lower triangle of the real tiles (global tile index < Kappa), NN over global row >= column into rows
+ * [0, Ml) and TN over global row > column into rows [Ml, Ml + Nl).  Xc: Nl x nrhs, Xr: Ml x nrhs (either may be NULL when
+ * the mode does not read it).  P_out / Q_out: nrhs columns.  ms_out: mean device time of one launch over reps. */
+int cflx_dbg_residual(int mode, int Ml, int Nl, const double* A, int v, int Kappa, int Px, int Py, int pi, int pj,
+                      int nrhs, const double* Xc, const double* Xr, double* P_out, double* Q_out, int reps, double* ms_out);
 /* partial-pivot LU of an n x v row-major panel: perm_out[v], A00_out[v*v] (L00\U00), LU_out[n*v] rows unpermuted */
 int cflx_dbg_panel(int n, int v, const double* panel, int* perm_out, double* A00_out, double* LU_out, int reps,
                    double* ms_out);
