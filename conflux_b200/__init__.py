@@ -350,19 +350,45 @@ class dbg:
 
     @staticmethod
     def gemm_tn(AT, B, C=None, alpha=1.0, beta=0.0, reps=1):
-        AT = np.ascontiguousarray(AT, dtype=np.float64)
-        B = np.ascontiguousarray(B, dtype=np.float64)
+        """D = beta*C + alpha * AT^T @ B on the trailing-update kernel (AT: K x M, B: K x N, C: M x N or None = zeros;
+        K % 4 == 0), on contiguous out-of-place buffers with M and N padded to even.  Returns (D, mean ms of one
+        launch)."""
+        AT = np.asarray(AT, dtype=np.float64)
+        B = np.asarray(B, dtype=np.float64)
         K, M = AT.shape
         N = B.shape[1]
-        D = np.empty((M, N))
-        ms = ctypes.c_double()
-        Cp = None
+        M2, N2 = M + (M & 1), N + (N & 1)
+        ATp = np.zeros((K, M2))
+        ATp[:, :M] = AT
+        Bp = np.zeros((K, N2))
+        Bp[:, :N] = B
+        Cp = np.zeros((M, N2))
         if C is not None:
-            C = np.ascontiguousarray(C, dtype=np.float64)
-            Cp = C.ctypes.data
-        check(lib().cflx_dbg_gemm_tn(M, N, K, AT.ctypes.data, B.ctypes.data, Cp, float(alpha), float(beta), D.ctypes.data,
-                                     int(reps), ctypes.byref(ms)), "dbg_gemm_tn")
-        return D, ms.value
+            Cp[:, :N] = C
+        D, _, ms = dbg.gemm_tn_window(ATp, Bp, Cp, M, N2, K, alpha, beta, in_place=False, reps=reps)
+        return D[:, :N], ms
+
+    @staticmethod
+    def gemm_tn_window(AT, B, C, M, N, K, alpha=1.0, beta=0.0, at_off=(0, 0), b_off=(0, 0), c_off=(0, 0), in_place=True,
+                       reps=1):
+        """The trailing-update kernel on a window of whole buffers, as the factorisation launches it: rows
+        [c_off[0], +M) x columns [c_off[1], +N) of C become beta*C + alpha * AT'^T @ B', with AT' the K x M block of AT
+        at (row, column) at_off and B' the K x N block of B at b_off.  in_place: D is C on the device (the trailing
+        update); else D starts as a device copy of C.  Every entry outside those blocks may hold anything (NaN canaries):
+        the kernel reads AT' with M rounded up to even, nothing else.  Returns (D, C, ms): the whole D and C buffers
+        after the call (the same array in place) and the mean ms of one launch."""
+        AT = np.ascontiguousarray(AT, dtype=np.float64)
+        B = np.ascontiguousarray(B, dtype=np.float64)
+        C = np.ascontiguousarray(C, dtype=np.float64)
+        D = np.empty_like(C)
+        Cout = D if in_place else np.empty_like(C)
+        ms = ctypes.c_double()
+        check(lib().cflx_dbg_gemm_tn(int(M), int(N), int(K), AT.ctypes.data, AT.shape[0], AT.shape[1],
+                                     at_off[0] * AT.shape[1] + at_off[1], B.ctypes.data, B.shape[0], B.shape[1],
+                                     b_off[0] * B.shape[1] + b_off[1], C.ctypes.data, C.shape[0], C.shape[1],
+                                     int(c_off[0]), int(c_off[1]), float(alpha), float(beta), 1 if in_place else 0,
+                                     D.ctypes.data, Cout.ctypes.data, int(reps), ctypes.byref(ms)), "dbg_gemm_tn")
+        return D, Cout, ms.value
 
     @staticmethod
     def gemm_narrow(A, B, C=None, alpha=1.0, beta=0.0, reps=1, out=None):
@@ -440,7 +466,10 @@ class dbg:
         return perm, A00, LU[:n], ms.value
 
     @staticmethod
-    def trsm(A00, B=None, R=None):
+    def trsm(A00, B=None, R=None, nb=0, ld=0):
+        """X = B @ inv(U) and Y = inv(L) @ R (A00 = L\\U, L unit lower) on the factorisation's TRSMs, with diagonal blocks
+        of nb (0 = the factorisation's default) and the device panels' leading dimension ld (0 = the minimum; the padding
+        holds NaN).  Returns (X, Y), None where B / R is None."""
         A00 = np.ascontiguousarray(A00, dtype=np.float64)
         v = A00.shape[0]
         X = Y = None
@@ -451,7 +480,7 @@ class dbg:
         if R is not None:
             R = np.ascontiguousarray(R, dtype=np.float64)
             Y = np.empty_like(R)
-        check(lib().cflx_dbg_trsm(n, v, A00.ctypes.data, B.ctypes.data if B is not None else None,
+        check(lib().cflx_dbg_trsm(n, v, int(nb), int(ld), A00.ctypes.data, B.ctypes.data if B is not None else None,
                                   X.ctypes.data if X is not None else None, R.ctypes.data if R is not None else None,
                                   Y.ctypes.data if Y is not None else None), "dbg_trsm")
         return X, Y
@@ -482,22 +511,26 @@ class dbg:
         return L, LT, info.value
 
     @staticmethod
-    def ozaki_gemm(AT, B, C=None, reps=1, want_planes=False):
-        """D = C - AT^T @ B on the int8 wgmma path.  Returns dict(D, ms, split_ms[, pa, pb, ea, eb])."""
+    def ozaki_gemm(AT, B, C=None, reps=1, want_planes=False, row0=0, col0=0, max_ctas=0):
+        """D = C - AT'^T @ B' on the int8 wgmma path, AT' = AT[:, row0:], B' = B[:, col0:] (the planes of all of AT and B
+        are made, as the factorisation makes them), on at most max_ctas CTAs (0 = one per SM).  Returns dict(D, ms,
+        split_ms[, pa, pb, ea, eb]) with the planes and exponents of all of AT and B."""
         AT = np.ascontiguousarray(AT, dtype=np.float64)
         B = np.ascontiguousarray(B, dtype=np.float64)
-        K, M = AT.shape
-        N = B.shape[1]
+        K, Ma = AT.shape
+        Nb = B.shape[1]
+        M, N = Ma - row0, Nb - col0
         D = np.empty((M, N))
         Cp = np.ascontiguousarray(C, dtype=np.float64) if C is not None else None
-        pa = np.zeros((8, M, K), dtype=np.int8) if want_planes else None
-        pb = np.zeros((8, N, K), dtype=np.int8) if want_planes else None
-        ea = np.zeros(M, dtype=np.int32) if want_planes else None
-        eb = np.zeros(N, dtype=np.int32) if want_planes else None
+        pa = np.zeros((8, Ma, K), dtype=np.int8) if want_planes else None
+        pb = np.zeros((8, Nb, K), dtype=np.int8) if want_planes else None
+        ea = np.zeros(Ma, dtype=np.int32) if want_planes else None
+        eb = np.zeros(Nb, dtype=np.int32) if want_planes else None
         ms, sms = ctypes.c_double(), ctypes.c_double()
         ptr = lambda a: a.ctypes.data if a is not None else None
-        check(lib().cflx_dbg_ozaki_gemm(M, N, K, AT.ctypes.data, B.ctypes.data, ptr(Cp), D.ctypes.data, ptr(pa), ptr(pb), ptr(ea),
-                                        ptr(eb), int(reps), ctypes.byref(ms), ctypes.byref(sms)), "dbg_ozaki_gemm")
+        check(lib().cflx_dbg_ozaki_gemm(M, N, K, int(row0), int(col0), int(max_ctas), AT.ctypes.data, B.ctypes.data, ptr(Cp),
+                                        D.ctypes.data, ptr(pa), ptr(pb), ptr(ea), ptr(eb), int(reps), ctypes.byref(ms),
+                                        ctypes.byref(sms)), "dbg_ozaki_gemm")
         return dict(D=D, ms=ms.value, split_ms=sms.value, pa=pa, pb=pb, ea=ea, eb=eb)
 
     @staticmethod

@@ -105,8 +105,10 @@ def lib():
                                        ctypes.c_void_p, ctypes.c_void_p]
         L.cflx_chol_launch_count.argtypes = [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int64), ctypes.c_int]
         L.cflx_init_matrix_host.argtypes = [ctypes.c_int] * 8 + [ctypes.c_void_p]
-        L.cflx_dbg_gemm_tn.argtypes = [ctypes.c_int] * 3 + [ctypes.c_void_p] * 3 + [ctypes.c_double] * 2 + [
-            ctypes.c_void_p, ctypes.c_int, c_double_p]
+        _buf = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int64]
+        L.cflx_dbg_gemm_tn.argtypes = [ctypes.c_int] * 3 + _buf + [ctypes.c_int64] + _buf + [ctypes.c_int64] + _buf + [
+            ctypes.c_int] * 2 + [ctypes.c_double] * 2 + [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int,
+                                                          c_double_p]
         L.cflx_dbg_gemm_narrow.argtypes = [ctypes.c_int] * 3 + [ctypes.c_void_p] * 3 + [ctypes.c_double] * 2 + [
             ctypes.c_void_p, ctypes.c_int, c_double_p]
         L.cflx_dbg_gemm_narrow_tn.argtypes = [ctypes.c_int] * 3 + [ctypes.c_void_p] * 3 + [ctypes.c_double] * 2 + [
@@ -114,12 +116,12 @@ def lib():
         L.cflx_dbg_residual.argtypes = [ctypes.c_int] * 3 + [ctypes.c_void_p] + [ctypes.c_int] * 7 + [ctypes.c_void_p] * 4 + [
             ctypes.c_int, c_double_p]
         L.cflx_dbg_panel.argtypes = [ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 4 + [ctypes.c_int, c_double_p]
-        L.cflx_dbg_trsm.argtypes = [ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 5
+        L.cflx_dbg_trsm.argtypes = [ctypes.c_int] * 3 + [ctypes.c_int64] + [ctypes.c_void_p] * 5
         L.cflx_dbg_diag_inverse.argtypes = [ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 3
         L.cflx_dbg_potrf_tile.argtypes = [ctypes.c_int] + [ctypes.c_void_p] * 4 + [ctypes.c_int]
         L.cflx_dbg_push_pivots.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
                                            ctypes.c_void_p, ctypes.c_void_p]
-        L.cflx_dbg_ozaki_gemm.argtypes = [ctypes.c_int] * 3 + [ctypes.c_void_p] * 8 + [ctypes.c_int, c_double_p, c_double_p]
+        L.cflx_dbg_ozaki_gemm.argtypes = [ctypes.c_int] * 6 + [ctypes.c_void_p] * 8 + [ctypes.c_int, c_double_p, c_double_p]
         L.cflx_dbg_wgmma_peak.argtypes = [ctypes.c_int, c_double_p]
         L.cflx_dbg_fp64_peak.argtypes = [ctypes.c_int, c_double_p]
         L.cflx_dbg_fp64_peak_ex.argtypes = [ctypes.c_int, c_double_p, c_double_p]

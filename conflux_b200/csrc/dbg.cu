@@ -2,6 +2,7 @@
 // They drive the SAME kernels the factorisation uses, with host buffers in and out, so that tests/ can check every
 // kernel in isolation against numpy / the oracle, and bench.py can time the dominant kernel alone.
 #include <algorithm>
+#include <limits>
 #include <vector>
 
 #include "../../include/conflux_b200.h"
@@ -146,34 +147,52 @@ int cflx_dbg_fp64_peak_ex(int which, double* burst_out, double* sustained_out) {
 }
 int cflx_dbg_fp64_peak(int which, double* tflops_out) { return cflx_dbg_fp64_peak_ex(which, tflops_out, nullptr); }
 
-int cflx_dbg_gemm_tn(int M, int N, int K, const double* AT, const double* B, const double* C, double alpha, double beta,
-                     double* D, int reps, double* ms_out) {
+// gemm_tn_kernel on a window of whole buffers, as the factorisation and the TRSMs launch it (see the header).  The
+// timed repetitions run first; then C (and D) are restored and the launch whose result is returned runs.
+int cflx_dbg_gemm_tn(int M, int N, int K, const double* AT, int at_rows, int64_t ldat, int64_t at_off, const double* B,
+                     int b_rows, int64_t ldb, int64_t b_off, const double* C, int c_rows, int64_t ldc, int row_off,
+                     int col_off, double alpha, double beta, int in_place, double* D_out, double* C_out, int reps,
+                     double* ms_out) {
     CFLX_TRY(check_device());
-    if (M <= 0 || N <= 0 || K <= 0) return CFLX_ERR_ARG;
-    const int64_t ldat = round_up(M, 2), ldb = round_up(N, 2), ldc = ldb;
-    DevBuf dA, dB, dC, dD;
-    CFLX_TRY(dA.alloc(sizeof(double) * K * ldat));
-    CFLX_TRY(dB.alloc(sizeof(double) * K * ldb));
-    CFLX_TRY(dC.alloc(sizeof(double) * M * ldc));
-    CFLX_TRY(dD.alloc(sizeof(double) * M * ldc));
-    CFLX_CUDA(cudaMemset(dA.p, 0, sizeof(double) * K * ldat));
-    CFLX_CUDA(cudaMemset(dB.p, 0, sizeof(double) * K * ldb));
-    CFLX_CUDA(cudaMemcpy2D(dA.p, ldat * 8, AT, (size_t)M * 8, (size_t)M * 8, K, cudaMemcpyHostToDevice));
-    CFLX_CUDA(cudaMemcpy2D(dB.p, ldb * 8, B, (size_t)N * 8, (size_t)N * 8, K, cudaMemcpyHostToDevice));
-    if (C) CFLX_CUDA(cudaMemcpy2D(dC.p, ldc * 8, C, (size_t)N * 8, (size_t)N * 8, M, cudaMemcpyHostToDevice));
-    else CFLX_CUDA(cudaMemset(dC.p, 0, sizeof(double) * M * ldc));
+    if (M <= 0 || N <= 0 || K <= 0 || !AT || !B || !C || at_rows <= 0 || b_rows <= 0 || c_rows <= 0 || ldat <= 0 ||
+        ldb <= 0 || ldc <= 0 || at_off < 0 || b_off < 0 || row_off < 0 || col_off < 0)
+        return CFLX_ERR_ARG;
+    // every element the kernel may touch lies inside the buffers: AT rows of round_up(M, 2) (the producer's even copy
+    // width), B rows of N, the C window; 16-byte alignment of every operand row needs even offsets
+    if ((at_off & 1) || (b_off & 1) || (col_off & 1) || at_off + (K - 1) * ldat + round_up(M, 2) > (int64_t)at_rows * ldat ||
+        b_off + (K - 1) * ldb + N > (int64_t)b_rows * ldb || row_off + M > c_rows || col_off + N > ldc) {
+        set_last_error("dbg_gemm_tn: window outside the buffers or misaligned");
+        return CFLX_ERR_ARG;
+    }
+    const size_t a_n = (size_t)at_rows * ldat, b_n = (size_t)b_rows * ldb, c_n = (size_t)c_rows * ldc;
+    DevBuf dA, dB, dC, dC0, dD;
+    CFLX_TRY(dA.alloc(sizeof(double) * a_n));
+    CFLX_TRY(dB.alloc(sizeof(double) * b_n));
+    CFLX_TRY(dC.alloc(sizeof(double) * c_n));
+    CFLX_TRY(dC0.alloc(sizeof(double) * c_n));
+    CFLX_TRY(dD.alloc(sizeof(double) * c_n));
+    CFLX_CUDA(cudaMemcpy(dA.p, AT, sizeof(double) * a_n, cudaMemcpyHostToDevice));
+    CFLX_CUDA(cudaMemcpy(dB.p, B, sizeof(double) * b_n, cudaMemcpyHostToDevice));
+    CFLX_CUDA(cudaMemcpy(dC0.p, C, sizeof(double) * c_n, cudaMemcpyHostToDevice));
+    auto restore = [&]() -> int {
+        CFLX_CUDA(cudaMemcpy(dC.p, dC0.p, sizeof(double) * c_n, cudaMemcpyDeviceToDevice));
+        CFLX_CUDA(cudaMemcpy(dD.p, dC0.p, sizeof(double) * c_n, cudaMemcpyDeviceToDevice));
+        return CFLX_OK;
+    };
+    const int64_t c_at = (int64_t)row_off * ldc + col_off;
     GemmArgs g{};
-    g.M = M; g.N = (int)ldb; g.K = K;
-    g.AT = dA.as<double>(); g.ldat = ldat;
-    g.B = dB.as<double>(); g.ldb = ldb;
-    g.C = dC.as<double>(); g.ldc = ldc;
-    g.D = dD.as<double>(); g.ldd = ldc;
+    g.M = M; g.N = N; g.K = K;
+    g.AT = dA.as<double>() + at_off; g.ldat = ldat;
+    g.B = dB.as<double>() + b_off; g.ldb = ldb;
+    g.C = dC.as<double>() + c_at; g.ldc = ldc;
+    g.D = (in_place ? dC.as<double>() : dD.as<double>()) + c_at; g.ldd = ldc;
     g.alpha = alpha; g.beta = beta;
+    CFLX_TRY(restore());
     cudaEvent_t e0, e1;
     CFLX_CUDA(cudaEventCreate(&e0));
     CFLX_CUDA(cudaEventCreate(&e1));
     if (reps < 1) reps = 1;
-    CFLX_TRY(launch_gemm_tn(g, 0));  // warm-up / the result
+    CFLX_TRY(launch_gemm_tn(g, 0));  // warm-up
     CFLX_CUDA(cudaEventRecord(e0));
     for (int r = 0; r < reps; ++r) CFLX_TRY(launch_gemm_tn(g, 0));
     CFLX_CUDA(cudaEventRecord(e1));
@@ -183,7 +202,10 @@ int cflx_dbg_gemm_tn(int M, int N, int K, const double* AT, const double* B, con
     if (ms_out) *ms_out = ms / reps;
     cudaEventDestroy(e0);
     cudaEventDestroy(e1);
-    if (D) CFLX_CUDA(cudaMemcpy2D(D, (size_t)N * 8, dD.p, ldc * 8, (size_t)N * 8, M, cudaMemcpyDeviceToHost));
+    CFLX_TRY(restore());
+    CFLX_TRY(launch_gemm_tn(g, 0));
+    if (D_out) CFLX_CUDA(cudaMemcpy(D_out, in_place ? dC.p : dD.p, sizeof(double) * c_n, cudaMemcpyDeviceToHost));
+    if (C_out) CFLX_CUDA(cudaMemcpy(C_out, dC.p, sizeof(double) * c_n, cudaMemcpyDeviceToHost));
     CFLX_CUDA(cudaDeviceSynchronize());
     return CFLX_OK;
 }
@@ -378,15 +400,20 @@ int cflx_dbg_panel(int n, int v, const double* panel, int* perm_out, double* A00
     return CFLX_OK;
 }
 
-int cflx_dbg_trsm(int n, int v, const double* A00, const double* B, double* X_out, const double* R, double* Y_out) {
+int cflx_dbg_trsm(int n, int v, int nb, int64_t ld, const double* A00, const double* B, double* X_out, const double* R,
+                  double* Y_out) {
     CFLX_TRY(check_device());
     if (n <= 0 || v <= 0 || v % 4 != 0) return CFLX_ERR_ARG;
-    int nb = 0;
-    for (int c : {128, 64, 32, 16, 8, 4})
-        if (!nb && v % c == 0) nb = c;
-    if (nb == 0) return CFLX_ERR_UNSUPPORTED;
-    const int64_t ld = round_up(n, 2);
-    std::vector<double> A00T((size_t)v * v), BT((size_t)v * ld, 0.0), RT((size_t)v * ld, 0.0);
+    if (nb == 0)
+        for (int c : {128, 64, 32, 16, 8, 4})
+            if (!nb && v % c == 0) nb = c;
+    if (nb != 4 && nb != 8 && nb != 16 && nb != 32 && nb != 64 && nb != 128) return CFLX_ERR_UNSUPPORTED;
+    if (v % nb != 0) return CFLX_ERR_ARG;
+    if (ld == 0) ld = round_up(n, 2);
+    if ((ld & 1) || ld < round_up(n, 2)) return CFLX_ERR_ARG;
+    // the padding columns [n, ld) of the operand panels hold NaN: they must not reach the n solved columns
+    const double nan = std::numeric_limits<double>::quiet_NaN();
+    std::vector<double> A00T((size_t)v * v), BT((size_t)v * ld, nan), RT((size_t)v * ld, nan);
     for (int i = 0; i < v; ++i)
         for (int j = 0; j < v; ++j) A00T[(size_t)j * v + i] = A00[(size_t)i * v + j];
     DevBuf dA, dAT, dUinv, dLinvT, dP, dL, dR, dU;
@@ -413,7 +440,7 @@ int cflx_dbg_trsm(int n, int v, const double* A00, const double* B, double* X_ou
         CFLX_CUDA(cudaMemcpy(dR.p, RT.data(), 8 * (size_t)v * ld, cudaMemcpyHostToDevice));
         CFLX_CUDA(cudaMemset(dU.p, 0, 8 * (size_t)v * ld));
         CFLX_TRY(trsm_left_lower_unit(dAT.as<double>(), dLinvT.as<double>(), v, nb, dR.as<double>(), dU.as<double>(), ld,
-                                      (int)ld, 0));
+                                      (int)round_up(n, 2), 0));
         CFLX_CUDA(cudaMemcpy(RT.data(), dU.p, 8 * (size_t)v * ld, cudaMemcpyDeviceToHost));
         for (int i = 0; i < v; ++i)
             for (int c = 0; c < n; ++c) Y_out[(size_t)i * n + c] = RT[(size_t)i * ld + c];
@@ -521,24 +548,27 @@ int cflx_dbg_push_pivots(int n_rows, int n_cols, double* A_inout, int npiv, cons
 // D = C - AT^T * B on the int8 wgmma path (ozaki.cu): AT [K x M], B [K x N], C/D [M x N] row-major dense host arrays,
 // K a multiple of 128, N even.  Optional outputs for tests: the digit planes [8][M][K] / [8][N][K] (int8) and the
 // exponents [M] / [N], exactly as the kernels produced them.  ms_out = mean device time of the GEMM kernel alone.
-int cflx_dbg_ozaki_gemm(int M, int N, int K, const double* AT, const double* B, const double* C, double* D,
-                        signed char* planesA_out, signed char* planesB_out, int* ea_out, int* eb_out, int reps,
-                        double* ms_out, double* split_ms_out) {
+int cflx_dbg_ozaki_gemm(int M, int N, int K, int row0, int col0, int max_ctas, const double* AT, const double* B,
+                        const double* C, double* D, signed char* planesA_out, signed char* planesB_out, int* ea_out,
+                        int* eb_out, int reps, double* ms_out, double* split_ms_out) {
     CFLX_TRY(check_device());
-    if (M <= 0 || N <= 0 || K <= 0 || (N & 1)) return CFLX_ERR_ARG;
-    const int64_t ldat = round_up(M, 2), ldb = N, ldc = N;
+    if (M <= 0 || N <= 0 || K <= 0 || (N & 1) || row0 < 0 || col0 < 0 || max_ctas < 0) return CFLX_ERR_ARG;
+    // AT holds row0 + M operand rows, B col0 + N columns; the planes of all of them are made (B's in the two windows
+    // [0, col0) and [col0, col0 + N), as the factorisation's look-ahead splits them), the product reads the window
+    const int Ma = row0 + M, Nb = col0 + N;
+    const int64_t ldat = round_up(Ma, 2), ldb = Nb, ldc = N;
     DevBuf dA, dB, dC, dC0;
     CFLX_TRY(dA.alloc(sizeof(double) * K * ldat));
     CFLX_TRY(dB.alloc(sizeof(double) * K * ldb));
     CFLX_TRY(dC.alloc(sizeof(double) * M * ldc));
     CFLX_TRY(dC0.alloc(sizeof(double) * M * ldc));
     CFLX_CUDA(cudaMemset(dA.p, 0, sizeof(double) * K * ldat));
-    CFLX_CUDA(cudaMemcpy2D(dA.p, ldat * 8, AT, (size_t)M * 8, (size_t)M * 8, K, cudaMemcpyHostToDevice));
+    CFLX_CUDA(cudaMemcpy2D(dA.p, ldat * 8, AT, (size_t)Ma * 8, (size_t)Ma * 8, K, cudaMemcpyHostToDevice));
     CFLX_CUDA(cudaMemcpy(dB.p, B, sizeof(double) * K * ldb, cudaMemcpyHostToDevice));
     if (C) CFLX_CUDA(cudaMemcpy(dC0.p, C, sizeof(double) * M * ldc, cudaMemcpyHostToDevice));
     else CFLX_CUDA(cudaMemset(dC0.p, 0, sizeof(double) * M * ldc));
     OzakiWorkspace ws;
-    int rc = ozaki_workspace_create(&ws, M, N, K);
+    int rc = ozaki_workspace_create(&ws, Ma, Nb, K);
     cudaEvent_t e0, e1, e2;
     cudaEventCreate(&e0);
     cudaEventCreate(&e1);
@@ -548,10 +578,11 @@ int cflx_dbg_ozaki_gemm(int M, int N, int K, const double* AT, const double* B, 
     for (int r = 0; r < reps + 1 && rc == CFLX_OK; ++r) {
         cudaMemcpyAsync(dC.p, dC0.p, sizeof(double) * M * ldc, cudaMemcpyDeviceToDevice, 0);
         cudaEventRecord(e0);
-        rc = ozaki_split_a(&ws, dA.as<double>(), ldat, M, 0);
-        if (!rc) rc = ozaki_split_b(&ws, dB.as<double>(), ldb, 0, N, 0);
+        rc = ozaki_split_a(&ws, dA.as<double>(), ldat, Ma, 0);
+        if (!rc && col0 > 0) rc = ozaki_split_b(&ws, dB.as<double>(), ldb, 0, col0, 0);
+        if (!rc) rc = ozaki_split_b(&ws, dB.as<double>(), ldb, col0, N, 0);
         cudaEventRecord(e1);
-        if (!rc) rc = launch_ozaki_gemm(&ws, M, N, 0, 0, dC.as<double>(), ldc, 0, 0);
+        if (!rc) rc = launch_ozaki_gemm(&ws, M, N, row0, col0, dC.as<double>(), ldc, max_ctas, 0);
         cudaEventRecord(e2);
         if (cudaEventSynchronize(e2) != cudaSuccess) {
             set_last_error("ozaki kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
@@ -571,11 +602,11 @@ int cflx_dbg_ozaki_gemm(int M, int N, int K, const double* AT, const double* B, 
     if (rc == CFLX_OK) {
         if (D) cudaMemcpy(D, dC.p, sizeof(double) * M * ldc, cudaMemcpyDeviceToHost);
         for (int s = 0; s < 8; ++s) {
-            if (planesA_out) cudaMemcpy(planesA_out + (size_t)s * M * K, ws.planesA + (size_t)s * ws.cap_a * K, (size_t)M * K, cudaMemcpyDeviceToHost);
-            if (planesB_out) cudaMemcpy(planesB_out + (size_t)s * N * K, ws.planesB + (size_t)s * ws.cap_b * K, (size_t)N * K, cudaMemcpyDeviceToHost);
+            if (planesA_out) cudaMemcpy(planesA_out + (size_t)s * Ma * K, ws.planesA + (size_t)s * ws.cap_a * K, (size_t)Ma * K, cudaMemcpyDeviceToHost);
+            if (planesB_out) cudaMemcpy(planesB_out + (size_t)s * Nb * K, ws.planesB + (size_t)s * ws.cap_b * K, (size_t)Nb * K, cudaMemcpyDeviceToHost);
         }
-        if (ea_out) cudaMemcpy(ea_out, ws.ea, sizeof(int) * M, cudaMemcpyDeviceToHost);
-        if (eb_out) cudaMemcpy(eb_out, ws.eb, sizeof(int) * N, cudaMemcpyDeviceToHost);
+        if (ea_out) cudaMemcpy(ea_out, ws.ea, sizeof(int) * Ma, cudaMemcpyDeviceToHost);
+        if (eb_out) cudaMemcpy(eb_out, ws.eb, sizeof(int) * Nb, cudaMemcpyDeviceToHost);
         if (cudaDeviceSynchronize() != cudaSuccess) rc = CFLX_ERR_CUDA;
     }
     ozaki_workspace_destroy(&ws);

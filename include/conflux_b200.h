@@ -189,9 +189,16 @@ int cflx_chol_launch_count(cflx_chol*, int64_t* count_out, int reset);
 void cflx_chol_destroy(cflx_chol*);
 
 /* ---- single-device building blocks exposed for tests and micro-benchmarks (host buffers in, host out) ----- */
-/* D = beta*C + alpha * AT^T * B with AT [K x M], B [K x N], C/D [M x N], all row-major, dense */
-int cflx_dbg_gemm_tn(int M, int N, int K, const double* AT, const double* B, const double* C, double alpha, double beta,
-                     double* D, int reps, double* ms_out);
+/* D = beta*C + alpha * AT^T * B on the trailing-update kernel, at a window of whole row-major host buffers, as the
+ * factorisation launches it: AT [at_rows x ldat] read from element at_off (K rows of M, rounded up to even), B
+ * [b_rows x ldb] from element b_off (K rows of N), C [c_rows x ldc] updated in rows [row_off, row_off + M) x columns
+ * [col_off, col_off + N).  in_place != 0: D is C on the device; else D is a device copy of C.  D_out / C_out (optional,
+ * c_rows x ldc) receive the whole D and C buffers after the call.  N, K % 4, ldat, ldb, ldc and the offsets (but row_off)
+ * even; the window must lie inside the buffers.  ms_out: mean device time of one launch over reps. */
+int cflx_dbg_gemm_tn(int M, int N, int K, const double* AT, int at_rows, int64_t ldat, int64_t at_off, const double* B,
+                     int b_rows, int64_t ldb, int64_t b_off, const double* C, int c_rows, int64_t ldc, int row_off,
+                     int col_off, double alpha, double beta, int in_place, double* D_out, double* C_out, int reps,
+                     double* ms_out);
 /* D = beta*C + alpha * A * B with A [M x K], B [K x N], C/D [M x N], all row-major, dense: the narrow GEMM of the solve */
 int cflx_dbg_gemm_narrow(int M, int N, int K, const double* A, const double* B, const double* C, double alpha, double beta,
                          double* D, int reps, double* ms_out);
@@ -209,8 +216,12 @@ int cflx_dbg_residual(int mode, int Ml, int Nl, const double* A, int v, int Kapp
 /* partial-pivot LU of an n x v row-major panel: perm_out[v], A00_out[v*v] (L00\U00), LU_out[n*v] rows unpermuted */
 int cflx_dbg_panel(int n, int v, const double* panel, int* perm_out, double* A00_out, double* LU_out, int reps,
                    double* ms_out);
-/* X = B * U^-1 (right, upper, non-unit; B n x v) and Y = L^-1 * R (left, lower, unit; R v x n), A00 = L\U packed */
-int cflx_dbg_trsm(int n, int v, const double* A00, const double* B, double* X_out, const double* R, double* Y_out);
+/* X = B * U^-1 (right, upper, non-unit; B n x v) and Y = L^-1 * R (left, lower, unit; R v x n), A00 = L\U packed.
+ * nb: the diagonal block size (4, 8, ..., 128 dividing v; 0 = the factorisation's default choice).  ld: the leading
+ * dimension of the K-major panels on the device (even, >= n rounded up to even; 0 = that minimum); their padding
+ * columns hold NaN. */
+int cflx_dbg_trsm(int n, int v, int nb, int64_t ld, const double* A00, const double* B, double* X_out, const double* R,
+                  double* Y_out);
 /* inverses of the nb x nb diagonal blocks of A00 = L\U (v x v, nb in 4, 8, ..., 128, v % nb == 0) as the TRSMs use them:
  * Uinv_out[v / nb][nb][nb] = inv(U_jj), LinvT_out[v / nb][nb][nb] = inv(L_jj)^T (L unit lower); only the blocks are read */
 int cflx_dbg_diag_inverse(int v, int nb, const double* A00, double* Uinv_out, double* LinvT_out);
@@ -218,12 +229,14 @@ int cflx_dbg_diag_inverse(int v, int nb, const double* A00, double* Uinv_out, do
  * 4 <= v <= 512; 1: the 128 x 128 block kernel, v == 128; 2: the 128-block tile driver, v % 128 == 0 and v >= 256.
  * L_out = L with zeros above the diagonal, LT_out = L^T, info_out = 1 + first non-positive pivot's column, or 0. */
 int cflx_dbg_potrf_tile(int v, const double* A, double* L_out, double* LT_out, int* info_out, int variant);
-/* D = C - AT^T * B on the int8 wgmma path (error-free digit planes, ozaki.cu); K % 128 == 0, N even.  Optional test
- * outputs: digit planes [8][M][K] / [8][N][K], exponents [M] / [N].  ms_out / split_ms_out: mean device time of the GEMM
- * kernel / of the two digit-plane kernels. */
-int cflx_dbg_ozaki_gemm(int M, int N, int K, const double* AT, const double* B, const double* C, double* D,
-                        signed char* planesA_out, signed char* planesB_out, int* ea_out, int* eb_out, int reps,
-                        double* ms_out, double* split_ms_out);
+/* D = C - AT^T * B on the int8 wgmma path (error-free digit planes, ozaki.cu); K % 128 == 0, N even.  AT is
+ * [K x (row0 + M)] and B [K x (col0 + N)]: the planes of every row / column are made, the product takes operand rows
+ * [row0, row0 + M) and columns [col0, col0 + N), on at most max_ctas CTAs (0 = one per SM).  C/D [M x N].  Optional test
+ * outputs: digit planes [8][row0 + M][K] / [8][col0 + N][K], exponents [row0 + M] / [col0 + N].  ms_out / split_ms_out:
+ * mean device time of the GEMM kernel / of the digit-plane kernels. */
+int cflx_dbg_ozaki_gemm(int M, int N, int K, int row0, int col0, int max_ctas, const double* AT, const double* B,
+                        const double* C, double* D, signed char* planesA_out, signed char* planesB_out, int* ea_out,
+                        int* eb_out, int reps, double* ms_out, double* split_ms_out);
 /* raw int8 tensor-core rate of back-to-back wgmma (64 x n x 32, n = 64/128/192/256, operands resident in shared memory,
  * two warpgroups per CTA, one CTA per SM).  tmacs_out = tera-MACs/s (x2 = TOP/s). */
 int cflx_dbg_wgmma_peak(int n, double* tmacs_out);

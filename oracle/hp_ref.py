@@ -20,7 +20,19 @@ Bounds (u = 2^-53, gamma_n = n u / (1 - n u); Higham, "Accuracy and Stability of
     kernels, and the bit-for-bit pins of the default path (tests/golden/chol_factor_bits.json);
   * forward error (Sun 1991): L^ is the exact factor of A + dA with dA = L^ L^T - A, so
         ||L^ - L||_F / ||L||_2 <= kappa_2(A) eps / (1 - kappa_2(A) eps),   eps = (the bound above on ||dA||_F) / ||A||_2
-    (Sun's constant is 2^-1/2; 1 is used)."""
+    (Sun's constant is 2^-1/2; 1 is used).
+
+The LU path (gemm_ok, lu_*_ok, trsm_*_ok):
+  * the update GEMM D = fl(alpha acc + fl(beta c)), acc = AT^T B summed in any order (Sec. 3.5, Lemma 3.3):
+        |D^ - (beta C + alpha A^T B)| <= gamma_{K+1} (|beta| |C| + |alpha| |A|^T |B|)      (derivation: gemm_ok)
+  * a panel factored by elimination, any summation order (Thm 9.3, rectangular n x v form):
+        |P A - L^ U^| <= gamma_v |L^| |U^|
+  * a factorisation whose U rows (and, with more than one process row, L panels) are solved with inverted nb x nb
+    diagonal blocks: the same argument as the Cholesky bound above,
+        ||P A - L^ U^||_F <= gamma_{n+1} (1 + 4 kappa_max) || |L^| |U^| ||_F,
+    kappa_max over the unit-lower diagonal blocks and, where the L panel is solved (trsm_right_upper_T), the upper ones;
+  * the two TRSMs (X U = B, L Y = R with inverted diagonal blocks of U, unit-lower L):
+        ||X^ U - B||_F <= gamma_{v+1} (1 + 4 kappa_max) || |X^| |U| ||_F,   ||L Y^ - R||_F <= the same with |L| |Y^|."""
 import numpy as np
 
 LD = np.longdouble
@@ -167,6 +179,104 @@ def inverse_componentwise_ok(T, X):
     R = np.abs(matmul(T, X) - np.eye(n, dtype=LD))
     M = np.abs(T) @ np.abs(X)
     return bool(np.all(np.isfinite(X)) and np.all(R <= LD(gamma(n)) * M.astype(LD)))
+
+
+# ------------------------------------------------------------------------------------------------ the LU path
+def gemm_ok(AT, B, C, alpha, beta, D):
+    """Componentwise bound of gemm_tn_kernel's D = beta*C + alpha * AT^T B (AT: K x M, B: K x N; C is not read when
+    beta == 0, so it may hold anything there):
+        |D^ - (beta C + alpha A^T B)| <= gamma_{K+1} (|beta| |C| + |alpha| |A|^T |B|).
+    Derivation.  The accumulator acc is the K-term dot product summed in some order with fma or separate roundings:
+    |acc - A^T B| <= gamma_K |A|^T |B| (Higham Sec. 3.5).  The epilogue forms t = fl(beta c) = beta c (1 + d1) and
+    D^ = fma(alpha, acc, t) = (alpha acc + t)(1 + d2), |d1|, |d2| <= u.  So
+        D^ - (beta c + alpha a^T b) = alpha (acc - a^T b)(1 + d2) + alpha a^T b d2 + beta c ((1 + d1)(1 + d2) - 1),
+    whose terms are bounded by (gamma_K (1 + u) + u) |alpha| |a|^T |b| <= gamma_{K+1} |alpha| |a|^T |b| (Lemma 3.3) and
+    gamma_2 |beta| |c| <= gamma_{K+1} |beta| |c|.  A product alpha*acc rounded before the add would be one more rounding:
+    still inside this bound, which is why the bit-for-bit tests on exact accumulators are the ones that see it."""
+    AT = np.asarray(AT, dtype=np.float64)
+    B = np.asarray(B, dtype=np.float64)
+    D = np.asarray(D, dtype=np.float64)
+    ref = LD(alpha) * matmul(AT.T, B)
+    M = abs(alpha) * (np.abs(AT).T @ np.abs(B))
+    if beta != 0:
+        C = np.asarray(C, dtype=np.float64)
+        ref = ref + LD(beta) * C.astype(LD)
+        M = M + abs(beta) * np.abs(C)
+    R = np.abs(D.astype(LD) - ref)
+    return bool(np.all(np.isfinite(D)) and np.all(R <= LD(gamma(AT.shape[0] + 1)) * M.astype(LD)))
+
+
+def lu_unpack(LU, v=None):
+    """(L, U) of a packed L\\U: LU is n x v (a panel, rows in pivoted order) or n x n; L unit lower n x v, U v x v"""
+    LU = np.asarray(LU, dtype=np.float64)
+    v = LU.shape[1] if v is None else v
+    L = np.tril(LU[:, :v], -1) + np.eye(LU.shape[0], v)
+    return L, np.triu(LU[:v, :v])
+
+
+def lu_residual(A, LU, perm):
+    """(|P A - L^ U^| in longdouble, |L^| |U^| in float64) with P A = A[perm] (perm[i] = the original row at pivoted
+    position i) and L\\U packed in LU, n x v: a whole factor (v = n) or a panel (L^ n x v, U^ v x v)"""
+    A = np.asarray(A, dtype=np.float64)
+    L, U = lu_unpack(LU)
+    # six slices: the product is exact down to 2^-144 of each row's largest multiplier, so tiny multipliers left by near-
+    # exact cancellations (integer inputs) are resolved to their last bit, as the componentwise check needs
+    R = np.abs(A[np.asarray(perm)].astype(LD) - matmul(L, U, count=6))
+    return R, np.abs(L) @ np.abs(U)
+
+
+def lu_componentwise_ok(A, LU, perm, res=None):
+    """Higham Thm 9.3 (the rectangular form): |P A - L^ U^| <= gamma_v |L^| |U^| in every entry, for a panel factored by
+    elimination.  Entry (i, j) is a sum of min(i, j) + 1 <= v terms (one division for the L part)."""
+    R, M = res if res is not None else lu_residual(A, LU, perm)
+    v = np.asarray(LU).shape[1]
+    return bool(np.all(np.isfinite(LU)) and np.all(R <= LD(gamma(v)) * M.astype(LD)))
+
+
+def lu_backward_bound(M, kappa_max):
+    """bound on ||P A - L^ U^||_F of a factorisation that solves with inverted diagonal blocks (module doc);
+    M = |L^| |U^|"""
+    return gamma(M.shape[0] + 1) * (1.0 + 4.0 * kappa_max) * float(np.linalg.norm(M))
+
+
+def lu_normwise_ok(A, LU, perm, kappa_max, res=None):
+    """||P A - L^ U^||_F <= gamma_{n+1} (1 + 4 kappa_max) || |L^| |U^| ||_F (module doc); kappa_max from lu_kappa_max"""
+    R, M = res if res is not None else lu_residual(A, LU, perm)
+    return bool(np.all(np.isfinite(LU)) and float(np.sqrt(np.sum(R * R))) <= lu_backward_bound(M, kappa_max))
+
+
+def lu_kappa_max(LU, nb, upper=False):
+    """largest condition number of the nb x nb unit-lower diagonal blocks of the packed factor, and with upper=True of
+    the upper ones too (the blocks the factorisation inverts)"""
+    L, U = lu_unpack(LU)
+    k = diag_block_kappa(L[:U.shape[0]], nb)
+    return max(k, diag_block_kappa(U, nb)) if upper else k
+
+
+def trsm_upper_ok(U, B, X, kappa_max):
+    """X^ = B inv(U) by trsm_right_upper_T (U v x v upper, B n x v):
+        ||X^ U - B||_F <= gamma_{v+1} (1 + 4 kappa_max) || |X^| |U| ||_F,
+    kappa_max over U's inverted nb x nb diagonal blocks.  The argument is the one of chol_backward_bound: each block of
+    X^ is a product with an inverse that has a componentwise error gamma_nb |inv(U_jj)| |U_jj| |inv(U_jj)| (Sec. 14.2),
+    the product adds gamma_nb, and the rank-nb updates gamma_v; moving the first two to the residual multiplies them by
+    kappa_2(U_jj), and the factor 2 over the first-order 2 kappa_max covers the second-order terms."""
+    U = np.triu(np.asarray(U, dtype=np.float64))
+    X = np.asarray(X, dtype=np.float64)
+    R = matmul(X, U) - np.asarray(B, dtype=np.float64).astype(LD)
+    M = np.abs(X) @ np.abs(U)
+    bound = gamma(U.shape[0] + 1) * (1.0 + 4.0 * kappa_max) * float(np.linalg.norm(M))
+    return bool(np.all(np.isfinite(X)) and float(np.sqrt(np.sum(R * R))) <= bound)
+
+
+def trsm_lower_unit_ok(L, R, Y, kappa_max):
+    """Y^ = inv(L) R by trsm_left_lower_unit (L v x v unit lower, R v x n): ||L Y^ - R||_F <= gamma_{v+1}
+    (1 + 4 kappa_max) || |L| |Y^| ||_F, kappa_max over L's inverted diagonal blocks (argument: trsm_upper_ok)"""
+    L = np.tril(np.asarray(L, dtype=np.float64), -1) + np.eye(np.asarray(L).shape[0])
+    Y = np.asarray(Y, dtype=np.float64)
+    Res = matmul(L, Y) - np.asarray(R, dtype=np.float64).astype(LD)
+    M = np.abs(L) @ np.abs(Y)
+    bound = gamma(L.shape[0] + 1) * (1.0 + 4.0 * kappa_max) * float(np.linalg.norm(M))
+    return bool(np.all(np.isfinite(Y)) and float(np.sqrt(np.sum(Res * Res))) <= bound)
 
 
 # ------------------------------------------------------------------------------------------------ test matrices
