@@ -15,7 +15,7 @@ import numpy as np
 
 from ._lib import ConfluxError, LIB_PATH, SYMBOLS, check, lib
 
-__all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "residual", "validate", "lu_solve", "lu_rcond", "lu_refine", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
+__all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "residual", "validate", "lu_solve", "lu_rcond", "lu_refine", "lu_equilibrate", "lu_svx", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
 
 
 def auto_grid(M, N, P):
@@ -249,6 +249,46 @@ def lu_refine(gv, B, X, trans=False, ferr=True):
     return X2.reshape(shape), (fe if ferr else None), be
 
 
+def lu_equilibrate(gv, apply=True, upload=True):
+    """LAPACK dgeequ (+ dlaqge when apply) on the padded input on the GPU grid.  upload=True first copies gv.data to the
+    device (cflx_lu_set_local), so that LU_rep(gv, upload=False) then factors the scaled matrix As, whose factors carry
+    the scaling to lu_svx.  Returns dict(r, c, rowcnd, colcnd, amax, equed, info) as dgeequ / dlaqge give them.
+    COLLECTIVE over gv.lu_comm; identical on every rank."""
+    if upload:
+        a = np.ascontiguousarray(gv.data, dtype=np.float64)
+        check(lib().cflx_lu_set_local(gv._h, a.ctypes.data), "lu_set_local")
+    r, c = np.zeros(gv.M), np.zeros(gv.M)
+    rowcnd, colcnd, amax, equed, info = (ctypes.c_double(), ctypes.c_double(), ctypes.c_double(), ctypes.c_char(),
+                                         ctypes.c_int())
+    check(lib().cflx_lu_equilibrate(gv._h, 1 if apply else 0, r.ctypes.data, c.ctypes.data, ctypes.byref(rowcnd),
+                                    ctypes.byref(colcnd), ctypes.byref(amax), ctypes.byref(equed), ctypes.byref(info)),
+          "lu_equilibrate")
+    return dict(r=r, c=c, rowcnd=rowcnd.value, colcnd=colcnd.value, amax=amax.value, equed=equed.value.decode(),
+                info=info.value)
+
+
+def lu_svx(gv, B, trans=False):
+    """LAPACK dgesvx with the factors of the last LU_rep and the scaling they carry (lu_equilibrate): solves A X = B (A^T
+    X = B when trans) with refinement.  Returns (X, dict(rcond, ferr, berr, rpvgrw, equed, info)); X is None when U has
+    an exactly zero pivot (info = k).  COLLECTIVE over gv.lu_comm; identical on every rank."""
+    B = np.asarray(B, dtype=np.float64)
+    if B.ndim not in (1, 2) or B.shape[0] != gv.M:
+        raise ValueError(f"lu_svx: B must have shape ({gv.M},) or ({gv.M}, nrhs), got {B.shape}")
+    B2 = np.ascontiguousarray(B.reshape(gv.M, -1))
+    nrhs = B2.shape[1]
+    X = np.empty_like(B2)
+    fe, be = np.empty(nrhs), np.empty(nrhs)
+    rcond, rpvgrw, equed, info = ctypes.c_double(), ctypes.c_double(), ctypes.c_char(), ctypes.c_int()
+    check(lib().cflx_lu_svx(gv._h, 1 if trans else 0, nrhs, B2.ctypes.data, nrhs, X.ctypes.data, nrhs, ctypes.byref(rcond),
+                            fe.ctypes.data, be.ctypes.data, ctypes.byref(rpvgrw), ctypes.byref(equed), ctypes.byref(info)),
+          "lu_svx")
+    k = info.value
+    solved = not (0 < k <= gv.M)
+    return (X.reshape(B.shape) if solved else None), dict(rcond=rcond.value, ferr=fe if solved else None,
+                                                          berr=be if solved else None, rpvgrw=rpvgrw.value,
+                                                          equed=equed.value.decode(), info=k)
+
+
 class cholesky:
     """Mirror of the reference's CONFCHOX driver interface (src/conflux/cholesky/Cholesky.h:20-22):
         initialize(N, v, grid, comm) -> object;  obj.parallelCholesky() -> ms;  obj.finalize().
@@ -320,6 +360,34 @@ class cholesky:
         check(lib().cflx_chol_refine(self._h, nrhs, B2.ctypes.data, nrhs, X2.ctypes.data, nrhs,
                                      fe.ctypes.data if ferr else None, be.ctypes.data), "chol_refine")
         return X2.reshape(shape), (fe if ferr else None), be
+
+    def equilibrate(self, apply=True, upload=True):
+        """LAPACK dpoequ (+ dlaqsy, lower, when apply) on the padded input on the GPU grid.  upload=True first copies
+        self.data to the device, so that parallelCholesky(upload=False) then factors the scaled matrix.  Returns dict(s,
+        scond, amax, equed, info).  COLLECTIVE; identical on every rank."""
+        if upload:
+            a = np.ascontiguousarray(self.data, dtype=np.float64)
+            check(lib().cflx_chol_set_local(self._h, a.ctypes.data), "chol_set_local")
+        s = np.zeros(self.N)
+        scond, amax, equed, info = ctypes.c_double(), ctypes.c_double(), ctypes.c_char(), ctypes.c_int()
+        check(lib().cflx_chol_equilibrate(self._h, 1 if apply else 0, s.ctypes.data, ctypes.byref(scond), ctypes.byref(amax),
+                                          ctypes.byref(equed), ctypes.byref(info)), "chol_equilibrate")
+        return dict(s=s, scond=scond.value, amax=amax.value, equed=equed.value.decode(), info=info.value)
+
+    def svx(self, B):
+        """LAPACK dposvx with the factor of the last parallelCholesky and the scaling it carries (equilibrate): returns
+        (X, dict(rcond, ferr, berr, equed, info)).  COLLECTIVE; identical on every rank."""
+        B = np.asarray(B, dtype=np.float64)
+        if B.ndim not in (1, 2) or B.shape[0] != self.N:
+            raise ValueError(f"cholesky.svx: B must have shape ({self.N},) or ({self.N}, nrhs), got {B.shape}")
+        B2 = np.ascontiguousarray(B.reshape(self.N, -1))
+        nrhs = B2.shape[1]
+        X = np.empty_like(B2)
+        fe, be = np.empty(nrhs), np.empty(nrhs)
+        rcond, equed, info = ctypes.c_double(), ctypes.c_char(), ctypes.c_int()
+        check(lib().cflx_chol_svx(self._h, nrhs, B2.ctypes.data, nrhs, X.ctypes.data, nrhs, ctypes.byref(rcond),
+                                  fe.ctypes.data, be.ctypes.data, ctypes.byref(equed), ctypes.byref(info)), "chol_svx")
+        return X.reshape(B.shape), dict(rcond=rcond.value, ferr=fe, berr=be, equed=equed.value.decode(), info=info.value)
 
     def finalize(self, clean=True):
         if self._h:
@@ -452,6 +520,32 @@ class dbg:
                                       int(grid[0]), int(grid[1]), int(pos[0]), int(pos[1]), nrhs, ptr(Xc), ptr(Xr),
                                       P.ctypes.data, Q.ctypes.data, int(reps), ctypes.byref(ms)), "dbg_residual")
         return P, Q, ms.value
+
+    @staticmethod
+    def equil(A, v, Kappa=None, grid=(1, 1), pos=(0, 0), M=None, r=None, c=None, equed="N", ncols=None):
+        """The per-share kernels of lu_equilibrate / cholesky.equilibrate / lu_svx on one layer-0 share A (Ml x Nl,
+        conflux layout of tile v at grid position pos of grid = (Px, Py)), over M global indices (default: the LU layout's
+        (Ml / v) Px v).  r, c: M-vectors (r is also the Cholesky's s; default ones).  Returns dict(rowmax, colmax, diag,
+        scaled, sym_scaled, growth, zero_pivot): the partial row maxima, the column maxima of |a| r, the diagonal of the
+        real tiles (global tile index < Kappa), the share after dlaqge's scaling for equed and after dlaqsy's, (max |a|
+        over global row <= column, max |a|) over the global columns < ncols (default M), and 1 + the first zero diagonal
+        entry (0: none)."""
+        A = np.ascontiguousarray(A, dtype=np.float64)
+        Ml, Nl = A.shape
+        Px, Py = (int(x) for x in grid)
+        M = int(M) if M is not None else (Ml // v) * Px * v
+        r = np.ascontiguousarray(np.ones(M) if r is None else r, dtype=np.float64)
+        c = np.ascontiguousarray(np.ones(M) if c is None else c, dtype=np.float64)
+        out = dict(rowmax=np.empty(M), colmax=np.empty(M), diag=np.empty(M), scaled=np.empty_like(A),
+                   sym_scaled=np.empty_like(A), growth=np.empty(2))
+        zp = ctypes.c_int()
+        check(lib().cflx_dbg_equil(Ml, Nl, int(v), int(Kappa if Kappa is not None else 1 << 30), Px, Py, int(pos[0]),
+                                   int(pos[1]), M, A.ctypes.data, r.ctypes.data, c.ctypes.data, equed.encode(),
+                                   int(ncols if ncols is not None else M), out["rowmax"].ctypes.data,
+                                   out["colmax"].ctypes.data, out["diag"].ctypes.data, out["scaled"].ctypes.data,
+                                   out["sym_scaled"].ctypes.data, out["growth"].ctypes.data, ctypes.byref(zp)), "dbg_equil")
+        out["zero_pivot"] = zp.value
+        return out
 
     @staticmethod
     def panel(P, reps=1):

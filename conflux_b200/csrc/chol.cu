@@ -44,6 +44,7 @@ struct cflx_chol {
     int64_t launches = 0;
     SubComm j_comm;                  // grid row of one layer (color pi * Pz + pk, key pj), made by the first solve
     SolveCache sv;                   // cflx_chol_solve: inv(L_jj) blocks forward, inv(L_jj)^T backward; rows of real tiles
+    EquilState eq;                   // cflx_chol_equilibrate / cflx_chol_svx (s is eq.*.r, scond eq.*.rowcnd)
 };
 
 namespace {
@@ -353,6 +354,7 @@ void free_chol(cflx_chol* ch) {
     cudaSetDevice(ch->comm->device);
     for (double* p : {ch->A0, ch->A11, ch->PT, ch->LT, ch->W, ch->G, ch->Bc, ch->D, ch->A00, ch->Uinv, ch->LinvT, ch->acc, ch->Q}) cudaFree(p);
     solve_cache_free(&ch->sv);
+    equil_free(&ch->eq);
     cudaFree(ch->info);
     if (ch->use_ozaki) ozaki_workspace_destroy(&ch->oz);
     if (ch->side) cudaStreamDestroy(ch->side);
@@ -797,6 +799,7 @@ int cflx_chol_set_local(cflx_chol* ch, const double* host_local) {
     ch->have_input = true;
     ch->factored = false;
     ch->sv.ready = false;
+    ch->eq.in.equed = 'N';
     return CFLX_OK;
 }
 
@@ -811,6 +814,7 @@ int cflx_chol_factor(cflx_chol* ch, double* ms_out) {
     cudaStream_t s = c->stream;
     CFLX_CUDA(cudaSetDevice(c->device));
     ch->sv.ready = false;
+    CFLX_TRY(equil_pass_on(&ch->eq, ch->N, false, s));  // the factor carries the input's scaling
     const int v = ch->v, Py = ch->Py, Ml = ch->Ml, Nl = ch->Nl;
     const int pj = ch->pj;
     CFLX_CUDA(cudaMemcpyAsync(ch->A11, ch->A0, (size_t)Ml * Nl * sizeof(double), cudaMemcpyDeviceToDevice, s));
@@ -1022,6 +1026,75 @@ int cflx_chol_refine(cflx_chol* ch, int nrhs, const double* B, int ldb, double* 
     const RefineOp op{ch->comm, ch->A0, ResidMode::SymLower, ch->N, ch->Ml, ch->Nl, ch->v, ch->Kappa, ch->Px, ch->Py,
                       ch->Pz, ch->pi, ch->pj, ch->pk, true, solve};
     return refine_run(&ch->sv.rf, op, nrhs, B, ldb, X, ldx, ferr_out, berr_out);
+}
+
+// COLLECTIVE.  LAPACK dpoequ (+ dlaqsy, UPLO = 'L', when apply) on the input A0 (equil.cu); drops the factorisation and
+// the solve cache, as cflx_chol_set_local does.
+int cflx_chol_equilibrate(cflx_chol* ch, int apply, double* s_out, double* scond_out, double* amax_out, char* equed_out,
+                          int* info_out) {
+    if (!ch || (apply != 0 && apply != 1) || !info_out) return CFLX_ERR_ARG;
+    if (!ch->have_input) {
+        set_last_error("cholesky equilibration requested before cflx_chol_set_local");
+        return CFLX_ERR_STATE;
+    }
+    if (apply && ch->eq.in.equed != 'N') {
+        set_last_error("cholesky equilibration refused: the input is already scaled (equed = 'Y'); upload it again first");
+        return CFLX_ERR_STATE;
+    }
+    CFLX_CUDA(cudaSetDevice(ch->comm->device));
+    ch->factored = false;
+    ch->sv.ready = false;
+    double scond = 0.0, amax = 0.0;
+    char equed = 'N';
+    int info = 0;
+    CFLX_TRY(poequ_grid(ch->comm, &ch->eq, ch->A0, ch->N, ch->Ml, ch->Nl, ch->v, ch->Kappa, ch->Px, ch->Py, ch->pi, ch->pj,
+                        ch->pk, apply != 0, s_out, &scond, &amax, &equed, &info));
+    // the input's record changes only when this call scaled it; a query (apply = 0) leaves the record and its scales
+    if (apply && info == 0)
+        CFLX_TRY(equil_record_set(&ch->eq.in, equed, scond, scond, ch->eq.qr, nullptr, ch->N, ch->comm->stream));
+    if (scond_out) *scond_out = scond;
+    if (amax_out) *amax_out = amax;
+    if (equed_out) *equed_out = equed;
+    *info_out = info;
+    return CFLX_OK;
+}
+
+// COLLECTIVE.  LAPACK dposvx after a successful factorisation, with the scaling the factor carries: B scaled by s,
+// dpocon, the solve, dporfs, X unscaled by s and ferr divided by scond.
+int cflx_chol_svx(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out,
+                  double* ferr_out, double* berr_out, char* equed_out, int* info_out) {
+    if (!ch || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B || !X || !rcond_out || !info_out) return CFLX_ERR_ARG;
+    if (!ch->factored) {
+        set_last_error("cholesky expert solve requested before a successful cflx_chol_factor, or after cflx_chol_set_local without one");
+        return CFLX_ERR_STATE;
+    }
+    CFLX_CUDA(cudaSetDevice(ch->comm->device));
+    cudaStream_t s = ch->comm->stream;
+    const EquilRecord& eq = ch->eq.fac;
+    const bool scaled = eq.equed == 'Y';
+    if (equed_out) *equed_out = eq.equed;
+    double rcond = 0.0;
+    CFLX_TRY(cflx_chol_rcond(ch, &rcond, nullptr));
+    *rcond_out = rcond;
+    const int N = ch->N, ldn = (int)round_up(nrhs, 8);
+    CFLX_TRY(equil_grow(&ch->eq, N, ldn));
+    double *dB = ch->eq.B, *dX = ch->eq.X;
+    CFLX_CUDA(cudaMemcpy2DAsync(dB, ldn * sizeof(double), B, (size_t)ldb * sizeof(double), nrhs * sizeof(double), N,
+                                cudaMemcpyDefault, s));
+    if (scaled) CFLX_TRY(launch_scale_rows(dB, ldn, N, nrhs, eq.r, s));
+    CFLX_TRY(cflx_chol_solve(ch, nrhs, dB, ldn, dX, ldn));
+    auto solve = [ch](bool, int n, const double* b, int lb, double* x, int lx) { return cflx_chol_solve(ch, n, b, lb, x, lx); };
+    const RefineOp op{ch->comm, ch->A0, ResidMode::SymLower, N, ch->Ml, ch->Nl, ch->v, ch->Kappa, ch->Px, ch->Py, ch->Pz,
+                      ch->pi, ch->pj, ch->pk, true, solve};
+    CFLX_TRY(refine_run(&ch->sv.rf, op, nrhs, dB, ldn, dX, ldn, ferr_out, berr_out));
+    if (scaled) CFLX_TRY(launch_scale_rows(dX, ldn, N, nrhs, eq.r, s));
+    CFLX_CUDA(cudaMemcpy2DAsync(X, (size_t)ldx * sizeof(double), dX, ldn * sizeof(double), nrhs * sizeof(double), N,
+                                cudaMemcpyDefault, s));
+    CFLX_CUDA(cudaStreamSynchronize(s));
+    if (ferr_out && scaled)
+        for (int j = 0; j < nrhs; ++j) ferr_out[j] /= eq.rowcnd;
+    *info_out = rcond < std::ldexp(1.0, -53) ? N + 1 : 0;
+    return CFLX_OK;
 }
 
 int cflx_chol_launch_count(cflx_chol* ch, int64_t* count_out, int reset) {

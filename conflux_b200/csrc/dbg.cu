@@ -2,12 +2,14 @@
 // They drive the SAME kernels the factorisation uses, with host buffers in and out, so that tests/ can check every
 // kernel in isolation against numpy / the oracle, and bench.py can time the dominant kernel alone.
 #include <algorithm>
+#include <climits>
 #include <limits>
 #include <vector>
 
 #include "../../include/conflux_b200.h"
 #include "common.cuh"
 #include "kernels.h"
+#include "lu_state.h"
 
 using namespace cflx;
 
@@ -293,6 +295,70 @@ int cflx_dbg_gemm_narrow_tn(int M, int N, int K, const double* AT, const double*
     double* out = alias ? dC.as<double>() : dT.as<double>();
     CFLX_TRY(run(out));
     if (D) CFLX_CUDA(cudaMemcpy(D, out, sizeof(double) * c_n, cudaMemcpyDeviceToHost));
+    CFLX_CUDA(cudaDeviceSynchronize());
+    return CFLX_OK;
+}
+
+// the per-share kernels of equilibration and of the pivot growth (equil.cu) on one layer-0 share at grid position
+// (pi, pj) of Px x Py; each output may be null
+int cflx_dbg_equil(int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, int M, const double* A,
+                   const double* r, const double* c, char equed, int ncols, double* rowmax_out, double* colmax_out,
+                   double* diag_out, double* scaled_out, double* sym_scaled_out, double* growth_out, int* zero_pivot_out) {
+    CFLX_TRY(check_device());
+    if (Ml < 0 || Nl < 0 || v < 1 || Ml % v || Nl % v || Px < 1 || Py < 1 || pi < 0 || pi >= Px || pj < 0 || pj >= Py ||
+        !A || !r || !c || M < (Ml / v) * Px * v || M < (Nl / v) * Py * v ||
+        (equed != 'N' && equed != 'R' && equed != 'C' && equed != 'B'))
+        return CFLX_ERR_ARG;
+    const size_t a_n = (size_t)Ml * Nl;
+    DevBuf dA, dW, dr, dc, dv, dg, dz;
+    CFLX_TRY(dA.alloc(sizeof(double) * a_n));
+    CFLX_TRY(dW.alloc(sizeof(double) * a_n));
+    CFLX_TRY(dr.alloc(sizeof(double) * M));
+    CFLX_TRY(dc.alloc(sizeof(double) * M));
+    CFLX_TRY(dv.alloc(sizeof(double) * M));
+    CFLX_TRY(dg.alloc(sizeof(double) * 2));
+    CFLX_TRY(dz.alloc(sizeof(int)));
+    CFLX_CUDA(cudaMemcpy(dA.p, A, sizeof(double) * a_n, cudaMemcpyHostToDevice));
+    CFLX_CUDA(cudaMemcpy(dr.p, r, sizeof(double) * M, cudaMemcpyHostToDevice));
+    CFLX_CUDA(cudaMemcpy(dc.p, c, sizeof(double) * M, cudaMemcpyHostToDevice));
+    const double* a = dA.as<double>();
+    double *w = dW.as<double>(), *vec = dv.as<double>();
+    auto vec_out = [&](double* out) -> int {
+        CFLX_CUDA(cudaMemcpy(out, vec, sizeof(double) * M, cudaMemcpyDeviceToHost));
+        return CFLX_OK;
+    };
+    if (rowmax_out) {
+        CFLX_TRY(equil_row_max(a, Ml, Nl, v, Px, pi, vec, M, 0));
+        CFLX_TRY(vec_out(rowmax_out));
+    }
+    if (colmax_out) {
+        CFLX_TRY(equil_col_max(a, Ml, Nl, v, Px, Py, pi, pj, dr.as<double>(), vec, M, 0));
+        CFLX_TRY(vec_out(colmax_out));
+    }
+    if (diag_out) {
+        CFLX_TRY(equil_diag(a, Ml, Nl, v, Kappa, Px, Py, pi, pj, vec, M, 0));
+        CFLX_TRY(vec_out(diag_out));
+    }
+    if (scaled_out) {
+        CFLX_CUDA(cudaMemcpy(w, a, sizeof(double) * a_n, cudaMemcpyDeviceToDevice));
+        CFLX_TRY(equil_apply(w, Ml, Nl, v, Px, Py, pi, pj, dr.as<double>(), dc.as<double>(), equed, 0));
+        CFLX_CUDA(cudaMemcpy(scaled_out, w, sizeof(double) * a_n, cudaMemcpyDeviceToHost));
+    }
+    if (sym_scaled_out) {  // s = r
+        CFLX_CUDA(cudaMemcpy(w, a, sizeof(double) * a_n, cudaMemcpyDeviceToDevice));
+        CFLX_TRY(equil_sym_apply(w, Ml, Nl, v, Kappa, Px, Py, pi, pj, dr.as<double>(), 0));
+        CFLX_CUDA(cudaMemcpy(sym_scaled_out, w, sizeof(double) * a_n, cudaMemcpyDeviceToHost));
+    }
+    if (growth_out) {  // the share is both L\U and the input
+        CFLX_TRY(equil_growth(a, a, Ml, Nl, v, Px, Py, pi, pj, ncols, dg.as<double>(), 0));
+        CFLX_CUDA(cudaMemcpy(growth_out, dg.p, sizeof(double) * 2, cudaMemcpyDeviceToHost));
+    }
+    if (zero_pivot_out) {
+        CFLX_TRY(equil_zero_pivot(a, Ml, Nl, v, M, Px, Py, pi, pj, dz.as<int>(), 0));
+        int z = 0;
+        CFLX_CUDA(cudaMemcpy(&z, dz.p, sizeof(int), cudaMemcpyDeviceToHost));
+        *zero_pivot_out = z == INT_MAX ? 0 : z;
+    }
     CFLX_CUDA(cudaDeviceSynchronize());
     return CFLX_OK;
 }

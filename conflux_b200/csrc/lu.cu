@@ -503,6 +503,7 @@ void free_lu(cflx_lu* lu) {
                    lu->idx_buf};
     for (int* p : ints) cudaFree(p);
     solve_cache_free(&lu->sv);
+    equil_free(&lu->eq);
     if (lu->h_npiv) cudaFreeHost(lu->h_npiv);
     if (lu->pws.slot_hdr) panel_workspace_destroy(&lu->pws);
     if (lu->use_ozaki) ozaki_workspace_destroy(&lu->oz);
@@ -887,6 +888,7 @@ int cflx_lu_set_local(cflx_lu* lu, const double* host_local) {
     lu->sv.ready = false;
     lu->a0_is_next = false;
     lu->next_host = nullptr;
+    lu->eq.in.equed = 'N';
     return CFLX_OK;
 }
 
@@ -928,6 +930,8 @@ int cflx_lu_factor(cflx_lu* lu, double* ms_out) {
     }
     lu->a0_is_next = false;
     lu->sv.ready = false;
+    // the factors carry the input's scaling; a queued next input arrives unscaled
+    CFLX_TRY(equil_pass_on(&lu->eq, lu->M, lu->next_host != nullptr, s));
     if (lu->next_host) {  // queued next input: overwrite A0 behind the working copy, concurrently with everything below
         CFLX_CUDA(cudaEventRecord(lu->ev_a0_read, s));
         CFLX_CUDA(cudaStreamWaitEvent(lu->copy, lu->ev_a0_read, 0));
@@ -1140,6 +1144,108 @@ int cflx_lu_refine(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, d
     const RefineOp op{lu->comm, lu->A0, t ? ResidMode::TN : ResidMode::NN, lu->M, lu->Ml, lu->Nl, lu->v, lu->Nt, lu->Px,
                       lu->Py, lu->Pz, lu->pi, lu->pj, lu->pk, false, solve};
     return refine_run(&lu->sv.rf, op, nrhs, B, ldb, X, ldx, ferr_out, berr_out);
+}
+
+// COLLECTIVE.  LAPACK dgeequ (+ dlaqge when apply) on the input A0 (equil.cu).  The input changes, so the factorisation
+// and the solve cache are dropped, as by cflx_lu_set_local.
+int cflx_lu_equilibrate(cflx_lu* lu, int apply, double* r_out, double* c_out, double* rowcnd_out, double* colcnd_out,
+                        double* amax_out, char* equed_out, int* info_out) {
+    if (!lu || (apply != 0 && apply != 1) || !info_out) return CFLX_ERR_ARG;
+    if (!lu->have_input) {
+        set_last_error("equilibration requested before cflx_lu_set_local");
+        return CFLX_ERR_STATE;
+    }
+    if (apply && lu->eq.in.equed != 'N') {
+        set_last_error("equilibration refused: the input is already scaled (equed = '%c'); upload it again first",
+                       lu->eq.in.equed);
+        return CFLX_ERR_STATE;
+    }
+    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    cudaStream_t s = lu->comm->stream;
+    if (lu->a0_is_next) CFLX_CUDA(cudaStreamWaitEvent(s, lu->ev_upload, 0));  // A0 holds a streamed next input
+    lu->factored = false;
+    lu->sv.ready = false;
+    double rowcnd = 0.0, colcnd = 0.0, amax = 0.0;
+    char equed = 'N';
+    int info = 0;
+    CFLX_TRY(geequ_grid(lu->comm, &lu->eq, lu->A0, lu->M, lu->Ml, lu->Nl, lu->v, lu->Px, lu->Py, lu->pi, lu->pj, lu->pk,
+                        apply != 0, r_out, c_out, &rowcnd, &colcnd, &amax, &equed, &info));
+    // the input's record changes only when this call scaled it; a query (apply = 0) leaves the record and its scales
+    if (apply && info == 0) CFLX_TRY(equil_record_set(&lu->eq.in, equed, rowcnd, colcnd, lu->eq.qr, lu->eq.qc, lu->M, s));
+    if (rowcnd_out) *rowcnd_out = rowcnd;
+    if (colcnd_out) *colcnd_out = colcnd;
+    if (amax_out) *amax_out = amax;
+    if (equed_out) *equed_out = equed;
+    *info_out = info;
+    return CFLX_OK;
+}
+
+// COLLECTIVE.  LAPACK dgesvx after the factorisation, with the scaling the factors carry: B scaled, the reciprocal pivot
+// growth and the first zero pivot, rcond (1-norm for trans 0, infinity-norm for trans 1), the solve, dgerfs, X unscaled.
+int cflx_lu_svx(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out,
+                double* ferr_out, double* berr_out, double* rpvgrw_out, char* equed_out, int* info_out) {
+    if (!lu || (trans != 0 && trans != 1) || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B || !X || !rcond_out || !info_out)
+        return CFLX_ERR_ARG;
+    if (!lu->factored) {
+        set_last_error("expert solve requested before cflx_lu_factor, or after cflx_lu_set_local without a factorisation");
+        return CFLX_ERR_STATE;
+    }
+    if (lu->a0_is_next) {
+        set_last_error("expert solve refused: the input buffer of the last run was handed to the queued next matrix");
+        return CFLX_ERR_STATE;
+    }
+    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    cudaStream_t s = lu->comm->stream;
+    const bool t = trans != 0;
+    const EquilRecord& eq = lu->eq.fac;
+    const bool rowequ = eq.equed == 'R' || eq.equed == 'B', colequ = eq.equed == 'C' || eq.equed == 'B';
+    if (equed_out) *equed_out = eq.equed;
+    if (!lu->sv.ready) CFLX_TRY(lu_solve_prepare(lu));
+    double rpvgrw = 1.0;
+    int info = 0;
+    CFLX_TRY(pivot_growth_grid(lu->comm, &lu->eq, lu->Cbuf, lu->A0, lu->M, lu->Ml, lu->Nl, lu->v, lu->Px, lu->Py, lu->pi,
+                               lu->pj, lu->pk, &rpvgrw, &info));
+    if (rpvgrw_out) *rpvgrw_out = rpvgrw;
+    *info_out = info;
+    if (info > 0) {  // exactly singular U: no solution
+        *rcond_out = 0.0;
+        return CFLX_OK;
+    }
+    // dgecon with NORM = '1' (trans 0, as cflx_lu_rcond) or 'I' (trans 1: the two kinds of product swap)
+    double anorm = 0.0, ainvnm = 0.0;
+    if (!t) CFLX_TRY(norm1_grid(lu->comm, lu->A0, lu->M, lu->Ml, lu->Nl, lu->v, lu->Nt, lu->Px, lu->Py, lu->pi, lu->pj,
+                                lu->pk, false, &anorm));
+    else CFLX_TRY(norminf_grid(lu->comm, lu->A0, lu->M, lu->Ml, lu->Nl, lu->v, lu->Px, lu->pi, lu->pk, &anorm));
+    if (anorm > 0.0) {
+        auto apply = [&](int kase, double* x) { return lu_sweeps(lu, (kase == 2) != t, true, 1, x, 1, x, 1); };
+        CFLX_TRY(estimate_inv_norm1(lu->M, apply, &ainvnm));
+    }
+    const double rcond = rcond_from(anorm, ainvnm);
+    *rcond_out = rcond;
+    // B scaled on the device, solved and refined there, X unscaled before the download
+    const int M = lu->M, ldn = (int)round_up(nrhs, 8);
+    CFLX_TRY(equil_grow(&lu->eq, M, ldn));
+    double *dB = lu->eq.B, *dX = lu->eq.X;
+    CFLX_CUDA(cudaMemcpy2DAsync(dB, ldn * sizeof(double), B, (size_t)ldb * sizeof(double), nrhs * sizeof(double), M,
+                                cudaMemcpyDefault, s));
+    if (!t && rowequ) CFLX_TRY(launch_scale_rows(dB, ldn, M, nrhs, eq.r, s));
+    if (t && colequ) CFLX_TRY(launch_scale_rows(dB, ldn, M, nrhs, eq.c, s));
+    CFLX_TRY(lu_sweeps(lu, t, false, nrhs, dB, ldn, dX, ldn));
+    auto solve = [lu, t](bool tk, int n, const double* b, int lb, double* x, int lx) {
+        return lu_sweeps(lu, t != tk, false, n, b, lb, x, lx);
+    };
+    const RefineOp op{lu->comm, lu->A0, t ? ResidMode::TN : ResidMode::NN, M, lu->Ml, lu->Nl, lu->v, lu->Nt, lu->Px,
+                      lu->Py, lu->Pz, lu->pi, lu->pj, lu->pk, false, solve};
+    CFLX_TRY(refine_run(&lu->sv.rf, op, nrhs, dB, ldn, dX, ldn, ferr_out, berr_out));
+    if (!t && colequ) CFLX_TRY(launch_scale_rows(dX, ldn, M, nrhs, eq.c, s));
+    if (t && rowequ) CFLX_TRY(launch_scale_rows(dX, ldn, M, nrhs, eq.r, s));
+    CFLX_CUDA(cudaMemcpy2DAsync(X, (size_t)ldx * sizeof(double), dX, ldn * sizeof(double), nrhs * sizeof(double), M,
+                                cudaMemcpyDefault, s));
+    CFLX_CUDA(cudaStreamSynchronize(s));
+    if (ferr_out && ((!t && colequ) || (t && rowequ)))
+        for (int j = 0; j < nrhs; ++j) ferr_out[j] /= t ? eq.rowcnd : eq.colcnd;
+    if (rcond < std::ldexp(1.0, -53)) *info_out = M + 1;
+    return CFLX_OK;
 }
 
 int cflx_host_alloc(size_t bytes, void** out) {

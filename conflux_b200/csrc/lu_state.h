@@ -79,6 +79,35 @@ struct RefineCache {
     size_t cap_m = 0, cap_c = 0, cap_r = 0, cap_part = 0, cap_all = 0, cap_berr = 0, cap_active = 0;
 };
 
+// ---------------------------------------------------------------- equilibration and the expert drivers (equil.cu)
+// The scaling an input carries (cflx_*_equilibrate), and the one the factors of that input carry on to cflx_*_svx:
+// equed 'N' (none), 'R', 'C', 'B' (LU) or 'Y' (Cholesky); r / c: the row and column scales on the device (M each, every
+// rank; the Cholesky's s is r), with rowcnd / colcnd (the Cholesky's scond is rowcnd).  Each record owns its scales:
+// nothing but equil_record_set writes them.
+struct EquilRecord {
+    char equed = 'N';
+    double rowcnd = 1.0, colcnd = 1.0;
+    double *r = nullptr, *c = nullptr;  // cap doubles each
+    size_t cap = 0;
+};
+// The records of the input and of the factors, the results of the last equilibrate call (which change no record unless
+// that call scaled the input), and the device work buffers of svx.  Buffers are grown, never shrunk.
+struct EquilState {
+    EquilRecord in, fac;
+    double *qr = nullptr, *qc = nullptr;  // the last call's scales (dgeequ's r, c; dpoequ's s in qr): qcap doubles each
+    size_t qcap = 0;
+    double *B = nullptr, *X = nullptr;    // svx: M x ldn each, cap doubles each
+    size_t cap = 0;
+    double* growth = nullptr;             // 2 doubles: max |triu(U)|, max |A|
+    int* ival = nullptr;                  // 1 int: the first zero pivot
+};
+void equil_free(EquilState* e);
+// *dst = {equed, rowcnd, colcnd} with device copies of r and c (n each; c may be null: then only r is kept)
+int equil_record_set(EquilRecord* dst, char equed, double rowcnd, double colcnd, const double* r, const double* c, int n,
+                     cudaStream_t s);
+// in -> fac; then, when `next_is_plain`, in becomes 'N' (a streamed next input)
+int equil_pass_on(EquilState* e, int M, bool next_is_plain, cudaStream_t s);
+
 // What a solve keeps between calls: prepared by the first solve after a factorisation, dropped (ready = false) by
 // set_local / factor, freed with the object.  The work buffers have ldn columns and are grown, never shrunk.
 struct SolveCache {
@@ -167,6 +196,7 @@ struct cflx_lu {
     cudaStream_t side = nullptr;  // high-priority look-ahead stream (null: no overlap)
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_npiv = nullptr;
     cflx::SolveCache sv;  // cflx_lu_solve: Linv blocks forward, Uinv blocks backward; rows: row of B of each row of P*B
+    cflx::EquilState eq;  // cflx_lu_equilibrate / cflx_lu_svx
 };
 
 namespace cflx {
@@ -241,9 +271,53 @@ struct RefineOp {
     bool symmetric;
     std::function<int(bool, int, const double*, int, double*, int)> solve;
 };
-// LAPACK dgerfs / dporfs on the grid (collective): X (host, M x nrhs, ldx) refined in place, ferr (may be null: no
-// estimator) and berr (may be null) per column.  Every column runs LAPACK's own decisions, all in lockstep.
+// LAPACK dgerfs / dporfs on the grid (collective): X (host or device, M x nrhs, ldx) refined in place from B (host or
+// device), ferr (may be null: no estimator) and berr (may be null) per column.  Every column runs LAPACK's own decisions, all in lockstep.
 int refine_run(RefineCache* rc, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx, double* ferr,
                double* berr);
 void refine_cache_free(RefineCache* rc);
+
+// norm.cu: the collective infinity-norm (maximum row sum) of the M x M matrix whose layer-0 shares are A (every local
+// entry counts), into *anorm (every rank).  Deterministic: no floating-point atomics.
+int norminf_grid(cflx_comm* c, const double* A, int M, int Ml, int Nl, int v, int Px, int pi, int pk, double* anorm);
+
+// equil.cu.  Per-share kernels (layer 0's share A, Ml x Nl, conflux layout); each writes an M-vector indexed by global
+// row / column with zeros where this share holds nothing:
+//   rowmax[g] = max |a_gj| over this share's row g;  colmax[g] = max |a_ig| r_i over this share's column g;
+//   diag[g] = a_gg where this share holds the diagonal entry (real tiles, global tile index < Kappa).
+// The apply passes scale A in place: equed 'R' a_ij = r_i a_ij, 'C' c_j a_ij, 'B' (c_j r_i) a_ij, over every local entry;
+// sym_apply: (s_j s_i) a_ij over the stored lower triangle of the real tiles only.
+int equil_row_max(const double* A, int Ml, int Nl, int v, int Px, int pi, double* rowmax, int M, cudaStream_t s);
+int equil_col_max(const double* A, int Ml, int Nl, int v, int Px, int Py, int pi, int pj, const double* r, double* colmax,
+                  int M, cudaStream_t s);
+int equil_diag(const double* A, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, double* diag, int M,
+               cudaStream_t s);
+int equil_apply(double* A, int Ml, int Nl, int v, int Px, int Py, int pi, int pj, const double* r, const double* c,
+                char equed, cudaStream_t s);
+int equil_sym_apply(double* A, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, const double* sc,
+                    cudaStream_t s);
+// On a share F of L\U (and A of the input): *zero_pivot = min(1 + g) over the global diagonal entries g < M the share
+// holds with F_gg == 0 (INT_MAX: none); out2 = {max |F| over global row <= global column, max |A|}, both over the global
+// columns < ncols (zeros where the share holds none).
+int equil_zero_pivot(const double* F, int Ml, int Nl, int v, int M, int Px, int Py, int pi, int pj, int* zero_pivot,
+                     cudaStream_t s);
+int equil_growth(const double* F, const double* A, int Ml, int Nl, int v, int Px, int Py, int pi, int pj, int ncols,
+                 double* out2, cudaStream_t s);
+// LAPACK dgeequ (+ dlaqge when `apply`) on the grid, COLLECTIVE: the scales into e->qr / e->qc (no record changes) and
+// the host results; r_out / c_out (M, may be null).  Scales are applied only when info == 0.
+int geequ_grid(cflx_comm* c, EquilState* e, double* A, int M, int Ml, int Nl, int v, int Px, int Py, int pi, int pj,
+               int pk, bool apply, double* r_out, double* c_out, double* rowcnd, double* colcnd, double* amax,
+               char* equed, int* info);
+// LAPACK dpoequ (+ dlaqsy, UPLO = 'L', when `apply`) on the grid, COLLECTIVE: s into e->qr (no record changes)
+int poequ_grid(cflx_comm* c, EquilState* e, double* A, int N, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi,
+               int pj, int pk, bool apply, double* s_out, double* scond, double* amax, char* equed, int* info);
+// dgesvx's reciprocal pivot growth on the grid, COLLECTIVE: F is L\U and A the input (both layer-0 shares of the M x M
+// matrix).  info = 1 + the first global k with U(k,k) == 0 (0: none); rpvgrw = max |A| / max |triu(U)| over the global
+// columns < (info ? info : M), or 1 when the denominator is 0.
+int pivot_growth_grid(cflx_comm* c, EquilState* e, const double* F, const double* A, int M, int Ml, int Nl, int v, int Px,
+                      int Py, int pi, int pj, int pk, double* rpvgrw, int* info);
+// the svx work buffers for nrhs columns (ldn = round_up(nrhs, 8)): e->B and e->X, M x ldn
+int equil_grow(EquilState* e, int M, int ldn);
+// X[i][j] *= d[i] for i < M, j < n (ld), on the device
+int launch_scale_rows(double* X, int64_t ld, int M, int n, const double* d, cudaStream_t s);
 }  // namespace cflx

@@ -92,7 +92,48 @@ __global__ void column_sums_kernel(const double* __restrict__ colp, int ncp, con
     }
     out[g] = s + sc;
 }
+// out[g] = the sum of |a| over local row r (global row g) of this share: one warp per row, each lane a compensated sum
+// over the columns lane, lane + 32, ..., then the same shuffle tree as the row sums above
+__global__ void row_abs_sums_kernel(const double* __restrict__ A, int Ml, int Nl, int v, int Px, int pi,
+                                    double* __restrict__ out) {
+    const int r = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (r >= Ml) return;
+    const double* a = A + (int64_t)r * Nl;
+    double t = 0.0, tc = 0.0;
+    for (int c = lane; c < Nl; c += 32) acc(t, tc, fabs(a[c]));
+    for (int o = 16; o > 0; o >>= 1) {
+        const double u = __shfl_xor_sync(0xffffffffu, t, o), uc = __shfl_xor_sync(0xffffffffu, tc, o);
+        tc += uc;
+        acc(t, tc, u);
+    }
+    if (lane == 0) out[((r / v) * Px + pi) * v + r % v] = t + tc;
+}
 }  // namespace
+
+int norminf_grid(cflx_comm* c, const double* A, int M, int Ml, int Nl, int v, int Px, int pi, int pk, double* anorm) {
+    cudaStream_t s = c->stream;
+    double* out = nullptr;
+    CFLX_TRY(dmalloc(&out, (size_t)M));
+    std::vector<double> h(M);
+    auto run = [&]() -> int {
+        CFLX_CUDA(cudaMemsetAsync(out, 0, sizeof(double) * M, s));
+        if (pk == 0 && Ml > 0) {  // only layer 0 holds the input
+            row_abs_sums_kernel<<<(Ml + 7) / 8, 256, 0, s>>>(A, Ml, Nl, v, Px, pi, out);
+            CFLX_CUDA(cudaGetLastError());
+        }
+        if (c->world_size > 1) CFLX_NCCL(ncclAllReduce(out, out, (size_t)M, ncclDouble, ncclSum, c->world, s));
+        CFLX_CUDA(cudaMemcpyAsync(h.data(), out, sizeof(double) * M, cudaMemcpyDeviceToHost, s));
+        CFLX_CUDA(cudaStreamSynchronize(s));
+        return CFLX_OK;
+    };
+    const int rc = run();
+    cudaFree(out);
+    if (rc) return rc;
+    double m = 0.0;
+    for (double x : h) m = std::isnan(x) ? x : std::max(m, x);  // dlange: a NaN row sum is the norm
+    *anorm = m;
+    return CFLX_OK;
+}
 
 int norm1_grid(cflx_comm* c, const double* A, int M, int Ml, int Nl, int v, int Nt, int Px, int Py, int pi, int pj,
                int pk, bool lower_sym, double* anorm) {

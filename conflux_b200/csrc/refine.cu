@@ -554,9 +554,9 @@ int refine_run(RefineCache* rc, const RefineOp& op, int nrhs, const double* B, i
     CFLX_CUDA(cudaMemsetAsync(rc->X, 0, sizeof(double) * mat, s));
     CFLX_CUDA(cudaMemsetAsync(rc->B, 0, sizeof(double) * mat, s));
     CFLX_CUDA(cudaMemcpy2DAsync(rc->X, ldn * sizeof(double), X, (size_t)ldx * sizeof(double), nrhs * sizeof(double), M,
-                                cudaMemcpyHostToDevice, s));
+                                cudaMemcpyDefault, s));
     CFLX_CUDA(cudaMemcpy2DAsync(rc->B, ldn * sizeof(double), B, (size_t)ldb * sizeof(double), nrhs * sizeof(double), M,
-                                cudaMemcpyHostToDevice, s));
+                                cudaMemcpyDefault, s));
 
     const double eps = std::ldexp(1.0, -53), safmin = std::ldexp(1.0, -1022);
     const double nz = (double)M + 1.0, safe1 = nz * safmin, safe2 = safe1 / eps;
@@ -668,7 +668,9 @@ int refine_run(RefineCache* rc, const RefineOp& op, int nrhs, const double* B, i
             ferr[j] = xmax != 0.0 ? est[j].est / xmax : est[j].est;
         }
     }
-    for (int i = 0; i < M; ++i) std::memcpy(X + (size_t)i * ldx, hX.data() + (size_t)i * ldn, sizeof(double) * nrhs);
+    CFLX_CUDA(cudaMemcpy2DAsync(X, (size_t)ldx * sizeof(double), rc->X, ldn * sizeof(double), nrhs * sizeof(double), M,
+                                cudaMemcpyDefault, s));
+    CFLX_CUDA(cudaStreamSynchronize(s));
     if (berr_out) std::copy(col_berr.begin(), col_berr.end(), berr_out);
     return CFLX_OK;
 }

@@ -109,5 +109,25 @@ inline void choleskyRefine(int nrhs, const double* B, int ldb, double* X, int ld
     if (!s.plan) throw CholeskyException("choleskyRefine() before initialize()");
     chol_detail::check(cflx_chol_refine(s.plan, nrhs, B, ldb, X, ldx, ferr, berr), "choleskyRefine");
 }
+// LAPACK dpoequ (+ dlaqsy, lower, when apply) on the input the device holds (cflx_chol_equilibrate, collective); s
+// (matrix_size()) may be null.  Returns info (0, or the first non-positive diagonal entry); equed is 'N' or 'Y'.
+inline int choleskyEquilibrate(bool apply = true, double* s_out = nullptr, double* scond = nullptr, double* amax = nullptr,
+                               char* equed = nullptr) {
+    auto& s = chol_detail::state();
+    if (!s.plan) throw CholeskyException("choleskyEquilibrate() before initialize()");
+    int info = 0;
+    chol_detail::check(cflx_chol_equilibrate(s.plan, apply ? 1 : 0, s_out, scond, amax, equed, &info), "choleskyEquilibrate");
+    return info;
+}
+// LAPACK dposvx after parallelCholesky(), with the scaling the factor carries (cflx_chol_svx, collective); ferr / berr /
+// equed may be null.  Returns info (0, or N + 1 when rcond < 2^-53).
+inline int choleskySvx(int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond, double* ferr = nullptr,
+                       double* berr = nullptr, char* equed = nullptr) {
+    auto& s = chol_detail::state();
+    if (!s.plan) throw CholeskyException("choleskySvx() before initialize()");
+    int info = 0;
+    chol_detail::check(cflx_chol_svx(s.plan, nrhs, B, ldb, X, ldx, rcond, ferr, berr, equed, &info), "choleskySvx");
+    return info;
+}
 
 }  // namespace conflux

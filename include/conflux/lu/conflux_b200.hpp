@@ -282,4 +282,27 @@ void LU_refine(lu_params<T>& gv, int nrhs, const T* B, int ldb, T* X, int ldx, d
     check(cflx_lu_refine(gv.plan, transposed ? 1 : 0, nrhs, B, ldb, X, ldx, ferr, berr), "LU_refine");
 }
 
+// LAPACK dgeequ (+ dlaqge when apply) on the input the device holds (cflx_lu_equilibrate, collective): the next LU_rep
+// with the input already on the device factors the scaled matrix, and LU_svx uses the scaling.  r / c (M each) may be
+// null.  Returns info (0, the first zero row, or M + the first zero column); equed is 'N', 'R', 'C' or 'B'.
+template <class T>
+int LU_equilibrate(lu_params<T>& gv, bool apply = true, T* r = nullptr, T* c = nullptr, double* rowcnd = nullptr,
+                   double* colcnd = nullptr, double* amax = nullptr, char* equed = nullptr) {
+    int info = 0;
+    check(cflx_lu_equilibrate(gv.plan, apply ? 1 : 0, r, c, rowcnd, colcnd, amax, equed, &info), "LU_equilibrate");
+    return info;
+}
+
+// LAPACK dgesvx after LU_rep, with the scaling the factors carry (cflx_lu_svx, collective): X (M x nrhs) solves A X = B
+// (A^T X = B when transposed) with refinement; ferr / berr / rpvgrw / equed may be null.  Returns info (0; k for an
+// exactly zero U(k,k), X not written; M + 1 when rcond < 2^-53).
+template <class T>
+int LU_svx(lu_params<T>& gv, int nrhs, const T* B, int ldb, T* X, int ldx, double* rcond, double* ferr = nullptr,
+           double* berr = nullptr, double* rpvgrw = nullptr, char* equed = nullptr, bool transposed = false) {
+    int info = 0;
+    check(cflx_lu_svx(gv.plan, transposed ? 1 : 0, nrhs, B, ldb, X, ldx, rcond, ferr, berr, rpvgrw, equed, &info),
+          "LU_svx");
+    return info;
+}
+
 }  // namespace conflux

@@ -122,6 +122,31 @@ int cflx_lu_rcond(cflx_lu*, double* rcond_out, double* anorm_out);
  * factors, the permutation, the input, later solves and the launch count as they are. */
 int cflx_lu_refine(cflx_lu*, int trans, int nrhs, const double* B, int ldb, double* X, int ldx, double* ferr_out,
                    double* berr_out);
+/* COLLECTIVE.  LAPACK dgeequ on the input the device holds (the padded M x M matrix of cflx_lu_set_local), and with
+ * apply = 1 dlaqge: the input is scaled in place, a_ij = (c_j r_i) a_ij (only r or only c for equed 'R' / 'C'), when
+ * rowcnd < 0.1, colcnd < 0.1 or amax is outside [dlamch('S') / dlamch('P'), its reciprocal].  r_out / c_out (M doubles,
+ * may be NULL): the row and column scales; rowcnd_out, colcnd_out, amax_out (may be NULL) as dgeequ; equed_out (may be
+ * NULL): 'N', 'R', 'C' or 'B' ('N' when apply = 0).  info_out: 0, i for the first zero row i, M + j for the first zero
+ * column j (1-based; the scales are then not applied, and r_out holds the row maxima as dgeequ leaves them).  The
+ * factorisation and the solve cache are dropped, as by cflx_lu_set_local; the next cflx_lu_factor factors the scaled
+ * matrix and its factors carry the scaling to cflx_lu_svx; cflx_lu_validate, _rcond and _refine then refer to the scaled
+ * matrix.  An input from cflx_lu_set_local or a queued upload carries no scaling; apply = 0 on an input that is already
+ * scaled is a query of the scaled matrix and leaves the scaling it carries as it was.  Identical results on every rank.
+ * CFLX_ERR_ARG for apply not 0 / 1 or a NULL info_out; CFLX_ERR_STATE before cflx_lu_set_local, and for apply = 1 on an
+ * input that is already scaled. */
+int cflx_lu_equilibrate(cflx_lu*, int apply, double* r_out, double* c_out, double* rowcnd_out, double* colcnd_out,
+                        double* amax_out, char* equed_out, int* info_out);
+/* COLLECTIVE.  LAPACK dgesvx after the factorisation (FACT = 'F' on this library's factors, with the scaling they carry
+ * from cflx_lu_equilibrate): trans 0: A X = B, 1: A^T X = B.  B is scaled by r (trans 0, equed R / B) or c (trans 1,
+ * equed C / B); rpvgrw_out (may be NULL) = max |A_s| / max |triu(U)|, or 1 when the latter is 0; rcond_out = dgecon of the
+ * scaled matrix in the 1-norm (trans 0, the bits of cflx_lu_rcond) or the infinity-norm (trans 1); X is solved, refined
+ * as cflx_lu_refine refines it (ferr_out / berr_out, nrhs doubles each, may be NULL), and unscaled by c (trans 0) or r
+ * (trans 1), ferr divided by colcnd or rowcnd.  equed_out (may be NULL): the factors' scaling.  info_out: k when U(k,k)
+ * is exactly zero (the first such k; rcond = 0, rpvgrw over the leading k columns, X not written); M + 1 when rcond <
+ * 2^-53 (X is still computed); 0 otherwise.  B, X, ldb, ldx as cflx_lu_refine; results identical on every rank.
+ * CFLX_ERR_ARG as cflx_lu_refine and for a NULL rcond_out or info_out; CFLX_ERR_STATE as cflx_lu_rcond. */
+int cflx_lu_svx(cflx_lu*, int trans, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out,
+                double* ferr_out, double* berr_out, double* rpvgrw_out, char* equed_out, int* info_out);
 /* 1 when this plan's trailing update runs on the int8 wgmma digit-plane path (ozaki.cu), 0 for the FP64 DMMA kernel
  * (gemm.cu) */
 int cflx_lu_uses_ozaki(const cflx_lu*);
@@ -184,6 +209,20 @@ int cflx_chol_rcond(cflx_chol*, double* rcond_out, double* anorm_out);
  * (its lower triangle); the arguments and results of cflx_lu_refine without trans.  CFLX_ERR_STATE as cflx_chol_solve. */
 int cflx_chol_refine(cflx_chol*, int nrhs, const double* B, int ldb, double* X, int ldx, double* ferr_out,
                      double* berr_out);
+/* COLLECTIVE.  LAPACK dpoequ on the input the device holds, and with apply = 1 dlaqsy (UPLO = 'L'): s_i = 1 / sqrt(a_ii),
+ * scond = sqrt(min a_ii) / sqrt(max a_ii), amax = max a_ii; the stored lower triangle of the real tiles is scaled in
+ * place, a_ij = (s_j s_i) a_ij, when scond < 0.1 or amax is outside [dlamch('S') / dlamch('P'), its reciprocal].
+ * s_out (N doubles), scond_out, amax_out, equed_out ('N' or 'Y') may be NULL.  info_out: i for the first a_ii <= 0
+ * (1-based; s_out then holds the diagonal and nothing is scaled), else 0.  State rules and the scaling record as
+ * cflx_lu_equilibrate. */
+int cflx_chol_equilibrate(cflx_chol*, int apply, double* s_out, double* scond_out, double* amax_out, char* equed_out,
+                          int* info_out);
+/* COLLECTIVE.  LAPACK dposvx after a successful factorisation, with the scaling the factor carries: B scaled by s,
+ * rcond_out = dpocon of the scaled matrix (the bits of cflx_chol_rcond), X solved, refined as cflx_chol_refine refines it
+ * and unscaled by s, ferr divided by scond.  info_out: N + 1 when rcond < 2^-53 (X is still computed), else 0.
+ * Arguments as cflx_chol_refine; CFLX_ERR_ARG also for a NULL rcond_out or info_out; CFLX_ERR_STATE as cflx_chol_solve. */
+int cflx_chol_svx(cflx_chol*, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out, double* ferr_out,
+                  double* berr_out, char* equed_out, int* info_out);
 /* number of kernels this object counted since the last reset (bench.py's gpu_launches); cflx_chol_solve adds none */
 int cflx_chol_launch_count(cflx_chol*, int64_t* count_out, int reset);
 void cflx_chol_destroy(cflx_chol*);
@@ -213,6 +252,18 @@ int cflx_dbg_gemm_narrow_tn(int M, int N, int K, const double* AT, const double*
  * the mode does not read it).  P_out / Q_out: nrhs columns.  ms_out: mean device time of one launch over reps. */
 int cflx_dbg_residual(int mode, int Ml, int Nl, const double* A, int v, int Kappa, int Px, int Py, int pi, int pj,
                       int nrhs, const double* Xc, const double* Xr, double* P_out, double* Q_out, int reps, double* ms_out);
+/* the per-share kernels of cflx_*_equilibrate and cflx_lu_svx on one layer-0 share A (Ml x Nl row-major, conflux layout of
+ * tile v at grid position (pi, pj) of Px x Py; Ml, Nl multiples of v; M >= (Ml / v) Px v and >= (Nl / v) Py v global
+ * indices).  r, c: M-vectors (r is also the Cholesky's s).  Each output may be NULL:
+ *   rowmax_out / colmax_out (M): max |a| by global row, max |a| r_i by global column, zeros where the share holds none;
+ *   diag_out (M): a_gg on the share's diagonal tiles with a global tile index < Kappa, zeros elsewhere;
+ *   scaled_out (Ml x Nl): the share after dlaqge's scaling for equed ('N', 'R', 'C', 'B');
+ *   sym_scaled_out (Ml x Nl): the share after dlaqsy's (s_j s_i) a on the real tiles' lower triangle, the rest untouched;
+ *   growth_out[2]: {max |a| over global row <= column, max |a|}, both over global columns < ncols (the share read as both
+ *   L\U and the input); zero_pivot_out: 1 + the first global g < M on the share's diagonal with a_gg == 0, or 0. */
+int cflx_dbg_equil(int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, int M, const double* A,
+                   const double* r, const double* c, char equed, int ncols, double* rowmax_out, double* colmax_out,
+                   double* diag_out, double* scaled_out, double* sym_scaled_out, double* growth_out, int* zero_pivot_out);
 /* partial-pivot LU of an n x v row-major panel: perm_out[v], A00_out[v*v] (L00\U00), LU_out[n*v] rows unpermuted */
 int cflx_dbg_panel(int n, int v, const double* panel, int* perm_out, double* A00_out, double* LU_out, int reps,
                    double* ms_out);
