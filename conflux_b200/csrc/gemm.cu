@@ -28,12 +28,23 @@ constexpr int BK = 16, STAGES = 4;
 // Register budget: ptxas sizes registers for the worst SM sub-partition, which holds 3 of the 9 (one CTA of <2,4,1>) or
 // 10 (two CTAs of <1,4,2>) warps, so both run at 16384 / (3 * 32) -> 168 registers per thread.  The 64 accumulators
 // take 128 of them, so a k-step holds all B fragments (8 doubles) but only one m16 tile's A fragment (4) at a time.
+//
+// C of the 128x128 tile goes through the ring (STAGE_C): as the last k-tiles drain the ring, the producer bulk-copies C
+// into the freed stages, so the C reads of all but the last stage overlap the main loop and the epilogue reads shared
+// memory instead of waiting on HBM slab after slab.  (An L2 prefetch of C at tile start measured slower: it competes
+// with the operand stream and the concurrent pivot search for HBM and L2.)  A stage's A part (16 x LDA doubles) holds the 16-row slab
+// of m16 tile i of warp row 0, its B part the same slab of warp row 1.  Row r of a slab starts at r * LDA + 4 (r & 1)
+// doubles: even and odd rows are 64 bytes apart modulo 128, so the epilogue's 16-byte reads (a quarter-warp covers
+// rows g, g + 1 at columns 2t..2t+1) are conflict-free, and the 16 rows end exactly at 16 * LDA.
 template <int WM, int WN>
 struct Cfg {
     static constexpr int BM = 64 * WM, BN = 32 * WN;
     static constexpr int LDA = BM + 4, LDB = BN + 4;  // strides == 4 (mod 16) doubles: conflict-free fragment loads
     static constexpr int NCONS = WM * WN, NTHREADS = (NCONS + 1) * 32;
-    static constexpr size_t SMEM = (size_t)STAGES * BK * (LDA + LDB) * sizeof(double) + 2 * STAGES * sizeof(uint64_t);
+    static constexpr bool STAGE_C = (WM == 2);
+    static constexpr int NBAR = 2 * STAGES + (STAGE_C ? WM * STAGES : 0);  // full, empty (, one per C slab)
+    static constexpr size_t SMEM = (size_t)STAGES * BK * (LDA + LDB) * sizeof(double) + NBAR * sizeof(uint64_t);
+    static_assert(!STAGE_C || (LDA == LDB && 64 / 16 == STAGES), "one slab per warp row and stage, in both parts");
 };
 
 // C may alias D (the trailing update is in place), so the read-only (.nc) path is off limits.  A plain coherent 16-byte
@@ -55,6 +66,7 @@ __global__ void __launch_bounds__(Cfg<WM, WN>::NTHREADS, MINB) gemm_tn_kernel(Ge
     double* sB = sA + STAGES * BK * LDA;
     uint64_t* full = reinterpret_cast<uint64_t*>(sB + STAGES * BK * LDB);
     uint64_t* empty = full + STAGES;
+    uint64_t* cfull = empty + STAGES;  // STAGE_C: [warp row][i], the slab of m16 tile i has landed
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
@@ -64,6 +76,8 @@ __global__ void __launch_bounds__(Cfg<WM, WN>::NTHREADS, MINB) gemm_tn_kernel(Ge
             mbar_init(&full[s], 1);
             mbar_init(&empty[s], NCONS);
         }
+        if constexpr (C::STAGE_C)
+            for (int b = 0; b < WM * STAGES; ++b) mbar_init(&cfull[b], 1);
         fence_barrier_init();
     }
     __syncthreads();
@@ -75,7 +89,9 @@ __global__ void __launch_bounds__(Cfg<WM, WN>::NTHREADS, MINB) gemm_tn_kernel(Ge
         int wn = g.N - n0;
         wn = wn > BN ? BN : ((wn + 1) & ~1);
         const int rr = lane & 15;
-        for (int kt = 0; kt * BK < g.K; ++kt) {
+        const int nkt = (g.K + BK - 1) / BK;
+        const bool use_c = (g.beta != 0.0);
+        for (int kt = 0; kt < nkt; ++kt) {
             const int s = kt % STAGES, u = kt / STAGES;
             if (u > 0) mbar_wait(&empty[s], (u - 1) & 1);
             const int rows = min(BK, g.K - kt * BK);
@@ -88,6 +104,23 @@ __global__ void __launch_bounds__(Cfg<WM, WN>::NTHREADS, MINB) gemm_tn_kernel(Ge
                 else
                     bulk_g2s(sB + (s * BK + rr) * LDB, g.B + k * g.ldb + n0, (uint32_t)(wn * sizeof(double)), &full[s]);
             }
+        }
+        if constexpr (C::STAGE_C) {
+            // C slabs into the stages in the order they drain: (nkt + i) % STAGES was last used by k-tile nkt + i -
+            // STAGES, or never (K < 64).  Lanes 0-15: the rows of warp row 0's slab, 16-31: warp row 1's.
+            if (use_c)
+                for (int i = 0; i < STAGES; ++i) {
+                    const int s = (nkt + i) % STAGES, kt = nkt + i - STAGES;
+                    if (kt >= 0) mbar_wait(&empty[s], (kt / STAGES) & 1);
+                    const int wr = lane >> 4, r0 = m0 + 64 * wr + 16 * i;
+                    const int rows = max(0, min(16, g.M - r0));
+                    uint64_t* bar = &cfull[wr * STAGES + i];
+                    if (rr == 0) mbar_arrive_expect_tx(bar, (uint32_t)(rows * wn * sizeof(double)));
+                    __syncwarp();
+                    if (rr < rows)
+                        bulk_g2s(sA + (wr * STAGES + s) * BK * LDA + rr * LDA + 4 * (rr & 1),
+                                 g.C + (int64_t)(r0 + rr) * g.ldc + n0, (uint32_t)(wn * sizeof(double)), bar);
+                }
         }
         return;
     }
@@ -102,7 +135,8 @@ __global__ void __launch_bounds__(Cfg<WM, WN>::NTHREADS, MINB) gemm_tn_kernel(Ge
 #pragma unroll
         for (int j = 0; j < 4; ++j) acc[i][j][0] = acc[i][j][1] = acc[i][j][2] = acc[i][j][3] = 0.0;
 
-    for (int kt = 0; kt * BK < g.K; ++kt) {
+    int kt = 0;  // after the loop: the number of k-tiles
+    for (; kt * BK < g.K; ++kt) {
         const int s = kt % STAGES, u = kt / STAGES;
         mbar_wait(&full[s], u & 1);
         const double* a_s = sA + s * BK * LDA + wm_off + g4;
@@ -136,31 +170,58 @@ __global__ void __launch_bounds__(Cfg<WM, WN>::NTHREADS, MINB) gemm_tn_kernel(Ge
         if (lane == 0) mbar_arrive(&empty[s]);
     }
 
-    // ===== epilogue: registers <-> HBM directly, 16-byte accesses (each quad covers one 64 B row segment).
-    // C and D may alias, so the compiler must not be left to order loads after earlier stores: all C loads of an
-    // 8-row slab are issued first (4 independent 16 B loads in flight per thread), then its stores.  One slab per
-    // batch: with all 128 accumulator registers live, a second slab's loads would not fit the register budget.
     const double alpha = g.alpha, beta = g.beta;
     const bool use_c = (beta != 0.0);
     const int row0 = m0 + wm_off + g4, col0 = n0 + wn_off + 2 * t4;
+    if constexpr (C::STAGE_C) {
+        // ===== epilogue: C from the ring (see Cfg), slabs in the order the producer filled them; D straight to HBM
+        // with 16-byte stores.  C and D may alias: every element's C is in shared memory before its store is issued.
+        const int wr = warp / WN, nkt = kt;
 #pragma unroll
-    for (int sl = 0; sl < 8; ++sl) {
-        const int row = row0 + 8 * sl;
-        double2 cv[4];
+        for (int i = 0; i < 4; ++i) {
+            const double* cs = sA + (wr * STAGES + (nkt + i) % STAGES) * BK * LDA + 4 * (g4 & 1) + wn_off + 2 * t4;
+            if (use_c) mbar_wait(&cfull[wr * STAGES + i], 0);
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int col = col0 + 8 * j;
-            cv[j] = make_double2(0.0, 0.0);
-            if (use_c && row < g.M && col < g.N) cv[j] = ld_c2(g.C + (int64_t)row * g.ldc + col);
+            for (int h = 0; h < 2; ++h) {
+                const int row = row0 + 16 * i + 8 * h;
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const int col = col0 + 8 * j;
+                    if (row < g.M && col < g.N) {
+                        double2 cv = make_double2(0.0, 0.0);
+                        if (use_c) cv = *reinterpret_cast<const double2*>(cs + (g4 + 8 * h) * LDA + 8 * j);
+                        double2 out;
+                        out.x = fma(alpha, acc[i][j][2 * h], beta * cv.x);
+                        out.y = fma(alpha, acc[i][j][2 * h + 1], beta * cv.y);
+                        *reinterpret_cast<double2*>(g.D + (int64_t)row * g.ldd + col) = out;
+                    }
+                }
+            }
         }
+    } else {
+        // ===== epilogue: registers <-> HBM directly, 16-byte accesses (each quad covers one 64 B row segment).
+        // C and D may alias, so the compiler must not be left to order loads after earlier stores: all C loads of an
+        // 8-row slab are issued first (4 independent 16 B loads in flight per thread), then its stores.  One slab per
+        // batch: with all 128 accumulator registers live, a second slab's loads would not fit the register budget.
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int col = col0 + 8 * j;
-            if (row < g.M && col < g.N) {
-                double2 out;
-                out.x = fma(alpha, acc[sl / 2][j][2 * (sl & 1)], beta * cv[j].x);
-                out.y = fma(alpha, acc[sl / 2][j][2 * (sl & 1) + 1], beta * cv[j].y);
-                *reinterpret_cast<double2*>(g.D + (int64_t)row * g.ldd + col) = out;
+        for (int sl = 0; sl < 8; ++sl) {
+            const int row = row0 + 8 * sl;
+            double2 cv[4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const int col = col0 + 8 * j;
+                cv[j] = make_double2(0.0, 0.0);
+                if (use_c && row < g.M && col < g.N) cv[j] = ld_c2(g.C + (int64_t)row * g.ldc + col);
+            }
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const int col = col0 + 8 * j;
+                if (row < g.M && col < g.N) {
+                    double2 out;
+                    out.x = fma(alpha, acc[sl / 2][j][2 * (sl & 1)], beta * cv[j].x);
+                    out.y = fma(alpha, acc[sl / 2][j][2 * (sl & 1) + 1], beta * cv[j].y);
+                    *reinterpret_cast<double2*>(g.D + (int64_t)row * g.ldd + col) = out;
+                }
             }
         }
     }
