@@ -201,15 +201,20 @@ def residual(gv):
     return validate(gv)[1]
 
 
+def _rhs(n, B, what):
+    """B as float64, checked to be (n,) or (n, nrhs): (B, B as a C-contiguous n x nrhs array, nrhs)."""
+    B = np.asarray(B, dtype=np.float64)
+    if B.ndim not in (1, 2) or B.shape[0] != n:
+        raise ValueError(f"{what}: B must have shape ({n},) or ({n}, nrhs), got {B.shape}")
+    B2 = np.ascontiguousarray(B.reshape(n, -1))
+    return B, B2, B2.shape[1]
+
+
 def lu_solve(gv, B, trans=False):
     """Solves A X = B (A^T X = B when trans) with the factors of the last LU_rep (P A = L U) on the GPU grid, like
     LAPACK's getrs.  COLLECTIVE over gv.lu_comm; every rank passes the same B, (M,) or (M, nrhs) with M = gv.M (the padded
     size), and gets the same X in the same shape.  The factors and the input matrix are left as they are."""
-    B = np.asarray(B, dtype=np.float64)
-    if B.ndim not in (1, 2) or B.shape[0] != gv.M:
-        raise ValueError(f"lu_solve: B must have shape ({gv.M},) or ({gv.M}, nrhs), got {B.shape}")
-    B2 = np.ascontiguousarray(B.reshape(gv.M, -1))
-    nrhs = B2.shape[1]
+    B, B2, nrhs = _rhs(gv.M, B, "lu_solve")
     X = np.empty_like(B2)
     fn = lib().cflx_lu_solve_trans if trans else lib().cflx_lu_solve
     check(fn(gv._h, nrhs, B2.ctypes.data, max(nrhs, 1), X.ctypes.data, max(nrhs, 1)), "lu_solve")
@@ -225,15 +230,11 @@ def lu_rcond(gv):
 
 
 def _refine_args(n, B, X, what):
-    B = np.asarray(B, dtype=np.float64)
+    B, B2, nrhs = _rhs(n, B, what)
     X = np.asarray(X, dtype=np.float64)
-    if B.ndim not in (1, 2) or B.shape[0] != n:
-        raise ValueError(f"{what}: B must have shape ({n},) or ({n}, nrhs), got {B.shape}")
     if X.shape != B.shape:
         raise ValueError(f"{what}: X must have the shape of B, {B.shape}, got {X.shape}")
-    B2 = np.ascontiguousarray(B.reshape(n, -1))
     X2 = np.array(X.reshape(n, -1), dtype=np.float64, order="C")
-    nrhs = B2.shape[1]
     return B.shape, B2, X2, nrhs, np.empty(nrhs), np.empty(nrhs)
 
 
@@ -271,11 +272,7 @@ def lu_svx(gv, B, trans=False):
     """LAPACK dgesvx with the factors of the last LU_rep and the scaling they carry (lu_equilibrate): solves A X = B (A^T
     X = B when trans) with refinement.  Returns (X, dict(rcond, ferr, berr, rpvgrw, equed, info)); X is None when U has
     an exactly zero pivot (info = k).  COLLECTIVE over gv.lu_comm; identical on every rank."""
-    B = np.asarray(B, dtype=np.float64)
-    if B.ndim not in (1, 2) or B.shape[0] != gv.M:
-        raise ValueError(f"lu_svx: B must have shape ({gv.M},) or ({gv.M}, nrhs), got {B.shape}")
-    B2 = np.ascontiguousarray(B.reshape(gv.M, -1))
-    nrhs = B2.shape[1]
+    B, B2, nrhs = _rhs(gv.M, B, "lu_svx")
     X = np.empty_like(B2)
     fe, be = np.empty(nrhs), np.empty(nrhs)
     rcond, rpvgrw, equed, info = ctypes.c_double(), ctypes.c_double(), ctypes.c_char(), ctypes.c_int()
@@ -337,11 +334,7 @@ class cholesky:
         """Solves A X = B with the factor of the last parallelCholesky (A = L L^T) on the GPU grid, like LAPACK's potrs.
         COLLECTIVE over the object's comm; every rank passes the same B, (N,) or (N, nrhs) with N = self.N (the padded
         size), and gets the same X in the same shape.  The factor and the input are left as they are."""
-        B = np.asarray(B, dtype=np.float64)
-        if B.ndim not in (1, 2) or B.shape[0] != self.N:
-            raise ValueError(f"cholesky.solve: B must have shape ({self.N},) or ({self.N}, nrhs), got {B.shape}")
-        B2 = np.ascontiguousarray(B.reshape(self.N, -1))
-        nrhs = B2.shape[1]
+        B, B2, nrhs = _rhs(self.N, B, "cholesky.solve")
         X = np.empty_like(B2)
         check(lib().cflx_chol_solve(self._h, nrhs, B2.ctypes.data, max(nrhs, 1), X.ctypes.data, max(nrhs, 1)), "chol_solve")
         return X.reshape(B.shape)
@@ -377,11 +370,7 @@ class cholesky:
     def svx(self, B):
         """LAPACK dposvx with the factor of the last parallelCholesky and the scaling it carries (equilibrate): returns
         (X, dict(rcond, ferr, berr, equed, info)).  COLLECTIVE; identical on every rank."""
-        B = np.asarray(B, dtype=np.float64)
-        if B.ndim not in (1, 2) or B.shape[0] != self.N:
-            raise ValueError(f"cholesky.svx: B must have shape ({self.N},) or ({self.N}, nrhs), got {B.shape}")
-        B2 = np.ascontiguousarray(B.reshape(self.N, -1))
-        nrhs = B2.shape[1]
+        B, B2, nrhs = _rhs(self.N, B, "cholesky.svx")
         X = np.empty_like(B2)
         fe, be = np.empty(nrhs), np.empty(nrhs)
         rcond, equed, info = ctypes.c_double(), ctypes.c_char(), ctypes.c_int()

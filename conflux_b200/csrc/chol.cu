@@ -27,11 +27,8 @@
 
 using namespace cflx;
 
-struct cflx_chol {
-    cflx_comm* comm = nullptr;
-    int N = 0, v = 0, Kappa = 0, Px = 1, Py = 1, Pz = 1, P = 1, Ml = 0, Nl = 0, nlayr = 0, nb = 0;
-    int pi = 0, pj = 0, pk = 0, rank = 0;
-    SubComm k_comm, i_comm;
+// The grid's M is the padded order N, its Nt the reference's Kappa.
+struct cflx_chol : Grid {
     double *A0 = nullptr, *A11 = nullptr, *PT = nullptr, *LT = nullptr, *G = nullptr /* [2] */, *Bc = nullptr /* [2] */, *D = nullptr, *A00 = nullptr,
            *W = nullptr, *Uinv = nullptr, *LinvT = nullptr, *acc = nullptr, *Q = nullptr /* scratch of the blocked tile Cholesky */;
     int* info = nullptr;
@@ -299,14 +296,12 @@ __global__ void gather_cols_kernel(GatherArgs a) {
 }
 // sum of squares of the lower triangle (global row >= global column) of a local block-cyclic array: partials[blockIdx.x]
 // = this CTA's share; launch_sum_partials then adds them in index order, so every call rounds the same way
-__global__ void sumsq_lower_kernel(const double* __restrict__ X, int Ml, int Nl, int v, int Px, int Py, int pi, int pj,
-                                   double* __restrict__ partials) {
+__global__ void sumsq_lower_kernel(const double* __restrict__ X, Layout L, double* __restrict__ partials) {
     double s = 0.0;
-    const int64_t total = (int64_t)Ml * Nl;
+    const int64_t total = (int64_t)L.Ml * L.Nl;
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
-        const int lr = (int)(e / Nl), lc = (int)(e % Nl);
-        const int64_t gr = ((int64_t)(lr / v) * Px + pi) * v + lr % v, gc = ((int64_t)(lc / v) * Py + pj) * v + lc % v;
-        if (gr >= gc) s = fma(X[e], X[e], s);
+        const int lr = (int)(e / L.Nl), lc = (int)(e % L.Nl);
+        if (L.row<int64_t>(lr) >= L.col<int64_t>(lc)) s = fma(X[e], X[e], s);
     }
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
     __shared__ double w[32];
@@ -322,8 +317,9 @@ __global__ void sumsq_lower_kernel(const double* __restrict__ X, int Ml, int Nl,
 // column over the grid
 __global__ void info_min_operand_kernel(int* info) { info[2] = info[1] ? info[1] : INT_MAX; }
 // validation: transposed panel of column block t out of the stored factor, the diagonal tile masked to its lower triangle
-__global__ void extract_l_panel_T_kernel(const double* __restrict__ A, int64_t lda, int row0, int col0, int n, int v, int Px,
-                                         int pi, int t, double* __restrict__ PT, int64_t ldp) {
+__global__ void extract_l_panel_T_kernel(const double* __restrict__ A, int64_t lda, int row0, int col0, int n, Layout L,
+                                         int t, double* __restrict__ PT, int64_t ldp) {
+    const int v = L.v;
     __shared__ double tile[32][33];
     const int r0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
     for (int dy = threadIdx.y; dy < 32; dy += blockDim.y) {
@@ -331,7 +327,7 @@ __global__ void extract_l_panel_T_kernel(const double* __restrict__ A, int64_t l
         double x = 0.0;
         if (r < n && c < v) {
             const int lr = row0 + r;
-            const int64_t gr = ((int64_t)(lr / v) * Px + pi) * v + lr % v, gc = (int64_t)t * v + c;
+            const int64_t gr = L.row<int64_t>(lr), gc = (int64_t)t * v + c;
             x = gr >= gc ? A[(int64_t)lr * lda + col0 + c] : 0.0;
         }
         tile[dy][threadIdx.x] = x;
@@ -362,8 +358,8 @@ void free_chol(cflx_chol* ch) {
         if (ch->ev_col[i]) cudaEventDestroy(ch->ev_col[i]);
         if (ch->ev_panel[i]) cudaEventDestroy(ch->ev_panel[i]);
     }
-    for (SubComm* sc : {&ch->k_comm, &ch->i_comm, &ch->j_comm})
-        if (sc->c) ncclCommDestroy(sc->c);
+    if (ch->j_comm.c) ncclCommDestroy(ch->j_comm.c);
+    grid_free(ch);
     delete ch;
 }
 
@@ -554,7 +550,7 @@ int potrf_tile(double* D, double* A00, double* Q, int* info, int col0, int v, cu
 
 namespace {
 // Panel pipeline of step k on stream s: z-reduce of tile column k, Cholesky of the diagonal tile, L_kk^T down the grid
-// column, the panel solve, the stores, and (k < Kappa - 1) the broadcast of the panel pieces into buffer set k & 1.
+// column, the panel solve, the stores, and (k < Nt - 1) the broadcast of the panel pieces into buffer set k & 1.
 int panel_step(cflx_chol* ch, int k, cudaStream_t s) {
     const int v = ch->v, Px = ch->Px, Py = ch->Py, Pz = ch->Pz, Ml = ch->Ml, Nl = ch->Nl;
     const int pi = ch->pi, pj = ch->pj, pk = ch->pk;
@@ -581,7 +577,7 @@ int panel_step(cflx_chol* ch, int k, cudaStream_t s) {
         CFLX_CUDA(cudaGetLastError());
         ch->launches += 3;
     }
-    if (k == ch->Kappa - 1) return CFLX_OK;
+    if (k == ch->Nt - 1) return CFLX_OK;
     // L_kk^T to the ranks that hold the tile column (layer 0)                           Cholesky.cpp:680-690
     if (on_col && pk == 0 && Px > 1)
         CFLX_NCCL(ncclBroadcast(ch->A00, ch->A00, (size_t)v * v, ncclDouble, pik, ch->i_comm.c, s));
@@ -603,13 +599,12 @@ int panel_step(cflx_chol* ch, int k, cudaStream_t s) {
 // ---------------------------------------------------------------------------------------------- solve, A X = B
 // After the factorisation, layer 0's A11 holds L: tile (gi, gj), gi >= gj, on rank (gi % Px, gj % Py, 0) at local tile
 // (gi / Px, gj / Py), the diagonal tiles with zeros above the diagonal.  The solve reads nothing else: not the tiles above
-// the diagonal (leftovers of the update), not the local tiles with a global index >= Kappa, not the layers pk != 0.  It
+// the diagonal (leftovers of the update), not the local tiles with a global index >= Nt, not the layers pk != 0.  It
 // is the engine's row-partial sweep L Y = B (W seeded with B's rows on the ranks (pi, 0, 0); Y_t kept at the owner's
 // local column t / Py of Z), then its column-partial sweep L^T X = Y.  The grid row and column are those of layer 0
 // (j_comm / i_comm, one layer each); the layers pk != 0 only join the final all-reduce.
 SolveFactor chol_solve_factor(cflx_chol* ch) {
-    return SolveFactor{ch->comm, ch->A11, ch->N, ch->Ml, ch->Nl, first_local_tile(ch->Kappa, ch->pi, ch->Px) * ch->v,
-                       ch->v, ch->nb, ch->Kappa, ch->P, ch->Px, ch->Py, ch->pi, ch->pj, ch->pk, &ch->j_comm, &ch->i_comm, 1};
+    return SolveFactor{*ch, ch->A11, first_local_tile(ch->Nt, ch->pi, ch->Px) * ch->v, &ch->j_comm, &ch->i_comm, 1};
 }
 
 // First call after a factorisation: the grid-row communicator (once per object), the inverses of the nb x nb diagonal
@@ -620,10 +615,9 @@ int chol_solve_prepare(cflx_chol* ch) {
     if (ch->pk == 0) {
         const SolveFactor f = chol_solve_factor(ch);
         CFLX_TRY(solve_inverses(&ch->sv, f, true));
-        if (ch->pj == 0 && !ch->sv.rows) {  // local row r of a real tile holds global row ((r / v) * Px + pi) * v + r % v
-            const int v = ch->v;
+        if (ch->pj == 0 && !ch->sv.rows) {  // local row r of a real tile holds global row ch->row(r)
             std::vector<int> rows(std::max(f.rows, 1), 0);
-            for (int r = 0; r < f.rows; ++r) rows[r] = ((r / v) * ch->Px + ch->pi) * v + r % v;
+            for (int r = 0; r < f.rows; ++r) rows[r] = ch->row(r);
             CFLX_TRY(solve_set_rows(&ch->sv.rows, rows, c->stream));
         }
     }
@@ -631,6 +625,19 @@ int chol_solve_prepare(cflx_chol* ch) {
     return CFLX_OK;
 }
 
+// CFLX_OK when `what` may run, after a successful factorisation; otherwise CFLX_ERR_STATE with the reason
+int chol_check(const cflx_chol* ch, const char* what) {
+    if (ch->factored) return CFLX_OK;
+    set_last_error("cholesky %s requested before a successful cflx_chol_factor, or after cflx_chol_set_local without one",
+                   what);
+    return CFLX_ERR_STATE;
+}
+
+// dporfs (UPLO = 'L') on the input A0: A is symmetric, so both kinds of product are cflx_chol_solve
+RefineOp chol_refine_op(cflx_chol* ch) {
+    auto solve = [ch](bool, int n, const double* b, int lb, double* x, int lx) { return cflx_chol_solve(ch, n, b, lb, x, lx); };
+    return RefineOp{*ch, ch->A0, ResidMode::SymLower, true, solve};
+}
 }  // namespace
 
 // ======================================================================================================== C ABI
@@ -726,21 +733,15 @@ int cflx_chol_create(cflx_comm* c, int N, int v, int Px, int Py, int Pz, cflx_ch
     int d[6];
     CFLX_TRY(cflx_chol_dims(N, v, Px, Py, Pz, d));
     auto* ch = new cflx_chol;
-    ch->comm = c;
-    ch->N = d[0]; ch->Kappa = d[1]; ch->Ml = d[2]; ch->Nl = d[3]; ch->nlayr = d[4]; ch->P = d[5];
-    ch->v = v; ch->Px = Px; ch->Py = Py; ch->Pz = Pz;
-    ch->rank = c->world_rank;  // like the LU path: rank = (pi * Py + pj) * Pz + pk
-    ch->pi = ch->rank / (Py * Pz);
-    ch->pj = (ch->rank / Pz) % Py;
-    ch->pk = ch->rank % Pz;
+    ch->M = d[0]; ch->Nt = d[1]; ch->Ml = d[2]; ch->Nl = d[3]; ch->nlayr = d[4];
+    ch->v = v;
     ch->nb = chol_pick_nb(v);
     int rc = CFLX_OK;
     auto fail = [&](int code) {
         free_chol(ch);
         return code;
     };
-    if ((rc = make_sub(c, ch->pi * Py + ch->pj, ch->pk, Pz, &ch->k_comm))) return fail(rc);
-    if ((rc = make_sub(c, ch->pj * Pz + ch->pk, ch->pi, Px, &ch->i_comm))) return fail(rc);
+    if ((rc = grid_init(ch, c, Px, Py, Pz))) return fail(rc);
     const size_t loc = (size_t)ch->Ml * ch->Nl, vv = (size_t)v * v;
     ch->ldp = round_up(ch->Ml, 2) + 2;
     ch->ldb = round_up(ch->Nl, 2) + 2;
@@ -785,7 +786,7 @@ int cflx_chol_create(cflx_comm* c, int N, int v, int Px, int Py, int Pz, cflx_ch
 // info_out[16] = {N, v, Kappa, Ml, Nl, nlayr, P, Px, Py, Pz, pi, pj, pk, rank, 0, 0}
 int cflx_chol_info(const cflx_chol* ch, int* o) {
     if (!ch || !o) return CFLX_ERR_ARG;
-    const int vals[16] = {ch->N, ch->v, ch->Kappa, ch->Ml, ch->Nl, ch->nlayr, ch->P, ch->Px, ch->Py, ch->Pz, ch->pi, ch->pj, ch->pk,
+    const int vals[16] = {ch->M, ch->v, ch->Nt, ch->Ml, ch->Nl, ch->nlayr, ch->P, ch->Px, ch->Py, ch->Pz, ch->pi, ch->pj, ch->pk,
                           ch->rank, 0, 0};
     std::memcpy(o, vals, sizeof(vals));
     return CFLX_OK;
@@ -814,7 +815,7 @@ int cflx_chol_factor(cflx_chol* ch, double* ms_out) {
     cudaStream_t s = c->stream;
     CFLX_CUDA(cudaSetDevice(c->device));
     ch->sv.ready = false;
-    CFLX_TRY(equil_pass_on(&ch->eq, ch->N, false, s));  // the factor carries the input's scaling
+    CFLX_TRY(equil_pass_on(&ch->eq, ch->M, false, s));  // the factor carries the input's scaling
     const int v = ch->v, Py = ch->Py, Ml = ch->Ml, Nl = ch->Nl;
     const int pj = ch->pj;
     CFLX_CUDA(cudaMemcpyAsync(ch->A11, ch->A0, (size_t)Ml * Nl * sizeof(double), cudaMemcpyDeviceToDevice, s));
@@ -832,7 +833,7 @@ int cflx_chol_factor(cflx_chol* ch, double* ms_out) {
     CFLX_CUDA(cudaStreamWaitEvent(sp, ch->ev_col[0], 0));
     CFLX_TRY(panel_step(ch, 0, sp));
     CFLX_CUDA(cudaEventRecord(ch->ev_panel[0], sp));
-    for (int k = 0; k + 1 < ch->Kappa; ++k) {
+    for (int k = 0; k + 1 < ch->Nt; ++k) {
         const int b = k & 1, nb1 = (k + 1) & 1;
         CFLX_CUDA(cudaStreamWaitEvent(s, ch->ev_panel[b], 0));             // pieces of step k are in buffer set b
         CFLX_TRY(split_planes(ch, k + 1, k + 1, b, s));                     // (int8 wgmma path) digit planes of both operands
@@ -845,7 +846,7 @@ int cflx_chol_factor(cflx_chol* ch, double* ms_out) {
         CFLX_CUDA(cudaEventRecord(ch->ev_panel[nb1], sp));
         CFLX_TRY(update_columns(ch, k + 1, k + 1, b, ch->A11, own_next ? ljn + 1 : 0, Nl / v, s, b));
     }
-    CFLX_CUDA(cudaStreamWaitEvent(s, ch->ev_panel[(ch->Kappa - 1) & 1], 0));
+    CFLX_CUDA(cudaStreamWaitEvent(s, ch->ev_panel[(ch->Nt - 1) & 1], 0));
     CFLX_CUDA(cudaEventRecord(e1, s));
     CFLX_CUDA(cudaEventSynchronize(e1));
     float ms = 0;
@@ -879,10 +880,7 @@ int cflx_chol_factor(cflx_chol* ch, double* ms_out) {
 // local share of L (Ml x Nl row-major, conflux tile layout; tiles above the diagonal are not meaningful)
 int cflx_chol_get_local(cflx_chol* ch, double* L_host) {
     if (!ch || !L_host) return CFLX_ERR_ARG;
-    if (!ch->factored) {
-        set_last_error("factor requested before cflx_chol_factor");
-        return CFLX_ERR_STATE;
-    }
+    CFLX_TRY(chol_check(ch, "factor"));
     CFLX_CUDA(cudaSetDevice(ch->comm->device));
     CFLX_CUDA(cudaMemcpyAsync(L_host, ch->A11, (size_t)ch->Ml * ch->Nl * sizeof(double), cudaMemcpyDeviceToHost, ch->comm->stream));
     CFLX_CUDA(cudaStreamSynchronize(ch->comm->stream));
@@ -894,10 +892,7 @@ int cflx_chol_get_local(cflx_chol* ch, double* L_host) {
 // 183-217, compares against LAPACKE_dpotrf on one node; tests/ do that at small sizes.)
 int cflx_chol_validate(cflx_chol* ch, double* abs_out, double* rel_out) {
     if (!ch) return CFLX_ERR_ARG;
-    if (!ch->factored) {
-        set_last_error("validation requested before cflx_chol_factor");
-        return CFLX_ERR_STATE;
-    }
+    CFLX_TRY(chol_check(ch, "validation"));
     cflx_comm* c = ch->comm;
     cudaStream_t s = c->stream;
     CFLX_CUDA(cudaSetDevice(c->device));
@@ -910,12 +905,12 @@ int cflx_chol_validate(cflx_chol* ch, double* abs_out, double* rel_out) {
     // zeroing the other layers' contribution (their A11 holds partial sums, not the factor)
     if (cudaMemcpyAsync(R, ch->A0, loc * sizeof(double), cudaMemcpyDeviceToDevice, s) != cudaSuccess) rc = CFLX_ERR_CUDA;
     const int nlayr_save = ch->nlayr, pk_save = ch->pk;
-    for (int t = 0; t < ch->Kappa && !rc; ++t) {
+    for (int t = 0; t < ch->Nt && !rc; ++t) {
         const int pjt = t % Py;
         const int row0 = first_local_tile(t, ch->pi, Px) * v, n0 = Ml - row0;
         if (ch->pj == pjt && pk_save == 0 && n0 > 0) {
             dim3 grid((n0 + 31) / 32, (v + 31) / 32), block(32, 8);
-            extract_l_panel_T_kernel<<<grid, block, 0, s>>>(ch->A11, Nl, row0, (t / Py) * v, n0, v, Px, ch->pi, t, ch->LT,
+            extract_l_panel_T_kernel<<<grid, block, 0, s>>>(ch->A11, Nl, row0, (t / Py) * v, n0, *ch, t, ch->LT,
                                                             piece_ld(ch, t, ch->pi));
         }
         // layer 0 applies the whole contraction, the other layers a zero-length slab (they only take part in the broadcasts)
@@ -943,11 +938,11 @@ int cflx_chol_validate(cflx_chol* ch, double* abs_out, double* rel_out) {
             CFLX_CUDA(cudaGetLastError());
             return CFLX_OK;
         };
-        sumsq_lower_kernel<<<SUMSQ_PARTIALS, 256, 0, s>>>(R, Ml, Nl, v, Px, Py, ch->pi, ch->pj, ch->acc + 2);
+        sumsq_lower_kernel<<<SUMSQ_PARTIALS, 256, 0, s>>>(R, *ch, ch->acc + 2);
         rc = launch_error();
         if (!rc) rc = launch_sum_partials(ch->acc + 2, SUMSQ_PARTIALS, ch->acc, s);
         if (!rc) {
-            sumsq_lower_kernel<<<SUMSQ_PARTIALS, 256, 0, s>>>(ch->A0, Ml, Nl, v, Px, Py, ch->pi, ch->pj, ch->acc + 2);
+            sumsq_lower_kernel<<<SUMSQ_PARTIALS, 256, 0, s>>>(ch->A0, *ch, ch->acc + 2);
             rc = launch_error();
         }
         if (!rc) rc = launch_sum_partials(ch->acc + 2, SUMSQ_PARTIALS, ch->acc + 1, s);
@@ -970,10 +965,7 @@ int cflx_chol_validate(cflx_chol* ch, double* abs_out, double* rel_out) {
 // are left as they are.
 int cflx_chol_solve(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X, int ldx) {
     if (!ch || nrhs < 1 || ldb < nrhs || (X && ldx < nrhs) || !B) return CFLX_ERR_ARG;
-    if (!ch->factored) {
-        set_last_error("cholesky solve requested before a successful cflx_chol_factor, or after cflx_chol_set_local without one");
-        return CFLX_ERR_STATE;
-    }
+    CFLX_TRY(chol_check(ch, "solve"));
     CFLX_CUDA(cudaSetDevice(ch->comm->device));
     if (!ch->sv.ready) CFLX_TRY(chol_solve_prepare(ch));
     const SolveFactor f = chol_solve_factor(ch);
@@ -992,20 +984,16 @@ int cflx_chol_solve(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X
 // the Hager-Higham estimate of ||inv(A)||_1, whose products inv(A) x are solves with the factor.
 int cflx_chol_rcond(cflx_chol* ch, double* rcond_out, double* anorm_out) {
     if (!ch || !rcond_out) return CFLX_ERR_ARG;
-    if (!ch->factored) {
-        set_last_error("cholesky condition estimate requested before a successful cflx_chol_factor, or after cflx_chol_set_local without one");
-        return CFLX_ERR_STATE;
-    }
+    CFLX_TRY(chol_check(ch, "condition estimate"));
     CFLX_CUDA(cudaSetDevice(ch->comm->device));
     double anorm = 0.0, ainvnm = 0.0;
-    CFLX_TRY(norm1_grid(ch->comm, ch->A0, ch->N, ch->Ml, ch->Nl, ch->v, ch->Kappa, ch->Px, ch->Py, ch->pi, ch->pj, ch->pk,
-                        true, &anorm));
+    CFLX_TRY(norm1_grid(*ch, ch->A0, true, &anorm));
     if (anorm > 0.0) {
         // every rank runs the estimator on the X of solve_finish, bit-identical on every rank, so every rank makes the
         // same choices and issues the same solves (the same collectives) in the same order; A is symmetric, so both
         // kinds of product are the same solve
         auto apply = [&](int, double* x) { return cflx_chol_solve(ch, 1, x, 1, x, 1); };
-        CFLX_TRY(estimate_inv_norm1(ch->N, apply, &ainvnm));
+        CFLX_TRY(estimate_inv_norm1(ch->M, apply, &ainvnm));
     }
     *rcond_out = rcond_from(anorm, ainvnm);
     if (anorm_out) *anorm_out = anorm;
@@ -1017,15 +1005,9 @@ int cflx_chol_rcond(cflx_chol* ch, double* rcond_out, double* anorm_out) {
 int cflx_chol_refine(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X, int ldx, double* ferr_out,
                      double* berr_out) {
     if (!ch || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B || !X) return CFLX_ERR_ARG;
-    if (!ch->factored) {
-        set_last_error("cholesky refinement requested before a successful cflx_chol_factor, or after cflx_chol_set_local without one");
-        return CFLX_ERR_STATE;
-    }
+    CFLX_TRY(chol_check(ch, "refinement"));
     CFLX_CUDA(cudaSetDevice(ch->comm->device));
-    auto solve = [ch](bool, int n, const double* b, int lb, double* x, int lx) { return cflx_chol_solve(ch, n, b, lb, x, lx); };
-    const RefineOp op{ch->comm, ch->A0, ResidMode::SymLower, ch->N, ch->Ml, ch->Nl, ch->v, ch->Kappa, ch->Px, ch->Py,
-                      ch->Pz, ch->pi, ch->pj, ch->pk, true, solve};
-    return refine_run(&ch->sv.rf, op, nrhs, B, ldb, X, ldx, ferr_out, berr_out);
+    return refine_run(&ch->sv.rf, chol_refine_op(ch), nrhs, B, ldb, X, ldx, ferr_out, berr_out);
 }
 
 // COLLECTIVE.  LAPACK dpoequ (+ dlaqsy, UPLO = 'L', when apply) on the input A0 (equil.cu); drops the factorisation and
@@ -1047,11 +1029,10 @@ int cflx_chol_equilibrate(cflx_chol* ch, int apply, double* s_out, double* scond
     double scond = 0.0, amax = 0.0;
     char equed = 'N';
     int info = 0;
-    CFLX_TRY(poequ_grid(ch->comm, &ch->eq, ch->A0, ch->N, ch->Ml, ch->Nl, ch->v, ch->Kappa, ch->Px, ch->Py, ch->pi, ch->pj,
-                        ch->pk, apply != 0, s_out, &scond, &amax, &equed, &info));
+    CFLX_TRY(poequ_grid(*ch, &ch->eq, ch->A0, apply != 0, s_out, &scond, &amax, &equed, &info));
     // the input's record changes only when this call scaled it; a query (apply = 0) leaves the record and its scales
     if (apply && info == 0)
-        CFLX_TRY(equil_record_set(&ch->eq.in, equed, scond, scond, ch->eq.qr, nullptr, ch->N, ch->comm->stream));
+        CFLX_TRY(equil_record_set(&ch->eq.in, equed, scond, scond, ch->eq.qr, nullptr, ch->M, ch->comm->stream));
     if (scond_out) *scond_out = scond;
     if (amax_out) *amax_out = amax;
     if (equed_out) *equed_out = equed;
@@ -1064,36 +1045,16 @@ int cflx_chol_equilibrate(cflx_chol* ch, int apply, double* s_out, double* scond
 int cflx_chol_svx(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out,
                   double* ferr_out, double* berr_out, char* equed_out, int* info_out) {
     if (!ch || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B || !X || !rcond_out || !info_out) return CFLX_ERR_ARG;
-    if (!ch->factored) {
-        set_last_error("cholesky expert solve requested before a successful cflx_chol_factor, or after cflx_chol_set_local without one");
-        return CFLX_ERR_STATE;
-    }
+    CFLX_TRY(chol_check(ch, "expert solve"));
     CFLX_CUDA(cudaSetDevice(ch->comm->device));
-    cudaStream_t s = ch->comm->stream;
     const EquilRecord& eq = ch->eq.fac;
-    const bool scaled = eq.equed == 'Y';
+    const double* s = eq.equed == 'Y' ? eq.r : nullptr;
     if (equed_out) *equed_out = eq.equed;
     double rcond = 0.0;
     CFLX_TRY(cflx_chol_rcond(ch, &rcond, nullptr));
     *rcond_out = rcond;
-    const int N = ch->N, ldn = (int)round_up(nrhs, 8);
-    CFLX_TRY(equil_grow(&ch->eq, N, ldn));
-    double *dB = ch->eq.B, *dX = ch->eq.X;
-    CFLX_CUDA(cudaMemcpy2DAsync(dB, ldn * sizeof(double), B, (size_t)ldb * sizeof(double), nrhs * sizeof(double), N,
-                                cudaMemcpyDefault, s));
-    if (scaled) CFLX_TRY(launch_scale_rows(dB, ldn, N, nrhs, eq.r, s));
-    CFLX_TRY(cflx_chol_solve(ch, nrhs, dB, ldn, dX, ldn));
-    auto solve = [ch](bool, int n, const double* b, int lb, double* x, int lx) { return cflx_chol_solve(ch, n, b, lb, x, lx); };
-    const RefineOp op{ch->comm, ch->A0, ResidMode::SymLower, N, ch->Ml, ch->Nl, ch->v, ch->Kappa, ch->Px, ch->Py, ch->Pz,
-                      ch->pi, ch->pj, ch->pk, true, solve};
-    CFLX_TRY(refine_run(&ch->sv.rf, op, nrhs, dB, ldn, dX, ldn, ferr_out, berr_out));
-    if (scaled) CFLX_TRY(launch_scale_rows(dX, ldn, N, nrhs, eq.r, s));
-    CFLX_CUDA(cudaMemcpy2DAsync(X, (size_t)ldx * sizeof(double), dX, ldn * sizeof(double), nrhs * sizeof(double), N,
-                                cudaMemcpyDefault, s));
-    CFLX_CUDA(cudaStreamSynchronize(s));
-    if (ferr_out && scaled)
-        for (int j = 0; j < nrhs; ++j) ferr_out[j] /= eq.rowcnd;
-    *info_out = rcond < std::ldexp(1.0, -53) ? N + 1 : 0;
+    CFLX_TRY(svx_tail(&ch->eq, &ch->sv.rf, chol_refine_op(ch), nrhs, B, ldb, X, ldx, ferr_out, berr_out, s, s, eq.rowcnd));
+    *info_out = rcond < std::ldexp(1.0, -53) ? ch->M + 1 : 0;
     return CFLX_OK;
 }
 

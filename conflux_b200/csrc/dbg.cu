@@ -323,38 +323,39 @@ int cflx_dbg_equil(int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int
     CFLX_CUDA(cudaMemcpy(dc.p, c, sizeof(double) * M, cudaMemcpyHostToDevice));
     const double* a = dA.as<double>();
     double *w = dW.as<double>(), *vec = dv.as<double>();
+    const Layout L{M, v, Kappa, Ml, Nl, Px, Py, pi, pj};
     auto vec_out = [&](double* out) -> int {
         CFLX_CUDA(cudaMemcpy(out, vec, sizeof(double) * M, cudaMemcpyDeviceToHost));
         return CFLX_OK;
     };
     if (rowmax_out) {
-        CFLX_TRY(equil_row_max(a, Ml, Nl, v, Px, pi, vec, M, 0));
+        CFLX_TRY(equil_row_max(a, L, vec, 0));
         CFLX_TRY(vec_out(rowmax_out));
     }
     if (colmax_out) {
-        CFLX_TRY(equil_col_max(a, Ml, Nl, v, Px, Py, pi, pj, dr.as<double>(), vec, M, 0));
+        CFLX_TRY(equil_col_max(a, L, dr.as<double>(), vec, 0));
         CFLX_TRY(vec_out(colmax_out));
     }
     if (diag_out) {
-        CFLX_TRY(equil_diag(a, Ml, Nl, v, Kappa, Px, Py, pi, pj, vec, M, 0));
+        CFLX_TRY(equil_diag(a, L, vec, 0));
         CFLX_TRY(vec_out(diag_out));
     }
     if (scaled_out) {
         CFLX_CUDA(cudaMemcpy(w, a, sizeof(double) * a_n, cudaMemcpyDeviceToDevice));
-        CFLX_TRY(equil_apply(w, Ml, Nl, v, Px, Py, pi, pj, dr.as<double>(), dc.as<double>(), equed, 0));
+        CFLX_TRY(equil_apply(w, L, dr.as<double>(), dc.as<double>(), equed, 0));
         CFLX_CUDA(cudaMemcpy(scaled_out, w, sizeof(double) * a_n, cudaMemcpyDeviceToHost));
     }
     if (sym_scaled_out) {  // s = r
         CFLX_CUDA(cudaMemcpy(w, a, sizeof(double) * a_n, cudaMemcpyDeviceToDevice));
-        CFLX_TRY(equil_sym_apply(w, Ml, Nl, v, Kappa, Px, Py, pi, pj, dr.as<double>(), 0));
+        CFLX_TRY(equil_sym_apply(w, L, dr.as<double>(), 0));
         CFLX_CUDA(cudaMemcpy(sym_scaled_out, w, sizeof(double) * a_n, cudaMemcpyDeviceToHost));
     }
     if (growth_out) {  // the share is both L\U and the input
-        CFLX_TRY(equil_growth(a, a, Ml, Nl, v, Px, Py, pi, pj, ncols, dg.as<double>(), 0));
+        CFLX_TRY(equil_growth(a, a, L, ncols, dg.as<double>(), 0));
         CFLX_CUDA(cudaMemcpy(growth_out, dg.p, sizeof(double) * 2, cudaMemcpyDeviceToHost));
     }
     if (zero_pivot_out) {
-        CFLX_TRY(equil_zero_pivot(a, Ml, Nl, v, M, Px, Py, pi, pj, dz.as<int>(), 0));
+        CFLX_TRY(equil_zero_pivot(a, L, dz.as<int>(), 0));
         int z = 0;
         CFLX_CUDA(cudaMemcpy(&z, dz.p, sizeof(int), cudaMemcpyDeviceToHost));
         *zero_pivot_out = z == INT_MAX ? 0 : z;
@@ -383,9 +384,10 @@ int cflx_dbg_residual(int mode, int Ml, int Nl, const double* A, int v, int Kapp
     CFLX_CUDA(cudaMemcpy(dA.p, A, sizeof(double) * a_n, cudaMemcpyHostToDevice));
     if (Xc) CFLX_CUDA(cudaMemcpy(dXc.p, Xc, sizeof(double) * (size_t)Nl * nrhs, cudaMemcpyHostToDevice));
     if (Xr) CFLX_CUDA(cudaMemcpy(dXr.p, Xr, sizeof(double) * (size_t)Ml * nrhs, cudaMemcpyHostToDevice));
+    const Layout L{0, v, Kappa, Ml, Nl, Px, Py, pi, pj};  // M: the kernels index by local row and column only
     auto run = [&]() {
-        return launch_residual(m, dA.as<double>(), Nl, Ml, Nl, v, Kappa, Px, Py, pi, pj, dXc.as<double>(), dXr.as<double>(),
-                               nrhs, nrhs, dP.as<double>(), dQ.as<double>(), nrhs, 0);
+        return launch_residual(m, dA.as<double>(), L, dXc.as<double>(), dXr.as<double>(), nrhs, nrhs, dP.as<double>(),
+                               dQ.as<double>(), nrhs, 0);
     };
     cudaEvent_t e0, e1;
     CFLX_CUDA(cudaEventCreate(&e0));

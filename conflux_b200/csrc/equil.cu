@@ -2,8 +2,8 @@
 // cflx_chol_equilibrate, cflx_chol_svx): LAPACK's dgeequ + dlaqge, dpoequ + dlaqsy and dgesvx's reciprocal pivot growth
 // on the GPU grid.
 //
-// Every pass reads layer 0's local share A (Ml x Nl, conflux layout: local (r, c) is global (((r / v) Px + pi) v + r % v,
-// ((c / v) Py + pj) v + c % v)) once; it is HBM-bound.  What the ranks combine are maxima (and, for the Cholesky diagonal,
+// Every pass reads layer 0's local share A (Ml x Nl, conflux layout: local (r, c) is global (L.row(r), L.col(c))) once;
+// it is HBM-bound.  What the ranks combine are maxima (and, for the Cholesky diagonal,
 // sums with exactly one non-zero contributor per element), which are exact whatever the order: each rank writes its
 // partial into an M-vector with zeros where it holds nothing, and one all-reduce over the world (ncclMax, or ncclSum for
 // the diagonal) makes the vector bit-identical on every rank.  Inside a share, maxima of non-negative doubles are taken
@@ -21,42 +21,38 @@ namespace {
 constexpr int EQ_COLS = 128;  // local columns per CTA (one per thread) of the column passes
 constexpr int EQ_ROWS = 256;  // local rows per CTA of the column passes
 
-__device__ __forceinline__ int gidx(int l, int P, int p, int v) { return ((l / v) * P + p) * v + l % v; }
 __device__ __forceinline__ void max_bits(double* out, double x) {  // x >= 0
     atomicMax(reinterpret_cast<unsigned long long*>(out), (unsigned long long)__double_as_longlong(x));
 }
 
 // one warp per local row: rowmax[g] = max_c |A[r][c]|
-__global__ void row_max_kernel(const double* __restrict__ A, int Ml, int Nl, int v, int Px, int pi,
-                               double* __restrict__ rowmax) {
+__global__ void row_max_kernel(const double* __restrict__ A, Layout L, double* __restrict__ rowmax) {
     const int r = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-    if (r >= Ml) return;
-    const double* a = A + (int64_t)r * Nl;
+    if (r >= L.Ml) return;
+    const double* a = A + (int64_t)r * L.Nl;
     double m = 0.0;
-    for (int c = lane; c < Nl; c += 32) m = fmax(m, fabs(a[c]));
+    for (int c = lane; c < L.Nl; c += 32) m = fmax(m, fabs(a[c]));
     for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
-    if (lane == 0) rowmax[gidx(r, Px, pi, v)] = m;
+    if (lane == 0) rowmax[L.row(r)] = m;
 }
 
 // colmax[g] = max over this CTA's rows of |A[r][c]| r[gr]; combined over the CTAs by atomicMax on the bits
-__global__ void __launch_bounds__(EQ_COLS) col_max_kernel(const double* __restrict__ A, int Ml, int Nl, int v, int Px,
-                                                          int Py, int pi, int pj, const double* __restrict__ rs,
-                                                          double* __restrict__ colmax) {
-    const int c = blockIdx.x * EQ_COLS + threadIdx.x, r0 = blockIdx.y * EQ_ROWS, r1 = min(r0 + EQ_ROWS, Ml);
-    if (c >= Nl) return;
+__global__ void __launch_bounds__(EQ_COLS) col_max_kernel(const double* __restrict__ A, Layout L,
+                                                          const double* __restrict__ rs, double* __restrict__ colmax) {
+    const int c = blockIdx.x * EQ_COLS + threadIdx.x, r0 = blockIdx.y * EQ_ROWS, r1 = min(r0 + EQ_ROWS, L.Ml);
+    if (c >= L.Nl) return;
     double m = 0.0;
-    for (int r = r0; r < r1; ++r) m = fmax(m, fabs(A[(int64_t)r * Nl + c]) * rs[gidx(r, Px, pi, v)]);
-    max_bits(colmax + gidx(c, Py, pj, v), m);
+    for (int r = r0; r < r1; ++r) m = fmax(m, fabs(A[(int64_t)r * L.Nl + c]) * rs[L.row(r)]);
+    max_bits(colmax + L.col(c), m);
 }
 
-// diag[g] = a_gg on the diagonal tiles this share holds (global tile index < Kappa)
-__global__ void diag_kernel(const double* __restrict__ A, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi,
-                            int pj, double* __restrict__ diag, int M) {
+// diag[g] = a_gg on the diagonal tiles this share holds (global tile index < Nt)
+__global__ void diag_kernel(const double* __restrict__ A, Layout L, double* __restrict__ diag) {
     const int g = blockIdx.x * blockDim.x + threadIdx.x;
-    if (g >= M) return;
-    const int t = g / v, e = g % v;
-    if (t >= Kappa || t % Px != pi || t % Py != pj || (t / Px) * v >= Ml || (t / Py) * v >= Nl) return;
-    diag[g] = A[(int64_t)((t / Px) * v + e) * Nl + (t / Py) * v + e];
+    if (g >= L.M) return;
+    const int t = g / L.v, e = g % L.v;
+    if (t >= L.Nt || !L.holds_diag(t)) return;
+    diag[g] = A[(int64_t)(L.diag_row(t) + e) * L.Nl + L.diag_col(t) + e];
 }
 
 // x = 1 / min(max(x, small), 1 / small) elementwise (dgeequ's reciprocal scales)
@@ -67,58 +63,55 @@ __global__ void recip_kernel(double* x, int n, double small, double big) {
 
 // dlaqge: 'R' r_i a, 'C' c_j a, 'B' (c_j r_i) a; a thread per local column, the rows strided over gridDim.y
 template <char EQ>
-__global__ void apply_kernel(double* __restrict__ A, int Ml, int Nl, int v, int Px, int Py, int pi, int pj,
-                             const double* __restrict__ rs, const double* __restrict__ cs) {
+__global__ void apply_kernel(double* __restrict__ A, Layout L, const double* __restrict__ rs,
+                             const double* __restrict__ cs) {
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c >= Nl) return;
-    const double cj = EQ == 'R' ? 1.0 : cs[gidx(c, Py, pj, v)];
-    for (int r = blockIdx.y; r < Ml; r += gridDim.y) {
-        const int64_t o = (int64_t)r * Nl + c;
-        if (EQ == 'R') A[o] = rs[gidx(r, Px, pi, v)] * A[o];
+    if (c >= L.Nl) return;
+    const double cj = EQ == 'R' ? 1.0 : cs[L.col(c)];
+    for (int r = blockIdx.y; r < L.Ml; r += gridDim.y) {
+        const int64_t o = (int64_t)r * L.Nl + c;
+        if (EQ == 'R') A[o] = rs[L.row(r)] * A[o];
         if (EQ == 'C') A[o] = cj * A[o];
-        if (EQ == 'B') A[o] = (cj * rs[gidx(r, Px, pi, v)]) * A[o];
+        if (EQ == 'B') A[o] = (cj * rs[L.row(r)]) * A[o];
     }
 }
 
 // dlaqsy (UPLO = 'L'): (s_j s_i) a on the real tiles' entries with global row >= global column; nothing else is read
-__global__ void sym_apply_kernel(double* __restrict__ A, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj,
-                                 const double* __restrict__ ss) {
+__global__ void sym_apply_kernel(double* __restrict__ A, Layout L, const double* __restrict__ ss) {
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c >= Nl) return;
-    const int gj = gidx(c, Py, pj, v);
-    if (gj / v >= Kappa) return;
-    for (int r = blockIdx.y; r < Ml; r += gridDim.y) {
-        const int gi = gidx(r, Px, pi, v);
-        if (gi / v >= Kappa || gi < gj) continue;
-        const int64_t o = (int64_t)r * Nl + c;
+    if (c >= L.Nl) return;
+    const int gj = L.col(c);
+    if (gj / L.v >= L.Nt) return;
+    for (int r = blockIdx.y; r < L.Ml; r += gridDim.y) {
+        const int gi = L.row(r);
+        if (gi / L.v >= L.Nt || gi < gj) continue;
+        const int64_t o = (int64_t)r * L.Nl + c;
         A[o] = (ss[gj] * ss[gi]) * A[o];
     }
 }
 
 // first zero on the diagonal of U: out = min(1 + g) over the global diagonal entries this share holds with F_gg == 0
-__global__ void zero_pivot_kernel(const double* __restrict__ F, int Ml, int Nl, int v, int M, int Px, int Py, int pi,
-                                  int pj, int* out) {
+__global__ void zero_pivot_kernel(const double* __restrict__ F, Layout L, int* out) {
     const int g = blockIdx.x * blockDim.x + threadIdx.x;
-    if (g >= M) return;
-    const int t = g / v, e = g % v;
-    if (t % Px != pi || t % Py != pj || (t / Px) * v >= Ml || (t / Py) * v >= Nl) return;
-    if (F[(int64_t)((t / Px) * v + e) * Nl + (t / Py) * v + e] == 0.0) atomicMin(out, g + 1);
+    if (g >= L.M) return;
+    const int t = g / L.v, e = g % L.v;
+    if (!L.holds_diag(t)) return;
+    if (F[(int64_t)(L.diag_row(t) + e) * L.Nl + L.diag_col(t) + e] == 0.0) atomicMin(out, g + 1);
 }
 
 // out[0] = max |triu(F)|, out[1] = max |A| over the global columns < ncols of this share
 __global__ void __launch_bounds__(EQ_COLS) growth_kernel(const double* __restrict__ F, const double* __restrict__ A,
-                                                         int Ml, int Nl, int v, int Px, int Py, int pi, int pj, int ncols,
-                                                         double* out) {
+                                                         Layout L, int ncols, double* out) {
     __shared__ double sh[2][EQ_COLS];
-    const int c = blockIdx.x * EQ_COLS + threadIdx.x, r0 = blockIdx.y * EQ_ROWS, r1 = min(r0 + EQ_ROWS, Ml);
+    const int c = blockIdx.x * EQ_COLS + threadIdx.x, r0 = blockIdx.y * EQ_ROWS, r1 = min(r0 + EQ_ROWS, L.Ml);
     double mu = 0.0, ma = 0.0;
-    if (c < Nl) {
-        const int gc = gidx(c, Py, pj, v);
+    if (c < L.Nl) {
+        const int gc = L.col(c);
         if (gc < ncols) {
             for (int r = r0; r < r1; ++r) {
-                const int64_t o = (int64_t)r * Nl + c;
+                const int64_t o = (int64_t)r * L.Nl + c;
                 ma = fmax(ma, fabs(A[o]));
-                if (gidx(r, Px, pi, v) <= gc) mu = fmax(mu, fabs(F[o]));
+                if (L.row(r) <= gc) mu = fmax(mu, fabs(F[o]));
             }
         }
     }
@@ -185,47 +178,43 @@ int launch_recip(double* x, int n, cudaStream_t s) {
 }  // namespace
 
 // ---------------------------------------------------------------- per-share launches
-int equil_row_max(const double* A, int Ml, int Nl, int v, int Px, int pi, double* rowmax, int M, cudaStream_t s) {
-    CFLX_CUDA(cudaMemsetAsync(rowmax, 0, sizeof(double) * M, s));
-    if (Ml > 0 && Nl > 0) row_max_kernel<<<(Ml + 7) / 8, 256, 0, s>>>(A, Ml, Nl, v, Px, pi, rowmax);
+int equil_row_max(const double* A, const Layout& L, double* rowmax, cudaStream_t s) {
+    CFLX_CUDA(cudaMemsetAsync(rowmax, 0, sizeof(double) * L.M, s));
+    if (L.Ml > 0 && L.Nl > 0) row_max_kernel<<<(L.Ml + 7) / 8, 256, 0, s>>>(A, L, rowmax);
     CFLX_CUDA(cudaGetLastError());
     return CFLX_OK;
 }
 
-int equil_col_max(const double* A, int Ml, int Nl, int v, int Px, int Py, int pi, int pj, const double* r, double* colmax,
-                  int M, cudaStream_t s) {
-    CFLX_CUDA(cudaMemsetAsync(colmax, 0, sizeof(double) * M, s));
-    if (Ml > 0 && Nl > 0) {
-        const dim3 grid((Nl + EQ_COLS - 1) / EQ_COLS, (Ml + EQ_ROWS - 1) / EQ_ROWS);
-        col_max_kernel<<<grid, EQ_COLS, 0, s>>>(A, Ml, Nl, v, Px, Py, pi, pj, r, colmax);
+int equil_col_max(const double* A, const Layout& L, const double* r, double* colmax, cudaStream_t s) {
+    CFLX_CUDA(cudaMemsetAsync(colmax, 0, sizeof(double) * L.M, s));
+    if (L.Ml > 0 && L.Nl > 0) {
+        const dim3 grid((L.Nl + EQ_COLS - 1) / EQ_COLS, (L.Ml + EQ_ROWS - 1) / EQ_ROWS);
+        col_max_kernel<<<grid, EQ_COLS, 0, s>>>(A, L, r, colmax);
     }
     CFLX_CUDA(cudaGetLastError());
     return CFLX_OK;
 }
 
-int equil_diag(const double* A, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, double* diag, int M,
-               cudaStream_t s) {
-    CFLX_CUDA(cudaMemsetAsync(diag, 0, sizeof(double) * M, s));
-    diag_kernel<<<(M + 255) / 256, 256, 0, s>>>(A, Ml, Nl, v, Kappa, Px, Py, pi, pj, diag, M);
+int equil_diag(const double* A, const Layout& L, double* diag, cudaStream_t s) {
+    CFLX_CUDA(cudaMemsetAsync(diag, 0, sizeof(double) * L.M, s));
+    diag_kernel<<<(L.M + 255) / 256, 256, 0, s>>>(A, L, diag);
     CFLX_CUDA(cudaGetLastError());
     return CFLX_OK;
 }
 
-int equil_apply(double* A, int Ml, int Nl, int v, int Px, int Py, int pi, int pj, const double* r, const double* c,
-                char equed, cudaStream_t s) {
-    if (Ml <= 0 || Nl <= 0 || equed == 'N') return CFLX_OK;
-    const dim3 grid((Nl + 255) / 256, std::min((unsigned)Ml, MAX_GRID_Y));
-    if (equed == 'R') apply_kernel<'R'><<<grid, 256, 0, s>>>(A, Ml, Nl, v, Px, Py, pi, pj, r, c);
-    else if (equed == 'C') apply_kernel<'C'><<<grid, 256, 0, s>>>(A, Ml, Nl, v, Px, Py, pi, pj, r, c);
-    else apply_kernel<'B'><<<grid, 256, 0, s>>>(A, Ml, Nl, v, Px, Py, pi, pj, r, c);
+int equil_apply(double* A, const Layout& L, const double* r, const double* c, char equed, cudaStream_t s) {
+    if (L.Ml <= 0 || L.Nl <= 0 || equed == 'N') return CFLX_OK;
+    const dim3 grid((L.Nl + 255) / 256, std::min((unsigned)L.Ml, MAX_GRID_Y));
+    if (equed == 'R') apply_kernel<'R'><<<grid, 256, 0, s>>>(A, L, r, c);
+    else if (equed == 'C') apply_kernel<'C'><<<grid, 256, 0, s>>>(A, L, r, c);
+    else apply_kernel<'B'><<<grid, 256, 0, s>>>(A, L, r, c);
     CFLX_CUDA(cudaGetLastError());
     return CFLX_OK;
 }
 
-int equil_sym_apply(double* A, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, const double* sc,
-                    cudaStream_t s) {
-    if (Ml <= 0 || Nl <= 0) return CFLX_OK;
-    sym_apply_kernel<<<dim3((Nl + 255) / 256, std::min((unsigned)Ml, MAX_GRID_Y)), 256, 0, s>>>(A, Ml, Nl, v, Kappa, Px, Py, pi, pj, sc);
+int equil_sym_apply(double* A, const Layout& L, const double* sc, cudaStream_t s) {
+    if (L.Ml <= 0 || L.Nl <= 0) return CFLX_OK;
+    sym_apply_kernel<<<dim3((L.Nl + 255) / 256, std::min((unsigned)L.Ml, MAX_GRID_Y)), 256, 0, s>>>(A, L, sc);
     CFLX_CUDA(cudaGetLastError());
     return CFLX_OK;
 }
@@ -269,11 +258,12 @@ int equil_grow(EquilState* e, int M, int ldn) {
 }
 
 // ---------------------------------------------------------------- dgeequ + dlaqge
-int geequ_grid(cflx_comm* c, EquilState* e, double* A, int M, int Ml, int Nl, int v, int Px, int Py, int pi, int pj,
-               int pk, bool apply, double* r_out, double* c_out, double* rowcnd, double* colcnd, double* amax,
-               char* equed, int* info) {
+int geequ_grid(const Grid& g, EquilState* e, double* A, bool apply, double* r_out, double* c_out, double* rowcnd,
+               double* colcnd, double* amax, char* equed, int* info) {
+    cflx_comm* c = g.comm;
     cudaStream_t s = c->stream;
-    const bool layer0 = pk == 0;
+    const int M = g.M;
+    const bool layer0 = g.pk == 0;
     CFLX_TRY(grow_pair(&e->qr, &e->qc, &e->qcap, (size_t)M));
     double *r = e->qr, *cs = e->qc;
     std::vector<double> h;
@@ -291,7 +281,7 @@ int geequ_grid(cflx_comm* c, EquilState* e, double* A, int M, int Ml, int Nl, in
         return 0;
     };
     // row maxima, then r = reciprocals
-    if (layer0) CFLX_TRY(equil_row_max(A, Ml, Nl, v, Px, pi, r, M, s));
+    if (layer0) CFLX_TRY(equil_row_max(A, g, r, s));
     else CFLX_CUDA(cudaMemsetAsync(r, 0, sizeof(double) * M, s));
     CFLX_TRY(reduce_vec(c, r, M, ncclMax, h));
     double rcmin, rcmax;
@@ -309,7 +299,7 @@ int geequ_grid(cflx_comm* c, EquilState* e, double* A, int M, int Ml, int Nl, in
     if (r_out) std::copy(h.begin(), h.end(), r_out);
     *rowcnd = std::max(rcmin, SAFMIN) / std::min(rcmax, 1.0 / SAFMIN);
     // column maxima of |a| r, then c = reciprocals
-    if (layer0) CFLX_TRY(equil_col_max(A, Ml, Nl, v, Px, Py, pi, pj, r, cs, M, s));
+    if (layer0) CFLX_TRY(equil_col_max(A, g, r, cs, s));
     else CFLX_CUDA(cudaMemsetAsync(cs, 0, sizeof(double) * M, s));
     CFLX_TRY(reduce_vec(c, cs, M, ncclMax, h));
     minmax(&rcmin, &rcmax);
@@ -328,22 +318,24 @@ int geequ_grid(cflx_comm* c, EquilState* e, double* A, int M, int Ml, int Nl, in
     const double large = 1.0 / LAQ_SMALL;
     if (*rowcnd >= THRESH && *amax >= LAQ_SMALL && *amax <= large) *equed = *colcnd >= THRESH ? 'N' : 'C';
     else *equed = *colcnd >= THRESH ? 'R' : 'B';
-    if (layer0) CFLX_TRY(equil_apply(A, Ml, Nl, v, Px, Py, pi, pj, r, cs, *equed, s));
+    if (layer0) CFLX_TRY(equil_apply(A, g, r, cs, *equed, s));
     CFLX_CUDA(cudaStreamSynchronize(s));
     return CFLX_OK;
 }
 
 // ---------------------------------------------------------------- dpoequ + dlaqsy
-int poequ_grid(cflx_comm* c, EquilState* e, double* A, int N, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi,
-               int pj, int pk, bool apply, double* s_out, double* scond, double* amax, char* equed, int* info) {
+int poequ_grid(const Grid& g, EquilState* e, double* A, bool apply, double* s_out, double* scond, double* amax,
+               char* equed, int* info) {
+    cflx_comm* c = g.comm;
     cudaStream_t s = c->stream;
+    const int N = g.M;
     CFLX_TRY(grow_pair(&e->qr, &e->qc, &e->qcap, (size_t)N));
     double* sc = e->qr;
     std::vector<double> h;
     *info = 0;
     *scond = 0.0;
     *equed = 'N';
-    if (pk == 0) CFLX_TRY(equil_diag(A, Ml, Nl, v, Kappa, Px, Py, pi, pj, sc, N, s));
+    if (g.pk == 0) CFLX_TRY(equil_diag(A, g, sc, s));
     else CFLX_CUDA(cudaMemsetAsync(sc, 0, sizeof(double) * N, s));
     CFLX_TRY(reduce_vec(c, sc, N, ncclSum, h));  // one non-zero contributor per element: exact
     double smin = h[0], smax = h[0];
@@ -362,41 +354,39 @@ int poequ_grid(cflx_comm* c, EquilState* e, double* A, int N, int Ml, int Nl, in
     if (apply) {
         const double large = 1.0 / LAQ_SMALL;
         *equed = (*scond >= THRESH && smax >= LAQ_SMALL && smax <= large) ? 'N' : 'Y';
-        if (*equed == 'Y' && pk == 0) CFLX_TRY(equil_sym_apply(A, Ml, Nl, v, Kappa, Px, Py, pi, pj, sc, s));
+        if (*equed == 'Y' && g.pk == 0) CFLX_TRY(equil_sym_apply(A, g, sc, s));
     }
     CFLX_CUDA(cudaStreamSynchronize(s));
     return CFLX_OK;
 }
 
 // ---------------------------------------------------------------- reciprocal pivot growth
-int equil_zero_pivot(const double* F, int Ml, int Nl, int v, int M, int Px, int Py, int pi, int pj, int* zero_pivot,
-                     cudaStream_t s) {
+int equil_zero_pivot(const double* F, const Layout& L, int* zero_pivot, cudaStream_t s) {
     const int big = INT_MAX;
     CFLX_CUDA(cudaMemcpyAsync(zero_pivot, &big, sizeof(int), cudaMemcpyHostToDevice, s));
-    zero_pivot_kernel<<<(M + 255) / 256, 256, 0, s>>>(F, Ml, Nl, v, M, Px, Py, pi, pj, zero_pivot);
+    zero_pivot_kernel<<<(L.M + 255) / 256, 256, 0, s>>>(F, L, zero_pivot);
     CFLX_CUDA(cudaGetLastError());
     CFLX_CUDA(cudaStreamSynchronize(s));  // `big` is a host temporary
     return CFLX_OK;
 }
 
-int equil_growth(const double* F, const double* A, int Ml, int Nl, int v, int Px, int Py, int pi, int pj, int ncols,
-                 double* out2, cudaStream_t s) {
+int equil_growth(const double* F, const double* A, const Layout& L, int ncols, double* out2, cudaStream_t s) {
     CFLX_CUDA(cudaMemsetAsync(out2, 0, 2 * sizeof(double), s));
-    if (Ml > 0 && Nl > 0) {
-        const dim3 grid((Nl + EQ_COLS - 1) / EQ_COLS, (Ml + EQ_ROWS - 1) / EQ_ROWS);
-        growth_kernel<<<grid, EQ_COLS, 0, s>>>(F, A, Ml, Nl, v, Px, Py, pi, pj, ncols, out2);
+    if (L.Ml > 0 && L.Nl > 0) {
+        const dim3 grid((L.Nl + EQ_COLS - 1) / EQ_COLS, (L.Ml + EQ_ROWS - 1) / EQ_ROWS);
+        growth_kernel<<<grid, EQ_COLS, 0, s>>>(F, A, L, ncols, out2);
     }
     CFLX_CUDA(cudaGetLastError());
     return CFLX_OK;
 }
 
-int pivot_growth_grid(cflx_comm* c, EquilState* e, const double* F, const double* A, int M, int Ml, int Nl, int v, int Px,
-                      int Py, int pi, int pj, int pk, double* rpvgrw, int* info) {
+int pivot_growth_grid(const Grid& g, EquilState* e, const double* F, const double* A, double* rpvgrw, int* info) {
+    cflx_comm* c = g.comm;
     cudaStream_t s = c->stream;
     if (!e->growth) CFLX_TRY(dmalloc(&e->growth, 2));
     if (!e->ival) CFLX_TRY(dmalloc(&e->ival, 1));
-    if (pk == 0) {
-        CFLX_TRY(equil_zero_pivot(F, Ml, Nl, v, M, Px, Py, pi, pj, e->ival, s));
+    if (g.pk == 0) {
+        CFLX_TRY(equil_zero_pivot(F, g, e->ival, s));
     } else {  // only layer 0 holds the factors: this rank offers no zero pivot
         const int big = INT_MAX;
         CFLX_CUDA(cudaMemcpyAsync(e->ival, &big, sizeof(int), cudaMemcpyHostToDevice, s));
@@ -407,14 +397,36 @@ int pivot_growth_grid(cflx_comm* c, EquilState* e, const double* F, const double
     CFLX_CUDA(cudaMemcpyAsync(&first, e->ival, sizeof(int), cudaMemcpyDeviceToHost, s));
     CFLX_CUDA(cudaStreamSynchronize(s));
     *info = first == INT_MAX ? 0 : first;
-    const int ncols = *info ? *info : M;
-    if (pk == 0) CFLX_TRY(equil_growth(F, A, Ml, Nl, v, Px, Py, pi, pj, ncols, e->growth, s));
+    const int ncols = *info ? *info : g.M;
+    if (g.pk == 0) CFLX_TRY(equil_growth(F, A, g, ncols, e->growth, s));
     else CFLX_CUDA(cudaMemsetAsync(e->growth, 0, 2 * sizeof(double), s));
     if (c->world_size > 1) CFLX_NCCL(ncclAllReduce(e->growth, e->growth, 2, ncclDouble, ncclMax, c->world, s));
     double h[2];
     CFLX_CUDA(cudaMemcpyAsync(h, e->growth, sizeof(h), cudaMemcpyDeviceToHost, s));
     CFLX_CUDA(cudaStreamSynchronize(s));
     *rpvgrw = h[0] == 0.0 ? 1.0 : h[1] / h[0];  // dgesvx: dlange('M', A) / dlantr('M', 'U', AF)
+    return CFLX_OK;
+}
+
+// ---------------------------------------------------------------- the expert drivers' solve
+// B is scaled on the device, solved and refined there, and X is unscaled before the download
+int svx_tail(EquilState* e, RefineCache* rc, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx,
+             double* ferr, double* berr, const double* pre, const double* post, double cnd) {
+    cudaStream_t s = op.grid.comm->stream;
+    const int M = op.grid.M, ldn = (int)round_up(nrhs, 8);
+    CFLX_TRY(equil_grow(e, M, ldn));
+    double *dB = e->B, *dX = e->X;
+    CFLX_CUDA(cudaMemcpy2DAsync(dB, ldn * sizeof(double), B, (size_t)ldb * sizeof(double), nrhs * sizeof(double), M,
+                                cudaMemcpyDefault, s));
+    if (pre) CFLX_TRY(launch_scale_rows(dB, ldn, M, nrhs, pre, s));
+    CFLX_TRY(op.solve(false, nrhs, dB, ldn, dX, ldn));
+    CFLX_TRY(refine_run(rc, op, nrhs, dB, ldn, dX, ldn, ferr, berr));
+    if (post) CFLX_TRY(launch_scale_rows(dX, ldn, M, nrhs, post, s));
+    CFLX_CUDA(cudaMemcpy2DAsync(X, (size_t)ldx * sizeof(double), dX, ldn * sizeof(double), nrhs * sizeof(double), M,
+                                cudaMemcpyDefault, s));
+    CFLX_CUDA(cudaStreamSynchronize(s));
+    if (ferr && post)
+        for (int j = 0; j < nrhs; ++j) ferr[j] /= cnd;
     return CFLX_OK;
 }
 

@@ -166,17 +166,7 @@ int launch_gemm_narrow_tn(int M, int N, int K, const double* AT, int64_t ldat, c
                           cudaStream_t stream);
 
 // ---------------------------------------------------------------- refine.cu
-// The residual kernels (refine.cu).  From layer 0's share A (Ml x Nl, conflux layout, lda even, 16-byte aligned, v % 4 == 0)
-// and X gathered by local column (Xc, Nl x nrhs) or by local row (Xr, Ml x nrhs), both with leading dimension ldx:
-//   NN:       P = A Xc, Q = |A| |Xc| by local row (Ml rows);
-//   TN:       P = A^T Xr, Q = |A|^T |Xr| by local column (Nl rows);
-//   SymLower: the stored lower triangle of the real tiles (global tile index < Kappa): the NN product of the entries
-//             with global row >= global column into rows [0, Ml), the TN product of those with global row > global
-//             column into rows [Ml, Ml + Nl).  Nothing else is read.
-// P and Q have leading dimension ldo.  Deterministic: no floating-point atomics.
+// what the residual kernels multiply (lu_state.h launch_residual)
 enum class ResidMode { NN, TN, SymLower };
-int launch_residual(ResidMode mode, const double* A, int64_t lda, int Ml, int Nl, int v, int Kappa, int Px, int Py,
-                    int pi, int pj, const double* Xc, const double* Xr, int64_t ldx, int nrhs, double* P, double* Q,
-                    int64_t ldo, cudaStream_t s);
 
 }  // namespace cflx

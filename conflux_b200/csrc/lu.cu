@@ -106,6 +106,20 @@ int grid_barrier(cflx_comm* c) {
     CFLX_CUDA(cudaStreamSynchronize(c->stream));
     return CFLX_OK;
 }
+int grid_init(Grid* g, cflx_comm* c, int Px, int Py, int Pz) {
+    g->comm = c;
+    g->Px = Px; g->Py = Py; g->Pz = Pz; g->P = Px * Py * Pz;
+    g->rank = c->world_rank;
+    g->pi = g->rank / (Py * Pz);
+    g->pj = (g->rank / Pz) % Py;
+    g->pk = g->rank % Pz;
+    CFLX_TRY(make_sub(c, g->pi * Py + g->pj, g->pk, Pz, &g->k_comm));
+    return make_sub(c, g->pj * Pz + g->pk, g->pi, Px, &g->i_comm);
+}
+void grid_free(Grid* g) {
+    for (SubComm* sc : {&g->k_comm, &g->i_comm})
+        if (sc->c) ncclCommDestroy(sc->c);
+}
 }  // namespace cflx
 
 namespace {
@@ -516,8 +530,9 @@ void free_lu(cflx_lu* lu) {
     if (lu->copy) cudaStreamDestroy(lu->copy);
     if (lu->ev_a0_read) cudaEventDestroy(lu->ev_a0_read);
     if (lu->ev_upload) cudaEventDestroy(lu->ev_upload);
-    for (SubComm* sc : {&lu->k_comm, &lu->i_comm, &lu->jk_comm, &lu->ik_comm})
+    for (SubComm* sc : {&lu->jk_comm, &lu->ik_comm})
         if (sc->c) ncclCommDestroy(sc->c);
+    grid_free(lu);
     delete lu;
 }
 
@@ -525,10 +540,7 @@ void free_lu(cflx_lu* lu) {
 // The factors in the conflux layout of the validation path (Cbuf, as cflx_lu_get_factors leaves them), described to the
 // solve engine (solve.cu).  Every layer joins the grid-row reduces and grid-column broadcasts (jk / ik communicators,
 // layer 0 at rank p * Pz), the layers pk != 0 with zeros.
-SolveFactor lu_solve_factor(cflx_lu* lu) {
-    return SolveFactor{lu->comm, lu->Cbuf, lu->M, lu->Ml, lu->Nl, lu->Ml, lu->v, lu->nb, lu->Nt, lu->P, lu->Px, lu->Py,
-                       lu->pi, lu->pj, lu->pk, &lu->jk_comm, &lu->ik_comm, lu->Pz};
-}
+SolveFactor lu_solve_factor(cflx_lu* lu) { return SolveFactor{*lu, lu->Cbuf, lu->Ml, &lu->jk_comm, &lu->ik_comm, lu->Pz}; }
 
 // First call after a factorisation: the factors redistributed into Cbuf, the diagonal-block inverses, and on the ranks
 // that seed the right-hand side, the row of B that each local row of P*B comes from.
@@ -610,6 +622,46 @@ int lu_sweeps(cflx_lu* lu, bool transposed, bool pa, int nrhs, const double* B, 
     CFLX_TRY(solve_col_sweep(sc, f, ldn, true, Tri::UpperT, sc->Z, lu->Py, true));
     CFLX_TRY(solve_col_sweep(sc, f, ldn, false, Tri::UnitLowerT, sc->X, 1, false));
     return solve_finish(sc, f, ldn, nrhs, X, ldx, pa ? nullptr : sc->unperm);
+}
+
+// CFLX_OK when `what` may run: after a factorisation and, with own_input, while A0 still holds the input of that
+// factorisation; otherwise CFLX_ERR_STATE with the reason
+int lu_check(const cflx_lu* lu, const char* what, bool own_input) {
+    if (!lu->factored) {
+        set_last_error("%s requested before cflx_lu_factor, or after cflx_lu_set_local without a factorisation", what);
+        return CFLX_ERR_STATE;
+    }
+    if (own_input && lu->a0_is_next) {
+        set_last_error("%s refused: the input buffer of the last run was handed to the queued next matrix", what);
+        return CFLX_ERR_STATE;
+    }
+    return CFLX_OK;
+}
+
+// LAPACK dgecon on the grid, NORM = '1' or (inf) 'I': the norm of the input A0 (the padded M x M matrix), and the
+// Hager-Higham estimate of ||inv(P A)||_1 = ||inv(A)||_1 from inv(U) inv(L) x and inv(L)^T inv(U)^T x, as dgecon runs it
+// on L and U alone; ||inv(A)||_inf is the same estimate with the two kinds of product swapped.
+int lu_rcond(cflx_lu* lu, bool inf, double* rcond_out, double* anorm_out) {
+    double anorm = 0.0, ainvnm = 0.0;
+    CFLX_TRY(inf ? norminf_grid(*lu, lu->A0, &anorm) : norm1_grid(*lu, lu->A0, false, &anorm));
+    if (anorm > 0.0) {
+        // every rank runs the estimator on the X of solve_finish, bit-identical on every rank, so every rank makes the
+        // same choices and issues the same solves (the same collectives) in the same order
+        auto apply = [&](int kase, double* x) { return lu_sweeps(lu, (kase == 2) != inf, true, 1, x, 1, x, 1); };
+        CFLX_TRY(estimate_inv_norm1(lu->M, apply, &ainvnm));
+    }
+    *rcond_out = rcond_from(anorm, ainvnm);
+    if (anorm_out) *anorm_out = anorm;
+    return CFLX_OK;
+}
+
+// dgerfs on the input A0 with the solves above.  For trans = 0 the estimator's kase 1 (inv(A)^T) is the transposed solve
+// and kase 2 the plain one; for trans = 1 they swap.
+RefineOp lu_refine_op(cflx_lu* lu, bool t) {
+    auto solve = [lu, t](bool tk, int n, const double* b, int lb, double* x, int lx) {
+        return lu_sweeps(lu, t != tk, false, n, b, lb, x, lx);
+    };
+    return RefineOp{*lu, lu->A0, t ? ResidMode::TN : ResidMode::NN, false, solve};
 }
 }  // namespace
 
@@ -731,14 +783,10 @@ int cflx_init_matrix_host(int M, int N, int v, int Px, int Py, int Pz, int rank,
     if (d[0] == d[1]) {
         std::vector<double> tab;
         if (fixed_input_matrix(d[0], &tab)) {
-            const int n = d[0], pi = rank / (Py * Pz), pj = (rank / Pz) % Py;
-            for (int lr = 0; lr < Ml; ++lr) {
-                const int gi = ((lr / v) * Px + pi) * v + lr % v;
-                for (int lc = 0; lc < Nl; ++lc) {
-                    const int gj = ((lc / v) * Py + pj) * v + lc % v;
-                    out[(size_t)lr * Nl + lc] = tab[(size_t)gi * n + gj];
-                }
-            }
+            const int n = d[0];
+            const Layout L{n, v, d[4], Ml, Nl, Px, Py, rank / (Py * Pz), (rank / Pz) % Py};
+            for (int lr = 0; lr < Ml; ++lr)
+                for (int lc = 0; lc < Nl; ++lc) out[(size_t)lr * Nl + lc] = tab[(size_t)L.row(lr) * n + L.col(lc)];
             return CFLX_OK;
         }
     }
@@ -771,28 +819,21 @@ int cflx_lu_create(cflx_comm* c, int M, int N, int v, int Px, int Py, int Pz, cf
     }
     int d[8];
     CFLX_TRY(cflx_lu_dims(M, N, v, Px, Py, Pz, d));
-    auto* lu = new cflx_lu;
-    lu->comm = c;
-    lu->M = d[0]; lu->N = d[1]; lu->Ml = d[2]; lu->Nl = d[3]; lu->Nt = d[4]; lu->nlayr = d[5]; lu->Mt = d[6]; lu->P = d[7];
-    lu->v = v; lu->Px = Px; lu->Py = Py; lu->Pz = Pz;
-    lu->rank = c->world_rank;  // row-major cart numbering: rank = (pi*Py + pj)*Pz + pk
-    lu->pi = lu->rank / (Py * Pz);
-    lu->pj = (lu->rank / Pz) % Py;
-    lu->pk = lu->rank % Pz;
-    lu->nb = pick_nb(v);
-    if (lu->M != lu->N) {
+    if (d[0] != d[1]) {
         set_last_error("only square matrices are supported (the miniapp passes M = N)");
-        delete lu;
         return CFLX_ERR_UNSUPPORTED;
     }
+    auto* lu = new cflx_lu;
+    lu->M = d[0]; lu->N = d[1]; lu->Ml = d[2]; lu->Nl = d[3]; lu->Nt = d[4]; lu->nlayr = d[5]; lu->Mt = d[6];
+    lu->v = v;
+    lu->nb = pick_nb(v);
     int rc = CFLX_OK;
     auto fail = [&](int code) {
         free_lu(lu);
         return code;
     };
     // sub-communicators (all ranks call all splits, same order)
-    if ((rc = make_sub(c, lu->pi * Py + lu->pj, lu->pk, Pz, &lu->k_comm))) return fail(rc);
-    if ((rc = make_sub(c, lu->pj * Pz + lu->pk, lu->pi, Px, &lu->i_comm))) return fail(rc);
+    if ((rc = grid_init(lu, c, Px, Py, Pz))) return fail(rc);
     if ((rc = make_sub(c, lu->pi, lu->pj * Pz + lu->pk, Py * Pz, &lu->jk_comm))) return fail(rc);
     if ((rc = make_sub(c, lu->pj, lu->pi * Pz + lu->pk, Px * Pz, &lu->ik_comm))) return fail(rc);
 
@@ -1016,10 +1057,7 @@ int cflx_lu_factor(cflx_lu* lu, double* ms_out) {
 
 int cflx_lu_get_permutation(cflx_lu* lu, int* perm_out) {
     if (!lu || !perm_out) return CFLX_ERR_ARG;
-    if (!lu->factored) {
-        set_last_error("permutation requested before cflx_lu_factor");
-        return CFLX_ERR_STATE;
-    }
+    CFLX_TRY(lu_check(lu, "permutation", false));
     CFLX_CUDA(cudaSetDevice(lu->comm->device));
     CFLX_CUDA(cudaMemcpyAsync(lu->h_hist.data(), lu->hist, sizeof(int) * lu->M, cudaMemcpyDeviceToHost, lu->comm->stream));
     CFLX_CUDA(cudaStreamSynchronize(lu->comm->stream));
@@ -1032,10 +1070,7 @@ int cflx_lu_get_permutation(cflx_lu* lu, int* perm_out) {
 // row (k / Px)*v + i (conflux_opt.hpp:1673-1699,1721-1754): an all-to-all of whole rows inside each grid column.
 int cflx_lu_get_factors(cflx_lu* lu, double* C_host, int* perm_out) {
     if (!lu) return CFLX_ERR_ARG;
-    if (!lu->factored) {
-        set_last_error("factors requested before cflx_lu_factor");
-        return CFLX_ERR_STATE;
-    }
+    CFLX_TRY(lu_check(lu, "factors", false));
     cflx_comm* c = lu->comm;
     cudaStream_t s = c->stream;
     CFLX_CUDA(cudaSetDevice(c->device));
@@ -1055,14 +1090,7 @@ int cflx_lu_get_factors(cflx_lu* lu, double* C_host, int* perm_out) {
 // relative to ||A||_F, computed on the device grid with the library's own GEMM + NCCL (validate.cu).  COLLECTIVE.
 int cflx_lu_validate(cflx_lu* lu, double* frob_abs_out, double* frob_rel_out) {
     if (!lu) return CFLX_ERR_ARG;
-    if (!lu->factored) {
-        set_last_error("residual requested before cflx_lu_factor");
-        return CFLX_ERR_STATE;
-    }
-    if (lu->a0_is_next) {
-        set_last_error("residual refused: the input buffer of the last run was handed to the queued next matrix");
-        return CFLX_ERR_STATE;
-    }
+    CFLX_TRY(lu_check(lu, "residual", true));
     CFLX_CUDA(cudaSetDevice(lu->comm->device));
     std::vector<int> hist(lu->M);
     CFLX_TRY(cflx_lu_get_permutation(lu, hist.data()));
@@ -1076,10 +1104,7 @@ int cflx_lu_residual(cflx_lu* lu, double* rel_out) {
 // Reads only the factors, so a run whose input buffer was handed to the queued next matrix can still be solved.
 int cflx_lu_solve(cflx_lu* lu, int nrhs, const double* B, int ldb, double* X, int ldx) {
     if (!lu || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B) return CFLX_ERR_ARG;
-    if (!lu->factored) {
-        set_last_error("solve requested before cflx_lu_factor, or after cflx_lu_set_local without a factorisation");
-        return CFLX_ERR_STATE;
-    }
+    CFLX_TRY(lu_check(lu, "solve", false));
     CFLX_CUDA(cudaSetDevice(lu->comm->device));
     return lu_sweeps(lu, false, false, nrhs, B, ldb, X, ldx);
 }
@@ -1087,63 +1112,27 @@ int cflx_lu_solve(cflx_lu* lu, int nrhs, const double* B, int ldb, double* X, in
 // A^T X = B with the same factors and state rules: U^T Y = B, L^T W = Y by column-partial sweeps, then X = P^T W.
 int cflx_lu_solve_trans(cflx_lu* lu, int nrhs, const double* B, int ldb, double* X, int ldx) {
     if (!lu || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B) return CFLX_ERR_ARG;
-    if (!lu->factored) {
-        set_last_error("transposed solve requested before cflx_lu_factor, or after cflx_lu_set_local without a factorisation");
-        return CFLX_ERR_STATE;
-    }
+    CFLX_TRY(lu_check(lu, "transposed solve", false));
     CFLX_CUDA(cudaSetDevice(lu->comm->device));
     return lu_sweeps(lu, true, false, nrhs, B, ldb, X, ldx);
 }
 
-// LAPACK dgecon (NORM = '1') on the grid: ||A||_1 of the input A0 (the padded M x M matrix), and the Hager-Higham estimate
-// of ||inv(P A)||_1 = ||inv(A)||_1 from inv(U) inv(L) x and inv(L)^T inv(U)^T x, as dgecon runs it on L and U alone.
+// LAPACK dgecon (NORM = '1') on the grid (lu_rcond).
 int cflx_lu_rcond(cflx_lu* lu, double* rcond_out, double* anorm_out) {
     if (!lu || !rcond_out) return CFLX_ERR_ARG;
-    if (!lu->factored) {
-        set_last_error("condition estimate requested before cflx_lu_factor, or after cflx_lu_set_local without a factorisation");
-        return CFLX_ERR_STATE;
-    }
-    if (lu->a0_is_next) {
-        set_last_error("condition estimate refused: the input buffer of the last run was handed to the queued next matrix");
-        return CFLX_ERR_STATE;
-    }
+    CFLX_TRY(lu_check(lu, "condition estimate", true));
     CFLX_CUDA(cudaSetDevice(lu->comm->device));
-    double anorm = 0.0, ainvnm = 0.0;
-    CFLX_TRY(norm1_grid(lu->comm, lu->A0, lu->M, lu->Ml, lu->Nl, lu->v, lu->Nt, lu->Px, lu->Py, lu->pi, lu->pj, lu->pk,
-                        false, &anorm));
-    if (anorm > 0.0) {
-        // every rank runs the estimator on the X of solve_finish, bit-identical on every rank, so every rank makes the
-        // same choices and issues the same solves (the same collectives) in the same order
-        auto apply = [&](int kase, double* x) { return lu_sweeps(lu, kase == 2, true, 1, x, 1, x, 1); };
-        CFLX_TRY(estimate_inv_norm1(lu->M, apply, &ainvnm));
-    }
-    *rcond_out = rcond_from(anorm, ainvnm);
-    if (anorm_out) *anorm_out = anorm;
-    return CFLX_OK;
+    return lu_rcond(lu, false, rcond_out, anorm_out);
 }
 
 // COLLECTIVE.  LAPACK dgerfs on the grid: residuals of the input A0 (refine.cu), corrections and the forward-error
-// estimator's products by the solves above.  For trans = 0 the estimator's kase 1 (inv(A)^T) is the transposed solve and
-// kase 2 the plain one; for trans = 1 they swap.
+// estimator's products by the solves above (lu_refine_op).
 int cflx_lu_refine(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, double* X, int ldx, double* ferr_out,
                    double* berr_out) {
     if (!lu || (trans != 0 && trans != 1) || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B || !X) return CFLX_ERR_ARG;
-    if (!lu->factored) {
-        set_last_error("refinement requested before cflx_lu_factor, or after cflx_lu_set_local without a factorisation");
-        return CFLX_ERR_STATE;
-    }
-    if (lu->a0_is_next) {
-        set_last_error("refinement refused: the input buffer of the last run was handed to the queued next matrix");
-        return CFLX_ERR_STATE;
-    }
+    CFLX_TRY(lu_check(lu, "refinement", true));
     CFLX_CUDA(cudaSetDevice(lu->comm->device));
-    const bool t = trans != 0;
-    auto solve = [lu, t](bool tk, int n, const double* b, int lb, double* x, int lx) {
-        return lu_sweeps(lu, t != tk, false, n, b, lb, x, lx);
-    };
-    const RefineOp op{lu->comm, lu->A0, t ? ResidMode::TN : ResidMode::NN, lu->M, lu->Ml, lu->Nl, lu->v, lu->Nt, lu->Px,
-                      lu->Py, lu->Pz, lu->pi, lu->pj, lu->pk, false, solve};
-    return refine_run(&lu->sv.rf, op, nrhs, B, ldb, X, ldx, ferr_out, berr_out);
+    return refine_run(&lu->sv.rf, lu_refine_op(lu, trans != 0), nrhs, B, ldb, X, ldx, ferr_out, berr_out);
 }
 
 // COLLECTIVE.  LAPACK dgeequ (+ dlaqge when apply) on the input A0 (equil.cu).  The input changes, so the factorisation
@@ -1168,8 +1157,7 @@ int cflx_lu_equilibrate(cflx_lu* lu, int apply, double* r_out, double* c_out, do
     double rowcnd = 0.0, colcnd = 0.0, amax = 0.0;
     char equed = 'N';
     int info = 0;
-    CFLX_TRY(geequ_grid(lu->comm, &lu->eq, lu->A0, lu->M, lu->Ml, lu->Nl, lu->v, lu->Px, lu->Py, lu->pi, lu->pj, lu->pk,
-                        apply != 0, r_out, c_out, &rowcnd, &colcnd, &amax, &equed, &info));
+    CFLX_TRY(geequ_grid(*lu, &lu->eq, lu->A0, apply != 0, r_out, c_out, &rowcnd, &colcnd, &amax, &equed, &info));
     // the input's record changes only when this call scaled it; a query (apply = 0) leaves the record and its scales
     if (apply && info == 0) CFLX_TRY(equil_record_set(&lu->eq.in, equed, rowcnd, colcnd, lu->eq.qr, lu->eq.qc, lu->M, s));
     if (rowcnd_out) *rowcnd_out = rowcnd;
@@ -1186,16 +1174,8 @@ int cflx_lu_svx(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, doub
                 double* ferr_out, double* berr_out, double* rpvgrw_out, char* equed_out, int* info_out) {
     if (!lu || (trans != 0 && trans != 1) || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B || !X || !rcond_out || !info_out)
         return CFLX_ERR_ARG;
-    if (!lu->factored) {
-        set_last_error("expert solve requested before cflx_lu_factor, or after cflx_lu_set_local without a factorisation");
-        return CFLX_ERR_STATE;
-    }
-    if (lu->a0_is_next) {
-        set_last_error("expert solve refused: the input buffer of the last run was handed to the queued next matrix");
-        return CFLX_ERR_STATE;
-    }
+    CFLX_TRY(lu_check(lu, "expert solve", true));
     CFLX_CUDA(cudaSetDevice(lu->comm->device));
-    cudaStream_t s = lu->comm->stream;
     const bool t = trans != 0;
     const EquilRecord& eq = lu->eq.fac;
     const bool rowequ = eq.equed == 'R' || eq.equed == 'B', colequ = eq.equed == 'C' || eq.equed == 'B';
@@ -1203,48 +1183,23 @@ int cflx_lu_svx(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, doub
     if (!lu->sv.ready) CFLX_TRY(lu_solve_prepare(lu));
     double rpvgrw = 1.0;
     int info = 0;
-    CFLX_TRY(pivot_growth_grid(lu->comm, &lu->eq, lu->Cbuf, lu->A0, lu->M, lu->Ml, lu->Nl, lu->v, lu->Px, lu->Py, lu->pi,
-                               lu->pj, lu->pk, &rpvgrw, &info));
+    CFLX_TRY(pivot_growth_grid(*lu, &lu->eq, lu->Cbuf, lu->A0, &rpvgrw, &info));
     if (rpvgrw_out) *rpvgrw_out = rpvgrw;
     *info_out = info;
     if (info > 0) {  // exactly singular U: no solution
         *rcond_out = 0.0;
         return CFLX_OK;
     }
-    // dgecon with NORM = '1' (trans 0, as cflx_lu_rcond) or 'I' (trans 1: the two kinds of product swap)
-    double anorm = 0.0, ainvnm = 0.0;
-    if (!t) CFLX_TRY(norm1_grid(lu->comm, lu->A0, lu->M, lu->Ml, lu->Nl, lu->v, lu->Nt, lu->Px, lu->Py, lu->pi, lu->pj,
-                                lu->pk, false, &anorm));
-    else CFLX_TRY(norminf_grid(lu->comm, lu->A0, lu->M, lu->Ml, lu->Nl, lu->v, lu->Px, lu->pi, lu->pk, &anorm));
-    if (anorm > 0.0) {
-        auto apply = [&](int kase, double* x) { return lu_sweeps(lu, (kase == 2) != t, true, 1, x, 1, x, 1); };
-        CFLX_TRY(estimate_inv_norm1(lu->M, apply, &ainvnm));
-    }
-    const double rcond = rcond_from(anorm, ainvnm);
+    // dgecon with NORM = '1' (trans 0, as cflx_lu_rcond) or 'I' (trans 1)
+    double rcond = 0.0;
+    CFLX_TRY(lu_rcond(lu, t, &rcond, nullptr));
     *rcond_out = rcond;
-    // B scaled on the device, solved and refined there, X unscaled before the download
-    const int M = lu->M, ldn = (int)round_up(nrhs, 8);
-    CFLX_TRY(equil_grow(&lu->eq, M, ldn));
-    double *dB = lu->eq.B, *dX = lu->eq.X;
-    CFLX_CUDA(cudaMemcpy2DAsync(dB, ldn * sizeof(double), B, (size_t)ldb * sizeof(double), nrhs * sizeof(double), M,
-                                cudaMemcpyDefault, s));
-    if (!t && rowequ) CFLX_TRY(launch_scale_rows(dB, ldn, M, nrhs, eq.r, s));
-    if (t && colequ) CFLX_TRY(launch_scale_rows(dB, ldn, M, nrhs, eq.c, s));
-    CFLX_TRY(lu_sweeps(lu, t, false, nrhs, dB, ldn, dX, ldn));
-    auto solve = [lu, t](bool tk, int n, const double* b, int lb, double* x, int lx) {
-        return lu_sweeps(lu, t != tk, false, n, b, lb, x, lx);
-    };
-    const RefineOp op{lu->comm, lu->A0, t ? ResidMode::TN : ResidMode::NN, M, lu->Ml, lu->Nl, lu->v, lu->Nt, lu->Px,
-                      lu->Py, lu->Pz, lu->pi, lu->pj, lu->pk, false, solve};
-    CFLX_TRY(refine_run(&lu->sv.rf, op, nrhs, dB, ldn, dX, ldn, ferr_out, berr_out));
-    if (!t && colequ) CFLX_TRY(launch_scale_rows(dX, ldn, M, nrhs, eq.c, s));
-    if (t && rowequ) CFLX_TRY(launch_scale_rows(dX, ldn, M, nrhs, eq.r, s));
-    CFLX_CUDA(cudaMemcpy2DAsync(X, (size_t)ldx * sizeof(double), dX, ldn * sizeof(double), nrhs * sizeof(double), M,
-                                cudaMemcpyDefault, s));
-    CFLX_CUDA(cudaStreamSynchronize(s));
-    if (ferr_out && ((!t && colequ) || (t && rowequ)))
-        for (int j = 0; j < nrhs; ++j) ferr_out[j] /= t ? eq.rowcnd : eq.colcnd;
-    if (rcond < std::ldexp(1.0, -53)) *info_out = M + 1;
+    // op(A) X = B: B is scaled by the scales of the rows of op(A), X by those of its columns
+    const double *r = rowequ ? eq.r : nullptr, *c = colequ ? eq.c : nullptr;
+    const RefineOp op = lu_refine_op(lu, t);
+    if (!t) CFLX_TRY(svx_tail(&lu->eq, &lu->sv.rf, op, nrhs, B, ldb, X, ldx, ferr_out, berr_out, r, c, eq.colcnd));
+    else CFLX_TRY(svx_tail(&lu->eq, &lu->sv.rf, op, nrhs, B, ldb, X, ldx, ferr_out, berr_out, c, r, eq.rowcnd));
+    if (rcond < std::ldexp(1.0, -53)) *info_out = lu->M + 1;
     return CFLX_OK;
 }
 

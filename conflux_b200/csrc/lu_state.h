@@ -67,6 +67,44 @@ int grid_barrier(cflx_comm* c);
 // first local tile row (column) whose global tile index is >= g, on grid row (column) p of P
 inline int first_local_tile(int g, int p, int P) { return g <= p ? 0 : (g - p + P - 1) / P; }
 
+// A rank's share of the M x M block-cyclic matrix, as every pass over the input reads it: global tile (I, J) lives on
+// grid position (I % Px, J % Py) at local tile (I / Px, J / Py) of the row-major Ml x Nl share.  Plain ints: kernels take
+// it by value.
+struct Layout {
+    int M = 0;   // padded global order
+    int v = 0;   // tile
+    int Nt = 0;  // real tiles on the diagonal (the LU's Nt, the reference's Kappa on the Cholesky path)
+    int Ml = 0, Nl = 0;
+    int Px = 1, Py = 1, pi = 0, pj = 0;
+
+    // global index of local index l at position p of a grid dimension of P
+    __host__ __device__ static int global(int l, int P, int p, int v) { return ((l / v) * P + p) * v + l % v; }
+    // the global row of local row r and the global column of local column c (I: the width of the result)
+    template <class I = int>
+    __host__ __device__ I row(int r) const { return ((I)(r / v) * Px + pi) * v + r % v; }
+    template <class I = int>
+    __host__ __device__ I col(int c) const { return ((I)(c / v) * Py + pj) * v + c % v; }
+    // this share holds diagonal tile t, at local rows / columns from diag_row(t) / diag_col(t)
+    __host__ __device__ bool holds_diag(int t) const {
+        return t % Px == pi && t % Py == pj && diag_row(t) < Ml && diag_col(t) < Nl;
+    }
+    __host__ __device__ int diag_row(int t) const { return (t / Px) * v; }
+    __host__ __device__ int diag_col(int t) const { return (t / Py) * v; }
+};
+
+// A handle's process grid: the layout of this rank's share, its place in the Px x Py x Pz grid (row-major numbering,
+// rank = (pi * Py + pj) * Pz + pk), and the sub-communicators every handle makes.
+struct Grid : Layout {
+    cflx_comm* comm = nullptr;
+    int Pz = 1, P = 1, pk = 0, rank = 0;
+    int nlayr = 0;  // contraction indices of one z layer
+    int nb = 0;     // diagonal inverse block
+    SubComm k_comm, i_comm;
+};
+// the rank's grid position, then the k (same (pi, pj)) and i (same (pj, pk)) splits, in this order on every rank
+int grid_init(Grid* g, cflx_comm* c, int Px, int Py, int Pz);
+void grid_free(Grid* g);
+
 // ---------------------------------------------------------------- the solve engine (solve.cu)
 // ---------------------------------------------------------------- iterative refinement (refine.cu)
 // Device buffers of cflx_lu_refine / cflx_chol_refine, grown and never shrunk, freed with the solve cache.  gl_cols /
@@ -142,26 +180,22 @@ struct SolveSeed {
     double* dst;
 };
 
-// One factor in the conflux block-cyclic layout, as the engine reads it: tile (I, J) on rank (I % Px, J % Py, 0) at
-// local tile (I / Px, J / Py) of F (layer 0, row-major, leading dimension Nl).  A rank's NCCL rank in the grid-row
-// communicator is pj * stride (+ pk), in the grid-column communicator pi * stride (+ pk).
+// One factor in the conflux block-cyclic layout of its grid g, as the engine reads it: tile (I, J) on rank
+// (I % Px, J % Py, 0) at local tile (I / Px, J / Py) of F (layer 0, row-major, leading dimension Nl; B and X have M rows).
+// A rank's NCCL rank in the grid-row communicator is pj * stride (+ pk), in the grid-column communicator pi * stride
+// (+ pk).
 struct SolveFactor {
-    cflx_comm* comm;
+    const Grid& g;
     const double* F;
-    int M, Ml, Nl;  // rows of B and X; local rows (of W) and columns (of F and Z)
-    int rows;       // local rows of the tiles the sweeps read and seed
-    int v, nb, Nt;  // tile, diagonal inverse block, tiles on the diagonal
-    int P, Px, Py, pi, pj, pk;
+    int rows;  // local rows of the tiles the sweeps read and seed
     const SubComm *row_comm, *col_comm;
     int stride;
 };
 }  // namespace cflx
 
-struct cflx_lu {
-    cflx_comm* comm = nullptr;
-    int M = 0, N = 0, v = 0, Px = 1, Py = 1, Pz = 1, P = 1, Ml = 0, Nl = 0, Nt = 0, Mt = 0, nlayr = 0;
-    int pi = 0, pj = 0, pk = 0, rank = 0, nb = 0;
-    cflx::SubComm k_comm, i_comm, jk_comm, ik_comm;
+struct cflx_lu : cflx::Grid {
+    int N = 0, Mt = 0;
+    cflx::SubComm jk_comm, ik_comm;
     // device memory
     double *A0 = nullptr, *A11 = nullptr, *PT = nullptr, *PT2 = nullptr, *W = nullptr, *LT = nullptr, *A01raw = nullptr,
            *U = nullptr, *tmp = nullptr, *A00 = nullptr, *A00T = nullptr, *Uinv = nullptr, *LinvT = nullptr,
@@ -237,11 +271,10 @@ int solve_finish(SolveCache* sc, const SolveFactor& f, int ldn, int nrhs, double
 // (kase 1) or inv(A)^T x (kase 2) and returns a status.  Pure host logic on x: ranks that pass bit-identical vectors
 // make the same choices, so every rank calls `apply` the same number of times with the same kase.
 int estimate_inv_norm1(int n, const std::function<int(int, double*)>& apply, double* est);
-// the collective 1-norm of the matrix whose layer-0 shares are A (Ml x Nl, conflux layout), into *anorm (every rank).
+// the collective 1-norm of the matrix whose layer-0 shares are A (g's layout), into *anorm (every rank).
 // lower_sym: only the lower triangle of the real tiles (global tile index < Nt) is stored and the matrix is its symmetric
 // completion; otherwise every local entry of the M x M matrix counts.  Deterministic: no floating-point atomics.
-int norm1_grid(cflx_comm* c, const double* A, int M, int Ml, int Nl, int v, int Nt, int Px, int Py, int pi, int pj,
-               int pk, bool lower_sym, double* anorm);
+int norm1_grid(const Grid& g, const double* A, bool lower_sym, double* anorm);
 // rcond = (1 / ainvnm) / anorm as LAPACK's dgecon / dpocon form it; 0 when anorm is 0 or the estimate is not finite
 double rcond_from(double anorm, double ainvnm);
 
@@ -260,14 +293,13 @@ struct Lacn2 {
     int step();
 };
 
-// What refine_run needs of a factorisation: the input's layer-0 share and its layout, and the solves.
+// What refine_run needs of a factorisation: its grid, the input's layer-0 share, and the solves.
 // solve(transposed, nrhs, B, ldb, X, ldx) overwrites X with inv(op A) B (transposed: inv(op A)^T B); B and X are host or
 // device arrays of M rows; it synchronises the stream.  symmetric: both kinds are the same solve.
 struct RefineOp {
-    cflx_comm* comm;
+    const Grid& grid;
     const double* A;
     ResidMode mode;
-    int M, Ml, Nl, v, Kappa, Px, Py, Pz, pi, pj, pk;
     bool symmetric;
     std::function<int(bool, int, const double*, int, double*, int)> solve;
 };
@@ -276,46 +308,53 @@ struct RefineOp {
 int refine_run(RefineCache* rc, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx, double* ferr,
                double* berr);
 void refine_cache_free(RefineCache* rc);
+// The residual kernels (refine.cu).  From layer 0's share A (L's layout, lda = Nl even, 16-byte aligned, v % 4 == 0)
+// and X gathered by local column (Xc, Nl x nrhs) or by local row (Xr, Ml x nrhs), both with leading dimension ldx:
+//   NN:       P = A Xc, Q = |A| |Xc| by local row (Ml rows);
+//   TN:       P = A^T Xr, Q = |A|^T |Xr| by local column (Nl rows);
+//   SymLower: the stored lower triangle of the real tiles (global tile index < Nt): the NN product of the entries
+//             with global row >= global column into rows [0, Ml), the TN product of those with global row > global
+//             column into rows [Ml, Ml + Nl).  Nothing else is read.
+// P and Q have leading dimension ldo.  Deterministic: no floating-point atomics.
+int launch_residual(ResidMode mode, const double* A, const Layout& L, const double* Xc, const double* Xr, int64_t ldx,
+                    int nrhs, double* P, double* Q, int64_t ldo, cudaStream_t s);
+// The solve and refinement of cflx_lu_svx / cflx_chol_svx (equil.cu), COLLECTIVE: B (host or device) to the device, its
+// rows scaled by pre (may be null), X = op.solve(false, B), refine_run, the rows of X scaled by post (may be null), X out;
+// when post is not null, ferr is divided by cnd.
+int svx_tail(EquilState* e, RefineCache* rc, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx,
+             double* ferr, double* berr, const double* pre, const double* post, double cnd);
 
 // norm.cu: the collective infinity-norm (maximum row sum) of the M x M matrix whose layer-0 shares are A (every local
 // entry counts), into *anorm (every rank).  Deterministic: no floating-point atomics.
-int norminf_grid(cflx_comm* c, const double* A, int M, int Ml, int Nl, int v, int Px, int pi, int pk, double* anorm);
+int norminf_grid(const Grid& g, const double* A, double* anorm);
 
-// equil.cu.  Per-share kernels (layer 0's share A, Ml x Nl, conflux layout); each writes an M-vector indexed by global
-// row / column with zeros where this share holds nothing:
+// equil.cu.  Per-share kernels (layer 0's share A in L's layout); each writes an M-vector indexed by global row / column
+// with zeros where this share holds nothing:
 //   rowmax[g] = max |a_gj| over this share's row g;  colmax[g] = max |a_ig| r_i over this share's column g;
-//   diag[g] = a_gg where this share holds the diagonal entry (real tiles, global tile index < Kappa).
+//   diag[g] = a_gg where this share holds the diagonal entry (real tiles, global tile index < Nt).
 // The apply passes scale A in place: equed 'R' a_ij = r_i a_ij, 'C' c_j a_ij, 'B' (c_j r_i) a_ij, over every local entry;
 // sym_apply: (s_j s_i) a_ij over the stored lower triangle of the real tiles only.
-int equil_row_max(const double* A, int Ml, int Nl, int v, int Px, int pi, double* rowmax, int M, cudaStream_t s);
-int equil_col_max(const double* A, int Ml, int Nl, int v, int Px, int Py, int pi, int pj, const double* r, double* colmax,
-                  int M, cudaStream_t s);
-int equil_diag(const double* A, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, double* diag, int M,
-               cudaStream_t s);
-int equil_apply(double* A, int Ml, int Nl, int v, int Px, int Py, int pi, int pj, const double* r, const double* c,
-                char equed, cudaStream_t s);
-int equil_sym_apply(double* A, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, const double* sc,
-                    cudaStream_t s);
+int equil_row_max(const double* A, const Layout& L, double* rowmax, cudaStream_t s);
+int equil_col_max(const double* A, const Layout& L, const double* r, double* colmax, cudaStream_t s);
+int equil_diag(const double* A, const Layout& L, double* diag, cudaStream_t s);
+int equil_apply(double* A, const Layout& L, const double* r, const double* c, char equed, cudaStream_t s);
+int equil_sym_apply(double* A, const Layout& L, const double* sc, cudaStream_t s);
 // On a share F of L\U (and A of the input): *zero_pivot = min(1 + g) over the global diagonal entries g < M the share
 // holds with F_gg == 0 (INT_MAX: none); out2 = {max |F| over global row <= global column, max |A|}, both over the global
 // columns < ncols (zeros where the share holds none).
-int equil_zero_pivot(const double* F, int Ml, int Nl, int v, int M, int Px, int Py, int pi, int pj, int* zero_pivot,
-                     cudaStream_t s);
-int equil_growth(const double* F, const double* A, int Ml, int Nl, int v, int Px, int Py, int pi, int pj, int ncols,
-                 double* out2, cudaStream_t s);
+int equil_zero_pivot(const double* F, const Layout& L, int* zero_pivot, cudaStream_t s);
+int equil_growth(const double* F, const double* A, const Layout& L, int ncols, double* out2, cudaStream_t s);
 // LAPACK dgeequ (+ dlaqge when `apply`) on the grid, COLLECTIVE: the scales into e->qr / e->qc (no record changes) and
 // the host results; r_out / c_out (M, may be null).  Scales are applied only when info == 0.
-int geequ_grid(cflx_comm* c, EquilState* e, double* A, int M, int Ml, int Nl, int v, int Px, int Py, int pi, int pj,
-               int pk, bool apply, double* r_out, double* c_out, double* rowcnd, double* colcnd, double* amax,
-               char* equed, int* info);
+int geequ_grid(const Grid& g, EquilState* e, double* A, bool apply, double* r_out, double* c_out, double* rowcnd,
+               double* colcnd, double* amax, char* equed, int* info);
 // LAPACK dpoequ (+ dlaqsy, UPLO = 'L', when `apply`) on the grid, COLLECTIVE: s into e->qr (no record changes)
-int poequ_grid(cflx_comm* c, EquilState* e, double* A, int N, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi,
-               int pj, int pk, bool apply, double* s_out, double* scond, double* amax, char* equed, int* info);
+int poequ_grid(const Grid& g, EquilState* e, double* A, bool apply, double* s_out, double* scond, double* amax,
+               char* equed, int* info);
 // dgesvx's reciprocal pivot growth on the grid, COLLECTIVE: F is L\U and A the input (both layer-0 shares of the M x M
 // matrix).  info = 1 + the first global k with U(k,k) == 0 (0: none); rpvgrw = max |A| / max |triu(U)| over the global
 // columns < (info ? info : M), or 1 when the denominator is 0.
-int pivot_growth_grid(cflx_comm* c, EquilState* e, const double* F, const double* A, int M, int Ml, int Nl, int v, int Px,
-                      int Py, int pi, int pj, int pk, double* rpvgrw, int* info);
+int pivot_growth_grid(const Grid& g, EquilState* e, const double* F, const double* A, double* rpvgrw, int* info);
 // the svx work buffers for nrhs columns (ldn = round_up(nrhs, 8)): e->B and e->X, M x ldn
 int equil_grow(EquilState* e, int M, int ldn);
 // X[i][j] *= d[i] for i < M, j < n (ld), on the device

@@ -1,7 +1,6 @@
 // conflux_b200/csrc/norm.cu -- ||A||_1 of the input a factorisation keeps on the device (cflx_lu_rcond, cflx_chol_rcond).
 //
-// One pass over layer 0's local share A (Ml x Nl, conflux layout: local (r, c) is global (((r / v) Px + pi) v + r % v,
-// ((c / v) Py + pj) v + c % v)) writes per-CTA partial sums of |a| by local column and, for a matrix stored as its lower
+// One pass over layer 0's local share A (Ml x Nl, conflux layout: local (r, c) is global (L.row(r), L.col(c))) writes per-CTA partial sums of |a| by local column and, for a matrix stored as its lower
 // triangle, by local row; a second kernel adds them in a fixed order into an M-vector of this rank's share of every
 // global column sum; an all-reduce over the world adds the ranks' shares, and the host takes the maximum.  No
 // floating-point atomics: every call, and every rank, gets the same bits.  Every sum is compensated (Neumaier), so a
@@ -32,9 +31,9 @@ __device__ __forceinline__ void acc(double& s, double& c, double a) {
 // colp[blockIdx.y][c] = sum of |A[r][c]| over this CTA's rows (masked); SYM: rowp[blockIdx.x][r] = the strictly lower
 // part of row r over this CTA's columns
 template <bool SYM>
-__global__ void __launch_bounds__(NCOL) abs_sums_kernel(const double* __restrict__ A, int Ml, int Nl, int v, int Nt, int Px,
-                                                        int Py, int pi, int pj, double* __restrict__ colp,
+__global__ void __launch_bounds__(NCOL) abs_sums_kernel(const double* __restrict__ A, Layout L, double* __restrict__ colp,
                                                         double* __restrict__ rowp) {
+    const int Ml = L.Ml, Nl = L.Nl, v = L.v, Nt = L.Nt, Px = L.Px, Py = L.Py, pi = L.pi, pj = L.pj;
     __shared__ double sh[SYM ? SUB : 1][NCOL + 1];
     const int c = blockIdx.x * NCOL + threadIdx.x, r0 = blockIdx.y * NROW, r1 = min(r0 + NROW, Ml);
     const bool cin = c < Nl;
@@ -77,7 +76,8 @@ __global__ void __launch_bounds__(NCOL) abs_sums_kernel(const double* __restrict
 // out[g] = this rank's share of the sum of |a| over global column g, from the partials in a fixed order
 template <bool SYM>
 __global__ void column_sums_kernel(const double* __restrict__ colp, int ncp, const double* __restrict__ rowp, int nrp,
-                                   int M, int Ml, int Nl, int v, int Px, int Py, int pi, int pj, double* __restrict__ out) {
+                                   Layout L, double* __restrict__ out) {
+    const int M = L.M, Ml = L.Ml, Nl = L.Nl, v = L.v, Px = L.Px, Py = L.Py, pi = L.pi, pj = L.pj;
     const int g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= M) return;
     const int gt = g / v, e = g % v;
@@ -94,31 +94,32 @@ __global__ void column_sums_kernel(const double* __restrict__ colp, int ncp, con
 }
 // out[g] = the sum of |a| over local row r (global row g) of this share: one warp per row, each lane a compensated sum
 // over the columns lane, lane + 32, ..., then the same shuffle tree as the row sums above
-__global__ void row_abs_sums_kernel(const double* __restrict__ A, int Ml, int Nl, int v, int Px, int pi,
-                                    double* __restrict__ out) {
+__global__ void row_abs_sums_kernel(const double* __restrict__ A, Layout L, double* __restrict__ out) {
     const int r = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-    if (r >= Ml) return;
-    const double* a = A + (int64_t)r * Nl;
+    if (r >= L.Ml) return;
+    const double* a = A + (int64_t)r * L.Nl;
     double t = 0.0, tc = 0.0;
-    for (int c = lane; c < Nl; c += 32) acc(t, tc, fabs(a[c]));
+    for (int c = lane; c < L.Nl; c += 32) acc(t, tc, fabs(a[c]));
     for (int o = 16; o > 0; o >>= 1) {
         const double u = __shfl_xor_sync(0xffffffffu, t, o), uc = __shfl_xor_sync(0xffffffffu, tc, o);
         tc += uc;
         acc(t, tc, u);
     }
-    if (lane == 0) out[((r / v) * Px + pi) * v + r % v] = t + tc;
+    if (lane == 0) out[L.row(r)] = t + tc;
 }
 }  // namespace
 
-int norminf_grid(cflx_comm* c, const double* A, int M, int Ml, int Nl, int v, int Px, int pi, int pk, double* anorm) {
+int norminf_grid(const Grid& g, const double* A, double* anorm) {
+    cflx_comm* c = g.comm;
     cudaStream_t s = c->stream;
+    const int M = g.M;
     double* out = nullptr;
     CFLX_TRY(dmalloc(&out, (size_t)M));
     std::vector<double> h(M);
     auto run = [&]() -> int {
         CFLX_CUDA(cudaMemsetAsync(out, 0, sizeof(double) * M, s));
-        if (pk == 0 && Ml > 0) {  // only layer 0 holds the input
-            row_abs_sums_kernel<<<(Ml + 7) / 8, 256, 0, s>>>(A, Ml, Nl, v, Px, pi, out);
+        if (g.pk == 0 && g.Ml > 0) {  // only layer 0 holds the input
+            row_abs_sums_kernel<<<(g.Ml + 7) / 8, 256, 0, s>>>(A, g, out);
             CFLX_CUDA(cudaGetLastError());
         }
         if (c->world_size > 1) CFLX_NCCL(ncclAllReduce(out, out, (size_t)M, ncclDouble, ncclSum, c->world, s));
@@ -135,9 +136,10 @@ int norminf_grid(cflx_comm* c, const double* A, int M, int Ml, int Nl, int v, in
     return CFLX_OK;
 }
 
-int norm1_grid(cflx_comm* c, const double* A, int M, int Ml, int Nl, int v, int Nt, int Px, int Py, int pi, int pj,
-               int pk, bool lower_sym, double* anorm) {
+int norm1_grid(const Grid& g, const double* A, bool lower_sym, double* anorm) {
+    cflx_comm* c = g.comm;
     cudaStream_t s = c->stream;
+    const int M = g.M, Ml = g.Ml, Nl = g.Nl, pk = g.pk;
     const int ncp = (Ml + NROW - 1) / NROW, nrp = (Nl + NCOL - 1) / NCOL;
     double *colp = nullptr, *rowp = nullptr, *out = nullptr;
     int rc = dmalloc(&out, (size_t)M);
@@ -151,11 +153,11 @@ int norm1_grid(cflx_comm* c, const double* A, int M, int Ml, int Nl, int v, int 
             const dim3 grid(nrp, ncp);
             const int fin = (M + 255) / 256;
             if (lower_sym) {
-                abs_sums_kernel<true><<<grid, NCOL, 0, s>>>(A, Ml, Nl, v, Nt, Px, Py, pi, pj, colp, rowp);
-                column_sums_kernel<true><<<fin, 256, 0, s>>>(colp, ncp, rowp, nrp, M, Ml, Nl, v, Px, Py, pi, pj, out);
+                abs_sums_kernel<true><<<grid, NCOL, 0, s>>>(A, g, colp, rowp);
+                column_sums_kernel<true><<<fin, 256, 0, s>>>(colp, ncp, rowp, nrp, g, out);
             } else {
-                abs_sums_kernel<false><<<grid, NCOL, 0, s>>>(A, Ml, Nl, v, Nt, Px, Py, pi, pj, colp, rowp);
-                column_sums_kernel<false><<<fin, 256, 0, s>>>(colp, ncp, rowp, nrp, M, Ml, Nl, v, Px, Py, pi, pj, out);
+                abs_sums_kernel<false><<<grid, NCOL, 0, s>>>(A, g, colp, rowp);
+                column_sums_kernel<false><<<fin, 256, 0, s>>>(colp, ncp, rowp, nrp, g, out);
             }
             CFLX_CUDA(cudaGetLastError());
         }

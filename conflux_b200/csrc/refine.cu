@@ -2,7 +2,7 @@
 // dgerfs / dporfs on the GPU grid.
 //
 // The residual kernels read layer 0's local share A (Ml x Nl, conflux layout: local (r, c) is global
-// (((r / v) Px + pi) v + r % v, ((c / v) Py + pj) v + c % v)) once and produce two partial products at once:
+// (Layout::row(r), Layout::col(c))) once and produce two partial products at once:
 // P = op(A) X and Q = |op(A)| |X|.  They are the narrow GEMMs of the solve (solve.cu) with a second accumulator set fed
 // by fabs of the same A and B fragments:
 //   NN:  P, Q by local row,    from X gathered by local column (the LU, A X);
@@ -39,10 +39,8 @@ struct ResidArgs {
     int Pm, pm, Pk, pk;    // grid extent and position of the output index (m) and of the reduction index (k)
 };
 
-// global index of local index l on grid position p of P
-__device__ __forceinline__ int gidx(int l, int P, int p, int v) { return ((l / v) * P + p) * v + l % v; }
 __device__ __forceinline__ int first_tile(int g, int p, int P) { return g <= p ? 0 : (g - p + P - 1) / P; }
-// number of local indices l (position p of P) with gidx(l) <= G
+// number of local indices l (position p of P) with Layout::global(l, P, p, v) <= G
 __device__ __forceinline__ int count_le(int G, int P, int p, int v) {
     const int T = G / v;
     return T % P == p ? (T / P) * v + G % v + 1 : first_tile(T + 1, p, P) * v;
@@ -91,11 +89,11 @@ __global__ void __launch_bounds__(NW * 32, 1) resid_nn_kernel(ResidArgs r) {
     bool live0 = true, live1 = true;
     if (MASK == MASK_LOWER) {
         const int rlo = blockIdx.x * BM, rhi = min(rlo + BM, r.M) - 1;
-        const int glo = gidx(rlo, r.Pm, r.pm, r.v), ghi = gidx(rhi, r.Pm, r.pm, r.v);
+        const int glo = Layout::global(rlo, r.Pm, r.pm, r.v), ghi = Layout::global(rhi, r.Pm, r.pm, r.v);
         K = glo / r.v >= r.Kappa ? 0 : min(K, min(count_le(ghi, r.Pk, r.pk, r.v), first_tile(r.Kappa, r.pk, r.Pk) * r.v));
         K = min(r.K, (K + 3) & ~3);  // a lane's four k indices lie in one tile (v % 4 == 0)
-        gm0 = gidx((int)row0, r.Pm, r.pm, r.v);
-        gm1 = gidx((int)row0 + 8, r.Pm, r.pm, r.v);
+        gm0 = Layout::global((int)row0, r.Pm, r.pm, r.v);
+        gm1 = Layout::global((int)row0 + 8, r.Pm, r.pm, r.v);
         live0 = gm0 / r.v < r.Kappa;
         live1 = gm1 / r.v < r.Kappa;
     }
@@ -121,7 +119,7 @@ __global__ void __launch_bounds__(NW * 32, 1) resid_nn_kernel(ResidArgs r) {
             a[s][2] = (ok1 && kin) ? __ldg(reinterpret_cast<const double2*>(a1p + k)) : z;
             a[s][3] = (ok1 && kin) ? __ldg(reinterpret_cast<const double2*>(a1p + k + 2)) : z;
             if (MASK == MASK_LOWER) {
-                const int gk = gidx(k, r.Pk, r.pk, r.v);
+                const int gk = Layout::global(k, r.Pk, r.pk, r.v);
                 a[s][0] = keep2(a[s][0], gk <= gm0, gk + 1 <= gm0);
                 a[s][1] = keep2(a[s][1], gk + 2 <= gm0, gk + 3 <= gm0);
                 a[s][2] = keep2(a[s][2], gk <= gm1, gk + 1 <= gm1);
@@ -180,12 +178,12 @@ __global__ void __launch_bounds__(NW * 32, 1) resid_tn_kernel(ResidArgs r) {
     int k_lo = 0, K = r.K, gma = 0, gmb = 0;
     bool live_a = true, live_b = true;
     if (MASK == MASK_STRICT_UPPER_T) {
-        const int glo = gidx(blockIdx.x * BM_TN, r.Pm, r.pm, r.v);
+        const int glo = Layout::global(blockIdx.x * BM_TN, r.Pm, r.pm, r.v);
         const int k_hi = min(r.K, first_tile(r.Kappa, r.pk, r.Pk) * r.v);
         k_lo = glo / r.v >= r.Kappa ? k_hi : min(k_hi, count_le(glo, r.Pk, r.pk, r.v));
         K = k_hi - k_lo;
-        gma = gidx((int)ma, r.Pm, r.pm, r.v);  // ma even, v even: ma + 1 is gma + 1
-        gmb = gidx((int)mb, r.Pm, r.pm, r.v);
+        gma = Layout::global((int)ma, r.Pm, r.pm, r.v);  // ma even, v even: ma + 1 is gma + 1
+        gmb = Layout::global((int)mb, r.Pm, r.pm, r.v);
         live_a = gma / r.v < r.Kappa;
         live_b = gmb / r.v < r.Kappa;
     }
@@ -213,7 +211,7 @@ __global__ void __launch_bounds__(NW * 32, 1) resid_tn_kernel(ResidArgs r) {
                 double2 xa = k < K && live_a ? load_pair(A + (int64_t)k * r.lda, ma) : z;
                 double2 xb = k < K && live_b ? load_pair(A + (int64_t)k * r.lda, mb) : z;
                 if (MASK == MASK_STRICT_UPPER_T) {
-                    const int gk = gidx(k_lo + k, r.Pk, r.pk, r.v);
+                    const int gk = Layout::global(k_lo + k, r.Pk, r.pk, r.v);
                     xa = make_double2(gk > gma ? xa.x : 0.0, gk > gma + 1 ? xa.y : 0.0);
                     xb = make_double2(gk > gmb ? xb.x : 0.0, gk > gmb + 1 ? xb.y : 0.0);
                 }
@@ -388,9 +386,10 @@ int grow(double** p, size_t n, size_t* have) {
 }
 }  // namespace
 
-int launch_residual(ResidMode mode, const double* A, int64_t lda, int Ml, int Nl, int v, int Kappa, int Px, int Py,
-                    int pi, int pj, const double* Xc, const double* Xr, int64_t ldx, int nrhs, double* P, double* Q,
-                    int64_t ldo, cudaStream_t s) {
+int launch_residual(ResidMode mode, const double* A, const Layout& L, const double* Xc, const double* Xr, int64_t ldx,
+                    int nrhs, double* P, double* Q, int64_t ldo, cudaStream_t s) {
+    const int64_t lda = L.Nl;
+    const int Ml = L.Ml, Nl = L.Nl, v = L.v;
     if (nrhs <= 0) return CFLX_OK;
     if ((lda & 1) || (reinterpret_cast<uintptr_t>(A) & 15) || (v & 3)) {
         set_last_error("residual: unsupported layout lda=%lld v=%d (need even lda, v %% 4 == 0, 16-byte aligned A)",
@@ -398,8 +397,8 @@ int launch_residual(ResidMode mode, const double* A, int64_t lda, int Ml, int Nl
         return CFLX_ERR_UNSUPPORTED;
     }
     // NN: output by local row (grid row position), reduction over local columns; TN: the other way round
-    const ResidArgs nn{Ml, nrhs, Nl, A, lda, Xc, ldx, P, Q, ldo, v, Kappa, Px, pi, Py, pj};
-    const ResidArgs tn{Nl, nrhs, Ml, A, lda, Xr, ldx, P, Q, ldo, v, Kappa, Py, pj, Px, pi};
+    const ResidArgs nn{Ml, nrhs, Nl, A, lda, Xc, ldx, P, Q, ldo, v, L.Nt, L.Px, L.pi, L.Py, L.pj};
+    const ResidArgs tn{Nl, nrhs, Ml, A, lda, Xr, ldx, P, Q, ldo, v, L.Nt, L.Py, L.pj, L.Px, L.pi};
     if (mode == ResidMode::NN) return Ml > 0 ? dispatch_nn<MASK_NONE>(nn, s) : CFLX_OK;
     if (mode == ResidMode::TN) return Nl > 0 ? dispatch_tn<MASK_NONE>(tn, s) : CFLX_OK;
     if (Ml > 0) CFLX_TRY(dispatch_nn<MASK_LOWER>(nn, s));
@@ -511,23 +510,24 @@ void refine_cache_free(RefineCache* rc) {
 
 int refine_run(RefineCache* rc, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx, double* ferr,
                double* berr_out) {
-    cflx_comm* c = op.comm;
+    const Grid& G = op.grid;
+    cflx_comm* c = G.comm;
     cudaStream_t s = c->stream;
-    const int M = op.M, Ml = op.Ml, Nl = op.Nl, v = op.v;
+    const int M = G.M, Ml = G.Ml, Nl = G.Nl, v = G.v;
     const int ldn = (int)round_up(nrhs, 8);
-    const bool nn = op.mode != ResidMode::TN, tn = op.mode != ResidMode::NN, layer0 = op.pk == 0;
-    // local index -> global row of X (clamped into X: masked entries never use the value)
-    auto make_map = [&](int** dst, int n, int P, int p) -> int {
+    const bool nn = op.mode != ResidMode::TN, tn = op.mode != ResidMode::NN, layer0 = G.pk == 0;
+    // local column (by_col) or row -> global row of X (clamped into X: masked entries never use the value)
+    auto make_map = [&](int** dst, int n, bool by_col) -> int {
         if (*dst || n <= 0) return CFLX_OK;
         std::vector<int> m(n);
         for (int l = 0; l < n; ++l) {
-            const int g = ((l / v) * P + p) * v + l % v;
+            const int g = by_col ? G.col(l) : G.row(l);
             m[l] = g < M ? g : 0;
         }
         return solve_set_rows(dst, m, s);
     };
-    if (layer0 && nn) CFLX_TRY(make_map(&rc->gl_cols, Nl, op.Py, op.pj));
-    if (layer0 && tn) CFLX_TRY(make_map(&rc->gl_rows, Ml, op.Px, op.pi));
+    if (layer0 && nn) CFLX_TRY(make_map(&rc->gl_cols, Nl, true));
+    if (layer0 && tn) CFLX_TRY(make_map(&rc->gl_rows, Ml, false));
     const int prow = (nn ? Ml : 0) + (tn ? Nl : 0);
     const size_t mat = (size_t)M * ldn, chunk = (size_t)prow * 2 * ldn;
     if (rc->cap_m < mat) {  // the M x ldn buffers, grown together
@@ -561,7 +561,7 @@ int refine_run(RefineCache* rc, const RefineOp& op, int nrhs, const double* B, i
     const double eps = std::ldexp(1.0, -53), safmin = std::ldexp(1.0, -1022);
     const double nz = (double)M + 1.0, safe1 = nz * safmin, safe2 = safe1 / eps;
     const double* all = c->world_size > 1 ? rc->all : rc->part;
-    const AssembleArgs aa{all, (int64_t)chunk, Ml, Nl, ldn, nrhs, M, nn, tn, v, op.Px, op.Py, op.Pz, rc->B, rc->R,
+    const AssembleArgs aa{all, (int64_t)chunk, Ml, Nl, ldn, nrhs, M, nn, tn, v, G.Px, G.Py, G.Pz, rc->B, rc->R,
                           rc->ratio, rc->W, safe1, safe2, nz * eps};
     std::vector<double> berr(nrhs);
     // one residual pass: R = B - op(A) X, the ratios, W, and berr on the host
@@ -569,8 +569,8 @@ int refine_run(RefineCache* rc, const RefineOp& op, int nrhs, const double* B, i
         if (layer0) {
             if (nn) CFLX_TRY(launch_gather_rows(rc->X, ldn, rc->gl_cols, Nl, ldn, rc->Xc, s));
             if (tn) CFLX_TRY(launch_gather_rows(rc->X, ldn, rc->gl_rows, Ml, ldn, rc->Xr, s));
-            CFLX_TRY(launch_residual(op.mode, op.A, Nl, Ml, Nl, v, op.Kappa, op.Px, op.Py, op.pi, op.pj, rc->Xc, rc->Xr, ldn,
-                                     nrhs, rc->part, rc->part + ldn, 2 * (int64_t)ldn, s));
+            CFLX_TRY(launch_residual(op.mode, op.A, G, rc->Xc, rc->Xr, ldn, nrhs, rc->part, rc->part + ldn,
+                                     2 * (int64_t)ldn, s));
         }
         if (c->world_size > 1) CFLX_NCCL(ncclAllGather(rc->part, rc->all, chunk, ncclDouble, c->world, s));
         assemble_kernel<<<dim3((unsigned)M, (unsigned)((nrhs + 127) / 128)), 128, 0, s>>>(aa);

@@ -284,14 +284,14 @@ int launch_transpose_blocks(const double* in, int nb, int64_t total, double* out
 
 // slot of diagonal tile t in SolveCache::inv on this rank (-1: not owned)
 int diag_slot(const SolveFactor& f, int t) {
-    if (f.pk != 0 || t % f.Px != f.pi || t % f.Py != f.pj) return -1;
+    if (f.g.pk != 0 || t % f.g.Px != f.g.pi || t % f.g.Py != f.g.pj) return -1;
     int n = 0;
-    for (int u = 0; u < t; ++u) n += (u % f.Px == f.pi && u % f.Py == f.pj);
+    for (int u = 0; u < t; ++u) n += (u % f.g.Px == f.g.pi && u % f.g.Py == f.g.pj);
     return n;
 }
 
 const double* diag_tile(const SolveFactor& f, int t) {
-    return f.F + (int64_t)(t / f.Px) * f.v * f.Nl + (int64_t)(t / f.Py) * f.v;
+    return f.F + (int64_t)f.g.diag_row(t) * f.g.Nl + f.g.diag_col(t);
 }
 
 // Y = T^-1 R on the owner of diagonal tile t, by an nb-block sweep with the cached inverses; R (v x ldn) is overwritten.
@@ -303,7 +303,7 @@ const double* diag_tile(const SolveFactor& f, int t) {
 //   UpperT:     T = U_tt^T:  Y_j = inv(U_jj)^T R_j (the backward inverse block read transposed), then R_i -= U_ji^T Y_j
 //               for i > j: one TN launch on block row j of U_tt right of its diagonal block
 int diag_solve(const SolveCache& sc, const SolveFactor& f, int t, Tri tri, double* R, int ldn, cudaStream_t s) {
-    const int v = f.v, nb = f.nb, Nl = f.Nl, nblk = v / nb;
+    const int v = f.g.v, nb = f.g.nb, Nl = f.g.Nl, nblk = v / nb;
     const bool fwd = tri == Tri::Lower, ascending = fwd || tri == Tri::UpperT;
     const bool fwd_half = fwd || tri == Tri::UnitLowerT, inv_tn = tri == Tri::UnitLowerT || tri == Tri::UpperT;
     const double* inv = sc.inv + diag_slot(f, t) * 2 * (size_t)v * nb + (fwd_half ? 0 : (size_t)v * nb);
@@ -355,11 +355,11 @@ int solve_cache_grow(SolveCache* sc, const SolveFactor& f, int ldn, bool work, b
         *p = nullptr;
     }
     sc->ldn = 0;
-    const size_t M = f.M, v = f.v;
-    if (f.pk == 0 && (f.pj == 0 || (sc->col_seed && f.pi == 0))) CFLX_TRY(dmalloc(&sc->B, M * ldn));
+    const size_t M = f.g.M, v = f.g.v;
+    if (f.g.pk == 0 && (f.g.pj == 0 || (sc->col_seed && f.g.pi == 0))) CFLX_TRY(dmalloc(&sc->B, M * ldn));
     if (work) {
-        CFLX_TRY(dmalloc(&sc->W, (size_t)f.Ml * ldn));
-        if (sc->col_partials) CFLX_TRY(dmalloc(&sc->Z, (size_t)f.Nl * ldn));
+        CFLX_TRY(dmalloc(&sc->W, (size_t)f.g.Ml * ldn));
+        if (sc->col_partials) CFLX_TRY(dmalloc(&sc->Z, (size_t)f.g.Nl * ldn));
         CFLX_TRY(dmalloc(&sc->R, v * ldn));
         CFLX_TRY(dmalloc(&sc->Y, v * ldn));
     }
@@ -370,18 +370,18 @@ int solve_cache_grow(SolveCache* sc, const SolveFactor& f, int ldn, bool work, b
 }
 
 int solve_inverses(SolveCache* sc, const SolveFactor& f, bool lower) {
-    cudaStream_t s = f.comm->stream;
-    const int v = f.v, nb = f.nb;
+    cudaStream_t s = f.g.comm->stream;
+    const int v = f.g.v, nb = f.g.nb;
     cudaFree(sc->inv);
     sc->inv = nullptr;
     int nown = 0;
-    for (int t = 0; t < f.Nt; ++t) nown += diag_slot(f, t) >= 0;
+    for (int t = 0; t < f.g.Nt; ++t) nown += diag_slot(f, t) >= 0;
     const size_t per = 2 * (size_t)v * nb;
     CFLX_TRY(dmalloc(&sc->inv, std::max(1, nown) * per));
     double *tile = nullptr, *linvT = nullptr;
     int rc = dmalloc(&tile, (size_t)v * v);
     if (!rc) rc = dmalloc(&linvT, (size_t)v * nb);
-    for (int t = 0; t < f.Nt && !rc; ++t) {
+    for (int t = 0; t < f.g.Nt && !rc; ++t) {
         const int slot = diag_slot(f, t);
         if (slot < 0) continue;
         double* inv = sc->inv + slot * per;
@@ -389,9 +389,9 @@ int solve_inverses(SolveCache* sc, const SolveFactor& f, bool lower) {
         // Uinv_j = inv(L_jj)^T is then the backward half, its block transpose inv(L_jj) the forward half, and the
         // unit-lower part is the identity.  For L\U, the forward half is the block transpose of LinvT.
         if (lower) {
-            rc = launch_extract_panel_T(f.F, f.Nl, (int64_t)(t / f.Px) * v, (int64_t)(t / f.Py) * v, v, v, tile, v, s);
-        } else if (cudaMemcpy2DAsync(tile, v * sizeof(double), diag_tile(f, t), f.Nl * sizeof(double), v * sizeof(double),
-                                     v, cudaMemcpyDeviceToDevice, s) != cudaSuccess) {
+            rc = launch_extract_panel_T(f.F, f.g.Nl, f.g.diag_row(t), f.g.diag_col(t), v, v, tile, v, s);
+        } else if (cudaMemcpy2DAsync(tile, v * sizeof(double), diag_tile(f, t), f.g.Nl * sizeof(double),
+                                     v * sizeof(double), v, cudaMemcpyDeviceToDevice, s) != cudaSuccess) {
             set_last_error("solve: diagonal tile copy failed");
             rc = CFLX_ERR_CUDA;
         }
@@ -412,15 +412,15 @@ int solve_set_rows(int** dst, const std::vector<int>& rows, cudaStream_t s) {
 }
 
 int solve_seed(SolveCache* sc, const SolveFactor& f, int ldn, int nrhs, const double* B, int ldb, const SolveSeed& at) {
-    cudaStream_t s = f.comm->stream;
-    CFLX_CUDA(cudaMemsetAsync(sc->X, 0, sizeof(double) * f.M * ldn, s));
-    if (sc->W) CFLX_CUDA(cudaMemsetAsync(sc->W, 0, sizeof(double) * f.Ml * ldn, s));
-    if (sc->Z) CFLX_CUDA(cudaMemsetAsync(sc->Z, 0, sizeof(double) * f.Nl * ldn, s));
-    const bool holds = f.pk == 0 && (at.by_col ? f.pi : f.pj) == 0;
+    cudaStream_t s = f.g.comm->stream;
+    CFLX_CUDA(cudaMemsetAsync(sc->X, 0, sizeof(double) * f.g.M * ldn, s));
+    if (sc->W) CFLX_CUDA(cudaMemsetAsync(sc->W, 0, sizeof(double) * f.g.Ml * ldn, s));
+    if (sc->Z) CFLX_CUDA(cudaMemsetAsync(sc->Z, 0, sizeof(double) * f.g.Nl * ldn, s));
+    const bool holds = f.g.pk == 0 && (at.by_col ? f.g.pi : f.g.pj) == 0;
     if (holds && at.n > 0) {
-        CFLX_CUDA(cudaMemsetAsync(sc->B, 0, sizeof(double) * f.M * ldn, s));
-        CFLX_CUDA(cudaMemcpy2DAsync(sc->B, ldn * sizeof(double), B, (size_t)ldb * sizeof(double), nrhs * sizeof(double), f.M,
-                                    cudaMemcpyDefault, s));
+        CFLX_CUDA(cudaMemsetAsync(sc->B, 0, sizeof(double) * f.g.M * ldn, s));
+        CFLX_CUDA(cudaMemcpy2DAsync(sc->B, ldn * sizeof(double), B, (size_t)ldb * sizeof(double), nrhs * sizeof(double),
+                                    f.g.M, cudaMemcpyDefault, s));
         CFLX_TRY(launch_gather_rows(sc->B, ldn, at.rows, at.n, ldn, at.dst, s));
     }
     return CFLX_OK;
@@ -428,13 +428,13 @@ int solve_seed(SolveCache* sc, const SolveFactor& f, int ldn, int nrhs, const do
 
 int solve_row_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward, double* keep, int keep_div,
                     bool clear_row) {
-    cudaStream_t s = f.comm->stream;
-    const int v = f.v, Px = f.Px, Py = f.Py, Nl = f.Nl, tiles = f.rows / v;
-    const bool layer0 = f.pk == 0;
+    cudaStream_t s = f.g.comm->stream;
+    const int v = f.g.v, Px = f.g.Px, Py = f.g.Py, Nl = f.g.Nl, tiles = f.rows / v;
+    const bool layer0 = f.g.pk == 0;
     const size_t tile = (size_t)v * ldn;
-    for (int i = 0; i < f.Nt; ++i) {
-        const int t = forward ? i : f.Nt - 1 - i;
-        const bool in_row = f.pi == t % Px, in_col = f.pj == t % Py, owner = layer0 && in_row && in_col;
+    for (int i = 0; i < f.g.Nt; ++i) {
+        const int t = forward ? i : f.g.Nt - 1 - i;
+        const bool in_row = f.g.pi == t % Px, in_col = f.g.pj == t % Py, owner = layer0 && in_row && in_col;
         double* const Wt = sc->W + (int64_t)(t / Px) * tile;
         double* R = Wt;  // tile t's rows of W, summed over the grid row onto the diagonal owner
         if (in_row && Py * f.stride > 1) {
@@ -451,8 +451,8 @@ int solve_row_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward,
         if (in_col && Px * f.stride > 1)
             CFLX_NCCL(ncclBroadcast(sc->Y, sc->Y, tile, ncclDouble, (t % Px) * f.stride, f.col_comm->c, s));
         // W[tiles I > t] -= L[I, t] Y_t (forward), W[tiles I < t] -= U[I, t] X_t (backward), on the grid column
-        const int lo = forward ? std::min(tiles, first_local_tile(t + 1, f.pi, Px)) * v : 0;
-        const int hi = forward ? f.rows : std::min(tiles, first_local_tile(t, f.pi, Px)) * v;
+        const int lo = forward ? std::min(tiles, first_local_tile(t + 1, f.g.pi, Px)) * v : 0;
+        const int hi = forward ? f.rows : std::min(tiles, first_local_tile(t, f.g.pi, Px)) * v;
         if (in_col && layer0 && lo < hi)
             CFLX_TRY(launch_gemm_narrow(hi - lo, ldn, v, f.F + (int64_t)lo * Nl + (int64_t)(t / Py) * v, Nl, sc->Y, ldn,
                                         sc->W + (int64_t)lo * ldn, ldn, sc->W + (int64_t)lo * ldn, ldn, -1.0, 1.0, s));
@@ -462,13 +462,13 @@ int solve_row_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward,
 
 int solve_col_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward, Tri tri, double* keep, int keep_div,
                     bool clear_col) {
-    cudaStream_t s = f.comm->stream;
-    const int v = f.v, Px = f.Px, Py = f.Py, Nl = f.Nl;
-    const bool layer0 = f.pk == 0;
+    cudaStream_t s = f.g.comm->stream;
+    const int v = f.g.v, Px = f.g.Px, Py = f.g.Py, Nl = f.g.Nl;
+    const bool layer0 = f.g.pk == 0;
     const size_t tile = (size_t)v * ldn;
-    for (int i = 0; i < f.Nt; ++i) {
-        const int t = forward ? i : f.Nt - 1 - i;
-        const bool in_row = f.pi == t % Px, in_col = f.pj == t % Py, owner = layer0 && in_row && in_col;
+    for (int i = 0; i < f.g.Nt; ++i) {
+        const int t = forward ? i : f.g.Nt - 1 - i;
+        const bool in_row = f.g.pi == t % Px, in_col = f.g.pj == t % Py, owner = layer0 && in_row && in_col;
         double* const Zt = sc->Z + (int64_t)(t / Py) * tile;
         double* R = Zt;  // tile t's columns of Z, summed over the grid column onto the owner
         if (in_col && Px * f.stride > 1) {
@@ -488,12 +488,12 @@ int solve_col_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward,
         if (!layer0) continue;
         const double* Ft = f.F + (int64_t)(t / Px) * v * Nl;  // local tile row t / Px
         if (forward) {  // Z[columns gj > t] -= U[t, gj]^T Y_t: a suffix of the tile row
-            const int lo = first_local_tile(t + 1, f.pj, Py) * v;
+            const int lo = first_local_tile(t + 1, f.g.pj, Py) * v;
             if (lo < Nl)
                 CFLX_TRY(launch_gemm_narrow_tn(Nl - lo, ldn, v, Ft + lo, Nl, sc->Y, ldn, sc->Z + (int64_t)lo * ldn, ldn,
                                                sc->Z + (int64_t)lo * ldn, ldn, -1.0, 1.0, s));
         } else {
-            const int m = first_local_tile(t, f.pj, Py) * v;  // local columns with gj < t: a prefix of the tile row
+            const int m = first_local_tile(t, f.g.pj, Py) * v;  // local columns with gj < t: a prefix of the tile row
             if (m > 0)  // Z[columns gj < t] -= L[t, gj]^T X_t
                 CFLX_TRY(launch_gemm_narrow_tn(m, ldn, v, Ft, Nl, sc->Y, ldn, sc->Z, ldn, sc->Z, ldn, -1.0, 1.0, s));
         }
@@ -502,17 +502,17 @@ int solve_col_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward,
 }
 
 int solve_finish(SolveCache* sc, const SolveFactor& f, int ldn, int nrhs, double* X, int ldx, const int* unperm) {
-    cudaStream_t s = f.comm->stream;
+    cudaStream_t s = f.g.comm->stream;
     // exactly one rank contributes each element: the sum is X itself, bit for bit, on every rank
-    if (f.P > 1) CFLX_NCCL(ncclAllReduce(sc->X, sc->X, (size_t)f.M * ldn, ncclDouble, ncclSum, f.comm->world, s));
+    if (f.g.P > 1) CFLX_NCCL(ncclAllReduce(sc->X, sc->X, (size_t)f.g.M * ldn, ncclDouble, ncclSum, f.g.comm->world, s));
     const double* out = sc->X;
     if (unperm) {
-        CFLX_TRY(launch_gather_rows(sc->X, ldn, unperm, f.M, ldn, sc->Xg, s));
+        CFLX_TRY(launch_gather_rows(sc->X, ldn, unperm, f.g.M, ldn, sc->Xg, s));
         out = sc->Xg;
     }
     if (X)
-        CFLX_CUDA(cudaMemcpy2DAsync(X, (size_t)ldx * sizeof(double), out, ldn * sizeof(double), nrhs * sizeof(double), f.M,
-                                    cudaMemcpyDefault, s));
+        CFLX_CUDA(cudaMemcpy2DAsync(X, (size_t)ldx * sizeof(double), out, ldn * sizeof(double), nrhs * sizeof(double),
+                                    f.g.M, cudaMemcpyDefault, s));
     CFLX_CUDA(cudaStreamSynchronize(s));
     return CFLX_OK;
 }
