@@ -15,7 +15,7 @@ import numpy as np
 
 from ._lib import ConfluxError, LIB_PATH, SYMBOLS, check, lib
 
-__all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "residual", "validate", "lu_solve", "lu_rcond", "lu_refine", "lu_equilibrate", "lu_svx", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
+__all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "residual", "validate", "lu_solve", "lu_rcond", "lu_refine", "lu_equilibrate", "lu_svx", "lu_inverse", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
 
 
 def auto_grid(M, N, P):
@@ -286,6 +286,39 @@ def lu_svx(gv, B, trans=False):
                                                           equed=equed.value.decode(), info=k)
 
 
+def _share_out(out, Ml, Nl, what):
+    """(pointer, array) of the Ml x Nl float64 C-contiguous share an inverse is written into: a new NumPy array when out is
+    None, else out itself -- a NumPy array, or any object with __cuda_array_interface__ (a torch CUDA tensor)."""
+    if out is None:
+        out = np.empty((Ml, Nl))
+    if isinstance(out, np.ndarray):
+        if out.dtype != np.float64 or not out.flags.c_contiguous or out.shape != (Ml, Nl):
+            raise ValueError(f"{what}: out must be a C-contiguous float64 array of shape ({Ml}, {Nl}), got {out.dtype} "
+                             f"{out.shape}")
+        return out.ctypes.data, out
+    cai = getattr(out, "__cuda_array_interface__", None)
+    if cai is None:
+        raise ValueError(f"{what}: out must be a NumPy array or expose __cuda_array_interface__")
+    shape, strides = tuple(cai["shape"]), cai.get("strides")
+    if cai["typestr"] != "<f8" or shape != (Ml, Nl) or strides not in (None, (8 * Nl, 8)):
+        raise ValueError(f"{what}: out must be a C-contiguous float64 device array of shape ({Ml}, {Nl}), got "
+                         f"{cai['typestr']} {shape} strides {strides}")
+    return cai["data"][0], out
+
+
+def lu_inverse(gv, out=None):
+    """inv(A) of the padded matrix of the last LU_rep (P A = L U) on the GPU grid, like LAPACK's dgetri: returns (share,
+    info), this rank's Ml x Nl share of inv(A) in the conflux layout (layers pk != 0 get layer 0's bits).  info = k when
+    U(k,k) is exactly zero (the first such k, counted from 1); the share is then None and out is left as it was.  out: the
+    share to write into, a NumPy array or a torch CUDA tensor (float64, C-contiguous, (Ml, Nl)).  The columns are solves
+    A X = I, so A X - I is the small residual.  COLLECTIVE over gv.lu_comm; the factors and later solves are left as they
+    are."""
+    ptr, arr = _share_out(out, gv.Ml, gv.Nl, "lu_inverse")
+    info = ctypes.c_int()
+    check(lib().cflx_lu_inverse(gv._h, ptr, ctypes.byref(info)), "lu_inverse")
+    return (None if info.value else arr), info.value
+
+
 class cholesky:
     """Mirror of the reference's CONFCHOX driver interface (src/conflux/cholesky/Cholesky.h:20-22):
         initialize(N, v, grid, comm) -> object;  obj.parallelCholesky() -> ms;  obj.finalize().
@@ -377,6 +410,14 @@ class cholesky:
         check(lib().cflx_chol_svx(self._h, nrhs, B2.ctypes.data, nrhs, X.ctypes.data, nrhs, ctypes.byref(rcond),
                                   fe.ctypes.data, be.ctypes.data, ctypes.byref(equed), ctypes.byref(info)), "chol_svx")
         return X.reshape(B.shape), dict(rcond=rcond.value, ferr=fe, berr=be, equed=equed.value.decode(), info=info.value)
+
+    def inverse(self, out=None):
+        """inv(A) from the factor of the last parallelCholesky on the GPU grid, like LAPACK's dpotri (lower): returns this
+        rank's Ml x Nl share, whose real tiles on and below the diagonal hold inv(A); the tiles above the diagonal and
+        those beyond Kappa are zero.  out as lu_inverse's.  COLLECTIVE; every layer gets layer 0's bits."""
+        ptr, arr = _share_out(out, self.Ml, self.Nl, "cholesky.inverse")
+        check(lib().cflx_chol_inverse(self._h, ptr), "chol_inverse")
+        return arr
 
     def finalize(self, clean=True):
         if self._h:
@@ -535,6 +576,32 @@ class dbg:
                                    out["sym_scaled"].ctypes.data, out["growth"].ctypes.data, ctypes.byref(zp)), "dbg_equil")
         out["zero_pivot"] = zp.value
         return out
+
+    @staticmethod
+    def inverse_share(mode, v, grid, pos, M, c0, nc, Ml, Nl, Kappa=None, rows=None, X=None, perm=None, share=None,
+                      zero_fill=False):
+        """The per-share kernels of lu_inverse (mode "lu") and cholesky.inverse (mode "chol") on one Ml x Nl share at grid
+        position pos of grid = (Px, Py), for the block of nc columns from global column c0.  Returns (W, share): W (Ml x
+        round_up(nc, 8)) is the seed of the first `rows` local rows (default Ml); share is a copy of `share` after the
+        scatter of X (M x nc or wider, by global row) to global column perm[c0 + j] ("lu") or c0 + j ("chol": real tiles,
+        global tile index < Kappa, on and below the diagonal), and with zero_fill ("chol") zeros on every entry the scatter
+        never writes.  share is None when X or share is None."""
+        m = {"lu": 0, "chol": 1}[mode]
+        Px, Py = (int(x) for x in grid)
+        ldn = -(-int(nc) // 8) * 8
+        W = np.empty((Ml, ldn))
+        ptr = lambda a: a.ctypes.data if a is not None else None
+        out = Xc = pm = None
+        if X is not None and share is not None:
+            Xc = np.ascontiguousarray(X, dtype=np.float64)
+            out = np.array(share, dtype=np.float64, order="C")
+            pm = np.ascontiguousarray(perm, dtype=np.int32) if perm is not None else None
+        check(lib().cflx_dbg_inverse_share(m, int(Ml), int(Nl), int(v), int(Kappa if Kappa is not None else 1 << 30), Px, Py,
+                                           int(pos[0]), int(pos[1]), int(M), int(c0), int(nc),
+                                           int(rows if rows is not None else Ml), ptr(Xc),
+                                           Xc.shape[1] if Xc is not None else 0, ptr(pm), W.ctypes.data, ptr(out),
+                                           1 if zero_fill else 0), "dbg_inverse_share")
+        return W, out
 
     @staticmethod
     def panel(P, reps=1):

@@ -980,6 +980,16 @@ int cflx_chol_solve(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X
     return solve_finish(sc, f, ldn, nrhs, X, ldx);
 }
 
+// COLLECTIVE.  LAPACK dpotri (UPLO = 'L') on the grid (inverse.cu): the block solves with the identity on the sweeps of
+// cflx_chol_solve, the lower tiles of each block column scattered into this rank's share, the rest of it zero.
+int cflx_chol_inverse(cflx_chol* ch, double* Ainv_local) {
+    if (!ch) return CFLX_ERR_ARG;
+    CFLX_TRY(chol_check(ch, "inverse"));
+    CFLX_CUDA(cudaSetDevice(ch->comm->device));
+    if (!ch->sv.ready) CFLX_TRY(chol_solve_prepare(ch));
+    return inverse_run(&ch->sv, chol_solve_factor(ch), InvKind::Chol, nullptr, Ainv_local);
+}
+
 // COLLECTIVE.  LAPACK dpocon on the grid: ||A||_1 of the symmetric input (its stored lower triangle, real tiles only) and
 // the Hager-Higham estimate of ||inv(A)||_1, whose products inv(A) x are solves with the factor.
 int cflx_chol_rcond(cflx_chol* ch, double* rcond_out, double* anorm_out) {

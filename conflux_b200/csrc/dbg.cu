@@ -364,6 +364,42 @@ int cflx_dbg_equil(int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int
     return CFLX_OK;
 }
 
+// the seed, scatter and zero-fill kernels of the inverse (inverse.cu) on one share at grid position (pi, pj) of Px x Py
+int cflx_dbg_inverse_share(int mode, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, int M, int c0,
+                           int nc, int rows, const double* X, int ldx, const int* perm, double* W_out,
+                           double* share_inout, int zero_fill) {
+    CFLX_TRY(check_device());
+    if ((mode != 0 && mode != 1) || Ml < 0 || Nl < 0 || v < 1 || Ml % v || Nl % v || Px < 1 || Py < 1 || pi < 0 ||
+        pi >= Px || pj < 0 || pj >= Py || M < (Ml / v) * Px * v || M < (Nl / v) * Py * v || c0 < 0 || nc < 1 ||
+        c0 + nc > M || rows < 0 || rows > Ml || (share_inout && (!X || ldx < nc || (mode == 0 && !perm))))
+        return CFLX_ERR_ARG;
+    const Layout L{M, v, Kappa, Ml, Nl, Px, Py, pi, pj};
+    const int ldn = (int)round_up(nc, 8);
+    if (W_out) {
+        DevBuf dW;
+        CFLX_TRY(dW.alloc(sizeof(double) * Ml * ldn));
+        CFLX_CUDA(cudaMemset(dW.p, 0, sizeof(double) * Ml * ldn));
+        CFLX_TRY(launch_inverse_seed(dW.as<double>(), ldn, L, rows, c0, nc, 0));
+        CFLX_CUDA(cudaMemcpy(W_out, dW.p, sizeof(double) * Ml * ldn, cudaMemcpyDeviceToHost));
+    }
+    if (share_inout) {
+        const size_t a_n = (size_t)Ml * Nl;
+        DevBuf dA, dX, dp;
+        CFLX_TRY(dA.alloc(sizeof(double) * a_n));
+        CFLX_TRY(dX.alloc(sizeof(double) * M * ldx));
+        CFLX_TRY(dp.alloc(sizeof(int) * M));
+        CFLX_CUDA(cudaMemcpy(dA.p, share_inout, sizeof(double) * a_n, cudaMemcpyHostToDevice));
+        CFLX_CUDA(cudaMemcpy(dX.p, X, sizeof(double) * M * ldx, cudaMemcpyHostToDevice));
+        if (mode == 0) CFLX_CUDA(cudaMemcpy(dp.p, perm, sizeof(int) * M, cudaMemcpyHostToDevice));
+        CFLX_TRY(launch_inverse_scatter(mode == 0 ? InvKind::LU : InvKind::Chol, dX.as<double>(), ldx, c0, nc,
+                                        mode == 0 ? dp.as<int>() : nullptr, L, dA.as<double>(), 0));
+        if (mode == 1 && zero_fill) CFLX_TRY(launch_inverse_zero(L, dA.as<double>(), 0));
+        CFLX_CUDA(cudaMemcpy(share_inout, dA.p, sizeof(double) * a_n, cudaMemcpyDeviceToHost));
+    }
+    CFLX_CUDA(cudaDeviceSynchronize());
+    return CFLX_OK;
+}
+
 // the residual kernels of the refinement (refine.cu) on one layer-0 share; the timed repetitions run first, then the
 // launch whose result is returned
 int cflx_dbg_residual(int mode, int Ml, int Nl, const double* A, int v, int Kappa, int Px, int Py, int pi, int pj,

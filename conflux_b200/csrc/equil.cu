@@ -380,10 +380,9 @@ int equil_growth(const double* F, const double* A, const Layout& L, int ncols, d
     return CFLX_OK;
 }
 
-int pivot_growth_grid(const Grid& g, EquilState* e, const double* F, const double* A, double* rpvgrw, int* info) {
+int zero_pivot_grid(const Grid& g, EquilState* e, const double* F, int* info) {
     cflx_comm* c = g.comm;
     cudaStream_t s = c->stream;
-    if (!e->growth) CFLX_TRY(dmalloc(&e->growth, 2));
     if (!e->ival) CFLX_TRY(dmalloc(&e->ival, 1));
     if (g.pk == 0) {
         CFLX_TRY(equil_zero_pivot(F, g, e->ival, s));
@@ -397,6 +396,14 @@ int pivot_growth_grid(const Grid& g, EquilState* e, const double* F, const doubl
     CFLX_CUDA(cudaMemcpyAsync(&first, e->ival, sizeof(int), cudaMemcpyDeviceToHost, s));
     CFLX_CUDA(cudaStreamSynchronize(s));
     *info = first == INT_MAX ? 0 : first;
+    return CFLX_OK;
+}
+
+int pivot_growth_grid(const Grid& g, EquilState* e, const double* F, const double* A, double* rpvgrw, int* info) {
+    cflx_comm* c = g.comm;
+    cudaStream_t s = c->stream;
+    if (!e->growth) CFLX_TRY(dmalloc(&e->growth, 2));
+    CFLX_TRY(zero_pivot_grid(g, e, F, info));
     const int ncols = *info ? *info : g.M;
     if (g.pk == 0) CFLX_TRY(equil_growth(F, A, g, ncols, e->growth, s));
     else CFLX_CUDA(cudaMemsetAsync(e->growth, 0, 2 * sizeof(double), s));

@@ -1125,6 +1125,21 @@ int cflx_lu_rcond(cflx_lu* lu, double* rcond_out, double* anorm_out) {
     return lu_rcond(lu, false, rcond_out, anorm_out);
 }
 
+// COLLECTIVE.  LAPACK dgetri on the grid (inverse.cu): the first exactly zero U(k,k) over the world, then the block
+// solves with the identity, each block column q of inv(P A) landing in column perm[q] of this rank's share.  Reads only
+// the factors and the permutation, like cflx_lu_solve.
+int cflx_lu_inverse(cflx_lu* lu, double* Ainv_local, int* info_out) {
+    if (!lu || !info_out) return CFLX_ERR_ARG;
+    CFLX_TRY(lu_check(lu, "inverse", false));
+    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    if (!lu->sv.ready) CFLX_TRY(lu_solve_prepare(lu));
+    int info = 0;
+    CFLX_TRY(zero_pivot_grid(*lu, &lu->eq, lu->Cbuf, &info));
+    *info_out = info;
+    if (info > 0) return CFLX_OK;  // exactly singular U: no inverse, nothing written
+    return inverse_run(&lu->sv, lu_solve_factor(lu), InvKind::LU, lu->hist, Ainv_local);
+}
+
 // COLLECTIVE.  LAPACK dgerfs on the grid: residuals of the input A0 (refine.cu), corrections and the forward-error
 // estimator's products by the solves above (lu_refine_op).
 int cflx_lu_refine(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, double* X, int ldx, double* ferr_out,

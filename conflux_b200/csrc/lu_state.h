@@ -253,15 +253,17 @@ int solve_set_rows(int** dst, const std::vector<int>& rows, cudaStream_t s);
 int solve_seed(SolveCache* sc, const SolveFactor& f, int ldn, int nrhs, const double* B, int ldb, const SolveSeed& at);
 // row-partial sweep over the tile diagonal: forward with the lower triangle (NN), backward with the upper one (NN).  The
 // diagonal owner keeps each solved tile t at tile t / keep_div of `keep`; with clear_row, keep is W and the other layer-0
-// ranks of the grid row zero their copy of that tile.
+// ranks of the grid row zero their copy of that tile.  [t_lo, t_hi) (t_hi < 0: Nt): the diagonal tiles the sweep visits,
+// in its direction; the default is every tile.
 int solve_row_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward, double* keep, int keep_div,
-                    bool clear_row);
+                    bool clear_row, int t_lo = 0, int t_hi = -1);
 // column-partial sweep over the tile diagonal (Z by local tile column, the factor read transposed): backward with L^T
-// (tri LowerT or UnitLowerT; update of the local columns gj < t), forward with U^T (UpperT; update of the columns
-// gj > t).  The diagonal owner keeps each solved tile t at tile t / keep_div of `keep`; with clear_col, keep is Z and the
-// other layer-0 ranks of the grid column zero their copy of that tile.  Ranks pk != 0 join the collectives only.
+// (tri LowerT or UnitLowerT; update of the local columns t_lo <= gj < t), forward with U^T (UpperT; update of the
+// columns gj > t).  The diagonal owner keeps each solved tile t at tile t / keep_div of `keep`; with clear_col, keep is Z
+// and the other layer-0 ranks of the grid column zero their copy of that tile.  Ranks pk != 0 join the collectives only.
+// [t_lo, t_hi) as solve_row_sweep.
 int solve_col_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward, Tri tri, double* keep, int keep_div,
-                    bool clear_col);
+                    bool clear_col, int t_lo = 0, int t_hi = -1);
 // X (nrhs columns, ldx; host or device) = the world sum of the owners' tiles of sc->X, copied when X is not null;
 // synchronises.
 // unperm (M rows, every rank): row i of X is row unperm[i] of that sum.
@@ -344,6 +346,9 @@ int equil_sym_apply(double* A, const Layout& L, const double* sc, cudaStream_t s
 // columns < ncols (zeros where the share holds none).
 int equil_zero_pivot(const double* F, const Layout& L, int* zero_pivot, cudaStream_t s);
 int equil_growth(const double* F, const double* A, const Layout& L, int ncols, double* out2, cudaStream_t s);
+// the first exactly zero U(k,k) of the layer-0 shares F of L\U on the grid, COLLECTIVE (ncclMin over the world): *info =
+// k (1-based), or 0 when there is none; the same on every rank
+int zero_pivot_grid(const Grid& g, EquilState* e, const double* F, int* info);
 // LAPACK dgeequ (+ dlaqge when `apply`) on the grid, COLLECTIVE: the scales into e->qr / e->qc (no record changes) and
 // the host results; r_out / c_out (M, may be null).  Scales are applied only when info == 0.
 int geequ_grid(const Grid& g, EquilState* e, double* A, bool apply, double* r_out, double* c_out, double* rowcnd,
@@ -359,4 +364,30 @@ int pivot_growth_grid(const Grid& g, EquilState* e, const double* F, const doubl
 int equil_grow(EquilState* e, int M, int ldn);
 // X[i][j] *= d[i] for i < M, j < n (ld), on the device
 int launch_scale_rows(double* X, int64_t ld, int M, int n, const double* d, cudaStream_t s);
+
+// ---------------------------------------------------------------- the explicit inverse (inverse.cu)
+// Columns of the inverse per block: a whole number of tiles near this width (all of M when M is smaller).  Measured at
+// N = 16384, v = 256 among 256 .. 2048 (DESIGN §7f).
+#ifndef CFLX_INV_NC
+#define CFLX_INV_NC 2048
+#endif
+int inverse_block_cols(int M, int v);
+// LU: inv(A) = inv(P A) P from L\U, column q of inv(P A) landing in column perm[q] (every entry of every share is written).
+// Cholesky: dpotri's lower triangle from L, column c landing in column c on the tiles on and below the diagonal of the real
+// tiles (global tile index < Nt); every other entry is set to zero.
+enum class InvKind { LU, Chol };
+// The per-share kernels (L: the layout of the share, global indices < L.M):
+//   seed:    W[r][j] = (L.row(r) == c0 + j && j < nc) for r < rows, j < ldn (the identity block of columns c0 .. c0 + nc - 1)
+//   scatter: column j < nc of X (M x ldx, by global row) into the share's column of block column c0 + j
+//            (LU: global column perm[c0 + j], every local row; Cholesky: global column c0 + j, the real tiles on and
+//            below the diagonal only)
+//   zero:    (Cholesky) zero every entry of the share the scatter never writes
+int launch_inverse_seed(double* W, int ldn, const Layout& L, int rows, int c0, int nc, cudaStream_t s);
+int launch_inverse_scatter(InvKind kind, const double* X, int ldx, int c0, int nc, const int* perm, const Layout& L,
+                           double* out, cudaStream_t s);
+int launch_inverse_zero(const Layout& L, double* out, cudaStream_t s);
+// COLLECTIVE.  The block loop: per block of nc = inverse_block_cols columns, seed, the sweeps (with the tile ranges
+// that skip the block's zero rows), solve_finish's all-reduce and the scatter into Ainv (Ml x Nl, host or device, may be
+// null).  The solve cache must be prepared; perm: the LU's permutation on the device (every rank).
+int inverse_run(SolveCache* sc, const SolveFactor& f, InvKind kind, const int* perm, double* Ainv);
 }  // namespace cflx

@@ -427,13 +427,14 @@ int solve_seed(SolveCache* sc, const SolveFactor& f, int ldn, int nrhs, const do
 }
 
 int solve_row_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward, double* keep, int keep_div,
-                    bool clear_row) {
+                    bool clear_row, int t_lo, int t_hi) {
     cudaStream_t s = f.g.comm->stream;
     const int v = f.g.v, Px = f.g.Px, Py = f.g.Py, Nl = f.g.Nl, tiles = f.rows / v;
     const bool layer0 = f.g.pk == 0;
     const size_t tile = (size_t)v * ldn;
-    for (int i = 0; i < f.g.Nt; ++i) {
-        const int t = forward ? i : f.g.Nt - 1 - i;
+    if (t_hi < 0) t_hi = f.g.Nt;
+    for (int i = t_lo; i < t_hi; ++i) {
+        const int t = forward ? i : t_lo + t_hi - 1 - i;
         const bool in_row = f.g.pi == t % Px, in_col = f.g.pj == t % Py, owner = layer0 && in_row && in_col;
         double* const Wt = sc->W + (int64_t)(t / Px) * tile;
         double* R = Wt;  // tile t's rows of W, summed over the grid row onto the diagonal owner
@@ -461,13 +462,15 @@ int solve_row_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward,
 }
 
 int solve_col_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward, Tri tri, double* keep, int keep_div,
-                    bool clear_col) {
+                    bool clear_col, int t_lo, int t_hi) {
     cudaStream_t s = f.g.comm->stream;
     const int v = f.g.v, Px = f.g.Px, Py = f.g.Py, Nl = f.g.Nl;
     const bool layer0 = f.g.pk == 0;
     const size_t tile = (size_t)v * ldn;
-    for (int i = 0; i < f.g.Nt; ++i) {
-        const int t = forward ? i : f.g.Nt - 1 - i;
+    if (t_hi < 0) t_hi = f.g.Nt;
+    const int c_lo = first_local_tile(t_lo, f.g.pj, Py) * v;  // local columns with gj < t_lo are never updated
+    for (int i = t_lo; i < t_hi; ++i) {
+        const int t = forward ? i : t_lo + t_hi - 1 - i;
         const bool in_row = f.g.pi == t % Px, in_col = f.g.pj == t % Py, owner = layer0 && in_row && in_col;
         double* const Zt = sc->Z + (int64_t)(t / Py) * tile;
         double* R = Zt;  // tile t's columns of Z, summed over the grid column onto the owner
@@ -494,8 +497,9 @@ int solve_col_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward,
                                                sc->Z + (int64_t)lo * ldn, ldn, -1.0, 1.0, s));
         } else {
             const int m = first_local_tile(t, f.g.pj, Py) * v;  // local columns with gj < t: a prefix of the tile row
-            if (m > 0)  // Z[columns gj < t] -= L[t, gj]^T X_t
-                CFLX_TRY(launch_gemm_narrow_tn(m, ldn, v, Ft, Nl, sc->Y, ldn, sc->Z, ldn, sc->Z, ldn, -1.0, 1.0, s));
+            if (m > c_lo)  // Z[columns t_lo <= gj < t] -= L[t, gj]^T X_t
+                CFLX_TRY(launch_gemm_narrow_tn(m - c_lo, ldn, v, Ft + c_lo, Nl, sc->Y, ldn, sc->Z + (int64_t)c_lo * ldn, ldn,
+                                               sc->Z + (int64_t)c_lo * ldn, ldn, -1.0, 1.0, s));
         }
     }
     return CFLX_OK;

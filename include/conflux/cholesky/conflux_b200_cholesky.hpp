@@ -129,5 +129,13 @@ inline int choleskySvx(int nrhs, const double* B, int ldb, double* X, int ldx, d
     chol_detail::check(cflx_chol_svx(s.plan, nrhs, B, ldb, X, ldx, rcond, ferr, berr, equed, &info), "choleskySvx");
     return info;
 }
+// LAPACK dpotri (lower) with the factor of the last parallelCholesky() (cflx_chol_inverse, collective): Ainv_local (Ml x
+// Nl; host or device memory; may be null) receives inv(A) on this rank's real tiles on and below the diagonal, zeros
+// elsewhere.
+inline void choleskyInverse(double* Ainv_local) {
+    auto& s = chol_detail::state();
+    if (!s.plan) throw CholeskyException("choleskyInverse() before initialize()");
+    chol_detail::check(cflx_chol_inverse(s.plan, Ainv_local), "choleskyInverse");
+}
 
 }  // namespace conflux

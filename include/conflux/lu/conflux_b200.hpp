@@ -305,4 +305,14 @@ int LU_svx(lu_params<T>& gv, int nrhs, const T* B, int ldb, T* X, int ldx, doubl
     return info;
 }
 
+// LAPACK dgetri with the factors of the last LU_rep on the GPU grid (cflx_lu_inverse, collective): Ainv_local (Ml x Nl,
+// the conflux layout; host or device memory; may be null) receives this rank's share of inv(A).  Returns info (0; k for
+// an exactly zero U(k,k), nothing written).
+template <class T>
+int LU_inverse(lu_params<T>& gv, T* Ainv_local) {
+    int info = 0;
+    check(cflx_lu_inverse(gv.plan, Ainv_local, &info), "LU_inverse");
+    return info;
+}
+
 }  // namespace conflux

@@ -147,6 +147,15 @@ int cflx_lu_equilibrate(cflx_lu*, int apply, double* r_out, double* c_out, doubl
  * CFLX_ERR_ARG as cflx_lu_refine and for a NULL rcond_out or info_out; CFLX_ERR_STATE as cflx_lu_rcond. */
 int cflx_lu_svx(cflx_lu*, int trans, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out,
                 double* ferr_out, double* berr_out, double* rpvgrw_out, char* equed_out, int* info_out);
+/* COLLECTIVE.  inv(A) of the padded M x M matrix factored by the last cflx_lu_factor (P A = L U), on the GPU grid, like
+ * LAPACK's dgetri.  Ainv_local: Ml x Nl row-major, the conflux layout of cflx_lu_set_local; host or device memory; may be
+ * NULL on any rank.  Every rank receives the share of its grid position (pi, pj); layers pk != 0 receive the bits of
+ * layer 0.  info_out: k when U(k,k) is exactly zero (the first such k, counted from 1; nothing is written); 0 otherwise.
+ * When the factors carry a scaling (cflx_lu_equilibrate), this is the inverse of the scaled matrix, as for
+ * cflx_lu_validate / _rcond.  The columns come from solves A X = I, so the right residual A X - I is small (dgetri bounds
+ * the left one, X A - I).  CFLX_ERR_ARG for a NULL info_out.  CFLX_ERR_STATE as cflx_lu_solve.  Leaves the factors, the
+ * permutation, the input, later solves and the launch count as they are. */
+int cflx_lu_inverse(cflx_lu*, double* Ainv_local, int* info_out);
 /* 1 when this plan's trailing update runs on the int8 wgmma digit-plane path (ozaki.cu), 0 for the FP64 DMMA kernel
  * (gemm.cu) */
 int cflx_lu_uses_ozaki(const cflx_lu*);
@@ -223,6 +232,12 @@ int cflx_chol_equilibrate(cflx_chol*, int apply, double* s_out, double* scond_ou
  * Arguments as cflx_chol_refine; CFLX_ERR_ARG also for a NULL rcond_out or info_out; CFLX_ERR_STATE as cflx_chol_solve. */
 int cflx_chol_svx(cflx_chol*, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out, double* ferr_out,
                   double* berr_out, char* equed_out, int* info_out);
+/* COLLECTIVE.  inv(A) from the factor of the last successful cflx_chol_factor (A = L L^T), like LAPACK's dpotri
+ * (UPLO = 'L'): the real tiles on and below the diagonal of this rank's Ml x Nl share hold inv(A), whole diagonal tiles
+ * included.  The tiles above the diagonal and the local tiles with a global index >= Kappa are zero.  Host or device
+ * memory; may be NULL.  Every layer receives the bits of layer 0.  As for cflx_lu_inverse, the right residual is the
+ * small one.  CFLX_ERR_STATE as cflx_chol_solve.  Adds nothing to cflx_chol_launch_count. */
+int cflx_chol_inverse(cflx_chol*, double* Ainv_local);
 /* number of kernels this object counted since the last reset (bench.py's gpu_launches); cflx_chol_solve adds none */
 int cflx_chol_launch_count(cflx_chol*, int64_t* count_out, int reset);
 void cflx_chol_destroy(cflx_chol*);
@@ -264,6 +279,17 @@ int cflx_dbg_residual(int mode, int Ml, int Nl, const double* A, int v, int Kapp
 int cflx_dbg_equil(int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, int M, const double* A,
                    const double* r, const double* c, char equed, int ncols, double* rowmax_out, double* colmax_out,
                    double* diag_out, double* scaled_out, double* sym_scaled_out, double* growth_out, int* zero_pivot_out);
+/* the per-share kernels of cflx_lu_inverse (mode 0) and cflx_chol_inverse (mode 1) on one share at grid position (pi, pj)
+ * of Px x Py (Ml x Nl row-major, Ml and Nl multiples of v; M >= (Ml / v) Px v and >= (Nl / v) Py v global indices; Kappa:
+ * the real tiles of mode 1), for the block of nc columns from global column c0 (c0 + nc <= M).  Each output may be NULL:
+ *   W_out (Ml x ldn, ldn = nc rounded up to a multiple of 8): the seed, W[r][j] = (global row of r == c0 + j) for the
+ *   first `rows` local rows, zero in the rest;
+ *   share_inout (Ml x Nl): column j < nc of X (M x ldx, by global row) scattered into the share, to global column
+ *   perm[c0 + j] (mode 0, perm: M ints) or c0 + j (mode 1, real tiles on and below the diagonal only); then, with
+ *   zero_fill in mode 1, zeros on every entry that scatter never writes.  Every other entry keeps its value. */
+int cflx_dbg_inverse_share(int mode, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, int M, int c0,
+                           int nc, int rows, const double* X, int ldx, const int* perm, double* W_out,
+                           double* share_inout, int zero_fill);
 /* partial-pivot LU of an n x v row-major panel: perm_out[v], A00_out[v*v] (L00\U00), LU_out[n*v] rows unpermuted */
 int cflx_dbg_panel(int n, int v, const double* panel, int* perm_out, double* A00_out, double* LU_out, int reps,
                    double* ms_out);
