@@ -467,6 +467,7 @@ int cflx_dbg_panel(int n, int v, const double* panel, int* perm_out, double* A00
     CFLX_CUDA(cudaMemset(dA00.p, 0, sizeof(double) * v * v));
     PanelWorkspace ws{};
     CFLX_TRY(panel_workspace_create(&ws));
+    if (const char* e = getenv("CFLX_PANEL_CTAS")) ws.cta_cap = atoi(e);  // time the search on the look-ahead's SM budget
     cudaEvent_t e0, e1;
     CFLX_CUDA(cudaEventCreate(&e0));
     CFLX_CUDA(cudaEventCreate(&e1));

@@ -986,6 +986,7 @@ int cflx_lu_factor(cflx_lu* lu, double* ms_out) {
     for (int sd = 0; sd < 2; ++sd)
         for (int r = 0; r < RG_COUNT; ++r) lu->region_ms[sd][r] = 0, lu->region_cnt[sd][r] = 0;
     lu->tl_recs.clear();
+    lu->tl_spans.clear();
     CFLX_TRY(grid_barrier(c));  // MPI_Barrier(lu_comm) before t1 (conflux_opt.hpp:531)
     cudaEvent_t e0, e1;
     CFLX_CUDA(cudaEventCreate(&e0));
@@ -1037,6 +1038,9 @@ int cflx_lu_factor(cflx_lu* lu, double* ms_out) {
                 lu->region_ms[r.side][r.region] += g;
                 lu->region_cnt[r.side][r.region]++;
                 lu->phase_ms[region_phase(r.region)] += g;
+                float st = 0;
+                if (cudaEventElapsedTime(&st, lu->tl_pool[0], lu->tl_pool[r.ev]) != cudaSuccess) cudaGetLastError();
+                lu->tl_spans.push_back({r.region, r.side, st, g});
             } else {
                 cudaGetLastError();
             }
@@ -1246,8 +1250,10 @@ int cflx_lu_set_profiling(cflx_lu* lu, int mode) {  // 0 off, 1 serialising phas
     lu->prof_mode = mode;
     return CFLX_OK;
 }
-// JSON text {"main": {region: [ms, count], ...}, "side": {...}} of the last profiled cflx_lu_factor; region names are the
-// reference's semiprof regions.  Returns the length needed (incl. the terminator) when buf is too small.
+// JSON text {"main": {region: [ms, count], ...}, "side": {...}, "records": [[region, "main" | "side", start ms, ms], ...]}
+// of the last profiled cflx_lu_factor; region names are the reference's semiprof regions.  "records" (profiling mode 2
+// only) lists every region instance in launch order, start relative to the first recorded event.  Returns the length
+// needed (incl. the terminator) when buf is too small.
 int cflx_lu_timeline(cflx_lu* lu, char* buf, int buf_len) {
     if (!lu) return CFLX_ERR_ARG;
     std::string o = "{";
@@ -1263,7 +1269,15 @@ int cflx_lu_timeline(cflx_lu* lu, char* buf, int buf_len) {
         }
         o += "}";
     }
-    o += "}";
+    o += ", \"records\": [";
+    for (size_t i = 0; i < lu->tl_spans.size(); ++i) {
+        const auto& sp = lu->tl_spans[i];
+        char tmp[160];
+        snprintf(tmp, sizeof(tmp), "%s[\"%s\", \"%s\", %.4f, %.4f]", i ? ", " : "", region_name(sp.region), sp.side ? "side" : "main",
+                 sp.start_ms, sp.ms);
+        o += tmp;
+    }
+    o += "]}";
     if (!buf || buf_len <= (int)o.size()) return (int)o.size() + 1;
     std::memcpy(buf, o.c_str(), o.size() + 1);
     return CFLX_OK;

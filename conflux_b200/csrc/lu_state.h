@@ -222,6 +222,8 @@ struct cflx_lu : cflx::Grid {
     struct TlRec { int region, side, ev; };
     std::vector<cudaEvent_t> tl_pool;
     std::vector<TlRec> tl_recs;
+    struct TlSpan { int region, side; float start_ms, ms; };  // resolved: start relative to the first recorded event
+    std::vector<TlSpan> tl_spans;                             // one per region instance, in launch order
     double region_ms[2][cflx::RG_COUNT] = {{0}};   // [main / side stream][region]
     int region_cnt[2][cflx::RG_COUNT] = {{0}};
     int prof_mode = 0;                              // 0 off, 1 serialising phase timers, 2 timeline

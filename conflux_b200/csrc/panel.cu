@@ -7,7 +7,7 @@
 //
 // Design (GPU-first, not a LAPACK translation):
 //   * the panel is stored TRANSPOSED, W[c][r]: a pivot search over column c is a coalesced scan of one row of W;
-//   * one persistent cooperative grid (<= 132 CTAs, one per SM of an H100); thread <-> matrix row; rows NEVER move: LAPACK's
+//   * one persistent cooperative grid (<= 132 CTAs, one per SM of an H100); owner thread <-> matrix row; rows NEVER move: LAPACK's
 //     interchanges are tracked as a per-row "position" so that idamax tie-breaking (first maximal |a| in the
 //     swapped order) is reproduced exactly (needed for the reference's integer test matrices);
 //   * right-looking with an NB-column inner block held in shared memory; per column ONE grid-wide exchange:
@@ -15,6 +15,14 @@
 //     global slot as "LL" words (payload + epoch in one 8-byte volatile store: the flag travels with the data), then
 //     polls all headers, picks the winner redundantly and reads the winner's row from its slot -- two dependent L2
 //     round trips per column, no reply from the owner, no grid barrier.
+//     A CTA is 8 row-owner warps plus one GATHER WARP that owns no rows.  On grids of <= 32 CTAs (every look-ahead launch)
+//     the gather warp alone runs the exchange of column j+1 -- one slot per lane, warp argmax, row fetch, 1 / pivot --
+//     from the moment the candidate is published, while the owners apply the rest of elimination j; the block barrier
+//     that publishes the winner's row is the one rendezvous of the column.  Slot reuse: column j+2 reuses the slot
+//     parity of column j.  A CTA publishes j+2 only after its rendezvous of column j+1, which its gather warp reaches
+//     only once EVERY CTA has published j+1, and a CTA publishes j+1 only after its own rendezvous of column j, i.e.
+//     after its gather warp has consumed every word of column j it reads.  So no word of column j is overwritten
+//     while a reader still needs it (model: oracle/panel_exchange_ref.py).  Larger grids poll with all threads and reduce with a block argmax.
 //     The LL words order only their own payload; the trailing columns of W that phase C writes with plain stores and
 //     that OTHER CTAs gather as pivot rows one block later are ordered by a gpu-scope fence pair per NB-column block
 //     (writer: __threadfence() after the phase-C write-back; reader: __threadfence() before the U12 gathers);
@@ -32,8 +40,10 @@
 namespace cflx {
 
 namespace {
-constexpr int PT_THREADS = 256;  // 8 warps: two per scheduler, so dependent DFMA/LDS chains of one warp are covered
+constexpr int PT_THREADS = 256;  // 8 row-owner warps: two per scheduler, so dependent DFMA/LDS chains of one warp are covered
 constexpr int PT_WARPS = PT_THREADS / 32;
+constexpr int PT_LAUNCH = PT_THREADS + 32;  // + the gather warp, which owns no rows (warp PT_WARPS)
+constexpr int PT_ALLWARPS = PT_LAUNCH / 32;
 constexpr int MAXG = 132;   // SMs of an H100 SXM
 constexpr int RPT_LIMIT = 8;  // rows per thread -> R <= 1024 rows per CTA
 
@@ -83,46 +93,50 @@ __device__ __forceinline__ Cand warp_argmax(Cand c) {
 __device__ __forceinline__ bool better(const Cand& a, const Cand& b) {  // a strictly better than b
     return a.key > b.key || (a.key == b.key && a.pos < b.pos);
 }
-// block-wide argmax; result identical in every thread.  red_* have 2 x PT_WARPS entries and `rb` alternates between
-// the two halves on every call, so ONE barrier per reduction is enough (the buffer of call i is rewritten by call
-// i+2, which every thread reaches only after the barrier of call i+1).
+// block-wide argmax over all PT_ALLWARPS warps; result identical in every thread.  red_* have 2 x PT_ALLWARPS entries and
+// `rb` alternates between the two halves on every call, so ONE barrier per reduction is enough (the buffer of call i is
+// rewritten by call i+2, which every thread reaches only after the barrier of call i+1).  The per-warp results are
+// reduced by a second warp_argmax (one entry per lane) in every warp: three shared loads and the redux chain instead
+// of 3 x PT_ALLWARPS dependent loads and compares per thread.
 __device__ __forceinline__ Cand block_argmax(Cand c, unsigned long long* red_key, int* red_pos, int* red_row, int& rb) {
     Cand w = warp_argmax(c);
-    const int warp = threadIdx.x >> 5;
-    const int o = rb * PT_WARPS;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int o = rb * PT_ALLWARPS;
     rb ^= 1;
-    if ((threadIdx.x & 31) == 0) {
+    if (lane == 0) {
         red_key[o + warp] = w.key;
         red_pos[o + warp] = w.pos;
         red_row[o + warp] = w.row;
     }
     __syncthreads();
-    Cand best{red_key[o], red_pos[o], red_row[o]};
-#pragma unroll
-    for (int i = 1; i < PT_WARPS; ++i) {
-        Cand x{red_key[o + i], red_pos[o + i], red_row[o + i]};
-        if (better(x, best)) best = x;
-    }
-    return best;
+    Cand x{0ull, INT_MAX, -1};
+    if (lane < PT_ALLWARPS) x = Cand{red_key[o + lane], red_pos[o + lane], red_row[o + lane]};
+    return warp_argmax(x);
 }
 
 template <int NB, int RPT_MAX>
-__global__ void __launch_bounds__(PT_THREADS, 1) panel_getrf_kernel(PanelArgs p) {
+__global__ void __launch_bounds__(PT_LAUNCH, 1) panel_getrf_kernel(PanelArgs p) {
     // layout and size: panel_smem_bytes<NB>
     extern __shared__ __align__(16) unsigned char smem_raw[];
     double* Ab = reinterpret_cast<double*>(smem_raw);  // [NB][Rpad] inner block, column-major per CTA
     double* U12 = Ab + (size_t)NB * p.Rpad;            // [NB][v]
     double* LU11 = U12 + (size_t)NB * p.v;             // [NB][NB+1] LU rows of this block's pivots
-    double* prow = LU11 + NB * (NB + 1);               // [2][NB] winner rows, double-buffered by column parity
-    unsigned long long* red_key = reinterpret_cast<unsigned long long*>(prow + 2 * NB);
-    int* red_pos = reinterpret_cast<int*>(red_key + 2 * PT_WARPS);
-    int* red_row = red_pos + 2 * PT_WARPS;
-    int* pivrow_blk = red_row + 2 * PT_WARPS;  // [NB]
+    double* prow = LU11 + NB * (NB + 1);               // [2][NB + 1] winner row and 1 / pivot, double-buffered by column parity
+    unsigned long long* red_key = reinterpret_cast<unsigned long long*>(prow + 2 * (NB + 1));
+    int* red_pos = reinterpret_cast<int*>(red_key + 2 * PT_ALLWARPS);
+    int* red_row = red_pos + 2 * PT_ALLWARPS;
+    int* pivrow_blk = red_row + 2 * PT_ALLWARPS;  // [NB]
     int* win_sh = pivrow_blk + NB;  // [2][2] winner {pos, row} broadcast by the gathering warp, by column parity
     unsigned char* s_act = reinterpret_cast<unsigned char*>(win_sh + 4);  // [Rpad] row still active?
     int rb = 0;
 
-    const int t = threadIdx.x;
+    const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
+    // Threads 0..PT_THREADS-1 own rows.  The last warp owns none: on grids of <= 32 CTAs it alone runs the exchange (one
+    // slot per lane), so the poll of column j+1 starts at once while the row owners still apply elimination j.  Larger
+    // grids poll with every thread and reduce with a block argmax.
+    const bool owner = t < PT_THREADS;
+    const bool small = p.G <= 32;
+    const bool fetcher = warp == (small ? PT_WARPS : 0);  // the warp that fetches the winner's row
     const int cta = blockIdx.x;
     const int row_base = cta * p.R;
     const int Rloc = max(0, min(p.R, p.n - row_base));
@@ -136,15 +150,15 @@ __global__ void __launch_bounds__(PT_THREADS, 1) panel_getrf_kernel(PanelArgs p)
     for (int q = 0; q < RPT_MAX; ++q) {
         const int lr = t + q * PT_THREADS;
         pos[q] = row_base + lr;
-        active[q] = lr < Rloc;
+        active[q] = owner && lr < Rloc;
     }
-    for (int lr = t; lr < Rpad; lr += PT_THREADS) s_act[lr] = lr < Rloc ? 1 : 0;
+    for (int lr = t; lr < Rpad; lr += PT_LAUNCH) s_act[lr] = lr < Rloc ? 1 : 0;
 
     for (int jb = 0; jb < p.nsteps; jb += NB) {
         const int nbc = min(NB, v - jb);         // columns in this block
         const int nsb = min(nbc, p.nsteps - jb);  // elimination steps in this block
         // ---- phase A: load the inner block of my rows (coalesced rows of W) ----
-        for (int e = t; e < nbc * Rpad; e += PT_THREADS) {  // all threads, coalesced along the rows of W
+        for (int e = t; e < nbc * Rpad; e += PT_LAUNCH) {  // all threads, coalesced along the rows of W
             const int c = e / Rpad, lr = e - c * Rpad;
             if (lr < Rloc) Ab[e] = W[(int64_t)(jb + c) * ldw + row_base + lr];
         }
@@ -153,8 +167,8 @@ __global__ void __launch_bounds__(PT_THREADS, 1) panel_getrf_kernel(PanelArgs p)
 
         // ---- phase B: nsb pivot steps, software-pipelined across columns ----
         // The candidate of column j+1 is found and PUBLISHED as soon as the multipliers of column j are known (only
-        // column j+1 of the inner block is updated first); the remaining columns of elimination j are applied while
-        // the exchange is in flight, so its latency hides the rank-1 update instead of adding to it.
+        // column j+1 of the inner block is updated first); the row owners apply the remaining columns of elimination j
+        // while the exchange is in flight, so its latency hides the rank-1 update instead of adding to it.
         auto local_candidate = [&](int col) -> Cand {
             Cand c{0ull, INT_MAX, -1};
 #pragma unroll
@@ -200,13 +214,13 @@ __global__ void __launch_bounds__(PT_THREADS, 1) panel_getrf_kernel(PanelArgs p)
         for (int j = 0; j < nsb; ++j) {
             const int jg = jb + j;
             const int par = jg & 1;
-            double* pr = prow + par * NB;  // the winner's inner-block row
-            {
-                // gather every CTA's candidate for column jg, pick the winner, fetch its inner-block row.  G <= 32: warp 0
-                // alone (one slot per lane, warp-level argmax, no block barrier); larger grids poll with all warps.
+            double* pr = prow + par * (NB + 1);  // the winner's inner-block row, then 1 / pivot
+            if (!small || fetcher) {
+                // gather every CTA's candidate for column jg, pick the winner, fetch its inner-block row.  G <= 32: the
+                // gather warp alone (one slot per lane, warp-level argmax, no block barrier); larger grids poll with all warps.
                 const unsigned epoch = (unsigned)(p.epoch_base + jg + 1);
                 Cand gc{0ull, INT_MAX, -1};
-                for (int g = t; g < p.G; g += PT_THREADS) {
+                for (int g = small ? lane : t; g < p.G; g += small ? 32 : PT_LAUNCH) {
                     const uint2* h = p.slot_hdr + (size_t)(par * MAXG + g) * 4;
                     uint4 a, b;
                     do {
@@ -216,24 +230,26 @@ __global__ void __launch_bounds__(PT_THREADS, 1) panel_getrf_kernel(PanelArgs p)
                     Cand o{((unsigned long long)a.z << 32) | a.x, (int)b.x, (int)b.z};
                     if (better(o, gc)) gc = o;
                 }
-                Cand w = gc;  // (G <= 32: only warp 0 reduces; the other warps go straight to the barrier)
-                if (p.G > 32) w = block_argmax(gc, red_key, red_pos, red_row, rb);
-                else if (t < 32) w = warp_argmax(gc);
+                const Cand w = small ? warp_argmax(gc) : block_argmax(gc, red_key, red_pos, red_row, rb);
                 // (w.row < 0 cannot happen while jg < nsteps = min(n, v): some row is still active)
-                if (t < nbc) {  // the winner's row: second L2 round trip
-                    const uint2* wr = p.slot_rows + (size_t)(par * MAXG + w.row / p.R) * 64 + 2 * t;
+                // the winner's slot: on the gather warp (one slot per lane) the lane that held its row, no integer division
+                const int wslot = small ? __ffs(__ballot_sync(0xffffffffu, gc.row == w.row)) - 1 : w.row / p.R;
+                if (fetcher && lane < nbc) {  // the winner's row: second L2 round trip
+                    const uint2* wr = p.slot_rows + (size_t)(par * MAXG + wslot) * 64 + 2 * lane;
                     uint4 a;
                     do {
                         a = ld_ll2(wr);
                     } while (a.y != epoch || a.w != epoch);
                     const double x = __longlong_as_double((long long)(((unsigned long long)a.z << 32) | a.x));
-                    // safe before the barrier below: prow is double-buffered by column parity, and the last reader of
-                    // prow[par] (elimination jg - 2) finished before the barrier of column jg - 1; LU11 row j is read
-                    // only by phase C and the A00 emission, after the block's later barriers
-                    pr[t] = x;
-                    LU11[j * (NB + 1) + t] = x;
+                    // safe before the barrier below: prow and win_sh are double-buffered by column parity, and the last
+                    // reader of prow[par] (elimination jg - 2) finished before the barrier of column jg - 1, which this
+                    // warp passed before it began this gather; LU11 row j is read only by phase C and the A00 emission,
+                    // after the block's later barriers
+                    pr[lane] = x;
+                    LU11[j * (NB + 1) + lane] = x;
+                    if (lane == j) pr[NB] = x != 0.0 ? 1.0 / x : 0.0;  // one IEEE division per CTA instead of one per thread
                 }
-                if (t == 0) {
+                if (fetcher && lane == 0) {
                     win_sh[2 * par] = w.pos;
                     win_sh[2 * par + 1] = w.row;
                 }
@@ -248,7 +264,7 @@ __global__ void __launch_bounds__(PT_THREADS, 1) panel_getrf_kernel(PanelArgs p)
                 if (cta == 0) p.perm_out[jg] = win.row;
             }
             const double pivot = pr[j];
-            const double rinv = pivot != 0.0 ? 1.0 / pivot : 0.0;
+            const double rinv = pr[NB];
             const bool have_next = (j + 1 < nbc);
             const double pnext = have_next ? pr[j + 1] : 0.0;
             double lq[RPT_MAX];
@@ -274,7 +290,7 @@ __global__ void __launch_bounds__(PT_THREADS, 1) panel_getrf_kernel(PanelArgs p)
                 publish(mine, jg + 1, j, pr);
                 __syncthreads();  // the candidate row's pre-update values have been read before its owner updates them
             }
-            {
+            if (owner) {
                 double* __restrict__ ab = Ab;
 #pragma unroll 4
                 for (int c2 = j + 2; c2 < nbc; ++c2) {
@@ -290,12 +306,12 @@ __global__ void __launch_bounds__(PT_THREADS, 1) panel_getrf_kernel(PanelArgs p)
 
         // ---- write the inner block back (L multipliers; pivot rows keep their LU row) ----
         __syncthreads();  // every row's inner block is final
-        for (int e = t; e < nbc * Rpad; e += PT_THREADS) {
+        for (int e = t; e < nbc * Rpad; e += PT_LAUNCH) {
             const int c = e / Rpad, lr = e - c * Rpad;
             if (lr < Rloc) W[(int64_t)(jb + c) * ldw + row_base + lr] = Ab[e];
         }
         if (cta == 0 && p.A00 != nullptr) {
-            for (int e = t; e < nsb * nbc; e += PT_THREADS) {
+            for (int e = t; e < nsb * nbc; e += PT_LAUNCH) {
                 const int i = e / nbc, c = e % nbc;
                 p.A00[(size_t)(jb + i) * v + jb + c] = LU11[i * (NB + 1) + c];
             }
@@ -309,7 +325,7 @@ __global__ void __launch_bounds__(PT_THREADS, 1) panel_getrf_kernel(PanelArgs p)
             __threadfence();  // acquire: the epochs observed in phase B order the owners' earlier W stores before my gathers
             // one trailing column per thread: NB independent scattered loads in flight, then the unit-lower forward
             // substitution entirely in registers (L11 broadcast from shared memory)
-            for (int cc = t; cc < rem; cc += PT_THREADS) {
+            for (int cc = t; cc < rem; cc += PT_LAUNCH) {
                 const double* col = W + (int64_t)(cstart + cc) * ldw;
                 double u[NB];
 #pragma unroll
@@ -386,7 +402,7 @@ __global__ void __launch_bounds__(PT_THREADS, 1) panel_getrf_kernel(PanelArgs p)
             if (RPT_MAX == 1 && p.R < PT_THREADS) {
                 const int nshare = PT_THREADS / p.R;  // threads per row
                 const int lr = t % p.R, part = t / p.R;
-                if (part < nshare && lr < Rloc && s_act[lr]) update_row(lr, 4 * part, 4 * nshare, part == 0);
+                if (owner && part < nshare && lr < Rloc && s_act[lr]) update_row(lr, 4 * part, 4 * nshare, part == 0);
             } else {
 #pragma unroll 1
                 for (int q = 0; q < RPT_MAX; ++q) {
@@ -403,7 +419,7 @@ __global__ void __launch_bounds__(PT_THREADS, 1) panel_getrf_kernel(PanelArgs p)
     }
     // identity tail of perm (n < v): LAPACK leaves perm[i] = i for i >= n (conflux_opt.hpp:150-165)
     if (cta == 0)
-        for (int i = p.nsteps + t; i < v; i += PT_THREADS) p.perm_out[i] = i;
+        for (int i = p.nsteps + t; i < v; i += PT_LAUNCH) p.perm_out[i] = i;
 }
 
 // =====================================================================================================================
@@ -603,8 +619,8 @@ int launch_stack_getrf(double* W, int64_t ldw, int n, int v, int* perm_out, Pane
 // the dynamic shared memory of panel_getrf_kernel<NB, *>, laid out in that order
 template <int NB>
 size_t panel_smem_bytes(int Rpad, int v) {
-    return ((size_t)NB * Rpad + (size_t)NB * v + NB * (NB + 1) + 2 * NB) * sizeof(double) +  // Ab, U12, LU11, prow
-           2 * PT_WARPS * (sizeof(unsigned long long) + 2 * sizeof(int)) +                  // red_key, red_pos, red_row
+    return ((size_t)NB * Rpad + (size_t)NB * v + NB * (NB + 1) + 2 * (NB + 1)) * sizeof(double) +  // Ab, U12, LU11, prow
+           2 * PT_ALLWARPS * (sizeof(unsigned long long) + 2 * sizeof(int)) +                     // red_key, red_pos, red_row
            (NB + 4) * sizeof(int) + (size_t)Rpad;                                           // pivrow_blk, win_sh, s_act
 }
 
@@ -628,7 +644,7 @@ int launch_nb_rpt(PanelArgs& a, cudaStream_t stream) {
     static PerDeviceMax cfg;
     if (cfg.raise(smem))
         CFLX_CUDA(cudaFuncSetAttribute(panel_getrf_kernel<NB, RPT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CFLX_CUDA(cudaLaunchCooperativeKernel((void*)panel_getrf_kernel<NB, RPT>, dim3(a.G), dim3(PT_THREADS), params, smem, stream));
+    CFLX_CUDA(cudaLaunchCooperativeKernel((void*)panel_getrf_kernel<NB, RPT>, dim3(a.G), dim3(PT_LAUNCH), params, smem, stream));
     return CFLX_OK;
 }
 template <int NB>
@@ -640,6 +656,7 @@ int launch_nb(PanelArgs& a, cudaStream_t stream) {
     return launch_nb_rpt<NB, 8>(a, stream);
 }
 }  // namespace
+
 
 int panel_workspace_create(PanelWorkspace* ws) {
     int dev = 0, sms = 0;
