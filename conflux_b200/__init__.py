@@ -15,7 +15,7 @@ import numpy as np
 
 from ._lib import ConfluxError, LIB_PATH, SYMBOLS, check, lib
 
-__all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "residual", "validate", "lu_solve", "lu_rcond", "lu_refine", "lu_equilibrate", "lu_svx", "lu_inverse", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
+__all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "residual", "validate", "lu_solve", "lu_rcond", "lu_refine", "lu_equilibrate", "lu_svx", "lu_inverse", "lu_det", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
 
 
 def auto_grid(M, N, P):
@@ -319,6 +319,20 @@ def lu_inverse(gv, out=None):
     return (None if info.value else arr), info.value
 
 
+def lu_det(gv, unscaled=False):
+    """det(A) of the padded matrix of the last LU_rep (P A = L U) on the GPU grid, as an exact-range pair that neither
+    overflows nor underflows: returns dict(sign, logabsdet, mantissa, exponent, info) with det = sign * mantissa *
+    2**exponent, mantissa in [0.5, 1) (0 when singular), logabsdet = log|det|.  info = k when U(k,k) is exactly zero (the
+    first such k, counted from 1): sign 0, logabsdet -inf.  A non-finite U(k,k) before any zero gives NaN.  unscaled=True
+    divides by the scales the factors carry (lu_equilibrate), giving det of the input before scaling.  COLLECTIVE over
+    gv.lu_comm; identical on every rank.  The factors, the permutation and later solves are left as they are."""
+    sign, lad, mant, exp, info = (ctypes.c_double(), ctypes.c_double(), ctypes.c_double(), ctypes.c_int64(),
+                                  ctypes.c_int())
+    check(lib().cflx_lu_det(gv._h, 1 if unscaled else 0, ctypes.byref(sign), ctypes.byref(lad), ctypes.byref(mant),
+                            ctypes.byref(exp), ctypes.byref(info)), "lu_det")
+    return dict(sign=sign.value, logabsdet=lad.value, mantissa=mant.value, exponent=exp.value, info=info.value)
+
+
 class cholesky:
     """Mirror of the reference's CONFCHOX driver interface (src/conflux/cholesky/Cholesky.h:20-22):
         initialize(N, v, grid, comm) -> object;  obj.parallelCholesky() -> ms;  obj.finalize().
@@ -418,6 +432,15 @@ class cholesky:
         ptr, arr = _share_out(out, self.Ml, self.Nl, "cholesky.inverse")
         check(lib().cflx_chol_inverse(self._h, ptr), "chol_inverse")
         return arr
+
+    def det(self, unscaled=False):
+        """det(A) = prod(l_ii)^2 of the padded matrix of the last parallelCholesky on the GPU grid: returns dict(logdet,
+        mantissa, exponent) with det = mantissa * 2**exponent, mantissa in [0.5, 1), as lu_det's pair.  unscaled=True
+        divides by prod(s)^2 of the scaling the factor carries (equilibrate).  COLLECTIVE; identical on every rank."""
+        ld, mant, exp = ctypes.c_double(), ctypes.c_double(), ctypes.c_int64()
+        check(lib().cflx_chol_det(self._h, 1 if unscaled else 0, ctypes.byref(ld), ctypes.byref(mant), ctypes.byref(exp)),
+              "chol_det")
+        return dict(logdet=ld.value, mantissa=mant.value, exponent=exp.value)
 
     def finalize(self, clean=True):
         if self._h:
@@ -602,6 +625,25 @@ class dbg:
                                            Xc.shape[1] if Xc is not None else 0, ptr(pm), W.ctypes.data, ptr(out),
                                            1 if zero_fill else 0), "dbg_inverse_share")
         return W, out
+
+    @staticmethod
+    def det(d, s1=None, s2=None, square=False):
+        """The product kernel of lu_det / cholesky.det on a host vector d (and divisors s1, s2 of its length): returns
+        dict(mantissa, exponent, neg, first_zero, nonfinite) with mantissa * 2**exponent = |prod d| (squared when square)
+        / |prod s1| / |prod s2|, neg the parity of the negative entries (0 when square), first_zero 1 + the first zero
+        index of d (0: none), nonfinite 1 when a non-finite entry (or a zero divisor) comes before it."""
+        d = np.ascontiguousarray(d, dtype=np.float64).ravel()
+        n = d.size
+        vec = lambda s: None if s is None else np.ascontiguousarray(s, dtype=np.float64).ravel()  # noqa: E731
+        s1, s2 = vec(s1), vec(s2)
+        for s in (s1, s2):
+            if s is not None and s.size != n:
+                raise ValueError(f"dbg.det: a divisor must have {n} entries, got {s.size}")
+        mant, exp, neg, fz, nf = ctypes.c_double(), ctypes.c_int64(), ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+        ptr = lambda a: a.ctypes.data if a is not None else None  # noqa: E731
+        check(lib().cflx_dbg_det(n, d.ctypes.data, ptr(s1), ptr(s2), 1 if square else 0, ctypes.byref(mant),
+                                 ctypes.byref(exp), ctypes.byref(neg), ctypes.byref(fz), ctypes.byref(nf)), "dbg_det")
+        return dict(mantissa=mant.value, exponent=exp.value, neg=neg.value, first_zero=fz.value, nonfinite=nf.value)
 
     @staticmethod
     def panel(P, reps=1):

@@ -990,6 +990,21 @@ int cflx_chol_inverse(cflx_chol* ch, double* Ainv_local) {
     return inverse_run(&ch->sv, chol_solve_factor(ch), InvKind::Chol, nullptr, Ainv_local);
 }
 
+// COLLECTIVE.  det(A) = prod(l_ii)^2 (det.cu): the diagonal of L from layer 0's A11, its exact-range product squared,
+// divided by prod(s)^2 when unscaled.
+int cflx_chol_det(cflx_chol* ch, int unscaled, double* logdet_out, double* mant_out, int64_t* exp_out) {
+    if (!ch || (unscaled != 0 && unscaled != 1)) return CFLX_ERR_ARG;
+    CFLX_TRY(chol_check(ch, "determinant"));
+    CFLX_CUDA(cudaSetDevice(ch->comm->device));
+    const double* s = unscaled && ch->eq.fac.equed == 'Y' ? ch->eq.fac.r : nullptr;
+    DetResult d{};
+    CFLX_TRY(det_grid(*ch, &ch->eq, ch->A11, true, s, nullptr, &d));
+    if (logdet_out) *logdet_out = det_log(d);
+    if (mant_out) *mant_out = d.mant;
+    if (exp_out) *exp_out = d.exp;
+    return CFLX_OK;
+}
+
 // COLLECTIVE.  LAPACK dpocon on the grid: ||A||_1 of the symmetric input (its stored lower triangle, real tiles only) and
 // the Hager-Higham estimate of ||inv(A)||_1, whose products inv(A) x are solves with the factor.
 int cflx_chol_rcond(cflx_chol* ch, double* rcond_out, double* anorm_out) {

@@ -400,6 +400,29 @@ int cflx_dbg_inverse_share(int mode, int Ml, int Nl, int v, int Kappa, int Px, i
     return CFLX_OK;
 }
 
+// the determinant's product kernel (det.cu) on host vectors
+int cflx_dbg_det(int n, const double* d, const double* s1, const double* s2, int square, double* mant_out,
+                 int64_t* exp_out, int* neg_out, int* first_zero_out, int* nonfinite_out) {
+    CFLX_TRY(check_device());
+    if (n < 1 || !d || (square != 0 && square != 1)) return CFLX_ERR_ARG;
+    DevBuf dv, dr;
+    CFLX_TRY(dv.alloc(sizeof(double) * 3 * (size_t)n));
+    CFLX_TRY(dr.alloc(sizeof(DetResult)));
+    double* v = dv.as<double>();
+    CFLX_CUDA(cudaMemcpy(v, d, sizeof(double) * n, cudaMemcpyHostToDevice));
+    if (s1) CFLX_CUDA(cudaMemcpy(v + n, s1, sizeof(double) * n, cudaMemcpyHostToDevice));
+    if (s2) CFLX_CUDA(cudaMemcpy(v + 2 * (size_t)n, s2, sizeof(double) * n, cudaMemcpyHostToDevice));
+    CFLX_TRY(launch_det(v, s1 ? v + n : nullptr, s2 ? v + 2 * (size_t)n : nullptr, n, square != 0, dr.as<DetResult>(), 0));
+    DetResult r{};
+    CFLX_CUDA(cudaMemcpy(&r, dr.p, sizeof(r), cudaMemcpyDeviceToHost));
+    if (mant_out) *mant_out = r.mant;
+    if (exp_out) *exp_out = r.exp;
+    if (neg_out) *neg_out = r.neg;
+    if (first_zero_out) *first_zero_out = r.first_zero;
+    if (nonfinite_out) *nonfinite_out = r.nonfinite;
+    return CFLX_OK;
+}
+
 // the residual kernels of the refinement (refine.cu) on one layer-0 share; the timed repetitions run first, then the
 // launch whose result is returned
 int cflx_dbg_residual(int mode, int Ml, int Nl, const double* A, int v, int Kappa, int Px, int Py, int pi, int pj,

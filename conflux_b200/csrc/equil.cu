@@ -202,6 +202,14 @@ int equil_diag(const double* A, const Layout& L, double* diag, cudaStream_t s) {
     return CFLX_OK;
 }
 
+int diag_grid(const Grid& g, const double* A, double* d) {
+    cflx_comm* c = g.comm;
+    if (g.pk == 0) CFLX_TRY(equil_diag(A, g, d, c->stream));
+    else CFLX_CUDA(cudaMemsetAsync(d, 0, sizeof(double) * g.M, c->stream));
+    if (c->world_size > 1) CFLX_NCCL(ncclAllReduce(d, d, (size_t)g.M, ncclDouble, ncclSum, c->world, c->stream));
+    return CFLX_OK;
+}
+
 int equil_apply(double* A, const Layout& L, const double* r, const double* c, char equed, cudaStream_t s) {
     if (L.Ml <= 0 || L.Nl <= 0 || equed == 'N') return CFLX_OK;
     const dim3 grid((L.Nl + 255) / 256, std::min((unsigned)L.Ml, MAX_GRID_Y));
@@ -229,7 +237,7 @@ int launch_scale_rows(double* X, int64_t ld, int M, int n, const double* d, cuda
 
 // ---------------------------------------------------------------- state
 void equil_free(EquilState* e) {
-    for (double* p : {e->in.r, e->in.c, e->fac.r, e->fac.c, e->qr, e->qc, e->B, e->X, e->growth}) cudaFree(p);
+    for (double* p : {e->in.r, e->in.c, e->fac.r, e->fac.c, e->qr, e->qc, e->B, e->X, e->growth, e->det}) cudaFree(p);
     cudaFree(e->ival);
     *e = EquilState{};
 }
@@ -335,9 +343,10 @@ int poequ_grid(const Grid& g, EquilState* e, double* A, bool apply, double* s_ou
     *info = 0;
     *scond = 0.0;
     *equed = 'N';
-    if (g.pk == 0) CFLX_TRY(equil_diag(A, g, sc, s));
-    else CFLX_CUDA(cudaMemsetAsync(sc, 0, sizeof(double) * N, s));
-    CFLX_TRY(reduce_vec(c, sc, N, ncclSum, h));  // one non-zero contributor per element: exact
+    CFLX_TRY(diag_grid(g, A, sc));
+    h.resize(N);
+    CFLX_CUDA(cudaMemcpyAsync(h.data(), sc, sizeof(double) * N, cudaMemcpyDeviceToHost, s));
+    CFLX_CUDA(cudaStreamSynchronize(s));
     double smin = h[0], smax = h[0];
     for (int i = 1; i < N; ++i) smin = std::min(smin, h[i]), smax = std::max(smax, h[i]);
     *amax = smax;

@@ -1144,6 +1144,38 @@ int cflx_lu_inverse(cflx_lu* lu, double* Ainv_local, int* info_out) {
     return inverse_run(&lu->sv, lu_solve_factor(lu), InvKind::LU, lu->hist, Ainv_local);
 }
 
+// COLLECTIVE.  det(A) = det(P) det(U) (det.cu): the diagonal of U from Cbuf, its exact-range product, divided by the
+// products of the scales when unscaled; det(P) from the cycles of the permutation, the same on every rank.
+int cflx_lu_det(cflx_lu* lu, int unscaled, double* sign_out, double* logabsdet_out, double* mant_out, int64_t* exp_out,
+                int* info_out) {
+    if (!lu || (unscaled != 0 && unscaled != 1) || !info_out) return CFLX_ERR_ARG;
+    CFLX_TRY(lu_check(lu, "determinant", false));
+    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    if (!lu->sv.ready) CFLX_TRY(lu_solve_prepare(lu));
+    const EquilRecord& eq = lu->eq.fac;
+    const double* r = unscaled && (eq.equed == 'R' || eq.equed == 'B') ? eq.r : nullptr;
+    const double* c = unscaled && (eq.equed == 'C' || eq.equed == 'B') ? eq.c : nullptr;
+    DetResult d{};
+    CFLX_TRY(det_grid(*lu, &lu->eq, lu->Cbuf, false, r, c, &d));
+    std::vector<int> perm(lu->M);
+    CFLX_TRY(cflx_lu_get_permutation(lu, perm.data()));
+    // det(P) = (-1)^(M - number of cycles): a cycle of length L is L - 1 transpositions
+    std::vector<char> seen(lu->M, 0);
+    int odd = d.neg;
+    for (int i = 0; i < lu->M; ++i)
+        for (int j = i; !seen[j]; j = perm[j]) {
+            seen[j] = 1;
+            odd ^= j != i;
+        }
+    const double sign = d.nonfinite ? std::nan("") : d.first_zero ? 0.0 : odd ? -1.0 : 1.0;
+    if (sign_out) *sign_out = sign;
+    if (logabsdet_out) *logabsdet_out = det_log(d);
+    if (mant_out) *mant_out = d.mant;
+    if (exp_out) *exp_out = d.exp;
+    *info_out = d.first_zero;
+    return CFLX_OK;
+}
+
 // COLLECTIVE.  LAPACK dgerfs on the grid: residuals of the input A0 (refine.cu), corrections and the forward-error
 // estimator's products by the solves above (lu_refine_op).
 int cflx_lu_refine(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, double* X, int ldx, double* ferr_out,

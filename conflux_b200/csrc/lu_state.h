@@ -138,6 +138,7 @@ struct EquilState {
     size_t cap = 0;
     double* growth = nullptr;             // 2 doubles: max |triu(U)|, max |A|
     int* ival = nullptr;                  // 1 int: the first zero pivot
+    double* det = nullptr;                // M + 4 doubles: the gathered diagonal, then det_grid's DetResult
 };
 void equil_free(EquilState* e);
 // *dst = {equed, rowcnd, colcnd} with device copies of r and c (n each; c may be null: then only r is kept)
@@ -341,6 +342,9 @@ int norminf_grid(const Grid& g, const double* A, double* anorm);
 int equil_row_max(const double* A, const Layout& L, double* rowmax, cudaStream_t s);
 int equil_col_max(const double* A, const Layout& L, const double* r, double* colmax, cudaStream_t s);
 int equil_diag(const double* A, const Layout& L, double* diag, cudaStream_t s);
+// COLLECTIVE: d (M doubles, device) = the diagonal of the layer-0 shares A on every rank, bit-identical (equil_diag on
+// layer 0, zeros on the other layers, one ncclSum over the world: one non-zero contributor per element)
+int diag_grid(const Grid& g, const double* A, double* d);
 int equil_apply(double* A, const Layout& L, const double* r, const double* c, char equed, cudaStream_t s);
 int equil_sym_apply(double* A, const Layout& L, const double* sc, cudaStream_t s);
 // On a share F of L\U (and A of the input): *zero_pivot = min(1 + g) over the global diagonal entries g < M the share
@@ -392,4 +396,23 @@ int launch_inverse_zero(const Layout& L, double* out, cudaStream_t s);
 // that skip the block's zero rows), solve_finish's all-reduce and the scatter into Ainv (Ml x Nl, host or device, may be
 // null).  The solve cache must be prepared; perm: the LU's permutation on the device (every rank).
 int inverse_run(SolveCache* sc, const SolveFactor& f, InvKind kind, const int* perm, double* Ainv);
+
+// ---------------------------------------------------------------- the determinant (det.cu)
+constexpr int DET_THREADS = 256;  // the one CTA of the product; part of its order (oracle/det_ref.py)
+// The exact-range product of an M-vector: |prod| = mant 2^exp, mant in [0.5, 1) (NaN / 0 as first_zero and nonfinite
+// say); neg: the parity of the negative entries; first_zero: 1 + the first zero entry of d, 0 when none; nonfinite: an
+// entry that is not finite (or a zero divisor) comes before the first zero.
+struct DetResult {
+    double mant;
+    long long exp;
+    int neg, first_zero, nonfinite, pad;
+};
+// the product kernel on device vectors (s1, s2 may be null), into *out (device)
+int launch_det(const double* d, const double* s1, const double* s2, int n, bool square, DetResult* out, cudaStream_t s);
+// COLLECTIVE: the diagonal of the layer-0 shares F gathered by diag_grid, its product (squared when `square`, divided by
+// the products of s1 and s2 when given: device M-vectors, every rank) and the host copy *res, the same bits on every rank
+int det_grid(const Grid& g, EquilState* e, const double* F, bool square, const double* s1, const double* s2,
+             DetResult* res);
+// log |det| from the pair: -inf with a zero, NaN with a non-finite entry
+double det_log(const DetResult& r);
 }  // namespace cflx

@@ -137,5 +137,14 @@ inline void choleskyInverse(double* Ainv_local) {
     if (!s.plan) throw CholeskyException("choleskyInverse() before initialize()");
     chol_detail::check(cflx_chol_inverse(s.plan, Ainv_local), "choleskyInverse");
 }
+// log det(A) = 2 sum log l_ii of the last parallelCholesky() (cflx_chol_det, collective); det = *mant * 2^*exp.  unscaled:
+// divided by prod(s)^2 of the scaling the factor carries (choleskyEquilibrate).  mant / exp may be null.
+inline double choleskyLogdet(bool unscaled = false, double* mant = nullptr, int64_t* exp = nullptr) {
+    auto& s = chol_detail::state();
+    if (!s.plan) throw CholeskyException("choleskyLogdet() before initialize()");
+    double ld = 0;
+    chol_detail::check(cflx_chol_det(s.plan, unscaled ? 1 : 0, &ld, mant, exp), "choleskyLogdet");
+    return ld;
+}
 
 }  // namespace conflux

@@ -315,4 +315,17 @@ int LU_inverse(lu_params<T>& gv, T* Ainv_local) {
     return info;
 }
 
+// det(A) of the padded matrix of the last LU_rep on the GPU grid (cflx_lu_det, collective): returns log |det| (-inf for
+// an exactly zero U(k,k)); det = *sign * *mant * 2^*exp; *info = k for the first exactly zero U(k,k), else 0.  unscaled:
+// divided by the scales the factors carry (LU_equilibrate).  Any pointer may be null.
+template <class T>
+double LU_det(lu_params<T>& gv, bool unscaled = false, double* sign = nullptr, double* mant = nullptr,
+              int64_t* exp = nullptr, int* info = nullptr) {
+    double lad = 0;
+    int k = 0;
+    check(cflx_lu_det(gv.plan, unscaled ? 1 : 0, sign, &lad, mant, exp, &k), "LU_det");
+    if (info) *info = k;
+    return lad;
+}
+
 }  // namespace conflux

@@ -156,6 +156,19 @@ int cflx_lu_svx(cflx_lu*, int trans, int nrhs, const double* B, int ldb, double*
  * the left one, X A - I).  CFLX_ERR_ARG for a NULL info_out.  CFLX_ERR_STATE as cflx_lu_solve.  Leaves the factors, the
  * permutation, the input, later solves and the launch count as they are. */
 int cflx_lu_inverse(cflx_lu*, double* Ainv_local, int* info_out);
+/* COLLECTIVE.  det of the matrix factored by the last cflx_lu_factor (P A = L U), det = sign mant 2^exp, without overflow
+ * or underflow: sign_out (+1, -1, 0), logabsdet_out (log |det|; -inf when singular), mant_out / exp_out (the exact-range
+ * det: |det| = mant 2^exp, mant in [0.5, 1), or 0 when singular), info_out (k for the first exactly zero U(k,k), counted
+ * from 1, else 0).  Any output may be NULL except info_out.  This is the determinant of the padded M x M matrix, as
+ * cflx_lu_rcond's anorm is its norm: a caller who pads with the identity gets det(A).  A U(k,k) that is inf or NaN with no
+ * zero before it gives sign, mant and logabsdet NaN.  unscaled = 0: the matrix the factors represent (the scaled one after
+ * cflx_lu_equilibrate, as cflx_lu_rcond / _inverse); 1: divided by the scales the factors carry (prod(r) for equed 'R',
+ * prod(c) for 'C', both for 'B'), i.e. det of the input before equilibration (the same bits as 0 when equed = 'N').
+ * Identical bits on every rank and on every call.  CFLX_ERR_ARG for unscaled not 0 / 1 or a NULL info_out;
+ * CFLX_ERR_STATE as cflx_lu_solve.  Leaves the factors, the permutation, the input, later solves and the launch count as
+ * they are. */
+int cflx_lu_det(cflx_lu*, int unscaled, double* sign_out, double* logabsdet_out, double* mant_out, int64_t* exp_out,
+                int* info_out);
 /* 1 when this plan's trailing update runs on the int8 wgmma digit-plane path (ozaki.cu), 0 for the FP64 DMMA kernel
  * (gemm.cu) */
 int cflx_lu_uses_ozaki(const cflx_lu*);
@@ -238,6 +251,11 @@ int cflx_chol_svx(cflx_chol*, int nrhs, const double* B, int ldb, double* X, int
  * memory; may be NULL.  Every layer receives the bits of layer 0.  As for cflx_lu_inverse, the right residual is the
  * small one.  CFLX_ERR_STATE as cflx_chol_solve.  Adds nothing to cflx_chol_launch_count. */
 int cflx_chol_inverse(cflx_chol*, double* Ainv_local);
+/* COLLECTIVE.  det = prod(l_ii)^2 of the padded N x N matrix of the last successful cflx_chol_factor: logdet_out, and the
+ * exact-range det mant_out 2^exp_out as cflx_lu_det's; unscaled = 1 divides by prod(s)^2 of the scaling the factor
+ * carries (equed 'Y').  Any output may be NULL.  Determinism and side effects as cflx_lu_det; CFLX_ERR_ARG for unscaled
+ * not 0 / 1; CFLX_ERR_STATE as cflx_chol_solve. */
+int cflx_chol_det(cflx_chol*, int unscaled, double* logdet_out, double* mant_out, int64_t* exp_out);
 /* number of kernels this object counted since the last reset (bench.py's gpu_launches); cflx_chol_solve adds none */
 int cflx_chol_launch_count(cflx_chol*, int64_t* count_out, int reset);
 void cflx_chol_destroy(cflx_chol*);
@@ -290,6 +308,14 @@ int cflx_dbg_equil(int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int
 int cflx_dbg_inverse_share(int mode, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, int M, int c0,
                            int nc, int rows, const double* X, int ldx, const int* perm, double* W_out,
                            double* share_inout, int zero_fill);
+/* the product kernel of cflx_lu_det / cflx_chol_det on host vectors of n doubles: d, and the divisors s1, s2 (may be
+ * NULL).  mant_out 2^exp_out = |prod d| (square = 1: its square) divided by |prod s1| and |prod s2| (squared too), in the
+ * kernel's fixed order; neg_out: the parity of the negative entries of d, s1 and s2 (0 when square); first_zero_out: 1 +
+ * the first index with d_i == 0, or 0; nonfinite_out: 1 when an entry of d that is inf or NaN, or of a divisor that is
+ * inf, NaN or zero, comes before the first zero (mant is then NaN; with a zero and no such entry before it, mant is 0).
+ * Any output may be NULL. */
+int cflx_dbg_det(int n, const double* d, const double* s1, const double* s2, int square, double* mant_out,
+                 int64_t* exp_out, int* neg_out, int* first_zero_out, int* nonfinite_out);
 /* partial-pivot LU of an n x v row-major panel: perm_out[v], A00_out[v*v] (L00\U00), LU_out[n*v] rows unpermuted */
 int cflx_dbg_panel(int n, int v, const double* panel, int* perm_out, double* A00_out, double* LU_out, int reps,
                    double* ms_out);
