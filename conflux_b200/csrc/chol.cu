@@ -27,21 +27,16 @@
 
 using namespace cflx;
 
-// The grid's M is the padded order N, its Nt the reference's Kappa.
-struct cflx_chol : Grid {
-    double *A0 = nullptr, *A11 = nullptr, *PT = nullptr, *LT = nullptr, *G = nullptr /* [2] */, *Bc = nullptr /* [2] */, *D = nullptr, *A00 = nullptr,
+// The grid's M is the padded order N, its Nt the reference's Kappa.  side: the panel pipeline of step k+1 (all NCCL
+// traffic lives there) under the update of step k.  sv (cflx_chol_solve): inv(L_jj) blocks forward, inv(L_jj)^T
+// backward; rows of real tiles.  eq: s is eq.*.r, scond eq.*.rowcnd.
+struct cflx_chol : Handle {
+    double *PT = nullptr, *LT = nullptr, *G = nullptr /* [2] */, *Bc = nullptr /* [2] */, *D = nullptr, *A00 = nullptr,
            *W = nullptr, *Uinv = nullptr, *LinvT = nullptr, *acc = nullptr, *Q = nullptr /* scratch of the blocked tile Cholesky */;
     int* info = nullptr;
     int64_t ldp = 0, ldb = 0;
-    OzakiWorkspace oz{};                    // digit planes of the int8 wgmma rank-v update (CFLX_GEMM=ozaki, v / Pz 128..512)
-    bool use_ozaki = false;
-    cudaStream_t side = nullptr;            // panel pipeline of step k+1 (all NCCL traffic lives here) under the update of step k
     cudaEvent_t ev_col[2] = {nullptr, nullptr}, ev_panel[2] = {nullptr, nullptr};
-    bool have_input = false, factored = false;
-    int64_t launches = 0;
     SubComm j_comm;                  // grid row of one layer (color pi * Pz + pk, key pj), made by the first solve
-    SolveCache sv;                   // cflx_chol_solve: inv(L_jj) blocks forward, inv(L_jj)^T backward; rows of real tiles
-    EquilState eq;                   // cflx_chol_equilibrate / cflx_chol_svx (s is eq.*.r, scond eq.*.rowcnd)
 };
 
 namespace {
@@ -348,18 +343,14 @@ int chol_pick_nb(int v) {
 void free_chol(cflx_chol* ch) {
     if (!ch) return;
     cudaSetDevice(ch->comm->device);
-    for (double* p : {ch->A0, ch->A11, ch->PT, ch->LT, ch->W, ch->G, ch->Bc, ch->D, ch->A00, ch->Uinv, ch->LinvT, ch->acc, ch->Q}) cudaFree(p);
-    solve_cache_free(&ch->sv);
-    equil_free(&ch->eq);
+    for (double* p : {ch->PT, ch->LT, ch->W, ch->G, ch->Bc, ch->D, ch->A00, ch->Uinv, ch->LinvT, ch->acc, ch->Q}) cudaFree(p);
     cudaFree(ch->info);
-    if (ch->use_ozaki) ozaki_workspace_destroy(&ch->oz);
-    if (ch->side) cudaStreamDestroy(ch->side);
     for (int i = 0; i < 2; ++i) {
         if (ch->ev_col[i]) cudaEventDestroy(ch->ev_col[i]);
         if (ch->ev_panel[i]) cudaEventDestroy(ch->ev_panel[i]);
     }
     if (ch->j_comm.c) ncclCommDestroy(ch->j_comm.c);
-    grid_free(ch);
+    handle_free(ch);
     delete ch;
 }
 
@@ -625,13 +616,10 @@ int chol_solve_prepare(cflx_chol* ch) {
     return CFLX_OK;
 }
 
-// CFLX_OK when `what` may run, after a successful factorisation; otherwise CFLX_ERR_STATE with the reason
-int chol_check(const cflx_chol* ch, const char* what) {
-    if (ch->factored) return CFLX_OK;
-    set_last_error("cholesky %s requested before a successful cflx_chol_factor, or after cflx_chol_set_local without one",
-                   what);
-    return CFLX_ERR_STATE;
-}
+const HandleTexts kCholTexts = {
+    "cholesky %s requested before a successful cflx_chol_factor, or after cflx_chol_set_local without one",
+    "cholesky equilibration requested before cflx_chol_set_local",
+    "cholesky equilibration refused: the input is already scaled (equed = '%c'); upload it again first"};
 
 // dporfs (UPLO = 'L') on the input A0: A is symmetric, so both kinds of product are cflx_chol_solve
 RefineOp chol_refine_op(cflx_chol* ch) {
@@ -741,12 +729,11 @@ int cflx_chol_create(cflx_comm* c, int N, int v, int Px, int Py, int Pz, cflx_ch
         free_chol(ch);
         return code;
     };
-    if ((rc = grid_init(ch, c, Px, Py, Pz))) return fail(rc);
-    const size_t loc = (size_t)ch->Ml * ch->Nl, vv = (size_t)v * v;
+    if ((rc = handle_init(ch, &kCholTexts, c, Px, Py, Pz))) return fail(rc);
+    const size_t vv = (size_t)v * v;
     ch->ldp = round_up(ch->Ml, 2) + 2;
     ch->ldb = round_up(ch->Nl, 2) + 2;
 #define ALLOC(ptr, n) if ((rc = dmalloc(&(ptr), (n)))) return fail(rc)
-    ALLOC(ch->A0, loc); ALLOC(ch->A11, loc);
     ALLOC(ch->PT, (size_t)v * ch->ldp); ALLOC(ch->LT, (size_t)v * ch->ldp); ALLOC(ch->W, (size_t)v * ch->ldp);
     ALLOC(ch->G, 2 * (size_t)Px * v * ch->ldp); ALLOC(ch->Bc, 2 * (size_t)v * ch->ldb);
     ALLOC(ch->D, vv); ALLOC(ch->A00, vv); ALLOC(ch->Uinv, vv); ALLOC(ch->LinvT, vv); ALLOC(ch->acc, 2 + SUMSQ_PARTIALS);
@@ -758,25 +745,14 @@ int cflx_chol_create(cflx_comm* c, int N, int v, int Px, int Py, int Pz, cflx_ch
     cudaMemsetAsync(ch->W, 0, (size_t)v * ch->ldp * sizeof(double), c->stream);
     cudaMemsetAsync(ch->G, 0, 2 * (size_t)Px * v * ch->ldp * sizeof(double), c->stream);
     cudaMemsetAsync(ch->Bc, 0, 2 * (size_t)v * ch->ldb * sizeof(double), c->stream);
-    cudaMemsetAsync(ch->A0, 0, loc * sizeof(double), c->stream);
+    cudaMemsetAsync(ch->A0, 0, (size_t)ch->Ml * ch->Nl * sizeof(double), c->stream);
     cudaMemsetAsync(ch->A00, 0, vv * sizeof(double), c->stream);
-    if ((rc = gemm_tn_setup())) return fail(rc);
-    {
-        const char* e = getenv("CFLX_GEMM");
-        if (e && !strcmp(e, "ozaki") && ch->nlayr % 128 == 0 && ch->nlayr <= 512) {   // as in cflx_lu_create
-            if ((rc = ozaki_workspace_create(&ch->oz, ch->Ml, ch->Nl, ch->nlayr))) return fail(rc);
-            ch->use_ozaki = true;
-        }
-    }
-    {
-        int lo = 0, hi = 0;
-        cudaDeviceGetStreamPriorityRange(&lo, &hi);
-        if (cudaStreamCreateWithPriority(&ch->side, cudaStreamNonBlocking, hi) != cudaSuccess) return fail(CFLX_ERR_CUDA);
-        for (int i = 0; i < 2; ++i)
-            if (cudaEventCreateWithFlags(&ch->ev_col[i], cudaEventDisableTiming) != cudaSuccess ||
-                cudaEventCreateWithFlags(&ch->ev_panel[i], cudaEventDisableTiming) != cudaSuccess)
-                return fail(CFLX_ERR_CUDA);
-    }
+    if ((rc = handle_update_setup(ch))) return fail(rc);
+    if ((rc = handle_side_stream(ch))) return fail(rc);
+    for (int i = 0; i < 2; ++i)
+        if (cudaEventCreateWithFlags(&ch->ev_col[i], cudaEventDisableTiming) != cudaSuccess ||
+            cudaEventCreateWithFlags(&ch->ev_panel[i], cudaEventDisableTiming) != cudaSuccess)
+            return fail(CFLX_ERR_CUDA);
     if ((rc = potrf_setup(v))) return fail(rc);
     if (cudaStreamSynchronize(c->stream) != cudaSuccess) return fail(CFLX_ERR_CUDA);
     *out = ch;
@@ -794,14 +770,7 @@ int cflx_chol_info(const cflx_chol* ch, int* o) {
 
 int cflx_chol_set_local(cflx_chol* ch, const double* host_local) {
     if (!ch || !host_local) return CFLX_ERR_ARG;
-    CFLX_CUDA(cudaSetDevice(ch->comm->device));
-    CFLX_CUDA(cudaMemcpyAsync(ch->A0, host_local, (size_t)ch->Ml * ch->Nl * sizeof(double), cudaMemcpyHostToDevice, ch->comm->stream));
-    CFLX_CUDA(cudaStreamSynchronize(ch->comm->stream));
-    ch->have_input = true;
-    ch->factored = false;
-    ch->sv.ready = false;
-    ch->eq.in.equed = 'N';
-    return CFLX_OK;
+    return handle_set_local(ch, host_local);
 }
 
 // COLLECTIVE.  parallelCholesky() (Cholesky.cpp:760-921): ms_out = device time of the factorisation loop.
@@ -821,10 +790,9 @@ int cflx_chol_factor(cflx_chol* ch, double* ms_out) {
     CFLX_CUDA(cudaMemcpyAsync(ch->A11, ch->A0, (size_t)Ml * Nl * sizeof(double), cudaMemcpyDeviceToDevice, s));
     CFLX_CUDA(cudaMemsetAsync(ch->info, 0, sizeof(int) * 4, s));
     CFLX_TRY(grid_barrier(c));
-    cudaEvent_t e0, e1;
-    CFLX_CUDA(cudaEventCreate(&e0));
-    CFLX_CUDA(cudaEventCreate(&e1));
-    CFLX_CUDA(cudaEventRecord(e0, s));
+    Events<2> loop;
+    CFLX_TRY(loop.create());
+    CFLX_CUDA(cudaEventRecord(loop[0], s));
     // Look-ahead: the panel pipeline of step k+1 (z-reduce, diagonal Cholesky, solve, piece broadcast -- and every NCCL
     // call of the factorisation) runs on the side stream while the main stream applies the rank-v update of step k; the
     // tile column of step k+1 is updated first so that the side stream can start.
@@ -847,12 +815,10 @@ int cflx_chol_factor(cflx_chol* ch, double* ms_out) {
         CFLX_TRY(update_columns(ch, k + 1, k + 1, b, ch->A11, own_next ? ljn + 1 : 0, Nl / v, s, b));
     }
     CFLX_CUDA(cudaStreamWaitEvent(s, ch->ev_panel[(ch->Nt - 1) & 1], 0));
-    CFLX_CUDA(cudaEventRecord(e1, s));
-    CFLX_CUDA(cudaEventSynchronize(e1));
+    CFLX_CUDA(cudaEventRecord(loop[1], s));
+    CFLX_CUDA(cudaEventSynchronize(loop[1]));
     float ms = 0;
-    CFLX_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
+    CFLX_CUDA(cudaEventElapsedTime(&ms, loop[0], loop[1]));
     CFLX_CUDA(cudaGetLastError());
     int h[4] = {0, 0, 0, 0};
     CFLX_CUDA(cudaMemcpy(h, ch->info, sizeof(h), cudaMemcpyDeviceToHost));
@@ -880,7 +846,7 @@ int cflx_chol_factor(cflx_chol* ch, double* ms_out) {
 // local share of L (Ml x Nl row-major, conflux tile layout; tiles above the diagonal are not meaningful)
 int cflx_chol_get_local(cflx_chol* ch, double* L_host) {
     if (!ch || !L_host) return CFLX_ERR_ARG;
-    CFLX_TRY(chol_check(ch, "factor"));
+    CFLX_TRY(handle_check(ch, "factor"));
     CFLX_CUDA(cudaSetDevice(ch->comm->device));
     CFLX_CUDA(cudaMemcpyAsync(L_host, ch->A11, (size_t)ch->Ml * ch->Nl * sizeof(double), cudaMemcpyDeviceToHost, ch->comm->stream));
     CFLX_CUDA(cudaStreamSynchronize(ch->comm->stream));
@@ -892,20 +858,21 @@ int cflx_chol_get_local(cflx_chol* ch, double* L_host) {
 // 183-217, compares against LAPACKE_dpotrf on one node; tests/ do that at small sizes.)
 int cflx_chol_validate(cflx_chol* ch, double* abs_out, double* rel_out) {
     if (!ch) return CFLX_ERR_ARG;
-    CFLX_TRY(chol_check(ch, "validation"));
+    CFLX_TRY(handle_check(ch, "validation"));
     cflx_comm* c = ch->comm;
     cudaStream_t s = c->stream;
     CFLX_CUDA(cudaSetDevice(c->device));
     const int v = ch->v, Px = ch->Px, Py = ch->Py, Ml = ch->Ml, Nl = ch->Nl;
     const size_t loc = (size_t)Ml * Nl;
-    double* R = nullptr;
-    CFLX_TRY(dmalloc(&R, loc));
-    int rc = CFLX_OK;
+    DevBuf Rbuf;
+    CFLX_TRY(Rbuf.alloc(loc * sizeof(double)));
+    double* R = Rbuf.as<double>();
     // every layer replays with the full contraction on layer 0's factor: only layer 0 holds L, so restrict to pk == 0 by
     // zeroing the other layers' contribution (their A11 holds partial sums, not the factor)
-    if (cudaMemcpyAsync(R, ch->A0, loc * sizeof(double), cudaMemcpyDeviceToDevice, s) != cudaSuccess) rc = CFLX_ERR_CUDA;
+    CFLX_CUDA(cudaMemcpyAsync(R, ch->A0, loc * sizeof(double), cudaMemcpyDeviceToDevice, s));
     const int nlayr_save = ch->nlayr, pk_save = ch->pk;
-    for (int t = 0; t < ch->Nt && !rc; ++t) {
+    for (int t = 0; t < ch->Nt; ++t) {
+        int rc = CFLX_OK;
         const int pjt = t % Py;
         const int row0 = first_local_tile(t, ch->pi, Px) * v, n0 = Ml - row0;
         if (ch->pj == pjt && pk_save == 0 && n0 > 0) {
@@ -931,31 +898,24 @@ int cflx_chol_validate(cflx_chol* ch, double* abs_out, double* rel_out) {
         }
         ch->nlayr = nlayr_save;
         ch->pk = pk_save;
+        CFLX_TRY(rc);
     }
-    if (!rc && cudaMemsetAsync(ch->acc, 0, 2 * sizeof(double), s) != cudaSuccess) rc = CFLX_ERR_CUDA;
-    if (!rc && pk_save == 0) {   // acc = {the two sums, the per-CTA partials}
-        auto launch_error = []() -> int {
-            CFLX_CUDA(cudaGetLastError());
-            return CFLX_OK;
-        };
+    CFLX_CUDA(cudaMemsetAsync(ch->acc, 0, 2 * sizeof(double), s));
+    if (pk_save == 0) {   // acc = {the two sums, the per-CTA partials}
         sumsq_lower_kernel<<<SUMSQ_PARTIALS, 256, 0, s>>>(R, *ch, ch->acc + 2);
-        rc = launch_error();
-        if (!rc) rc = launch_sum_partials(ch->acc + 2, SUMSQ_PARTIALS, ch->acc, s);
-        if (!rc) {
-            sumsq_lower_kernel<<<SUMSQ_PARTIALS, 256, 0, s>>>(ch->A0, *ch, ch->acc + 2);
-            rc = launch_error();
-        }
-        if (!rc) rc = launch_sum_partials(ch->acc + 2, SUMSQ_PARTIALS, ch->acc + 1, s);
+        CFLX_CUDA(cudaGetLastError());
+        CFLX_TRY(launch_sum_partials(ch->acc + 2, SUMSQ_PARTIALS, ch->acc, s));
+        sumsq_lower_kernel<<<SUMSQ_PARTIALS, 256, 0, s>>>(ch->A0, *ch, ch->acc + 2);
+        CFLX_CUDA(cudaGetLastError());
+        CFLX_TRY(launch_sum_partials(ch->acc + 2, SUMSQ_PARTIALS, ch->acc + 1, s));
     }
-    if (!rc && ch->P > 1 && ncclAllReduce(ch->acc, ch->acc, 2, ncclDouble, ncclSum, c->world, s) != ncclSuccess) rc = CFLX_ERR_NCCL;
+    if (ch->P > 1) CFLX_NCCL(ncclAllReduce(ch->acc, ch->acc, 2, ncclDouble, ncclSum, c->world, s));
     double h[2] = {0, 0};
-    if (!rc && cudaMemcpyAsync(h, ch->acc, sizeof(h), cudaMemcpyDeviceToHost, s) != cudaSuccess) rc = CFLX_ERR_CUDA;
-    if (cudaStreamSynchronize(s) != cudaSuccess && !rc) {
+    CFLX_CUDA(cudaMemcpyAsync(h, ch->acc, sizeof(h), cudaMemcpyDeviceToHost, s));
+    if (cudaStreamSynchronize(s) != cudaSuccess) {
         set_last_error("cholesky validation: %s", cudaGetErrorString(cudaGetLastError()));
-        rc = CFLX_ERR_CUDA;
+        return CFLX_ERR_CUDA;
     }
-    cudaFree(R);
-    if (rc) return rc;
     if (abs_out) *abs_out = std::sqrt(h[0]);
     if (rel_out) *rel_out = std::sqrt(h[0]) / std::sqrt(h[1]);
     return CFLX_OK;
@@ -965,7 +925,7 @@ int cflx_chol_validate(cflx_chol* ch, double* abs_out, double* rel_out) {
 // are left as they are.
 int cflx_chol_solve(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X, int ldx) {
     if (!ch || nrhs < 1 || ldb < nrhs || (X && ldx < nrhs) || !B) return CFLX_ERR_ARG;
-    CFLX_TRY(chol_check(ch, "solve"));
+    CFLX_TRY(handle_check(ch, "solve"));
     CFLX_CUDA(cudaSetDevice(ch->comm->device));
     if (!ch->sv.ready) CFLX_TRY(chol_solve_prepare(ch));
     const SolveFactor f = chol_solve_factor(ch);
@@ -984,7 +944,7 @@ int cflx_chol_solve(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X
 // cflx_chol_solve, the lower tiles of each block column scattered into this rank's share, the rest of it zero.
 int cflx_chol_inverse(cflx_chol* ch, double* Ainv_local) {
     if (!ch) return CFLX_ERR_ARG;
-    CFLX_TRY(chol_check(ch, "inverse"));
+    CFLX_TRY(handle_check(ch, "inverse"));
     CFLX_CUDA(cudaSetDevice(ch->comm->device));
     if (!ch->sv.ready) CFLX_TRY(chol_solve_prepare(ch));
     return inverse_run(&ch->sv, chol_solve_factor(ch), InvKind::Chol, nullptr, Ainv_local);
@@ -994,7 +954,7 @@ int cflx_chol_inverse(cflx_chol* ch, double* Ainv_local) {
 // divided by prod(s)^2 when unscaled.
 int cflx_chol_det(cflx_chol* ch, int unscaled, double* logdet_out, double* mant_out, int64_t* exp_out) {
     if (!ch || (unscaled != 0 && unscaled != 1)) return CFLX_ERR_ARG;
-    CFLX_TRY(chol_check(ch, "determinant"));
+    CFLX_TRY(handle_check(ch, "determinant"));
     CFLX_CUDA(cudaSetDevice(ch->comm->device));
     const double* s = unscaled && ch->eq.fac.equed == 'Y' ? ch->eq.fac.r : nullptr;
     DetResult d{};
@@ -1009,7 +969,7 @@ int cflx_chol_det(cflx_chol* ch, int unscaled, double* logdet_out, double* mant_
 // the Hager-Higham estimate of ||inv(A)||_1, whose products inv(A) x are solves with the factor.
 int cflx_chol_rcond(cflx_chol* ch, double* rcond_out, double* anorm_out) {
     if (!ch || !rcond_out) return CFLX_ERR_ARG;
-    CFLX_TRY(chol_check(ch, "condition estimate"));
+    CFLX_TRY(handle_check(ch, "condition estimate"));
     CFLX_CUDA(cudaSetDevice(ch->comm->device));
     double anorm = 0.0, ainvnm = 0.0;
     CFLX_TRY(norm1_grid(*ch, ch->A0, true, &anorm));
@@ -1030,7 +990,7 @@ int cflx_chol_rcond(cflx_chol* ch, double* rcond_out, double* anorm_out) {
 int cflx_chol_refine(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X, int ldx, double* ferr_out,
                      double* berr_out) {
     if (!ch || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B || !X) return CFLX_ERR_ARG;
-    CFLX_TRY(chol_check(ch, "refinement"));
+    CFLX_TRY(handle_check(ch, "refinement"));
     CFLX_CUDA(cudaSetDevice(ch->comm->device));
     return refine_run(&ch->sv.rf, chol_refine_op(ch), nrhs, B, ldb, X, ldx, ferr_out, berr_out);
 }
@@ -1040,24 +1000,12 @@ int cflx_chol_refine(cflx_chol* ch, int nrhs, const double* B, int ldb, double* 
 int cflx_chol_equilibrate(cflx_chol* ch, int apply, double* s_out, double* scond_out, double* amax_out, char* equed_out,
                           int* info_out) {
     if (!ch || (apply != 0 && apply != 1) || !info_out) return CFLX_ERR_ARG;
-    if (!ch->have_input) {
-        set_last_error("cholesky equilibration requested before cflx_chol_set_local");
-        return CFLX_ERR_STATE;
-    }
-    if (apply && ch->eq.in.equed != 'N') {
-        set_last_error("cholesky equilibration refused: the input is already scaled (equed = 'Y'); upload it again first");
-        return CFLX_ERR_STATE;
-    }
-    CFLX_CUDA(cudaSetDevice(ch->comm->device));
-    ch->factored = false;
-    ch->sv.ready = false;
+    CFLX_TRY(handle_equil_begin(ch, apply != 0));
     double scond = 0.0, amax = 0.0;
     char equed = 'N';
     int info = 0;
     CFLX_TRY(poequ_grid(*ch, &ch->eq, ch->A0, apply != 0, s_out, &scond, &amax, &equed, &info));
-    // the input's record changes only when this call scaled it; a query (apply = 0) leaves the record and its scales
-    if (apply && info == 0)
-        CFLX_TRY(equil_record_set(&ch->eq.in, equed, scond, scond, ch->eq.qr, nullptr, ch->M, ch->comm->stream));
+    CFLX_TRY(handle_equil_end(ch, apply != 0, info, equed, scond, scond, nullptr));
     if (scond_out) *scond_out = scond;
     if (amax_out) *amax_out = amax;
     if (equed_out) *equed_out = equed;
@@ -1070,7 +1018,7 @@ int cflx_chol_equilibrate(cflx_chol* ch, int apply, double* s_out, double* scond
 int cflx_chol_svx(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out,
                   double* ferr_out, double* berr_out, char* equed_out, int* info_out) {
     if (!ch || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B || !X || !rcond_out || !info_out) return CFLX_ERR_ARG;
-    CFLX_TRY(chol_check(ch, "expert solve"));
+    CFLX_TRY(handle_check(ch, "expert solve"));
     CFLX_CUDA(cudaSetDevice(ch->comm->device));
     const EquilRecord& eq = ch->eq.fac;
     const double* s = eq.equed == 'Y' ? eq.r : nullptr;
@@ -1078,17 +1026,11 @@ int cflx_chol_svx(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X, 
     double rcond = 0.0;
     CFLX_TRY(cflx_chol_rcond(ch, &rcond, nullptr));
     *rcond_out = rcond;
-    CFLX_TRY(svx_tail(&ch->eq, &ch->sv.rf, chol_refine_op(ch), nrhs, B, ldb, X, ldx, ferr_out, berr_out, s, s, eq.rowcnd));
-    *info_out = rcond < std::ldexp(1.0, -53) ? ch->M + 1 : 0;
-    return CFLX_OK;
+    return svx_tail(&ch->eq, &ch->sv.rf, chol_refine_op(ch), nrhs, B, ldb, X, ldx, ferr_out, berr_out, s, s, eq.rowcnd,
+                    rcond, info_out);
 }
 
-int cflx_chol_launch_count(cflx_chol* ch, int64_t* count_out, int reset) {
-    if (!ch || !count_out) return CFLX_ERR_ARG;
-    *count_out = ch->launches;
-    if (reset) ch->launches = 0;
-    return CFLX_OK;
-}
+int cflx_chol_launch_count(cflx_chol* ch, int64_t* count_out, int reset) { return handle_launch_count(ch, count_out, reset); }
 
 void cflx_chol_destroy(cflx_chol* ch) { free_chol(ch); }
 

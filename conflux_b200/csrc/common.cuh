@@ -29,6 +29,37 @@ void set_last_error(const char* fmt, ...);
 
 static inline int64_t round_up(int64_t x, int64_t m) { return (x + m - 1) / m * m; }
 
+// ---- scope-owned device temporaries and timing events: released on every return path ------------------------
+struct DevBuf {
+    void* p = nullptr;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { cudaFree(p); }
+    int alloc(size_t bytes) {
+        CFLX_CUDA(cudaMalloc(&p, bytes + 4096));  // tail pad: bulk copies may over-read
+        return CFLX_OK;
+    }
+    template <class T>
+    T* as() { return (T*)p; }
+};
+template <int N>
+struct Events {
+    cudaEvent_t e[N] = {};
+    Events() = default;
+    Events(const Events&) = delete;
+    Events& operator=(const Events&) = delete;
+    ~Events() {
+        for (cudaEvent_t x : e)
+            if (x) cudaEventDestroy(x);
+    }
+    int create() {
+        for (cudaEvent_t& x : e) CFLX_CUDA(cudaEventCreate(&x));
+        return CFLX_OK;
+    }
+    cudaEvent_t operator[](int i) const { return e[i]; }
+};
+
 // cudaFuncSetAttribute is per DEVICE: ranks may be threads of one process driving different GPUs, so the
 // "already configured" bookkeeping is kept per device ordinal (values only grow; a benign race re-applies it).
 struct PerDeviceMax {

@@ -14,16 +14,6 @@
 using namespace cflx;
 
 namespace {
-struct DevBuf {
-    void* p = nullptr;
-    ~DevBuf() { cudaFree(p); }
-    int alloc(size_t bytes) {
-        CFLX_CUDA(cudaMalloc(&p, bytes + 4096));
-        return CFLX_OK;
-    }
-    template <class T>
-    T* as() { return (T*)p; }
-};
 int check_device() {
     int n = 0;
     if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
@@ -31,6 +21,24 @@ int check_device() {
         set_last_error("no CUDA device visible: conflux_b200 has no CPU fallback");
         return CFLX_ERR_NO_DEVICE;
     }
+    return CFLX_OK;
+}
+
+// *ms_out (may be null) = the mean device time of `reps` (at least 1) back-to-back calls of run() on the default
+// stream, after one warm-up call
+template <class Run>
+int time_reps(Run&& run, int reps, double* ms_out) {
+    Events<2> ev;
+    CFLX_TRY(ev.create());
+    if (reps < 1) reps = 1;
+    CFLX_TRY(run());  // warm-up
+    CFLX_CUDA(cudaEventRecord(ev[0]));
+    for (int r = 0; r < reps; ++r) CFLX_TRY(run());
+    CFLX_CUDA(cudaEventRecord(ev[1]));
+    CFLX_CUDA(cudaEventSynchronize(ev[1]));
+    float ms = 0;
+    CFLX_CUDA(cudaEventElapsedTime(&ms, ev[0], ev[1]));
+    if (ms_out) *ms_out = ms / reps;
     return CFLX_OK;
 }
 
@@ -107,16 +115,15 @@ int cflx_dbg_fp64_peak_ex(int which, double* burst_out, double* sustained_out) {
     const int threads = 256, blocks = sms * 4;
     DevBuf out;
     CFLX_TRY(out.alloc(sizeof(double) * threads * blocks));
-    cudaEvent_t e0, e1;
-    CFLX_CUDA(cudaEventCreate(&e0));
-    CFLX_CUDA(cudaEventCreate(&e1));
+    Events<2> ev;
+    CFLX_TRY(ev.create());
     // flop per warp instruction: m16n8kK = 2*16*8*K (1024 / 2048 / 4096), m8n8k4 = 512; DFMA = 2 flop per lane.
     // The larger shapes run proportionally fewer iterations, so every probe's launches do about the same work.
     const double per_warp_instr = which == 2 ? 1024.0 : which == 3 ? 2048.0 : which == 4 ? 4096.0 : 512.0;
     const int shrink = which == 1 ? 1 : (int)(per_warp_instr / 512.0);
     auto run = [&](int iters, double* tf) -> int {
         iters /= shrink;
-        CFLX_CUDA(cudaEventRecord(e0));
+        CFLX_CUDA(cudaEventRecord(ev[0]));
         switch (which) {
             case 1: dfma_peak_kernel<<<blocks, threads>>>(out.as<double>(), iters); break;
             case 2: dmma16x8_peak_kernel<4><<<blocks, threads>>>(out.as<double>(), iters); break;
@@ -125,10 +132,10 @@ int cflx_dbg_fp64_peak_ex(int which, double* burst_out, double* sustained_out) {
             default: dmma_peak_kernel<<<blocks, threads>>>(out.as<double>(), iters); break;
         }
         CFLX_CUDA(cudaGetLastError());
-        CFLX_CUDA(cudaEventRecord(e1));
-        CFLX_CUDA(cudaEventSynchronize(e1));
+        CFLX_CUDA(cudaEventRecord(ev[1]));
+        CFLX_CUDA(cudaEventSynchronize(ev[1]));
         float ms = 0;
-        CFLX_CUDA(cudaEventElapsedTime(&ms, e0, e1));
+        CFLX_CUDA(cudaEventElapsedTime(&ms, ev[0], ev[1]));
         const double flop = which == 1 ? (double)blocks * threads * iters * 16 * 2.0
                                        : (double)blocks * (threads / 32) * iters * 16 * per_warp_instr;
         *tf = flop / (ms * 1e-3) / 1e12;
@@ -141,8 +148,6 @@ int cflx_dbg_fp64_peak_ex(int which, double* burst_out, double* sustained_out) {
     }
     double sustained = 0;
     CFLX_TRY(run(262144, &sustained));
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
     if (burst_out) *burst_out = burst;
     if (sustained_out) *sustained_out = sustained;
     return CFLX_OK;
@@ -190,20 +195,7 @@ int cflx_dbg_gemm_tn(int M, int N, int K, const double* AT, int at_rows, int64_t
     g.D = (in_place ? dC.as<double>() : dD.as<double>()) + c_at; g.ldd = ldc;
     g.alpha = alpha; g.beta = beta;
     CFLX_TRY(restore());
-    cudaEvent_t e0, e1;
-    CFLX_CUDA(cudaEventCreate(&e0));
-    CFLX_CUDA(cudaEventCreate(&e1));
-    if (reps < 1) reps = 1;
-    CFLX_TRY(launch_gemm_tn(g, 0));  // warm-up
-    CFLX_CUDA(cudaEventRecord(e0));
-    for (int r = 0; r < reps; ++r) CFLX_TRY(launch_gemm_tn(g, 0));
-    CFLX_CUDA(cudaEventRecord(e1));
-    CFLX_CUDA(cudaEventSynchronize(e1));
-    float ms = 0;
-    CFLX_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-    if (ms_out) *ms_out = ms / reps;
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
+    CFLX_TRY(time_reps([&] { return launch_gemm_tn(g, 0); }, reps, ms_out));
     CFLX_TRY(restore());
     CFLX_TRY(launch_gemm_tn(g, 0));
     if (D_out) CFLX_CUDA(cudaMemcpy(D_out, in_place ? dC.p : dD.p, sizeof(double) * c_n, cudaMemcpyDeviceToHost));
@@ -233,20 +225,7 @@ int cflx_dbg_gemm_narrow(int M, int N, int K, const double* A, const double* B, 
     auto run = [&](double* out) {
         return launch_gemm_narrow(M, N, K, dA.as<double>(), K, dB.as<double>(), N, dC.as<double>(), N, out, N, alpha, beta, 0);
     };
-    cudaEvent_t e0, e1;
-    CFLX_CUDA(cudaEventCreate(&e0));
-    CFLX_CUDA(cudaEventCreate(&e1));
-    if (reps < 1) reps = 1;
-    CFLX_TRY(run(dT.as<double>()));  // warm-up
-    CFLX_CUDA(cudaEventRecord(e0));
-    for (int r = 0; r < reps; ++r) CFLX_TRY(run(dT.as<double>()));
-    CFLX_CUDA(cudaEventRecord(e1));
-    CFLX_CUDA(cudaEventSynchronize(e1));
-    float ms = 0;
-    CFLX_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-    if (ms_out) *ms_out = ms / reps;
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
+    CFLX_TRY(time_reps([&] { return run(dT.as<double>()); }, reps, ms_out));
     double* out = alias ? dC.as<double>() : dT.as<double>();
     CFLX_TRY(run(out));
     if (D) CFLX_CUDA(cudaMemcpy(D, out, sizeof(double) * c_n, cudaMemcpyDeviceToHost));
@@ -278,20 +257,7 @@ int cflx_dbg_gemm_narrow_tn(int M, int N, int K, const double* AT, const double*
         return launch_gemm_narrow_tn(M, N, K, dA.as<double>(), ldat, dB.as<double>(), N, dC.as<double>(), N, out, N, alpha,
                                      beta, 0);
     };
-    cudaEvent_t e0, e1;
-    CFLX_CUDA(cudaEventCreate(&e0));
-    CFLX_CUDA(cudaEventCreate(&e1));
-    if (reps < 1) reps = 1;
-    CFLX_TRY(run(dT.as<double>()));  // warm-up
-    CFLX_CUDA(cudaEventRecord(e0));
-    for (int r = 0; r < reps; ++r) CFLX_TRY(run(dT.as<double>()));
-    CFLX_CUDA(cudaEventRecord(e1));
-    CFLX_CUDA(cudaEventSynchronize(e1));
-    float ms = 0;
-    CFLX_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-    if (ms_out) *ms_out = ms / reps;
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
+    CFLX_TRY(time_reps([&] { return run(dT.as<double>()); }, reps, ms_out));
     double* out = alias ? dC.as<double>() : dT.as<double>();
     CFLX_TRY(run(out));
     if (D) CFLX_CUDA(cudaMemcpy(D, out, sizeof(double) * c_n, cudaMemcpyDeviceToHost));
@@ -448,20 +414,7 @@ int cflx_dbg_residual(int mode, int Ml, int Nl, const double* A, int v, int Kapp
         return launch_residual(m, dA.as<double>(), L, dXc.as<double>(), dXr.as<double>(), nrhs, nrhs, dP.as<double>(),
                                dQ.as<double>(), nrhs, 0);
     };
-    cudaEvent_t e0, e1;
-    CFLX_CUDA(cudaEventCreate(&e0));
-    CFLX_CUDA(cudaEventCreate(&e1));
-    if (reps < 1) reps = 1;
-    CFLX_TRY(run());  // warm-up
-    CFLX_CUDA(cudaEventRecord(e0));
-    for (int r = 0; r < reps; ++r) CFLX_TRY(run());
-    CFLX_CUDA(cudaEventRecord(e1));
-    CFLX_CUDA(cudaEventSynchronize(e1));
-    float ms = 0;
-    CFLX_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-    if (ms_out) *ms_out = ms / reps;
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
+    CFLX_TRY(time_reps(run, reps, ms_out));
     CFLX_CUDA(cudaMemset(dP.p, 0, sizeof(double) * o_n));
     CFLX_CUDA(cudaMemset(dQ.p, 0, sizeof(double) * o_n));
     CFLX_TRY(run());
@@ -488,27 +441,24 @@ int cflx_dbg_panel(int n, int v, const double* panel, int* perm_out, double* A00
     CFLX_TRY(dperm.alloc(sizeof(int) * 2 * v));
     CFLX_CUDA(cudaMemcpy(dW0.p, WT.data(), sizeof(double) * v * ld, cudaMemcpyHostToDevice));
     CFLX_CUDA(cudaMemset(dA00.p, 0, sizeof(double) * v * v));
+    Events<2> ev;
+    CFLX_TRY(ev.create());
     PanelWorkspace ws{};
     CFLX_TRY(panel_workspace_create(&ws));
     if (const char* e = getenv("CFLX_PANEL_CTAS")) ws.cta_cap = atoi(e);  // time the search on the look-ahead's SM budget
-    cudaEvent_t e0, e1;
-    CFLX_CUDA(cudaEventCreate(&e0));
-    CFLX_CUDA(cudaEventCreate(&e1));
     if (reps < 1) reps = 1;
     float total = 0;
     int nb = 0, rc = CFLX_OK;
     for (int r = 0; r < reps + 1 && rc == CFLX_OK; ++r) {
         cudaMemcpyAsync(dW.p, dW0.p, sizeof(double) * v * ld, cudaMemcpyDeviceToDevice, 0);
-        cudaEventRecord(e0);
+        cudaEventRecord(ev[0]);
         rc = launch_panel_getrf_a00(dW.as<double>(), ld, n, v, dperm.as<int>(), dA00.as<double>(), &nb, &ws, 0);
-        cudaEventRecord(e1);
-        if (cudaEventSynchronize(e1) != cudaSuccess) rc = CFLX_ERR_CUDA;
+        cudaEventRecord(ev[1]);
+        if (cudaEventSynchronize(ev[1]) != cudaSuccess) rc = CFLX_ERR_CUDA;
         float ms = 0;
-        cudaEventElapsedTime(&ms, e0, e1);
+        cudaEventElapsedTime(&ms, ev[0], ev[1]);
         if (r > 0) total += ms;
     }
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
     if (rc == CFLX_OK && n >= v)
         rc = launch_gather_a00(dW.as<double>(), ld, dperm.as<int>(), v, nb, dA00.as<double>(), dA00T.as<double>(), 0);
     panel_workspace_destroy(&ws);
@@ -695,38 +645,33 @@ int cflx_dbg_ozaki_gemm(int M, int N, int K, int row0, int col0, int max_ctas, c
     CFLX_CUDA(cudaMemcpy(dB.p, B, sizeof(double) * K * ldb, cudaMemcpyHostToDevice));
     if (C) CFLX_CUDA(cudaMemcpy(dC0.p, C, sizeof(double) * M * ldc, cudaMemcpyHostToDevice));
     else CFLX_CUDA(cudaMemset(dC0.p, 0, sizeof(double) * M * ldc));
+    Events<3> ev;
+    CFLX_TRY(ev.create());
     OzakiWorkspace ws;
     int rc = ozaki_workspace_create(&ws, Ma, Nb, K);
-    cudaEvent_t e0, e1, e2;
-    cudaEventCreate(&e0);
-    cudaEventCreate(&e1);
-    cudaEventCreate(&e2);
     if (reps < 1) reps = 1;
     float ms = 0, ms_split = 0;
     for (int r = 0; r < reps + 1 && rc == CFLX_OK; ++r) {
         cudaMemcpyAsync(dC.p, dC0.p, sizeof(double) * M * ldc, cudaMemcpyDeviceToDevice, 0);
-        cudaEventRecord(e0);
+        cudaEventRecord(ev[0]);
         rc = ozaki_split_a(&ws, dA.as<double>(), ldat, Ma, 0);
         if (!rc && col0 > 0) rc = ozaki_split_b(&ws, dB.as<double>(), ldb, 0, col0, 0);
         if (!rc) rc = ozaki_split_b(&ws, dB.as<double>(), ldb, col0, N, 0);
-        cudaEventRecord(e1);
+        cudaEventRecord(ev[1]);
         if (!rc) rc = launch_ozaki_gemm(&ws, M, N, row0, col0, dC.as<double>(), ldc, max_ctas, 0);
-        cudaEventRecord(e2);
-        if (cudaEventSynchronize(e2) != cudaSuccess) {
+        cudaEventRecord(ev[2]);
+        if (cudaEventSynchronize(ev[2]) != cudaSuccess) {
             set_last_error("ozaki kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
             rc = CFLX_ERR_CUDA;
         }
         float a = 0, b = 0;
-        cudaEventElapsedTime(&a, e0, e1);
-        cudaEventElapsedTime(&b, e1, e2);
+        cudaEventElapsedTime(&a, ev[0], ev[1]);
+        cudaEventElapsedTime(&b, ev[1], ev[2]);
         if (r > 0) {
             ms_split += a;
             ms += b;
         }
     }
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    cudaEventDestroy(e2);
     if (rc == CFLX_OK) {
         if (D) cudaMemcpy(D, dC.p, sizeof(double) * M * ldc, cudaMemcpyDeviceToHost);
         for (int s = 0; s < 8; ++s) {

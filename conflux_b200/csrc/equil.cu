@@ -427,7 +427,7 @@ int pivot_growth_grid(const Grid& g, EquilState* e, const double* F, const doubl
 // ---------------------------------------------------------------- the expert drivers' solve
 // B is scaled on the device, solved and refined there, and X is unscaled before the download
 int svx_tail(EquilState* e, RefineCache* rc, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx,
-             double* ferr, double* berr, const double* pre, const double* post, double cnd) {
+             double* ferr, double* berr, const double* pre, const double* post, double cnd, double rcond, int* info) {
     cudaStream_t s = op.grid.comm->stream;
     const int M = op.grid.M, ldn = (int)round_up(nrhs, 8);
     CFLX_TRY(equil_grow(e, M, ldn));
@@ -443,6 +443,7 @@ int svx_tail(EquilState* e, RefineCache* rc, const RefineOp& op, int nrhs, const
     CFLX_CUDA(cudaStreamSynchronize(s));
     if (ferr && post)
         for (int j = 0; j < nrhs; ++j) ferr[j] /= cnd;
+    *info = rcond < std::ldexp(1.0, -53) ? M + 1 : 0;
     return CFLX_OK;
 }
 

@@ -129,7 +129,8 @@ int inverse_run(SolveCache* sc, const SolveFactor& f, InvKind kind, const int* p
     const int ncb = inverse_block_cols(g.M, g.v), ldn = (int)round_up(ncb, 8);
     CFLX_TRY(solve_cache_grow(sc, f, ldn, kind == InvKind::LU || g.pk == 0, kind == InvKind::Chol));
     // device output is written in place; host output goes through one temporary share, copied out once
-    double *dst = nullptr, *tmp = nullptr;
+    double* dst = nullptr;
+    DevBuf tmp;
     const size_t n = (size_t)g.Ml * g.Nl;
     if (Ainv) {
         cudaPointerAttributes at{};
@@ -137,20 +138,19 @@ int inverse_run(SolveCache* sc, const SolveFactor& f, InvKind kind, const int* p
                          (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged);
         cudaGetLastError();  // an unknown host pointer is not an error here
         if (dev) dst = Ainv;
-        else CFLX_TRY(dmalloc(&tmp, n));
-        if (tmp) dst = tmp;
+        else CFLX_TRY(tmp.alloc(n * sizeof(double)));
+        if (tmp.p) dst = tmp.as<double>();
     }
-    int rc = inverse_blocks(sc, f, kind, perm, dst, ldn, ncb);
-    if (!rc && tmp && cudaMemcpyAsync(Ainv, tmp, n * sizeof(double), cudaMemcpyDefault, s) != cudaSuccess) {
+    CFLX_TRY(inverse_blocks(sc, f, kind, perm, dst, ldn, ncb));
+    if (tmp.p && cudaMemcpyAsync(Ainv, tmp.p, n * sizeof(double), cudaMemcpyDefault, s) != cudaSuccess) {
         set_last_error("inverse: copy of the share to the host failed");
-        rc = CFLX_ERR_CUDA;
+        return CFLX_ERR_CUDA;
     }
-    if (cudaStreamSynchronize(s) != cudaSuccess && !rc) {
+    if (cudaStreamSynchronize(s) != cudaSuccess) {
         set_last_error("inverse: %s", cudaGetErrorString(cudaGetLastError()));
-        rc = CFLX_ERR_CUDA;
+        return CFLX_ERR_CUDA;
     }
-    cudaFree(tmp);
-    return rc;
+    return CFLX_OK;
 }
 
 }  // namespace cflx

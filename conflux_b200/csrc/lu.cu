@@ -120,6 +120,81 @@ void grid_free(Grid* g) {
     for (SubComm* sc : {&g->k_comm, &g->i_comm})
         if (sc->c) ncclCommDestroy(sc->c);
 }
+
+int handle_init(Handle* h, const HandleTexts* texts, cflx_comm* c, int Px, int Py, int Pz) {
+    h->texts = texts;
+    CFLX_TRY(grid_init(h, c, Px, Py, Pz));
+    CFLX_TRY(dmalloc(&h->A0, (size_t)h->Ml * h->Nl));
+    return dmalloc(&h->A11, (size_t)h->Ml * h->Nl);
+}
+int handle_update_setup(Handle* h) {
+    CFLX_TRY(gemm_tn_setup());
+    // Trailing update: the FP64 DMMA kernel (gemm.cu).  On H100 the FP64 tensor rate (67 TFLOP/s) is above what the int8
+    // digit-plane path can reach (989 int8 TMAC/s / 36 plane products = 55 TFLOP/s FP64-equivalent), so the int8 wgmma
+    // path (ozaki.cu) runs only on request, CFLX_GEMM=ozaki, where the layer's contraction length is a whole number of
+    // 128-element k chunks.
+    const char* e = getenv("CFLX_GEMM");
+    if (e && !strcmp(e, "ozaki") && h->nlayr % 128 == 0 && h->nlayr <= 512) {
+        CFLX_TRY(ozaki_workspace_create(&h->oz, h->Ml, h->Nl, h->nlayr));
+        h->use_ozaki = true;
+    }
+    return CFLX_OK;
+}
+int handle_side_stream(Handle* h) {
+    int lo = 0, hi = 0;
+    cudaDeviceGetStreamPriorityRange(&lo, &hi);
+    CFLX_CUDA(cudaStreamCreateWithPriority(&h->side, cudaStreamNonBlocking, hi));
+    return CFLX_OK;
+}
+void handle_free(Handle* h) {
+    cudaFree(h->A0);
+    cudaFree(h->A11);
+    solve_cache_free(&h->sv);
+    equil_free(&h->eq);
+    if (h->use_ozaki) ozaki_workspace_destroy(&h->oz);
+    if (h->side) cudaStreamDestroy(h->side);
+    grid_free(h);
+}
+int handle_set_local(Handle* h, const double* host_local) {
+    CFLX_CUDA(cudaSetDevice(h->comm->device));
+    cudaStream_t s = h->comm->stream;
+    CFLX_CUDA(cudaMemcpyAsync(h->A0, host_local, (size_t)h->Ml * h->Nl * sizeof(double), cudaMemcpyHostToDevice, s));
+    CFLX_CUDA(cudaStreamSynchronize(s));
+    h->have_input = true;
+    h->factored = false;
+    h->sv.ready = false;
+    h->eq.in.equed = 'N';
+    return CFLX_OK;
+}
+int handle_check(const Handle* h, const char* what) {
+    if (h->factored) return CFLX_OK;
+    set_last_error(h->texts->unfactored, what);
+    return CFLX_ERR_STATE;
+}
+int handle_equil_begin(Handle* h, bool apply) {
+    if (!h->have_input) {
+        set_last_error("%s", h->texts->no_input);
+        return CFLX_ERR_STATE;
+    }
+    if (apply && h->eq.in.equed != 'N') {
+        set_last_error(h->texts->scaled, h->eq.in.equed);
+        return CFLX_ERR_STATE;
+    }
+    CFLX_CUDA(cudaSetDevice(h->comm->device));
+    h->factored = false;
+    h->sv.ready = false;
+    return CFLX_OK;
+}
+int handle_equil_end(Handle* h, bool apply, int info, char equed, double rowcnd, double colcnd, const double* c) {
+    if (apply && info == 0) CFLX_TRY(equil_record_set(&h->eq.in, equed, rowcnd, colcnd, h->eq.qr, c, h->M, h->comm->stream));
+    return CFLX_OK;
+}
+int handle_launch_count(Handle* h, int64_t* count_out, int reset) {
+    if (!h || !count_out) return CFLX_ERR_ARG;
+    *count_out = h->launches;
+    if (reset) h->launches = 0;
+    return CFLX_OK;
+}
 }  // namespace cflx
 
 namespace {
@@ -510,20 +585,16 @@ int finish_step(cflx_lu* lu, int k, int& fnpr) {
 void free_lu(cflx_lu* lu) {
     if (!lu) return;
     cudaSetDevice(lu->comm->device);
-    double* dbl[] = {lu->A0, lu->A11, lu->PT, lu->PT2, lu->W, lu->LT, lu->A01raw, lu->U, lu->tmp, lu->A00, lu->A00T,
-                     lu->Uinv, lu->LinvT, lu->candH, lu->S, lu->W2, lu->bcast, lu->Cbuf, lu->xbuf};
+    double* dbl[] = {lu->PT, lu->PT2, lu->W, lu->LT, lu->A01raw, lu->U, lu->tmp, lu->A00, lu->A00T, lu->Uinv, lu->LinvT,
+                     lu->candH, lu->S, lu->W2, lu->bcast, lu->Cbuf, lu->xbuf};
     for (double* p : dbl) cudaFree(p);
     int* ints[] = {lu->gri, lu->gri_tmp, lu->igri, lu->perm, lu->gpivots, lu->tagsH, lu->tagsS, lu->hist, lu->plan_mem,
                    lu->idx_buf};
     for (int* p : ints) cudaFree(p);
-    solve_cache_free(&lu->sv);
-    equil_free(&lu->eq);
     if (lu->h_npiv) cudaFreeHost(lu->h_npiv);
     if (lu->pws.slot_hdr) panel_workspace_destroy(&lu->pws);
-    if (lu->use_ozaki) ozaki_workspace_destroy(&lu->oz);
     for (auto& e : lu->ev) cudaEventDestroy(e);
     for (auto& e : lu->tl_pool) cudaEventDestroy(e);
-    if (lu->side) cudaStreamDestroy(lu->side);
     if (lu->ev_fork) cudaEventDestroy(lu->ev_fork);
     if (lu->ev_join) cudaEventDestroy(lu->ev_join);
     if (lu->ev_npiv) cudaEventDestroy(lu->ev_npiv);
@@ -532,7 +603,7 @@ void free_lu(cflx_lu* lu) {
     if (lu->ev_upload) cudaEventDestroy(lu->ev_upload);
     for (SubComm* sc : {&lu->jk_comm, &lu->ik_comm})
         if (sc->c) ncclCommDestroy(sc->c);
-    grid_free(lu);
+    handle_free(lu);
     delete lu;
 }
 
@@ -624,13 +695,15 @@ int lu_sweeps(cflx_lu* lu, bool transposed, bool pa, int nrhs, const double* B, 
     return solve_finish(sc, f, ldn, nrhs, X, ldx, pa ? nullptr : sc->unperm);
 }
 
+const HandleTexts kLuTexts = {
+    "%s requested before cflx_lu_factor, or after cflx_lu_set_local without a factorisation",
+    "equilibration requested before cflx_lu_set_local",
+    "equilibration refused: the input is already scaled (equed = '%c'); upload it again first"};
+
 // CFLX_OK when `what` may run: after a factorisation and, with own_input, while A0 still holds the input of that
 // factorisation; otherwise CFLX_ERR_STATE with the reason
 int lu_check(const cflx_lu* lu, const char* what, bool own_input) {
-    if (!lu->factored) {
-        set_last_error("%s requested before cflx_lu_factor, or after cflx_lu_set_local without a factorisation", what);
-        return CFLX_ERR_STATE;
-    }
+    CFLX_TRY(handle_check(lu, what));
     if (own_input && lu->a0_is_next) {
         set_last_error("%s refused: the input buffer of the last run was handed to the queued next matrix", what);
         return CFLX_ERR_STATE;
@@ -833,16 +906,14 @@ int cflx_lu_create(cflx_comm* c, int M, int N, int v, int Px, int Py, int Pz, cf
         return code;
     };
     // sub-communicators (all ranks call all splits, same order)
-    if ((rc = grid_init(lu, c, Px, Py, Pz))) return fail(rc);
+    if ((rc = handle_init(lu, &kLuTexts, c, Px, Py, Pz))) return fail(rc);
     if ((rc = make_sub(c, lu->pi, lu->pj * Pz + lu->pk, Py * Pz, &lu->jk_comm))) return fail(rc);
     if ((rc = make_sub(c, lu->pj, lu->pi * Pz + lu->pk, Px * Pz, &lu->ik_comm))) return fail(rc);
 
-    const size_t loc = (size_t)lu->Ml * lu->Nl;
     const int64_t ldp = round_up(lu->Ml, 2) + 2;
     lu->ldp_max = ldp;
     const size_t pan = (size_t)v * ldp, upan = (size_t)v * (lu->Nl + 2), vv = (size_t)v * v;
 #define ALLOC(ptr, n) if ((rc = dmalloc(&(ptr), (n)))) return fail(rc)
-    ALLOC(lu->A0, loc); ALLOC(lu->A11, loc);
     ALLOC(lu->PT, pan); ALLOC(lu->PT2, pan); ALLOC(lu->W, pan); ALLOC(lu->LT, pan);
     ALLOC(lu->A01raw, upan); ALLOC(lu->U, upan); ALLOC(lu->tmp, (size_t)v * lu->Nl);
     ALLOC(lu->A00, 2 * vv); ALLOC(lu->A00T, 2 * vv); ALLOC(lu->Uinv, vv); ALLOC(lu->LinvT, vv);
@@ -863,19 +934,7 @@ int cflx_lu_create(cflx_comm* c, int M, int N, int v, int Px, int Py, int Pz, cf
     if (cudaMallocHost((void**)&lu->h_npiv, sizeof(int)) != cudaSuccess) return fail(CFLX_ERR_CUDA);
     if (cudaEventCreateWithFlags(&lu->ev_npiv, cudaEventDisableTiming) != cudaSuccess) return fail(CFLX_ERR_CUDA);
     if ((rc = panel_workspace_create(&lu->pws))) return fail(rc);
-    if ((rc = gemm_tn_setup())) return fail(rc);
-    {
-        // Trailing update: the FP64 DMMA kernel (gemm.cu).  On H100 the FP64 tensor rate (67 TFLOP/s) is above what
-        // the int8 digit-plane path can reach (989 int8 TMAC/s / 36 plane products = 55 TFLOP/s FP64-equivalent), so the
-        // int8 wgmma path (ozaki.cu) runs only on request, CFLX_GEMM=ozaki, where the layer's contraction length is a
-        // whole number of 128-element k chunks.
-        const char* e = getenv("CFLX_GEMM");
-        const bool want = e && !strcmp(e, "ozaki");
-        if (want && lu->nlayr % 128 == 0 && lu->nlayr <= 512) {
-            if ((rc = ozaki_workspace_create(&lu->oz, lu->Ml, lu->Nl, lu->nlayr))) return fail(rc);
-            lu->use_ozaki = true;
-        }
-    }
+    if ((rc = handle_update_setup(lu))) return fail(rc);
     lu->h_hist.assign(lu->M, -1);
     {
         // look-ahead: pivot search of iteration k+1 (extract, layer reduce, local search, tournament exchanges) on a
@@ -886,9 +945,7 @@ int cflx_lu_create(cflx_comm* c, int M, int N, int v, int Px, int Py, int Pz, cf
         const char* em = getenv("CFLX_LOOKAHEAD_MULTI");  // multi-rank grids: on by default (validated on 2x2x1 / 1x1x2)
         const bool want = (e ? atoi(e) != 0 : true) && (lu->P == 1 || !em || atoi(em) != 0);
         if (want) {
-            int lo = 0, hi = 0;
-            cudaDeviceGetStreamPriorityRange(&lo, &hi);
-            if (cudaStreamCreateWithPriority(&lu->side, cudaStreamNonBlocking, hi) != cudaSuccess) return fail(CFLX_ERR_CUDA);
+            if ((rc = handle_side_stream(lu))) return fail(rc);
             if (cudaEventCreateWithFlags(&lu->ev_fork, cudaEventDisableTiming) != cudaSuccess) return fail(CFLX_ERR_CUDA);
             if (cudaEventCreateWithFlags(&lu->ev_join, cudaEventDisableTiming) != cudaSuccess) return fail(CFLX_ERR_CUDA);
             const char* c = getenv("CFLX_PANEL_CTAS");
@@ -904,7 +961,7 @@ int cflx_lu_create(cflx_comm* c, int M, int N, int v, int Px, int Py, int Pz, cf
     cudaMemsetAsync(lu->W, 0, pan * sizeof(double), c->stream);
     cudaMemsetAsync(lu->A01raw, 0, upan * sizeof(double), c->stream);
     cudaMemsetAsync(lu->U, 0, upan * sizeof(double), c->stream);
-    cudaMemsetAsync(lu->A0, 0, loc * sizeof(double), c->stream);
+    cudaMemsetAsync(lu->A0, 0, (size_t)lu->Ml * lu->Nl * sizeof(double), c->stream);
     if (cudaStreamSynchronize(c->stream) != cudaSuccess) return fail(CFLX_ERR_CUDA);
     *out = lu;
     return CFLX_OK;
@@ -920,16 +977,9 @@ int cflx_lu_info(const cflx_lu* lu, int* o) {
 
 int cflx_lu_set_local(cflx_lu* lu, const double* host_local) {
     if (!lu || !host_local) return CFLX_ERR_ARG;
-    CFLX_CUDA(cudaSetDevice(lu->comm->device));
-    const size_t loc = (size_t)lu->Ml * lu->Nl;
-    CFLX_CUDA(cudaMemcpyAsync(lu->A0, host_local, loc * sizeof(double), cudaMemcpyHostToDevice, lu->comm->stream));
-    CFLX_CUDA(cudaStreamSynchronize(lu->comm->stream));
-    lu->have_input = true;
-    lu->factored = false;
-    lu->sv.ready = false;
+    CFLX_TRY(handle_set_local(lu, host_local));
     lu->a0_is_next = false;
     lu->next_host = nullptr;
-    lu->eq.in.equed = 'N';
     return CFLX_OK;
 }
 
@@ -988,10 +1038,9 @@ int cflx_lu_factor(cflx_lu* lu, double* ms_out) {
     lu->tl_recs.clear();
     lu->tl_spans.clear();
     CFLX_TRY(grid_barrier(c));  // MPI_Barrier(lu_comm) before t1 (conflux_opt.hpp:531)
-    cudaEvent_t e0, e1;
-    CFLX_CUDA(cudaEventCreate(&e0));
-    CFLX_CUDA(cudaEventCreate(&e1));
-    CFLX_CUDA(cudaEventRecord(e0, s));
+    Events<2> loop;
+    CFLX_TRY(loop.create());
+    CFLX_CUDA(cudaEventRecord(loop[0], s));
     int fnpr = 0;
     lu->gemm_flops = 0;
     lu->gemm_ms = 0;
@@ -1007,27 +1056,17 @@ int cflx_lu_factor(cflx_lu* lu, double* ms_out) {
             CFLX_CUDA(cudaEventRecord(lu->ev_fork, s));
             CFLX_CUDA(cudaStreamWaitEvent(side, lu->ev_fork, 0));
         }
-        int rc0 = panel_phase(lu, 0, 0, side ? side : s);
-        if (rc0 != CFLX_OK) return rc0;
+        CFLX_TRY(panel_phase(lu, 0, 0, side ? side : s));
         if (side) {
             CFLX_CUDA(cudaEventRecord(lu->ev_join, side));
             CFLX_CUDA(cudaStreamWaitEvent(s, lu->ev_join, 0));
         }
     }
-    for (int k = 0; k < lu->Nt; ++k) {
-        int rc = finish_step(lu, k, fnpr);
-        if (rc != CFLX_OK) {
-            cudaEventDestroy(e0);
-            cudaEventDestroy(e1);
-            return rc;
-        }
-    }
-    CFLX_CUDA(cudaEventRecord(e1, s));
-    CFLX_CUDA(cudaEventSynchronize(e1));
+    for (int k = 0; k < lu->Nt; ++k) CFLX_TRY(finish_step(lu, k, fnpr));
+    CFLX_CUDA(cudaEventRecord(loop[1], s));
+    CFLX_CUDA(cudaEventSynchronize(loop[1]));
     float ms = 0;
-    CFLX_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
+    CFLX_CUDA(cudaEventElapsedTime(&ms, loop[0], loop[1]));
     CFLX_CUDA(cudaGetLastError());
     if (ms_out) *ms_out = ms;
     if (lu->prof_mode == 2) {  // resolve the timeline: every event has completed (e1 was synchronised, the side stream joined)
@@ -1191,26 +1230,13 @@ int cflx_lu_refine(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, d
 int cflx_lu_equilibrate(cflx_lu* lu, int apply, double* r_out, double* c_out, double* rowcnd_out, double* colcnd_out,
                         double* amax_out, char* equed_out, int* info_out) {
     if (!lu || (apply != 0 && apply != 1) || !info_out) return CFLX_ERR_ARG;
-    if (!lu->have_input) {
-        set_last_error("equilibration requested before cflx_lu_set_local");
-        return CFLX_ERR_STATE;
-    }
-    if (apply && lu->eq.in.equed != 'N') {
-        set_last_error("equilibration refused: the input is already scaled (equed = '%c'); upload it again first",
-                       lu->eq.in.equed);
-        return CFLX_ERR_STATE;
-    }
-    CFLX_CUDA(cudaSetDevice(lu->comm->device));
-    cudaStream_t s = lu->comm->stream;
-    if (lu->a0_is_next) CFLX_CUDA(cudaStreamWaitEvent(s, lu->ev_upload, 0));  // A0 holds a streamed next input
-    lu->factored = false;
-    lu->sv.ready = false;
+    CFLX_TRY(handle_equil_begin(lu, apply != 0));
+    if (lu->a0_is_next) CFLX_CUDA(cudaStreamWaitEvent(lu->comm->stream, lu->ev_upload, 0));  // A0 holds a streamed next input
     double rowcnd = 0.0, colcnd = 0.0, amax = 0.0;
     char equed = 'N';
     int info = 0;
     CFLX_TRY(geequ_grid(*lu, &lu->eq, lu->A0, apply != 0, r_out, c_out, &rowcnd, &colcnd, &amax, &equed, &info));
-    // the input's record changes only when this call scaled it; a query (apply = 0) leaves the record and its scales
-    if (apply && info == 0) CFLX_TRY(equil_record_set(&lu->eq.in, equed, rowcnd, colcnd, lu->eq.qr, lu->eq.qc, lu->M, s));
+    CFLX_TRY(handle_equil_end(lu, apply != 0, info, equed, rowcnd, colcnd, lu->eq.qc));
     if (rowcnd_out) *rowcnd_out = rowcnd;
     if (colcnd_out) *colcnd_out = colcnd;
     if (amax_out) *amax_out = amax;
@@ -1247,11 +1273,8 @@ int cflx_lu_svx(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, doub
     *rcond_out = rcond;
     // op(A) X = B: B is scaled by the scales of the rows of op(A), X by those of its columns
     const double *r = rowequ ? eq.r : nullptr, *c = colequ ? eq.c : nullptr;
-    const RefineOp op = lu_refine_op(lu, t);
-    if (!t) CFLX_TRY(svx_tail(&lu->eq, &lu->sv.rf, op, nrhs, B, ldb, X, ldx, ferr_out, berr_out, r, c, eq.colcnd));
-    else CFLX_TRY(svx_tail(&lu->eq, &lu->sv.rf, op, nrhs, B, ldb, X, ldx, ferr_out, berr_out, c, r, eq.rowcnd));
-    if (rcond < std::ldexp(1.0, -53)) *info_out = lu->M + 1;
-    return CFLX_OK;
+    return svx_tail(&lu->eq, &lu->sv.rf, lu_refine_op(lu, t), nrhs, B, ldb, X, ldx, ferr_out, berr_out, t ? c : r,
+                    t ? r : c, t ? eq.rowcnd : eq.colcnd, rcond, info_out);
 }
 
 int cflx_host_alloc(size_t bytes, void** out) {
@@ -1271,12 +1294,7 @@ int cflx_host_free(void* p) {
 }
 
 int cflx_lu_uses_ozaki(const cflx_lu* lu) { return lu && lu->use_ozaki ? 1 : 0; }
-int cflx_lu_launch_count(cflx_lu* lu, int64_t* count_out, int reset) {
-    if (!lu || !count_out) return CFLX_ERR_ARG;
-    *count_out = lu->launches;
-    if (reset) lu->launches = 0;
-    return CFLX_OK;
-}
+int cflx_lu_launch_count(cflx_lu* lu, int64_t* count_out, int reset) { return handle_launch_count(lu, count_out, reset); }
 int cflx_lu_set_profiling(cflx_lu* lu, int mode) {  // 0 off, 1 serialising phase timers, 2 non-serialising timeline
     if (!lu || mode < 0 || mode > 2) return CFLX_ERR_ARG;
     lu->prof_mode = mode;

@@ -192,32 +192,72 @@ struct SolveFactor {
     const SubComm *row_comm, *col_comm;
     int stride;
 };
+
+// How a kind of handle words its state errors (callers match these texts)
+struct HandleTexts {
+    const char* unfactored;  // format, %s: what was requested
+    const char* no_input;    // equilibration before the first upload
+    const char* scaled;      // format, %c: the input's equed
+};
+
+// What the LU and Cholesky handles share: the input and its working copy, the state rules between set_local,
+// equilibrate and factor, the trailing-update choice, the look-ahead stream, the solve cache and the scaling records.
+struct Handle : Grid {
+    const HandleTexts* texts = nullptr;
+    double *A0 = nullptr, *A11 = nullptr;  // the input share and the working copy the factorisation overwrites, Ml x Nl
+    bool have_input = false, factored = false;
+    int64_t launches = 0;
+    cudaStream_t side = nullptr;  // high-priority look-ahead stream (null: no overlap)
+    OzakiWorkspace oz{};          // digit planes of the int8 wgmma trailing update (CFLX_GEMM=ozaki)
+    bool use_ozaki = false;
+    SolveCache sv;
+    EquilState eq;  // cflx_*_equilibrate / cflx_*_svx
+};
+// grid_init, then A0 and A11 (not zeroed)
+int handle_init(Handle* h, const HandleTexts* texts, cflx_comm* c, int Px, int Py, int Pz);
+// the trailing update: the FP64 DMMA kernel, or the int8 digit planes with CFLX_GEMM=ozaki where a layer's contraction
+// length allows.  Called after the handle's own buffers are allocated: loading the update kernels first moves those
+// buffers in device memory, and the one-GPU LU step time moves with them.
+int handle_update_setup(Handle* h);
+// h->side, at the device's highest stream priority
+int handle_side_stream(Handle* h);
+// what handle_init and handle_side_stream made, the solve cache, the scaling records, then grid_free
+void handle_free(Handle* h);
+// host_local into A0, waited for: a new unscaled input, without factors or a solve cache
+int handle_set_local(Handle* h, const double* host_local);
+// CFLX_OK when `what` may run, after a successful factorisation; otherwise CFLX_ERR_STATE with the reason
+int handle_check(const Handle* h, const char* what);
+// equilibrate needs an input, and scales (apply) only an unscaled one; the input then changes, so the factors and the
+// solve cache are dropped, as by set_local
+int handle_equil_begin(Handle* h, bool apply);
+// the input's record changes only when the call scaled it (apply, info == 0): equed with eq.qr and c (may be null); a
+// query leaves the record and its scales
+int handle_equil_end(Handle* h, bool apply, int info, char equed, double rowcnd, double colcnd, const double* c);
+int handle_launch_count(Handle* h, int64_t* count_out, int reset);
 }  // namespace cflx
 
-struct cflx_lu : cflx::Grid {
+// sv (cflx_lu_solve): Linv blocks forward, Uinv blocks backward; rows: row of B of each row of P*B
+struct cflx_lu : cflx::Handle {
     int N = 0, Mt = 0;
     cflx::SubComm jk_comm, ik_comm;
     // device memory
-    double *A0 = nullptr, *A11 = nullptr, *PT = nullptr, *PT2 = nullptr, *W = nullptr, *LT = nullptr, *A01raw = nullptr,
-           *U = nullptr, *tmp = nullptr, *A00 = nullptr, *A00T = nullptr, *Uinv = nullptr, *LinvT = nullptr,
-           *candH = nullptr, *S = nullptr, *W2 = nullptr, *bcast = nullptr, *Cbuf = nullptr, *xbuf = nullptr;
+    double *PT = nullptr, *PT2 = nullptr, *W = nullptr, *LT = nullptr, *A01raw = nullptr, *U = nullptr, *tmp = nullptr,
+           *A00 = nullptr, *A00T = nullptr, *Uinv = nullptr, *LinvT = nullptr, *candH = nullptr, *S = nullptr,
+           *W2 = nullptr, *bcast = nullptr, *Cbuf = nullptr, *xbuf = nullptr;
     int *gri = nullptr, *gri_tmp = nullptr, *igri = nullptr, *perm = nullptr, *gpivots = nullptr, *tagsH = nullptr,
         *tagsS = nullptr, *hist = nullptr, *plan_mem = nullptr, *idx_buf = nullptr;
     cflx::MovePlan plan{};
     cflx::PanelWorkspace pws{};
-    cflx::OzakiWorkspace oz{};   // digit planes of the int8 wgmma trailing update (CFLX_GEMM=ozaki)
-    bool use_ozaki = false;
     int64_t ldp_max = 0;
     int* h_npiv = nullptr;  // pinned
     std::vector<int> h_hist;
-    bool have_input = false, factored = false, time_gemm = false;
+    bool time_gemm = false;
     // double-buffered input streaming (cflx_lu_queue_next_local): the upload of the NEXT matrix overlaps this factorisation
     const double* next_host = nullptr;
     bool a0_is_next = false;  // A0 already holds (or is receiving) the next input: validation of the last run is refused
     cudaStream_t copy = nullptr;
     cudaEvent_t ev_a0_read = nullptr, ev_upload = nullptr;
     double gemm_ms = 0, gemm_flops = 0;
-    int64_t launches = 0;
     double phase_ms[cflx::PH_COUNT] = {0};
     // non-serialising timeline (profiling mode 2): event pairs recorded on the launching stream, resolved after the run
     struct TlRec { int region, side, ev; };
@@ -230,10 +270,7 @@ struct cflx_lu : cflx::Grid {
     int prof_mode = 0;                              // 0 off, 1 serialising phase timers, 2 timeline
     std::vector<cudaEvent_t> ev;
     std::vector<char> ev_used;
-    cudaStream_t side = nullptr;  // high-priority look-ahead stream (null: no overlap)
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_npiv = nullptr;
-    cflx::SolveCache sv;  // cflx_lu_solve: Linv blocks forward, Uinv blocks backward; rows: row of B of each row of P*B
-    cflx::EquilState eq;  // cflx_lu_equilibrate / cflx_lu_svx
 };
 
 namespace cflx {
@@ -325,9 +362,10 @@ int launch_residual(ResidMode mode, const double* A, const Layout& L, const doub
                     int nrhs, double* P, double* Q, int64_t ldo, cudaStream_t s);
 // The solve and refinement of cflx_lu_svx / cflx_chol_svx (equil.cu), COLLECTIVE: B (host or device) to the device, its
 // rows scaled by pre (may be null), X = op.solve(false, B), refine_run, the rows of X scaled by post (may be null), X out;
-// when post is not null, ferr is divided by cnd.
+// when post is not null, ferr is divided by cnd.  Then *info = M + 1 when rcond < 2^-53 (dgesvx / dposvx: the matrix is
+// singular to working precision), else 0.
 int svx_tail(EquilState* e, RefineCache* rc, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx,
-             double* ferr, double* berr, const double* pre, const double* post, double cnd);
+             double* ferr, double* berr, const double* pre, const double* post, double cnd, double rcond, int* info);
 
 // norm.cu: the collective infinity-norm (maximum row sum) of the M x M matrix whose layer-0 shares are A (every local
 // entry counts), into *anorm (every rank).  Deterministic: no floating-point atomics.

@@ -430,26 +430,22 @@ int wgmma_peak_probe(int n, double* tmacs_out) {
     CFLX_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     const size_t smem = 1024 + 4096 + 16384;
     CFLX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int* sink = nullptr;
-    CFLX_CUDA(cudaMalloc((void**)&sink, sizeof(int)));
-    cudaEvent_t e0, e1;
-    CFLX_CUDA(cudaEventCreate(&e0));
-    CFLX_CUDA(cudaEventCreate(&e1));
+    DevBuf sink;
+    CFLX_TRY(sink.alloc(sizeof(int)));
+    Events<2> ev;
+    CFLX_TRY(ev.create());
     const int iters = 20000;
     double best = 0;
     for (int rep = 0; rep < 3; ++rep) {
-        CFLX_CUDA(cudaEventRecord(e0));
-        kern<<<sms, 256, smem>>>(iters, sink);
-        CFLX_CUDA(cudaEventRecord(e1));
-        CFLX_CUDA(cudaEventSynchronize(e1));
+        CFLX_CUDA(cudaEventRecord(ev[0]));
+        kern<<<sms, 256, smem>>>(iters, sink.as<int>());
+        CFLX_CUDA(cudaEventRecord(ev[1]));
+        CFLX_CUDA(cudaEventSynchronize(ev[1]));
         float ms = 0;
-        CFLX_CUDA(cudaEventElapsedTime(&ms, e0, e1));
+        CFLX_CUDA(cudaEventElapsedTime(&ms, ev[0], ev[1]));
         const double macs = (double)sms * 2 * iters * 2 * 64.0 * n * 32.0;
         best = std::max(best, macs / (ms * 1e-3) / 1e12);
     }
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    cudaFree(sink);
     CFLX_CUDA(cudaGetLastError());
     *tmacs_out = best;
     return CFLX_OK;
