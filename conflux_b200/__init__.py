@@ -15,7 +15,7 @@ import numpy as np
 
 from ._lib import ConfluxError, LIB_PATH, SYMBOLS, check, lib
 
-__all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "residual", "validate", "lu_solve", "lu_rcond", "lu_refine", "lu_equilibrate", "lu_svx", "lu_inverse", "lu_det", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
+__all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "residual", "validate", "lu_solve", "lu_rcond", "lu_refine", "lu_refine_x", "lu_equilibrate", "lu_svx", "lu_inverse", "lu_det", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
 
 
 def auto_grid(M, N, P):
@@ -250,6 +250,28 @@ def lu_refine(gv, B, X, trans=False, ferr=True):
     return X2.reshape(shape), (fe if ferr else None), be
 
 
+def _refine_x(fn, n, B, X, cwise, what, *lead):
+    shape, B2, X2, nrhs, be, _ = _refine_args(n, B, X, what)
+    en, ec = np.zeros((nrhs, 3)), np.zeros((nrhs, 3))
+    rcond, info = ctypes.c_double(), ctypes.c_int()
+    check(fn(*lead, nrhs, B2.ctypes.data, nrhs, X2.ctypes.data, nrhs, ctypes.byref(rcond), be.ctypes.data, en.ctypes.data,
+             ec.ctypes.data if cwise else None, ctypes.byref(info)), what)
+    return X2.reshape(shape), dict(rcond=rcond.value, berr=be, err_norm=en, err_comp=ec if cwise else None,
+                                   info=info.value)
+
+
+def lu_refine_x(gv, B, X, trans=False, cwise=True):
+    """LAPACK dgerfsx with the factors of the last LU_rep on the GPU grid: refines X, a solution of A X = B (A^T X = B
+    when trans), with residuals in double-double, to full working accuracy whenever the problem is not too
+    ill-conditioned.  Returns (X, dict(rcond, berr, err_norm, err_comp, info)): err_norm and err_comp are nrhs x 3 rows
+    {trust, err, rcond} (LAPACK's ERR_BNDS) bounding the normwise and componentwise relative errors of the solution,
+    trusted where trust is 1; cwise=False neither pursues nor estimates componentwise accuracy (err_comp is None).  info
+    = k for an exactly zero U(k,k) (X returned as given), M + j when column j's bound was set to 1 because the problem is
+    too ill-conditioned, else 0.  COLLECTIVE over gv.lu_comm; identical on every rank.  The factors, the input and
+    later solves are left as they are."""
+    return _refine_x(lib().cflx_lu_refine_x, gv.M, B, X, cwise, "lu_refine_x", gv._h, 1 if trans else 0)
+
+
 def lu_equilibrate(gv, apply=True, upload=True):
     """LAPACK dgeequ (+ dlaqge when apply) on the padded input on the GPU grid.  upload=True first copies gv.data to the
     device (cflx_lu_set_local), so that LU_rep(gv, upload=False) then factors the scaled matrix As, whose factors carry
@@ -400,6 +422,11 @@ class cholesky:
         check(lib().cflx_chol_refine(self._h, nrhs, B2.ctypes.data, nrhs, X2.ctypes.data, nrhs,
                                      fe.ctypes.data if ferr else None, be.ctypes.data), "chol_refine")
         return X2.reshape(shape), (fe if ferr else None), be
+
+    def refine_x(self, B, X, cwise=True):
+        """LAPACK dporfsx with the factor of the last parallelCholesky on the GPU grid: returns (X, dict(rcond, berr,
+        err_norm, err_comp, info)) as lu_refine_x does.  COLLECTIVE; identical on every rank."""
+        return _refine_x(lib().cflx_chol_refine_x, self.N, B, X, cwise, "cholesky.refine_x", self._h)
 
     def equilibrate(self, apply=True, upload=True):
         """LAPACK dpoequ (+ dlaqsy, lower, when apply) on the padded input on the GPU grid.  upload=True first copies
@@ -573,6 +600,27 @@ class dbg:
                                       int(grid[0]), int(grid[1]), int(pos[0]), int(pos[1]), nrhs, ptr(Xc), ptr(Xr),
                                       P.ctypes.data, Q.ctypes.data, int(reps), ctypes.byref(ms)), "dbg_residual")
         return P, Q, ms.value
+
+    @staticmethod
+    def residual_x(A, mode, v, Kappa=None, grid=(1, 1), pos=(0, 0), Xc=None, Xr=None, Xc_tail=None, Xr_tail=None,
+                   reps=1):
+        """The double-double residual kernels of lu_refine_x / cholesky.refine_x, arguments and modes as residual's,
+        with the tails of X (None: zero).  Returns (Hi, Lo, mean ms of one launch): Hi + Lo = op(A) (X + X_tail)."""
+        A = np.ascontiguousarray(A, dtype=np.float64)
+        Ml, Nl = A.shape
+        m = {"nn": 0, "tn": 1, "sym": 2}[mode]
+        cvt = lambda X: None if X is None else np.ascontiguousarray(np.asarray(X, dtype=np.float64).reshape(X.shape[0], -1))
+        Xc, Xr, Xct, Xrt = cvt(Xc), cvt(Xr), cvt(Xc_tail), cvt(Xr_tail)
+        nrhs = (Xc if Xc is not None else Xr).shape[1]
+        rows = (Ml, Nl, Ml + Nl)[m]
+        H, L = np.empty((rows, nrhs)), np.empty((rows, nrhs))
+        ms = ctypes.c_double()
+        ptr = lambda a: a.ctypes.data if a is not None else None
+        check(lib().cflx_dbg_residual_x(m, Ml, Nl, A.ctypes.data, int(v), int(Kappa if Kappa is not None else 1 << 30),
+                                        int(grid[0]), int(grid[1]), int(pos[0]), int(pos[1]), nrhs, ptr(Xc), ptr(Xct),
+                                        ptr(Xr), ptr(Xrt), H.ctypes.data, L.ctypes.data, int(reps), ctypes.byref(ms)),
+              "dbg_residual_x")
+        return H, L, ms.value
 
     @staticmethod
     def equil(A, v, Kappa=None, grid=(1, 1), pos=(0, 0), M=None, r=None, c=None, equed="N", ncols=None):

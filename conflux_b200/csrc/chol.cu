@@ -995,6 +995,21 @@ int cflx_chol_refine(cflx_chol* ch, int nrhs, const double* B, int ldb, double* 
     return refine_run(&ch->sv.rf, chol_refine_op(ch), nrhs, B, ldb, X, ldx, ferr_out, berr_out);
 }
 
+// COLLECTIVE.  LAPACK dporfsx (UPLO = 'L') on the grid: dpocon, then refine_x_run with the symmetric residual and the
+// scales s of the solution's rows (equed Y).  A successful factorisation has no zero pivot.
+int cflx_chol_refine_x(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out,
+                       double* berr_out, double* err_bnds_norm_out, double* err_bnds_comp_out, int* info_out) {
+    if (!ch || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B || !X || !err_bnds_norm_out || !info_out) return CFLX_ERR_ARG;
+    CFLX_TRY(handle_check(ch, "extra-precise refinement"));
+    CFLX_CUDA(cudaSetDevice(ch->comm->device));
+    double rcond = 0.0;
+    CFLX_TRY(cflx_chol_rcond(ch, &rcond, nullptr));
+    if (rcond_out) *rcond_out = rcond;
+    const EquilRecord& eq = ch->eq.fac;
+    return refine_x_run(&ch->sv.rf, chol_refine_op(ch), nrhs, B, ldb, X, ldx, eq.equed == 'Y' ? eq.r : nullptr, rcond,
+                        err_bnds_comp_out != nullptr, berr_out, err_bnds_norm_out, err_bnds_comp_out, info_out);
+}
+
 // COLLECTIVE.  LAPACK dpoequ (+ dlaqsy, UPLO = 'L', when apply) on the input A0 (equil.cu); drops the factorisation and
 // the solve cache, as cflx_chol_set_local does.
 int cflx_chol_equilibrate(cflx_chol* ch, int apply, double* s_out, double* scond_out, double* amax_out, char* equed_out,

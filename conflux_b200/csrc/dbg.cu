@@ -424,6 +424,46 @@ int cflx_dbg_residual(int mode, int Ml, int Nl, const double* A, int v, int Kapp
     return CFLX_OK;
 }
 
+int cflx_dbg_residual_x(int mode, int Ml, int Nl, const double* A, int v, int Kappa, int Px, int Py, int pi, int pj,
+                        int nrhs, const double* Xc, const double* Xct, const double* Xr, const double* Xrt, double* hi_out,
+                        double* lo_out, int reps, double* ms_out) {
+    CFLX_TRY(check_device());
+    if (mode < 0 || mode > 2 || Ml < 0 || Nl < 0 || v < 1 || nrhs < 1 || !A || Px < 1 || Py < 1 || pi < 0 || pi >= Px ||
+        pj < 0 || pj >= Py || (mode != 1 && !Xc) || (mode != 0 && !Xr))
+        return CFLX_ERR_ARG;
+    const ResidMode m = mode == 0 ? ResidMode::NN : mode == 1 ? ResidMode::TN : ResidMode::SymLower;
+    const int rows = mode == 0 ? Ml : mode == 1 ? Nl : Ml + Nl;
+    const size_t a_n = (size_t)Ml * Nl, o_n = (size_t)std::max(rows, 1) * nrhs;
+    const size_t c_n = (size_t)Nl * nrhs, r_n = (size_t)Ml * nrhs;
+    DevBuf dA, dXc, dXct, dXr, dXrt, dH, dL;
+    CFLX_TRY(dA.alloc(sizeof(double) * a_n));
+    CFLX_TRY(dXc.alloc(sizeof(double) * c_n));
+    CFLX_TRY(dXct.alloc(sizeof(double) * c_n));
+    CFLX_TRY(dXr.alloc(sizeof(double) * r_n));
+    CFLX_TRY(dXrt.alloc(sizeof(double) * r_n));
+    CFLX_TRY(dH.alloc(sizeof(double) * o_n));
+    CFLX_TRY(dL.alloc(sizeof(double) * o_n));
+    CFLX_CUDA(cudaMemcpy(dA.p, A, sizeof(double) * a_n, cudaMemcpyHostToDevice));
+    if (Xc) CFLX_CUDA(cudaMemcpy(dXc.p, Xc, sizeof(double) * c_n, cudaMemcpyHostToDevice));
+    if (Xct) CFLX_CUDA(cudaMemcpy(dXct.p, Xct, sizeof(double) * c_n, cudaMemcpyHostToDevice));
+    if (Xr) CFLX_CUDA(cudaMemcpy(dXr.p, Xr, sizeof(double) * r_n, cudaMemcpyHostToDevice));
+    if (Xrt) CFLX_CUDA(cudaMemcpy(dXrt.p, Xrt, sizeof(double) * r_n, cudaMemcpyHostToDevice));
+    const Layout L{0, v, Kappa, Ml, Nl, Px, Py, pi, pj};
+    auto run = [&]() {
+        return launch_residual_x(m, dA.as<double>(), L, dXc.as<double>(), Xct ? dXct.as<double>() : nullptr,
+                                 dXr.as<double>(), Xrt ? dXrt.as<double>() : nullptr, nrhs, nrhs, dH.as<double>(),
+                                 dL.as<double>(), nrhs, 0);
+    };
+    CFLX_TRY(time_reps(run, reps, ms_out));
+    CFLX_CUDA(cudaMemset(dH.p, 0, sizeof(double) * o_n));
+    CFLX_CUDA(cudaMemset(dL.p, 0, sizeof(double) * o_n));
+    CFLX_TRY(run());
+    if (hi_out) CFLX_CUDA(cudaMemcpy(hi_out, dH.p, sizeof(double) * (size_t)rows * nrhs, cudaMemcpyDeviceToHost));
+    if (lo_out) CFLX_CUDA(cudaMemcpy(lo_out, dL.p, sizeof(double) * (size_t)rows * nrhs, cudaMemcpyDeviceToHost));
+    CFLX_CUDA(cudaDeviceSynchronize());
+    return CFLX_OK;
+}
+
 int cflx_dbg_panel(int n, int v, const double* panel, int* perm_out, double* A00_out, double* LU_out, int reps,
                    double* ms_out) {
     CFLX_TRY(check_device());

@@ -1225,6 +1225,36 @@ int cflx_lu_refine(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, d
     return refine_run(&lu->sv.rf, lu_refine_op(lu, trans != 0), nrhs, B, ldb, X, ldx, ferr_out, berr_out);
 }
 
+// COLLECTIVE.  LAPACK dgerfsx on the grid: the first exactly zero U(k,k), dgecon of A0 in the infinity-norm (trans 0) or
+// the 1-norm (trans 1), then refine_x_run with the scales of the solution's rows: c for trans 0 (equed C / B), r for
+// trans 1 (equed R / B).
+int cflx_lu_refine_x(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out,
+                     double* berr_out, double* err_bnds_norm_out, double* err_bnds_comp_out, int* info_out) {
+    if (!lu || (trans != 0 && trans != 1) || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B || !X || !err_bnds_norm_out ||
+        !info_out)
+        return CFLX_ERR_ARG;
+    CFLX_TRY(lu_check(lu, "extra-precise refinement", true));
+    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    const bool t = trans != 0;
+    if (!lu->sv.ready) CFLX_TRY(lu_solve_prepare(lu));
+    int info = 0;
+    CFLX_TRY(zero_pivot_grid(*lu, &lu->eq, lu->Cbuf, &info));
+    *info_out = info;
+    if (info > 0) {  // exactly singular U: X is left as it was
+        if (rcond_out) *rcond_out = 0.0;
+        return CFLX_OK;
+    }
+    double rcond = 0.0;
+    CFLX_TRY(lu_rcond(lu, !t, &rcond, nullptr));
+    if (rcond_out) *rcond_out = rcond;
+    const EquilRecord& eq = lu->eq.fac;
+    const double* d = !t && (eq.equed == 'C' || eq.equed == 'B') ? eq.c
+                      : t && (eq.equed == 'R' || eq.equed == 'B') ? eq.r
+                                                                   : nullptr;
+    return refine_x_run(&lu->sv.rf, lu_refine_op(lu, t), nrhs, B, ldb, X, ldx, d, rcond, err_bnds_comp_out != nullptr,
+                        berr_out, err_bnds_norm_out, err_bnds_comp_out, info_out);
+}
+
 // COLLECTIVE.  LAPACK dgeequ (+ dlaqge when apply) on the input A0 (equil.cu).  The input changes, so the factorisation
 // and the solve cache are dropped, as by cflx_lu_set_local.
 int cflx_lu_equilibrate(cflx_lu* lu, int apply, double* r_out, double* c_out, double* rowcnd_out, double* colcnd_out,

@@ -5,6 +5,7 @@
 #include <nccl.h>
 
 #include <algorithm>
+#include <cmath>
 #include <functional>
 #include <vector>
 
@@ -115,6 +116,9 @@ struct RefineCache {
     double *X = nullptr, *B = nullptr, *R = nullptr, *D = nullptr, *rhs = nullptr, *ratio = nullptr, *W = nullptr;
     double *Xc = nullptr, *Xr = nullptr, *part = nullptr, *all = nullptr, *berr = nullptr;
     size_t cap_m = 0, cap_c = 0, cap_r = 0, cap_part = 0, cap_all = 0, cap_berr = 0, cap_active = 0;
+    // cflx_*_refine_x only: the tail of X (M x ldn) and its gathered copies, the per-column statistics of a round
+    double *T = nullptr, *Xct = nullptr, *Xrt = nullptr, *stats = nullptr;
+    size_t cap_t = 0, cap_ct = 0, cap_rt = 0, cap_stats = 0;
 };
 
 // ---------------------------------------------------------------- equilibration and the expert drivers (equil.cu)
@@ -350,6 +354,28 @@ struct RefineOp {
 int refine_run(RefineCache* rc, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx, double* ferr,
                double* berr);
 void refine_cache_free(RefineCache* rc);
+// One column of LAPACK's dla_gerfsx_extended / dla_porfsx_extended: its precision state and the normwise (x) and
+// componentwise (z) convergence states, with LAPACK's initial values.  round() takes the statistics of one round,
+// {normy, normx, normdx, dz_z, ymin} (refine.cu column_stats_kernel), and returns what to do with the correction dy:
+// 0 stop (no update), 1 y += dy, 2 (y, y_tail) += dy in double-double.  finish() sets the error estimates.
+struct RefineXColumn {
+    enum { UNSTABLE = 0, WORKING = 1, CONV = 2, NOPROG = 3 };
+    enum { EXTRA_RESIDUAL = 1, EXTRA_Y = 2 };
+    int x_state = WORKING, z_state = UNSTABLE, y_prec = EXTRA_RESIDUAL;
+    bool done = false;
+    double dx_x = INFINITY, dz_z = INFINITY, prev_normdx = INFINITY, prev_dz_z = INFINITY;
+    double dxratmax = 0.0, dzratmax = 0.0, final_dx_x = INFINITY, final_dz_z = INFINITY;
+    double err_norm = 0.0, err_comp = 0.0;
+    int round(const double st[5], double rcond, bool ignore_cwise, int cnt, int M);
+    void finish();
+};
+// LAPACK dgerfsx / dporfsx on the grid (collective), after the caller's zero-pivot check: X (host or device, M x nrhs,
+// ldx) refined in place from B with residuals in double-double (launch_residual_x); d (device, M; null: ones) the scales
+// of the unscaled solution diag(d) y; rcond the dgecon / dpocon estimate the precision switch uses.  Per column: berr
+// (may be null), err_norm and (when cwise) err_comp as nrhs x 3 {trust, err, rcond}.  *info = M + j for the first
+// column j (1-based) with a bound set to 1 for an ill-conditioned problem, else 0.
+int refine_x_run(RefineCache* rc, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx,
+                 const double* d, double rcond, bool cwise, double* berr, double* err_norm, double* err_comp, int* info);
 // The residual kernels (refine.cu).  From layer 0's share A (L's layout, lda = Nl even, 16-byte aligned, v % 4 == 0)
 // and X gathered by local column (Xc, Nl x nrhs) or by local row (Xr, Ml x nrhs), both with leading dimension ldx:
 //   NN:       P = A Xc, Q = |A| |Xc| by local row (Ml rows);
@@ -360,6 +386,12 @@ void refine_cache_free(RefineCache* rc);
 // P and Q have leading dimension ldo.  Deterministic: no floating-point atomics.
 int launch_residual(ResidMode mode, const double* A, const Layout& L, const double* Xc, const double* Xr, int64_t ldx,
                     int nrhs, double* P, double* Q, int64_t ldo, cudaStream_t s);
+// Their double-double counterparts (SIMT FP64, Dot2): Hi + Lo = op(A) (X + Xt) in the same modes, layouts and masks, from
+// the head Xc / Xr and the tail Xct / Xrt (either tail may be null: zero).  The entries are combined in a fixed order
+// (lanes, then warps, by double-double additions): deterministic, no atomics.
+int launch_residual_x(ResidMode mode, const double* A, const Layout& L, const double* Xc, const double* Xct,
+                      const double* Xr, const double* Xrt, int64_t ldx, int nrhs, double* Hi, double* Lo, int64_t ldo,
+                      cudaStream_t s);
 // The solve and refinement of cflx_lu_svx / cflx_chol_svx (equil.cu), COLLECTIVE: B (host or device) to the device, its
 // rows scaled by pre (may be null), X = op.solve(false, B), refine_run, the rows of X scaled by post (may be null), X out;
 // when post is not null, ferr is divided by cnd.  Then *info = M + 1 when rcond < 2^-53 (dgesvx / dposvx: the matrix is

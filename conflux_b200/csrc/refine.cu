@@ -1,5 +1,6 @@
 // conflux_b200/csrc/refine.cu -- iterative refinement with error bounds (cflx_lu_refine, cflx_chol_refine): LAPACK's
-// dgerfs / dporfs on the GPU grid.
+// dgerfs / dporfs on the GPU grid; and extra-precise refinement with trusted error bounds (cflx_lu_refine_x,
+// cflx_chol_refine_x): dgerfsx / dporfsx, whose residuals come from the double-double kernels below (DESIGN.md §7h).
 //
 // The residual kernels read layer 0's local share A (Ml x Nl, conflux layout: local (r, c) is global
 // (Layout::row(r), Layout::col(c))) once and produce two partial products at once:
@@ -299,6 +300,162 @@ int dispatch_tn(const ResidArgs& r, cudaStream_t s) {
     return launch_tn<4, MASK>(r, s);
 }
 
+// ---------------------------------------------------------------- the double-double residual kernels (refine_x)
+// Error-free transformations with the rounding spelled out (__dadd_rn / __dmul_rn are never contracted into an fma).
+struct DD {
+    double hi, lo;
+};
+__device__ __forceinline__ void two_sum(double a, double b, double& s, double& e) {
+    s = __dadd_rn(a, b);
+    const double bb = __dsub_rn(s, a);
+    e = __dadd_rn(__dsub_rn(a, __dsub_rn(s, bb)), __dsub_rn(b, bb));
+}
+__device__ __forceinline__ DD dd_add(DD a, DD b) {
+    double s, e;
+    two_sum(a.hi, b.hi, s, e);
+    e = __dadd_rn(e, __dadd_rn(a.lo, b.lo));
+    DD r;
+    two_sum(s, e, r.hi, r.lo);
+    return r;
+}
+// Dot2 (Ogita, Rump, Oishi 2005) over the terms a (y + t): s collects the rounded products, c every rounding error
+// (TwoProd by fma, TwoSum), and the tail's product, whose own rounding is second order
+__device__ __forceinline__ void dot2_step(double a, double y, double t, double& s, double& c) {
+    const double p = __dmul_rn(a, y), pe = fma(a, y, -p);
+    double s2, q;
+    two_sum(s, p, s2, q);
+    s = s2;
+    c = fma(a, t, __dadd_rn(c, __dadd_rn(q, pe)));
+}
+
+struct ResidXArgs {
+    int M, N, K;  // output rows, right-hand sides, reduction length (local indices)
+    const double* A;
+    int64_t lda;
+    const double *Y, *T;  // [K x N], ldb: the head and the tail of X gathered (T may be null: zero)
+    int64_t ldb;
+    double *Hi, *Lo;  // [M x N], ldo
+    int64_t ldo;
+    int v, Kappa, mask;
+    int Pm, pm, Pk, pk;
+};
+
+__device__ __forceinline__ bool keep_entry(const ResidXArgs& r, int gm, int gk) {
+    if (r.mask == MASK_NONE) return true;
+    if (gm / r.v >= r.Kappa || gk / r.v >= r.Kappa) return false;
+    return r.mask == MASK_LOWER ? gm >= gk : gk > gm;
+}
+
+constexpr int XW = 8;         // warps per CTA
+constexpr int XROWS = 2;      // NN: output rows per warp
+// NN: warp w of the CTA owns output rows blockIdx.x * XW * XROWS + w * XROWS + (0, 1); lane l reduces k = l, l + 32, ...
+// (A read coalesced along its rows); the 32 lanes are combined by a butterfly of double-double additions.
+template <int NB>
+__global__ void __launch_bounds__(XW * 32) resid_x_nn_kernel(ResidXArgs r) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int m0 = (blockIdx.x * XW + warp) * XROWS, n0 = blockIdx.y * NB;
+    double s[XROWS][NB], c[XROWS][NB];
+    int gm[XROWS];
+#pragma unroll
+    for (int i = 0; i < XROWS; ++i) {
+        gm[i] = Layout::global(m0 + i, r.Pm, r.pm, r.v);
+#pragma unroll
+        for (int j = 0; j < NB; ++j) s[i][j] = c[i][j] = 0.0;
+    }
+    for (int k = lane; k < r.K; k += 32) {
+        const int gk = Layout::global(k, r.Pk, r.pk, r.v);
+        double y[NB], t[NB];
+#pragma unroll
+        for (int j = 0; j < NB; ++j) {
+            const bool in = n0 + j < r.N;
+            y[j] = in ? r.Y[(int64_t)k * r.ldb + n0 + j] : 0.0;
+            t[j] = in && r.T ? r.T[(int64_t)k * r.ldb + n0 + j] : 0.0;
+        }
+#pragma unroll
+        for (int i = 0; i < XROWS; ++i) {
+            if (m0 + i >= r.M) continue;
+            const double raw = r.A[(int64_t)(m0 + i) * r.lda + k];
+            const double a = keep_entry(r, gm[i], gk) ? raw : 0.0;  // selected away, never multiplied
+#pragma unroll
+            for (int j = 0; j < NB; ++j) dot2_step(a, y[j], t[j], s[i][j], c[i][j]);
+        }
+    }
+#pragma unroll
+    for (int i = 0; i < XROWS; ++i)
+#pragma unroll
+        for (int j = 0; j < NB; ++j) {
+            DD p;
+            two_sum(s[i][j], c[i][j], p.hi, p.lo);
+#pragma unroll
+            for (int w = 16; w > 0; w >>= 1) {
+                const DD o{__shfl_xor_sync(0xffffffffu, p.hi, w), __shfl_xor_sync(0xffffffffu, p.lo, w)};
+                p = lane & w ? dd_add(o, p) : dd_add(p, o);  // both lanes of a pair form the same sum
+            }
+            if (lane == 0 && m0 + i < r.M && n0 + j < r.N) {
+                r.Hi[(int64_t)(m0 + i) * r.ldo + n0 + j] = p.hi;
+                r.Lo[(int64_t)(m0 + i) * r.ldo + n0 + j] = p.lo;
+            }
+        }
+}
+
+// TN: lane l of every warp owns output m = blockIdx.x * 32 + l (A^T: column m of A, read coalesced along A's rows);
+// warp w reduces k = w, w + XW, ...; the XW warps' partials are combined in shared memory by a fixed tree.
+template <int NB>
+__global__ void __launch_bounds__(XW * 32) resid_x_tn_kernel(ResidXArgs r) {
+    __shared__ DD sh[XW][32][NB];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int m = blockIdx.x * 32 + lane, n0 = blockIdx.y * NB;
+    const bool live = m < r.M;
+    const int gm = Layout::global(live ? m : 0, r.Pm, r.pm, r.v);
+    double s[NB], c[NB];
+#pragma unroll
+    for (int j = 0; j < NB; ++j) s[j] = c[j] = 0.0;
+    for (int k = warp; k < r.K; k += XW) {
+        const int gk = Layout::global(k, r.Pk, r.pk, r.v);
+        const double raw = live ? r.A[(int64_t)k * r.lda + m] : 0.0;
+        const double a = live && keep_entry(r, gm, gk) ? raw : 0.0;
+#pragma unroll
+        for (int j = 0; j < NB; ++j) {
+            const bool in = n0 + j < r.N;
+            const double y = in ? r.Y[(int64_t)k * r.ldb + n0 + j] : 0.0;
+            const double t = in && r.T ? r.T[(int64_t)k * r.ldb + n0 + j] : 0.0;
+            dot2_step(a, y, t, s[j], c[j]);
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < NB; ++j) two_sum(s[j], c[j], sh[warp][lane][j].hi, sh[warp][lane][j].lo);
+    __syncthreads();
+    for (int w = XW / 2; w > 0; w >>= 1) {
+        if (warp < w)
+#pragma unroll
+            for (int j = 0; j < NB; ++j) sh[warp][lane][j] = dd_add(sh[warp][lane][j], sh[warp + w][lane][j]);
+        __syncthreads();
+    }
+    if (warp == 0 && live)
+#pragma unroll
+        for (int j = 0; j < NB; ++j)
+            if (n0 + j < r.N) {
+                r.Hi[(int64_t)m * r.ldo + n0 + j] = sh[0][lane][j].hi;
+                r.Lo[(int64_t)m * r.ldo + n0 + j] = sh[0][lane][j].lo;
+            }
+}
+
+template <int NB>
+int launch_x(const ResidXArgs& r, bool tn, cudaStream_t s) {
+    if (r.M <= 0) return CFLX_OK;
+    const unsigned gy = (unsigned)((r.N + NB - 1) / NB);
+    if (tn) resid_x_tn_kernel<NB><<<dim3((unsigned)((r.M + 31) / 32), gy), XW * 32, 0, s>>>(r);
+    else resid_x_nn_kernel<NB><<<dim3((unsigned)((r.M + XW * XROWS - 1) / (XW * XROWS)), gy), XW * 32, 0, s>>>(r);
+    CFLX_CUDA(cudaGetLastError());
+    return CFLX_OK;
+}
+int dispatch_x(const ResidXArgs& r, bool tn, cudaStream_t s) {
+    if (r.N <= 1) return launch_x<1>(r, tn, s);
+    if (r.N <= 2) return launch_x<2>(r, tn, s);
+    if (r.N <= 4) return launch_x<4>(r, tn, s);
+    return launch_x<8>(r, tn, s);  // slabs of 8 columns, one per blockIdx.y
+}
+
 // ---------------------------------------------------------------- assembly and the per-column backward error
 struct AssembleArgs {
     const double* all;  // the partials of every world rank, `chunk` doubles apart: rows of 2 ldn (P, then Q)
@@ -309,6 +466,8 @@ struct AssembleArgs {
     const double* B;       // [M x ldn]
     double *R, *ratio, *W;  // [M x ldn]: b - op(A) x, the backward-error ratio, dgerfs' w
     double safe1, safe2, nzeps;
+    bool lin_berr;      // refine_x: ratio = (|r_i| + safe1) / s_i where s_i != 0, else 0 (LAPACK dla_lin_berr); no W
+    double* Q;          // refine_x (may be null): |op(A)| |x|
 };
 
 // every rank adds the same partials in the same order: for global row g (tile T), the NN partials of the ranks
@@ -338,6 +497,11 @@ __global__ void assemble_kernel(AssembleArgs a) {
     const int64_t o = (int64_t)g * a.ldn + c;
     const double b = a.B[o], r = b - p, s = q + fabs(b);
     a.R[o] = r;
+    if (a.Q) a.Q[o] = q;
+    if (a.lin_berr) {
+        a.ratio[o] = s != 0.0 ? (fabs(r) + a.safe1) / s : 0.0;
+        return;
+    }
     // dgerfs: s_i > safe2 ? |r_i| / s_i : (|r_i| + safe1) / (s_i + safe1);  w_i = |r_i| + nz eps s_i (+ safe1)
     a.ratio[o] = s > a.safe2 ? fabs(r) / s : (fabs(r) + a.safe1) / (s + a.safe1);
     a.W[o] = s > a.safe2 ? fabs(r) + a.nzeps * s : fabs(r) + a.nzeps * s + a.safe1;
@@ -375,6 +539,86 @@ __global__ void add_cols_kernel(double* __restrict__ X, const double* __restrict
     if (active[e % ldn]) X[e] = X[e] + D[e];
 }
 
+// refine_x: R = b - sum of the double-double partials (rows of 2 ldn: Hi, then Lo), added in assemble_kernel's order in
+// double-double, b subtracted in double-double and rounded once
+__global__ void assemble_x_kernel(AssembleArgs a) {
+    const int g = blockIdx.x, c = threadIdx.x + blockIdx.y * blockDim.x;
+    if (g >= a.M || c >= a.nrhs) return;
+    const int T = g / a.v, e = g % a.v;
+    const int64_t ld2 = 2 * (int64_t)a.ldn;
+    DD p{0.0, 0.0};
+    if (a.nn) {
+        const int64_t row = (int64_t)(T / a.Px) * a.v + e;
+        for (int pj = 0; pj < a.Py; ++pj) {
+            const double* src = a.all + (int64_t)(((T % a.Px) * a.Py + pj) * a.Pz) * a.chunk + row * ld2;
+            p = dd_add(p, DD{src[c], src[a.ldn + c]});
+        }
+    }
+    if (a.tn) {
+        const int64_t row = (a.nn ? a.Ml : 0) + (int64_t)(T / a.Py) * a.v + e;
+        for (int pi = 0; pi < a.Px; ++pi) {
+            const double* src = a.all + (int64_t)((pi * a.Py + T % a.Py) * a.Pz) * a.chunk + row * ld2;
+            p = dd_add(p, DD{src[c], src[a.ldn + c]});
+        }
+    }
+    const int64_t o = (int64_t)g * a.ldn + c;
+    double s, err;
+    two_sum(a.B[o], -p.hi, s, err);
+    a.R[o] = __dadd_rn(s, __dsub_rn(err, p.lo));
+}
+
+// refine_x's per-column quantities of one round, by a fixed tree: {normy = max |y|, normx = max |y| d, normdx =
+// max |dy| d, dz_z = max |dy| / |y| (+inf where y = 0 != dy), ymin = min |y|} (d null: ones; NaN wins)
+constexpr int NSTAT = 5;
+__global__ void __launch_bounds__(MAXT) column_stats_kernel(const double* __restrict__ Y, const double* __restrict__ DY,
+                                                            const double* __restrict__ d, int M, int ldn,
+                                                            double* __restrict__ out) {
+    __shared__ double sh[NSTAT][MAXT];
+    const int c = blockIdx.x;
+    auto mx = [](double a, double b) { return (b > a || b != b) ? b : a; };
+    auto mn = [](double a, double b) { return (b < a || b != b) ? b : a; };
+    double v[NSTAT] = {0.0, 0.0, 0.0, 0.0, INFINITY};
+    for (int i = threadIdx.x; i < M; i += MAXT) {
+        const double yk = fabs(Y[(int64_t)i * ldn + c]), dyk = fabs(DY[(int64_t)i * ldn + c]), di = d ? d[i] : 1.0;
+        v[0] = mx(v[0], yk);
+        v[1] = mx(v[1], d ? yk * di : yk);
+        v[2] = mx(v[2], d ? dyk * di : dyk);
+        v[3] = mx(v[3], yk != 0.0 ? dyk / yk : dyk != 0.0 ? INFINITY : 0.0);
+        v[4] = mn(v[4], yk);
+    }
+#pragma unroll
+    for (int q = 0; q < NSTAT; ++q) sh[q][threadIdx.x] = v[q];
+    __syncthreads();
+    for (int w = MAXT / 2; w > 0; w >>= 1) {
+        if (threadIdx.x < w) {
+#pragma unroll
+            for (int q = 0; q < NSTAT - 1; ++q) sh[q][threadIdx.x] = mx(sh[q][threadIdx.x], sh[q][threadIdx.x + w]);
+            sh[4][threadIdx.x] = mn(sh[4][threadIdx.x], sh[4][threadIdx.x + w]);
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x < NSTAT) out[(int64_t)c * NSTAT + threadIdx.x] = sh[threadIdx.x][0];
+}
+
+// refine_x's update of column c by how[c]: 1 y += dy; 2 (y, y_tail) += dy as LAPACK dla_wwaddw; 0 nothing
+__global__ void update_x_kernel(double* __restrict__ Y, double* __restrict__ T, const double* __restrict__ DY,
+                                const int* __restrict__ how, int M, int ldn) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= (int64_t)M * ldn) return;
+    const int h = how[e % ldn];
+    if (h == 1) {
+        Y[e] = __dadd_rn(Y[e], DY[e]);
+    } else if (h == 2) {
+        const double x = Y[e], w = DY[e];
+        double s = __dadd_rn(x, w);
+        s = __dsub_rn(__dadd_rn(s, s), s);
+        double t = __dadd_rn(__dadd_rn(__dsub_rn(x, s), w), T[e]);
+        const double xn = __dadd_rn(s, t);
+        T[e] = __dadd_rn(__dsub_rn(s, xn), t);
+        Y[e] = xn;
+    }
+}
+
 int grow(double** p, size_t n, size_t* have) {
     if (*p && n <= *have) return CFLX_OK;
     cudaFree(*p);
@@ -406,6 +650,25 @@ int launch_residual(ResidMode mode, const double* A, const Layout& L, const doub
     t2.P = P + (int64_t)Ml * ldo;
     t2.Q = Q + (int64_t)Ml * ldo;
     return Nl > 0 ? dispatch_tn<MASK_STRICT_UPPER_T>(t2, s) : CFLX_OK;
+}
+
+int launch_residual_x(ResidMode mode, const double* A, const Layout& L, const double* Xc, const double* Xct,
+                      const double* Xr, const double* Xrt, int64_t ldx, int nrhs, double* Hi, double* Lo, int64_t ldo,
+                      cudaStream_t s) {
+    if (nrhs <= 0) return CFLX_OK;
+    const int64_t lda = L.Nl;
+    const int Ml = L.Ml, Nl = L.Nl, v = L.v;
+    const ResidXArgs nn{Ml, nrhs, Nl, A, lda, Xc, Xct, ldx, Hi, Lo, ldo, v, L.Nt, MASK_NONE, L.Px, L.pi, L.Py, L.pj};
+    const ResidXArgs tn{Nl, nrhs, Ml, A, lda, Xr, Xrt, ldx, Hi, Lo, ldo, v, L.Nt, MASK_NONE, L.Py, L.pj, L.Px, L.pi};
+    if (mode == ResidMode::NN) return dispatch_x(nn, false, s);
+    if (mode == ResidMode::TN) return dispatch_x(tn, true, s);
+    ResidXArgs n2 = nn, t2 = tn;
+    n2.mask = MASK_LOWER;
+    t2.mask = MASK_STRICT_UPPER_T;
+    t2.Hi = Hi + (int64_t)Ml * ldo;
+    t2.Lo = Lo + (int64_t)Ml * ldo;
+    CFLX_TRY(dispatch_x(n2, false, s));
+    return dispatch_x(t2, true, s);
 }
 
 // ---------------------------------------------------------------- LAPACK dlacn2 as a reverse-communication step
@@ -500,95 +763,232 @@ int Lacn2::step() {
     }
 }
 
-// ---------------------------------------------------------------- the refinement driver
+// ---------------------------------------------------------------- the refinement drivers
 void refine_cache_free(RefineCache* rc) {
-    for (double* p : {rc->X, rc->B, rc->R, rc->D, rc->rhs, rc->ratio, rc->W, rc->Xc, rc->Xr, rc->part, rc->all, rc->berr})
+    for (double* p : {rc->X, rc->B, rc->R, rc->D, rc->rhs, rc->ratio, rc->W, rc->Xc, rc->Xr, rc->part, rc->all, rc->berr,
+                      rc->T, rc->Xct, rc->Xrt, rc->stats})
         cudaFree(p);
     for (int* p : {rc->gl_rows, rc->gl_cols, rc->active}) cudaFree(p);
     *rc = RefineCache{};
 }
 
-int refine_run(RefineCache* rc, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx, double* ferr,
-               double* berr_out) {
-    const Grid& G = op.grid;
-    cflx_comm* c = G.comm;
-    cudaStream_t s = c->stream;
-    const int M = G.M, Ml = G.Ml, Nl = G.Nl, v = G.v;
-    const int ldn = (int)round_up(nrhs, 8);
-    const bool nn = op.mode != ResidMode::TN, tn = op.mode != ResidMode::NN, layer0 = G.pk == 0;
-    // local column (by_col) or row -> global row of X (clamped into X: masked entries never use the value)
-    auto make_map = [&](int** dst, int n, bool by_col) -> int {
-        if (*dst || n <= 0) return CFLX_OK;
-        std::vector<int> m(n);
-        for (int l = 0; l < n; ++l) {
-            const int g = by_col ? G.col(l) : G.row(l);
-            m[l] = g < M ? g : 0;
-        }
-        return solve_set_rows(dst, m, s);
-    };
-    if (layer0 && nn) CFLX_TRY(make_map(&rc->gl_cols, Nl, true));
-    if (layer0 && tn) CFLX_TRY(make_map(&rc->gl_rows, Ml, false));
-    const int prow = (nn ? Ml : 0) + (tn ? Nl : 0);
-    const size_t mat = (size_t)M * ldn, chunk = (size_t)prow * 2 * ldn;
-    if (rc->cap_m < mat) {  // the M x ldn buffers, grown together
-        const std::initializer_list<double**> bufs = {&rc->X, &rc->B, &rc->R, &rc->D, &rc->rhs, &rc->ratio, &rc->W};
-        for (double** p : bufs) {
-            cudaFree(*p);
-            *p = nullptr;
-        }
-        rc->cap_m = 0;
-        for (double** p : bufs) CFLX_TRY(dmalloc(p, mat));
-        rc->cap_m = mat;
-    }
-    CFLX_TRY(grow(&rc->Xc, (size_t)Nl * ldn, &rc->cap_c));
-    CFLX_TRY(grow(&rc->Xr, (size_t)Ml * ldn, &rc->cap_r));
-    CFLX_TRY(grow(&rc->part, chunk, &rc->cap_part));
-    if (c->world_size > 1) CFLX_TRY(grow(&rc->all, chunk * c->world_size, &rc->cap_all));
-    CFLX_TRY(grow(&rc->berr, (size_t)ldn, &rc->cap_berr));
-    if (!rc->active || rc->cap_active < (size_t)ldn) {
-        cudaFree(rc->active);
-        rc->active = nullptr;
-        CFLX_TRY(dmalloc(&rc->active, (size_t)ldn));
-        rc->cap_active = ldn;
-    }
-    CFLX_CUDA(cudaMemsetAsync(rc->X, 0, sizeof(double) * mat, s));
-    CFLX_CUDA(cudaMemsetAsync(rc->B, 0, sizeof(double) * mat, s));
-    CFLX_CUDA(cudaMemcpy2DAsync(rc->X, ldn * sizeof(double), X, (size_t)ldx * sizeof(double), nrhs * sizeof(double), M,
-                                cudaMemcpyDefault, s));
-    CFLX_CUDA(cudaMemcpy2DAsync(rc->B, ldn * sizeof(double), B, (size_t)ldb * sizeof(double), nrhs * sizeof(double), M,
-                                cudaMemcpyDefault, s));
+namespace {
+// What both drivers share: the gather maps and the buffers for nrhs columns, X and B uploaded, and one residual pass.
+struct RefinePass {
+    RefineCache* rc;
+    const RefineOp& op;
+    int nrhs, ldn;
+    bool nn, tn, layer0;
+    size_t mat, chunk;
+    AssembleArgs aa;
+    std::vector<double> berr;
 
-    const double eps = std::ldexp(1.0, -53), safmin = std::ldexp(1.0, -1022);
-    const double nz = (double)M + 1.0, safe1 = nz * safmin, safe2 = safe1 / eps;
-    const double* all = c->world_size > 1 ? rc->all : rc->part;
-    const AssembleArgs aa{all, (int64_t)chunk, Ml, Nl, ldn, nrhs, M, nn, tn, v, G.Px, G.Py, G.Pz, rc->B, rc->R,
+    RefinePass(RefineCache* rc_, const RefineOp& op_, int nrhs_) : rc(rc_), op(op_), nrhs(nrhs_), berr(nrhs_) {
+        const Grid& G = op.grid;
+        ldn = (int)round_up(nrhs, 8);
+        nn = op.mode != ResidMode::TN;
+        tn = op.mode != ResidMode::NN;
+        layer0 = G.pk == 0;
+        mat = (size_t)G.M * ldn;
+        chunk = (size_t)((nn ? G.Ml : 0) + (tn ? G.Nl : 0)) * 2 * ldn;
+    }
+
+    // extended: the tail of X and its gathered copies, the per-column statistics and the update selector
+    int setup(const double* B, int ldb, const double* X, int ldx, bool extended) {
+        const Grid& G = op.grid;
+        cflx_comm* c = G.comm;
+        cudaStream_t s = c->stream;
+        const int M = G.M, Ml = G.Ml, Nl = G.Nl;
+        // local column (by_col) or row -> global row of X (clamped into X: masked entries never use the value)
+        auto make_map = [&](int** dst, int n, bool by_col) -> int {
+            if (*dst || n <= 0) return CFLX_OK;
+            std::vector<int> m(n);
+            for (int l = 0; l < n; ++l) {
+                const int g = by_col ? G.col(l) : G.row(l);
+                m[l] = g < M ? g : 0;
+            }
+            return solve_set_rows(dst, m, s);
+        };
+        if (layer0 && nn) CFLX_TRY(make_map(&rc->gl_cols, Nl, true));
+        if (layer0 && tn) CFLX_TRY(make_map(&rc->gl_rows, Ml, false));
+        if (rc->cap_m < mat) {  // the M x ldn buffers, grown together
+            const std::initializer_list<double**> bufs = {&rc->X, &rc->B, &rc->R, &rc->D, &rc->rhs, &rc->ratio, &rc->W};
+            for (double** p : bufs) {
+                cudaFree(*p);
+                *p = nullptr;
+            }
+            rc->cap_m = 0;
+            for (double** p : bufs) CFLX_TRY(dmalloc(p, mat));
+            rc->cap_m = mat;
+        }
+        CFLX_TRY(grow(&rc->Xc, (size_t)Nl * ldn, &rc->cap_c));
+        CFLX_TRY(grow(&rc->Xr, (size_t)Ml * ldn, &rc->cap_r));
+        CFLX_TRY(grow(&rc->part, chunk, &rc->cap_part));
+        if (c->world_size > 1) CFLX_TRY(grow(&rc->all, chunk * c->world_size, &rc->cap_all));
+        CFLX_TRY(grow(&rc->berr, (size_t)ldn, &rc->cap_berr));
+        if (!rc->active || rc->cap_active < (size_t)ldn) {
+            cudaFree(rc->active);
+            rc->active = nullptr;
+            CFLX_TRY(dmalloc(&rc->active, (size_t)ldn));
+            rc->cap_active = ldn;
+        }
+        if (extended) {
+            CFLX_TRY(grow(&rc->T, mat, &rc->cap_t));
+            CFLX_TRY(grow(&rc->Xct, (size_t)Nl * ldn, &rc->cap_ct));
+            CFLX_TRY(grow(&rc->Xrt, (size_t)Ml * ldn, &rc->cap_rt));
+            CFLX_TRY(grow(&rc->stats, (size_t)ldn * NSTAT, &rc->cap_stats));
+            CFLX_CUDA(cudaMemsetAsync(rc->T, 0, sizeof(double) * mat, s));
+        }
+        CFLX_CUDA(cudaMemsetAsync(rc->X, 0, sizeof(double) * mat, s));
+        CFLX_CUDA(cudaMemsetAsync(rc->B, 0, sizeof(double) * mat, s));
+        CFLX_CUDA(cudaMemcpy2DAsync(rc->X, ldn * sizeof(double), X, (size_t)ldx * sizeof(double), nrhs * sizeof(double), M,
+                                    cudaMemcpyDefault, s));
+        CFLX_CUDA(cudaMemcpy2DAsync(rc->B, ldn * sizeof(double), B, (size_t)ldb * sizeof(double), nrhs * sizeof(double), M,
+                                    cudaMemcpyDefault, s));
+        const double eps = std::ldexp(1.0, -53), safmin = std::ldexp(1.0, -1022);
+        const double nz = (double)M + 1.0, safe1 = nz * safmin, safe2 = safe1 / eps;
+        const double* all = c->world_size > 1 ? rc->all : rc->part;
+        aa = AssembleArgs{all, (int64_t)chunk, Ml, Nl, ldn, nrhs, M, nn, tn, G.v, G.Px, G.Py, G.Pz, rc->B, rc->R,
                           rc->ratio, rc->W, safe1, safe2, nz * eps};
-    std::vector<double> berr(nrhs);
-    // one residual pass: R = B - op(A) X, the ratios, W, and berr on the host
-    auto pass = [&]() -> int {
+        return CFLX_OK;
+    }
+
+    // the partials of op(A) (X + T) of every layer-0 rank on every rank (T: the tail, extended passes only)
+    int partials(const double* X, const double* T) {
+        const Grid& G = op.grid;
+        cflx_comm* c = G.comm;
+        cudaStream_t s = c->stream;
         if (layer0) {
-            if (nn) CFLX_TRY(launch_gather_rows(rc->X, ldn, rc->gl_cols, Nl, ldn, rc->Xc, s));
-            if (tn) CFLX_TRY(launch_gather_rows(rc->X, ldn, rc->gl_rows, Ml, ldn, rc->Xr, s));
-            CFLX_TRY(launch_residual(op.mode, op.A, G, rc->Xc, rc->Xr, ldn, nrhs, rc->part, rc->part + ldn,
-                                     2 * (int64_t)ldn, s));
+            if (nn) CFLX_TRY(launch_gather_rows(X, ldn, rc->gl_cols, G.Nl, ldn, rc->Xc, s));
+            if (tn) CFLX_TRY(launch_gather_rows(X, ldn, rc->gl_rows, G.Ml, ldn, rc->Xr, s));
+            if (T) {
+                if (nn) CFLX_TRY(launch_gather_rows(T, ldn, rc->gl_cols, G.Nl, ldn, rc->Xct, s));
+                if (tn) CFLX_TRY(launch_gather_rows(T, ldn, rc->gl_rows, G.Ml, ldn, rc->Xrt, s));
+                CFLX_TRY(launch_residual_x(op.mode, op.A, G, rc->Xc, rc->Xct, rc->Xr, rc->Xrt, ldn, nrhs, rc->part,
+                                           rc->part + ldn, 2 * (int64_t)ldn, s));
+            } else {
+                CFLX_TRY(launch_residual(op.mode, op.A, G, rc->Xc, rc->Xr, ldn, nrhs, rc->part, rc->part + ldn,
+                                         2 * (int64_t)ldn, s));
+            }
         }
         if (c->world_size > 1) CFLX_NCCL(ncclAllGather(rc->part, rc->all, chunk, ncclDouble, c->world, s));
-        assemble_kernel<<<dim3((unsigned)M, (unsigned)((nrhs + 127) / 128)), 128, 0, s>>>(aa);
-        column_max_kernel<<<nrhs, MAXT, 0, s>>>(rc->ratio, M, ldn, rc->berr);
+        return CFLX_OK;
+    }
+
+    // one working-precision pass over X (M x ldn): R = B - op(A) X, the ratios (and W, or Q when lin_berr), and the
+    // per-column maximum ratio into berr on the host
+    int run(const double* X, bool lin_berr = false, double* Q = nullptr) {
+        cudaStream_t s = op.grid.comm->stream;
+        CFLX_TRY(partials(X, nullptr));
+        AssembleArgs a = aa;
+        a.lin_berr = lin_berr;
+        a.Q = Q;
+        assemble_kernel<<<dim3((unsigned)op.grid.M, (unsigned)((nrhs + 127) / 128)), 128, 0, s>>>(a);
+        column_max_kernel<<<nrhs, MAXT, 0, s>>>(rc->ratio, op.grid.M, ldn, rc->berr);
         CFLX_CUDA(cudaGetLastError());
         CFLX_CUDA(cudaMemcpyAsync(berr.data(), rc->berr, sizeof(double) * nrhs, cudaMemcpyDeviceToHost, s));
         CFLX_CUDA(cudaStreamSynchronize(s));
         return CFLX_OK;
+    }
+
+    // R = B - op(A) (X + T) in double-double, rounded once
+    int run_x() {
+        cudaStream_t s = op.grid.comm->stream;
+        CFLX_TRY(partials(rc->X, rc->T));
+        assemble_x_kernel<<<dim3((unsigned)op.grid.M, (unsigned)((nrhs + 127) / 128)), 128, 0, s>>>(aa);
+        CFLX_CUDA(cudaGetLastError());
+        return CFLX_OK;
+    }
+
+    // D = inv(op A) R on the columns where active (the others get 0)
+    int correction(const std::vector<int>& active) {
+        cudaStream_t s = op.grid.comm->stream;
+        CFLX_CUDA(cudaMemcpyAsync(rc->active, active.data(), sizeof(int) * ldn, cudaMemcpyHostToDevice, s));
+        select_cols_kernel<<<blocks(), 256, 0, s>>>(rc->R, rc->active, op.grid.M, ldn, rc->rhs);
+        CFLX_CUDA(cudaGetLastError());
+        return op.solve(false, nrhs, rc->rhs, ldn, rc->D, ldn);  // synchronises: `active` may change after it
+    }
+
+    unsigned blocks() const { return (unsigned)((mat + 255) / 256); }
+};
+
+// dlacn2 on every column j with want[j], all in lockstep: a round issues one solve per kind over the columns that ask for
+// it.  Column j estimates the 1-norm of diag(l_j) inv(op A)^T diag(r_j) (kase 1) / diag(r_j) inv(op A) diag(l_j) (kase
+// 2): l and r are host M x ld arrays (r may be null: ones; where r_div[j], r_j is applied by division, as LAPACK's
+// dla_gercond applies inv(C) with CMODE 1).  est[j] = the estimate (0 where not wanted).
+int lacn2_columns(const RefineOp& op, int ncols, int ld, const std::vector<double>& l, const std::vector<double>* r,
+                  const std::vector<char>* r_div, const std::vector<char>& want, std::vector<double>& est_out) {
+    const int M = op.grid.M;
+    std::vector<Lacn2> est(ncols);
+    for (int j = 0; j < ncols; ++j)
+        if (want[j]) est[j].start(M);
+    auto R = [&](size_t o, double x) { return !r ? x : (*r_div)[o % ld] ? x / (*r)[o] : x * (*r)[o]; };
+    std::vector<double> in((size_t)M * ld), out((size_t)M * ld);
+    auto solve_round = [&](bool transposed, bool want1, bool want2) -> int {
+        bool any = false;
+        std::fill(in.begin(), in.end(), 0.0);
+        for (int j = 0; j < ncols; ++j) {
+            const int k = est[j].kase;
+            if (!((k == 1 && want1) || (k == 2 && want2))) continue;
+            any = true;
+            for (int i = 0; i < M; ++i) {
+                const size_t o = (size_t)i * ld + j;
+                in[o] = k == 2 ? l[o] * est[j].x[i] : R(o, est[j].x[i]);
+            }
+        }
+        if (!any) return CFLX_OK;
+        CFLX_TRY(op.solve(transposed, ncols, in.data(), ld, out.data(), ld));
+        for (int j = 0; j < ncols; ++j) {
+            const int k = est[j].kase;
+            if (!((k == 1 && want1) || (k == 2 && want2))) continue;
+            for (int i = 0; i < M; ++i) {
+                const size_t o = (size_t)i * ld + j;
+                est[j].x[i] = k == 1 ? l[o] * out[o] : R(o, out[o]);
+            }
+            est[j].pending = true;
+        }
+        return CFLX_OK;
     };
+    for (;;) {
+        bool any = false;
+        for (int j = 0; j < ncols; ++j) any |= est[j].kase != 0;
+        if (!any) break;
+        if (op.symmetric) {
+            CFLX_TRY(solve_round(false, true, true));
+        } else {
+            CFLX_TRY(solve_round(true, true, false));
+            CFLX_TRY(solve_round(false, false, true));
+        }
+        for (int j = 0; j < ncols; ++j)
+            if (est[j].pending) {
+                est[j].pending = false;
+                est[j].step();
+            }
+    }
+    est_out.assign(ncols, 0.0);
+    for (int j = 0; j < ncols; ++j) est_out[j] = est[j].est;
+    return CFLX_OK;
+}
+}  // namespace
+
+int refine_run(RefineCache* rc, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx, double* ferr,
+               double* berr_out) {
+    cudaStream_t s = op.grid.comm->stream;
+    const int M = op.grid.M;
+    RefinePass pass(rc, op, nrhs);
+    CFLX_TRY(pass.setup(B, ldb, X, ldx, false));
+    const int ldn = pass.ldn;
+    const size_t mat = pass.mat;
+    const std::vector<double>& berr = pass.berr;
+    const double eps = std::ldexp(1.0, -53);
 
     // dgerfs, every column in lockstep: iterate while berr > eps, berr <= lstres / 2 and count <= ITMAX
     constexpr int ITMAX = 5;
     std::vector<int> count(nrhs, 1), active(ldn, 0);
     std::vector<double> lstres(nrhs, 3.0), col_berr(nrhs, 0.0);
     std::vector<char> refining(nrhs, 1);
-    const unsigned eblocks = (unsigned)((mat + 255) / 256);
     for (;;) {
-        CFLX_TRY(pass());
+        CFLX_TRY(pass.run(rc->X));
         bool any = false;
         for (int j = 0; j < nrhs; ++j) {
             active[j] = 0;
@@ -604,74 +1004,198 @@ int refine_run(RefineCache* rc, const RefineOp& op, int nrhs, const double* B, i
             }
         }
         if (!any) break;
-        CFLX_CUDA(cudaMemcpyAsync(rc->active, active.data(), sizeof(int) * ldn, cudaMemcpyHostToDevice, s));
-        select_cols_kernel<<<eblocks, 256, 0, s>>>(rc->R, rc->active, M, ldn, rc->rhs);
-        CFLX_CUDA(cudaGetLastError());
-        CFLX_TRY(op.solve(false, nrhs, rc->rhs, ldn, rc->D, ldn));  // synchronises: `active` may change after it
-        add_cols_kernel<<<eblocks, 256, 0, s>>>(rc->X, rc->D, rc->active, M, ldn);
+        CFLX_TRY(pass.correction(active));
+        add_cols_kernel<<<pass.blocks(), 256, 0, s>>>(rc->X, rc->D, rc->active, M, ldn);
         CFLX_CUDA(cudaGetLastError());
     }
-    std::vector<double> hX((size_t)M * ldn);
+    std::vector<double> hX(mat);
     CFLX_CUDA(cudaMemcpyAsync(hX.data(), rc->X, sizeof(double) * mat, cudaMemcpyDeviceToHost, s));
     CFLX_CUDA(cudaStreamSynchronize(s));
 
     if (ferr) {
         // ||inv(op A)| w|_inf by dlacn2 on diag(w) inv(op A)^T (kase 1) and inv(op A) diag(w) (kase 2), one estimator per
-        // column, all in lockstep: a round issues one solve per kind over the columns that ask for it
-        std::vector<double> w(mat);
+        // column
+        std::vector<double> w(mat), est;
         CFLX_CUDA(cudaMemcpyAsync(w.data(), rc->W, sizeof(double) * mat, cudaMemcpyDeviceToHost, s));
         CFLX_CUDA(cudaStreamSynchronize(s));
-        std::vector<Lacn2> est(nrhs);
-        for (int j = 0; j < nrhs; ++j) est[j].start(M);
-        std::vector<double> in(mat), out(mat);
-        auto solve_round = [&](bool transposed, bool want1, bool want2) -> int {
-            bool any = false;
-            std::fill(in.begin(), in.end(), 0.0);
-            for (int j = 0; j < nrhs; ++j) {
-                const int k = est[j].kase;
-                if (!((k == 1 && want1) || (k == 2 && want2))) continue;
-                any = true;
-                for (int i = 0; i < M; ++i) in[(size_t)i * ldn + j] = k == 2 ? w[(size_t)i * ldn + j] * est[j].x[i] : est[j].x[i];
-            }
-            if (!any) return CFLX_OK;
-            CFLX_TRY(op.solve(transposed, nrhs, in.data(), ldn, out.data(), ldn));
-            for (int j = 0; j < nrhs; ++j) {
-                const int k = est[j].kase;
-                if (!((k == 1 && want1) || (k == 2 && want2))) continue;
-                for (int i = 0; i < M; ++i) {
-                    const double y = out[(size_t)i * ldn + j];
-                    est[j].x[i] = k == 1 ? w[(size_t)i * ldn + j] * y : y;
-                }
-                est[j].pending = true;
-            }
-            return CFLX_OK;
-        };
-        for (;;) {
-            bool any = false;
-            for (int j = 0; j < nrhs; ++j) any |= est[j].kase != 0;
-            if (!any) break;
-            if (op.symmetric) {
-                CFLX_TRY(solve_round(false, true, true));
-            } else {
-                CFLX_TRY(solve_round(true, true, false));
-                CFLX_TRY(solve_round(false, false, true));
-            }
-            for (int j = 0; j < nrhs; ++j)
-                if (est[j].pending) {
-                    est[j].pending = false;
-                    est[j].step();
-                }
-        }
+        CFLX_TRY(lacn2_columns(op, nrhs, ldn, w, nullptr, nullptr, std::vector<char>(nrhs, 1), est));
         for (int j = 0; j < nrhs; ++j) {
             double xmax = 0.0;
             for (int i = 0; i < M; ++i) xmax = std::max(xmax, std::fabs(hX[(size_t)i * ldn + j]));
-            ferr[j] = xmax != 0.0 ? est[j].est / xmax : est[j].est;
+            ferr[j] = xmax != 0.0 ? est[j] / xmax : est[j];
         }
     }
     CFLX_CUDA(cudaMemcpy2DAsync(X, (size_t)ldx * sizeof(double), rc->X, ldn * sizeof(double), nrhs * sizeof(double), M,
                                 cudaMemcpyDefault, s));
     CFLX_CUDA(cudaStreamSynchronize(s));
     if (berr_out) std::copy(col_berr.begin(), col_berr.end(), berr_out);
+    return CFLX_OK;
+}
+
+// ---------------------------------------------------------------- extra-precise refinement (dgerfsx / dporfsx)
+int RefineXColumn::round(const double st[5], double rcond, bool ignore_cwise, int cnt, int M) {
+    const double eps = std::ldexp(1.0, -53), incr_thresh = (double)M * eps;
+    constexpr double RTHRESH = 0.5, DZ_UB = 0.25;
+    const double normy = st[0], normx = st[1], normdx = st[2], ymin = st[4];
+    dz_z = st[3];
+    dx_x = normx != 0.0 ? normdx / normx : normdx == 0.0 ? 0.0 : INFINITY;
+    const double dxrat = normdx / prev_normdx, dzrat = dz_z / prev_dz_z;
+    bool incr_prec = !ignore_cwise && ymin * rcond < incr_thresh * normy && y_prec < EXTRA_Y;
+
+    if (x_state == NOPROG && dxrat <= RTHRESH) x_state = WORKING;
+    if (x_state == WORKING) {
+        if (dx_x <= eps) {
+            x_state = CONV;
+        } else if (dxrat > RTHRESH) {
+            if (y_prec != EXTRA_Y) incr_prec = true;
+            else x_state = NOPROG;
+        } else if (dxrat > dxratmax) {
+            dxratmax = dxrat;
+        }
+        if (x_state > WORKING) final_dx_x = dx_x;
+    }
+    if (z_state == UNSTABLE && dz_z <= DZ_UB) z_state = WORKING;
+    if (z_state == NOPROG && dzrat <= RTHRESH) z_state = WORKING;
+    if (z_state == WORKING) {
+        if (dz_z <= eps) {
+            z_state = CONV;
+        } else if (dz_z > DZ_UB) {
+            z_state = UNSTABLE;
+            dzratmax = 0.0;
+            final_dz_z = INFINITY;
+        } else if (dzrat > RTHRESH) {
+            if (y_prec != EXTRA_Y) incr_prec = true;
+            else z_state = NOPROG;
+        } else if (dzrat > dzratmax) {
+            dzratmax = dzrat;
+        }
+        if (z_state > WORKING) final_dz_z = dz_z;
+    }
+    if (x_state != WORKING &&
+        (ignore_cwise || z_state == NOPROG || z_state == CONV || (z_state == UNSTABLE && cnt > 1))) {
+        done = true;
+        return 0;
+    }
+    if (incr_prec) y_prec = EXTRA_Y;  // the tail is zero until the first double-double update
+    prev_normdx = normdx;
+    prev_dz_z = dz_z;
+    return y_prec == EXTRA_Y ? 2 : 1;
+}
+
+void RefineXColumn::finish() {
+    if (x_state == WORKING) final_dx_x = dx_x;
+    if (z_state == WORKING) final_dz_z = dz_z;
+    err_norm = final_dx_x / (1.0 - dxratmax);
+    err_comp = final_dz_z / (1.0 - dzratmax);
+}
+
+int refine_x_run(RefineCache* rc, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx,
+                 const double* d, double rcond, bool cwise, double* berr_out, double* err_norm, double* err_comp,
+                 int* info) {
+    cudaStream_t s = op.grid.comm->stream;
+    const int M = op.grid.M;
+    RefinePass pass(rc, op, nrhs);
+    CFLX_TRY(pass.setup(B, ldb, X, ldx, true));
+    const int ldn = pass.ldn;
+    const size_t mat = pass.mat;
+    constexpr int ITHRESH = 10;
+
+    // dla_gerfsx_extended / dla_porfsx_extended, every column in lockstep from the extra-residual state
+    std::vector<RefineXColumn> col(nrhs);
+    std::vector<int> active(ldn, 0), how(ldn, 0);
+    std::vector<double> st((size_t)ldn * NSTAT);
+    for (int cnt = 1; cnt <= ITHRESH; ++cnt) {
+        bool any = false;
+        for (int j = 0; j < nrhs; ++j) any |= (active[j] = !col[j].done) != 0;
+        if (!any) break;
+        CFLX_TRY(pass.run_x());
+        CFLX_TRY(pass.correction(active));
+        column_stats_kernel<<<nrhs, MAXT, 0, s>>>(rc->X, rc->D, d, M, ldn, rc->stats);
+        CFLX_CUDA(cudaGetLastError());
+        CFLX_CUDA(cudaMemcpyAsync(st.data(), rc->stats, sizeof(double) * nrhs * NSTAT, cudaMemcpyDeviceToHost, s));
+        CFLX_CUDA(cudaStreamSynchronize(s));
+        for (int j = 0; j < nrhs; ++j) how[j] = active[j] ? col[j].round(&st[(size_t)j * NSTAT], rcond, !cwise, cnt, M) : 0;
+        CFLX_CUDA(cudaMemcpyAsync(rc->active, how.data(), sizeof(int) * ldn, cudaMemcpyHostToDevice, s));
+        update_x_kernel<<<pass.blocks(), 256, 0, s>>>(rc->X, rc->T, rc->D, rc->active, M, ldn);
+        CFLX_CUDA(cudaGetLastError());
+    }
+    for (RefineXColumn& c : col) c.finish();
+
+    // berr (dla_lin_berr) from one working-precision pass, which also gives |op(A)| |y| for the componentwise condition
+    CFLX_TRY(pass.run(rc->X, true, rc->W));
+    std::vector<double> hY(mat), ayq;
+    CFLX_CUDA(cudaMemcpyAsync(hY.data(), rc->X, sizeof(double) * mat, cudaMemcpyDeviceToHost, s));
+    if (cwise) {
+        ayq.resize(mat);
+        CFLX_CUDA(cudaMemcpyAsync(ayq.data(), rc->W, sizeof(double) * mat, cudaMemcpyDeviceToHost, s));
+    }
+    CFLX_CUDA(cudaStreamSynchronize(s));
+    if (berr_out) std::copy(pass.berr.begin(), pass.berr.end(), berr_out);
+
+    // The condition estimates, all in lockstep: column j < nrhs the componentwise one of y_j (dla_gercond CMODE 1:
+    // l = |op(A)| |y_j|, applied with inv(diag(y_j))), where its bound is below sqrt(eps); column nrhs the normwise one
+    // of op(A) inv(diag(d)) (CMODE -1: l = |op(A)| |1 / d|, applied with diag(d); CMODE 0 without d: l = |op(A)| 1).
+    const int ncols = nrhs + 1, ld = (int)round_up(ncols, 8);
+    std::vector<double> l((size_t)M * ld, 0.0), r((size_t)M * ld, 1.0);
+    std::vector<char> want(ncols, 0), r_div(ld, 1);
+    const double eps = std::ldexp(1.0, -53), cwise_wrong = std::sqrt(eps);
+    {
+        // |op(A)| |1 / d| by one more working-precision pass with 1 / d (or ones) in column 0
+        std::vector<double> hd(M, 1.0), one(mat, 0.0);
+        if (d) {
+            CFLX_CUDA(cudaMemcpyAsync(hd.data(), d, sizeof(double) * M, cudaMemcpyDeviceToHost, s));
+            CFLX_CUDA(cudaStreamSynchronize(s));
+        }
+        for (int i = 0; i < M; ++i) one[(size_t)i * ldn] = d ? 1.0 / hd[i] : 1.0;
+        CFLX_CUDA(cudaMemcpyAsync(rc->rhs, one.data(), sizeof(double) * mat, cudaMemcpyHostToDevice, s));
+        CFLX_TRY(pass.run(rc->rhs, true, rc->W));
+        std::vector<double> g(mat);
+        CFLX_CUDA(cudaMemcpyAsync(g.data(), rc->W, sizeof(double) * mat, cudaMemcpyDeviceToHost, s));
+        CFLX_CUDA(cudaStreamSynchronize(s));
+        for (int i = 0; i < M; ++i) {
+            l[(size_t)i * ld + nrhs] = g[(size_t)i * ldn];
+            r[(size_t)i * ld + nrhs] = hd[i];
+        }
+        want[nrhs] = 1;
+        r_div[nrhs] = 0;
+    }
+    if (cwise)
+        for (int j = 0; j < nrhs; ++j) {
+            want[j] = col[j].err_comp < cwise_wrong;
+            for (int i = 0; i < M; ++i) {
+                l[(size_t)i * ld + j] = ayq[(size_t)i * ldn + j];
+                r[(size_t)i * ld + j] = hY[(size_t)i * ldn + j];
+            }
+        }
+    std::vector<double> est;
+    CFLX_TRY(lacn2_columns(op, ncols, ld, l, &r, &r_div, want, est));
+    auto cond = [&](int j) { return est[j] != 0.0 ? 1.0 / est[j] : 0.0; };
+
+    const double illrcond_thresh = (double)M * eps, err_lbnd = std::max(10.0, std::sqrt((double)M)) * eps;
+    int first_ill = 0;
+    auto bound = [&](double err, double rc_, int j, double* out) {
+        double trust = 1.0;
+        err = std::min(err, 1.0);
+        if (rc_ < illrcond_thresh) {
+            err = 1.0;
+            trust = 0.0;
+            if (!first_ill) first_ill = j + 1;
+        } else if (err < err_lbnd) {
+            err = err_lbnd;
+        }
+        out[3 * j] = trust;
+        out[3 * j + 1] = err;
+        out[3 * j + 2] = rc_;
+    };
+    const double rcond_norm = cond(nrhs);
+    for (int j = 0; j < nrhs; ++j) {
+        bound(col[j].err_norm, rcond_norm, j, err_norm);
+        if (cwise) bound(col[j].err_comp, want[j] ? cond(j) : 0.0, j, err_comp);
+    }
+    *info = first_ill ? M + first_ill : 0;
+    CFLX_CUDA(cudaMemcpy2DAsync(X, (size_t)ldx * sizeof(double), rc->X, ldn * sizeof(double), nrhs * sizeof(double), M,
+                                cudaMemcpyDefault, s));
+    CFLX_CUDA(cudaStreamSynchronize(s));
     return CFLX_OK;
 }
 

@@ -109,6 +109,17 @@ inline void choleskyRefine(int nrhs, const double* B, int ldb, double* X, int ld
     if (!s.plan) throw CholeskyException("choleskyRefine() before initialize()");
     chol_detail::check(cflx_chol_refine(s.plan, nrhs, B, ldb, X, ldx, ferr, berr), "choleskyRefine");
 }
+// LAPACK dporfsx with the factor of the last parallelCholesky() (cflx_chol_refine_x, collective): arguments and result
+// as conflux::LU_refine_x without transposed.
+inline int choleskyRefineX(int nrhs, const double* B, int ldb, double* X, int ldx, double* err_norm,
+                           double* err_comp = nullptr, double* rcond = nullptr, double* berr = nullptr) {
+    auto& s = chol_detail::state();
+    if (!s.plan) throw CholeskyException("choleskyRefineX() before initialize()");
+    int info = 0;
+    chol_detail::check(cflx_chol_refine_x(s.plan, nrhs, B, ldb, X, ldx, rcond, berr, err_norm, err_comp, &info),
+                       "choleskyRefineX");
+    return info;
+}
 // LAPACK dpoequ (+ dlaqsy, lower, when apply) on the input the device holds (cflx_chol_equilibrate, collective); s
 // (matrix_size()) may be null.  Returns info (0, or the first non-positive diagonal entry); equed is 'N' or 'Y'.
 inline int choleskyEquilibrate(bool apply = true, double* s_out = nullptr, double* scond = nullptr, double* amax = nullptr,

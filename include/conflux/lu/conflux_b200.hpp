@@ -282,6 +282,18 @@ void LU_refine(lu_params<T>& gv, int nrhs, const T* B, int ldb, T* X, int ldx, d
     check(cflx_lu_refine(gv.plan, transposed ? 1 : 0, nrhs, B, ldb, X, ldx, ferr, berr), "LU_refine");
 }
 
+// LAPACK dgerfsx with the factors of the last LU_rep (cflx_lu_refine_x, collective): X refined in place with
+// double-double residuals; err_norm (nrhs x 3, {trust, err, rcond} per column) required, err_comp null skips the
+// componentwise bounds; rcond / berr may be null.  Returns info (0; k for an exactly zero U(k,k), X untouched; M + j).
+template <class T>
+int LU_refine_x(lu_params<T>& gv, int nrhs, const T* B, int ldb, T* X, int ldx, double* err_norm,
+                double* err_comp = nullptr, double* rcond = nullptr, double* berr = nullptr, bool transposed = false) {
+    int info = 0;
+    check(cflx_lu_refine_x(gv.plan, transposed ? 1 : 0, nrhs, B, ldb, X, ldx, rcond, berr, err_norm, err_comp, &info),
+          "LU_refine_x");
+    return info;
+}
+
 // LAPACK dgeequ (+ dlaqge when apply) on the input the device holds (cflx_lu_equilibrate, collective): the next LU_rep
 // with the input already on the device factors the scaled matrix, and LU_svx uses the scaling.  r / c (M each) may be
 // null.  Returns info (0, the first zero row, or M + the first zero column); equed is 'N', 'R', 'C' or 'B'.

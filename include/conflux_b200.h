@@ -122,6 +122,21 @@ int cflx_lu_rcond(cflx_lu*, double* rcond_out, double* anorm_out);
  * factors, the permutation, the input, later solves and the launch count as they are. */
 int cflx_lu_refine(cflx_lu*, int trans, int nrhs, const double* B, int ldb, double* X, int ldx, double* ferr_out,
                    double* berr_out);
+/* COLLECTIVE.  LAPACK dgerfsx on the GPU grid: refinement with the residual b - op(A)(y + y_tail) in double-double,
+ * converging to full working accuracy whenever cond * 2^-53 is safely below 1, with error bounds and a trust flag per
+ * right-hand side.  trans, B, X, ldb, ldx and the state rules as cflx_lu_refine; the matrix is the one the factors
+ * represent (the scaled A_s after cflx_lu_equilibrate).  rcond_out (may be NULL): dgecon of A_s in the infinity-norm
+ * (trans 0) or the 1-norm (trans 1).  berr_out (nrhs, may be NULL): max_i (|r_i| + (M + 1) safmin) / (|op(A_s)| |y| +
+ * |b|)_i.  err_bnds_norm_out / err_bnds_comp_out: nrhs x 3 row-major, row j = {trust, err, rcond} of column j (LAPACK's
+ * ERR_BNDS(j, 1..3)), bounding ||x - x_true||_inf / ||x||_inf and max_i |x_i - x_true,i| / |x_i| of the unscaled
+ * x = diag(d) y (d: c for trans 0 with equed C / B, r for trans 1 with equed R / B, else ones); err_bnds_comp_out NULL:
+ * componentwise convergence is neither pursued nor estimated.  info_out: k for the first exactly zero U(k,k) (X left as
+ * it was, rcond 0, nothing else written); M + j for the first column j whose bound was set to 1 because its condition
+ * estimate is below M 2^-53; 0 otherwise.  CFLX_ERR_ARG as cflx_lu_refine and for a NULL err_bnds_norm_out or info_out;
+ * CFLX_ERR_STATE as cflx_lu_rcond.  Results identical on every rank; leaves the factors, the permutation, the input,
+ * later solves and the launch count as they are. */
+int cflx_lu_refine_x(cflx_lu*, int trans, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out,
+                     double* berr_out, double* err_bnds_norm_out, double* err_bnds_comp_out, int* info_out);
 /* COLLECTIVE.  LAPACK dgeequ on the input the device holds (the padded M x M matrix of cflx_lu_set_local), and with
  * apply = 1 dlaqge: the input is scaled in place, a_ij = (c_j r_i) a_ij (only r or only c for equed 'R' / 'C'), when
  * rowcnd < 0.1, colcnd < 0.1 or amax is outside [dlamch('S') / dlamch('P'), its reciprocal].  r_out / c_out (M doubles,
@@ -231,6 +246,11 @@ int cflx_chol_rcond(cflx_chol*, double* rcond_out, double* anorm_out);
  * (its lower triangle); the arguments and results of cflx_lu_refine without trans.  CFLX_ERR_STATE as cflx_chol_solve. */
 int cflx_chol_refine(cflx_chol*, int nrhs, const double* B, int ldb, double* X, int ldx, double* ferr_out,
                      double* berr_out);
+/* COLLECTIVE.  LAPACK dporfsx (UPLO = 'L'): cflx_lu_refine_x without trans, with the symmetric residual from the stored
+ * lower triangle, rcond_out = dpocon, and d = s for equed Y.  info_out: M + j as cflx_lu_refine_x, else 0.
+ * CFLX_ERR_STATE as cflx_chol_solve. */
+int cflx_chol_refine_x(cflx_chol*, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out,
+                       double* berr_out, double* err_bnds_norm_out, double* err_bnds_comp_out, int* info_out);
 /* COLLECTIVE.  LAPACK dpoequ on the input the device holds, and with apply = 1 dlaqsy (UPLO = 'L'): s_i = 1 / sqrt(a_ii),
  * scond = sqrt(min a_ii) / sqrt(max a_ii), amax = max a_ii; the stored lower triangle of the real tiles is scaled in
  * place, a_ij = (s_j s_i) a_ij, when scond < 0.1 or amax is outside [dlamch('S') / dlamch('P'), its reciprocal].
@@ -285,6 +305,11 @@ int cflx_dbg_gemm_narrow_tn(int M, int N, int K, const double* AT, const double*
  * the mode does not read it).  P_out / Q_out: nrhs columns.  ms_out: mean device time of one launch over reps. */
 int cflx_dbg_residual(int mode, int Ml, int Nl, const double* A, int v, int Kappa, int Px, int Py, int pi, int pj,
                       int nrhs, const double* Xc, const double* Xr, double* P_out, double* Q_out, int reps, double* ms_out);
+/* the double-double residual kernels of cflx_*_refine_x, arguments as cflx_dbg_residual: hi_out + lo_out = op(A) (X +
+ * X_tail) in mode 0, 1 or 2, from Xc + Xct (NN) or Xr + Xrt (TN); either tail may be NULL (zero). */
+int cflx_dbg_residual_x(int mode, int Ml, int Nl, const double* A, int v, int Kappa, int Px, int Py, int pi, int pj,
+                        int nrhs, const double* Xc, const double* Xct, const double* Xr, const double* Xrt, double* hi_out,
+                        double* lo_out, int reps, double* ms_out);
 /* the per-share kernels of cflx_*_equilibrate and cflx_lu_svx on one layer-0 share A (Ml x Nl row-major, conflux layout of
  * tile v at grid position (pi, pj) of Px x Py; Ml, Nl multiples of v; M >= (Ml / v) Px v and >= (Nl / v) Py v global
  * indices).  r, c: M-vectors (r is also the Cholesky's s).  Each output may be NULL:
