@@ -15,7 +15,7 @@ import numpy as np
 
 from ._lib import ConfluxError, LIB_PATH, SYMBOLS, check, lib
 
-__all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "residual", "validate", "lu_solve", "lu_rcond", "lu_refine", "lu_refine_x", "lu_equilibrate", "lu_svx", "lu_inverse", "lu_det", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
+__all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "residual", "validate", "lu_solve", "lu_rcond", "lu_refine", "lu_refine_x", "lu_equilibrate", "lu_svx", "lu_equilibrate_b", "lu_svxx", "lu_inverse", "lu_det", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
 
 
 def auto_grid(M, N, P):
@@ -272,22 +272,57 @@ def lu_refine_x(gv, B, X, trans=False, cwise=True):
     return _refine_x(lib().cflx_lu_refine_x, gv.M, B, X, cwise, "lu_refine_x", gv._h, 1 if trans else 0)
 
 
-def lu_equilibrate(gv, apply=True, upload=True):
-    """LAPACK dgeequ (+ dlaqge when apply) on the padded input on the GPU grid.  upload=True first copies gv.data to the
-    device (cflx_lu_set_local), so that LU_rep(gv, upload=False) then factors the scaled matrix As, whose factors carry
-    the scaling to lu_svx.  Returns dict(r, c, rowcnd, colcnd, amax, equed, info) as dgeequ / dlaqge give them.
-    COLLECTIVE over gv.lu_comm; identical on every rank."""
+def _lu_equilibrate(gv, apply, upload, fn, what):
     if upload:
         a = np.ascontiguousarray(gv.data, dtype=np.float64)
         check(lib().cflx_lu_set_local(gv._h, a.ctypes.data), "lu_set_local")
     r, c = np.zeros(gv.M), np.zeros(gv.M)
     rowcnd, colcnd, amax, equed, info = (ctypes.c_double(), ctypes.c_double(), ctypes.c_double(), ctypes.c_char(),
                                          ctypes.c_int())
-    check(lib().cflx_lu_equilibrate(gv._h, 1 if apply else 0, r.ctypes.data, c.ctypes.data, ctypes.byref(rowcnd),
-                                    ctypes.byref(colcnd), ctypes.byref(amax), ctypes.byref(equed), ctypes.byref(info)),
-          "lu_equilibrate")
+    check(fn(gv._h, 1 if apply else 0, r.ctypes.data, c.ctypes.data, ctypes.byref(rowcnd), ctypes.byref(colcnd),
+             ctypes.byref(amax), ctypes.byref(equed), ctypes.byref(info)), what)
     return dict(r=r, c=c, rowcnd=rowcnd.value, colcnd=colcnd.value, amax=amax.value, equed=equed.value.decode(),
                 info=info.value)
+
+
+def lu_equilibrate(gv, apply=True, upload=True):
+    """LAPACK dgeequ (+ dlaqge when apply) on the padded input on the GPU grid.  upload=True first copies gv.data to the
+    device (cflx_lu_set_local), so that LU_rep(gv, upload=False) then factors the scaled matrix As, whose factors carry
+    the scaling to lu_svx.  Returns dict(r, c, rowcnd, colcnd, amax, equed, info) as dgeequ / dlaqge give them.
+    COLLECTIVE over gv.lu_comm; identical on every rank."""
+    return _lu_equilibrate(gv, apply, upload, lib().cflx_lu_equilibrate, "lu_equilibrate")
+
+
+def lu_equilibrate_b(gv, apply=True, upload=True):
+    """LAPACK dgeequb (+ dlaqge when apply): lu_equilibrate with the scales rounded to powers of two, so that scaling A
+    and B and unscaling X are exact.  Arguments and result as lu_equilibrate; the factors carry the scaling to lu_svxx
+    (or lu_svx).  COLLECTIVE over gv.lu_comm; identical on every rank."""
+    return _lu_equilibrate(gv, apply, upload, lib().cflx_lu_equilibrate_b, "lu_equilibrate_b")
+
+
+def _svxx(fn, n, B, cwise, what, *lead):
+    B, B2, nrhs = _rhs(n, B, what)
+    X = np.empty_like(B2)
+    be, en, ec = np.empty(nrhs), np.zeros((nrhs, 3)), np.zeros((nrhs, 3))
+    rcond, rpvgrw, equed, info = ctypes.c_double(), ctypes.c_double(), ctypes.c_char(), ctypes.c_int()
+    check(fn(*lead, nrhs, B2.ctypes.data, nrhs, X.ctypes.data, nrhs, ctypes.byref(rcond), ctypes.byref(rpvgrw),
+             be.ctypes.data, en.ctypes.data, ec.ctypes.data if cwise else None, ctypes.byref(equed), ctypes.byref(info)),
+          what)
+    k = info.value
+    solved = not (0 < k <= n)
+    return (X.reshape(B.shape) if solved else None), dict(rcond=rcond.value, rpvgrw=rpvgrw.value,
+                                                          berr=be if solved else None, err_norm=en if solved else None,
+                                                          err_comp=ec if solved and cwise else None,
+                                                          equed=equed.value.decode(), info=k)
+
+
+def lu_svxx(gv, B, trans=False, cwise=True):
+    """LAPACK dgesvxx with the factors of the last LU_rep and the scaling they carry (lu_equilibrate_b or
+    lu_equilibrate): solves A X = B (A^T X = B when trans) with extra-precise refinement.  Returns (X, dict(rcond,
+    rpvgrw, berr, err_norm, err_comp, equed, info)): rpvgrw is dla_gerpvgrw's per-column reciprocal pivot growth, the
+    rest as lu_refine_x returns it for the unscaled solution.  X (and berr, err_norm, err_comp) is None when U has an
+    exactly zero pivot (info = k).  COLLECTIVE over gv.lu_comm; identical on every rank."""
+    return _svxx(lib().cflx_lu_svxx, gv.M, B, cwise, "lu_svxx", gv._h, 1 if trans else 0)
 
 
 def lu_svx(gv, B, trans=False):
@@ -428,18 +463,32 @@ class cholesky:
         err_norm, err_comp, info)) as lu_refine_x does.  COLLECTIVE; identical on every rank."""
         return _refine_x(lib().cflx_chol_refine_x, self.N, B, X, cwise, "cholesky.refine_x", self._h)
 
-    def equilibrate(self, apply=True, upload=True):
-        """LAPACK dpoequ (+ dlaqsy, lower, when apply) on the padded input on the GPU grid.  upload=True first copies
-        self.data to the device, so that parallelCholesky(upload=False) then factors the scaled matrix.  Returns dict(s,
-        scond, amax, equed, info).  COLLECTIVE; identical on every rank."""
+    def _equilibrate(self, apply, upload, fn, what):
         if upload:
             a = np.ascontiguousarray(self.data, dtype=np.float64)
             check(lib().cflx_chol_set_local(self._h, a.ctypes.data), "chol_set_local")
         s = np.zeros(self.N)
         scond, amax, equed, info = ctypes.c_double(), ctypes.c_double(), ctypes.c_char(), ctypes.c_int()
-        check(lib().cflx_chol_equilibrate(self._h, 1 if apply else 0, s.ctypes.data, ctypes.byref(scond), ctypes.byref(amax),
-                                          ctypes.byref(equed), ctypes.byref(info)), "chol_equilibrate")
+        check(fn(self._h, 1 if apply else 0, s.ctypes.data, ctypes.byref(scond), ctypes.byref(amax), ctypes.byref(equed),
+                 ctypes.byref(info)), what)
         return dict(s=s, scond=scond.value, amax=amax.value, equed=equed.value.decode(), info=info.value)
+
+    def equilibrate(self, apply=True, upload=True):
+        """LAPACK dpoequ (+ dlaqsy, lower, when apply) on the padded input on the GPU grid.  upload=True first copies
+        self.data to the device, so that parallelCholesky(upload=False) then factors the scaled matrix.  Returns dict(s,
+        scond, amax, equed, info).  COLLECTIVE; identical on every rank."""
+        return self._equilibrate(apply, upload, lib().cflx_chol_equilibrate, "chol_equilibrate")
+
+    def equilibrate_b(self, apply=True, upload=True):
+        """LAPACK dpoequb (+ dlaqsy, lower, when apply): equilibrate with the scales rounded to powers of two.
+        Arguments and result as equilibrate.  COLLECTIVE; identical on every rank."""
+        return self._equilibrate(apply, upload, lib().cflx_chol_equilibrate_b, "chol_equilibrate_b")
+
+    def svxx(self, B, cwise=True):
+        """LAPACK dposvxx with the factor of the last parallelCholesky and the scaling it carries (equilibrate_b or
+        equilibrate): returns (X, dict(rcond, rpvgrw, berr, err_norm, err_comp, equed, info)) as lu_svxx does, rpvgrw
+        being dla_porpvgrw's.  COLLECTIVE; identical on every rank."""
+        return _svxx(lib().cflx_chol_svxx, self.N, B, cwise, "cholesky.svxx", self._h)
 
     def svx(self, B):
         """LAPACK dposvx with the factor of the last parallelCholesky and the scaling it carries (equilibrate): returns
@@ -647,6 +696,24 @@ class dbg:
                                    out["sym_scaled"].ctypes.data, out["growth"].ctypes.data, ctypes.byref(zp)), "dbg_equil")
         out["zero_pivot"] = zp.value
         return out
+
+    @staticmethod
+    def growth_cols(mode, F, A, v, Kappa=None, grid=(1, 1), pos=(0, 0), M=None, ncols=None):
+        """The per-column pivot growth pass of lu_svxx (mode "lu") and cholesky.svxx (mode "chol") on one layer-0 share
+        F (the factor) and A (the input), both Ml x Nl in dbg.equil's layout.  Returns (amax, fmax), M-vectors by global
+        column j < ncols (default M), zeros elsewhere: "lu" max |a_ij| over every row and max |f_ij| over the rows
+        i <= j; "chol" both over the real tiles' (global tile index < Kappa) rows j <= i < ncols."""
+        F = np.ascontiguousarray(F, dtype=np.float64)
+        A = np.ascontiguousarray(A, dtype=np.float64)
+        Ml, Nl = A.shape
+        Px, Py = (int(x) for x in grid)
+        M = int(M) if M is not None else (Ml // v) * Px * v
+        amax, fmax = np.empty(M), np.empty(M)
+        check(lib().cflx_dbg_growth_cols({"lu": 0, "chol": 1}[mode], Ml, Nl, int(v),
+                                         int(Kappa if Kappa is not None else 1 << 30), Px, Py, int(pos[0]), int(pos[1]),
+                                         M, int(ncols if ncols is not None else M), F.ctypes.data, A.ctypes.data,
+                                         amax.ctypes.data, fmax.ctypes.data), "dbg_growth_cols")
+        return amax, fmax
 
     @staticmethod
     def inverse_share(mode, v, grid, pos, M, c0, nc, Ml, Nl, Kappa=None, rows=None, X=None, perm=None, share=None,

@@ -626,6 +626,23 @@ RefineOp chol_refine_op(cflx_chol* ch) {
     auto solve = [ch](bool, int n, const double* b, int lb, double* x, int lx) { return cflx_chol_solve(ch, n, b, lb, x, lx); };
     return RefineOp{*ch, ch->A0, ResidMode::SymLower, true, solve};
 }
+
+// cflx_chol_equilibrate (dpoequ) and, with pow2, cflx_chol_equilibrate_b (dpoequb)
+int chol_equilibrate(cflx_chol* ch, int apply, bool pow2, double* s_out, double* scond_out, double* amax_out,
+                     char* equed_out, int* info_out) {
+    if (!ch || (apply != 0 && apply != 1) || !info_out) return CFLX_ERR_ARG;
+    CFLX_TRY(handle_equil_begin(ch, apply != 0));
+    double scond = 0.0, amax = 0.0;
+    char equed = 'N';
+    int info = 0;
+    CFLX_TRY(poequ_grid(*ch, &ch->eq, ch->A0, apply != 0, pow2, s_out, &scond, &amax, &equed, &info));
+    CFLX_TRY(handle_equil_end(ch, apply != 0, info, equed, scond, scond, nullptr));
+    if (scond_out) *scond_out = scond;
+    if (amax_out) *amax_out = amax;
+    if (equed_out) *equed_out = equed;
+    *info_out = info;
+    return CFLX_OK;
+}
 }  // namespace
 
 // ======================================================================================================== C ABI
@@ -1014,18 +1031,13 @@ int cflx_chol_refine_x(cflx_chol* ch, int nrhs, const double* B, int ldb, double
 // the solve cache, as cflx_chol_set_local does.
 int cflx_chol_equilibrate(cflx_chol* ch, int apply, double* s_out, double* scond_out, double* amax_out, char* equed_out,
                           int* info_out) {
-    if (!ch || (apply != 0 && apply != 1) || !info_out) return CFLX_ERR_ARG;
-    CFLX_TRY(handle_equil_begin(ch, apply != 0));
-    double scond = 0.0, amax = 0.0;
-    char equed = 'N';
-    int info = 0;
-    CFLX_TRY(poequ_grid(*ch, &ch->eq, ch->A0, apply != 0, s_out, &scond, &amax, &equed, &info));
-    CFLX_TRY(handle_equil_end(ch, apply != 0, info, equed, scond, scond, nullptr));
-    if (scond_out) *scond_out = scond;
-    if (amax_out) *amax_out = amax;
-    if (equed_out) *equed_out = equed;
-    *info_out = info;
-    return CFLX_OK;
+    return chol_equilibrate(ch, apply, false, s_out, scond_out, amax_out, equed_out, info_out);
+}
+
+// COLLECTIVE.  LAPACK dpoequb (+ dlaqsy when apply): cflx_chol_equilibrate with the scales rounded to powers of two.
+int cflx_chol_equilibrate_b(cflx_chol* ch, int apply, double* s_out, double* scond_out, double* amax_out,
+                            char* equed_out, int* info_out) {
+    return chol_equilibrate(ch, apply, true, s_out, scond_out, amax_out, equed_out, info_out);
 }
 
 // COLLECTIVE.  LAPACK dposvx after a successful factorisation, with the scaling the factor carries: B scaled by s,
@@ -1041,8 +1053,31 @@ int cflx_chol_svx(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X, 
     double rcond = 0.0;
     CFLX_TRY(cflx_chol_rcond(ch, &rcond, nullptr));
     *rcond_out = rcond;
-    return svx_tail(&ch->eq, &ch->sv.rf, chol_refine_op(ch), nrhs, B, ldb, X, ldx, ferr_out, berr_out, s, s, eq.rowcnd,
-                    rcond, info_out);
+    return svx_run(&ch->eq, &ch->sv.rf, chol_refine_op(ch), nrhs, B, ldb, X, ldx, ferr_out, berr_out, s, s, eq.rowcnd,
+                   rcond, info_out);
+}
+
+// COLLECTIVE.  LAPACK dposvxx after a successful factorisation, with the scaling the factor carries: dla_porpvgrw of the
+// stored lower triangles of the input and of L, dpocon, B scaled by s, the solve, dporfsx's refinement as
+// cflx_chol_refine_x runs it, X unscaled by s.
+int cflx_chol_svxx(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out,
+                   double* rpvgrw_out, double* berr_out, double* err_bnds_norm_out, double* err_bnds_comp_out,
+                   char* equed_out, int* info_out) {
+    if (!ch || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B || !X || !rcond_out || !err_bnds_norm_out || !info_out)
+        return CFLX_ERR_ARG;
+    CFLX_TRY(handle_check(ch, "extra-precise expert solve"));
+    CFLX_CUDA(cudaSetDevice(ch->comm->device));
+    const EquilRecord& eq = ch->eq.fac;
+    const double* s = eq.equed == 'Y' ? eq.r : nullptr;
+    if (equed_out) *equed_out = eq.equed;
+    std::vector<double> h;
+    CFLX_TRY(growth_cols_grid(*ch, &ch->eq, true, ch->A11, ch->A0, ch->M, h));
+    if (rpvgrw_out) *rpvgrw_out = rpvgrw_cols(h, ch->M, ch->M);
+    double rcond = 0.0;
+    CFLX_TRY(cflx_chol_rcond(ch, &rcond, nullptr));
+    *rcond_out = rcond;
+    return svxx_run(&ch->eq, &ch->sv.rf, chol_refine_op(ch), nrhs, B, ldb, X, ldx, s, s, s, rcond,
+                    err_bnds_comp_out != nullptr, berr_out, err_bnds_norm_out, err_bnds_comp_out, info_out);
 }
 
 int cflx_chol_launch_count(cflx_chol* ch, int64_t* count_out, int reset) { return handle_launch_count(ch, count_out, reset); }

@@ -282,7 +282,7 @@ int cflx_dbg_equil(int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int
     CFLX_TRY(dr.alloc(sizeof(double) * M));
     CFLX_TRY(dc.alloc(sizeof(double) * M));
     CFLX_TRY(dv.alloc(sizeof(double) * M));
-    CFLX_TRY(dg.alloc(sizeof(double) * 2));
+    CFLX_TRY(dg.alloc(sizeof(double) * 2 * M));
     CFLX_TRY(dz.alloc(sizeof(int)));
     CFLX_CUDA(cudaMemcpy(dA.p, A, sizeof(double) * a_n, cudaMemcpyHostToDevice));
     CFLX_CUDA(cudaMemcpy(dr.p, r, sizeof(double) * M, cudaMemcpyHostToDevice));
@@ -316,9 +316,12 @@ int cflx_dbg_equil(int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int
         CFLX_TRY(equil_sym_apply(w, L, dr.as<double>(), 0));
         CFLX_CUDA(cudaMemcpy(sym_scaled_out, w, sizeof(double) * a_n, cudaMemcpyDeviceToHost));
     }
-    if (growth_out) {  // the share is both L\U and the input
-        CFLX_TRY(equil_growth(a, a, L, ncols, dg.as<double>(), 0));
-        CFLX_CUDA(cudaMemcpy(growth_out, dg.p, sizeof(double) * 2, cudaMemcpyDeviceToHost));
+    if (growth_out) {  // the share is both L\U and the input; dgesvx's maxima are those of the columns' maxima
+        CFLX_TRY(equil_growth_cols(a, a, L, false, ncols, dg.as<double>(), 0));
+        std::vector<double> h(2 * (size_t)M);
+        CFLX_CUDA(cudaMemcpy(h.data(), dg.p, sizeof(double) * 2 * M, cudaMemcpyDeviceToHost));
+        growth_out[0] = *std::max_element(h.begin() + M, h.end());
+        growth_out[1] = *std::max_element(h.begin(), h.begin() + M);
     }
     if (zero_pivot_out) {
         CFLX_TRY(equil_zero_pivot(a, L, dz.as<int>(), 0));
@@ -326,6 +329,29 @@ int cflx_dbg_equil(int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int
         CFLX_CUDA(cudaMemcpy(&z, dz.p, sizeof(int), cudaMemcpyDeviceToHost));
         *zero_pivot_out = z == INT_MAX ? 0 : z;
     }
+    CFLX_CUDA(cudaDeviceSynchronize());
+    return CFLX_OK;
+}
+
+// the per-column pivot growth pass (equil.cu) on one layer-0 share F (the factor) and A (the input) at grid position
+// (pi, pj) of Px x Py; mode 0 LU, 1 Cholesky; either output may be null
+int cflx_dbg_growth_cols(int mode, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, int M, int ncols,
+                         const double* F, const double* A, double* amax_out, double* fmax_out) {
+    CFLX_TRY(check_device());
+    if ((mode != 0 && mode != 1) || Ml < 0 || Nl < 0 || v < 1 || Ml % v || Nl % v || Px < 1 || Py < 1 || pi < 0 ||
+        pi >= Px || pj < 0 || pj >= Py || !F || !A || M < (Ml / v) * Px * v || M < (Nl / v) * Py * v)
+        return CFLX_ERR_ARG;
+    const size_t a_n = (size_t)Ml * Nl;
+    DevBuf dF, dA, dg;
+    CFLX_TRY(dF.alloc(sizeof(double) * a_n));
+    CFLX_TRY(dA.alloc(sizeof(double) * a_n));
+    CFLX_TRY(dg.alloc(sizeof(double) * 2 * M));
+    CFLX_CUDA(cudaMemcpy(dF.p, F, sizeof(double) * a_n, cudaMemcpyHostToDevice));
+    CFLX_CUDA(cudaMemcpy(dA.p, A, sizeof(double) * a_n, cudaMemcpyHostToDevice));
+    const Layout L{M, v, Kappa, Ml, Nl, Px, Py, pi, pj};
+    CFLX_TRY(equil_growth_cols(dF.as<double>(), dA.as<double>(), L, mode == 1, ncols, dg.as<double>(), 0));
+    if (amax_out) CFLX_CUDA(cudaMemcpy(amax_out, dg.p, sizeof(double) * M, cudaMemcpyDeviceToHost));
+    if (fmax_out) CFLX_CUDA(cudaMemcpy(fmax_out, dg.as<double>() + M, sizeof(double) * M, cudaMemcpyDeviceToHost));
     CFLX_CUDA(cudaDeviceSynchronize());
     return CFLX_OK;
 }

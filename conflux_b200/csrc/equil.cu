@@ -1,6 +1,7 @@
-// conflux_b200/csrc/equil.cu -- equilibration and the expert drivers' device passes (cflx_lu_equilibrate, cflx_lu_svx,
-// cflx_chol_equilibrate, cflx_chol_svx): LAPACK's dgeequ + dlaqge, dpoequ + dlaqsy and dgesvx's reciprocal pivot growth
-// on the GPU grid.
+// conflux_b200/csrc/equil.cu -- equilibration and the expert drivers' device passes (cflx_lu_equilibrate[_b],
+// cflx_lu_svx[x], cflx_chol_equilibrate[_b], cflx_chol_svx[x]): LAPACK's dgeequ / dgeequb + dlaqge, dpoequ / dpoequb +
+// dlaqsy, and the reciprocal pivot growth of dgesvx and of dgesvxx / dposvxx (dla_gerpvgrw / dla_porpvgrw) on the GPU
+// grid.
 //
 // Every pass reads layer 0's local share A (Ml x Nl, conflux layout: local (r, c) is global (L.row(r), L.col(c))) once;
 // it is HBM-bound.  What the ranks combine are maxima (and, for the Cholesky diagonal,
@@ -99,36 +100,34 @@ __global__ void zero_pivot_kernel(const double* __restrict__ F, Layout L, int* o
     if (F[(int64_t)(L.diag_row(t) + e) * L.Nl + L.diag_col(t) + e] == 0.0) atomicMin(out, g + 1);
 }
 
-// out[0] = max |triu(F)|, out[1] = max |A| over the global columns < ncols of this share
-__global__ void __launch_bounds__(EQ_COLS) growth_kernel(const double* __restrict__ F, const double* __restrict__ A,
-                                                         Layout L, int ncols, double* out) {
-    __shared__ double sh[2][EQ_COLS];
+// amax[g] = max |a_ig|, fmx[g] = max |f_ig| over this CTA's rows of global column g < ncols, combined over the CTAs by
+// atomicMax on the bits.  LU (SYM false): every row of A, the rows i <= g of F (U).  Cholesky (SYM): the real tiles'
+// entries with g <= i < ncols of both.  Nothing outside the mask is read.
+template <bool SYM>
+__global__ void __launch_bounds__(EQ_COLS) growth_cols_kernel(const double* __restrict__ F, const double* __restrict__ A,
+                                                              Layout L, int ncols, double* __restrict__ amax,
+                                                              double* __restrict__ fmx) {
     const int c = blockIdx.x * EQ_COLS + threadIdx.x, r0 = blockIdx.y * EQ_ROWS, r1 = min(r0 + EQ_ROWS, L.Ml);
-    double mu = 0.0, ma = 0.0;
-    if (c < L.Nl) {
-        const int gc = L.col(c);
-        if (gc < ncols) {
-            for (int r = r0; r < r1; ++r) {
-                const int64_t o = (int64_t)r * L.Nl + c;
+    if (c >= L.Nl) return;
+    const int gc = L.col(c);
+    if (gc >= ncols || (SYM && gc / L.v >= L.Nt)) return;
+    double ma = 0.0, mf = 0.0;
+#pragma unroll 4
+    for (int r = r0; r < r1; ++r) {
+        const int gr = L.row(r);
+        const int64_t o = (int64_t)r * L.Nl + c;
+        if (SYM) {
+            if (gr >= gc && gr < ncols && gr / L.v < L.Nt) {
                 ma = fmax(ma, fabs(A[o]));
-                if (L.row(r) <= gc) mu = fmax(mu, fabs(F[o]));
+                mf = fmax(mf, fabs(F[o]));
             }
+        } else {
+            ma = fmax(ma, fabs(A[o]));
+            if (gr <= gc) mf = fmax(mf, fabs(F[o]));
         }
     }
-    sh[0][threadIdx.x] = mu;
-    sh[1][threadIdx.x] = ma;
-    __syncthreads();
-    for (int w = EQ_COLS / 2; w > 0; w >>= 1) {
-        if (threadIdx.x < w) {
-            sh[0][threadIdx.x] = fmax(sh[0][threadIdx.x], sh[0][threadIdx.x + w]);
-            sh[1][threadIdx.x] = fmax(sh[1][threadIdx.x], sh[1][threadIdx.x + w]);
-        }
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) {
-        max_bits(out, sh[0][0]);
-        max_bits(out + 1, sh[1][0]);
-    }
+    max_bits(amax + gc, ma);
+    max_bits(fmx + gc, mf);
 }
 
 __global__ void scale_rows_kernel(double* __restrict__ X, int64_t ld, int M, int n, const double* __restrict__ d) {
@@ -141,6 +140,13 @@ __global__ void scale_rows_kernel(double* __restrict__ X, int64_t ld, int M, int
 // dlamch('S') and dlamch('S') / dlamch('P') (LAPACK's SMLNUM of dgeequ and SMALL of dlaqge / dlaqsy)
 const double SAFMIN = std::ldexp(1.0, -1022), LAQ_SMALL = std::ldexp(1.0, -1022) / std::ldexp(1.0, -52);
 constexpr double THRESH = 0.1;
+
+// RADIX**n of dgeequb / dpoequb for RADIX = 2, as an integer power evaluates it: 2^n, or 1 / 2^-n for n < 0 (0 once 2^-n
+// overflows)
+double pow2i(int n) { return n >= 0 ? std::ldexp(1.0, n) : 1.0 / std::ldexp(1.0, -n); }
+// dgeequb's rounding of a positive maximum x to RADIX**INT(LOG(x) / LOGRDX).  The exponent comes from the host's log,
+// the libm LAPACK calls: at an exact power of two it depends on how log rounds.
+double round_pow2(double x) { return x > 0.0 ? pow2i((int)(std::log(x) / std::log(2.0))) : x; }
 
 // *a and *b (when b is not null) hold at least n doubles each; *cap is their common capacity
 int grow_pair(double** a, double** b, size_t* cap, size_t n) {
@@ -265,9 +271,9 @@ int equil_grow(EquilState* e, int M, int ldn) {
     return grow_pair(&e->B, &e->X, &e->cap, (size_t)M * ldn);
 }
 
-// ---------------------------------------------------------------- dgeequ + dlaqge
-int geequ_grid(const Grid& g, EquilState* e, double* A, bool apply, double* r_out, double* c_out, double* rowcnd,
-               double* colcnd, double* amax, char* equed, int* info) {
+// ---------------------------------------------------------------- dgeequ / dgeequb + dlaqge
+int geequ_grid(const Grid& g, EquilState* e, double* A, bool apply, bool pow2, double* r_out, double* c_out,
+               double* rowcnd, double* colcnd, double* amax, char* equed, int* info) {
     cflx_comm* c = g.comm;
     cudaStream_t s = c->stream;
     const int M = g.M;
@@ -288,10 +294,18 @@ int geequ_grid(const Grid& g, EquilState* e, double* A, bool apply, double* r_ou
             if (h[i] == 0.0) return i + 1;
         return 0;
     };
+    // dgeequb: the maxima rounded to powers of two on the host (h and its device copy d), before anything reads them
+    auto rounded = [&](double* d) -> int {
+        if (!pow2) return CFLX_OK;
+        for (double& x : h) x = round_pow2(x);
+        CFLX_CUDA(cudaMemcpyAsync(d, h.data(), sizeof(double) * M, cudaMemcpyHostToDevice, s));
+        return CFLX_OK;
+    };
     // row maxima, then r = reciprocals
     if (layer0) CFLX_TRY(equil_row_max(A, g, r, s));
     else CFLX_CUDA(cudaMemsetAsync(r, 0, sizeof(double) * M, s));
     CFLX_TRY(reduce_vec(c, r, M, ncclMax, h));
+    CFLX_TRY(rounded(r));
     double rcmin, rcmax;
     minmax(&rcmin, &rcmax);
     *amax = rcmax;
@@ -310,6 +324,7 @@ int geequ_grid(const Grid& g, EquilState* e, double* A, bool apply, double* r_ou
     if (layer0) CFLX_TRY(equil_col_max(A, g, r, cs, s));
     else CFLX_CUDA(cudaMemsetAsync(cs, 0, sizeof(double) * M, s));
     CFLX_TRY(reduce_vec(c, cs, M, ncclMax, h));
+    CFLX_TRY(rounded(cs));
     minmax(&rcmin, &rcmax);
     if (rcmin == 0.0) {
         *info = M + first_zero();
@@ -331,9 +346,9 @@ int geequ_grid(const Grid& g, EquilState* e, double* A, bool apply, double* r_ou
     return CFLX_OK;
 }
 
-// ---------------------------------------------------------------- dpoequ + dlaqsy
-int poequ_grid(const Grid& g, EquilState* e, double* A, bool apply, double* s_out, double* scond, double* amax,
-               char* equed, int* info) {
+// ---------------------------------------------------------------- dpoequ / dpoequb + dlaqsy
+int poequ_grid(const Grid& g, EquilState* e, double* A, bool apply, bool pow2, double* s_out, double* scond,
+               double* amax, char* equed, int* info) {
     cflx_comm* c = g.comm;
     cudaStream_t s = c->stream;
     const int N = g.M;
@@ -356,7 +371,8 @@ int poequ_grid(const Grid& g, EquilState* e, double* A, bool apply, double* s_ou
         if (s_out) std::copy(h.begin(), h.end(), s_out);
         return CFLX_OK;
     }
-    for (double& x : h) x = 1.0 / std::sqrt(x);
+    const double tmp = -0.5 / std::log(2.0);  // dpoequb: RADIX**INT(TMP * LOG(a_ii)), the log on the host as in geequ_grid
+    for (double& x : h) x = pow2 ? pow2i((int)(tmp * std::log(x))) : 1.0 / std::sqrt(x);
     if (s_out) std::copy(h.begin(), h.end(), s_out);
     CFLX_CUDA(cudaMemcpyAsync(sc, h.data(), sizeof(double) * N, cudaMemcpyHostToDevice, s));
     *scond = std::sqrt(smin) / std::sqrt(smax);
@@ -379,11 +395,13 @@ int equil_zero_pivot(const double* F, const Layout& L, int* zero_pivot, cudaStre
     return CFLX_OK;
 }
 
-int equil_growth(const double* F, const double* A, const Layout& L, int ncols, double* out2, cudaStream_t s) {
-    CFLX_CUDA(cudaMemsetAsync(out2, 0, 2 * sizeof(double), s));
+int equil_growth_cols(const double* F, const double* A, const Layout& L, bool sym, int ncols, double* out,
+                      cudaStream_t s) {
+    CFLX_CUDA(cudaMemsetAsync(out, 0, 2 * sizeof(double) * L.M, s));
     if (L.Ml > 0 && L.Nl > 0) {
         const dim3 grid((L.Nl + EQ_COLS - 1) / EQ_COLS, (L.Ml + EQ_ROWS - 1) / EQ_ROWS);
-        growth_kernel<<<grid, EQ_COLS, 0, s>>>(F, A, L, ncols, out2);
+        if (sym) growth_cols_kernel<true><<<grid, EQ_COLS, 0, s>>>(F, A, L, ncols, out, out + L.M);
+        else growth_cols_kernel<false><<<grid, EQ_COLS, 0, s>>>(F, A, L, ncols, out, out + L.M);
     }
     CFLX_CUDA(cudaGetLastError());
     return CFLX_OK;
@@ -408,26 +426,47 @@ int zero_pivot_grid(const Grid& g, EquilState* e, const double* F, int* info) {
     return CFLX_OK;
 }
 
-int pivot_growth_grid(const Grid& g, EquilState* e, const double* F, const double* A, double* rpvgrw, int* info) {
+int growth_cols_grid(const Grid& g, EquilState* e, bool sym, const double* F, const double* A, int ncols,
+                     std::vector<double>& h) {
     cflx_comm* c = g.comm;
-    cudaStream_t s = c->stream;
-    if (!e->growth) CFLX_TRY(dmalloc(&e->growth, 2));
+    const int M = g.M;
+    CFLX_TRY(grow_pair(&e->growth, nullptr, &e->growth_cap, 2 * (size_t)M));
+    if (g.pk == 0) CFLX_TRY(equil_growth_cols(F, A, g, sym, ncols, e->growth, c->stream));
+    else CFLX_CUDA(cudaMemsetAsync(e->growth, 0, 2 * sizeof(double) * M, c->stream));
+    return reduce_vec(c, e->growth, 2 * M, ncclMax, h);
+}
+
+double rpvgrw_cols(const std::vector<double>& h, int M, int ncols) {
+    double rpvgrw = 1.0;
+    for (int j = 0; j < ncols; ++j)
+        if (h[M + j] != 0.0) rpvgrw = std::min(h[j] / h[M + j], rpvgrw);
+    return rpvgrw;
+}
+
+int pivot_growth_grid(const Grid& g, EquilState* e, const double* F, const double* A, bool per_column, double* rpvgrw,
+                      int* info) {
+    const int M = g.M;
     CFLX_TRY(zero_pivot_grid(g, e, F, info));
-    const int ncols = *info ? *info : g.M;
-    if (g.pk == 0) CFLX_TRY(equil_growth(F, A, g, ncols, e->growth, s));
-    else CFLX_CUDA(cudaMemsetAsync(e->growth, 0, 2 * sizeof(double), s));
-    if (c->world_size > 1) CFLX_NCCL(ncclAllReduce(e->growth, e->growth, 2, ncclDouble, ncclMax, c->world, s));
-    double h[2];
-    CFLX_CUDA(cudaMemcpyAsync(h, e->growth, sizeof(h), cudaMemcpyDeviceToHost, s));
-    CFLX_CUDA(cudaStreamSynchronize(s));
-    *rpvgrw = h[0] == 0.0 ? 1.0 : h[1] / h[0];  // dgesvx: dlange('M', A) / dlantr('M', 'U', AF)
+    const int ncols = *info ? *info : M;
+    std::vector<double> h;
+    CFLX_TRY(growth_cols_grid(g, e, false, F, A, ncols, h));
+    if (per_column) {
+        *rpvgrw = rpvgrw_cols(h, M, ncols);
+        return CFLX_OK;
+    }
+    // dgesvx: dlange('M', A) / dlantr('M', 'U', AF), the maxima of the two vectors (exact)
+    double am = 0.0, fm = 0.0;
+    for (int j = 0; j < M; ++j) am = std::max(am, h[j]), fm = std::max(fm, h[M + j]);
+    *rpvgrw = fm == 0.0 ? 1.0 : am / fm;
     return CFLX_OK;
 }
 
 // ---------------------------------------------------------------- the expert drivers' solve
-// B is scaled on the device, solved and refined there, and X is unscaled before the download
-int svx_tail(EquilState* e, RefineCache* rc, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx,
-             double* ferr, double* berr, const double* pre, const double* post, double cnd, double rcond, int* info) {
+// B is scaled on the device by pre, solved there, refined by the caller's step, and X is unscaled by post before the
+// download.  refine(B, ldb, X, ldx) refines the device X in place.
+using SvxRefine = std::function<int(const double*, int, double*, int)>;
+static int svx_tail(EquilState* e, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx,
+                    const double* pre, const double* post, const SvxRefine& refine) {
     cudaStream_t s = op.grid.comm->stream;
     const int M = op.grid.M, ldn = (int)round_up(nrhs, 8);
     CFLX_TRY(equil_grow(e, M, ldn));
@@ -436,15 +475,33 @@ int svx_tail(EquilState* e, RefineCache* rc, const RefineOp& op, int nrhs, const
                                 cudaMemcpyDefault, s));
     if (pre) CFLX_TRY(launch_scale_rows(dB, ldn, M, nrhs, pre, s));
     CFLX_TRY(op.solve(false, nrhs, dB, ldn, dX, ldn));
-    CFLX_TRY(refine_run(rc, op, nrhs, dB, ldn, dX, ldn, ferr, berr));
+    CFLX_TRY(refine(dB, ldn, dX, ldn));
     if (post) CFLX_TRY(launch_scale_rows(dX, ldn, M, nrhs, post, s));
     CFLX_CUDA(cudaMemcpy2DAsync(X, (size_t)ldx * sizeof(double), dX, ldn * sizeof(double), nrhs * sizeof(double), M,
                                 cudaMemcpyDefault, s));
     CFLX_CUDA(cudaStreamSynchronize(s));
+    return CFLX_OK;
+}
+
+int svx_run(EquilState* e, RefineCache* rc, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx,
+            double* ferr, double* berr, const double* pre, const double* post, double cnd, double rcond, int* info) {
+    auto refine = [&](const double* dB, int ldb_, double* dX, int ldx_) {
+        return refine_run(rc, op, nrhs, dB, ldb_, dX, ldx_, ferr, berr);
+    };
+    CFLX_TRY(svx_tail(e, op, nrhs, B, ldb, X, ldx, pre, post, refine));
     if (ferr && post)
         for (int j = 0; j < nrhs; ++j) ferr[j] /= cnd;
-    *info = rcond < std::ldexp(1.0, -53) ? M + 1 : 0;
+    *info = rcond < std::ldexp(1.0, -53) ? op.grid.M + 1 : 0;
     return CFLX_OK;
+}
+
+int svxx_run(EquilState* e, RefineCache* rc, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx,
+             const double* pre, const double* post, const double* d, double rcond, bool cwise, double* berr,
+             double* err_norm, double* err_comp, int* info) {
+    auto refine = [&](const double* dB, int ldb_, double* dX, int ldx_) {
+        return refine_x_run(rc, op, nrhs, dB, ldb_, dX, ldx_, d, rcond, cwise, berr, err_norm, err_comp, info);
+    };
+    return svx_tail(e, op, nrhs, B, ldb, X, ldx, pre, post, refine);
 }
 
 }  // namespace cflx

@@ -736,6 +736,25 @@ RefineOp lu_refine_op(cflx_lu* lu, bool t) {
     };
     return RefineOp{*lu, lu->A0, t ? ResidMode::TN : ResidMode::NN, false, solve};
 }
+
+// cflx_lu_equilibrate (dgeequ) and, with pow2, cflx_lu_equilibrate_b (dgeequb)
+int lu_equilibrate(cflx_lu* lu, int apply, bool pow2, double* r_out, double* c_out, double* rowcnd_out,
+                   double* colcnd_out, double* amax_out, char* equed_out, int* info_out) {
+    if (!lu || (apply != 0 && apply != 1) || !info_out) return CFLX_ERR_ARG;
+    CFLX_TRY(handle_equil_begin(lu, apply != 0));
+    if (lu->a0_is_next) CFLX_CUDA(cudaStreamWaitEvent(lu->comm->stream, lu->ev_upload, 0));  // A0 holds a streamed next input
+    double rowcnd = 0.0, colcnd = 0.0, amax = 0.0;
+    char equed = 'N';
+    int info = 0;
+    CFLX_TRY(geequ_grid(*lu, &lu->eq, lu->A0, apply != 0, pow2, r_out, c_out, &rowcnd, &colcnd, &amax, &equed, &info));
+    CFLX_TRY(handle_equil_end(lu, apply != 0, info, equed, rowcnd, colcnd, lu->eq.qc));
+    if (rowcnd_out) *rowcnd_out = rowcnd;
+    if (colcnd_out) *colcnd_out = colcnd;
+    if (amax_out) *amax_out = amax;
+    if (equed_out) *equed_out = equed;
+    *info_out = info;
+    return CFLX_OK;
+}
 }  // namespace
 
 // ======================================================================================================== C ABI
@@ -1259,20 +1278,47 @@ int cflx_lu_refine_x(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb,
 // and the solve cache are dropped, as by cflx_lu_set_local.
 int cflx_lu_equilibrate(cflx_lu* lu, int apply, double* r_out, double* c_out, double* rowcnd_out, double* colcnd_out,
                         double* amax_out, char* equed_out, int* info_out) {
-    if (!lu || (apply != 0 && apply != 1) || !info_out) return CFLX_ERR_ARG;
-    CFLX_TRY(handle_equil_begin(lu, apply != 0));
-    if (lu->a0_is_next) CFLX_CUDA(cudaStreamWaitEvent(lu->comm->stream, lu->ev_upload, 0));  // A0 holds a streamed next input
-    double rowcnd = 0.0, colcnd = 0.0, amax = 0.0;
-    char equed = 'N';
+    return lu_equilibrate(lu, apply, false, r_out, c_out, rowcnd_out, colcnd_out, amax_out, equed_out, info_out);
+}
+
+// COLLECTIVE.  LAPACK dgeequb (+ dlaqge when apply): cflx_lu_equilibrate with the scales rounded to powers of two.
+int cflx_lu_equilibrate_b(cflx_lu* lu, int apply, double* r_out, double* c_out, double* rowcnd_out, double* colcnd_out,
+                          double* amax_out, char* equed_out, int* info_out) {
+    return lu_equilibrate(lu, apply, true, r_out, c_out, rowcnd_out, colcnd_out, amax_out, equed_out, info_out);
+}
+
+// COLLECTIVE.  LAPACK dgesvxx after the factorisation, with the scaling the factors carry: the first zero pivot and
+// dla_gerpvgrw, then B scaled, the solve, dgerfsx's refinement as cflx_lu_refine_x runs it, X unscaled.
+int cflx_lu_svxx(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out,
+                 double* rpvgrw_out, double* berr_out, double* err_bnds_norm_out, double* err_bnds_comp_out,
+                 char* equed_out, int* info_out) {
+    if (!lu || (trans != 0 && trans != 1) || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B || !X || !rcond_out ||
+        !err_bnds_norm_out || !info_out)
+        return CFLX_ERR_ARG;
+    CFLX_TRY(lu_check(lu, "extra-precise expert solve", true));
+    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    const bool t = trans != 0;
+    const EquilRecord& eq = lu->eq.fac;
+    const bool rowequ = eq.equed == 'R' || eq.equed == 'B', colequ = eq.equed == 'C' || eq.equed == 'B';
+    if (equed_out) *equed_out = eq.equed;
+    if (!lu->sv.ready) CFLX_TRY(lu_solve_prepare(lu));
+    double rpvgrw = 1.0;
     int info = 0;
-    CFLX_TRY(geequ_grid(*lu, &lu->eq, lu->A0, apply != 0, r_out, c_out, &rowcnd, &colcnd, &amax, &equed, &info));
-    CFLX_TRY(handle_equil_end(lu, apply != 0, info, equed, rowcnd, colcnd, lu->eq.qc));
-    if (rowcnd_out) *rowcnd_out = rowcnd;
-    if (colcnd_out) *colcnd_out = colcnd;
-    if (amax_out) *amax_out = amax;
-    if (equed_out) *equed_out = equed;
+    CFLX_TRY(pivot_growth_grid(*lu, &lu->eq, lu->Cbuf, lu->A0, true, &rpvgrw, &info));
+    if (rpvgrw_out) *rpvgrw_out = rpvgrw;
     *info_out = info;
-    return CFLX_OK;
+    if (info > 0) {  // exactly singular U: X is left as it was
+        *rcond_out = 0.0;
+        return CFLX_OK;
+    }
+    // dgecon as cflx_lu_refine_x: the infinity-norm for trans 0, the 1-norm for trans 1
+    double rcond = 0.0;
+    CFLX_TRY(lu_rcond(lu, !t, &rcond, nullptr));
+    *rcond_out = rcond;
+    // B is scaled by the scales of the rows of op(A), X (and the bounds' d) by those of its columns
+    const double *r = rowequ ? eq.r : nullptr, *c = colequ ? eq.c : nullptr;
+    return svxx_run(&lu->eq, &lu->sv.rf, lu_refine_op(lu, t), nrhs, B, ldb, X, ldx, t ? c : r, t ? r : c, t ? r : c,
+                    rcond, err_bnds_comp_out != nullptr, berr_out, err_bnds_norm_out, err_bnds_comp_out, info_out);
 }
 
 // COLLECTIVE.  LAPACK dgesvx after the factorisation, with the scaling the factors carry: B scaled, the reciprocal pivot
@@ -1290,7 +1336,7 @@ int cflx_lu_svx(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, doub
     if (!lu->sv.ready) CFLX_TRY(lu_solve_prepare(lu));
     double rpvgrw = 1.0;
     int info = 0;
-    CFLX_TRY(pivot_growth_grid(*lu, &lu->eq, lu->Cbuf, lu->A0, &rpvgrw, &info));
+    CFLX_TRY(pivot_growth_grid(*lu, &lu->eq, lu->Cbuf, lu->A0, false, &rpvgrw, &info));
     if (rpvgrw_out) *rpvgrw_out = rpvgrw;
     *info_out = info;
     if (info > 0) {  // exactly singular U: no solution
@@ -1303,8 +1349,8 @@ int cflx_lu_svx(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, doub
     *rcond_out = rcond;
     // op(A) X = B: B is scaled by the scales of the rows of op(A), X by those of its columns
     const double *r = rowequ ? eq.r : nullptr, *c = colequ ? eq.c : nullptr;
-    return svx_tail(&lu->eq, &lu->sv.rf, lu_refine_op(lu, t), nrhs, B, ldb, X, ldx, ferr_out, berr_out, t ? c : r,
-                    t ? r : c, t ? eq.rowcnd : eq.colcnd, rcond, info_out);
+    return svx_run(&lu->eq, &lu->sv.rf, lu_refine_op(lu, t), nrhs, B, ldb, X, ldx, ferr_out, berr_out, t ? c : r,
+                   t ? r : c, t ? eq.rowcnd : eq.colcnd, rcond, info_out);
 }
 
 int cflx_host_alloc(size_t bytes, void** out) {

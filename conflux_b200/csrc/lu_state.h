@@ -140,7 +140,8 @@ struct EquilState {
     size_t qcap = 0;
     double *B = nullptr, *X = nullptr;    // svx: M x ldn each, cap doubles each
     size_t cap = 0;
-    double* growth = nullptr;             // 2 doubles: max |triu(U)|, max |A|
+    double* growth = nullptr;             // the pivot growth's maxima by column: amax (M), then fmax (M); growth_cap
+    size_t growth_cap = 0;                // doubles
     int* ival = nullptr;                  // 1 int: the first zero pivot
     double* det = nullptr;                // M + 4 doubles: the gathered diagonal, then det_grid's DetResult
 };
@@ -396,8 +397,13 @@ int launch_residual_x(ResidMode mode, const double* A, const Layout& L, const do
 // rows scaled by pre (may be null), X = op.solve(false, B), refine_run, the rows of X scaled by post (may be null), X out;
 // when post is not null, ferr is divided by cnd.  Then *info = M + 1 when rcond < 2^-53 (dgesvx / dposvx: the matrix is
 // singular to working precision), else 0.
-int svx_tail(EquilState* e, RefineCache* rc, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx,
-             double* ferr, double* berr, const double* pre, const double* post, double cnd, double rcond, int* info);
+int svx_run(EquilState* e, RefineCache* rc, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx,
+            double* ferr, double* berr, const double* pre, const double* post, double cnd, double rcond, int* info);
+// The same steps for cflx_lu_svxx / cflx_chol_svxx, with refine_x_run (d, rcond, cwise, berr, err_norm, err_comp and
+// info as there) in place of refine_run.  The bounds already refer to the unscaled x: nothing is divided.
+int svxx_run(EquilState* e, RefineCache* rc, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx,
+             const double* pre, const double* post, const double* d, double rcond, bool cwise, double* berr,
+             double* err_norm, double* err_comp, int* info);
 
 // norm.cu: the collective infinity-norm (maximum row sum) of the M x M matrix whose layer-0 shares are A (every local
 // entry counts), into *anorm (every rank).  Deterministic: no floating-point atomics.
@@ -418,24 +424,37 @@ int diag_grid(const Grid& g, const double* A, double* d);
 int equil_apply(double* A, const Layout& L, const double* r, const double* c, char equed, cudaStream_t s);
 int equil_sym_apply(double* A, const Layout& L, const double* sc, cudaStream_t s);
 // On a share F of L\U (and A of the input): *zero_pivot = min(1 + g) over the global diagonal entries g < M the share
-// holds with F_gg == 0 (INT_MAX: none); out2 = {max |F| over global row <= global column, max |A|}, both over the global
-// columns < ncols (zeros where the share holds none).
+// holds with F_gg == 0 (INT_MAX: none).
 int equil_zero_pivot(const double* F, const Layout& L, int* zero_pivot, cudaStream_t s);
-int equil_growth(const double* F, const double* A, const Layout& L, int ncols, double* out2, cudaStream_t s);
+// The pivot growth's maxima by global column g < ncols, out = {amax (M), fmax (M)} with zeros where the share holds
+// nothing.  LU (!sym, F = L\U): amax_g = max |a_ig| over every row, fmax_g = max |f_ig| over the rows i <= g.  Cholesky
+// (sym, F = L, both the stored lower triangles): the real tiles' entries with g <= i < ncols of A and of F.  Nothing
+// outside these masks is read.
+int equil_growth_cols(const double* F, const double* A, const Layout& L, bool sym, int ncols, double* out,
+                      cudaStream_t s);
 // the first exactly zero U(k,k) of the layer-0 shares F of L\U on the grid, COLLECTIVE (ncclMin over the world): *info =
 // k (1-based), or 0 when there is none; the same on every rank
 int zero_pivot_grid(const Grid& g, EquilState* e, const double* F, int* info);
-// LAPACK dgeequ (+ dlaqge when `apply`) on the grid, COLLECTIVE: the scales into e->qr / e->qc (no record changes) and
-// the host results; r_out / c_out (M, may be null).  Scales are applied only when info == 0.
-int geequ_grid(const Grid& g, EquilState* e, double* A, bool apply, double* r_out, double* c_out, double* rowcnd,
-               double* colcnd, double* amax, char* equed, int* info);
-// LAPACK dpoequ (+ dlaqsy, UPLO = 'L', when `apply`) on the grid, COLLECTIVE: s into e->qr (no record changes)
-int poequ_grid(const Grid& g, EquilState* e, double* A, bool apply, double* s_out, double* scond, double* amax,
-               char* equed, int* info);
-// dgesvx's reciprocal pivot growth on the grid, COLLECTIVE: F is L\U and A the input (both layer-0 shares of the M x M
-// matrix).  info = 1 + the first global k with U(k,k) == 0 (0: none); rpvgrw = max |A| / max |triu(U)| over the global
-// columns < (info ? info : M), or 1 when the denominator is 0.
-int pivot_growth_grid(const Grid& g, EquilState* e, const double* F, const double* A, double* rpvgrw, int* info);
+// LAPACK dgeequ, or dgeequb when pow2 (+ dlaqge when `apply`) on the grid, COLLECTIVE: the scales into e->qr / e->qc (no
+// record changes) and the host results; r_out / c_out (M, may be null).  Scales are applied only when info == 0.
+int geequ_grid(const Grid& g, EquilState* e, double* A, bool apply, bool pow2, double* r_out, double* c_out,
+               double* rowcnd, double* colcnd, double* amax, char* equed, int* info);
+// LAPACK dpoequ, or dpoequb when pow2 (+ dlaqsy, UPLO = 'L', when `apply`) on the grid, COLLECTIVE: s into e->qr (no
+// record changes)
+int poequ_grid(const Grid& g, EquilState* e, double* A, bool apply, bool pow2, double* s_out, double* scond,
+               double* amax, char* equed, int* info);
+// COLLECTIVE: equil_growth_cols on layer 0 (zeros on the other layers), one ncclMax over the world, and the host copy h
+// = {amax (M), fmax (M)}, bit-identical on every rank
+int growth_cols_grid(const Grid& g, EquilState* e, bool sym, const double* F, const double* A, int ncols,
+                     std::vector<double>& h);
+// dla_gerpvgrw / dla_porpvgrw from growth_cols_grid's h: the minimum of 1 and of amax_j / fmax_j over j < ncols with
+// fmax_j != 0
+double rpvgrw_cols(const std::vector<double>& h, int M, int ncols);
+// The reciprocal pivot growth of the LU on the grid, COLLECTIVE: F is L\U and A the input (both layer-0 shares of the
+// M x M matrix).  info = 1 + the first global k with U(k,k) == 0 (0: none); over the global columns < (info ? info : M),
+// rpvgrw is dgesvx's max |A| / max |triu(U)| (1 when the denominator is 0), or with per_column dgesvxx's dla_gerpvgrw.
+int pivot_growth_grid(const Grid& g, EquilState* e, const double* F, const double* A, bool per_column, double* rpvgrw,
+                      int* info);
 // the svx work buffers for nrhs columns (ldn = round_up(nrhs, 8)): e->B and e->X, M x ldn
 int equil_grow(EquilState* e, int M, int ldn);
 // X[i][j] *= d[i] for i < M, j < n (ld), on the device

@@ -140,6 +140,29 @@ inline int choleskySvx(int nrhs, const double* B, int ldb, double* X, int ldx, d
     chol_detail::check(cflx_chol_svx(s.plan, nrhs, B, ldb, X, ldx, rcond, ferr, berr, equed, &info), "choleskySvx");
     return info;
 }
+// LAPACK dpoequb (+ dlaqsy, lower, when apply) on the input the device holds (cflx_chol_equilibrate_b, collective):
+// choleskyEquilibrate with the scales rounded to powers of two.
+inline int choleskyEquilibrateB(bool apply = true, double* s_out = nullptr, double* scond = nullptr,
+                                double* amax = nullptr, char* equed = nullptr) {
+    auto& s = chol_detail::state();
+    if (!s.plan) throw CholeskyException("choleskyEquilibrateB() before initialize()");
+    int info = 0;
+    chol_detail::check(cflx_chol_equilibrate_b(s.plan, apply ? 1 : 0, s_out, scond, amax, equed, &info),
+                       "choleskyEquilibrateB");
+    return info;
+}
+// LAPACK dposvxx after parallelCholesky(), with the scaling the factor carries (cflx_chol_svxx, collective): arguments
+// and result as conflux::LU_svxx without transposed.
+inline int choleskySvxx(int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond, double* err_norm,
+                        double* err_comp = nullptr, double* rpvgrw = nullptr, double* berr = nullptr,
+                        char* equed = nullptr) {
+    auto& s = chol_detail::state();
+    if (!s.plan) throw CholeskyException("choleskySvxx() before initialize()");
+    int info = 0;
+    chol_detail::check(cflx_chol_svxx(s.plan, nrhs, B, ldb, X, ldx, rcond, rpvgrw, berr, err_norm, err_comp, equed, &info),
+                       "choleskySvxx");
+    return info;
+}
 // LAPACK dpotri (lower) with the factor of the last parallelCholesky() (cflx_chol_inverse, collective): Ainv_local (Ml x
 // Nl; host or device memory; may be null) receives inv(A) on this rank's real tiles on and below the diagonal, zeros
 // elsewhere.

@@ -317,6 +317,32 @@ int LU_svx(lu_params<T>& gv, int nrhs, const T* B, int ldb, T* X, int ldx, doubl
     return info;
 }
 
+// LAPACK dgeequb (+ dlaqge when apply) on the input the device holds (cflx_lu_equilibrate_b, collective): LU_equilibrate
+// with the scales rounded to powers of two, so that scaling A and B and unscaling X are exact.  Arguments and result as
+// LU_equilibrate; the factors of the next LU_rep carry the scaling to LU_svxx.
+template <class T>
+int LU_equilibrate_b(lu_params<T>& gv, bool apply = true, T* r = nullptr, T* c = nullptr, double* rowcnd = nullptr,
+                     double* colcnd = nullptr, double* amax = nullptr, char* equed = nullptr) {
+    int info = 0;
+    check(cflx_lu_equilibrate_b(gv.plan, apply ? 1 : 0, r, c, rowcnd, colcnd, amax, equed, &info), "LU_equilibrate_b");
+    return info;
+}
+
+// LAPACK dgesvxx after LU_rep, with the scaling the factors carry (cflx_lu_svxx, collective): X (M x nrhs) solves A X = B
+// (A^T X = B when transposed) with extra-precise refinement; err_norm (nrhs x 3) required, err_comp null skips the
+// componentwise bounds; rpvgrw / berr / equed may be null.  Returns info (0; k for an exactly zero U(k,k), X untouched;
+// M + j as LU_refine_x).
+template <class T>
+int LU_svxx(lu_params<T>& gv, int nrhs, const T* B, int ldb, T* X, int ldx, double* rcond, double* err_norm,
+            double* err_comp = nullptr, double* rpvgrw = nullptr, double* berr = nullptr, char* equed = nullptr,
+            bool transposed = false) {
+    int info = 0;
+    check(cflx_lu_svxx(gv.plan, transposed ? 1 : 0, nrhs, B, ldb, X, ldx, rcond, rpvgrw, berr, err_norm, err_comp, equed,
+                       &info),
+          "LU_svxx");
+    return info;
+}
+
 // LAPACK dgetri with the factors of the last LU_rep on the GPU grid (cflx_lu_inverse, collective): Ainv_local (Ml x Nl,
 // the conflux layout; host or device memory; may be null) receives this rank's share of inv(A).  Returns info (0; k for
 // an exactly zero U(k,k), nothing written).

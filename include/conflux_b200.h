@@ -162,6 +162,28 @@ int cflx_lu_equilibrate(cflx_lu*, int apply, double* r_out, double* c_out, doubl
  * CFLX_ERR_ARG as cflx_lu_refine and for a NULL rcond_out or info_out; CFLX_ERR_STATE as cflx_lu_rcond. */
 int cflx_lu_svx(cflx_lu*, int trans, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out,
                 double* ferr_out, double* berr_out, double* rpvgrw_out, char* equed_out, int* info_out);
+/* COLLECTIVE.  LAPACK dgeequb (+ dlaqge when apply): cflx_lu_equilibrate with the scales rounded to powers of two.  The
+ * row maxima are rounded to 2^INT(log(x) / log(2)) before rcmin, rcmax and amax are taken, then the column maxima of
+ * |a| r likewise; the exponents come from the host's log, as LAPACK's.  r_out / c_out hold the rounded maxima on the
+ * info paths.  Scaling A, scaling B and unscaling X are then exact (barring underflow), so the factors of the scaled
+ * matrix are those of diag(r) A diag(c) and cflx_lu_svxx's bounds carry over to the unscaled solution.  Arguments,
+ * state rules and the scaling record as cflx_lu_equilibrate. */
+int cflx_lu_equilibrate_b(cflx_lu*, int apply, double* r_out, double* c_out, double* rowcnd_out, double* colcnd_out,
+                          double* amax_out, char* equed_out, int* info_out);
+/* COLLECTIVE.  LAPACK dgesvxx after the factorisation (FACT = 'F' on this library's factors, with the scaling they carry
+ * from cflx_lu_equilibrate_b, cflx_lu_equilibrate or none): trans 0: A X = B, 1: A^T X = B.  rpvgrw_out (may be NULL):
+ * dla_gerpvgrw, the minimum of 1 and of max_i |a_ij| / max_{i <= j} |u_ij| over the columns j with a non-zero
+ * denominator.  B is scaled by r (trans 0, equed R / B) or c (trans 1, equed C / B), solved, refined as
+ * cflx_lu_refine_x refines it (rcond_out, berr_out, err_bnds_norm_out and err_bnds_comp_out as there, the bounds for
+ * the unscaled solution, so nothing is divided by colcnd), and X is unscaled by c (trans 0) or r (trans 1).  equed_out
+ * (may be NULL): the factors' scaling.  info_out: k for the first exactly zero U(k,k) (rpvgrw over the leading k columns,
+ * rcond 0, nothing else written, X left as it was); M + j from the refinement as cflx_lu_refine_x (there is no
+ * dgesvx-style M + 1); 0 otherwise.  CFLX_ERR_ARG as cflx_lu_refine_x and for a NULL rcond_out; CFLX_ERR_STATE as
+ * cflx_lu_rcond.  Results identical on every rank; leaves the factors, the permutation, the input, the scaling record,
+ * later solves and the launch count as they are. */
+int cflx_lu_svxx(cflx_lu*, int trans, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out,
+                 double* rpvgrw_out, double* berr_out, double* err_bnds_norm_out, double* err_bnds_comp_out,
+                 char* equed_out, int* info_out);
 /* COLLECTIVE.  inv(A) of the padded M x M matrix factored by the last cflx_lu_factor (P A = L U), on the GPU grid, like
  * LAPACK's dgetri.  Ainv_local: Ml x Nl row-major, the conflux layout of cflx_lu_set_local; host or device memory; may be
  * NULL on any rank.  Every rank receives the share of its grid position (pi, pj); layers pk != 0 receive the bits of
@@ -265,6 +287,20 @@ int cflx_chol_equilibrate(cflx_chol*, int apply, double* s_out, double* scond_ou
  * Arguments as cflx_chol_refine; CFLX_ERR_ARG also for a NULL rcond_out or info_out; CFLX_ERR_STATE as cflx_chol_solve. */
 int cflx_chol_svx(cflx_chol*, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out, double* ferr_out,
                   double* berr_out, char* equed_out, int* info_out);
+/* COLLECTIVE.  LAPACK dpoequb (+ dlaqsy when apply): cflx_chol_equilibrate with s_i = 2^INT((-0.5 / log(2)) log(a_ii)),
+ * the exponents from the host's log, as LAPACK's; scond, amax, info and s_out on the info path as dpoequ.  Arguments,
+ * state rules and the scaling record as cflx_chol_equilibrate. */
+int cflx_chol_equilibrate_b(cflx_chol*, int apply, double* s_out, double* scond_out, double* amax_out, char* equed_out,
+                            int* info_out);
+/* COLLECTIVE.  LAPACK dposvxx (UPLO = 'L') after a successful factorisation, with the scaling the factor carries:
+ * rpvgrw_out (may be NULL) = dla_porpvgrw, the minimum of 1 and of max |a_ij| / max |l_ij| over the rows i >= j of the
+ * stored lower triangles, per column j with a non-zero denominator; rcond_out = dpocon; B scaled by s, solved, refined as
+ * cflx_chol_refine_x refines it and unscaled by s.  info_out: N + j from the refinement, else 0.  A factorisation that
+ * found a non-positive pivot is refused (CFLX_ERR_STATE), where dposvxx would return info = k.  Arguments, results and
+ * side effects otherwise as cflx_lu_svxx without trans. */
+int cflx_chol_svxx(cflx_chol*, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out,
+                   double* rpvgrw_out, double* berr_out, double* err_bnds_norm_out, double* err_bnds_comp_out,
+                   char* equed_out, int* info_out);
 /* COLLECTIVE.  inv(A) from the factor of the last successful cflx_chol_factor (A = L L^T), like LAPACK's dpotri
  * (UPLO = 'L'): the real tiles on and below the diagonal of this rank's Ml x Nl share hold inv(A), whole diagonal tiles
  * included.  The tiles above the diagonal and the local tiles with a global index >= Kappa are zero.  Host or device
@@ -322,6 +358,13 @@ int cflx_dbg_residual_x(int mode, int Ml, int Nl, const double* A, int v, int Ka
 int cflx_dbg_equil(int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, int M, const double* A,
                    const double* r, const double* c, char equed, int ncols, double* rowmax_out, double* colmax_out,
                    double* diag_out, double* scaled_out, double* sym_scaled_out, double* growth_out, int* zero_pivot_out);
+/* the per-column pivot growth pass of cflx_lu_svxx (mode 0), cflx_chol_svxx (mode 1) and cflx_lu_svx on one layer-0
+ * share F (the factor) and A (the input), both Ml x Nl in the layout of cflx_dbg_equil (Kappa: the real tiles of mode 1).
+ * amax_out / fmax_out (M each, may be NULL), by global column j < ncols, zeros elsewhere: mode 0 max |a_ij| over every
+ * row and max |f_ij| over the rows i <= j; mode 1 both over the real tiles' rows j <= i < ncols.  Nothing outside these
+ * masks is read. */
+int cflx_dbg_growth_cols(int mode, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, int M, int ncols,
+                         const double* F, const double* A, double* amax_out, double* fmax_out);
 /* the per-share kernels of cflx_lu_inverse (mode 0) and cflx_chol_inverse (mode 1) on one share at grid position (pi, pj)
  * of Px x Py (Ml x Nl row-major, Ml and Nl multiples of v; M >= (Ml / v) Px v and >= (Nl / v) Py v global indices; Kappa:
  * the real tiles of mode 1), for the block of nc columns from global column c0 (c0 + nc <= M).  Each output may be NULL:
