@@ -15,7 +15,7 @@ import numpy as np
 
 from ._lib import ConfluxError, LIB_PATH, SYMBOLS, check, lib
 
-__all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "residual", "validate", "lu_solve", "lu_rcond", "lu_refine", "lu_refine_x", "lu_equilibrate", "lu_svx", "lu_equilibrate_b", "lu_svxx", "lu_inverse", "lu_det", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
+__all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "residual", "validate", "lu_solve", "lu_rcond", "lu_refine", "lu_refine_x", "lu_equilibrate", "lu_svx", "lu_equilibrate_b", "lu_svxx", "lu_inverse", "lu_det", "rhs_local_cols", "lu_solve_local", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
 
 
 def auto_grid(M, N, P):
@@ -343,24 +343,43 @@ def lu_svx(gv, B, trans=False):
                                                           equed=equed.value.decode(), info=k)
 
 
-def _share_out(out, Ml, Nl, what):
-    """(pointer, array) of the Ml x Nl float64 C-contiguous share an inverse is written into: a new NumPy array when out is
-    None, else out itself -- a NumPy array, or any object with __cuda_array_interface__ (a torch CUDA tensor)."""
+def _share_out(out, Ml, Nl, what, strided=False, name="out"):
+    """(pointer, array, ld) of the Ml x Nl float64 share an inverse or a distributed solve reads or writes: a new NumPy
+    array when out is None, else out itself -- a NumPy array, or any object with __cuda_array_interface__ (a torch CUDA
+    tensor).  The share must be C-contiguous (ld = Nl); with strided, any (Ml, n >= Nl) array whose rows are contiguous
+    is accepted, ld being its row stride in elements."""
     if out is None:
         out = np.empty((Ml, Nl))
     if isinstance(out, np.ndarray):
+        if strided:
+            return out.ctypes.data, out, _rows_share(out.dtype == np.float64, out.shape, out.strides, Ml, Nl, what, name,
+                                                     "array")
         if out.dtype != np.float64 or not out.flags.c_contiguous or out.shape != (Ml, Nl):
-            raise ValueError(f"{what}: out must be a C-contiguous float64 array of shape ({Ml}, {Nl}), got {out.dtype} "
+            raise ValueError(f"{what}: {name} must be a C-contiguous float64 array of shape ({Ml}, {Nl}), got {out.dtype} "
                              f"{out.shape}")
-        return out.ctypes.data, out
+        return out.ctypes.data, out, Nl
     cai = getattr(out, "__cuda_array_interface__", None)
     if cai is None:
-        raise ValueError(f"{what}: out must be a NumPy array or expose __cuda_array_interface__")
+        raise ValueError(f"{what}: {name} must be a NumPy array or expose __cuda_array_interface__")
     shape, strides = tuple(cai["shape"]), cai.get("strides")
+    if strided:
+        if strides is None and len(shape) == 2:
+            strides = (8 * shape[1], 8)
+        return cai["data"][0], out, _rows_share(cai["typestr"] == "<f8", shape, strides, Ml, Nl, what, name,
+                                                "device array")
     if cai["typestr"] != "<f8" or shape != (Ml, Nl) or strides not in (None, (8 * Nl, 8)):
-        raise ValueError(f"{what}: out must be a C-contiguous float64 device array of shape ({Ml}, {Nl}), got "
+        raise ValueError(f"{what}: {name} must be a C-contiguous float64 device array of shape ({Ml}, {Nl}), got "
                          f"{cai['typestr']} {shape} strides {strides}")
-    return cai["data"][0], out
+    return cai["data"][0], out, Nl
+
+
+def _rows_share(f8, shape, strides, Ml, Nl, what, name, kind):
+    """the row stride in elements of a float64 (Ml, n >= Nl) share with contiguous rows, else ValueError"""
+    if (not f8 or len(shape) != 2 or shape[0] != Ml or shape[1] < Nl or strides is None or strides[1] != 8
+            or strides[0] % 8 or strides[0] < 8 * shape[1]):
+        raise ValueError(f"{what}: {name} must be a float64 {kind} of shape ({Ml}, n >= {Nl}) with contiguous rows, got "
+                         f"shape {tuple(shape)} strides {strides}")
+    return strides[0] // 8
 
 
 def lu_inverse(gv, out=None):
@@ -370,10 +389,47 @@ def lu_inverse(gv, out=None):
     share to write into, a NumPy array or a torch CUDA tensor (float64, C-contiguous, (Ml, Nl)).  The columns are solves
     A X = I, so A X - I is the small residual.  COLLECTIVE over gv.lu_comm; the factors and later solves are left as they
     are."""
-    ptr, arr = _share_out(out, gv.Ml, gv.Nl, "lu_inverse")
+    ptr, arr, _ = _share_out(out, gv.Ml, gv.Nl, "lu_inverse")
     info = ctypes.c_int()
     check(lib().cflx_lu_inverse(gv._h, ptr, ctypes.byref(info)), "lu_inverse")
     return (None if info.value else arr), info.value
+
+
+def rhs_local_cols(nrhs, v, Py):
+    """The local columns of an M x nrhs right-hand side share on a grid with Py grid columns (lu_solve_local,
+    cholesky.solve_local): v * ceil(ceil(nrhs / v) / Py), so nrhs = M gives the matrix's Nl."""
+    n = ctypes.c_int()
+    check(lib().cflx_rhs_local_cols(int(nrhs), int(v), int(Py), ctypes.byref(n)), "rhs_local_cols")
+    return n.value
+
+
+def _solve_local(fn, what, Ml, v, Py, layer0, B_share, nrhs, out, *lead):
+    """B_share / out checked as (Ml, n >= rhs_local_cols) float64 shares with contiguous rows; out None: a new zeroed NumPy
+    array; B_share None is allowed off layer 0 (it is not read there)"""
+    ncl = rhs_local_cols(nrhs, v, Py)
+    bptr, ldb = None, ncl
+    if B_share is not None:
+        bptr, _, ldb = _share_out(B_share, Ml, ncl, what, strided=True, name="B_share")
+    elif layer0:
+        raise ValueError(f"{what}: B_share is read on layer 0 and may not be None there")
+    if out is None:
+        out = np.zeros((Ml, ncl))
+    xptr, out, ldx = _share_out(out, Ml, ncl, what, strided=True)
+    check(fn(*lead, int(nrhs), bptr, ldb, xptr, ldx), what)
+    return out
+
+
+def lu_solve_local(gv, B_share, nrhs, trans=False, out=None):
+    """Solves A X = B (A^T X = B when trans) with the factors of the last LU_rep, like ScaLAPACK's pdgetrs, with B and X
+    distributed like A: M x nrhs matrices tiled v x v, global tile (I, J) on grid position (I % Px, J % Py) at local tile
+    (I / Px, J / Py).  B_share: this rank's share, (gv.Ml, n >= rhs_local_cols(nrhs, gv.v, gv.Py)) float64 with
+    contiguous rows, a NumPy array or any __cuda_array_interface__ object (a torch CUDA tensor on this rank's device);
+    read on layer 0 only (None elsewhere).  out: X's share, the same kinds; a new zeroed NumPy array when None, and
+    `out is B_share` solves in place.  Local columns whose global index is >= nrhs are neither read nor written.  Returns
+    out; every layer gets layer 0's bits.  COLLECTIVE over gv.lu_comm; every rank passes the same nrhs and trans.  The
+    factors, the input and later solves are left as they are."""
+    return _solve_local(lib().cflx_lu_solve_local, "lu_solve_local", gv.Ml, gv.v, gv.Py, gv.pk == 0, B_share, nrhs, out,
+                        gv._h, 1 if trans else 0)
 
 
 def lu_det(gv, unscaled=False):
@@ -443,6 +499,13 @@ class cholesky:
         check(lib().cflx_chol_solve(self._h, nrhs, B2.ctypes.data, max(nrhs, 1), X.ctypes.data, max(nrhs, 1)), "chol_solve")
         return X.reshape(B.shape)
 
+    def solve_local(self, B_share, nrhs, out=None):
+        """Solves A X = B with the factor of the last parallelCholesky, like ScaLAPACK's pdpotrs, with B and X distributed
+        like A; arguments and result as lu_solve_local's.  Only the rows of real tiles (global tile index < Kappa) are
+        read or written.  COLLECTIVE; every rank passes the same nrhs."""
+        return _solve_local(lib().cflx_chol_solve_local, "cholesky.solve_local", self.Ml, self.v, self.PY, self.pz == 0,
+                            B_share, nrhs, out, self._h)
+
     def rcond(self):
         """LAPACK dpocon of the last parallelCholesky on the GPU grid: (rcond, anorm) with anorm = ||A||_1 of the padded
         symmetric input and rcond = 1 / (anorm * estimate of ||A^-1||_1).  COLLECTIVE; identical on every rank."""
@@ -505,7 +568,7 @@ class cholesky:
         """inv(A) from the factor of the last parallelCholesky on the GPU grid, like LAPACK's dpotri (lower): returns this
         rank's Ml x Nl share, whose real tiles on and below the diagonal hold inv(A); the tiles above the diagonal and
         those beyond Kappa are zero.  out as lu_inverse's.  COLLECTIVE; every layer gets layer 0's bits."""
-        ptr, arr = _share_out(out, self.Ml, self.Nl, "cholesky.inverse")
+        ptr, arr, _ = _share_out(out, self.Ml, self.Nl, "cholesky.inverse")
         check(lib().cflx_chol_inverse(self._h, ptr), "chol_inverse")
         return arr
 
@@ -740,6 +803,29 @@ class dbg:
                                            Xc.shape[1] if Xc is not None else 0, ptr(pm), W.ctypes.data, ptr(out),
                                            1 if zero_fill else 0), "dbg_inverse_share")
         return W, out
+
+    @staticmethod
+    def solve_local_share(mode, v, grid, pos, M, nrhs, c0, w, Ml, Kappa=None, B=None, Xk=None, X=None):
+        """The pack and scatter kernels of lu_solve_local (mode "lu") and cholesky.solve_local (mode "chol") on one
+        right-hand side share of Ml rows at grid position pos of grid = (Px, Py), for the block of w columns from global
+        column c0 of an M x nrhs matrix.  Returns (Bk, X): Bk (M x round_up(w, 8)) the pack of B (Ml x n >=
+        rhs_local_cols, every local row for "lu", the real tiles' rows, global tile index < Kappa, for "chol"), and a copy
+        of X after the scatter of Xk (M x round_up(w, 8), by global row) into it.  Either is None when its inputs are."""
+        m = {"lu": 0, "chol": 1}[mode]
+        Px, Py = (int(x) for x in grid)
+        ldn = -(-int(w) // 8) * 8
+        Bc = np.ascontiguousarray(B, dtype=np.float64) if B is not None else None
+        Bk = np.empty((int(M), ldn)) if Bc is not None else None
+        out = Xc = None
+        if X is not None and Xk is not None:
+            Xc = np.ascontiguousarray(Xk, dtype=np.float64)
+            out = np.array(X, dtype=np.float64, order="C")
+        ptr = lambda a: a.ctypes.data if a is not None else None  # noqa: E731
+        check(lib().cflx_dbg_solve_local_share(m, int(Ml), int(v), int(Kappa if Kappa is not None else 1 << 30), Px, Py,
+                                               int(pos[0]), int(pos[1]), int(M), int(nrhs), int(c0), int(w), ptr(Bc),
+                                               Bc.shape[1] if Bc is not None else 0, ptr(Bk), ptr(Xc), ptr(out),
+                                               out.shape[1] if out is not None else 0), "dbg_solve_local_share")
+        return Bk, out
 
     @staticmethod
     def det(d, s1=None, s2=None, square=False):

@@ -616,6 +616,22 @@ int chol_solve_prepare(cflx_chol* ch) {
     return CFLX_OK;
 }
 
+// One solve with the factor of the last successful factorisation (cflx_chol_solve, cflx_chol_solve_local); B host or
+// device, X may be null (the solution then stays in ch->sv.X).
+int chol_sweeps(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X, int ldx) {
+    if (!ch->sv.ready) CFLX_TRY(chol_solve_prepare(ch));
+    const SolveFactor f = chol_solve_factor(ch);
+    SolveCache* sc = &ch->sv;
+    const int ldn = (int)round_up(nrhs, 8);
+    CFLX_TRY(solve_cache_grow(sc, f, ldn, ch->pk == 0, true));
+    CFLX_TRY(solve_seed(sc, f, ldn, nrhs, B, ldb, SolveSeed{false, sc->rows, f.rows, sc->W}));
+    if (ch->pk == 0) {  // L Y = B keeping Y_t in Z, then L^T X = Y from Z
+        CFLX_TRY(solve_row_sweep(sc, f, ldn, true, sc->Z, ch->Py, false));
+        CFLX_TRY(solve_col_sweep(sc, f, ldn, false, Tri::LowerT, sc->X, 1, false));
+    }
+    return solve_finish(sc, f, ldn, nrhs, X, ldx);
+}
+
 const HandleTexts kCholTexts = {
     "cholesky %s requested before a successful cflx_chol_factor, or after cflx_chol_set_local without one",
     "cholesky equilibration requested before cflx_chol_set_local",
@@ -944,17 +960,23 @@ int cflx_chol_solve(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X
     if (!ch || nrhs < 1 || ldb < nrhs || (X && ldx < nrhs) || !B) return CFLX_ERR_ARG;
     CFLX_TRY(handle_check(ch, "solve"));
     CFLX_CUDA(cudaSetDevice(ch->comm->device));
-    if (!ch->sv.ready) CFLX_TRY(chol_solve_prepare(ch));
-    const SolveFactor f = chol_solve_factor(ch);
-    SolveCache* sc = &ch->sv;
-    const int ldn = (int)round_up(nrhs, 8);
-    CFLX_TRY(solve_cache_grow(sc, f, ldn, ch->pk == 0, true));
-    CFLX_TRY(solve_seed(sc, f, ldn, nrhs, B, ldb, SolveSeed{false, sc->rows, f.rows, sc->W}));
-    if (ch->pk == 0) {  // L Y = B keeping Y_t in Z, then L^T X = Y from Z
-        CFLX_TRY(solve_row_sweep(sc, f, ldn, true, sc->Z, ch->Py, false));
-        CFLX_TRY(solve_col_sweep(sc, f, ldn, false, Tri::LowerT, sc->X, 1, false));
-    }
-    return solve_finish(sc, f, ldn, nrhs, X, ldx);
+    return chol_sweeps(ch, nrhs, B, ldb, X, ldx);
+}
+
+// COLLECTIVE.  A X = B with B and X distributed like A (solve_local.cu): each block of columns assembled on the device
+// and solved by the sweeps of cflx_chol_solve, then scattered into the real rows of X's share.
+int cflx_chol_solve_local(cflx_chol* ch, int nrhs, const double* B_local, int ldb, double* X_local, int ldx) {
+    if (!ch) return CFLX_ERR_ARG;
+    SolveLocalArgs a{};
+    CFLX_TRY(solve_local_args(*ch, nrhs, B_local, ldb, X_local, ldx, &a));
+    CFLX_TRY(handle_check(ch, "solve"));
+    CFLX_CUDA(cudaSetDevice(ch->comm->device));
+    auto solve = [ch](int w, const double* Bk, int ldn, const double** Xk) -> int {
+        CFLX_TRY(chol_sweeps(ch, w, Bk, ldn, nullptr, 0));
+        *Xk = ch->sv.X;
+        return CFLX_OK;
+    };
+    return solve_local_run(*ch, solve_local_rows(*ch, true), a, solve);
 }
 
 // COLLECTIVE.  LAPACK dpotri (UPLO = 'L') on the grid (inverse.cu): the block solves with the identity on the sweeps of

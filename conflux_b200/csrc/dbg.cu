@@ -392,6 +392,38 @@ int cflx_dbg_inverse_share(int mode, int Ml, int Nl, int v, int Kappa, int Px, i
     return CFLX_OK;
 }
 
+// the pack and scatter kernels of the distributed solves (solve_local.cu) on one share at grid position (pi, pj) of Px x Py
+int cflx_dbg_solve_local_share(int mode, int Ml, int v, int Kappa, int Px, int Py, int pi, int pj, int M, int nrhs, int c0,
+                               int w, const double* B, int ldb, double* Bk_out, const double* Xk, double* X_inout, int ldx) {
+    CFLX_TRY(check_device());
+    if ((mode != 0 && mode != 1) || Ml < 0 || v < 1 || Ml % v || Px < 1 || Py < 1 || pi < 0 || pi >= Px || pj < 0 ||
+        pj >= Py || M < (Ml / v) * Px * v || nrhs < 1 || c0 < 0 || w < 1 || c0 + w > nrhs)
+        return CFLX_ERR_ARG;
+    const int ncl = rhs_local_cols(nrhs, v, Py), ldn = (int)round_up(w, 8);
+    if ((Bk_out && (!B || ldb < ncl)) || (X_inout && (!Xk || ldx < ncl))) return CFLX_ERR_ARG;
+    const Layout L{M, v, Kappa, Ml, ncl, Px, Py, pi, pj};
+    const int rows = solve_local_rows(L, mode == 1);
+    if (Bk_out) {
+        DevBuf dB, dK;
+        CFLX_TRY(dB.alloc(sizeof(double) * Ml * ldb));
+        CFLX_TRY(dK.alloc(sizeof(double) * M * ldn));
+        CFLX_CUDA(cudaMemcpy(dB.p, B, sizeof(double) * Ml * ldb, cudaMemcpyHostToDevice));
+        CFLX_TRY(launch_solve_local_pack(dB.as<double>(), ldb, L, rows, c0, w, dK.as<double>(), ldn, 0));
+        CFLX_CUDA(cudaMemcpy(Bk_out, dK.p, sizeof(double) * M * ldn, cudaMemcpyDeviceToHost));
+    }
+    if (X_inout) {
+        DevBuf dX, dK;
+        CFLX_TRY(dX.alloc(sizeof(double) * Ml * ldx));
+        CFLX_TRY(dK.alloc(sizeof(double) * M * ldn));
+        CFLX_CUDA(cudaMemcpy(dX.p, X_inout, sizeof(double) * Ml * ldx, cudaMemcpyHostToDevice));
+        CFLX_CUDA(cudaMemcpy(dK.p, Xk, sizeof(double) * M * ldn, cudaMemcpyHostToDevice));
+        CFLX_TRY(launch_solve_local_scatter(dK.as<double>(), ldn, L, rows, c0, w, dX.as<double>(), ldx, 0));
+        CFLX_CUDA(cudaMemcpy(X_inout, dX.p, sizeof(double) * Ml * ldx, cudaMemcpyDeviceToHost));
+    }
+    CFLX_CUDA(cudaDeviceSynchronize());
+    return CFLX_OK;
+}
+
 // the determinant's product kernel (det.cu) on host vectors
 int cflx_dbg_det(int n, const double* d, const double* s1, const double* s2, int square, double* mant_out,
                  int64_t* exp_out, int* neg_out, int* first_zero_out, int* nonfinite_out) {

@@ -1179,6 +1179,22 @@ int cflx_lu_solve_trans(cflx_lu* lu, int nrhs, const double* B, int ldb, double*
     return lu_sweeps(lu, true, false, nrhs, B, ldb, X, ldx);
 }
 
+// COLLECTIVE.  A X = B or A^T X = B with B and X distributed like A (solve_local.cu): each block of columns assembled on
+// the device and solved by the sweeps of cflx_lu_solve / cflx_lu_solve_trans, then scattered into X's share.
+int cflx_lu_solve_local(cflx_lu* lu, int trans, int nrhs, const double* B_local, int ldb, double* X_local, int ldx) {
+    if (!lu || (trans != 0 && trans != 1)) return CFLX_ERR_ARG;
+    SolveLocalArgs a{};
+    CFLX_TRY(solve_local_args(*lu, nrhs, B_local, ldb, X_local, ldx, &a));
+    CFLX_TRY(lu_check(lu, trans ? "transposed solve" : "solve", false));
+    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    auto solve = [lu, trans](int w, const double* Bk, int ldn, const double** Xk) -> int {
+        CFLX_TRY(lu_sweeps(lu, trans != 0, false, w, Bk, ldn, nullptr, 0));
+        *Xk = trans ? lu->sv.Xg : lu->sv.X;  // the transposed solve's P^T lands in Xg
+        return CFLX_OK;
+    };
+    return solve_local_run(*lu, solve_local_rows(*lu, false), a, solve);
+}
+
 // LAPACK dgecon (NORM = '1') on the grid (lu_rcond).
 int cflx_lu_rcond(cflx_lu* lu, double* rcond_out, double* anorm_out) {
     if (!lu || !rcond_out) return CFLX_ERR_ARG;

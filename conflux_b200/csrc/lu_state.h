@@ -486,6 +486,41 @@ int launch_inverse_zero(const Layout& L, double* out, cudaStream_t s);
 // null).  The solve cache must be prepared; perm: the LU's permutation on the device (every rank).
 int inverse_run(SolveCache* sc, const SolveFactor& f, InvKind kind, const int* perm, double* Ainv);
 
+// ---------------------------------------------------------------- distributed right-hand sides (solve_local.cu)
+// The local columns of an M x nrhs right-hand side share on a grid with Py grid columns: v * ceil(ceil(nrhs / v) / Py)
+int rhs_local_cols(int nrhs, int v, int Py);
+// The local rows a distributed solve reads and writes: every row (LU), or those before the first local tile with a
+// global index >= Nt (Cholesky, chol)
+int solve_local_rows(const Layout& L, bool chol);
+// The per-share kernels (L: the layout of the share; B / X row-major with leading dimensions ldb / ldx):
+//   pack:    Bk (M x ldn, by global row) zeroed, then Bk[L.row(r)][j] = B[r][local column of c0 + j] for r < rows, j < w
+//            and the block columns this share holds (B null: zeros only)
+//   scatter: X[r][local column of c0 + j] = Xk[L.row(r)][j] for the same entries
+int launch_solve_local_pack(const double* B, int64_t ldb, const Layout& L, int rows, int c0, int w, double* Bk, int ldn,
+                            cudaStream_t s);
+int launch_solve_local_scatter(const double* Xk, int ldn, const Layout& L, int rows, int c0, int w, double* X, int64_t ldx,
+                               cudaStream_t s);
+// A distributed solve's shares after solve_local_args: B null on the layers pk != 0 (never read there); *_dev: device
+// memory of this rank's device, else host memory
+struct SolveLocalArgs {
+    int nrhs;
+    const double* B;
+    int ldb;
+    bool b_dev;
+    double* X;
+    int ldx;
+    bool x_dev;
+};
+// CFLX_ERR_ARG for nrhs < 1, a NULL B on layer 0, ldb (layer 0) or ldx (X set) below rhs_local_cols, X == B with
+// ldx != ldb, or device memory of another device; CFLX_OK with *a filled otherwise.  No collective.
+int solve_local_args(const Grid& g, int nrhs, const double* B, int ldb, const double* X, int ldx, SolveLocalArgs* a);
+// solve(w, Bk, ldn, &Xk): the sweeps on the assembled block Bk (M x ldn device, w columns, the same on every rank), the
+// solution left in *Xk (M x ldn device, the same on every rank)
+using BlockSolve = std::function<int(int, const double*, int, const double**)>;
+// COLLECTIVE.  The block loop of cflx_lu_solve_local / cflx_chol_solve_local: per block of inverse_block_cols columns,
+// pack, the world all-reduce that assembles the block, solve, and the scatter into X (may be null); synchronises.
+int solve_local_run(const Grid& g, int rows, const SolveLocalArgs& a, const BlockSolve& solve);
+
 // ---------------------------------------------------------------- the determinant (det.cu)
 constexpr int DET_THREADS = 256;  // the one CTA of the product; part of its order (oracle/det_ref.py)
 // The exact-range product of an M-vector: |prod| = mant 2^exp, mant in [0.5, 1) (NaN / 0 as first_zero and nonfinite

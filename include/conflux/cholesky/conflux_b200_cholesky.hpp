@@ -91,6 +91,14 @@ inline void choleskySolve(int nrhs, const double* B, int ldb, double* X, int ldx
     if (!s.plan) throw CholeskyException("choleskySolve() before initialize()");
     chol_detail::check(cflx_chol_solve(s.plan, nrhs, B, ldb, X, ldx), "choleskySolve");
 }
+// A X = B with the factor of the last parallelCholesky(), like ScaLAPACK's pdpotrs, with B and X distributed like A
+// (cflx_chol_solve_local, collective): the shares and rules of conflux::LU_solve_local; only the rows of real tiles are
+// read or written.
+inline void choleskySolveLocal(int nrhs, const double* B_local, int ldb, double* X_local, int ldx) {
+    auto& s = chol_detail::state();
+    if (!s.plan) throw CholeskyException("choleskySolveLocal() before initialize()");
+    chol_detail::check(cflx_chol_solve_local(s.plan, nrhs, B_local, ldb, X_local, ldx), "choleskySolveLocal");
+}
 // LAPACK dpocon of the last parallelCholesky() (cflx_chol_rcond, collective).  Returns the estimate of
 // 1 / (||A||_1 ||A^-1||_1); *anorm = ||A||_1 of the padded symmetric input.
 inline double choleskyRcond(double* anorm = nullptr) {

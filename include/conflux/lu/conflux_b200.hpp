@@ -263,6 +263,15 @@ void LU_solve(lu_params<T>& gv, int nrhs, const T* B, int ldb, T* X, int ldx, bo
     else check(cflx_lu_solve(gv.plan, nrhs, B, ldb, X, ldx), "LU_solve");
 }
 
+// Solves A X = B (A^T X = B when transposed) with the factors of the last LU_rep, like ScaLAPACK's pdgetrs, with B and X
+// distributed like A (cflx_lu_solve_local, collective): this rank's row-major shares of gv.Ml x cflx_rhs_local_cols(nrhs,
+// gv.v, gv.Py), leading dimensions ldb / ldx; host or device memory.  B_local is read on layer 0 only (may be null on the
+// other layers), X_local may be null on any rank, and X_local == B_local (with ldx == ldb) solves in place.
+template <class T>
+void LU_solve_local(lu_params<T>& gv, int nrhs, const T* B_local, int ldb, T* X_local, int ldx, bool transposed = false) {
+    check(cflx_lu_solve_local(gv.plan, transposed ? 1 : 0, nrhs, B_local, ldb, X_local, ldx), "LU_solve_local");
+}
+
 // LAPACK dgecon (1-norm) of the last LU_rep on the GPU grid.  Collective.  Returns the estimate of 1 / (||A||_1 ||A^-1||_1)
 // (0 for an exactly singular U); *anorm = ||A||_1 of the padded input.
 template <class T>

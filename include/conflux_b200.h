@@ -104,6 +104,27 @@ int cflx_lu_solve(cflx_lu*, int nrhs, const double* B, int ldb, double* X, int l
 /* COLLECTIVE.  Solves A^T X = B with the factors of the last cflx_lu_factor, on the GPU grid, like LAPACK's getrs with
  * TRANS = 'T'.  Arguments, state rules and caching as cflx_lu_solve. */
 int cflx_lu_solve_trans(cflx_lu*, int nrhs, const double* B, int ldb, double* X, int ldx);
+/* Pure host.  cols_out: the local columns of an M x nrhs right-hand side share (cflx_lu_solve_local,
+ * cflx_chol_solve_local) on any rank of a grid with Py grid columns, v * ceil(ceil(nrhs / v) / Py): lu_params' padding
+ * rule applied to nrhs, so nrhs = M gives the matrix's Nl.  CFLX_ERR_ARG for nrhs, v or Py < 1 or a NULL cols_out. */
+int cflx_rhs_local_cols(int nrhs, int v, int Py, int* cols_out);
+/* COLLECTIVE.  Solves A X = B (trans 0) or A^T X = B (trans 1) with the factors of the last cflx_lu_factor, like
+ * ScaLAPACK's pdgetrs, with B and X distributed like A: M x nrhs matrices (M the padded size) tiled v x v, global tile
+ * (I, J) on grid position (I % Px, J % Py) at local tile (I / Px, J / Py) of this rank's row-major share of Ml x
+ * cflx_rhs_local_cols(nrhs, v, Py), leading dimensions ldb / ldx.  With nrhs = M a share has the shape of A's share.
+ * Local columns whose global index is >= nrhs, and the ld padding, are neither read (B) nor written (X).  Shares may be
+ * in host or device memory; device memory must be on this rank's device; a host share goes through one temporary device
+ * share.  B_local is read on layer pk == 0 only and may be NULL on layers pk != 0; X_local may be NULL on any rank; every
+ * layer receives the bits of layer 0.  X_local == B_local (the same host or device pointer) solves in place and needs
+ * ldx == ldb; shares that overlap otherwise are not allowed.  The columns are solved in blocks of the width of
+ * cflx_lu_inverse, each assembled on the device and computed exactly as cflx_lu_solve (or cflx_lu_solve_trans) computes
+ * those columns alone, so device memory is bounded by one block whatever nrhs is.  The matrix solved is the one the
+ * factors represent (the scaled one after cflx_lu_equilibrate), as for cflx_lu_solve.  No singularity check (like getrs).
+ * CFLX_ERR_ARG for trans not 0 / 1, nrhs < 1, ldb (layer 0) or ldx (X set) below the local column count, a NULL B_local
+ * on layer 0, X_local == B_local with ldx != ldb, or device memory of another device.  CFLX_ERR_STATE as cflx_lu_solve.
+ * Every rank passes the same trans and nrhs.  Leaves the factors, the permutation, the input, the scaling record, later
+ * solves and the launch count as they are. */
+int cflx_lu_solve_local(cflx_lu*, int trans, int nrhs, const double* B_local, int ldb, double* X_local, int ldx);
 /* COLLECTIVE.  LAPACK dgecon (NORM = '1') on the GPU grid: rcond_out = 1 / (||A||_1 ||inv(A)||_1) with ||inv(A)||_1
  * estimated by Hager-Higham's method (dlacn2: at most 5 iterations, a few solves with one right-hand side), anorm_out
  * (may be NULL) = ||A||_1 of the padded M x M input.  rcond is 0 when ||A||_1 is 0 or the estimate is not finite (an
@@ -260,6 +281,13 @@ int cflx_chol_validate(cflx_chol*, double* frob_abs_out, double* frob_rel_out);
  * after a factorisation prepares and caches per-rank solve data; cflx_chol_set_local / cflx_chol_factor drop it.  Does not
  * modify the factor or the input. */
 int cflx_chol_solve(cflx_chol*, int nrhs, const double* B, int ldb, double* X, int ldx);
+/* COLLECTIVE.  Solves A X = B with the factor of the last successful cflx_chol_factor, like ScaLAPACK's pdpotrs, with B
+ * and X distributed like A: the layout, memory, layer, in-place and block rules of cflx_lu_solve_local, each block
+ * computed exactly as cflx_chol_solve computes those columns alone.  Only the rows of real tiles (global tile index <
+ * Kappa) are read or written.  The matrix solved is the scaled one after cflx_chol_equilibrate, as for cflx_chol_solve.
+ * CFLX_ERR_ARG as cflx_lu_solve_local (without trans); CFLX_ERR_STATE as cflx_chol_solve.  Every rank passes the same
+ * nrhs.  Side effects as cflx_lu_solve_local. */
+int cflx_chol_solve_local(cflx_chol*, int nrhs, const double* B_local, int ldb, double* X_local, int ldx);
 /* COLLECTIVE.  LAPACK dpocon on the GPU grid: rcond_out = 1 / (||A||_1 ||inv(A)||_1), ||A||_1 of the symmetric input
  * whose lower triangle is stored (anorm_out, may be NULL), ||inv(A)||_1 estimated by Hager-Higham's method with solves.
  * Identical on every rank.  CFLX_ERR_STATE as cflx_chol_solve.  Leaves the factor and any later solve as they are. */
@@ -376,6 +404,16 @@ int cflx_dbg_growth_cols(int mode, int Ml, int Nl, int v, int Kappa, int Px, int
 int cflx_dbg_inverse_share(int mode, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, int M, int c0,
                            int nc, int rows, const double* X, int ldx, const int* perm, double* W_out,
                            double* share_inout, int zero_fill);
+/* the pack and scatter kernels of cflx_lu_solve_local (mode 0) and cflx_chol_solve_local (mode 1) on one right-hand side
+ * share at grid position (pi, pj) of Px x Py (Ml rows, a multiple of v; M >= (Ml / v) Px v global rows; Kappa: the real
+ * tiles of mode 1), for the block of w columns from global column c0 of an M x nrhs matrix (c0 + w <= nrhs).  The rows
+ * are every local row (mode 0) or those of real tiles (mode 1).  Each output may be NULL:
+ *   Bk_out (M x ldn, ldn = w rounded up to a multiple of 8): the pack of B (Ml x ldb, ldb >= cflx_rhs_local_cols), the
+ *   share's entries of the block by global row, zero elsewhere;
+ *   X_inout (Ml x ldx, ldx >= cflx_rhs_local_cols): Xk (M x ldn, by global row) scattered into the share's columns of
+ *   the block.  Every other entry keeps its value. */
+int cflx_dbg_solve_local_share(int mode, int Ml, int v, int Kappa, int Px, int Py, int pi, int pj, int M, int nrhs, int c0,
+                               int w, const double* B, int ldb, double* Bk_out, const double* Xk, double* X_inout, int ldx);
 /* the product kernel of cflx_lu_det / cflx_chol_det on host vectors of n doubles: d, and the divisors s1, s2 (may be
  * NULL).  mant_out 2^exp_out = |prod d| (square = 1: its square) divided by |prod s1| and |prod s2| (squared too), in the
  * kernel's fixed order; neg_out: the parity of the negative entries of d, s1 and s2 (0 when square); first_zero_out: 1 +
