@@ -828,6 +828,105 @@ class dbg:
         return Bk, out
 
     @staticmethod
+    def norm_share(mode, A, v, Kappa=None, grid=(1, 1), pos=(0, 0), M=None):
+        """The per-share pass of lu_rcond / cholesky.rcond's 1-norm and of the infinity-norm on one layer-0 share A (Ml x
+        Nl, dbg.equil's layout), before the sum over the grid.  mode "col": the column sums of |a| over every entry;
+        "sym": the column sums of the symmetric matrix stored as the lower triangle of its real tiles (global tile index
+        < Kappa); "row": the row sums.  Returns an M-vector (default M: (Ml / v) Px v) by global index, zero where the
+        share holds nothing."""
+        A = np.ascontiguousarray(A, dtype=np.float64)
+        Ml, Nl = A.shape
+        Px, Py = (int(x) for x in grid)
+        M = int(M) if M is not None else (Ml // v) * Px * v
+        out = np.empty(M)
+        check(lib().cflx_dbg_norm_share({"col": 0, "sym": 1, "row": 2}[mode], Ml, Nl, int(v),
+                                        int(Kappa if Kappa is not None else 1 << 30), Px, Py, int(pos[0]), int(pos[1]), M,
+                                        A.ctypes.data, out.ctypes.data), "dbg_norm_share")
+        return out
+
+    @staticmethod
+    def chol_validate_share(A, v, Kappa, grid=(1, 1), pos=(0, 0), t=0):
+        """cholesky.validate's per-share kernels on one layer-0 share A (Ml x Nl, dbg.equil's layout).  Returns (PT,
+        sumsq): PT (v x (Ml rounded up to even, + 2)) the masked transposed panel of step t as the validation extracts it
+        (NaN where nothing is written, all NaN off grid column t % Py), sumsq the sum of squares of the lower triangle of
+        the real tiles (global row >= column, global row < Kappa v)."""
+        A = np.ascontiguousarray(A, dtype=np.float64)
+        Ml, Nl = A.shape
+        Px, Py = (int(x) for x in grid)
+        PT = np.empty((int(v), Ml + (Ml & 1) + 2))
+        ss = ctypes.c_double()
+        check(lib().cflx_dbg_chol_validate_share(Ml, Nl, int(v), int(Kappa), Px, Py, int(pos[0]), int(pos[1]), A.ctypes.data,
+                                                 int(t), PT.ctypes.data, ctypes.byref(ss)), "dbg_chol_validate_share")
+        return PT, ss.value
+
+    @staticmethod
+    def lu_validate_share(C, v, grid=(1, 1), pos=(0, 0), t=0):
+        """The two extract kernels of step t of lu_validate's sweep on one layer-0 share C of the packed factors (Ml x Nl,
+        dbg.equil's layout), under the sweep's owner guards.  Returns (LT, U): LT (v x (Ml rounded up to even)) the
+        transposed block of unit-lower L in tile column t by local row, U (v x Nl) the block of U in tile row t by local
+        column; NaN where nothing is written."""
+        C = np.ascontiguousarray(C, dtype=np.float64)
+        Ml, Nl = C.shape
+        Px, Py = (int(x) for x in grid)
+        LT, U = np.empty((int(v), Ml + (Ml & 1))), np.empty((int(v), Nl))
+        check(lib().cflx_dbg_lu_validate_share(Ml, Nl, int(v), Px, Py, int(pos[0]), int(pos[1]), C.ctypes.data, int(t),
+                                               LT.ctypes.data, U.ctypes.data), "dbg_lu_validate_share")
+        return LT, U
+
+    @staticmethod
+    def chol_gather_cols(pieces, v, Px, Py, pj, Ml, Nl, gfirst):
+        """The Cholesky trailing update's column-operand gather on one Ml x Nl share at grid column pj of Px x Py, from
+        the Px broadcast pieces of the transposed panel of the global tiles >= gfirst (a list: piece p is v x ld_p, ld_p
+        = grid row p's rows from its first tile >= gfirst on, rounded up to even, >= 2).  Returns Bc (v x Nl): tile t
+        the panel's rows of the global tile of local column tile lj0 + t (lj0: the first with a global index >=
+        gfirst), NaN in the tiles after the last."""
+        flat = np.ascontiguousarray(np.concatenate([np.asarray(p, dtype=np.float64).ravel() for p in pieces]))
+        Bc = np.empty((int(v), int(Nl)))
+        check(lib().cflx_dbg_chol_gather_cols(int(v), int(Px), int(Py), int(pj), int(Ml), int(Nl), int(gfirst),
+                                              flat.ctypes.data, Bc.ctypes.data), "dbg_chol_gather_cols")
+        return Bc
+
+    @staticmethod
+    def refine_assemble(mode, all_chunks, B, grid, v, M, Ml, Nl, nn, tn, nrhs):
+        """The refinement's assembly from the partials of the Px x Py x Pz ranks of grid: all_chunks (Px Py Pz chunks in
+        rank order, each ((nn ? Ml : 0) + (tn ? Nl : 0)) x 2 ldn) and B (M x ldn).  mode "gerfs": (R, ratio, W) as
+        lu_refine assembles them; "lin_berr": (R, ratio, Q) as refine_x's backward error; "x": R = b - the double-double
+        sum of the (Hi, Lo) partials, rounded once.  Returns a dict of M x ldn arrays (NaN past column nrhs)."""
+        m = {"gerfs": 0, "lin_berr": 1, "x": 2}[mode]
+        Px, Py, Pz = (int(x) for x in grid)
+        B = np.ascontiguousarray(B, dtype=np.float64)
+        ldn = B.shape[1]
+        flat = np.ascontiguousarray(np.asarray(all_chunks, dtype=np.float64).ravel())
+        out = {k: np.empty((int(M), ldn)) for k in ("R", "ratio", "W", "Q")}
+        check(lib().cflx_dbg_refine_assemble(m, Px, Py, Pz, int(v), int(M), int(Ml), int(Nl), int(bool(nn)), int(bool(tn)),
+                                             int(nrhs), ldn, flat.ctypes.data, B.ctypes.data, out["R"].ctypes.data,
+                                             out["ratio"].ctypes.data, out["W"].ctypes.data, out["Q"].ctypes.data),
+              "dbg_refine_assemble")
+        return out
+
+    @staticmethod
+    def refine_columns(A, D, sel, nrhs, d=None, T=None):
+        """The refinement's per-column steps on M x ldn arrays A and D (first nrhs columns) with the per-column selector
+        sel (ldn ints).  Returns dict(max, stats, select, add, Y, T): column maxima of A (NaN wins); nrhs x 5 statistics of
+        y = A, dy = D, scales d (None: ones); A where sel, else 0; A + D where sel; and (Y, T) = (A, T) updated by D with
+        how = sel (1 plain, 2 dla_wwaddw, 0 none; T default zeros)."""
+        A = np.ascontiguousarray(A, dtype=np.float64)
+        D = np.ascontiguousarray(D, dtype=np.float64)
+        M, ldn = A.shape
+        sel = np.ascontiguousarray(sel, dtype=np.int32)
+        dd = np.ascontiguousarray(d, dtype=np.float64) if d is not None else None
+        Tio = np.array(np.zeros_like(A) if T is None else T, dtype=np.float64, order="C")
+        out = dict(max=np.empty(nrhs), stats=np.empty((nrhs, 5)), select=np.empty_like(A), add=np.empty_like(A),
+                   Y=np.empty_like(A))
+        check(lib().cflx_dbg_refine_columns(M, ldn, int(nrhs), A.ctypes.data, D.ctypes.data,
+                                            dd.ctypes.data if dd is not None else None, sel.ctypes.data,
+                                            out["max"].ctypes.data, out["stats"].ctypes.data, out["select"].ctypes.data,
+                                            out["add"].ctypes.data, out["Y"].ctypes.data, Tio.ctypes.data),
+              "dbg_refine_columns")
+        out["T"] = Tio
+        return out
+
+    @staticmethod
     def det(d, s1=None, s2=None, square=False):
         """The product kernel of lu_det / cholesky.det on a host vector d (and divisors s1, s2 of its length): returns
         dict(mantissa, exponent, neg, first_zero, nonfinite) with mantissa * 2**exponent = |prod d| (squared when square)

@@ -289,14 +289,16 @@ __global__ void gather_cols_kernel(GatherArgs a) {
     double* dst = a.Bc + (int64_t)c * a.ldb + (int64_t)t * a.v;
     for (int x = threadIdx.x; x < a.v; x += blockDim.x) dst[x] = src[x];
 }
-// sum of squares of the lower triangle (global row >= global column) of a local block-cyclic array: partials[blockIdx.x]
-// = this CTA's share; launch_sum_partials then adds them in index order, so every call rounds the same way
+// sum of squares of the lower triangle of the real tiles (global row >= global column, global row < Nt v: the column
+// is then below that bound too) of a local block-cyclic array: partials[blockIdx.x] = this CTA's share;
+// launch_sum_partials then adds them in index order, so every call rounds the same way
 __global__ void sumsq_lower_kernel(const double* __restrict__ X, Layout L, double* __restrict__ partials) {
     double s = 0.0;
-    const int64_t total = (int64_t)L.Ml * L.Nl;
+    const int64_t total = (int64_t)L.Ml * L.Nl, nreal = (int64_t)L.Nt * L.v;
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
         const int lr = (int)(e / L.Nl), lc = (int)(e % L.Nl);
-        if (L.row<int64_t>(lr) >= L.col<int64_t>(lc)) s = fma(X[e], X[e], s);
+        const int64_t gr = L.row<int64_t>(lr);
+        if (gr < nreal && gr >= L.col<int64_t>(lc)) s = fma(X[e], X[e], s);
     }
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
     __shared__ double w[32];
@@ -357,10 +359,7 @@ void free_chol(cflx_chol* ch) {
 // Broadcast the Px pieces of the (transposed) panel of column block t to every rank and apply
 //   X[i][j] -= L[i][t] * L[j][t]^T   to the local tiles with global tile row i >= tile column j >= jmin (lower triangle),
 // each z layer with its own slab of the v contraction indices.  piece_rows0(p) = first local row of piece p.
-int piece_ld(const cflx_chol* ch, int gfirst, int p) {  // leading dimension of piece p: its active rows, even, >= 2
-    const int rows = ch->Ml - first_local_tile(gfirst, p, ch->Px) * ch->v;
-    return (int)std::max<int64_t>(2, round_up(std::max(rows, 0), 2));
-}
+int piece_ld(const cflx_chol* ch, int gfirst, int p) { return chol_piece_ld(*ch, gfirst, p); }
 // Broadcast the Px pieces of the (transposed) panel of column block t (rows of global tiles >= gfirst) to every rank into
 // buffer set `buf`, and assemble the column operand for the local column tiles with global index >= jmin.
 int broadcast_pieces(cflx_chol* ch, int t, int gfirst, int jmin, int buf, cudaStream_t s) {
@@ -386,9 +385,7 @@ int broadcast_pieces(cflx_chol* ch, int t, int gfirst, int jmin, int buf, cudaSt
     const int lj0 = first_local_tile(jmin, ch->pj, Py);
     const int ntc = Nl / v - lj0;
     if (ntc <= 0) return CFLX_OK;
-    GatherArgs ga{G, piece_stride, Bc, ch->ldb, v, Px, Py, ch->pj, lj0, ntc, gfirst, Ml};
-    gather_cols_kernel<<<dim3(ntc, v), 128, 0, s>>>(ga);
-    CFLX_CUDA(cudaGetLastError());
+    CFLX_TRY(launch_gather_cols(G, piece_stride, Bc, ch->ldb, v, Px, Py, ch->pj, lj0, ntc, gfirst, Ml, s));
     ch->launches++;
     return CFLX_OK;
 }
@@ -535,6 +532,29 @@ int potrf_tile(double* D, double* A00, double* Q, int* info, int col0, int v, cu
     tri_clean_kernel<<<(v * v + 255) / 256, 256, 0, s>>>(D, A00, v);
     CFLX_CUDA(cudaGetLastError());
     ++*launches;
+    return CFLX_OK;
+}
+
+int launch_gather_cols(const double* G, int64_t piece_stride, double* Bc, int64_t ldb, int v, int Px, int Py, int pj,
+                       int lj0, int ntiles, int gfirst, int Ml, cudaStream_t s) {
+    GatherArgs ga{G, piece_stride, Bc, ldb, v, Px, Py, pj, lj0, ntiles, gfirst, Ml};
+    gather_cols_kernel<<<dim3(ntiles, v), 128, 0, s>>>(ga);
+    CFLX_CUDA(cudaGetLastError());
+    return CFLX_OK;
+}
+
+int launch_sumsq_lower(const double* X, const Layout& L, double* partials, double* out, cudaStream_t s) {
+    sumsq_lower_kernel<<<SUMSQ_PARTIALS, 256, 0, s>>>(X, L, partials);
+    CFLX_CUDA(cudaGetLastError());
+    return launch_sum_partials(partials, SUMSQ_PARTIALS, out, s);
+}
+
+int launch_extract_l_panel_T(const double* A, int64_t lda, int row0, int col0, int n, const Layout& L, int t, double* PT,
+                             int64_t ldp, cudaStream_t s) {
+    if (n <= 0) return CFLX_OK;
+    dim3 grid((n + 31) / 32, (L.v + 31) / 32), block(32, 8);
+    extract_l_panel_T_kernel<<<grid, block, 0, s>>>(A, lda, row0, col0, n, L, t, PT, ldp);
+    CFLX_CUDA(cudaGetLastError());
     return CFLX_OK;
 }
 }  // namespace cflx
@@ -764,7 +784,7 @@ int cflx_chol_create(cflx_comm* c, int N, int v, int Px, int Py, int Pz, cflx_ch
     };
     if ((rc = handle_init(ch, &kCholTexts, c, Px, Py, Pz))) return fail(rc);
     const size_t vv = (size_t)v * v;
-    ch->ldp = round_up(ch->Ml, 2) + 2;
+    ch->ldp = chol_panel_ld(ch->Ml);
     ch->ldb = round_up(ch->Nl, 2) + 2;
 #define ALLOC(ptr, n) if ((rc = dmalloc(&(ptr), (n)))) return fail(rc)
     ALLOC(ch->PT, (size_t)v * ch->ldp); ALLOC(ch->LT, (size_t)v * ch->ldp); ALLOC(ch->W, (size_t)v * ch->ldp);
@@ -908,11 +928,8 @@ int cflx_chol_validate(cflx_chol* ch, double* abs_out, double* rel_out) {
         int rc = CFLX_OK;
         const int pjt = t % Py;
         const int row0 = first_local_tile(t, ch->pi, Px) * v, n0 = Ml - row0;
-        if (ch->pj == pjt && pk_save == 0 && n0 > 0) {
-            dim3 grid((n0 + 31) / 32, (v + 31) / 32), block(32, 8);
-            extract_l_panel_T_kernel<<<grid, block, 0, s>>>(ch->A11, Nl, row0, (t / Py) * v, n0, *ch, t, ch->LT,
-                                                            piece_ld(ch, t, ch->pi));
-        }
+        if (ch->pj == pjt && pk_save == 0)
+            CFLX_TRY(launch_extract_l_panel_T(ch->A11, Nl, row0, (t / Py) * v, n0, *ch, t, ch->LT, piece_ld(ch, t, ch->pi), s));
         // layer 0 applies the whole contraction, the other layers a zero-length slab (they only take part in the broadcasts)
         ch->nlayr = pk_save == 0 ? v : 0;
         ch->pk = 0;
@@ -935,12 +952,8 @@ int cflx_chol_validate(cflx_chol* ch, double* abs_out, double* rel_out) {
     }
     CFLX_CUDA(cudaMemsetAsync(ch->acc, 0, 2 * sizeof(double), s));
     if (pk_save == 0) {   // acc = {the two sums, the per-CTA partials}
-        sumsq_lower_kernel<<<SUMSQ_PARTIALS, 256, 0, s>>>(R, *ch, ch->acc + 2);
-        CFLX_CUDA(cudaGetLastError());
-        CFLX_TRY(launch_sum_partials(ch->acc + 2, SUMSQ_PARTIALS, ch->acc, s));
-        sumsq_lower_kernel<<<SUMSQ_PARTIALS, 256, 0, s>>>(ch->A0, *ch, ch->acc + 2);
-        CFLX_CUDA(cudaGetLastError());
-        CFLX_TRY(launch_sum_partials(ch->acc + 2, SUMSQ_PARTIALS, ch->acc + 1, s));
+        CFLX_TRY(launch_sumsq_lower(R, *ch, ch->acc + 2, ch->acc, s));
+        CFLX_TRY(launch_sumsq_lower(ch->A0, *ch, ch->acc + 2, ch->acc + 1, s));
     }
     if (ch->P > 1) CFLX_NCCL(ncclAllReduce(ch->acc, ch->acc, 2, ncclDouble, ncclSum, c->world, s));
     double h[2] = {0, 0};

@@ -424,6 +424,239 @@ int cflx_dbg_solve_local_share(int mode, int Ml, int v, int Kappa, int Px, int P
     return CFLX_OK;
 }
 
+// the per-share passes of the 1-norm and the infinity-norm (norm.cu) on one layer-0 share at grid position (pi, pj) of
+// Px x Py: mode 0 the column sums, 1 the column sums of the symmetric matrix stored as its lower triangle, 2 the row sums
+int cflx_dbg_norm_share(int mode, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, int M, const double* A,
+                        double* out) {
+    CFLX_TRY(check_device());
+    if (mode < 0 || mode > 2 || Ml < 1 || Nl < 1 || v < 1 || Ml % v || Nl % v || Px < 1 || Py < 1 || pi < 0 || pi >= Px ||
+        pj < 0 || pj >= Py || !A || !out || M < (Ml / v) * Px * v || M < (Nl / v) * Py * v)
+        return CFLX_ERR_ARG;
+    const Layout L{M, v, Kappa, Ml, Nl, Px, Py, pi, pj};
+    const size_t a_n = (size_t)Ml * Nl;
+    int ncp = 0, nrp = 0;
+    norm1_partials(L, &ncp, &nrp);
+    DevBuf dA, dcol, drow, dout;
+    CFLX_TRY(dA.alloc(sizeof(double) * a_n));
+    CFLX_TRY(dcol.alloc(sizeof(double) * ncp * Nl));
+    CFLX_TRY(drow.alloc(sizeof(double) * nrp * Ml));
+    CFLX_TRY(dout.alloc(sizeof(double) * M));
+    CFLX_CUDA(cudaMemcpy(dA.p, A, sizeof(double) * a_n, cudaMemcpyHostToDevice));
+    double* o = dout.as<double>();
+    if (mode == 2) {  // norminf_grid zeroes the vector; the column sums write every entry (NaN shows one they miss)
+        CFLX_CUDA(cudaMemset(o, 0, sizeof(double) * M));
+        CFLX_TRY(launch_norminf_share(dA.as<double>(), L, o, 0));
+    } else {
+        CFLX_TRY(launch_fill(o, M, std::numeric_limits<double>::quiet_NaN(), 0));
+        CFLX_TRY(launch_norm1_share(dA.as<double>(), L, mode == 1, dcol.as<double>(), drow.as<double>(), o, 0));
+    }
+    CFLX_CUDA(cudaMemcpy(out, o, sizeof(double) * M, cudaMemcpyDeviceToHost));
+    CFLX_CUDA(cudaDeviceSynchronize());
+    return CFLX_OK;
+}
+
+// cflx_chol_validate's per-share kernels on one layer-0 share at grid position (pi, pj) of Px x Py (each output may be
+// null): the sum of squares of its lower triangle of the real tiles, and the masked transposed panel of step t
+int cflx_dbg_chol_validate_share(int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, const double* A, int t,
+                                 double* PT_out, double* sumsq_out) {
+    CFLX_TRY(check_device());
+    if (Ml < 1 || Nl < 1 || v < 1 || Ml % v || Nl % v || Kappa < 1 || Px < 1 || Py < 1 || pi < 0 || pi >= Px || pj < 0 ||
+        pj >= Py || !A || t < 0 || t >= Kappa || (t / Py + 1) * v > Nl)
+        return CFLX_ERR_ARG;
+    const int M = std::max((Ml / v) * Px, (Nl / v) * Py) * v;
+    const Layout L{M, v, Kappa, Ml, Nl, Px, Py, pi, pj};
+    const size_t a_n = (size_t)Ml * Nl;
+    const int64_t ldp = chol_panel_ld(Ml);
+    DevBuf dA, dacc, dPT;
+    CFLX_TRY(dA.alloc(sizeof(double) * a_n));
+    CFLX_TRY(dacc.alloc(sizeof(double) * (1 + SUMSQ_PARTIALS)));
+    CFLX_TRY(dPT.alloc(sizeof(double) * v * ldp));
+    CFLX_CUDA(cudaMemcpy(dA.p, A, sizeof(double) * a_n, cudaMemcpyHostToDevice));
+    if (sumsq_out) {
+        double* acc = dacc.as<double>();
+        CFLX_CUDA(cudaMemset(acc, 0, sizeof(double)));
+        CFLX_TRY(launch_sumsq_lower(dA.as<double>(), L, acc + 1, acc, 0));
+        CFLX_CUDA(cudaMemcpy(sumsq_out, acc, sizeof(double), cudaMemcpyDeviceToHost));
+    }
+    if (PT_out) {  // v x chol_panel_ld(Ml); NaN where the kernel writes nothing (and everywhere off grid column t % Py)
+        CFLX_TRY(launch_fill(dPT.as<double>(), v * ldp, std::numeric_limits<double>::quiet_NaN(), 0));
+        const int row0 = first_local_tile(t, pi, Px) * v;
+        if (pj == t % Py)  // the guard and the arguments of cflx_chol_validate
+            CFLX_TRY(launch_extract_l_panel_T(dA.as<double>(), Nl, row0, (t / Py) * v, Ml - row0, L, t, dPT.as<double>(),
+                                              chol_piece_ld(L, t, pi), 0));
+        CFLX_CUDA(cudaMemcpy(PT_out, dPT.p, sizeof(double) * v * ldp, cudaMemcpyDeviceToHost));
+    }
+    CFLX_CUDA(cudaDeviceSynchronize());
+    return CFLX_OK;
+}
+
+// the two extract kernels of cflx_lu_validate's sweep, step t, on one layer-0 share C of the packed factors at grid
+// position (pi, pj) of Px x Py, under the owner guards of the sweep (each output may be null)
+int cflx_dbg_lu_validate_share(int Ml, int Nl, int v, int Px, int Py, int pi, int pj, const double* C, int t, double* LT_out,
+                               double* U_out) {
+    CFLX_TRY(check_device());
+    if (Ml < 1 || Nl < 1 || v < 1 || Ml % v || Nl % v || Px < 1 || Py < 1 || pi < 0 || pi >= Px || pj < 0 || pj >= Py ||
+        !C || t < 0 || (Ml / v) * Px != (Nl / v) * Py)  // the LU's shares of an M x M matrix
+        return CFLX_ERR_ARG;
+    const int M = (Ml / v) * Px * v;
+    if (t >= M / v) return CFLX_ERR_ARG;
+    const Layout L{M, v, M / v, Ml, Nl, Px, Py, pi, pj};
+    const size_t a_n = (size_t)Ml * Nl;
+    const int64_t ldp = round_up(Ml, 2);
+    const double nan = std::numeric_limits<double>::quiet_NaN();
+    DevBuf dC, dLT, dU;
+    CFLX_TRY(dC.alloc(sizeof(double) * a_n));
+    CFLX_TRY(dLT.alloc(sizeof(double) * v * ldp));
+    CFLX_TRY(dU.alloc(sizeof(double) * v * Nl));
+    CFLX_CUDA(cudaMemcpy(dC.p, C, sizeof(double) * a_n, cudaMemcpyHostToDevice));
+    if (LT_out) {  // v x round_up(Ml, 2), NaN where the kernel writes nothing
+        CFLX_TRY(launch_fill(dLT.as<double>(), v * ldp, nan, 0));
+        CFLX_TRY(launch_lu_extract_l(dC.as<double>(), L, t, dLT.as<double>(), ldp, 0));
+        CFLX_CUDA(cudaMemcpy(LT_out, dLT.p, sizeof(double) * v * ldp, cudaMemcpyDeviceToHost));
+    }
+    if (U_out) {  // v x Nl
+        CFLX_TRY(launch_fill(dU.as<double>(), (int64_t)v * Nl, nan, 0));
+        CFLX_TRY(launch_lu_extract_u(dC.as<double>(), L, t, dU.as<double>(), Nl, 0));
+        CFLX_CUDA(cudaMemcpy(U_out, dU.p, sizeof(double) * v * Nl, cudaMemcpyDeviceToHost));
+    }
+    CFLX_CUDA(cudaDeviceSynchronize());
+    return CFLX_OK;
+}
+
+// the Cholesky update's column-operand gather (chol.cu) on one share of Ml x Nl at grid column pj of Px x Py, from the
+// Px broadcast pieces of the panel of global tiles >= gfirst (host: piece p is v x chol_piece_ld(p), back to back), for
+// the local column tiles with global index >= gfirst (Bc's tile t: local tile lj0 + t); Bc_out is v x Nl, NaN where
+// nothing is written
+int cflx_dbg_chol_gather_cols(int v, int Px, int Py, int pj, int Ml, int Nl, int gfirst, const double* pieces,
+                              double* Bc_out) {
+    CFLX_TRY(check_device());
+    if (v < 1 || Px < 1 || Py < 1 || pj < 0 || pj >= Py || Ml < 1 || Nl < 1 || Ml % v || Nl % v || gfirst < 0 || !pieces ||
+        !Bc_out)
+        return CFLX_ERR_ARG;
+    const Layout L{0, v, 0, Ml, Nl, Px, Py, 0, pj};  // chol_piece_ld reads Ml, v and Px only
+    const int64_t ldp = chol_panel_ld(Ml), piece_stride = (int64_t)v * ldp, ldb = Nl;
+    const double nan = std::numeric_limits<double>::quiet_NaN();
+    DevBuf dG, dB;
+    CFLX_TRY(dG.alloc(sizeof(double) * Px * piece_stride));
+    CFLX_TRY(dB.alloc(sizeof(double) * v * ldb));
+    CFLX_TRY(launch_fill(dG.as<double>(), Px * piece_stride, nan, 0));
+    CFLX_TRY(launch_fill(dB.as<double>(), v * ldb, nan, 0));
+    size_t off = 0;
+    for (int p = 0; p < Px; ++p) {  // what broadcast_pieces sends: v chol_piece_ld doubles of the pieces with active rows
+        const size_t n = (size_t)v * chol_piece_ld(L, gfirst, p);
+        if (Ml - first_local_tile(gfirst, p, Px) * v > 0)
+            CFLX_CUDA(cudaMemcpy(dG.as<double>() + p * piece_stride, pieces + off, sizeof(double) * n, cudaMemcpyHostToDevice));
+        off += n;
+    }
+    const int lj0 = first_local_tile(gfirst, pj, Py), ntc = Nl / v - lj0;
+    for (int t = 0; t < ntc; ++t) {  // every read of the kernel lies inside the Px piece slots
+        const int j = (lj0 + t) * Py + pj, p = j % Px, first = first_local_tile(gfirst, p, Px);
+        const int64_t ldg = std::max(2, (Ml - first * v + 1) & ~1);
+        if (j / Px < first || p * piece_stride + (v - 1) * ldg + (int64_t)(j / Px - first + 1) * v > Px * piece_stride) {
+            set_last_error("dbg_chol_gather_cols: column tile %d reads outside the pieces", j);
+            return CFLX_ERR_ARG;
+        }
+    }
+    if (ntc > 0)
+        CFLX_TRY(launch_gather_cols(dG.as<double>(), piece_stride, dB.as<double>(), ldb, v, Px, Py, pj, lj0, ntc, gfirst, Ml, 0));
+    CFLX_CUDA(cudaMemcpy(Bc_out, dB.p, sizeof(double) * v * ldb, cudaMemcpyDeviceToHost));
+    CFLX_CUDA(cudaDeviceSynchronize());
+    return CFLX_OK;
+}
+
+// the refinement's assembly (refine.cu) from the host chunks of Px Py Pz ranks: mode 0 dgerfs' R, ratio and W; 1
+// dla_lin_berr's R, ratio and Q; 2 the double-double R.  safe1, safe2 and nz eps are refine_safe's for M.
+int cflx_dbg_refine_assemble(int mode, int Px, int Py, int Pz, int v, int M, int Ml, int Nl, int nn, int tn, int nrhs,
+                             int ldn, const double* all, const double* B, double* R_out, double* ratio_out, double* W_out,
+                             double* Q_out) {
+    CFLX_TRY(check_device());
+    if (mode < 0 || mode > 2 || Px < 1 || Py < 1 || Pz < 1 || v < 1 || M < 1 || Ml < 0 || Nl < 0 || Ml % v || Nl % v ||
+        (!nn && !tn) || nrhs < 1 || ldn < nrhs || !all || !B || (nn && M > (Ml / v) * Px * v) ||
+        (tn && M > (Nl / v) * Py * v))
+        return CFLX_ERR_ARG;
+    const int64_t chunk = (int64_t)((nn ? Ml : 0) + (tn ? Nl : 0)) * 2 * ldn, mat = (int64_t)M * ldn;
+    const int64_t all_n = chunk * Px * Py * Pz;
+    DevBuf dall, dB, dR, dratio, dW, dQ;
+    CFLX_TRY(dall.alloc(sizeof(double) * all_n));
+    for (DevBuf* b : {&dB, &dR, &dratio, &dW, &dQ}) CFLX_TRY(b->alloc(sizeof(double) * mat));
+    CFLX_CUDA(cudaMemcpy(dall.p, all, sizeof(double) * all_n, cudaMemcpyHostToDevice));
+    CFLX_CUDA(cudaMemcpy(dB.p, B, sizeof(double) * mat, cudaMemcpyHostToDevice));
+    const double nan = std::numeric_limits<double>::quiet_NaN();
+    for (DevBuf* b : {&dR, &dratio, &dW, &dQ}) CFLX_TRY(launch_fill(b->as<double>(), mat, nan, 0));
+    double safe1, safe2, nzeps;
+    refine_safe(M, &safe1, &safe2, &nzeps);
+    AssembleArgs a{dall.as<double>(), chunk, Ml, Nl, ldn, nrhs, M, nn != 0, tn != 0, v, Px, Py, Pz, dB.as<double>(),
+                   dR.as<double>(), dratio.as<double>(), mode == 1 ? nullptr : dW.as<double>(), safe1, safe2, nzeps};
+    a.lin_berr = mode == 1;
+    a.Q = mode == 1 ? dQ.as<double>() : nullptr;
+    CFLX_TRY(launch_assemble(a, mode == 2, 0));
+    auto out = [&](double* h, DevBuf& d) -> int {
+        if (h) CFLX_CUDA(cudaMemcpy(h, d.p, sizeof(double) * mat, cudaMemcpyDeviceToHost));
+        return CFLX_OK;
+    };
+    CFLX_TRY(out(R_out, dR));
+    CFLX_TRY(out(ratio_out, dratio));
+    CFLX_TRY(out(W_out, dW));
+    CFLX_TRY(out(Q_out, dQ));
+    CFLX_CUDA(cudaDeviceSynchronize());
+    return CFLX_OK;
+}
+
+// the refinement's per-column steps (refine.cu) on host M x ldn arrays A and D, nrhs columns, sel (ldn ints) the
+// per-column selector; each output may be null: max_out (nrhs) column_max of A; stats_out (nrhs x 5) column_stats of
+// y = A, dy = D (d: M scales or null); select_out select_cols of A; add_out add_cols of D into A; Y_out / T_inout
+// update_x of (A, T_inout) by D with how = sel
+int cflx_dbg_refine_columns(int M, int ldn, int nrhs, const double* A, const double* D, const double* d, const int* sel,
+                            double* max_out, double* stats_out, double* select_out, double* add_out, double* Y_out,
+                            double* T_inout) {
+    CFLX_TRY(check_device());
+    if (M < 1 || nrhs < 1 || ldn < nrhs || !A || ((stats_out || add_out || Y_out) && !D) ||
+        ((select_out || add_out || Y_out) && !sel) || (!Y_out != !T_inout))
+        return CFLX_ERR_ARG;
+    const int64_t mat = (int64_t)M * ldn;
+    DevBuf dA, dD, dd, dsel, dW, dT, dv;
+    CFLX_TRY(dA.alloc(sizeof(double) * mat));
+    CFLX_TRY(dD.alloc(sizeof(double) * mat));
+    CFLX_TRY(dd.alloc(sizeof(double) * M));
+    CFLX_TRY(dsel.alloc(sizeof(int) * ldn));
+    CFLX_TRY(dW.alloc(sizeof(double) * mat));
+    CFLX_TRY(dT.alloc(sizeof(double) * mat));
+    CFLX_TRY(dv.alloc(sizeof(double) * nrhs * REFINE_NSTAT));
+    CFLX_CUDA(cudaMemcpy(dA.p, A, sizeof(double) * mat, cudaMemcpyHostToDevice));
+    if (D) CFLX_CUDA(cudaMemcpy(dD.p, D, sizeof(double) * mat, cudaMemcpyHostToDevice));
+    if (d) CFLX_CUDA(cudaMemcpy(dd.p, d, sizeof(double) * M, cudaMemcpyHostToDevice));
+    if (sel) CFLX_CUDA(cudaMemcpy(dsel.p, sel, sizeof(int) * ldn, cudaMemcpyHostToDevice));
+    const double* a = dA.as<double>();
+    double* w = dW.as<double>();
+    if (max_out) {
+        CFLX_TRY(launch_column_max(a, M, ldn, nrhs, dv.as<double>(), 0));
+        CFLX_CUDA(cudaMemcpy(max_out, dv.p, sizeof(double) * nrhs, cudaMemcpyDeviceToHost));
+    }
+    if (stats_out) {
+        CFLX_TRY(launch_column_stats(a, dD.as<double>(), d ? dd.as<double>() : nullptr, M, ldn, nrhs, dv.as<double>(), 0));
+        CFLX_CUDA(cudaMemcpy(stats_out, dv.p, sizeof(double) * nrhs * REFINE_NSTAT, cudaMemcpyDeviceToHost));
+    }
+    if (select_out) {
+        CFLX_TRY(launch_fill(w, mat, std::numeric_limits<double>::quiet_NaN(), 0));
+        CFLX_TRY(launch_select_cols(a, dsel.as<int>(), M, ldn, w, 0));
+        CFLX_CUDA(cudaMemcpy(select_out, w, sizeof(double) * mat, cudaMemcpyDeviceToHost));
+    }
+    if (add_out) {
+        CFLX_CUDA(cudaMemcpy(w, a, sizeof(double) * mat, cudaMemcpyDeviceToDevice));
+        CFLX_TRY(launch_add_cols(w, dD.as<double>(), dsel.as<int>(), M, ldn, 0));
+        CFLX_CUDA(cudaMemcpy(add_out, w, sizeof(double) * mat, cudaMemcpyDeviceToHost));
+    }
+    if (Y_out) {
+        CFLX_CUDA(cudaMemcpy(w, a, sizeof(double) * mat, cudaMemcpyDeviceToDevice));
+        CFLX_CUDA(cudaMemcpy(dT.p, T_inout, sizeof(double) * mat, cudaMemcpyHostToDevice));
+        CFLX_TRY(launch_update_x(w, dT.as<double>(), dD.as<double>(), dsel.as<int>(), M, ldn, 0));
+        CFLX_CUDA(cudaMemcpy(Y_out, w, sizeof(double) * mat, cudaMemcpyDeviceToHost));
+        CFLX_CUDA(cudaMemcpy(T_inout, dT.p, sizeof(double) * mat, cudaMemcpyDeviceToHost));
+    }
+    CFLX_CUDA(cudaDeviceSynchronize());
+    return CFLX_OK;
+}
+
 // the determinant's product kernel (det.cu) on host vectors
 int cflx_dbg_det(int n, const double* d, const double* s1, const double* s2, int square, double* mant_out,
                  int64_t* exp_out, int* neg_out, int* first_zero_out, int* nonfinite_out) {

@@ -282,6 +282,36 @@ namespace cflx {
 // validate.cu
 int redistribute_pivoted_rows(cflx_lu* lu, const std::vector<int>& hist, bool factors, const double* src, double* dst);
 int lu_residual_grid(cflx_lu* lu, const std::vector<int>& hist, double* abs_out, double* rel_out);
+// Step t of lu_residual_grid's sweep on one layer-0 share C of the packed factors (L's layout, leading dimension Nl), each
+// a no-op on the ranks that do not hold the block:
+//   extract_l (grid column t % Py): LT[c][r] = L(global row of r, t v + c) for the local rows r from the first local tile
+//             row with a global index >= t: the multiplier below the diagonal, 1 on it, 0 above;
+//   extract_u (grid row t % Px): U[r][lc] = U(t v + r, global column of lc) for the local columns lc from the first
+//             local tile column with a global index >= t: the entry on and above the diagonal, 0 below.
+int launch_lu_extract_l(const double* C, const Layout& L, int t, double* LT, int64_t ldp, cudaStream_t s);
+int launch_lu_extract_u(const double* C, const Layout& L, int t, double* U, int64_t ldu, cudaStream_t s);
+
+// The Cholesky panel buffers' leading dimension (LT, PT, W, and the slot of each broadcast piece: a piece stride of
+// v chol_panel_ld), and the leading dimension of piece p of the panel of global tiles >= gfirst: its active rows, even,
+// >= 2 (what is broadcast is v chol_piece_ld doubles)
+inline int64_t chol_panel_ld(int Ml) { return round_up(Ml, 2) + 2; }
+inline int chol_piece_ld(const Layout& L, int gfirst, int p) {
+    const int rows = L.Ml - first_local_tile(gfirst, p, L.Px) * L.v;
+    return (int)std::max<int64_t>(2, round_up(std::max(rows, 0), 2));
+}
+// chol.cu, the kernels of the timed column operand and of cflx_chol_validate.
+//   gather_cols: Bc[c][t v + x] = piece p = j % Px of G (piece p at G + p piece_stride, [v][ld_p] with ld_p its active
+//                rows from global tile gfirst on, rounded up to even, >= 2) at row (j / Px - first_p) v + x, for the
+//                ntiles local column tiles t from lj0 (global tile j = (lj0 + t) Py + pj)
+//   sumsq_lower: *out += the sum of squares of X's entries in the lower triangle of the real tiles (global row >= global
+//                column, global row < Nt v); partials: SUMSQ_PARTIALS doubles of scratch
+//   extract_l_panel_T: PT[c][r] = A[row0 + r][col0 + c] for r < n, c < v where the global row of local row row0 + r is
+//                >= the global column t v + c, else 0
+int launch_gather_cols(const double* G, int64_t piece_stride, double* Bc, int64_t ldb, int v, int Px, int Py, int pj,
+                       int lj0, int ntiles, int gfirst, int Ml, cudaStream_t s);
+int launch_sumsq_lower(const double* X, const Layout& L, double* partials, double* out, cudaStream_t s);
+int launch_extract_l_panel_T(const double* A, int64_t lda, int row0, int col0, int n, const Layout& L, int t, double* PT,
+                             int64_t ldp, cudaStream_t s);
 
 // solve.cu: the solve engine.  Every function returns CFLX_OK or an error code; all work goes on f.comm->stream.
 void solve_cache_free(SolveCache* sc);
@@ -322,6 +352,15 @@ int estimate_inv_norm1(int n, const std::function<int(int, double*)>& apply, dou
 // lower_sym: only the lower triangle of the real tiles (global tile index < Nt) is stored and the matrix is its symmetric
 // completion; otherwise every local entry of the M x M matrix counts.  Deterministic: no floating-point atomics.
 int norm1_grid(const Grid& g, const double* A, bool lower_sym, double* anorm);
+// norm1_grid's and norminf_grid's per-share passes on one layer-0 share A (L's layout, M-vectors by global index):
+//   norm1_share: out[g] = this share's part of global column g's sum of |a| (lower_sym as norm1_grid), for every g < M,
+//                from the per-CTA partials colp (ncp x Nl) and, when lower_sym, rowp (nrp x Ml) (norm1_partials)
+//   norminf_share: out[g] = the sum of |a| over this share's row g, for the global rows it holds; out is not written
+//                elsewhere
+void norm1_partials(const Layout& L, int* ncp, int* nrp);
+int launch_norm1_share(const double* A, const Layout& L, bool lower_sym, double* colp, double* rowp, double* out,
+                       cudaStream_t s);
+int launch_norminf_share(const double* A, const Layout& L, double* out, cudaStream_t s);
 // rcond = (1 / ainvnm) / anorm as LAPACK's dgecon / dpocon form it; 0 when anorm is 0 or the estimate is not finite
 double rcond_from(double anorm, double ainvnm);
 
@@ -393,6 +432,38 @@ int launch_residual(ResidMode mode, const double* A, const Layout& L, const doub
 int launch_residual_x(ResidMode mode, const double* A, const Layout& L, const double* Xc, const double* Xct,
                       const double* Xr, const double* Xrt, int64_t ldx, int nrhs, double* Hi, double* Lo, int64_t ldo,
                       cudaStream_t s);
+// The refinement's assembly of the grid's partials (refine.cu).  For global row g (tile T) every rank adds, in this order,
+// the NN partials of the ranks (T % Px, pj, 0), pj ascending, then the TN partials of the ranks (pi, T % Py, 0), pi
+// ascending, each out of its chunk of `all`.
+struct AssembleArgs {
+    const double* all;  // the partials of every world rank, `chunk` doubles apart: rows of 2 ldn (P, then Q)
+    int64_t chunk;
+    int Ml, Nl, ldn, nrhs, M;
+    bool nn, tn;           // which partials a rank holds: NN rows [0, Ml), then TN rows [nn ? Ml : 0, + Nl)
+    int v, Px, Py, Pz;
+    const double* B;       // [M x ldn]
+    double *R, *ratio, *W;  // [M x ldn]: b - op(A) x, the backward-error ratio, dgerfs' w
+    double safe1, safe2, nzeps;
+    bool lin_berr;      // refine_x: ratio = (|r_i| + safe1) / s_i where s_i != 0, else 0 (LAPACK dla_lin_berr); no W
+    double* Q;          // refine_x (may be null): |op(A)| |x|
+};
+// dgerfs' safe1 = (M + 1) safmin, safe2 = safe1 / eps and (M + 1) eps of an order-M system
+void refine_safe(int M, double* safe1, double* safe2, double* nzeps);
+// assemble (extended: the double-double partials, R = b - their sum rounded once; otherwise R, ratio and W or Q)
+int launch_assemble(const AssembleArgs& a, bool extended, cudaStream_t s);
+// The per-column steps on M x ldn arrays, nrhs columns:
+//   column_max:   berr[c] = max over the rows of ratio[:, c] (NaN wins)
+//   column_stats: out[c][0..4] = {max |y|, max |y| d, max |dy| d, max |dy| / |y| (+inf where y = 0 != dy, 0 where
+//                 y = dy = 0), min |y|} (d null: ones; NaN wins)
+//   select_cols:  out[:, c] = active[c] ? in[:, c] : 0;  add_cols: X[:, c] += D[:, c] where active[c]
+//   update_x:     how[c] 1: Y += DY; 2: (Y, T) += DY as LAPACK's dla_wwaddw; 0: nothing
+constexpr int REFINE_NSTAT = 5;
+int launch_column_max(const double* ratio, int M, int ldn, int nrhs, double* berr, cudaStream_t s);
+int launch_column_stats(const double* Y, const double* DY, const double* d, int M, int ldn, int nrhs, double* out,
+                        cudaStream_t s);
+int launch_select_cols(const double* in, const int* active, int M, int ldn, double* out, cudaStream_t s);
+int launch_add_cols(double* X, const double* D, const int* active, int M, int ldn, cudaStream_t s);
+int launch_update_x(double* Y, double* T, const double* DY, const int* how, int M, int ldn, cudaStream_t s);
 // The solve and refinement of cflx_lu_svx / cflx_chol_svx (equil.cu), COLLECTIVE: B (host or device) to the device, its
 // rows scaled by pre (may be null), X = op.solve(false, B), refine_run, the rows of X scaled by post (may be null), X out;
 // when post is not null, ferr is divided by cnd.  Then *info = M + 1 when rcond < 2^-53 (dgesvx / dposvx: the matrix is

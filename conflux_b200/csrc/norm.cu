@@ -109,6 +109,35 @@ __global__ void row_abs_sums_kernel(const double* __restrict__ A, Layout L, doub
 }
 }  // namespace
 
+void norm1_partials(const Layout& L, int* ncp, int* nrp) {
+    *ncp = (L.Ml + NROW - 1) / NROW;
+    *nrp = (L.Nl + NCOL - 1) / NCOL;
+}
+
+int launch_norm1_share(const double* A, const Layout& L, bool lower_sym, double* colp, double* rowp, double* out,
+                       cudaStream_t s) {
+    int ncp = 0, nrp = 0;
+    norm1_partials(L, &ncp, &nrp);
+    const dim3 grid(nrp, ncp);
+    const int fin = (L.M + 255) / 256;
+    if (lower_sym) {
+        abs_sums_kernel<true><<<grid, NCOL, 0, s>>>(A, L, colp, rowp);
+        column_sums_kernel<true><<<fin, 256, 0, s>>>(colp, ncp, rowp, nrp, L, out);
+    } else {
+        abs_sums_kernel<false><<<grid, NCOL, 0, s>>>(A, L, colp, rowp);
+        column_sums_kernel<false><<<fin, 256, 0, s>>>(colp, ncp, rowp, nrp, L, out);
+    }
+    CFLX_CUDA(cudaGetLastError());
+    return CFLX_OK;
+}
+
+int launch_norminf_share(const double* A, const Layout& L, double* out, cudaStream_t s) {
+    if (L.Ml <= 0) return CFLX_OK;
+    row_abs_sums_kernel<<<(L.Ml + 7) / 8, 256, 0, s>>>(A, L, out);
+    CFLX_CUDA(cudaGetLastError());
+    return CFLX_OK;
+}
+
 int norminf_grid(const Grid& g, const double* A, double* anorm) {
     cflx_comm* c = g.comm;
     cudaStream_t s = c->stream;
@@ -118,10 +147,7 @@ int norminf_grid(const Grid& g, const double* A, double* anorm) {
     std::vector<double> h(M);
     auto run = [&]() -> int {
         CFLX_CUDA(cudaMemsetAsync(out, 0, sizeof(double) * M, s));
-        if (g.pk == 0 && g.Ml > 0) {  // only layer 0 holds the input
-            row_abs_sums_kernel<<<(g.Ml + 7) / 8, 256, 0, s>>>(A, g, out);
-            CFLX_CUDA(cudaGetLastError());
-        }
+        if (g.pk == 0) CFLX_TRY(launch_norminf_share(A, g, out, s));  // only layer 0 holds the input
         if (c->world_size > 1) CFLX_NCCL(ncclAllReduce(out, out, (size_t)M, ncclDouble, ncclSum, c->world, s));
         CFLX_CUDA(cudaMemcpyAsync(h.data(), out, sizeof(double) * M, cudaMemcpyDeviceToHost, s));
         CFLX_CUDA(cudaStreamSynchronize(s));
@@ -140,7 +166,8 @@ int norm1_grid(const Grid& g, const double* A, bool lower_sym, double* anorm) {
     cflx_comm* c = g.comm;
     cudaStream_t s = c->stream;
     const int M = g.M, Ml = g.Ml, Nl = g.Nl, pk = g.pk;
-    const int ncp = (Ml + NROW - 1) / NROW, nrp = (Nl + NCOL - 1) / NCOL;
+    int ncp = 0, nrp = 0;
+    norm1_partials(g, &ncp, &nrp);
     double *colp = nullptr, *rowp = nullptr, *out = nullptr;
     int rc = dmalloc(&out, (size_t)M);
     if (!rc && pk == 0) rc = dmalloc(&colp, (size_t)ncp * Nl);
@@ -150,16 +177,7 @@ int norm1_grid(const Grid& g, const double* A, bool lower_sym, double* anorm) {
         if (pk != 0) {  // only layer 0 holds the input
             CFLX_CUDA(cudaMemsetAsync(out, 0, sizeof(double) * M, s));
         } else {
-            const dim3 grid(nrp, ncp);
-            const int fin = (M + 255) / 256;
-            if (lower_sym) {
-                abs_sums_kernel<true><<<grid, NCOL, 0, s>>>(A, g, colp, rowp);
-                column_sums_kernel<true><<<fin, 256, 0, s>>>(colp, ncp, rowp, nrp, g, out);
-            } else {
-                abs_sums_kernel<false><<<grid, NCOL, 0, s>>>(A, g, colp, rowp);
-                column_sums_kernel<false><<<fin, 256, 0, s>>>(colp, ncp, rowp, nrp, g, out);
-            }
-            CFLX_CUDA(cudaGetLastError());
+            CFLX_TRY(launch_norm1_share(A, g, lower_sym, colp, rowp, out, s));
         }
         if (c->world_size > 1) CFLX_NCCL(ncclAllReduce(out, out, (size_t)M, ncclDouble, ncclSum, c->world, s));
         CFLX_CUDA(cudaMemcpyAsync(h.data(), out, sizeof(double) * M, cudaMemcpyDeviceToHost, s));

@@ -457,19 +457,7 @@ int dispatch_x(const ResidXArgs& r, bool tn, cudaStream_t s) {
 }
 
 // ---------------------------------------------------------------- assembly and the per-column backward error
-struct AssembleArgs {
-    const double* all;  // the partials of every world rank, `chunk` doubles apart: rows of 2 ldn (P, then Q)
-    int64_t chunk;
-    int Ml, Nl, ldn, nrhs, M;
-    bool nn, tn;           // which partials a rank holds: NN rows [0, Ml), then TN rows [nn ? Ml : 0, + Nl)
-    int v, Px, Py, Pz;
-    const double* B;       // [M x ldn]
-    double *R, *ratio, *W;  // [M x ldn]: b - op(A) x, the backward-error ratio, dgerfs' w
-    double safe1, safe2, nzeps;
-    bool lin_berr;      // refine_x: ratio = (|r_i| + safe1) / s_i where s_i != 0, else 0 (LAPACK dla_lin_berr); no W
-    double* Q;          // refine_x (may be null): |op(A)| |x|
-};
-
+// (AssembleArgs: lu_state.h)
 // every rank adds the same partials in the same order: for global row g (tile T), the NN partials of the ranks
 // (T % Px, pj, 0), pj ascending, then the TN partials of the ranks (pi, T % Py, 0), pi ascending
 __global__ void assemble_kernel(AssembleArgs a) {
@@ -569,7 +557,7 @@ __global__ void assemble_x_kernel(AssembleArgs a) {
 
 // refine_x's per-column quantities of one round, by a fixed tree: {normy = max |y|, normx = max |y| d, normdx =
 // max |dy| d, dz_z = max |dy| / |y| (+inf where y = 0 != dy), ymin = min |y|} (d null: ones; NaN wins)
-constexpr int NSTAT = 5;
+constexpr int NSTAT = REFINE_NSTAT;
 __global__ void __launch_bounds__(MAXT) column_stats_kernel(const double* __restrict__ Y, const double* __restrict__ DY,
                                                             const double* __restrict__ d, int M, int ldn,
                                                             double* __restrict__ out) {
@@ -629,6 +617,48 @@ int grow(double** p, size_t n, size_t* have) {
     return CFLX_OK;
 }
 }  // namespace
+
+void refine_safe(int M, double* safe1, double* safe2, double* nzeps) {
+    const double eps = std::ldexp(1.0, -53), safmin = std::ldexp(1.0, -1022);
+    const double nz = (double)M + 1.0;
+    *safe1 = nz * safmin;
+    *safe2 = *safe1 / eps;
+    *nzeps = nz * eps;
+}
+int launch_assemble(const AssembleArgs& a, bool extended, cudaStream_t s) {
+    const dim3 grid((unsigned)a.M, (unsigned)((a.nrhs + 127) / 128));
+    if (extended) assemble_x_kernel<<<grid, 128, 0, s>>>(a);
+    else assemble_kernel<<<grid, 128, 0, s>>>(a);
+    CFLX_CUDA(cudaGetLastError());
+    return CFLX_OK;
+}
+int launch_column_max(const double* ratio, int M, int ldn, int nrhs, double* berr, cudaStream_t s) {
+    column_max_kernel<<<nrhs, MAXT, 0, s>>>(ratio, M, ldn, berr);
+    CFLX_CUDA(cudaGetLastError());
+    return CFLX_OK;
+}
+int launch_column_stats(const double* Y, const double* DY, const double* d, int M, int ldn, int nrhs, double* out,
+                        cudaStream_t s) {
+    column_stats_kernel<<<nrhs, MAXT, 0, s>>>(Y, DY, d, M, ldn, out);
+    CFLX_CUDA(cudaGetLastError());
+    return CFLX_OK;
+}
+static unsigned refine_blocks(int M, int ldn) { return (unsigned)(((size_t)M * ldn + 255) / 256); }
+int launch_select_cols(const double* in, const int* active, int M, int ldn, double* out, cudaStream_t s) {
+    select_cols_kernel<<<refine_blocks(M, ldn), 256, 0, s>>>(in, active, M, ldn, out);
+    CFLX_CUDA(cudaGetLastError());
+    return CFLX_OK;
+}
+int launch_add_cols(double* X, const double* D, const int* active, int M, int ldn, cudaStream_t s) {
+    add_cols_kernel<<<refine_blocks(M, ldn), 256, 0, s>>>(X, D, active, M, ldn);
+    CFLX_CUDA(cudaGetLastError());
+    return CFLX_OK;
+}
+int launch_update_x(double* Y, double* T, const double* DY, const int* how, int M, int ldn, cudaStream_t s) {
+    update_x_kernel<<<refine_blocks(M, ldn), 256, 0, s>>>(Y, T, DY, how, M, ldn);
+    CFLX_CUDA(cudaGetLastError());
+    return CFLX_OK;
+}
 
 int launch_residual(ResidMode mode, const double* A, const Layout& L, const double* Xc, const double* Xr, int64_t ldx,
                     int nrhs, double* P, double* Q, int64_t ldo, cudaStream_t s) {
@@ -845,11 +875,11 @@ struct RefinePass {
                                     cudaMemcpyDefault, s));
         CFLX_CUDA(cudaMemcpy2DAsync(rc->B, ldn * sizeof(double), B, (size_t)ldb * sizeof(double), nrhs * sizeof(double), M,
                                     cudaMemcpyDefault, s));
-        const double eps = std::ldexp(1.0, -53), safmin = std::ldexp(1.0, -1022);
-        const double nz = (double)M + 1.0, safe1 = nz * safmin, safe2 = safe1 / eps;
+        double safe1, safe2, nzeps;
+        refine_safe(M, &safe1, &safe2, &nzeps);
         const double* all = c->world_size > 1 ? rc->all : rc->part;
         aa = AssembleArgs{all, (int64_t)chunk, Ml, Nl, ldn, nrhs, M, nn, tn, G.v, G.Px, G.Py, G.Pz, rc->B, rc->R,
-                          rc->ratio, rc->W, safe1, safe2, nz * eps};
+                          rc->ratio, rc->W, safe1, safe2, nzeps};
         return CFLX_OK;
     }
 
@@ -883,9 +913,8 @@ struct RefinePass {
         AssembleArgs a = aa;
         a.lin_berr = lin_berr;
         a.Q = Q;
-        assemble_kernel<<<dim3((unsigned)op.grid.M, (unsigned)((nrhs + 127) / 128)), 128, 0, s>>>(a);
-        column_max_kernel<<<nrhs, MAXT, 0, s>>>(rc->ratio, op.grid.M, ldn, rc->berr);
-        CFLX_CUDA(cudaGetLastError());
+        CFLX_TRY(launch_assemble(a, false, s));
+        CFLX_TRY(launch_column_max(rc->ratio, op.grid.M, ldn, nrhs, rc->berr, s));
         CFLX_CUDA(cudaMemcpyAsync(berr.data(), rc->berr, sizeof(double) * nrhs, cudaMemcpyDeviceToHost, s));
         CFLX_CUDA(cudaStreamSynchronize(s));
         return CFLX_OK;
@@ -895,17 +924,14 @@ struct RefinePass {
     int run_x() {
         cudaStream_t s = op.grid.comm->stream;
         CFLX_TRY(partials(rc->X, rc->T));
-        assemble_x_kernel<<<dim3((unsigned)op.grid.M, (unsigned)((nrhs + 127) / 128)), 128, 0, s>>>(aa);
-        CFLX_CUDA(cudaGetLastError());
-        return CFLX_OK;
+        return launch_assemble(aa, true, s);
     }
 
     // D = inv(op A) R on the columns where active (the others get 0)
     int correction(const std::vector<int>& active) {
         cudaStream_t s = op.grid.comm->stream;
         CFLX_CUDA(cudaMemcpyAsync(rc->active, active.data(), sizeof(int) * ldn, cudaMemcpyHostToDevice, s));
-        select_cols_kernel<<<blocks(), 256, 0, s>>>(rc->R, rc->active, op.grid.M, ldn, rc->rhs);
-        CFLX_CUDA(cudaGetLastError());
+        CFLX_TRY(launch_select_cols(rc->R, rc->active, op.grid.M, ldn, rc->rhs, s));
         return op.solve(false, nrhs, rc->rhs, ldn, rc->D, ldn);  // synchronises: `active` may change after it
     }
 
@@ -1005,8 +1031,7 @@ int refine_run(RefineCache* rc, const RefineOp& op, int nrhs, const double* B, i
         }
         if (!any) break;
         CFLX_TRY(pass.correction(active));
-        add_cols_kernel<<<pass.blocks(), 256, 0, s>>>(rc->X, rc->D, rc->active, M, ldn);
-        CFLX_CUDA(cudaGetLastError());
+        CFLX_TRY(launch_add_cols(rc->X, rc->D, rc->active, M, ldn, s));
     }
     std::vector<double> hX(mat);
     CFLX_CUDA(cudaMemcpyAsync(hX.data(), rc->X, sizeof(double) * mat, cudaMemcpyDeviceToHost, s));
@@ -1110,14 +1135,12 @@ int refine_x_run(RefineCache* rc, const RefineOp& op, int nrhs, const double* B,
         if (!any) break;
         CFLX_TRY(pass.run_x());
         CFLX_TRY(pass.correction(active));
-        column_stats_kernel<<<nrhs, MAXT, 0, s>>>(rc->X, rc->D, d, M, ldn, rc->stats);
-        CFLX_CUDA(cudaGetLastError());
+        CFLX_TRY(launch_column_stats(rc->X, rc->D, d, M, ldn, nrhs, rc->stats, s));
         CFLX_CUDA(cudaMemcpyAsync(st.data(), rc->stats, sizeof(double) * nrhs * NSTAT, cudaMemcpyDeviceToHost, s));
         CFLX_CUDA(cudaStreamSynchronize(s));
         for (int j = 0; j < nrhs; ++j) how[j] = active[j] ? col[j].round(&st[(size_t)j * NSTAT], rcond, !cwise, cnt, M) : 0;
         CFLX_CUDA(cudaMemcpyAsync(rc->active, how.data(), sizeof(int) * ldn, cudaMemcpyHostToDevice, s));
-        update_x_kernel<<<pass.blocks(), 256, 0, s>>>(rc->X, rc->T, rc->D, rc->active, M, ldn);
-        CFLX_CUDA(cudaGetLastError());
+        CFLX_TRY(launch_update_x(rc->X, rc->T, rc->D, rc->active, M, ldn, s));
     }
     for (RefineXColumn& c : col) c.finish();
 

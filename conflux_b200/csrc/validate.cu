@@ -79,6 +79,24 @@ __global__ void extract_u_block_kernel(const double* __restrict__ C, int64_t ldc
 }
 }  // namespace
 
+int launch_lu_extract_l(const double* C, const Layout& L, int t, double* LT, int64_t ldp, cudaStream_t s) {
+    const int v = L.v, row_lo = std::min(L.Ml, first_local_tile(t, L.pi, L.Px) * v);
+    if (L.pj != t % L.Py || row_lo >= L.Ml) return CFLX_OK;  // the grid column of tile column t holds L's block
+    dim3 grid((L.Ml - row_lo + 31) / 32, (v + 31) / 32), block(32, 8);
+    extract_l_block_T_kernel<<<grid, block, 0, s>>>(C, L.Nl, L, t, (t / L.Py) * v, row_lo, LT, ldp);
+    CFLX_CUDA(cudaGetLastError());
+    return CFLX_OK;
+}
+
+int launch_lu_extract_u(const double* C, const Layout& L, int t, double* U, int64_t ldu, cudaStream_t s) {
+    const int v = L.v, col_lo = std::min(L.Nl, first_local_tile(t, L.pj, L.Py) * v);
+    if (L.pi != t % L.Px || col_lo >= L.Nl) return CFLX_OK;  // the grid row of tile row t holds U's block
+    dim3 grid(std::max(1, std::min(32, (L.Nl - col_lo) / 256)), v);
+    extract_u_block_kernel<<<grid, 256, 0, s>>>(C, L.Nl, L, t, (t / L.Px) * v, col_lo, U, ldu);
+    CFLX_CUDA(cudaGetLastError());
+    return CFLX_OK;
+}
+
 int launch_gather_rows(const double* A, int64_t lda, const int* src_rows, int nrows, int ncols, double* out,
                        cudaStream_t stream) {
     if (nrows <= 0 || ncols <= 0) return CFLX_OK;
@@ -186,13 +204,12 @@ int lu_residual_grid(cflx_lu* lu, const std::vector<int>& hist, double* abs_out,
         return rc;
     }
     const int64_t ldp = lu->ldp_max, ldu = Nl;
+    int krc = CFLX_OK;
     for (int t = 0; t < Nt && !rc; ++t) {
         const int ltr = (t - pi + Px - 1) / Px, ltc = (t - pj + Py - 1) / Py;  // first local tile row / col with global tile >= t
         const int row_lo = std::min(Ml, ltr * v), col_lo = std::min(Nl, ltc * v);
-        if (layer0 && pj == t % Py && row_lo < Ml) {
-            dim3 grid((Ml - row_lo + 31) / 32, (v + 31) / 32), block(32, 8);
-            extract_l_block_T_kernel<<<grid, block, 0, s>>>(lu->Cbuf, Nl, *lu, t, (t / Py) * v, row_lo, lu->PT, ldp);
-        }
+        // a failed extract launch is recorded and the sweep goes on, so that every rank still reaches the broadcasts
+        if (layer0 && !krc) krc = launch_lu_extract_l(lu->Cbuf, *lu, t, lu->PT, ldp, s);
         if (Py * Pz > 1) {
             ncclResult_t r = ncclBroadcast(lu->PT, lu->PT, (size_t)v * ldp, ncclDouble, (t % Py) * Pz, lu->jk_comm.c, s);
             if (r != ncclSuccess) {
@@ -201,10 +218,7 @@ int lu_residual_grid(cflx_lu* lu, const std::vector<int>& hist, double* abs_out,
                 break;
             }
         }
-        if (layer0 && pi == t % Px && col_lo < Nl) {
-            dim3 grid(std::max(1, std::min(32, (Nl - col_lo) / 256)), v);
-            extract_u_block_kernel<<<grid, 256, 0, s>>>(lu->Cbuf, Nl, *lu, t, (t / Px) * v, col_lo, lu->U, ldu);
-        }
+        if (layer0 && !krc) krc = launch_lu_extract_u(lu->Cbuf, *lu, t, lu->U, ldu, s);
         if (Px * Pz > 1) {
             ncclResult_t r = ncclBroadcast(lu->U, lu->U, (size_t)v * ldu, ncclDouble, (t % Px) * Pz, lu->ik_comm.c, s);
             if (r != ncclSuccess) {
@@ -224,6 +238,7 @@ int lu_residual_grid(cflx_lu* lu, const std::vector<int>& hist, double* abs_out,
             rc = launch_gemm_tn(g, s);
         }
     }
+    if (!rc) rc = krc;
     if (!rc && cudaGetLastError() != cudaSuccess) rc = CFLX_ERR_CUDA;
     if (!rc && layer0) {
         rc = launch_sumsq(R, (int64_t)loc, acc, acc + 2, s);

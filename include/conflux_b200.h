@@ -414,6 +414,61 @@ int cflx_dbg_inverse_share(int mode, int Ml, int Nl, int v, int Kappa, int Px, i
  *   the block.  Every other entry keeps its value. */
 int cflx_dbg_solve_local_share(int mode, int Ml, int v, int Kappa, int Px, int Py, int pi, int pj, int M, int nrhs, int c0,
                                int w, const double* B, int ldb, double* Bk_out, const double* Xk, double* X_inout, int ldx);
+/* the per-share pass of cflx_lu_rcond's and cflx_chol_rcond's 1-norm (mode 0: every entry; mode 1: the symmetric matrix
+ * stored as the lower triangle of its real tiles, global tile index < Kappa) and of the infinity-norm (mode 2) on one
+ * layer-0 share A (Ml x Nl row-major, multiples of v, both >= v) at grid position (pi, pj) of Px x Py, before the
+ * all-reduce over the grid.  out (M doubles, M >= (Ml / v) Px v and >= (Nl / v) Py v): by global index, this share's part
+ * of the column sums of |a| (modes 0, 1) or of the row sums (mode 2), zero where it holds nothing. */
+int cflx_dbg_norm_share(int mode, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, int M, const double* A,
+                        double* out);
+/* cflx_chol_validate's per-share kernels on one layer-0 share A (Ml x Nl row-major, multiples of v) at grid position
+ * (pi, pj) of Px x Py, with Kappa real tiles; each output may be NULL:
+ *   sumsq_out: the sum of squares of the entries with global row >= global column and global row < Kappa v;
+ *   PT_out (v x ldp, ldp = Ml rounded up to even, + 2): the transposed panel of step t (0 <= t < Kappa) as the validation
+ *   extracts it on grid column t % Py, PT[c][r] = A[row0 + r][(t / Py) v + c] (row0: the first local row of a tile with a
+ *   global index >= t) where the global row is >= t v + c, else 0; its leading dimension is that of the broadcast piece
+ *   (the active rows rounded up to even, >= 2).  Entries the kernel does not write, and all of PT off that grid column,
+ *   are NaN. */
+int cflx_dbg_chol_validate_share(int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, const double* A, int t,
+                                 double* PT_out, double* sumsq_out);
+/* the two extract kernels of step t of cflx_lu_validate's sweep on one layer-0 share C of the packed factors (Ml x Nl
+ * row-major, multiples of v) at grid position (pi, pj) of Px x Py, under the sweep's owner guards; each output may be
+ * NULL, and entries the kernels do not write are NaN:
+ *   LT_out (v x ldp, ldp = Ml rounded up to even; grid column t % Py): LT[c][r] = the unit lower factor's entry at the
+ *   global row of r and global column t v + c, for the local rows r of tiles with a global index >= t;
+ *   U_out (v x Nl; grid row t % Px): U[r][lc] = the upper factor's entry at global row t v + r and the global column of
+ *   lc, for the local columns lc of tiles with a global index >= t. */
+int cflx_dbg_lu_validate_share(int Ml, int Nl, int v, int Px, int Py, int pi, int pj, const double* C, int t, double* LT_out,
+                               double* U_out);
+/* the column-operand gather of the Cholesky trailing update on one Ml x Nl share (multiples of v) at grid column pj of
+ * Px x Py, from the Px broadcast pieces of the transposed panel of the global tiles >= gfirst: pieces holds piece p as
+ * v x ldp_p row-major, back to back, ldp_p = the rows of grid row p's share from its first tile >= gfirst on, rounded up
+ * to even, >= 2 (what the factorisation broadcasts).  Bc_out (v x Nl): column tile t = the panel's rows of the global
+ * tile of the share's local column tile lj0 + t, lj0 its first with a global index >= gfirst; NaN in the tiles after the
+ * last one. */
+int cflx_dbg_chol_gather_cols(int v, int Px, int Py, int pj, int Ml, int Nl, int gfirst, const double* pieces,
+                              double* Bc_out);
+/* the assembly of the refinement's residual from the partials of the Px x Py x Pz ranks: all holds Px Py Pz chunks in
+ * rank order ((pi Py + pj) Pz + pk), each ((nn ? Ml : 0) + (tn ? Nl : 0)) rows of 2 ldn (P then Q, or Hi then Lo; NN rows
+ * first), of which only the layer-0 chunks are read; B, and each output (may be NULL), M x ldn.  Row g (tile T) adds the
+ * NN partials of ranks (T % Px, pj, 0), pj ascending, then the TN partials of ranks (pi, T % Py, 0), pi ascending.
+ * mode 0 (cflx_*_refine): R = b - p, ratio and W as LAPACK dgerfs; 1 (cflx_*_refine_x): R, ratio as dla_lin_berr and
+ * Q = q; 2 (cflx_*_refine_x): R = b - (the double-double sum of the (Hi, Lo) pairs), rounded once.  Entries outside the
+ * first nrhs columns, and outputs a mode does not write, are NaN. */
+int cflx_dbg_refine_assemble(int mode, int Px, int Py, int Pz, int v, int M, int Ml, int Nl, int nn, int tn, int nrhs,
+                             int ldn, const double* all, const double* B, double* R_out, double* ratio_out, double* W_out,
+                             double* Q_out);
+/* the refinement's per-column steps on M x ldn row-major host arrays A and D (first nrhs columns), sel: ldn ints; each
+ * output may be NULL:
+ *   max_out (nrhs): the maximum of each column of A, NaN wins;
+ *   stats_out (nrhs x 5): {max |y|, max |y| d, max |dy| d, max |dy| / |y| (+inf where y = 0 != dy), min |y|} of y = A,
+ *   dy = D (d: M scales, NULL: ones), NaN wins;
+ *   select_out: A where sel[c] != 0, else 0;  add_out: A + D where sel[c] != 0, else A;
+ *   Y_out, T_inout (both or neither): (A, T) updated by D with how = sel: 1 y += dy, 2 (y, t) += dy as LAPACK
+ *   dla_wwaddw, 0 unchanged. */
+int cflx_dbg_refine_columns(int M, int ldn, int nrhs, const double* A, const double* D, const double* d, const int* sel,
+                            double* max_out, double* stats_out, double* select_out, double* add_out, double* Y_out,
+                            double* T_inout);
 /* the product kernel of cflx_lu_det / cflx_chol_det on host vectors of n doubles: d, and the divisors s1, s2 (may be
  * NULL).  mant_out 2^exp_out = |prod d| (square = 1: its square) divided by |prod s1| and |prod s2| (squared too), in the
  * kernel's fixed order; neg_out: the parity of the negative entries of d, s1 and s2 (0 when square); first_zero_out: 1 +

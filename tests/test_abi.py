@@ -104,3 +104,12 @@ def test_device_entry_points_refuse_without_gpu():
         cb.Comm(1, 0, None, 0)
     with pytest.raises(cb.ConfluxError, match="no CPU fallback"):
         cb.dbg.gemm_tn(np.ones((4, 4)), np.ones((4, 4)))
+    A = np.ones((8, 8))
+    for call in (lambda: cb.dbg.norm_share("sym", A, 4, Kappa=2),
+                 lambda: cb.dbg.chol_validate_share(A, 4, 2),
+                 lambda: cb.dbg.lu_validate_share(A, 4),
+                 lambda: cb.dbg.chol_gather_cols([np.ones((4, 8))], 4, 1, 1, 0, 8, 8, 0),
+                 lambda: cb.dbg.refine_assemble("x", np.zeros((8, 16)), np.zeros((8, 8)), (1, 1, 1), 4, 8, 8, 8, 1, 0, 8),
+                 lambda: cb.dbg.refine_columns(A, A, np.ones(8), 8)):
+        with pytest.raises(cb.ConfluxError, match="no CPU fallback"):
+            call()
