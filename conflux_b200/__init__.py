@@ -13,7 +13,7 @@ import ctypes
 
 import numpy as np
 
-from ._lib import ConfluxError, LIB_PATH, SYMBOLS, check, lib
+from ._lib import ConfluxError, LIB_PATH, SYMBOLS, ShareLayout, check, lib
 
 __all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "residual", "validate", "lu_solve", "lu_rcond", "lu_refine", "lu_refine_x", "lu_equilibrate", "lu_svx", "lu_equilibrate_b", "lu_svxx", "lu_inverse", "lu_det", "rhs_local_cols", "lu_solve_local", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
 
@@ -605,6 +605,24 @@ def chol_auto_grid(P, N):
     return tuple(g)
 
 
+def _ptr(a):
+    return a.ctypes.data if a is not None else None
+
+
+def _tiles(n, v):
+    """whole tiles of v in n; v < 1 is left for the hook to refuse"""
+    return int(n) // max(int(v), 1)
+
+
+def _share(v, Ml, Nl, grid=(1, 1), pos=(0, 0), Kappa=None, M=None):
+    """the cflx_share_layout of an Ml x Nl share at grid position pos of grid = (Px, Py); M defaults to the LU layout's
+    (Ml / v) Px v, Kappa to no padding tiles"""
+    Px, Py = (int(x) for x in grid)
+    M = int(M) if M is not None else _tiles(Ml, v) * Px * int(v)
+    return ShareLayout(M, int(v), int(Kappa if Kappa is not None else 1 << 30), int(Ml), int(Nl), Px, Py, int(pos[0]),
+                       int(pos[1]))
+
+
 class dbg:
     """Single-kernel hooks (tests and micro-benchmarks)."""
 
@@ -707,10 +725,8 @@ class dbg:
         rows = (Ml, Nl, Ml + Nl)[m]
         P, Q = np.empty((rows, nrhs)), np.empty((rows, nrhs))
         ms = ctypes.c_double()
-        ptr = lambda a: a.ctypes.data if a is not None else None
-        check(lib().cflx_dbg_residual(m, Ml, Nl, A.ctypes.data, int(v), int(Kappa if Kappa is not None else 1 << 30),
-                                      int(grid[0]), int(grid[1]), int(pos[0]), int(pos[1]), nrhs, ptr(Xc), ptr(Xr),
-                                      P.ctypes.data, Q.ctypes.data, int(reps), ctypes.byref(ms)), "dbg_residual")
+        check(lib().cflx_dbg_residual(m, _share(v, Ml, Nl, grid, pos, Kappa, M=0), A.ctypes.data, nrhs, _ptr(Xc),
+                                      _ptr(Xr), P.ctypes.data, Q.ctypes.data, int(reps), ctypes.byref(ms)), "dbg_residual")
         return P, Q, ms.value
 
     @staticmethod
@@ -727,11 +743,9 @@ class dbg:
         rows = (Ml, Nl, Ml + Nl)[m]
         H, L = np.empty((rows, nrhs)), np.empty((rows, nrhs))
         ms = ctypes.c_double()
-        ptr = lambda a: a.ctypes.data if a is not None else None
-        check(lib().cflx_dbg_residual_x(m, Ml, Nl, A.ctypes.data, int(v), int(Kappa if Kappa is not None else 1 << 30),
-                                        int(grid[0]), int(grid[1]), int(pos[0]), int(pos[1]), nrhs, ptr(Xc), ptr(Xct),
-                                        ptr(Xr), ptr(Xrt), H.ctypes.data, L.ctypes.data, int(reps), ctypes.byref(ms)),
-              "dbg_residual_x")
+        check(lib().cflx_dbg_residual_x(m, _share(v, Ml, Nl, grid, pos, Kappa, M=0), A.ctypes.data, nrhs, _ptr(Xc),
+                                        _ptr(Xct), _ptr(Xr), _ptr(Xrt), H.ctypes.data, L.ctypes.data, int(reps),
+                                        ctypes.byref(ms)), "dbg_residual_x")
         return H, L, ms.value
 
     @staticmethod
@@ -744,16 +758,14 @@ class dbg:
         over global row <= column, max |a|) over the global columns < ncols (default M), and 1 + the first zero diagonal
         entry (0: none)."""
         A = np.ascontiguousarray(A, dtype=np.float64)
-        Ml, Nl = A.shape
-        Px, Py = (int(x) for x in grid)
-        M = int(M) if M is not None else (Ml // v) * Px * v
+        sh = _share(v, *A.shape, grid, pos, Kappa, M)
+        M = sh.M
         r = np.ascontiguousarray(np.ones(M) if r is None else r, dtype=np.float64)
         c = np.ascontiguousarray(np.ones(M) if c is None else c, dtype=np.float64)
         out = dict(rowmax=np.empty(M), colmax=np.empty(M), diag=np.empty(M), scaled=np.empty_like(A),
                    sym_scaled=np.empty_like(A), growth=np.empty(2))
         zp = ctypes.c_int()
-        check(lib().cflx_dbg_equil(Ml, Nl, int(v), int(Kappa if Kappa is not None else 1 << 30), Px, Py, int(pos[0]),
-                                   int(pos[1]), M, A.ctypes.data, r.ctypes.data, c.ctypes.data, equed.encode(),
+        check(lib().cflx_dbg_equil(sh, A.ctypes.data, r.ctypes.data, c.ctypes.data, equed.encode(),
                                    int(ncols if ncols is not None else M), out["rowmax"].ctypes.data,
                                    out["colmax"].ctypes.data, out["diag"].ctypes.data, out["scaled"].ctypes.data,
                                    out["sym_scaled"].ctypes.data, out["growth"].ctypes.data, ctypes.byref(zp)), "dbg_equil")
@@ -768,14 +780,11 @@ class dbg:
         i <= j; "chol" both over the real tiles' (global tile index < Kappa) rows j <= i < ncols."""
         F = np.ascontiguousarray(F, dtype=np.float64)
         A = np.ascontiguousarray(A, dtype=np.float64)
-        Ml, Nl = A.shape
-        Px, Py = (int(x) for x in grid)
-        M = int(M) if M is not None else (Ml // v) * Px * v
-        amax, fmax = np.empty(M), np.empty(M)
-        check(lib().cflx_dbg_growth_cols({"lu": 0, "chol": 1}[mode], Ml, Nl, int(v),
-                                         int(Kappa if Kappa is not None else 1 << 30), Px, Py, int(pos[0]), int(pos[1]),
-                                         M, int(ncols if ncols is not None else M), F.ctypes.data, A.ctypes.data,
-                                         amax.ctypes.data, fmax.ctypes.data), "dbg_growth_cols")
+        sh = _share(v, *A.shape, grid, pos, Kappa, M)
+        amax, fmax = np.empty(sh.M), np.empty(sh.M)
+        check(lib().cflx_dbg_growth_cols({"lu": 0, "chol": 1}[mode], sh, int(ncols if ncols is not None else sh.M),
+                                         F.ctypes.data, A.ctypes.data, amax.ctypes.data, fmax.ctypes.data),
+              "dbg_growth_cols")
         return amax, fmax
 
     @staticmethod
@@ -788,19 +797,16 @@ class dbg:
         global tile index < Kappa, on and below the diagonal), and with zero_fill ("chol") zeros on every entry the scatter
         never writes.  share is None when X or share is None."""
         m = {"lu": 0, "chol": 1}[mode]
-        Px, Py = (int(x) for x in grid)
         ldn = -(-int(nc) // 8) * 8
         W = np.empty((Ml, ldn))
-        ptr = lambda a: a.ctypes.data if a is not None else None
         out = Xc = pm = None
         if X is not None and share is not None:
             Xc = np.ascontiguousarray(X, dtype=np.float64)
             out = np.array(share, dtype=np.float64, order="C")
             pm = np.ascontiguousarray(perm, dtype=np.int32) if perm is not None else None
-        check(lib().cflx_dbg_inverse_share(m, int(Ml), int(Nl), int(v), int(Kappa if Kappa is not None else 1 << 30), Px, Py,
-                                           int(pos[0]), int(pos[1]), int(M), int(c0), int(nc),
-                                           int(rows if rows is not None else Ml), ptr(Xc),
-                                           Xc.shape[1] if Xc is not None else 0, ptr(pm), W.ctypes.data, ptr(out),
+        check(lib().cflx_dbg_inverse_share(m, _share(v, Ml, Nl, grid, pos, Kappa, M), int(c0), int(nc),
+                                           int(rows if rows is not None else Ml), _ptr(Xc),
+                                           Xc.shape[1] if Xc is not None else 0, _ptr(pm), W.ctypes.data, _ptr(out),
                                            1 if zero_fill else 0), "dbg_inverse_share")
         return W, out
 
@@ -812,7 +818,7 @@ class dbg:
         rhs_local_cols, every local row for "lu", the real tiles' rows, global tile index < Kappa, for "chol"), and a copy
         of X after the scatter of Xk (M x round_up(w, 8), by global row) into it.  Either is None when its inputs are."""
         m = {"lu": 0, "chol": 1}[mode]
-        Px, Py = (int(x) for x in grid)
+        sh = _share(v, Ml, rhs_local_cols(nrhs, v, grid[1]), grid, pos, Kappa, M)
         ldn = -(-int(w) // 8) * 8
         Bc = np.ascontiguousarray(B, dtype=np.float64) if B is not None else None
         Bk = np.empty((int(M), ldn)) if Bc is not None else None
@@ -820,10 +826,8 @@ class dbg:
         if X is not None and Xk is not None:
             Xc = np.ascontiguousarray(Xk, dtype=np.float64)
             out = np.array(X, dtype=np.float64, order="C")
-        ptr = lambda a: a.ctypes.data if a is not None else None  # noqa: E731
-        check(lib().cflx_dbg_solve_local_share(m, int(Ml), int(v), int(Kappa if Kappa is not None else 1 << 30), Px, Py,
-                                               int(pos[0]), int(pos[1]), int(M), int(nrhs), int(c0), int(w), ptr(Bc),
-                                               Bc.shape[1] if Bc is not None else 0, ptr(Bk), ptr(Xc), ptr(out),
+        check(lib().cflx_dbg_solve_local_share(m, sh, int(nrhs), int(c0), int(w), _ptr(Bc),
+                                               Bc.shape[1] if Bc is not None else 0, _ptr(Bk), _ptr(Xc), _ptr(out),
                                                out.shape[1] if out is not None else 0), "dbg_solve_local_share")
         return Bk, out
 
@@ -835,13 +839,10 @@ class dbg:
         < Kappa); "row": the row sums.  Returns an M-vector (default M: (Ml / v) Px v) by global index, zero where the
         share holds nothing."""
         A = np.ascontiguousarray(A, dtype=np.float64)
-        Ml, Nl = A.shape
-        Px, Py = (int(x) for x in grid)
-        M = int(M) if M is not None else (Ml // v) * Px * v
-        out = np.empty(M)
-        check(lib().cflx_dbg_norm_share({"col": 0, "sym": 1, "row": 2}[mode], Ml, Nl, int(v),
-                                        int(Kappa if Kappa is not None else 1 << 30), Px, Py, int(pos[0]), int(pos[1]), M,
-                                        A.ctypes.data, out.ctypes.data), "dbg_norm_share")
+        sh = _share(v, *A.shape, grid, pos, Kappa, M)
+        out = np.empty(sh.M)
+        check(lib().cflx_dbg_norm_share({"col": 0, "sym": 1, "row": 2}[mode], sh, A.ctypes.data, out.ctypes.data),
+              "dbg_norm_share")
         return out
 
     @staticmethod
@@ -852,11 +853,11 @@ class dbg:
         the real tiles (global row >= column, global row < Kappa v)."""
         A = np.ascontiguousarray(A, dtype=np.float64)
         Ml, Nl = A.shape
-        Px, Py = (int(x) for x in grid)
+        M = max(_tiles(Ml, v) * int(grid[0]), _tiles(Nl, v) * int(grid[1])) * int(v)
         PT = np.empty((int(v), Ml + (Ml & 1) + 2))
         ss = ctypes.c_double()
-        check(lib().cflx_dbg_chol_validate_share(Ml, Nl, int(v), int(Kappa), Px, Py, int(pos[0]), int(pos[1]), A.ctypes.data,
-                                                 int(t), PT.ctypes.data, ctypes.byref(ss)), "dbg_chol_validate_share")
+        check(lib().cflx_dbg_chol_validate_share(_share(v, Ml, Nl, grid, pos, Kappa, M), A.ctypes.data, int(t),
+                                                 PT.ctypes.data, ctypes.byref(ss)), "dbg_chol_validate_share")
         return PT, ss.value
 
     @staticmethod
@@ -867,9 +868,9 @@ class dbg:
         column; NaN where nothing is written."""
         C = np.ascontiguousarray(C, dtype=np.float64)
         Ml, Nl = C.shape
-        Px, Py = (int(x) for x in grid)
         LT, U = np.empty((int(v), Ml + (Ml & 1))), np.empty((int(v), Nl))
-        check(lib().cflx_dbg_lu_validate_share(Ml, Nl, int(v), Px, Py, int(pos[0]), int(pos[1]), C.ctypes.data, int(t),
+        sh = _share(v, Ml, Nl, grid, pos, _tiles(Ml, v) * int(grid[0]))           # Kappa = M / v
+        check(lib().cflx_dbg_lu_validate_share(sh, C.ctypes.data, int(t),
                                                LT.ctypes.data, U.ctypes.data), "dbg_lu_validate_share")
         return LT, U
 
@@ -882,7 +883,7 @@ class dbg:
         gfirst), NaN in the tiles after the last."""
         flat = np.ascontiguousarray(np.concatenate([np.asarray(p, dtype=np.float64).ravel() for p in pieces]))
         Bc = np.empty((int(v), int(Nl)))
-        check(lib().cflx_dbg_chol_gather_cols(int(v), int(Px), int(Py), int(pj), int(Ml), int(Nl), int(gfirst),
+        check(lib().cflx_dbg_chol_gather_cols(_share(v, Ml, Nl, (Px, Py), (0, pj), Kappa=0, M=0), int(gfirst),
                                               flat.ctypes.data, Bc.ctypes.data), "dbg_chol_gather_cols")
         return Bc
 
@@ -940,8 +941,7 @@ class dbg:
             if s is not None and s.size != n:
                 raise ValueError(f"dbg.det: a divisor must have {n} entries, got {s.size}")
         mant, exp, neg, fz, nf = ctypes.c_double(), ctypes.c_int64(), ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
-        ptr = lambda a: a.ctypes.data if a is not None else None  # noqa: E731
-        check(lib().cflx_dbg_det(n, d.ctypes.data, ptr(s1), ptr(s2), 1 if square else 0, ctypes.byref(mant),
+        check(lib().cflx_dbg_det(n, d.ctypes.data, _ptr(s1), _ptr(s2), 1 if square else 0, ctypes.byref(mant),
                                  ctypes.byref(exp), ctypes.byref(neg), ctypes.byref(fz), ctypes.byref(nf)), "dbg_det")
         return dict(mantissa=mant.value, exponent=exp.value, neg=neg.value, first_zero=fz.value, nonfinite=nf.value)
 
@@ -1019,10 +1019,9 @@ class dbg:
         ea = np.zeros(Ma, dtype=np.int32) if want_planes else None
         eb = np.zeros(Nb, dtype=np.int32) if want_planes else None
         ms, sms = ctypes.c_double(), ctypes.c_double()
-        ptr = lambda a: a.ctypes.data if a is not None else None
-        check(lib().cflx_dbg_ozaki_gemm(M, N, K, int(row0), int(col0), int(max_ctas), AT.ctypes.data, B.ctypes.data, ptr(Cp),
-                                        D.ctypes.data, ptr(pa), ptr(pb), ptr(ea), ptr(eb), int(reps), ctypes.byref(ms),
-                                        ctypes.byref(sms)), "dbg_ozaki_gemm")
+        check(lib().cflx_dbg_ozaki_gemm(M, N, K, int(row0), int(col0), int(max_ctas), AT.ctypes.data, B.ctypes.data,
+                                        _ptr(Cp), D.ctypes.data, _ptr(pa), _ptr(pb), _ptr(ea), _ptr(eb), int(reps),
+                                        ctypes.byref(ms), ctypes.byref(sms)), "dbg_ozaki_gemm")
         return dict(D=D, ms=ms.value, split_ms=sms.value, pa=pa, pb=pb, ea=ea, eb=eb)
 
     @staticmethod

@@ -17,6 +17,11 @@ class ConfluxError(RuntimeError):
     pass
 
 
+class ShareLayout(ctypes.Structure):
+    """cflx_share_layout: one rank's Ml x Nl share of the block-cyclic matrix (see include/conflux_b200.h)"""
+    _fields_ = [(f, ctypes.c_int) for f in ("M", "v", "Kappa", "Ml", "Nl", "Px", "Py", "pi", "pj")]
+
+
 # every exported symbol of include/conflux_b200.h (checked by tests/test_abi.py)
 SYMBOLS = [
     "cflx_last_error", "cflx_version", "cflx_device_count", "cflx_get_unique_id", "cflx_comm_create",
@@ -138,21 +143,22 @@ def lib():
             ctypes.c_void_p, ctypes.c_int, c_double_p]
         L.cflx_dbg_gemm_narrow_tn.argtypes = [ctypes.c_int] * 3 + [ctypes.c_void_p] * 3 + [ctypes.c_double] * 2 + [
             ctypes.c_void_p, ctypes.c_int, c_double_p]
-        L.cflx_dbg_residual.argtypes = [ctypes.c_int] * 3 + [ctypes.c_void_p] + [ctypes.c_int] * 7 + [ctypes.c_void_p] * 4 + [
+        share = ctypes.POINTER(ShareLayout)
+        L.cflx_dbg_residual.argtypes = [ctypes.c_int, share, ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 4 + [
             ctypes.c_int, c_double_p]
-        L.cflx_dbg_residual_x.argtypes = [ctypes.c_int] * 3 + [ctypes.c_void_p] + [ctypes.c_int] * 7 + [ctypes.c_void_p] * 6 + [
-            ctypes.c_int, c_double_p]
-        L.cflx_dbg_equil.argtypes = [ctypes.c_int] * 9 + [ctypes.c_void_p] * 3 + [ctypes.c_char, ctypes.c_int] + [
+        L.cflx_dbg_residual_x.argtypes = [ctypes.c_int, share, ctypes.c_void_p, ctypes.c_int] + [
+            ctypes.c_void_p] * 6 + [ctypes.c_int, c_double_p]
+        L.cflx_dbg_equil.argtypes = [share] + [ctypes.c_void_p] * 3 + [ctypes.c_char, ctypes.c_int] + [
             ctypes.c_void_p] * 7
-        L.cflx_dbg_growth_cols.argtypes = [ctypes.c_int] * 11 + [ctypes.c_void_p] * 4
-        L.cflx_dbg_inverse_share.argtypes = [ctypes.c_int] * 13 + [ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 3 + [
-            ctypes.c_int]
-        L.cflx_dbg_solve_local_share.argtypes = [ctypes.c_int] * 12 + [ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 3 + [
-            ctypes.c_int]
-        L.cflx_dbg_norm_share.argtypes = [ctypes.c_int] * 10 + [ctypes.c_void_p] * 2
-        L.cflx_dbg_chol_validate_share.argtypes = [ctypes.c_int] * 8 + [ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 2
-        L.cflx_dbg_lu_validate_share.argtypes = [ctypes.c_int] * 7 + [ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 2
-        L.cflx_dbg_chol_gather_cols.argtypes = [ctypes.c_int] * 7 + [ctypes.c_void_p] * 2
+        L.cflx_dbg_growth_cols.argtypes = [ctypes.c_int, share, ctypes.c_int] + [ctypes.c_void_p] * 4
+        L.cflx_dbg_inverse_share.argtypes = [ctypes.c_int, share] + [ctypes.c_int] * 3 + [
+            ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 3 + [ctypes.c_int]
+        L.cflx_dbg_solve_local_share.argtypes = [ctypes.c_int, share] + [ctypes.c_int] * 3 + [
+            ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 3 + [ctypes.c_int]
+        L.cflx_dbg_norm_share.argtypes = [ctypes.c_int, share] + [ctypes.c_void_p] * 2
+        L.cflx_dbg_chol_validate_share.argtypes = [share, ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 2
+        L.cflx_dbg_lu_validate_share.argtypes = [share, ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 2
+        L.cflx_dbg_chol_gather_cols.argtypes = [share, ctypes.c_int] + [ctypes.c_void_p] * 2
         L.cflx_dbg_refine_assemble.argtypes = [ctypes.c_int] * 12 + [ctypes.c_void_p] * 6
         L.cflx_dbg_refine_columns.argtypes = [ctypes.c_int] * 3 + [ctypes.c_void_p] * 10
         L.cflx_dbg_det.argtypes = [ctypes.c_int] + [ctypes.c_void_p] * 3 + [ctypes.c_int] + [ctypes.c_void_p] * 5

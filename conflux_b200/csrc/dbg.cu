@@ -24,6 +24,48 @@ int check_device() {
     return CFLX_OK;
 }
 
+// a refused call of hook `who`: the error names the hook and the condition that failed
+int refuse(const char* who, const char* what, int status = CFLX_ERR_ARG) {
+    set_last_error("%s: refused, %s", who, what);
+    return status;
+}
+#define REFUSE_IF(cond) do { if (cond) return refuse(__func__, #cond); } while (0)
+
+// the conditions on a cflx_share_layout that differ between hooks (see the header)
+enum : unsigned { TILED = 1, COVERED = 2, NONEMPTY = 4 };
+
+// *L = the share *s describes, or the refusal of hook `who` naming the first condition it fails: those of every share,
+// then those `need` adds
+int share_layout(const char* who, const cflx_share_layout* s, unsigned need, Layout* L) {
+    if (!s) return refuse(who, "no share layout");
+    const auto [M, v, Kappa, Ml, Nl, Px, Py, pi, pj] = *s;
+    if (v < 1) return refuse(who, "v < 1");
+    if (Px < 1 || Py < 1) return refuse(who, "Px or Py < 1");
+    if (pi < 0 || pi >= Px) return refuse(who, "pi outside [0, Px)");
+    if (pj < 0 || pj >= Py) return refuse(who, "pj outside [0, Py)");
+    if (Ml < 0 || Nl < 0) return refuse(who, "Ml or Nl < 0");
+    if ((need & NONEMPTY) && (Ml < 1 || Nl < 1)) return refuse(who, "Ml or Nl < 1");
+    if ((need & TILED) && (Ml % v || Nl % v)) return refuse(who, "Ml or Nl not a multiple of v");
+    if ((need & COVERED) && (M < (Ml / v) * Px * v || M < (Nl / v) * Py * v))
+        return refuse(who, "M < (Ml / v) Px v or M < (Nl / v) Py v");
+    *L = Layout{M, v, Kappa, Ml, Nl, Px, Py, pi, pj};
+    return CFLX_OK;
+}
+
+// d = a device buffer of n T (with DevBuf's tail pad) holding the host array h, or uninitialised when h is null
+template <class T = double>
+int stage(DevBuf& d, size_t n, const T* h = nullptr) {
+    CFLX_TRY(d.alloc(sizeof(T) * n));
+    if (h) CFLX_CUDA(cudaMemcpy(d.p, h, sizeof(T) * n, cudaMemcpyHostToDevice));
+    return CFLX_OK;
+}
+// h = the first n T of the device array d, when h is not null
+template <class T>
+int fetch(T* h, const void* d, size_t n) {
+    if (h) CFLX_CUDA(cudaMemcpy(h, d, sizeof(T) * n, cudaMemcpyDeviceToHost));
+    return CFLX_OK;
+}
+
 // *ms_out (may be null) = the mean device time of `reps` (at least 1) back-to-back calls of run() on the default
 // stream, after one warm-up call
 template <class Run>
@@ -39,6 +81,50 @@ int time_reps(Run&& run, int reps, double* ms_out) {
     float ms = 0;
     CFLX_CUDA(cudaEventElapsedTime(&ms, ev[0], ev[1]));
     if (ms_out) *ms_out = ms / reps;
+    return CFLX_OK;
+}
+
+// a residual kernel (refine.cu) on the share A of layout L: launch(mode, A, Xc, Xr, P, Q) runs it on the device copies
+// of A, Xc (Nl x nrhs) and Xr (Ml x nrhs).  The timed repetitions run first, then the launch whose result is returned,
+// into zeroed outputs of rows x nrhs (Ml, Nl or Ml + Nl rows by mode).
+template <class Launch>
+int residual_run(int mode, const Layout& L, const double* A, int nrhs, const double* Xc, const double* Xr, double* P_out,
+                 double* Q_out, int reps, double* ms_out, Launch&& launch) {
+    const ResidMode m = mode == 0 ? ResidMode::NN : mode == 1 ? ResidMode::TN : ResidMode::SymLower;
+    const int rows = mode == 0 ? L.Ml : mode == 1 ? L.Nl : L.Ml + L.Nl;
+    const size_t o_n = (size_t)std::max(rows, 1) * nrhs;
+    DevBuf dA, dXc, dXr, dP, dQ;
+    CFLX_TRY(stage(dA, (size_t)L.Ml * L.Nl, A));
+    CFLX_TRY(stage(dXc, (size_t)L.Nl * nrhs, Xc));
+    CFLX_TRY(stage(dXr, (size_t)L.Ml * nrhs, Xr));
+    CFLX_TRY(stage(dP, o_n));
+    CFLX_TRY(stage(dQ, o_n));
+    double *p = dP.as<double>(), *q = dQ.as<double>();
+    auto run = [&] { return launch(m, dA.as<double>(), dXc.as<double>(), dXr.as<double>(), p, q); };
+    CFLX_TRY(time_reps(run, reps, ms_out));
+    CFLX_CUDA(cudaMemset(dP.p, 0, sizeof(double) * o_n));
+    CFLX_CUDA(cudaMemset(dQ.p, 0, sizeof(double) * o_n));
+    CFLX_TRY(run());
+    CFLX_TRY(fetch(P_out, dP.p, (size_t)rows * nrhs));
+    CFLX_TRY(fetch(Q_out, dQ.p, (size_t)rows * nrhs));
+    CFLX_CUDA(cudaDeviceSynchronize());
+    return CFLX_OK;
+}
+
+// one of the solve's narrow GEMMs on staged operands: launch(C, D) runs it on the device copy of C (M x N, c_n entries;
+// null: zeros).  The timed repetitions write a separate output; the result is one more launch on the pristine inputs,
+// into C itself when D == C (the kernel with D aliasing C).
+template <class Launch>
+int narrow_gemm(size_t c_n, const double* C, double* D, int reps, double* ms_out, Launch&& launch) {
+    DevBuf dC, dT;
+    CFLX_TRY(stage(dC, c_n, C));
+    CFLX_TRY(stage(dT, c_n));
+    if (!C) CFLX_CUDA(cudaMemset(dC.p, 0, sizeof(double) * c_n));
+    CFLX_TRY(time_reps([&] { return launch(dC.as<double>(), dT.as<double>()); }, reps, ms_out));
+    double* out = C && D == C ? dC.as<double>() : dT.as<double>();
+    CFLX_TRY(launch(dC.as<double>(), out));
+    CFLX_TRY(fetch(D, out, c_n));
+    CFLX_CUDA(cudaDeviceSynchronize());
     return CFLX_OK;
 }
 
@@ -161,26 +247,22 @@ int cflx_dbg_gemm_tn(int M, int N, int K, const double* AT, int at_rows, int64_t
                      int col_off, double alpha, double beta, int in_place, double* D_out, double* C_out, int reps,
                      double* ms_out) {
     CFLX_TRY(check_device());
-    if (M <= 0 || N <= 0 || K <= 0 || !AT || !B || !C || at_rows <= 0 || b_rows <= 0 || c_rows <= 0 || ldat <= 0 ||
-        ldb <= 0 || ldc <= 0 || at_off < 0 || b_off < 0 || row_off < 0 || col_off < 0)
-        return CFLX_ERR_ARG;
+    REFUSE_IF(M <= 0 || N <= 0 || K <= 0);
+    REFUSE_IF(!AT || !B || !C);
+    REFUSE_IF(at_rows <= 0 || b_rows <= 0 || c_rows <= 0 || ldat <= 0 || ldb <= 0 || ldc <= 0);
+    REFUSE_IF(at_off < 0 || b_off < 0 || row_off < 0 || col_off < 0);
     // every element the kernel may touch lies inside the buffers: AT rows of round_up(M, 2) (the producer's even copy
     // width), B rows of N, the C window; 16-byte alignment of every operand row needs even offsets
     if ((at_off & 1) || (b_off & 1) || (col_off & 1) || at_off + (K - 1) * ldat + round_up(M, 2) > (int64_t)at_rows * ldat ||
-        b_off + (K - 1) * ldb + N > (int64_t)b_rows * ldb || row_off + M > c_rows || col_off + N > ldc) {
-        set_last_error("dbg_gemm_tn: window outside the buffers or misaligned");
-        return CFLX_ERR_ARG;
-    }
+        b_off + (K - 1) * ldb + N > (int64_t)b_rows * ldb || row_off + M > c_rows || col_off + N > ldc)
+        return refuse(__func__, "window outside the buffers or misaligned");
     const size_t a_n = (size_t)at_rows * ldat, b_n = (size_t)b_rows * ldb, c_n = (size_t)c_rows * ldc;
     DevBuf dA, dB, dC, dC0, dD;
-    CFLX_TRY(dA.alloc(sizeof(double) * a_n));
-    CFLX_TRY(dB.alloc(sizeof(double) * b_n));
-    CFLX_TRY(dC.alloc(sizeof(double) * c_n));
-    CFLX_TRY(dC0.alloc(sizeof(double) * c_n));
-    CFLX_TRY(dD.alloc(sizeof(double) * c_n));
-    CFLX_CUDA(cudaMemcpy(dA.p, AT, sizeof(double) * a_n, cudaMemcpyHostToDevice));
-    CFLX_CUDA(cudaMemcpy(dB.p, B, sizeof(double) * b_n, cudaMemcpyHostToDevice));
-    CFLX_CUDA(cudaMemcpy(dC0.p, C, sizeof(double) * c_n, cudaMemcpyHostToDevice));
+    CFLX_TRY(stage(dA, a_n, AT));
+    CFLX_TRY(stage(dB, b_n, B));
+    CFLX_TRY(stage(dC, c_n));
+    CFLX_TRY(stage(dC0, c_n, C));
+    CFLX_TRY(stage(dD, c_n));
     auto restore = [&]() -> int {
         CFLX_CUDA(cudaMemcpy(dC.p, dC0.p, sizeof(double) * c_n, cudaMemcpyDeviceToDevice));
         CFLX_CUDA(cudaMemcpy(dD.p, dC0.p, sizeof(double) * c_n, cudaMemcpyDeviceToDevice));
@@ -198,39 +280,26 @@ int cflx_dbg_gemm_tn(int M, int N, int K, const double* AT, int at_rows, int64_t
     CFLX_TRY(time_reps([&] { return launch_gemm_tn(g, 0); }, reps, ms_out));
     CFLX_TRY(restore());
     CFLX_TRY(launch_gemm_tn(g, 0));
-    if (D_out) CFLX_CUDA(cudaMemcpy(D_out, in_place ? dC.p : dD.p, sizeof(double) * c_n, cudaMemcpyDeviceToHost));
-    if (C_out) CFLX_CUDA(cudaMemcpy(C_out, dC.p, sizeof(double) * c_n, cudaMemcpyDeviceToHost));
+    CFLX_TRY(fetch(D_out, in_place ? dC.p : dD.p, c_n));
+    CFLX_TRY(fetch(C_out, dC.p, c_n));
     CFLX_CUDA(cudaDeviceSynchronize());
     return CFLX_OK;
 }
 
 // D = beta*C + alpha * A * B on the narrow GEMM of the solve (solve.cu); A [M x K], B [K x N], C / D [M x N] dense
-// row-major.  D == C (the same host array) runs the kernel with D aliasing C on the device.  The timed repetitions run
-// first, into a separate output, and the result is one more launch on the pristine inputs.
+// row-major.  D == C (the same host array) runs the kernel with D aliasing C on the device.
 int cflx_dbg_gemm_narrow(int M, int N, int K, const double* A, const double* B, const double* C, double alpha, double beta,
                          double* D, int reps, double* ms_out) {
     CFLX_TRY(check_device());
-    if (M <= 0 || N <= 0 || K < 0 || (K & 3) || !A || !B) return CFLX_ERR_ARG;
-    const size_t a_n = (size_t)M * K, b_n = (size_t)K * N, c_n = (size_t)M * N;
-    DevBuf dA, dB, dC, dT;
-    CFLX_TRY(dA.alloc(sizeof(double) * a_n));
-    CFLX_TRY(dB.alloc(sizeof(double) * b_n));
-    CFLX_TRY(dC.alloc(sizeof(double) * c_n));
-    CFLX_TRY(dT.alloc(sizeof(double) * c_n));
-    CFLX_CUDA(cudaMemcpy(dA.p, A, sizeof(double) * a_n, cudaMemcpyHostToDevice));
-    CFLX_CUDA(cudaMemcpy(dB.p, B, sizeof(double) * b_n, cudaMemcpyHostToDevice));
-    if (C) CFLX_CUDA(cudaMemcpy(dC.p, C, sizeof(double) * c_n, cudaMemcpyHostToDevice));
-    else CFLX_CUDA(cudaMemset(dC.p, 0, sizeof(double) * c_n));
-    const bool alias = C && D == C;
-    auto run = [&](double* out) {
-        return launch_gemm_narrow(M, N, K, dA.as<double>(), K, dB.as<double>(), N, dC.as<double>(), N, out, N, alpha, beta, 0);
-    };
-    CFLX_TRY(time_reps([&] { return run(dT.as<double>()); }, reps, ms_out));
-    double* out = alias ? dC.as<double>() : dT.as<double>();
-    CFLX_TRY(run(out));
-    if (D) CFLX_CUDA(cudaMemcpy(D, out, sizeof(double) * c_n, cudaMemcpyDeviceToHost));
-    CFLX_CUDA(cudaDeviceSynchronize());
-    return CFLX_OK;
+    REFUSE_IF(M <= 0 || N <= 0 || K < 0);
+    REFUSE_IF(K & 3);
+    REFUSE_IF(!A || !B);
+    DevBuf dA, dB;
+    CFLX_TRY(stage(dA, (size_t)M * K, A));
+    CFLX_TRY(stage(dB, (size_t)K * N, B));
+    return narrow_gemm((size_t)M * N, C, D, reps, ms_out, [&](const double* c, double* out) {
+        return launch_gemm_narrow(M, N, K, dA.as<double>(), K, dB.as<double>(), N, c, N, out, N, alpha, beta, 0);
+    });
 }
 
 // D = beta*C + alpha * AT^T * B on the transposed narrow GEMM (solve.cu), like cflx_dbg_gemm_narrow; AT [K x M] is stored
@@ -238,245 +307,211 @@ int cflx_dbg_gemm_narrow(int M, int N, int K, const double* A, const double* B, 
 int cflx_dbg_gemm_narrow_tn(int M, int N, int K, const double* AT, const double* B, const double* C, double alpha,
                             double beta, double* D, int reps, double* ms_out) {
     CFLX_TRY(check_device());
-    if (M <= 0 || N <= 0 || K < 0 || !AT || !B) return CFLX_ERR_ARG;
+    REFUSE_IF(M <= 0 || N <= 0 || K < 0);
+    REFUSE_IF(!AT || !B);
     const int64_t ldat = round_up(M, 2);
-    const size_t a_n = (size_t)K * ldat, b_n = (size_t)K * N, c_n = (size_t)M * N;
-    DevBuf dA, dB, dC, dT;
-    CFLX_TRY(dA.alloc(sizeof(double) * a_n));
-    CFLX_TRY(dB.alloc(sizeof(double) * b_n));
-    CFLX_TRY(dC.alloc(sizeof(double) * c_n));
-    CFLX_TRY(dT.alloc(sizeof(double) * c_n));
-    if (K > 0) {
-        CFLX_CUDA(cudaMemcpy2D(dA.p, ldat * 8, AT, (size_t)M * 8, (size_t)M * 8, K, cudaMemcpyHostToDevice));
-        CFLX_CUDA(cudaMemcpy(dB.p, B, sizeof(double) * b_n, cudaMemcpyHostToDevice));
-    }
-    if (C) CFLX_CUDA(cudaMemcpy(dC.p, C, sizeof(double) * c_n, cudaMemcpyHostToDevice));
-    else CFLX_CUDA(cudaMemset(dC.p, 0, sizeof(double) * c_n));
-    const bool alias = C && D == C;
-    auto run = [&](double* out) {
-        return launch_gemm_narrow_tn(M, N, K, dA.as<double>(), ldat, dB.as<double>(), N, dC.as<double>(), N, out, N, alpha,
-                                     beta, 0);
-    };
-    CFLX_TRY(time_reps([&] { return run(dT.as<double>()); }, reps, ms_out));
-    double* out = alias ? dC.as<double>() : dT.as<double>();
-    CFLX_TRY(run(out));
-    if (D) CFLX_CUDA(cudaMemcpy(D, out, sizeof(double) * c_n, cudaMemcpyDeviceToHost));
-    CFLX_CUDA(cudaDeviceSynchronize());
-    return CFLX_OK;
+    DevBuf dA, dB;
+    CFLX_TRY(stage(dA, K * ldat));
+    CFLX_TRY(stage(dB, (size_t)K * N, B));
+    if (K > 0) CFLX_CUDA(cudaMemcpy2D(dA.p, ldat * 8, AT, (size_t)M * 8, (size_t)M * 8, K, cudaMemcpyHostToDevice));
+    return narrow_gemm((size_t)M * N, C, D, reps, ms_out, [&](const double* c, double* out) {
+        return launch_gemm_narrow_tn(M, N, K, dA.as<double>(), ldat, dB.as<double>(), N, c, N, out, N, alpha, beta, 0);
+    });
 }
 
-// the per-share kernels of equilibration and of the pivot growth (equil.cu) on one layer-0 share at grid position
-// (pi, pj) of Px x Py; each output may be null
-int cflx_dbg_equil(int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, int M, const double* A,
-                   const double* r, const double* c, char equed, int ncols, double* rowmax_out, double* colmax_out,
-                   double* diag_out, double* scaled_out, double* sym_scaled_out, double* growth_out, int* zero_pivot_out) {
+// the per-share kernels of equilibration and of the pivot growth (equil.cu) on one layer-0 share; each output may be null
+int cflx_dbg_equil(const cflx_share_layout* share, const double* A, const double* r, const double* c, char equed, int ncols,
+                   double* rowmax_out, double* colmax_out, double* diag_out, double* scaled_out, double* sym_scaled_out,
+                   double* growth_out, int* zero_pivot_out) {
     CFLX_TRY(check_device());
-    if (Ml < 0 || Nl < 0 || v < 1 || Ml % v || Nl % v || Px < 1 || Py < 1 || pi < 0 || pi >= Px || pj < 0 || pj >= Py ||
-        !A || !r || !c || M < (Ml / v) * Px * v || M < (Nl / v) * Py * v ||
-        (equed != 'N' && equed != 'R' && equed != 'C' && equed != 'B'))
-        return CFLX_ERR_ARG;
-    const size_t a_n = (size_t)Ml * Nl;
+    Layout L;
+    CFLX_TRY(share_layout(__func__, share, TILED | COVERED, &L));
+    REFUSE_IF(!A || !r || !c);
+    REFUSE_IF(equed != 'N' && equed != 'R' && equed != 'C' && equed != 'B');
+    const int M = L.M;
+    const size_t a_n = (size_t)L.Ml * L.Nl;
     DevBuf dA, dW, dr, dc, dv, dg, dz;
-    CFLX_TRY(dA.alloc(sizeof(double) * a_n));
-    CFLX_TRY(dW.alloc(sizeof(double) * a_n));
-    CFLX_TRY(dr.alloc(sizeof(double) * M));
-    CFLX_TRY(dc.alloc(sizeof(double) * M));
-    CFLX_TRY(dv.alloc(sizeof(double) * M));
-    CFLX_TRY(dg.alloc(sizeof(double) * 2 * M));
-    CFLX_TRY(dz.alloc(sizeof(int)));
-    CFLX_CUDA(cudaMemcpy(dA.p, A, sizeof(double) * a_n, cudaMemcpyHostToDevice));
-    CFLX_CUDA(cudaMemcpy(dr.p, r, sizeof(double) * M, cudaMemcpyHostToDevice));
-    CFLX_CUDA(cudaMemcpy(dc.p, c, sizeof(double) * M, cudaMemcpyHostToDevice));
+    CFLX_TRY(stage(dA, a_n, A));
+    CFLX_TRY(stage(dW, a_n));
+    CFLX_TRY(stage(dr, M, r));
+    CFLX_TRY(stage(dc, M, c));
+    CFLX_TRY(stage(dv, M));
+    CFLX_TRY(stage(dg, 2 * (size_t)M));
+    CFLX_TRY(stage<int>(dz, 1));
     const double* a = dA.as<double>();
     double *w = dW.as<double>(), *vec = dv.as<double>();
-    const Layout L{M, v, Kappa, Ml, Nl, Px, Py, pi, pj};
-    auto vec_out = [&](double* out) -> int {
-        CFLX_CUDA(cudaMemcpy(out, vec, sizeof(double) * M, cudaMemcpyDeviceToHost));
-        return CFLX_OK;
-    };
-    if (rowmax_out) {
-        CFLX_TRY(equil_row_max(a, L, vec, 0));
-        CFLX_TRY(vec_out(rowmax_out));
-    }
-    if (colmax_out) {
-        CFLX_TRY(equil_col_max(a, L, dr.as<double>(), vec, 0));
-        CFLX_TRY(vec_out(colmax_out));
-    }
-    if (diag_out) {
-        CFLX_TRY(equil_diag(a, L, vec, 0));
-        CFLX_TRY(vec_out(diag_out));
-    }
+    if (rowmax_out) CFLX_TRY(equil_row_max(a, L, vec, 0));
+    CFLX_TRY(fetch(rowmax_out, vec, M));
+    if (colmax_out) CFLX_TRY(equil_col_max(a, L, dr.as<double>(), vec, 0));
+    CFLX_TRY(fetch(colmax_out, vec, M));
+    if (diag_out) CFLX_TRY(equil_diag(a, L, vec, 0));
+    CFLX_TRY(fetch(diag_out, vec, M));
     if (scaled_out) {
         CFLX_CUDA(cudaMemcpy(w, a, sizeof(double) * a_n, cudaMemcpyDeviceToDevice));
         CFLX_TRY(equil_apply(w, L, dr.as<double>(), dc.as<double>(), equed, 0));
-        CFLX_CUDA(cudaMemcpy(scaled_out, w, sizeof(double) * a_n, cudaMemcpyDeviceToHost));
+        CFLX_TRY(fetch(scaled_out, w, a_n));
     }
     if (sym_scaled_out) {  // s = r
         CFLX_CUDA(cudaMemcpy(w, a, sizeof(double) * a_n, cudaMemcpyDeviceToDevice));
         CFLX_TRY(equil_sym_apply(w, L, dr.as<double>(), 0));
-        CFLX_CUDA(cudaMemcpy(sym_scaled_out, w, sizeof(double) * a_n, cudaMemcpyDeviceToHost));
+        CFLX_TRY(fetch(sym_scaled_out, w, a_n));
     }
     if (growth_out) {  // the share is both L\U and the input; dgesvx's maxima are those of the columns' maxima
         CFLX_TRY(equil_growth_cols(a, a, L, false, ncols, dg.as<double>(), 0));
         std::vector<double> h(2 * (size_t)M);
-        CFLX_CUDA(cudaMemcpy(h.data(), dg.p, sizeof(double) * 2 * M, cudaMemcpyDeviceToHost));
+        CFLX_TRY(fetch(h.data(), dg.p, h.size()));
         growth_out[0] = *std::max_element(h.begin() + M, h.end());
         growth_out[1] = *std::max_element(h.begin(), h.begin() + M);
     }
     if (zero_pivot_out) {
         CFLX_TRY(equil_zero_pivot(a, L, dz.as<int>(), 0));
         int z = 0;
-        CFLX_CUDA(cudaMemcpy(&z, dz.p, sizeof(int), cudaMemcpyDeviceToHost));
+        CFLX_TRY(fetch(&z, dz.p, 1));
         *zero_pivot_out = z == INT_MAX ? 0 : z;
     }
     CFLX_CUDA(cudaDeviceSynchronize());
     return CFLX_OK;
 }
 
-// the per-column pivot growth pass (equil.cu) on one layer-0 share F (the factor) and A (the input) at grid position
-// (pi, pj) of Px x Py; mode 0 LU, 1 Cholesky; either output may be null
-int cflx_dbg_growth_cols(int mode, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, int M, int ncols,
-                         const double* F, const double* A, double* amax_out, double* fmax_out) {
+// the per-column pivot growth pass (equil.cu) on one layer-0 share F (the factor) and A (the input); mode 0 LU, 1
+// Cholesky; either output may be null
+int cflx_dbg_growth_cols(int mode, const cflx_share_layout* share, int ncols, const double* F, const double* A,
+                         double* amax_out, double* fmax_out) {
     CFLX_TRY(check_device());
-    if ((mode != 0 && mode != 1) || Ml < 0 || Nl < 0 || v < 1 || Ml % v || Nl % v || Px < 1 || Py < 1 || pi < 0 ||
-        pi >= Px || pj < 0 || pj >= Py || !F || !A || M < (Ml / v) * Px * v || M < (Nl / v) * Py * v)
-        return CFLX_ERR_ARG;
-    const size_t a_n = (size_t)Ml * Nl;
+    Layout L;
+    CFLX_TRY(share_layout(__func__, share, TILED | COVERED, &L));
+    REFUSE_IF(mode != 0 && mode != 1);
+    REFUSE_IF(!F || !A);
+    const size_t a_n = (size_t)L.Ml * L.Nl;
     DevBuf dF, dA, dg;
-    CFLX_TRY(dF.alloc(sizeof(double) * a_n));
-    CFLX_TRY(dA.alloc(sizeof(double) * a_n));
-    CFLX_TRY(dg.alloc(sizeof(double) * 2 * M));
-    CFLX_CUDA(cudaMemcpy(dF.p, F, sizeof(double) * a_n, cudaMemcpyHostToDevice));
-    CFLX_CUDA(cudaMemcpy(dA.p, A, sizeof(double) * a_n, cudaMemcpyHostToDevice));
-    const Layout L{M, v, Kappa, Ml, Nl, Px, Py, pi, pj};
+    CFLX_TRY(stage(dF, a_n, F));
+    CFLX_TRY(stage(dA, a_n, A));
+    CFLX_TRY(stage(dg, 2 * (size_t)L.M));
     CFLX_TRY(equil_growth_cols(dF.as<double>(), dA.as<double>(), L, mode == 1, ncols, dg.as<double>(), 0));
-    if (amax_out) CFLX_CUDA(cudaMemcpy(amax_out, dg.p, sizeof(double) * M, cudaMemcpyDeviceToHost));
-    if (fmax_out) CFLX_CUDA(cudaMemcpy(fmax_out, dg.as<double>() + M, sizeof(double) * M, cudaMemcpyDeviceToHost));
+    CFLX_TRY(fetch(amax_out, dg.p, L.M));
+    CFLX_TRY(fetch(fmax_out, dg.as<double>() + L.M, L.M));
     CFLX_CUDA(cudaDeviceSynchronize());
     return CFLX_OK;
 }
 
-// the seed, scatter and zero-fill kernels of the inverse (inverse.cu) on one share at grid position (pi, pj) of Px x Py
-int cflx_dbg_inverse_share(int mode, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, int M, int c0,
-                           int nc, int rows, const double* X, int ldx, const int* perm, double* W_out,
-                           double* share_inout, int zero_fill) {
+// the seed, scatter and zero-fill kernels of the inverse (inverse.cu) on one share
+int cflx_dbg_inverse_share(int mode, const cflx_share_layout* share, int c0, int nc, int rows, const double* X, int ldx,
+                           const int* perm, double* W_out, double* share_inout, int zero_fill) {
     CFLX_TRY(check_device());
-    if ((mode != 0 && mode != 1) || Ml < 0 || Nl < 0 || v < 1 || Ml % v || Nl % v || Px < 1 || Py < 1 || pi < 0 ||
-        pi >= Px || pj < 0 || pj >= Py || M < (Ml / v) * Px * v || M < (Nl / v) * Py * v || c0 < 0 || nc < 1 ||
-        c0 + nc > M || rows < 0 || rows > Ml || (share_inout && (!X || ldx < nc || (mode == 0 && !perm))))
-        return CFLX_ERR_ARG;
-    const Layout L{M, v, Kappa, Ml, Nl, Px, Py, pi, pj};
-    const int ldn = (int)round_up(nc, 8);
+    Layout L;
+    CFLX_TRY(share_layout(__func__, share, TILED | COVERED, &L));
+    REFUSE_IF(mode != 0 && mode != 1);
+    REFUSE_IF(c0 < 0 || nc < 1 || c0 + nc > L.M);
+    REFUSE_IF(rows < 0 || rows > L.Ml);
+    REFUSE_IF(share_inout && (!X || (mode == 0 && !perm)));
+    REFUSE_IF(share_inout && ldx < nc);
+    const size_t w_n = (size_t)L.Ml * round_up(nc, 8);
     if (W_out) {
         DevBuf dW;
-        CFLX_TRY(dW.alloc(sizeof(double) * Ml * ldn));
-        CFLX_CUDA(cudaMemset(dW.p, 0, sizeof(double) * Ml * ldn));
-        CFLX_TRY(launch_inverse_seed(dW.as<double>(), ldn, L, rows, c0, nc, 0));
-        CFLX_CUDA(cudaMemcpy(W_out, dW.p, sizeof(double) * Ml * ldn, cudaMemcpyDeviceToHost));
+        CFLX_TRY(stage(dW, w_n));
+        CFLX_CUDA(cudaMemset(dW.p, 0, sizeof(double) * w_n));
+        CFLX_TRY(launch_inverse_seed(dW.as<double>(), (int)round_up(nc, 8), L, rows, c0, nc, 0));
+        CFLX_TRY(fetch(W_out, dW.p, w_n));
     }
     if (share_inout) {
-        const size_t a_n = (size_t)Ml * Nl;
+        const size_t a_n = (size_t)L.Ml * L.Nl;
         DevBuf dA, dX, dp;
-        CFLX_TRY(dA.alloc(sizeof(double) * a_n));
-        CFLX_TRY(dX.alloc(sizeof(double) * M * ldx));
-        CFLX_TRY(dp.alloc(sizeof(int) * M));
-        CFLX_CUDA(cudaMemcpy(dA.p, share_inout, sizeof(double) * a_n, cudaMemcpyHostToDevice));
-        CFLX_CUDA(cudaMemcpy(dX.p, X, sizeof(double) * M * ldx, cudaMemcpyHostToDevice));
-        if (mode == 0) CFLX_CUDA(cudaMemcpy(dp.p, perm, sizeof(int) * M, cudaMemcpyHostToDevice));
+        CFLX_TRY(stage(dA, a_n, share_inout));
+        CFLX_TRY(stage(dX, (size_t)L.M * ldx, X));
+        CFLX_TRY(stage(dp, L.M, mode == 0 ? perm : nullptr));
         CFLX_TRY(launch_inverse_scatter(mode == 0 ? InvKind::LU : InvKind::Chol, dX.as<double>(), ldx, c0, nc,
                                         mode == 0 ? dp.as<int>() : nullptr, L, dA.as<double>(), 0));
         if (mode == 1 && zero_fill) CFLX_TRY(launch_inverse_zero(L, dA.as<double>(), 0));
-        CFLX_CUDA(cudaMemcpy(share_inout, dA.p, sizeof(double) * a_n, cudaMemcpyDeviceToHost));
+        CFLX_TRY(fetch(share_inout, dA.p, a_n));
     }
     CFLX_CUDA(cudaDeviceSynchronize());
     return CFLX_OK;
 }
 
-// the pack and scatter kernels of the distributed solves (solve_local.cu) on one share at grid position (pi, pj) of Px x Py
-int cflx_dbg_solve_local_share(int mode, int Ml, int v, int Kappa, int Px, int Py, int pi, int pj, int M, int nrhs, int c0,
-                               int w, const double* B, int ldb, double* Bk_out, const double* Xk, double* X_inout, int ldx) {
+// the pack and scatter kernels of the distributed solves (solve_local.cu) on one right-hand side share
+int cflx_dbg_solve_local_share(int mode, const cflx_share_layout* share, int nrhs, int c0, int w, const double* B, int ldb,
+                               double* Bk_out, const double* Xk, double* X_inout, int ldx) {
     CFLX_TRY(check_device());
-    if ((mode != 0 && mode != 1) || Ml < 0 || v < 1 || Ml % v || Px < 1 || Py < 1 || pi < 0 || pi >= Px || pj < 0 ||
-        pj >= Py || M < (Ml / v) * Px * v || nrhs < 1 || c0 < 0 || w < 1 || c0 + w > nrhs)
-        return CFLX_ERR_ARG;
-    const int ncl = rhs_local_cols(nrhs, v, Py), ldn = (int)round_up(w, 8);
-    if ((Bk_out && (!B || ldb < ncl)) || (X_inout && (!Xk || ldx < ncl))) return CFLX_ERR_ARG;
-    const Layout L{M, v, Kappa, Ml, ncl, Px, Py, pi, pj};
-    const int rows = solve_local_rows(L, mode == 1);
+    Layout L;
+    CFLX_TRY(share_layout(__func__, share, TILED, &L));
+    const auto [M, v, Kappa, Ml, Nl, Px, Py, pi, pj] = *share;
+    REFUSE_IF(mode != 0 && mode != 1);
+    REFUSE_IF(M < (Ml / v) * Px * v);
+    REFUSE_IF(nrhs < 1);
+    REFUSE_IF(c0 < 0 || w < 1 || c0 + w > nrhs);
+    REFUSE_IF(Nl != rhs_local_cols(nrhs, v, Py));
+    REFUSE_IF(Bk_out && (!B || ldb < Nl));
+    REFUSE_IF(X_inout && (!Xk || ldx < Nl));
+    const int rows = solve_local_rows(L, mode == 1), ldn = (int)round_up(w, 8);
+    const size_t k_n = (size_t)M * ldn;
     if (Bk_out) {
         DevBuf dB, dK;
-        CFLX_TRY(dB.alloc(sizeof(double) * Ml * ldb));
-        CFLX_TRY(dK.alloc(sizeof(double) * M * ldn));
-        CFLX_CUDA(cudaMemcpy(dB.p, B, sizeof(double) * Ml * ldb, cudaMemcpyHostToDevice));
+        CFLX_TRY(stage(dB, (size_t)Ml * ldb, B));
+        CFLX_TRY(stage(dK, k_n));
         CFLX_TRY(launch_solve_local_pack(dB.as<double>(), ldb, L, rows, c0, w, dK.as<double>(), ldn, 0));
-        CFLX_CUDA(cudaMemcpy(Bk_out, dK.p, sizeof(double) * M * ldn, cudaMemcpyDeviceToHost));
+        CFLX_TRY(fetch(Bk_out, dK.p, k_n));
     }
     if (X_inout) {
         DevBuf dX, dK;
-        CFLX_TRY(dX.alloc(sizeof(double) * Ml * ldx));
-        CFLX_TRY(dK.alloc(sizeof(double) * M * ldn));
-        CFLX_CUDA(cudaMemcpy(dX.p, X_inout, sizeof(double) * Ml * ldx, cudaMemcpyHostToDevice));
-        CFLX_CUDA(cudaMemcpy(dK.p, Xk, sizeof(double) * M * ldn, cudaMemcpyHostToDevice));
+        CFLX_TRY(stage(dX, (size_t)Ml * ldx, X_inout));
+        CFLX_TRY(stage(dK, k_n, Xk));
         CFLX_TRY(launch_solve_local_scatter(dK.as<double>(), ldn, L, rows, c0, w, dX.as<double>(), ldx, 0));
-        CFLX_CUDA(cudaMemcpy(X_inout, dX.p, sizeof(double) * Ml * ldx, cudaMemcpyDeviceToHost));
+        CFLX_TRY(fetch(X_inout, dX.p, (size_t)Ml * ldx));
     }
     CFLX_CUDA(cudaDeviceSynchronize());
     return CFLX_OK;
 }
 
-// the per-share passes of the 1-norm and the infinity-norm (norm.cu) on one layer-0 share at grid position (pi, pj) of
-// Px x Py: mode 0 the column sums, 1 the column sums of the symmetric matrix stored as its lower triangle, 2 the row sums
-int cflx_dbg_norm_share(int mode, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, int M, const double* A,
-                        double* out) {
+// the per-share passes of the 1-norm and the infinity-norm (norm.cu) on one layer-0 share: mode 0 the column sums, 1 the
+// column sums of the symmetric matrix stored as its lower triangle, 2 the row sums
+int cflx_dbg_norm_share(int mode, const cflx_share_layout* share, const double* A, double* out) {
     CFLX_TRY(check_device());
-    if (mode < 0 || mode > 2 || Ml < 1 || Nl < 1 || v < 1 || Ml % v || Nl % v || Px < 1 || Py < 1 || pi < 0 || pi >= Px ||
-        pj < 0 || pj >= Py || !A || !out || M < (Ml / v) * Px * v || M < (Nl / v) * Py * v)
-        return CFLX_ERR_ARG;
-    const Layout L{M, v, Kappa, Ml, Nl, Px, Py, pi, pj};
-    const size_t a_n = (size_t)Ml * Nl;
+    Layout L;
+    CFLX_TRY(share_layout(__func__, share, TILED | COVERED | NONEMPTY, &L));
+    REFUSE_IF(mode < 0 || mode > 2);
+    REFUSE_IF(!A || !out);
     int ncp = 0, nrp = 0;
     norm1_partials(L, &ncp, &nrp);
     DevBuf dA, dcol, drow, dout;
-    CFLX_TRY(dA.alloc(sizeof(double) * a_n));
-    CFLX_TRY(dcol.alloc(sizeof(double) * ncp * Nl));
-    CFLX_TRY(drow.alloc(sizeof(double) * nrp * Ml));
-    CFLX_TRY(dout.alloc(sizeof(double) * M));
-    CFLX_CUDA(cudaMemcpy(dA.p, A, sizeof(double) * a_n, cudaMemcpyHostToDevice));
+    CFLX_TRY(stage(dA, (size_t)L.Ml * L.Nl, A));
+    CFLX_TRY(stage(dcol, (size_t)ncp * L.Nl));
+    CFLX_TRY(stage(drow, (size_t)nrp * L.Ml));
+    CFLX_TRY(stage(dout, L.M));
     double* o = dout.as<double>();
     if (mode == 2) {  // norminf_grid zeroes the vector; the column sums write every entry (NaN shows one they miss)
-        CFLX_CUDA(cudaMemset(o, 0, sizeof(double) * M));
+        CFLX_CUDA(cudaMemset(o, 0, sizeof(double) * L.M));
         CFLX_TRY(launch_norminf_share(dA.as<double>(), L, o, 0));
     } else {
-        CFLX_TRY(launch_fill(o, M, std::numeric_limits<double>::quiet_NaN(), 0));
+        CFLX_TRY(launch_fill(o, L.M, std::numeric_limits<double>::quiet_NaN(), 0));
         CFLX_TRY(launch_norm1_share(dA.as<double>(), L, mode == 1, dcol.as<double>(), drow.as<double>(), o, 0));
     }
-    CFLX_CUDA(cudaMemcpy(out, o, sizeof(double) * M, cudaMemcpyDeviceToHost));
+    CFLX_TRY(fetch(out, o, L.M));
     CFLX_CUDA(cudaDeviceSynchronize());
     return CFLX_OK;
 }
 
-// cflx_chol_validate's per-share kernels on one layer-0 share at grid position (pi, pj) of Px x Py (each output may be
-// null): the sum of squares of its lower triangle of the real tiles, and the masked transposed panel of step t
-int cflx_dbg_chol_validate_share(int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, const double* A, int t,
-                                 double* PT_out, double* sumsq_out) {
+// cflx_chol_validate's per-share kernels on one layer-0 share (each output may be null): the sum of squares of its lower
+// triangle of the real tiles, and the masked transposed panel of step t
+int cflx_dbg_chol_validate_share(const cflx_share_layout* share, const double* A, int t, double* PT_out, double* sumsq_out) {
     CFLX_TRY(check_device());
-    if (Ml < 1 || Nl < 1 || v < 1 || Ml % v || Nl % v || Kappa < 1 || Px < 1 || Py < 1 || pi < 0 || pi >= Px || pj < 0 ||
-        pj >= Py || !A || t < 0 || t >= Kappa || (t / Py + 1) * v > Nl)
-        return CFLX_ERR_ARG;
-    const int M = std::max((Ml / v) * Px, (Nl / v) * Py) * v;
-    const Layout L{M, v, Kappa, Ml, Nl, Px, Py, pi, pj};
-    const size_t a_n = (size_t)Ml * Nl;
+    Layout L;
+    CFLX_TRY(share_layout(__func__, share, TILED | NONEMPTY, &L));
+    const auto [M, v, Kappa, Ml, Nl, Px, Py, pi, pj] = *share;
+    REFUSE_IF(M != std::max((Ml / v) * Px, (Nl / v) * Py) * v);
+    REFUSE_IF(Kappa < 1);
+    REFUSE_IF(!A);
+    REFUSE_IF(t < 0 || t >= Kappa);
+    REFUSE_IF((t / Py + 1) * v > Nl);
     const int64_t ldp = chol_panel_ld(Ml);
     DevBuf dA, dacc, dPT;
-    CFLX_TRY(dA.alloc(sizeof(double) * a_n));
-    CFLX_TRY(dacc.alloc(sizeof(double) * (1 + SUMSQ_PARTIALS)));
-    CFLX_TRY(dPT.alloc(sizeof(double) * v * ldp));
-    CFLX_CUDA(cudaMemcpy(dA.p, A, sizeof(double) * a_n, cudaMemcpyHostToDevice));
+    CFLX_TRY(stage(dA, (size_t)Ml * Nl, A));
+    CFLX_TRY(stage(dacc, 1 + SUMSQ_PARTIALS));
+    CFLX_TRY(stage(dPT, v * ldp));
     if (sumsq_out) {
         double* acc = dacc.as<double>();
         CFLX_CUDA(cudaMemset(acc, 0, sizeof(double)));
         CFLX_TRY(launch_sumsq_lower(dA.as<double>(), L, acc + 1, acc, 0));
-        CFLX_CUDA(cudaMemcpy(sumsq_out, acc, sizeof(double), cudaMemcpyDeviceToHost));
+        CFLX_TRY(fetch(sumsq_out, acc, 1));
     }
     if (PT_out) {  // v x chol_panel_ld(Ml); NaN where the kernel writes nothing (and everywhere off grid column t % Py)
         CFLX_TRY(launch_fill(dPT.as<double>(), v * ldp, std::numeric_limits<double>::quiet_NaN(), 0));
@@ -484,61 +519,59 @@ int cflx_dbg_chol_validate_share(int Ml, int Nl, int v, int Kappa, int Px, int P
         if (pj == t % Py)  // the guard and the arguments of cflx_chol_validate
             CFLX_TRY(launch_extract_l_panel_T(dA.as<double>(), Nl, row0, (t / Py) * v, Ml - row0, L, t, dPT.as<double>(),
                                               chol_piece_ld(L, t, pi), 0));
-        CFLX_CUDA(cudaMemcpy(PT_out, dPT.p, sizeof(double) * v * ldp, cudaMemcpyDeviceToHost));
+        CFLX_TRY(fetch(PT_out, dPT.p, v * ldp));
     }
     CFLX_CUDA(cudaDeviceSynchronize());
     return CFLX_OK;
 }
 
-// the two extract kernels of cflx_lu_validate's sweep, step t, on one layer-0 share C of the packed factors at grid
-// position (pi, pj) of Px x Py, under the owner guards of the sweep (each output may be null)
-int cflx_dbg_lu_validate_share(int Ml, int Nl, int v, int Px, int Py, int pi, int pj, const double* C, int t, double* LT_out,
-                               double* U_out) {
+// the two extract kernels of cflx_lu_validate's sweep, step t, on one layer-0 share C of the packed factors, under the
+// owner guards of the sweep (each output may be null)
+int cflx_dbg_lu_validate_share(const cflx_share_layout* share, const double* C, int t, double* LT_out, double* U_out) {
     CFLX_TRY(check_device());
-    if (Ml < 1 || Nl < 1 || v < 1 || Ml % v || Nl % v || Px < 1 || Py < 1 || pi < 0 || pi >= Px || pj < 0 || pj >= Py ||
-        !C || t < 0 || (Ml / v) * Px != (Nl / v) * Py)  // the LU's shares of an M x M matrix
-        return CFLX_ERR_ARG;
-    const int M = (Ml / v) * Px * v;
-    if (t >= M / v) return CFLX_ERR_ARG;
-    const Layout L{M, v, M / v, Ml, Nl, Px, Py, pi, pj};
-    const size_t a_n = (size_t)Ml * Nl;
+    Layout L;
+    CFLX_TRY(share_layout(__func__, share, TILED | NONEMPTY, &L));
+    const auto [M, v, Kappa, Ml, Nl, Px, Py, pi, pj] = *share;
+    REFUSE_IF((Ml / v) * Px != (Nl / v) * Py);  // the LU's shares of an M x M matrix
+    REFUSE_IF(M != (Ml / v) * Px * v);
+    REFUSE_IF(Kappa != M / v);
+    REFUSE_IF(!C);
+    REFUSE_IF(t < 0 || t >= Kappa);
     const int64_t ldp = round_up(Ml, 2);
     const double nan = std::numeric_limits<double>::quiet_NaN();
     DevBuf dC, dLT, dU;
-    CFLX_TRY(dC.alloc(sizeof(double) * a_n));
-    CFLX_TRY(dLT.alloc(sizeof(double) * v * ldp));
-    CFLX_TRY(dU.alloc(sizeof(double) * v * Nl));
-    CFLX_CUDA(cudaMemcpy(dC.p, C, sizeof(double) * a_n, cudaMemcpyHostToDevice));
+    CFLX_TRY(stage(dC, (size_t)Ml * Nl, C));
+    CFLX_TRY(stage(dLT, v * ldp));
+    CFLX_TRY(stage(dU, (size_t)v * Nl));
     if (LT_out) {  // v x round_up(Ml, 2), NaN where the kernel writes nothing
         CFLX_TRY(launch_fill(dLT.as<double>(), v * ldp, nan, 0));
         CFLX_TRY(launch_lu_extract_l(dC.as<double>(), L, t, dLT.as<double>(), ldp, 0));
-        CFLX_CUDA(cudaMemcpy(LT_out, dLT.p, sizeof(double) * v * ldp, cudaMemcpyDeviceToHost));
+        CFLX_TRY(fetch(LT_out, dLT.p, v * ldp));
     }
     if (U_out) {  // v x Nl
         CFLX_TRY(launch_fill(dU.as<double>(), (int64_t)v * Nl, nan, 0));
         CFLX_TRY(launch_lu_extract_u(dC.as<double>(), L, t, dU.as<double>(), Nl, 0));
-        CFLX_CUDA(cudaMemcpy(U_out, dU.p, sizeof(double) * v * Nl, cudaMemcpyDeviceToHost));
+        CFLX_TRY(fetch(U_out, dU.p, (size_t)v * Nl));
     }
     CFLX_CUDA(cudaDeviceSynchronize());
     return CFLX_OK;
 }
 
-// the Cholesky update's column-operand gather (chol.cu) on one share of Ml x Nl at grid column pj of Px x Py, from the
-// Px broadcast pieces of the panel of global tiles >= gfirst (host: piece p is v x chol_piece_ld(p), back to back), for
-// the local column tiles with global index >= gfirst (Bc's tile t: local tile lj0 + t); Bc_out is v x Nl, NaN where
-// nothing is written
-int cflx_dbg_chol_gather_cols(int v, int Px, int Py, int pj, int Ml, int Nl, int gfirst, const double* pieces,
-                              double* Bc_out) {
+// the Cholesky update's column-operand gather (chol.cu) on one share at grid column pj, from the Px broadcast pieces of
+// the panel of global tiles >= gfirst (host: piece p is v x chol_piece_ld(p), back to back), for the local column tiles
+// with global index >= gfirst (Bc's tile t: local tile lj0 + t); Bc_out is v x Nl, NaN where nothing is written
+int cflx_dbg_chol_gather_cols(const cflx_share_layout* share, int gfirst, const double* pieces, double* Bc_out) {
     CFLX_TRY(check_device());
-    if (v < 1 || Px < 1 || Py < 1 || pj < 0 || pj >= Py || Ml < 1 || Nl < 1 || Ml % v || Nl % v || gfirst < 0 || !pieces ||
-        !Bc_out)
-        return CFLX_ERR_ARG;
-    const Layout L{0, v, 0, Ml, Nl, Px, Py, 0, pj};  // chol_piece_ld reads Ml, v and Px only
+    Layout L;
+    CFLX_TRY(share_layout(__func__, share, TILED | NONEMPTY, &L));
+    REFUSE_IF(gfirst < 0);
+    REFUSE_IF(!pieces || !Bc_out);
+    const int v = L.v, Ml = L.Ml, Nl = L.Nl, Px = L.Px, Py = L.Py, pj = L.pj;
     const int64_t ldp = chol_panel_ld(Ml), piece_stride = (int64_t)v * ldp, ldb = Nl;
     const double nan = std::numeric_limits<double>::quiet_NaN();
     DevBuf dG, dB;
-    CFLX_TRY(dG.alloc(sizeof(double) * Px * piece_stride));
-    CFLX_TRY(dB.alloc(sizeof(double) * v * ldb));
+    CFLX_TRY(stage(dG, Px * piece_stride));
+    CFLX_TRY(stage(dB, v * ldb));
     CFLX_TRY(launch_fill(dG.as<double>(), Px * piece_stride, nan, 0));
     CFLX_TRY(launch_fill(dB.as<double>(), v * ldb, nan, 0));
     size_t off = 0;
@@ -553,13 +586,13 @@ int cflx_dbg_chol_gather_cols(int v, int Px, int Py, int pj, int Ml, int Nl, int
         const int j = (lj0 + t) * Py + pj, p = j % Px, first = first_local_tile(gfirst, p, Px);
         const int64_t ldg = std::max(2, (Ml - first * v + 1) & ~1);
         if (j / Px < first || p * piece_stride + (v - 1) * ldg + (int64_t)(j / Px - first + 1) * v > Px * piece_stride) {
-            set_last_error("dbg_chol_gather_cols: column tile %d reads outside the pieces", j);
+            set_last_error("cflx_dbg_chol_gather_cols: refused, column tile %d reads outside the pieces", j);
             return CFLX_ERR_ARG;
         }
     }
     if (ntc > 0)
         CFLX_TRY(launch_gather_cols(dG.as<double>(), piece_stride, dB.as<double>(), ldb, v, Px, Py, pj, lj0, ntc, gfirst, Ml, 0));
-    CFLX_CUDA(cudaMemcpy(Bc_out, dB.p, sizeof(double) * v * ldb, cudaMemcpyDeviceToHost));
+    CFLX_TRY(fetch(Bc_out, dB.p, v * ldb));
     CFLX_CUDA(cudaDeviceSynchronize());
     return CFLX_OK;
 }
@@ -570,19 +603,23 @@ int cflx_dbg_refine_assemble(int mode, int Px, int Py, int Pz, int v, int M, int
                              int ldn, const double* all, const double* B, double* R_out, double* ratio_out, double* W_out,
                              double* Q_out) {
     CFLX_TRY(check_device());
-    if (mode < 0 || mode > 2 || Px < 1 || Py < 1 || Pz < 1 || v < 1 || M < 1 || Ml < 0 || Nl < 0 || Ml % v || Nl % v ||
-        (!nn && !tn) || nrhs < 1 || ldn < nrhs || !all || !B || (nn && M > (Ml / v) * Px * v) ||
-        (tn && M > (Nl / v) * Py * v))
-        return CFLX_ERR_ARG;
+    REFUSE_IF(mode < 0 || mode > 2);
+    REFUSE_IF(Px < 1 || Py < 1 || Pz < 1 || v < 1 || M < 1 || Ml < 0 || Nl < 0);
+    REFUSE_IF(Ml % v || Nl % v);
+    REFUSE_IF(!nn && !tn);
+    REFUSE_IF(nrhs < 1 || ldn < nrhs);
+    REFUSE_IF(!all || !B);
+    REFUSE_IF((nn && M > (Ml / v) * Px * v) || (tn && M > (Nl / v) * Py * v));
     const int64_t chunk = (int64_t)((nn ? Ml : 0) + (tn ? Nl : 0)) * 2 * ldn, mat = (int64_t)M * ldn;
     const int64_t all_n = chunk * Px * Py * Pz;
     DevBuf dall, dB, dR, dratio, dW, dQ;
-    CFLX_TRY(dall.alloc(sizeof(double) * all_n));
-    for (DevBuf* b : {&dB, &dR, &dratio, &dW, &dQ}) CFLX_TRY(b->alloc(sizeof(double) * mat));
-    CFLX_CUDA(cudaMemcpy(dall.p, all, sizeof(double) * all_n, cudaMemcpyHostToDevice));
-    CFLX_CUDA(cudaMemcpy(dB.p, B, sizeof(double) * mat, cudaMemcpyHostToDevice));
+    CFLX_TRY(stage(dall, all_n, all));
+    CFLX_TRY(stage(dB, mat, B));
     const double nan = std::numeric_limits<double>::quiet_NaN();
-    for (DevBuf* b : {&dR, &dratio, &dW, &dQ}) CFLX_TRY(launch_fill(b->as<double>(), mat, nan, 0));
+    for (DevBuf* b : {&dR, &dratio, &dW, &dQ}) {
+        CFLX_TRY(stage(*b, mat));
+        CFLX_TRY(launch_fill(b->as<double>(), mat, nan, 0));
+    }
     double safe1, safe2, nzeps;
     refine_safe(M, &safe1, &safe2, &nzeps);
     AssembleArgs a{dall.as<double>(), chunk, Ml, Nl, ldn, nrhs, M, nn != 0, tn != 0, v, Px, Py, Pz, dB.as<double>(),
@@ -590,14 +627,10 @@ int cflx_dbg_refine_assemble(int mode, int Px, int Py, int Pz, int v, int M, int
     a.lin_berr = mode == 1;
     a.Q = mode == 1 ? dQ.as<double>() : nullptr;
     CFLX_TRY(launch_assemble(a, mode == 2, 0));
-    auto out = [&](double* h, DevBuf& d) -> int {
-        if (h) CFLX_CUDA(cudaMemcpy(h, d.p, sizeof(double) * mat, cudaMemcpyDeviceToHost));
-        return CFLX_OK;
-    };
-    CFLX_TRY(out(R_out, dR));
-    CFLX_TRY(out(ratio_out, dratio));
-    CFLX_TRY(out(W_out, dW));
-    CFLX_TRY(out(Q_out, dQ));
+    CFLX_TRY(fetch(R_out, dR.p, mat));
+    CFLX_TRY(fetch(ratio_out, dratio.p, mat));
+    CFLX_TRY(fetch(W_out, dW.p, mat));
+    CFLX_TRY(fetch(Q_out, dQ.p, mat));
     CFLX_CUDA(cudaDeviceSynchronize());
     return CFLX_OK;
 }
@@ -610,48 +643,42 @@ int cflx_dbg_refine_columns(int M, int ldn, int nrhs, const double* A, const dou
                             double* max_out, double* stats_out, double* select_out, double* add_out, double* Y_out,
                             double* T_inout) {
     CFLX_TRY(check_device());
-    if (M < 1 || nrhs < 1 || ldn < nrhs || !A || ((stats_out || add_out || Y_out) && !D) ||
-        ((select_out || add_out || Y_out) && !sel) || (!Y_out != !T_inout))
-        return CFLX_ERR_ARG;
+    REFUSE_IF(M < 1 || nrhs < 1 || ldn < nrhs);
+    REFUSE_IF(!A);
+    REFUSE_IF((stats_out || add_out || Y_out) && !D);
+    REFUSE_IF((select_out || add_out || Y_out) && !sel);
+    REFUSE_IF(!Y_out != !T_inout);
     const int64_t mat = (int64_t)M * ldn;
     DevBuf dA, dD, dd, dsel, dW, dT, dv;
-    CFLX_TRY(dA.alloc(sizeof(double) * mat));
-    CFLX_TRY(dD.alloc(sizeof(double) * mat));
-    CFLX_TRY(dd.alloc(sizeof(double) * M));
-    CFLX_TRY(dsel.alloc(sizeof(int) * ldn));
-    CFLX_TRY(dW.alloc(sizeof(double) * mat));
-    CFLX_TRY(dT.alloc(sizeof(double) * mat));
-    CFLX_TRY(dv.alloc(sizeof(double) * nrhs * REFINE_NSTAT));
-    CFLX_CUDA(cudaMemcpy(dA.p, A, sizeof(double) * mat, cudaMemcpyHostToDevice));
-    if (D) CFLX_CUDA(cudaMemcpy(dD.p, D, sizeof(double) * mat, cudaMemcpyHostToDevice));
-    if (d) CFLX_CUDA(cudaMemcpy(dd.p, d, sizeof(double) * M, cudaMemcpyHostToDevice));
-    if (sel) CFLX_CUDA(cudaMemcpy(dsel.p, sel, sizeof(int) * ldn, cudaMemcpyHostToDevice));
+    CFLX_TRY(stage(dA, mat, A));
+    CFLX_TRY(stage(dD, mat, D));
+    CFLX_TRY(stage(dd, M, d));
+    CFLX_TRY(stage(dsel, ldn, sel));
+    CFLX_TRY(stage(dW, mat));
+    CFLX_TRY(stage(dT, mat, T_inout));
+    CFLX_TRY(stage(dv, (size_t)nrhs * REFINE_NSTAT));
     const double* a = dA.as<double>();
     double* w = dW.as<double>();
-    if (max_out) {
-        CFLX_TRY(launch_column_max(a, M, ldn, nrhs, dv.as<double>(), 0));
-        CFLX_CUDA(cudaMemcpy(max_out, dv.p, sizeof(double) * nrhs, cudaMemcpyDeviceToHost));
-    }
-    if (stats_out) {
+    if (max_out) CFLX_TRY(launch_column_max(a, M, ldn, nrhs, dv.as<double>(), 0));
+    CFLX_TRY(fetch(max_out, dv.p, nrhs));
+    if (stats_out)
         CFLX_TRY(launch_column_stats(a, dD.as<double>(), d ? dd.as<double>() : nullptr, M, ldn, nrhs, dv.as<double>(), 0));
-        CFLX_CUDA(cudaMemcpy(stats_out, dv.p, sizeof(double) * nrhs * REFINE_NSTAT, cudaMemcpyDeviceToHost));
-    }
+    CFLX_TRY(fetch(stats_out, dv.p, (size_t)nrhs * REFINE_NSTAT));
     if (select_out) {
         CFLX_TRY(launch_fill(w, mat, std::numeric_limits<double>::quiet_NaN(), 0));
         CFLX_TRY(launch_select_cols(a, dsel.as<int>(), M, ldn, w, 0));
-        CFLX_CUDA(cudaMemcpy(select_out, w, sizeof(double) * mat, cudaMemcpyDeviceToHost));
+        CFLX_TRY(fetch(select_out, w, mat));
     }
     if (add_out) {
         CFLX_CUDA(cudaMemcpy(w, a, sizeof(double) * mat, cudaMemcpyDeviceToDevice));
         CFLX_TRY(launch_add_cols(w, dD.as<double>(), dsel.as<int>(), M, ldn, 0));
-        CFLX_CUDA(cudaMemcpy(add_out, w, sizeof(double) * mat, cudaMemcpyDeviceToHost));
+        CFLX_TRY(fetch(add_out, w, mat));
     }
     if (Y_out) {
         CFLX_CUDA(cudaMemcpy(w, a, sizeof(double) * mat, cudaMemcpyDeviceToDevice));
-        CFLX_CUDA(cudaMemcpy(dT.p, T_inout, sizeof(double) * mat, cudaMemcpyHostToDevice));
         CFLX_TRY(launch_update_x(w, dT.as<double>(), dD.as<double>(), dsel.as<int>(), M, ldn, 0));
-        CFLX_CUDA(cudaMemcpy(Y_out, w, sizeof(double) * mat, cudaMemcpyDeviceToHost));
-        CFLX_CUDA(cudaMemcpy(T_inout, dT.p, sizeof(double) * mat, cudaMemcpyDeviceToHost));
+        CFLX_TRY(fetch(Y_out, w, mat));
+        CFLX_TRY(fetch(T_inout, dT.p, mat));
     }
     CFLX_CUDA(cudaDeviceSynchronize());
     return CFLX_OK;
@@ -661,17 +688,18 @@ int cflx_dbg_refine_columns(int M, int ldn, int nrhs, const double* A, const dou
 int cflx_dbg_det(int n, const double* d, const double* s1, const double* s2, int square, double* mant_out,
                  int64_t* exp_out, int* neg_out, int* first_zero_out, int* nonfinite_out) {
     CFLX_TRY(check_device());
-    if (n < 1 || !d || (square != 0 && square != 1)) return CFLX_ERR_ARG;
-    DevBuf dv, dr;
-    CFLX_TRY(dv.alloc(sizeof(double) * 3 * (size_t)n));
-    CFLX_TRY(dr.alloc(sizeof(DetResult)));
-    double* v = dv.as<double>();
-    CFLX_CUDA(cudaMemcpy(v, d, sizeof(double) * n, cudaMemcpyHostToDevice));
-    if (s1) CFLX_CUDA(cudaMemcpy(v + n, s1, sizeof(double) * n, cudaMemcpyHostToDevice));
-    if (s2) CFLX_CUDA(cudaMemcpy(v + 2 * (size_t)n, s2, sizeof(double) * n, cudaMemcpyHostToDevice));
-    CFLX_TRY(launch_det(v, s1 ? v + n : nullptr, s2 ? v + 2 * (size_t)n : nullptr, n, square != 0, dr.as<DetResult>(), 0));
+    REFUSE_IF(n < 1);
+    REFUSE_IF(!d);
+    REFUSE_IF(square != 0 && square != 1);
+    DevBuf dd, ds1, ds2, dr;
+    CFLX_TRY(stage(dd, n, d));
+    CFLX_TRY(stage(ds1, n, s1));
+    CFLX_TRY(stage(ds2, n, s2));
+    CFLX_TRY(stage<DetResult>(dr, 1));
+    CFLX_TRY(launch_det(dd.as<double>(), s1 ? ds1.as<double>() : nullptr, s2 ? ds2.as<double>() : nullptr, n, square != 0,
+                        dr.as<DetResult>(), 0));
     DetResult r{};
-    CFLX_CUDA(cudaMemcpy(&r, dr.p, sizeof(r), cudaMemcpyDeviceToHost));
+    CFLX_TRY(fetch(&r, dr.p, 1));
     if (mant_out) *mant_out = r.mant;
     if (exp_out) *exp_out = r.exp;
     if (neg_out) *neg_out = r.neg;
@@ -680,97 +708,57 @@ int cflx_dbg_det(int n, const double* d, const double* s1, const double* s2, int
     return CFLX_OK;
 }
 
-// the residual kernels of the refinement (refine.cu) on one layer-0 share; the timed repetitions run first, then the
-// launch whose result is returned
-int cflx_dbg_residual(int mode, int Ml, int Nl, const double* A, int v, int Kappa, int Px, int Py, int pi, int pj,
-                      int nrhs, const double* Xc, const double* Xr, double* P_out, double* Q_out, int reps, double* ms_out) {
+// the residual kernels of the refinement (refine.cu) on one layer-0 share
+int cflx_dbg_residual(int mode, const cflx_share_layout* share, const double* A, int nrhs, const double* Xc,
+                      const double* Xr, double* P_out, double* Q_out, int reps, double* ms_out) {
     CFLX_TRY(check_device());
-    if (mode < 0 || mode > 2 || Ml < 0 || Nl < 0 || (Nl & 1) || v < 4 || (v & 3) || nrhs < 1 || !A || Px < 1 || Py < 1 ||
-        pi < 0 || pi >= Px || pj < 0 || pj >= Py || (mode != 1 && !Xc) || (mode != 0 && !Xr))
-        return CFLX_ERR_ARG;
-    const ResidMode m = mode == 0 ? ResidMode::NN : mode == 1 ? ResidMode::TN : ResidMode::SymLower;
-    const int rows = mode == 0 ? Ml : mode == 1 ? Nl : Ml + Nl;
-    const size_t a_n = (size_t)Ml * Nl, o_n = (size_t)std::max(rows, 1) * nrhs;
-    DevBuf dA, dXc, dXr, dP, dQ;
-    CFLX_TRY(dA.alloc(sizeof(double) * a_n));
-    CFLX_TRY(dXc.alloc(sizeof(double) * (size_t)Nl * nrhs));
-    CFLX_TRY(dXr.alloc(sizeof(double) * (size_t)Ml * nrhs));
-    CFLX_TRY(dP.alloc(sizeof(double) * o_n));
-    CFLX_TRY(dQ.alloc(sizeof(double) * o_n));
-    CFLX_CUDA(cudaMemcpy(dA.p, A, sizeof(double) * a_n, cudaMemcpyHostToDevice));
-    if (Xc) CFLX_CUDA(cudaMemcpy(dXc.p, Xc, sizeof(double) * (size_t)Nl * nrhs, cudaMemcpyHostToDevice));
-    if (Xr) CFLX_CUDA(cudaMemcpy(dXr.p, Xr, sizeof(double) * (size_t)Ml * nrhs, cudaMemcpyHostToDevice));
-    const Layout L{0, v, Kappa, Ml, Nl, Px, Py, pi, pj};  // M: the kernels index by local row and column only
-    auto run = [&]() {
-        return launch_residual(m, dA.as<double>(), L, dXc.as<double>(), dXr.as<double>(), nrhs, nrhs, dP.as<double>(),
-                               dQ.as<double>(), nrhs, 0);
-    };
-    CFLX_TRY(time_reps(run, reps, ms_out));
-    CFLX_CUDA(cudaMemset(dP.p, 0, sizeof(double) * o_n));
-    CFLX_CUDA(cudaMemset(dQ.p, 0, sizeof(double) * o_n));
-    CFLX_TRY(run());
-    if (P_out) CFLX_CUDA(cudaMemcpy(P_out, dP.p, sizeof(double) * (size_t)rows * nrhs, cudaMemcpyDeviceToHost));
-    if (Q_out) CFLX_CUDA(cudaMemcpy(Q_out, dQ.p, sizeof(double) * (size_t)rows * nrhs, cudaMemcpyDeviceToHost));
-    CFLX_CUDA(cudaDeviceSynchronize());
-    return CFLX_OK;
+    Layout L;  // M unused: the kernels index by local row and column only
+    CFLX_TRY(share_layout(__func__, share, 0, &L));
+    REFUSE_IF(mode < 0 || mode > 2);
+    REFUSE_IF(L.v & 3);
+    REFUSE_IF(L.Nl & 1);
+    REFUSE_IF(nrhs < 1);
+    REFUSE_IF(!A || (mode != 1 && !Xc) || (mode != 0 && !Xr));
+    return residual_run(mode, L, A, nrhs, Xc, Xr, P_out, Q_out, reps, ms_out,
+                        [&](ResidMode m, const double* a, const double* xc, const double* xr, double* p, double* q) {
+                            return launch_residual(m, a, L, xc, xr, nrhs, nrhs, p, q, nrhs, 0);
+                        });
 }
 
-int cflx_dbg_residual_x(int mode, int Ml, int Nl, const double* A, int v, int Kappa, int Px, int Py, int pi, int pj,
-                        int nrhs, const double* Xc, const double* Xct, const double* Xr, const double* Xrt, double* hi_out,
-                        double* lo_out, int reps, double* ms_out) {
+int cflx_dbg_residual_x(int mode, const cflx_share_layout* share, const double* A, int nrhs, const double* Xc,
+                        const double* Xct, const double* Xr, const double* Xrt, double* hi_out, double* lo_out, int reps,
+                        double* ms_out) {
     CFLX_TRY(check_device());
-    if (mode < 0 || mode > 2 || Ml < 0 || Nl < 0 || v < 1 || nrhs < 1 || !A || Px < 1 || Py < 1 || pi < 0 || pi >= Px ||
-        pj < 0 || pj >= Py || (mode != 1 && !Xc) || (mode != 0 && !Xr))
-        return CFLX_ERR_ARG;
-    const ResidMode m = mode == 0 ? ResidMode::NN : mode == 1 ? ResidMode::TN : ResidMode::SymLower;
-    const int rows = mode == 0 ? Ml : mode == 1 ? Nl : Ml + Nl;
-    const size_t a_n = (size_t)Ml * Nl, o_n = (size_t)std::max(rows, 1) * nrhs;
-    const size_t c_n = (size_t)Nl * nrhs, r_n = (size_t)Ml * nrhs;
-    DevBuf dA, dXc, dXct, dXr, dXrt, dH, dL;
-    CFLX_TRY(dA.alloc(sizeof(double) * a_n));
-    CFLX_TRY(dXc.alloc(sizeof(double) * c_n));
-    CFLX_TRY(dXct.alloc(sizeof(double) * c_n));
-    CFLX_TRY(dXr.alloc(sizeof(double) * r_n));
-    CFLX_TRY(dXrt.alloc(sizeof(double) * r_n));
-    CFLX_TRY(dH.alloc(sizeof(double) * o_n));
-    CFLX_TRY(dL.alloc(sizeof(double) * o_n));
-    CFLX_CUDA(cudaMemcpy(dA.p, A, sizeof(double) * a_n, cudaMemcpyHostToDevice));
-    if (Xc) CFLX_CUDA(cudaMemcpy(dXc.p, Xc, sizeof(double) * c_n, cudaMemcpyHostToDevice));
-    if (Xct) CFLX_CUDA(cudaMemcpy(dXct.p, Xct, sizeof(double) * c_n, cudaMemcpyHostToDevice));
-    if (Xr) CFLX_CUDA(cudaMemcpy(dXr.p, Xr, sizeof(double) * r_n, cudaMemcpyHostToDevice));
-    if (Xrt) CFLX_CUDA(cudaMemcpy(dXrt.p, Xrt, sizeof(double) * r_n, cudaMemcpyHostToDevice));
-    const Layout L{0, v, Kappa, Ml, Nl, Px, Py, pi, pj};
-    auto run = [&]() {
-        return launch_residual_x(m, dA.as<double>(), L, dXc.as<double>(), Xct ? dXct.as<double>() : nullptr,
-                                 dXr.as<double>(), Xrt ? dXrt.as<double>() : nullptr, nrhs, nrhs, dH.as<double>(),
-                                 dL.as<double>(), nrhs, 0);
-    };
-    CFLX_TRY(time_reps(run, reps, ms_out));
-    CFLX_CUDA(cudaMemset(dH.p, 0, sizeof(double) * o_n));
-    CFLX_CUDA(cudaMemset(dL.p, 0, sizeof(double) * o_n));
-    CFLX_TRY(run());
-    if (hi_out) CFLX_CUDA(cudaMemcpy(hi_out, dH.p, sizeof(double) * (size_t)rows * nrhs, cudaMemcpyDeviceToHost));
-    if (lo_out) CFLX_CUDA(cudaMemcpy(lo_out, dL.p, sizeof(double) * (size_t)rows * nrhs, cudaMemcpyDeviceToHost));
-    CFLX_CUDA(cudaDeviceSynchronize());
-    return CFLX_OK;
+    Layout L;  // M unused, as in cflx_dbg_residual
+    CFLX_TRY(share_layout(__func__, share, 0, &L));
+    REFUSE_IF(mode < 0 || mode > 2);
+    REFUSE_IF(nrhs < 1);
+    REFUSE_IF(!A || (mode != 1 && !Xc) || (mode != 0 && !Xr));
+    DevBuf dXct, dXrt;
+    CFLX_TRY(stage(dXct, (size_t)L.Nl * nrhs, Xct));
+    CFLX_TRY(stage(dXrt, (size_t)L.Ml * nrhs, Xrt));
+    return residual_run(mode, L, A, nrhs, Xc, Xr, hi_out, lo_out, reps, ms_out,
+                        [&](ResidMode m, const double* a, const double* xc, const double* xr, double* hi, double* lo) {
+                            return launch_residual_x(m, a, L, xc, Xct ? dXct.as<double>() : nullptr, xr,
+                                                     Xrt ? dXrt.as<double>() : nullptr, nrhs, nrhs, hi, lo, nrhs, 0);
+                        });
 }
 
 int cflx_dbg_panel(int n, int v, const double* panel, int* perm_out, double* A00_out, double* LU_out, int reps,
                    double* ms_out) {
     CFLX_TRY(check_device());
-    if (n < 0 || v <= 0) return CFLX_ERR_ARG;
+    REFUSE_IF(n < 0 || v <= 0);
     const int64_t ld = std::max<int64_t>(2, round_up(n, 2));
     // host transpose into the kernel's K-major layout
     std::vector<double> WT((size_t)v * ld, 0.0);
     for (int r = 0; r < n; ++r)
         for (int c = 0; c < v; ++c) WT[(size_t)c * ld + r] = panel[(size_t)r * v + c];
     DevBuf dW, dW0, dA00, dA00T, dperm;
-    CFLX_TRY(dW.alloc(sizeof(double) * v * ld));
-    CFLX_TRY(dW0.alloc(sizeof(double) * v * ld));
-    CFLX_TRY(dA00.alloc(sizeof(double) * v * v));
-    CFLX_TRY(dA00T.alloc(sizeof(double) * v * v));
-    CFLX_TRY(dperm.alloc(sizeof(int) * 2 * v));
-    CFLX_CUDA(cudaMemcpy(dW0.p, WT.data(), sizeof(double) * v * ld, cudaMemcpyHostToDevice));
+    CFLX_TRY(stage(dW, WT.size()));
+    CFLX_TRY(stage(dW0, WT.size(), WT.data()));
+    CFLX_TRY(stage(dA00, (size_t)v * v));
+    CFLX_TRY(stage(dA00T, (size_t)v * v));
+    CFLX_TRY(stage<int>(dperm, 2 * (size_t)v));
     CFLX_CUDA(cudaMemset(dA00.p, 0, sizeof(double) * v * v));
     Events<2> ev;
     CFLX_TRY(ev.create());
@@ -798,10 +786,10 @@ int cflx_dbg_panel(int n, int v, const double* panel, int* perm_out, double* A00
         return rc;
     }
     if (ms_out) *ms_out = total / reps;
-    if (perm_out) CFLX_CUDA(cudaMemcpy(perm_out, dperm.p, sizeof(int) * v, cudaMemcpyDeviceToHost));
-    if (A00_out) CFLX_CUDA(cudaMemcpy(A00_out, dA00.p, sizeof(double) * v * v, cudaMemcpyDeviceToHost));
+    CFLX_TRY(fetch(perm_out, dperm.p, v));
+    CFLX_TRY(fetch(A00_out, dA00.p, (size_t)v * v));
     if (LU_out) {
-        CFLX_CUDA(cudaMemcpy(WT.data(), dW.p, sizeof(double) * v * ld, cudaMemcpyDeviceToHost));
+        CFLX_TRY(fetch(WT.data(), dW.p, WT.size()));
         for (int r = 0; r < n; ++r)
             for (int c = 0; c < v; ++c) LU_out[(size_t)r * v + c] = WT[(size_t)c * ld + r];
     }
@@ -812,45 +800,49 @@ int cflx_dbg_panel(int n, int v, const double* panel, int* perm_out, double* A00
 int cflx_dbg_trsm(int n, int v, int nb, int64_t ld, const double* A00, const double* B, double* X_out, const double* R,
                   double* Y_out) {
     CFLX_TRY(check_device());
-    if (n <= 0 || v <= 0 || v % 4 != 0) return CFLX_ERR_ARG;
+    REFUSE_IF(n <= 0 || v <= 0 || v % 4 != 0);
     if (nb == 0)
         for (int c : {128, 64, 32, 16, 8, 4})
             if (!nb && v % c == 0) nb = c;
-    if (nb != 4 && nb != 8 && nb != 16 && nb != 32 && nb != 64 && nb != 128) return CFLX_ERR_UNSUPPORTED;
-    if (v % nb != 0) return CFLX_ERR_ARG;
+    if (nb != 4 && nb != 8 && nb != 16 && nb != 32 && nb != 64 && nb != 128)
+        return refuse(__func__, "nb not 4, 8, 16, 32, 64 or 128", CFLX_ERR_UNSUPPORTED);
+    REFUSE_IF(v % nb != 0);
     if (ld == 0) ld = round_up(n, 2);
-    if ((ld & 1) || ld < round_up(n, 2)) return CFLX_ERR_ARG;
+    REFUSE_IF((ld & 1) || ld < round_up(n, 2));
     // the padding columns [n, ld) of the operand panels hold NaN: they must not reach the n solved columns
     const double nan = std::numeric_limits<double>::quiet_NaN();
     std::vector<double> A00T((size_t)v * v), BT((size_t)v * ld, nan), RT((size_t)v * ld, nan);
     for (int i = 0; i < v; ++i)
         for (int j = 0; j < v; ++j) A00T[(size_t)j * v + i] = A00[(size_t)i * v + j];
-    DevBuf dA, dAT, dUinv, dLinvT, dP, dL, dR, dU;
-    CFLX_TRY(dA.alloc(8 * (size_t)v * v)); CFLX_TRY(dAT.alloc(8 * (size_t)v * v));
-    CFLX_TRY(dUinv.alloc(8 * (size_t)v * v)); CFLX_TRY(dLinvT.alloc(8 * (size_t)v * v));
-    CFLX_TRY(dP.alloc(8 * (size_t)v * ld)); CFLX_TRY(dL.alloc(8 * (size_t)v * ld));
-    CFLX_TRY(dR.alloc(8 * (size_t)v * ld)); CFLX_TRY(dU.alloc(8 * (size_t)v * ld));
-    CFLX_CUDA(cudaMemcpy(dA.p, A00, 8 * (size_t)v * v, cudaMemcpyHostToDevice));
-    CFLX_CUDA(cudaMemcpy(dAT.p, A00T.data(), 8 * (size_t)v * v, cudaMemcpyHostToDevice));
+    const size_t vv = (size_t)v * v, panel = (size_t)v * ld;
+    DevBuf dA, dAT, dUinv, dLinvT;
+    CFLX_TRY(stage(dA, vv, A00));
+    CFLX_TRY(stage(dAT, vv, A00T.data()));
+    CFLX_TRY(stage(dUinv, vv));
+    CFLX_TRY(stage(dLinvT, vv));
     CFLX_TRY(launch_diag_inverses(dA.as<double>(), v, nb, dUinv.as<double>(), dLinvT.as<double>(), 0));
     if (B && X_out) {  // X = B * U^-1, B is n x v row-major
         for (int r = 0; r < n; ++r)
             for (int c = 0; c < v; ++c) BT[(size_t)c * ld + r] = B[(size_t)r * v + c];
-        CFLX_CUDA(cudaMemcpy(dP.p, BT.data(), 8 * (size_t)v * ld, cudaMemcpyHostToDevice));
-        CFLX_CUDA(cudaMemset(dL.p, 0, 8 * (size_t)v * ld));
+        DevBuf dP, dL;
+        CFLX_TRY(stage(dP, panel, BT.data()));
+        CFLX_TRY(stage(dL, panel));
+        CFLX_CUDA(cudaMemset(dL.p, 0, 8 * panel));
         CFLX_TRY(trsm_right_upper_T(dA.as<double>(), dUinv.as<double>(), v, nb, dP.as<double>(), dL.as<double>(), ld, n, 0));
-        CFLX_CUDA(cudaMemcpy(BT.data(), dL.p, 8 * (size_t)v * ld, cudaMemcpyDeviceToHost));
+        CFLX_TRY(fetch(BT.data(), dL.p, panel));
         for (int r = 0; r < n; ++r)
             for (int c = 0; c < v; ++c) X_out[(size_t)r * v + c] = BT[(size_t)c * ld + r];
     }
     if (R && Y_out) {  // Y = L^-1 * R, R is v x n row-major
         for (int i = 0; i < v; ++i)
             for (int c = 0; c < n; ++c) RT[(size_t)i * ld + c] = R[(size_t)i * n + c];
-        CFLX_CUDA(cudaMemcpy(dR.p, RT.data(), 8 * (size_t)v * ld, cudaMemcpyHostToDevice));
-        CFLX_CUDA(cudaMemset(dU.p, 0, 8 * (size_t)v * ld));
+        DevBuf dR, dU;
+        CFLX_TRY(stage(dR, panel, RT.data()));
+        CFLX_TRY(stage(dU, panel));
+        CFLX_CUDA(cudaMemset(dU.p, 0, 8 * panel));
         CFLX_TRY(trsm_left_lower_unit(dAT.as<double>(), dLinvT.as<double>(), v, nb, dR.as<double>(), dU.as<double>(), ld,
                                       (int)round_up(n, 2), 0));
-        CFLX_CUDA(cudaMemcpy(RT.data(), dU.p, 8 * (size_t)v * ld, cudaMemcpyDeviceToHost));
+        CFLX_TRY(fetch(RT.data(), dU.p, panel));
         for (int i = 0; i < v; ++i)
             for (int c = 0; c < n; ++c) Y_out[(size_t)i * n + c] = RT[(size_t)i * ld + c];
     }
@@ -861,16 +853,16 @@ int cflx_dbg_trsm(int n, int v, int nb, int64_t ld, const double* A00, const dou
 // inverses of the nb x nb diagonal blocks of the v x v row-major A00 = L\U: Uinv_out / LinvT_out are [v / nb][nb][nb]
 int cflx_dbg_diag_inverse(int v, int nb, const double* A00, double* Uinv_out, double* LinvT_out) {
     CFLX_TRY(check_device());
-    if (v <= 0 || nb <= 0 || v % nb != 0 || !A00) return CFLX_ERR_ARG;
+    REFUSE_IF(v <= 0 || nb <= 0 || v % nb != 0);
+    REFUSE_IF(!A00);
     const size_t vv = (size_t)v * v, blocks = (size_t)v * nb;
     DevBuf dA, dU, dL;
-    CFLX_TRY(dA.alloc(8 * vv));
-    CFLX_TRY(dU.alloc(8 * blocks));
-    CFLX_TRY(dL.alloc(8 * blocks));
-    CFLX_CUDA(cudaMemcpy(dA.p, A00, 8 * vv, cudaMemcpyHostToDevice));
+    CFLX_TRY(stage(dA, vv, A00));
+    CFLX_TRY(stage(dU, blocks));
+    CFLX_TRY(stage(dL, blocks));
     CFLX_TRY(launch_diag_inverses(dA.as<double>(), v, nb, dU.as<double>(), dL.as<double>(), 0));
-    if (Uinv_out) CFLX_CUDA(cudaMemcpy(Uinv_out, dU.p, 8 * blocks, cudaMemcpyDeviceToHost));
-    if (LinvT_out) CFLX_CUDA(cudaMemcpy(LinvT_out, dL.p, 8 * blocks, cudaMemcpyDeviceToHost));
+    CFLX_TRY(fetch(Uinv_out, dU.p, blocks));
+    CFLX_TRY(fetch(LinvT_out, dL.p, blocks));
     CFLX_CUDA(cudaDeviceSynchronize());
     return CFLX_OK;
 }
@@ -880,17 +872,16 @@ int cflx_dbg_diag_inverse(int v, int nb, const double* A00, double* Uinv_out, do
 // (v % 128 == 0, v >= 256).  L_out = L (zeros above the diagonal), LT_out = L^T, info_out = 1 + first failing column or 0.
 int cflx_dbg_potrf_tile(int v, const double* A, double* L_out, double* LT_out, int* info_out, int variant) {
     CFLX_TRY(check_device());
-    if (!A || v < 4 || v > 512 || variant < 0 || variant > 2 || (variant == 1 && v != 128) ||
-        (variant == 2 && potrf_tile_scratch(v) == 0))
-        return CFLX_ERR_ARG;
+    REFUSE_IF(!A);
+    REFUSE_IF(variant < 0 || variant > 2);
+    REFUSE_IF(v < 4 || v > 512 || (variant == 1 && v != 128) || (variant == 2 && potrf_tile_scratch(v) == 0));
     const size_t vv = (size_t)v * v;
     DevBuf dD, dUT, dUc, dQ, dinfo;
-    CFLX_TRY(dD.alloc(8 * vv));
-    CFLX_TRY(dUT.alloc(8 * vv));
-    CFLX_TRY(dUc.alloc(8 * vv));
-    CFLX_TRY(dinfo.alloc(sizeof(int)));
-    if (variant == 2) CFLX_TRY(dQ.alloc(8 * potrf_tile_scratch(v)));
-    CFLX_CUDA(cudaMemcpy(dD.p, A, 8 * vv, cudaMemcpyHostToDevice));
+    CFLX_TRY(stage(dD, vv, A));
+    CFLX_TRY(stage(dUT, vv));
+    CFLX_TRY(stage(dUc, vv));
+    CFLX_TRY(stage<int>(dinfo, 1));
+    if (variant == 2) CFLX_TRY(stage(dQ, potrf_tile_scratch(v)));
     CFLX_CUDA(cudaMemset(dUT.p, 0, 8 * vv));
     CFLX_CUDA(cudaMemset(dinfo.p, 0, sizeof(int)));
     CFLX_TRY(potrf_setup(v));
@@ -899,9 +890,9 @@ int cflx_dbg_potrf_tile(int v, const double* A, double* L_out, double* LT_out, i
         CFLX_TRY(potrf_block128(dD.as<double>(), v, dUT.as<double>(), v, dUc.as<double>(), dinfo.as<int>(), 0, 0));
     else
         CFLX_TRY(potrf_tile(dD.as<double>(), dUT.as<double>(), dQ.as<double>(), dinfo.as<int>(), 0, v, 0, &launches));
-    if (L_out) CFLX_CUDA(cudaMemcpy(L_out, dD.p, 8 * vv, cudaMemcpyDeviceToHost));
-    if (LT_out) CFLX_CUDA(cudaMemcpy(LT_out, dUT.p, 8 * vv, cudaMemcpyDeviceToHost));
-    if (info_out) CFLX_CUDA(cudaMemcpy(info_out, dinfo.p, sizeof(int), cudaMemcpyDeviceToHost));
+    CFLX_TRY(fetch(L_out, dD.p, vv));
+    CFLX_TRY(fetch(LT_out, dUT.p, vv));
+    CFLX_TRY(fetch(info_out, dinfo.p, 1));
     CFLX_CUDA(cudaDeviceSynchronize());
     return CFLX_OK;
 }
@@ -913,23 +904,24 @@ int cflx_dbg_potrf_tile(int v, const double* A, double* L_out, double* LT_out, i
 int cflx_dbg_push_pivots(int n_rows, int n_cols, double* A_inout, int npiv, const int* pivot_rows, int fnpr, int* gri_out,
                          double* a01_out) {
     CFLX_TRY(check_device());
-    if (n_rows <= 0 || n_cols <= 0 || (n_cols & 1) || npiv < 0 || npiv > n_rows - fnpr || fnpr < 0) return CFLX_ERR_ARG;
+    REFUSE_IF(n_rows <= 0 || n_cols <= 0 || (n_cols & 1));
+    REFUSE_IF(npiv < 0 || fnpr < 0 || npiv > n_rows - fnpr);
     if (npiv == 0) {
         if (gri_out) for (int i = 0; i < n_rows; ++i) gri_out[i] = i;
         return CFLX_OK;
     }
+    REFUSE_IF(!A_inout || !pivot_rows);
     const int v = npiv;  // every pivot of the "tile" lives on this rank
+    const size_t a_n = (size_t)n_rows * n_cols;
     DevBuf dA, dtmp, da01, dplan, dgp, dgri, dgrit, digri;
-    CFLX_TRY(dA.alloc(8 * (size_t)n_rows * n_cols));
-    CFLX_TRY(dtmp.alloc(8 * (size_t)v * n_cols));
-    CFLX_TRY(da01.alloc(8 * (size_t)v * n_cols));
-    CFLX_TRY(dplan.alloc(sizeof(int) * (6 * (size_t)v + 8 + n_rows)));
-    CFLX_TRY(dgp.alloc(sizeof(int) * v));
-    CFLX_TRY(dgri.alloc(sizeof(int) * n_rows));
-    CFLX_TRY(dgrit.alloc(sizeof(int) * n_rows));
-    CFLX_TRY(digri.alloc(sizeof(int) * n_rows));
-    CFLX_CUDA(cudaMemcpy(dA.p, A_inout, 8 * (size_t)n_rows * n_cols, cudaMemcpyHostToDevice));
-    CFLX_CUDA(cudaMemcpy(dgp.p, pivot_rows, sizeof(int) * v, cudaMemcpyHostToDevice));
+    CFLX_TRY(stage(dA, a_n, A_inout));
+    CFLX_TRY(stage(dtmp, (size_t)v * n_cols));
+    CFLX_TRY(stage(da01, (size_t)v * n_cols));
+    CFLX_TRY(stage<int>(dplan, 6 * (size_t)v + 8 + n_rows));
+    CFLX_TRY(stage(dgp, v, pivot_rows));
+    CFLX_TRY(stage<int>(dgri, n_rows));
+    CFLX_TRY(stage<int>(dgrit, n_rows));
+    CFLX_TRY(stage<int>(digri, n_rows));
     MovePlan plan{};
     int* pm = dplan.as<int>();
     plan.npiv = pm; plan.nel = pm + 4; pm += 8;
@@ -947,9 +939,9 @@ int cflx_dbg_push_pivots(int n_rows, int n_cols, double* A_inout, int npiv, cons
     CFLX_TRY(launch_push_phase2(dA.as<double>(), n_cols, n_cols, 0, plan, v, 0));
     CFLX_TRY(launch_push_phase3(dA.as<double>(), n_cols, n_cols, 0, fnpr, plan, v, dtmp.as<double>(), 0));
     CFLX_TRY(launch_update_gri(dgri.as<int>(), dgrit.as<int>(), digri.as<int>(), plan.rowsrc, fnpr, n_rows, n_rows, 1, 0));
-    CFLX_CUDA(cudaMemcpy(A_inout, dA.p, 8 * (size_t)n_rows * n_cols, cudaMemcpyDeviceToHost));
-    if (gri_out) CFLX_CUDA(cudaMemcpy(gri_out, dgri.p, sizeof(int) * n_rows, cudaMemcpyDeviceToHost));
-    if (a01_out) CFLX_CUDA(cudaMemcpy(a01_out, da01.p, 8 * (size_t)v * n_cols, cudaMemcpyDeviceToHost));
+    CFLX_TRY(fetch(A_inout, dA.p, a_n));
+    CFLX_TRY(fetch(gri_out, dgri.p, n_rows));
+    CFLX_TRY(fetch(a01_out, da01.p, (size_t)v * n_cols));
     CFLX_CUDA(cudaDeviceSynchronize());
     return CFLX_OK;
 }
@@ -961,21 +953,22 @@ int cflx_dbg_ozaki_gemm(int M, int N, int K, int row0, int col0, int max_ctas, c
                         const double* C, double* D, signed char* planesA_out, signed char* planesB_out, int* ea_out,
                         int* eb_out, int reps, double* ms_out, double* split_ms_out) {
     CFLX_TRY(check_device());
-    if (M <= 0 || N <= 0 || K <= 0 || (N & 1) || row0 < 0 || col0 < 0 || max_ctas < 0) return CFLX_ERR_ARG;
+    REFUSE_IF(M <= 0 || N <= 0 || K <= 0 || (N & 1));
+    REFUSE_IF(row0 < 0 || col0 < 0 || max_ctas < 0);
+    REFUSE_IF(!AT || !B);
     // AT holds row0 + M operand rows, B col0 + N columns; the planes of all of them are made (B's in the two windows
     // [0, col0) and [col0, col0 + N), as the factorisation's look-ahead splits them), the product reads the window
     const int Ma = row0 + M, Nb = col0 + N;
     const int64_t ldat = round_up(Ma, 2), ldb = Nb, ldc = N;
+    const size_t c_n = (size_t)M * ldc;
     DevBuf dA, dB, dC, dC0;
-    CFLX_TRY(dA.alloc(sizeof(double) * K * ldat));
-    CFLX_TRY(dB.alloc(sizeof(double) * K * ldb));
-    CFLX_TRY(dC.alloc(sizeof(double) * M * ldc));
-    CFLX_TRY(dC0.alloc(sizeof(double) * M * ldc));
+    CFLX_TRY(stage(dA, K * ldat));
+    CFLX_TRY(stage(dB, K * ldb, B));
+    CFLX_TRY(stage(dC, c_n));
+    CFLX_TRY(stage(dC0, c_n, C));
     CFLX_CUDA(cudaMemset(dA.p, 0, sizeof(double) * K * ldat));
     CFLX_CUDA(cudaMemcpy2D(dA.p, ldat * 8, AT, (size_t)Ma * 8, (size_t)Ma * 8, K, cudaMemcpyHostToDevice));
-    CFLX_CUDA(cudaMemcpy(dB.p, B, sizeof(double) * K * ldb, cudaMemcpyHostToDevice));
-    if (C) CFLX_CUDA(cudaMemcpy(dC0.p, C, sizeof(double) * M * ldc, cudaMemcpyHostToDevice));
-    else CFLX_CUDA(cudaMemset(dC0.p, 0, sizeof(double) * M * ldc));
+    if (!C) CFLX_CUDA(cudaMemset(dC0.p, 0, sizeof(double) * c_n));
     Events<3> ev;
     CFLX_TRY(ev.create());
     OzakiWorkspace ws;
@@ -983,7 +976,7 @@ int cflx_dbg_ozaki_gemm(int M, int N, int K, int row0, int col0, int max_ctas, c
     if (reps < 1) reps = 1;
     float ms = 0, ms_split = 0;
     for (int r = 0; r < reps + 1 && rc == CFLX_OK; ++r) {
-        cudaMemcpyAsync(dC.p, dC0.p, sizeof(double) * M * ldc, cudaMemcpyDeviceToDevice, 0);
+        cudaMemcpyAsync(dC.p, dC0.p, sizeof(double) * c_n, cudaMemcpyDeviceToDevice, 0);
         cudaEventRecord(ev[0]);
         rc = ozaki_split_a(&ws, dA.as<double>(), ldat, Ma, 0);
         if (!rc && col0 > 0) rc = ozaki_split_b(&ws, dB.as<double>(), ldb, 0, col0, 0);
@@ -1003,16 +996,15 @@ int cflx_dbg_ozaki_gemm(int M, int N, int K, int row0, int col0, int max_ctas, c
             ms += b;
         }
     }
-    if (rc == CFLX_OK) {
-        if (D) cudaMemcpy(D, dC.p, sizeof(double) * M * ldc, cudaMemcpyDeviceToHost);
-        for (int s = 0; s < 8; ++s) {
-            if (planesA_out) cudaMemcpy(planesA_out + (size_t)s * Ma * K, ws.planesA + (size_t)s * ws.cap_a * K, (size_t)Ma * K, cudaMemcpyDeviceToHost);
-            if (planesB_out) cudaMemcpy(planesB_out + (size_t)s * Nb * K, ws.planesB + (size_t)s * ws.cap_b * K, (size_t)Nb * K, cudaMemcpyDeviceToHost);
-        }
-        if (ea_out) cudaMemcpy(ea_out, ws.ea, sizeof(int) * Ma, cudaMemcpyDeviceToHost);
-        if (eb_out) cudaMemcpy(eb_out, ws.eb, sizeof(int) * Nb, cudaMemcpyDeviceToHost);
-        if (cudaDeviceSynchronize() != cudaSuccess) rc = CFLX_ERR_CUDA;
+    if (rc == CFLX_OK) rc = fetch(D, dC.p, c_n);
+    for (int s = 0; s < 8 && rc == CFLX_OK; ++s) {
+        if (planesA_out) rc = fetch(planesA_out + (size_t)s * Ma * K, ws.planesA + (size_t)s * ws.cap_a * K, (size_t)Ma * K);
+        if (planesB_out && rc == CFLX_OK)
+            rc = fetch(planesB_out + (size_t)s * Nb * K, ws.planesB + (size_t)s * ws.cap_b * K, (size_t)Nb * K);
     }
+    if (rc == CFLX_OK) rc = fetch(ea_out, ws.ea, Ma);
+    if (rc == CFLX_OK) rc = fetch(eb_out, ws.eb, Nb);
+    if (rc == CFLX_OK && cudaDeviceSynchronize() != cudaSuccess) rc = CFLX_ERR_CUDA;
     ozaki_workspace_destroy(&ws);
     if (ms_out) *ms_out = ms / reps;
     if (split_ms_out) *split_ms_out = ms_split / reps;
@@ -1023,7 +1015,7 @@ int cflx_dbg_ozaki_gemm(int M, int N, int K, int row0, int col0, int max_ctas, c
 // operands resident in shared memory).  Returns tera-MACs per second (x2 = TOP/s).
 int cflx_dbg_wgmma_peak(int n, double* tmacs_out) {
     CFLX_TRY(check_device());
-    if (!tmacs_out) return CFLX_ERR_ARG;
+    REFUSE_IF(!tmacs_out);
     return wgmma_peak_probe(n, tmacs_out);
 }
 

@@ -362,92 +362,94 @@ int cflx_dbg_gemm_narrow(int M, int N, int K, const double* A, const double* B, 
  * of the Cholesky solve.  On the device AT gets an even leading dimension >= M, so any M >= 1 can be run. */
 int cflx_dbg_gemm_narrow_tn(int M, int N, int K, const double* AT, const double* B, const double* C, double alpha,
                             double beta, double* D, int reps, double* ms_out);
-/* the residual kernels of cflx_*_refine on one layer-0 share A (Ml x Nl row-major, conflux layout of tile v on grid
- * position (pi, pj) of Px x Py): mode 0 (NN) P = A Xc, Q = |A| |Xc| (Ml rows); 1 (TN) P = A^T Xr, Q = |A|^T |Xr| (Nl rows);
- * 2 the stored lower triangle of the real tiles (global tile index < Kappa), NN over global row >= column into rows
- * [0, Ml) and TN over global row > column into rows [Ml, Ml + Nl).  Xc: Nl x nrhs, Xr: Ml x nrhs (either may be NULL when
- * the mode does not read it).  P_out / Q_out: nrhs columns.  ms_out: mean device time of one launch over reps. */
-int cflx_dbg_residual(int mode, int Ml, int Nl, const double* A, int v, int Kappa, int Px, int Py, int pi, int pj,
-                      int nrhs, const double* Xc, const double* Xr, double* P_out, double* Q_out, int reps, double* ms_out);
-/* the double-double residual kernels of cflx_*_refine_x, arguments as cflx_dbg_residual: hi_out + lo_out = op(A) (X +
- * X_tail) in mode 0, 1 or 2, from Xc + Xct (NN) or Xr + Xrt (TN); either tail may be NULL (zero). */
-int cflx_dbg_residual_x(int mode, int Ml, int Nl, const double* A, int v, int Kappa, int Px, int Py, int pi, int pj,
-                        int nrhs, const double* Xc, const double* Xct, const double* Xr, const double* Xrt, double* hi_out,
-                        double* lo_out, int reps, double* ms_out);
-/* the per-share kernels of cflx_*_equilibrate and cflx_lu_svx on one layer-0 share A (Ml x Nl row-major, conflux layout of
- * tile v at grid position (pi, pj) of Px x Py; Ml, Nl multiples of v; M >= (Ml / v) Px v and >= (Nl / v) Py v global
- * indices).  r, c: M-vectors (r is also the Cholesky's s).  Each output may be NULL:
+/* The share a per-share hook runs on: one rank's row-major Ml x Nl share of a block-cyclic matrix of v x v tiles on a
+ * Px x Py grid.  Global tile (I, J) lives on grid position (I % Px, J % Py) at local tile (I / Px, J / Py), so local row
+ * r of the share at (pi, pj) is global row ((r / v) Px + pi) v + r % v, and local column c likewise with Py and pj.
+ *   M       the global order: M-vectors and M-row buffers are indexed by global row or column;
+ *   v       the tile;  Ml, Nl  the share's rows and columns;  Px, Py  the grid;  pi, pj  the share's position on it;
+ *   Kappa   the real tiles: global tiles with an index >= Kappa are padding, which the symmetric (Cholesky) passes
+ *           neither read nor write.
+ * Every hook that takes one refuses v < 1, Px or Py < 1, a position off the grid (pi outside [0, Px), pj outside
+ * [0, Py)) and Ml or Nl < 0.  Where a hook says so it also needs the share tiled (Ml and Nl multiples of v), covered
+ * (M >= (Ml / v) Px v and M >= (Nl / v) Py v) or non-empty (Ml and Nl >= 1).  A refusal names the condition. */
+typedef struct { int M, v, Kappa, Ml, Nl, Px, Py, pi, pj; } cflx_share_layout;
+/* the residual kernels of cflx_*_refine on one layer-0 share A (Ml x Nl, M unused; Nl even, v a multiple of 4): mode 0
+ * (NN) P = A Xc, Q = |A| |Xc| (Ml rows); 1 (TN) P = A^T Xr, Q = |A|^T |Xr| (Nl rows); 2 the stored lower triangle of the
+ * real tiles, NN over global row >= column into rows [0, Ml) and TN over global row > column into rows [Ml, Ml + Nl).
+ * Xc: Nl x nrhs, Xr: Ml x nrhs (either may be NULL when the mode does not read it).  P_out / Q_out: nrhs columns.
+ * ms_out: mean device time of one launch over reps. */
+int cflx_dbg_residual(int mode, const cflx_share_layout* share, const double* A, int nrhs, const double* Xc,
+                      const double* Xr, double* P_out, double* Q_out, int reps, double* ms_out);
+/* the double-double residual kernels of cflx_*_refine_x, arguments as cflx_dbg_residual but any v: hi_out + lo_out =
+ * op(A) (X + X_tail) in mode 0, 1 or 2, from Xc + Xct (NN) or Xr + Xrt (TN); either tail may be NULL (zero). */
+int cflx_dbg_residual_x(int mode, const cflx_share_layout* share, const double* A, int nrhs, const double* Xc,
+                        const double* Xct, const double* Xr, const double* Xrt, double* hi_out, double* lo_out, int reps,
+                        double* ms_out);
+/* the per-share kernels of cflx_*_equilibrate and cflx_lu_svx on one layer-0 share A (tiled, covered).  r, c: M-vectors
+ * (r is also the Cholesky's s).  Each output may be NULL:
  *   rowmax_out / colmax_out (M): max |a| by global row, max |a| r_i by global column, zeros where the share holds none;
  *   diag_out (M): a_gg on the share's diagonal tiles with a global tile index < Kappa, zeros elsewhere;
  *   scaled_out (Ml x Nl): the share after dlaqge's scaling for equed ('N', 'R', 'C', 'B');
  *   sym_scaled_out (Ml x Nl): the share after dlaqsy's (s_j s_i) a on the real tiles' lower triangle, the rest untouched;
  *   growth_out[2]: {max |a| over global row <= column, max |a|}, both over global columns < ncols (the share read as both
  *   L\U and the input); zero_pivot_out: 1 + the first global g < M on the share's diagonal with a_gg == 0, or 0. */
-int cflx_dbg_equil(int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, int M, const double* A,
-                   const double* r, const double* c, char equed, int ncols, double* rowmax_out, double* colmax_out,
-                   double* diag_out, double* scaled_out, double* sym_scaled_out, double* growth_out, int* zero_pivot_out);
+int cflx_dbg_equil(const cflx_share_layout* share, const double* A, const double* r, const double* c, char equed, int ncols,
+                   double* rowmax_out, double* colmax_out, double* diag_out, double* scaled_out, double* sym_scaled_out,
+                   double* growth_out, int* zero_pivot_out);
 /* the per-column pivot growth pass of cflx_lu_svxx (mode 0), cflx_chol_svxx (mode 1) and cflx_lu_svx on one layer-0
- * share F (the factor) and A (the input), both Ml x Nl in the layout of cflx_dbg_equil (Kappa: the real tiles of mode 1).
- * amax_out / fmax_out (M each, may be NULL), by global column j < ncols, zeros elsewhere: mode 0 max |a_ij| over every
- * row and max |f_ij| over the rows i <= j; mode 1 both over the real tiles' rows j <= i < ncols.  Nothing outside these
- * masks is read. */
-int cflx_dbg_growth_cols(int mode, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, int M, int ncols,
-                         const double* F, const double* A, double* amax_out, double* fmax_out);
-/* the per-share kernels of cflx_lu_inverse (mode 0) and cflx_chol_inverse (mode 1) on one share at grid position (pi, pj)
- * of Px x Py (Ml x Nl row-major, Ml and Nl multiples of v; M >= (Ml / v) Px v and >= (Nl / v) Py v global indices; Kappa:
- * the real tiles of mode 1), for the block of nc columns from global column c0 (c0 + nc <= M).  Each output may be NULL:
+ * share (tiled, covered): F the factor and A the input, both Ml x Nl.  amax_out / fmax_out (M each, may be NULL), by
+ * global column j < ncols, zeros elsewhere: mode 0 max |a_ij| over every row and max |f_ij| over the rows i <= j; mode 1
+ * both over the real tiles' rows j <= i < ncols.  Nothing outside these masks is read. */
+int cflx_dbg_growth_cols(int mode, const cflx_share_layout* share, int ncols, const double* F, const double* A,
+                         double* amax_out, double* fmax_out);
+/* the per-share kernels of cflx_lu_inverse (mode 0) and cflx_chol_inverse (mode 1) on one share (tiled, covered), for
+ * the block of nc columns from global column c0 (c0 + nc <= M).  Each output may be NULL:
  *   W_out (Ml x ldn, ldn = nc rounded up to a multiple of 8): the seed, W[r][j] = (global row of r == c0 + j) for the
  *   first `rows` local rows, zero in the rest;
  *   share_inout (Ml x Nl): column j < nc of X (M x ldx, by global row) scattered into the share, to global column
  *   perm[c0 + j] (mode 0, perm: M ints) or c0 + j (mode 1, real tiles on and below the diagonal only); then, with
  *   zero_fill in mode 1, zeros on every entry that scatter never writes.  Every other entry keeps its value. */
-int cflx_dbg_inverse_share(int mode, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, int M, int c0,
-                           int nc, int rows, const double* X, int ldx, const int* perm, double* W_out,
-                           double* share_inout, int zero_fill);
+int cflx_dbg_inverse_share(int mode, const cflx_share_layout* share, int c0, int nc, int rows, const double* X, int ldx,
+                           const int* perm, double* W_out, double* share_inout, int zero_fill);
 /* the pack and scatter kernels of cflx_lu_solve_local (mode 0) and cflx_chol_solve_local (mode 1) on one right-hand side
- * share at grid position (pi, pj) of Px x Py (Ml rows, a multiple of v; M >= (Ml / v) Px v global rows; Kappa: the real
- * tiles of mode 1), for the block of w columns from global column c0 of an M x nrhs matrix (c0 + w <= nrhs).  The rows
- * are every local row (mode 0) or those of real tiles (mode 1).  Each output may be NULL:
- *   Bk_out (M x ldn, ldn = w rounded up to a multiple of 8): the pack of B (Ml x ldb, ldb >= cflx_rhs_local_cols), the
- *   share's entries of the block by global row, zero elsewhere;
- *   X_inout (Ml x ldx, ldx >= cflx_rhs_local_cols): Xk (M x ldn, by global row) scattered into the share's columns of
- *   the block.  Every other entry keeps its value. */
-int cflx_dbg_solve_local_share(int mode, int Ml, int v, int Kappa, int Px, int Py, int pi, int pj, int M, int nrhs, int c0,
-                               int w, const double* B, int ldb, double* Bk_out, const double* Xk, double* X_inout, int ldx);
+ * share (tiled; Nl = cflx_rhs_local_cols(nrhs, v, Py); M >= (Ml / v) Px v), for the block of w columns from global
+ * column c0 of an M x nrhs matrix (c0 + w <= nrhs).  The rows are every local row (mode 0) or those of real tiles (mode
+ * 1).  Each output may be NULL:
+ *   Bk_out (M x ldn, ldn = w rounded up to a multiple of 8): the pack of B (Ml x ldb, ldb >= Nl), the share's entries of
+ *   the block by global row, zero elsewhere;
+ *   X_inout (Ml x ldx, ldx >= Nl): Xk (M x ldn, by global row) scattered into the share's columns of the block.  Every
+ *   other entry keeps its value. */
+int cflx_dbg_solve_local_share(int mode, const cflx_share_layout* share, int nrhs, int c0, int w, const double* B, int ldb,
+                               double* Bk_out, const double* Xk, double* X_inout, int ldx);
 /* the per-share pass of cflx_lu_rcond's and cflx_chol_rcond's 1-norm (mode 0: every entry; mode 1: the symmetric matrix
- * stored as the lower triangle of its real tiles, global tile index < Kappa) and of the infinity-norm (mode 2) on one
- * layer-0 share A (Ml x Nl row-major, multiples of v, both >= v) at grid position (pi, pj) of Px x Py, before the
- * all-reduce over the grid.  out (M doubles, M >= (Ml / v) Px v and >= (Nl / v) Py v): by global index, this share's part
- * of the column sums of |a| (modes 0, 1) or of the row sums (mode 2), zero where it holds nothing. */
-int cflx_dbg_norm_share(int mode, int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, int M, const double* A,
-                        double* out);
-/* cflx_chol_validate's per-share kernels on one layer-0 share A (Ml x Nl row-major, multiples of v) at grid position
- * (pi, pj) of Px x Py, with Kappa real tiles; each output may be NULL:
+ * stored as the lower triangle of its real tiles) and of the infinity-norm (mode 2) on one layer-0 share A (tiled,
+ * covered, non-empty), before the all-reduce over the grid.  out (M doubles): by global index, this share's part of the
+ * column sums of |a| (modes 0, 1) or of the row sums (mode 2), zero where it holds nothing. */
+int cflx_dbg_norm_share(int mode, const cflx_share_layout* share, const double* A, double* out);
+/* cflx_chol_validate's per-share kernels on one layer-0 share A (tiled, non-empty; M = the larger of (Ml / v) Px v and
+ * (Nl / v) Py v; Kappa >= 1); each output may be NULL:
  *   sumsq_out: the sum of squares of the entries with global row >= global column and global row < Kappa v;
- *   PT_out (v x ldp, ldp = Ml rounded up to even, + 2): the transposed panel of step t (0 <= t < Kappa) as the validation
- *   extracts it on grid column t % Py, PT[c][r] = A[row0 + r][(t / Py) v + c] (row0: the first local row of a tile with a
- *   global index >= t) where the global row is >= t v + c, else 0; its leading dimension is that of the broadcast piece
- *   (the active rows rounded up to even, >= 2).  Entries the kernel does not write, and all of PT off that grid column,
- *   are NaN. */
-int cflx_dbg_chol_validate_share(int Ml, int Nl, int v, int Kappa, int Px, int Py, int pi, int pj, const double* A, int t,
-                                 double* PT_out, double* sumsq_out);
-/* the two extract kernels of step t of cflx_lu_validate's sweep on one layer-0 share C of the packed factors (Ml x Nl
- * row-major, multiples of v) at grid position (pi, pj) of Px x Py, under the sweep's owner guards; each output may be
- * NULL, and entries the kernels do not write are NaN:
+ *   PT_out (v x ldp, ldp = Ml rounded up to even, + 2): the transposed panel of step t (0 <= t < Kappa, (t / Py + 1) v
+ *   <= Nl) as the validation extracts it on grid column t % Py, PT[c][r] = A[row0 + r][(t / Py) v + c] (row0: the first
+ *   local row of a tile with a global index >= t) where the global row is >= t v + c, else 0; its leading dimension is
+ *   that of the broadcast piece (the active rows rounded up to even, >= 2).  Entries the kernel does not write, and all
+ *   of PT off that grid column, are NaN. */
+int cflx_dbg_chol_validate_share(const cflx_share_layout* share, const double* A, int t, double* PT_out, double* sumsq_out);
+/* the two extract kernels of step t of cflx_lu_validate's sweep on one layer-0 share C of the packed factors (tiled,
+ * non-empty, the LU's share of a square matrix: (Ml / v) Px == (Nl / v) Py, M = (Ml / v) Px v, Kappa = M / v; 0 <= t <
+ * Kappa), under the sweep's owner guards; each output may be NULL, and entries the kernels do not write are NaN:
  *   LT_out (v x ldp, ldp = Ml rounded up to even; grid column t % Py): LT[c][r] = the unit lower factor's entry at the
  *   global row of r and global column t v + c, for the local rows r of tiles with a global index >= t;
  *   U_out (v x Nl; grid row t % Px): U[r][lc] = the upper factor's entry at global row t v + r and the global column of
  *   lc, for the local columns lc of tiles with a global index >= t. */
-int cflx_dbg_lu_validate_share(int Ml, int Nl, int v, int Px, int Py, int pi, int pj, const double* C, int t, double* LT_out,
-                               double* U_out);
-/* the column-operand gather of the Cholesky trailing update on one Ml x Nl share (multiples of v) at grid column pj of
- * Px x Py, from the Px broadcast pieces of the transposed panel of the global tiles >= gfirst: pieces holds piece p as
- * v x ldp_p row-major, back to back, ldp_p = the rows of grid row p's share from its first tile >= gfirst on, rounded up
- * to even, >= 2 (what the factorisation broadcasts).  Bc_out (v x Nl): column tile t = the panel's rows of the global
- * tile of the share's local column tile lj0 + t, lj0 its first with a global index >= gfirst; NaN in the tiles after the
- * last one. */
-int cflx_dbg_chol_gather_cols(int v, int Px, int Py, int pj, int Ml, int Nl, int gfirst, const double* pieces,
-                              double* Bc_out);
+int cflx_dbg_lu_validate_share(const cflx_share_layout* share, const double* C, int t, double* LT_out, double* U_out);
+/* the column-operand gather of the Cholesky trailing update on one share (tiled, non-empty; M and Kappa unused; pi is
+ * not read but must lie on the grid like every position) at grid column pj, from the Px broadcast pieces of the
+ * transposed panel of the global tiles >= gfirst: pieces holds piece p as v x ldp_p row-major, back to back, ldp_p =
+ * the rows of grid row p's share from its first tile >= gfirst on, rounded up to even, >= 2 (what the factorisation
+ * broadcasts). Bc_out (v x Nl): column tile t = the panel's rows of the global tile of the share's local column tile
+ * lj0 + t, lj0 its first with a global index >= gfirst; NaN in the tiles after the last one. */
+int cflx_dbg_chol_gather_cols(const cflx_share_layout* share, int gfirst, const double* pieces, double* Bc_out);
 /* the assembly of the refinement's residual from the partials of the Px x Py x Pz ranks: all holds Px Py Pz chunks in
  * rank order ((pi Py + pj) Pz + pk), each ((nn ? Ml : 0) + (tn ? Nl : 0)) rows of 2 ldn (P then Q, or Hi then Lo; NN rows
  * first), of which only the layer-0 chunks are read; B, and each output (may be NULL), M x ldn.  Row g (tile T) adds the

@@ -535,6 +535,48 @@ def test_refine_columns(M):
     assert _same(o["T"][:, :nrhs], wantT)
 
 
+# ----------------------------------------------------------------------------------------------- refusals
+_Z, _X = np.zeros((32, 32)), np.zeros((32, 1))
+# each hook on the share of a 32-row tile-16 matrix at grid row pi = Px = 2 (chol_gather_cols: column pj = Py = 2), off
+# the grid, with every other argument valid
+OFF_GRID = {
+    "residual": lambda: cb.dbg.residual(_Z, "nn", 16, grid=(2, 1), pos=(2, 0), Xc=_X),
+    "residual_x": lambda: cb.dbg.residual_x(_Z, "nn", 16, grid=(2, 1), pos=(2, 0), Xc=_X),
+    "equil": lambda: cb.dbg.equil(_Z, 16, grid=(2, 1), pos=(2, 0)),
+    "growth_cols": lambda: cb.dbg.growth_cols("lu", _Z, _Z, 16, grid=(2, 1), pos=(2, 0)),
+    "inverse_share": lambda: cb.dbg.inverse_share("lu", 16, (2, 1), (2, 0), 64, 0, 8, 32, 64),
+    "solve_local_share": lambda: cb.dbg.solve_local_share("lu", 16, (2, 1), (2, 0), 64, 8, 0, 8, 32, B=_Z[:, :16]),
+    "norm_share": lambda: cb.dbg.norm_share("col", _Z, 16, grid=(2, 1), pos=(2, 0)),
+    "chol_validate_share": lambda: cb.dbg.chol_validate_share(_Z, 16, 2, (2, 1), (2, 0)),
+    "lu_validate_share": lambda: cb.dbg.lu_validate_share(np.zeros((32, 64)), 16, (2, 1), (2, 0)),
+    "chol_gather_cols": lambda: cb.dbg.chol_gather_cols([np.zeros((16, 32))], 16, 1, 2, 2, 32, 32, 0),
+}
+
+
+@pytest.mark.parametrize("hook", list(OFF_GRID))
+def test_share_hooks_refuse_off_grid(hook):
+    """a share off the grid is refused before any kernel runs, with an error that names the hook and the condition,
+    not the text of an earlier failure"""
+    with pytest.raises(cb.ConfluxError, match="unknown probe"):
+        cb.dbg.fp64_peak_ex(99)
+    with pytest.raises(cb.ConfluxError) as e:
+        OFF_GRID[hook]()
+    cond = "pj outside [0, Py)" if hook == "chol_gather_cols" else "pi outside [0, Px)"
+    assert f"cflx_dbg_{hook}: refused, {cond}" in str(e.value)
+    assert "unknown probe" not in str(e.value)
+
+
+def test_hooks_refuse_null_inputs():
+    """a missing input array is refused before anything is uploaded or launched; with no pivots to push, push_pivots
+    reads no array and accepts NULL"""
+    lib = cb.lib()
+    with pytest.raises(cb.ConfluxError, match=r"push_pivots: refused, !A_inout \|\| !pivot_rows"):
+        cb.check(lib.cflx_dbg_push_pivots(8, 8, None, 1, None, 0, None, None), "push_pivots")
+    assert lib.cflx_dbg_push_pivots(8, 8, None, 0, None, 0, None, None) == 0
+    with pytest.raises(cb.ConfluxError, match=r"ozaki_gemm: refused, !AT \|\| !B"):
+        cb.check(lib.cflx_dbg_ozaki_gemm(2, 2, 128, 0, 0, 0, *[None] * 8, 1, None, None), "ozaki_gemm")
+
+
 # ----------------------------------------------------------------------------------------------- end to end
 def test_multi_gpu_chol_padded_grid():
     """N = 288, v = 32 on 2 x 1 x 1: Kappa = 9, so rank (1, 0) holds padding tile row 9 under every column.  With NaN in
