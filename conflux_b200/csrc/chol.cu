@@ -31,11 +31,11 @@ using namespace cflx;
 // traffic lives there) under the update of step k.  sv (cflx_chol_solve): inv(L_jj) blocks forward, inv(L_jj)^T
 // backward; rows of real tiles.  eq: s is eq.*.r, scond eq.*.rowcnd.
 struct cflx_chol : Handle {
-    double *PT = nullptr, *LT = nullptr, *G = nullptr /* [2] */, *Bc = nullptr /* [2] */, *D = nullptr, *A00 = nullptr,
-           *W = nullptr, *Uinv = nullptr, *LinvT = nullptr, *acc = nullptr, *Q = nullptr /* scratch of the blocked tile Cholesky */;
-    int* info = nullptr;
+    DevBuf<double> PT, LT, G /* [2] */, Bc /* [2] */, D, A00, W, Uinv, LinvT, acc;
+    DevBuf<double> Q;  // scratch of the blocked tile Cholesky
+    DevBuf<int> info;
     int64_t ldp = 0, ldb = 0;
-    cudaEvent_t ev_col[2] = {nullptr, nullptr}, ev_panel[2] = {nullptr, nullptr};
+    Events<2> ev_col, ev_panel;
     SubComm j_comm;                  // grid row of one layer (color pi * Pz + pk, key pj), made by the first solve
 };
 
@@ -340,20 +340,6 @@ int chol_pick_nb(int v) {
     for (int nb : {128, 64, 32, 16, 8, 4})
         if (v % nb == 0) return nb;
     return 0;
-}
-
-void free_chol(cflx_chol* ch) {
-    if (!ch) return;
-    cudaSetDevice(ch->comm->device);
-    for (double* p : {ch->PT, ch->LT, ch->W, ch->G, ch->Bc, ch->D, ch->A00, ch->Uinv, ch->LinvT, ch->acc, ch->Q}) cudaFree(p);
-    cudaFree(ch->info);
-    for (int i = 0; i < 2; ++i) {
-        if (ch->ev_col[i]) cudaEventDestroy(ch->ev_col[i]);
-        if (ch->ev_panel[i]) cudaEventDestroy(ch->ev_panel[i]);
-    }
-    if (ch->j_comm.c) ncclCommDestroy(ch->j_comm.c);
-    handle_free(ch);
-    delete ch;
 }
 
 // Broadcast the Px pieces of the (transposed) panel of column block t to every rank and apply
@@ -773,26 +759,20 @@ int cflx_chol_create(cflx_comm* c, int N, int v, int Px, int Py, int Pz, cflx_ch
     }
     int d[6];
     CFLX_TRY(cflx_chol_dims(N, v, Px, Py, Pz, d));
-    auto* ch = new cflx_chol;
+    std::unique_ptr<cflx_chol, void (*)(cflx_chol*)> ch(new cflx_chol, cflx_chol_destroy);
     ch->M = d[0]; ch->Nt = d[1]; ch->Ml = d[2]; ch->Nl = d[3]; ch->nlayr = d[4];
     ch->v = v;
     ch->nb = chol_pick_nb(v);
-    int rc = CFLX_OK;
-    auto fail = [&](int code) {
-        free_chol(ch);
-        return code;
-    };
-    if ((rc = handle_init(ch, &kCholTexts, c, Px, Py, Pz))) return fail(rc);
+    CFLX_TRY(handle_init(ch.get(), &kCholTexts, c, Px, Py, Pz));
     const size_t vv = (size_t)v * v;
     ch->ldp = chol_panel_ld(ch->Ml);
     ch->ldb = round_up(ch->Nl, 2) + 2;
-#define ALLOC(ptr, n) if ((rc = dmalloc(&(ptr), (n)))) return fail(rc)
-    ALLOC(ch->PT, (size_t)v * ch->ldp); ALLOC(ch->LT, (size_t)v * ch->ldp); ALLOC(ch->W, (size_t)v * ch->ldp);
-    ALLOC(ch->G, 2 * (size_t)Px * v * ch->ldp); ALLOC(ch->Bc, 2 * (size_t)v * ch->ldb);
-    ALLOC(ch->D, vv); ALLOC(ch->A00, vv); ALLOC(ch->Uinv, vv); ALLOC(ch->LinvT, vv); ALLOC(ch->acc, 2 + SUMSQ_PARTIALS);
-    ALLOC(ch->info, 4);
-    if (potrf_tile_scratch(v)) ALLOC(ch->Q, potrf_tile_scratch(v));
-#undef ALLOC
+    CFLX_TRY(ch->PT.alloc((size_t)v * ch->ldp)); CFLX_TRY(ch->LT.alloc((size_t)v * ch->ldp));
+    CFLX_TRY(ch->W.alloc((size_t)v * ch->ldp)); CFLX_TRY(ch->G.alloc(2 * (size_t)Px * v * ch->ldp));
+    CFLX_TRY(ch->Bc.alloc(2 * (size_t)v * ch->ldb)); CFLX_TRY(ch->D.alloc(vv)); CFLX_TRY(ch->A00.alloc(vv));
+    CFLX_TRY(ch->Uinv.alloc(vv)); CFLX_TRY(ch->LinvT.alloc(vv)); CFLX_TRY(ch->acc.alloc(2 + SUMSQ_PARTIALS));
+    CFLX_TRY(ch->info.alloc(4));
+    if (potrf_tile_scratch(v)) CFLX_TRY(ch->Q.alloc(potrf_tile_scratch(v)));
     cudaMemsetAsync(ch->PT, 0, (size_t)v * ch->ldp * sizeof(double), c->stream);
     cudaMemsetAsync(ch->LT, 0, (size_t)v * ch->ldp * sizeof(double), c->stream);
     cudaMemsetAsync(ch->W, 0, (size_t)v * ch->ldp * sizeof(double), c->stream);
@@ -800,15 +780,13 @@ int cflx_chol_create(cflx_comm* c, int N, int v, int Px, int Py, int Pz, cflx_ch
     cudaMemsetAsync(ch->Bc, 0, 2 * (size_t)v * ch->ldb * sizeof(double), c->stream);
     cudaMemsetAsync(ch->A0, 0, (size_t)ch->Ml * ch->Nl * sizeof(double), c->stream);
     cudaMemsetAsync(ch->A00, 0, vv * sizeof(double), c->stream);
-    if ((rc = handle_update_setup(ch))) return fail(rc);
-    if ((rc = handle_side_stream(ch))) return fail(rc);
-    for (int i = 0; i < 2; ++i)
-        if (cudaEventCreateWithFlags(&ch->ev_col[i], cudaEventDisableTiming) != cudaSuccess ||
-            cudaEventCreateWithFlags(&ch->ev_panel[i], cudaEventDisableTiming) != cudaSuccess)
-            return fail(CFLX_ERR_CUDA);
-    if ((rc = potrf_setup(v))) return fail(rc);
-    if (cudaStreamSynchronize(c->stream) != cudaSuccess) return fail(CFLX_ERR_CUDA);
-    *out = ch;
+    CFLX_TRY(handle_update_setup(ch.get()));
+    CFLX_TRY(handle_side_stream(ch.get()));
+    CFLX_TRY(ch->ev_col.create(cudaEventDisableTiming));
+    CFLX_TRY(ch->ev_panel.create(cudaEventDisableTiming));
+    CFLX_TRY(potrf_setup(v));
+    if (cudaStreamSynchronize(c->stream) != cudaSuccess) return CFLX_ERR_CUDA;
+    *out = ch.release();
     return CFLX_OK;
 }
 
@@ -917,7 +895,7 @@ int cflx_chol_validate(cflx_chol* ch, double* abs_out, double* rel_out) {
     CFLX_CUDA(cudaSetDevice(c->device));
     const int v = ch->v, Px = ch->Px, Py = ch->Py, Ml = ch->Ml, Nl = ch->Nl;
     const size_t loc = (size_t)Ml * Nl;
-    DevBuf Rbuf;
+    DevBuf<> Rbuf;
     CFLX_TRY(Rbuf.alloc(loc * sizeof(double)));
     double* R = Rbuf.as<double>();
     // every layer replays with the full contraction on layer 0's factor: only layer 0 holds L, so restrict to pk == 0 by
@@ -1008,7 +986,7 @@ int cflx_chol_det(cflx_chol* ch, int unscaled, double* logdet_out, double* mant_
     if (!ch || (unscaled != 0 && unscaled != 1)) return CFLX_ERR_ARG;
     CFLX_TRY(handle_check(ch, "determinant"));
     CFLX_CUDA(cudaSetDevice(ch->comm->device));
-    const double* s = unscaled && ch->eq.fac.equed == 'Y' ? ch->eq.fac.r : nullptr;
+    const double* s = unscaled && ch->eq.fac.equed == 'Y' ? ch->eq.fac.r.p : nullptr;
     DetResult d{};
     CFLX_TRY(det_grid(*ch, &ch->eq, ch->A11, true, s, nullptr, &d));
     if (logdet_out) *logdet_out = det_log(d);
@@ -1058,7 +1036,7 @@ int cflx_chol_refine_x(cflx_chol* ch, int nrhs, const double* B, int ldb, double
     CFLX_TRY(cflx_chol_rcond(ch, &rcond, nullptr));
     if (rcond_out) *rcond_out = rcond;
     const EquilRecord& eq = ch->eq.fac;
-    return refine_x_run(&ch->sv.rf, chol_refine_op(ch), nrhs, B, ldb, X, ldx, eq.equed == 'Y' ? eq.r : nullptr, rcond,
+    return refine_x_run(&ch->sv.rf, chol_refine_op(ch), nrhs, B, ldb, X, ldx, eq.equed == 'Y' ? eq.r.p : nullptr, rcond,
                         err_bnds_comp_out != nullptr, berr_out, err_bnds_norm_out, err_bnds_comp_out, info_out);
 }
 
@@ -1083,7 +1061,7 @@ int cflx_chol_svx(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X, 
     CFLX_TRY(handle_check(ch, "expert solve"));
     CFLX_CUDA(cudaSetDevice(ch->comm->device));
     const EquilRecord& eq = ch->eq.fac;
-    const double* s = eq.equed == 'Y' ? eq.r : nullptr;
+    const double* s = eq.equed == 'Y' ? eq.r.p : nullptr;
     if (equed_out) *equed_out = eq.equed;
     double rcond = 0.0;
     CFLX_TRY(cflx_chol_rcond(ch, &rcond, nullptr));
@@ -1103,7 +1081,7 @@ int cflx_chol_svxx(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X,
     CFLX_TRY(handle_check(ch, "extra-precise expert solve"));
     CFLX_CUDA(cudaSetDevice(ch->comm->device));
     const EquilRecord& eq = ch->eq.fac;
-    const double* s = eq.equed == 'Y' ? eq.r : nullptr;
+    const double* s = eq.equed == 'Y' ? eq.r.p : nullptr;
     if (equed_out) *equed_out = eq.equed;
     std::vector<double> h;
     CFLX_TRY(growth_cols_grid(*ch, &ch->eq, true, ch->A11, ch->A0, ch->M, h));
@@ -1117,6 +1095,12 @@ int cflx_chol_svxx(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X,
 
 int cflx_chol_launch_count(cflx_chol* ch, int64_t* count_out, int reset) { return handle_launch_count(ch, count_out, reset); }
 
-void cflx_chol_destroy(cflx_chol* ch) { free_chol(ch); }
+void cflx_chol_destroy(cflx_chol* ch) {
+    if (!ch) return;
+    cudaSetDevice(ch->comm->device);
+    if (ch->j_comm.c) ncclCommDestroy(ch->j_comm.c);
+    grid_free(ch);
+    delete ch;
+}
 
 }  // extern "C"

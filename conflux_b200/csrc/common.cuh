@@ -4,8 +4,12 @@
 
 #include "../../include/conflux_b200.h"
 
+#include <algorithm>
 #include <cstdint>
 #include <cstdio>
+#include <initializer_list>
+#include <type_traits>
+#include <utility>
 
 namespace cflx {
 
@@ -29,35 +33,111 @@ void set_last_error(const char* fmt, ...);
 
 static inline int64_t round_up(int64_t x, int64_t m) { return (x + m - 1) / m * m; }
 
-// ---- scope-owned device temporaries and timing events: released on every return path ------------------------
+// ---- owned device memory, pinned host memory, events and streams: released by their destructors, so a scope or an
+// object that holds them frees them on every path.  Not copyable.  The current device must be the one they were made on.
+//
+// A device array of T, used as a T*.  alloc(n): max(n, 1) elements and a 4096-byte tail pad (bulk copies may
+// over-read); alloc_exact(n): n elements, no pad.  grow(n) allocates again, with alloc, only when fewer than n elements are held.
+template <class T = char>
 struct DevBuf {
-    void* p = nullptr;
+    T* p = nullptr;
+    size_t n = 0;  // elements held
     DevBuf() = default;
-    DevBuf(const DevBuf&) = delete;
-    DevBuf& operator=(const DevBuf&) = delete;
+    DevBuf(DevBuf&& o) noexcept : p(std::exchange(o.p, nullptr)), n(std::exchange(o.n, 0)) {}
+    DevBuf& operator=(DevBuf&& o) noexcept {
+        std::swap(p, o.p);
+        std::swap(n, o.n);
+        return *this;
+    }
     ~DevBuf() { cudaFree(p); }
-    int alloc(size_t bytes) {
-        CFLX_CUDA(cudaMalloc(&p, bytes + 4096));  // tail pad: bulk copies may over-read
+    void reset() {
+        cudaFree(p);
+        p = nullptr;
+        n = 0;
+    }
+    int alloc(size_t count) { return alloc_bytes(count, std::max<size_t>(count, 1) * sizeof(T) + 4096); }
+    int alloc_exact(size_t count) { return alloc_bytes(count, count * sizeof(T)); }
+    bool holds(size_t count) const { return p && count <= n; }
+    int grow(size_t count) { return holds(count) ? CFLX_OK : alloc(count); }
+    operator T*() const { return p; }
+    template <class U>
+    U* as() const { return (U*)p; }
+
+  private:
+    int alloc_bytes(size_t count, size_t bytes) {
+        reset();
+        CFLX_CUDA(cudaMalloc((void**)&p, bytes));
+        n = count;
         return CFLX_OK;
     }
-    template <class T>
-    T* as() { return (T*)p; }
 };
+// Buffers used together, grown together: unless every one holds n elements, all are freed, then all allocated, so the
+// group is never held twice
+template <class T>
+int grow_together(std::initializer_list<DevBuf<T>*> group, size_t n) {
+    if (std::all_of(group.begin(), group.end(), [n](const DevBuf<T>* b) { return b->holds(n); })) return CFLX_OK;
+    for (DevBuf<T>* b : group) b->reset();
+    for (DevBuf<T>* b : group) CFLX_TRY(b->alloc(n));
+    return CFLX_OK;
+}
+
+// Page-locked host memory of n T, used as a T*
+template <class T>
+struct PinnedBuf {
+    T* p = nullptr;
+    PinnedBuf() = default;
+    PinnedBuf(const PinnedBuf&) = delete;
+    PinnedBuf& operator=(const PinnedBuf&) = delete;
+    ~PinnedBuf() { cudaFreeHost(p); }
+    int alloc(size_t n) {
+        CFLX_CUDA(cudaMallocHost((void**)&p, n * sizeof(T)));
+        return CFLX_OK;
+    }
+    operator T*() const { return p; }
+};
+
+// N events, made by create(flags); Events<1> (Event) is used as the cudaEvent_t itself
 template <int N>
 struct Events {
     cudaEvent_t e[N] = {};
     Events() = default;
-    Events(const Events&) = delete;
-    Events& operator=(const Events&) = delete;
+    Events(Events&& o) noexcept { std::swap(e, o.e); }
+    Events& operator=(Events&& o) noexcept {
+        std::swap(e, o.e);
+        return *this;
+    }
     ~Events() {
         for (cudaEvent_t x : e)
             if (x) cudaEventDestroy(x);
     }
-    int create() {
-        for (cudaEvent_t& x : e) CFLX_CUDA(cudaEventCreate(&x));
+    int create(unsigned flags = cudaEventDefault) {
+        for (cudaEvent_t& x : e) CFLX_CUDA(cudaEventCreateWithFlags(&x, flags));
         return CFLX_OK;
     }
     cudaEvent_t operator[](int i) const { return e[i]; }
+    template <int M = N, class = std::enable_if_t<M == 1>>
+    operator cudaEvent_t() const { return e[0]; }
+};
+using Event = Events<1>;
+
+// A stream made by create(flags), or create(flags, priority)
+struct Stream {
+    cudaStream_t s = nullptr;
+    Stream() = default;
+    Stream(const Stream&) = delete;
+    Stream& operator=(const Stream&) = delete;
+    ~Stream() {
+        if (s) cudaStreamDestroy(s);
+    }
+    int create(unsigned flags) {
+        CFLX_CUDA(cudaStreamCreateWithFlags(&s, flags));
+        return CFLX_OK;
+    }
+    int create(unsigned flags, int priority) {
+        CFLX_CUDA(cudaStreamCreateWithPriority(&s, flags, priority));
+        return CFLX_OK;
+    }
+    operator cudaStream_t() const { return s; }
 };
 
 // cudaFuncSetAttribute is per DEVICE: ranks may be threads of one process driving different GPUs, so the

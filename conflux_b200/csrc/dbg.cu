@@ -54,7 +54,7 @@ int share_layout(const char* who, const cflx_share_layout* s, unsigned need, Lay
 
 // d = a device buffer of n T (with DevBuf's tail pad) holding the host array h, or uninitialised when h is null
 template <class T = double>
-int stage(DevBuf& d, size_t n, const T* h = nullptr) {
+int stage(DevBuf<>& d, size_t n, const T* h = nullptr) {
     CFLX_TRY(d.alloc(sizeof(T) * n));
     if (h) CFLX_CUDA(cudaMemcpy(d.p, h, sizeof(T) * n, cudaMemcpyHostToDevice));
     return CFLX_OK;
@@ -93,7 +93,7 @@ int residual_run(int mode, const Layout& L, const double* A, int nrhs, const dou
     const ResidMode m = mode == 0 ? ResidMode::NN : mode == 1 ? ResidMode::TN : ResidMode::SymLower;
     const int rows = mode == 0 ? L.Ml : mode == 1 ? L.Nl : L.Ml + L.Nl;
     const size_t o_n = (size_t)std::max(rows, 1) * nrhs;
-    DevBuf dA, dXc, dXr, dP, dQ;
+    DevBuf<> dA, dXc, dXr, dP, dQ;
     CFLX_TRY(stage(dA, (size_t)L.Ml * L.Nl, A));
     CFLX_TRY(stage(dXc, (size_t)L.Nl * nrhs, Xc));
     CFLX_TRY(stage(dXr, (size_t)L.Ml * nrhs, Xr));
@@ -116,7 +116,7 @@ int residual_run(int mode, const Layout& L, const double* A, int nrhs, const dou
 // into C itself when D == C (the kernel with D aliasing C).
 template <class Launch>
 int narrow_gemm(size_t c_n, const double* C, double* D, int reps, double* ms_out, Launch&& launch) {
-    DevBuf dC, dT;
+    DevBuf<> dC, dT;
     CFLX_TRY(stage(dC, c_n, C));
     CFLX_TRY(stage(dT, c_n));
     if (!C) CFLX_CUDA(cudaMemset(dC.p, 0, sizeof(double) * c_n));
@@ -199,7 +199,7 @@ int cflx_dbg_fp64_peak_ex(int which, double* burst_out, double* sustained_out) {
     CFLX_CUDA(cudaGetDevice(&dev));
     CFLX_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     const int threads = 256, blocks = sms * 4;
-    DevBuf out;
+    DevBuf<> out;
     CFLX_TRY(out.alloc(sizeof(double) * threads * blocks));
     Events<2> ev;
     CFLX_TRY(ev.create());
@@ -257,7 +257,7 @@ int cflx_dbg_gemm_tn(int M, int N, int K, const double* AT, int at_rows, int64_t
         b_off + (K - 1) * ldb + N > (int64_t)b_rows * ldb || row_off + M > c_rows || col_off + N > ldc)
         return refuse(__func__, "window outside the buffers or misaligned");
     const size_t a_n = (size_t)at_rows * ldat, b_n = (size_t)b_rows * ldb, c_n = (size_t)c_rows * ldc;
-    DevBuf dA, dB, dC, dC0, dD;
+    DevBuf<> dA, dB, dC, dC0, dD;
     CFLX_TRY(stage(dA, a_n, AT));
     CFLX_TRY(stage(dB, b_n, B));
     CFLX_TRY(stage(dC, c_n));
@@ -294,7 +294,7 @@ int cflx_dbg_gemm_narrow(int M, int N, int K, const double* A, const double* B, 
     REFUSE_IF(M <= 0 || N <= 0 || K < 0);
     REFUSE_IF(K & 3);
     REFUSE_IF(!A || !B);
-    DevBuf dA, dB;
+    DevBuf<> dA, dB;
     CFLX_TRY(stage(dA, (size_t)M * K, A));
     CFLX_TRY(stage(dB, (size_t)K * N, B));
     return narrow_gemm((size_t)M * N, C, D, reps, ms_out, [&](const double* c, double* out) {
@@ -310,7 +310,7 @@ int cflx_dbg_gemm_narrow_tn(int M, int N, int K, const double* AT, const double*
     REFUSE_IF(M <= 0 || N <= 0 || K < 0);
     REFUSE_IF(!AT || !B);
     const int64_t ldat = round_up(M, 2);
-    DevBuf dA, dB;
+    DevBuf<> dA, dB;
     CFLX_TRY(stage(dA, K * ldat));
     CFLX_TRY(stage(dB, (size_t)K * N, B));
     if (K > 0) CFLX_CUDA(cudaMemcpy2D(dA.p, ldat * 8, AT, (size_t)M * 8, (size_t)M * 8, K, cudaMemcpyHostToDevice));
@@ -330,7 +330,7 @@ int cflx_dbg_equil(const cflx_share_layout* share, const double* A, const double
     REFUSE_IF(equed != 'N' && equed != 'R' && equed != 'C' && equed != 'B');
     const int M = L.M;
     const size_t a_n = (size_t)L.Ml * L.Nl;
-    DevBuf dA, dW, dr, dc, dv, dg, dz;
+    DevBuf<> dA, dW, dr, dc, dv, dg, dz;
     CFLX_TRY(stage(dA, a_n, A));
     CFLX_TRY(stage(dW, a_n));
     CFLX_TRY(stage(dr, M, r));
@@ -383,7 +383,7 @@ int cflx_dbg_growth_cols(int mode, const cflx_share_layout* share, int ncols, co
     REFUSE_IF(mode != 0 && mode != 1);
     REFUSE_IF(!F || !A);
     const size_t a_n = (size_t)L.Ml * L.Nl;
-    DevBuf dF, dA, dg;
+    DevBuf<> dF, dA, dg;
     CFLX_TRY(stage(dF, a_n, F));
     CFLX_TRY(stage(dA, a_n, A));
     CFLX_TRY(stage(dg, 2 * (size_t)L.M));
@@ -407,7 +407,7 @@ int cflx_dbg_inverse_share(int mode, const cflx_share_layout* share, int c0, int
     REFUSE_IF(share_inout && ldx < nc);
     const size_t w_n = (size_t)L.Ml * round_up(nc, 8);
     if (W_out) {
-        DevBuf dW;
+        DevBuf<> dW;
         CFLX_TRY(stage(dW, w_n));
         CFLX_CUDA(cudaMemset(dW.p, 0, sizeof(double) * w_n));
         CFLX_TRY(launch_inverse_seed(dW.as<double>(), (int)round_up(nc, 8), L, rows, c0, nc, 0));
@@ -415,7 +415,7 @@ int cflx_dbg_inverse_share(int mode, const cflx_share_layout* share, int c0, int
     }
     if (share_inout) {
         const size_t a_n = (size_t)L.Ml * L.Nl;
-        DevBuf dA, dX, dp;
+        DevBuf<> dA, dX, dp;
         CFLX_TRY(stage(dA, a_n, share_inout));
         CFLX_TRY(stage(dX, (size_t)L.M * ldx, X));
         CFLX_TRY(stage(dp, L.M, mode == 0 ? perm : nullptr));
@@ -445,14 +445,14 @@ int cflx_dbg_solve_local_share(int mode, const cflx_share_layout* share, int nrh
     const int rows = solve_local_rows(L, mode == 1), ldn = (int)round_up(w, 8);
     const size_t k_n = (size_t)M * ldn;
     if (Bk_out) {
-        DevBuf dB, dK;
+        DevBuf<> dB, dK;
         CFLX_TRY(stage(dB, (size_t)Ml * ldb, B));
         CFLX_TRY(stage(dK, k_n));
         CFLX_TRY(launch_solve_local_pack(dB.as<double>(), ldb, L, rows, c0, w, dK.as<double>(), ldn, 0));
         CFLX_TRY(fetch(Bk_out, dK.p, k_n));
     }
     if (X_inout) {
-        DevBuf dX, dK;
+        DevBuf<> dX, dK;
         CFLX_TRY(stage(dX, (size_t)Ml * ldx, X_inout));
         CFLX_TRY(stage(dK, k_n, Xk));
         CFLX_TRY(launch_solve_local_scatter(dK.as<double>(), ldn, L, rows, c0, w, dX.as<double>(), ldx, 0));
@@ -472,7 +472,7 @@ int cflx_dbg_norm_share(int mode, const cflx_share_layout* share, const double* 
     REFUSE_IF(!A || !out);
     int ncp = 0, nrp = 0;
     norm1_partials(L, &ncp, &nrp);
-    DevBuf dA, dcol, drow, dout;
+    DevBuf<> dA, dcol, drow, dout;
     CFLX_TRY(stage(dA, (size_t)L.Ml * L.Nl, A));
     CFLX_TRY(stage(dcol, (size_t)ncp * L.Nl));
     CFLX_TRY(stage(drow, (size_t)nrp * L.Ml));
@@ -503,7 +503,7 @@ int cflx_dbg_chol_validate_share(const cflx_share_layout* share, const double* A
     REFUSE_IF(t < 0 || t >= Kappa);
     REFUSE_IF((t / Py + 1) * v > Nl);
     const int64_t ldp = chol_panel_ld(Ml);
-    DevBuf dA, dacc, dPT;
+    DevBuf<> dA, dacc, dPT;
     CFLX_TRY(stage(dA, (size_t)Ml * Nl, A));
     CFLX_TRY(stage(dacc, 1 + SUMSQ_PARTIALS));
     CFLX_TRY(stage(dPT, v * ldp));
@@ -539,7 +539,7 @@ int cflx_dbg_lu_validate_share(const cflx_share_layout* share, const double* C, 
     REFUSE_IF(t < 0 || t >= Kappa);
     const int64_t ldp = round_up(Ml, 2);
     const double nan = std::numeric_limits<double>::quiet_NaN();
-    DevBuf dC, dLT, dU;
+    DevBuf<> dC, dLT, dU;
     CFLX_TRY(stage(dC, (size_t)Ml * Nl, C));
     CFLX_TRY(stage(dLT, v * ldp));
     CFLX_TRY(stage(dU, (size_t)v * Nl));
@@ -569,7 +569,7 @@ int cflx_dbg_chol_gather_cols(const cflx_share_layout* share, int gfirst, const 
     const int v = L.v, Ml = L.Ml, Nl = L.Nl, Px = L.Px, Py = L.Py, pj = L.pj;
     const int64_t ldp = chol_panel_ld(Ml), piece_stride = (int64_t)v * ldp, ldb = Nl;
     const double nan = std::numeric_limits<double>::quiet_NaN();
-    DevBuf dG, dB;
+    DevBuf<> dG, dB;
     CFLX_TRY(stage(dG, Px * piece_stride));
     CFLX_TRY(stage(dB, v * ldb));
     CFLX_TRY(launch_fill(dG.as<double>(), Px * piece_stride, nan, 0));
@@ -612,11 +612,11 @@ int cflx_dbg_refine_assemble(int mode, int Px, int Py, int Pz, int v, int M, int
     REFUSE_IF((nn && M > (Ml / v) * Px * v) || (tn && M > (Nl / v) * Py * v));
     const int64_t chunk = (int64_t)((nn ? Ml : 0) + (tn ? Nl : 0)) * 2 * ldn, mat = (int64_t)M * ldn;
     const int64_t all_n = chunk * Px * Py * Pz;
-    DevBuf dall, dB, dR, dratio, dW, dQ;
+    DevBuf<> dall, dB, dR, dratio, dW, dQ;
     CFLX_TRY(stage(dall, all_n, all));
     CFLX_TRY(stage(dB, mat, B));
     const double nan = std::numeric_limits<double>::quiet_NaN();
-    for (DevBuf* b : {&dR, &dratio, &dW, &dQ}) {
+    for (DevBuf<>* b : {&dR, &dratio, &dW, &dQ}) {
         CFLX_TRY(stage(*b, mat));
         CFLX_TRY(launch_fill(b->as<double>(), mat, nan, 0));
     }
@@ -649,7 +649,7 @@ int cflx_dbg_refine_columns(int M, int ldn, int nrhs, const double* A, const dou
     REFUSE_IF((select_out || add_out || Y_out) && !sel);
     REFUSE_IF(!Y_out != !T_inout);
     const int64_t mat = (int64_t)M * ldn;
-    DevBuf dA, dD, dd, dsel, dW, dT, dv;
+    DevBuf<> dA, dD, dd, dsel, dW, dT, dv;
     CFLX_TRY(stage(dA, mat, A));
     CFLX_TRY(stage(dD, mat, D));
     CFLX_TRY(stage(dd, M, d));
@@ -691,7 +691,7 @@ int cflx_dbg_det(int n, const double* d, const double* s1, const double* s2, int
     REFUSE_IF(n < 1);
     REFUSE_IF(!d);
     REFUSE_IF(square != 0 && square != 1);
-    DevBuf dd, ds1, ds2, dr;
+    DevBuf<> dd, ds1, ds2, dr;
     CFLX_TRY(stage(dd, n, d));
     CFLX_TRY(stage(ds1, n, s1));
     CFLX_TRY(stage(ds2, n, s2));
@@ -734,7 +734,7 @@ int cflx_dbg_residual_x(int mode, const cflx_share_layout* share, const double* 
     REFUSE_IF(mode < 0 || mode > 2);
     REFUSE_IF(nrhs < 1);
     REFUSE_IF(!A || (mode != 1 && !Xc) || (mode != 0 && !Xr));
-    DevBuf dXct, dXrt;
+    DevBuf<> dXct, dXrt;
     CFLX_TRY(stage(dXct, (size_t)L.Nl * nrhs, Xct));
     CFLX_TRY(stage(dXrt, (size_t)L.Ml * nrhs, Xrt));
     return residual_run(mode, L, A, nrhs, Xc, Xr, hi_out, lo_out, reps, ms_out,
@@ -753,7 +753,7 @@ int cflx_dbg_panel(int n, int v, const double* panel, int* perm_out, double* A00
     std::vector<double> WT((size_t)v * ld, 0.0);
     for (int r = 0; r < n; ++r)
         for (int c = 0; c < v; ++c) WT[(size_t)c * ld + r] = panel[(size_t)r * v + c];
-    DevBuf dW, dW0, dA00, dA00T, dperm;
+    DevBuf<> dW, dW0, dA00, dA00T, dperm;
     CFLX_TRY(stage(dW, WT.size()));
     CFLX_TRY(stage(dW0, WT.size(), WT.data()));
     CFLX_TRY(stage(dA00, (size_t)v * v));
@@ -780,7 +780,6 @@ int cflx_dbg_panel(int n, int v, const double* panel, int* perm_out, double* A00
     }
     if (rc == CFLX_OK && n >= v)
         rc = launch_gather_a00(dW.as<double>(), ld, dperm.as<int>(), v, nb, dA00.as<double>(), dA00T.as<double>(), 0);
-    panel_workspace_destroy(&ws);
     if (rc != CFLX_OK) {
         if (rc == CFLX_ERR_CUDA) set_last_error("panel kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
         return rc;
@@ -815,7 +814,7 @@ int cflx_dbg_trsm(int n, int v, int nb, int64_t ld, const double* A00, const dou
     for (int i = 0; i < v; ++i)
         for (int j = 0; j < v; ++j) A00T[(size_t)j * v + i] = A00[(size_t)i * v + j];
     const size_t vv = (size_t)v * v, panel = (size_t)v * ld;
-    DevBuf dA, dAT, dUinv, dLinvT;
+    DevBuf<> dA, dAT, dUinv, dLinvT;
     CFLX_TRY(stage(dA, vv, A00));
     CFLX_TRY(stage(dAT, vv, A00T.data()));
     CFLX_TRY(stage(dUinv, vv));
@@ -824,7 +823,7 @@ int cflx_dbg_trsm(int n, int v, int nb, int64_t ld, const double* A00, const dou
     if (B && X_out) {  // X = B * U^-1, B is n x v row-major
         for (int r = 0; r < n; ++r)
             for (int c = 0; c < v; ++c) BT[(size_t)c * ld + r] = B[(size_t)r * v + c];
-        DevBuf dP, dL;
+        DevBuf<> dP, dL;
         CFLX_TRY(stage(dP, panel, BT.data()));
         CFLX_TRY(stage(dL, panel));
         CFLX_CUDA(cudaMemset(dL.p, 0, 8 * panel));
@@ -836,7 +835,7 @@ int cflx_dbg_trsm(int n, int v, int nb, int64_t ld, const double* A00, const dou
     if (R && Y_out) {  // Y = L^-1 * R, R is v x n row-major
         for (int i = 0; i < v; ++i)
             for (int c = 0; c < n; ++c) RT[(size_t)i * ld + c] = R[(size_t)i * n + c];
-        DevBuf dR, dU;
+        DevBuf<> dR, dU;
         CFLX_TRY(stage(dR, panel, RT.data()));
         CFLX_TRY(stage(dU, panel));
         CFLX_CUDA(cudaMemset(dU.p, 0, 8 * panel));
@@ -856,7 +855,7 @@ int cflx_dbg_diag_inverse(int v, int nb, const double* A00, double* Uinv_out, do
     REFUSE_IF(v <= 0 || nb <= 0 || v % nb != 0);
     REFUSE_IF(!A00);
     const size_t vv = (size_t)v * v, blocks = (size_t)v * nb;
-    DevBuf dA, dU, dL;
+    DevBuf<> dA, dU, dL;
     CFLX_TRY(stage(dA, vv, A00));
     CFLX_TRY(stage(dU, blocks));
     CFLX_TRY(stage(dL, blocks));
@@ -876,7 +875,7 @@ int cflx_dbg_potrf_tile(int v, const double* A, double* L_out, double* LT_out, i
     REFUSE_IF(variant < 0 || variant > 2);
     REFUSE_IF(v < 4 || v > 512 || (variant == 1 && v != 128) || (variant == 2 && potrf_tile_scratch(v) == 0));
     const size_t vv = (size_t)v * v;
-    DevBuf dD, dUT, dUc, dQ, dinfo;
+    DevBuf<> dD, dUT, dUc, dQ, dinfo;
     CFLX_TRY(stage(dD, vv, A));
     CFLX_TRY(stage(dUT, vv));
     CFLX_TRY(stage(dUc, vv));
@@ -913,7 +912,7 @@ int cflx_dbg_push_pivots(int n_rows, int n_cols, double* A_inout, int npiv, cons
     REFUSE_IF(!A_inout || !pivot_rows);
     const int v = npiv;  // every pivot of the "tile" lives on this rank
     const size_t a_n = (size_t)n_rows * n_cols;
-    DevBuf dA, dtmp, da01, dplan, dgp, dgri, dgrit, digri;
+    DevBuf<> dA, dtmp, da01, dplan, dgp, dgri, dgrit, digri;
     CFLX_TRY(stage(dA, a_n, A_inout));
     CFLX_TRY(stage(dtmp, (size_t)v * n_cols));
     CFLX_TRY(stage(da01, (size_t)v * n_cols));
@@ -961,7 +960,7 @@ int cflx_dbg_ozaki_gemm(int M, int N, int K, int row0, int col0, int max_ctas, c
     const int Ma = row0 + M, Nb = col0 + N;
     const int64_t ldat = round_up(Ma, 2), ldb = Nb, ldc = N;
     const size_t c_n = (size_t)M * ldc;
-    DevBuf dA, dB, dC, dC0;
+    DevBuf<> dA, dB, dC, dC0;
     CFLX_TRY(stage(dA, K * ldat));
     CFLX_TRY(stage(dB, K * ldb, B));
     CFLX_TRY(stage(dC, c_n));
@@ -1005,7 +1004,6 @@ int cflx_dbg_ozaki_gemm(int M, int N, int K, int row0, int col0, int max_ctas, c
     if (rc == CFLX_OK) rc = fetch(ea_out, ws.ea, Ma);
     if (rc == CFLX_OK) rc = fetch(eb_out, ws.eb, Nb);
     if (rc == CFLX_OK && cudaDeviceSynchronize() != cudaSuccess) rc = CFLX_ERR_CUDA;
-    ozaki_workspace_destroy(&ws);
     if (ms_out) *ms_out = ms / reps;
     if (split_ms_out) *split_ms_out = ms_split / reps;
     return rc;

@@ -112,7 +112,7 @@ int launch_det(const double* d, const double* s1, const double* s2, int n, bool 
 int det_grid(const Grid& g, EquilState* e, const double* F, bool square, const double* s1, const double* s2,
              DetResult* res) {
     cudaStream_t s = g.comm->stream;
-    if (!e->det) CFLX_TRY(dmalloc(&e->det, (size_t)g.M + 4));  // the M-vector, then the DetResult
+    if (!e->det) CFLX_TRY(e->det.alloc((size_t)g.M + 4));  // the M-vector, then the DetResult
     DetResult* dr = reinterpret_cast<DetResult*>(e->det + g.M);
     CFLX_TRY(diag_grid(g, F, e->det));
     CFLX_TRY(launch_det(e->det, s1, s2, g.M, square, dr, s));

@@ -148,22 +148,6 @@ double pow2i(int n) { return n >= 0 ? std::ldexp(1.0, n) : 1.0 / std::ldexp(1.0,
 // the libm LAPACK calls: at an exact power of two it depends on how log rounds.
 double round_pow2(double x) { return x > 0.0 ? pow2i((int)(std::log(x) / std::log(2.0))) : x; }
 
-// *a and *b (when b is not null) hold at least n doubles each; *cap is their common capacity
-int grow_pair(double** a, double** b, size_t* cap, size_t n) {
-    if (*a && n <= *cap) return CFLX_OK;
-    cudaFree(*a);
-    *a = nullptr;
-    if (b) {
-        cudaFree(*b);
-        *b = nullptr;
-    }
-    *cap = 0;
-    CFLX_TRY(dmalloc(a, n));
-    if (b) CFLX_TRY(dmalloc(b, n));
-    *cap = n;
-    return CFLX_OK;
-}
-
 constexpr unsigned MAX_GRID_Y = 65535;
 
 // all-reduce of an M-vector over the world, then its host copy
@@ -242,19 +226,13 @@ int launch_scale_rows(double* X, int64_t ld, int M, int n, const double* d, cuda
 }
 
 // ---------------------------------------------------------------- state
-void equil_free(EquilState* e) {
-    for (double* p : {e->in.r, e->in.c, e->fac.r, e->fac.c, e->qr, e->qc, e->B, e->X, e->growth, e->det}) cudaFree(p);
-    cudaFree(e->ival);
-    *e = EquilState{};
-}
-
 int equil_record_set(EquilRecord* dst, char equed, double rowcnd, double colcnd, const double* r, const double* c, int n,
                      cudaStream_t s) {
     dst->equed = equed;
     dst->rowcnd = rowcnd;
     dst->colcnd = colcnd;
     if (equed == 'N') return CFLX_OK;
-    CFLX_TRY(grow_pair(&dst->r, &dst->c, &dst->cap, (size_t)n));
+    CFLX_TRY(grow_together({&dst->r, &dst->c}, (size_t)n));
     CFLX_CUDA(cudaMemcpyAsync(dst->r, r, sizeof(double) * n, cudaMemcpyDeviceToDevice, s));
     if (c) CFLX_CUDA(cudaMemcpyAsync(dst->c, c, sizeof(double) * n, cudaMemcpyDeviceToDevice, s));
     return CFLX_OK;
@@ -268,7 +246,7 @@ int equil_pass_on(EquilState* e, int M, bool next_is_plain, cudaStream_t s) {
 }
 
 int equil_grow(EquilState* e, int M, int ldn) {
-    return grow_pair(&e->B, &e->X, &e->cap, (size_t)M * ldn);
+    return grow_together({&e->B, &e->X}, (size_t)M * ldn);
 }
 
 // ---------------------------------------------------------------- dgeequ / dgeequb + dlaqge
@@ -278,7 +256,7 @@ int geequ_grid(const Grid& g, EquilState* e, double* A, bool apply, bool pow2, d
     cudaStream_t s = c->stream;
     const int M = g.M;
     const bool layer0 = g.pk == 0;
-    CFLX_TRY(grow_pair(&e->qr, &e->qc, &e->qcap, (size_t)M));
+    CFLX_TRY(grow_together({&e->qr, &e->qc}, (size_t)M));
     double *r = e->qr, *cs = e->qc;
     std::vector<double> h;
     *info = 0;
@@ -352,7 +330,7 @@ int poequ_grid(const Grid& g, EquilState* e, double* A, bool apply, bool pow2, d
     cflx_comm* c = g.comm;
     cudaStream_t s = c->stream;
     const int N = g.M;
-    CFLX_TRY(grow_pair(&e->qr, &e->qc, &e->qcap, (size_t)N));
+    CFLX_TRY(grow_together({&e->qr, &e->qc}, (size_t)N));
     double* sc = e->qr;
     std::vector<double> h;
     *info = 0;
@@ -410,7 +388,7 @@ int equil_growth_cols(const double* F, const double* A, const Layout& L, bool sy
 int zero_pivot_grid(const Grid& g, EquilState* e, const double* F, int* info) {
     cflx_comm* c = g.comm;
     cudaStream_t s = c->stream;
-    if (!e->ival) CFLX_TRY(dmalloc(&e->ival, 1));
+    if (!e->ival) CFLX_TRY(e->ival.alloc(1));
     if (g.pk == 0) {
         CFLX_TRY(equil_zero_pivot(F, g, e->ival, s));
     } else {  // only layer 0 holds the factors: this rank offers no zero pivot
@@ -430,7 +408,7 @@ int growth_cols_grid(const Grid& g, EquilState* e, bool sym, const double* F, co
                      std::vector<double>& h) {
     cflx_comm* c = g.comm;
     const int M = g.M;
-    CFLX_TRY(grow_pair(&e->growth, nullptr, &e->growth_cap, 2 * (size_t)M));
+    CFLX_TRY(e->growth.grow(2 * (size_t)M));
     if (g.pk == 0) CFLX_TRY(equil_growth_cols(F, A, g, sym, ncols, e->growth, c->stream));
     else CFLX_CUDA(cudaMemsetAsync(e->growth, 0, 2 * sizeof(double) * M, c->stream));
     return reduce_vec(c, e->growth, 2 * M, ncclMax, h);

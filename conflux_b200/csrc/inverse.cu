@@ -130,7 +130,7 @@ int inverse_run(SolveCache* sc, const SolveFactor& f, InvKind kind, const int* p
     CFLX_TRY(solve_cache_grow(sc, f, ldn, kind == InvKind::LU || g.pk == 0, kind == InvKind::Chol));
     // device output is written in place; host output goes through one temporary share, copied out once
     double* dst = nullptr;
-    DevBuf tmp;
+    DevBuf<> tmp;
     const size_t n = (size_t)g.Ml * g.Nl;
     if (Ainv) {
         cudaPointerAttributes at{};

@@ -4,6 +4,9 @@
 #include <cuda_runtime.h>
 
 #include <cstdint>
+#include <memory>
+
+#include "common.cuh"
 
 namespace cflx {
 
@@ -26,16 +29,18 @@ int launch_gemm_tn(const GemmArgs& g, cudaStream_t stream);
 // ---------------------------------------------------------------- ozaki.cu
 // FP64 trailing update on the int8 wgmma path (error-free digit planes): C -= L * U with L^T, U K-major in HBM.
 struct OzakiWorkspace {
-    struct Maps;              // the two CUtensorMap objects (kept out of this header)
-    int8_t* planesA = nullptr;  // [8][cap_a][K]
-    int8_t* planesB = nullptr;  // [8][cap_b][K]
-    int* ea = nullptr;          // [cap_a]
-    int* eb = nullptr;          // [cap_b]
-    Maps* maps = nullptr;
+    struct Maps;                // the two CUtensorMap objects (kept out of this header)
+    DevBuf<int8_t> planesA;     // [8][cap_a][K]
+    DevBuf<int8_t> planesB;     // [8][cap_b][K]
+    DevBuf<int> ea;             // [cap_a]
+    DevBuf<int> eb;             // [cap_b]
+    std::unique_ptr<Maps> maps;
     int K = 0, cap_a = 0, cap_b = 0, sms = 0;
+    OzakiWorkspace();
+    ~OzakiWorkspace();  // where Maps is complete
 };
+// on a new workspace
 int ozaki_workspace_create(OzakiWorkspace* ws, int max_rows, int max_cols, int K);
-void ozaki_workspace_destroy(OzakiWorkspace* ws);
 int ozaki_split_a(OzakiWorkspace* ws, const double* LT, int64_t ld, int n, cudaStream_t s);
 int ozaki_split_b(OzakiWorkspace* ws, const double* U, int64_t ld, int col0, int n, cudaStream_t s);
 int wgmma_peak_probe(int n, double* tmacs_out);
@@ -47,20 +52,20 @@ int launch_ozaki_gemm(OzakiWorkspace* ws, int M, int N, int row0, int col0, doub
 // multipliers only for the others).  perm_out[0..v) = LAPACK-equivalent winners (row index chosen at step j,
 // identity beyond min(n, v)); see panel.cu for the tie-breaking contract.
 struct PanelWorkspace {
-    void* slot_hdr;     // [2][132][4]  LL words (payload32, epoch)
-    void* slot_rows;    // [2][132][64] LL words
+    DevBuf<uint2> slot_hdr;   // [2][132][4]  LL words (payload32, epoch)
+    DevBuf<uint2> slot_rows;  // [2][132][64] LL words
     int epoch;          // host-side running epoch (monotonic across launches)
     int max_ctas;       // co-resident CTA budget (<= 132)
     int cta_cap;        // optional cap on the grid (look-ahead: leave SMs to the trailing update); 0 = none
     // column-owner kernel for panels of <= 1024 rows (tournament stacks)
-    unsigned* sk_flags;  // [1024] epoch of the last publication of column block b
-    int* sk_ppos;        // [v] LAPACK position of every pivot when it was chosen
-    unsigned* sk_ticket; // logical CTA ids in start order
+    DevBuf<unsigned> sk_flags;   // [1024] epoch of the last publication of column block b
+    DevBuf<int> sk_ppos;         // [v] LAPACK position of every pivot when it was chosen
+    DevBuf<unsigned> sk_ticket;  // logical CTA ids in start order
     unsigned sk_epoch, sk_ticket_count;
     int sk_enabled;
 };
+// on a new workspace
 int panel_workspace_create(PanelWorkspace* ws);
-void panel_workspace_destroy(PanelWorkspace* ws);
 int launch_panel_getrf(double* W, int64_t ldw, int n, int v, int* perm_out, PanelWorkspace* ws, cudaStream_t stream);
 // same, and CTA 0 also emits into A00 (v x v) the columns >= (i / nb) * nb of pivot i's L\U row; *nb_used = nb
 int launch_panel_getrf_a00(double* W, int64_t ldw, int n, int v, int* perm_out, double* A00, int* nb_used,

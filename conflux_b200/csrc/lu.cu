@@ -124,8 +124,8 @@ void grid_free(Grid* g) {
 int handle_init(Handle* h, const HandleTexts* texts, cflx_comm* c, int Px, int Py, int Pz) {
     h->texts = texts;
     CFLX_TRY(grid_init(h, c, Px, Py, Pz));
-    CFLX_TRY(dmalloc(&h->A0, (size_t)h->Ml * h->Nl));
-    return dmalloc(&h->A11, (size_t)h->Ml * h->Nl);
+    CFLX_TRY(h->A0.alloc((size_t)h->Ml * h->Nl));
+    return h->A11.alloc((size_t)h->Ml * h->Nl);
 }
 int handle_update_setup(Handle* h) {
     CFLX_TRY(gemm_tn_setup());
@@ -143,17 +143,7 @@ int handle_update_setup(Handle* h) {
 int handle_side_stream(Handle* h) {
     int lo = 0, hi = 0;
     cudaDeviceGetStreamPriorityRange(&lo, &hi);
-    CFLX_CUDA(cudaStreamCreateWithPriority(&h->side, cudaStreamNonBlocking, hi));
-    return CFLX_OK;
-}
-void handle_free(Handle* h) {
-    cudaFree(h->A0);
-    cudaFree(h->A11);
-    solve_cache_free(&h->sv);
-    equil_free(&h->eq);
-    if (h->use_ozaki) ozaki_workspace_destroy(&h->oz);
-    if (h->side) cudaStreamDestroy(h->side);
-    grid_free(h);
+    return h->side.create(cudaStreamNonBlocking, hi);
 }
 int handle_set_local(Handle* h, const double* host_local) {
     CFLX_CUDA(cudaSetDevice(h->comm->device));
@@ -205,20 +195,18 @@ struct PhaseTimer {
     cflx_lu* lu;
     int rg;
     cudaStream_t st;
-    cudaEvent_t a = nullptr, b = nullptr;
+    Events<2> ab;
     int ev = -1;
     PhaseTimer(cflx_lu* l, int region, cudaStream_t stream) : lu(l), rg(region), st(stream) {
         nvtxRangePushA(region_name(rg));
         if (lu->prof_mode == 1) {
-            cudaEventCreate(&a);
-            cudaEventCreate(&b);
-            cudaEventRecord(a, st);
+            ab.create();
+            cudaEventRecord(ab[0], st);
         } else if (lu->prof_mode == 2) {
             ev = (int)lu->tl_recs.size() * 2;
             while ((int)lu->tl_pool.size() < ev + 2) {
-                cudaEvent_t e;
-                cudaEventCreate(&e);
-                lu->tl_pool.push_back(e);
+                lu->tl_pool.emplace_back();
+                lu->tl_pool.back().create();
             }
             lu->tl_recs.push_back({rg, st == lu->comm->stream ? 0 : 1, ev});
             cudaEventRecord(lu->tl_pool[ev], st);
@@ -226,15 +214,13 @@ struct PhaseTimer {
     }
     ~PhaseTimer() {
         if (lu->prof_mode == 1) {
-            cudaEventRecord(b, st);
-            cudaEventSynchronize(b);
+            cudaEventRecord(ab[1], st);
+            cudaEventSynchronize(ab[1]);
             float ms = 0;
-            cudaEventElapsedTime(&ms, a, b);
+            cudaEventElapsedTime(&ms, ab[0], ab[1]);
             lu->phase_ms[region_phase(rg)] += ms;
             lu->region_ms[st == lu->comm->stream ? 0 : 1][rg] += ms;
             lu->region_cnt[st == lu->comm->stream ? 0 : 1][rg]++;
-            cudaEventDestroy(a);
-            cudaEventDestroy(b);
         } else if (lu->prof_mode == 2) {
             cudaEventRecord(lu->tl_pool[ev + 1], st);
         }
@@ -464,8 +450,8 @@ int finish_step(cflx_lu* lu, int k, int& fnpr) {
         }
         const int col_lo = layer0 ? 0 : loff;
         const int64_t ldu0 = std::max(2, ncols);
-        CFLX_TRY(launch_push_phase1(lu->A11, Nl, Nl, col_lo, lu->plan, v, lu->tmp, ncols > 0 ? lu->A01raw : nullptr, ldu0, c0,
-                                    s));
+        CFLX_TRY(launch_push_phase1(lu->A11, Nl, Nl, col_lo, lu->plan, v, lu->tmp, ncols > 0 ? lu->A01raw.p : nullptr, ldu0,
+                                    c0, s));
         CFLX_TRY(launch_push_phase2(lu->A11, Nl, Nl, col_lo, lu->plan, v, s));
         CFLX_TRY(launch_push_phase3(lu->A11, Nl, Nl, col_lo, fnpr_old, lu->plan, v, lu->tmp, s));
         CFLX_TRY(launch_update_gri(lu->gri, lu->gri_tmp, lu->igri, lu->plan.rowsrc, fnpr_old, Ml, v, Px, s));
@@ -557,7 +543,7 @@ int finish_step(cflx_lu* lu, int k, int& fnpr) {
     if (next_col) {
         const int w = std::min(v, ncols);
         CFLX_TRY(trailing_gemm(lu, k, 0, fnpr, n_act, c0, w, ld2, ldu, 0, s));
-        cudaStream_t side = (lu->prof_mode == 1) ? nullptr : lu->side;  // phase profiling serialises everything
+        cudaStream_t side = (lu->prof_mode == 1) ? nullptr : lu->side.s;  // phase profiling serialises everything
         cudaStream_t sp = side ? side : s;
         if (side) {
             CFLX_CUDA(cudaEventRecord(lu->ev_fork, s));
@@ -582,31 +568,6 @@ int finish_step(cflx_lu* lu, int k, int& fnpr) {
     return CFLX_OK;
 }
 
-void free_lu(cflx_lu* lu) {
-    if (!lu) return;
-    cudaSetDevice(lu->comm->device);
-    double* dbl[] = {lu->PT, lu->PT2, lu->W, lu->LT, lu->A01raw, lu->U, lu->tmp, lu->A00, lu->A00T, lu->Uinv, lu->LinvT,
-                     lu->candH, lu->S, lu->W2, lu->bcast, lu->Cbuf, lu->xbuf};
-    for (double* p : dbl) cudaFree(p);
-    int* ints[] = {lu->gri, lu->gri_tmp, lu->igri, lu->perm, lu->gpivots, lu->tagsH, lu->tagsS, lu->hist, lu->plan_mem,
-                   lu->idx_buf};
-    for (int* p : ints) cudaFree(p);
-    if (lu->h_npiv) cudaFreeHost(lu->h_npiv);
-    if (lu->pws.slot_hdr) panel_workspace_destroy(&lu->pws);
-    for (auto& e : lu->ev) cudaEventDestroy(e);
-    for (auto& e : lu->tl_pool) cudaEventDestroy(e);
-    if (lu->ev_fork) cudaEventDestroy(lu->ev_fork);
-    if (lu->ev_join) cudaEventDestroy(lu->ev_join);
-    if (lu->ev_npiv) cudaEventDestroy(lu->ev_npiv);
-    if (lu->copy) cudaStreamDestroy(lu->copy);
-    if (lu->ev_a0_read) cudaEventDestroy(lu->ev_a0_read);
-    if (lu->ev_upload) cudaEventDestroy(lu->ev_upload);
-    for (SubComm* sc : {&lu->jk_comm, &lu->ik_comm})
-        if (sc->c) ncclCommDestroy(sc->c);
-    handle_free(lu);
-    delete lu;
-}
-
 // ---------------------------------------------------------------------------------------------- solve, A X = B
 // The factors in the conflux layout of the validation path (Cbuf, as cflx_lu_get_factors leaves them), described to the
 // solve engine (solve.cu).  Every layer joins the grid-row reduces and grid-column broadcasts (jk / ik communicators,
@@ -621,12 +582,10 @@ int lu_solve_prepare(cflx_lu* lu) {
     std::vector<int> hist(lu->M);
     CFLX_TRY(cflx_lu_get_permutation(lu, hist.data()));
     if (lu->pk == 0) {
-        cudaFree(lu->sv.inv);  // before the redistribution allocates its staging
-        lu->sv.inv = nullptr;
-        if (!lu->Cbuf) CFLX_TRY(dmalloc(&lu->Cbuf, (size_t)Ml * lu->Nl));
+        lu->sv.inv.reset();  // before the redistribution allocates its staging
+        if (!lu->Cbuf) CFLX_TRY(lu->Cbuf.alloc((size_t)Ml * lu->Nl));
         int rc = redistribute_pivoted_rows(lu, hist, true, lu->A11, lu->Cbuf);
-        cudaFree(lu->xbuf);  // 2 x local matrix of staging: do not keep it alive
-        lu->xbuf = nullptr;
+        lu->xbuf.reset();  // 2 x local matrix of staging: do not keep it alive
         if (rc) return rc;
         CFLX_TRY(solve_inverses(&lu->sv, lu_solve_factor(lu), false));
         if (lu->pj == 0) {  // local row (k / Px)*v + i of P*B is row hist[k*v + i] of B, for the tiles k of this grid row
@@ -692,7 +651,7 @@ int lu_sweeps(cflx_lu* lu, bool transposed, bool pa, int nrhs, const double* B, 
     CFLX_TRY(solve_seed(sc, f, ldn, nrhs, B, ldb, SolveSeed{true, sc->cols, lu->Nl, sc->Z}));
     CFLX_TRY(solve_col_sweep(sc, f, ldn, true, Tri::UpperT, sc->Z, lu->Py, true));
     CFLX_TRY(solve_col_sweep(sc, f, ldn, false, Tri::UnitLowerT, sc->X, 1, false));
-    return solve_finish(sc, f, ldn, nrhs, X, ldx, pa ? nullptr : sc->unperm);
+    return solve_finish(sc, f, ldn, nrhs, X, ldx, pa ? nullptr : sc->unperm.p);
 }
 
 const HandleTexts kLuTexts = {
@@ -795,12 +754,12 @@ int cflx_comm_create(int world_size, int world_rank, const void* unique_id, int 
         return CFLX_ERR_ARG;
     }
     CFLX_CUDA(cudaSetDevice(device));
-    auto* c = new cflx_comm;
+    std::unique_ptr<cflx_comm> c(new cflx_comm);
     c->world_size = world_size;
     c->world_rank = world_rank;
     c->device = device;
-    CFLX_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-    CFLX_CUDA(cudaMalloc((void**)&c->d_scratch, sizeof(double)));
+    CFLX_TRY(c->stream.create(cudaStreamNonBlocking));
+    CFLX_TRY(c->d_scratch.alloc_exact(1));
     CFLX_CUDA(cudaMemset(c->d_scratch, 0, sizeof(double)));
     if (world_size > 1) {
         if (!unique_id) {
@@ -811,7 +770,7 @@ int cflx_comm_create(int world_size, int world_rank, const void* unique_id, int 
         std::memcpy(&id, unique_id, sizeof(id));
         CFLX_NCCL(ncclCommInitRank(&c->world, world_size, id, world_rank));
     }
-    *out = c;
+    *out = c.release();
     return CFLX_OK;
 }
 
@@ -825,8 +784,6 @@ void cflx_comm_destroy(cflx_comm* c) {
     if (!c) return;
     cudaSetDevice(c->device);
     if (c->world) ncclCommDestroy(c->world);
-    if (c->stream) cudaStreamDestroy(c->stream);
-    cudaFree(c->d_scratch);
     delete c;
 }
 
@@ -915,32 +872,27 @@ int cflx_lu_create(cflx_comm* c, int M, int N, int v, int Px, int Py, int Pz, cf
         set_last_error("only square matrices are supported (the miniapp passes M = N)");
         return CFLX_ERR_UNSUPPORTED;
     }
-    auto* lu = new cflx_lu;
+    std::unique_ptr<cflx_lu, void (*)(cflx_lu*)> lu(new cflx_lu, cflx_lu_destroy);
     lu->M = d[0]; lu->N = d[1]; lu->Ml = d[2]; lu->Nl = d[3]; lu->Nt = d[4]; lu->nlayr = d[5]; lu->Mt = d[6];
     lu->v = v;
     lu->nb = pick_nb(v);
-    int rc = CFLX_OK;
-    auto fail = [&](int code) {
-        free_lu(lu);
-        return code;
-    };
     // sub-communicators (all ranks call all splits, same order)
-    if ((rc = handle_init(lu, &kLuTexts, c, Px, Py, Pz))) return fail(rc);
-    if ((rc = make_sub(c, lu->pi, lu->pj * Pz + lu->pk, Py * Pz, &lu->jk_comm))) return fail(rc);
-    if ((rc = make_sub(c, lu->pj, lu->pi * Pz + lu->pk, Px * Pz, &lu->ik_comm))) return fail(rc);
+    CFLX_TRY(handle_init(lu.get(), &kLuTexts, c, Px, Py, Pz));
+    CFLX_TRY(make_sub(c, lu->pi, lu->pj * Pz + lu->pk, Py * Pz, &lu->jk_comm));
+    CFLX_TRY(make_sub(c, lu->pj, lu->pi * Pz + lu->pk, Px * Pz, &lu->ik_comm));
 
     const int64_t ldp = round_up(lu->Ml, 2) + 2;
     lu->ldp_max = ldp;
     const size_t pan = (size_t)v * ldp, upan = (size_t)v * (lu->Nl + 2), vv = (size_t)v * v;
-#define ALLOC(ptr, n) if ((rc = dmalloc(&(ptr), (n)))) return fail(rc)
-    ALLOC(lu->PT, pan); ALLOC(lu->PT2, pan); ALLOC(lu->W, pan); ALLOC(lu->LT, pan);
-    ALLOC(lu->A01raw, upan); ALLOC(lu->U, upan); ALLOC(lu->tmp, (size_t)v * lu->Nl);
-    ALLOC(lu->A00, 2 * vv); ALLOC(lu->A00T, 2 * vv); ALLOC(lu->Uinv, vv); ALLOC(lu->LinvT, vv);
-    ALLOC(lu->candH, 2 * vv); ALLOC(lu->S, 2 * vv); ALLOC(lu->W2, 2 * vv); ALLOC(lu->bcast, vv + v);
-    ALLOC(lu->gri, lu->Ml); ALLOC(lu->gri_tmp, lu->Ml); ALLOC(lu->igri, lu->Ml); ALLOC(lu->perm, 2 * v);
-    ALLOC(lu->gpivots, v); ALLOC(lu->tagsH, 2 * v); ALLOC(lu->tagsS, 2 * v); ALLOC(lu->hist, lu->M);
-    ALLOC(lu->plan_mem, 6 * (size_t)v + 8 + lu->Ml);
-#undef ALLOC
+    CFLX_TRY(lu->PT.alloc(pan)); CFLX_TRY(lu->PT2.alloc(pan)); CFLX_TRY(lu->W.alloc(pan)); CFLX_TRY(lu->LT.alloc(pan));
+    CFLX_TRY(lu->A01raw.alloc(upan)); CFLX_TRY(lu->U.alloc(upan)); CFLX_TRY(lu->tmp.alloc((size_t)v * lu->Nl));
+    CFLX_TRY(lu->A00.alloc(2 * vv)); CFLX_TRY(lu->A00T.alloc(2 * vv)); CFLX_TRY(lu->Uinv.alloc(vv));
+    CFLX_TRY(lu->LinvT.alloc(vv)); CFLX_TRY(lu->candH.alloc(2 * vv)); CFLX_TRY(lu->S.alloc(2 * vv));
+    CFLX_TRY(lu->W2.alloc(2 * vv)); CFLX_TRY(lu->bcast.alloc(vv + v));
+    CFLX_TRY(lu->gri.alloc(lu->Ml)); CFLX_TRY(lu->gri_tmp.alloc(lu->Ml)); CFLX_TRY(lu->igri.alloc(lu->Ml));
+    CFLX_TRY(lu->perm.alloc(2 * v)); CFLX_TRY(lu->gpivots.alloc(v)); CFLX_TRY(lu->tagsH.alloc(2 * v));
+    CFLX_TRY(lu->tagsS.alloc(2 * v)); CFLX_TRY(lu->hist.alloc(lu->M));
+    CFLX_TRY(lu->plan_mem.alloc(6 * (size_t)v + 8 + lu->Ml));
     int* pm = lu->plan_mem;
     lu->plan.npiv = pm; lu->plan.nel = pm + 4; pm += 8;
     lu->plan.cur_piv = pm; pm += v;
@@ -950,10 +902,10 @@ int cflx_lu_create(cflx_comm* c, int M, int N, int v, int Px, int Py, int Pz, cf
     lu->plan.late = pm; pm += v;
     pm += v;
     lu->plan.rowsrc = pm;
-    if (cudaMallocHost((void**)&lu->h_npiv, sizeof(int)) != cudaSuccess) return fail(CFLX_ERR_CUDA);
-    if (cudaEventCreateWithFlags(&lu->ev_npiv, cudaEventDisableTiming) != cudaSuccess) return fail(CFLX_ERR_CUDA);
-    if ((rc = panel_workspace_create(&lu->pws))) return fail(rc);
-    if ((rc = handle_update_setup(lu))) return fail(rc);
+    CFLX_TRY(lu->h_npiv.alloc(1));
+    CFLX_TRY(lu->ev_npiv.create(cudaEventDisableTiming));
+    CFLX_TRY(panel_workspace_create(&lu->pws));
+    CFLX_TRY(handle_update_setup(lu.get()));
     lu->h_hist.assign(lu->M, -1);
     {
         // look-ahead: pivot search of iteration k+1 (extract, layer reduce, local search, tournament exchanges) on a
@@ -964,9 +916,9 @@ int cflx_lu_create(cflx_comm* c, int M, int N, int v, int Px, int Py, int Pz, cf
         const char* em = getenv("CFLX_LOOKAHEAD_MULTI");  // multi-rank grids: on by default (validated on 2x2x1 / 1x1x2)
         const bool want = (e ? atoi(e) != 0 : true) && (lu->P == 1 || !em || atoi(em) != 0);
         if (want) {
-            if ((rc = handle_side_stream(lu))) return fail(rc);
-            if (cudaEventCreateWithFlags(&lu->ev_fork, cudaEventDisableTiming) != cudaSuccess) return fail(CFLX_ERR_CUDA);
-            if (cudaEventCreateWithFlags(&lu->ev_join, cudaEventDisableTiming) != cudaSuccess) return fail(CFLX_ERR_CUDA);
+            CFLX_TRY(handle_side_stream(lu.get()));
+            CFLX_TRY(lu->ev_fork.create(cudaEventDisableTiming));
+            CFLX_TRY(lu->ev_join.create(cudaEventDisableTiming));
             const char* c = getenv("CFLX_PANEL_CTAS");
             // SMs of the look-ahead pivot search: fewer on one GPU (no tournament), more where the tournament exchanges
             // sit on the critical path; CFLX_PANEL_CTAS overrides
@@ -981,8 +933,8 @@ int cflx_lu_create(cflx_comm* c, int M, int N, int v, int Px, int Py, int Pz, cf
     cudaMemsetAsync(lu->A01raw, 0, upan * sizeof(double), c->stream);
     cudaMemsetAsync(lu->U, 0, upan * sizeof(double), c->stream);
     cudaMemsetAsync(lu->A0, 0, (size_t)lu->Ml * lu->Nl * sizeof(double), c->stream);
-    if (cudaStreamSynchronize(c->stream) != cudaSuccess) return fail(CFLX_ERR_CUDA);
-    *out = lu;
+    if (cudaStreamSynchronize(c->stream) != cudaSuccess) return CFLX_ERR_CUDA;
+    *out = lu.release();
     return CFLX_OK;
 }
 
@@ -1014,9 +966,9 @@ int cflx_lu_queue_next_local(cflx_lu* lu, const double* host_next) {
     }
     CFLX_CUDA(cudaSetDevice(lu->comm->device));
     if (!lu->copy) {
-        CFLX_CUDA(cudaStreamCreateWithFlags(&lu->copy, cudaStreamNonBlocking));
-        CFLX_CUDA(cudaEventCreateWithFlags(&lu->ev_a0_read, cudaEventDisableTiming));
-        CFLX_CUDA(cudaEventCreateWithFlags(&lu->ev_upload, cudaEventDisableTiming));
+        CFLX_TRY(lu->copy.create(cudaStreamNonBlocking));
+        CFLX_TRY(lu->ev_a0_read.create(cudaEventDisableTiming));
+        CFLX_TRY(lu->ev_upload.create(cudaEventDisableTiming));
     }
     lu->next_host = host_next;
     return CFLX_OK;
@@ -1064,13 +1016,12 @@ int cflx_lu_factor(cflx_lu* lu, double* ms_out) {
     lu->gemm_flops = 0;
     lu->gemm_ms = 0;
     if (lu->time_gemm && (int)lu->ev.size() < 4 * lu->Nt) {
-        for (auto& e : lu->ev) cudaEventDestroy(e);
-        lu->ev.assign(4 * lu->Nt, nullptr);
-        for (auto& e : lu->ev) CFLX_CUDA(cudaEventCreate(&e));
+        lu->ev = std::vector<Event>(4 * lu->Nt);
+        for (Event& e : lu->ev) CFLX_TRY(e.create());
     }
     lu->ev_used.assign(2 * lu->Nt, 0);
     {
-        cudaStream_t side = (lu->prof_mode == 1) ? nullptr : lu->side;
+        cudaStream_t side = (lu->prof_mode == 1) ? nullptr : lu->side.s;
         if (side) {
             CFLX_CUDA(cudaEventRecord(lu->ev_fork, s));
             CFLX_CUDA(cudaStreamWaitEvent(side, lu->ev_fork, 0));
@@ -1141,7 +1092,7 @@ int cflx_lu_get_factors(cflx_lu* lu, double* C_host, int* perm_out) {
     if (perm_out) std::memcpy(perm_out, hist.data(), sizeof(int) * lu->M);
     if (lu->pk != 0) return CFLX_OK;  // only layer 0 holds factors
     const size_t loc = (size_t)lu->Ml * lu->Nl;
-    if (!lu->Cbuf) CFLX_TRY(dmalloc(&lu->Cbuf, loc));
+    if (!lu->Cbuf) CFLX_TRY(lu->Cbuf.alloc(loc));
     CFLX_TRY(redistribute_pivoted_rows(lu, hist, true, lu->A11, lu->Cbuf));
     if (C_host) CFLX_CUDA(cudaMemcpyAsync(C_host, lu->Cbuf, loc * sizeof(double), cudaMemcpyDeviceToHost, s));
     CFLX_CUDA(cudaStreamSynchronize(s));
@@ -1227,8 +1178,8 @@ int cflx_lu_det(cflx_lu* lu, int unscaled, double* sign_out, double* logabsdet_o
     CFLX_CUDA(cudaSetDevice(lu->comm->device));
     if (!lu->sv.ready) CFLX_TRY(lu_solve_prepare(lu));
     const EquilRecord& eq = lu->eq.fac;
-    const double* r = unscaled && (eq.equed == 'R' || eq.equed == 'B') ? eq.r : nullptr;
-    const double* c = unscaled && (eq.equed == 'C' || eq.equed == 'B') ? eq.c : nullptr;
+    const double* r = unscaled && (eq.equed == 'R' || eq.equed == 'B') ? eq.r.p : nullptr;
+    const double* c = unscaled && (eq.equed == 'C' || eq.equed == 'B') ? eq.c.p : nullptr;
     DetResult d{};
     CFLX_TRY(det_grid(*lu, &lu->eq, lu->Cbuf, false, r, c, &d));
     std::vector<int> perm(lu->M);
@@ -1283,8 +1234,8 @@ int cflx_lu_refine_x(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb,
     CFLX_TRY(lu_rcond(lu, !t, &rcond, nullptr));
     if (rcond_out) *rcond_out = rcond;
     const EquilRecord& eq = lu->eq.fac;
-    const double* d = !t && (eq.equed == 'C' || eq.equed == 'B') ? eq.c
-                      : t && (eq.equed == 'R' || eq.equed == 'B') ? eq.r
+    const double* d = !t && (eq.equed == 'C' || eq.equed == 'B') ? eq.c.p
+                      : t && (eq.equed == 'R' || eq.equed == 'B') ? eq.r.p
                                                                    : nullptr;
     return refine_x_run(&lu->sv.rf, lu_refine_op(lu, t), nrhs, B, ldb, X, ldx, d, rcond, err_bnds_comp_out != nullptr,
                         berr_out, err_bnds_norm_out, err_bnds_comp_out, info_out);
@@ -1332,7 +1283,7 @@ int cflx_lu_svxx(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, dou
     CFLX_TRY(lu_rcond(lu, !t, &rcond, nullptr));
     *rcond_out = rcond;
     // B is scaled by the scales of the rows of op(A), X (and the bounds' d) by those of its columns
-    const double *r = rowequ ? eq.r : nullptr, *c = colequ ? eq.c : nullptr;
+    const double *r = rowequ ? eq.r.p : nullptr, *c = colequ ? eq.c.p : nullptr;
     return svxx_run(&lu->eq, &lu->sv.rf, lu_refine_op(lu, t), nrhs, B, ldb, X, ldx, t ? c : r, t ? r : c, t ? r : c,
                     rcond, err_bnds_comp_out != nullptr, berr_out, err_bnds_norm_out, err_bnds_comp_out, info_out);
 }
@@ -1364,7 +1315,7 @@ int cflx_lu_svx(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, doub
     CFLX_TRY(lu_rcond(lu, t, &rcond, nullptr));
     *rcond_out = rcond;
     // op(A) X = B: B is scaled by the scales of the rows of op(A), X by those of its columns
-    const double *r = rowequ ? eq.r : nullptr, *c = colequ ? eq.c : nullptr;
+    const double *r = rowequ ? eq.r.p : nullptr, *c = colequ ? eq.c.p : nullptr;
     return svx_run(&lu->eq, &lu->sv.rf, lu_refine_op(lu, t), nrhs, B, ldb, X, ldx, ferr_out, berr_out, t ? c : r,
                    t ? r : c, t ? eq.rowcnd : eq.colcnd, rcond, info_out);
 }
@@ -1440,6 +1391,13 @@ int cflx_lu_trailing_stats(cflx_lu* lu, double* ms_out, double* flops_out) {
     *flops_out = lu->gemm_flops;
     return CFLX_OK;
 }
-void cflx_lu_destroy(cflx_lu* lu) { free_lu(lu); }
+void cflx_lu_destroy(cflx_lu* lu) {
+    if (!lu) return;
+    cudaSetDevice(lu->comm->device);
+    for (SubComm* sc : {&lu->jk_comm, &lu->ik_comm})
+        if (sc->c) ncclCommDestroy(sc->c);
+    grid_free(lu);
+    delete lu;
+}
 
 }  // extern "C"

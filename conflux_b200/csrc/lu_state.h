@@ -25,8 +25,8 @@
 struct cflx_comm {
     int world_size = 1, world_rank = 0, device = 0;
     ncclComm_t world = nullptr;
-    cudaStream_t stream = nullptr;
-    double* d_scratch = nullptr;  // 1 double for barriers
+    cflx::Stream stream;
+    cflx::DevBuf<double> d_scratch;  // 1 double for barriers
 };
 
 namespace cflx {
@@ -57,11 +57,6 @@ inline int region_phase(int r) {
     return p[r];
 }
 
-template <class T>
-inline int dmalloc(T** p, size_t n) {
-    CFLX_CUDA(cudaMalloc((void**)p, std::max<size_t>(n, 1) * sizeof(T) + 4096));  // tail pad: bulk copies may over-read
-    return CFLX_OK;
-}
 int make_sub(cflx_comm* c, int color, int key, int size, SubComm* out);
 int grid_barrier(cflx_comm* c);
 
@@ -112,13 +107,11 @@ void grid_free(Grid* g);
 // gl_rows: the row of X that each local column / row of the layer-0 share multiplies (made on first use; the layout does
 // not change with the matrix).
 struct RefineCache {
-    int *gl_rows = nullptr, *gl_cols = nullptr, *active = nullptr;
-    double *X = nullptr, *B = nullptr, *R = nullptr, *D = nullptr, *rhs = nullptr, *ratio = nullptr, *W = nullptr;
-    double *Xc = nullptr, *Xr = nullptr, *part = nullptr, *all = nullptr, *berr = nullptr;
-    size_t cap_m = 0, cap_c = 0, cap_r = 0, cap_part = 0, cap_all = 0, cap_berr = 0, cap_active = 0;
+    DevBuf<int> gl_rows, gl_cols, active;
+    DevBuf<double> X, B, R, D, rhs, ratio, W;  // M x ldn each, grown together
+    DevBuf<double> Xc, Xr, part, all, berr;
     // cflx_*_refine_x only: the tail of X (M x ldn) and its gathered copies, the per-column statistics of a round
-    double *T = nullptr, *Xct = nullptr, *Xrt = nullptr, *stats = nullptr;
-    size_t cap_t = 0, cap_ct = 0, cap_rt = 0, cap_stats = 0;
+    DevBuf<double> T, Xct, Xrt, stats;
 };
 
 // ---------------------------------------------------------------- equilibration and the expert drivers (equil.cu)
@@ -129,23 +122,18 @@ struct RefineCache {
 struct EquilRecord {
     char equed = 'N';
     double rowcnd = 1.0, colcnd = 1.0;
-    double *r = nullptr, *c = nullptr;  // cap doubles each
-    size_t cap = 0;
+    DevBuf<double> r, c;  // grown together
 };
 // The records of the input and of the factors, the results of the last equilibrate call (which change no record unless
 // that call scaled the input), and the device work buffers of svx.  Buffers are grown, never shrunk.
 struct EquilState {
     EquilRecord in, fac;
-    double *qr = nullptr, *qc = nullptr;  // the last call's scales (dgeequ's r, c; dpoequ's s in qr): qcap doubles each
-    size_t qcap = 0;
-    double *B = nullptr, *X = nullptr;    // svx: M x ldn each, cap doubles each
-    size_t cap = 0;
-    double* growth = nullptr;             // the pivot growth's maxima by column: amax (M), then fmax (M); growth_cap
-    size_t growth_cap = 0;                // doubles
-    int* ival = nullptr;                  // 1 int: the first zero pivot
-    double* det = nullptr;                // M + 4 doubles: the gathered diagonal, then det_grid's DetResult
+    DevBuf<double> qr, qc;  // the last call's scales (dgeequ's r, c; dpoequ's s in qr), grown together
+    DevBuf<double> B, X;    // svx: M x ldn each, grown together
+    DevBuf<double> growth;  // the pivot growth's maxima by column: amax (M), then fmax (M)
+    DevBuf<int> ival;       // 1 int: the first zero pivot
+    DevBuf<double> det;     // M + 4 doubles: the gathered diagonal, then det_grid's DetResult
 };
-void equil_free(EquilState* e);
 // *dst = {equed, rowcnd, colcnd} with device copies of r and c (n each; c may be null: then only r is kept)
 int equil_record_set(EquilRecord* dst, char equed, double rowcnd, double colcnd, const double* r, const double* c, int n,
                      cudaStream_t s);
@@ -156,15 +144,15 @@ int equil_pass_on(EquilState* e, int M, bool next_is_plain, cudaStream_t s);
 // set_local / factor, freed with the object.  The work buffers have ldn columns and are grown, never shrunk.
 struct SolveCache {
     bool ready = false;
-    double* inv = nullptr;  // per owned diagonal tile: the forward inverse blocks (v x nb, row-major nb x nb each), then
-                            // the backward ones
-    int* rows = nullptr;    // row of B of each seeded local row (ranks (pi, 0, 0))
+    DevBuf<double> inv;  // per owned diagonal tile: the forward inverse blocks (v x nb, row-major nb x nb each), then
+                         // the backward ones
+    DevBuf<int> rows;    // row of B of each seeded local row (ranks (pi, 0, 0))
     // the transposed LU solve and the LU condition estimate, prepared on first use after solve data is prepared
     bool trans_ready = false;
-    int* rows_id = nullptr;  // identity row map by local tile row (ranks (pi, 0, 0)): P*A solved without P
-    int* cols = nullptr;     // row of B of each seeded local column (ranks (0, pj, 0))
-    int* unperm = nullptr;   // row of the solved system that lands in each row of X: X[perm[q]] = W[q] (every rank)
-    double *B = nullptr, *W = nullptr, *Z = nullptr, *R = nullptr, *Y = nullptr, *X = nullptr, *Xg = nullptr;
+    DevBuf<int> rows_id;  // identity row map by local tile row (ranks (pi, 0, 0)): P*A solved without P
+    DevBuf<int> cols;     // row of B of each seeded local column (ranks (0, pj, 0))
+    DevBuf<int> unperm;   // row of the solved system that lands in each row of X: X[perm[q]] = W[q] (every rank)
+    DevBuf<double> B, W, Z, R, Y, X, Xg;  // grown together
     int ldn = 0;
     bool col_partials = false, col_seed = false;  // what the buffers were grown for (kept across growth)
     RefineCache rf;
@@ -209,11 +197,11 @@ struct HandleTexts {
 // equilibrate and factor, the trailing-update choice, the look-ahead stream, the solve cache and the scaling records.
 struct Handle : Grid {
     const HandleTexts* texts = nullptr;
-    double *A0 = nullptr, *A11 = nullptr;  // the input share and the working copy the factorisation overwrites, Ml x Nl
+    DevBuf<double> A0, A11;  // the input share and the working copy the factorisation overwrites, Ml x Nl
     bool have_input = false, factored = false;
     int64_t launches = 0;
-    cudaStream_t side = nullptr;  // high-priority look-ahead stream (null: no overlap)
-    OzakiWorkspace oz{};          // digit planes of the int8 wgmma trailing update (CFLX_GEMM=ozaki)
+    Stream side;        // high-priority look-ahead stream (null: no overlap)
+    OzakiWorkspace oz;  // digit planes of the int8 wgmma trailing update (CFLX_GEMM=ozaki)
     bool use_ozaki = false;
     SolveCache sv;
     EquilState eq;  // cflx_*_equilibrate / cflx_*_svx
@@ -226,8 +214,6 @@ int handle_init(Handle* h, const HandleTexts* texts, cflx_comm* c, int Px, int P
 int handle_update_setup(Handle* h);
 // h->side, at the device's highest stream priority
 int handle_side_stream(Handle* h);
-// what handle_init and handle_side_stream made, the solve cache, the scaling records, then grid_free
-void handle_free(Handle* h);
 // host_local into A0, waited for: a new unscaled input, without factors or a solve cache
 int handle_set_local(Handle* h, const double* host_local);
 // CFLX_OK when `what` may run, after a successful factorisation; otherwise CFLX_ERR_STATE with the reason
@@ -246,36 +232,33 @@ struct cflx_lu : cflx::Handle {
     int N = 0, Mt = 0;
     cflx::SubComm jk_comm, ik_comm;
     // device memory
-    double *PT = nullptr, *PT2 = nullptr, *W = nullptr, *LT = nullptr, *A01raw = nullptr, *U = nullptr, *tmp = nullptr,
-           *A00 = nullptr, *A00T = nullptr, *Uinv = nullptr, *LinvT = nullptr, *candH = nullptr, *S = nullptr,
-           *W2 = nullptr, *bcast = nullptr, *Cbuf = nullptr, *xbuf = nullptr;
-    int *gri = nullptr, *gri_tmp = nullptr, *igri = nullptr, *perm = nullptr, *gpivots = nullptr, *tagsH = nullptr,
-        *tagsS = nullptr, *hist = nullptr, *plan_mem = nullptr, *idx_buf = nullptr;
+    cflx::DevBuf<double> PT, PT2, W, LT, A01raw, U, tmp, A00, A00T, Uinv, LinvT, candH, S, W2, bcast, Cbuf, xbuf;
+    cflx::DevBuf<int> gri, gri_tmp, igri, perm, gpivots, tagsH, tagsS, hist, plan_mem, idx_buf;
     cflx::MovePlan plan{};
     cflx::PanelWorkspace pws{};
     int64_t ldp_max = 0;
-    int* h_npiv = nullptr;  // pinned
+    cflx::PinnedBuf<int> h_npiv;
     std::vector<int> h_hist;
     bool time_gemm = false;
     // double-buffered input streaming (cflx_lu_queue_next_local): the upload of the NEXT matrix overlaps this factorisation
     const double* next_host = nullptr;
     bool a0_is_next = false;  // A0 already holds (or is receiving) the next input: validation of the last run is refused
-    cudaStream_t copy = nullptr;
-    cudaEvent_t ev_a0_read = nullptr, ev_upload = nullptr;
+    cflx::Stream copy;
+    cflx::Event ev_a0_read, ev_upload;
     double gemm_ms = 0, gemm_flops = 0;
     double phase_ms[cflx::PH_COUNT] = {0};
     // non-serialising timeline (profiling mode 2): event pairs recorded on the launching stream, resolved after the run
     struct TlRec { int region, side, ev; };
-    std::vector<cudaEvent_t> tl_pool;
+    std::vector<cflx::Event> tl_pool;
     std::vector<TlRec> tl_recs;
     struct TlSpan { int region, side; float start_ms, ms; };  // resolved: start relative to the first recorded event
     std::vector<TlSpan> tl_spans;                             // one per region instance, in launch order
     double region_ms[2][cflx::RG_COUNT] = {{0}};   // [main / side stream][region]
     int region_cnt[2][cflx::RG_COUNT] = {{0}};
     int prof_mode = 0;                              // 0 off, 1 serialising phase timers, 2 timeline
-    std::vector<cudaEvent_t> ev;
+    std::vector<cflx::Event> ev;
     std::vector<char> ev_used;
-    cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_npiv = nullptr;
+    cflx::Event ev_fork, ev_join, ev_npiv;
 };
 
 namespace cflx {
@@ -314,7 +297,6 @@ int launch_extract_l_panel_T(const double* A, int64_t lda, int row0, int col0, i
                              int64_t ldp, cudaStream_t s);
 
 // solve.cu: the solve engine.  Every function returns CFLX_OK or an error code; all work goes on f.comm->stream.
-void solve_cache_free(SolveCache* sc);
 // grow the work buffers to ldn columns: B (M rows) on rank (pi, 0, 0), W (Ml) and R, Y (v) where `work`, Z (Nl) where
 // `work && col_partials`, X (M) on every rank.  col_seed: also B on rank (0, pj, 0) and Xg (M) on every rank.  What was
 // once asked for stays allocated.
@@ -323,7 +305,7 @@ int solve_cache_grow(SolveCache* sc, const SolveFactor& f, int ldn, bool work, b
 // lower: the tile is L with its own diagonal and zeros above, inverted as A00 = L^T; otherwise it is L\U with a unit L.
 int solve_inverses(SolveCache* sc, const SolveFactor& f, bool lower);
 // *dst = rows (allocated on first use), waited for
-int solve_set_rows(int** dst, const std::vector<int>& rows, cudaStream_t s);
+int solve_set_rows(DevBuf<int>* dst, const std::vector<int>& rows, cudaStream_t s);
 // zero X, W and Z, and on the ranks holding B (`at`): at.dst[r] = B[at.rows[r]] for r < at.n; B is a host or device array
 int solve_seed(SolveCache* sc, const SolveFactor& f, int ldn, int nrhs, const double* B, int ldb, const SolveSeed& at);
 // row-partial sweep over the tile diagonal: forward with the lower triangle (NN), backward with the upper one (NN).  The
@@ -393,7 +375,6 @@ struct RefineOp {
 // device), ferr (may be null: no estimator) and berr (may be null) per column.  Every column runs LAPACK's own decisions, all in lockstep.
 int refine_run(RefineCache* rc, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx, double* ferr,
                double* berr);
-void refine_cache_free(RefineCache* rc);
 // One column of LAPACK's dla_gerfsx_extended / dla_porfsx_extended: its precision state and the normwise (x) and
 // componentwise (z) convergence states, with LAPACK's initial values.  round() takes the statistics of one round,
 // {normy, normx, normdx, dz_z, ymin} (refine.cu column_stats_kernel), and returns what to do with the correction dy:

@@ -142,20 +142,14 @@ int norminf_grid(const Grid& g, const double* A, double* anorm) {
     cflx_comm* c = g.comm;
     cudaStream_t s = c->stream;
     const int M = g.M;
-    double* out = nullptr;
-    CFLX_TRY(dmalloc(&out, (size_t)M));
+    DevBuf<double> out;
+    CFLX_TRY(out.alloc((size_t)M));
     std::vector<double> h(M);
-    auto run = [&]() -> int {
-        CFLX_CUDA(cudaMemsetAsync(out, 0, sizeof(double) * M, s));
-        if (g.pk == 0) CFLX_TRY(launch_norminf_share(A, g, out, s));  // only layer 0 holds the input
-        if (c->world_size > 1) CFLX_NCCL(ncclAllReduce(out, out, (size_t)M, ncclDouble, ncclSum, c->world, s));
-        CFLX_CUDA(cudaMemcpyAsync(h.data(), out, sizeof(double) * M, cudaMemcpyDeviceToHost, s));
-        CFLX_CUDA(cudaStreamSynchronize(s));
-        return CFLX_OK;
-    };
-    const int rc = run();
-    cudaFree(out);
-    if (rc) return rc;
+    CFLX_CUDA(cudaMemsetAsync(out, 0, sizeof(double) * M, s));
+    if (g.pk == 0) CFLX_TRY(launch_norminf_share(A, g, out, s));  // only layer 0 holds the input
+    if (c->world_size > 1) CFLX_NCCL(ncclAllReduce(out, out, (size_t)M, ncclDouble, ncclSum, c->world, s));
+    CFLX_CUDA(cudaMemcpyAsync(h.data(), out, sizeof(double) * M, cudaMemcpyDeviceToHost, s));
+    CFLX_CUDA(cudaStreamSynchronize(s));
     double m = 0.0;
     for (double x : h) m = std::isnan(x) ? x : std::max(m, x);  // dlange: a NaN row sum is the norm
     *anorm = m;
@@ -168,27 +162,19 @@ int norm1_grid(const Grid& g, const double* A, bool lower_sym, double* anorm) {
     const int M = g.M, Ml = g.Ml, Nl = g.Nl, pk = g.pk;
     int ncp = 0, nrp = 0;
     norm1_partials(g, &ncp, &nrp);
-    double *colp = nullptr, *rowp = nullptr, *out = nullptr;
-    int rc = dmalloc(&out, (size_t)M);
-    if (!rc && pk == 0) rc = dmalloc(&colp, (size_t)ncp * Nl);
-    if (!rc && pk == 0 && lower_sym) rc = dmalloc(&rowp, (size_t)nrp * Ml);
+    DevBuf<double> colp, rowp, out;
+    CFLX_TRY(out.alloc((size_t)M));
+    if (pk == 0) CFLX_TRY(colp.alloc((size_t)ncp * Nl));
+    if (pk == 0 && lower_sym) CFLX_TRY(rowp.alloc((size_t)nrp * Ml));
     std::vector<double> h(M);
-    auto run = [&]() -> int {
-        if (pk != 0) {  // only layer 0 holds the input
-            CFLX_CUDA(cudaMemsetAsync(out, 0, sizeof(double) * M, s));
-        } else {
-            CFLX_TRY(launch_norm1_share(A, g, lower_sym, colp, rowp, out, s));
-        }
-        if (c->world_size > 1) CFLX_NCCL(ncclAllReduce(out, out, (size_t)M, ncclDouble, ncclSum, c->world, s));
-        CFLX_CUDA(cudaMemcpyAsync(h.data(), out, sizeof(double) * M, cudaMemcpyDeviceToHost, s));
-        CFLX_CUDA(cudaStreamSynchronize(s));
-        return CFLX_OK;
-    };
-    if (!rc) rc = run();
-    cudaFree(out);
-    cudaFree(colp);
-    cudaFree(rowp);
-    if (rc) return rc;
+    if (pk != 0) {  // only layer 0 holds the input
+        CFLX_CUDA(cudaMemsetAsync(out, 0, sizeof(double) * M, s));
+    } else {
+        CFLX_TRY(launch_norm1_share(A, g, lower_sym, colp, rowp, out, s));
+    }
+    if (c->world_size > 1) CFLX_NCCL(ncclAllReduce(out, out, (size_t)M, ncclDouble, ncclSum, c->world, s));
+    CFLX_CUDA(cudaMemcpyAsync(h.data(), out, sizeof(double) * M, cudaMemcpyDeviceToHost, s));
+    CFLX_CUDA(cudaStreamSynchronize(s));
     double m = 0.0;
     for (double x : h) m = std::isnan(x) ? x : std::max(m, x);  // dlange: a NaN column sum is the norm
     *anorm = m;

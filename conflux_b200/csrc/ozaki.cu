@@ -382,8 +382,10 @@ struct OzakiWorkspace::Maps {
     CUtensorMap a, b;
 };
 
+OzakiWorkspace::OzakiWorkspace() = default;
+OzakiWorkspace::~OzakiWorkspace() = default;
+
 int ozaki_workspace_create(OzakiWorkspace* ws, int max_rows, int max_cols, int K) {
-    *ws = OzakiWorkspace{};
     if (K <= 0 || K % OZ_SPLIT_KC != 0 || K > 512) {
         set_last_error("ozaki: contraction length %d unsupported (multiple of 128, <= 512)", K);
         return CFLX_ERR_UNSUPPORTED;
@@ -391,15 +393,15 @@ int ozaki_workspace_create(OzakiWorkspace* ws, int max_rows, int max_cols, int K
     ws->K = K;
     ws->cap_a = (int)round_up(max_rows, OZ_BM);
     ws->cap_b = (int)round_up(max_cols, OZ_BN);
-    CFLX_CUDA(cudaMalloc((void**)&ws->planesA, (size_t)OZ_S * ws->cap_a * K));
-    CFLX_CUDA(cudaMalloc((void**)&ws->planesB, (size_t)OZ_S * ws->cap_b * K));
+    CFLX_TRY(ws->planesA.alloc_exact((size_t)OZ_S * ws->cap_a * K));
+    CFLX_TRY(ws->planesB.alloc_exact((size_t)OZ_S * ws->cap_b * K));
     CFLX_CUDA(cudaMemset(ws->planesA, 0, (size_t)OZ_S * ws->cap_a * K));
     CFLX_CUDA(cudaMemset(ws->planesB, 0, (size_t)OZ_S * ws->cap_b * K));
-    CFLX_CUDA(cudaMalloc((void**)&ws->ea, sizeof(int) * ws->cap_a));
-    CFLX_CUDA(cudaMalloc((void**)&ws->eb, sizeof(int) * ws->cap_b));
+    CFLX_TRY(ws->ea.alloc_exact(ws->cap_a));
+    CFLX_TRY(ws->eb.alloc_exact(ws->cap_b));
     CFLX_CUDA(cudaMemset(ws->ea, 0, sizeof(int) * ws->cap_a));
     CFLX_CUDA(cudaMemset(ws->eb, 0, sizeof(int) * ws->cap_b));
-    ws->maps = new OzakiWorkspace::Maps;
+    ws->maps = std::make_unique<OzakiWorkspace::Maps>();
     CFLX_TRY(make_plane_map(&ws->maps->a, ws->planesA, K, ws->cap_a, OZ_BM));
     CFLX_TRY(make_plane_map(&ws->maps->b, ws->planesB, K, ws->cap_b, OZ_BN));
     static PerDeviceMax cfg;
@@ -409,14 +411,6 @@ int ozaki_workspace_create(OzakiWorkspace* ws, int max_rows, int max_cols, int K
     CFLX_CUDA(cudaGetDevice(&dev));
     CFLX_CUDA(cudaDeviceGetAttribute(&ws->sms, cudaDevAttrMultiProcessorCount, dev));
     return CFLX_OK;
-}
-void ozaki_workspace_destroy(OzakiWorkspace* ws) {
-    cudaFree(ws->planesA);
-    cudaFree(ws->planesB);
-    cudaFree(ws->ea);
-    cudaFree(ws->eb);
-    delete ws->maps;
-    *ws = OzakiWorkspace{};
 }
 
 // Tera-MACs/s of back-to-back int8 wgmma 64 x n x 32 instructions (n = 64, 128, 192 or 256), two warpgroups per CTA,
@@ -430,7 +424,7 @@ int wgmma_peak_probe(int n, double* tmacs_out) {
     CFLX_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     const size_t smem = 1024 + 4096 + 16384;
     CFLX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    DevBuf sink;
+    DevBuf<> sink;
     CFLX_TRY(sink.alloc(sizeof(int)));
     Events<2> ev;
     CFLX_TRY(ev.create());

@@ -665,14 +665,14 @@ int panel_workspace_create(PanelWorkspace* ws) {
     ws->max_ctas = sms < MAXG ? sms : MAXG;
     ws->epoch = 1;
     ws->cta_cap = 0;
-    CFLX_CUDA(cudaMalloc(&ws->slot_hdr, sizeof(uint2) * 2 * MAXG * 4));
-    CFLX_CUDA(cudaMalloc(&ws->slot_rows, sizeof(uint2) * 2 * MAXG * 64));
+    CFLX_TRY(ws->slot_hdr.alloc_exact(2 * MAXG * 4));
+    CFLX_TRY(ws->slot_rows.alloc_exact(2 * MAXG * 64));
     CFLX_CUDA(cudaMemset(ws->slot_hdr, 0, sizeof(uint2) * 2 * MAXG * 4));
     CFLX_CUDA(cudaMemset(ws->slot_rows, 0, sizeof(uint2) * 2 * MAXG * 64));
     // column-owner kernel for panels of <= 1024 rows: per-block flags, pivot positions, the CTA ticket
-    CFLX_CUDA(cudaMalloc(&ws->sk_flags, sizeof(unsigned) * 1024));
-    CFLX_CUDA(cudaMalloc(&ws->sk_ppos, sizeof(int) * 16384));
-    CFLX_CUDA(cudaMalloc(&ws->sk_ticket, sizeof(unsigned)));
+    CFLX_TRY(ws->sk_flags.alloc_exact(1024));
+    CFLX_TRY(ws->sk_ppos.alloc_exact(16384));
+    CFLX_TRY(ws->sk_ticket.alloc_exact(1));
     CFLX_CUDA(cudaMemset(ws->sk_flags, 0, sizeof(unsigned) * 1024));
     CFLX_CUDA(cudaMemset(ws->sk_ticket, 0, sizeof(unsigned)));
     ws->sk_epoch = 0;
@@ -682,14 +682,6 @@ int panel_workspace_create(PanelWorkspace* ws) {
         ws->sk_enabled = e ? atoi(e) : 1;
     }
     return CFLX_OK;
-}
-void panel_workspace_destroy(PanelWorkspace* ws) {
-    cudaFree(ws->slot_hdr);
-    cudaFree(ws->slot_rows);
-    cudaFree(ws->sk_flags);
-    cudaFree(ws->sk_ppos);
-    cudaFree(ws->sk_ticket);
-    *ws = PanelWorkspace{};
 }
 
 // A00 (optional, v x v row-major) receives, for pivot i, the columns >= (i / NB) * NB of its L\U row; the
@@ -732,8 +724,8 @@ int launch_panel_getrf_a00(double* W, int64_t ldw, int n, int v, int* perm_out, 
     a.G = G;
     a.perm_out = perm_out;
     a.A00 = A00;
-    a.slot_hdr = reinterpret_cast<uint2*>(ws->slot_hdr);
-    a.slot_rows = reinterpret_cast<uint2*>(ws->slot_rows);
+    a.slot_hdr = ws->slot_hdr;
+    a.slot_rows = ws->slot_rows;
     a.epoch_base = ws->epoch;
     ws->epoch += v + 2 + (v & 1);  // keep the base even so slot parity == column parity
     const int nb = panel_nb(a.Rpad, v);

@@ -606,16 +606,6 @@ __global__ void update_x_kernel(double* __restrict__ Y, double* __restrict__ T, 
         Y[e] = xn;
     }
 }
-
-int grow(double** p, size_t n, size_t* have) {
-    if (*p && n <= *have) return CFLX_OK;
-    cudaFree(*p);
-    *p = nullptr;
-    *have = 0;
-    CFLX_TRY(dmalloc(p, n));
-    *have = n;
-    return CFLX_OK;
-}
 }  // namespace
 
 void refine_safe(int M, double* safe1, double* safe2, double* nzeps) {
@@ -794,14 +784,6 @@ int Lacn2::step() {
 }
 
 // ---------------------------------------------------------------- the refinement drivers
-void refine_cache_free(RefineCache* rc) {
-    for (double* p : {rc->X, rc->B, rc->R, rc->D, rc->rhs, rc->ratio, rc->W, rc->Xc, rc->Xr, rc->part, rc->all, rc->berr,
-                      rc->T, rc->Xct, rc->Xrt, rc->stats})
-        cudaFree(p);
-    for (int* p : {rc->gl_rows, rc->gl_cols, rc->active}) cudaFree(p);
-    *rc = RefineCache{};
-}
-
 namespace {
 // What both drivers share: the gather maps and the buffers for nrhs columns, X and B uploaded, and one residual pass.
 struct RefinePass {
@@ -830,7 +812,7 @@ struct RefinePass {
         cudaStream_t s = c->stream;
         const int M = G.M, Ml = G.Ml, Nl = G.Nl;
         // local column (by_col) or row -> global row of X (clamped into X: masked entries never use the value)
-        auto make_map = [&](int** dst, int n, bool by_col) -> int {
+        auto make_map = [&](DevBuf<int>* dst, int n, bool by_col) -> int {
             if (*dst || n <= 0) return CFLX_OK;
             std::vector<int> m(n);
             for (int l = 0; l < n; ++l) {
@@ -841,32 +823,18 @@ struct RefinePass {
         };
         if (layer0 && nn) CFLX_TRY(make_map(&rc->gl_cols, Nl, true));
         if (layer0 && tn) CFLX_TRY(make_map(&rc->gl_rows, Ml, false));
-        if (rc->cap_m < mat) {  // the M x ldn buffers, grown together
-            const std::initializer_list<double**> bufs = {&rc->X, &rc->B, &rc->R, &rc->D, &rc->rhs, &rc->ratio, &rc->W};
-            for (double** p : bufs) {
-                cudaFree(*p);
-                *p = nullptr;
-            }
-            rc->cap_m = 0;
-            for (double** p : bufs) CFLX_TRY(dmalloc(p, mat));
-            rc->cap_m = mat;
-        }
-        CFLX_TRY(grow(&rc->Xc, (size_t)Nl * ldn, &rc->cap_c));
-        CFLX_TRY(grow(&rc->Xr, (size_t)Ml * ldn, &rc->cap_r));
-        CFLX_TRY(grow(&rc->part, chunk, &rc->cap_part));
-        if (c->world_size > 1) CFLX_TRY(grow(&rc->all, chunk * c->world_size, &rc->cap_all));
-        CFLX_TRY(grow(&rc->berr, (size_t)ldn, &rc->cap_berr));
-        if (!rc->active || rc->cap_active < (size_t)ldn) {
-            cudaFree(rc->active);
-            rc->active = nullptr;
-            CFLX_TRY(dmalloc(&rc->active, (size_t)ldn));
-            rc->cap_active = ldn;
-        }
+        CFLX_TRY(grow_together({&rc->X, &rc->B, &rc->R, &rc->D, &rc->rhs, &rc->ratio, &rc->W}, mat));
+        CFLX_TRY(rc->Xc.grow((size_t)Nl * ldn));
+        CFLX_TRY(rc->Xr.grow((size_t)Ml * ldn));
+        CFLX_TRY(rc->part.grow(chunk));
+        if (c->world_size > 1) CFLX_TRY(rc->all.grow(chunk * c->world_size));
+        CFLX_TRY(rc->berr.grow((size_t)ldn));
+        CFLX_TRY(rc->active.grow((size_t)ldn));
         if (extended) {
-            CFLX_TRY(grow(&rc->T, mat, &rc->cap_t));
-            CFLX_TRY(grow(&rc->Xct, (size_t)Nl * ldn, &rc->cap_ct));
-            CFLX_TRY(grow(&rc->Xrt, (size_t)Ml * ldn, &rc->cap_rt));
-            CFLX_TRY(grow(&rc->stats, (size_t)ldn * NSTAT, &rc->cap_stats));
+            CFLX_TRY(rc->T.grow(mat));
+            CFLX_TRY(rc->Xct.grow((size_t)Nl * ldn));
+            CFLX_TRY(rc->Xrt.grow((size_t)Ml * ldn));
+            CFLX_TRY(rc->stats.grow((size_t)ldn * NSTAT));
             CFLX_CUDA(cudaMemsetAsync(rc->T, 0, sizeof(double) * mat, s));
         }
         CFLX_CUDA(cudaMemsetAsync(rc->X, 0, sizeof(double) * mat, s));

@@ -338,33 +338,23 @@ int diag_solve(const SolveCache& sc, const SolveFactor& f, int t, Tri tri, doubl
 }
 }  // namespace
 
-void solve_cache_free(SolveCache* sc) {
-    for (double* p : {sc->inv, sc->B, sc->W, sc->Z, sc->R, sc->Y, sc->X, sc->Xg}) cudaFree(p);
-    for (int* p : {sc->rows, sc->rows_id, sc->cols, sc->unperm}) cudaFree(p);
-    refine_cache_free(&sc->rf);
-    *sc = SolveCache{};
-}
-
 int solve_cache_grow(SolveCache* sc, const SolveFactor& f, int ldn, bool work, bool col_partials, bool col_seed) {
     if (ldn <= sc->ldn && (sc->col_partials || !col_partials) && (sc->col_seed || !col_seed)) return CFLX_OK;
     ldn = std::max(ldn, sc->ldn);
     sc->col_partials |= col_partials;
     sc->col_seed |= col_seed;
-    for (double** p : {&sc->B, &sc->W, &sc->Z, &sc->R, &sc->Y, &sc->X, &sc->Xg}) {
-        cudaFree(*p);
-        *p = nullptr;
-    }
+    for (DevBuf<double>* p : {&sc->B, &sc->W, &sc->Z, &sc->R, &sc->Y, &sc->X, &sc->Xg}) p->reset();
     sc->ldn = 0;
     const size_t M = f.g.M, v = f.g.v;
-    if (f.g.pk == 0 && (f.g.pj == 0 || (sc->col_seed && f.g.pi == 0))) CFLX_TRY(dmalloc(&sc->B, M * ldn));
+    if (f.g.pk == 0 && (f.g.pj == 0 || (sc->col_seed && f.g.pi == 0))) CFLX_TRY(sc->B.alloc(M * ldn));
     if (work) {
-        CFLX_TRY(dmalloc(&sc->W, (size_t)f.g.Ml * ldn));
-        if (sc->col_partials) CFLX_TRY(dmalloc(&sc->Z, (size_t)f.g.Nl * ldn));
-        CFLX_TRY(dmalloc(&sc->R, v * ldn));
-        CFLX_TRY(dmalloc(&sc->Y, v * ldn));
+        CFLX_TRY(sc->W.alloc((size_t)f.g.Ml * ldn));
+        if (sc->col_partials) CFLX_TRY(sc->Z.alloc((size_t)f.g.Nl * ldn));
+        CFLX_TRY(sc->R.alloc(v * ldn));
+        CFLX_TRY(sc->Y.alloc(v * ldn));
     }
-    CFLX_TRY(dmalloc(&sc->X, M * ldn));
-    if (sc->col_seed) CFLX_TRY(dmalloc(&sc->Xg, M * ldn));
+    CFLX_TRY(sc->X.alloc(M * ldn));
+    if (sc->col_seed) CFLX_TRY(sc->Xg.alloc(M * ldn));
     sc->ldn = ldn;
     return CFLX_OK;
 }
@@ -372,15 +362,15 @@ int solve_cache_grow(SolveCache* sc, const SolveFactor& f, int ldn, bool work, b
 int solve_inverses(SolveCache* sc, const SolveFactor& f, bool lower) {
     cudaStream_t s = f.g.comm->stream;
     const int v = f.g.v, nb = f.g.nb;
-    cudaFree(sc->inv);
-    sc->inv = nullptr;
+    sc->inv.reset();
     int nown = 0;
     for (int t = 0; t < f.g.Nt; ++t) nown += diag_slot(f, t) >= 0;
     const size_t per = 2 * (size_t)v * nb;
-    CFLX_TRY(dmalloc(&sc->inv, std::max(1, nown) * per));
-    double *tile = nullptr, *linvT = nullptr;
-    int rc = dmalloc(&tile, (size_t)v * v);
-    if (!rc) rc = dmalloc(&linvT, (size_t)v * nb);
+    CFLX_TRY(sc->inv.alloc(std::max(1, nown) * per));
+    DevBuf<double> tile, linvT;
+    CFLX_TRY(tile.alloc((size_t)v * v));
+    CFLX_TRY(linvT.alloc((size_t)v * nb));
+    int rc = CFLX_OK;
     for (int t = 0; t < f.g.Nt && !rc; ++t) {
         const int slot = diag_slot(f, t);
         if (slot < 0) continue;
@@ -396,16 +386,14 @@ int solve_inverses(SolveCache* sc, const SolveFactor& f, bool lower) {
             rc = CFLX_ERR_CUDA;
         }
         if (!rc) rc = launch_diag_inverses(tile, v, nb, inv + (size_t)v * nb, linvT, s);
-        if (!rc) rc = launch_transpose_blocks(lower ? inv + (size_t)v * nb : linvT, nb, (int64_t)v * nb, inv, s);
+        if (!rc) rc = launch_transpose_blocks(lower ? inv + (size_t)v * nb : linvT.p, nb, (int64_t)v * nb, inv, s);
     }
     if (cudaStreamSynchronize(s) != cudaSuccess && !rc) rc = CFLX_ERR_CUDA;
-    cudaFree(tile);
-    cudaFree(linvT);
     return rc;
 }
 
-int solve_set_rows(int** dst, const std::vector<int>& rows, cudaStream_t s) {
-    if (!*dst) CFLX_TRY(dmalloc(dst, rows.size()));
+int solve_set_rows(DevBuf<int>* dst, const std::vector<int>& rows, cudaStream_t s) {
+    if (!*dst) CFLX_TRY(dst->alloc(rows.size()));
     CFLX_CUDA(cudaMemcpyAsync(*dst, rows.data(), sizeof(int) * rows.size(), cudaMemcpyHostToDevice, s));
     CFLX_CUDA(cudaStreamSynchronize(s));  // `rows` is a host temporary
     return CFLX_OK;

@@ -121,7 +121,7 @@ int solve_local_run(const Grid& g, int rows, const SolveLocalArgs& a, const Bloc
     const int ncl = rhs_local_cols(a.nrhs, g.v, g.Py), cols = valid_cols(a.nrhs, g.v, g.Py, g.pj);
     const bool copy = rows > 0 && cols > 0;
     // a host share goes through one temporary device share (ld ncl), which holds B and then receives X when both are host
-    DevBuf tmp;
+    DevBuf<> tmp;
     if ((a.B && !a.b_dev) || (a.X && !a.x_dev)) CFLX_TRY(tmp.alloc(sizeof(double) * std::max<size_t>(1, (size_t)rows * ncl)));
     const double* src = a.B;
     int64_t lds = a.ldb;
@@ -139,7 +139,7 @@ int solve_local_run(const Grid& g, int rows, const SolveLocalArgs& a, const Bloc
         ldd = ncl;
     }
     const int nc = inverse_block_cols(g.M, g.v);
-    DevBuf Bk;
+    DevBuf<> Bk;
     CFLX_TRY(Bk.alloc(sizeof(double) * g.M * round_up(std::min(nc, a.nrhs), 8)));
     for (int c0 = 0; c0 < a.nrhs; c0 += nc) {
         const int w = std::min(nc, a.nrhs - c0), ldn = (int)round_up(w, 8);

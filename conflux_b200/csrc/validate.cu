@@ -114,7 +114,7 @@ int redistribute_pivoted_rows(cflx_lu* lu, const std::vector<int>& hist, bool fa
     cudaStream_t s = c->stream;
     const int v = lu->v, Px = lu->Px, Ml = lu->Ml, Nl = lu->Nl;
     const size_t loc = (size_t)Ml * Nl;
-    if (!lu->idx_buf) CFLX_TRY(dmalloc(&lu->idx_buf, 2 * (size_t)Ml));
+    if (!lu->idx_buf) CFLX_TRY(lu->idx_buf.alloc(2 * (size_t)Ml));
     std::vector<int> next_local(Px, 0);
     std::vector<std::vector<int>> send_rows(Px), recv_rows(Px);  // send_rows[dst rank] = my source rows; recv_rows[src rank] = my dest rows
     for (int q = 0; q < lu->M; ++q) {
@@ -147,7 +147,7 @@ int redistribute_pivoted_rows(cflx_lu* lu, const std::vector<int>& hist, bool fa
         CFLX_CUDA(cudaStreamSynchronize(s));  // the index vectors above are stack/heap temporaries
         return CFLX_OK;
     }
-    if (!lu->xbuf) CFLX_TRY(dmalloc(&lu->xbuf, 2 * loc));
+    if (!lu->xbuf) CFLX_TRY(lu->xbuf.alloc(2 * loc));
     double* sendbuf = lu->xbuf;
     double* recvbuf = lu->xbuf + loc;
     gather_rows_kernel<<<grid, 256, 0, s>>>(src, Nl, lu->idx_buf, Ml, Nl, sendbuf);
@@ -181,26 +181,20 @@ int lu_residual_grid(cflx_lu* lu, const std::vector<int>& hist, double* abs_out,
     const int pi = lu->pi, pj = lu->pj;
     const bool layer0 = lu->pk == 0;
     const size_t loc = (size_t)Ml * Nl;
-    double *R = nullptr, *acc = nullptr;
+    DevBuf<double> R, acc;
     int rc = CFLX_OK;
-    auto cleanup = [&]() {
-        cudaFree(R);
-        cudaFree(acc);
-        cudaFree(lu->xbuf);  // 2 x local matrix of staging: do not keep it alive after validation
-        lu->xbuf = nullptr;
-    };
-    if ((rc = dmalloc(&acc, 2 + SUMSQ_PARTIALS))) return rc;  // the two sums, then the partials of launch_sumsq
+    if ((rc = acc.alloc(2 + SUMSQ_PARTIALS))) return rc;  // the two sums, then the partials of launch_sumsq
     if (cudaMemsetAsync(acc, 0, 2 * sizeof(double), s) != cudaSuccess) rc = CFLX_ERR_CUDA;
     if (!rc && layer0) {
-        if (!lu->Cbuf) rc = dmalloc(&lu->Cbuf, loc);
-        if (!rc) rc = dmalloc(&R, loc);
+        if (!lu->Cbuf) rc = lu->Cbuf.alloc(loc);
+        if (!rc) rc = R.alloc(loc);
         if (!rc) rc = redistribute_pivoted_rows(lu, hist, true, lu->A11, lu->Cbuf);   // C   (conflux layout)
         if (!rc) rc = redistribute_pivoted_rows(lu, hist, false, lu->A0, R);          // P*A (conflux layout)
     }
     // every rank must reach the collectives below even after a local failure above would deadlock the others: a
     // failure here is an allocation failure, which the caller treats as fatal for the whole grid anyway
     if (rc) {
-        cleanup();
+        lu->xbuf.reset();  // 2 x local matrix of staging: do not keep it alive after validation
         return rc;
     }
     const int64_t ldp = lu->ldp_max, ldu = Nl;
@@ -257,7 +251,7 @@ int lu_residual_grid(cflx_lu* lu, const std::vector<int>& hist, double* abs_out,
         set_last_error("residual: %s", cudaGetErrorString(cudaGetLastError()));
         rc = CFLX_ERR_CUDA;
     }
-    cleanup();
+    lu->xbuf.reset();
     // the panels were used as staging: restore the zero padding the factorisation relies on
     if (!rc) {
         cudaMemsetAsync(lu->PT, 0, (size_t)v * ldp * sizeof(double), s);
