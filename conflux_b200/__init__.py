@@ -15,7 +15,7 @@ import numpy as np
 
 from ._lib import ConfluxError, LIB_PATH, SYMBOLS, ShareLayout, check, lib
 
-__all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "residual", "validate", "lu_solve", "lu_rcond", "lu_refine", "lu_refine_x", "lu_equilibrate", "lu_svx", "lu_equilibrate_b", "lu_svxx", "lu_inverse", "lu_det", "rhs_local_cols", "lu_solve_local", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
+__all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "LU_rep_fixed", "residual", "validate", "lu_solve", "lu_rcond", "lu_refine", "lu_refine_x", "lu_equilibrate", "lu_svx", "lu_equilibrate_b", "lu_svxx", "lu_inverse", "lu_det", "rhs_local_cols", "lu_solve_local", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
 
 
 def auto_grid(M, N, P):
@@ -176,6 +176,38 @@ def LU_rep(gv, C=None, permutation=None, upload=True, next_data=None):
         assert permutation.dtype == np.int32 and permutation.size >= gv.M
         check(lib().cflx_lu_get_permutation(gv._h, permutation.ctypes.data), "lu_get_permutation")
     return ms.value
+
+
+def LU_rep_fixed(gv, perm=None, tiny=0.0, C=None, permutation=None, upload=True, next_data=None):
+    """LU_rep with a prescribed row order instead of the pivot search (cflx_lu_factor_fixed): P A = L U with row q of
+    P A = row perm[q] of A.  perm (M ints, the same on every rank) defaults to the permutation of the last completed
+    factorisation of gv, so that a nearby matrix is factored with the pivots of the previous one.  tiny >= 0: pivots
+    with |u| < tiny become copysign(tiny, u) (+tiny for +-0).  C, permutation, upload and next_data as LU_rep.
+    COLLECTIVE.  Returns (ms, nrepl, info): the main loop's device time, the pivots replaced over the grid, and 1 + the
+    global column of the first exactly zero pivot (0: none), identical on every rank."""
+    if upload:
+        a = np.ascontiguousarray(gv.data, dtype=np.float64)
+        check(lib().cflx_lu_set_local(gv._h, a.ctypes.data), "lu_set_local")
+    if next_data is not None:
+        assert next_data.dtype == np.float64 and next_data.flags.c_contiguous and next_data.size == gv.Ml * gv.Nl
+        check(lib().cflx_lu_queue_next_local(gv._h, next_data.ctypes.data), "lu_queue_next_local")
+    p = None
+    if perm is not None:
+        p = np.ascontiguousarray(perm, dtype=np.int32)
+        if p.shape != (gv.M,):
+            raise ValueError(f"LU_rep_fixed: perm must have shape ({gv.M},), got {p.shape}")
+    ms, nrepl, info = ctypes.c_double(), ctypes.c_int(), ctypes.c_int()
+    check(lib().cflx_lu_factor_fixed(gv._h, _ptr(p), float(tiny), ctypes.byref(nrepl), ctypes.byref(info),
+                                     ctypes.byref(ms)), "lu_factor_fixed")
+    if C is not None:
+        assert C.dtype == np.float64 and C.flags.c_contiguous and C.size >= gv.Ml * gv.Nl
+        if permutation is None:
+            permutation = np.empty(gv.M, dtype=np.int32)
+        check(lib().cflx_lu_get_factors(gv._h, C.ctypes.data, permutation.ctypes.data), "lu_get_factors")
+    elif permutation is not None:
+        assert permutation.dtype == np.int32 and permutation.size >= gv.M
+        check(lib().cflx_lu_get_permutation(gv._h, permutation.ctypes.data), "lu_get_permutation")
+    return ms.value, nrepl.value, info.value
 
 
 def timeline(gv):
@@ -1001,6 +1033,20 @@ class dbg:
         check(lib().cflx_dbg_potrf_tile(v, A.ctypes.data, L.ctypes.data, LT.ctypes.data, ctypes.byref(info), int(variant)),
               "dbg_potrf_tile")
         return L, LT, info.value
+
+    @staticmethod
+    def getrf_nopiv_tile(A, tiny=0.0, variant=0):
+        """Unpivoted LU of one v x v block as LU_rep_fixed runs it: variant 0 the one-CTA kernel on the whole block, 1 the
+        128-block driver (v % 128 == 0, v >= 256; what the factorisation runs there).  Returns
+        (LU, nrepl, info): L\\U with unit L, the pivots replaced by the tiny rule, 1 + the first exactly zero pivot's
+        column (0: none)."""
+        A = np.ascontiguousarray(A, dtype=np.float64)
+        v = A.shape[0]
+        LU = np.empty((v, v))
+        nrepl, info = ctypes.c_int(), ctypes.c_int()
+        check(lib().cflx_dbg_getrf_nopiv_tile(v, A.ctypes.data, float(tiny), LU.ctypes.data, ctypes.byref(nrepl),
+                                              ctypes.byref(info), int(variant)), "dbg_getrf_nopiv_tile")
+        return LU, nrepl.value, info.value
 
     @staticmethod
     def ozaki_gemm(AT, B, C=None, reps=1, want_planes=False, row0=0, col0=0, max_ctas=0):

@@ -896,6 +896,40 @@ int cflx_dbg_potrf_tile(int v, const double* A, double* L_out, double* LT_out, i
     return CFLX_OK;
 }
 
+// unpivoted LU of one v x v row-major block as cflx_lu_factor_fixed runs it: variant 0 the one-CTA kernel on the whole
+// block, 1 the 128-block driver (v % 128 == 0, v >= 256; what the factorisation runs there)
+int cflx_dbg_getrf_nopiv_tile(int v, const double* A, double tiny, double* LU_out, int* nrepl_out, int* info_out,
+                              int variant) {
+    CFLX_TRY(check_device());
+    REFUSE_IF(!A || !LU_out || !info_out);
+    REFUSE_IF(variant != 0 && variant != 1);
+    REFUSE_IF(v < 4 || v > 1024 || v % 4 != 0);
+    REFUSE_IF(variant == 1 && !getrf_nopiv_blocked(v));
+    REFUSE_IF(!(tiny >= 0.0));
+    const size_t vv = (size_t)v * v;
+    std::vector<double> At(vv);  // the tile takes the block transposed, as the gather leaves it
+    for (int i = 0; i < v; ++i)
+        for (int c = 0; c < v; ++c) At[(size_t)c * v + i] = A[(size_t)i * v + c];
+    DevBuf<> dB, dA, drec, dws;
+    CFLX_TRY(stage(dB, vv, At.data()));
+    CFLX_TRY(stage(dA, vv));
+    CFLX_TRY(stage<int>(drec, 4));
+    const size_t ws = getrf_nopiv_scratch(v, variant == 1);
+    if (ws) CFLX_TRY(stage(dws, ws));
+    CFLX_CUDA(cudaMemset(drec.p, 0, 4 * sizeof(int)));
+    if (variant == 1) CFLX_TRY(gemm_tn_setup());
+    int64_t launches = 0;
+    CFLX_TRY(launch_getrf_nopiv_tile(dB.as<double>(), v, tiny, dA.as<double>(), nullptr, nullptr, nullptr, drec.as<int>(),
+                                     0, variant == 1, ws ? dws.as<double>() : nullptr, 0, &launches));
+    int rec[4];
+    CFLX_TRY(fetch(LU_out, dA.p, vv));
+    CFLX_TRY(fetch(rec, drec.p, 4));
+    CFLX_CUDA(cudaDeviceSynchronize());
+    if (nrepl_out) *nrepl_out = rec[0];
+    *info_out = rec[1];
+    return CFLX_OK;
+}
+
 // step 2 of the LU loop in isolation on ONE rank (Px = 1): plan_moves (analyze_pivots) + push_phase1..3 (push_pivots_up,
 // conflux_opt.hpp:176-218) + the gri/igri bookkeeping, on an n_rows x n_cols row-major matrix (n_cols even).  The npiv
 // pivot rows (local indices >= fnpr, tournament order) end up in rows [fnpr, fnpr+npiv) in that order.

@@ -153,6 +153,24 @@ int potrf_tile(double* D, double* UT, double* Q, int* info, int col0, int v, cud
 // one 128 x 128 block (leading dimensions ldd / ldu) on potrf128_kernel; Uc: a contiguous 128 x 128 copy of L^T
 int potrf_block128(double* D, int ldd, double* UT, int ldu, double* Uc, int* info, int col0, cudaStream_t stream);
 
+// ---------------------------------------------------------------- fixed.cu (cflx_lu_factor_fixed)
+// Unpivoted LU of one v x v block: Bt is the block transposed (Bt[c][i], as launch_gather_winners leaves it), A
+// receives L\U row-major (unit L) and AT (may be null) its transpose; tags_out[i] = tags_in[i] (both may be null).  A
+// pivot u with |u| < tiny becomes copysign(tiny, u) (+tiny for +-0).  rec (may be null): rec[0] += the replacements,
+// rec[1] = col0 + 1 + the column of the first exactly zero pivot when rec[1] is 0.  blocked (getrf_nopiv_blocked(v)
+// only): 128-wide block columns, the diagonal blocks on the one-CTA kernel, the rest on the TRSMs and gemm_tn;
+// otherwise the one-CTA kernel on the whole block.  scratch: getrf_nopiv_scratch(v, blocked) doubles of device memory,
+// or null when that is 0.  *launches grows by the kernels launched.  Deterministic.  gemm_tn_setup() first.
+bool getrf_nopiv_blocked(int v);
+size_t getrf_nopiv_scratch(int v, bool blocked);
+int launch_getrf_nopiv_tile(const double* Bt, int v, double tiny, double* A, double* AT, const int* tags_in, int* tags_out,
+                            int* rec, int col0, bool blocked, double* scratch, cudaStream_t stream, int64_t* launches);
+// pos[i] = active panel position (local row - fnpr) of global row rows[i] where grid row pi owns it, else n_old
+int launch_fixed_locate(const int* rows, int v, int Px, int pi, int fnpr, int n_old, const int* igri, int* pos,
+                        cudaStream_t stream);
+// rec[2] = rec[1], or INT_MAX when it is 0
+int launch_fixed_info_operand(int* rec, cudaStream_t stream);
+
 // ---------------------------------------------------------------- validate.cu
 // out[i][c] = A[src_rows[i] * lda + c] for i < nrows, c < ncols (ncols, lda even; 16-byte aligned rows)
 int launch_gather_rows(const double* A, int64_t lda, const int* src_rows, int nrows, int ncols, double* out,

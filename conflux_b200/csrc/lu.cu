@@ -13,6 +13,7 @@
 //   * all communication is NCCL on the rank's stream; at Px == 1 the whole factorisation is enqueued without a
 //     single host synchronisation, at Px > 1 the host reads back one int (this rank's pivot count) per step.
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdarg>
 #include <cstdlib>
@@ -279,6 +280,29 @@ __global__ void stack_kernel(const double* __restrict__ candH, const int* __rest
     }
     if (e < 2 * v) tagsS[e] = tagsH[e];
 }
+
+// ---- step 1 of iteration k in a prescribed row order (cflx_lu_factor_fixed), in place of the pivot search: the rows
+// perm[kv, kv + v) located in this rank's panel and gathered (zeros for the rows other grid rows own), summed onto grid
+// row k % Px (one contributor per element: the bits travel exactly as integers), and factored there without pivoting
+// into A00 / A00T, with tagsH = the rows.  Everything after it in finish_step takes any v rows from any mix of ranks.
+int fixed_panel(cflx_lu* lu, int k, int fnpr, int n_old, int64_t ldk, double* A00, double* A00T, cudaStream_t s) {
+    const int v = lu->v, Px = lu->Px;
+    const int* rows = lu->fix_perm + (size_t)k * v;
+    {
+        PhaseTimer t(lu, RG_step1_rowpermute, s);
+        CFLX_TRY(launch_fixed_locate(rows, v, Px, lu->pi, fnpr, n_old, lu->igri, lu->perm, s));
+        CFLX_TRY(launch_gather_winners(lu->PT, ldk, lu->gri + fnpr, n_old, lu->perm, v, lu->candH, v, lu->tagsS, 0, s));
+        lu->launches += 2;
+    }
+    if (Px > 1) {
+        PhaseTimer t(lu, RG_step1_pivoting, s);
+        CFLX_NCCL(ncclReduce(lu->candH, lu->candH, (size_t)v * v, ncclUint64, ncclSum, k % Px, lu->i_comm.c, s));
+    }
+    if (lu->pi != k % Px) return CFLX_OK;
+    PhaseTimer t(lu, RG_step1_lup, s);
+    return launch_getrf_nopiv_tile(lu->candH, v, lu->fix_tiny, A00, A00T, rows, lu->tagsH, lu->fix_rec, k * v,
+                                   getrf_nopiv_blocked(v), lu->fix_ws.p, s, &lu->launches);
+}
 // ---- steps 0 + 1 of iteration k: panel extract (+ layer reduce), local pivot search, tournament.  Runs on stream
 // `s`; with look-ahead that is the high-priority side stream and overlaps the trailing update of iteration k-1.
 // Touches only: PT, W, perm, candH/tagsH/S/W2/tagsS, A00/A00T (outputs consumed by finish_step(k) after the join).
@@ -306,6 +330,7 @@ int panel_phase(cflx_lu* lu, int k, int fnpr, cudaStream_t s) {
         CFLX_NCCL(ncclReduce(lu->PT, lu->PT, (size_t)v * ldk, ncclDouble, ncclSum, 0, lu->k_comm.c, s));
     }
     if (pk != 0) return CFLX_OK;
+    if (lu->fixed) return fixed_panel(lu, k, fnpr, n_old, ldk, A00, A00T, s);
     // ---- step 1: local pivot search + tournament on column pj == k % Py, layer 0   conflux_opt.hpp:693-816
     int my_half = 0;
     {
@@ -444,7 +469,7 @@ int finish_step(cflx_lu* lu, int k, int& fnpr) {
         PhaseTimer t(lu, RG_step2_pushingpivots, s);
         CFLX_TRY(launch_plan_moves(lu->gpivots, v, Px, pi, fnpr_old, Ml, lu->igri, lu->plan, s));
         lu->launches++;
-        if (Px > 1) {
+        if (Px > 1 && !lu->fixed) {  // a prescribed order gives the count on the host
             CFLX_CUDA(cudaMemcpyAsync(lu->h_npiv, lu->plan.npiv, sizeof(int), cudaMemcpyDeviceToHost, s));
             CFLX_CUDA(cudaEventRecord(lu->ev_npiv, s));
         }
@@ -459,8 +484,9 @@ int finish_step(cflx_lu* lu, int k, int& fnpr) {
     }
     const int64_t ldu = std::max(2, ncols);
     // At Px == 1 the local pivot search IS the panel factorisation: its multipliers are the L panel (same values a
-    // LAPACK getrf leaves behind; the reference recomputes them with dtrsm against A00, conflux_opt.hpp:1347).
-    const bool fused_l = (nR == 0);
+    // LAPACK getrf leaves behind; the reference recomputes them with dtrsm against A00, conflux_opt.hpp:1347).  A
+    // prescribed order has no panel factorisation: L comes from the TRSM, as on Px > 1 grids.
+    const bool fused_l = (nR == 0) && !lu->fixed;
     // ---- steps 2b/3: pivot rows summed over layers and gathered on row pi == k % Px   conflux_opt.hpp:1164-1260
     if (ncols > 0 && Px * Pz > 1) {
         PhaseTimer t(lu, RG_step2_reduce, s);
@@ -502,7 +528,9 @@ int finish_step(cflx_lu* lu, int k, int& fnpr) {
     if (!split_u) CFLX_TRY(store_factors());
     // ---- now the pivot count: sizes of the L panel and of the trailing update
     int npiv = v;
-    if (Px > 1) {
+    if (lu->fixed) {
+        npiv = lu->fix_npiv[k];
+    } else if (Px > 1) {
         CFLX_CUDA(cudaEventSynchronize(lu->ev_npiv));
         npiv = *lu->h_npiv;
     }
@@ -974,16 +1002,16 @@ int cflx_lu_queue_next_local(cflx_lu* lu, const double* host_next) {
     return CFLX_OK;
 }
 
-int cflx_lu_factor(cflx_lu* lu, double* ms_out) {
-    if (!lu) return CFLX_ERR_ARG;
-    if (!lu->have_input) {
-        set_last_error("cflx_lu_factor before cflx_lu_set_local");
-        return CFLX_ERR_STATE;
-    }
+}  // extern "C"
+
+namespace {
+// The factorisation both entry points share, from the working copy of the input to the timeline: the pivot search of
+// cflx_lu_factor, or with lu->fixed the prescribed order of cflx_lu_factor_fixed (fixed_panel).  COLLECTIVE.
+int lu_factor_run(cflx_lu* lu, double* ms_out) {
     cflx_comm* c = lu->comm;
     cudaStream_t s = c->stream;
-    CFLX_CUDA(cudaSetDevice(c->device));
     const size_t loc = (size_t)lu->Ml * lu->Nl;
+    lu->perm_done = false;
     // "init" region of the reference (conflux_opt.hpp:347-515): A11Buff = copy of gv.data, gri, counters
     {
         PhaseTimer t(lu, RG_init, s);
@@ -1065,6 +1093,132 @@ int cflx_lu_factor(cflx_lu* lu, double* ms_out) {
     }
     if (lu->a0_is_next) CFLX_CUDA(cudaStreamSynchronize(lu->copy));  // the caller's staging buffer is free again
     lu->factored = true;
+    lu->perm_done = true;
+    return CFLX_OK;
+}
+
+// FNV-1a over the words of the order: what the ranks compare before a fixed factorisation
+unsigned long long order_hash(const std::vector<int>& p) {
+    unsigned long long h = 1469598103934665603ull;
+    for (int x : p) {
+        h ^= (unsigned)x;
+        h *= 1099511628211ull;
+    }
+    return h;
+}
+
+// COLLECTIVE (world): *same = every rank has ok and the same hash, from one ncclMin over {h, ~h, ok}: min(~h) = ~max(h)
+int fixed_agree(cflx_lu* lu, bool ok, unsigned long long h, bool* same) {
+    cflx_comm* c = lu->comm;
+    if (c->world_size == 1) {
+        *same = ok;
+        return CFLX_OK;
+    }
+    unsigned long long w[3] = {h, ~h, ok ? 1ull : 0ull};
+    if (!lu->fix_agree) CFLX_TRY(lu->fix_agree.alloc(3));
+    CFLX_CUDA(cudaMemcpyAsync(lu->fix_agree, w, sizeof(w), cudaMemcpyHostToDevice, c->stream));
+    CFLX_NCCL(ncclAllReduce(lu->fix_agree, lu->fix_agree, 3, ncclUint64, ncclMin, c->world, c->stream));
+    CFLX_CUDA(cudaMemcpyAsync(w, lu->fix_agree, sizeof(w), cudaMemcpyDeviceToHost, c->stream));
+    CFLX_CUDA(cudaStreamSynchronize(c->stream));
+    *same = w[2] == 1 && w[0] == ~w[1];
+    return CFLX_OK;
+}
+
+// The checks of cflx_lu_factor_fixed that need no other rank; on success lu->fix_perm_h holds the order and the
+// device buffers of the fixed path exist
+int fixed_prepare(cflx_lu* lu, const int* perm, double tiny, const int* info_out) {
+    if (!(tiny >= 0.0) || !info_out) {
+        set_last_error("cflx_lu_factor_fixed: tiny must be >= 0 and info_out not NULL");
+        return CFLX_ERR_ARG;
+    }
+    if (!lu->have_input) {
+        set_last_error("cflx_lu_factor_fixed before cflx_lu_set_local");
+        return CFLX_ERR_STATE;
+    }
+    const int M = lu->M;
+    std::vector<int>& p = lu->fix_perm_h;
+    if (perm) {
+        p.assign(perm, perm + M);
+    } else {
+        if (!lu->perm_done) {
+            set_last_error("cflx_lu_factor_fixed with perm = NULL before any factorisation of this handle completed");
+            return CFLX_ERR_STATE;
+        }
+        // stream-ordered like every reader of hist (cflx_lu_get_permutation refuses after set_local, which keeps hist)
+        p.resize(M);
+        CFLX_CUDA(cudaMemcpyAsync(p.data(), lu->hist, sizeof(int) * M, cudaMemcpyDeviceToHost, lu->comm->stream));
+        CFLX_CUDA(cudaStreamSynchronize(lu->comm->stream));
+    }
+    std::vector<char> seen(M, 0);
+    for (int x : p) {
+        if (x < 0 || x >= M || seen[x]) {
+            set_last_error("cflx_lu_factor_fixed: perm is not a permutation of [0, %d)", M);
+            return CFLX_ERR_ARG;
+        }
+        seen[x] = 1;
+    }
+    if (!lu->fix_perm) CFLX_TRY(lu->fix_perm.alloc(M));
+    if (!lu->fix_rec) CFLX_TRY(lu->fix_rec.alloc(4));
+    const size_t ws = getrf_nopiv_scratch(lu->v, getrf_nopiv_blocked(lu->v));
+    if (ws && !lu->fix_ws) CFLX_TRY(lu->fix_ws.alloc(ws));
+    return CFLX_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int cflx_lu_factor(cflx_lu* lu, double* ms_out) {
+    if (!lu) return CFLX_ERR_ARG;
+    if (!lu->have_input) {
+        set_last_error("cflx_lu_factor before cflx_lu_set_local");
+        return CFLX_ERR_STATE;
+    }
+    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    return lu_factor_run(lu, ms_out);
+}
+
+// COLLECTIVE.  P A = L U with the P of a prescribed order: the arguments agreed on by every rank first (one world
+// all-reduce, so that a refusal anywhere is a refusal everywhere and no rank enters the loop alone), then the shared
+// factorisation with fixed_panel in place of the pivot search, then the replacements (sum) and the first zero pivot (min)
+// combined over the world.
+int cflx_lu_factor_fixed(cflx_lu* lu, const int* perm, double tiny, int* nrepl_out, int* info_out, double* ms_out) {
+    if (!lu) return CFLX_ERR_ARG;
+    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    cflx_comm* c = lu->comm;
+    cudaStream_t s = c->stream;
+    const int rc = fixed_prepare(lu, perm, tiny, info_out);
+    bool same = false;
+    CFLX_TRY(fixed_agree(lu, rc == CFLX_OK, rc == CFLX_OK ? order_hash(lu->fix_perm_h) : 0, &same));
+    if (rc != CFLX_OK) return rc;
+    if (!same) {
+        set_last_error("cflx_lu_factor_fixed: the ranks passed different orders, or another rank refused its arguments");
+        return CFLX_ERR_ARG;
+    }
+    const int v = lu->v, Px = lu->Px;
+    const std::vector<int>& p = lu->fix_perm_h;
+    lu->fix_npiv.assign(lu->Nt, 0);
+    for (int q = 0; q < lu->Nt * v; ++q)
+        if ((p[q] / v) % Px == lu->pi) lu->fix_npiv[q / v]++;
+    CFLX_CUDA(cudaMemcpyAsync(lu->fix_perm, p.data(), sizeof(int) * lu->M, cudaMemcpyHostToDevice, s));
+    CFLX_CUDA(cudaMemsetAsync(lu->fix_rec, 0, 4 * sizeof(int), s));
+    lu->fix_tiny = tiny;
+    lu->fixed = true;
+    const int run = lu_factor_run(lu, ms_out);
+    lu->fixed = false;
+    CFLX_TRY(run);
+    CFLX_TRY(launch_fixed_info_operand(lu->fix_rec, s));
+    lu->launches++;
+    if (c->world_size > 1) {
+        CFLX_NCCL(ncclGroupStart());
+        CFLX_NCCL(ncclAllReduce(lu->fix_rec, lu->fix_rec, 1, ncclInt, ncclSum, c->world, s));
+        CFLX_NCCL(ncclAllReduce(lu->fix_rec + 2, lu->fix_rec + 2, 1, ncclInt, ncclMin, c->world, s));
+        CFLX_NCCL(ncclGroupEnd());
+    }
+    int rec[4] = {0, 0, 0, 0};
+    CFLX_CUDA(cudaMemcpyAsync(rec, lu->fix_rec, sizeof(rec), cudaMemcpyDeviceToHost, s));
+    CFLX_CUDA(cudaStreamSynchronize(s));
+    if (nrepl_out) *nrepl_out = rec[0];
+    *info_out = rec[2] == INT_MAX ? 0 : rec[2];
     return CFLX_OK;
 }
 

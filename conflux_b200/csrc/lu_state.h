@@ -259,6 +259,18 @@ struct cflx_lu : cflx::Handle {
     std::vector<cflx::Event> ev;
     std::vector<char> ev_used;
     cflx::Event ev_fork, ev_join, ev_npiv;
+    // hist holds the permutation of a completed factorisation (cleared when one starts, set when it completes)
+    bool perm_done = false;
+    // cflx_lu_factor_fixed: the plan's fixed-order flag, the prescribed order (host and device, M each), this rank's
+    // pivot count per step, the tiny-pivot threshold, and the device record {replacements, first zero pivot, its min
+    // operand} (4 ints), the agreement operands (3 words) and the tile kernel's scratch (getrf_nopiv_scratch(v)); the
+    // device buffers are made by the first fixed call
+    bool fixed = false;
+    std::vector<int> fix_perm_h, fix_npiv;
+    double fix_tiny = 0.0;
+    cflx::DevBuf<int> fix_perm, fix_rec;
+    cflx::DevBuf<unsigned long long> fix_agree;
+    cflx::DevBuf<double> fix_ws;
 };
 
 namespace cflx {

@@ -244,6 +244,21 @@ std::size_t LU_rep(lu_params<T>& gv, T* C, int* permutation) {
     return (std::size_t)ms;
 }
 
+// LU_rep with a prescribed row order instead of the pivot search (cflx_lu_factor_fixed, collective): row q of P A is row
+// perm[q] of A (M ints, the same on every rank; null: the permutation of the last completed factorisation, for a nearby
+// matrix).  Pivots with |u| < tiny become copysign(tiny, u).  *nrepl (may be null) = the replacements over the grid;
+// returns 1 + the global column of the first exactly zero pivot, 0 when there is none.  C / permutation as LU_rep.
+template <class T>
+int LU_rep_fixed(lu_params<T>& gv, const int* perm, double tiny, T* C, int* permutation, int* nrepl = nullptr,
+                 double* ms_out = nullptr) {
+    int info = 0;
+    check(cflx_lu_set_local(gv.plan, gv.data.data()), "LU_rep_fixed: upload");
+    check(cflx_lu_factor_fixed(gv.plan, perm, tiny, nrepl, &info, ms_out), "LU_rep_fixed: factor");
+    if (C) check(cflx_lu_get_factors(gv.plan, C, permutation), "LU_rep_fixed: factors");
+    else if (permutation) check(cflx_lu_get_permutation(gv.plan, permutation), "LU_rep_fixed: permutation");
+    return info;
+}
+
 // The reference's validation (examples/conflux_miniapp.cpp:349-500) of the last LU_rep, on the GPU grid.  Collective.
 // Returns ||P*A - L*U||_F (what the reference prints as "Total Frobenius norm"); *relative = that / ||A||_F.
 template <class T>

@@ -83,6 +83,20 @@ int cflx_lu_queue_next_local(cflx_lu*, const double* host_next);
 /* COLLECTIVE.  Runs steps 0..Nt-1 on the GPU(s).  ms_out = device time of the main loop only (CUDA events on
  * this rank's stream, after a grid barrier) -- the region the reference times (conflux_opt.hpp:531-532,1805). */
 int cflx_lu_factor(cflx_lu*, double* ms_out);
+/* COLLECTIVE.  LU of the input with a prescribed row order: P A = L U with the P of `perm`, no pivot search (MAGMA's
+ * dgetrf_nopiv on a permuted matrix; static pivoting when tiny > 0).  perm: M ints (M the padded size), row q of P A is
+ * row perm[q] of A, the convention of cflx_lu_get_permutation; the same on every rank.  perm = NULL takes the
+ * permutation of the last completed factorisation of this handle (pivoted or fixed), which cflx_lu_set_local,
+ * cflx_lu_queue_next_local and cflx_lu_equilibrate* keep: a new matrix with the old pivots.  tiny (>= 0, absolute): a
+ * pivot u with |u| < tiny becomes copysign(tiny, u), +tiny for +-0; nrepl_out (may be NULL) counts the replacements over
+ * the grid.  info_out: 1 + the global column of the first exactly zero pivot (only with tiny = 0), else 0; the
+ * factorisation still completes, and entries computed from a zero pivot may be inf or NaN.  nrepl and info are the same
+ * on every rank.  ms_out, the input streaming, the scaling the factors carry, and every later call on the factors
+ * (solves, rcond, refinement, svx, inverse, det, validate, get_permutation = perm) as cflx_lu_factor.  CFLX_ERR_ARG for
+ * tiny < 0 or NaN, a perm that is not a permutation of [0, M), a NULL info_out, or perm differing between ranks (found
+ * by one world all-reduce before the first step: every rank returns the error); CFLX_ERR_STATE before cflx_lu_set_local
+ * and for perm = NULL before any factorisation completed. */
+int cflx_lu_factor_fixed(cflx_lu*, const int* perm, double tiny, int* nrepl_out, int* info_out, double* ms_out);
 /* COLLECTIVE.  C_host (Ml x Nl, may be NULL on layers pk != 0): L\U of P*A in the conflux layout, row
  * (k/Px)*v + i of rank (k%Px, pj, 0) = pivoted row k*v + i; permutation_out[M] = pivotIndsBuff. */
 int cflx_lu_get_factors(cflx_lu*, double* C_host, int* permutation_out);
@@ -495,6 +509,12 @@ int cflx_dbg_diag_inverse(int v, int nb, const double* A00, double* Uinv_out, do
  * 4 <= v <= 512; 1: the 128 x 128 block kernel, v == 128; 2: the 128-block tile driver, v % 128 == 0 and v >= 256.
  * L_out = L with zeros above the diagonal, LT_out = L^T, info_out = 1 + first non-positive pivot's column, or 0. */
 int cflx_dbg_potrf_tile(int v, const double* A, double* L_out, double* LT_out, int* info_out, int variant);
+/* Unpivoted LU of one v x v row-major block as cflx_lu_factor_fixed runs it (4 <= v <= 1024, v % 4 == 0).  variant 0:
+ * the one-CTA kernel on the whole block; 1: the 128-block driver (v % 128 == 0, v >= 256, what the factorisation runs
+ * there: 128 x 128 diagonal blocks on the one-CTA kernel, the rest on the TRSMs and the FP64 GEMM).  LU_out = L\U with unit L, pivots |u| < tiny replaced by copysign(tiny, u) (+tiny for
+ * +-0), nrepl_out (may be NULL) = the replacements, info_out = 1 + the first exactly zero pivot's column, or 0. */
+int cflx_dbg_getrf_nopiv_tile(int v, const double* A, double tiny, double* LU_out, int* nrepl_out, int* info_out,
+                              int variant);
 /* D = C - AT^T * B on the int8 wgmma path (error-free digit planes, ozaki.cu); K % 128 == 0, N even.  AT is
  * [K x (row0 + M)] and B [K x (col0 + N)]: the planes of every row / column are made, the product takes operand rows
  * [row0, row0 + M) and columns [col0, col0 + N), on at most max_ctas CTAs (0 = one per SM).  C/D [M x N].  Optional test
