@@ -15,7 +15,7 @@ import numpy as np
 
 from ._lib import ConfluxError, LIB_PATH, SYMBOLS, ShareLayout, check, lib
 
-__all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "LU_rep_fixed", "residual", "validate", "lu_solve", "lu_rcond", "lu_refine", "lu_refine_x", "lu_equilibrate", "lu_svx", "lu_equilibrate_b", "lu_svxx", "lu_inverse", "lu_det", "rhs_local_cols", "lu_solve_local", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
+__all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "LU_rep_fixed", "rbt_multipliers", "LU_rep_rbt", "lu_rbt_solve", "lu_rbt_apply_local", "residual", "validate", "lu_solve", "lu_rcond", "lu_refine", "lu_refine_x", "lu_equilibrate", "lu_svx", "lu_equilibrate_b", "lu_svxx", "lu_inverse", "lu_det", "rhs_local_cols", "lu_solve_local", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
 
 
 def auto_grid(M, N, P):
@@ -208,6 +208,58 @@ def LU_rep_fixed(gv, perm=None, tiny=0.0, C=None, permutation=None, upload=True,
         assert permutation.dtype == np.int32 and permutation.size >= gv.M
         check(lib().cflx_lu_get_permutation(gv._h, permutation.ctypes.data), "lu_get_permutation")
     return ms.value, nrepl.value, info.value
+
+
+def rbt_multipliers(M, depth, seed):
+    """The multipliers r of cflx_lu_rbt's butterflies U and V for an order-M matrix (cflx_rbt_multipliers, pure host):
+    (u, v), two (depth, M) arrays, row l = level l, every r in [e^-0.05, e^0.05]."""
+    u, v = np.empty((int(depth), int(M))), np.empty((int(depth), int(M)))
+    check(lib().cflx_rbt_multipliers(int(M), int(depth), ctypes.c_uint64(int(seed)), u.ctypes.data, v.ctypes.data),
+          "rbt_multipliers")
+    return u, v
+
+
+def LU_rep_rbt(gv, depth=2, seed=0, tiny=0.0, upload=True, C=None, permutation=None, u_out=None, v_out=None):
+    """The LU of a random butterfly transform of the input, without the pivot search (MAGMA's dgesv_rbt): cflx_lu_rbt
+    replaces the input A by W = U^T A V (U, V random recursive butterflies of `depth` levels from `seed`, the same on every
+    rank), then cflx_lu_factor_fixed factors W in the identity order with the tiny rule of LU_rep_fixed.  Solve with
+    lu_rbt_solve, or lu_rbt_apply_local around lu_solve_local.  Every other call on the factors (lu_solve, lu_rcond, lu_svx,
+    validate, ...) refers to W.  gv.M must be a multiple of 2**depth * v * Px.  upload=True copies gv.data to the device
+    first; upload=False transforms the input already there.  C and permutation as LU_rep; u_out / v_out ((depth, M)
+    float64 arrays) receive the multipliers.  COLLECTIVE.  Returns (ms, nrepl, info) as LU_rep_fixed."""
+    if upload:
+        a = np.ascontiguousarray(gv.data, dtype=np.float64)
+        check(lib().cflx_lu_set_local(gv._h, a.ctypes.data), "lu_set_local")
+    for o in (u_out, v_out):
+        if o is not None:
+            assert o.dtype == np.float64 and o.flags.c_contiguous and o.size == depth * gv.M
+    check(lib().cflx_lu_rbt(gv._h, int(depth), ctypes.c_uint64(int(seed)), _ptr(u_out), _ptr(v_out)), "lu_rbt")
+    return LU_rep_fixed(gv, perm=np.arange(gv.M, dtype=np.int32), tiny=tiny, C=C, permutation=permutation, upload=False)
+
+
+def lu_rbt_solve(gv, B, trans=False, refine=True):
+    """Solves A X = B (A^T X = B when trans) with factors of a transformed input (LU_rep_rbt): X = V inv(W) U^T B, or
+    U inv(W)^T V^T B.  refine=True refines the transformed system's solution as lu_refine does.  Returns (X, ferr, berr):
+    X in B's shape, and with refine the forward and backward errors of the transformed system (None without).  B as
+    lu_solve.  COLLECTIVE over gv.lu_comm; identical on every rank."""
+    B, B2, nrhs = _rhs(gv.M, B, "lu_rbt_solve")
+    X = np.empty_like(B2)
+    fe, be = np.empty(nrhs), np.empty(nrhs)
+    check(lib().cflx_lu_rbt_solve(gv._h, 1 if trans else 0, nrhs, B2.ctypes.data, nrhs, X.ctypes.data, nrhs,
+                                  1 if refine else 0, fe.ctypes.data, be.ctypes.data), "lu_rbt_solve")
+    return X.reshape(B.shape), (fe if refine else None), (be if refine else None)
+
+
+def lu_rbt_apply_local(gv, op, B_share, nrhs):
+    """One butterfly of the factors' transform (LU_rep_rbt) on the rows of this rank's right-hand side share, in place:
+    op 0 U^T, 1 V, 2 V^T, 3 U.  B_share as lu_solve_local's (a NumPy array or a torch CUDA tensor, (gv.Ml, n >=
+    rhs_local_cols(nrhs, gv.v, gv.Py)) float64 with contiguous rows).  A X = B distributed: lu_rbt_apply_local(gv, 0, B),
+    lu_solve_local, lu_rbt_apply_local(gv, 1, X); A^T X = B: ops 2 and 3 around the transposed solve.  Not collective.
+    Returns B_share."""
+    ptr, out, ld = _share_out(B_share, gv.Ml, rhs_local_cols(nrhs, gv.v, gv.Py), "lu_rbt_apply_local", strided=True,
+                              name="B_share")
+    check(lib().cflx_lu_rbt_apply_local(gv._h, int(op), int(nrhs), ptr, ld), "lu_rbt_apply_local")
+    return out
 
 
 def timeline(gv):
@@ -864,6 +916,19 @@ class dbg:
         return Bk, out
 
     @staticmethod
+    def rbt_share(op, X, v, depth, u=None, vv=None, grid=(1, 1), pos=(0, 0), M=None):
+        """cflx_dbg_rbt_share: op 0 U^T, 1 V, 2 V^T, 3 U on the rows of the right-hand side share X (Ml x ncols), or 4 W =
+        U^T X V on the matrix share X (Ml x Nl), with the r values u / vv ((depth, M) arrays, as rbt_multipliers gives
+        them).  M defaults to the covered order.  Returns the transformed copy."""
+        X = np.array(X, dtype=np.float64, order="C")
+        Ml, n = X.shape
+        lay = _share(v, Ml, n if op == 4 else 0, grid, pos, M=M)
+        ua = None if u is None else np.ascontiguousarray(u, dtype=np.float64)
+        va = None if vv is None else np.ascontiguousarray(vv, dtype=np.float64)
+        check(lib().cflx_dbg_rbt_share(int(op), ctypes.byref(lay), int(depth), _ptr(ua), _ptr(va), n, X.ctypes.data, n),
+              "dbg_rbt_share")
+        return X
+
     def norm_share(mode, A, v, Kappa=None, grid=(1, 1), pos=(0, 0), M=None):
         """The per-share pass of lu_rcond / cholesky.rcond's 1-norm and of the infinity-norm on one layer-0 share A (Ml x
         Nl, dbg.equil's layout), before the sum over the grid.  mode "col": the column sums of |a| over every entry;

@@ -462,6 +462,36 @@ int cflx_dbg_solve_local_share(int mode, const cflx_share_layout* share, int nrh
     return CFLX_OK;
 }
 
+// the random butterfly transforms (rbt.cu) on one share, with the multipliers formed as cflx_lu_rbt forms them
+int cflx_dbg_rbt_share(int op, const cflx_share_layout* share, int depth, const double* u, const double* v, int ncols,
+                       double* share_inout, int ld) {
+    CFLX_TRY(check_device());
+    Layout L;
+    CFLX_TRY(share_layout(__func__, share, op == 4 ? TILED | COVERED : TILED, &L));
+    REFUSE_IF(op < 0 || op > 4);
+    REFUSE_IF(depth < 1 || depth > 4);
+    REFUSE_IF(L.Ml % (L.v << depth));
+    REFUSE_IF(op == 4 && L.Nl % (L.v << depth));
+    REFUSE_IF(op != 4 && L.M < (L.Ml / L.v) * L.Px * L.v);
+    REFUSE_IF(op != 4 && ncols < 1);
+    const int w = op == 4 ? L.Nl : ncols;
+    REFUSE_IF(!share_inout || ld < w);
+    REFUSE_IF(!u && op != 1 && op != 2);
+    REFUSE_IF(!v && op != 0 && op != 3);
+    const size_t n = (size_t)depth * L.M;
+    std::vector<double> sc(2 * n, 0.0);
+    if (u) rbt_scales(u, n, sc.data());
+    if (v) rbt_scales(v, n, sc.data() + n);
+    const size_t x_n = (size_t)L.Ml * ld;
+    DevBuf<> dX, ds;
+    CFLX_TRY(stage(dX, x_n, share_inout));
+    CFLX_TRY(stage(ds, 2 * n, sc.data()));
+    CFLX_TRY(launch_rbt((RbtOp)op, dX.as<double>(), ld, L, w, INT_MAX, depth, ds.as<double>(), ds.as<double>() + n, 0));
+    CFLX_TRY(fetch(share_inout, dX.p, x_n));
+    CFLX_CUDA(cudaDeviceSynchronize());
+    return CFLX_OK;
+}
+
 // the per-share passes of the 1-norm and the infinity-norm (norm.cu) on one layer-0 share: mode 0 the column sums, 1 the
 // column sums of the symmetric matrix stored as its lower triangle, 2 the row sums
 int cflx_dbg_norm_share(int mode, const cflx_share_layout* share, const double* A, double* out) {

@@ -440,25 +440,28 @@ int pivot_growth_grid(const Grid& g, EquilState* e, const double* F, const doubl
 }
 
 // ---------------------------------------------------------------- the expert drivers' solve
-// B is scaled on the device by pre, solved there, refined by the caller's step, and X is unscaled by post before the
-// download.  refine(B, ldb, X, ldx) refines the device X in place.
-using SvxRefine = std::function<int(const double*, int, double*, int)>;
-static int svx_tail(EquilState* e, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx,
-                    const double* pre, const double* post, const SvxRefine& refine) {
+int svx_tail(EquilState* e, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx,
+             const RowTransform& pre, const RowTransform& post, const SvxRefine& refine) {
     cudaStream_t s = op.grid.comm->stream;
     const int M = op.grid.M, ldn = (int)round_up(nrhs, 8);
     CFLX_TRY(equil_grow(e, M, ldn));
     double *dB = e->B, *dX = e->X;
     CFLX_CUDA(cudaMemcpy2DAsync(dB, ldn * sizeof(double), B, (size_t)ldb * sizeof(double), nrhs * sizeof(double), M,
                                 cudaMemcpyDefault, s));
-    if (pre) CFLX_TRY(launch_scale_rows(dB, ldn, M, nrhs, pre, s));
+    if (pre) CFLX_TRY(pre(dB, ldn, nrhs));
     CFLX_TRY(op.solve(false, nrhs, dB, ldn, dX, ldn));
     CFLX_TRY(refine(dB, ldn, dX, ldn));
-    if (post) CFLX_TRY(launch_scale_rows(dX, ldn, M, nrhs, post, s));
+    if (post) CFLX_TRY(post(dX, ldn, nrhs));
     CFLX_CUDA(cudaMemcpy2DAsync(X, (size_t)ldx * sizeof(double), dX, ldn * sizeof(double), nrhs * sizeof(double), M,
                                 cudaMemcpyDefault, s));
     CFLX_CUDA(cudaStreamSynchronize(s));
     return CFLX_OK;
+}
+
+// the diagonal scaling by d (null: none) as a row transform of an M-row array
+static RowTransform scale_rows(const Grid& g, const double* d) {
+    if (!d) return RowTransform();
+    return [&g, d](double* X, int64_t ld, int n) { return launch_scale_rows(X, ld, g.M, n, d, g.comm->stream); };
 }
 
 int svx_run(EquilState* e, RefineCache* rc, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx,
@@ -466,7 +469,7 @@ int svx_run(EquilState* e, RefineCache* rc, const RefineOp& op, int nrhs, const 
     auto refine = [&](const double* dB, int ldb_, double* dX, int ldx_) {
         return refine_run(rc, op, nrhs, dB, ldb_, dX, ldx_, ferr, berr);
     };
-    CFLX_TRY(svx_tail(e, op, nrhs, B, ldb, X, ldx, pre, post, refine));
+    CFLX_TRY(svx_tail(e, op, nrhs, B, ldb, X, ldx, scale_rows(op.grid, pre), scale_rows(op.grid, post), refine));
     if (ferr && post)
         for (int j = 0; j < nrhs; ++j) ferr[j] /= cnd;
     *info = rcond < std::ldexp(1.0, -53) ? op.grid.M + 1 : 0;
@@ -479,7 +482,7 @@ int svxx_run(EquilState* e, RefineCache* rc, const RefineOp& op, int nrhs, const
     auto refine = [&](const double* dB, int ldb_, double* dX, int ldx_) {
         return refine_x_run(rc, op, nrhs, dB, ldb_, dX, ldx_, d, rcond, cwise, berr, err_norm, err_comp, info);
     };
-    return svx_tail(e, op, nrhs, B, ldb, X, ldx, pre, post, refine);
+    return svx_tail(e, op, nrhs, B, ldb, X, ldx, scale_rows(op.grid, pre), scale_rows(op.grid, post), refine);
 }
 
 }  // namespace cflx

@@ -728,6 +728,11 @@ RefineOp lu_refine_op(cflx_lu* lu, bool t) {
 int lu_equilibrate(cflx_lu* lu, int apply, bool pow2, double* r_out, double* c_out, double* rowcnd_out,
                    double* colcnd_out, double* amax_out, char* equed_out, int* info_out) {
     if (!lu || (apply != 0 && apply != 1) || !info_out) return CFLX_ERR_ARG;
+    if (apply && lu->rbt.in.depth) {
+        set_last_error("equilibration refused: the input carries a random butterfly transform (cflx_lu_rbt); upload it "
+                       "again first");
+        return CFLX_ERR_STATE;
+    }
     CFLX_TRY(handle_equil_begin(lu, apply != 0));
     if (lu->a0_is_next) CFLX_CUDA(cudaStreamWaitEvent(lu->comm->stream, lu->ev_upload, 0));  // A0 holds a streamed next input
     double rowcnd = 0.0, colcnd = 0.0, amax = 0.0;
@@ -977,6 +982,7 @@ int cflx_lu_info(const cflx_lu* lu, int* o) {
 int cflx_lu_set_local(cflx_lu* lu, const double* host_local) {
     if (!lu || !host_local) return CFLX_ERR_ARG;
     CFLX_TRY(handle_set_local(lu, host_local));
+    lu->rbt.in.depth = 0;
     lu->a0_is_next = false;
     lu->next_host = nullptr;
     return CFLX_OK;
@@ -1020,8 +1026,9 @@ int lu_factor_run(cflx_lu* lu, double* ms_out) {
     }
     lu->a0_is_next = false;
     lu->sv.ready = false;
-    // the factors carry the input's scaling; a queued next input arrives unscaled
+    // the factors carry the input's scaling and transform; a queued next input arrives unscaled and untransformed
     CFLX_TRY(equil_pass_on(&lu->eq, lu->M, lu->next_host != nullptr, s));
+    CFLX_TRY(rbt_pass_on(&lu->rbt, lu->M, lu->next_host != nullptr, s));
     if (lu->next_host) {  // queued next input: overwrite A0 behind the working copy, concurrently with everything below
         CFLX_CUDA(cudaEventRecord(lu->ev_a0_read, s));
         CFLX_CUDA(cudaStreamWaitEvent(lu->copy, lu->ev_a0_read, 0));
@@ -1107,20 +1114,25 @@ unsigned long long order_hash(const std::vector<int>& p) {
     return h;
 }
 
-// COLLECTIVE (world): *same = every rank has ok and the same hash, from one ncclMin over {h, ~h, ok}: min(~h) = ~max(h)
-int fixed_agree(cflx_lu* lu, bool ok, unsigned long long h, bool* same) {
+// COLLECTIVE (world): *same = every rank has ok and the same words, from one ncclMin over {w.., ~w.., ok}: min(~w) =
+// ~max(w)
+int world_agree(cflx_lu* lu, bool ok, std::initializer_list<unsigned long long> words, bool* same) {
     cflx_comm* c = lu->comm;
     if (c->world_size == 1) {
         *same = ok;
         return CFLX_OK;
     }
-    unsigned long long w[3] = {h, ~h, ok ? 1ull : 0ull};
-    if (!lu->fix_agree) CFLX_TRY(lu->fix_agree.alloc(3));
-    CFLX_CUDA(cudaMemcpyAsync(lu->fix_agree, w, sizeof(w), cudaMemcpyHostToDevice, c->stream));
-    CFLX_NCCL(ncclAllReduce(lu->fix_agree, lu->fix_agree, 3, ncclUint64, ncclMin, c->world, c->stream));
-    CFLX_CUDA(cudaMemcpyAsync(w, lu->fix_agree, sizeof(w), cudaMemcpyDeviceToHost, c->stream));
+    const size_t n = words.size();
+    std::vector<unsigned long long> w(words);
+    for (unsigned long long x : words) w.push_back(~x);
+    w.push_back(ok ? 1ull : 0ull);
+    CFLX_TRY(lu->agree.grow(w.size()));
+    CFLX_CUDA(cudaMemcpyAsync(lu->agree, w.data(), sizeof(w[0]) * w.size(), cudaMemcpyHostToDevice, c->stream));
+    CFLX_NCCL(ncclAllReduce(lu->agree, lu->agree, w.size(), ncclUint64, ncclMin, c->world, c->stream));
+    CFLX_CUDA(cudaMemcpyAsync(w.data(), lu->agree, sizeof(w[0]) * w.size(), cudaMemcpyDeviceToHost, c->stream));
     CFLX_CUDA(cudaStreamSynchronize(c->stream));
-    *same = w[2] == 1 && w[0] == ~w[1];
+    *same = w[2 * n] == 1;
+    for (size_t i = 0; i < n; ++i) *same = *same && w[i] == ~w[n + i];
     return CFLX_OK;
 }
 
@@ -1163,6 +1175,43 @@ int fixed_prepare(cflx_lu* lu, const int* perm, double tiny, const int* info_out
     if (ws && !lu->fix_ws) CFLX_TRY(lu->fix_ws.alloc(ws));
     return CFLX_OK;
 }
+
+// The checks of cflx_lu_rbt that need no other rank
+int rbt_prepare(cflx_lu* lu, int depth) {
+    if (depth < 1 || depth > 4) {
+        set_last_error("cflx_lu_rbt: depth must be in [1, 4], got %d", depth);
+        return CFLX_ERR_ARG;
+    }
+    if (!lu->have_input) {
+        set_last_error("cflx_lu_rbt before cflx_lu_set_local");
+        return CFLX_ERR_STATE;
+    }
+    if (lu->rbt.in.depth) {
+        set_last_error("cflx_lu_rbt refused: the input is already transformed; upload it again first");
+        return CFLX_ERR_STATE;
+    }
+    if (lu->eq.in.equed != 'N') {
+        set_last_error("cflx_lu_rbt refused: the input is scaled (equed = '%c'); upload it again first", lu->eq.in.equed);
+        return CFLX_ERR_STATE;
+    }
+    const long long q = (long long)lu->v * lu->Px << depth;
+    if (lu->M % q) {
+        set_last_error("cflx_lu_rbt: M = %d is not a multiple of 2^%d v Px = %lld; the smallest M that works is %lld: "
+                       "pad A with the identity to that order", lu->M, depth, q, (lu->M + q - 1) / q * q);
+        return CFLX_ERR_UNSUPPORTED;
+    }
+    return CFLX_OK;
+}
+
+// The transform the factors carry, as a row transform of an M-row device array (the replicated right-hand sides)
+RowTransform rbt_rows(cflx_lu* lu, RbtOp op) {
+    const RbtRecord& f = lu->rbt.fac;
+    const Layout rows{lu->M, lu->v, lu->Nt, lu->M, 0, 1, 1, 0, 0};  // global row r is row r
+    const double *su = f.s, *sv = f.s + (size_t)f.depth * lu->M;
+    cudaStream_t s = lu->comm->stream;
+    const int depth = f.depth;
+    return [=](double* X, int64_t ld, int n) { return launch_rbt(op, X, ld, rows, n, INT_MAX, depth, su, sv, s); };
+}
 }  // namespace
 
 extern "C" {
@@ -1188,7 +1237,7 @@ int cflx_lu_factor_fixed(cflx_lu* lu, const int* perm, double tiny, int* nrepl_o
     cudaStream_t s = c->stream;
     const int rc = fixed_prepare(lu, perm, tiny, info_out);
     bool same = false;
-    CFLX_TRY(fixed_agree(lu, rc == CFLX_OK, rc == CFLX_OK ? order_hash(lu->fix_perm_h) : 0, &same));
+    CFLX_TRY(world_agree(lu, rc == CFLX_OK, {rc == CFLX_OK ? order_hash(lu->fix_perm_h) : 0}, &same));
     if (rc != CFLX_OK) return rc;
     if (!same) {
         set_last_error("cflx_lu_factor_fixed: the ranks passed different orders, or another rank refused its arguments");
@@ -1219,6 +1268,96 @@ int cflx_lu_factor_fixed(cflx_lu* lu, const int* perm, double tiny, int* nrepl_o
     CFLX_CUDA(cudaStreamSynchronize(s));
     if (nrepl_out) *nrepl_out = rec[0];
     *info_out = rec[2] == INT_MAX ? 0 : rec[2];
+    return CFLX_OK;
+}
+
+// COLLECTIVE.  A0 <- U^T A0 V on every rank's share (rbt.cu), after the ranks agreed on depth and seed with one world
+// all-reduce, so that a refusal anywhere is a refusal everywhere.  The input changes: the factors and the solve cache
+// are dropped, as by an equilibration that scales the input.
+int cflx_lu_rbt(cflx_lu* lu, int depth, uint64_t seed, double* u_out, double* v_out) {
+    if (!lu) return CFLX_ERR_ARG;
+    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    const int rc = rbt_prepare(lu, depth);
+    bool same = false;
+    CFLX_TRY(world_agree(lu, rc == CFLX_OK, {seed, (unsigned long long)depth}, &same));
+    if (rc != CFLX_OK) return rc;
+    if (!same) {
+        set_last_error("cflx_lu_rbt: the ranks passed different depths or seeds, or another rank refused its arguments");
+        return CFLX_ERR_ARG;
+    }
+    const int M = lu->M;
+    const size_t n = (size_t)depth * M;
+    std::vector<double> r(2 * n), sc(2 * n);
+    rbt_multipliers(M, depth, seed, 0, r.data());
+    rbt_multipliers(M, depth, seed, 1, r.data() + n);
+    if (u_out) std::memcpy(u_out, r.data(), sizeof(double) * n);
+    if (v_out) std::memcpy(v_out, r.data() + n, sizeof(double) * n);
+    rbt_scales(r.data(), 2 * n, sc.data());
+    cudaStream_t s = lu->comm->stream;
+    if (lu->a0_is_next) CFLX_CUDA(cudaStreamWaitEvent(s, lu->ev_upload, 0));  // A0 holds a streamed next input
+    lu->factored = false;
+    lu->sv.ready = false;
+    RbtRecord& in = lu->rbt.in;
+    CFLX_TRY(rbt_record_set(&in, depth, seed, sc.data(), M, s));
+    if (lu->pk == 0) CFLX_TRY(launch_rbt(RbtOp::W, lu->A0, lu->Nl, *lu, lu->Nl, INT_MAX, depth, in.s, in.s + n, s));
+    CFLX_CUDA(cudaStreamSynchronize(s));  // sc is a host temporary
+    return CFLX_OK;
+}
+
+// COLLECTIVE.  op(A) X = B through the transformed system the factors represent: B to the device, U^T (V^T) on its rows,
+// the solve with W (W^T), dgerfs on that system with refine, V (U) on the rows of X; svx_tail with the butterflies as its
+// row transforms.
+int cflx_lu_rbt_solve(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, double* X, int ldx, int refine,
+                      double* ferr_out, double* berr_out) {
+    if (!lu || (trans != 0 && trans != 1) || (refine != 0 && refine != 1) || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B ||
+        !X)
+        return CFLX_ERR_ARG;
+    CFLX_TRY(lu_check(lu, "RBT solve", refine != 0));
+    if (!lu->rbt.fac.depth) {
+        set_last_error("cflx_lu_rbt_solve: the factors carry no random butterfly transform (cflx_lu_rbt before the "
+                       "factorisation)");
+        return CFLX_ERR_STATE;
+    }
+    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    const bool t = trans != 0;
+    const RefineOp op = lu_refine_op(lu, t);
+    auto refine_step = [&](const double* dB, int lb, double* dX, int lx) {
+        return refine ? refine_run(&lu->sv.rf, op, nrhs, dB, lb, dX, lx, ferr_out, berr_out) : CFLX_OK;
+    };
+    return svx_tail(&lu->eq, op, nrhs, B, ldb, X, ldx, rbt_rows(lu, t ? RbtOp::VT : RbtOp::UT),
+                    rbt_rows(lu, t ? RbtOp::U : RbtOp::V), refine_step);
+}
+
+// Not collective.  One of the factors' butterflies on the rows of this rank's right-hand side share (rbt.cu); a host
+// share goes through one temporary device share.
+int cflx_lu_rbt_apply_local(cflx_lu* lu, int op, int nrhs, double* B_local, int ldb) {
+    if (!lu || op < 0 || op > 3 || nrhs < 1 || !B_local) return CFLX_ERR_ARG;
+    const int ncl = rhs_local_cols(nrhs, lu->v, lu->Py);
+    if (ldb < ncl) return CFLX_ERR_ARG;
+    CFLX_TRY(lu_check(lu, "RBT apply", false));
+    const RbtRecord& f = lu->rbt.fac;
+    if (!f.depth) {
+        set_last_error("cflx_lu_rbt_apply_local: the factors carry no random butterfly transform (cflx_lu_rbt before "
+                       "the factorisation)");
+        return CFLX_ERR_STATE;
+    }
+    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    bool dev = false;
+    CFLX_TRY(share_kind(*lu, B_local, "B_local", &dev));
+    cudaStream_t s = lu->comm->stream;
+    const size_t row = sizeof(double) * ncl;
+    DevBuf<double> tmp;
+    double* X = B_local;
+    int64_t ld = ldb;
+    if (!dev) {
+        CFLX_TRY(tmp.alloc((size_t)lu->Ml * ncl));
+        CFLX_CUDA(cudaMemcpy2DAsync(tmp, row, B_local, sizeof(double) * ldb, row, lu->Ml, cudaMemcpyHostToDevice, s));
+        X = tmp;
+        ld = ncl;
+    }
+    CFLX_TRY(launch_rbt((RbtOp)op, X, ld, *lu, ncl, nrhs, f.depth, f.s, f.s + (size_t)f.depth * lu->M, s));
+    if (!dev) CFLX_CUDA(cudaMemcpy2DAsync(B_local, sizeof(double) * ldb, tmp, row, row, lu->Ml, cudaMemcpyDeviceToHost, s));
+    CFLX_CUDA(cudaStreamSynchronize(s));
     return CFLX_OK;
 }
 

@@ -140,6 +140,34 @@ int equil_record_set(EquilRecord* dst, char equed, double rowcnd, double colcnd,
 // in -> fac; then, when `next_is_plain`, in becomes 'N' (a streamed next input)
 int equil_pass_on(EquilState* e, int M, bool next_is_plain, cudaStream_t s);
 
+// ---------------------------------------------------------------- random butterfly transforms (rbt.cu)
+// The transform an input carries (cflx_lu_rbt: A0 <- U^T A0 V), and the one the factors of that input carry on to
+// cflx_lu_rbt_solve / cflx_lu_rbt_apply_local, kept like EquilState's records: depth 0 (none) or 1 .. 4, the seed, and
+// s: the device multipliers s = fl(r fl(1/sqrt 2)), U's d x M then V's d x M (every rank).
+struct RbtRecord {
+    int depth = 0;
+    uint64_t seed = 0;
+    DevBuf<double> s;
+};
+struct RbtState {
+    RbtRecord in, fac;
+};
+// *dst = {depth, seed} with a copy of s (2 depth M doubles, host or device) when depth > 0
+int rbt_record_set(RbtRecord* dst, int depth, uint64_t seed, const double* s, int M, cudaStream_t st);
+// in -> fac; then, when `next_is_plain`, in carries no transform (a streamed next input)
+int rbt_pass_on(RbtState* t, int M, bool next_is_plain, cudaStream_t s);
+// r (depth x M, level l at l M) of side 0 (U) or 1 (V): r = exp((w - 0.5) / 10) with w the top 53 bits of splitmix64's
+// finaliser of seed + 0x9E3779B97F4A7C15 (((2 l + side) << 32) + i + 1), in [e^-0.05, e^0.05]; pure host
+void rbt_multipliers(int M, int depth, uint64_t seed, int side, double* r);
+// s[i] = fl(r[i] fl(1/sqrt 2)) for i < n
+void rbt_scales(const double* r, size_t n, double* s);
+// The operations on a share X (ld) of L's rows: U^T, V, V^T, U on the local columns c < ncols with L.col(c) < col_lim
+// (a right-hand side), or W = U^T X V on the whole Ml x ncols share (ncols = L.Nl).  Needs Ml (and for W ncols) a multiple
+// of 2^depth v; su / sv: the device multipliers of U and V (depth x L.M each).  Bits as oracle/rbt_ref.py.
+enum class RbtOp { UT = 0, V = 1, VT = 2, U = 3, W = 4 };
+int launch_rbt(RbtOp op, double* X, int64_t ld, const Layout& L, int ncols, int col_lim, int depth, const double* su,
+               const double* sv, cudaStream_t s);
+
 // What a solve keeps between calls: prepared by the first solve after a factorisation, dropped (ready = false) by
 // set_local / factor, freed with the object.  The work buffers have ldn columns and are grown, never shrunk.
 struct SolveCache {
@@ -263,14 +291,16 @@ struct cflx_lu : cflx::Handle {
     bool perm_done = false;
     // cflx_lu_factor_fixed: the plan's fixed-order flag, the prescribed order (host and device, M each), this rank's
     // pivot count per step, the tiny-pivot threshold, and the device record {replacements, first zero pivot, its min
-    // operand} (4 ints), the agreement operands (3 words) and the tile kernel's scratch (getrf_nopiv_scratch(v)); the
-    // device buffers are made by the first fixed call
+    // operand} (4 ints) and the tile kernel's scratch (getrf_nopiv_scratch(v)); the device buffers are made by the first
+    // fixed call.  agree: the words the ranks compare before a fixed factorisation or a transform (world_agree)
     bool fixed = false;
     std::vector<int> fix_perm_h, fix_npiv;
     double fix_tiny = 0.0;
     cflx::DevBuf<int> fix_perm, fix_rec;
-    cflx::DevBuf<unsigned long long> fix_agree;
+    cflx::DevBuf<unsigned long long> agree;
     cflx::DevBuf<double> fix_ws;
+    // cflx_lu_rbt: the transform of the input and of the factors
+    cflx::RbtState rbt;
 };
 
 namespace cflx {
@@ -457,6 +487,13 @@ int launch_column_stats(const double* Y, const double* DY, const double* d, int 
 int launch_select_cols(const double* in, const int* active, int M, int ldn, double* out, cudaStream_t s);
 int launch_add_cols(double* X, const double* D, const int* active, int M, int ldn, cudaStream_t s);
 int launch_update_x(double* Y, double* T, const double* DY, const int* how, int M, int ldn, cudaStream_t s);
+// The expert drivers' solve (equil.cu), COLLECTIVE: B (host or device, M x nrhs) to the device, pre on its rows, X =
+// op.solve(false, B), refine(B, ldb, X, ldx) on the device X in place, post on the rows of X, X out; synchronises.  A
+// row transform (empty: none) runs in place on an M x n device array with leading dimension ld, on the grid's stream.
+using RowTransform = std::function<int(double* X, int64_t ld, int n)>;
+using SvxRefine = std::function<int(const double*, int, double*, int)>;
+int svx_tail(EquilState* e, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx,
+             const RowTransform& pre, const RowTransform& post, const SvxRefine& refine);
 // The solve and refinement of cflx_lu_svx / cflx_chol_svx (equil.cu), COLLECTIVE: B (host or device) to the device, its
 // rows scaled by pre (may be null), X = op.solve(false, B), refine_run, the rows of X scaled by post (may be null), X out;
 // when post is not null, ferr is divided by cnd.  Then *info = M + 1 when rcond < 2^-53 (dgesvx / dposvx: the matrix is
@@ -575,6 +612,8 @@ struct SolveLocalArgs {
     int ldx;
     bool x_dev;
 };
+// *dev: p is device (or managed) memory, which must be on this rank's device (else CFLX_ERR_ARG)
+int share_kind(const Grid& g, const void* p, const char* what, bool* dev);
 // CFLX_ERR_ARG for nrhs < 1, a NULL B on layer 0, ldb (layer 0) or ldx (X set) below rhs_local_cols, X == B with
 // ldx != ldb, or device memory of another device; CFLX_OK with *a filled otherwise.  No collective.
 int solve_local_args(const Grid& g, int nrhs, const double* B, int ldb, const double* X, int ldx, SolveLocalArgs* a);

@@ -62,7 +62,8 @@ int valid_cols(int nrhs, int v, int Py, int pj) {
     return n;
 }
 
-// *dev: p is device (or managed) memory, which must be on this rank's device
+}  // namespace
+
 int share_kind(const Grid& g, const void* p, const char* what, bool* dev) {
     cudaPointerAttributes at{};
     *dev = cudaPointerGetAttributes(&at, p) == cudaSuccess &&
@@ -75,7 +76,6 @@ int share_kind(const Grid& g, const void* p, const char* what, bool* dev) {
     }
     return CFLX_OK;
 }
-}  // namespace
 
 int rhs_local_cols(int nrhs, int v, int Py) { return v * (((nrhs + v - 1) / v + Py - 1) / Py); }
 

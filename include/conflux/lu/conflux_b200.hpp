@@ -259,6 +259,32 @@ int LU_rep_fixed(lu_params<T>& gv, const int* perm, double tiny, T* C, int* perm
     return info;
 }
 
+// The LU of a random butterfly transform of the input, without the pivot search (cflx_lu_rbt, then cflx_lu_factor_fixed
+// in the identity order; collective): A is replaced by W = U^T A V with butterflies of `depth` levels from `seed` (the same
+// on every rank; gv.M a multiple of 2^depth v Px), and W is factored with the tiny rule of LU_rep_fixed.  Solve with
+// LU_rbt_solve.  Returns 1 + the global column of the first exactly zero pivot of W, 0 when there is none.
+template <class T>
+int LU_rep_rbt(lu_params<T>& gv, int depth = 2, uint64_t seed = 0, double tiny = 0.0, int* nrepl = nullptr,
+               double* ms_out = nullptr) {
+    int info = 0;
+    std::vector<int> ident(gv.M);
+    for (int i = 0; i < gv.M; ++i) ident[i] = i;
+    check(cflx_lu_set_local(gv.plan, gv.data.data()), "LU_rep_rbt: upload");
+    check(cflx_lu_rbt(gv.plan, depth, seed, nullptr, nullptr), "LU_rep_rbt: transform");
+    check(cflx_lu_factor_fixed(gv.plan, ident.data(), tiny, nrepl, &info, ms_out), "LU_rep_rbt: factor");
+    return info;
+}
+
+// Solves A X = B (A^T X = B when transposed) with the factors of LU_rep_rbt (cflx_lu_rbt_solve, collective): X = V inv(W)
+// U^T B, refined on the transformed system when `refine`; ferr / berr (nrhs each, may be null) are that system's errors.
+// B / X as LU_solve.
+template <class T>
+void LU_rbt_solve(lu_params<T>& gv, int nrhs, const T* B, int ldb, T* X, int ldx, bool transposed = false,
+                  bool refine = true, double* ferr = nullptr, double* berr = nullptr) {
+    check(cflx_lu_rbt_solve(gv.plan, transposed ? 1 : 0, nrhs, B, ldb, X, ldx, refine ? 1 : 0, ferr, berr),
+          "LU_rbt_solve");
+}
+
 // The reference's validation (examples/conflux_miniapp.cpp:349-500) of the last LU_rep, on the GPU grid.  Collective.
 // Returns ||P*A - L*U||_F (what the reference prints as "Total Frobenius norm"); *relative = that / ||A||_F.
 template <class T>

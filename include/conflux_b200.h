@@ -65,6 +65,11 @@ int cflx_auto_grid(int M, int N, int P, int* Px, int* Py, int* Pz);
 int cflx_lu_dims(int M, int N, int v, int Px, int Py, int Pz, int* dims_out);
 /* lu_params::InitMatrix, random branch: fills the Ml x Nl row-major local array of `rank` (layers pk != 0 zero) */
 int cflx_init_matrix_host(int M, int N, int v, int Px, int Py, int Pz, int rank, int seed, double* local_out);
+/* The multipliers of cflx_lu_rbt's random butterflies U (u_out) and V (v_out), depth x M doubles each (row l = level l),
+ * either may be NULL: r = exp((w - 0.5) / 10) with the host C library's exp, w = (z >> 11) 2^-53, z = splitmix64's
+ * finaliser of seed + 0x9E3779B97F4A7C15 (((2 l + side) << 32) + i + 1) mod 2^64 (side 0 for U, 1 for V); every r lies in
+ * [e^-0.05, e^0.05].  CFLX_ERR_ARG for depth outside [1, 4], M < 1, M % 2^depth != 0, or both outputs NULL. */
+int cflx_rbt_multipliers(int M, int depth, uint64_t seed, double* u_out, double* v_out);
 
 /* ---- the factorisation ----------------------------------------------------------------------------------- */
 /* COLLECTIVE.  Px <= 0 selects cflx_auto_grid(world_size).  Requires Px == Py, Px*Py*Pz == world_size,
@@ -97,6 +102,37 @@ int cflx_lu_factor(cflx_lu*, double* ms_out);
  * by one world all-reduce before the first step: every rank returns the error); CFLX_ERR_STATE before cflx_lu_set_local
  * and for perm = NULL before any factorisation completed. */
 int cflx_lu_factor_fixed(cflx_lu*, const int* perm, double tiny, int* nrepl_out, int* info_out, double* ms_out);
+/* COLLECTIVE.  Random butterfly transform of the input the device holds (MAGMA's dgesv_rbt; Baboulin, Dongarra,
+ * Herrmann and Tomov, ACM TOMS 39(2), 2013): A <- W = U^T A V in place, with U and V random recursive butterflies of
+ * depth 1 .. 4 (2 in practice) from the multipliers of cflx_rbt_multipliers(M, depth, seed) (u_out / v_out, may be NULL,
+ * as there).  With probability one W needs no pivoting: factor it with cflx_lu_factor_fixed in the identity order, then
+ * solve with cflx_lu_rbt_solve or cflx_lu_rbt_apply_local.  Each rank transforms its own share, with no communication
+ * beyond one world all-reduce that first checks every rank's depth and seed.  Every later call on the factors (solves,
+ * rcond, refinement, svx, inverse, det, validate) refers to W, as after an equilibration.  The factors and the solve
+ * cache are dropped, as by cflx_lu_set_local; the next factorisation's factors carry the transform.  An input from
+ * cflx_lu_set_local or a queued upload carries none.  CFLX_ERR_ARG for depth outside [1, 4], or ranks that differ in
+ * depth or seed or refused their arguments (every rank returns the error); CFLX_ERR_UNSUPPORTED when M is not a multiple
+ * of 2^depth v Px (the message names the smallest M that works: pad A with the identity); CFLX_ERR_STATE before
+ * cflx_lu_set_local, on an input that is already transformed, and on a scaled input (cflx_lu_equilibrate*, apply = 1,
+ * which in turn refuses a transformed input). */
+int cflx_lu_rbt(cflx_lu*, int depth, uint64_t seed, double* u_out, double* v_out);
+/* COLLECTIVE.  Solves A X = B (trans 0) or A^T X = B (trans 1) with factors that carry a transform (cflx_lu_rbt, then a
+ * factorisation): X = V inv(W) U^T B, or X = U inv(W)^T V^T B.  B, X, ldb, ldx as cflx_lu_refine.  refine = 1 refines the
+ * solution of the transformed system W Y = U^T B (W^T Y = V^T B) as cflx_lu_refine does, so ferr_out and berr_out (nrhs
+ * each, may be NULL; not written with refine = 0) are the forward and backward errors of Y in that system, not of X in
+ * A X = B.  No singularity check (like getrs).  CFLX_ERR_ARG as cflx_lu_refine, and for refine not 0 / 1; CFLX_ERR_STATE
+ * as cflx_lu_solve (with refine = 1 as cflx_lu_refine), and when the factors carry no transform.  Results identical on
+ * every rank; leaves the factors, the input, later solves and the launch count as they are. */
+int cflx_lu_rbt_solve(cflx_lu*, int trans, int nrhs, const double* B, int ldb, double* X, int ldx, int refine,
+                      double* ferr_out, double* berr_out);
+/* Not collective.  One butterfly of the factors' transform on the rows of this rank's right-hand side share, in place:
+ * op 0 U^T, 1 V, 2 V^T, 3 U.  B_local: the share of cflx_lu_solve_local's layout, Ml x cflx_rhs_local_cols(nrhs, v, Py),
+ * leading dimension ldb, host or device memory as there; columns whose global index is >= nrhs are left as they are.
+ * A X = B with B and X distributed is apply_local(0) on B, cflx_lu_solve_local, apply_local(1) on X; A^T X = B is
+ * apply_local(2), the transposed solve, apply_local(3).  CFLX_ERR_ARG for op outside [0, 3], nrhs < 1, a NULL B_local,
+ * ldb below the local column count, or device memory of another device; CFLX_ERR_STATE as cflx_lu_solve, and when the
+ * factors carry no transform. */
+int cflx_lu_rbt_apply_local(cflx_lu*, int op, int nrhs, double* B_local, int ldb);
 /* COLLECTIVE.  C_host (Ml x Nl, may be NULL on layers pk != 0): L\U of P*A in the conflux layout, row
  * (k/Px)*v + i of rank (k%Px, pj, 0) = pivoted row k*v + i; permutation_out[M] = pivotIndsBuff. */
 int cflx_lu_get_factors(cflx_lu*, double* C_host, int* permutation_out);
@@ -440,6 +476,12 @@ int cflx_dbg_solve_local_share(int mode, const cflx_share_layout* share, int nrh
  * covered, non-empty), before the all-reduce over the grid.  out (M doubles): by global index, this share's part of the
  * column sums of |a| (modes 0, 1) or of the row sums (mode 2), zero where it holds nothing. */
 int cflx_dbg_norm_share(int mode, const cflx_share_layout* share, const double* A, double* out);
+/* cflx_lu_rbt's butterflies on one share (tiled; Ml, and for op 4 Nl, a multiple of 2^depth v), in place: op 0 U^T, 1 V,
+ * 2 V^T, 3 U on the rows of an Ml x ncols right-hand side share (M >= (Ml / v) Px v; Nl is not read), every column; op 4 W = U^T X V on
+ * an Ml x Nl matrix share (covered; ncols is not read).  u / v: the r values of cflx_rbt_multipliers (depth x M each; the
+ * side an op does not use may be NULL), formed into the library's s = fl(r fl(1/sqrt 2)) here.  ld >= ncols (op 4: Nl). */
+int cflx_dbg_rbt_share(int op, const cflx_share_layout* share, int depth, const double* u, const double* v, int ncols,
+                       double* share_inout, int ld);
 /* cflx_chol_validate's per-share kernels on one layer-0 share A (tiled, non-empty; M = the larger of (Ml / v) Px v and
  * (Nl / v) Py v; Kappa >= 1); each output may be NULL:
  *   sumsq_out: the sum of squares of the entries with global row >= global column and global row < Kappa v;
