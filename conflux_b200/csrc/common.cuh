@@ -25,6 +25,18 @@ void set_last_error(const char* fmt, ...);
         }                                                                                              \
     } while (0)
 
+// A refused call of `who`: the error reads "<who>: refused, <what>"
+inline int refuse(const char* who, const char* what, int status = CFLX_ERR_ARG) {
+    set_last_error("%s: refused, %s", who, what);
+    return status;
+}
+// CFLX_ERR_ARG naming the function and the condition that failed; REFUSE_FOR refuses in the name of a caller `who`
+#define REFUSE_FOR(who, cond)                                 \
+    do {                                                      \
+        if (cond) return ::cflx::refuse((who), #cond);        \
+    } while (0)
+#define REFUSE_IF(cond) REFUSE_FOR(__func__, cond)
+
 #define CFLX_TRY(call)              \
     do {                            \
         int rc__ = (call);          \

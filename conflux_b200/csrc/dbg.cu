@@ -24,13 +24,6 @@ int check_device() {
     return CFLX_OK;
 }
 
-// a refused call of hook `who`: the error names the hook and the condition that failed
-int refuse(const char* who, const char* what, int status = CFLX_ERR_ARG) {
-    set_last_error("%s: refused, %s", who, what);
-    return status;
-}
-#define REFUSE_IF(cond) do { if (cond) return refuse(__func__, #cond); } while (0)
-
 // the conditions on a cflx_share_layout that differ between hooks (see the header)
 enum : unsigned { TILED = 1, COVERED = 2, NONEMPTY = 4 };
 

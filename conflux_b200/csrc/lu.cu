@@ -147,41 +147,40 @@ int handle_side_stream(Handle* h) {
     return h->side.create(cudaStreamNonBlocking, hi);
 }
 int handle_set_local(Handle* h, const double* host_local) {
-    CFLX_CUDA(cudaSetDevice(h->comm->device));
     cudaStream_t s = h->comm->stream;
     CFLX_CUDA(cudaMemcpyAsync(h->A0, host_local, (size_t)h->Ml * h->Nl * sizeof(double), cudaMemcpyHostToDevice, s));
     CFLX_CUDA(cudaStreamSynchronize(s));
     h->have_input = true;
     h->factored = false;
+    h->a0_is_next = false;
     h->sv.ready = false;
     h->eq.in.equed = 'N';
     return CFLX_OK;
 }
-int handle_check(const Handle* h, const char* what) {
-    if (h->factored) return CFLX_OK;
-    set_last_error(h->texts->unfactored, what);
-    return CFLX_ERR_STATE;
-}
-int handle_equil_begin(Handle* h, bool apply) {
-    if (!h->have_input) {
-        set_last_error("%s", h->texts->no_input);
-        return CFLX_ERR_STATE;
-    }
-    if (apply && h->eq.in.equed != 'N') {
-        set_last_error(h->texts->scaled, h->eq.in.equed);
+int enter(Handle* h, const char* who, unsigned need) {
+    const HandleTexts& t = *h->texts;
+    char why[256] = "";
+    if ((need & NEED_INPUT) && !h->have_input) snprintf(why, sizeof(why), "%s", t.no_input);
+    else if ((need & NEED_UNSCALED) && h->eq.in.equed != 'N') snprintf(why, sizeof(why), t.scaled, h->eq.in.equed);
+    else if ((need & NEED_FACTORS) && !h->factored) snprintf(why, sizeof(why), "%s", t.unfactored);
+    else if ((need & NEED_OWN_INPUT) && h->a0_is_next)
+        snprintf(why, sizeof(why), "refused: the input buffer of the last run was handed to the queued next matrix");
+    if (why[0]) {
+        set_last_error("%s: %s", who, why);
         return CFLX_ERR_STATE;
     }
     CFLX_CUDA(cudaSetDevice(h->comm->device));
+    return CFLX_OK;
+}
+void handle_equil_begin(Handle* h) {
     h->factored = false;
     h->sv.ready = false;
-    return CFLX_OK;
 }
 int handle_equil_end(Handle* h, bool apply, int info, char equed, double rowcnd, double colcnd, const double* c) {
     if (apply && info == 0) CFLX_TRY(equil_record_set(&h->eq.in, equed, rowcnd, colcnd, h->eq.qr, c, h->M, h->comm->stream));
     return CFLX_OK;
 }
 int handle_launch_count(Handle* h, int64_t* count_out, int reset) {
-    if (!h || !count_out) return CFLX_ERR_ARG;
     *count_out = h->launches;
     if (reset) h->launches = 0;
     return CFLX_OK;
@@ -602,13 +601,21 @@ int finish_step(cflx_lu* lu, int k, int& fnpr) {
 // layer 0 at rank p * Pz), the layers pk != 0 with zeros.
 SolveFactor lu_solve_factor(cflx_lu* lu) { return SolveFactor{*lu, lu->Cbuf, lu->Ml, &lu->jk_comm, &lu->ik_comm, lu->Pz}; }
 
+// *perm = the permutation of the last factorisation (M ints), in stream order
+int lu_permutation(cflx_lu* lu, std::vector<int>* perm) {
+    perm->resize(lu->M);
+    CFLX_CUDA(cudaMemcpyAsync(perm->data(), lu->hist, sizeof(int) * lu->M, cudaMemcpyDeviceToHost, lu->comm->stream));
+    CFLX_CUDA(cudaStreamSynchronize(lu->comm->stream));
+    return CFLX_OK;
+}
+
 // First call after a factorisation: the factors redistributed into Cbuf, the diagonal-block inverses, and on the ranks
 // that seed the right-hand side, the row of B that each local row of P*B comes from.
 int lu_solve_prepare(cflx_lu* lu) {
     cudaStream_t s = lu->comm->stream;
     const int v = lu->v, Px = lu->Px, Ml = lu->Ml;
-    std::vector<int> hist(lu->M);
-    CFLX_TRY(cflx_lu_get_permutation(lu, hist.data()));
+    std::vector<int> hist;
+    CFLX_TRY(lu_permutation(lu, &hist));
     if (lu->pk == 0) {
         lu->sv.inv.reset();  // before the redistribution allocates its staging
         if (!lu->Cbuf) CFLX_TRY(lu->Cbuf.alloc((size_t)Ml * lu->Nl));
@@ -636,8 +643,8 @@ int lu_solve_prepare(cflx_lu* lu) {
 int lu_solve_prepare_trans(cflx_lu* lu) {
     cudaStream_t s = lu->comm->stream;
     const int v = lu->v, Px = lu->Px, Py = lu->Py;
-    std::vector<int> hist(lu->M);
-    CFLX_TRY(cflx_lu_get_permutation(lu, hist.data()));
+    std::vector<int> hist;
+    CFLX_TRY(lu_permutation(lu, &hist));
     std::vector<int> unperm(lu->M);
     for (int q = 0; q < lu->M; ++q) unperm[hist[q]] = q;
     CFLX_TRY(solve_set_rows(&lu->sv.unperm, unperm, s));
@@ -683,20 +690,9 @@ int lu_sweeps(cflx_lu* lu, bool transposed, bool pa, int nrhs, const double* B, 
 }
 
 const HandleTexts kLuTexts = {
-    "%s requested before cflx_lu_factor, or after cflx_lu_set_local without a factorisation",
-    "equilibration requested before cflx_lu_set_local",
-    "equilibration refused: the input is already scaled (equed = '%c'); upload it again first"};
-
-// CFLX_OK when `what` may run: after a factorisation and, with own_input, while A0 still holds the input of that
-// factorisation; otherwise CFLX_ERR_STATE with the reason
-int lu_check(const cflx_lu* lu, const char* what, bool own_input) {
-    CFLX_TRY(handle_check(lu, what));
-    if (own_input && lu->a0_is_next) {
-        set_last_error("%s refused: the input buffer of the last run was handed to the queued next matrix", what);
-        return CFLX_ERR_STATE;
-    }
-    return CFLX_OK;
-}
+    "requested before cflx_lu_factor, or after cflx_lu_set_local without a factorisation",
+    "requested before cflx_lu_set_local",
+    "refused: the input is already scaled (equed = '%c'); upload it again first"};
 
 // LAPACK dgecon on the grid, NORM = '1' or (inf) 'I': the norm of the input A0 (the padded M x M matrix), and the
 // Hager-Higham estimate of ||inv(P A)||_1 = ||inv(A)||_1 from inv(U) inv(L) x and inv(L)^T inv(U)^T x, as dgecon runs it
@@ -724,16 +720,19 @@ RefineOp lu_refine_op(cflx_lu* lu, bool t) {
     return RefineOp{*lu, lu->A0, t ? ResidMode::TN : ResidMode::NN, false, solve};
 }
 
-// cflx_lu_equilibrate (dgeequ) and, with pow2, cflx_lu_equilibrate_b (dgeequb)
-int lu_equilibrate(cflx_lu* lu, int apply, bool pow2, double* r_out, double* c_out, double* rowcnd_out,
+// cflx_lu_equilibrate (dgeequ) and, with pow2, cflx_lu_equilibrate_b (dgeequb), as `who`
+int lu_equilibrate(const char* who, cflx_lu* lu, int apply, bool pow2, double* r_out, double* c_out, double* rowcnd_out,
                    double* colcnd_out, double* amax_out, char* equed_out, int* info_out) {
-    if (!lu || (apply != 0 && apply != 1) || !info_out) return CFLX_ERR_ARG;
+    REFUSE_FOR(who, !lu);
+    REFUSE_FOR(who, apply != 0 && apply != 1);
+    REFUSE_FOR(who, !info_out);
     if (apply && lu->rbt.in.depth) {
-        set_last_error("equilibration refused: the input carries a random butterfly transform (cflx_lu_rbt); upload it "
-                       "again first");
+        set_last_error("%s: refused, the input carries a random butterfly transform (cflx_lu_rbt); upload it again first",
+                       who);
         return CFLX_ERR_STATE;
     }
-    CFLX_TRY(handle_equil_begin(lu, apply != 0));
+    CFLX_TRY(enter(lu, who, NEED_INPUT | (apply ? NEED_UNSCALED : 0u)));
+    handle_equil_begin(lu);
     if (lu->a0_is_next) CFLX_CUDA(cudaStreamWaitEvent(lu->comm->stream, lu->ev_upload, 0));  // A0 holds a streamed next input
     double rowcnd = 0.0, colcnd = 0.0, amax = 0.0;
     char equed = 'N';
@@ -747,6 +746,62 @@ int lu_equilibrate(cflx_lu* lu, int apply, bool pow2, double* r_out, double* c_o
     *info_out = info;
     return CFLX_OK;
 }
+
+// cflx_lu_validate as `who`
+int lu_validate(const char* who, cflx_lu* lu, double* abs_out, double* rel_out) {
+    CFLX_TRY(enter(lu, who, NEED_FACTORS | NEED_OWN_INPUT));
+    std::vector<int> hist;
+    CFLX_TRY(lu_permutation(lu, &hist));
+    return lu_residual_grid(lu, hist, abs_out, rel_out);
+}
+
+// the visible CUDA devices (0 when the runtime finds none)
+int device_count() {
+    int n = 0;
+    if (cudaGetDeviceCount(&n) != cudaSuccess) {
+        n = 0;
+        cudaGetLastError();
+    }
+    return n;
+}
+
+// lu_params::get_p_grid (lu_params.hpp:21-47) for M, N, P >= 1
+void auto_grid(int M, int N, int P, int* Px, int* Py, int* Pz) {
+    const double ratio = 1.0 * std::max(M, N) / std::min(M, N);
+    const int p1 = (int)std::cbrt(P / ratio);
+    const int psq = (int)std::sqrt(P / ratio);
+    const int phs = (int)std::sqrt(P / (2 * ratio));
+    if (P == psq * psq) {
+        *Px = psq; *Py = psq; *Pz = 1;
+        return;
+    }
+    if (phs * phs == P / 2) {
+        *Px = phs; *Py = phs; *Pz = 2;
+        return;
+    }
+    int d[3] = {p1, (int)(ratio * p1), 0};
+    d[2] = P / (d[0] * d[1]);
+    std::sort(d, d + 3, [](int a, int b) { return a > b; });
+    *Px = d[0]; *Py = d[1]; *Pz = d[2];
+}
+
+// lu_params::initialize's sizes (lu_params.hpp:67-82) into o[8] (cflx_lu_dims), refused in the name of `who`
+int lu_dims(const char* who, int M, int N, int v, int Px, int Py, int Pz, int* o) {
+    REFUSE_FOR(who, M <= 0);
+    REFUSE_FOR(who, N <= 0);
+    REFUSE_FOR(who, v <= 0);
+    REFUSE_FOR(who, Px <= 0);
+    REFUSE_FOR(who, Py <= 0);
+    REFUSE_FOR(who, Pz <= 0);
+    const int tx = (int)std::ceil((double)M / (v * Px)), ty = (int)std::ceil((double)N / (v * Py));
+    const int Mp = v * Px * tx, Np = v * Py * ty;
+    const int Nt = (int)std::ceil((double)Np / v), Mt = (int)std::ceil((double)Mp / v);
+    o[0] = Mp; o[1] = Np;
+    o[2] = (int)std::ceil((double)Mt / Px) * v;
+    o[3] = (int)std::ceil((double)Nt / Py) * v;
+    o[4] = Nt; o[5] = (v + Pz - 1) / Pz; o[6] = Mt; o[7] = Px * Py * Pz;
+    return CFLX_OK;
+}
 }  // namespace
 
 // ======================================================================================================== C ABI
@@ -756,13 +811,7 @@ const char* cflx_last_error(void) { return g_err; }
 const char* cflx_version(void) { return "conflux_b200 0.1 (sm_90a)"; }
 
 int cflx_device_count(int* count) {
-    int n = 0;
-    cudaError_t e = cudaGetDeviceCount(&n);
-    if (e != cudaSuccess) {
-        n = 0;
-        cudaGetLastError();
-    }
-    *count = n;
+    *count = device_count();
     return CFLX_OK;
 }
 
@@ -775,15 +824,17 @@ int cflx_get_unique_id(void* id_out) {
 }
 
 int cflx_comm_create(int world_size, int world_rank, const void* unique_id, int device, cflx_comm** out) {
-    if (!out || world_size < 1 || world_rank < 0 || world_rank >= world_size) return CFLX_ERR_ARG;
-    int ndev = 0;
-    cflx_device_count(&ndev);
+    REFUSE_IF(!out);
+    REFUSE_IF(world_size < 1);
+    REFUSE_IF(world_rank < 0);
+    REFUSE_IF(world_rank >= world_size);
+    const int ndev = device_count();
     if (ndev == 0) {
-        set_last_error("no CUDA device visible: conflux_b200 has no CPU fallback");
+        set_last_error("%s: no CUDA device visible: conflux_b200 has no CPU fallback", __func__);
         return CFLX_ERR_NO_DEVICE;
     }
     if (device < 0 || device >= ndev) {
-        set_last_error("device %d out of range (%d visible)", device, ndev);
+        set_last_error("%s: device %d out of range (%d visible)", __func__, device, ndev);
         return CFLX_ERR_ARG;
     }
     CFLX_CUDA(cudaSetDevice(device));
@@ -795,10 +846,7 @@ int cflx_comm_create(int world_size, int world_rank, const void* unique_id, int 
     CFLX_TRY(c->d_scratch.alloc_exact(1));
     CFLX_CUDA(cudaMemset(c->d_scratch, 0, sizeof(double)));
     if (world_size > 1) {
-        if (!unique_id) {
-            set_last_error("unique_id required for world_size > 1");
-            return CFLX_ERR_ARG;
-        }
+        REFUSE_IF(!unique_id);
         ncclUniqueId id;
         std::memcpy(&id, unique_id, sizeof(id));
         CFLX_NCCL(ncclCommInitRank(&c->world, world_size, id, world_rank));
@@ -808,7 +856,7 @@ int cflx_comm_create(int world_size, int world_rank, const void* unique_id, int 
 }
 
 int cflx_comm_barrier(cflx_comm* c) {
-    if (!c) return CFLX_ERR_ARG;
+    REFUSE_IF(!c);
     CFLX_CUDA(cudaSetDevice(c->device));
     return grid_barrier(c);
 }
@@ -820,44 +868,26 @@ void cflx_comm_destroy(cflx_comm* c) {
     delete c;
 }
 
-int cflx_auto_grid(int M, int N, int P, int* Px, int* Py, int* Pz) {  // lu_params.hpp:21-47
-    if (M <= 0 || N <= 0 || P <= 0) return CFLX_ERR_ARG;
-    const double ratio = 1.0 * std::max(M, N) / std::min(M, N);
-    const int p1 = (int)std::cbrt(P / ratio);
-    const int psq = (int)std::sqrt(P / ratio);
-    const int phs = (int)std::sqrt(P / (2 * ratio));
-    if (P == psq * psq) {
-        *Px = psq; *Py = psq; *Pz = 1;
-        return CFLX_OK;
-    }
-    if (phs * phs == P / 2) {
-        *Px = phs; *Py = phs; *Pz = 2;
-        return CFLX_OK;
-    }
-    int d[3] = {p1, (int)(ratio * p1), 0};
-    d[2] = P / (d[0] * d[1]);
-    std::sort(d, d + 3, [](int a, int b) { return a > b; });
-    *Px = d[0]; *Py = d[1]; *Pz = d[2];
+int cflx_auto_grid(int M, int N, int P, int* Px, int* Py, int* Pz) {
+    REFUSE_IF(M <= 0);
+    REFUSE_IF(N <= 0);
+    REFUSE_IF(P <= 0);
+    auto_grid(M, N, P, Px, Py, Pz);
     return CFLX_OK;
 }
 
-int cflx_lu_dims(int M, int N, int v, int Px, int Py, int Pz, int* o) {  // lu_params.hpp:67-82
-    if (M <= 0 || N <= 0 || v <= 0 || Px <= 0 || Py <= 0 || Pz <= 0 || !o) return CFLX_ERR_ARG;
-    const int tx = (int)std::ceil((double)M / (v * Px)), ty = (int)std::ceil((double)N / (v * Py));
-    const int Mp = v * Px * tx, Np = v * Py * ty;
-    const int Nt = (int)std::ceil((double)Np / v), Mt = (int)std::ceil((double)Mp / v);
-    o[0] = Mp; o[1] = Np;
-    o[2] = (int)std::ceil((double)Mt / Px) * v;
-    o[3] = (int)std::ceil((double)Nt / Py) * v;
-    o[4] = Nt; o[5] = (v + Pz - 1) / Pz; o[6] = Mt; o[7] = Px * Py * Pz;
-    return CFLX_OK;
+int cflx_lu_dims(int M, int N, int v, int Px, int Py, int Pz, int* o) {
+    REFUSE_IF(!o);
+    return lu_dims(__func__, M, N, v, Px, Py, Pz, o);
 }
 
 int cflx_init_matrix_host(int M, int N, int v, int Px, int Py, int Pz, int rank, int seed, double* out) {
     int d[8];
-    CFLX_TRY(cflx_lu_dims(M, N, v, Px, Py, Pz, d));
+    CFLX_TRY(lu_dims(__func__, M, N, v, Px, Py, Pz, d));
     const int Ml = d[2], Nl = d[3];
-    if (rank < 0 || rank >= d[7] || !out) return CFLX_ERR_ARG;
+    REFUSE_IF(rank < 0);
+    REFUSE_IF(rank >= Px * Py * Pz);
+    REFUSE_IF(!out);
     std::fill(out, out + (size_t)Ml * Nl, 0.0);
     if (rank % Pz != 0) return CFLX_OK;  // layers pk != 0 start at zero (lu_params.hpp:149-155)
     // lu_params.hpp:157-363: for (padded) M == N in {8, 9, 16, 20, 27, 32} the reference fills a FIXED matrix,
@@ -884,28 +914,33 @@ int cflx_init_matrix_host(int M, int N, int v, int Px, int Py, int Pz, int rank,
 }
 
 int cflx_lu_create(cflx_comm* c, int M, int N, int v, int Px, int Py, int Pz, cflx_lu** out) {
-    if (!c || !out || M <= 0 || N <= 0 || v <= 0) return CFLX_ERR_ARG;
+    REFUSE_IF(!c);
+    REFUSE_IF(!out);
+    REFUSE_IF(M <= 0);
+    REFUSE_IF(N <= 0);
+    REFUSE_IF(v <= 0);
     CFLX_CUDA(cudaSetDevice(c->device));
-    if (Px <= 0 || Py <= 0 || Pz <= 0) CFLX_TRY(cflx_auto_grid(M, N, c->world_size, &Px, &Py, &Pz));
+    if (Px <= 0 || Py <= 0 || Pz <= 0) auto_grid(M, N, c->world_size, &Px, &Py, &Pz);
     if (Px != Py) {
-        set_last_error("grid %dx%dx%d: the CONFLUX LU path requires Px == Py (SURVEY.md fact 6)", Px, Py, Pz);
+        set_last_error("%s: grid %dx%dx%d: the CONFLUX LU path requires Px == Py (SURVEY.md fact 6)", __func__, Px, Py, Pz);
         return CFLX_ERR_UNSUPPORTED;
     }
     if (Px * Py * Pz != c->world_size) {
-        set_last_error("grid %dx%dx%d does not match the %d ranks of the communicator", Px, Py, Pz, c->world_size);
+        set_last_error("%s: grid %dx%dx%d does not match the %d ranks of the communicator", __func__, Px, Py, Pz,
+                       c->world_size);
         return CFLX_ERR_ARG;
     }
     if (v % 4 != 0 || v % Pz != 0 || (v / Pz) % 4 != 0 || pick_nb(v) == 0) {
-        set_last_error("tile size v=%d unsupported: need v %% 4 == 0 and (v / Pz) %% 4 == 0", v);
+        set_last_error("%s: tile size v=%d unsupported: need v %% 4 == 0 and (v / Pz) %% 4 == 0", __func__, v);
         return CFLX_ERR_UNSUPPORTED;
     }
     int d[8];
-    CFLX_TRY(cflx_lu_dims(M, N, v, Px, Py, Pz, d));
+    CFLX_TRY(lu_dims(__func__, M, N, v, Px, Py, Pz, d));
     if (d[0] != d[1]) {
-        set_last_error("only square matrices are supported (the miniapp passes M = N)");
+        set_last_error("%s: only square matrices are supported (the miniapp passes M = N)", __func__);
         return CFLX_ERR_UNSUPPORTED;
     }
-    std::unique_ptr<cflx_lu, void (*)(cflx_lu*)> lu(new cflx_lu, cflx_lu_destroy);
+    std::unique_ptr<cflx_lu> lu(new cflx_lu);
     lu->M = d[0]; lu->N = d[1]; lu->Ml = d[2]; lu->Nl = d[3]; lu->Nt = d[4]; lu->nlayr = d[5]; lu->Mt = d[6];
     lu->v = v;
     lu->nb = pick_nb(v);
@@ -939,7 +974,6 @@ int cflx_lu_create(cflx_comm* c, int M, int N, int v, int Px, int Py, int Pz, cf
     CFLX_TRY(lu->ev_npiv.create(cudaEventDisableTiming));
     CFLX_TRY(panel_workspace_create(&lu->pws));
     CFLX_TRY(handle_update_setup(lu.get()));
-    lu->h_hist.assign(lu->M, -1);
     {
         // look-ahead: pivot search of iteration k+1 (extract, layer reduce, local search, tournament exchanges) on a
         // high-priority side stream, on a capped number of SMs, while the trailing update of iteration k runs on the
@@ -966,13 +1000,14 @@ int cflx_lu_create(cflx_comm* c, int M, int N, int v, int Px, int Py, int Pz, cf
     cudaMemsetAsync(lu->A01raw, 0, upan * sizeof(double), c->stream);
     cudaMemsetAsync(lu->U, 0, upan * sizeof(double), c->stream);
     cudaMemsetAsync(lu->A0, 0, (size_t)lu->Ml * lu->Nl * sizeof(double), c->stream);
-    if (cudaStreamSynchronize(c->stream) != cudaSuccess) return CFLX_ERR_CUDA;
+    CFLX_CUDA(cudaStreamSynchronize(c->stream));
     *out = lu.release();
     return CFLX_OK;
 }
 
 int cflx_lu_info(const cflx_lu* lu, int* o) {
-    if (!lu || !o) return CFLX_ERR_ARG;
+    REFUSE_IF(!lu);
+    REFUSE_IF(!o);
     const int vals[16] = {lu->M, lu->N, lu->Ml, lu->Nl, lu->Nt, lu->nlayr, lu->P, lu->Px, lu->Py, lu->Pz, lu->pi, lu->pj,
                           lu->pk, lu->rank, lu->v, 0};
     std::memcpy(o, vals, sizeof(vals));
@@ -980,10 +1015,11 @@ int cflx_lu_info(const cflx_lu* lu, int* o) {
 }
 
 int cflx_lu_set_local(cflx_lu* lu, const double* host_local) {
-    if (!lu || !host_local) return CFLX_ERR_ARG;
+    REFUSE_IF(!lu);
+    REFUSE_IF(!host_local);
+    CFLX_TRY(enter(lu, __func__, 0));
     CFLX_TRY(handle_set_local(lu, host_local));
     lu->rbt.in.depth = 0;
-    lu->a0_is_next = false;
     lu->next_host = nullptr;
     return CFLX_OK;
 }
@@ -993,12 +1029,9 @@ int cflx_lu_set_local(cflx_lu* lu, const double* host_local) {
 // the current input, so the 8*Ml*Nl-byte transfer overlaps the factorisation; the factorisation after that consumes it
 // without a cflx_lu_set_local.  The residual of a run whose input buffer was handed to the next matrix is refused.
 int cflx_lu_queue_next_local(cflx_lu* lu, const double* host_next) {
-    if (!lu || !host_next) return CFLX_ERR_ARG;
-    if (!lu->have_input) {
-        set_last_error("cflx_lu_queue_next_local needs a current input (cflx_lu_set_local) first");
-        return CFLX_ERR_STATE;
-    }
-    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    REFUSE_IF(!lu);
+    REFUSE_IF(!host_next);
+    CFLX_TRY(enter(lu, __func__, NEED_INPUT));
     if (!lu->copy) {
         CFLX_TRY(lu->copy.create(cudaStreamNonBlocking));
         CFLX_TRY(lu->ev_a0_read.create(cudaEventDisableTiming));
@@ -1136,35 +1169,28 @@ int world_agree(cflx_lu* lu, bool ok, std::initializer_list<unsigned long long> 
     return CFLX_OK;
 }
 
-// The checks of cflx_lu_factor_fixed that need no other rank; on success lu->fix_perm_h holds the order and the
+// The checks of cflx_lu_factor_fixed (`who`) that need no other rank; on success lu->fix_perm_h holds the order and the
 // device buffers of the fixed path exist
-int fixed_prepare(cflx_lu* lu, const int* perm, double tiny, const int* info_out) {
-    if (!(tiny >= 0.0) || !info_out) {
-        set_last_error("cflx_lu_factor_fixed: tiny must be >= 0 and info_out not NULL");
-        return CFLX_ERR_ARG;
-    }
-    if (!lu->have_input) {
-        set_last_error("cflx_lu_factor_fixed before cflx_lu_set_local");
-        return CFLX_ERR_STATE;
-    }
+int fixed_prepare(const char* who, cflx_lu* lu, const int* perm, double tiny, const int* info_out) {
+    REFUSE_FOR(who, !(tiny >= 0.0));
+    REFUSE_FOR(who, !info_out);
+    CFLX_TRY(enter(lu, who, NEED_INPUT));
     const int M = lu->M;
     std::vector<int>& p = lu->fix_perm_h;
     if (perm) {
         p.assign(perm, perm + M);
     } else {
         if (!lu->perm_done) {
-            set_last_error("cflx_lu_factor_fixed with perm = NULL before any factorisation of this handle completed");
+            set_last_error("%s: perm = NULL before any factorisation of this handle completed", who);
             return CFLX_ERR_STATE;
         }
-        // stream-ordered like every reader of hist (cflx_lu_get_permutation refuses after set_local, which keeps hist)
-        p.resize(M);
-        CFLX_CUDA(cudaMemcpyAsync(p.data(), lu->hist, sizeof(int) * M, cudaMemcpyDeviceToHost, lu->comm->stream));
-        CFLX_CUDA(cudaStreamSynchronize(lu->comm->stream));
+        // the permutation of the last factorisation, which set_local keeps
+        CFLX_TRY(lu_permutation(lu, &p));
     }
     std::vector<char> seen(M, 0);
     for (int x : p) {
         if (x < 0 || x >= M || seen[x]) {
-            set_last_error("cflx_lu_factor_fixed: perm is not a permutation of [0, %d)", M);
+            set_last_error("%s: perm is not a permutation of [0, %d)", who, M);
             return CFLX_ERR_ARG;
         }
         seen[x] = 1;
@@ -1176,28 +1202,19 @@ int fixed_prepare(cflx_lu* lu, const int* perm, double tiny, const int* info_out
     return CFLX_OK;
 }
 
-// The checks of cflx_lu_rbt that need no other rank
-int rbt_prepare(cflx_lu* lu, int depth) {
-    if (depth < 1 || depth > 4) {
-        set_last_error("cflx_lu_rbt: depth must be in [1, 4], got %d", depth);
-        return CFLX_ERR_ARG;
-    }
-    if (!lu->have_input) {
-        set_last_error("cflx_lu_rbt before cflx_lu_set_local");
-        return CFLX_ERR_STATE;
-    }
+// The checks of cflx_lu_rbt (`who`) that need no other rank
+int rbt_prepare(const char* who, cflx_lu* lu, int depth) {
+    REFUSE_FOR(who, depth < 1);
+    REFUSE_FOR(who, depth > 4);
     if (lu->rbt.in.depth) {
-        set_last_error("cflx_lu_rbt refused: the input is already transformed; upload it again first");
+        set_last_error("%s: refused, the input is already transformed; upload it again first", who);
         return CFLX_ERR_STATE;
     }
-    if (lu->eq.in.equed != 'N') {
-        set_last_error("cflx_lu_rbt refused: the input is scaled (equed = '%c'); upload it again first", lu->eq.in.equed);
-        return CFLX_ERR_STATE;
-    }
+    CFLX_TRY(enter(lu, who, NEED_INPUT | NEED_UNSCALED));
     const long long q = (long long)lu->v * lu->Px << depth;
     if (lu->M % q) {
-        set_last_error("cflx_lu_rbt: M = %d is not a multiple of 2^%d v Px = %lld; the smallest M that works is %lld: "
-                       "pad A with the identity to that order", lu->M, depth, q, (lu->M + q - 1) / q * q);
+        set_last_error("%s: M = %d is not a multiple of 2^%d v Px = %lld; the smallest M that works is %lld: "
+                       "pad A with the identity to that order", who, lu->M, depth, q, (lu->M + q - 1) / q * q);
         return CFLX_ERR_UNSUPPORTED;
     }
     return CFLX_OK;
@@ -1217,12 +1234,8 @@ RowTransform rbt_rows(cflx_lu* lu, RbtOp op) {
 extern "C" {
 
 int cflx_lu_factor(cflx_lu* lu, double* ms_out) {
-    if (!lu) return CFLX_ERR_ARG;
-    if (!lu->have_input) {
-        set_last_error("cflx_lu_factor before cflx_lu_set_local");
-        return CFLX_ERR_STATE;
-    }
-    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    REFUSE_IF(!lu);
+    CFLX_TRY(enter(lu, __func__, NEED_INPUT));
     return lu_factor_run(lu, ms_out);
 }
 
@@ -1231,16 +1244,16 @@ int cflx_lu_factor(cflx_lu* lu, double* ms_out) {
 // factorisation with fixed_panel in place of the pivot search, then the replacements (sum) and the first zero pivot (min)
 // combined over the world.
 int cflx_lu_factor_fixed(cflx_lu* lu, const int* perm, double tiny, int* nrepl_out, int* info_out, double* ms_out) {
-    if (!lu) return CFLX_ERR_ARG;
-    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    REFUSE_IF(!lu);
+    CFLX_TRY(enter(lu, __func__, 0));  // the device of world_agree, whatever fixed_prepare finds
     cflx_comm* c = lu->comm;
     cudaStream_t s = c->stream;
-    const int rc = fixed_prepare(lu, perm, tiny, info_out);
+    const int rc = fixed_prepare(__func__, lu, perm, tiny, info_out);
     bool same = false;
     CFLX_TRY(world_agree(lu, rc == CFLX_OK, {rc == CFLX_OK ? order_hash(lu->fix_perm_h) : 0}, &same));
     if (rc != CFLX_OK) return rc;
     if (!same) {
-        set_last_error("cflx_lu_factor_fixed: the ranks passed different orders, or another rank refused its arguments");
+        set_last_error("%s: the ranks passed different orders, or another rank refused its arguments", __func__);
         return CFLX_ERR_ARG;
     }
     const int v = lu->v, Px = lu->Px;
@@ -1275,14 +1288,14 @@ int cflx_lu_factor_fixed(cflx_lu* lu, const int* perm, double tiny, int* nrepl_o
 // all-reduce, so that a refusal anywhere is a refusal everywhere.  The input changes: the factors and the solve cache
 // are dropped, as by an equilibration that scales the input.
 int cflx_lu_rbt(cflx_lu* lu, int depth, uint64_t seed, double* u_out, double* v_out) {
-    if (!lu) return CFLX_ERR_ARG;
-    CFLX_CUDA(cudaSetDevice(lu->comm->device));
-    const int rc = rbt_prepare(lu, depth);
+    REFUSE_IF(!lu);
+    CFLX_TRY(enter(lu, __func__, 0));  // the device of world_agree, whatever rbt_prepare finds
+    const int rc = rbt_prepare(__func__, lu, depth);
     bool same = false;
     CFLX_TRY(world_agree(lu, rc == CFLX_OK, {seed, (unsigned long long)depth}, &same));
     if (rc != CFLX_OK) return rc;
     if (!same) {
-        set_last_error("cflx_lu_rbt: the ranks passed different depths or seeds, or another rank refused its arguments");
+        set_last_error("%s: the ranks passed different depths or seeds, or another rank refused its arguments", __func__);
         return CFLX_ERR_ARG;
     }
     const int M = lu->M;
@@ -1309,16 +1322,16 @@ int cflx_lu_rbt(cflx_lu* lu, int depth, uint64_t seed, double* u_out, double* v_
 // row transforms.
 int cflx_lu_rbt_solve(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, double* X, int ldx, int refine,
                       double* ferr_out, double* berr_out) {
-    if (!lu || (trans != 0 && trans != 1) || (refine != 0 && refine != 1) || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B ||
-        !X)
-        return CFLX_ERR_ARG;
-    CFLX_TRY(lu_check(lu, "RBT solve", refine != 0));
+    REFUSE_IF(!lu);
+    REFUSE_IF(trans != 0 && trans != 1);
+    REFUSE_IF(refine != 0 && refine != 1);
+    CFLX_TRY(rhs_args(__func__, nrhs, B, ldb, X, ldx, true));
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | (refine ? NEED_OWN_INPUT : 0u)));
     if (!lu->rbt.fac.depth) {
-        set_last_error("cflx_lu_rbt_solve: the factors carry no random butterfly transform (cflx_lu_rbt before the "
-                       "factorisation)");
+        set_last_error("%s: the factors carry no random butterfly transform (cflx_lu_rbt before the factorisation)",
+                       __func__);
         return CFLX_ERR_STATE;
     }
-    CFLX_CUDA(cudaSetDevice(lu->comm->device));
     const bool t = trans != 0;
     const RefineOp op = lu_refine_op(lu, t);
     auto refine_step = [&](const double* dB, int lb, double* dX, int lx) {
@@ -1331,19 +1344,22 @@ int cflx_lu_rbt_solve(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb
 // Not collective.  One of the factors' butterflies on the rows of this rank's right-hand side share (rbt.cu); a host
 // share goes through one temporary device share.
 int cflx_lu_rbt_apply_local(cflx_lu* lu, int op, int nrhs, double* B_local, int ldb) {
-    if (!lu || op < 0 || op > 3 || nrhs < 1 || !B_local) return CFLX_ERR_ARG;
+    REFUSE_IF(!lu);
+    REFUSE_IF(op < 0);
+    REFUSE_IF(op > 3);
+    REFUSE_IF(nrhs < 1);
+    REFUSE_IF(!B_local);
     const int ncl = rhs_local_cols(nrhs, lu->v, lu->Py);
-    if (ldb < ncl) return CFLX_ERR_ARG;
-    CFLX_TRY(lu_check(lu, "RBT apply", false));
+    REFUSE_IF(ldb < ncl);
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS));
     const RbtRecord& f = lu->rbt.fac;
     if (!f.depth) {
-        set_last_error("cflx_lu_rbt_apply_local: the factors carry no random butterfly transform (cflx_lu_rbt before "
-                       "the factorisation)");
+        set_last_error("%s: the factors carry no random butterfly transform (cflx_lu_rbt before the factorisation)",
+                       __func__);
         return CFLX_ERR_STATE;
     }
-    CFLX_CUDA(cudaSetDevice(lu->comm->device));
     bool dev = false;
-    CFLX_TRY(share_kind(*lu, B_local, "B_local", &dev));
+    CFLX_TRY(share_kind(__func__, *lu, B_local, "B_local", &dev));
     cudaStream_t s = lu->comm->stream;
     const size_t row = sizeof(double) * ncl;
     DevBuf<double> tmp;
@@ -1362,12 +1378,12 @@ int cflx_lu_rbt_apply_local(cflx_lu* lu, int op, int nrhs, double* B_local, int 
 }
 
 int cflx_lu_get_permutation(cflx_lu* lu, int* perm_out) {
-    if (!lu || !perm_out) return CFLX_ERR_ARG;
-    CFLX_TRY(lu_check(lu, "permutation", false));
-    CFLX_CUDA(cudaSetDevice(lu->comm->device));
-    CFLX_CUDA(cudaMemcpyAsync(lu->h_hist.data(), lu->hist, sizeof(int) * lu->M, cudaMemcpyDeviceToHost, lu->comm->stream));
-    CFLX_CUDA(cudaStreamSynchronize(lu->comm->stream));
-    std::memcpy(perm_out, lu->h_hist.data(), sizeof(int) * lu->M);
+    REFUSE_IF(!lu);
+    REFUSE_IF(!perm_out);
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS));
+    std::vector<int> hist;
+    CFLX_TRY(lu_permutation(lu, &hist));
+    std::memcpy(perm_out, hist.data(), sizeof(int) * lu->M);
     return CFLX_OK;
 }
 
@@ -1375,13 +1391,11 @@ int cflx_lu_get_permutation(cflx_lu* lu, int* perm_out) {
 // promoted).  The reference's validation layout wants pivoted row q = k*v + i on rank (k % Px, pj, 0) at local
 // row (k / Px)*v + i (conflux_opt.hpp:1673-1699,1721-1754): an all-to-all of whole rows inside each grid column.
 int cflx_lu_get_factors(cflx_lu* lu, double* C_host, int* perm_out) {
-    if (!lu) return CFLX_ERR_ARG;
-    CFLX_TRY(lu_check(lu, "factors", false));
-    cflx_comm* c = lu->comm;
-    cudaStream_t s = c->stream;
-    CFLX_CUDA(cudaSetDevice(c->device));
-    std::vector<int> hist(lu->M);
-    CFLX_TRY(cflx_lu_get_permutation(lu, hist.data()));
+    REFUSE_IF(!lu);
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS));
+    cudaStream_t s = lu->comm->stream;
+    std::vector<int> hist;
+    CFLX_TRY(lu_permutation(lu, &hist));
     if (perm_out) std::memcpy(perm_out, hist.data(), sizeof(int) * lu->M);
     if (lu->pk != 0) return CFLX_OK;  // only layer 0 holds factors
     const size_t loc = (size_t)lu->Ml * lu->Nl;
@@ -1395,42 +1409,39 @@ int cflx_lu_get_factors(cflx_lu* lu, double* C_host, int* perm_out) {
 // ||P A - L U||_F (absolute, what the reference's validation build prints, conflux_miniapp.cpp:494-500) and the same
 // relative to ||A||_F, computed on the device grid with the library's own GEMM + NCCL (validate.cu).  COLLECTIVE.
 int cflx_lu_validate(cflx_lu* lu, double* frob_abs_out, double* frob_rel_out) {
-    if (!lu) return CFLX_ERR_ARG;
-    CFLX_TRY(lu_check(lu, "residual", true));
-    CFLX_CUDA(cudaSetDevice(lu->comm->device));
-    std::vector<int> hist(lu->M);
-    CFLX_TRY(cflx_lu_get_permutation(lu, hist.data()));
-    return lu_residual_grid(lu, hist, frob_abs_out, frob_rel_out);
+    REFUSE_IF(!lu);
+    return lu_validate(__func__, lu, frob_abs_out, frob_rel_out);
 }
 int cflx_lu_residual(cflx_lu* lu, double* rel_out) {
-    if (!rel_out) return CFLX_ERR_ARG;
-    return cflx_lu_validate(lu, nullptr, rel_out);
+    REFUSE_IF(!lu);
+    REFUSE_IF(!rel_out);
+    return lu_validate(__func__, lu, nullptr, rel_out);
 }
 
 // Reads only the factors, so a run whose input buffer was handed to the queued next matrix can still be solved.
 int cflx_lu_solve(cflx_lu* lu, int nrhs, const double* B, int ldb, double* X, int ldx) {
-    if (!lu || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B) return CFLX_ERR_ARG;
-    CFLX_TRY(lu_check(lu, "solve", false));
-    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    REFUSE_IF(!lu);
+    CFLX_TRY(rhs_args(__func__, nrhs, B, ldb, X, ldx, false));
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS));
     return lu_sweeps(lu, false, false, nrhs, B, ldb, X, ldx);
 }
 
 // A^T X = B with the same factors and state rules: U^T Y = B, L^T W = Y by column-partial sweeps, then X = P^T W.
 int cflx_lu_solve_trans(cflx_lu* lu, int nrhs, const double* B, int ldb, double* X, int ldx) {
-    if (!lu || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B) return CFLX_ERR_ARG;
-    CFLX_TRY(lu_check(lu, "transposed solve", false));
-    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    REFUSE_IF(!lu);
+    CFLX_TRY(rhs_args(__func__, nrhs, B, ldb, X, ldx, false));
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS));
     return lu_sweeps(lu, true, false, nrhs, B, ldb, X, ldx);
 }
 
 // COLLECTIVE.  A X = B or A^T X = B with B and X distributed like A (solve_local.cu): each block of columns assembled on
 // the device and solved by the sweeps of cflx_lu_solve / cflx_lu_solve_trans, then scattered into X's share.
 int cflx_lu_solve_local(cflx_lu* lu, int trans, int nrhs, const double* B_local, int ldb, double* X_local, int ldx) {
-    if (!lu || (trans != 0 && trans != 1)) return CFLX_ERR_ARG;
+    REFUSE_IF(!lu);
+    REFUSE_IF(trans != 0 && trans != 1);
     SolveLocalArgs a{};
-    CFLX_TRY(solve_local_args(*lu, nrhs, B_local, ldb, X_local, ldx, &a));
-    CFLX_TRY(lu_check(lu, trans ? "transposed solve" : "solve", false));
-    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    CFLX_TRY(solve_local_args(__func__, *lu, nrhs, B_local, ldb, X_local, ldx, &a));
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS));
     auto solve = [lu, trans](int w, const double* Bk, int ldn, const double** Xk) -> int {
         CFLX_TRY(lu_sweeps(lu, trans != 0, false, w, Bk, ldn, nullptr, 0));
         *Xk = trans ? lu->sv.Xg : lu->sv.X;  // the transposed solve's P^T lands in Xg
@@ -1441,9 +1452,9 @@ int cflx_lu_solve_local(cflx_lu* lu, int trans, int nrhs, const double* B_local,
 
 // LAPACK dgecon (NORM = '1') on the grid (lu_rcond).
 int cflx_lu_rcond(cflx_lu* lu, double* rcond_out, double* anorm_out) {
-    if (!lu || !rcond_out) return CFLX_ERR_ARG;
-    CFLX_TRY(lu_check(lu, "condition estimate", true));
-    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    REFUSE_IF(!lu);
+    REFUSE_IF(!rcond_out);
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_OWN_INPUT));
     return lu_rcond(lu, false, rcond_out, anorm_out);
 }
 
@@ -1451,9 +1462,9 @@ int cflx_lu_rcond(cflx_lu* lu, double* rcond_out, double* anorm_out) {
 // solves with the identity, each block column q of inv(P A) landing in column perm[q] of this rank's share.  Reads only
 // the factors and the permutation, like cflx_lu_solve.
 int cflx_lu_inverse(cflx_lu* lu, double* Ainv_local, int* info_out) {
-    if (!lu || !info_out) return CFLX_ERR_ARG;
-    CFLX_TRY(lu_check(lu, "inverse", false));
-    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    REFUSE_IF(!lu);
+    REFUSE_IF(!info_out);
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS));
     if (!lu->sv.ready) CFLX_TRY(lu_solve_prepare(lu));
     int info = 0;
     CFLX_TRY(zero_pivot_grid(*lu, &lu->eq, lu->Cbuf, &info));
@@ -1466,17 +1477,18 @@ int cflx_lu_inverse(cflx_lu* lu, double* Ainv_local, int* info_out) {
 // products of the scales when unscaled; det(P) from the cycles of the permutation, the same on every rank.
 int cflx_lu_det(cflx_lu* lu, int unscaled, double* sign_out, double* logabsdet_out, double* mant_out, int64_t* exp_out,
                 int* info_out) {
-    if (!lu || (unscaled != 0 && unscaled != 1) || !info_out) return CFLX_ERR_ARG;
-    CFLX_TRY(lu_check(lu, "determinant", false));
-    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    REFUSE_IF(!lu);
+    REFUSE_IF(unscaled != 0 && unscaled != 1);
+    REFUSE_IF(!info_out);
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS));
     if (!lu->sv.ready) CFLX_TRY(lu_solve_prepare(lu));
     const EquilRecord& eq = lu->eq.fac;
     const double* r = unscaled && (eq.equed == 'R' || eq.equed == 'B') ? eq.r.p : nullptr;
     const double* c = unscaled && (eq.equed == 'C' || eq.equed == 'B') ? eq.c.p : nullptr;
     DetResult d{};
     CFLX_TRY(det_grid(*lu, &lu->eq, lu->Cbuf, false, r, c, &d));
-    std::vector<int> perm(lu->M);
-    CFLX_TRY(cflx_lu_get_permutation(lu, perm.data()));
+    std::vector<int> perm;
+    CFLX_TRY(lu_permutation(lu, &perm));
     // det(P) = (-1)^(M - number of cycles): a cycle of length L is L - 1 transpositions
     std::vector<char> seen(lu->M, 0);
     int odd = d.neg;
@@ -1498,9 +1510,10 @@ int cflx_lu_det(cflx_lu* lu, int unscaled, double* sign_out, double* logabsdet_o
 // estimator's products by the solves above (lu_refine_op).
 int cflx_lu_refine(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, double* X, int ldx, double* ferr_out,
                    double* berr_out) {
-    if (!lu || (trans != 0 && trans != 1) || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B || !X) return CFLX_ERR_ARG;
-    CFLX_TRY(lu_check(lu, "refinement", true));
-    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    REFUSE_IF(!lu);
+    REFUSE_IF(trans != 0 && trans != 1);
+    CFLX_TRY(rhs_args(__func__, nrhs, B, ldb, X, ldx, true));
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_OWN_INPUT));
     return refine_run(&lu->sv.rf, lu_refine_op(lu, trans != 0), nrhs, B, ldb, X, ldx, ferr_out, berr_out);
 }
 
@@ -1509,11 +1522,12 @@ int cflx_lu_refine(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, d
 // trans 1 (equed R / B).
 int cflx_lu_refine_x(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out,
                      double* berr_out, double* err_bnds_norm_out, double* err_bnds_comp_out, int* info_out) {
-    if (!lu || (trans != 0 && trans != 1) || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B || !X || !err_bnds_norm_out ||
-        !info_out)
-        return CFLX_ERR_ARG;
-    CFLX_TRY(lu_check(lu, "extra-precise refinement", true));
-    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    REFUSE_IF(!lu);
+    REFUSE_IF(trans != 0 && trans != 1);
+    CFLX_TRY(rhs_args(__func__, nrhs, B, ldb, X, ldx, true));
+    REFUSE_IF(!err_bnds_norm_out);
+    REFUSE_IF(!info_out);
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_OWN_INPUT));
     const bool t = trans != 0;
     if (!lu->sv.ready) CFLX_TRY(lu_solve_prepare(lu));
     int info = 0;
@@ -1538,13 +1552,13 @@ int cflx_lu_refine_x(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb,
 // and the solve cache are dropped, as by cflx_lu_set_local.
 int cflx_lu_equilibrate(cflx_lu* lu, int apply, double* r_out, double* c_out, double* rowcnd_out, double* colcnd_out,
                         double* amax_out, char* equed_out, int* info_out) {
-    return lu_equilibrate(lu, apply, false, r_out, c_out, rowcnd_out, colcnd_out, amax_out, equed_out, info_out);
+    return lu_equilibrate(__func__, lu, apply, false, r_out, c_out, rowcnd_out, colcnd_out, amax_out, equed_out, info_out);
 }
 
 // COLLECTIVE.  LAPACK dgeequb (+ dlaqge when apply): cflx_lu_equilibrate with the scales rounded to powers of two.
 int cflx_lu_equilibrate_b(cflx_lu* lu, int apply, double* r_out, double* c_out, double* rowcnd_out, double* colcnd_out,
                           double* amax_out, char* equed_out, int* info_out) {
-    return lu_equilibrate(lu, apply, true, r_out, c_out, rowcnd_out, colcnd_out, amax_out, equed_out, info_out);
+    return lu_equilibrate(__func__, lu, apply, true, r_out, c_out, rowcnd_out, colcnd_out, amax_out, equed_out, info_out);
 }
 
 // COLLECTIVE.  LAPACK dgesvxx after the factorisation, with the scaling the factors carry: the first zero pivot and
@@ -1552,11 +1566,13 @@ int cflx_lu_equilibrate_b(cflx_lu* lu, int apply, double* r_out, double* c_out, 
 int cflx_lu_svxx(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out,
                  double* rpvgrw_out, double* berr_out, double* err_bnds_norm_out, double* err_bnds_comp_out,
                  char* equed_out, int* info_out) {
-    if (!lu || (trans != 0 && trans != 1) || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B || !X || !rcond_out ||
-        !err_bnds_norm_out || !info_out)
-        return CFLX_ERR_ARG;
-    CFLX_TRY(lu_check(lu, "extra-precise expert solve", true));
-    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    REFUSE_IF(!lu);
+    REFUSE_IF(trans != 0 && trans != 1);
+    CFLX_TRY(rhs_args(__func__, nrhs, B, ldb, X, ldx, true));
+    REFUSE_IF(!rcond_out);
+    REFUSE_IF(!err_bnds_norm_out);
+    REFUSE_IF(!info_out);
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_OWN_INPUT));
     const bool t = trans != 0;
     const EquilRecord& eq = lu->eq.fac;
     const bool rowequ = eq.equed == 'R' || eq.equed == 'B', colequ = eq.equed == 'C' || eq.equed == 'B';
@@ -1585,10 +1601,12 @@ int cflx_lu_svxx(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, dou
 // growth and the first zero pivot, rcond (1-norm for trans 0, infinity-norm for trans 1), the solve, dgerfs, X unscaled.
 int cflx_lu_svx(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out,
                 double* ferr_out, double* berr_out, double* rpvgrw_out, char* equed_out, int* info_out) {
-    if (!lu || (trans != 0 && trans != 1) || nrhs < 1 || ldb < nrhs || ldx < nrhs || !B || !X || !rcond_out || !info_out)
-        return CFLX_ERR_ARG;
-    CFLX_TRY(lu_check(lu, "expert solve", true));
-    CFLX_CUDA(cudaSetDevice(lu->comm->device));
+    REFUSE_IF(!lu);
+    REFUSE_IF(trans != 0 && trans != 1);
+    CFLX_TRY(rhs_args(__func__, nrhs, B, ldb, X, ldx, true));
+    REFUSE_IF(!rcond_out);
+    REFUSE_IF(!info_out);
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_OWN_INPUT));
     const bool t = trans != 0;
     const EquilRecord& eq = lu->eq.fac;
     const bool rowequ = eq.equed == 'R' || eq.equed == 'B', colequ = eq.equed == 'C' || eq.equed == 'B';
@@ -1614,11 +1632,9 @@ int cflx_lu_svx(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, doub
 }
 
 int cflx_host_alloc(size_t bytes, void** out) {
-    if (!out) return CFLX_ERR_ARG;
-    int n = 0;
-    cflx_device_count(&n);
-    if (n == 0) {
-        set_last_error("no CUDA device visible: conflux_b200 has no CPU fallback");
+    REFUSE_IF(!out);
+    if (device_count() == 0) {
+        set_last_error("%s: no CUDA device visible: conflux_b200 has no CPU fallback", __func__);
         return CFLX_ERR_NO_DEVICE;
     }
     CFLX_CUDA(cudaHostAlloc(out, bytes, cudaHostAllocPortable));
@@ -1630,9 +1646,15 @@ int cflx_host_free(void* p) {
 }
 
 int cflx_lu_uses_ozaki(const cflx_lu* lu) { return lu && lu->use_ozaki ? 1 : 0; }
-int cflx_lu_launch_count(cflx_lu* lu, int64_t* count_out, int reset) { return handle_launch_count(lu, count_out, reset); }
+int cflx_lu_launch_count(cflx_lu* lu, int64_t* count_out, int reset) {
+    REFUSE_IF(!lu);
+    REFUSE_IF(!count_out);
+    return handle_launch_count(lu, count_out, reset);
+}
 int cflx_lu_set_profiling(cflx_lu* lu, int mode) {  // 0 off, 1 serialising phase timers, 2 non-serialising timeline
-    if (!lu || mode < 0 || mode > 2) return CFLX_ERR_ARG;
+    REFUSE_IF(!lu);
+    REFUSE_IF(mode < 0);
+    REFUSE_IF(mode > 2);
     lu->prof_mode = mode;
     return CFLX_OK;
 }
@@ -1641,7 +1663,7 @@ int cflx_lu_set_profiling(cflx_lu* lu, int mode) {  // 0 off, 1 serialising phas
 // only) lists every region instance in launch order, start relative to the first recorded event.  Returns the length
 // needed (incl. the terminator) when buf is too small.
 int cflx_lu_timeline(cflx_lu* lu, char* buf, int buf_len) {
-    if (!lu) return CFLX_ERR_ARG;
+    REFUSE_IF(!lu);
     std::string o = "{";
     for (int sd = 0; sd < 2; ++sd) {
         o += sd ? ", \"side\": {" : "\"main\": {";
@@ -1669,28 +1691,31 @@ int cflx_lu_timeline(cflx_lu* lu, char* buf, int buf_len) {
     return CFLX_OK;
 }
 int cflx_lu_phase_ms(cflx_lu* lu, double* ms_out) {
-    if (!lu || !ms_out) return CFLX_ERR_ARG;
+    REFUSE_IF(!lu);
+    REFUSE_IF(!ms_out);
     for (int i = 0; i < PH_COUNT; ++i) ms_out[i] = lu->phase_ms[i];
     return CFLX_OK;
 }
 int cflx_lu_set_kernel_timing(cflx_lu* lu, int enabled) {
-    if (!lu) return CFLX_ERR_ARG;
+    REFUSE_IF(!lu);
     lu->time_gemm = enabled != 0;
     return CFLX_OK;
 }
 int cflx_lu_trailing_stats(cflx_lu* lu, double* ms_out, double* flops_out) {
-    if (!lu || !ms_out || !flops_out) return CFLX_ERR_ARG;
+    REFUSE_IF(!lu);
+    REFUSE_IF(!ms_out);
+    REFUSE_IF(!flops_out);
     *ms_out = lu->gemm_ms;
     *flops_out = lu->gemm_flops;
     return CFLX_OK;
 }
-void cflx_lu_destroy(cflx_lu* lu) {
-    if (!lu) return;
-    cudaSetDevice(lu->comm->device);
-    for (SubComm* sc : {&lu->jk_comm, &lu->ik_comm})
-        if (sc->c) ncclCommDestroy(sc->c);
-    grid_free(lu);
-    delete lu;
-}
+void cflx_lu_destroy(cflx_lu* lu) { delete lu; }
 
 }  // extern "C"
+
+cflx_lu::~cflx_lu() {
+    cudaSetDevice(comm->device);
+    for (SubComm* sc : {&jk_comm, &ik_comm})
+        if (sc->c) ncclCommDestroy(sc->c);
+    grid_free(this);
+}

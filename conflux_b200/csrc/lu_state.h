@@ -214,10 +214,10 @@ struct SolveFactor {
     int stride;
 };
 
-// How a kind of handle words its state errors (callers match these texts)
+// How a kind of handle words its state errors, after "<function>: " (callers match these texts)
 struct HandleTexts {
-    const char* unfactored;  // format, %s: what was requested
-    const char* no_input;    // equilibration before the first upload
+    const char* unfactored;  // no factorisation to work on
+    const char* no_input;    // before the first upload
     const char* scaled;      // format, %c: the input's equed
 };
 
@@ -227,6 +227,7 @@ struct Handle : Grid {
     const HandleTexts* texts = nullptr;
     DevBuf<double> A0, A11;  // the input share and the working copy the factorisation overwrites, Ml x Nl
     bool have_input = false, factored = false;
+    bool a0_is_next = false;  // A0 already holds (or is receiving) the next input (LU input streaming)
     int64_t launches = 0;
     Stream side;        // high-priority look-ahead stream (null: no overlap)
     OzakiWorkspace oz;  // digit planes of the int8 wgmma trailing update (CFLX_GEMM=ozaki)
@@ -244,11 +245,18 @@ int handle_update_setup(Handle* h);
 int handle_side_stream(Handle* h);
 // host_local into A0, waited for: a new unscaled input, without factors or a solve cache
 int handle_set_local(Handle* h, const double* host_local);
-// CFLX_OK when `what` may run, after a successful factorisation; otherwise CFLX_ERR_STATE with the reason
-int handle_check(const Handle* h, const char* what);
-// equilibrate needs an input, and scales (apply) only an unscaled one; the input then changes, so the factors and the
-// solve cache are dropped, as by set_local
-int handle_equil_begin(Handle* h, bool apply);
+// What an entry point needs of its handle's state (enter)
+enum Need : unsigned {
+    NEED_INPUT = 1,      // an input (set_local)
+    NEED_UNSCALED = 2,   // an input that carries no scaling
+    NEED_FACTORS = 4,    // a successful factorisation
+    NEED_OWN_INPUT = 8,  // A0 still holds the input of that factorisation (not a queued next one)
+};
+// The prologue of every entry point `who` on a handle, after its argument checks: CFLX_ERR_STATE with "<who>: <reason>"
+// unless h's state has what `need` asks for, then h's device made current
+int enter(Handle* h, const char* who, unsigned need);
+// the input changes, so the factors and the solve cache are dropped, as by set_local
+void handle_equil_begin(Handle* h);
 // the input's record changes only when the call scaled it (apply, info == 0): equed with eq.qr and c (may be null); a
 // query leaves the record and its scales
 int handle_equil_end(Handle* h, bool apply, int info, char equed, double rowcnd, double colcnd, const double* c);
@@ -266,11 +274,9 @@ struct cflx_lu : cflx::Handle {
     cflx::PanelWorkspace pws{};
     int64_t ldp_max = 0;
     cflx::PinnedBuf<int> h_npiv;
-    std::vector<int> h_hist;
     bool time_gemm = false;
     // double-buffered input streaming (cflx_lu_queue_next_local): the upload of the NEXT matrix overlaps this factorisation
     const double* next_host = nullptr;
-    bool a0_is_next = false;  // A0 already holds (or is receiving) the next input: validation of the last run is refused
     cflx::Stream copy;
     cflx::Event ev_a0_read, ev_upload;
     double gemm_ms = 0, gemm_flops = 0;
@@ -301,6 +307,7 @@ struct cflx_lu : cflx::Handle {
     cflx::DevBuf<double> fix_ws;
     // cflx_lu_rbt: the transform of the input and of the factors
     cflx::RbtState rbt;
+    ~cflx_lu();  // the handle's device made current, the sub-communicators destroyed, then the members freed
 };
 
 namespace cflx {
@@ -612,11 +619,16 @@ struct SolveLocalArgs {
     int ldx;
     bool x_dev;
 };
-// *dev: p is device (or managed) memory, which must be on this rank's device (else CFLX_ERR_ARG)
-int share_kind(const Grid& g, const void* p, const char* what, bool* dev);
-// CFLX_ERR_ARG for nrhs < 1, a NULL B on layer 0, ldb (layer 0) or ldx (X set) below rhs_local_cols, X == B with
-// ldx != ldb, or device memory of another device; CFLX_OK with *a filled otherwise.  No collective.
-int solve_local_args(const Grid& g, int nrhs, const double* B, int ldb, const double* X, int ldx, SolveLocalArgs* a);
+// *dev: p is device (or managed) memory, which must be on this rank's device (else CFLX_ERR_ARG in the name of `who`)
+int share_kind(const char* who, const Grid& g, const void* p, const char* what, bool* dev);
+// The right-hand sides of the replicated solves (M x nrhs, leading dimensions ldb / ldx): CFLX_ERR_ARG in the name of
+// `who` unless nrhs >= 1, B is set, ldb >= nrhs, X is set (when x_required) and ldx >= nrhs (when X is set)
+int rhs_args(const char* who, int nrhs, const double* B, int ldb, const double* X, int ldx, bool x_required);
+// CFLX_ERR_ARG in the name of `who` for nrhs < 1, a NULL B on layer 0, ldb (layer 0) or ldx (X set) below
+// rhs_local_cols, X == B with ldx != ldb, or device memory of another device; CFLX_OK with *a filled otherwise.  No
+// collective.
+int solve_local_args(const char* who, const Grid& g, int nrhs, const double* B, int ldb, const double* X, int ldx,
+                     SolveLocalArgs* a);
 // solve(w, Bk, ldn, &Xk): the sweeps on the assembled block Bk (M x ldn device, w columns, the same on every rank), the
 // solution left in *Xk (M x ldn device, the same on every rank)
 using BlockSolve = std::function<int(int, const double*, int, const double**)>;

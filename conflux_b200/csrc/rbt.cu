@@ -178,7 +178,7 @@ int launch_rbt(RbtOp op, double* X, int64_t ld, const Layout& L, int ncols, int 
         case RbtOp::U: return launch_levels<true, false>(X, ld, L, ncols, col_lim, depth, su, nullptr, s);
         case RbtOp::W: return launch_levels<false, true>(X, ld, L, ncols, col_lim, depth, su, sv, s);
     }
-    return CFLX_ERR_ARG;
+    return refuse(__func__, "op is not an RbtOp");
 }
 
 int rbt_record_set(RbtRecord* dst, int depth, uint64_t seed, const double* s, int M, cudaStream_t st) {
@@ -200,10 +200,11 @@ int rbt_pass_on(RbtState* t, int M, bool next_is_plain, cudaStream_t s) {
 }  // namespace cflx
 
 extern "C" int cflx_rbt_multipliers(int M, int depth, uint64_t seed, double* u_out, double* v_out) {
-    if (depth < 1 || depth > 4 || M < 1 || M % (1 << depth) || (!u_out && !v_out)) {
-        cflx::set_last_error("cflx_rbt_multipliers: needs depth in [1, 4], M >= 1 a multiple of 2^depth, and an output");
-        return CFLX_ERR_ARG;
-    }
+    REFUSE_IF(depth < 1);
+    REFUSE_IF(depth > 4);
+    REFUSE_IF(M < 1);
+    REFUSE_IF(M % (1 << depth) != 0);
+    REFUSE_IF(!u_out && !v_out);
     if (u_out) cflx::rbt_multipliers(M, depth, seed, 0, u_out);
     if (v_out) cflx::rbt_multipliers(M, depth, seed, 1, v_out);
     return CFLX_OK;

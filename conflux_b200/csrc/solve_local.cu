@@ -64,13 +64,13 @@ int valid_cols(int nrhs, int v, int Py, int pj) {
 
 }  // namespace
 
-int share_kind(const Grid& g, const void* p, const char* what, bool* dev) {
+int share_kind(const char* who, const Grid& g, const void* p, const char* what, bool* dev) {
     cudaPointerAttributes at{};
     *dev = cudaPointerGetAttributes(&at, p) == cudaSuccess &&
            (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged);
     cudaGetLastError();  // an unknown host pointer is not an error here
     if (*dev && at.device != g.comm->device) {
-        set_last_error("distributed solve: %s is device memory of device %d, not this rank's device %d", what, at.device,
+        set_last_error("%s: %s is device memory of device %d, not this rank's device %d", who, what, at.device,
                        g.comm->device);
         return CFLX_ERR_ARG;
     }
@@ -100,19 +100,30 @@ int launch_solve_local_scatter(const double* Xk, int ldn, const Layout& L, int r
     return CFLX_OK;
 }
 
-int solve_local_args(const Grid& g, int nrhs, const double* B, int ldb, const double* X, int ldx, SolveLocalArgs* a) {
-    if (nrhs < 1) return CFLX_ERR_ARG;
-    const int ncl = rhs_local_cols(nrhs, g.v, g.Py);
+int rhs_args(const char* who, int nrhs, const double* B, int ldb, const double* X, int ldx, bool x_required) {
+    REFUSE_FOR(who, nrhs < 1);
+    REFUSE_FOR(who, !B);
+    REFUSE_FOR(who, ldb < nrhs);
+    REFUSE_FOR(who, x_required && !X);
+    REFUSE_FOR(who, X && ldx < nrhs);
+    return CFLX_OK;
+}
+
+int solve_local_args(const char* who, const Grid& g, int nrhs, const double* B, int ldb, const double* X, int ldx,
+                     SolveLocalArgs* a) {
+    REFUSE_FOR(who, nrhs < 1);
+    const int local_cols = rhs_local_cols(nrhs, g.v, g.Py);
     if (g.pk != 0) B = nullptr;  // read on layer 0 only
-    if (g.pk == 0 && (!B || ldb < ncl)) return CFLX_ERR_ARG;
-    if (X && ldx < ncl) return CFLX_ERR_ARG;
+    REFUSE_FOR(who, g.pk == 0 && !B);
+    REFUSE_FOR(who, g.pk == 0 && ldb < local_cols);
+    REFUSE_FOR(who, X && ldx < local_cols);
     if (B && X == B && ldx != ldb) {
-        set_last_error("distributed solve: X_local == B_local needs ldx == ldb (%d != %d)", ldx, ldb);
+        set_last_error("%s: X_local == B_local needs ldx == ldb (%d != %d)", who, ldx, ldb);
         return CFLX_ERR_ARG;
     }
     *a = SolveLocalArgs{nrhs, B, ldb, false, const_cast<double*>(X), ldx, false};
-    if (B) CFLX_TRY(share_kind(g, B, "B_local", &a->b_dev));
-    if (X) CFLX_TRY(share_kind(g, X, "X_local", &a->x_dev));
+    if (B) CFLX_TRY(share_kind(who, g, B, "B_local", &a->b_dev));
+    if (X) CFLX_TRY(share_kind(who, g, X, "X_local", &a->x_dev));
     return CFLX_OK;
 }
 
@@ -163,7 +174,10 @@ int solve_local_run(const Grid& g, int rows, const SolveLocalArgs& a, const Bloc
 }  // namespace cflx
 
 extern "C" int cflx_rhs_local_cols(int nrhs, int v, int Py, int* cols_out) {
-    if (nrhs < 1 || v < 1 || Py < 1 || !cols_out) return CFLX_ERR_ARG;
+    REFUSE_IF(nrhs < 1);
+    REFUSE_IF(v < 1);
+    REFUSE_IF(Py < 1);
+    REFUSE_IF(!cols_out);
     *cols_out = cflx::rhs_local_cols(nrhs, v, Py);
     return CFLX_OK;
 }

@@ -182,9 +182,15 @@ int lu_residual_grid(cflx_lu* lu, const std::vector<int>& hist, double* abs_out,
     const bool layer0 = lu->pk == 0;
     const size_t loc = (size_t)Ml * Nl;
     DevBuf<double> R, acc;
+    // CFLX_ERR_CUDA with a message for a failed call e, else CFLX_OK
+    auto cuda_rc = [](cudaError_t e, const char* call) {
+        if (e == cudaSuccess) return (int)CFLX_OK;
+        set_last_error("residual: %s -> %s", call, cudaGetErrorString(e));
+        return (int)CFLX_ERR_CUDA;
+    };
     int rc = CFLX_OK;
     if ((rc = acc.alloc(2 + SUMSQ_PARTIALS))) return rc;  // the two sums, then the partials of launch_sumsq
-    if (cudaMemsetAsync(acc, 0, 2 * sizeof(double), s) != cudaSuccess) rc = CFLX_ERR_CUDA;
+    rc = cuda_rc(cudaMemsetAsync(acc, 0, 2 * sizeof(double), s), "cudaMemsetAsync(acc)");
     if (!rc && layer0) {
         if (!lu->Cbuf) rc = lu->Cbuf.alloc(loc);
         if (!rc) rc = R.alloc(loc);
@@ -233,7 +239,7 @@ int lu_residual_grid(cflx_lu* lu, const std::vector<int>& hist, double* abs_out,
         }
     }
     if (!rc) rc = krc;
-    if (!rc && cudaGetLastError() != cudaSuccess) rc = CFLX_ERR_CUDA;
+    if (!rc) rc = cuda_rc(cudaGetLastError(), "the sweep's launches");
     if (!rc && layer0) {
         rc = launch_sumsq(R, (int64_t)loc, acc, acc + 2, s);
         if (!rc) rc = launch_sumsq(lu->A0, (int64_t)loc, acc + 1, acc + 2, s);
@@ -246,7 +252,7 @@ int lu_residual_grid(cflx_lu* lu, const std::vector<int>& hist, double* abs_out,
         }
     }
     double h[2] = {0, 0};
-    if (!rc && cudaMemcpyAsync(h, acc, sizeof(h), cudaMemcpyDeviceToHost, s) != cudaSuccess) rc = CFLX_ERR_CUDA;
+    if (!rc) rc = cuda_rc(cudaMemcpyAsync(h, acc, sizeof(h), cudaMemcpyDeviceToHost, s), "cudaMemcpyAsync(h)");
     if (cudaStreamSynchronize(s) != cudaSuccess && !rc) {
         set_last_error("residual: %s", cudaGetErrorString(cudaGetLastError()));
         rc = CFLX_ERR_CUDA;
@@ -256,7 +262,7 @@ int lu_residual_grid(cflx_lu* lu, const std::vector<int>& hist, double* abs_out,
     if (!rc) {
         cudaMemsetAsync(lu->PT, 0, (size_t)v * ldp * sizeof(double), s);
         cudaMemsetAsync(lu->U, 0, (size_t)v * (Nl + 2) * sizeof(double), s);
-        if (cudaStreamSynchronize(s) != cudaSuccess) rc = CFLX_ERR_CUDA;
+        rc = cuda_rc(cudaStreamSynchronize(s), "cudaStreamSynchronize after restoring the panels");
     }
     if (rc) return rc;
     if (abs_out) *abs_out = std::sqrt(h[0]);

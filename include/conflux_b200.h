@@ -4,7 +4,8 @@
  * This is the drop-in boundary for ONE path of eth-cscs/conflux: conflux::LU_rep<double> and the parts of
  * conflux::lu_params<double> it needs.  Plain pointers and sizes only; every function returns 0 on success or
  * a negative status code (never throws, never aborts); cflx_last_error() gives the message of the last failure
- * on the calling thread.  SPMD like the reference: one host thread (or process) per rank = per GPU; every
+ * on the calling thread; the message of a refused call (CFLX_ERR_ARG, CFLX_ERR_STATE) starts with the name of the function
+ * and names the condition that failed.  SPMD like the reference: one host thread (or process) per rank = per GPU; every
  * entry point that is marked COLLECTIVE must be called by all ranks of the grid in the same order.
  *
  * Reference interfaces replaced (file:line relative to the reference repository):
@@ -147,12 +148,14 @@ int cflx_lu_validate(cflx_lu*, double* frob_abs_out, double* frob_rel_out);
 int cflx_lu_residual(cflx_lu*, double* rel_out);
 /* COLLECTIVE.  Solves A X = B with the factors of the last cflx_lu_factor (P A = L U), on the GPU grid.
  * B: M x nrhs row-major host array (M = the padded size, info_out[0]), leading dimension ldb >= nrhs, the same on every
- * rank.  X: M x nrhs row-major, ldx >= nrhs, may be NULL on any rank; the result is identical on every rank.
- * The first call after a factorisation prepares and caches per-rank solve data; cflx_lu_set_local / cflx_lu_factor
- * drop it.  Does not modify the factors or the input.  No singularity check (like getrs). */
+ * rank.  X: M x nrhs row-major, ldx >= nrhs, may be NULL on any rank (ldx is then not read); the result is identical on
+ * every rank.  The first call after a factorisation prepares and caches per-rank solve data; cflx_lu_set_local /
+ * cflx_lu_factor drop it.  Does not modify the factors or the input.  No singularity check (like getrs).
+ * CFLX_ERR_ARG for nrhs < 1, a NULL B, ldb < nrhs, or ldx < nrhs with X set; CFLX_ERR_STATE before cflx_lu_factor and
+ * after cflx_lu_set_local. */
 int cflx_lu_solve(cflx_lu*, int nrhs, const double* B, int ldb, double* X, int ldx);
 /* COLLECTIVE.  Solves A^T X = B with the factors of the last cflx_lu_factor, on the GPU grid, like LAPACK's getrs with
- * TRANS = 'T'.  Arguments, state rules and caching as cflx_lu_solve. */
+ * TRANS = 'T'.  Arguments (ldx is not read when X is NULL), refusals, state rules and caching as cflx_lu_solve. */
 int cflx_lu_solve_trans(cflx_lu*, int nrhs, const double* B, int ldb, double* X, int ldx);
 /* Pure host.  cols_out: the local columns of an M x nrhs right-hand side share (cflx_lu_solve_local,
  * cflx_chol_solve_local) on any rank of a grid with Py grid columns, v * ceil(ceil(nrhs / v) / Py): lu_params' padding
