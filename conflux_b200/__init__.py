@@ -794,6 +794,48 @@ class dbg:
         return D, ms.value
 
     @staticmethod
+    def gemm_narrow_window(A, B, C, M, N, K, alpha=1.0, beta=0.0, a_off=(0, 0), b_off=(0, 0), c_off=(0, 0), trans=False,
+                           in_place=True):
+        """The solve's narrow GEMM on a window of whole buffers, as the solve engine launches it: rows [c_off[0], +M) x
+        columns [c_off[1], +N) of C become beta*C + alpha * op(A') @ B', with A' the block of A at (row, column) a_off
+        (M x K, or with trans K x M and op(A') = A'^T on the transposed kernel) and B' the K x N block of B at b_off.  C
+        is read only when beta != 0.  in_place: D is C on the device; else D starts as a device copy of C.  Entries
+        outside the blocks may hold anything (NaN canaries).  Returns (D, C): the whole buffers after the call (the same
+        array in place)."""
+        A = np.ascontiguousarray(A, dtype=np.float64)
+        B = np.ascontiguousarray(B, dtype=np.float64)
+        C = np.ascontiguousarray(C, dtype=np.float64)
+        D = np.empty_like(C)
+        Cout = D if in_place else np.empty_like(C)
+        check(lib().cflx_dbg_gemm_narrow_window(
+            1 if trans else 0, int(M), int(N), int(K), A.ctypes.data, A.shape[0], A.shape[1], int(a_off[0]),
+            int(a_off[1]), B.ctypes.data, B.shape[0], B.shape[1], int(b_off[0]), int(b_off[1]), C.ctypes.data,
+            C.shape[0], C.shape[1], int(c_off[0]), int(c_off[1]), float(alpha), float(beta), 1 if in_place else 0,
+            D.ctypes.data, Cout.ctypes.data), "dbg_gemm_narrow_window")
+        return D, Cout
+
+    DIAG_SOLVE_MODES = {"lower": 0, "upper": 1, "lower_t": 2, "unit_lower_t": 3, "upper_t": 4}
+
+    @staticmethod
+    def diag_solve(mode, share, R, v, nb, pos=(0, 0), lower=False):
+        """One diagonal tile of the solve engine: the v x v tile at (row, column) pos of share (lower: the Cholesky
+        factor L, zeros above its diagonal; else the LU's L\\U), its nb x nb diagonal blocks inverted as the solves cache
+        them, then Y = T^-1 R (R: v x ldn) by the solves' block sweep.  mode: "lower" (T = L), "upper" (U), "lower_t"
+        (L^T of the Cholesky tile), "unit_lower_t" (L^T of the LU's unit L), "upper_t" (U^T).  Returns (Y, inv) with inv
+        (2, v // nb, nb, nb): the forward blocks inv(L_jj), then the backward ones (inv(U_jj), or inv(L_jj)^T)."""
+        share = np.ascontiguousarray(share, dtype=np.float64)
+        R = np.ascontiguousarray(R, dtype=np.float64)
+        if R.ndim != 2 or R.shape[0] != v:
+            raise ValueError(f"diag_solve: R must have {v} rows, got shape {R.shape}")
+        Y = np.empty_like(R)
+        inv = np.empty((2, max(int(v) // max(int(nb), 1), 1), max(int(nb), 1), max(int(nb), 1)))
+        tri = dbg.DIAG_SOLVE_MODES[mode] if isinstance(mode, str) else int(mode)
+        check(lib().cflx_dbg_diag_solve(tri, 1 if lower else 0, int(v), int(nb), share.ctypes.data, share.shape[0],
+                                        share.shape[1], int(pos[0]), int(pos[1]), R.shape[1], R.ctypes.data,
+                                        Y.ctypes.data, inv.ctypes.data), "dbg_diag_solve")
+        return Y, inv
+
+    @staticmethod
     def residual(A, mode, v, Kappa=None, grid=(1, 1), pos=(0, 0), Xc=None, Xr=None, reps=1):
         """The residual kernels of lu_refine / cholesky.refine on one layer-0 share A (Ml x Nl, conflux layout of tile v at
         grid position pos of grid = (Px, Py)).  mode "nn": P = A @ Xc, Q = |A| @ |Xc| (Xc: Nl x nrhs, X by local column);

@@ -30,7 +30,7 @@ SYMBOLS = [
     "cflx_lu_get_permutation", "cflx_lu_residual", "cflx_lu_validate", "cflx_lu_solve", "cflx_lu_solve_trans", "cflx_rhs_local_cols", "cflx_lu_solve_local", "cflx_lu_rcond", "cflx_lu_refine", "cflx_lu_refine_x", "cflx_lu_equilibrate", "cflx_lu_svx", "cflx_lu_equilibrate_b", "cflx_lu_svxx", "cflx_lu_inverse", "cflx_lu_det", "cflx_lu_launch_count", "cflx_lu_uses_ozaki", "cflx_lu_set_profiling", "cflx_lu_phase_ms", "cflx_lu_timeline",
     "cflx_lu_set_kernel_timing", "cflx_lu_trailing_stats", "cflx_lu_destroy", "cflx_chol_auto_grid", "cflx_chol_auto_tile", "cflx_chol_dims", "cflx_chol_init_matrix_host",
     "cflx_chol_create", "cflx_chol_info", "cflx_chol_set_local", "cflx_chol_factor", "cflx_chol_get_local", "cflx_chol_validate",
-    "cflx_chol_solve", "cflx_chol_solve_local", "cflx_chol_rcond", "cflx_chol_refine", "cflx_chol_refine_x", "cflx_chol_equilibrate", "cflx_chol_svx", "cflx_chol_equilibrate_b", "cflx_chol_svxx", "cflx_chol_inverse", "cflx_chol_det", "cflx_chol_launch_count", "cflx_chol_destroy", "cflx_dbg_gemm_tn", "cflx_dbg_gemm_narrow", "cflx_dbg_gemm_narrow_tn", "cflx_dbg_residual", "cflx_dbg_residual_x", "cflx_dbg_equil", "cflx_dbg_growth_cols", "cflx_dbg_inverse_share", "cflx_dbg_solve_local_share", "cflx_dbg_norm_share", "cflx_dbg_rbt_share", "cflx_dbg_chol_validate_share", "cflx_dbg_lu_validate_share", "cflx_dbg_chol_gather_cols", "cflx_dbg_refine_assemble", "cflx_dbg_refine_columns", "cflx_dbg_det", "cflx_dbg_panel", "cflx_dbg_trsm", "cflx_dbg_diag_inverse", "cflx_dbg_potrf_tile", "cflx_dbg_getrf_nopiv_tile", "cflx_dbg_push_pivots", "cflx_dbg_ozaki_gemm", "cflx_dbg_wgmma_peak", "cflx_dbg_fp64_peak", "cflx_dbg_fp64_peak_ex",
+    "cflx_chol_solve", "cflx_chol_solve_local", "cflx_chol_rcond", "cflx_chol_refine", "cflx_chol_refine_x", "cflx_chol_equilibrate", "cflx_chol_svx", "cflx_chol_equilibrate_b", "cflx_chol_svxx", "cflx_chol_inverse", "cflx_chol_det", "cflx_chol_launch_count", "cflx_chol_destroy", "cflx_dbg_gemm_tn", "cflx_dbg_gemm_narrow", "cflx_dbg_gemm_narrow_tn", "cflx_dbg_gemm_narrow_window", "cflx_dbg_diag_solve", "cflx_dbg_residual", "cflx_dbg_residual_x", "cflx_dbg_equil", "cflx_dbg_growth_cols", "cflx_dbg_inverse_share", "cflx_dbg_solve_local_share", "cflx_dbg_norm_share", "cflx_dbg_rbt_share", "cflx_dbg_chol_validate_share", "cflx_dbg_lu_validate_share", "cflx_dbg_chol_gather_cols", "cflx_dbg_refine_assemble", "cflx_dbg_refine_columns", "cflx_dbg_det", "cflx_dbg_panel", "cflx_dbg_trsm", "cflx_dbg_diag_inverse", "cflx_dbg_potrf_tile", "cflx_dbg_getrf_nopiv_tile", "cflx_dbg_push_pivots", "cflx_dbg_ozaki_gemm", "cflx_dbg_wgmma_peak", "cflx_dbg_fp64_peak", "cflx_dbg_fp64_peak_ex",
 ]
 
 
@@ -149,6 +149,11 @@ def lib():
             ctypes.c_void_p, ctypes.c_int, c_double_p]
         L.cflx_dbg_gemm_narrow_tn.argtypes = [ctypes.c_int] * 3 + [ctypes.c_void_p] * 3 + [ctypes.c_double] * 2 + [
             ctypes.c_void_p, ctypes.c_int, c_double_p]
+        _blk = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_int, ctypes.c_int]
+        L.cflx_dbg_gemm_narrow_window.argtypes = [ctypes.c_int] * 4 + _blk * 3 + [ctypes.c_double] * 2 + [
+            ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
+        L.cflx_dbg_diag_solve.argtypes = [ctypes.c_int] * 4 + [ctypes.c_void_p, ctypes.c_int, ctypes.c_int64] + [
+            ctypes.c_int] * 3 + [ctypes.c_void_p] * 3
         share = ctypes.POINTER(ShareLayout)
         L.cflx_dbg_residual.argtypes = [ctypes.c_int, share, ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 4 + [
             ctypes.c_int, c_double_p]

@@ -312,6 +312,82 @@ int cflx_dbg_gemm_narrow_tn(int M, int N, int K, const double* AT, const double*
     });
 }
 
+// the narrow GEMM (trans: the transposed one) on a window of whole buffers, as the solve engine launches it (see the
+// header)
+int cflx_dbg_gemm_narrow_window(int trans, int M, int N, int K, const double* A, int a_rows, int64_t lda, int a_row,
+                                int a_col, const double* B, int b_rows, int64_t ldb, int b_row, int b_col, const double* C,
+                                int c_rows, int64_t ldc, int c_row, int c_col, double alpha, double beta, int in_place,
+                                double* D_out, double* C_out) {
+    CFLX_TRY(check_device());
+    const char* who = __func__;
+    if (M < 1 || N < 1 || K < 0) return refuse(who, "M < 1, N < 1 or K < 0");
+    if (!A || !B || !C) return refuse(who, "A, B or C is null");
+    if (a_rows < 1 || b_rows < 1 || c_rows < 1 || lda < 1 || ldb < 1 || ldc < 1)
+        return refuse(who, "a buffer with no rows or a leading dimension < 1");
+    if (a_row < 0 || a_col < 0 || b_row < 0 || b_col < 0 || c_row < 0 || c_col < 0) return refuse(who, "negative offset");
+    if (!trans && (K & 3)) return refuse(who, "K not a multiple of 4");
+    if ((lda & 1) || (a_col & 1)) return refuse(who, "odd lda or A column offset (A rows must be 16-byte aligned)");
+    // the A block: M rows of K (trans: K rows of M); B: K rows of N; the C window: M rows of N
+    const int a_h = trans ? K : M, a_w = trans ? M : K;
+    if ((int64_t)a_row + a_h > a_rows || a_col + (int64_t)a_w > lda) return refuse(who, "A block outside its buffer");
+    if ((int64_t)b_row + K > b_rows || b_col + (int64_t)N > ldb) return refuse(who, "B block outside its buffer");
+    if ((int64_t)c_row + M > c_rows || c_col + (int64_t)N > ldc) return refuse(who, "C window outside its buffer");
+    const size_t a_n = (size_t)a_rows * lda, b_n = (size_t)b_rows * ldb, c_n = (size_t)c_rows * ldc;
+    DevBuf<> dA, dB, dC, dD;
+    CFLX_TRY(stage(dA, a_n, A));
+    CFLX_TRY(stage(dB, b_n, B));
+    CFLX_TRY(stage(dC, c_n, C));
+    CFLX_TRY(stage(dD, c_n, C));
+    const double* a = dA.as<double>() + (int64_t)a_row * lda + a_col;
+    const double* b = dB.as<double>() + (int64_t)b_row * ldb + b_col;
+    const int64_t c_at = (int64_t)c_row * ldc + c_col;
+    double* c = dC.as<double>() + c_at;
+    double* d = (in_place ? dC.as<double>() : dD.as<double>()) + c_at;
+    if (trans)
+        CFLX_TRY(launch_gemm_narrow_tn(M, N, K, a, lda, b, ldb, c, ldc, d, ldc, alpha, beta, 0));
+    else
+        CFLX_TRY(launch_gemm_narrow(M, N, K, a, lda, b, ldb, c, ldc, d, ldc, alpha, beta, 0));
+    CFLX_TRY(fetch(D_out, in_place ? dC.p : dD.p, c_n));
+    CFLX_TRY(fetch(C_out, dC.p, c_n));
+    CFLX_CUDA(cudaDeviceSynchronize());
+    return CFLX_OK;
+}
+
+// one diagonal tile of the solve engine: its inverse blocks as solve_inverses makes them, then diag_solve (see the header)
+int cflx_dbg_diag_solve(int tri, int lower, int v, int nb, const double* share, int rows, int64_t ld, int row0, int col0,
+                        int ldn, const double* R, double* Y_out, double* inv_out) {
+    CFLX_TRY(check_device());
+    const char* who = __func__;
+    if (tri < 0 || tri > 4) return refuse(who, "tri outside 0 .. 4");
+    if (lower != 0 && lower != 1) return refuse(who, "lower not 0 or 1");
+    const Tri t = static_cast<Tri>(tri);
+    if (lower ? (t != Tri::Lower && t != Tri::LowerT) : t == Tri::LowerT)
+        return refuse(who, "tri not one the solves use on this kind of tile");
+    if (nb != 4 && nb != 8 && nb != 16 && nb != 32 && nb != 64 && nb != 128)
+        return refuse(who, "nb not 4, 8, 16, 32, 64 or 128", CFLX_ERR_UNSUPPORTED);
+    if (v < nb || v % nb) return refuse(who, "v not a positive multiple of nb");
+    if (ldn < 1) return refuse(who, "ldn < 1");
+    if (!share || !R || !Y_out) return refuse(who, "share, R or Y_out is null");
+    if (row0 < 0 || col0 < 0) return refuse(who, "negative tile offset");
+    if ((ld & 1) || (col0 & 1)) return refuse(who, "odd ld or col0 (the tile's rows must be 16-byte aligned)");
+    if ((int64_t)row0 + v > rows || col0 + (int64_t)v > ld) return refuse(who, "tile outside the share");
+    const size_t blocks = 2 * (size_t)v * nb, rn = (size_t)v * ldn;
+    DevBuf<> dS, dInv, dTile, dLinvT, dR, dY;
+    CFLX_TRY(stage(dS, (size_t)rows * ld, share));
+    CFLX_TRY(stage(dInv, blocks));
+    CFLX_TRY(stage(dTile, (size_t)v * v));
+    CFLX_TRY(stage(dLinvT, (size_t)v * nb));
+    CFLX_TRY(stage(dR, rn, R));
+    CFLX_TRY(stage(dY, rn));
+    const double* ftt = dS.as<double>() + (int64_t)row0 * ld + col0;
+    CFLX_TRY(solve_tile_inverses(ftt, ld, v, nb, lower != 0, dInv.as<double>(), dTile.as<double>(), dLinvT.as<double>(), 0));
+    CFLX_TRY(diag_solve(dInv.as<double>(), ftt, ld, v, nb, t, dR.as<double>(), dY.as<double>(), ldn, 0));
+    CFLX_TRY(fetch(Y_out, dY.p, rn));
+    CFLX_TRY(fetch(inv_out, dInv.p, blocks));
+    CFLX_CUDA(cudaDeviceSynchronize());
+    return CFLX_OK;
+}
+
 // the per-share kernels of equilibration and of the pivot growth (equil.cu) on one layer-0 share; each output may be null
 int cflx_dbg_equil(const cflx_share_layout* share, const double* A, const double* r, const double* c, char equed, int ncols,
                    double* rowmax_out, double* colmax_out, double* diag_out, double* scaled_out, double* sym_scaled_out,

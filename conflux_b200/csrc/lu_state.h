@@ -353,6 +353,14 @@ int solve_cache_grow(SolveCache* sc, const SolveFactor& f, int ldn, bool work, b
 // the inverses of the nb x nb diagonal blocks of every owned diagonal tile, into sc->inv (freed and allocated again here).
 // lower: the tile is L with its own diagonal and zeros above, inverted as A00 = L^T; otherwise it is L\U with a unit L.
 int solve_inverses(SolveCache* sc, const SolveFactor& f, bool lower);
+// solve_inverses' work on one diagonal tile T (v x v at leading dimension ld): the inverse blocks into inv (2 v nb: the
+// forward half, then the backward one), with scratch tile (v x v) and linvT (v x nb)
+int solve_tile_inverses(const double* T, int64_t ld, int v, int nb, bool lower, double* inv, double* tile, double* linvT,
+                        cudaStream_t s);
+// Y (v x ldn) = T^-1 R by the nb-block sweep over one diagonal tile ftt (leading dimension Nl) with its inverse blocks
+// tile_inv (solve_tile_inverses' inv); tri says which triangle of ftt is T and how it is read.  R is overwritten.
+int diag_solve(const double* tile_inv, const double* ftt, int64_t Nl, int v, int nb, Tri tri, double* R, double* Y,
+               int ldn, cudaStream_t s);
 // *dst = rows (allocated on first use), waited for
 int solve_set_rows(DevBuf<int>* dst, const std::vector<int>& rows, cudaStream_t s);
 // zero X, W and Z, and on the ranks holding B (`at`): at.dst[r] = B[at.rows[r]] for r < at.n; B is a host or device array

@@ -294,7 +294,30 @@ const double* diag_tile(const SolveFactor& f, int t) {
     return f.F + (int64_t)f.g.diag_row(t) * f.g.Nl + f.g.diag_col(t);
 }
 
-// Y = T^-1 R on the owner of diagonal tile t, by an nb-block sweep with the cached inverses; R (v x ldn) is overwritten.
+// diag_solve on the owner of diagonal tile t, with its cached inverses, into sc.Y
+int diag_solve_tile(const SolveCache& sc, const SolveFactor& f, int t, Tri tri, double* R, int ldn, cudaStream_t s) {
+    const double* inv = sc.inv + diag_slot(f, t) * 2 * (size_t)f.g.v * f.g.nb;
+    return diag_solve(inv, diag_tile(f, t), f.g.Nl, f.g.v, f.g.nb, tri, R, sc.Y, ldn, s);
+}
+}  // namespace
+
+int solve_tile_inverses(const double* T, int64_t ld, int v, int nb, bool lower, double* inv, double* tile, double* linvT,
+                        cudaStream_t s) {
+    // launch_diag_inverses takes an A00 = L\U.  A lower L goes in as L_tt^T, as the Cholesky panel step runs it:
+    // Uinv_j = inv(L_jj)^T is then the backward half, its block transpose inv(L_jj) the forward half, and the
+    // unit-lower part is the identity.  For L\U, the forward half is the block transpose of LinvT.
+    if (lower) {
+        CFLX_TRY(launch_extract_panel_T(T, ld, 0, 0, v, v, tile, v, s));
+    } else if (cudaMemcpy2DAsync(tile, v * sizeof(double), T, ld * sizeof(double), v * sizeof(double), v,
+                                 cudaMemcpyDeviceToDevice, s) != cudaSuccess) {
+        set_last_error("solve: diagonal tile copy failed");
+        return CFLX_ERR_CUDA;
+    }
+    CFLX_TRY(launch_diag_inverses(tile, v, nb, inv + (size_t)v * nb, linvT, s));
+    return launch_transpose_blocks(lower ? inv + (size_t)v * nb : linvT, nb, (int64_t)v * nb, inv, s);
+}
+
+// Y = T^-1 R by an nb-block sweep with the cached inverses; R (v x ldn) is overwritten.
 //   Lower:      T = L_tt:    Y_j = inv(L_jj) R_j, then R_i -= L_ij Y_j for i > j (the forward inverses)
 //   Upper:      T = U_tt:    Y_j = inv(U_jj) R_j, then R_i -= U_ij Y_j for i < j (the backward inverses)
 //   LowerT:     T = L_tt^T:  Y_j = inv(L_jj)^T R_j, then R_i -= L_ji^T Y_j for i < j (the backward inverses; L_tt read
@@ -302,13 +325,12 @@ const double* diag_tile(const SolveFactor& f, int t) {
 //   UnitLowerT: as LowerT, but inv(L_jj)^T is the forward inverse block read transposed (the LU's unit L)
 //   UpperT:     T = U_tt^T:  Y_j = inv(U_jj)^T R_j (the backward inverse block read transposed), then R_i -= U_ji^T Y_j
 //               for i > j: one TN launch on block row j of U_tt right of its diagonal block
-int diag_solve(const SolveCache& sc, const SolveFactor& f, int t, Tri tri, double* R, int ldn, cudaStream_t s) {
-    const int v = f.g.v, nb = f.g.nb, Nl = f.g.Nl, nblk = v / nb;
+int diag_solve(const double* tile_inv, const double* ftt, int64_t Nl, int v, int nb, Tri tri, double* R, double* Y,
+               int ldn, cudaStream_t s) {
+    const int nblk = v / nb;
     const bool fwd = tri == Tri::Lower, ascending = fwd || tri == Tri::UpperT;
     const bool fwd_half = fwd || tri == Tri::UnitLowerT, inv_tn = tri == Tri::UnitLowerT || tri == Tri::UpperT;
-    const double* inv = sc.inv + diag_slot(f, t) * 2 * (size_t)v * nb + (fwd_half ? 0 : (size_t)v * nb);
-    const double* ftt = diag_tile(f, t);
-    double* Y = sc.Y;
+    const double* inv = tile_inv + (fwd_half ? 0 : (size_t)v * nb);
     for (int i = 0; i < nblk; ++i) {
         const int j = ascending ? i : nblk - 1 - i;
         const int64_t o = (int64_t)j * nb * ldn;
@@ -336,7 +358,6 @@ int diag_solve(const SolveCache& sc, const SolveFactor& f, int t, Tri tri, doubl
     }
     return CFLX_OK;
 }
-}  // namespace
 
 int solve_cache_grow(SolveCache* sc, const SolveFactor& f, int ldn, bool work, bool col_partials, bool col_seed) {
     if (ldn <= sc->ldn && (sc->col_partials || !col_partials) && (sc->col_seed || !col_seed)) return CFLX_OK;
@@ -374,19 +395,7 @@ int solve_inverses(SolveCache* sc, const SolveFactor& f, bool lower) {
     for (int t = 0; t < f.g.Nt && !rc; ++t) {
         const int slot = diag_slot(f, t);
         if (slot < 0) continue;
-        double* inv = sc->inv + slot * per;
-        // launch_diag_inverses takes an A00 = L\U.  A lower L goes in as L_tt^T, as the Cholesky panel step runs it:
-        // Uinv_j = inv(L_jj)^T is then the backward half, its block transpose inv(L_jj) the forward half, and the
-        // unit-lower part is the identity.  For L\U, the forward half is the block transpose of LinvT.
-        if (lower) {
-            rc = launch_extract_panel_T(f.F, f.g.Nl, f.g.diag_row(t), f.g.diag_col(t), v, v, tile, v, s);
-        } else if (cudaMemcpy2DAsync(tile, v * sizeof(double), diag_tile(f, t), f.g.Nl * sizeof(double),
-                                     v * sizeof(double), v, cudaMemcpyDeviceToDevice, s) != cudaSuccess) {
-            set_last_error("solve: diagonal tile copy failed");
-            rc = CFLX_ERR_CUDA;
-        }
-        if (!rc) rc = launch_diag_inverses(tile, v, nb, inv + (size_t)v * nb, linvT, s);
-        if (!rc) rc = launch_transpose_blocks(lower ? inv + (size_t)v * nb : linvT.p, nb, (int64_t)v * nb, inv, s);
+        rc = solve_tile_inverses(diag_tile(f, t), f.g.Nl, v, nb, lower, sc->inv + slot * per, tile, linvT, s);
     }
     if (cudaStreamSynchronize(s) != cudaSuccess && !rc) rc = CFLX_ERR_CUDA;
     return rc;
@@ -431,7 +440,7 @@ int solve_row_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward,
             R = sc->R;
         }
         if (owner) {
-            CFLX_TRY(diag_solve(*sc, f, t, forward ? Tri::Lower : Tri::Upper, R, ldn, s));
+            CFLX_TRY(diag_solve_tile(*sc, f, t, forward ? Tri::Lower : Tri::Upper, R, ldn, s));
             CFLX_CUDA(cudaMemcpyAsync(keep + (int64_t)(t / keep_div) * tile, sc->Y, tile * sizeof(double),
                                       cudaMemcpyDeviceToDevice, s));
         } else if (clear_row && in_row && layer0) {
@@ -467,7 +476,7 @@ int solve_col_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward,
             R = sc->R;
         }
         if (owner) {
-            CFLX_TRY(diag_solve(*sc, f, t, tri, R, ldn, s));
+            CFLX_TRY(diag_solve_tile(*sc, f, t, tri, R, ldn, s));
             CFLX_CUDA(cudaMemcpyAsync(keep + (int64_t)(t / keep_div) * tile, sc->Y, tile * sizeof(double),
                                       cudaMemcpyDeviceToDevice, s));
         } else if (clear_col && in_col && layer0) {

@@ -415,6 +415,26 @@ int cflx_dbg_gemm_narrow(int M, int N, int K, const double* A, const double* B, 
  * of the Cholesky solve.  On the device AT gets an even leading dimension >= M, so any M >= 1 can be run. */
 int cflx_dbg_gemm_narrow_tn(int M, int N, int K, const double* AT, const double* B, const double* C, double alpha,
                             double beta, double* D, int reps, double* ms_out);
+/* D = beta*C + alpha * op(A) * B on the solve's narrow GEMM (trans == 0: op(A) = A, the block of M rows and K columns of
+ * A at row a_row, column a_col; trans != 0: the transposed kernel, op(A) = A^T with A's block K rows of M), at windows
+ * of whole row-major host buffers, as the solve engine launches it: A [a_rows x lda], B [b_rows x ldb] read from its
+ * block of K rows of N at (b_row, b_col), C [c_rows x ldc] updated in rows [c_row, c_row + M) x columns
+ * [c_col, c_col + N).  C is read only when beta != 0.  in_place != 0: D is C on the device; else D is a device copy of
+ * C.  D_out / C_out (optional, c_rows x ldc) receive the whole D and C buffers after the call.  Refused: a block or
+ * window outside its buffer, K < 0, K % 4 != 0 (trans == 0), an odd lda or a_col (A's rows 16-byte aligned). */
+int cflx_dbg_gemm_narrow_window(int trans, int M, int N, int K, const double* A, int a_rows, int64_t lda, int a_row,
+                                int a_col, const double* B, int b_rows, int64_t ldb, int b_row, int b_col, const double* C,
+                                int c_rows, int64_t ldc, int c_row, int c_col, double alpha, double beta, int in_place,
+                                double* D_out, double* C_out);
+/* One diagonal tile of the solve engine: the v x v tile at (row0, col0) of the row-major share [rows x ld] (lower != 0:
+ * the Cholesky factor L with zeros above its diagonal; 0: the LU's L\U with a unit L), its nb x nb diagonal blocks
+ * inverted as the solves cache them, then Y_out = T^-1 R (R and Y_out v x ldn) by the solves' block sweep, with tri
+ * 0 .. 4 = T = L (Lower), U (Upper), L^T (LowerT, Cholesky), L^T (UnitLowerT, the LU's unit L), U^T (UpperT).  The
+ * Cholesky tile takes Lower or LowerT, the LU tile any but LowerT.  inv_out (optional, 2 v nb) receives the cached
+ * blocks: v / nb row-major nb x nb forward blocks (inv(L_jj)), then v / nb backward ones (inv(U_jj), or inv(L_jj)^T of
+ * the Cholesky tile).  nb in 4, 8, ..., 128 with v % nb == 0; ld and col0 even; the tile inside the share. */
+int cflx_dbg_diag_solve(int tri, int lower, int v, int nb, const double* share, int rows, int64_t ld, int row0, int col0,
+                        int ldn, const double* R, double* Y_out, double* inv_out);
 /* The share a per-share hook runs on: one rank's row-major Ml x Nl share of a block-cyclic matrix of v x v tiles on a
  * Px x Py grid.  Global tile (I, J) lives on grid position (I % Px, J % Py) at local tile (I / Px, J / Py), so local row
  * r of the share at (pi, pj) is global row ((r / v) Px + pi) v + r % v, and local column c likewise with Py and pj.

@@ -279,6 +279,29 @@ def trsm_lower_unit_ok(L, R, Y, kappa_max):
     return bool(np.all(np.isfinite(Y)) and float(np.sqrt(np.sum(Res * Res))) <= bound)
 
 
+def trsm_left_ok(T, R, Y, nb):
+    """Y^ = inv(T) R by the solve engine's diagonal-tile sweep (T v x v triangular, as given: lower or upper, unit or not,
+    a factor or its transpose; R v x n):
+        ||T Y^ - R||_F <= gamma_{v+1} (1 + 4 kappa_max) || |T| |Y^| ||_F,
+    kappa_max over T's nb x nb diagonal blocks.  Derivation.  The sweep takes the blocks j in the order of elimination
+    (down for a lower T, up for an upper one): Y_j = fl(Xi_j R'_j) with Xi_j the cached inverse of T_jj, then
+    R'_i = fl(R'_i - T_ij Y_j) for the blocks i still to solve.  Xi_j was formed by substitution, so T_jj Xi_j = I + F_j
+    with |F_j| <= gamma_nb |T_jj| |Xi_j| (Sec. 14.2; a transposed or unit T_jj is the same substitution); the product adds
+    Y_j = Xi_j R'_j + G_j, |G_j| <= gamma_nb |Xi_j| |R'_j| (Sec. 3.5); the updates are narrow GEMMs with
+    gamma_{nb+1} (gemm_ok), and R'_j - R_j gathers at most v - nb of their terms, so the block row j of the residual is
+        T_jj Y_j - R'_j + (R'_j - R_j + sum_{i<>j} T_ji Y_i) = F_j R'_j + T_jj G_j + E_j,
+    with ||E_j||_F <= gamma_{v+1} || |T| |Y^| ||_F over the sweep.  Since R'_j ~ T_jj Y_j, the first two terms are at
+    most gamma_nb kappa_2(T_jj) || |T_jj| |Y_j| ||_F each to first order.  So the bound is that of trsm_upper_ok, with
+    the same factor 2 over the first-order 2 kappa_max for the second-order terms; reading T transposed in place
+    changes which entries are summed, not how."""
+    T = np.asarray(T, dtype=np.float64)
+    Y = np.asarray(Y, dtype=np.float64)
+    Res = matmul(T, Y) - np.asarray(R, dtype=np.float64).astype(LD)
+    M = np.abs(T) @ np.abs(Y)
+    bound = gamma(T.shape[0] + 1) * (1.0 + 4.0 * diag_block_kappa(T, nb)) * float(np.linalg.norm(M))
+    return bool(np.all(np.isfinite(Y)) and float(np.sqrt(np.sum(Res * Res))) <= bound)
+
+
 # ------------------------------------------------------------------------------------------------ test matrices
 def random_spd(n, kappa, rng):
     """Q diag(logspace) Q^T with 2-norm condition number kappa (Q Haar-random orthogonal), as float64"""

@@ -110,6 +110,8 @@ def test_device_entry_points_refuse_without_gpu():
                  lambda: cb.dbg.lu_validate_share(A, 4),
                  lambda: cb.dbg.chol_gather_cols([np.ones((4, 8))], 4, 1, 1, 0, 8, 8, 0),
                  lambda: cb.dbg.refine_assemble("x", np.zeros((8, 16)), np.zeros((8, 8)), (1, 1, 1), 4, 8, 8, 8, 1, 0, 8),
-                 lambda: cb.dbg.refine_columns(A, A, np.ones(8), 8)):
+                 lambda: cb.dbg.refine_columns(A, A, np.ones(8), 8),
+                 lambda: cb.dbg.gemm_narrow_window(A, A, A, 4, 4, 4),
+                 lambda: cb.dbg.diag_solve("lower", A, np.ones((8, 2)), 8, 4)):
         with pytest.raises(cb.ConfluxError, match="no CPU fallback"):
             call()

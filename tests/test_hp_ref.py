@@ -275,6 +275,45 @@ def test_trsm_checks_accept_the_blocked_solve_and_reject_defects(v, nb):
     assert not hp.trsm_lower_unit_ok(L, R, _inv_sweep_lower_unit(Ld, R, nb), kL)
 
 
+def _inv_sweep(T, R, nb):
+    """inv(T) R in float64 the way the solve engine's diagonal-tile sweep runs it: blocks in elimination order, each the
+    product with the inverse of its diagonal block, then the update of the blocks still to solve"""
+    v = T.shape[0]
+    lower = not np.triu(T, 1).any()
+    R = R.copy()
+    Y = np.zeros_like(R)
+    for j in (range(0, v, nb) if lower else range(v - nb, -1, -nb)):
+        b = slice(j, j + nb)
+        Y[b] = np.linalg.inv(T[b, b]) @ R[b]
+        rest = slice(j + nb, v) if lower else slice(0, j)
+        R[rest] -= T[rest, b] @ Y[b]
+    return Y
+
+
+@pytest.mark.parametrize("form", ["lower", "upper", "lower_t", "unit_lower_t", "upper_t"])
+def test_left_trsm_check_accepts_the_block_sweep_and_rejects_defects(form):
+    v, nb, n = 128, 16, 24
+    rng = np.random.default_rng(len(form))
+    L = np.tril(rng.uniform(-1, 1, (v, v)), -1) * (2 / np.sqrt(v)) + np.diag(1 + rng.random(v))
+    U = np.triu(rng.uniform(-1, 1, (v, v)), 1) * (2 / np.sqrt(v)) + np.diag(1 + rng.random(v))
+    Lu = np.tril(L, -1) + np.eye(v)
+    T = {"lower": L, "upper": U, "lower_t": L.T, "unit_lower_t": Lu.T, "upper_t": U.T}[form]
+    lower = not np.triu(T, 1).any()
+    R = rng.standard_normal((v, n))
+    Y = _inv_sweep(T, R, nb)
+    assert hp.trsm_left_ok(T, R, Y, nb)
+    assert hp.trsm_left_ok(T, R, scipy.linalg.solve_triangular(T, R, lower=lower), nb)
+    wrong = Y.copy()
+    wrong[v // 2, 7] += 1e-9 * np.abs(Y).max()
+    shift = Y.copy()
+    shift[:, 1:] = Y[:, :-1]
+    for bad in (wrong, shift):
+        assert not hp.trsm_left_ok(T, R, bad, nb)
+    Td = T.copy()                                             # one term of one block update missing
+    Td[(v - 1, 0) if lower else (0, v - 1)] = 0.0
+    assert not hp.trsm_left_ok(T, R, _inv_sweep(Td, R, nb), nb)
+
+
 def test_power_of_two_grading_commutes_with_the_factorisation():
     """the property the graded GPU test relies on: for D = diag(2^k), the float64 factor of D S D is D times the float64
     factor of S, bit for bit (in every order of summation; shown here for the right-looking restatement)"""
