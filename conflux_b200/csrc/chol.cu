@@ -464,10 +464,12 @@ size_t potrf_tile_scratch(int v) { return (v % QBK == 0 && v >= 2 * QBK) ? (size
 // raise-only: a smaller v (another object, a test hook) never lowers the limit a live object relies on
 int potrf_setup(int v) {
     static PerDeviceMax tile_cfg, blk_cfg;
-    if (tile_cfg.raise(potrf_tile_smem(v)))
-        CFLX_CUDA(cudaFuncSetAttribute(potrf_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)potrf_tile_smem(v)));
-    if (blk_cfg.raise(QBK * QPITCH * sizeof(double)))
-        CFLX_CUDA(cudaFuncSetAttribute(potrf128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(QBK * QPITCH * sizeof(double))));
+    CFLX_CUDA(tile_cfg.raise(potrf_tile_smem(v), [&] {
+        return cudaFuncSetAttribute(potrf_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)potrf_tile_smem(v));
+    }));
+    CFLX_CUDA(blk_cfg.raise(QBK * QPITCH * sizeof(double), [&] {
+        return cudaFuncSetAttribute(potrf128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(QBK * QPITCH * sizeof(double)));
+    }));
     return CFLX_OK;
 }
 
@@ -741,6 +743,9 @@ int cflx_chol_dims(int N, int v, int Px, int Py, int Pz, int* o) {
 // CholeskyIO.cpp:100-172: T = lower triangle of R^T R with R = v x v uniform(-1, 1) from rand() after srand(1) (same on
 // every rank); every tile of the (lower triangle of the) matrix is T, the global diagonal is 2 * Kappa * max_i sum_j |T_ij|.
 // Layers pz != 0 start at zero.  (The reference leaves the upper triangle of its tile buffer unwritten; zeros here.)
+// The sequence is glibc's rand() after srand(1), drawn from a state of this call's own (random_r with the 128-byte
+// state srand uses): ranks that are threads of one process call this at the same time, and the shared state of rand()
+// would deal each of them a different, interleaved R.
 int cflx_chol_init_matrix_host(int N, int v, int Px, int Py, int Pz, int rank, double* out) {
     int d[6];
     CFLX_TRY(chol_dims(__func__, N, v, Px, Py, Pz, d));
@@ -752,8 +757,14 @@ int cflx_chol_init_matrix_host(int N, int v, int Px, int Py, int Pz, int rank, d
     if (rank % Pz != 0) return CFLX_OK;
     const int pi = rank / (Py * Pz), pj = (rank / Pz) % Py;
     std::vector<double> R((size_t)v * v), T((size_t)v * v, 0.0);
-    srand(1);
-    for (size_t i = 0; i < (size_t)v * v; ++i) R[i] = (double)rand() / RAND_MAX * 2 - 1;
+    alignas(int32_t) char state[128];  // initstate_r keeps its state as int32_t words
+    random_data rd{};
+    initstate_r(1, state, sizeof(state), &rd);
+    for (size_t i = 0; i < (size_t)v * v; ++i) {
+        int32_t x = 0;
+        random_r(&rd, &x);
+        R[i] = (double)x / RAND_MAX * 2 - 1;
+    }
     for (int i = 0; i < v; ++i)                 // T = lower(R^T R)  (cblas_dsyrk RowMajor, Lower, Trans)
         for (int j = 0; j <= i; ++j) {
             double s = 0.0;

@@ -8,6 +8,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <initializer_list>
+#include <mutex>
 #include <type_traits>
 #include <utility>
 
@@ -152,20 +153,25 @@ struct Stream {
     operator cudaStream_t() const { return s; }
 };
 
-// cudaFuncSetAttribute is per DEVICE: ranks may be threads of one process driving different GPUs, so the
-// "already configured" bookkeeping is kept per device ordinal (values only grow; a benign race re-applies it).
+// cudaFuncSetAttribute is per DEVICE: ranks may be threads of one process driving different GPUs, or several threads
+// (ranks, or independent handles) driving the same one.  raise(want, set) runs set() on the current device when `want`
+// exceeds what was configured there, and records it only once set() succeeded.  The lock makes every other thread
+// that needs the attribute wait until it is in place: recording first and setting after would let a second thread
+// launch with more shared memory than the function allows yet.
 struct PerDeviceMax {
+    std::mutex m;
     size_t v[64] = {0};
-    // returns true when `want` exceeds what was configured on the current device (and records it)
-    bool raise(size_t want) {
+    template <class F>
+    cudaError_t raise(size_t want, F&& set) {
         int dev = 0;
-        cudaGetDevice(&dev);
+        cudaError_t e = cudaGetDevice(&dev);
+        if (e != cudaSuccess) return e;
         dev &= 63;
-        if (want > v[dev]) {
-            v[dev] = want;
-            return true;
-        }
-        return false;
+        std::lock_guard<std::mutex> lk(m);
+        if (want <= v[dev]) return cudaSuccess;
+        e = set();
+        if (e == cudaSuccess) v[dev] = want;
+        return e;
     }
 };
 

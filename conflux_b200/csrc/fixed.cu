@@ -183,8 +183,9 @@ int block_lu(double* A, int lda, int n, double tiny, double* Ac, double* ATc, in
              cudaStream_t s) {
     static PerDeviceMax cfg;
     const size_t smem = gpanel ? 0 : tile_smem(n);
-    if (cfg.raise(smem))
-        CFLX_CUDA(cudaFuncSetAttribute(getrf_nopiv_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CFLX_CUDA(cfg.raise(smem, [&] {
+        return cudaFuncSetAttribute(getrf_nopiv_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    }));
     getrf_nopiv_block_kernel<<<1, FTHREADS, smem, s>>>(A, lda, n, tiny, Ac, ATc, rec, col0, gpanel);
     CFLX_CUDA(cudaGetLastError());
     return CFLX_OK;

@@ -232,9 +232,9 @@ namespace {
 template <int WM, int WN, int MINB>
 int setup_one() {
     static PerDeviceMax cfg;
-    if (cfg.raise(Cfg<WM, WN>::SMEM))
-        CFLX_CUDA(cudaFuncSetAttribute(gemm_tn_kernel<WM, WN, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)Cfg<WM, WN>::SMEM));
+    CFLX_CUDA(cfg.raise(Cfg<WM, WN>::SMEM, [&] {
+        return cudaFuncSetAttribute(gemm_tn_kernel<WM, WN, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg<WM, WN>::SMEM);
+    }));
     return CFLX_OK;
 }
 template <int WM, int WN, int MINB>

@@ -405,8 +405,9 @@ int ozaki_workspace_create(OzakiWorkspace* ws, int max_rows, int max_cols, int K
     CFLX_TRY(make_plane_map(&ws->maps->a, ws->planesA, K, ws->cap_a, OZ_BM));
     CFLX_TRY(make_plane_map(&ws->maps->b, ws->planesB, K, ws->cap_b, OZ_BN));
     static PerDeviceMax cfg;
-    if (cfg.raise(OZ_SMEM))
-        CFLX_CUDA(cudaFuncSetAttribute(ozaki_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)OZ_SMEM));
+    CFLX_CUDA(cfg.raise(OZ_SMEM, [&] {
+        return cudaFuncSetAttribute(ozaki_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)OZ_SMEM);
+    }));
     int dev = 0;
     CFLX_CUDA(cudaGetDevice(&dev));
     CFLX_CUDA(cudaDeviceGetAttribute(&ws->sms, cudaDevAttrMultiProcessorCount, dev));

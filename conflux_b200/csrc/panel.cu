@@ -605,10 +605,12 @@ int launch_stack_getrf(double* W, int64_t ldw, int n, int v, int* perm_out, Pane
     ws->sk_ticket_count += (unsigned)C;
     const int threads = (int)round_up(n, 32);
     static PerDeviceMax cfg;
-    if (cfg.raise((size_t)SK_CB * 1024 * sizeof(double))) {
-        CFLX_CUDA(cudaFuncSetAttribute(stack_getrf_kernel<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, SK_CB * 1024 * 8));
-        CFLX_CUDA(cudaFuncSetAttribute(stack_getrf_kernel<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, SK_CB * 512 * 8));
-    }
+    CFLX_CUDA(cfg.raise((size_t)SK_CB * 1024 * sizeof(double), [&] {
+        const cudaError_t e =
+            cudaFuncSetAttribute(stack_getrf_kernel<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, SK_CB * 1024 * 8);
+        if (e != cudaSuccess) return e;
+        return cudaFuncSetAttribute(stack_getrf_kernel<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, SK_CB * 512 * 8);
+    }));
     if (threads <= 256) stack_getrf_kernel<256><<<C, threads, SK_CB * 256 * sizeof(double), stream>>>(a);
     else if (threads <= 512) stack_getrf_kernel<512><<<C, threads, SK_CB * 512 * sizeof(double), stream>>>(a);
     else stack_getrf_kernel<1024><<<C, threads, SK_CB * 1024 * sizeof(double), stream>>>(a);
@@ -642,8 +644,9 @@ int launch_nb_rpt(PanelArgs& a, cudaStream_t stream) {
     const size_t smem = panel_smem_bytes<NB>(a.Rpad, a.v);
     void* params[] = {&a};
     static PerDeviceMax cfg;
-    if (cfg.raise(smem))
-        CFLX_CUDA(cudaFuncSetAttribute(panel_getrf_kernel<NB, RPT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CFLX_CUDA(cfg.raise(smem, [&] {
+        return cudaFuncSetAttribute(panel_getrf_kernel<NB, RPT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    }));
     CFLX_CUDA(cudaLaunchCooperativeKernel((void*)panel_getrf_kernel<NB, RPT>, dim3(a.G), dim3(PT_LAUNCH), params, smem, stream));
     return CFLX_OK;
 }

@@ -267,8 +267,9 @@ template <int NT, int MASK>
 int launch_nn(const ResidArgs& r, cudaStream_t s) {
     using C = NarrowCfg<NT>;
     static PerDeviceMax cfg;
-    if (cfg.raise(C::SMEM))
-        CFLX_CUDA(cudaFuncSetAttribute(resid_nn_kernel<NT, MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
+    CFLX_CUDA(cfg.raise(C::SMEM, [&] {
+        return cudaFuncSetAttribute(resid_nn_kernel<NT, MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM);
+    }));
     dim3 grid((unsigned)((r.M + BM - 1) / BM), (unsigned)((r.N + C::BN - 1) / C::BN));
     resid_nn_kernel<NT, MASK><<<grid, NW * 32, C::SMEM, s>>>(r);
     CFLX_CUDA(cudaGetLastError());
@@ -279,8 +280,9 @@ template <int NT, int MASK>
 int launch_tn(const ResidArgs& r, cudaStream_t s) {
     using C = NarrowCfg<NT>;
     static PerDeviceMax cfg;
-    if (cfg.raise(C::SMEM))
-        CFLX_CUDA(cudaFuncSetAttribute(resid_tn_kernel<NT, MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
+    CFLX_CUDA(cfg.raise(C::SMEM, [&] {
+        return cudaFuncSetAttribute(resid_tn_kernel<NT, MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM);
+    }));
     dim3 grid((unsigned)((r.M + BM_TN - 1) / BM_TN), (unsigned)((r.N + C::BN - 1) / C::BN));
     resid_tn_kernel<NT, MASK><<<grid, NW * 32, C::SMEM, s>>>(r);
     CFLX_CUDA(cudaGetLastError());

@@ -125,8 +125,9 @@ template <int NT>
 int launch_narrow_nt(const NarrowArgs& g, cudaStream_t s) {
     using C = NarrowCfg<NT>;
     static PerDeviceMax cfg;
-    if (cfg.raise(C::SMEM))
-        CFLX_CUDA(cudaFuncSetAttribute(gemm_narrow_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
+    CFLX_CUDA(cfg.raise(C::SMEM, [&] {
+        return cudaFuncSetAttribute(gemm_narrow_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM);
+    }));
     dim3 grid((unsigned)((g.M + BM - 1) / BM), (unsigned)((g.N + C::BN - 1) / C::BN));
     gemm_narrow_kernel<NT><<<grid, NW * 32, C::SMEM, s>>>(g);
     CFLX_CUDA(cudaGetLastError());
@@ -226,8 +227,9 @@ template <int NT>
 int launch_narrow_tn(const NarrowArgs& g, cudaStream_t s) {
     using C = NarrowCfg<NT>;
     static PerDeviceMax cfg;
-    if (cfg.raise(C::SMEM))
-        CFLX_CUDA(cudaFuncSetAttribute(gemm_narrow_tn_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
+    CFLX_CUDA(cfg.raise(C::SMEM, [&] {
+        return cudaFuncSetAttribute(gemm_narrow_tn_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM);
+    }));
     dim3 grid((unsigned)((g.M + BM_TN - 1) / BM_TN), (unsigned)((g.N + C::BN - 1) / C::BN));
     gemm_narrow_tn_kernel<NT><<<grid, NW * 32, C::SMEM, s>>>(g);
     CFLX_CUDA(cudaGetLastError());

@@ -91,8 +91,9 @@ int launch_diag_nb(const double* A00, int v, double* Uinv, double* LinvT, cudaSt
     constexpr int CS = NB > 64 ? NB / 32 : 1;   // 128-wide blocks: 4 CTAs x 32 columns, one column per warp
     const int warps = NB < 32 ? NB : 32;
     static PerDeviceMax cfg;
-    if (cfg.raise(smem))
-        CFLX_CUDA(cudaFuncSetAttribute(diag_inverse_kernel<NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CFLX_CUDA(cfg.raise(smem, [&] {
+        return cudaFuncSetAttribute(diag_inverse_kernel<NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    }));
     diag_inverse_kernel<NB><<<dim3(v / NB, 2, CS), 32 * warps, smem, stream>>>(A00, v, Uinv, LinvT);
     CFLX_CUDA(cudaGetLastError());
     return CFLX_OK;

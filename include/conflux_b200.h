@@ -309,7 +309,9 @@ void cflx_lu_destroy(cflx_lu*);
  *   parallelCholesky()                  Cholesky.cpp:760-921                              -> cflx_chol_factor
  *   finalize(clean)                     Cholesky.cpp:160-175                              -> cflx_chol_destroy
  * Local data: row-major Ml x Nl, tile (gi, gj) of the v x v tiling on rank (gi % Px, gj % Py) at local tile (gi / Px,
- * gj / Py); ranks are numbered (pi * Py + pj) * Pz + pk like the LU path; only the lower triangle is referenced. */
+ * gj / Py); ranks are numbered (pi * Py + pj) * Pz + pk like the LU path; only the lower triangle is referenced.  The
+ * layers pk != 0 hold zeros, as cflx_chol_init_matrix_host leaves them: the factorisation sums every layer's share
+ * into the tiles of layer 0. */
 typedef struct cflx_chol cflx_chol;
 int cflx_chol_auto_grid(int P, int N, int* grid3_out);
 int cflx_chol_auto_tile(int N, int P, int Pz);

@@ -42,9 +42,10 @@ def _same_bits(a, b):
 
 def _child(fn, arg, env, tmp_path):
     """fn(arg) of this module in a fresh interpreter with env added (switches read once per process); returns what it
-    wrote to tmp_path as JSON"""
+    wrote to tmp_path as JSON.  Under the NCCL loopback the child runs its grids on one device as the parent does."""
     out = os.path.join(str(tmp_path), f"{fn}.json")
-    code = (f"import sys; sys.path.insert(0, {ROOT!r}); import json; from tests import test_gpu_lu_edges as t; "
+    code = (f"import sys; sys.path.insert(0, {ROOT!r}); from tests import _loopback; _loopback.install_if_preloaded(); "
+            f"import json; from tests import test_gpu_lu_edges as t; "
             f"json.dump(t.{fn}({arg!r}), open({out!r}, 'w'))")
     flags = ["-s"] if sys.flags.no_user_site else []
     r = subprocess.run([sys.executable] + flags + ["-c", code], env=dict(os.environ, **env), cwd=ROOT, timeout=900,

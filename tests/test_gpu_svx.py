@@ -359,7 +359,8 @@ def test_multi_gpu_chol_svx(N, v, grid):
         pytest.skip(f"needs {P} GPUs")
     n = chol_ref.dims(N, v, *grid)["N"]
     A = _spd(n, "scaled", N)
-    locs = chol_solve_ref.scatter(A, N, v, *grid, upper=np.nan, pad=np.nan, layers=np.nan)
+    # layers pk != 0 hold zeros: the factorisation sums every layer's share into layer 0's tiles
+    locs = chol_solve_ref.scatter(A, N, v, *grid, upper=np.nan, pad=np.nan, layers=0.0)
     B = np.random.default_rng(N).standard_normal((n, 3))
 
     def body(comm):
