@@ -4,10 +4,12 @@ over `reps` launches, mean ms of one launch):
   * 16128 x 16128 x 256 (the whole update of step 0), with K = 16 as well: K = 256 minus K = 16 is the main loop, the
     rest is the per-tile fixed cost (operand fill, epilogue);
   * part 0 (n_act x 256, the look-ahead columns) and part 1 (n_act x (n_act - 256)) of steps k = 0, 16, 32, 48, 60,
-    n_act = 16384 - 256 (k + 1), and the local pivot search (cb.dbg.panel) on the n_act x 256 panel of the same step.
+    n_act = 16384 - 256 (k + 1), and the local pivot search (cb.dbg.panel) on the n_act x 256 panel of the same step;
+  * the GEMMs of the U solve at the same steps (M = 128, K = 128, the TRSM sweep with nb = 128): the look-ahead
+    columns (N = 256) and the rest (N = n_act - 256), beta = 0 the diagonal block, beta = 1 the update below it.
 Every GEMM shape runs with beta = 1 and beta = 0; beta = 0 reads no C, so the difference is what the C read costs.
 C has the factorisation's leading dimension (Nl = 16384).  Prints one JSON line with the card's name, power limit and
-SM clock.
+SM clock, and the tile CFLX_GEMM_TILE fixes (empty: chosen per launch).
     python tools/gemm_speed.py [--root TREE] [--out FILE]
 --root imports conflux_b200 from another checkout (to compare two builds in one process each)."""
 import argparse
@@ -51,7 +53,8 @@ def gemm(M, Ncols, K, beta, col_off):
             "tflops": round(2.0 * M * Ncols * K / (ms * 1e-3) / 1e12, 2)}
 
 
-rec = {"tool": "gemm_speed", "root": os.path.abspath(a.root), "card": card(), "shapes": [], "panel": []}
+rec = {"tool": "gemm_speed", "root": os.path.abspath(a.root), "tile": os.environ.get("CFLX_GEMM_TILE", ""),
+       "card": card(), "shapes": [], "panel": []}
 M0 = N - V
 for K in (256, 16):
     for beta in (1.0, 0.0):
@@ -61,6 +64,9 @@ for k in STEPS:
     for part, (cols, off) in enumerate(((V, 0), (n_act - V, V))):
         for beta in (1.0, 0.0):
             rec["shapes"].append(dict(gemm(n_act, cols, V, beta, off), name=f"step{k}_part{part}"))
+    for cols in (V, n_act - V):
+        for beta in (1.0, 0.0):
+            rec["shapes"].append(dict(gemm(128, cols, 128, beta, 0), name=f"step{k}_usolve_N{cols}"))
     _, _, _, pms = cb.dbg.panel(np.ascontiguousarray(Cbig[:n_act, :V]), reps=5)
     rec["panel"].append({"step": k, "n_act": n_act, "ms": round(pms, 4)})
 rec["card_after"] = card()
