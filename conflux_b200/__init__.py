@@ -564,6 +564,66 @@ class cholesky:
         check(lib().cflx_chol_factor(self._h, ctypes.byref(ms)), "chol_factor")
         return ms.value
 
+    def factor_ldlt(self, tiny=0.0, upload=True):
+        """The signed Cholesky A = R S R^T of the padded input without pivoting (cflx_chol_factor_ldlt), for symmetric
+        indefinite matrices: R lower triangular with a positive diagonal (local_factor), S = diag(signs()).  tiny: pivots
+        with |d| < tiny become copysign(tiny, d).  upload=True copies self.data to the device first.  Returns (nrepl,
+        inertia, info, ms): the replaced pivots, (positive, negative, zero) pivots, 1 + the first exactly zero pivot's
+        column (0: none) and the loop's device ms.  Every later call (solve, rcond, refine, svx, inverse, det, validate)
+        refers to R S R^T.  COLLECTIVE; identical on every rank."""
+        if upload:
+            a = np.ascontiguousarray(self.data, dtype=np.float64)
+            check(lib().cflx_chol_set_local(self._h, a.ctypes.data), "chol_set_local")
+        nrepl, info, ms = ctypes.c_int(), ctypes.c_int(), ctypes.c_double()
+        inertia = (ctypes.c_int64 * 3)()
+        check(lib().cflx_chol_factor_ldlt(self._h, float(tiny), ctypes.byref(nrepl), inertia, ctypes.byref(info),
+                                          ctypes.byref(ms)), "chol_factor_ldlt")
+        return nrepl.value, tuple(inertia), info.value, ms.value
+
+    def rbt(self, depth=2, seed=0, upload=True):
+        """Symmetric random butterfly transform of the input (cflx_chol_rbt): A <- W = U^T A U, after the stored lower
+        triangle is completed to the symmetric matrix.  Then factor_ldlt(upload=False) and rbt_solve.  N must be a
+        multiple of 2**depth * v * lcm(PX, PY).  upload=True copies self.data to the device first.  Returns u, the
+        (depth, N) multipliers of U (rbt_multipliers(N, depth, seed)[0]).  COLLECTIVE."""
+        if upload:
+            a = np.ascontiguousarray(self.data, dtype=np.float64)
+            check(lib().cflx_chol_set_local(self._h, a.ctypes.data), "chol_set_local")
+        u = np.empty((int(depth), self.N))
+        check(lib().cflx_chol_rbt(self._h, int(depth), ctypes.c_uint64(int(seed)), u.ctypes.data), "chol_rbt")
+        return u
+
+    def rbt_solve(self, B, refine=True):
+        """Solves A X = B with a factor of a transformed input (rbt, then factor_ldlt): X = U inv(W) U^T B; refine=True
+        refines the transformed system's solution as refine does.  Returns (X, ferr, berr) as lu_rbt_solve.
+        COLLECTIVE; identical on every rank."""
+        B, B2, nrhs = _rhs(self.N, B, "cholesky.rbt_solve")
+        X = np.empty_like(B2)
+        fe, be = np.empty(nrhs), np.empty(nrhs)
+        check(lib().cflx_chol_rbt_solve(self._h, nrhs, B2.ctypes.data, nrhs, X.ctypes.data, nrhs, 1 if refine else 0,
+                                        fe.ctypes.data, be.ctypes.data), "chol_rbt_solve")
+        return X.reshape(B.shape), (fe if refine else None), (be if refine else None)
+
+    def rbt_apply_local(self, op, B_share, nrhs):
+        """U^T (op 0) or U (op 1) of the factor's transform on the rows of this rank's right-hand side share, in place
+        (cflx_chol_rbt_apply_local); B_share as solve_local's.  rbt_apply_local(0, B), solve_local, rbt_apply_local(1, X)
+        solves A X = B distributed.  Not collective.  Returns B_share."""
+        ptr, out, ld = _share_out(B_share, self.Ml, rhs_local_cols(nrhs, self.v, self.PY), "cholesky.rbt_apply_local",
+                                  strided=True, name="B_share")
+        check(lib().cflx_chol_rbt_apply_local(self._h, int(op), int(nrhs), ptr, ld), "chol_rbt_apply_local")
+        return out
+
+    def signs(self):
+        """The signs S (N,) of the last factorisation: factor_ldlt's, all +1 after parallelCholesky."""
+        s = np.empty(self.N)
+        check(lib().cflx_chol_get_signs(self._h, s.ctypes.data), "chol_get_signs")
+        return s
+
+    def local_input(self):
+        """This rank's share of the input as the factorisations read it (after equilibrate(apply) and rbt)."""
+        A = np.empty((self.Ml, self.Nl))
+        check(lib().cflx_chol_get_input(self._h, A.ctypes.data), "chol_get_input")
+        return A
+
     def local_factor(self):
         L = np.empty((self.Ml, self.Nl))
         check(lib().cflx_chol_get_local(self._h, L.ctypes.data), "chol_get_local")
@@ -658,7 +718,8 @@ class cholesky:
 
     def det(self, unscaled=False):
         """det(A) = prod(l_ii)^2 of the padded matrix of the last parallelCholesky on the GPU grid: returns dict(logdet,
-        mantissa, exponent) with det = mantissa * 2**exponent, mantissa in [0.5, 1), as lu_det's pair.  unscaled=True
+        mantissa, exponent) with det = mantissa * 2**exponent, mantissa in [0.5, 1), as lu_det's pair.  After factor_ldlt,
+        det = prod(s_i r_ii^2): the mantissa carries its sign and logdet is log|det|.  unscaled=True
         divides by prod(s)^2 of the scaling the factor carries (equilibrate).  COLLECTIVE; identical on every rank."""
         ld, mant, exp = ctypes.c_double(), ctypes.c_double(), ctypes.c_int64()
         check(lib().cflx_chol_det(self._h, 1 if unscaled else 0, ctypes.byref(ld), ctypes.byref(mant), ctypes.byref(exp)),
@@ -1140,6 +1201,31 @@ class dbg:
         check(lib().cflx_dbg_potrf_tile(v, A.ctypes.data, L.ctypes.data, LT.ctypes.data, ctypes.byref(info), int(variant)),
               "dbg_potrf_tile")
         return L, LT, info.value
+
+    @staticmethod
+    def ldlt_tile(A, tiny=0.0, variant=0):
+        """Signed Cholesky A = R S R^T of one v x v tile (lower triangle read) on factor_ldlt's kernels, variants as
+        potrf_tile.  Returns dict(R, SRT, s, nrepl, inertia, info): SRT = S R^T, s the signs, inertia (positive,
+        negative, zero) pivots, info = 1 + the first exactly zero pivot's column (0: none)."""
+        A = np.ascontiguousarray(A, dtype=np.float64)
+        v = A.shape[0]
+        R, SRT, sg = np.empty((v, v)), np.empty((v, v)), np.empty(v)
+        nrepl, info = ctypes.c_int(), ctypes.c_int()
+        inertia = (ctypes.c_int * 3)()
+        check(lib().cflx_dbg_ldlt_tile(v, A.ctypes.data, float(tiny), R.ctypes.data, SRT.ctypes.data, sg.ctypes.data,
+                                       ctypes.byref(nrepl), inertia, ctypes.byref(info), int(variant)), "dbg_ldlt_tile")
+        return dict(R=R, SRT=SRT, s=sg, nrepl=nrepl.value, inertia=tuple(inertia), info=info.value)
+
+    @staticmethod
+    def solve_signs(Z, sgn, v, grid=(1, 1), pos=(0, 0), M=None):
+        """cflx_dbg_solve_signs: the sign pass of a signed Cholesky solve on the column-partial buffer Z (Nl x ldn) of
+        the share at grid position pos; sgn: the M signs.  Returns the scaled copy."""
+        Z = np.array(Z, dtype=np.float64, order="C")
+        sg = np.ascontiguousarray(sgn, dtype=np.float64)
+        Nl, ldn = Z.shape
+        lay = _share(v, v, Nl, grid, pos, M=M if M is not None else len(sg))
+        check(lib().cflx_dbg_solve_signs(ctypes.byref(lay), int(ldn), sg.ctypes.data, Z.ctypes.data), "dbg_solve_signs")
+        return Z
 
     @staticmethod
     def getrf_nopiv_tile(A, tiny=0.0, variant=0):

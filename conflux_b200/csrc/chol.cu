@@ -22,6 +22,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <numeric>
 
 #include "lu_state.h"
 
@@ -33,8 +34,13 @@ using namespace cflx;
 struct cflx_chol : Handle {
     DevBuf<double> PT, LT, G /* [2] */, Bc /* [2] */, D, A00, W, Uinv, LinvT, acc;
     DevBuf<double> Q;  // scratch of the blocked tile Cholesky
-    DevBuf<int> info;
+    DevBuf<int> info;  // {-, first failing column, its min operand, -, the signed counts (LdltArgs::cnt)}
     int64_t ldp = 0, ldb = 0;
+    // cflx_chol_factor_ldlt: the factor is signed (A = R S R^T), sgn holds S (M doubles, the same on every rank; made by
+    // the first signed factorisation), tiny its pivot rule.  A plain factor has S = I.
+    bool ldlt = false;
+    double tiny = 0.0;
+    DevBuf<double> sgn;
     Events<2> ev_col, ev_panel;
     SubComm j_comm;                  // grid row of one layer (color pi * Pz + pk, key pj), made by the first solve
     ~cflx_chol();  // the handle's device made current, the sub-communicators destroyed, then the members freed
@@ -43,6 +49,25 @@ struct cflx_chol : Handle {
 namespace {
 
 // ---------------------------------------------------------------------------------------------- diagonal tile
+// The signed tile kernels' pivot rule (see potrf_tile_kernel): d, or copysign(tiny, d) (+tiny for +-0) when |d| < tiny;
+// cnt (the one thread that counts, else null) += {replaced, positive, negative, zero}
+__device__ __forceinline__ double ldlt_pivot(double d, double tiny, int* cnt) {
+    const bool rep = fabs(d) < tiny;
+    if (rep) d = d == 0.0 ? tiny : copysign(tiny, d);
+    if (cnt) {
+        cnt[0] += rep;
+        cnt[1] += d > 0.0;
+        cnt[2] += !(d > 0.0) && d != 0.0;
+        cnt[3] += d == 0.0;
+    }
+    return d;
+}
+// the signs of a signed tile kernel's n columns and its counts out of shared memory (after its last __syncthreads)
+__device__ __forceinline__ void ldlt_tile_out(const double* s_sg, const int* s_cnt, int n, const LdltArgs& sa) {
+    __syncthreads();
+    for (int e = threadIdx.x; e < n; e += blockDim.x) sa.sg[e] = s_sg[e];
+    if (threadIdx.x < 4 && s_cnt[threadIdx.x]) atomicAdd(sa.cnt + threadIdx.x, s_cnt[threadIdx.x]);
+}
 // Cholesky of one v x v tile (row-major, lower triangle referenced) by ONE CTA: right-looking, 32-column blocks.
 //   D   in: the tile; out: L in the lower triangle, zeros above
 //   UT  out: L^T (upper triangular, row-major) -- the operand of the panel TRSM and what is broadcast
@@ -50,16 +75,28 @@ namespace {
 // atomicCAS(info, 0, .), so the first failure of a factorisation is kept: after it, NaNs reach every later diagonal
 // block, and each of those fails again.
 constexpr int PB = 32;
+//
+// SIGNED (cflx_chol_factor_ldlt): the signed Cholesky A = R S R^T, S = diag(s), s_c = +-1, with R in D and S R^T (rows of
+// R^T scaled by the signs) in UT and Uc.  Column c's pivot is d = a_cc - sum_{j<c} s_j r_cj^2; |d| < tiny becomes
+// copysign(tiny, d) (+tiny for +-0), counted in sa.cnt[0]; then s_c = +1 for d > 0, else -1, r_cc = sqrt|d| and r_ic =
+// (a_ic - sum_{j<c} r_ij s_j r_cj) / (s_c r_cc).  sa.sg receives the signs; sa.cnt[1..3] count the positive, negative
+// and zero pivots; the failure *info records is an exactly zero d.  On s = +1 every operation is the unsigned one.
+//
 // D: v x v window (leading dimension ldd) of the tile, UT: the same window of L^T (leading dimension ldu); Uc (optional): a
 // contiguous v x v copy of the factored block's L^T; col_off: global column of the window's first column (for *info)
+template <bool SIGNED>
 __global__ void __launch_bounds__(1024) potrf_tile_kernel(double* __restrict__ D, int v, int ldd, double* __restrict__ UT, int ldu,
-                                                          double* __restrict__ Uc, int* __restrict__ info, int col_off) {
+                                                          double* __restrict__ Uc, int* __restrict__ info, int col_off,
+                                                          LdltArgs sa) {
     extern __shared__ double sm[];
     double* Ld = sm;                 // [PB][PB + 1] factored diagonal block
     double* Xs = sm + PB * (PB + 1);  // [v][PB + 1] panel below it
     __shared__ int s_bad;
+    __shared__ double s_sg[SIGNED ? 512 : 1];
+    __shared__ int s_cnt[SIGNED ? 4 : 1];
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
     if (t == 0) s_bad = 0;
+    if (SIGNED && t < 4) s_cnt[t] = 0;
     for (int jb = 0; jb < v; jb += PB) {
         const int nb = min(PB, v - jb), m = v - jb - nb;
         for (int e = t; e < nb * nb; e += blockDim.x) Ld[(e / nb) * (PB + 1) + e % nb] = D[(size_t)(jb + e / nb) * ldd + jb + e % nb];
@@ -71,14 +108,22 @@ __global__ void __launch_bounds__(1024) potrf_tile_kernel(double* __restrict__ D
 #pragma unroll
             for (int c = 0; c < PB; ++c) {
                 if (c < nb) {
-                    const double d = __shfl_sync(0xffffffffu, a[c], c);
-                    if (!(d > 0.0) && lane == 0 && s_bad == 0) s_bad = col_off + jb + c + 1;
-                    const double sq = sqrt(d);
+                    double d = __shfl_sync(0xffffffffu, a[c], c), sgc = 1.0;
+                    if (SIGNED) {
+                        d = ldlt_pivot(d, sa.tiny, lane == 0 ? s_cnt : nullptr);
+                        sgc = d > 0.0 ? 1.0 : -1.0;
+                        if (lane == 0) s_sg[jb + c] = sgc;
+                        if (d == 0.0 && lane == 0 && s_bad == 0) s_bad = col_off + jb + c + 1;
+                    } else if (!(d > 0.0) && lane == 0 && s_bad == 0) {
+                        s_bad = col_off + jb + c + 1;
+                    }
+                    const double sq = SIGNED ? sqrt(fabs(d)) : sqrt(d);
                     if (lane == c) a[c] = sq;
-                    else if (lane > c) a[c] = a[c] / sq;
+                    else if (lane > c) a[c] = a[c] / (SIGNED ? sgc * sq : sq);
 #pragma unroll
                     for (int c2 = c + 1; c2 < PB; ++c2) {
-                        const double l2 = __shfl_sync(0xffffffffu, a[c], c2);  // L[c2][c]
+                        double l2 = __shfl_sync(0xffffffffu, a[c], c2);  // L[c2][c]
+                        if (SIGNED) l2 *= sgc;
                         if (lane >= c2) a[c2] = fma(-a[c], l2, a[c2]);
                     }
                 }
@@ -93,7 +138,7 @@ __global__ void __launch_bounds__(1024) potrf_tile_kernel(double* __restrict__ D
             const int r = e / nb, c = e % nb;
             const double x = Ld[r * (PB + 1) + c];
             D[(size_t)(jb + r) * ldd + jb + c] = x;
-            UT[(size_t)(jb + c) * ldu + jb + r] = x;          // UT[c][r] = L[r][c] (zero for c > r)
+            UT[(size_t)(jb + c) * ldu + jb + r] = SIGNED && c <= r ? s_sg[jb + c] * x : x;  // UT[c][r] = s_c L[r][c] (zero for c > r)
         }
         // panel below: X = P * L_d^-T, one thread per row (forward substitution against the block in shared memory)
         for (int i = t; i < m; i += blockDim.x) {
@@ -106,8 +151,8 @@ __global__ void __launch_bounds__(1024) potrf_tile_kernel(double* __restrict__ D
                 if (c < nb) {
                     double s = x[c];
 #pragma unroll
-                    for (int q = 0; q < c; ++q) s = fma(-x[q], Ld[c * (PB + 1) + q], s);
-                    x[c] = s / Ld[c * (PB + 1) + c];
+                    for (int q = 0; q < c; ++q) s = fma(-x[q], SIGNED ? s_sg[jb + q] * Ld[c * (PB + 1) + q] : Ld[c * (PB + 1) + q], s);
+                    x[c] = s / (SIGNED ? s_sg[jb + c] * Ld[c * (PB + 1) + c] : Ld[c * (PB + 1) + c]);
                 }
             }
 #pragma unroll
@@ -115,7 +160,7 @@ __global__ void __launch_bounds__(1024) potrf_tile_kernel(double* __restrict__ D
                 if (c < nb) {
                     prow[c] = x[c];
                     Xs[i * (PB + 1) + c] = x[c];
-                    UT[(size_t)(jb + c) * ldu + jb + nb + i] = x[c];   // L^T
+                    UT[(size_t)(jb + c) * ldu + jb + nb + i] = SIGNED ? s_sg[jb + c] * x[c] : x[c];   // L^T (S R^T)
                 }
             }
         }
@@ -142,7 +187,8 @@ __global__ void __launch_bounds__(1024) potrf_tile_kernel(double* __restrict__ D
                     if (i < m && j < m && j <= i) {
                         double s = 0.0;
 #pragma unroll
-                        for (int c = 0; c < PB; ++c) s = fma(Xs[i * (PB + 1) + c], Xs[j * (PB + 1) + c], s);
+                        for (int c = 0; c < PB; ++c)
+                            s = fma(Xs[i * (PB + 1) + c], SIGNED ? s_sg[jb + c] * Xs[j * (PB + 1) + c] : Xs[j * (PB + 1) + c], s);
                         tv[q] -= s;
                     }
                 }
@@ -167,6 +213,7 @@ __global__ void __launch_bounds__(1024) potrf_tile_kernel(double* __restrict__ D
         __syncthreads();
         for (int e = t; e < v * v; e += blockDim.x) Uc[e] = UT[(size_t)(e / v) * ldu + e % v];
     }
+    if (SIGNED) ldlt_tile_out(s_sg, s_cnt, v, sa);
     if (t == 0 && s_bad) atomicCAS(info, 0, s_bad);
 }
 
@@ -177,12 +224,18 @@ __global__ void __launch_bounds__(1024) potrf_tile_kernel(double* __restrict__ D
 constexpr int QBK = 128;
 constexpr int QPITCH = QBK + 1;
 constexpr int QTHREADS = 512;
+// SIGNED: the signed Cholesky of the block, as potrf_tile_kernel's.
+template <bool SIGNED>
 __global__ void __launch_bounds__(QTHREADS) potrf128_kernel(double* __restrict__ D, int ldd, double* __restrict__ UT, int ldu,
-                                                        double* __restrict__ Uc, int* __restrict__ info, int col_off) {
+                                                        double* __restrict__ Uc, int* __restrict__ info, int col_off,
+                                                        LdltArgs sa) {
     extern __shared__ double As[];  // [QBK][QPITCH], lower triangle
     __shared__ int s_bad;
+    __shared__ double s_sg[SIGNED ? QBK : 1];
+    __shared__ int s_cnt[SIGNED ? 4 : 1];
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
     if (t == 0) s_bad = 0;
+    if (SIGNED && t < 4) s_cnt[t] = 0;
     for (int e = t; e < QBK * QBK; e += QTHREADS) {
         const int r = e / QBK, c = e % QBK;
         As[r * QPITCH + c] = (c <= r) ? D[(size_t)r * ldd + c] : 0.0;
@@ -194,19 +247,26 @@ __global__ void __launch_bounds__(QTHREADS) potrf128_kernel(double* __restrict__
                           // indexed by the unrolled column loop ends up in local memory, which is what made the old kernel slow)
             double* B = As + jb * QPITCH + jb;
             for (int c = 0; c < PB; ++c) {
-                const double d = B[c * QPITCH + c];
-                if (!(d > 0.0) && lane == 0 && s_bad == 0) s_bad = col_off + jb + c + 1;
-                const double sq = sqrt(d);
+                double d = B[c * QPITCH + c], sgc = 1.0;
+                if (SIGNED) {
+                    d = ldlt_pivot(d, sa.tiny, lane == 0 ? s_cnt : nullptr);
+                    sgc = d > 0.0 ? 1.0 : -1.0;
+                    if (lane == 0) s_sg[jb + c] = sgc;
+                    if (d == 0.0 && lane == 0 && s_bad == 0) s_bad = col_off + jb + c + 1;
+                } else if (!(d > 0.0) && lane == 0 && s_bad == 0) {
+                    s_bad = col_off + jb + c + 1;
+                }
+                const double sq = SIGNED ? sqrt(fabs(d)) : sqrt(d);
                 double l = 0.0;
                 if (lane == c) B[c * QPITCH + c] = sq;
                 else if (lane > c) {
-                    l = B[lane * QPITCH + c] / sq;
+                    l = B[lane * QPITCH + c] / (SIGNED ? sgc * sq : sq);
                     B[lane * QPITCH + c] = l;
                 }
                 __syncwarp();
 #pragma unroll 4
                 for (int c2 = c + 1; c2 < PB; ++c2) {
-                    const double l2 = B[c2 * QPITCH + c];  // L[c2][c], broadcast
+                    const double l2 = SIGNED ? sgc * B[c2 * QPITCH + c] : B[c2 * QPITCH + c];  // (s_c) L[c2][c], broadcast
                     if (lane >= c2) B[lane * QPITCH + c2] = fma(-l, l2, B[lane * QPITCH + c2]);
                 }
                 __syncwarp();
@@ -221,12 +281,17 @@ __global__ void __launch_bounds__(QTHREADS) potrf128_kernel(double* __restrict__
 #pragma unroll 4
             for (int c = 0; c < PB; ++c) {
                 double sacc = prow[c];
-                for (int q = 0; q < c; ++q) sacc = fma(-prow[q], Ld[c * QPITCH + q], sacc);
-                prow[c] = sacc / Ld[c * QPITCH + c];
+                for (int q = 0; q < c; ++q) sacc = fma(-prow[q], SIGNED ? s_sg[jb + q] * Ld[c * QPITCH + q] : Ld[c * QPITCH + q], sacc);
+                prow[c] = sacc / (SIGNED ? s_sg[jb + c] * Ld[c * QPITCH + c] : Ld[c * QPITCH + c]);
             }
         }
         __syncthreads();
-        // trailing part (lower triangle): T[i][k] -= X[i][:] . X[k][:], one element per thread and pass
+        // trailing part (lower triangle): T[i][k] -= X[i][:] . X[k][:], one element per thread and pass (signed: the
+        // block's signs held in registers)
+        double sgr[SIGNED ? PB : 1];
+        if (SIGNED)
+#pragma unroll
+            for (int c = 0; c < PB; ++c) sgr[c] = s_sg[jb + c];
         for (int e = t; e < m * m; e += QTHREADS) {
             const int i = e / m, k = e % m;
             if (k > i) continue;
@@ -234,7 +299,7 @@ __global__ void __launch_bounds__(QTHREADS) potrf128_kernel(double* __restrict__
             const double* xk = As + (jb + PB + k) * QPITCH + jb;
             double sacc = 0.0;
 #pragma unroll
-            for (int c = 0; c < PB; ++c) sacc = fma(xi[c], xk[c], sacc);
+            for (int c = 0; c < PB; ++c) sacc = fma(xi[c], SIGNED ? sgr[c] * xk[c] : xk[c], sacc);
             As[(jb + PB + i) * QPITCH + jb + PB + k] -= sacc;
         }
         __syncthreads();
@@ -243,13 +308,20 @@ __global__ void __launch_bounds__(QTHREADS) potrf128_kernel(double* __restrict__
     for (int e = t; e < QBK * QBK; e += QTHREADS) {
         const int r = e / QBK, c = e % QBK;
         D[(size_t)r * ldd + c] = As[r * QPITCH + c];            // (zeros above the diagonal were loaded as zeros)
-        const double lt = As[c * QPITCH + r];                    // L^T[r][c] = L[c][r]
+        const double lt = SIGNED && c >= r ? s_sg[r] * As[c * QPITCH + r] : As[c * QPITCH + r];  // (s_r) L^T[r][c] = L[c][r]
         UT[(size_t)r * ldu + c] = lt;
         Uc[e] = lt;
     }
+    if (SIGNED) ldlt_tile_out(s_sg, s_cnt, QBK, sa);
     if (t == 0 && s_bad) atomicCAS(info, 0, s_bad);
 }
 
+// out[r][x] = sg[r] X[r][x] for x < n (both leading dimension ld): a row r per blockIdx.y
+__global__ void row_signs_kernel(const double* __restrict__ X, int64_t ld, int n, const double* __restrict__ sg,
+                                 double* __restrict__ out) {
+    const int x = blockIdx.x * blockDim.x + threadIdx.x, r = blockIdx.y;
+    if (x < n) out[(int64_t)r * ld + x] = sg[r] * X[(int64_t)r * ld + x];
+}
 // zeros above the diagonal of D (= L) and below the diagonal of UT (= L^T)
 __global__ void tri_clean_kernel(double* __restrict__ D, double* __restrict__ UT, int v) {
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
@@ -277,7 +349,10 @@ struct GatherArgs {
     double* Bc;
     int64_t ldb;
     int v, Px, Py, pj, lj0, ntiles, gfirst, Ml;
+    const double* sg;      // the v signs of the step (signed update), or null
 };
+// SIGNED: Bc's row c times a.sg[c], the sign of contraction index c (S_k R_jk^T of the signed update)
+template <bool SIGNED>
 __global__ void gather_cols_kernel(GatherArgs a) {
     const int t = blockIdx.x, c = blockIdx.y;
     const int j = (a.lj0 + t) * a.Py + a.pj;            // global tile index of this local column tile
@@ -288,7 +363,12 @@ __global__ void gather_cols_kernel(GatherArgs a) {
     const int64_t ldg = max(2, (rows + 1) & ~1);
     const double* src = a.G + (int64_t)p * a.piece_stride + (int64_t)c * ldg + (int64_t)(j / a.Px - first) * a.v;
     double* dst = a.Bc + (int64_t)c * a.ldb + (int64_t)t * a.v;
-    for (int x = threadIdx.x; x < a.v; x += blockDim.x) dst[x] = src[x];
+    if (SIGNED) {
+        const double sg = a.sg[c];
+        for (int x = threadIdx.x; x < a.v; x += blockDim.x) dst[x] = sg * src[x];
+    } else {
+        for (int x = threadIdx.x; x < a.v; x += blockDim.x) dst[x] = src[x];
+    }
 }
 // sum of squares of the lower triangle of the real tiles (global row >= global column, global row < Nt v: the column
 // is then below that bound too) of a local block-cyclic array: partials[blockIdx.x] = this CTA's share;
@@ -349,30 +429,40 @@ int chol_pick_nb(int v) {
 int piece_ld(const cflx_chol* ch, int gfirst, int p) { return chol_piece_ld(*ch, gfirst, p); }
 // Broadcast the Px pieces of the (transposed) panel of column block t (rows of global tiles >= gfirst) to every rank into
 // buffer set `buf`, and assemble the column operand for the local column tiles with global index >= jmin.
-int broadcast_pieces(cflx_chol* ch, int t, int gfirst, int jmin, int buf, cudaStream_t s) {
+// carry_signs (the signed factorisation): the diagonal owner's piece also carries the step's v signs, written after
+// its v ld_p values (the owner put them there), and every rank copies them into its sign vector.  The gather applies the
+// signs whenever the factor is signed.
+int broadcast_pieces(cflx_chol* ch, int t, int gfirst, int jmin, int buf, cudaStream_t s, bool carry_signs = false) {
     const int v = ch->v, Px = ch->Px, Py = ch->Py, Pz = ch->Pz, Ml = ch->Ml, Nl = ch->Nl;
     const int pjt = t % Py;
     const int64_t piece_stride = (int64_t)v * ch->ldp;
     double* G = ch->G + (int64_t)buf * Px * piece_stride;
     double* Bc = ch->Bc + (int64_t)buf * v * ch->ldb;
     if (ch->P > 1) {
+        const int pd = t % Px;
         CFLX_NCCL(ncclGroupStart());
         for (int p = 0; p < Px; ++p) {
             const int rows = Ml - first_local_tile(gfirst, p, Px) * v;
-            if (rows <= 0) continue;
+            const bool signs = carry_signs && p == pd;
+            if (rows <= 0 && !signs) continue;
             const int root = (p * Py + pjt) * Pz;
             double* dst = G + (int64_t)p * piece_stride;
             const double* src = (ch->rank == root) ? ch->LT : dst;
-            CFLX_NCCL(ncclBroadcast(src, dst, (size_t)v * piece_ld(ch, gfirst, p), ncclDouble, root, ch->comm->world, s));
+            CFLX_NCCL(ncclBroadcast(src, dst, (size_t)v * (piece_ld(ch, gfirst, p) + signs), ncclDouble, root,
+                                    ch->comm->world, s));
         }
         CFLX_NCCL(ncclGroupEnd());
+        if (carry_signs)
+            CFLX_CUDA(cudaMemcpyAsync(ch->sgn + (int64_t)t * v, G + (int64_t)pd * piece_stride + (int64_t)v * piece_ld(ch, gfirst, pd),
+                                      (size_t)v * sizeof(double), cudaMemcpyDeviceToDevice, s));
     } else {
         CFLX_CUDA(cudaMemcpyAsync(G, ch->LT, (size_t)v * piece_ld(ch, gfirst, 0) * sizeof(double), cudaMemcpyDeviceToDevice, s));
     }
     const int lj0 = first_local_tile(jmin, ch->pj, Py);
     const int ntc = Nl / v - lj0;
     if (ntc <= 0) return CFLX_OK;
-    CFLX_TRY(launch_gather_cols(G, piece_stride, Bc, ch->ldb, v, Px, Py, ch->pj, lj0, ntc, gfirst, Ml, s));
+    CFLX_TRY(launch_gather_cols(G, piece_stride, Bc, ch->ldb, v, Px, Py, ch->pj, lj0, ntc, gfirst, Ml, s,
+                                ch->ldlt ? ch->sgn + (int64_t)t * v : nullptr));
     ch->launches++;
     return CFLX_OK;
 }
@@ -465,16 +555,26 @@ size_t potrf_tile_scratch(int v) { return (v % QBK == 0 && v >= 2 * QBK) ? (size
 int potrf_setup(int v) {
     static PerDeviceMax tile_cfg, blk_cfg;
     CFLX_CUDA(tile_cfg.raise(potrf_tile_smem(v), [&] {
-        return cudaFuncSetAttribute(potrf_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)potrf_tile_smem(v));
+        cudaError_t e = cudaFuncSetAttribute(potrf_tile_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)potrf_tile_smem(v));
+        if (e == cudaSuccess)
+            e = cudaFuncSetAttribute(potrf_tile_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)potrf_tile_smem(v));
+        return e;
     }));
     CFLX_CUDA(blk_cfg.raise(QBK * QPITCH * sizeof(double), [&] {
-        return cudaFuncSetAttribute(potrf128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(QBK * QPITCH * sizeof(double)));
+        cudaError_t e = cudaFuncSetAttribute(potrf128_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(QBK * QPITCH * sizeof(double)));
+        if (e == cudaSuccess)
+            e = cudaFuncSetAttribute(potrf128_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(QBK * QPITCH * sizeof(double)));
+        return e;
     }));
     return CFLX_OK;
 }
 
-int potrf_block128(double* D, int ldd, double* UT, int ldu, double* Uc, int* info, int col0, cudaStream_t s) {
-    potrf128_kernel<<<1, QTHREADS, QBK * QPITCH * sizeof(double), s>>>(D, ldd, UT, ldu, Uc, info, col0);
+int potrf_block128(double* D, int ldd, double* UT, int ldu, double* Uc, int* info, int col0, cudaStream_t s,
+                   const LdltArgs* sa) {
+    if (sa)
+        potrf128_kernel<true><<<1, QTHREADS, QBK * QPITCH * sizeof(double), s>>>(D, ldd, UT, ldu, Uc, info, col0, *sa);
+    else
+        potrf128_kernel<false><<<1, QTHREADS, QBK * QPITCH * sizeof(double), s>>>(D, ldd, UT, ldu, Uc, info, col0, LdltArgs{});
     CFLX_CUDA(cudaGetLastError());
     return CFLX_OK;
 }
@@ -483,10 +583,14 @@ int potrf_block128(double* D, int ldd, double* UT, int ldu, double* Uc, int* inf
 // the critical path of every step), so the tile is itself factored in 128-wide block columns: the 128 x 128 diagonal block on one CTA, the
 // block column below it by ONE GEMM with the inverted block, the trailing part of the tile by one rank-128 GEMM -- both on
 // the whole GPU (FP64 DMMA kernel).  Tiles that are not a multiple of 128 (tests), or Q == nullptr, keep the one-CTA kernel.
-int potrf_tile(double* D, double* A00, double* Q, int* info, int col0, int v, cudaStream_t s, int64_t* launches) {
+// With sa, the signed Cholesky (potrf_tile_kernel): block jb's signs go to sa->sg + jb, and the rank-128 update of the
+// trailing part is T -= X S X^T, its second operand (and A00's copy of the block column) S X^T.
+int potrf_tile(double* D, double* A00, double* Q, int* info, int col0, int v, cudaStream_t s, int64_t* launches,
+               const LdltArgs* sa) {
     constexpr int QB = 128;
     if (v % QB != 0 || v < 2 * QB || Q == nullptr) {
-        potrf_tile_kernel<<<1, 1024, potrf_tile_smem(v), s>>>(D, v, v, A00, v, nullptr, info, col0);
+        if (sa) potrf_tile_kernel<true><<<1, 1024, potrf_tile_smem(v), s>>>(D, v, v, A00, v, nullptr, info, col0, *sa);
+        else potrf_tile_kernel<false><<<1, 1024, potrf_tile_smem(v), s>>>(D, v, v, A00, v, nullptr, info, col0, LdltArgs{});
         CFLX_CUDA(cudaGetLastError());
         return CFLX_OK;
     }
@@ -498,20 +602,30 @@ int potrf_tile(double* D, double* A00, double* Q, int* info, int col0, int v, cu
     static_assert(QB == QBK, "block width of the tile Cholesky");
     for (int jb = 0; jb < v; jb += QB) {
         const int m = v - jb - QB;
-        CFLX_TRY(potrf_block128(D + (size_t)jb * v + jb, v, A00 + (size_t)jb * v + jb, v, U128, info, col0 + jb, s));
+        LdltArgs sb{};
+        if (sa) sb = LdltArgs{sa->tiny, sa->sg + jb, sa->cnt};
+        CFLX_TRY(potrf_block128(D + (size_t)jb * v + jb, v, A00 + (size_t)jb * v + jb, v, U128, info, col0 + jb, s,
+                                sa ? &sb : nullptr));
         ++*launches;
         if (m <= 0) break;
         const int64_t ldx = m;
         CFLX_TRY(launch_extract_panel_T(D, v, jb + QB, jb, m, QB, XT0, ldx, s));
         CFLX_TRY(launch_diag_inverses(U128, QB, QB, Ui, Li, s));
-        CFLX_TRY(trsm_right_upper_T(U128, Ui, QB, QB, XT0, XT, ldx, m, s));          // X^T = L_d^-1 P^T
+        CFLX_TRY(trsm_right_upper_T(U128, Ui, QB, QB, XT0, XT, ldx, m, s));          // X^T = L_d^-1 P^T (signed: S R_d^T)
         CFLX_TRY(launch_store_panel_T(D, v, jb + QB, jb, m, QB, XT, ldx, s));
-        CFLX_CUDA(cudaMemcpy2DAsync(A00 + (size_t)jb * v + jb + QB, (size_t)v * sizeof(double), XT, ldx * sizeof(double),
+        const double* XS = XT;                                                        // S X^T (X^T unsigned)
+        if (sa) {
+            row_signs_kernel<<<dim3((m + 255) / 256, QB), 256, 0, s>>>(XT, ldx, m, sb.sg, XT0);
+            CFLX_CUDA(cudaGetLastError());
+            ++*launches;
+            XS = XT0;
+        }
+        CFLX_CUDA(cudaMemcpy2DAsync(A00 + (size_t)jb * v + jb + QB, (size_t)v * sizeof(double), XS, ldx * sizeof(double),
                                     (size_t)m * sizeof(double), QB, cudaMemcpyDeviceToDevice, s));
-        GemmArgs g{};                                                                 // T -= X X^T
+        GemmArgs g{};                                                                 // T -= X X^T (X S X^T)
         g.M = m; g.N = m; g.K = QB;
         g.AT = XT; g.ldat = ldx;
-        g.B = XT; g.ldb = ldx;
+        g.B = XS; g.ldb = ldx;
         g.C = D + (size_t)(jb + QB) * v + jb + QB; g.ldc = v;
         g.D = D + (size_t)(jb + QB) * v + jb + QB; g.ldd = v;
         g.alpha = -1.0; g.beta = 1.0;
@@ -525,9 +639,10 @@ int potrf_tile(double* D, double* A00, double* Q, int* info, int col0, int v, cu
 }
 
 int launch_gather_cols(const double* G, int64_t piece_stride, double* Bc, int64_t ldb, int v, int Px, int Py, int pj,
-                       int lj0, int ntiles, int gfirst, int Ml, cudaStream_t s) {
-    GatherArgs ga{G, piece_stride, Bc, ldb, v, Px, Py, pj, lj0, ntiles, gfirst, Ml};
-    gather_cols_kernel<<<dim3(ntiles, v), 128, 0, s>>>(ga);
+                       int lj0, int ntiles, int gfirst, int Ml, cudaStream_t s, const double* sg) {
+    GatherArgs ga{G, piece_stride, Bc, ldb, v, Px, Py, pj, lj0, ntiles, gfirst, Ml, sg};
+    if (sg) gather_cols_kernel<true><<<dim3(ntiles, v), 128, 0, s>>>(ga);
+    else gather_cols_kernel<false><<<dim3(ntiles, v), 128, 0, s>>>(ga);
     CFLX_CUDA(cudaGetLastError());
     return CFLX_OK;
 }
@@ -572,7 +687,8 @@ int panel_step(cflx_chol* ch, int k, cudaStream_t s) {
     // (1) Cholesky of the diagonal tile                                                 Cholesky.cpp:188-193
     if (owner) {
         tile_from_panel_kernel<<<(v * v + 255) / 256, 256, 0, s>>>(ch->PT, ld, v, ch->D);
-        CFLX_TRY(potrf_tile(ch->D, ch->A00, ch->Q, ch->info + 1, k * v, v, s, &ch->launches));
+        const LdltArgs sa{ch->tiny, ch->sgn + (int64_t)k * v, ch->info + 4};
+        CFLX_TRY(potrf_tile(ch->D, ch->A00, ch->Q, ch->info + 1, k * v, v, s, &ch->launches, ch->ldlt ? &sa : nullptr));
         tile_store_kernel<<<(v * v + 255) / 256, 256, 0, s>>>(ch->D, v, ch->A11 + (int64_t)row0 * Nl + loff, Nl);
         CFLX_CUDA(cudaGetLastError());
         ch->launches += 3;
@@ -592,8 +708,12 @@ int panel_step(cflx_chol* ch, int k, cudaStream_t s) {
         CFLX_TRY(launch_store_panel_T(ch->A11, Nl, row1, loff, n1, v, ch->LT, ld1, s));
         ch->launches += 2 * (v / ch->nb) + 1;
     }
+    // the signs of step k ride on the owner's piece (after its v ld1 values)
+    if (owner && ch->ldlt && ch->P > 1)
+        CFLX_CUDA(cudaMemcpyAsync(ch->LT + (int64_t)v * ld1, ch->sgn + (int64_t)k * v, (size_t)v * sizeof(double),
+                                  cudaMemcpyDeviceToDevice, s));
     // the reference's A10 -> A01 representative exchange                                 Cholesky.cpp:205-330
-    return broadcast_pieces(ch, k, k + 1, k + 1, k & 1, s);
+    return broadcast_pieces(ch, k, k + 1, k + 1, k & 1, s, ch->ldlt);
 }
 
 // ---------------------------------------------------------------------------------------------- solve, A X = B
@@ -604,7 +724,8 @@ int panel_step(cflx_chol* ch, int k, cudaStream_t s) {
 // local column t / Py of Z), then its column-partial sweep L^T X = Y.  The grid row and column are those of layer 0
 // (j_comm / i_comm, one layer each); the layers pk != 0 only join the final all-reduce.
 SolveFactor chol_solve_factor(cflx_chol* ch) {
-    return SolveFactor{*ch, ch->A11, first_local_tile(ch->Nt, ch->pi, ch->Px) * ch->v, &ch->j_comm, &ch->i_comm, 1};
+    return SolveFactor{*ch, ch->A11, first_local_tile(ch->Nt, ch->pi, ch->Px) * ch->v, &ch->j_comm, &ch->i_comm, 1,
+                       ch->ldlt ? ch->sgn.p : nullptr};
 }
 
 // First call after a factorisation: the grid-row communicator (once per object), the inverses of the nb x nb diagonal
@@ -634,8 +755,9 @@ int chol_sweeps(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X, in
     const int ldn = (int)round_up(nrhs, 8);
     CFLX_TRY(solve_cache_grow(sc, f, ldn, ch->pk == 0, true));
     CFLX_TRY(solve_seed(sc, f, ldn, nrhs, B, ldb, SolveSeed{false, sc->rows, f.rows, sc->W}));
-    if (ch->pk == 0) {  // L Y = B keeping Y_t in Z, then L^T X = Y from Z
+    if (ch->pk == 0) {  // L Y = B keeping Y_t in Z, then L^T X = Y from Z (signed: R Y = B, R^T X = S Y)
         CFLX_TRY(solve_row_sweep(sc, f, ldn, true, sc->Z, ch->Py, false));
+        CFLX_TRY(solve_apply_signs(sc, f, ldn));
         CFLX_TRY(solve_col_sweep(sc, f, ldn, false, Tri::LowerT, sc->X, 1, false));
     }
     return solve_finish(sc, f, ldn, nrhs, X, ldx);
@@ -675,6 +797,11 @@ int chol_equilibrate(const char* who, cflx_chol* ch, int apply, bool pow2, doubl
     REFUSE_FOR(who, !ch);
     REFUSE_FOR(who, apply != 0 && apply != 1);
     REFUSE_FOR(who, !info_out);
+    if (apply && ch->rbt.in.depth) {
+        set_last_error("%s: refused, the input carries a random butterfly transform (cflx_chol_rbt); upload it again first",
+                       who);
+        return CFLX_ERR_STATE;
+    }
     CFLX_TRY(enter(ch, who, NEED_INPUT | (apply ? NEED_UNSCALED : 0u)));
     handle_equil_begin(ch);
     double scond = 0.0, amax = 0.0;
@@ -686,6 +813,25 @@ int chol_equilibrate(const char* who, cflx_chol* ch, int apply, bool pow2, doubl
     if (amax_out) *amax_out = amax;
     if (equed_out) *equed_out = equed;
     *info_out = info;
+    return CFLX_OK;
+}
+
+// The checks of cflx_chol_rbt (`who`) that need no other rank: the rows pair within a rank when 2^d v Px divides N,
+// the columns when 2^d v Py does
+int chol_rbt_prepare(const char* who, cflx_chol* ch, int depth) {
+    REFUSE_FOR(who, depth < 1);
+    REFUSE_FOR(who, depth > 4);
+    if (ch->rbt.in.depth) {
+        set_last_error("%s: refused, the input is already transformed; upload it again first", who);
+        return CFLX_ERR_STATE;
+    }
+    CFLX_TRY(enter(ch, who, NEED_INPUT | NEED_UNSCALED));
+    const long long q = ((long long)ch->v * std::lcm(ch->Px, ch->Py)) << depth;
+    if (ch->M % q) {
+        set_last_error("%s: N = %d is not a multiple of 2^%d v lcm(Px, Py) = %lld; the smallest N that works is %lld: "
+                       "pad A with the identity to that order", who, ch->M, depth, q, (ch->M + q - 1) / q * q);
+        return CFLX_ERR_UNSUPPORTED;
+    }
     return CFLX_OK;
 }
 
@@ -824,7 +970,7 @@ int cflx_chol_create(cflx_comm* c, int N, int v, int Px, int Py, int Pz, cflx_ch
     CFLX_TRY(ch->W.alloc((size_t)v * ch->ldp)); CFLX_TRY(ch->G.alloc(2 * (size_t)Px * v * ch->ldp));
     CFLX_TRY(ch->Bc.alloc(2 * (size_t)v * ch->ldb)); CFLX_TRY(ch->D.alloc(vv)); CFLX_TRY(ch->A00.alloc(vv));
     CFLX_TRY(ch->Uinv.alloc(vv)); CFLX_TRY(ch->LinvT.alloc(vv)); CFLX_TRY(ch->acc.alloc(2 + SUMSQ_PARTIALS));
-    CFLX_TRY(ch->info.alloc(4));
+    CFLX_TRY(ch->info.alloc(8));
     if (potrf_tile_scratch(v)) CFLX_TRY(ch->Q.alloc(potrf_tile_scratch(v)));
     cudaMemsetAsync(ch->PT, 0, (size_t)v * ch->ldp * sizeof(double), c->stream);
     cudaMemsetAsync(ch->LT, 0, (size_t)v * ch->ldp * sizeof(double), c->stream);
@@ -857,21 +1003,33 @@ int cflx_chol_set_local(cflx_chol* ch, const double* host_local) {
     REFUSE_IF(!ch);
     REFUSE_IF(!host_local);
     CFLX_TRY(enter(ch, __func__, 0));
-    return handle_set_local(ch, host_local);
+    CFLX_TRY(handle_set_local(ch, host_local));
+    ch->rbt.in.depth = 0;
+    return CFLX_OK;
 }
 
-// COLLECTIVE.  parallelCholesky() (Cholesky.cpp:760-921): ms_out = device time of the factorisation loop.
-int cflx_chol_factor(cflx_chol* ch, double* ms_out) {
-    REFUSE_IF(!ch);
-    CFLX_TRY(enter(ch, __func__, NEED_INPUT));
+}  // extern "C"
+
+namespace {
+// The factorisation both entry points share (COLLECTIVE), ch->ldlt choosing the signed one: the working copy of the
+// input, the look-ahead loop, then *bad = 1 + the first failing column over the grid (0: none), the same on every rank.
+// Signed, the last tile's signs (never broadcast) and the counts join the all-reduce of the first failure, into ch->sgn
+// and cnt[4].  *ms = device time of the loop.
+int chol_factor_run(cflx_chol* ch, float* ms_out, int* bad_out, int* cnt) {
     cflx_comm* c = ch->comm;
     cudaStream_t s = c->stream;
     ch->sv.ready = false;
-    CFLX_TRY(equil_pass_on(&ch->eq, ch->M, false, s));  // the factor carries the input's scaling
+    ch->factored = false;
+    CFLX_TRY(equil_pass_on(&ch->eq, ch->M, false, s));  // the factor carries the input's scaling and transform
+    CFLX_TRY(rbt_pass_on(&ch->rbt, ch->M, false, s));
     const int v = ch->v, Py = ch->Py, Ml = ch->Ml, Nl = ch->Nl;
     const int pj = ch->pj;
     CFLX_CUDA(cudaMemcpyAsync(ch->A11, ch->A0, (size_t)Ml * Nl * sizeof(double), cudaMemcpyDeviceToDevice, s));
-    CFLX_CUDA(cudaMemsetAsync(ch->info, 0, sizeof(int) * 4, s));
+    CFLX_CUDA(cudaMemsetAsync(ch->info, 0, sizeof(int) * 8, s));
+    if (ch->ldlt) {
+        CFLX_TRY(ch->sgn.grow(ch->M));
+        CFLX_CUDA(cudaMemsetAsync(ch->sgn, 0, sizeof(double) * ch->M, s));  // the last tile's signs are summed
+    }
     CFLX_TRY(grid_barrier(c));
     Events<2> loop;
     CFLX_TRY(loop.create());
@@ -903,7 +1061,7 @@ int cflx_chol_factor(cflx_chol* ch, double* ms_out) {
     float ms = 0;
     CFLX_CUDA(cudaEventElapsedTime(&ms, loop[0], loop[1]));
     CFLX_CUDA(cudaGetLastError());
-    int h[4] = {0, 0, 0, 0};
+    int h[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     CFLX_CUDA(cudaMemcpy(h, ch->info, sizeof(h), cudaMemcpyDeviceToHost));
     int bad = h[1];   // 1 + first failing global column of the diagonal tiles this rank factored, 0 = none
     if (ch->P > 1) {  // the first one over the grid, so that every rank returns the same status and column
@@ -911,18 +1069,67 @@ int cflx_chol_factor(cflx_chol* ch, double* ms_out) {
         // the factorisation, so it is not counted)
         info_min_operand_kernel<<<1, 1, 0, s>>>(ch->info);
         CFLX_CUDA(cudaGetLastError());
+        if (ch->ldlt) CFLX_NCCL(ncclGroupStart());
         CFLX_NCCL(ncclAllReduce(ch->info + 2, ch->info + 2, 1, ncclInt, ncclMin, c->world, s));
-        int x = 0;
-        CFLX_CUDA(cudaMemcpyAsync(&x, ch->info + 2, sizeof(int), cudaMemcpyDeviceToHost, s));
+        if (ch->ldlt) {  // one owner contributes each sign and each count
+            double* last = ch->sgn + (int64_t)(ch->Nt - 1) * v;
+            CFLX_NCCL(ncclAllReduce(ch->info + 4, ch->info + 4, 4, ncclInt, ncclSum, c->world, s));
+            CFLX_NCCL(ncclAllReduce(last, last, v, ncclDouble, ncclSum, c->world, s));
+            CFLX_NCCL(ncclGroupEnd());
+        }
+        CFLX_CUDA(cudaMemcpyAsync(h, ch->info, sizeof(h), cudaMemcpyDeviceToHost, s));
         CFLX_CUDA(cudaStreamSynchronize(s));
-        bad = x == INT_MAX ? 0 : x;
+        bad = h[2] == INT_MAX ? 0 : h[2];
     }
+    *bad_out = bad;
+    if (cnt) std::memcpy(cnt, h + 4, 4 * sizeof(int));
+    *ms_out = ms;
+    return CFLX_OK;
+}
+}  // namespace
+
+extern "C" {
+
+// COLLECTIVE.  parallelCholesky() (Cholesky.cpp:760-921): ms_out = device time of the factorisation loop.
+int cflx_chol_factor(cflx_chol* ch, double* ms_out) {
+    REFUSE_IF(!ch);
+    CFLX_TRY(enter(ch, __func__, NEED_INPUT));
+    ch->ldlt = false;
+    float ms = 0;
+    int bad = 0;
+    CFLX_TRY(chol_factor_run(ch, &ms, &bad, nullptr));
     if (bad != 0) {
         set_last_error("%s: the matrix is not positive definite (first non-positive pivot in column %d, counted from 1 like LAPACK dpotrf's info)", __func__, bad);
         return CFLX_ERR_STATE;
     }
     if (ms_out) *ms_out = ms;
     ch->factored = true;
+    return CFLX_OK;
+}
+
+// COLLECTIVE.  The signed Cholesky A = R S R^T without pivoting (chol_factor_run with ch->ldlt): the factorisation
+// completes whatever its pivots; the counts of every rank's diagonal tiles and the first zero pivot come back the same on
+// every rank.
+int cflx_chol_factor_ldlt(cflx_chol* ch, double tiny, int* nrepl_out, int64_t* inertia_out, int* info_out, double* ms_out) {
+    REFUSE_IF(!ch);
+    REFUSE_IF(!(tiny >= 0.0));
+    REFUSE_IF(!info_out);
+    CFLX_TRY(enter(ch, __func__, NEED_INPUT));
+    ch->ldlt = true;
+    ch->tiny = tiny;
+    float ms = 0;
+    int bad = 0, cnt[4] = {0, 0, 0, 0};
+    const int rc = chol_factor_run(ch, &ms, &bad, cnt);
+    if (rc != CFLX_OK) {
+        ch->ldlt = false;
+        return rc;
+    }
+    ch->factored = true;
+    if (nrepl_out) *nrepl_out = cnt[0];
+    if (inertia_out)
+        for (int i = 0; i < 3; ++i) inertia_out[i] = cnt[1 + i];
+    *info_out = bad;
+    if (ms_out) *ms_out = ms;
     return CFLX_OK;
 }
 
@@ -1044,6 +1251,11 @@ int cflx_chol_det(cflx_chol* ch, int unscaled, double* logdet_out, double* mant_
     const double* s = unscaled && ch->eq.fac.equed == 'Y' ? ch->eq.fac.r.p : nullptr;
     DetResult d{};
     CFLX_TRY(det_grid(*ch, &ch->eq, ch->A11, true, s, nullptr, &d));
+    if (ch->ldlt) {  // det = prod(s_i) prod(r_ii)^2: the sign is the parity of the negative signs
+        std::vector<double> sg(ch->M);
+        CFLX_CUDA(cudaMemcpy(sg.data(), ch->sgn, sizeof(double) * ch->M, cudaMemcpyDeviceToHost));
+        if (std::count(sg.begin(), sg.end(), -1.0) & 1) d.mant = -d.mant;
+    }
     if (logdet_out) *logdet_out = det_log(d);
     if (mant_out) *mant_out = d.mant;
     if (exp_out) *exp_out = d.exp;
@@ -1140,6 +1352,101 @@ int cflx_chol_svxx(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X,
     *rcond_out = rcond;
     return svxx_run(&ch->eq, &ch->sv.rf, chol_refine_op(ch), nrhs, B, ldb, X, ldx, s, s, s, rcond,
                     err_bnds_comp_out != nullptr, berr_out, err_bnds_norm_out, err_bnds_comp_out, info_out);
+}
+
+// The signs S of the last factorisation: those of cflx_chol_factor_ldlt, or all +1 after cflx_chol_factor
+int cflx_chol_get_signs(cflx_chol* ch, double* s_out) {
+    REFUSE_IF(!ch);
+    REFUSE_IF(!s_out);
+    CFLX_TRY(enter(ch, __func__, NEED_FACTORS));
+    if (!ch->ldlt) {
+        std::fill(s_out, s_out + ch->M, 1.0);
+        return CFLX_OK;
+    }
+    CFLX_CUDA(cudaMemcpy(s_out, ch->sgn, sizeof(double) * ch->M, cudaMemcpyDeviceToHost));
+    return CFLX_OK;
+}
+
+// the input share as the factorisations read it (after an equilibration that scaled it, after cflx_chol_rbt)
+int cflx_chol_get_input(cflx_chol* ch, double* A_host) {
+    REFUSE_IF(!ch);
+    REFUSE_IF(!A_host);
+    CFLX_TRY(enter(ch, __func__, NEED_INPUT));
+    CFLX_CUDA(cudaMemcpyAsync(A_host, ch->A0, (size_t)ch->Ml * ch->Nl * sizeof(double), cudaMemcpyDeviceToHost, ch->comm->stream));
+    CFLX_CUDA(cudaStreamSynchronize(ch->comm->stream));
+    return CFLX_OK;
+}
+
+// COLLECTIVE.  A0 <- W = U^T A0 U on every rank's share (rbt.cu), after the ranks agreed on depth and seed with one world
+// all-reduce, so that a refusal anywhere is a refusal everywhere: first the symmetric completion of the stored lower
+// triangle (sym_mirror), since a butterfly row pair mixes both triangles, then the two-sided transform with V = U.  Every
+// layer transforms its own share (the transform is linear).  The factor and the solve cache are dropped.  The input
+// carries the transform only once both passes succeeded; a failure after the mirror began leaves no input at all (a
+// half-transformed share must be uploaded again).
+int cflx_chol_rbt(cflx_chol* ch, int depth, uint64_t seed, double* u_out) {
+    REFUSE_IF(!ch);
+    CFLX_TRY(enter(ch, __func__, 0));  // the device of world_agree, whatever chol_rbt_prepare finds
+    const int rc = chol_rbt_prepare(__func__, ch, depth);
+    bool same = false;
+    CFLX_TRY(world_agree(ch, rc == CFLX_OK, {seed, (unsigned long long)depth}, &same));
+    if (rc != CFLX_OK) return rc;
+    if (!same) {
+        set_last_error("%s: the ranks passed different depths or seeds, or another rank refused its arguments", __func__);
+        return CFLX_ERR_ARG;
+    }
+    const int M = ch->M;
+    const size_t n = (size_t)depth * M;
+    std::vector<double> r(n), sc(2 * n);
+    rbt_multipliers(M, depth, seed, 0, r.data());
+    if (u_out) std::memcpy(u_out, r.data(), sizeof(double) * n);
+    rbt_scales(r.data(), n, sc.data());
+    std::memcpy(sc.data() + n, sc.data(), sizeof(double) * n);  // the record's V is U
+    cudaStream_t s = ch->comm->stream;
+    ch->factored = false;
+    ch->sv.ready = false;
+    RbtRecord& in = ch->rbt.in;
+    int rc2 = sym_mirror(*ch, ch->A0);
+    if (rc2 == CFLX_OK) rc2 = rbt_record_set(&in, depth, seed, sc.data(), M, s);
+    if (rc2 == CFLX_OK) rc2 = launch_rbt(RbtOp::W, ch->A0, ch->Nl, *ch, ch->Nl, INT_MAX, depth, in.s, in.s, s);
+    if (rc2 == CFLX_OK && cudaStreamSynchronize(s) != cudaSuccess) {  // sc is a host temporary
+        set_last_error("%s: %s", __func__, cudaGetErrorString(cudaGetLastError()));
+        rc2 = CFLX_ERR_CUDA;
+    }
+    if (rc2 != CFLX_OK) {
+        in.depth = 0;
+        ch->have_input = false;
+    }
+    return rc2;
+}
+
+// COLLECTIVE.  A X = B through the transformed system the factor represents: X = U inv(W) U^T B, with dporfs on the
+// transformed system when refine (svx_tail with the butterflies as its row transforms).
+int cflx_chol_rbt_solve(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X, int ldx, int refine,
+                        double* ferr_out, double* berr_out) {
+    REFUSE_IF(!ch);
+    REFUSE_IF(refine != 0 && refine != 1);
+    CFLX_TRY(rhs_args(__func__, nrhs, B, ldb, X, ldx, true));
+    CFLX_TRY(enter(ch, __func__, NEED_FACTORS));
+    if (!ch->rbt.fac.depth) {
+        set_last_error("%s: the factor carries no random butterfly transform (cflx_chol_rbt before the factorisation)",
+                       __func__);
+        return CFLX_ERR_STATE;
+    }
+    const RefineOp op = chol_refine_op(ch);
+    auto refine_step = [&](const double* dB, int lb, double* dX, int lx) {
+        return refine ? refine_run(&ch->sv.rf, op, nrhs, dB, lb, dX, lx, ferr_out, berr_out) : CFLX_OK;
+    };
+    return svx_tail(&ch->eq, op, nrhs, B, ldb, X, ldx, rbt_rows(*ch, RbtOp::UT), rbt_rows(*ch, RbtOp::U), refine_step);
+}
+
+// Not collective.  U^T (op 0) or U (op 1) of the factor's transform on the rows of this rank's right-hand side share.
+int cflx_chol_rbt_apply_local(cflx_chol* ch, int op, int nrhs, double* B_local, int ldb) {
+    REFUSE_IF(!ch);
+    REFUSE_IF(op != 0 && op != 1);
+    REFUSE_IF(nrhs < 1);
+    REFUSE_IF(!B_local);
+    REFUSE_IF(ldb < rhs_local_cols(nrhs, ch->v, ch->Py));
+    return rbt_apply_local(__func__, "cflx_chol_rbt", ch, op ? RbtOp::U : RbtOp::UT, nrhs, B_local, ldb);
 }
 
 int cflx_chol_launch_count(cflx_chol* ch, int64_t* count_out, int reset) {

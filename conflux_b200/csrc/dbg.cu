@@ -561,6 +561,24 @@ int cflx_dbg_rbt_share(int op, const cflx_share_layout* share, int depth, const 
     return CFLX_OK;
 }
 
+// the sign pass between the sweeps of a signed Cholesky solve (solve.cu launch_solve_signs) on one share's Z
+int cflx_dbg_solve_signs(const cflx_share_layout* share, int ldn, const double* sgn, double* Z_inout) {
+    CFLX_TRY(check_device());
+    Layout L;
+    CFLX_TRY(share_layout(__func__, share, TILED, &L));
+    REFUSE_IF(ldn < 1);
+    REFUSE_IF(!sgn);
+    REFUSE_IF(!Z_inout);
+    const size_t n = (size_t)L.Nl * ldn;
+    DevBuf<> dZ, ds;
+    CFLX_TRY(stage(dZ, n, Z_inout));
+    CFLX_TRY(stage(ds, (size_t)L.M, sgn));
+    CFLX_TRY(launch_solve_signs(dZ.as<double>(), ldn, L, ds.as<double>(), 0));
+    CFLX_TRY(fetch(Z_inout, dZ.p, n));
+    CFLX_CUDA(cudaDeviceSynchronize());
+    return CFLX_OK;
+}
+
 // the per-share passes of the 1-norm and the infinity-norm (norm.cu) on one layer-0 share: mode 0 the column sums, 1 the
 // column sums of the symmetric matrix stored as its lower triangle, 2 the row sums
 int cflx_dbg_norm_share(int mode, const cflx_share_layout* share, const double* A, double* out) {
@@ -992,6 +1010,46 @@ int cflx_dbg_potrf_tile(int v, const double* A, double* L_out, double* LT_out, i
     CFLX_TRY(fetch(LT_out, dUT.p, vv));
     CFLX_TRY(fetch(info_out, dinfo.p, 1));
     CFLX_CUDA(cudaDeviceSynchronize());
+    return CFLX_OK;
+}
+
+// The signed Cholesky of one tile on the kernels of cflx_chol_factor_ldlt, variants as cflx_dbg_potrf_tile
+int cflx_dbg_ldlt_tile(int v, const double* A, double tiny, double* R_out, double* SRT_out, double* s_out, int* nrepl_out,
+                       int* inertia_out, int* info_out, int variant) {
+    CFLX_TRY(check_device());
+    REFUSE_IF(!A);
+    REFUSE_IF(!(tiny >= 0.0));
+    REFUSE_IF(variant < 0 || variant > 2);
+    REFUSE_IF(v < 4 || v > 512 || (variant == 1 && v != 128) || (variant == 2 && potrf_tile_scratch(v) == 0));
+    const size_t vv = (size_t)v * v;
+    DevBuf<> dD, dUT, dUc, dQ, dinfo, dcnt, dsg;
+    CFLX_TRY(stage(dD, vv, A));
+    CFLX_TRY(stage(dUT, vv));
+    CFLX_TRY(stage(dUc, vv));
+    CFLX_TRY(stage(dsg, (size_t)v));
+    CFLX_TRY(stage<int>(dinfo, 1));
+    CFLX_TRY(stage<int>(dcnt, 4));
+    if (variant == 2) CFLX_TRY(stage(dQ, potrf_tile_scratch(v)));
+    CFLX_CUDA(cudaMemset(dUT.p, 0, 8 * vv));
+    CFLX_CUDA(cudaMemset(dinfo.p, 0, sizeof(int)));
+    CFLX_CUDA(cudaMemset(dcnt.p, 0, 4 * sizeof(int)));
+    CFLX_TRY(potrf_setup(v));
+    const LdltArgs sa{tiny, dsg.as<double>(), dcnt.as<int>()};
+    int64_t launches = 0;
+    if (variant == 1)
+        CFLX_TRY(potrf_block128(dD.as<double>(), v, dUT.as<double>(), v, dUc.as<double>(), dinfo.as<int>(), 0, 0, &sa));
+    else
+        CFLX_TRY(potrf_tile(dD.as<double>(), dUT.as<double>(), dQ.as<double>(), dinfo.as<int>(), 0, v, 0, &launches, &sa));
+    int cnt[4];
+    CFLX_TRY(fetch(R_out, dD.p, vv));
+    CFLX_TRY(fetch(SRT_out, dUT.p, vv));
+    CFLX_TRY(fetch(s_out, dsg.p, (size_t)v));
+    CFLX_TRY(fetch(cnt, dcnt.p, 4));
+    CFLX_TRY(fetch(info_out, dinfo.p, 1));
+    CFLX_CUDA(cudaDeviceSynchronize());
+    if (nrepl_out) *nrepl_out = cnt[0];
+    if (inertia_out)
+        for (int i = 0; i < 3; ++i) inertia_out[i] = cnt[1 + i];
     return CFLX_OK;
 }
 

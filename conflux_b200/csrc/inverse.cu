@@ -113,6 +113,7 @@ int inverse_blocks(SolveCache* sc, const SolveFactor& f, InvKind kind, const int
             CFLX_TRY(solve_row_sweep(sc, f, ldn, false, sc->X, 1, false));
         } else if (g.pk == 0) {  // L Y = E from tile T0 keeping Y_t in Z, then L^T X = Y down to tile T0
             CFLX_TRY(solve_row_sweep(sc, f, ldn, true, sc->Z, g.Py, false, T0));
+            CFLX_TRY(solve_apply_signs(sc, f, ldn));  // a signed factor: L^T X = S Y
             CFLX_TRY(solve_col_sweep(sc, f, ldn, false, Tri::LowerT, sc->X, 1, false, T0));
         }
         CFLX_TRY(solve_finish(sc, f, ldn, nc, nullptr, 0));

@@ -149,9 +149,20 @@ int trsm_left_lower_unit(const double* A00T, const double* LinvT, int v, int nb,
 // unless *info is already non-zero.  *launches grows by the launches the 128-block path counts.  potrf_setup(v) first.
 size_t potrf_tile_scratch(int v);
 int potrf_setup(int v);
-int potrf_tile(double* D, double* UT, double* Q, int* info, int col0, int v, cudaStream_t stream, int64_t* launches);
+// The signed Cholesky A = R S R^T of cflx_chol_factor_ldlt (chol.cu potrf_tile_kernel): the tiny rule's threshold, the
+// device signs of the tile's columns (sg[c] = s_c = +-1) and the device counts cnt[4] += {replacements, positive,
+// negative, zero pivots}.  R goes where L goes, S R^T where L^T goes.
+struct LdltArgs {
+    double tiny;
+    double* sg;
+    int* cnt;
+};
+// sa (may be null: the Cholesky): the signed factorisation of the tile
+int potrf_tile(double* D, double* UT, double* Q, int* info, int col0, int v, cudaStream_t stream, int64_t* launches,
+               const LdltArgs* sa = nullptr);
 // one 128 x 128 block (leading dimensions ldd / ldu) on potrf128_kernel; Uc: a contiguous 128 x 128 copy of L^T
-int potrf_block128(double* D, int ldd, double* UT, int ldu, double* Uc, int* info, int col0, cudaStream_t stream);
+int potrf_block128(double* D, int ldd, double* UT, int ldu, double* Uc, int* info, int col0, cudaStream_t stream,
+                   const LdltArgs* sa = nullptr);
 
 // ---------------------------------------------------------------- fixed.cu (cflx_lu_factor_fixed)
 // Unpivoted LU of one v x v block: Bt is the block transposed (Bt[c][i], as launch_gather_winners leaves it), A

@@ -1147,9 +1147,10 @@ unsigned long long order_hash(const std::vector<int>& p) {
     return h;
 }
 
-// COLLECTIVE (world): *same = every rank has ok and the same words, from one ncclMin over {w.., ~w.., ok}: min(~w) =
-// ~max(w)
-int world_agree(cflx_lu* lu, bool ok, std::initializer_list<unsigned long long> words, bool* same) {
+}  // namespace
+
+// min(~w) = ~max(w)
+int cflx::world_agree(Handle* lu, bool ok, std::initializer_list<unsigned long long> words, bool* same) {
     cflx_comm* c = lu->comm;
     if (c->world_size == 1) {
         *same = ok;
@@ -1168,6 +1169,8 @@ int world_agree(cflx_lu* lu, bool ok, std::initializer_list<unsigned long long> 
     for (size_t i = 0; i < n; ++i) *same = *same && w[i] == ~w[n + i];
     return CFLX_OK;
 }
+
+namespace {
 
 // The checks of cflx_lu_factor_fixed (`who`) that need no other rank; on success lu->fix_perm_h holds the order and the
 // device buffers of the fixed path exist
@@ -1220,15 +1223,6 @@ int rbt_prepare(const char* who, cflx_lu* lu, int depth) {
     return CFLX_OK;
 }
 
-// The transform the factors carry, as a row transform of an M-row device array (the replicated right-hand sides)
-RowTransform rbt_rows(cflx_lu* lu, RbtOp op) {
-    const RbtRecord& f = lu->rbt.fac;
-    const Layout rows{lu->M, lu->v, lu->Nt, lu->M, 0, 1, 1, 0, 0};  // global row r is row r
-    const double *su = f.s, *sv = f.s + (size_t)f.depth * lu->M;
-    cudaStream_t s = lu->comm->stream;
-    const int depth = f.depth;
-    return [=](double* X, int64_t ld, int n) { return launch_rbt(op, X, ld, rows, n, INT_MAX, depth, su, sv, s); };
-}
 }  // namespace
 
 extern "C" {
@@ -1337,8 +1331,8 @@ int cflx_lu_rbt_solve(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb
     auto refine_step = [&](const double* dB, int lb, double* dX, int lx) {
         return refine ? refine_run(&lu->sv.rf, op, nrhs, dB, lb, dX, lx, ferr_out, berr_out) : CFLX_OK;
     };
-    return svx_tail(&lu->eq, op, nrhs, B, ldb, X, ldx, rbt_rows(lu, t ? RbtOp::VT : RbtOp::UT),
-                    rbt_rows(lu, t ? RbtOp::U : RbtOp::V), refine_step);
+    return svx_tail(&lu->eq, op, nrhs, B, ldb, X, ldx, rbt_rows(*lu, t ? RbtOp::VT : RbtOp::UT),
+                    rbt_rows(*lu, t ? RbtOp::U : RbtOp::V), refine_step);
 }
 
 // Not collective.  One of the factors' butterflies on the rows of this rank's right-hand side share (rbt.cu); a host
@@ -1351,30 +1345,7 @@ int cflx_lu_rbt_apply_local(cflx_lu* lu, int op, int nrhs, double* B_local, int 
     REFUSE_IF(!B_local);
     const int ncl = rhs_local_cols(nrhs, lu->v, lu->Py);
     REFUSE_IF(ldb < ncl);
-    CFLX_TRY(enter(lu, __func__, NEED_FACTORS));
-    const RbtRecord& f = lu->rbt.fac;
-    if (!f.depth) {
-        set_last_error("%s: the factors carry no random butterfly transform (cflx_lu_rbt before the factorisation)",
-                       __func__);
-        return CFLX_ERR_STATE;
-    }
-    bool dev = false;
-    CFLX_TRY(share_kind(__func__, *lu, B_local, "B_local", &dev));
-    cudaStream_t s = lu->comm->stream;
-    const size_t row = sizeof(double) * ncl;
-    DevBuf<double> tmp;
-    double* X = B_local;
-    int64_t ld = ldb;
-    if (!dev) {
-        CFLX_TRY(tmp.alloc((size_t)lu->Ml * ncl));
-        CFLX_CUDA(cudaMemcpy2DAsync(tmp, row, B_local, sizeof(double) * ldb, row, lu->Ml, cudaMemcpyHostToDevice, s));
-        X = tmp;
-        ld = ncl;
-    }
-    CFLX_TRY(launch_rbt((RbtOp)op, X, ld, *lu, ncl, nrhs, f.depth, f.s, f.s + (size_t)f.depth * lu->M, s));
-    if (!dev) CFLX_CUDA(cudaMemcpy2DAsync(B_local, sizeof(double) * ldb, tmp, row, row, lu->Ml, cudaMemcpyDeviceToHost, s));
-    CFLX_CUDA(cudaStreamSynchronize(s));
-    return CFLX_OK;
+    return rbt_apply_local(__func__, "cflx_lu_rbt", lu, (RbtOp)op, nrhs, B_local, ldb);
 }
 
 int cflx_lu_get_permutation(cflx_lu* lu, int* perm_out) {

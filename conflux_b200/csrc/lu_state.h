@@ -212,6 +212,7 @@ struct SolveFactor {
     int rows;  // local rows of the tiles the sweeps read and seed
     const SubComm *row_comm, *col_comm;
     int stride;
+    const double* sgn = nullptr;  // a signed Cholesky factor's S (M, device, every rank): A = F S F^T; null: S = I
 };
 
 // How a kind of handle words its state errors, after "<function>: " (callers match these texts)
@@ -234,6 +235,8 @@ struct Handle : Grid {
     bool use_ozaki = false;
     SolveCache sv;
     EquilState eq;  // cflx_*_equilibrate / cflx_*_svx
+    RbtState rbt;   // cflx_*_rbt: the transform of the input and of the factors
+    DevBuf<unsigned long long> agree;  // the words the ranks compare before a fixed factorisation or a transform
 };
 // grid_init, then A0 and A11 (not zeroed)
 int handle_init(Handle* h, const HandleTexts* texts, cflx_comm* c, int Px, int Py, int Pz);
@@ -261,6 +264,8 @@ void handle_equil_begin(Handle* h);
 // query leaves the record and its scales
 int handle_equil_end(Handle* h, bool apply, int info, char equed, double rowcnd, double colcnd, const double* c);
 int handle_launch_count(Handle* h, int64_t* count_out, int reset);
+// COLLECTIVE (world): *same = every rank has ok and the same words, from one ncclMin over {w.., ~w.., ok}
+int world_agree(Handle* h, bool ok, std::initializer_list<unsigned long long> words, bool* same);
 }  // namespace cflx
 
 // sv (cflx_lu_solve): Linv blocks forward, Uinv blocks backward; rows: row of B of each row of P*B
@@ -298,15 +303,12 @@ struct cflx_lu : cflx::Handle {
     // cflx_lu_factor_fixed: the plan's fixed-order flag, the prescribed order (host and device, M each), this rank's
     // pivot count per step, the tiny-pivot threshold, and the device record {replacements, first zero pivot, its min
     // operand} (4 ints) and the tile kernel's scratch (getrf_nopiv_scratch(v)); the device buffers are made by the first
-    // fixed call.  agree: the words the ranks compare before a fixed factorisation or a transform (world_agree)
+    // fixed call
     bool fixed = false;
     std::vector<int> fix_perm_h, fix_npiv;
     double fix_tiny = 0.0;
     cflx::DevBuf<int> fix_perm, fix_rec;
-    cflx::DevBuf<unsigned long long> agree;
     cflx::DevBuf<double> fix_ws;
-    // cflx_lu_rbt: the transform of the input and of the factors
-    cflx::RbtState rbt;
     ~cflx_lu();  // the handle's device made current, the sub-communicators destroyed, then the members freed
 };
 
@@ -339,8 +341,9 @@ inline int chol_piece_ld(const Layout& L, int gfirst, int p) {
 //                column, global row < Nt v); partials: SUMSQ_PARTIALS doubles of scratch
 //   extract_l_panel_T: PT[c][r] = A[row0 + r][col0 + c] for r < n, c < v where the global row of local row row0 + r is
 //                >= the global column t v + c, else 0
+//                sg (may be null): Bc's row c times sg[c] (the signs of the step, cflx_chol_factor_ldlt)
 int launch_gather_cols(const double* G, int64_t piece_stride, double* Bc, int64_t ldb, int v, int Px, int Py, int pj,
-                       int lj0, int ntiles, int gfirst, int Ml, cudaStream_t s);
+                       int lj0, int ntiles, int gfirst, int Ml, cudaStream_t s, const double* sg = nullptr);
 int launch_sumsq_lower(const double* X, const Layout& L, double* partials, double* out, cudaStream_t s);
 int launch_extract_l_panel_T(const double* A, int64_t lda, int row0, int col0, int n, const Layout& L, int t, double* PT,
                              int64_t ldp, cudaStream_t s);
@@ -378,6 +381,11 @@ int solve_row_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward,
 // [t_lo, t_hi) as solve_row_sweep.
 int solve_col_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward, Tri tri, double* keep, int keep_div,
                     bool clear_col, int t_lo = 0, int t_hi = -1);
+// between the two sweeps of a signed factor (f.sgn): Y <- S Y on the Y_t the row sweep kept in Z (by local tile column;
+// every other entry of Z is zero then), on layer 0; nothing without f.sgn
+int solve_apply_signs(SolveCache* sc, const SolveFactor& f, int ldn);
+// its kernel on one share: Z[r][j] *= sgn[L.col(r)] for r < L.Nl with L.col(r) < L.M, j < ldn (Z: Nl x ldn, device)
+int launch_solve_signs(double* Z, int ldn, const Layout& L, const double* sgn, cudaStream_t s);
 // X (nrhs columns, ldx; host or device) = the world sum of the owners' tiles of sc->X, copied when X is not null;
 // synchronises.
 // unperm (M rows, every rank): row i of X is row unperm[i] of that sum.
@@ -509,6 +517,18 @@ using RowTransform = std::function<int(double* X, int64_t ld, int n)>;
 using SvxRefine = std::function<int(const double*, int, double*, int)>;
 int svx_tail(EquilState* e, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx,
              const RowTransform& pre, const RowTransform& post, const SvxRefine& refine);
+// rbt.cu.  The transform h's factors carry, as a row transform of an M-row device array (the replicated right-hand sides)
+RowTransform rbt_rows(const Handle& h, RbtOp op);
+// Not collective.  One of the factors' butterflies on the rows of this rank's right-hand side share B_local (host or
+// device, ldb >= rhs_local_cols: checked by the caller), in the name of `who`; CFLX_ERR_STATE when the factors carry no
+// transform (`rbt_call` names the call that makes one)
+int rbt_apply_local(const char* who, const char* rbt_call, Handle* h, RbtOp op, int nrhs, double* B_local, int ldb);
+// COLLECTIVE within each layer.  The symmetric completion of the stored lower triangle of the real tiles of the shares
+// A (h's layout): tile (I, J), I < J < Nt, receives tile (J, I)^T from rank (J % Px, I % Py) -- transposed in place
+// when that is this rank, else packed per peer and exchanged in one group of ncclSend / ncclRecv (staging buffers of
+// the exchanged tiles only) -- and every diagonal tile's upper triangle its lower one transposed.  Nothing else is
+// written.  Synchronises.
+int sym_mirror(const Grid& h, double* A);
 // The solve and refinement of cflx_lu_svx / cflx_chol_svx (equil.cu), COLLECTIVE: B (host or device) to the device, its
 // rows scaled by pre (may be null), X = op.solve(false, B), refine_run, the rows of X scaled by post (may be null), X out;
 // when post is not null, ferr is divided by cnd.  Then *info = M + 1 when rcond < 2^-53 (dgesvx / dposvx: the matrix is

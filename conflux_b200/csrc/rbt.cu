@@ -17,7 +17,9 @@
 //
 // A thread takes the 2^n rows (2^n x 2^n entries for W) that n consecutive levels mix, and runs those levels on them in
 // registers: depth 2 is one read and one write of the share, depth 3 and 4 two.
+#include <climits>
 #include <cmath>
+#include <vector>
 
 #include "lu_state.h"
 
@@ -145,6 +147,64 @@ int launch_levels(double* X, int64_t ld, const Layout& L, int ncols, int col_lim
     return CFLX_OK;
 }
 
+// The mirror's tile moves (sym_mirror), one tile k of a list per blockIdx.y stride (the lists can be far longer than a
+// grid's y extent); pack and transpose go through shared memory (transpose_tile):
+//   pack:      buf[k][r][c] = A tile at (off[2k], off[2k + 1]) [c][r] (the tile transposed, contiguous)
+//   unpack:    A tile at (off[2k], off[2k + 1]) [r][c] = buf[k][r][c]
+//   transpose: A tile at (off[4k], off[4k + 1]) [r][c] = A tile at (off[4k + 2], off[4k + 3]) [c][r] (distinct tiles)
+//   diag:      A tile at (off[2k], off[2k + 1]) [r][c] = the same tile [c][r] for c > r (upper from lower)
+// D[r][c] = S[c][r] for one v x v tile, 32 x 32 blocks through shared memory (both sides coalesced): block blockIdx.x
+// of the destination tile, a (32, 8) CTA
+__device__ __forceinline__ void transpose_tile(const double* __restrict__ S, int64_t lds, double* __restrict__ D, int64_t ldd,
+                                               int v, double (*t)[33]) {
+    const int nbx = (v + 31) / 32, bi = blockIdx.x / nbx, bj = blockIdx.x % nbx;
+    for (int y = threadIdx.y; y < 32; y += blockDim.y) {
+        const int sr = bj * 32 + y, sc = bi * 32 + threadIdx.x;
+        if (sr < v && sc < v) t[y][threadIdx.x] = S[(int64_t)sr * lds + sc];
+    }
+    __syncthreads();
+    for (int y = threadIdx.y; y < 32; y += blockDim.y) {
+        const int dr = bi * 32 + y, dc = bj * 32 + threadIdx.x;
+        if (dr < v && dc < v) D[(int64_t)dr * ldd + dc] = t[threadIdx.x][y];
+    }
+    __syncthreads();
+}
+__global__ void tiles_pack_kernel(const double* __restrict__ A, int64_t ld, const int* __restrict__ off, int ntiles, int v,
+                                  double* __restrict__ buf) {
+    __shared__ double t[32][33];
+    for (int k = blockIdx.y; k < ntiles; k += gridDim.y)
+        transpose_tile(A + (int64_t)off[2 * k] * ld + off[2 * k + 1], ld, buf + (int64_t)k * v * v, v, v, t);
+}
+__global__ void tiles_unpack_kernel(const double* __restrict__ buf, const int* __restrict__ off, int ntiles, int v,
+                                    double* __restrict__ A, int64_t ld) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= v * v) return;
+    for (int k = blockIdx.y; k < ntiles; k += gridDim.y)
+        A[(int64_t)(off[2 * k] + e / v) * ld + off[2 * k + 1] + e % v] = buf[(int64_t)k * v * v + e];
+}
+__global__ void tiles_transpose_kernel(double* __restrict__ A, int64_t ld, const int* __restrict__ off, int ntiles, int v) {
+    __shared__ double t[32][33];
+    for (int k = blockIdx.y; k < ntiles; k += gridDim.y)
+        transpose_tile(A + (int64_t)off[4 * k + 2] * ld + off[4 * k + 3], ld, A + (int64_t)off[4 * k] * ld + off[4 * k + 1],
+                       ld, v, t);
+}
+__global__ void tiles_diag_mirror_kernel(double* __restrict__ A, int64_t ld, const int* __restrict__ off, int ntiles, int v) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= v * v) return;
+    const int r = e / v, c = e % v;
+    if (c <= r) return;
+    for (int k = blockIdx.y; k < ntiles; k += gridDim.y) {
+        double* T = A + (int64_t)off[2 * k] * ld + off[2 * k + 1];
+        T[(int64_t)r * ld + c] = T[(int64_t)c * ld + r];
+    }
+}
+// the grid of a tile-list kernel: v^2 / 256 CTAs (transposes: one per 32 x 32 block) along x, the tiles along y
+// (capped, the kernels stride)
+dim3 tiles_grid(int v, size_t ntiles, bool transpose = false) {
+    const unsigned x = transpose ? (unsigned)(((v + 31) / 32) * ((v + 31) / 32)) : (unsigned)((v * v + 255) / 256);
+    return dim3(x, (unsigned)std::min<size_t>(ntiles, RBT_MAX_GRID_Y));
+}
+
 // splitmix64's finaliser (Steele, Lea and Flood, OOPSLA 2014)
 uint64_t splitmix_final(uint64_t z) {
     z ^= z >> 30;
@@ -194,6 +254,110 @@ int rbt_record_set(RbtRecord* dst, int depth, uint64_t seed, const double* s, in
 int rbt_pass_on(RbtState* t, int M, bool next_is_plain, cudaStream_t s) {
     CFLX_TRY(rbt_record_set(&t->fac, t->in.depth, t->in.seed, t->in.s, M, s));
     if (next_is_plain) t->in.depth = 0;
+    return CFLX_OK;
+}
+
+RowTransform rbt_rows(const Handle& h, RbtOp op) {
+    const RbtRecord& f = h.rbt.fac;
+    const Layout rows{h.M, h.v, h.Nt, h.M, 0, 1, 1, 0, 0};  // global row r is row r
+    const double *su = f.s, *sv = f.s + (size_t)f.depth * h.M;
+    cudaStream_t s = h.comm->stream;
+    const int depth = f.depth;
+    return [=](double* X, int64_t ld, int n) { return launch_rbt(op, X, ld, rows, n, INT_MAX, depth, su, sv, s); };
+}
+
+int rbt_apply_local(const char* who, const char* rbt_call, Handle* h, RbtOp op, int nrhs, double* B_local, int ldb) {
+    CFLX_TRY(enter(h, who, NEED_FACTORS));
+    const RbtRecord& f = h->rbt.fac;
+    if (!f.depth) {
+        set_last_error("%s: the factors carry no random butterfly transform (%s before the factorisation)", who, rbt_call);
+        return CFLX_ERR_STATE;
+    }
+    const int ncl = rhs_local_cols(nrhs, h->v, h->Py);
+    bool dev = false;
+    CFLX_TRY(share_kind(who, *h, B_local, "B_local", &dev));
+    cudaStream_t s = h->comm->stream;
+    const size_t row = sizeof(double) * ncl;
+    DevBuf<double> tmp;
+    double* X = B_local;
+    int64_t ld = ldb;
+    if (!dev) {
+        CFLX_TRY(tmp.alloc((size_t)h->Ml * ncl));
+        CFLX_CUDA(cudaMemcpy2DAsync(tmp, row, B_local, sizeof(double) * ldb, row, h->Ml, cudaMemcpyHostToDevice, s));
+        X = tmp;
+        ld = ncl;
+    }
+    CFLX_TRY(launch_rbt(op, X, ld, *h, ncl, nrhs, f.depth, f.s, f.s + (size_t)f.depth * h->M, s));
+    if (!dev) CFLX_CUDA(cudaMemcpy2DAsync(B_local, sizeof(double) * ldb, tmp, row, row, h->Ml, cudaMemcpyDeviceToHost, s));
+    CFLX_CUDA(cudaStreamSynchronize(s));
+    return CFLX_OK;
+}
+
+int sym_mirror(const Grid& g, double* A) {
+    cflx_comm* c = g.comm;
+    cudaStream_t s = c->stream;
+    const int v = g.v, Px = g.Px, Py = g.Py, Nt = g.Nt, me = g.pi * Py + g.pj;
+    const int npeer = Px * Py;
+    // per other peer (grid position q = qi Py + qj of this layer), in the order (I, J) on both sides: the offsets of the
+    // tiles (J, I) this rank sends and of the tiles (I, J) it receives; the pairs {(I, J), (J, I)} this rank holds both
+    // of, transposed in place; the diagonal tiles it holds
+    std::vector<std::vector<int>> snd(npeer), rcv(npeer);
+    std::vector<int> loc, diag;
+    for (int I = 0; I < Nt; ++I)
+        for (int J = I; J < Nt; ++J) {
+            const int dq = (I % Px) * Py + J % Py, sq = (J % Px) * Py + I % Py;
+            if (I == J) {
+                if (dq == me) diag.insert(diag.end(), {(I / Px) * v, (I / Py) * v});
+            } else if (sq == me && dq == me) {
+                loc.insert(loc.end(), {(I / Px) * v, (J / Py) * v, (J / Px) * v, (I / Py) * v});
+            } else if (sq == me) {
+                snd[dq].insert(snd[dq].end(), {(J / Px) * v, (I / Py) * v});
+            } else if (dq == me) {
+                rcv[sq].insert(rcv[sq].end(), {(I / Px) * v, (J / Py) * v});
+            }
+        }
+    std::vector<int> off;  // the send list, the receive list (peers ascending), the local pairs, the diagonal tiles
+    std::vector<size_t> sfirst(npeer + 1, 0), rfirst(npeer + 1, 0);
+    for (int q = 0; q < npeer; ++q) {
+        off.insert(off.end(), snd[q].begin(), snd[q].end());
+        sfirst[q + 1] = sfirst[q] + snd[q].size() / 2;
+    }
+    for (int q = 0; q < npeer; ++q) {
+        off.insert(off.end(), rcv[q].begin(), rcv[q].end());
+        rfirst[q + 1] = rfirst[q] + rcv[q].size() / 2;
+    }
+    off.insert(off.end(), loc.begin(), loc.end());
+    off.insert(off.end(), diag.begin(), diag.end());
+    const size_t ns = sfirst[npeer], nr = rfirst[npeer], nl = loc.size() / 4, nd = diag.size() / 2, vv = (size_t)v * v;
+    DevBuf<int> doff;
+    CFLX_TRY(doff.alloc(off.size()));
+    CFLX_CUDA(cudaMemcpyAsync(doff, off.data(), sizeof(int) * off.size(), cudaMemcpyHostToDevice, s));
+    const int* d_loc = doff + 2 * (ns + nr);
+    const int* d_diag = d_loc + 4 * nl;
+    if (nl) tiles_transpose_kernel<<<tiles_grid(v, nl, true), dim3(32, 8), 0, s>>>(A, g.Nl, d_loc, (int)nl, v);
+    CFLX_CUDA(cudaGetLastError());
+    if (nd) tiles_diag_mirror_kernel<<<tiles_grid(v, nd), 256, 0, s>>>(A, g.Nl, d_diag, (int)nd, v);
+    CFLX_CUDA(cudaGetLastError());
+    if (ns + nr) {  // the tiles of other ranks: packed per peer, one group of sends and receives in this layer
+        DevBuf<double> sbuf, rbuf;
+        CFLX_TRY(sbuf.alloc(ns * vv));
+        CFLX_TRY(rbuf.alloc(nr * vv));
+        if (ns) tiles_pack_kernel<<<tiles_grid(v, ns, true), dim3(32, 8), 0, s>>>(A, g.Nl, doff, (int)ns, v, sbuf);
+        CFLX_CUDA(cudaGetLastError());
+        CFLX_NCCL(ncclGroupStart());
+        for (int q = 0; q < npeer; ++q) {
+            const int peer = q * g.Pz + g.pk;  // world rank of grid position q on this layer
+            if (sfirst[q + 1] > sfirst[q])
+                CFLX_NCCL(ncclSend(sbuf + sfirst[q] * vv, (sfirst[q + 1] - sfirst[q]) * vv, ncclDouble, peer, c->world, s));
+            if (rfirst[q + 1] > rfirst[q])
+                CFLX_NCCL(ncclRecv(rbuf + rfirst[q] * vv, (rfirst[q + 1] - rfirst[q]) * vv, ncclDouble, peer, c->world, s));
+        }
+        CFLX_NCCL(ncclGroupEnd());
+        if (nr) tiles_unpack_kernel<<<tiles_grid(v, nr), 256, 0, s>>>(rbuf, doff + 2 * ns, (int)nr, v, A, g.Nl);
+        CFLX_CUDA(cudaGetLastError());
+        CFLX_CUDA(cudaStreamSynchronize(s));  // before the buffers are freed
+    }
+    CFLX_CUDA(cudaStreamSynchronize(s));  // the offsets are a temporary
     return CFLX_OK;
 }
 

@@ -410,6 +410,16 @@ int solve_set_rows(DevBuf<int>* dst, const std::vector<int>& rows, cudaStream_t 
     return CFLX_OK;
 }
 
+// Z[r][j] *= sgn[global column of local column r], for the local columns of real tiles (global index < M); a
+// grid-stride loop over the Nl x ldn entries
+__global__ void solve_signs_kernel(double* __restrict__ Z, int ldn, Layout L, const double* __restrict__ sgn) {
+    const int64_t n = (int64_t)L.Nl * ldn;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
+        const int gc = L.col((int)(e / ldn));
+        if (gc < L.M) Z[e] *= sgn[gc];
+    }
+}
+
 int solve_seed(SolveCache* sc, const SolveFactor& f, int ldn, int nrhs, const double* B, int ldb, const SolveSeed& at) {
     cudaStream_t s = f.g.comm->stream;
     CFLX_CUDA(cudaMemsetAsync(sc->X, 0, sizeof(double) * f.g.M * ldn, s));
@@ -501,6 +511,19 @@ int solve_col_sweep(SolveCache* sc, const SolveFactor& f, int ldn, bool forward,
                                                sc->Z + (int64_t)c_lo * ldn, ldn, -1.0, 1.0, s));
         }
     }
+    return CFLX_OK;
+}
+
+int solve_apply_signs(SolveCache* sc, const SolveFactor& f, int ldn) {
+    if (!f.sgn || f.g.pk != 0) return CFLX_OK;
+    return launch_solve_signs(sc->Z, ldn, f.g, f.sgn, f.g.comm->stream);
+}
+
+int launch_solve_signs(double* Z, int ldn, const Layout& L, const double* sgn, cudaStream_t s) {
+    const int64_t n = (int64_t)L.Nl * ldn;
+    if (n <= 0) return CFLX_OK;
+    solve_signs_kernel<<<(unsigned)std::min<int64_t>((n + 255) / 256, 4096), 256, 0, s>>>(Z, ldn, L, sgn);
+    CFLX_CUDA(cudaGetLastError());
     return CFLX_OK;
 }
 

@@ -91,6 +91,31 @@ inline void choleskySolve(int nrhs, const double* B, int ldb, double* X, int ldx
     if (!s.plan) throw CholeskyException("choleskySolve() before initialize()");
     chol_detail::check(cflx_chol_solve(s.plan, nrhs, B, ldb, X, ldx), "choleskySolve");
 }
+// The signed Cholesky A = R S R^T of the current input without pivoting (cflx_chol_factor_ldlt, collective), for
+// symmetric indefinite matrices: every later call refers to R S R^T.  Returns info (1 + the first exactly zero pivot's
+// column, 0: none); *nrepl the pivots the tiny rule replaced, inertia[3] the positive, negative and zero pivots.
+inline int parallelLDLT(double tiny = 0.0, int* nrepl = nullptr, int64_t* inertia = nullptr, double* ms = nullptr) {
+    auto& s = chol_detail::state();
+    if (!s.plan) throw CholeskyException("parallelLDLT() before initialize()");
+    int info = 0;
+    chol_detail::check(cflx_chol_factor_ldlt(s.plan, tiny, nrepl, inertia, &info, ms), "parallelLDLT");
+    return info;
+}
+// The symmetric random butterfly transform of the current input, A <- U^T A U (cflx_chol_rbt, collective); then
+// parallelLDLT() and choleskyRbtSolve().  u (depth x matrix_size(), may be nullptr) receives U's multipliers.
+inline void choleskyRbt(int depth = 2, uint64_t seed = 0, double* u = nullptr) {
+    auto& s = chol_detail::state();
+    if (!s.plan) throw CholeskyException("choleskyRbt() before initialize()");
+    chol_detail::check(cflx_chol_rbt(s.plan, depth, seed, u), "choleskyRbt");
+}
+// A X = B with a factor of a transformed input (cflx_chol_rbt_solve, collective): X = U inv(W) U^T B, refined on the
+// transformed system when refine; ferr / berr as choleskyRefine.
+inline void choleskyRbtSolve(int nrhs, const double* B, int ldb, double* X, int ldx, bool refine = true,
+                             double* ferr = nullptr, double* berr = nullptr) {
+    auto& s = chol_detail::state();
+    if (!s.plan) throw CholeskyException("choleskyRbtSolve() before initialize()");
+    chol_detail::check(cflx_chol_rbt_solve(s.plan, nrhs, B, ldb, X, ldx, refine ? 1 : 0, ferr, berr), "choleskyRbtSolve");
+}
 // A X = B with the factor of the last parallelCholesky(), like ScaLAPACK's pdpotrs, with B and X distributed like A
 // (cflx_chol_solve_local, collective): the shares and rules of conflux::LU_solve_local; only the rows of real tiles are
 // read or written.

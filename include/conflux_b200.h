@@ -325,6 +325,50 @@ int cflx_chol_info(const cflx_chol*, int* info_out);
 int cflx_chol_set_local(cflx_chol*, const double* host_local);
 /* COLLECTIVE.  ms_out = device time of the factorisation loop (the region the reference's miniapp times). */
 int cflx_chol_factor(cflx_chol*, double* ms_out);
+/* COLLECTIVE.  Signed Cholesky A = R S R^T of the input the device holds, without pivoting, for symmetric indefinite
+ * matrices (the LDL^T of Becker, Baboulin and Dongarra, PPAM 2011, with L = R diag(R)^-1 and D = S diag(R)^2): R lower
+ * triangular with a positive diagonal, S = diag(s), s_i = +-1.  Column c's pivot is d = a_cc - sum_{j<c} s_j r_cj^2;
+ * tiny (>= 0, absolute): |d| < tiny becomes copysign(tiny, d), +tiny for +-0, and nrepl_out (may be NULL) counts the
+ * replacements over the grid; then s_c = +1 for d > 0, else -1, and r_cc = sqrt|d|.  inertia_out[3] (may be NULL): the
+ * positive, negative and zero pivots over the padded order, by Sylvester's law the inertia of A when nrepl = 0.
+ * info_out: 1 + the global column of the first exactly zero pivot (only with tiny = 0), else 0; the factorisation still
+ * completes, and entries computed from a zero pivot may be inf or NaN.  On a positive definite input every s_i = +1 and
+ * R has the bits of cflx_chol_factor's L.  nrepl, inertia, info and the signs are the same on every rank.  ms_out, the
+ * scaling the factor carries and the state rules as cflx_chol_factor.  Every later call on the factor (solves, rcond,
+ * refinement, svx, svxx, inverse, det, validate, get_local = R) refers to R S R^T.  A random butterfly transform first
+ * (cflx_chol_rbt) makes a zero pivot unlikely.  CFLX_ERR_ARG for tiny < 0 or NaN, or a NULL info_out; CFLX_ERR_STATE
+ * before cflx_chol_set_local. */
+int cflx_chol_factor_ldlt(cflx_chol*, double tiny, int* nrepl_out, int64_t* inertia_out, int* info_out, double* ms_out);
+/* COLLECTIVE.  Symmetric random butterfly transform of the input the device holds: A <- W = U^T A U in place, U the
+ * random recursive butterfly of depth 1 .. 4 (2 in practice) from side 0 of cflx_rbt_multipliers(N, depth, seed) (u_out,
+ * depth x N, may be NULL).  The stored lower triangle is first completed to the symmetric matrix (tile (I, J), I < J,
+ * receives tile (J, I)^T, exchanged within each layer); the rounding of the transform leaves W only nearly symmetric, and
+ * the matrix every later call refers to is the stored lower triangle of W.  Each layer transforms its own share.  Factor
+ * W with cflx_chol_factor_ldlt (or cflx_chol_factor: a congruence keeps positive definiteness), then solve with
+ * cflx_chol_rbt_solve or cflx_chol_rbt_apply_local.  The factor and the solve cache are dropped; the next factorisation's
+ * factor carries the transform; cflx_chol_set_local gives an input without one.  CFLX_ERR_ARG for depth outside [1, 4],
+ * or ranks that differ in depth or seed or refused their arguments (one world all-reduce first: every rank returns the
+ * error); CFLX_ERR_UNSUPPORTED when N is not a multiple of 2^depth v lcm(Px, Py) (the message names the smallest N that
+ * works: pad A with the identity); CFLX_ERR_STATE before cflx_chol_set_local, on an input that is already transformed,
+ * and on a scaled input (cflx_chol_equilibrate*, apply = 1, which in turn refuses a transformed input).  Any other failure
+ * (CUDA, NCCL, device memory) after the mirror began leaves no input and no transform: upload the matrix again. */
+int cflx_chol_rbt(cflx_chol*, int depth, uint64_t seed, double* u_out);
+/* COLLECTIVE.  Solves A X = B with a factor that carries a transform (cflx_chol_rbt, then a factorisation): X = U inv(W)
+ * U^T B.  refine = 1 refines the solution of W Y = U^T B as cflx_chol_refine does, so ferr_out and berr_out (nrhs each,
+ * may be NULL; not written with refine = 0) are the errors of Y in that system.  Arguments, errors and side effects as
+ * cflx_lu_rbt_solve without trans. */
+int cflx_chol_rbt_solve(cflx_chol*, int nrhs, const double* B, int ldb, double* X, int ldx, int refine, double* ferr_out,
+                        double* berr_out);
+/* Not collective.  U^T (op 0) or U (op 1) of the factor's transform on the rows of this rank's right-hand side share, in
+ * place, in cflx_chol_solve_local's layout: apply_local(0) on B, cflx_chol_solve_local, apply_local(1) on X solves A X =
+ * B.  Arguments and errors as cflx_lu_rbt_apply_local, with op in [0, 1]. */
+int cflx_chol_rbt_apply_local(cflx_chol*, int op, int nrhs, double* B_local, int ldb);
+/* s_out (N doubles): the signs S of the last successful factorisation, those of cflx_chol_factor_ldlt, all +1 after
+ * cflx_chol_factor.  CFLX_ERR_STATE as cflx_chol_solve. */
+int cflx_chol_get_signs(cflx_chol*, double* s_out);
+/* A_host (Ml x Nl): this rank's share of the input as the factorisations read it, after cflx_chol_equilibrate*
+ * (apply = 1) and after cflx_chol_rbt.  CFLX_ERR_STATE before cflx_chol_set_local. */
+int cflx_chol_get_input(cflx_chol*, double* A_host);
 int cflx_chol_get_local(cflx_chol*, double* L_host);
 /* COLLECTIVE.  ||A - L L^T||_F over the lower triangle, absolute and relative to ||A||_F, computed on the GPU grid. */
 int cflx_chol_validate(cflx_chol*, double* frob_abs_out, double* frob_rel_out);
@@ -377,7 +421,7 @@ int cflx_chol_equilibrate_b(cflx_chol*, int apply, double* s_out, double* scond_
                             int* info_out);
 /* COLLECTIVE.  LAPACK dposvxx (UPLO = 'L') after a successful factorisation, with the scaling the factor carries:
  * rpvgrw_out (may be NULL) = dla_porpvgrw, the minimum of 1 and of max |a_ij| / max |l_ij| over the rows i >= j of the
- * stored lower triangles, per column j with a non-zero denominator; rcond_out = dpocon; B scaled by s, solved, refined as
+ * stored lower triangles, per column j with a non-zero denominator (after cflx_chol_factor_ldlt, of R); rcond_out = dpocon; B scaled by s, solved, refined as
  * cflx_chol_refine_x refines it and unscaled by s.  info_out: N + j from the refinement, else 0.  A factorisation that
  * found a non-positive pivot is refused (CFLX_ERR_STATE), where dposvxx would return info = k.  Arguments, results and
  * side effects otherwise as cflx_lu_svxx without trans. */
@@ -392,7 +436,8 @@ int cflx_chol_svxx(cflx_chol*, int nrhs, const double* B, int ldb, double* X, in
 int cflx_chol_inverse(cflx_chol*, double* Ainv_local);
 /* COLLECTIVE.  det = prod(l_ii)^2 of the padded N x N matrix of the last successful cflx_chol_factor: logdet_out, and the
  * exact-range det mant_out 2^exp_out as cflx_lu_det's; unscaled = 1 divides by prod(s)^2 of the scaling the factor
- * carries (equed 'Y').  Any output may be NULL.  Determinism and side effects as cflx_lu_det; CFLX_ERR_ARG for unscaled
+ * carries (equed 'Y').  After cflx_chol_factor_ldlt, det = prod(s_i r_ii^2): mant_out carries its sign and logdet_out is
+ * log |det|.  Any output may be NULL.  Determinism and side effects as cflx_lu_det; CFLX_ERR_ARG for unscaled
  * not 0 / 1; CFLX_ERR_STATE as cflx_chol_solve. */
 int cflx_chol_det(cflx_chol*, int unscaled, double* logdet_out, double* mant_out, int64_t* exp_out);
 /* number of kernels this object counted since the last reset (bench.py's gpu_launches); cflx_chol_solve adds none */
@@ -576,6 +621,16 @@ int cflx_dbg_diag_inverse(int v, int nb, const double* A00, double* Uinv_out, do
  * 4 <= v <= 512; 1: the 128 x 128 block kernel, v == 128; 2: the 128-block tile driver, v % 128 == 0 and v >= 256.
  * L_out = L with zeros above the diagonal, LT_out = L^T, info_out = 1 + first non-positive pivot's column, or 0. */
 int cflx_dbg_potrf_tile(int v, const double* A, double* L_out, double* LT_out, int* info_out, int variant);
+/* the sign pass between the two sweeps of a solve with a signed Cholesky factor (cflx_chol_factor_ldlt) on one share's
+ * column-partial buffer Z (Nl x ldn row-major, tiled share): Z[r][j] *= sgn[global column of local column r] where that
+ * global column is < M; sgn: M doubles */
+int cflx_dbg_solve_signs(const cflx_share_layout* share, int ldn, const double* sgn, double* Z_inout);
+/* The signed Cholesky A = R S R^T of one v x v row-major tile (lower triangle read) on the kernels of
+ * cflx_chol_factor_ldlt, variants and v as cflx_dbg_potrf_tile: R_out = R (zeros above the diagonal), SRT_out = S R^T,
+ * s_out[v] the signs, nrepl_out the tiny rule's replacements, inertia_out[3] the positive, negative and zero pivots,
+ * info_out = 1 + the first exactly zero pivot's column or 0. */
+int cflx_dbg_ldlt_tile(int v, const double* A, double tiny, double* R_out, double* SRT_out, double* s_out, int* nrepl_out,
+                       int* inertia_out, int* info_out, int variant);
 /* Unpivoted LU of one v x v row-major block as cflx_lu_factor_fixed runs it (4 <= v <= 1024, v % 4 == 0).  variant 0:
  * the one-CTA kernel on the whole block; 1: the 128-block driver (v % 128 == 0, v >= 256, what the factorisation runs
  * there: 128 x 128 diagonal blocks on the one-CTA kernel, the rest on the TRSMs and the FP64 GEMM).  LU_out = L\U with unit L, pivots |u| < tiny replaced by copysign(tiny, u) (+tiny for
