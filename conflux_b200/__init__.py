@@ -305,6 +305,35 @@ def lu_solve(gv, B, trans=False):
     return X.reshape(B.shape)
 
 
+_PREC = {"tf32": 1, "tf32x3": 3}
+
+
+def _sv_mixed(fn, what, h, n, B, prec, itmax):
+    if prec not in _PREC:
+        raise ValueError(f"{what}: prec must be one of {sorted(_PREC)}, got {prec!r}")
+    B, B2, nrhs = _rhs(n, B, what)
+    X = np.empty_like(B2)
+    be = np.empty(nrhs)
+    it, ms = ctypes.c_int(), ctypes.c_double()
+    check(fn(h, _PREC[prec], nrhs, B2.ctypes.data, nrhs, X.ctypes.data, nrhs, int(itmax), ctypes.byref(it), be.ctypes.data,
+             ctypes.byref(ms)), what)
+    return X.reshape(B.shape), it.value, be
+
+
+def lu_sv_mixed(gv, B, prec="tf32x3", itmax=0, upload=True):
+    """LAPACK dsgesv on the GPU grid: factors the input (upload=True copies gv.data to the device first; upload=False
+    takes the one already there) with the trailing update on the TF32 tensor cores (prec "tf32": one term, "tf32x3": three), then refines x in FP64 against
+    that input until ||b - A x||_inf <= ||x||_inf ||A||_inf eps sqrt(M) for every column, at most itmax corrections (0:
+    30).  Returns (X, iter, berr): X in B's shape; iter the corrections taken, -3 (a zero pivot) or -31 (no convergence),
+    in which case X comes from an FP64 refactorisation exactly as LU_rep + lu_solve give it; berr per column ||r||_inf /
+    (||A||_inf ||x||_inf).  After a converged run the handle holds the low-precision factors: lu_solve, lu_refine and the
+    other calls that need FP64 factors refuse until the next LU_rep.  COLLECTIVE; identical on every rank."""
+    if upload:
+        a = np.ascontiguousarray(gv.data, dtype=np.float64)
+        check(lib().cflx_lu_set_local(gv._h, a.ctypes.data), "lu_set_local")
+    return _sv_mixed(lib().cflx_lu_sv_mixed, "lu_sv_mixed", gv._h, gv.M, B, prec, itmax)
+
+
 def lu_rcond(gv):
     """LAPACK dgecon (1-norm) of the last LU_rep on the GPU grid: (rcond, anorm) with anorm = ||A||_1 of the padded input
     and rcond = 1 / (anorm * estimate of ||A^-1||_1), 0 for an exactly singular U.  COLLECTIVE; identical on every rank."""
@@ -642,6 +671,16 @@ class cholesky:
         X = np.empty_like(B2)
         check(lib().cflx_chol_solve(self._h, nrhs, B2.ctypes.data, max(nrhs, 1), X.ctypes.data, max(nrhs, 1)), "chol_solve")
         return X.reshape(B.shape)
+
+    def sv_mixed(self, B, prec="tf32x3", itmax=0, upload=True):
+        """LAPACK dsposv on the GPU grid: lu_sv_mixed's loop on the Cholesky path (upload=True copies self.data to the
+        device first).  Returns (X, iter, berr) as lu_sv_mixed; iter -3 when the low-precision factorisation met a
+        non-positive pivot.  Raises ConfluxError when the FP64 fallback finds the matrix not positive definite.
+        COLLECTIVE; identical on every rank."""
+        if upload:
+            a = np.ascontiguousarray(self.data, dtype=np.float64)
+            check(lib().cflx_chol_set_local(self._h, a.ctypes.data), "chol_set_local")
+        return _sv_mixed(lib().cflx_chol_sv_mixed, "cholesky.sv_mixed", self._h, self.N, B, prec, itmax)
 
     def solve_local(self, B_share, nrhs, out=None):
         """Solves A X = B with the factor of the last parallelCholesky, like ScaLAPACK's pdpotrs, with B and X distributed
@@ -1262,6 +1301,28 @@ class dbg:
                                         _ptr(Cp), D.ctypes.data, _ptr(pa), _ptr(pb), _ptr(ea), _ptr(eb), int(reps),
                                         ctypes.byref(ms), ctypes.byref(sms)), "dbg_ozaki_gemm")
         return dict(D=D, ms=ms.value, split_ms=sms.value, pa=pa, pb=pb, ea=ea, eb=eb)
+
+    @staticmethod
+    def gemm_tf32(terms, AT, B, C=None, reps=1, row0=0, col0=0, max_ctas=0):
+        """D = C - AT[:, row0:]^T B[:, col0:] on the TF32 wgmma path (terms 1 or 3); AT (K, row0 + M), B (K, col0 + N).
+        Returns dict(D, ms, split_ms, hiA, loA, hiB, loB, ea, eb): the split terms as float32 (rows, KP) arrays (lo None
+        with one term) and the int32 exponents, exactly as the kernels produced them."""
+        AT = np.ascontiguousarray(AT, dtype=np.float64)
+        B = np.ascontiguousarray(B, dtype=np.float64)
+        K, Ma = AT.shape
+        Nb = B.shape[1]
+        M, N = Ma - int(row0), Nb - int(col0)
+        KP = (K + 7) // 8 * 8
+        Cp = None if C is None else np.ascontiguousarray(C, dtype=np.float64)
+        D = np.empty((M, N))
+        hiA, hiB = np.empty((Ma, KP), np.float32), np.empty((Nb, KP), np.float32)
+        loA, loB = (np.empty((Ma, KP), np.float32), np.empty((Nb, KP), np.float32)) if terms == 3 else (None, None)
+        ea, eb = np.empty(Ma, np.int32), np.empty(Nb, np.int32)
+        ms, sms = ctypes.c_double(), ctypes.c_double()
+        check(lib().cflx_dbg_gemm_tf32(int(terms), M, N, K, int(row0), int(col0), int(max_ctas), AT.ctypes.data,
+                                       B.ctypes.data, _ptr(Cp), D.ctypes.data, _ptr(hiA), _ptr(loA), _ptr(hiB), _ptr(loB),
+                                       _ptr(ea), _ptr(eb), int(reps), ctypes.byref(ms), ctypes.byref(sms)), "dbg_gemm_tf32")
+        return dict(D=D, ms=ms.value, split_ms=sms.value, hiA=hiA, loA=loA, hiB=hiB, loB=loB, ea=ea, eb=eb)
 
     @staticmethod
     def push_pivots(A, pivot_rows, fnpr):

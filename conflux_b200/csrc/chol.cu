@@ -512,7 +512,10 @@ int update_columns(cflx_chol* ch, int gfirst, int jmin, int buf, double* X, int 
         g.D = const_cast<double*>(g.C);
         g.ldd = Nl;
         g.alpha = -1.0; g.beta = 1.0;
-        if (ch->use_ozaki && planes_buf == buf)   // planes of this buffer set are current (see split_planes)
+        if (ch->update_terms && planes_buf == buf)   // TF32 terms of this buffer set are current (see split_planes)
+            CFLX_TRY(launch_tf32_gemm(&ch->tf, ch->update_terms, M, g.N, (li - my_first) * v, (lj - lj0) * v, g.D, Nl,
+                                      ch->tf.sms - chol_leave_sms(), s));
+        else if (ch->use_ozaki && planes_buf == buf)   // planes of this buffer set are current (see split_planes)
             CFLX_TRY(launch_ozaki_gemm(&ch->oz, M, g.N, (li - my_first) * v, (lj - lj0) * v, g.D, Nl, ch->oz.sms - chol_leave_sms(), s));
         else
             CFLX_TRY(launch_gemm_tn(g, s));
@@ -522,10 +525,11 @@ int update_columns(cflx_chol* ch, int gfirst, int jmin, int buf, double* X, int 
     (void)my_rows;
     return CFLX_OK;
 }
-// digit planes of the operands of one update sweep: my piece (rows) and the gathered column operand, this layer's slab
+// digit planes (or, in a TF32 update mode, the TF32 terms) of the operands of one update sweep: my piece (rows) and the
+// gathered column operand, this layer's slab
 int split_planes(cflx_chol* ch, int gfirst, int jmin, int buf, cudaStream_t s);
 int split_planes(cflx_chol* ch, int gfirst, int jmin, int buf, cudaStream_t s) {
-    if (!ch->use_ozaki) return CFLX_OK;
+    if (!ch->use_ozaki && !ch->update_terms) return CFLX_OK;
     const int v = ch->v, Px = ch->Px;
     const int64_t piece_stride = (int64_t)v * ch->ldp;
     const double* G = ch->G + (int64_t)buf * Px * piece_stride;
@@ -534,8 +538,15 @@ int split_planes(cflx_chol* ch, int gfirst, int jmin, int buf, cudaStream_t s) {
     const int rows = ch->Ml - my_first * v;
     const int ncols = ch->Nl - first_local_tile(jmin, ch->pj, ch->Py) * v;
     const int64_t ldg = piece_ld(ch, gfirst, ch->pi);
-    if (rows > 0) CFLX_TRY(ozaki_split_a(&ch->oz, G + (int64_t)ch->pi * piece_stride + (int64_t)ch->pk * ch->nlayr * ldg, ldg, rows, s));
-    if (ncols > 0) CFLX_TRY(ozaki_split_b(&ch->oz, Bc + (int64_t)ch->pk * ch->nlayr * ch->ldb, ch->ldb, 0, ncols, s));
+    const double* A = G + (int64_t)ch->pi * piece_stride + (int64_t)ch->pk * ch->nlayr * ldg;
+    const double* B = Bc + (int64_t)ch->pk * ch->nlayr * ch->ldb;
+    if (ch->update_terms) {
+        if (rows > 0) CFLX_TRY(tf32_split_a(&ch->tf, ch->update_terms, A, ldg, rows, s));
+        if (ncols > 0) CFLX_TRY(tf32_split_b(&ch->tf, ch->update_terms, B, ch->ldb, 0, ncols, s));
+    } else {
+        if (rows > 0) CFLX_TRY(ozaki_split_a(&ch->oz, A, ldg, rows, s));
+        if (ncols > 0) CFLX_TRY(ozaki_split_b(&ch->oz, B, ch->ldb, 0, ncols, s));
+    }
     ch->launches += 2;
     return CFLX_OK;
 }
@@ -1082,6 +1093,7 @@ int chol_factor_run(cflx_chol* ch, float* ms_out, int* bad_out, int* cnt) {
         bad = h[2] == INT_MAX ? 0 : h[2];
     }
     *bad_out = bad;
+    ch->low_prec = ch->update_terms != 0;
     if (cnt) std::memcpy(cnt, h + 4, 4 * sizeof(int));
     *ms_out = ms;
     return CFLX_OK;
@@ -1214,7 +1226,7 @@ int cflx_chol_validate(cflx_chol* ch, double* abs_out, double* rel_out) {
 int cflx_chol_solve(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X, int ldx) {
     REFUSE_IF(!ch);
     CFLX_TRY(rhs_args(__func__, nrhs, B, ldb, X, ldx, false));
-    CFLX_TRY(enter(ch, __func__, NEED_FACTORS));
+    CFLX_TRY(enter(ch, __func__, NEED_FACTORS | NEED_FP64));
     return chol_sweeps(ch, nrhs, B, ldb, X, ldx);
 }
 
@@ -1224,7 +1236,7 @@ int cflx_chol_solve_local(cflx_chol* ch, int nrhs, const double* B_local, int ld
     REFUSE_IF(!ch);
     SolveLocalArgs a{};
     CFLX_TRY(solve_local_args(__func__, *ch, nrhs, B_local, ldb, X_local, ldx, &a));
-    CFLX_TRY(enter(ch, __func__, NEED_FACTORS));
+    CFLX_TRY(enter(ch, __func__, NEED_FACTORS | NEED_FP64));
     auto solve = [ch](int w, const double* Bk, int ldn, const double** Xk) -> int {
         CFLX_TRY(chol_sweeps(ch, w, Bk, ldn, nullptr, 0));
         *Xk = ch->sv.X;
@@ -1237,7 +1249,7 @@ int cflx_chol_solve_local(cflx_chol* ch, int nrhs, const double* B_local, int ld
 // cflx_chol_solve, the lower tiles of each block column scattered into this rank's share, the rest of it zero.
 int cflx_chol_inverse(cflx_chol* ch, double* Ainv_local) {
     REFUSE_IF(!ch);
-    CFLX_TRY(enter(ch, __func__, NEED_FACTORS));
+    CFLX_TRY(enter(ch, __func__, NEED_FACTORS | NEED_FP64));
     if (!ch->sv.ready) CFLX_TRY(chol_solve_prepare(ch));
     return inverse_run(&ch->sv, chol_solve_factor(ch), InvKind::Chol, nullptr, Ainv_local);
 }
@@ -1247,7 +1259,7 @@ int cflx_chol_inverse(cflx_chol* ch, double* Ainv_local) {
 int cflx_chol_det(cflx_chol* ch, int unscaled, double* logdet_out, double* mant_out, int64_t* exp_out) {
     REFUSE_IF(!ch);
     REFUSE_IF(unscaled != 0 && unscaled != 1);
-    CFLX_TRY(enter(ch, __func__, NEED_FACTORS));
+    CFLX_TRY(enter(ch, __func__, NEED_FACTORS | NEED_FP64));
     const double* s = unscaled && ch->eq.fac.equed == 'Y' ? ch->eq.fac.r.p : nullptr;
     DetResult d{};
     CFLX_TRY(det_grid(*ch, &ch->eq, ch->A11, true, s, nullptr, &d));
@@ -1266,7 +1278,7 @@ int cflx_chol_det(cflx_chol* ch, int unscaled, double* logdet_out, double* mant_
 int cflx_chol_rcond(cflx_chol* ch, double* rcond_out, double* anorm_out) {
     REFUSE_IF(!ch);
     REFUSE_IF(!rcond_out);
-    CFLX_TRY(enter(ch, __func__, NEED_FACTORS));
+    CFLX_TRY(enter(ch, __func__, NEED_FACTORS | NEED_FP64));
     return chol_rcond(ch, rcond_out, anorm_out);
 }
 
@@ -1276,7 +1288,7 @@ int cflx_chol_refine(cflx_chol* ch, int nrhs, const double* B, int ldb, double* 
                      double* berr_out) {
     REFUSE_IF(!ch);
     CFLX_TRY(rhs_args(__func__, nrhs, B, ldb, X, ldx, true));
-    CFLX_TRY(enter(ch, __func__, NEED_FACTORS));
+    CFLX_TRY(enter(ch, __func__, NEED_FACTORS | NEED_FP64));
     return refine_run(&ch->sv.rf, chol_refine_op(ch), nrhs, B, ldb, X, ldx, ferr_out, berr_out);
 }
 
@@ -1288,7 +1300,7 @@ int cflx_chol_refine_x(cflx_chol* ch, int nrhs, const double* B, int ldb, double
     CFLX_TRY(rhs_args(__func__, nrhs, B, ldb, X, ldx, true));
     REFUSE_IF(!err_bnds_norm_out);
     REFUSE_IF(!info_out);
-    CFLX_TRY(enter(ch, __func__, NEED_FACTORS));
+    CFLX_TRY(enter(ch, __func__, NEED_FACTORS | NEED_FP64));
     double rcond = 0.0;
     CFLX_TRY(chol_rcond(ch, &rcond, nullptr));
     if (rcond_out) *rcond_out = rcond;
@@ -1318,7 +1330,7 @@ int cflx_chol_svx(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X, 
     CFLX_TRY(rhs_args(__func__, nrhs, B, ldb, X, ldx, true));
     REFUSE_IF(!rcond_out);
     REFUSE_IF(!info_out);
-    CFLX_TRY(enter(ch, __func__, NEED_FACTORS));
+    CFLX_TRY(enter(ch, __func__, NEED_FACTORS | NEED_FP64));
     const EquilRecord& eq = ch->eq.fac;
     const double* s = eq.equed == 'Y' ? eq.r.p : nullptr;
     if (equed_out) *equed_out = eq.equed;
@@ -1340,7 +1352,7 @@ int cflx_chol_svxx(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X,
     REFUSE_IF(!rcond_out);
     REFUSE_IF(!err_bnds_norm_out);
     REFUSE_IF(!info_out);
-    CFLX_TRY(enter(ch, __func__, NEED_FACTORS));
+    CFLX_TRY(enter(ch, __func__, NEED_FACTORS | NEED_FP64));
     const EquilRecord& eq = ch->eq.fac;
     const double* s = eq.equed == 'Y' ? eq.r.p : nullptr;
     if (equed_out) *equed_out = eq.equed;
@@ -1352,6 +1364,57 @@ int cflx_chol_svxx(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X,
     *rcond_out = rcond;
     return svxx_run(&ch->eq, &ch->sv.rf, chol_refine_op(ch), nrhs, B, ldb, X, ldx, s, s, s, rcond,
                     err_bnds_comp_out != nullptr, berr_out, err_bnds_norm_out, err_bnds_comp_out, info_out);
+}
+
+// COLLECTIVE.  LAPACK dsposv on the grid: the input factored with the TF32 trailing update (prec 1: one term, 3: three),
+// then mixed_run's refinement in FP64 on the stored lower triangle of A0.  When the low-precision factorisation meets a
+// non-positive pivot (iter -3) or the loop does not converge (-31), the input is factored again in FP64 and solved, as
+// cflx_chol_factor + cflx_chol_solve do; the handle then holds that FP64 factor, or none when the FP64 factorisation
+// fails too (CFLX_ERR_STATE as cflx_chol_factor, with *iter_out set).
+int cflx_chol_sv_mixed(cflx_chol* ch, int prec, int nrhs, const double* B, int ldb, double* X, int ldx, int itmax,
+                       int* iter_out, double* berr_out, double* ms_out) {
+    REFUSE_IF(!ch);
+    REFUSE_IF(prec != CFLX_PREC_TF32 && prec != CFLX_PREC_TF32X3);
+    REFUSE_IF(!iter_out);
+    CFLX_TRY(rhs_args(__func__, nrhs, B, ldb, X, ldx, true));
+    CFLX_TRY(enter(ch, __func__, NEED_INPUT | NEED_UNSCALED));
+    if (ch->rbt.in.depth) {
+        set_last_error("%s: refused, the input carries a random butterfly transform (cflx_chol_rbt); upload it again first",
+                       __func__);
+        return CFLX_ERR_STATE;
+    }
+    ch->ldlt = false;
+    CFLX_TRY(handle_tf32_begin(ch, prec));
+    float ms = 0;
+    int bad = 0;
+    const int run = chol_factor_run(ch, &ms, &bad, nullptr);
+    ch->update_terms = 0;
+    CFLX_TRY(run);
+    double anorm = 0.0;  // the infinity-norm of the symmetric matrix is its 1-norm
+    CFLX_TRY(norm1_grid(*ch, ch->A0, true, &anorm));
+    int iter = MIXED_LOW_PREC_FAILED;
+    if (bad == 0) {
+        ch->factored = true;
+        CFLX_TRY(mixed_run(&ch->sv.rf, chol_refine_op(ch), anorm, itmax > 0 ? itmax : MIXED_ITMAX, nrhs, B, ldb, X, ldx,
+                           &iter, berr_out));
+    }
+    *iter_out = iter;
+    double total = ms;
+    if (iter < 0) {
+        CFLX_TRY(chol_factor_run(ch, &ms, &bad, nullptr));
+        total += ms;
+        if (ms_out) *ms_out = total;
+        if (bad != 0) {
+            set_last_error("%s: the matrix is not positive definite (first non-positive pivot of the FP64 factorisation in "
+                           "column %d, counted from 1 like LAPACK dpotrf's info)", __func__, bad);
+            return CFLX_ERR_STATE;
+        }
+        ch->factored = true;
+        CFLX_TRY(chol_sweeps(ch, nrhs, B, ldb, X, ldx));
+        if (berr_out) CFLX_TRY(mixed_berr(&ch->sv.rf, chol_refine_op(ch), anorm, nrhs, B, ldb, X, ldx, berr_out));
+    }
+    if (ms_out) *ms_out = total;
+    return CFLX_OK;
 }
 
 // The signs S of the last factorisation: those of cflx_chol_factor_ldlt, or all +1 after cflx_chol_factor
@@ -1426,7 +1489,7 @@ int cflx_chol_rbt_solve(cflx_chol* ch, int nrhs, const double* B, int ldb, doubl
     REFUSE_IF(!ch);
     REFUSE_IF(refine != 0 && refine != 1);
     CFLX_TRY(rhs_args(__func__, nrhs, B, ldb, X, ldx, true));
-    CFLX_TRY(enter(ch, __func__, NEED_FACTORS));
+    CFLX_TRY(enter(ch, __func__, NEED_FACTORS | NEED_FP64));
     if (!ch->rbt.fac.depth) {
         set_last_error("%s: the factor carries no random butterfly transform (cflx_chol_rbt before the factorisation)",
                        __func__);

@@ -1200,6 +1200,66 @@ int cflx_dbg_ozaki_gemm(int M, int N, int K, int row0, int col0, int max_ctas, c
     return rc;
 }
 
+// D = C - AT^T * B on the TF32 wgmma path (tf32.cu): the split of every operand row, then one launch of the product
+int cflx_dbg_gemm_tf32(int terms, int M, int N, int K, int row0, int col0, int max_ctas, const double* AT, const double* B,
+                       const double* C, double* D, float* hiA_out, float* loA_out, float* hiB_out, float* loB_out,
+                       int* ea_out, int* eb_out, int reps, double* ms_out, double* split_ms_out) {
+    CFLX_TRY(check_device());
+    REFUSE_IF(terms != 1 && terms != 3);
+    REFUSE_IF(M <= 0 || N <= 0 || K <= 0);
+    REFUSE_IF(row0 < 0 || col0 < 0 || max_ctas < 0);
+    REFUSE_IF(!AT || !B || !D);
+    const int Ma = row0 + M, Nb = col0 + N;
+    const int64_t ldat = Ma, ldb = Nb, ldc = round_up(N, 2);
+    DevBuf<> dA, dB, dC, dC0;
+    CFLX_TRY(stage(dA, K * ldat, AT));
+    CFLX_TRY(stage(dB, K * ldb, B));
+    CFLX_TRY(stage(dC, (size_t)M * ldc));
+    CFLX_TRY(stage(dC0, (size_t)M * ldc));
+    CFLX_CUDA(cudaMemset(dC0.p, 0, sizeof(double) * M * ldc));
+    if (C) CFLX_CUDA(cudaMemcpy2D(dC0.p, ldc * 8, C, (size_t)N * 8, (size_t)N * 8, M, cudaMemcpyHostToDevice));
+    Events<3> ev;
+    CFLX_TRY(ev.create());
+    Tf32Workspace ws;
+    int rc = tf32_workspace_create(&ws, Ma, Nb, K);
+    if (reps < 1) reps = 1;
+    float ms = 0, ms_split = 0;
+    for (int r = 0; r < reps + 1 && rc == CFLX_OK; ++r) {
+        cudaMemcpyAsync(dC.p, dC0.p, sizeof(double) * M * ldc, cudaMemcpyDeviceToDevice, 0);
+        cudaEventRecord(ev[0]);
+        rc = tf32_split_a(&ws, terms, dA.as<double>(), ldat, Ma, 0);
+        if (!rc && col0 > 0) rc = tf32_split_b(&ws, terms, dB.as<double>(), ldb, 0, col0, 0);
+        if (!rc) rc = tf32_split_b(&ws, terms, dB.as<double>(), ldb, col0, N, 0);
+        cudaEventRecord(ev[1]);
+        if (!rc) rc = launch_tf32_gemm(&ws, terms, M, N, row0, col0, dC.as<double>(), ldc, max_ctas, 0);
+        cudaEventRecord(ev[2]);
+        if (cudaEventSynchronize(ev[2]) != cudaSuccess) {
+            set_last_error("tf32 kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
+            rc = CFLX_ERR_CUDA;
+        }
+        float a = 0, b = 0;
+        cudaEventElapsedTime(&a, ev[0], ev[1]);
+        cudaEventElapsedTime(&b, ev[1], ev[2]);
+        if (r > 0) {
+            ms_split += a;
+            ms += b;
+        }
+    }
+    if (rc == CFLX_OK && cudaMemcpy2D(D, (size_t)N * 8, dC.p, ldc * 8, (size_t)N * 8, M, cudaMemcpyDeviceToHost) != cudaSuccess)
+        rc = CFLX_ERR_CUDA;
+    const size_t na = (size_t)Ma * ws.KP, nb = (size_t)Nb * ws.KP;
+    if (rc == CFLX_OK) rc = fetch(hiA_out, ws.hiA.p, na);
+    if (rc == CFLX_OK && terms == 3) rc = fetch(loA_out, ws.loA.p, na);
+    if (rc == CFLX_OK) rc = fetch(hiB_out, ws.hiB.p, nb);
+    if (rc == CFLX_OK && terms == 3) rc = fetch(loB_out, ws.loB.p, nb);
+    if (rc == CFLX_OK) rc = fetch(ea_out, ws.ea, Ma);
+    if (rc == CFLX_OK) rc = fetch(eb_out, ws.eb, Nb);
+    if (rc == CFLX_OK && cudaDeviceSynchronize() != cudaSuccess) rc = CFLX_ERR_CUDA;
+    if (ms_out) *ms_out = ms / reps;
+    if (split_ms_out) *split_ms_out = ms_split / reps;
+    return rc;
+}
+
 // raw int8 tensor-core rate of back-to-back wgmma 64 x n x 32 instructions (two warpgroups per CTA, one CTA per SM,
 // operands resident in shared memory).  Returns tera-MACs per second (x2 = TOP/s).
 int cflx_dbg_wgmma_peak(int n, double* tmacs_out) {

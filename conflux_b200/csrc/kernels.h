@@ -46,6 +46,29 @@ int ozaki_split_b(OzakiWorkspace* ws, const double* U, int64_t ld, int col0, int
 int wgmma_peak_probe(int n, double* tmacs_out);
 int launch_ozaki_gemm(OzakiWorkspace* ws, int M, int N, int row0, int col0, double* C, int64_t ldc, int max_ctas, cudaStream_t s);
 
+// ---------------------------------------------------------------- tf32.cu
+// The low-precision trailing update of the mixed-precision drivers on the TF32 wgmma path: C -= L * U with L^T, U K-major
+// in HBM, split into per-row power-of-two scaled TF32 terms (hi, and lo for terms = 3), FP32 accumulation, FP64 C.
+struct Tf32Workspace {
+    struct Maps;               // the four CUtensorMap objects (kept out of this header)
+    DevBuf<float> hiA, loA;    // [cap_a][KP]
+    DevBuf<float> hiB, loB;    // [cap_b][KP]
+    DevBuf<int> ea;            // [cap_a]
+    DevBuf<int> eb;            // [cap_b]
+    std::unique_ptr<Maps> maps;
+    int K = 0, KP = 0, cap_a = 0, cap_b = 0, sms = 0;  // KP: K rounded up to 8 (the tail is zero)
+    Tf32Workspace();
+    ~Tf32Workspace();  // where Maps is complete
+};
+// on a new workspace; any K >= 1
+int tf32_workspace_create(Tf32Workspace* ws, int max_rows, int max_cols, int K);
+// terms 1 or 3 (3 also writes the lo slabs)
+int tf32_split_a(Tf32Workspace* ws, int terms, const double* LT, int64_t ld, int n, cudaStream_t s);
+int tf32_split_b(Tf32Workspace* ws, int terms, const double* U, int64_t ld, int col0, int n, cudaStream_t s);
+// launch_ozaki_gemm's window; ldc even, C 16-byte aligned, any M, N >= 1
+int launch_tf32_gemm(Tf32Workspace* ws, int terms, int M, int N, int row0, int col0, double* C, int64_t ldc, int max_ctas,
+                     cudaStream_t s);
+
 // ---------------------------------------------------------------- panel.cu
 // Partial-pivot LU of the n x v panel stored TRANSPOSED in W (W[c][r], ld = ldw), in place, rows never move:
 // afterwards W[:, r] holds row r of L\U (multipliers left of its pivot column, U from it on, for pivot rows;

@@ -165,6 +165,9 @@ int enter(Handle* h, const char* who, unsigned need) {
     else if ((need & NEED_FACTORS) && !h->factored) snprintf(why, sizeof(why), "%s", t.unfactored);
     else if ((need & NEED_OWN_INPUT) && h->a0_is_next)
         snprintf(why, sizeof(why), "refused: the input buffer of the last run was handed to the queued next matrix");
+    else if ((need & NEED_FP64) && h->low_prec)
+        snprintf(why, sizeof(why), "refused: the factors come from the TF32 trailing update of a mixed-precision driver, "
+                                   "not from an FP64 factorisation; factor again first");
     if (why[0]) {
         set_last_error("%s: %s", who, why);
         return CFLX_ERR_STATE;
@@ -178,6 +181,11 @@ void handle_equil_begin(Handle* h) {
 }
 int handle_equil_end(Handle* h, bool apply, int info, char equed, double rowcnd, double colcnd, const double* c) {
     if (apply && info == 0) CFLX_TRY(equil_record_set(&h->eq.in, equed, rowcnd, colcnd, h->eq.qr, c, h->M, h->comm->stream));
+    return CFLX_OK;
+}
+int handle_tf32_begin(Handle* h, int terms) {
+    if (!h->tf.maps) CFLX_TRY(tf32_workspace_create(&h->tf, h->Ml, h->Nl, std::max(h->nlayr, 1)));
+    h->update_terms = terms;
     return CFLX_OK;
 }
 int handle_launch_count(Handle* h, int64_t* count_out, int reset) {
@@ -383,17 +391,22 @@ int panel_phase(cflx_lu* lu, int k, int fnpr, cudaStream_t s) {
 }
 
 // digit planes of the operands of this step's trailing update (int8 wgmma path): L^T slab of this layer, U slab columns
+// (or, in a TF32 update mode, the TF32 terms of both slabs)
 int ozaki_planes_a(cflx_lu* lu, int n_act, int64_t ld2, cudaStream_t s) {
-    if (!lu->use_ozaki || n_act <= 0) return CFLX_OK;
+    if (!(lu->use_ozaki || lu->update_terms) || n_act <= 0) return CFLX_OK;
     PhaseTimer t(lu, RG_step6_dgemm, s);
     lu->launches++;
-    return ozaki_split_a(&lu->oz, lu->LT + (int64_t)lu->pk * lu->nlayr * ld2, ld2, n_act, s);
+    const double* LT = lu->LT + (int64_t)lu->pk * lu->nlayr * ld2;
+    if (lu->update_terms) return tf32_split_a(&lu->tf, lu->update_terms, LT, ld2, n_act, s);
+    return ozaki_split_a(&lu->oz, LT, ld2, n_act, s);
 }
 int ozaki_planes_b(cflx_lu* lu, int col0, int n, int64_t ldu, cudaStream_t s) {
-    if (!lu->use_ozaki || n <= 0) return CFLX_OK;
+    if (!(lu->use_ozaki || lu->update_terms) || n <= 0) return CFLX_OK;
     PhaseTimer t(lu, RG_step6_dgemm, s);
     lu->launches++;
-    return ozaki_split_b(&lu->oz, lu->U + (int64_t)lu->pk * lu->nlayr * ldu, ldu, col0, n, s);
+    const double* U = lu->U + (int64_t)lu->pk * lu->nlayr * ldu;
+    if (lu->update_terms) return tf32_split_b(&lu->tf, lu->update_terms, U, ldu, col0, n, s);
+    return ozaki_split_b(&lu->oz, U, ldu, col0, n, s);
 }
 
 int trailing_gemm(cflx_lu* lu, int k, int part, int fnpr, int n_act, int col_lo, int ncols, int64_t ld2, int64_t ldu,
@@ -416,7 +429,9 @@ int trailing_gemm(cflx_lu* lu, int k, int part, int fnpr, int n_act, int col_lo,
     g.beta = 1.0;
     const int e = 4 * k + 2 * part;
     if (lu->time_gemm) CFLX_CUDA(cudaEventRecord(lu->ev[e], s));
-    if (lu->use_ozaki) CFLX_TRY(launch_ozaki_gemm(&lu->oz, g.M, g.N, 0, u_col_off, g.D, g.ldd, max_ctas, s));
+    if (lu->update_terms)
+        CFLX_TRY(launch_tf32_gemm(&lu->tf, lu->update_terms, g.M, g.N, 0, u_col_off, g.D, g.ldd, max_ctas, s));
+    else if (lu->use_ozaki) CFLX_TRY(launch_ozaki_gemm(&lu->oz, g.M, g.N, 0, u_col_off, g.D, g.ldd, max_ctas, s));
     else CFLX_TRY(launch_gemm_tn(g, s));
     if (lu->time_gemm) CFLX_CUDA(cudaEventRecord(lu->ev[e + 1], s));
     lu->ev_used[e / 2] = lu->time_gemm;
@@ -585,9 +600,10 @@ int finish_step(cflx_lu* lu, int k, int& fnpr) {
         }
         if (split_u) CFLX_TRY(store_factors());
         if (split_u && n_act > 0) CFLX_TRY(ozaki_planes_b(lu, w, ncols - w, ldu, s));
-        // the persistent int8 kernel leaves the SMs of the concurrent pivot search alone
-        const int leave = (side && lu->use_ozaki) ? lu->pws.cta_cap : 0;
-        CFLX_TRY(trailing_gemm(lu, k, 1, fnpr, n_act, c0 + w, ncols - w, ld2, ldu, w, s, leave > 0 ? lu->oz.sms - leave : 0));
+        // the persistent int8 and TF32 kernels leave the SMs of the concurrent pivot search alone
+        const int leave = (side && (lu->use_ozaki || lu->update_terms)) ? lu->pws.cta_cap : 0;
+        const int sms = lu->update_terms ? lu->tf.sms : lu->oz.sms;
+        CFLX_TRY(trailing_gemm(lu, k, 1, fnpr, n_act, c0 + w, ncols - w, ld2, ldu, w, s, leave > 0 ? sms - leave : 0));
         if (side) CFLX_CUDA(cudaStreamWaitEvent(s, lu->ev_join, 0));
     } else {
         CFLX_TRY(trailing_gemm(lu, k, 0, fnpr, n_act, c0, ncols, ld2, ldu, 0, s));
@@ -1133,6 +1149,7 @@ int lu_factor_run(cflx_lu* lu, double* ms_out) {
     }
     if (lu->a0_is_next) CFLX_CUDA(cudaStreamSynchronize(lu->copy));  // the caller's staging buffer is free again
     lu->factored = true;
+    lu->low_prec = lu->update_terms != 0;
     lu->perm_done = true;
     return CFLX_OK;
 }
@@ -1320,7 +1337,7 @@ int cflx_lu_rbt_solve(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb
     REFUSE_IF(trans != 0 && trans != 1);
     REFUSE_IF(refine != 0 && refine != 1);
     CFLX_TRY(rhs_args(__func__, nrhs, B, ldb, X, ldx, true));
-    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | (refine ? NEED_OWN_INPUT : 0u)));
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_FP64 | (refine ? NEED_OWN_INPUT : 0u)));
     if (!lu->rbt.fac.depth) {
         set_last_error("%s: the factors carry no random butterfly transform (cflx_lu_rbt before the factorisation)",
                        __func__);
@@ -1393,7 +1410,7 @@ int cflx_lu_residual(cflx_lu* lu, double* rel_out) {
 int cflx_lu_solve(cflx_lu* lu, int nrhs, const double* B, int ldb, double* X, int ldx) {
     REFUSE_IF(!lu);
     CFLX_TRY(rhs_args(__func__, nrhs, B, ldb, X, ldx, false));
-    CFLX_TRY(enter(lu, __func__, NEED_FACTORS));
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_FP64));
     return lu_sweeps(lu, false, false, nrhs, B, ldb, X, ldx);
 }
 
@@ -1401,7 +1418,7 @@ int cflx_lu_solve(cflx_lu* lu, int nrhs, const double* B, int ldb, double* X, in
 int cflx_lu_solve_trans(cflx_lu* lu, int nrhs, const double* B, int ldb, double* X, int ldx) {
     REFUSE_IF(!lu);
     CFLX_TRY(rhs_args(__func__, nrhs, B, ldb, X, ldx, false));
-    CFLX_TRY(enter(lu, __func__, NEED_FACTORS));
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_FP64));
     return lu_sweeps(lu, true, false, nrhs, B, ldb, X, ldx);
 }
 
@@ -1412,7 +1429,7 @@ int cflx_lu_solve_local(cflx_lu* lu, int trans, int nrhs, const double* B_local,
     REFUSE_IF(trans != 0 && trans != 1);
     SolveLocalArgs a{};
     CFLX_TRY(solve_local_args(__func__, *lu, nrhs, B_local, ldb, X_local, ldx, &a));
-    CFLX_TRY(enter(lu, __func__, NEED_FACTORS));
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_FP64));
     auto solve = [lu, trans](int w, const double* Bk, int ldn, const double** Xk) -> int {
         CFLX_TRY(lu_sweeps(lu, trans != 0, false, w, Bk, ldn, nullptr, 0));
         *Xk = trans ? lu->sv.Xg : lu->sv.X;  // the transposed solve's P^T lands in Xg
@@ -1425,7 +1442,7 @@ int cflx_lu_solve_local(cflx_lu* lu, int trans, int nrhs, const double* B_local,
 int cflx_lu_rcond(cflx_lu* lu, double* rcond_out, double* anorm_out) {
     REFUSE_IF(!lu);
     REFUSE_IF(!rcond_out);
-    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_OWN_INPUT));
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_FP64 | NEED_OWN_INPUT));
     return lu_rcond(lu, false, rcond_out, anorm_out);
 }
 
@@ -1435,7 +1452,7 @@ int cflx_lu_rcond(cflx_lu* lu, double* rcond_out, double* anorm_out) {
 int cflx_lu_inverse(cflx_lu* lu, double* Ainv_local, int* info_out) {
     REFUSE_IF(!lu);
     REFUSE_IF(!info_out);
-    CFLX_TRY(enter(lu, __func__, NEED_FACTORS));
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_FP64));
     if (!lu->sv.ready) CFLX_TRY(lu_solve_prepare(lu));
     int info = 0;
     CFLX_TRY(zero_pivot_grid(*lu, &lu->eq, lu->Cbuf, &info));
@@ -1451,7 +1468,7 @@ int cflx_lu_det(cflx_lu* lu, int unscaled, double* sign_out, double* logabsdet_o
     REFUSE_IF(!lu);
     REFUSE_IF(unscaled != 0 && unscaled != 1);
     REFUSE_IF(!info_out);
-    CFLX_TRY(enter(lu, __func__, NEED_FACTORS));
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_FP64));
     if (!lu->sv.ready) CFLX_TRY(lu_solve_prepare(lu));
     const EquilRecord& eq = lu->eq.fac;
     const double* r = unscaled && (eq.equed == 'R' || eq.equed == 'B') ? eq.r.p : nullptr;
@@ -1484,7 +1501,7 @@ int cflx_lu_refine(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, d
     REFUSE_IF(!lu);
     REFUSE_IF(trans != 0 && trans != 1);
     CFLX_TRY(rhs_args(__func__, nrhs, B, ldb, X, ldx, true));
-    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_OWN_INPUT));
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_FP64 | NEED_OWN_INPUT));
     return refine_run(&lu->sv.rf, lu_refine_op(lu, trans != 0), nrhs, B, ldb, X, ldx, ferr_out, berr_out);
 }
 
@@ -1498,7 +1515,7 @@ int cflx_lu_refine_x(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb,
     CFLX_TRY(rhs_args(__func__, nrhs, B, ldb, X, ldx, true));
     REFUSE_IF(!err_bnds_norm_out);
     REFUSE_IF(!info_out);
-    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_OWN_INPUT));
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_FP64 | NEED_OWN_INPUT));
     const bool t = trans != 0;
     if (!lu->sv.ready) CFLX_TRY(lu_solve_prepare(lu));
     int info = 0;
@@ -1543,7 +1560,7 @@ int cflx_lu_svxx(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, dou
     REFUSE_IF(!rcond_out);
     REFUSE_IF(!err_bnds_norm_out);
     REFUSE_IF(!info_out);
-    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_OWN_INPUT));
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_FP64 | NEED_OWN_INPUT));
     const bool t = trans != 0;
     const EquilRecord& eq = lu->eq.fac;
     const bool rowequ = eq.equed == 'R' || eq.equed == 'B', colequ = eq.equed == 'C' || eq.equed == 'B';
@@ -1577,7 +1594,7 @@ int cflx_lu_svx(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, doub
     CFLX_TRY(rhs_args(__func__, nrhs, B, ldb, X, ldx, true));
     REFUSE_IF(!rcond_out);
     REFUSE_IF(!info_out);
-    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_OWN_INPUT));
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_FP64 | NEED_OWN_INPUT));
     const bool t = trans != 0;
     const EquilRecord& eq = lu->eq.fac;
     const bool rowequ = eq.equed == 'R' || eq.equed == 'B', colequ = eq.equed == 'C' || eq.equed == 'B';
@@ -1600,6 +1617,52 @@ int cflx_lu_svx(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, doub
     const double *r = rowequ ? eq.r.p : nullptr, *c = colequ ? eq.c.p : nullptr;
     return svx_run(&lu->eq, &lu->sv.rf, lu_refine_op(lu, t), nrhs, B, ldb, X, ldx, ferr_out, berr_out, t ? c : r,
                    t ? r : c, t ? eq.rowcnd : eq.colcnd, rcond, info_out);
+}
+
+// COLLECTIVE.  LAPACK dsgesv on the grid: the input factored with the TF32 trailing update (prec 1: one term, 3: three),
+// a zero pivot of that U checked over the world, then mixed_run's refinement in FP64 on A0.  When the low-precision
+// factors fail (iter -3) or the loop does not converge (-31), the input is factored again in FP64 and solved, as
+// cflx_lu_factor + cflx_lu_solve do; the handle then holds those FP64 factors.
+int cflx_lu_sv_mixed(cflx_lu* lu, int prec, int nrhs, const double* B, int ldb, double* X, int ldx, int itmax,
+                     int* iter_out, double* berr_out, double* ms_out) {
+    REFUSE_IF(!lu);
+    REFUSE_IF(prec != CFLX_PREC_TF32 && prec != CFLX_PREC_TF32X3);
+    REFUSE_IF(!iter_out);
+    CFLX_TRY(rhs_args(__func__, nrhs, B, ldb, X, ldx, true));
+    CFLX_TRY(enter(lu, __func__, NEED_INPUT | NEED_UNSCALED));
+    if (lu->rbt.in.depth) {
+        set_last_error("%s: refused, the input carries a random butterfly transform (cflx_lu_rbt); upload it again first",
+                       __func__);
+        return CFLX_ERR_STATE;
+    }
+    if (lu->next_host) {
+        set_last_error("%s: refused, a next input is queued (cflx_lu_queue_next_local): the refinement reads this input "
+                       "after the factorisation", __func__);
+        return CFLX_ERR_STATE;
+    }
+    CFLX_TRY(handle_tf32_begin(lu, prec));
+    double ms = 0.0;
+    const int run = lu_factor_run(lu, &ms);
+    lu->update_terms = 0;
+    CFLX_TRY(run);
+    double anorm = 0.0;
+    CFLX_TRY(norminf_grid(*lu, lu->A0, &anorm));
+    CFLX_TRY(lu_solve_prepare(lu));
+    int zero = 0, iter = MIXED_LOW_PREC_FAILED;
+    CFLX_TRY(zero_pivot_grid(*lu, &lu->eq, lu->Cbuf, &zero));
+    if (zero == 0)
+        CFLX_TRY(mixed_run(&lu->sv.rf, lu_refine_op(lu, false), anorm, itmax > 0 ? itmax : MIXED_ITMAX, nrhs, B, ldb, X,
+                           ldx, &iter, berr_out));
+    if (iter < 0) {
+        double ms2 = 0.0;
+        CFLX_TRY(lu_factor_run(lu, &ms2));
+        ms += ms2;
+        CFLX_TRY(lu_sweeps(lu, false, false, nrhs, B, ldb, X, ldx));
+        if (berr_out) CFLX_TRY(mixed_berr(&lu->sv.rf, lu_refine_op(lu, false), anorm, nrhs, B, ldb, X, ldx, berr_out));
+    }
+    *iter_out = iter;
+    if (ms_out) *ms_out = ms;
+    return CFLX_OK;
 }
 
 int cflx_host_alloc(size_t bytes, void** out) {

@@ -233,6 +233,12 @@ struct Handle : Grid {
     Stream side;        // high-priority look-ahead stream (null: no overlap)
     OzakiWorkspace oz;  // digit planes of the int8 wgmma trailing update (CFLX_GEMM=ozaki)
     bool use_ozaki = false;
+    // The trailing update of the next factorisation: FP64 (the DMMA kernel, or ozaki as above), or the TF32 wgmma path
+    // with one or three terms (tf32.cu).  Only the mixed-precision drivers set a TF32 mode, for one factorisation; the
+    // split workspace is made on first use.  low_prec: the factors of the last factorisation came from a TF32 update.
+    int update_terms = 0;  // 0: FP64, 1: TF32, 3: TF32x3
+    Tf32Workspace tf;
+    bool low_prec = false;
     SolveCache sv;
     EquilState eq;  // cflx_*_equilibrate / cflx_*_svx
     RbtState rbt;   // cflx_*_rbt: the transform of the input and of the factors
@@ -254,6 +260,7 @@ enum Need : unsigned {
     NEED_UNSCALED = 2,   // an input that carries no scaling
     NEED_FACTORS = 4,    // a successful factorisation
     NEED_OWN_INPUT = 8,  // A0 still holds the input of that factorisation (not a queued next one)
+    NEED_FP64 = 16,      // factors of an FP64 trailing update (not those a mixed-precision driver left)
 };
 // The prologue of every entry point `who` on a handle, after its argument checks: CFLX_ERR_STATE with "<who>: <reason>"
 // unless h's state has what `need` asks for, then h's device made current
@@ -264,6 +271,8 @@ void handle_equil_begin(Handle* h);
 // query leaves the record and its scales
 int handle_equil_end(Handle* h, bool apply, int info, char equed, double rowcnd, double colcnd, const double* c);
 int handle_launch_count(Handle* h, int64_t* count_out, int reset);
+// h->tf for the next factorisation's TF32 update with `terms` (1 or 3), made on first use; h->update_terms = terms
+int handle_tf32_begin(Handle* h, int terms);
 // COLLECTIVE (world): *same = every rank has ok and the same words, from one ncclMin over {w.., ~w.., ok}
 int world_agree(Handle* h, bool ok, std::initializer_list<unsigned long long> words, bool* same);
 }  // namespace cflx
@@ -440,6 +449,19 @@ struct RefineOp {
 // device), ferr (may be null: no estimator) and berr (may be null) per column.  Every column runs LAPACK's own decisions, all in lockstep.
 int refine_run(RefineCache* rc, const RefineOp& op, int nrhs, const double* B, int ldb, double* X, int ldx, double* ferr,
                double* berr);
+// LAPACK dsgesv / dsposv's refinement loop on the grid (collective), after a factorisation with a TF32 update: X =
+// op.solve(B), then R = B - op(A) X in FP64 from op.A and, until every column has ||r||_inf <= ||x||_inf anorm eps
+// sqrt(M) (eps = 2^-53), X += op.solve(R), at most itmax times.  *iter = the corrections taken when the loop converged,
+// MIXED_NO_CONVERGENCE when it did not within itmax or a norm is not finite.  berr (may be null): ||r||_inf / (anorm
+// ||x||_inf) per column of the last residual.  X (host or device, ldx) is written in every case.
+constexpr int MIXED_ITMAX = 30;               // dsgesv's ITERMAX
+constexpr int MIXED_NO_CONVERGENCE = -31;     // dsgesv's -ITERMAX - 1
+constexpr int MIXED_LOW_PREC_FAILED = -3;     // the low-precision factorisation met a zero or non-positive pivot
+int mixed_run(RefineCache* rc, const RefineOp& op, double anorm, int itmax, int nrhs, const double* B, int ldb, double* X,
+              int ldx, int* iter, double* berr);
+// the same backward errors of a given X (host or device)
+int mixed_berr(RefineCache* rc, const RefineOp& op, double anorm, int nrhs, const double* B, int ldb, const double* X,
+               int ldx, double* berr);
 // One column of LAPACK's dla_gerfsx_extended / dla_porfsx_extended: its precision state and the normwise (x) and
 // componentwise (z) convergence states, with LAPACK's initial values.  round() takes the statistics of one round,
 // {normy, normx, normdx, dz_z, ymin} (refine.cu column_stats_kernel), and returns what to do with the correction dy:

@@ -1027,6 +1027,67 @@ int refine_run(RefineCache* rc, const RefineOp& op, int nrhs, const double* B, i
     return CFLX_OK;
 }
 
+// ---------------------------------------------------------------- the mixed-precision drivers' loop (dsgesv / dsposv)
+namespace {
+// R = B - op(A) X for the X in rc->X, then per column ||x||_inf and ||r||_inf: *conv when every column has ||r|| <=
+// ||x|| cte, *finite when every norm is finite; berr (may be null) = ||r|| / (anorm ||x||)
+int mixed_check(RefinePass& pass, double anorm, double cte, double* berr, bool* conv, bool* finite) {
+    RefineCache* rc = pass.rc;
+    cudaStream_t s = pass.op.grid.comm->stream;
+    CFLX_TRY(pass.run(rc->X));
+    CFLX_TRY(launch_column_stats(rc->X, rc->R, nullptr, pass.op.grid.M, pass.ldn, pass.nrhs, rc->stats, s));
+    std::vector<double> st((size_t)pass.nrhs * NSTAT);
+    CFLX_CUDA(cudaMemcpyAsync(st.data(), rc->stats, sizeof(double) * st.size(), cudaMemcpyDeviceToHost, s));
+    CFLX_CUDA(cudaStreamSynchronize(s));
+    *conv = *finite = true;
+    for (int j = 0; j < pass.nrhs; ++j) {
+        const double xn = st[(size_t)j * NSTAT], rn = st[(size_t)j * NSTAT + 2];
+        *finite = *finite && std::isfinite(xn) && std::isfinite(rn);
+        *conv = *conv && rn <= xn * cte;
+        if (berr) berr[j] = rn / (anorm * xn);
+    }
+    return CFLX_OK;
+}
+double mixed_cte(double anorm, int M) { return anorm * std::ldexp(1.0, -53) * std::sqrt((double)M); }
+}  // namespace
+
+int mixed_run(RefineCache* rc, const RefineOp& op, double anorm, int itmax, int nrhs, const double* B, int ldb, double* X,
+              int ldx, int* iter, double* berr) {
+    cudaStream_t s = op.grid.comm->stream;
+    const int M = op.grid.M;
+    RefinePass pass(rc, op, nrhs);
+    CFLX_TRY(pass.setup(B, ldb, B, ldb, false));  // rc->X is overwritten by the first solve
+    const int ldn = pass.ldn;
+    CFLX_TRY(rc->stats.grow((size_t)ldn * NSTAT));
+    const std::vector<int> all(ldn, 1);
+    CFLX_CUDA(cudaMemcpyAsync(rc->active, all.data(), sizeof(int) * ldn, cudaMemcpyHostToDevice, s));
+    CFLX_TRY(op.solve(false, nrhs, rc->B, ldn, rc->X, ldn));
+    const double cte = mixed_cte(anorm, M);
+    bool conv = false, finite = true;
+    CFLX_TRY(mixed_check(pass, anorm, cte, berr, &conv, &finite));
+    int it = 0;
+    while (!conv && finite && it < itmax) {
+        CFLX_TRY(op.solve(false, nrhs, rc->R, ldn, rc->D, ldn));
+        CFLX_TRY(launch_add_cols(rc->X, rc->D, rc->active, M, ldn, s));
+        ++it;
+        CFLX_TRY(mixed_check(pass, anorm, cte, berr, &conv, &finite));
+    }
+    *iter = conv ? it : MIXED_NO_CONVERGENCE;
+    CFLX_CUDA(cudaMemcpy2DAsync(X, (size_t)ldx * sizeof(double), rc->X, ldn * sizeof(double), nrhs * sizeof(double), M,
+                                cudaMemcpyDefault, s));
+    CFLX_CUDA(cudaStreamSynchronize(s));
+    return CFLX_OK;
+}
+
+int mixed_berr(RefineCache* rc, const RefineOp& op, double anorm, int nrhs, const double* B, int ldb, const double* X,
+               int ldx, double* berr) {
+    RefinePass pass(rc, op, nrhs);
+    CFLX_TRY(pass.setup(B, ldb, X, ldx, false));
+    CFLX_TRY(rc->stats.grow((size_t)pass.ldn * NSTAT));
+    bool conv = false, finite = true;
+    return mixed_check(pass, anorm, mixed_cte(anorm, op.grid.M), berr, &conv, &finite);
+}
+
 // ---------------------------------------------------------------- extra-precise refinement (dgerfsx / dporfsx)
 int RefineXColumn::round(const double st[5], double rcond, bool ignore_cwise, int cnt, int M) {
     const double eps = std::ldexp(1.0, -53), incr_thresh = (double)M * eps;

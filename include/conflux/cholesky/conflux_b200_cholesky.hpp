@@ -91,6 +91,19 @@ inline void choleskySolve(int nrhs, const double* B, int ldb, double* X, int ldx
     if (!s.plan) throw CholeskyException("choleskySolve() before initialize()");
     chol_detail::check(cflx_chol_solve(s.plan, nrhs, B, ldb, X, ldx), "choleskySolve");
 }
+// LAPACK dsposv on the GPU grid (cflx_chol_sv_mixed, collective): the current input factored with the trailing update on
+// the TF32 tensor cores (prec CFLX_PREC_TF32 or CFLX_PREC_TF32X3), refined in FP64, or factored again in FP64 when that
+// fails.  B / X as choleskySolve (X required); itmax <= 0: 30; berr (nrhs, may be null).  Returns the corrections taken,
+// -3 or -31 when the FP64 fallback solved the system.
+inline int choleskySvMixed(int prec, int nrhs, const double* B, int ldb, double* X, int ldx, int itmax = 0,
+                           double* berr = nullptr) {
+    auto& s = chol_detail::state();
+    if (!s.plan) throw CholeskyException("choleskySvMixed() before initialize()");
+    int iter = 0;
+    chol_detail::check(cflx_chol_sv_mixed(s.plan, prec, nrhs, B, ldb, X, ldx, itmax, &iter, berr, nullptr),
+                       "choleskySvMixed");
+    return iter;
+}
 // The signed Cholesky A = R S R^T of the current input without pivoting (cflx_chol_factor_ldlt, collective), for
 // symmetric indefinite matrices: every later call refers to R S R^T.  Returns info (1 + the first exactly zero pivot's
 // column, 0: none); *nrepl the pivots the tiny rule replaced, inertia[3] the positive, negative and zero pivots.

@@ -304,6 +304,18 @@ void LU_solve(lu_params<T>& gv, int nrhs, const T* B, int ldb, T* X, int ldx, bo
     else check(cflx_lu_solve(gv.plan, nrhs, B, ldb, X, ldx), "LU_solve");
 }
 
+// LAPACK dsgesv on the GPU grid (cflx_lu_sv_mixed, collective): the input the device holds (the last LU_rep's) factored
+// with the trailing update on the TF32 tensor cores (prec CFLX_PREC_TF32 or CFLX_PREC_TF32X3), refined in FP64 to
+// working accuracy, or factored again in FP64 when that fails.  B / X as LU_solve (X required); itmax <= 0: 30; berr
+// (nrhs, may be null).  Returns the corrections taken, -3 or -31 when the FP64 fallback solved the system.
+template <class T>
+int LU_sv_mixed(lu_params<T>& gv, int prec, int nrhs, const T* B, int ldb, T* X, int ldx, int itmax = 0,
+                double* berr = nullptr) {
+    int iter = 0;
+    check(cflx_lu_sv_mixed(gv.plan, prec, nrhs, B, ldb, X, ldx, itmax, &iter, berr, nullptr), "LU_sv_mixed");
+    return iter;
+}
+
 // Solves A X = B (A^T X = B when transposed) with the factors of the last LU_rep, like ScaLAPACK's pdgetrs, with B and X
 // distributed like A (cflx_lu_solve_local, collective): this rank's row-major shares of gv.Ml x cflx_rhs_local_cols(nrhs,
 // gv.v, gv.Py), leading dimensions ldb / ldx; host or device memory.  B_local is read on layer 0 only (may be null on the

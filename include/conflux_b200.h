@@ -236,6 +236,25 @@ int cflx_lu_equilibrate(cflx_lu*, int apply, double* r_out, double* c_out, doubl
  * CFLX_ERR_ARG as cflx_lu_refine and for a NULL rcond_out or info_out; CFLX_ERR_STATE as cflx_lu_rcond. */
 int cflx_lu_svx(cflx_lu*, int trans, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out,
                 double* ferr_out, double* berr_out, double* rpvgrw_out, char* equed_out, int* info_out);
+/* The precisions of the mixed-precision drivers' trailing update: TF32 tensor cores with one term (A_hi B_hi) or three
+ * (3xTF32: A_hi B_hi + A_hi B_lo + A_lo B_hi), every operand row scaled by a power of two first, FP32 accumulation. */
+#define CFLX_PREC_TF32 1
+#define CFLX_PREC_TF32X3 3
+/* COLLECTIVE.  LAPACK dsgesv on the GPU grid: the input the device holds (cflx_lu_set_local) factored with the trailing
+ * update in `prec` (the panel search, the triangular solves and the diagonal blocks stay FP64), x = solve(b), then until
+ * every column has ||r||_inf <= ||x||_inf ||A||_inf eps sqrt(M) (eps = 2^-53): r = b - A x in FP64 from the input,
+ * x += solve(r), at most itmax times (itmax <= 0: 30).  iter_out (required, the same on every rank): the corrections
+ * taken when the loop converged; -3 when the low-precision U has an exactly zero pivot, -31 when the loop did not
+ * converge within itmax (or a norm became non-finite).  On a negative iter_out the input is factored again in FP64 and
+ * solved, with the bits of cflx_lu_factor + cflx_lu_solve; the handle then holds those factors.  After a converged run
+ * it holds the low-precision factors: cflx_lu_get_factors, cflx_lu_get_permutation, cflx_lu_validate and
+ * cflx_lu_residual read them, while every call that treats them as FP64 factors (the solves, rcond, refine, refine_x,
+ * svx, svxx, inverse, det) returns CFLX_ERR_STATE until the next cflx_lu_factor.  berr_out (nrhs, may be NULL): each
+ * column's final ||r||_inf / (||A||_inf ||x||_inf).  ms_out (may be NULL): device time of the factorisation(s).  B and X
+ * replicated as cflx_lu_solve.  CFLX_ERR_ARG for an unknown prec, a NULL iter_out and as cflx_lu_refine;
+ * CFLX_ERR_STATE before cflx_lu_set_local, for a scaled or transformed input, or with a queued next input. */
+int cflx_lu_sv_mixed(cflx_lu*, int prec, int nrhs, const double* B, int ldb, double* X, int ldx, int itmax,
+                     int* iter_out, double* berr_out, double* ms_out);
 /* COLLECTIVE.  LAPACK dgeequb (+ dlaqge when apply): cflx_lu_equilibrate with the scales rounded to powers of two.  The
  * row maxima are rounded to 2^INT(log(x) / log(2)) before rcmin, rcmax and amax are taken, then the column maxima of
  * |a| r likewise; the exponents come from the host's log, as LAPACK's.  r_out / c_out hold the rounded maxima on the
@@ -428,6 +447,15 @@ int cflx_chol_equilibrate_b(cflx_chol*, int apply, double* s_out, double* scond_
 int cflx_chol_svxx(cflx_chol*, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out,
                    double* rpvgrw_out, double* berr_out, double* err_bnds_norm_out, double* err_bnds_comp_out,
                    char* equed_out, int* info_out);
+/* COLLECTIVE.  LAPACK dsposv on the GPU grid: cflx_lu_sv_mixed's loop with the Cholesky factored with the trailing
+ * update in `prec` and the residual from the stored lower triangle of the input.  iter_out -3 when the low-precision
+ * factorisation met a non-positive pivot.  On a negative iter_out the input is factored again in FP64 and solved, with
+ * the bits of cflx_chol_factor + cflx_chol_solve; when that factorisation fails too, CFLX_ERR_STATE as cflx_chol_factor
+ * (iter_out and ms_out are still set, X is not written).  After a converged run cflx_chol_get_local, cflx_chol_validate
+ * and cflx_chol_get_signs read the low-precision factor, while the solves, rcond, refine, refine_x, svx, svxx, inverse
+ * and det return CFLX_ERR_STATE until the next cflx_chol_factor.  Arguments and the other results as cflx_lu_sv_mixed. */
+int cflx_chol_sv_mixed(cflx_chol*, int prec, int nrhs, const double* B, int ldb, double* X, int ldx, int itmax,
+                       int* iter_out, double* berr_out, double* ms_out);
 /* COLLECTIVE.  inv(A) from the factor of the last successful cflx_chol_factor (A = L L^T), like LAPACK's dpotri
  * (UPLO = 'L'): the real tiles on and below the diagonal of this rank's Ml x Nl share hold inv(A), whole diagonal tiles
  * included.  The tiles above the diagonal and the local tiles with a global index >= Kappa are zero.  Host or device
@@ -645,6 +673,16 @@ int cflx_dbg_getrf_nopiv_tile(int v, const double* A, double tiny, double* LU_ou
 int cflx_dbg_ozaki_gemm(int M, int N, int K, int row0, int col0, int max_ctas, const double* AT, const double* B,
                         const double* C, double* D, signed char* planesA_out, signed char* planesB_out, int* ea_out,
                         int* eb_out, int reps, double* ms_out, double* split_ms_out);
+/* D = C - AT^T * B on the TF32 wgmma path of the mixed-precision drivers (tf32.cu) with terms = 1 or 3: AT [K x (row0 +
+ * M)], B [K x (col0 + N)] and C/D [M x N] row-major dense host arrays (C may be NULL: zeros), any K >= 1.  The whole of
+ * AT and B is split (B in the windows [0, col0) and [col0, col0 + N), as the look-ahead does); the product reads rows
+ * [row0, row0 + M) and columns [col0, col0 + N), on at most max_ctas CTAs (0 = one per SM).  Optional test outputs:
+ * the split terms as FP32 [row0 + M][KP] / [col0 + N][KP] (hi, then lo; lo only with three terms), KP = K rounded up
+ * to 8, and the exponents [row0 + M] / [col0 + N].  ms_out / split_ms_out: mean device time of the GEMM kernel / of the
+ * split kernels over reps runs. */
+int cflx_dbg_gemm_tf32(int terms, int M, int N, int K, int row0, int col0, int max_ctas, const double* AT, const double* B,
+                       const double* C, double* D, float* hiA_out, float* loA_out, float* hiB_out, float* loB_out,
+                       int* ea_out, int* eb_out, int reps, double* ms_out, double* split_ms_out);
 /* raw int8 tensor-core rate of back-to-back wgmma (64 x n x 32, n = 64/128/192/256, operands resident in shared memory,
  * two warpgroups per CTA, one CTA per SM).  tmacs_out = tera-MACs/s (x2 = TOP/s). */
 int cflx_dbg_wgmma_peak(int n, double* tmacs_out);
