@@ -8,7 +8,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libconflux_b200.so")
-SOURCES = ["gemm.cu", "ozaki.cu", "tf32.cu", "panel.cu", "rows.cu", "trsm.cu", "lu.cu", "validate.cu", "solve.cu", "norm.cu", "refine.cu", "equil.cu", "inverse.cu", "solve_local.cu", "det.cu", "fixed.cu", "rbt.cu", "chol.cu", "dbg.cu"]
+SOURCES = ["gemm.cu", "ozaki.cu", "tf32.cu", "update.cu", "panel.cu", "rows.cu", "trsm.cu", "lu.cu", "validate.cu", "solve.cu", "norm.cu", "refine.cu", "equil.cu", "inverse.cu", "solve_local.cu", "det.cu", "fixed.cu", "rbt.cu", "chol.cu", "dbg.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC,-O3",

@@ -480,7 +480,10 @@ static int chol_leave_sms() {
     return leave;
 }
 
-int update_columns(cflx_chol* ch, int gfirst, int jmin, int buf, double* X, int lj_lo, int lj_hi, cudaStream_t s, int planes_buf = -1) {
+// fp64: the FP64 kernel whatever the handle's update (the validation's update); otherwise the handle's update on the
+// operands split_planes split from buffer set buf
+int update_columns(cflx_chol* ch, int gfirst, int jmin, int buf, double* X, int lj_lo, int lj_hi, cudaStream_t s,
+                   bool fp64 = false) {
     const int v = ch->v, Px = ch->Px, Py = ch->Py, Ml = ch->Ml, Nl = ch->Nl;
     const int pi = ch->pi, pj = ch->pj, pk = ch->pk;
     const int64_t piece_stride = (int64_t)v * ch->ldp;
@@ -512,24 +515,18 @@ int update_columns(cflx_chol* ch, int gfirst, int jmin, int buf, double* X, int 
         g.D = const_cast<double*>(g.C);
         g.ldd = Nl;
         g.alpha = -1.0; g.beta = 1.0;
-        if (ch->update_terms && planes_buf == buf)   // TF32 terms of this buffer set are current (see split_planes)
-            CFLX_TRY(launch_tf32_gemm(&ch->tf, ch->update_terms, M, g.N, (li - my_first) * v, (lj - lj0) * v, g.D, Nl,
-                                      ch->tf.sms - chol_leave_sms(), s));
-        else if (ch->use_ozaki && planes_buf == buf)   // planes of this buffer set are current (see split_planes)
-            CFLX_TRY(launch_ozaki_gemm(&ch->oz, M, g.N, (li - my_first) * v, (lj - lj0) * v, g.D, Nl, ch->oz.sms - chol_leave_sms(), s));
-        else
-            CFLX_TRY(launch_gemm_tn(g, s));
+        if (fp64) CFLX_TRY(launch_gemm_tn(g, s));
+        else CFLX_TRY(ch->update.apply(g, (li - my_first) * v, (lj - lj0) * v, chol_leave_sms(), s));
         ch->launches++;
         lj += gcols;
     }
     (void)my_rows;
     return CFLX_OK;
 }
-// digit planes (or, in a TF32 update mode, the TF32 terms) of the operands of one update sweep: my piece (rows) and the
-// gathered column operand, this layer's slab
-int split_planes(cflx_chol* ch, int gfirst, int jmin, int buf, cudaStream_t s);
+// the operands of one update sweep, split for a split kind: my piece (rows) and the gathered column operand, this
+// layer's slab
 int split_planes(cflx_chol* ch, int gfirst, int jmin, int buf, cudaStream_t s) {
-    if (!ch->use_ozaki && !ch->update_terms) return CFLX_OK;
+    if (!ch->update.splits()) return CFLX_OK;
     const int v = ch->v, Px = ch->Px;
     const int64_t piece_stride = (int64_t)v * ch->ldp;
     const double* G = ch->G + (int64_t)buf * Px * piece_stride;
@@ -540,20 +537,15 @@ int split_planes(cflx_chol* ch, int gfirst, int jmin, int buf, cudaStream_t s) {
     const int64_t ldg = piece_ld(ch, gfirst, ch->pi);
     const double* A = G + (int64_t)ch->pi * piece_stride + (int64_t)ch->pk * ch->nlayr * ldg;
     const double* B = Bc + (int64_t)ch->pk * ch->nlayr * ch->ldb;
-    if (ch->update_terms) {
-        if (rows > 0) CFLX_TRY(tf32_split_a(&ch->tf, ch->update_terms, A, ldg, rows, s));
-        if (ncols > 0) CFLX_TRY(tf32_split_b(&ch->tf, ch->update_terms, B, ch->ldb, 0, ncols, s));
-    } else {
-        if (rows > 0) CFLX_TRY(ozaki_split_a(&ch->oz, A, ldg, rows, s));
-        if (ncols > 0) CFLX_TRY(ozaki_split_b(&ch->oz, B, ch->ldb, 0, ncols, s));
-    }
+    if (rows > 0) CFLX_TRY(ch->update.split_a(A, ldg, rows, s));
+    if (ncols > 0) CFLX_TRY(ch->update.split_b(B, ch->ldb, 0, ncols, s));
     ch->launches += 2;
     return CFLX_OK;
 }
 int broadcast_and_update(cflx_chol* ch, int t, int jmin, bool below_only, double* X, cudaStream_t s) {
     const int gfirst = below_only ? t + 1 : t;
     CFLX_TRY(broadcast_pieces(ch, t, gfirst, jmin, 0, s));
-    return update_columns(ch, gfirst, jmin, 0, X, 0, ch->Nl / ch->v, s);
+    return update_columns(ch, gfirst, jmin, 0, X, 0, ch->Nl / ch->v, s, true);
 }
 
 size_t potrf_tile_smem(int v) { return ((size_t)PB * (PB + 1) + (size_t)v * (PB + 1)) * sizeof(double); }
@@ -1056,15 +1048,15 @@ int chol_factor_run(cflx_chol* ch, float* ms_out, int* bad_out, int* cnt) {
     for (int k = 0; k + 1 < ch->Nt; ++k) {
         const int b = k & 1, nb1 = (k + 1) & 1;
         CFLX_CUDA(cudaStreamWaitEvent(s, ch->ev_panel[b], 0));             // pieces of step k are in buffer set b
-        CFLX_TRY(split_planes(ch, k + 1, k + 1, b, s));                     // (int8 wgmma path) digit planes of both operands
+        CFLX_TRY(split_planes(ch, k + 1, k + 1, b, s));                     // (split kinds) both operands
         const int ljn = (k + 1) / Py;                                        // local tile of column k+1 on its owners
         const bool own_next = (pj == (k + 1) % Py);
-        if (own_next) CFLX_TRY(update_columns(ch, k + 1, k + 1, b, ch->A11, ljn, ljn + 1, s, b));
+        if (own_next) CFLX_TRY(update_columns(ch, k + 1, k + 1, b, ch->A11, ljn, ljn + 1, s));
         CFLX_CUDA(cudaEventRecord(ch->ev_col[nb1], s));
         CFLX_CUDA(cudaStreamWaitEvent(sp, ch->ev_col[nb1], 0));
         CFLX_TRY(panel_step(ch, k + 1, sp));
         CFLX_CUDA(cudaEventRecord(ch->ev_panel[nb1], sp));
-        CFLX_TRY(update_columns(ch, k + 1, k + 1, b, ch->A11, own_next ? ljn + 1 : 0, Nl / v, s, b));
+        CFLX_TRY(update_columns(ch, k + 1, k + 1, b, ch->A11, own_next ? ljn + 1 : 0, Nl / v, s));
     }
     CFLX_CUDA(cudaStreamWaitEvent(s, ch->ev_panel[(ch->Nt - 1) & 1], 0));
     CFLX_CUDA(cudaEventRecord(loop[1], s));
@@ -1093,7 +1085,7 @@ int chol_factor_run(cflx_chol* ch, float* ms_out, int* bad_out, int* cnt) {
         bad = h[2] == INT_MAX ? 0 : h[2];
     }
     *bad_out = bad;
-    ch->low_prec = ch->update_terms != 0;
+    ch->low_prec = ch->update.tf32();
     if (cnt) std::memcpy(cnt, h + 4, 4 * sizeof(int));
     *ms_out = ms;
     return CFLX_OK;
@@ -1384,12 +1376,9 @@ int cflx_chol_sv_mixed(cflx_chol* ch, int prec, int nrhs, const double* B, int l
         return CFLX_ERR_STATE;
     }
     ch->ldlt = false;
-    CFLX_TRY(handle_tf32_begin(ch, prec));
     float ms = 0;
     int bad = 0;
-    const int run = chol_factor_run(ch, &ms, &bad, nullptr);
-    ch->update_terms = 0;
-    CFLX_TRY(run);
+    CFLX_TRY(ch->update.with_tf32(prec, [&] { return chol_factor_run(ch, &ms, &bad, nullptr); }));
     double anorm = 0.0;  // the infinity-norm of the symmetric matrix is its 1-norm
     CFLX_TRY(norm1_grid(*ch, ch->A0, true, &anorm));
     int iter = MIXED_LOW_PREC_FAILED;

@@ -77,6 +77,66 @@ int time_reps(Run&& run, int reps, double* ms_out) {
     return CFLX_OK;
 }
 
+// The split-update hooks' shared work on u (a split kind): AT (K x (row0 + M)), B (K x (col0 + N)) and C (M x N, null:
+// zeros) staged; then one warm-up and `reps` (at least 1) timed repetitions of C restored, every operand row split (B's
+// in the two windows [0, col0) and [col0, col0 + N), as the factorisation's look-ahead splits them) and the product on
+// the window (max_ctas > 0: at most that many CTAs); D (may be null) and the exponents fetched.  *ms_out /
+// *split_ms_out (may be null): the mean device times of the product and of the splits.
+int split_update(TrailingUpdate& u, int M, int N, int K, int row0, int col0, int max_ctas, const double* AT,
+                 const double* B, const double* C, double* D, int* ea_out, int* eb_out, int reps, double* ms_out,
+                 double* split_ms_out) {
+    const SplitWorkspace& ws = u.terms ? static_cast<const SplitWorkspace&>(u.tf) : u.oz;
+    const int Ma = row0 + M, Nb = col0 + N;
+    const int64_t ldat = round_up(Ma, 2), ldb = Nb, ldc = round_up(N, 2);
+    const size_t c_n = (size_t)M * ldc;
+    DevBuf<> dA, dB, dC, dC0;
+    CFLX_TRY(stage(dA, K * ldat));
+    CFLX_TRY(stage(dB, K * ldb, B));
+    CFLX_TRY(stage(dC, c_n));
+    CFLX_TRY(stage(dC0, c_n));
+    CFLX_CUDA(cudaMemset(dA.p, 0, sizeof(double) * K * ldat));
+    CFLX_CUDA(cudaMemcpy2D(dA.p, ldat * 8, AT, (size_t)Ma * 8, (size_t)Ma * 8, K, cudaMemcpyHostToDevice));
+    CFLX_CUDA(cudaMemset(dC0.p, 0, sizeof(double) * c_n));
+    if (C) CFLX_CUDA(cudaMemcpy2D(dC0.p, ldc * 8, C, (size_t)N * 8, (size_t)N * 8, M, cudaMemcpyHostToDevice));
+    GemmArgs g{};
+    g.M = M; g.N = N; g.D = dC.as<double>(); g.ldd = ldc;
+    const int leave = max_ctas > 0 ? ws.sms - max_ctas : 0;
+    Events<3> ev;
+    CFLX_TRY(ev.create());
+    if (reps < 1) reps = 1;
+    float ms = 0, ms_split = 0;
+    int rc = CFLX_OK;
+    for (int r = 0; r < reps + 1 && rc == CFLX_OK; ++r) {
+        cudaMemcpyAsync(dC.p, dC0.p, sizeof(double) * c_n, cudaMemcpyDeviceToDevice, 0);
+        cudaEventRecord(ev[0]);
+        rc = u.split_a(dA.as<double>(), ldat, Ma, 0);
+        if (!rc && col0 > 0) rc = u.split_b(dB.as<double>(), ldb, 0, col0, 0);
+        if (!rc) rc = u.split_b(dB.as<double>(), ldb, col0, N, 0);
+        cudaEventRecord(ev[1]);
+        if (!rc) rc = u.apply(g, row0, col0, leave, 0);
+        cudaEventRecord(ev[2]);
+        if (cudaEventSynchronize(ev[2]) != cudaSuccess) {
+            set_last_error("split update kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
+            rc = CFLX_ERR_CUDA;
+        }
+        float a = 0, b = 0;
+        cudaEventElapsedTime(&a, ev[0], ev[1]);
+        cudaEventElapsedTime(&b, ev[1], ev[2]);
+        if (r > 0) {
+            ms_split += a;
+            ms += b;
+        }
+    }
+    if (ms_out) *ms_out = ms / reps;
+    if (split_ms_out) *split_ms_out = ms_split / reps;
+    if (rc == CFLX_OK && D &&
+        cudaMemcpy2D(D, (size_t)N * 8, dC.p, ldc * 8, (size_t)N * 8, M, cudaMemcpyDeviceToHost) != cudaSuccess)
+        rc = CFLX_ERR_CUDA;
+    if (rc == CFLX_OK) rc = fetch(ea_out, ws.ea, Ma);
+    if (rc == CFLX_OK) rc = fetch(eb_out, ws.eb, Nb);
+    return rc;
+}
+
 // a residual kernel (refine.cu) on the share A of layout L: launch(mode, A, Xc, Xr, P, Q) runs it on the device copies
 // of A, Xc (Nl x nrhs) and Xr (Ml x nrhs).  The timed repetitions run first, then the launch whose result is returned,
 // into zeroed outputs of rows x nrhs (Ml, Nl or Ml + Nl rows by mode).
@@ -1146,57 +1206,18 @@ int cflx_dbg_ozaki_gemm(int M, int N, int K, int row0, int col0, int max_ctas, c
     REFUSE_IF(M <= 0 || N <= 0 || K <= 0 || (N & 1));
     REFUSE_IF(row0 < 0 || col0 < 0 || max_ctas < 0);
     REFUSE_IF(!AT || !B);
-    // AT holds row0 + M operand rows, B col0 + N columns; the planes of all of them are made (B's in the two windows
-    // [0, col0) and [col0, col0 + N), as the factorisation's look-ahead splits them), the product reads the window
     const int Ma = row0 + M, Nb = col0 + N;
-    const int64_t ldat = round_up(Ma, 2), ldb = Nb, ldc = N;
-    const size_t c_n = (size_t)M * ldc;
-    DevBuf<> dA, dB, dC, dC0;
-    CFLX_TRY(stage(dA, K * ldat));
-    CFLX_TRY(stage(dB, K * ldb, B));
-    CFLX_TRY(stage(dC, c_n));
-    CFLX_TRY(stage(dC0, c_n, C));
-    CFLX_CUDA(cudaMemset(dA.p, 0, sizeof(double) * K * ldat));
-    CFLX_CUDA(cudaMemcpy2D(dA.p, ldat * 8, AT, (size_t)Ma * 8, (size_t)Ma * 8, K, cudaMemcpyHostToDevice));
-    if (!C) CFLX_CUDA(cudaMemset(dC0.p, 0, sizeof(double) * c_n));
-    Events<3> ev;
-    CFLX_TRY(ev.create());
-    OzakiWorkspace ws;
-    int rc = ozaki_workspace_create(&ws, Ma, Nb, K);
-    if (reps < 1) reps = 1;
-    float ms = 0, ms_split = 0;
-    for (int r = 0; r < reps + 1 && rc == CFLX_OK; ++r) {
-        cudaMemcpyAsync(dC.p, dC0.p, sizeof(double) * c_n, cudaMemcpyDeviceToDevice, 0);
-        cudaEventRecord(ev[0]);
-        rc = ozaki_split_a(&ws, dA.as<double>(), ldat, Ma, 0);
-        if (!rc && col0 > 0) rc = ozaki_split_b(&ws, dB.as<double>(), ldb, 0, col0, 0);
-        if (!rc) rc = ozaki_split_b(&ws, dB.as<double>(), ldb, col0, N, 0);
-        cudaEventRecord(ev[1]);
-        if (!rc) rc = launch_ozaki_gemm(&ws, M, N, row0, col0, dC.as<double>(), ldc, max_ctas, 0);
-        cudaEventRecord(ev[2]);
-        if (cudaEventSynchronize(ev[2]) != cudaSuccess) {
-            set_last_error("ozaki kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
-            rc = CFLX_ERR_CUDA;
-        }
-        float a = 0, b = 0;
-        cudaEventElapsedTime(&a, ev[0], ev[1]);
-        cudaEventElapsedTime(&b, ev[1], ev[2]);
-        if (r > 0) {
-            ms_split += a;
-            ms += b;
-        }
-    }
-    if (rc == CFLX_OK) rc = fetch(D, dC.p, c_n);
+    TrailingUpdate u;
+    int rc = u.create(Ma, Nb, K, true);
+    if (rc == CFLX_OK)
+        rc = split_update(u, M, N, K, row0, col0, max_ctas, AT, B, C, D, ea_out, eb_out, reps, ms_out, split_ms_out);
+    const OzakiWorkspace& ws = u.oz;
     for (int s = 0; s < 8 && rc == CFLX_OK; ++s) {
         if (planesA_out) rc = fetch(planesA_out + (size_t)s * Ma * K, ws.planesA + (size_t)s * ws.cap_a * K, (size_t)Ma * K);
         if (planesB_out && rc == CFLX_OK)
             rc = fetch(planesB_out + (size_t)s * Nb * K, ws.planesB + (size_t)s * ws.cap_b * K, (size_t)Nb * K);
     }
-    if (rc == CFLX_OK) rc = fetch(ea_out, ws.ea, Ma);
-    if (rc == CFLX_OK) rc = fetch(eb_out, ws.eb, Nb);
     if (rc == CFLX_OK && cudaDeviceSynchronize() != cudaSuccess) rc = CFLX_ERR_CUDA;
-    if (ms_out) *ms_out = ms / reps;
-    if (split_ms_out) *split_ms_out = ms_split / reps;
     return rc;
 }
 
@@ -1210,53 +1231,20 @@ int cflx_dbg_gemm_tf32(int terms, int M, int N, int K, int row0, int col0, int m
     REFUSE_IF(row0 < 0 || col0 < 0 || max_ctas < 0);
     REFUSE_IF(!AT || !B || !D);
     const int Ma = row0 + M, Nb = col0 + N;
-    const int64_t ldat = Ma, ldb = Nb, ldc = round_up(N, 2);
-    DevBuf<> dA, dB, dC, dC0;
-    CFLX_TRY(stage(dA, K * ldat, AT));
-    CFLX_TRY(stage(dB, K * ldb, B));
-    CFLX_TRY(stage(dC, (size_t)M * ldc));
-    CFLX_TRY(stage(dC0, (size_t)M * ldc));
-    CFLX_CUDA(cudaMemset(dC0.p, 0, sizeof(double) * M * ldc));
-    if (C) CFLX_CUDA(cudaMemcpy2D(dC0.p, ldc * 8, C, (size_t)N * 8, (size_t)N * 8, M, cudaMemcpyHostToDevice));
-    Events<3> ev;
-    CFLX_TRY(ev.create());
-    Tf32Workspace ws;
-    int rc = tf32_workspace_create(&ws, Ma, Nb, K);
-    if (reps < 1) reps = 1;
-    float ms = 0, ms_split = 0;
-    for (int r = 0; r < reps + 1 && rc == CFLX_OK; ++r) {
-        cudaMemcpyAsync(dC.p, dC0.p, sizeof(double) * M * ldc, cudaMemcpyDeviceToDevice, 0);
-        cudaEventRecord(ev[0]);
-        rc = tf32_split_a(&ws, terms, dA.as<double>(), ldat, Ma, 0);
-        if (!rc && col0 > 0) rc = tf32_split_b(&ws, terms, dB.as<double>(), ldb, 0, col0, 0);
-        if (!rc) rc = tf32_split_b(&ws, terms, dB.as<double>(), ldb, col0, N, 0);
-        cudaEventRecord(ev[1]);
-        if (!rc) rc = launch_tf32_gemm(&ws, terms, M, N, row0, col0, dC.as<double>(), ldc, max_ctas, 0);
-        cudaEventRecord(ev[2]);
-        if (cudaEventSynchronize(ev[2]) != cudaSuccess) {
-            set_last_error("tf32 kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
-            rc = CFLX_ERR_CUDA;
-        }
-        float a = 0, b = 0;
-        cudaEventElapsedTime(&a, ev[0], ev[1]);
-        cudaEventElapsedTime(&b, ev[1], ev[2]);
-        if (r > 0) {
-            ms_split += a;
-            ms += b;
-        }
-    }
-    if (rc == CFLX_OK && cudaMemcpy2D(D, (size_t)N * 8, dC.p, ldc * 8, (size_t)N * 8, M, cudaMemcpyDeviceToHost) != cudaSuccess)
-        rc = CFLX_ERR_CUDA;
+    TrailingUpdate u;
+    int rc = u.create(Ma, Nb, K, false);
+    if (rc == CFLX_OK)
+        rc = u.with_tf32(terms, [&] {
+            return split_update(u, M, N, K, row0, col0, max_ctas, AT, B, C, D, ea_out, eb_out, reps, ms_out,
+                                split_ms_out);
+        });
+    const Tf32Workspace& ws = u.tf;
     const size_t na = (size_t)Ma * ws.KP, nb = (size_t)Nb * ws.KP;
     if (rc == CFLX_OK) rc = fetch(hiA_out, ws.hiA.p, na);
     if (rc == CFLX_OK && terms == 3) rc = fetch(loA_out, ws.loA.p, na);
     if (rc == CFLX_OK) rc = fetch(hiB_out, ws.hiB.p, nb);
     if (rc == CFLX_OK && terms == 3) rc = fetch(loB_out, ws.loB.p, nb);
-    if (rc == CFLX_OK) rc = fetch(ea_out, ws.ea, Ma);
-    if (rc == CFLX_OK) rc = fetch(eb_out, ws.eb, Nb);
     if (rc == CFLX_OK && cudaDeviceSynchronize() != cudaSuccess) rc = CFLX_ERR_CUDA;
-    if (ms_out) *ms_out = ms / reps;
-    if (split_ms_out) *split_ms_out = ms_split / reps;
     return rc;
 }
 

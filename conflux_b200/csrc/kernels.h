@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 
 #include <cstdint>
+#include <functional>
 #include <memory>
 
 #include "common.cuh"
@@ -26,16 +27,39 @@ struct GemmArgs {
 int gemm_tn_setup();
 int launch_gemm_tn(const GemmArgs& g, cudaStream_t stream);
 
-// ---------------------------------------------------------------- ozaki.cu
+// ---------------------------------------------------------------- ozaki.cu, tf32.cu: the split updates
+// What the workspaces of the wgmma updates share: the per-row power-of-two exponents of both operands (cap_a / cap_b
+// rows, whole CTA tiles of bm / bn rows), the contraction length and the SM count their persistent grids are capped at.
+struct SplitWorkspace {
+    DevBuf<int> ea;  // [cap_a]
+    DevBuf<int> eb;  // [cap_b]
+    int K = 0, cap_a = 0, cap_b = 0, sms = 0;
+    int init(int max_rows, int max_cols, int k, int bm, int bn) {
+        K = k;
+        cap_a = (int)round_up(max_rows > 1 ? max_rows : 1, bm);
+        cap_b = (int)round_up(max_cols > 1 ? max_cols : 1, bn);
+        CFLX_TRY(ea.alloc_exact(cap_a));
+        CFLX_TRY(eb.alloc_exact(cap_b));
+        CFLX_CUDA(cudaMemset(ea, 0, sizeof(int) * cap_a));
+        CFLX_CUDA(cudaMemset(eb, 0, sizeof(int) * cap_b));
+        int dev = 0;
+        CFLX_CUDA(cudaGetDevice(&dev));
+        CFLX_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+        return CFLX_OK;
+    }
+    // CTAs of a persistent launch over `tiles` tiles: at most one per SM, and at most max_ctas when it is > 0
+    int grid(int tiles, int max_ctas) const {
+        const int cap = max_ctas > 0 && max_ctas < sms ? max_ctas : sms;
+        return tiles < cap ? tiles : cap;
+    }
+};
+
 // FP64 trailing update on the int8 wgmma path (error-free digit planes): C -= L * U with L^T, U K-major in HBM.
-struct OzakiWorkspace {
+struct OzakiWorkspace : SplitWorkspace {
     struct Maps;                // the two CUtensorMap objects (kept out of this header)
     DevBuf<int8_t> planesA;     // [8][cap_a][K]
     DevBuf<int8_t> planesB;     // [8][cap_b][K]
-    DevBuf<int> ea;             // [cap_a]
-    DevBuf<int> eb;             // [cap_b]
     std::unique_ptr<Maps> maps;
-    int K = 0, cap_a = 0, cap_b = 0, sms = 0;
     OzakiWorkspace();
     ~OzakiWorkspace();  // where Maps is complete
 };
@@ -46,17 +70,14 @@ int ozaki_split_b(OzakiWorkspace* ws, const double* U, int64_t ld, int col0, int
 int wgmma_peak_probe(int n, double* tmacs_out);
 int launch_ozaki_gemm(OzakiWorkspace* ws, int M, int N, int row0, int col0, double* C, int64_t ldc, int max_ctas, cudaStream_t s);
 
-// ---------------------------------------------------------------- tf32.cu
 // The low-precision trailing update of the mixed-precision drivers on the TF32 wgmma path: C -= L * U with L^T, U K-major
 // in HBM, split into per-row power-of-two scaled TF32 terms (hi, and lo for terms = 3), FP32 accumulation, FP64 C.
-struct Tf32Workspace {
+struct Tf32Workspace : SplitWorkspace {
     struct Maps;               // the four CUtensorMap objects (kept out of this header)
     DevBuf<float> hiA, loA;    // [cap_a][KP]
     DevBuf<float> hiB, loB;    // [cap_b][KP]
-    DevBuf<int> ea;            // [cap_a]
-    DevBuf<int> eb;            // [cap_b]
     std::unique_ptr<Maps> maps;
-    int K = 0, KP = 0, cap_a = 0, cap_b = 0, sms = 0;  // KP: K rounded up to 8 (the tail is zero)
+    int KP = 0;  // K rounded up to 8 (the tail is zero)
     Tf32Workspace();
     ~Tf32Workspace();  // where Maps is complete
 };
@@ -68,6 +89,35 @@ int tf32_split_b(Tf32Workspace* ws, int terms, const double* U, int64_t ld, int 
 // launch_ozaki_gemm's window; ldc even, C 16-byte aligned, any M, N >= 1
 int launch_tf32_gemm(Tf32Workspace* ws, int terms, int M, int N, int row0, int col0, double* C, int64_t ldc, int max_ctas,
                      cudaStream_t s);
+
+// ---------------------------------------------------------------- update.cu
+// The trailing update C -= L U of a factorisation.  Its kind is fixed at creation: the FP64 DMMA kernel (gemm.cu), or
+// the int8 digit planes (ozaki.cu); a TF32 or TF32x3 kind (tf32.cu) takes over for the factorisations of one
+// mixed-precision driver (with_tf32).  The split kinds run a persistent kernel on operands split beforehand: split_a /
+// split_b fill them (no-ops for FP64, see splits()), apply reads a window of them.
+struct TrailingUpdate {
+    OzakiWorkspace oz;  // the int8 kind's digit planes
+    Tf32Workspace tf;   // the TF32 terms, made by the first with_tf32
+    int rows = 0, cols = 0, K = 0;
+    bool int8 = false;
+    int terms = 0;  // with_tf32's kind while it runs: 1 (TF32) or 3 (TF32x3); 0 otherwise
+
+    // operands of up to rows of L^T and cols of U with contraction length K; the int8 kind when `int8`, else FP64
+    int create(int rows, int cols, int K, bool int8);
+    // fn() on the TF32 kind of `terms` (1 or 3) terms; the kind of create again on return
+    int with_tf32(int terms, const std::function<int()>& fn);
+    // a persistent split kernel runs: split_a / split_b launch their kernel (callers count the launches by this)
+    bool splits() const { return int8 || terms; }
+    // the TF32 kind runs (the factors are not those of an FP64 update)
+    bool tf32() const { return terms != 0; }
+    // rows [0, n) of L^T (AT[k][row], ld) -> the A operand
+    int split_a(const double* AT, int64_t ld, int n, cudaStream_t s);
+    // columns [col0, col0 + n) of U (B[k][col], ld) -> the B operand, rows col0 ..
+    int split_b(const double* B, int64_t ld, int col0, int n, cudaStream_t s);
+    // The FP64 kind: launch_gemm_tn(g).  A split kind: g.D (g.M x g.N, g.ldd) -= A operand rows row0 .. times B operand
+    // rows col0 .., on all SMs but leave_sms (when > 0).
+    int apply(const GemmArgs& g, int row0, int col0, int leave_sms, cudaStream_t s);
+};
 
 // ---------------------------------------------------------------- panel.cu
 // Partial-pivot LU of the n x v panel stored TRANSPOSED in W (W[c][r], ld = ldw), in place, rows never move:

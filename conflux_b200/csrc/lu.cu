@@ -135,11 +135,8 @@ int handle_update_setup(Handle* h) {
     // path (ozaki.cu) runs only on request, CFLX_GEMM=ozaki, where the layer's contraction length is a whole number of
     // 128-element k chunks.
     const char* e = getenv("CFLX_GEMM");
-    if (e && !strcmp(e, "ozaki") && h->nlayr % 128 == 0 && h->nlayr <= 512) {
-        CFLX_TRY(ozaki_workspace_create(&h->oz, h->Ml, h->Nl, h->nlayr));
-        h->use_ozaki = true;
-    }
-    return CFLX_OK;
+    const bool int8 = e && !strcmp(e, "ozaki") && h->nlayr % 128 == 0 && h->nlayr <= 512;
+    return h->update.create(h->Ml, h->Nl, h->nlayr, int8);
 }
 int handle_side_stream(Handle* h) {
     int lo = 0, hi = 0;
@@ -181,11 +178,6 @@ void handle_equil_begin(Handle* h) {
 }
 int handle_equil_end(Handle* h, bool apply, int info, char equed, double rowcnd, double colcnd, const double* c) {
     if (apply && info == 0) CFLX_TRY(equil_record_set(&h->eq.in, equed, rowcnd, colcnd, h->eq.qr, c, h->M, h->comm->stream));
-    return CFLX_OK;
-}
-int handle_tf32_begin(Handle* h, int terms) {
-    if (!h->tf.maps) CFLX_TRY(tf32_workspace_create(&h->tf, h->Ml, h->Nl, std::max(h->nlayr, 1)));
-    h->update_terms = terms;
     return CFLX_OK;
 }
 int handle_launch_count(Handle* h, int64_t* count_out, int reset) {
@@ -390,27 +382,23 @@ int panel_phase(cflx_lu* lu, int k, int fnpr, cudaStream_t s) {
     return CFLX_OK;
 }
 
-// digit planes of the operands of this step's trailing update (int8 wgmma path): L^T slab of this layer, U slab columns
-// (or, in a TF32 update mode, the TF32 terms of both slabs)
-int ozaki_planes_a(cflx_lu* lu, int n_act, int64_t ld2, cudaStream_t s) {
-    if (!(lu->use_ozaki || lu->update_terms) || n_act <= 0) return CFLX_OK;
+// the operands of this step's trailing update, split for a split kind: this layer's slab of L^T, and columns
+// [col0, col0 + n) of its slab of U
+int update_split_a(cflx_lu* lu, int n_act, int64_t ld2, cudaStream_t s) {
+    if (!lu->update.splits() || n_act <= 0) return CFLX_OK;
     PhaseTimer t(lu, RG_step6_dgemm, s);
     lu->launches++;
-    const double* LT = lu->LT + (int64_t)lu->pk * lu->nlayr * ld2;
-    if (lu->update_terms) return tf32_split_a(&lu->tf, lu->update_terms, LT, ld2, n_act, s);
-    return ozaki_split_a(&lu->oz, LT, ld2, n_act, s);
+    return lu->update.split_a(lu->LT + (int64_t)lu->pk * lu->nlayr * ld2, ld2, n_act, s);
 }
-int ozaki_planes_b(cflx_lu* lu, int col0, int n, int64_t ldu, cudaStream_t s) {
-    if (!(lu->use_ozaki || lu->update_terms) || n <= 0) return CFLX_OK;
+int update_split_b(cflx_lu* lu, int col0, int n, int64_t ldu, cudaStream_t s) {
+    if (!lu->update.splits() || n <= 0) return CFLX_OK;
     PhaseTimer t(lu, RG_step6_dgemm, s);
     lu->launches++;
-    const double* U = lu->U + (int64_t)lu->pk * lu->nlayr * ldu;
-    if (lu->update_terms) return tf32_split_b(&lu->tf, lu->update_terms, U, ldu, col0, n, s);
-    return ozaki_split_b(&lu->oz, U, ldu, col0, n, s);
+    return lu->update.split_b(lu->U + (int64_t)lu->pk * lu->nlayr * ldu, ldu, col0, n, s);
 }
 
 int trailing_gemm(cflx_lu* lu, int k, int part, int fnpr, int n_act, int col_lo, int ncols, int64_t ld2, int64_t ldu,
-                  int u_col_off, cudaStream_t s, int max_ctas = 0) {
+                  int u_col_off, cudaStream_t s, int leave_sms = 0) {
     if (n_act <= 0 || ncols <= 0) return CFLX_OK;
     PhaseTimer t(lu, RG_step6_dgemm, s);
     GemmArgs g{};
@@ -429,10 +417,7 @@ int trailing_gemm(cflx_lu* lu, int k, int part, int fnpr, int n_act, int col_lo,
     g.beta = 1.0;
     const int e = 4 * k + 2 * part;
     if (lu->time_gemm) CFLX_CUDA(cudaEventRecord(lu->ev[e], s));
-    if (lu->update_terms)
-        CFLX_TRY(launch_tf32_gemm(&lu->tf, lu->update_terms, g.M, g.N, 0, u_col_off, g.D, g.ldd, max_ctas, s));
-    else if (lu->use_ozaki) CFLX_TRY(launch_ozaki_gemm(&lu->oz, g.M, g.N, 0, u_col_off, g.D, g.ldd, max_ctas, s));
-    else CFLX_TRY(launch_gemm_tn(g, s));
+    CFLX_TRY(lu->update.apply(g, 0, u_col_off, leave_sms, s));
     if (lu->time_gemm) CFLX_CUDA(cudaEventRecord(lu->ev[e + 1], s));
     lu->ev_used[e / 2] = lu->time_gemm;
     lu->gemm_flops += 2.0 * g.M * (double)g.N * g.K;
@@ -580,8 +565,8 @@ int finish_step(cflx_lu* lu, int k, int& fnpr) {
     // Look-ahead: the rank that owns panel k+1 updates those v columns first (they are its first live block), forks
     // the pivot search of iteration k+1 onto the side stream, and only then updates the remaining columns.
     const bool next_col = (k + 1 < lu->Nt) && (pj == (k + 1) % Py);
-    CFLX_TRY(ozaki_planes_a(lu, n_act, ld2, s));
-    if (n_act > 0) CFLX_TRY(ozaki_planes_b(lu, 0, split_u ? std::min(v, ncols) : ncols, ldu, s));
+    CFLX_TRY(update_split_a(lu, n_act, ld2, s));
+    if (n_act > 0) CFLX_TRY(update_split_b(lu, 0, split_u ? std::min(v, ncols) : ncols, ldu, s));
     if (next_col) {
         const int w = std::min(v, ncols);
         CFLX_TRY(trailing_gemm(lu, k, 0, fnpr, n_act, c0, w, ld2, ldu, 0, s));
@@ -599,11 +584,9 @@ int finish_step(cflx_lu* lu, int k, int& fnpr) {
             lu->launches += 2 * (v / lu->nb) - 1;
         }
         if (split_u) CFLX_TRY(store_factors());
-        if (split_u && n_act > 0) CFLX_TRY(ozaki_planes_b(lu, w, ncols - w, ldu, s));
-        // the persistent int8 and TF32 kernels leave the SMs of the concurrent pivot search alone
-        const int leave = (side && (lu->use_ozaki || lu->update_terms)) ? lu->pws.cta_cap : 0;
-        const int sms = lu->update_terms ? lu->tf.sms : lu->oz.sms;
-        CFLX_TRY(trailing_gemm(lu, k, 1, fnpr, n_act, c0 + w, ncols - w, ld2, ldu, w, s, leave > 0 ? sms - leave : 0));
+        if (split_u && n_act > 0) CFLX_TRY(update_split_b(lu, w, ncols - w, ldu, s));
+        // the persistent split kernels leave the SMs of the concurrent pivot search alone
+        CFLX_TRY(trailing_gemm(lu, k, 1, fnpr, n_act, c0 + w, ncols - w, ld2, ldu, w, s, side ? lu->pws.cta_cap : 0));
         if (side) CFLX_CUDA(cudaStreamWaitEvent(s, lu->ev_join, 0));
     } else {
         CFLX_TRY(trailing_gemm(lu, k, 0, fnpr, n_act, c0, ncols, ld2, ldu, 0, s));
@@ -1149,7 +1132,7 @@ int lu_factor_run(cflx_lu* lu, double* ms_out) {
     }
     if (lu->a0_is_next) CFLX_CUDA(cudaStreamSynchronize(lu->copy));  // the caller's staging buffer is free again
     lu->factored = true;
-    lu->low_prec = lu->update_terms != 0;
+    lu->low_prec = lu->update.tf32();
     lu->perm_done = true;
     return CFLX_OK;
 }
@@ -1640,11 +1623,8 @@ int cflx_lu_sv_mixed(cflx_lu* lu, int prec, int nrhs, const double* B, int ldb, 
                        "after the factorisation", __func__);
         return CFLX_ERR_STATE;
     }
-    CFLX_TRY(handle_tf32_begin(lu, prec));
     double ms = 0.0;
-    const int run = lu_factor_run(lu, &ms);
-    lu->update_terms = 0;
-    CFLX_TRY(run);
+    CFLX_TRY(lu->update.with_tf32(prec, [&] { return lu_factor_run(lu, &ms); }));
     double anorm = 0.0;
     CFLX_TRY(norminf_grid(*lu, lu->A0, &anorm));
     CFLX_TRY(lu_solve_prepare(lu));
@@ -1679,7 +1659,7 @@ int cflx_host_free(void* p) {
     return CFLX_OK;
 }
 
-int cflx_lu_uses_ozaki(const cflx_lu* lu) { return lu && lu->use_ozaki ? 1 : 0; }
+int cflx_lu_uses_ozaki(const cflx_lu* lu) { return lu && lu->update.int8 ? 1 : 0; }
 int cflx_lu_launch_count(cflx_lu* lu, int64_t* count_out, int reset) {
     REFUSE_IF(!lu);
     REFUSE_IF(!count_out);

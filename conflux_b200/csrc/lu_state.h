@@ -230,15 +230,9 @@ struct Handle : Grid {
     bool have_input = false, factored = false;
     bool a0_is_next = false;  // A0 already holds (or is receiving) the next input (LU input streaming)
     int64_t launches = 0;
-    Stream side;        // high-priority look-ahead stream (null: no overlap)
-    OzakiWorkspace oz;  // digit planes of the int8 wgmma trailing update (CFLX_GEMM=ozaki)
-    bool use_ozaki = false;
-    // The trailing update of the next factorisation: FP64 (the DMMA kernel, or ozaki as above), or the TF32 wgmma path
-    // with one or three terms (tf32.cu).  Only the mixed-precision drivers set a TF32 mode, for one factorisation; the
-    // split workspace is made on first use.  low_prec: the factors of the last factorisation came from a TF32 update.
-    int update_terms = 0;  // 0: FP64, 1: TF32, 3: TF32x3
-    Tf32Workspace tf;
-    bool low_prec = false;
+    Stream side;            // high-priority look-ahead stream (null: no overlap)
+    TrailingUpdate update;  // handle_update_setup; TF32 for the factorisations of a mixed-precision driver
+    bool low_prec = false;  // the factors of the last factorisation came from a TF32 update
     SolveCache sv;
     EquilState eq;  // cflx_*_equilibrate / cflx_*_svx
     RbtState rbt;   // cflx_*_rbt: the transform of the input and of the factors
@@ -271,8 +265,6 @@ void handle_equil_begin(Handle* h);
 // query leaves the record and its scales
 int handle_equil_end(Handle* h, bool apply, int info, char equed, double rowcnd, double colcnd, const double* c);
 int handle_launch_count(Handle* h, int64_t* count_out, int reset);
-// h->tf for the next factorisation's TF32 update with `terms` (1 or 3), made on first use; h->update_terms = terms
-int handle_tf32_begin(Handle* h, int terms);
 // COLLECTIVE (world): *same = every rank has ok and the same words, from one ncclMin over {w.., ~w.., ok}
 int world_agree(Handle* h, bool ok, std::initializer_list<unsigned long long> words, bool* same);
 }  // namespace cflx

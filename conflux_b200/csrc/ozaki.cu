@@ -24,14 +24,10 @@
 //                  pass.  The B planes t, t+1, ... of a stage are contiguous 64-row tiles and the accumulators of their
 //                  groups are contiguous registers: all planes of one A_s in the pass go through ONE wgmma of
 //                  N = 64 * planes, so A_s is read from shared memory once per pass and k step.
-#include <cuda.h>
-
 #include <algorithm>
-#include <cstdlib>
-#include <cstring>
 
-#include "common.cuh"
 #include "kernels.h"
+#include "wgmma.cuh"
 
 namespace cflx {
 
@@ -47,25 +43,6 @@ constexpr int OZ_CONS_WARPS = 8;
 constexpr int OZ_THREADS = 32 * OZ_CONS_WARPS + 32;
 constexpr size_t OZ_SMEM = 1024 /*alignment slack*/ + (size_t)OZ_STAGES * OZ_STAGE_BYTES + 64 /*barriers*/;
 constexpr int OZ_SPLIT_KC = 128;                      // k-chunk of the digit-plane split (K is a multiple of it)
-
-// ---------------------------------------------------------------------------------------------- PTX wrappers
-__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* map, int c0, int c1, int c2, uint64_t* bar) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];" ::"r"(
-            smem_u32(smem_dst)),
-        "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar))
-        : "memory");
-}
-// shared-memory matrix descriptor of a K-major, 64-byte-swizzled operand tile (rows of 64 bytes, 8-row groups 512 B
-// apart): start address >> 4 | LBO (unused for swizzled K-major) = 1 at bit 16 | SBO = 512 >> 4 at bit 32 |
-// SWIZZLE_64B (2) at bit 62.  Stepping 32 bytes along K inside the swizzle atom adds 2 to the start address field.
-__device__ __forceinline__ uint64_t smem_desc_sw64(uint32_t saddr) {
-    return (uint64_t)((saddr & 0x3FFFF) >> 4) | (1ull << 16) | ((uint64_t)(512 >> 4) << 32) | (2ull << 62);
-}
-__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
 // D(64 x n, int32 registers in the wgmma accumulator layout) += A(64 x 32, smem desc) * B(32 x n, smem desc), int8.
 // Accumulator layout (thread T of the warpgroup, warp w = T / 32, lane l): d[4j + 2h + x] is row 16w + l/4 + 8h,
@@ -140,8 +117,8 @@ __device__ __forceinline__ void pass_products(int* acc, uint32_t a_base, uint32_
         constexpr int PLANES = G1 - S - T_LO + 1;
 #pragma unroll
         for (int k = 0; k < OZ_KC / 32; ++k)
-            wgmma_s8<PLANES>(acc + 32 * (S + T_LO - G0), smem_desc_sw64(a_base + S * OZ_A_BYTES + 32 * k),
-                             smem_desc_sw64(b_base + T_LO * OZ_B_BYTES + 32 * k));
+            wgmma_s8<PLANES>(acc + 32 * (S + T_LO - G0), smem_desc<64>(a_base + S * OZ_A_BYTES + 32 * k),
+                             smem_desc<64>(b_base + T_LO * OZ_B_BYTES + 32 * k));
         pass_products<G0, S + 1>(acc, a_base, b_base);
     }
 }
@@ -277,7 +254,7 @@ __global__ void __launch_bounds__(256, 1) wgmma_peak_kernel(int iters, int* sink
     wgmma_fence();
     for (int it = 0; it < iters; ++it) {
 #pragma unroll
-        for (int k = 0; k < 2; ++k) wgmma_s8<PLANES>(acc, smem_desc_sw64(a + 32 * k), smem_desc_sw64(b + 32 * k));
+        for (int k = 0; k < 2; ++k) wgmma_s8<PLANES>(acc, smem_desc<64>(a + 32 * k), smem_desc<64>(b + 32 * k));
         wgmma_commit();
         wgmma_wait<1>();
     }
@@ -344,37 +321,12 @@ __global__ void __launch_bounds__(256) ozaki_split_kernel(const double* __restri
 }
 
 // ---------------------------------------------------------------------------------------------- host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn encode_fn() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess && p) fn = (EncodeTiledFn)p;
-        cudaGetLastError();
-    }
-    return fn;
-}
 // planes: [OZ_S][cap_rows][K] int8; box = 64 bytes of k x box_rows rows of one plane, 64-byte swizzle
 int make_plane_map(CUtensorMap* map, const int8_t* planes, int K, int cap_rows, int box_rows) {
-    EncodeTiledFn fn = encode_fn();
-    if (!fn) {
-        set_last_error("cuTensorMapEncodeTiled is not available from the driver");
-        return CFLX_ERR_CUDA;
-    }
-    cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)cap_rows, (cuuint64_t)OZ_S};
-    cuuint64_t strides[2] = {(cuuint64_t)K, (cuuint64_t)K * (cuuint64_t)cap_rows};
-    cuuint32_t box[3] = {(cuuint32_t)OZ_KC, (cuuint32_t)box_rows, 1};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, (void*)planes, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        set_last_error("cuTensorMapEncodeTiled failed (%d) for K=%d rows=%d", (int)r, K, cap_rows);
-        return CFLX_ERR_CUDA;
-    }
-    return CFLX_OK;
+    const cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)cap_rows, (cuuint64_t)OZ_S};
+    const cuuint64_t strides[2] = {(cuuint64_t)K, (cuuint64_t)K * (cuuint64_t)cap_rows};
+    const cuuint32_t box[3] = {(cuuint32_t)OZ_KC, (cuuint32_t)box_rows, 1};
+    return make_tensor_map(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, planes, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_64B);
 }
 }  // namespace
 
@@ -390,17 +342,11 @@ int ozaki_workspace_create(OzakiWorkspace* ws, int max_rows, int max_cols, int K
         set_last_error("ozaki: contraction length %d unsupported (multiple of 128, <= 512)", K);
         return CFLX_ERR_UNSUPPORTED;
     }
-    ws->K = K;
-    ws->cap_a = (int)round_up(max_rows, OZ_BM);
-    ws->cap_b = (int)round_up(max_cols, OZ_BN);
+    CFLX_TRY(ws->init(max_rows, max_cols, K, OZ_BM, OZ_BN));
     CFLX_TRY(ws->planesA.alloc_exact((size_t)OZ_S * ws->cap_a * K));
     CFLX_TRY(ws->planesB.alloc_exact((size_t)OZ_S * ws->cap_b * K));
     CFLX_CUDA(cudaMemset(ws->planesA, 0, (size_t)OZ_S * ws->cap_a * K));
     CFLX_CUDA(cudaMemset(ws->planesB, 0, (size_t)OZ_S * ws->cap_b * K));
-    CFLX_TRY(ws->ea.alloc_exact(ws->cap_a));
-    CFLX_TRY(ws->eb.alloc_exact(ws->cap_b));
-    CFLX_CUDA(cudaMemset(ws->ea, 0, sizeof(int) * ws->cap_a));
-    CFLX_CUDA(cudaMemset(ws->eb, 0, sizeof(int) * ws->cap_b));
     ws->maps = std::make_unique<OzakiWorkspace::Maps>();
     CFLX_TRY(make_plane_map(&ws->maps->a, ws->planesA, K, ws->cap_a, OZ_BM));
     CFLX_TRY(make_plane_map(&ws->maps->b, ws->planesB, K, ws->cap_b, OZ_BN));
@@ -408,9 +354,6 @@ int ozaki_workspace_create(OzakiWorkspace* ws, int max_rows, int max_cols, int K
     CFLX_CUDA(cfg.raise(OZ_SMEM, [&] {
         return cudaFuncSetAttribute(ozaki_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)OZ_SMEM);
     }));
-    int dev = 0;
-    CFLX_CUDA(cudaGetDevice(&dev));
-    CFLX_CUDA(cudaDeviceGetAttribute(&ws->sms, cudaDevAttrMultiProcessorCount, dev));
     return CFLX_OK;
 }
 
@@ -477,11 +420,7 @@ int launch_ozaki_gemm(OzakiWorkspace* ws, int M, int N, int row0, int col0, doub
     g.ea = ws->ea; g.eb = ws->eb;
     g.tiles_m = (M + OZ_BM - 1) / OZ_BM;
     g.tiles_n = (N + OZ_BN - 1) / OZ_BN;
-    int grid = g.tiles_m * g.tiles_n;
-    int cap = ws->sms;
-    if (max_ctas > 0 && max_ctas < cap) cap = max_ctas;
-    if (grid > cap) grid = cap;
-    ozaki_gemm_kernel<<<grid, OZ_THREADS, OZ_SMEM, s>>>(ws->maps->a, ws->maps->b, g);
+    ozaki_gemm_kernel<<<ws->grid(g.tiles_m * g.tiles_n, max_ctas), OZ_THREADS, OZ_SMEM, s>>>(ws->maps->a, ws->maps->b, g);
     CFLX_CUDA(cudaGetLastError());
     return CFLX_OK;
 }

@@ -17,14 +17,8 @@
 //                  the consumers finish the current one;
 //   warps 0-7      two warpgroups, 64 rows of the tile each, 64 FP32 accumulators per thread; a stage is released once
 //                  the wgmma group that read it has completed (wait_group 1), so one group is always in flight.
-#include <cuda.h>
-
-#include <algorithm>
-#include <cstdlib>
-#include <cstring>
-
-#include "common.cuh"
 #include "kernels.h"
+#include "wgmma.cuh"
 
 namespace cflx {
 
@@ -42,24 +36,6 @@ struct TfCfg {
     static constexpr int STAGES = TERMS == 1 ? 6 : 3;
     static constexpr size_t SMEM = 1024 /*alignment slack*/ + (size_t)STAGES * STAGE_BYTES + 128 /*barriers*/;
 };
-
-__device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
-            smem_u32(smem_dst)),
-        "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar))
-        : "memory");
-}
-// shared-memory matrix descriptor of a K-major, 128-byte-swizzled operand tile (rows of 128 bytes, 8-row groups 1024 B
-// apart): start address >> 4 | LBO (unused for swizzled K-major) = 1 at bit 16 | SBO = 1024 >> 4 at bit 32 |
-// SWIZZLE_128B (1) at bit 62.  Stepping 8 TF32 (32 bytes) along K inside the swizzle atom adds 2 to the start field.
-__device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t saddr) {
-    return (uint64_t)((saddr & 0x3FFFF) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
-}
-__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
 // D(64 x 128, FP32 registers in the wgmma accumulator layout) += A(64 x 8, smem desc) * B(8 x 128, smem desc), TF32.
 // Accumulator layout (thread T of the warpgroup, warp w = T / 32, lane l): d[4j + 2h + x] is row 16w + l/4 + 8h,
@@ -164,10 +140,10 @@ tf32_gemm_kernel(const __grid_constant__ CUtensorMap mapAh, const __grid_constan
             for (int k = 0; k < TF_KC / 8; ++k) {
                 if constexpr (TERMS == 3) {
                     const uint32_t a_lo = a_hi + TF_A_BYTES + TF_B_BYTES, b_lo = b_hi + TF_A_BYTES + TF_B_BYTES;
-                    wgmma_tf32_n128(acc, smem_desc_sw128(a_lo + 32 * k), smem_desc_sw128(b_hi + 32 * k));
-                    wgmma_tf32_n128(acc, smem_desc_sw128(a_hi + 32 * k), smem_desc_sw128(b_lo + 32 * k));
+                    wgmma_tf32_n128(acc, smem_desc<128>(a_lo + 32 * k), smem_desc<128>(b_hi + 32 * k));
+                    wgmma_tf32_n128(acc, smem_desc<128>(a_hi + 32 * k), smem_desc<128>(b_lo + 32 * k));
                 }
-                wgmma_tf32_n128(acc, smem_desc_sw128(a_hi + 32 * k), smem_desc_sw128(b_hi + 32 * k));
+                wgmma_tf32_n128(acc, smem_desc<128>(a_hi + 32 * k), smem_desc<128>(b_hi + 32 * k));
             }
             wgmma_commit();
             wgmma_wait<1>();                                      // the group of the previous stage has completed
@@ -261,37 +237,12 @@ __global__ void __launch_bounds__(256) tf32_split_kernel(const double* __restric
 }
 
 // ---------------------------------------------------------------------------------------------- host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn encode_fn() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess && p) fn = (EncodeTiledFn)p;
-        cudaGetLastError();
-    }
-    return fn;
-}
 // slab: [rows][KP] FP32; box = 32 k x box_rows rows, 128-byte swizzle; what lies beyond KP or rows is read as zero
 int make_slab_map(CUtensorMap* map, const float* slab, int KP, int rows, int box_rows) {
-    EncodeTiledFn fn = encode_fn();
-    if (!fn) {
-        set_last_error("cuTensorMapEncodeTiled is not available from the driver");
-        return CFLX_ERR_CUDA;
-    }
-    cuuint64_t dims[2] = {(cuuint64_t)KP, (cuuint64_t)rows};
-    cuuint64_t strides[1] = {(cuuint64_t)KP * sizeof(float)};
-    cuuint32_t box[2] = {(cuuint32_t)TF_KC, (cuuint32_t)box_rows};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)slab, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        set_last_error("cuTensorMapEncodeTiled failed (%d) for KP=%d rows=%d", (int)r, KP, rows);
-        return CFLX_ERR_CUDA;
-    }
-    return CFLX_OK;
+    const cuuint64_t dims[2] = {(cuuint64_t)KP, (cuuint64_t)rows};
+    const cuuint64_t strides[1] = {(cuuint64_t)KP * sizeof(float)};
+    const cuuint32_t box[2] = {(cuuint32_t)TF_KC, (cuuint32_t)box_rows};
+    return make_tensor_map(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, slab, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 template <int TERMS>
@@ -317,10 +268,8 @@ int tf32_workspace_create(Tf32Workspace* ws, int max_rows, int max_cols, int K) 
         set_last_error("tf32: contraction length %d unsupported", K);
         return CFLX_ERR_UNSUPPORTED;
     }
-    ws->K = K;
+    CFLX_TRY(ws->init(max_rows, max_cols, K, TF_BM, TF_BN));
     ws->KP = (int)round_up(K, 8);
-    ws->cap_a = (int)round_up(std::max(max_rows, 1), TF_BM);
-    ws->cap_b = (int)round_up(std::max(max_cols, 1), TF_BN);
     const size_t na = (size_t)ws->cap_a * ws->KP, nb = (size_t)ws->cap_b * ws->KP;
     for (auto* b : {&ws->hiA, &ws->loA}) {
         CFLX_TRY(b->alloc_exact(na));
@@ -330,21 +279,13 @@ int tf32_workspace_create(Tf32Workspace* ws, int max_rows, int max_cols, int K) 
         CFLX_TRY(b->alloc_exact(nb));
         CFLX_CUDA(cudaMemset(b->p, 0, nb * sizeof(float)));
     }
-    CFLX_TRY(ws->ea.alloc_exact(ws->cap_a));
-    CFLX_TRY(ws->eb.alloc_exact(ws->cap_b));
-    CFLX_CUDA(cudaMemset(ws->ea, 0, sizeof(int) * ws->cap_a));
-    CFLX_CUDA(cudaMemset(ws->eb, 0, sizeof(int) * ws->cap_b));
     ws->maps = std::make_unique<Tf32Workspace::Maps>();
     CFLX_TRY(make_slab_map(&ws->maps->ah, ws->hiA, ws->KP, ws->cap_a, TF_BM));
     CFLX_TRY(make_slab_map(&ws->maps->al, ws->loA, ws->KP, ws->cap_a, TF_BM));
     CFLX_TRY(make_slab_map(&ws->maps->bh, ws->hiB, ws->KP, ws->cap_b, TF_BN));
     CFLX_TRY(make_slab_map(&ws->maps->bl, ws->loB, ws->KP, ws->cap_b, TF_BN));
     CFLX_TRY(tf32_kernel_setup<1>());
-    CFLX_TRY(tf32_kernel_setup<3>());
-    int dev = 0;
-    CFLX_CUDA(cudaGetDevice(&dev));
-    CFLX_CUDA(cudaDeviceGetAttribute(&ws->sms, cudaDevAttrMultiProcessorCount, dev));
-    return CFLX_OK;
+    return tf32_kernel_setup<3>();
 }
 
 // rows [0, n) of L^T (LT[k][row], ld) -> the A slabs
@@ -384,10 +325,7 @@ int launch_tf32_gemm(Tf32Workspace* ws, int terms, int M, int N, int row0, int c
     g.ea = ws->ea; g.eb = ws->eb;
     g.tiles_m = (M + TF_BM - 1) / TF_BM;
     g.tiles_n = (N + TF_BN - 1) / TF_BN;
-    int grid = g.tiles_m * g.tiles_n;
-    int cap = ws->sms;
-    if (max_ctas > 0 && max_ctas < cap) cap = max_ctas;
-    if (grid > cap) grid = cap;
+    const int grid = ws->grid(g.tiles_m * g.tiles_n, max_ctas);
     const Tf32Workspace::Maps& m = *ws->maps;
     if (terms == 1) tf32_gemm_kernel<1><<<grid, TF_THREADS, TfCfg<1>::SMEM, s>>>(m.ah, m.bh, m.al, m.bl, g);
     else tf32_gemm_kernel<3><<<grid, TF_THREADS, TfCfg<3>::SMEM, s>>>(m.ah, m.bh, m.al, m.bl, g);

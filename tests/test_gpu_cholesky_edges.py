@@ -11,8 +11,6 @@ Constants: every tolerance is one of the hp_ref bounds (gamma_n = n u / (1 - n u
     kappa_max = the largest condition number of an inverted diagonal block (128 for the tile driver, nb of the panel
     TRSM), and the forward error against the longdouble factor ||L^ - L||_F / ||L||_2 <= kappa(A) eps / (1 - kappa(A) eps)
     with eps that bound over ||A||_2."""
-import json
-import os
 import re
 
 import numpy as np
@@ -243,13 +241,14 @@ def test_factor_graded_matrix_rowwise(N, v):
     assert hp.chol_normwise_ok(A, L, _kappa_max(L, v))
 
 
-@pytest.mark.parametrize("kind,N,v", chol_ref.BITS_CASES)
-def test_default_path_factor_bits_are_pinned(kind, N, v, golden_dir):
-    """the factor of the default update path and the launch count of one factorisation are those recorded in
-    tests/golden/chol_factor_bits.json (tests/golden/make_chol_golden.py)"""
-    with open(os.path.join(golden_dir, "chol_factor_bits.json")) as f:
-        want = json.load(f)[f"{kind}_{N}_{v}"]
-    assert make_chol_golden.factor_bits(kind, N, v) == want
+@pytest.mark.parametrize("update,kind,N,v",
+                         [(u,) + c for u in make_chol_golden.UPDATES for c in make_chol_golden.update_cases(u)])
+def test_default_path_factor_bits_are_pinned(update, kind, N, v, golden_dir):
+    """the factor and the launch count of one factorisation of each trailing-update kind are those recorded in
+    tests/golden/chol_factor_bits.json (the default FP64 update) and update_factor_bits.json (int8, TF32, TF32x3), by
+    tests/golden/make_chol_golden.py"""
+    want = make_chol_golden.golden(update, golden_dir)[f"{kind}_{N}_{v}"]
+    assert make_chol_golden.factor_bits(kind, N, v, update) == want
 
 
 @pytest.mark.parametrize("v", [128, 256, 512])

@@ -388,13 +388,13 @@ def test_factor_hard_inputs_and_column_scaling(N, v, kind):
     assert _same_bits(LUd, want)
 
 
-@pytest.mark.parametrize("kind,N,v", make_lu_golden.CASES)
-def test_default_path_factor_bits_are_pinned(kind, N, v, golden_dir):
-    """the factor, the permutation and the launch count of the default path are those recorded in
-    tests/golden/lu_factor_bits.json (tests/golden/make_lu_golden.py)"""
-    with open(os.path.join(golden_dir, "lu_factor_bits.json")) as f:
-        want = json.load(f)[f"{kind}_{N}_{v}"]
-    assert make_lu_golden.factor_bits(kind, N, v) == want
+@pytest.mark.parametrize("update,kind,N,v", [(u,) + c for u in make_lu_golden.UPDATES for c in make_lu_golden.update_cases(u)])
+def test_default_path_factor_bits_are_pinned(update, kind, N, v, golden_dir):
+    """the factor, the permutation and the launch count of each trailing-update kind are those recorded in
+    tests/golden/lu_factor_bits.json (the default FP64 update) and update_factor_bits.json (int8, TF32, TF32x3), by
+    tests/golden/make_lu_golden.py"""
+    want = make_lu_golden.golden(update, golden_dir)[f"{kind}_{N}_{v}"]
+    assert make_lu_golden.factor_bits(kind, N, v, update) == want
 
 
 # ----------------------------------------------------------------------------------------------- run-time switches
