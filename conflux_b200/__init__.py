@@ -15,7 +15,7 @@ import numpy as np
 
 from ._lib import ConfluxError, LIB_PATH, SYMBOLS, ShareLayout, check, lib
 
-__all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "LU_rep_fixed", "rbt_multipliers", "LU_rep_rbt", "lu_rbt_solve", "lu_rbt_apply_local", "residual", "validate", "lu_solve", "lu_rcond", "lu_refine", "lu_refine_x", "lu_equilibrate", "lu_svx", "lu_equilibrate_b", "lu_svxx", "lu_inverse", "lu_det", "rhs_local_cols", "lu_solve_local", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
+__all__ = ["pinned_empty", "pinned_free", "Comm", "lu_params", "LU_rep", "LU_rep_fixed", "rbt_multipliers", "LU_rep_rbt", "lu_rbt_solve", "lu_rbt_apply_local", "residual", "validate", "lu_solve", "lu_rcond", "lu_refine", "lu_refine_x", "lu_equilibrate", "lu_svx", "lu_equilibrate_b", "lu_svxx", "lu_inverse", "lu_det", "rhs_local_cols", "lu_solve_local", "refine_block_cols", "lu_refine_local", "lu_refine_x_local", "lu_svx_local", "lu_svxx_local", "timeline", "auto_grid", "lu_dims", "init_matrix_host", "ConfluxError", "dbg", "cholesky", "chol_dims", "chol_auto_grid"]
 
 
 def auto_grid(M, N, P):
@@ -516,20 +516,88 @@ def rhs_local_cols(nrhs, v, Py):
     return n.value
 
 
-def _solve_local(fn, what, Ml, v, Py, layer0, B_share, nrhs, out, *lead):
-    """B_share / out checked as (Ml, n >= rhs_local_cols) float64 shares with contiguous rows; out None: a new zeroed NumPy
-    array; B_share None is allowed off layer 0 (it is not read there)"""
+def refine_block_cols(v):
+    """The block width of the distributed refinement and expert drivers (lu_refine_local ... cholesky.svxx_local) for
+    tile size v: the whole number of tiles nearest 256 columns, at least one tile."""
+    n = ctypes.c_int()
+    check(lib().cflx_refine_block_cols(int(v), ctypes.byref(n)), "refine_block_cols")
+    return n.value
+
+
+def _local_args(what, Ml, v, Py, layer0, B_share, nrhs, X_share, x_in, x_name="out"):
+    """(B pointer, ldb, X pointer, ldx, X) of a distributed call: B_share / X_share checked as (Ml, n >= rhs_local_cols)
+    float64 shares with contiguous rows.  B_share None is allowed off layer 0 (it is not read there).  x_in: X_share is
+    the solution on entry, required on layer 0 and None allowed elsewhere (not written); else X_share None is a new zeroed
+    NumPy array."""
     ncl = rhs_local_cols(nrhs, v, Py)
     bptr, ldb = None, ncl
     if B_share is not None:
         bptr, _, ldb = _share_out(B_share, Ml, ncl, what, strided=True, name="B_share")
     elif layer0:
         raise ValueError(f"{what}: B_share is read on layer 0 and may not be None there")
-    if out is None:
-        out = np.zeros((Ml, ncl))
-    xptr, out, ldx = _share_out(out, Ml, ncl, what, strided=True)
+    if X_share is None and x_in:
+        if layer0:
+            raise ValueError(f"{what}: {x_name} is read on layer 0 and may not be None there")
+        return bptr, ldb, None, ncl, None
+    if X_share is None:
+        X_share = np.zeros((Ml, ncl))
+    xptr, X_share, ldx = _share_out(X_share, Ml, ncl, what, strided=True, name=x_name)
+    return bptr, ldb, xptr, ldx, X_share
+
+
+def _solve_local(fn, what, Ml, v, Py, layer0, B_share, nrhs, out, *lead):
+    """B_share / out checked as (Ml, n >= rhs_local_cols) float64 shares with contiguous rows; out None: a new zeroed NumPy
+    array; B_share None is allowed off layer 0 (it is not read there)"""
+    bptr, ldb, xptr, ldx, out = _local_args(what, Ml, v, Py, layer0, B_share, nrhs, out, False)
     check(fn(*lead, int(nrhs), bptr, ldb, xptr, ldx), what)
     return out
+
+
+def _refine_local(fn, what, Ml, v, Py, layer0, B_share, X_share, nrhs, ferr, *lead):
+    bptr, ldb, xptr, ldx, X = _local_args(what, Ml, v, Py, layer0, B_share, nrhs, X_share, True, "X_share")
+    fe, be = np.empty(nrhs), np.empty(nrhs)
+    check(fn(*lead, int(nrhs), bptr, ldb, xptr, ldx, fe.ctypes.data if ferr else None, be.ctypes.data), what)
+    return X, (fe if ferr else None), be
+
+
+def _refine_x_local(fn, what, Ml, v, Py, layer0, B_share, X_share, nrhs, cwise, *lead):
+    bptr, ldb, xptr, ldx, X = _local_args(what, Ml, v, Py, layer0, B_share, nrhs, X_share, True, "X_share")
+    be, en, ec = np.empty(nrhs), np.zeros((nrhs, 3)), np.zeros((nrhs, 3))
+    rcond, info = ctypes.c_double(), ctypes.c_int()
+    check(fn(*lead, int(nrhs), bptr, ldb, xptr, ldx, ctypes.byref(rcond), be.ctypes.data, en.ctypes.data,
+             ec.ctypes.data if cwise else None, ctypes.byref(info)), what)
+    return X, dict(rcond=rcond.value, berr=be, err_norm=en, err_comp=ec if cwise else None, info=info.value)
+
+
+def _svx_local(fn, what, M, Ml, v, Py, layer0, B_share, nrhs, out, growth, *lead):
+    """cflx_*_svx_local: (X or None when the factors have an exactly zero pivot, dict(rcond, ferr, berr, [rpvgrw,] equed,
+    info)); growth: the LU's signature, with rpvgrw_out"""
+    bptr, ldb, xptr, ldx, out = _local_args(what, Ml, v, Py, layer0, B_share, nrhs, out, False)
+    fe, be = np.empty(nrhs), np.empty(nrhs)
+    rcond, rpvgrw, equed, info = ctypes.c_double(), ctypes.c_double(), ctypes.c_char(), ctypes.c_int()
+    mid = [ctypes.byref(rpvgrw)] if growth else []
+    check(fn(*lead, int(nrhs), bptr, ldb, xptr, ldx, ctypes.byref(rcond), fe.ctypes.data, be.ctypes.data, *mid,
+             ctypes.byref(equed), ctypes.byref(info)), what)
+    k = info.value
+    solved = not (0 < k <= M)
+    res = dict(rcond=rcond.value, ferr=fe if solved else None, berr=be if solved else None, equed=equed.value.decode(),
+               info=k)
+    if growth:
+        res["rpvgrw"] = rpvgrw.value
+    return (out if solved else None), res
+
+
+def _svxx_local(fn, what, M, Ml, v, Py, layer0, B_share, nrhs, out, cwise, *lead):
+    bptr, ldb, xptr, ldx, out = _local_args(what, Ml, v, Py, layer0, B_share, nrhs, out, False)
+    be, en, ec = np.empty(nrhs), np.zeros((nrhs, 3)), np.zeros((nrhs, 3))
+    rcond, rpvgrw, equed, info = ctypes.c_double(), ctypes.c_double(), ctypes.c_char(), ctypes.c_int()
+    check(fn(*lead, int(nrhs), bptr, ldb, xptr, ldx, ctypes.byref(rcond), ctypes.byref(rpvgrw), be.ctypes.data,
+             en.ctypes.data, ec.ctypes.data if cwise else None, ctypes.byref(equed), ctypes.byref(info)), what)
+    k = info.value
+    solved = not (0 < k <= M)
+    return (out if solved else None), dict(rcond=rcond.value, rpvgrw=rpvgrw.value, berr=be if solved else None,
+                                           err_norm=en if solved else None, err_comp=ec if solved and cwise else None,
+                                           equed=equed.value.decode(), info=k)
 
 
 def lu_solve_local(gv, B_share, nrhs, trans=False, out=None):
@@ -543,6 +611,40 @@ def lu_solve_local(gv, B_share, nrhs, trans=False, out=None):
     factors, the input and later solves are left as they are."""
     return _solve_local(lib().cflx_lu_solve_local, "lu_solve_local", gv.Ml, gv.v, gv.Py, gv.pk == 0, B_share, nrhs, out,
                         gv._h, 1 if trans else 0)
+
+
+def lu_refine_local(gv, B_share, X_share, nrhs, trans=False, ferr=True):
+    """lu_refine with B and X distributed like A (cflx_lu_refine_local, ScaLAPACK's pdgerfs): B_share and X_share are
+    this rank's shares in lu_solve_local's layout, NumPy arrays or torch CUDA tensors.  X_share holds the solution on
+    entry (read on layer 0, where it is required; may be None elsewhere) and the refined one on return, every layer
+    getting layer 0's bits; it must not overlap B_share.  Returns (X_share, ferr, berr) with ferr and berr per column,
+    identical on every rank.  The columns go in blocks of refine_block_cols(gv.v), each with the bits lu_refine gives
+    those columns alone.  COLLECTIVE over gv.lu_comm."""
+    return _refine_local(lib().cflx_lu_refine_local, "lu_refine_local", gv.Ml, gv.v, gv.Py, gv.pk == 0, B_share, X_share,
+                         nrhs, ferr, gv._h, 1 if trans else 0)
+
+
+def lu_refine_x_local(gv, B_share, X_share, nrhs, trans=False, cwise=True):
+    """lu_refine_x with B and X distributed like A (cflx_lu_refine_x_local): shares as lu_refine_local; returns
+    (X_share, dict(rcond, berr, err_norm, err_comp, info)) as lu_refine_x, info = M + j with j the first global column
+    whose bound was set to 1.  COLLECTIVE over gv.lu_comm."""
+    return _refine_x_local(lib().cflx_lu_refine_x_local, "lu_refine_x_local", gv.Ml, gv.v, gv.Py, gv.pk == 0, B_share,
+                           X_share, nrhs, cwise, gv._h, 1 if trans else 0)
+
+
+def lu_svx_local(gv, B_share, nrhs, trans=False, out=None):
+    """lu_svx with B and X distributed like A (cflx_lu_svx_local): B_share and out as lu_solve_local's (`out is B_share`
+    solves in place).  Returns (out, dict(rcond, ferr, berr, rpvgrw, equed, info)); out is None (and left as it was) when
+    U has an exactly zero pivot (info = k).  COLLECTIVE over gv.lu_comm; identical on every rank."""
+    return _svx_local(lib().cflx_lu_svx_local, "lu_svx_local", gv.M, gv.Ml, gv.v, gv.Py, gv.pk == 0, B_share, nrhs, out,
+                      True, gv._h, 1 if trans else 0)
+
+
+def lu_svxx_local(gv, B_share, nrhs, trans=False, cwise=True, out=None):
+    """lu_svxx with B and X distributed like A (cflx_lu_svxx_local): shares as lu_svx_local; returns (out, dict(rcond,
+    rpvgrw, berr, err_norm, err_comp, equed, info)) as lu_svxx.  COLLECTIVE over gv.lu_comm; identical on every rank."""
+    return _svxx_local(lib().cflx_lu_svxx_local, "lu_svxx_local", gv.M, gv.Ml, gv.v, gv.Py, gv.pk == 0, B_share, nrhs,
+                       out, cwise, gv._h, 1 if trans else 0)
 
 
 def lu_det(gv, unscaled=False):
@@ -688,6 +790,28 @@ class cholesky:
         read or written.  COLLECTIVE; every rank passes the same nrhs."""
         return _solve_local(lib().cflx_chol_solve_local, "cholesky.solve_local", self.Ml, self.v, self.PY, self.pz == 0,
                             B_share, nrhs, out, self._h)
+
+    def refine_local(self, B_share, X_share, nrhs, ferr=True):
+        """refine with B and X distributed like A (cflx_chol_refine_local): arguments and results as lu_refine_local's;
+        only the rows of real tiles are read and written.  COLLECTIVE."""
+        return _refine_local(lib().cflx_chol_refine_local, "cholesky.refine_local", self.Ml, self.v, self.PY,
+                             self.pz == 0, B_share, X_share, nrhs, ferr, self._h)
+
+    def refine_x_local(self, B_share, X_share, nrhs, cwise=True):
+        """refine_x with B and X distributed like A (cflx_chol_refine_x_local), as lu_refine_x_local.  COLLECTIVE."""
+        return _refine_x_local(lib().cflx_chol_refine_x_local, "cholesky.refine_x_local", self.Ml, self.v, self.PY,
+                               self.pz == 0, B_share, X_share, nrhs, cwise, self._h)
+
+    def svx_local(self, B_share, nrhs, out=None):
+        """svx with B and X distributed like A (cflx_chol_svx_local): (out, dict(rcond, ferr, berr, equed, info)), shares
+        as lu_svx_local's.  COLLECTIVE."""
+        return _svx_local(lib().cflx_chol_svx_local, "cholesky.svx_local", self.N, self.Ml, self.v, self.PY,
+                          self.pz == 0, B_share, nrhs, out, False, self._h)
+
+    def svxx_local(self, B_share, nrhs, cwise=True, out=None):
+        """svxx with B and X distributed like A (cflx_chol_svxx_local), as lu_svxx_local.  COLLECTIVE."""
+        return _svxx_local(lib().cflx_chol_svxx_local, "cholesky.svxx_local", self.N, self.Ml, self.v, self.PY,
+                           self.pz == 0, B_share, nrhs, out, cwise, self._h)
 
     def rcond(self):
         """LAPACK dpocon of the last parallelCholesky on the GPU grid: (rcond, anorm) with anorm = ||A||_1 of the padded

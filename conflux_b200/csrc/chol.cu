@@ -794,6 +794,20 @@ int chol_rcond(cflx_chol* ch, double* rcond_out, double* anorm_out) {
     return CFLX_OK;
 }
 
+// What refine_x, svx and svxx compute of the matrix, once per call whatever the right-hand sides: with rpvgrw set,
+// dla_porpvgrw of the stored lower triangles of the input and the factor; then dpocon.
+int chol_expert_pre(cflx_chol* ch, double* rpvgrw, double* rcond) {
+    if (rpvgrw) {
+        std::vector<double> h;
+        CFLX_TRY(growth_cols_grid(*ch, &ch->eq, true, ch->A11, ch->A0, ch->M, h));
+        *rpvgrw = rpvgrw_cols(h, ch->M, ch->M);
+    }
+    return chol_rcond(ch, rcond, nullptr);
+}
+
+// the scales s the factor carries (equed Y), else null
+const double* chol_scales(const cflx_chol* ch) { return ch->eq.fac.equed == 'Y' ? ch->eq.fac.r.p : nullptr; }
+
 // cflx_chol_equilibrate (dpoequ) and, with pow2, cflx_chol_equilibrate_b (dpoequb), as `who`
 int chol_equilibrate(const char* who, cflx_chol* ch, int apply, bool pow2, double* s_out, double* scond_out,
                      double* amax_out, char* equed_out, int* info_out) {
@@ -1229,12 +1243,12 @@ int cflx_chol_solve_local(cflx_chol* ch, int nrhs, const double* B_local, int ld
     SolveLocalArgs a{};
     CFLX_TRY(solve_local_args(__func__, *ch, nrhs, B_local, ldb, X_local, ldx, &a));
     CFLX_TRY(enter(ch, __func__, NEED_FACTORS | NEED_FP64));
-    auto solve = [ch](int w, const double* Bk, int ldn, const double** Xk) -> int {
+    auto solve = [ch](int, int w, double* Bk, double*, int ldn, const double** Xk) -> int {
         CFLX_TRY(chol_sweeps(ch, w, Bk, ldn, nullptr, 0));
         *Xk = ch->sv.X;
         return CFLX_OK;
     };
-    return solve_local_run(*ch, solve_local_rows(*ch, true), a, solve);
+    return solve_local_run(*ch, solve_local_rows(*ch, true), a, inverse_block_cols(ch->M, ch->v), false, solve);
 }
 
 // COLLECTIVE.  LAPACK dpotri (UPLO = 'L') on the grid (inverse.cu): the block solves with the identity on the sweeps of
@@ -1294,10 +1308,9 @@ int cflx_chol_refine_x(cflx_chol* ch, int nrhs, const double* B, int ldb, double
     REFUSE_IF(!info_out);
     CFLX_TRY(enter(ch, __func__, NEED_FACTORS | NEED_FP64));
     double rcond = 0.0;
-    CFLX_TRY(chol_rcond(ch, &rcond, nullptr));
+    CFLX_TRY(chol_expert_pre(ch, nullptr, &rcond));
     if (rcond_out) *rcond_out = rcond;
-    const EquilRecord& eq = ch->eq.fac;
-    return refine_x_run(&ch->sv.rf, chol_refine_op(ch), nrhs, B, ldb, X, ldx, eq.equed == 'Y' ? eq.r.p : nullptr, rcond,
+    return refine_x_run(&ch->sv.rf, chol_refine_op(ch), nrhs, B, ldb, X, ldx, chol_scales(ch), rcond,
                         err_bnds_comp_out != nullptr, berr_out, err_bnds_norm_out, err_bnds_comp_out, info_out);
 }
 
@@ -1323,14 +1336,13 @@ int cflx_chol_svx(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X, 
     REFUSE_IF(!rcond_out);
     REFUSE_IF(!info_out);
     CFLX_TRY(enter(ch, __func__, NEED_FACTORS | NEED_FP64));
-    const EquilRecord& eq = ch->eq.fac;
-    const double* s = eq.equed == 'Y' ? eq.r.p : nullptr;
-    if (equed_out) *equed_out = eq.equed;
+    const double* s = chol_scales(ch);
+    if (equed_out) *equed_out = ch->eq.fac.equed;
     double rcond = 0.0;
-    CFLX_TRY(chol_rcond(ch, &rcond, nullptr));
+    CFLX_TRY(chol_expert_pre(ch, nullptr, &rcond));
     *rcond_out = rcond;
-    return svx_run(&ch->eq, &ch->sv.rf, chol_refine_op(ch), nrhs, B, ldb, X, ldx, ferr_out, berr_out, s, s, eq.rowcnd,
-                   rcond, info_out);
+    return svx_run(&ch->eq, &ch->sv.rf, chol_refine_op(ch), nrhs, B, ldb, X, ldx, ferr_out, berr_out, s, s,
+                   ch->eq.fac.rowcnd, rcond, info_out);
 }
 
 // COLLECTIVE.  LAPACK dposvxx after a successful factorisation, with the scaling the factor carries: dla_porpvgrw of the
@@ -1345,17 +1357,122 @@ int cflx_chol_svxx(cflx_chol* ch, int nrhs, const double* B, int ldb, double* X,
     REFUSE_IF(!err_bnds_norm_out);
     REFUSE_IF(!info_out);
     CFLX_TRY(enter(ch, __func__, NEED_FACTORS | NEED_FP64));
-    const EquilRecord& eq = ch->eq.fac;
-    const double* s = eq.equed == 'Y' ? eq.r.p : nullptr;
-    if (equed_out) *equed_out = eq.equed;
-    std::vector<double> h;
-    CFLX_TRY(growth_cols_grid(*ch, &ch->eq, true, ch->A11, ch->A0, ch->M, h));
-    if (rpvgrw_out) *rpvgrw_out = rpvgrw_cols(h, ch->M, ch->M);
-    double rcond = 0.0;
-    CFLX_TRY(chol_rcond(ch, &rcond, nullptr));
+    const double* s = chol_scales(ch);
+    if (equed_out) *equed_out = ch->eq.fac.equed;
+    double rpvgrw = 1.0, rcond = 0.0;
+    CFLX_TRY(chol_expert_pre(ch, &rpvgrw, &rcond));
+    if (rpvgrw_out) *rpvgrw_out = rpvgrw;
     *rcond_out = rcond;
     return svxx_run(&ch->eq, &ch->sv.rf, chol_refine_op(ch), nrhs, B, ldb, X, ldx, s, s, s, rcond,
                     err_bnds_comp_out != nullptr, berr_out, err_bnds_norm_out, err_bnds_comp_out, info_out);
+}
+
+// ---------------------------------------------------------------- refinement and the expert drivers, B and X distributed
+// As the LU's (lu.cu): blocks of refine_block_cols columns through the replicated driver's core, the matrix-level parts
+// once before the loop; only the rows of real tiles are read and written.
+
+// COLLECTIVE.  cflx_chol_refine with B and X distributed like A.
+int cflx_chol_refine_local(cflx_chol* ch, int nrhs, const double* B_local, int ldb, double* X_local, int ldx,
+                           double* ferr_out, double* berr_out) {
+    REFUSE_IF(!ch);
+    SolveLocalArgs a{};
+    CFLX_TRY(refine_local_args(__func__, *ch, nrhs, B_local, ldb, X_local, ldx, true, &a));
+    CFLX_TRY(enter(ch, __func__, NEED_FACTORS | NEED_FP64));
+    const RefineOp op = chol_refine_op(ch);
+    auto run = [&](int c0, int w, double* Bk, double* Xk, int ldn, const double** out) -> int {
+        *out = Xk;
+        return refine_run(&ch->sv.rf, op, w, Bk, ldn, Xk, ldn, ferr_out ? ferr_out + c0 : nullptr,
+                          berr_out ? berr_out + c0 : nullptr);
+    };
+    return solve_local_run(*ch, solve_local_rows(*ch, true), a, refine_block_cols(ch->v), true, run);
+}
+
+// COLLECTIVE.  cflx_chol_refine_x with B and X distributed like A: dpocon once, then the blocks.
+int cflx_chol_refine_x_local(cflx_chol* ch, int nrhs, const double* B_local, int ldb, double* X_local, int ldx,
+                             double* rcond_out, double* berr_out, double* err_bnds_norm_out, double* err_bnds_comp_out,
+                             int* info_out) {
+    REFUSE_IF(!ch);
+    SolveLocalArgs a{};
+    CFLX_TRY(refine_local_args(__func__, *ch, nrhs, B_local, ldb, X_local, ldx, true, &a));
+    REFUSE_IF(!err_bnds_norm_out);
+    REFUSE_IF(!info_out);
+    CFLX_TRY(enter(ch, __func__, NEED_FACTORS | NEED_FP64));
+    double rcond = 0.0;
+    CFLX_TRY(chol_expert_pre(ch, nullptr, &rcond));
+    if (rcond_out) *rcond_out = rcond;
+    const RefineOp op = chol_refine_op(ch);
+    const double* d = chol_scales(ch);
+    int info = 0;
+    auto run = [&](int c0, int w, double* Bk, double* Xk, int ldn, const double** out) -> int {
+        *out = Xk;
+        int bi = 0;
+        CFLX_TRY(refine_x_run(&ch->sv.rf, op, w, Bk, ldn, Xk, ldn, d, rcond, err_bnds_comp_out != nullptr,
+                              berr_out ? berr_out + c0 : nullptr, err_bnds_norm_out + 3 * (size_t)c0,
+                              err_bnds_comp_out ? err_bnds_comp_out + 3 * (size_t)c0 : nullptr, &bi));
+        merge_block_info(&info, bi, c0);
+        return CFLX_OK;
+    };
+    CFLX_TRY(solve_local_run(*ch, solve_local_rows(*ch, true), a, refine_block_cols(ch->v), true, run));
+    *info_out = info;
+    return CFLX_OK;
+}
+
+// COLLECTIVE.  cflx_chol_svx with B and X distributed like A: dpocon once, then the blocks; X output only.
+int cflx_chol_svx_local(cflx_chol* ch, int nrhs, const double* B_local, int ldb, double* X_local, int ldx,
+                        double* rcond_out, double* ferr_out, double* berr_out, char* equed_out, int* info_out) {
+    REFUSE_IF(!ch);
+    SolveLocalArgs a{};
+    CFLX_TRY(refine_local_args(__func__, *ch, nrhs, B_local, ldb, X_local, ldx, false, &a));
+    REFUSE_IF(!rcond_out);
+    REFUSE_IF(!info_out);
+    CFLX_TRY(enter(ch, __func__, NEED_FACTORS | NEED_FP64));
+    const double* s = chol_scales(ch);
+    if (equed_out) *equed_out = ch->eq.fac.equed;
+    double rcond = 0.0;
+    CFLX_TRY(chol_expert_pre(ch, nullptr, &rcond));
+    *rcond_out = rcond;
+    *info_out = 0;
+    const RefineOp op = chol_refine_op(ch);
+    auto run = [&](int c0, int w, double* Bk, double*, int ldn, const double** out) -> int {
+        *out = Bk;  // svx_tail reads B before it writes X
+        return svx_run(&ch->eq, &ch->sv.rf, op, w, Bk, ldn, Bk, ldn, ferr_out ? ferr_out + c0 : nullptr,
+                       berr_out ? berr_out + c0 : nullptr, s, s, ch->eq.fac.rowcnd, rcond, info_out);
+    };
+    return solve_local_run(*ch, solve_local_rows(*ch, true), a, refine_block_cols(ch->v), false, run);
+}
+
+// COLLECTIVE.  cflx_chol_svxx with B and X distributed like A: dla_porpvgrw and dpocon once, then the blocks; X output
+// only.
+int cflx_chol_svxx_local(cflx_chol* ch, int nrhs, const double* B_local, int ldb, double* X_local, int ldx,
+                         double* rcond_out, double* rpvgrw_out, double* berr_out, double* err_bnds_norm_out,
+                         double* err_bnds_comp_out, char* equed_out, int* info_out) {
+    REFUSE_IF(!ch);
+    SolveLocalArgs a{};
+    CFLX_TRY(refine_local_args(__func__, *ch, nrhs, B_local, ldb, X_local, ldx, false, &a));
+    REFUSE_IF(!rcond_out);
+    REFUSE_IF(!err_bnds_norm_out);
+    REFUSE_IF(!info_out);
+    CFLX_TRY(enter(ch, __func__, NEED_FACTORS | NEED_FP64));
+    const double* s = chol_scales(ch);
+    if (equed_out) *equed_out = ch->eq.fac.equed;
+    double rpvgrw = 1.0, rcond = 0.0;
+    CFLX_TRY(chol_expert_pre(ch, &rpvgrw, &rcond));
+    if (rpvgrw_out) *rpvgrw_out = rpvgrw;
+    *rcond_out = rcond;
+    const RefineOp op = chol_refine_op(ch);
+    int info = 0;
+    auto run = [&](int c0, int w, double* Bk, double*, int ldn, const double** out) -> int {
+        *out = Bk;
+        int bi = 0;
+        CFLX_TRY(svxx_run(&ch->eq, &ch->sv.rf, op, w, Bk, ldn, Bk, ldn, s, s, s, rcond, err_bnds_comp_out != nullptr,
+                          berr_out ? berr_out + c0 : nullptr, err_bnds_norm_out + 3 * (size_t)c0,
+                          err_bnds_comp_out ? err_bnds_comp_out + 3 * (size_t)c0 : nullptr, &bi));
+        merge_block_info(&info, bi, c0);
+        return CFLX_OK;
+    };
+    CFLX_TRY(solve_local_run(*ch, solve_local_rows(*ch, true), a, refine_block_cols(ch->v), false, run));
+    *info_out = info;
+    return CFLX_OK;
 }
 
 // COLLECTIVE.  LAPACK dsposv on the grid: the input factored with the TF32 trailing update (prec 1: one term, 3: three),

@@ -719,6 +719,30 @@ RefineOp lu_refine_op(cflx_lu* lu, bool t) {
     return RefineOp{*lu, lu->A0, t ? ResidMode::TN : ResidMode::NN, false, solve};
 }
 
+// What refine_x, svx and svxx compute of the matrix, once per call whatever the right-hand sides: the first exactly zero
+// U(k,k) over the world (with rpvgrw set, through the pivot growth: dla_gerpvgrw when per_column, else dgesvx's), then,
+// when there is none, dgecon in the infinity-norm (inf) or the 1-norm; rcond is 0 when there is one.
+int lu_expert_pre(cflx_lu* lu, bool inf, double* rpvgrw, bool per_column, double* rcond, int* info) {
+    if (!lu->sv.ready) CFLX_TRY(lu_solve_prepare(lu));
+    *rcond = 0.0;
+    if (rpvgrw) CFLX_TRY(pivot_growth_grid(*lu, &lu->eq, lu->Cbuf, lu->A0, per_column, rpvgrw, info));
+    else CFLX_TRY(zero_pivot_grid(*lu, &lu->eq, lu->Cbuf, info));
+    return *info > 0 ? CFLX_OK : lu_rcond(lu, inf, rcond, nullptr);
+}
+
+// The scales of op(A) X = B the factors carry: pre for the rows of B (r for trans 0, c for trans 1; null when the
+// factors carry none), post for the rows of X and the error bounds' d (the other one), cnd the ratio that divides ferr.
+struct LuScales {
+    const double *pre, *post;
+    double cnd;
+};
+LuScales lu_scales(const cflx_lu* lu, bool t) {
+    const EquilRecord& eq = lu->eq.fac;
+    const double* r = eq.equed == 'R' || eq.equed == 'B' ? eq.r.p : nullptr;
+    const double* c = eq.equed == 'C' || eq.equed == 'B' ? eq.c.p : nullptr;
+    return LuScales{t ? c : r, t ? r : c, t ? eq.rowcnd : eq.colcnd};
+}
+
 // cflx_lu_equilibrate (dgeequ) and, with pow2, cflx_lu_equilibrate_b (dgeequb), as `who`
 int lu_equilibrate(const char* who, cflx_lu* lu, int apply, bool pow2, double* r_out, double* c_out, double* rowcnd_out,
                    double* colcnd_out, double* amax_out, char* equed_out, int* info_out) {
@@ -1413,12 +1437,12 @@ int cflx_lu_solve_local(cflx_lu* lu, int trans, int nrhs, const double* B_local,
     SolveLocalArgs a{};
     CFLX_TRY(solve_local_args(__func__, *lu, nrhs, B_local, ldb, X_local, ldx, &a));
     CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_FP64));
-    auto solve = [lu, trans](int w, const double* Bk, int ldn, const double** Xk) -> int {
+    auto solve = [lu, trans](int, int w, double* Bk, double*, int ldn, const double** Xk) -> int {
         CFLX_TRY(lu_sweeps(lu, trans != 0, false, w, Bk, ldn, nullptr, 0));
         *Xk = trans ? lu->sv.Xg : lu->sv.X;  // the transposed solve's P^T lands in Xg
         return CFLX_OK;
     };
-    return solve_local_run(*lu, solve_local_rows(*lu, false), a, solve);
+    return solve_local_run(*lu, solve_local_rows(*lu, false), a, inverse_block_cols(lu->M, lu->v), false, solve);
 }
 
 // LAPACK dgecon (NORM = '1') on the grid (lu_rcond).
@@ -1500,23 +1524,14 @@ int cflx_lu_refine_x(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb,
     REFUSE_IF(!info_out);
     CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_FP64 | NEED_OWN_INPUT));
     const bool t = trans != 0;
-    if (!lu->sv.ready) CFLX_TRY(lu_solve_prepare(lu));
-    int info = 0;
-    CFLX_TRY(zero_pivot_grid(*lu, &lu->eq, lu->Cbuf, &info));
-    *info_out = info;
-    if (info > 0) {  // exactly singular U: X is left as it was
-        if (rcond_out) *rcond_out = 0.0;
-        return CFLX_OK;
-    }
     double rcond = 0.0;
-    CFLX_TRY(lu_rcond(lu, !t, &rcond, nullptr));
+    int info = 0;
+    CFLX_TRY(lu_expert_pre(lu, !t, nullptr, false, &rcond, &info));
+    *info_out = info;
     if (rcond_out) *rcond_out = rcond;
-    const EquilRecord& eq = lu->eq.fac;
-    const double* d = !t && (eq.equed == 'C' || eq.equed == 'B') ? eq.c.p
-                      : t && (eq.equed == 'R' || eq.equed == 'B') ? eq.r.p
-                                                                   : nullptr;
-    return refine_x_run(&lu->sv.rf, lu_refine_op(lu, t), nrhs, B, ldb, X, ldx, d, rcond, err_bnds_comp_out != nullptr,
-                        berr_out, err_bnds_norm_out, err_bnds_comp_out, info_out);
+    if (info > 0) return CFLX_OK;  // exactly singular U: X is left as it was
+    return refine_x_run(&lu->sv.rf, lu_refine_op(lu, t), nrhs, B, ldb, X, ldx, lu_scales(lu, t).post, rcond,
+                        err_bnds_comp_out != nullptr, berr_out, err_bnds_norm_out, err_bnds_comp_out, info_out);
 }
 
 // COLLECTIVE.  LAPACK dgeequ (+ dlaqge when apply) on the input A0 (equil.cu).  The input changes, so the factorisation
@@ -1545,27 +1560,19 @@ int cflx_lu_svxx(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, dou
     REFUSE_IF(!info_out);
     CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_FP64 | NEED_OWN_INPUT));
     const bool t = trans != 0;
-    const EquilRecord& eq = lu->eq.fac;
-    const bool rowequ = eq.equed == 'R' || eq.equed == 'B', colequ = eq.equed == 'C' || eq.equed == 'B';
-    if (equed_out) *equed_out = eq.equed;
-    if (!lu->sv.ready) CFLX_TRY(lu_solve_prepare(lu));
-    double rpvgrw = 1.0;
+    if (equed_out) *equed_out = lu->eq.fac.equed;
+    double rpvgrw = 1.0, rcond = 0.0;
     int info = 0;
-    CFLX_TRY(pivot_growth_grid(*lu, &lu->eq, lu->Cbuf, lu->A0, true, &rpvgrw, &info));
+    // dgecon as cflx_lu_refine_x: the infinity-norm for trans 0, the 1-norm for trans 1
+    CFLX_TRY(lu_expert_pre(lu, !t, &rpvgrw, true, &rcond, &info));
     if (rpvgrw_out) *rpvgrw_out = rpvgrw;
     *info_out = info;
-    if (info > 0) {  // exactly singular U: X is left as it was
-        *rcond_out = 0.0;
-        return CFLX_OK;
-    }
-    // dgecon as cflx_lu_refine_x: the infinity-norm for trans 0, the 1-norm for trans 1
-    double rcond = 0.0;
-    CFLX_TRY(lu_rcond(lu, !t, &rcond, nullptr));
     *rcond_out = rcond;
+    if (info > 0) return CFLX_OK;  // exactly singular U: X is left as it was
     // B is scaled by the scales of the rows of op(A), X (and the bounds' d) by those of its columns
-    const double *r = rowequ ? eq.r.p : nullptr, *c = colequ ? eq.c.p : nullptr;
-    return svxx_run(&lu->eq, &lu->sv.rf, lu_refine_op(lu, t), nrhs, B, ldb, X, ldx, t ? c : r, t ? r : c, t ? r : c,
-                    rcond, err_bnds_comp_out != nullptr, berr_out, err_bnds_norm_out, err_bnds_comp_out, info_out);
+    const LuScales sc = lu_scales(lu, t);
+    return svxx_run(&lu->eq, &lu->sv.rf, lu_refine_op(lu, t), nrhs, B, ldb, X, ldx, sc.pre, sc.post, sc.post, rcond,
+                    err_bnds_comp_out != nullptr, berr_out, err_bnds_norm_out, err_bnds_comp_out, info_out);
 }
 
 // COLLECTIVE.  LAPACK dgesvx after the factorisation, with the scaling the factors carry: B scaled, the reciprocal pivot
@@ -1579,27 +1586,145 @@ int cflx_lu_svx(cflx_lu* lu, int trans, int nrhs, const double* B, int ldb, doub
     REFUSE_IF(!info_out);
     CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_FP64 | NEED_OWN_INPUT));
     const bool t = trans != 0;
-    const EquilRecord& eq = lu->eq.fac;
-    const bool rowequ = eq.equed == 'R' || eq.equed == 'B', colequ = eq.equed == 'C' || eq.equed == 'B';
-    if (equed_out) *equed_out = eq.equed;
-    if (!lu->sv.ready) CFLX_TRY(lu_solve_prepare(lu));
-    double rpvgrw = 1.0;
+    if (equed_out) *equed_out = lu->eq.fac.equed;
+    double rpvgrw = 1.0, rcond = 0.0;
     int info = 0;
-    CFLX_TRY(pivot_growth_grid(*lu, &lu->eq, lu->Cbuf, lu->A0, false, &rpvgrw, &info));
+    // dgecon with NORM = '1' (trans 0, as cflx_lu_rcond) or 'I' (trans 1)
+    CFLX_TRY(lu_expert_pre(lu, t, &rpvgrw, false, &rcond, &info));
     if (rpvgrw_out) *rpvgrw_out = rpvgrw;
     *info_out = info;
-    if (info > 0) {  // exactly singular U: no solution
-        *rcond_out = 0.0;
-        return CFLX_OK;
-    }
-    // dgecon with NORM = '1' (trans 0, as cflx_lu_rcond) or 'I' (trans 1)
-    double rcond = 0.0;
-    CFLX_TRY(lu_rcond(lu, t, &rcond, nullptr));
     *rcond_out = rcond;
+    if (info > 0) return CFLX_OK;  // exactly singular U: no solution
     // op(A) X = B: B is scaled by the scales of the rows of op(A), X by those of its columns
-    const double *r = rowequ ? eq.r.p : nullptr, *c = colequ ? eq.c.p : nullptr;
-    return svx_run(&lu->eq, &lu->sv.rf, lu_refine_op(lu, t), nrhs, B, ldb, X, ldx, ferr_out, berr_out, t ? c : r,
-                   t ? r : c, t ? eq.rowcnd : eq.colcnd, rcond, info_out);
+    const LuScales sc = lu_scales(lu, t);
+    return svx_run(&lu->eq, &lu->sv.rf, lu_refine_op(lu, t), nrhs, B, ldb, X, ldx, ferr_out, berr_out, sc.pre, sc.post,
+                   sc.cnd, rcond, info_out);
+}
+
+// ---------------------------------------------------------------- refinement and the expert drivers, B and X distributed
+// Each block of refine_block_cols columns is assembled as cflx_lu_solve_local assembles it (with X for refine and
+// refine_x), run through the replicated driver's core on device buffers, and scattered; the matrix-level parts run once
+// before the loop.  So each block's bits are those of the replicated driver called on those columns alone.
+
+// COLLECTIVE.  cflx_lu_refine with B and X distributed like A.
+int cflx_lu_refine_local(cflx_lu* lu, int trans, int nrhs, const double* B_local, int ldb, double* X_local, int ldx,
+                         double* ferr_out, double* berr_out) {
+    REFUSE_IF(!lu);
+    REFUSE_IF(trans != 0 && trans != 1);
+    SolveLocalArgs a{};
+    CFLX_TRY(refine_local_args(__func__, *lu, nrhs, B_local, ldb, X_local, ldx, true, &a));
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_FP64 | NEED_OWN_INPUT));
+    const RefineOp op = lu_refine_op(lu, trans != 0);
+    auto run = [&](int c0, int w, double* Bk, double* Xk, int ldn, const double** out) -> int {
+        *out = Xk;
+        return refine_run(&lu->sv.rf, op, w, Bk, ldn, Xk, ldn, ferr_out ? ferr_out + c0 : nullptr,
+                          berr_out ? berr_out + c0 : nullptr);
+    };
+    return solve_local_run(*lu, solve_local_rows(*lu, false), a, refine_block_cols(lu->v), true, run);
+}
+
+// COLLECTIVE.  cflx_lu_refine_x with B and X distributed like A: the zero-pivot check and dgecon once, then the blocks.
+int cflx_lu_refine_x_local(cflx_lu* lu, int trans, int nrhs, const double* B_local, int ldb, double* X_local, int ldx,
+                           double* rcond_out, double* berr_out, double* err_bnds_norm_out, double* err_bnds_comp_out,
+                           int* info_out) {
+    REFUSE_IF(!lu);
+    REFUSE_IF(trans != 0 && trans != 1);
+    SolveLocalArgs a{};
+    CFLX_TRY(refine_local_args(__func__, *lu, nrhs, B_local, ldb, X_local, ldx, true, &a));
+    REFUSE_IF(!err_bnds_norm_out);
+    REFUSE_IF(!info_out);
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_FP64 | NEED_OWN_INPUT));
+    const bool t = trans != 0;
+    double rcond = 0.0;
+    int info = 0;
+    CFLX_TRY(lu_expert_pre(lu, !t, nullptr, false, &rcond, &info));
+    *info_out = info;
+    if (rcond_out) *rcond_out = rcond;
+    if (info > 0) return CFLX_OK;  // exactly singular U: X is left as it was
+    const RefineOp op = lu_refine_op(lu, t);
+    const double* d = lu_scales(lu, t).post;
+    auto run = [&](int c0, int w, double* Bk, double* Xk, int ldn, const double** out) -> int {
+        *out = Xk;
+        int bi = 0;
+        CFLX_TRY(refine_x_run(&lu->sv.rf, op, w, Bk, ldn, Xk, ldn, d, rcond, err_bnds_comp_out != nullptr,
+                              berr_out ? berr_out + c0 : nullptr, err_bnds_norm_out + 3 * (size_t)c0,
+                              err_bnds_comp_out ? err_bnds_comp_out + 3 * (size_t)c0 : nullptr, &bi));
+        merge_block_info(&info, bi, c0);
+        return CFLX_OK;
+    };
+    CFLX_TRY(solve_local_run(*lu, solve_local_rows(*lu, false), a, refine_block_cols(lu->v), true, run));
+    *info_out = info;
+    return CFLX_OK;
+}
+
+// COLLECTIVE.  cflx_lu_svx with B and X distributed like A: the pivot growth, the zero-pivot check and dgecon once,
+// then the blocks; X output only.
+int cflx_lu_svx_local(cflx_lu* lu, int trans, int nrhs, const double* B_local, int ldb, double* X_local, int ldx,
+                      double* rcond_out, double* ferr_out, double* berr_out, double* rpvgrw_out, char* equed_out,
+                      int* info_out) {
+    REFUSE_IF(!lu);
+    REFUSE_IF(trans != 0 && trans != 1);
+    SolveLocalArgs a{};
+    CFLX_TRY(refine_local_args(__func__, *lu, nrhs, B_local, ldb, X_local, ldx, false, &a));
+    REFUSE_IF(!rcond_out);
+    REFUSE_IF(!info_out);
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_FP64 | NEED_OWN_INPUT));
+    const bool t = trans != 0;
+    if (equed_out) *equed_out = lu->eq.fac.equed;
+    double rpvgrw = 1.0, rcond = 0.0;
+    int info = 0;
+    CFLX_TRY(lu_expert_pre(lu, t, &rpvgrw, false, &rcond, &info));
+    if (rpvgrw_out) *rpvgrw_out = rpvgrw;
+    *info_out = info;
+    *rcond_out = rcond;
+    if (info > 0) return CFLX_OK;  // exactly singular U: X is not written
+    const RefineOp op = lu_refine_op(lu, t);
+    const LuScales sc = lu_scales(lu, t);
+    auto run = [&](int c0, int w, double* Bk, double*, int ldn, const double** out) -> int {
+        *out = Bk;  // svx_tail reads B before it writes X
+        return svx_run(&lu->eq, &lu->sv.rf, op, w, Bk, ldn, Bk, ldn, ferr_out ? ferr_out + c0 : nullptr,
+                       berr_out ? berr_out + c0 : nullptr, sc.pre, sc.post, sc.cnd, rcond, info_out);
+    };
+    return solve_local_run(*lu, solve_local_rows(*lu, false), a, refine_block_cols(lu->v), false, run);
+}
+
+// COLLECTIVE.  cflx_lu_svxx with B and X distributed like A: dla_gerpvgrw, the zero-pivot check and dgecon once, then
+// the blocks; X output only.
+int cflx_lu_svxx_local(cflx_lu* lu, int trans, int nrhs, const double* B_local, int ldb, double* X_local, int ldx,
+                       double* rcond_out, double* rpvgrw_out, double* berr_out, double* err_bnds_norm_out,
+                       double* err_bnds_comp_out, char* equed_out, int* info_out) {
+    REFUSE_IF(!lu);
+    REFUSE_IF(trans != 0 && trans != 1);
+    SolveLocalArgs a{};
+    CFLX_TRY(refine_local_args(__func__, *lu, nrhs, B_local, ldb, X_local, ldx, false, &a));
+    REFUSE_IF(!rcond_out);
+    REFUSE_IF(!err_bnds_norm_out);
+    REFUSE_IF(!info_out);
+    CFLX_TRY(enter(lu, __func__, NEED_FACTORS | NEED_FP64 | NEED_OWN_INPUT));
+    const bool t = trans != 0;
+    if (equed_out) *equed_out = lu->eq.fac.equed;
+    double rpvgrw = 1.0, rcond = 0.0;
+    int info = 0;
+    CFLX_TRY(lu_expert_pre(lu, !t, &rpvgrw, true, &rcond, &info));
+    if (rpvgrw_out) *rpvgrw_out = rpvgrw;
+    *info_out = info;
+    *rcond_out = rcond;
+    if (info > 0) return CFLX_OK;  // exactly singular U: X is not written
+    const RefineOp op = lu_refine_op(lu, t);
+    const LuScales sc = lu_scales(lu, t);
+    auto run = [&](int c0, int w, double* Bk, double*, int ldn, const double** out) -> int {
+        *out = Bk;
+        int bi = 0;
+        CFLX_TRY(svxx_run(&lu->eq, &lu->sv.rf, op, w, Bk, ldn, Bk, ldn, sc.pre, sc.post, sc.post, rcond,
+                          err_bnds_comp_out != nullptr, berr_out ? berr_out + c0 : nullptr,
+                          err_bnds_norm_out + 3 * (size_t)c0, err_bnds_comp_out ? err_bnds_comp_out + 3 * (size_t)c0 : nullptr,
+                          &bi));
+        merge_block_info(&info, bi, c0);
+        return CFLX_OK;
+    };
+    CFLX_TRY(solve_local_run(*lu, solve_local_rows(*lu, false), a, refine_block_cols(lu->v), false, run));
+    *info_out = info;
+    return CFLX_OK;
 }
 
 // COLLECTIVE.  LAPACK dsgesv on the grid: the input factored with the TF32 trailing update (prec 1: one term, 3: three),

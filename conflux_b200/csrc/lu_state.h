@@ -671,12 +671,28 @@ int rhs_args(const char* who, int nrhs, const double* B, int ldb, const double* 
 // collective.
 int solve_local_args(const char* who, const Grid& g, int nrhs, const double* B, int ldb, const double* X, int ldx,
                      SolveLocalArgs* a);
-// solve(w, Bk, ldn, &Xk): the sweeps on the assembled block Bk (M x ldn device, w columns, the same on every rank), the
-// solution left in *Xk (M x ldn device, the same on every rank)
-using BlockSolve = std::function<int(int, const double*, int, const double**)>;
-// COLLECTIVE.  The block loop of cflx_lu_solve_local / cflx_chol_solve_local: per block of inverse_block_cols columns,
-// pack, the world all-reduce that assembles the block, solve, and the scatter into X (may be null); synchronises.
-int solve_local_run(const Grid& g, int rows, const SolveLocalArgs& a, const BlockSolve& solve);
+// run(c0, w, Bk, Xk, ldn, &out): block [c0, c0 + w) of the columns, assembled in Bk (M x ldn device, the same on every
+// rank) and, when the loop assembles X, X's block in Xk (else null); the result to scatter left in *out (M x ldn device,
+// the same on every rank)
+using BlockRun = std::function<int(int, int, double*, double*, int, const double**)>;
+// COLLECTIVE.  The block loop of the distributed solves and drivers: per block of nc columns, pack B (and with x_in, X
+// on layer 0), the world all-reduce that assembles the block, run, and the scatter into X (may be null); synchronises.
+int solve_local_run(const Grid& g, int rows, const SolveLocalArgs& a, int nc, bool x_in, const BlockRun& run);
+// The block width of the distributed refinement and expert drivers: the whole number of tiles nearest CFLX_REFINE_NC
+// columns (at least one tile).  Their device workspace grows with this width, not with nrhs (DESIGN.md section 7o).
+#ifndef CFLX_REFINE_NC
+#define CFLX_REFINE_NC 256
+#endif
+int refine_block_cols(int v);
+// solve_local_args for cflx_*_refine*_local (x_in: X is the solution on entry, required on layer 0 and not overlapping
+// B there) and cflx_*_svx*_local (X output only, may be B itself)
+int refine_local_args(const char* who, const Grid& g, int nrhs, const double* B, int ldb, const double* X, int ldx,
+                      bool x_in, SolveLocalArgs* a);
+// The info of refine_x and svxx over the blocks: the first block's M + j (j counted in the block) moved to the global
+// column, j + c0
+inline void merge_block_info(int* info, int block_info, int c0) {
+    if (*info == 0 && block_info > 0) *info = block_info + c0;
+}
 
 // ---------------------------------------------------------------- the determinant (det.cu)
 constexpr int DET_THREADS = 256;  // the one CTA of the product; part of its order (oracle/det_ref.py)

@@ -15,6 +15,11 @@
 // Block j is packed before it is scattered, and the blocks' columns are disjoint, so X may be B itself.  Host shares go
 // through one temporary device share: the rows and columns the call reads and writes are a prefix of each (local rows
 // before the first tile >= Kappa, local columns before the first global column >= nrhs).
+//
+// The distributed refinement and expert drivers (cflx_lu_refine_local ... cflx_chol_svxx_local) run the same loop with
+// blocks of refine_block_cols(v) columns: for refine and refine_x, X's block is packed and assembled with B's (one
+// all-reduce over both), and the block goes through the replicated driver's core (refine_run, refine_x_run, svx_run,
+// svxx_run) on device buffers before it is scattered.
 #include <algorithm>
 
 #include "lu_state.h"
@@ -127,16 +132,38 @@ int solve_local_args(const char* who, const Grid& g, int nrhs, const double* B, 
     return CFLX_OK;
 }
 
-int solve_local_run(const Grid& g, int rows, const SolveLocalArgs& a, const BlockSolve& solve) {
+int refine_block_cols(int v) { return std::max(1, (CFLX_REFINE_NC + v / 2) / v) * v; }
+
+int refine_local_args(const char* who, const Grid& g, int nrhs, const double* B, int ldb, const double* X, int ldx,
+                      bool x_in, SolveLocalArgs* a) {
+    CFLX_TRY(solve_local_args(who, g, nrhs, B, ldb, X, ldx, a));
+    if (!x_in) return CFLX_OK;
+    REFUSE_FOR(who, g.pk == 0 && !X);
+    if (a->B && g.Ml > 0) {  // the bytes each share spans, padding included
+        const int ncl = rhs_local_cols(nrhs, g.v, g.Py);
+        const char *b0 = reinterpret_cast<const char*>(a->B), *x0 = reinterpret_cast<const char*>(X);
+        const char *b1 = b0 + sizeof(double) * ((int64_t)(g.Ml - 1) * ldb + ncl);
+        const char *x1 = x0 + sizeof(double) * ((int64_t)(g.Ml - 1) * ldx + ncl);
+        if (x0 < b1 && b0 < x1) {
+            set_last_error("%s: refused, X_local overlaps B_local (X_local is the solution on entry)", who);
+            return CFLX_ERR_ARG;
+        }
+    }
+    return CFLX_OK;
+}
+
+int solve_local_run(const Grid& g, int rows, const SolveLocalArgs& a, int nc, bool x_in, const BlockRun& run) {
     cudaStream_t s = g.comm->stream;
     const int ncl = rhs_local_cols(a.nrhs, g.v, g.Py), cols = valid_cols(a.nrhs, g.v, g.Py, g.pj);
-    const bool copy = rows > 0 && cols > 0;
+    const bool copy = rows > 0 && cols > 0, b_host = a.B && !a.b_dev, x_host = a.X && !a.x_dev;
+    const size_t share = sizeof(double) * std::max<size_t>(1, (size_t)rows * ncl);
     // a host share goes through one temporary device share (ld ncl), which holds B and then receives X when both are host
-    DevBuf<> tmp;
-    if ((a.B && !a.b_dev) || (a.X && !a.x_dev)) CFLX_TRY(tmp.alloc(sizeof(double) * std::max<size_t>(1, (size_t)rows * ncl)));
+    // and X is output only; an X read on entry has a temporary of its own
+    DevBuf<> tmp, tmpx;
+    if (b_host || (x_host && !x_in)) CFLX_TRY(tmp.alloc(share));
     const double* src = a.B;
     int64_t lds = a.ldb;
-    if (a.B && !a.b_dev) {
+    if (b_host) {
         if (copy)
             CFLX_CUDA(cudaMemcpy2DAsync(tmp.p, sizeof(double) * ncl, a.B, sizeof(double) * a.ldb, sizeof(double) * cols,
                                         rows, cudaMemcpyHostToDevice, s));
@@ -145,24 +172,34 @@ int solve_local_run(const Grid& g, int rows, const SolveLocalArgs& a, const Bloc
     }
     double* dst = a.X;
     int64_t ldd = a.ldx;
-    if (a.X && !a.x_dev) {
-        dst = tmp.as<double>();
+    if (x_host) {
+        if (x_in) {
+            CFLX_TRY(tmpx.alloc(share));
+            if (copy && g.pk == 0)  // read on layer 0 only
+                CFLX_CUDA(cudaMemcpy2DAsync(tmpx.p, sizeof(double) * ncl, a.X, sizeof(double) * a.ldx,
+                                            sizeof(double) * cols, rows, cudaMemcpyHostToDevice, s));
+        }
+        dst = x_in ? tmpx.as<double>() : tmp.as<double>();
         ldd = ncl;
     }
-    const int nc = inverse_block_cols(g.M, g.v);
-    DevBuf<> Bk;
-    CFLX_TRY(Bk.alloc(sizeof(double) * g.M * round_up(std::min(nc, a.nrhs), 8)));
+    // the block's B, then (x_in) its X: one buffer, assembled by one all-reduce
+    const size_t mat = (size_t)g.M * round_up(std::min(nc, a.nrhs), 8);
+    DevBuf<> buf;
+    CFLX_TRY(buf.alloc(sizeof(double) * mat * (x_in ? 2 : 1)));
     for (int c0 = 0; c0 < a.nrhs; c0 += nc) {
         const int w = std::min(nc, a.nrhs - c0), ldn = (int)round_up(w, 8);
-        CFLX_TRY(launch_solve_local_pack(src, lds, g, rows, c0, w, Bk.as<double>(), ldn, s));
+        double* Bk = buf.as<double>();
+        double* Xk = x_in ? Bk + (size_t)g.M * ldn : nullptr;
+        CFLX_TRY(launch_solve_local_pack(src, lds, g, rows, c0, w, Bk, ldn, s));
+        if (x_in) CFLX_TRY(launch_solve_local_pack(g.pk == 0 ? dst : nullptr, ldd, g, rows, c0, w, Xk, ldn, s));
         if (g.P > 1)
-            CFLX_NCCL(ncclAllReduce(Bk.p, Bk.p, (size_t)g.M * ldn, ncclUint64, ncclSum, g.comm->world, s));
-        const double* Xk = nullptr;
-        CFLX_TRY(solve(w, Bk.as<double>(), ldn, &Xk));
-        if (dst) CFLX_TRY(launch_solve_local_scatter(Xk, ldn, g, rows, c0, w, dst, ldd, s));
+            CFLX_NCCL(ncclAllReduce(Bk, Bk, (size_t)g.M * ldn * (x_in ? 2 : 1), ncclUint64, ncclSum, g.comm->world, s));
+        const double* out = nullptr;
+        CFLX_TRY(run(c0, w, Bk, Xk, ldn, &out));
+        if (dst) CFLX_TRY(launch_solve_local_scatter(out, ldn, g, rows, c0, w, dst, ldd, s));
     }
-    if (a.X && !a.x_dev && copy)
-        CFLX_CUDA(cudaMemcpy2DAsync(a.X, sizeof(double) * a.ldx, tmp.p, sizeof(double) * ncl, sizeof(double) * cols, rows,
+    if (x_host && copy)
+        CFLX_CUDA(cudaMemcpy2DAsync(a.X, sizeof(double) * a.ldx, dst, sizeof(double) * ncl, sizeof(double) * cols, rows,
                                     cudaMemcpyDeviceToHost, s));
     if (cudaStreamSynchronize(s) != cudaSuccess) {
         set_last_error("distributed solve: %s", cudaGetErrorString(cudaGetLastError()));
@@ -179,5 +216,12 @@ extern "C" int cflx_rhs_local_cols(int nrhs, int v, int Py, int* cols_out) {
     REFUSE_IF(Py < 1);
     REFUSE_IF(!cols_out);
     *cols_out = cflx::rhs_local_cols(nrhs, v, Py);
+    return CFLX_OK;
+}
+
+extern "C" int cflx_refine_block_cols(int v, int* cols_out) {
+    REFUSE_IF(v < 1);
+    REFUSE_IF(!cols_out);
+    *cols_out = cflx::refine_block_cols(v);
     return CFLX_OK;
 }

@@ -209,6 +209,46 @@ inline int choleskySvxx(int nrhs, const double* B, int ldb, double* X, int ldx, 
                        "choleskySvxx");
     return info;
 }
+// choleskyRefine, choleskyRefineX, choleskySvx and choleskySvxx with B and X distributed like A
+// (cflx_chol_refine_local ... cflx_chol_svxx_local, collective): arguments and results as conflux::LU_refine_local ...
+// LU_svxx_local without transposed, in choleskySolveLocal's layout.
+inline void choleskyRefineLocal(int nrhs, const double* B_local, int ldb, double* X_local, int ldx,
+                                double* ferr = nullptr, double* berr = nullptr) {
+    auto& s = chol_detail::state();
+    if (!s.plan) throw CholeskyException("choleskyRefineLocal() before initialize()");
+    chol_detail::check(cflx_chol_refine_local(s.plan, nrhs, B_local, ldb, X_local, ldx, ferr, berr),
+                       "choleskyRefineLocal");
+}
+inline int choleskyRefineXLocal(int nrhs, const double* B_local, int ldb, double* X_local, int ldx, double* err_norm,
+                                double* err_comp = nullptr, double* rcond = nullptr, double* berr = nullptr) {
+    auto& s = chol_detail::state();
+    if (!s.plan) throw CholeskyException("choleskyRefineXLocal() before initialize()");
+    int info = 0;
+    chol_detail::check(cflx_chol_refine_x_local(s.plan, nrhs, B_local, ldb, X_local, ldx, rcond, berr, err_norm,
+                                                err_comp, &info),
+                       "choleskyRefineXLocal");
+    return info;
+}
+inline int choleskySvxLocal(int nrhs, const double* B_local, int ldb, double* X_local, int ldx, double* rcond,
+                            double* ferr = nullptr, double* berr = nullptr, char* equed = nullptr) {
+    auto& s = chol_detail::state();
+    if (!s.plan) throw CholeskyException("choleskySvxLocal() before initialize()");
+    int info = 0;
+    chol_detail::check(cflx_chol_svx_local(s.plan, nrhs, B_local, ldb, X_local, ldx, rcond, ferr, berr, equed, &info),
+                       "choleskySvxLocal");
+    return info;
+}
+inline int choleskySvxxLocal(int nrhs, const double* B_local, int ldb, double* X_local, int ldx, double* rcond,
+                             double* err_norm, double* err_comp = nullptr, double* rpvgrw = nullptr,
+                             double* berr = nullptr, char* equed = nullptr) {
+    auto& s = chol_detail::state();
+    if (!s.plan) throw CholeskyException("choleskySvxxLocal() before initialize()");
+    int info = 0;
+    chol_detail::check(cflx_chol_svxx_local(s.plan, nrhs, B_local, ldb, X_local, ldx, rcond, rpvgrw, berr, err_norm,
+                                            err_comp, equed, &info),
+                       "choleskySvxxLocal");
+    return info;
+}
 // LAPACK dpotri (lower) with the factor of the last parallelCholesky() (cflx_chol_inverse, collective): Ainv_local (Ml x
 // Nl; host or device memory; may be null) receives inv(A) on this rank's real tiles on and below the diagonal, zeros
 // elsewhere.

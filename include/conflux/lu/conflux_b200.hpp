@@ -405,6 +405,48 @@ int LU_svxx(lu_params<T>& gv, int nrhs, const T* B, int ldb, T* X, int ldx, doub
     return info;
 }
 
+// LU_refine, LU_refine_x, LU_svx and LU_svxx with B and X distributed like A (cflx_lu_refine_local ...
+// cflx_lu_svxx_local, collective): the shares and memory rules of LU_solve_local.  For the refinements X_local holds the
+// solution on entry (read on layer 0, required there) and must not overlap B_local; for svx / svxx it is output only
+// (may be null, may be B_local with ldx == ldb).  The columns go in blocks of cflx_refine_block_cols(gv.v), each with
+// the bits the replicated call gives those columns alone; per-column outputs and results as the replicated calls.
+template <class T>
+void LU_refine_local(lu_params<T>& gv, int nrhs, const T* B_local, int ldb, T* X_local, int ldx, double* ferr = nullptr,
+                     double* berr = nullptr, bool transposed = false) {
+    check(cflx_lu_refine_local(gv.plan, transposed ? 1 : 0, nrhs, B_local, ldb, X_local, ldx, ferr, berr),
+          "LU_refine_local");
+}
+template <class T>
+int LU_refine_x_local(lu_params<T>& gv, int nrhs, const T* B_local, int ldb, T* X_local, int ldx, double* err_norm,
+                      double* err_comp = nullptr, double* rcond = nullptr, double* berr = nullptr,
+                      bool transposed = false) {
+    int info = 0;
+    check(cflx_lu_refine_x_local(gv.plan, transposed ? 1 : 0, nrhs, B_local, ldb, X_local, ldx, rcond, berr, err_norm,
+                                 err_comp, &info),
+          "LU_refine_x_local");
+    return info;
+}
+template <class T>
+int LU_svx_local(lu_params<T>& gv, int nrhs, const T* B_local, int ldb, T* X_local, int ldx, double* rcond,
+                 double* ferr = nullptr, double* berr = nullptr, double* rpvgrw = nullptr, char* equed = nullptr,
+                 bool transposed = false) {
+    int info = 0;
+    check(cflx_lu_svx_local(gv.plan, transposed ? 1 : 0, nrhs, B_local, ldb, X_local, ldx, rcond, ferr, berr, rpvgrw,
+                            equed, &info),
+          "LU_svx_local");
+    return info;
+}
+template <class T>
+int LU_svxx_local(lu_params<T>& gv, int nrhs, const T* B_local, int ldb, T* X_local, int ldx, double* rcond,
+                  double* err_norm, double* err_comp = nullptr, double* rpvgrw = nullptr, double* berr = nullptr,
+                  char* equed = nullptr, bool transposed = false) {
+    int info = 0;
+    check(cflx_lu_svxx_local(gv.plan, transposed ? 1 : 0, nrhs, B_local, ldb, X_local, ldx, rcond, rpvgrw, berr,
+                             err_norm, err_comp, equed, &info),
+          "LU_svxx_local");
+    return info;
+}
+
 // LAPACK dgetri with the factors of the last LU_rep on the GPU grid (cflx_lu_inverse, collective): Ainv_local (Ml x Nl,
 // the conflux layout; host or device memory; may be null) receives this rank's share of inv(A).  Returns info (0; k for
 // an exactly zero U(k,k), nothing written).

@@ -236,6 +236,51 @@ int cflx_lu_equilibrate(cflx_lu*, int apply, double* r_out, double* c_out, doubl
  * CFLX_ERR_ARG as cflx_lu_refine and for a NULL rcond_out or info_out; CFLX_ERR_STATE as cflx_lu_rcond. */
 int cflx_lu_svx(cflx_lu*, int trans, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out,
                 double* ferr_out, double* berr_out, double* rpvgrw_out, char* equed_out, int* info_out);
+/* COLLECTIVE.  Refinement and the expert drivers with B and X distributed like A (ScaLAPACK's pdgerfs / pdgesvx):
+ * cflx_lu_refine, cflx_lu_refine_x, cflx_lu_svx and cflx_lu_svxx with the same arguments in the same order, except that
+ * B and X are replaced by this rank's shares B_local / X_local (ldb / ldx) in the layout of cflx_lu_solve_local.  Its
+ * layout and memory rules hold: host or device memory, device memory on this rank's device, a host share through one
+ * temporary device share (an X read on entry through one more), local columns at or beyond nrhs and the ld padding
+ * neither read nor written.  B_local is read on layer pk == 0 only and may be NULL on other layers.  For refine_local and
+ * refine_x_local, X_local is the solution on entry: it is read on layer 0 only, is required there, and must not overlap
+ * B_local; for svx_local and svxx_local it is output only, may be NULL on any rank, and may be B_local itself when
+ * ldx == ldb.  Every layer receives layer 0's bits.  ferr_out, berr_out (nrhs) and err_bnds_*_out (nrhs x 3) are host
+ * arrays, identical on every rank.
+ * The columns are processed in blocks [c0, c0 + w) of w <= cflx_refine_block_cols(v) columns: each block of B (and, for
+ * refine and refine_x, of X) is packed and assembled as in cflx_lu_solve_local, by one world all-reduce summed as 64-bit
+ * integers with one contributor per element; it is then refined by the replicated driver's own core on device buffers,
+ * and X's block is scattered back.  The zero-pivot check, the pivot growth and the dgecon rcond that refine_x, svx and
+ * svxx use are computed once per call, before the blocks.  So, for every block, X's bits and the per-column outputs
+ * equal those of the replicated driver called on those w columns alone, and rcond, rpvgrw and equed equal its bits.
+ * info_out: k for the first exactly zero U(k,k), as the replicated driver (X_local keeps its value and the per-column
+ * outputs are not written); M + 1 for svx as cflx_lu_svx; M + j for refine_x and svxx with j the first global column
+ * (1-based, over all blocks) whose bound was set to 1; else 0.
+ * The device workspace grows with the block width, not with nrhs: with ldn = round_up(w, 8) it is at most
+ * ldn (15 M + 2 v + (2 P + 5)(Ml + Nl)) + 2 M doubles (P = Px Py Pz; the refinement's M x ldn buffers, the
+ * block's B and X, the solves' work buffers, the gathered heads and tails, the all-gathered residual partials, and the
+ * pivot growth's column maxima), plus the temporary shares of host B_local / X_local.
+ * CFLX_ERR_ARG as cflx_lu_solve_local (without the in-place rule for refine*), for X_local NULL on layer 0 or
+ * overlapping B_local (refine*), and for a NULL rcond_out, info_out or err_bnds_norm_out where the replicated driver
+ * refuses one.  CFLX_ERR_STATE as cflx_lu_rcond: before a factorisation, after cflx_lu_set_local, on the low-precision
+ * factors of cflx_lu_sv_mixed, and when the input buffer was handed to a queued next matrix.  The matrix is the one the
+ * factors represent (scaled after cflx_lu_equilibrate, W after cflx_lu_rbt).  Every rank passes the same trans and
+ * nrhs.  Leaves the factors, the permutation, the input, the scaling record, later solves and the launch count as they
+ * are. */
+int cflx_lu_refine_local(cflx_lu*, int trans, int nrhs, const double* B_local, int ldb, double* X_local, int ldx,
+                         double* ferr_out, double* berr_out);
+int cflx_lu_refine_x_local(cflx_lu*, int trans, int nrhs, const double* B_local, int ldb, double* X_local, int ldx,
+                           double* rcond_out, double* berr_out, double* err_bnds_norm_out, double* err_bnds_comp_out,
+                           int* info_out);
+int cflx_lu_svx_local(cflx_lu*, int trans, int nrhs, const double* B_local, int ldb, double* X_local, int ldx,
+                      double* rcond_out, double* ferr_out, double* berr_out, double* rpvgrw_out, char* equed_out,
+                      int* info_out);
+int cflx_lu_svxx_local(cflx_lu*, int trans, int nrhs, const double* B_local, int ldb, double* X_local, int ldx,
+                       double* rcond_out, double* rpvgrw_out, double* berr_out, double* err_bnds_norm_out,
+                       double* err_bnds_comp_out, char* equed_out, int* info_out);
+/* Pure host.  cols_out: the block width of the distributed refinement and expert drivers (cflx_lu_refine_local ...
+ * cflx_chol_svxx_local) for tile size v: the whole number of tiles nearest CFLX_REFINE_NC = 256 columns, at least one
+ * tile.  CFLX_ERR_ARG for v < 1 or a NULL cols_out. */
+int cflx_refine_block_cols(int v, int* cols_out);
 /* The precisions of the mixed-precision drivers' trailing update: TF32 tensor cores with one term (A_hi B_hi) or three
  * (3xTF32: A_hi B_hi + A_hi B_lo + A_lo B_hi), every operand row scaled by a power of two first, FP32 accumulation. */
 #define CFLX_PREC_TF32 1
@@ -447,6 +492,23 @@ int cflx_chol_equilibrate_b(cflx_chol*, int apply, double* s_out, double* scond_
 int cflx_chol_svxx(cflx_chol*, int nrhs, const double* B, int ldb, double* X, int ldx, double* rcond_out,
                    double* rpvgrw_out, double* berr_out, double* err_bnds_norm_out, double* err_bnds_comp_out,
                    char* equed_out, int* info_out);
+/* COLLECTIVE.  cflx_chol_refine, cflx_chol_refine_x, cflx_chol_svx and cflx_chol_svxx with B and X distributed like A
+ * (ScaLAPACK's pdporfs / pdposvx): the shares, rules, block schedule, results and workspace of cflx_lu_refine_local ...
+ * cflx_lu_svxx_local without trans, in the layout of cflx_chol_solve_local (only the rows of real tiles are read and
+ * written).  dpocon (and for svxx dla_porpvgrw) runs once per call.  info_out: N + 1 for svx as cflx_chol_svx, N + j
+ * with j the first global column for refine_x and svxx, else 0.  CFLX_ERR_ARG as there; CFLX_ERR_STATE as
+ * cflx_chol_solve.  The matrix is the one the factor represents (scaled after cflx_chol_equilibrate, W after
+ * cflx_chol_rbt; a signed factor after cflx_chol_factor_ldlt).  Side effects as cflx_lu_refine_local. */
+int cflx_chol_refine_local(cflx_chol*, int nrhs, const double* B_local, int ldb, double* X_local, int ldx,
+                           double* ferr_out, double* berr_out);
+int cflx_chol_refine_x_local(cflx_chol*, int nrhs, const double* B_local, int ldb, double* X_local, int ldx,
+                             double* rcond_out, double* berr_out, double* err_bnds_norm_out, double* err_bnds_comp_out,
+                             int* info_out);
+int cflx_chol_svx_local(cflx_chol*, int nrhs, const double* B_local, int ldb, double* X_local, int ldx,
+                        double* rcond_out, double* ferr_out, double* berr_out, char* equed_out, int* info_out);
+int cflx_chol_svxx_local(cflx_chol*, int nrhs, const double* B_local, int ldb, double* X_local, int ldx,
+                         double* rcond_out, double* rpvgrw_out, double* berr_out, double* err_bnds_norm_out,
+                         double* err_bnds_comp_out, char* equed_out, int* info_out);
 /* COLLECTIVE.  LAPACK dsposv on the GPU grid: cflx_lu_sv_mixed's loop with the Cholesky factored with the trailing
  * update in `prec` and the residual from the stored lower triangle of the input.  iter_out -3 when the low-precision
  * factorisation met a non-positive pivot.  On a negative iter_out the input is factored again in FP64 and solved, with
